@@ -243,7 +243,7 @@ int Pipeline::enqueue(const float *d_img, int pitch, double initBlur, float thre
   dp.numLevels = nl; dp.totalTiles = tiles; dp.tiles = d_tiles;
   if (tiles != numTiles) { set_error("detector tile list out of sync"); return CS_E_ARG; }
   dp.thresh = thresh; dp.edgeLimit = 10.0f; dp.factor = 1.0f / CS_NUM_SCALES;   // cudaSiftH.cu:213
-  dp.pts = d_pts; dp.counters = d_counters; dp.maxPts = maxPts; dp.dbgSkip = g_detect_skip;
+  dp.pts = d_pts; dp.counters = d_counters; dp.maxPts = maxPts;
   if ((r = launch_detect(dp, st)) < 0) return r;
   if (ev) cudaEventRecord(ev[3], st);
 
@@ -728,10 +728,7 @@ unsigned long long cs_launch_count(void) { return cs::g_launches; }
 
 int cs_set_tuning(const char *key, int value)
 {
-  if (key && strcmp(key, "detect_variant") == 0) { cs::g_detect_variant = value; return 0; }
-  if (key && strcmp(key, "detect_skip") == 0) { cs::g_detect_skip = value; return 0; }
   if (key && strcmp(key, "legacy") == 0) { cs::g_legacy = value ? 1 : 0; return 0; }
-  if (key && strcmp(key, "d2_variant") == 0) { cs::g_d2_variant = value; return 0; }
   if (key && strcmp(key, "d2_hs") == 0) { cs::g_d2_hs = value; return 0; }
   if (key && strcmp(key, "pa_rows") == 0) { cs::g_pa_rows = value; return 0; }
   if (key && strcmp(key, "sd_split") == 0) { cs::g_sd_split = value; return 0; }

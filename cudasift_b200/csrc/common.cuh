@@ -110,10 +110,7 @@ struct DetectParams {
   SiftPoint *pts;
   unsigned int *counters;   // [0] detected (primaries), [1] total incl. secondaries
   int maxPts;
-  int dbgSkip;              // diagnostics: bit0 staging, bit1 vertical, bit2 horizontal, bit3 extrema, bit4 refinement are skipped
 };
-extern int g_detect_skip;      // tuning (cs_set_tuning "detect_skip")
-extern int g_detect_variant;   // tuning (cs_set_tuning "detect_variant")
 int launch_detect(const DetectParams &p, cudaStream_t st);
 #define CS_DETECT_TILE_W 62   // interior (tested) pixels per detector tile
 #define CS_DETECT_TILE_H 14

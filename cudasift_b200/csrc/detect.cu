@@ -36,6 +36,10 @@ namespace cs {
 #define DT_PH 4               // scales blurred per phase (2 phases)
 #define DT_VS 74              // float2 stride of a vertical-result row (37 16-byte chunks: odd -> the 8 row
                               // pairs of a quarter warp hit 8 different bank groups)
+#define DT_THREADS 160        // CTA size
+#define DT_NC 4               // DoG columns per thread in the horizontal pass (64*8/DT_NC tasks)
+#define DT_VR 4               // row pairs per thread in the vertical pass (72*8/DT_VR tasks)
+#define DT_MINB 4             // CTAs per SM (detect_kernel)
 // shared memory, in float2 units
 #define DT_SM_IN (2 * DT_HP * DT_IW)                  // staged input pairs P[j] = (in[j], in[j+8]), j = 0..15
 #define DT_SM_V (DT_PH * DT_HP * DT_VS)               // vertical results of one phase
@@ -75,7 +79,6 @@ __device__ __forceinline__ void cp_async4(float *dst_smem, const float *src)
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-template <int DT_THREADS>
 __device__ __forceinline__ void tile_prefetch(float2 *s_in, const float *__restrict__ img, int w, int h,
                                               int pitch, int x0, int y0)
 {
@@ -116,15 +119,13 @@ __device__ __forceinline__ void tile_prefetch(float2 *s_in, const float *__restr
 // interior pixel whose |DoG| exceeds `thresh` in one of the five testable planes, decided on the
 // register copies of the DoG values -- the extrema test then only visits those pixels.
 // `mid()` runs when s_in is dead (after the last vertical pass): the caller refills it there.
-// DT_THREADS: CTA size; DT_NC: DoG columns per thread in the horizontal pass (64*8/DT_NC tasks);
-// DT_VR: row pairs per thread in the vertical pass (72*8/DT_VR tasks).
 // Two phases of 4 scales each.  Vertical pass: task = (column, DT_VR row pairs), pair sums shared
 // by the scales.  Horizontal pass + DoG: task = (row pair, DT_NC consecutive columns); the 8 lanes
 // of a quarter warp take the 8 row pairs so that 128-bit shared accesses are conflict free.
-template <int DT_THREADS, int DT_NC, int DT_VR, typename Mid>
+template <typename Mid>
 __device__ __forceinline__ unsigned int dog_tile(int w, int h, int x0, int y0, const LaplaceTaps &taps,
                                                  const float2 *s_in, float2 *s_v, float2 *s_dog,
-                                                 float thresh, int skip, Mid mid)
+                                                 float thresh, Mid mid)
 {
   const int tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5;
@@ -142,7 +143,7 @@ __device__ __forceinline__ unsigned int dog_tile(int w, int h, int x0, int y0, c
 #pragma unroll
     for (int vt0 = 0; vt0 < VTASKS; vt0 += DT_THREADS) {
       const int vt = vt0 + tid;
-      if (vt < VTASKS && !(skip & 2)) {
+      if (vt < VTASKS) {
         const int vh = vt / DT_IW, vc = vt - vh * DT_IW;
         f32x2 in[DT_VR + 8];
 #pragma unroll
@@ -160,7 +161,7 @@ __device__ __forceinline__ unsigned int dog_tile(int w, int h, int x0, int y0, c
     }
     __syncthreads();
     if (ph == CS_LAPLACE_S / DT_PH - 1) mid();
-    if (hact && !(skip & 4)) {
+    if (hact) {
 #pragma unroll
       for (int s = 0; s < DT_PH; s++) {
         const int sg = DT_PH * ph + s;
@@ -214,7 +215,6 @@ __device__ __forceinline__ unsigned int dog_tile(int w, int h, int x0, int y0, c
 }
 
 // Append the pixels of a candidate mask (see dog_tile) to the tile's list as row*64+col.
-template <int DT_NC>
 __device__ __forceinline__ void list_append(unsigned int mask, unsigned short *s_list, int *s_cnt)
 {
   if (mask) {
@@ -317,8 +317,7 @@ __device__ __forceinline__ TilePos decode_tile(const DetectParams &P, int t)
   return tp;
 }
 
-template <int DT_THREADS, int NC, int VR, int MINB>
-__global__ void __launch_bounds__(DT_THREADS, MINB)
+__global__ void __launch_bounds__(DT_THREADS, DT_MINB)
 detect_kernel(const __grid_constant__ DetectParams P)
 {
   extern __shared__ __align__(16) float2 smem2[];
@@ -332,14 +331,13 @@ detect_kernel(const __grid_constant__ DetectParams P)
   __shared__ Keypoint s_kq[DT_KQ];
   const float thresh = P.thresh;
   const float *dogf = reinterpret_cast<const float *>(s_dog);
-  const int skip = P.dbgSkip;
 
   int t = blockIdx.x;
   unsigned int req = 0;
   if (threadIdx.x == 0) req = gridDim.x + atomicAdd(&P.counters[2], 1u);
   TilePos tp = decode_tile(P, t);
   if (threadIdx.x == 0) { s_cnt = 0; s_kn = 0; }
-  if (!(skip & 1)) tile_prefetch<DT_THREADS>(s_in, P.lev[tp.level].img, P.lev[tp.level].w, P.lev[tp.level].h, P.lev[tp.level].pitch, tp.x0, tp.y0);
+  tile_prefetch(s_in, P.lev[tp.level].img, P.lev[tp.level].w, P.lev[tp.level].h, P.lev[tp.level].pitch, tp.x0, tp.y0);
 
   for (;;) {
     const DetectLevel &L = P.lev[tp.level];
@@ -361,26 +359,26 @@ detect_kernel(const __grid_constant__ DetectParams P)
     int tn = 0;
     bool more = false;
     TilePos tpn = tp;
-    const unsigned int mask = dog_tile<DT_THREADS, NC, VR>(L.w, L.h, x0, y0, L.taps, s_in, s_v, s_dog, thresh, skip, [&]() {
+    const unsigned int mask = dog_tile(L.w, L.h, x0, y0, L.taps, s_in, s_v, s_dog, thresh, [&]() {
       // the staging area is free: start the next tile's copies, retire the parked keypoints
       tn = s_next;
       more = tn < P.totalTiles;
       if (more) {
         tpn = decode_tile(P, tn);
         const DetectLevel &Ln = P.lev[tpn.level];
-        if (!(skip & 1)) tile_prefetch<DT_THREADS>(s_in, Ln.img, Ln.w, Ln.h, Ln.pitch, tpn.x0, tpn.y0);
+        tile_prefetch(s_in, Ln.img, Ln.w, Ln.h, Ln.pitch, tpn.x0, tpn.y0);
       }
       if ((int)threadIdx.x < nkq) store_keypoint(P, slot, s_kq[threadIdx.x]);
       if (threadIdx.x == 0) { s_kn = 0; s_cnt = 0; }
     });
-    list_append<NC>(mask, s_list, &s_cnt);
+    list_append(mask, s_list, &s_cnt);
     __syncthreads();
 
     // 3x3x3 extrema, only on the pixels the blur pass flagged (|DoG| > thresh at some scale); one work
     // item per (flagged pixel, scale).  Sparse tiles (the finest octave: ~2 flagged pixels per tile)
     // give a warp per item, lane j < 27 holding neighbour j of the 3x3x3 cube -- a short critical path;
     // dense tiles (coarse octaves: up to 20 % of the pixels) give a thread per item.
-    const int nitems = (skip & 8) ? 0 : s_cnt * CS_NUM_SCALES;
+    const int nitems = s_cnt * CS_NUM_SCALES;
     if (nitems <= 4 * (DT_THREADS / 32)) {
       const int lane = threadIdx.x & 31;
       const int pz = lane / 9, py = (lane - 9 * pz) / 3, px = lane - 9 * pz - 3 * py;
@@ -396,7 +394,7 @@ detect_kernel(const __grid_constant__ DetectParams P)
         const bool other = lane < 27 && lane != 13;
         const bool mx = __all_sync(0xffffffffu, !other || c > tt);
         const bool mn = __all_sync(0xffffffffu, !other || c < tt);
-        if ((c > 0.0f ? mx : mn) && lane == 0 && !(skip & 16)) refine(pl, r, d, x0 + d, y0 + r, sc, L, P, s_kq, &s_kn);
+        if ((c > 0.0f ? mx : mn) && lane == 0) refine(pl, r, d, x0 + d, y0 + r, sc, L, P, s_kq, &s_kn);
       }
     } else {
       for (int i = threadIdx.x; i < nitems; i += DT_THREADS) {
@@ -419,7 +417,7 @@ detect_kernel(const __grid_constant__ DetectParams P)
                 mx = mx && (c > tt); mn = mn && (c < tt);
               }
           }
-        if ((c > 0.0f ? mx : mn) && !(skip & 16)) refine(pl, r, d, x0 + d, y0 + r, sc, L, P, s_kq, &s_kn);
+        if (c > 0.0f ? mx : mn) refine(pl, r, d, x0 + d, y0 + r, sc, L, P, s_kq, &s_kn);
       }
     }
     if (!more) break;
@@ -430,48 +428,21 @@ detect_kernel(const __grid_constant__ DetectParams P)
   if ((int)threadIdx.x < nkq) store_keypoint(P, atomicAdd(&P.counters[0], 1u), s_kq[threadIdx.x]);
 }
 
-// Tuning variants (thread count, columns per horizontal task, row pairs per vertical task, CTAs/SM).
-int g_detect_variant = -1;
-int g_detect_skip = 0;
-template <int T, int NC, int VR, int MINB>
-static int launch_variant(const DetectParams &p, cudaStream_t st)
+int launch_detect(const DetectParams &p, cudaStream_t st)
 {
+  if (p.totalTiles <= 0) return 0;
   // per device: cudaFuncSetAttribute applies to the current device only, and SM counts may differ
   static int smsOf[64];
   int dev = 0;
   CS_CUDA(cudaGetDevice(&dev));
   dev &= 63;
   if (smsOf[dev] == 0) {
-    CS_CUDA(cudaFuncSetAttribute(detect_kernel<T, NC, VR, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, DT_SMEM_BYTES));
+    CS_CUDA(cudaFuncSetAttribute(detect_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DT_SMEM_BYTES));
     CS_CUDA(cudaDeviceGetAttribute(&smsOf[dev], cudaDevAttrMultiProcessorCount, dev));
   }
   const int sms = smsOf[dev];
-  const int grid = p.totalTiles < MINB * sms ? p.totalTiles : MINB * sms;
-  detect_kernel<T, NC, VR, MINB><<<grid, T, DT_SMEM_BYTES, st>>>(p);
-  return 0;
-}
-
-int launch_detect(const DetectParams &p, cudaStream_t st)
-{
-  if (g_detect_variant < 0) {
-    const char *e = getenv("CUDASIFT_DETECT_VARIANT");
-    g_detect_variant = e ? atoi(e) : 0;
-    const char *k = getenv("CUDASIFT_DETECT_SKIP");      // diagnostics, see DetectParams::dbgSkip
-    if (k) g_detect_skip = atoi(k);
-  }
-  if (p.totalTiles <= 0) return 0;
-  int r;
-  switch (g_detect_variant) {
-    case 1: r = launch_variant<160, 8, 4, 4>(p, st); break;
-    case 2: r = launch_variant<320, 2, 2, 4>(p, st); break;
-    case 3: r = launch_variant<320, 2, 2, 3>(p, st); break;
-    case 4: r = launch_variant<320, 4, 2, 4>(p, st); break;
-    case 5: r = launch_variant<256, 2, 2, 4>(p, st); break;
-    case 6: r = launch_variant<288, 2, 2, 4>(p, st); break;
-    case 7: r = launch_variant<288, 4, 2, 4>(p, st); break;
-    default: r = launch_variant<160, 4, 4, 4>(p, st); break;
-  }
-  if (r < 0) return r;
+  const int grid = p.totalTiles < DT_MINB * sms ? p.totalTiles : DT_MINB * sms;
+  detect_kernel<<<grid, DT_THREADS, DT_SMEM_BYTES, st>>>(p);
   count_launch();
   CS_CUDA(cudaGetLastError());
   return 0;
@@ -479,7 +450,6 @@ int launch_detect(const DetectParams &p, cudaStream_t st)
 
 // Stage-level entry point (parity tests): materialise the 7 DoG planes exactly as the
 // fused detector computes them.  Plane stride = h*pitch floats (cudaSiftH.cu:184).
-#define DT_THREADS 160
 __global__ void __launch_bounds__(DT_THREADS)
 dog_planes_kernel(const float *__restrict__ img, float *__restrict__ dog, int w, int h, int pitch,
                   int tilesX, const __grid_constant__ LaplaceTaps taps)
@@ -490,10 +460,10 @@ dog_planes_kernel(const float *__restrict__ img, float *__restrict__ dog, int w,
   float2 *s_in = s_dog + DT_SM_DOG;
   const int by = blockIdx.x / tilesX, bx = blockIdx.x - by * tilesX;
   const int x0 = bx * (DT_W - 2), y0 = by * (DT_H - 2);
-  tile_prefetch<DT_THREADS>(s_in, img, w, h, pitch, x0, y0);
+  tile_prefetch(s_in, img, w, h, pitch, x0, y0);
   cp_async_wait_all();
   __syncthreads();
-  dog_tile<DT_THREADS, 4, 4>(w, h, x0, y0, taps, s_in, s_v, s_dog, 0.0f, 0, []() {});
+  dog_tile(w, h, x0, y0, taps, s_in, s_v, s_dog, 0.0f, []() {});
   const float *dogf = reinterpret_cast<const float *>(s_dog);
   const size_t plane = (size_t)h * pitch;
   for (int i = threadIdx.x; i < (CS_LAPLACE_S - 1) * DT_H * DT_W; i += DT_THREADS) {

@@ -1,5 +1,5 @@
 // detect2.cu -- marching detector: 8-scale blur + DoG + 3x3x3 extrema + sub-pixel refinement, all octaves of
-// a whole BATCH of images in one launch.
+// a whole BATCH of images in one launch (detect3_kernel).
 //
 // Behavioural spec: reference LaplaceMultiMem (cudaSiftD.cu:1753-1793, host :460-487) and
 // FindPointsMultiNew (cudaSiftD.cu:1292-1431, host :489-514).  Same per-pixel arithmetic as detect.cu
@@ -13,14 +13,28 @@
 //  * Input rows arrive by TMA (cp.async.bulk.tensor.2d, one 256x1 box per row and stream, row index clamped
 //    by the issuing thread, columns clamped by the reading thread) into an 8-deep ring -> no address
 //    arithmetic and no global loads in the loop.
-//  * Vertical pass: thread = 2 columns x 4 scales (warps 0-3: scales 0-3, warps 4-7: scales 4-7); the 20 taps
-//    are 20 registers; results go to shared
-//    memory once (STS.64).
-//  * Horizontal pass + DoG: lane = (scale, 8 columns); 8 conflict-free LDS.128 fetch the 16 pairs, the DoG
-//    difference takes the neighbouring scale from the neighbouring lane (shuffle), the 7 DoG planes of the row
-//    pair go to a 4-row ring in shared memory (only 3 rows of DoG ever exist).
+//  * Warp-specialised, one CTA of 16 warps per SM:
+//      warps 12-15 (producers): vertical pass of all 8 scales (thread = columns c and c+128, 9-row register
+//                              window, 40 taps in registers) and the TMA row ring -- the serial critical path, kept
+//                              short; results go to shared memory once (STS.64)
+//      warps 0-3 / 4-7 / 8-11 (consumer groups 0 / 1 / 2): horizontal pass + DoG + candidate flags of the steps
+//                              k = g mod 3 (2 x 16 column groups), then the extrema tests of row k-4; each group has
+//                              three steps of time for one step of work.  Lane = (scale, 8 columns): 8 conflict-free
+//                              LDS.128 fetch the 16 pairs, the DoG difference takes the neighbouring scale from the
+//                              neighbouring lane (shuffle), the DoG row goes to an 8-deep ring in shared memory.
 //  * |DoG| > thresh is decided on the register copies; flagged (pixel, plane) candidates are listed and tested
-//    two steps later, when the rows above and below exist, by whichever thread is free.
+//    four steps later, when the rows above and below exist.
+//
+// The producers run ahead of the consumers through three vertical-result buffers (buffer = group); hand-over is by
+// named barriers (bar.arrive / bar.sync) instead of CTA-wide barriers:
+//   FULL[g]  producers -> group g: v[g] written        EMPTY[g] group g -> producers: v[g] is in registers
+//   DONE[g]  group g -> producers: the DoG row and the candidate list of its step are written (the extrema tests of
+//            an older row follow, off the producers' critical path)
+//   LATE[g]  group g -> producers: its previous step is complete, tests included (signalled at the start of the next step)
+//            The producers check DONE of step m-3 and LATE of step m-4 just before they signal FULL of step m.  Hence,
+//            when a group passes FULL of step k, every DoG row <= k-3 is written and every step <= k-4 of every group
+//            is complete: it may test the extrema of row k-4 (rows k-5..k-3) and overwrite ring slot k mod 8 (last
+//            read for rows k-9..k-7 in steps k-5, k-4 and -- by this same group -- k-3).
 //
 // Shared memory per row pair and step: 128 (vertical STS) + 256 (horizontal LDS) + 128 (shuffles) + 112 (DoG
 // STS) wavefronts for 2 x 244 pixels x 8 scales = 1.3 wavefronts per pixel (detect.cu: 2.7).
@@ -28,7 +42,6 @@
 
 namespace cs {
 
-#define D2_THREADS 256
 #define D2_IW 256            // staged input columns per strip (one TMA box row)
 #define D2_TESTED CS_D2_STRIP // tested DoG columns per strip: 1..244 (DoG column d <-> input column d + 4); a multiple of 4,
                              // because TMA wants the first column of a box (x0 - 4) on a 16-byte boundary
@@ -40,10 +53,6 @@ namespace cs {
 #define D2_LCAP 510          // candidate list capacity per step (more: the step is scanned exhaustively)
 #define D2_KQ 32             // keypoints parked per item before the slots are allocated
 #define D2_SMEM_IN (D2_NS * 2 * D2_IW * 4)            // 16384
-#define D2_SMEM_V (2 * D2_VBUF2 * 8)                  // 33024
-#define D2_SMEM_RING (4 * D2_RSLOTF * 4)              // 56000
-#define D2_SMEM_LIST (4 * 512 * 2)                    // 4096
-#define D2_SMEM_BYTES (D2_SMEM_IN + D2_SMEM_V + D2_SMEM_RING + D2_SMEM_LIST)   // 109504 -> 2 CTAs per SM
 
 // cudaSiftD.cu:1769-1772 / 1779-1788: sum = k0*c; sum += kj*(x[-j]+x[+j]), j=1..4.
 // SASS: FMUL(k1,p1); FFMA(k0,c); FFMA(k2,p2); FFMA(k3,p3); FFMA(k4,p4)  -- here on both halves at once.
@@ -56,32 +65,6 @@ __device__ __forceinline__ f32x2 d2_sym9(const float (&k)[5], f32x2 c, f32x2 p1,
   s = fma2(pk2(k[3], k[3]), p3, s);
   s = fma2(pk2(k[4], k[4]), p4, s);
   return s;
-}
-
-// One step of the vertical pass: the newest input row pair enters window slot PH (the oldest one leaves),
-// then this thread's 4 scales of both columns are written to the vertical-result buffer.
-template <int PH>
-__device__ __forceinline__ void d2_vertical(f32x2 (&W0)[9], f32x2 (&W1)[9], f32x2 n0, f32x2 n1,
-                                            const float (&kv)[4][5], float2 *vdst)
-{
-#define D2_WI(i) ((PH + 1 + (i)) % 9)
-  W0[PH] = n0;
-  W1[PH] = n1;
-  {
-    const f32x2 c = W0[D2_WI(4)];
-    const f32x2 p1 = add2(W0[D2_WI(3)], W0[D2_WI(5)]), p2 = add2(W0[D2_WI(2)], W0[D2_WI(6)]);
-    const f32x2 p3 = add2(W0[D2_WI(1)], W0[D2_WI(7)]), p4 = add2(W0[D2_WI(0)], W0[D2_WI(8)]);
-#pragma unroll
-    for (int s = 0; s < 4; s++) vdst[s * D2_VROW2] = upk(d2_sym9(kv[s], c, p1, p2, p3, p4));
-  }
-  {
-    const f32x2 c = W1[D2_WI(4)];
-    const f32x2 p1 = add2(W1[D2_WI(3)], W1[D2_WI(5)]), p2 = add2(W1[D2_WI(2)], W1[D2_WI(6)]);
-    const f32x2 p3 = add2(W1[D2_WI(1)], W1[D2_WI(7)]), p4 = add2(W1[D2_WI(0)], W1[D2_WI(8)]);
-#pragma unroll
-    for (int s = 0; s < 4; s++) vdst[s * D2_VROW2 + 128] = upk(d2_sym9(kv[s], c, p1, p2, p3, p4));
-  }
-#undef D2_WI
 }
 
 struct D2Keypoint { float x, y, scale, sharpness, edgeness, subsampling; unsigned int tag; };
@@ -162,278 +145,6 @@ __device__ __forceinline__ void d2_refine(const float (&v)[3][3][3], int gx, int
   else d2_store_keypoint(pts, maxPts, atomicAdd(counter, 1u), kp);
 }
 
-template <int MINB>
-__global__ void __launch_bounds__(D2_THREADS, MINB)
-detect2_kernel(const __grid_constant__ Detect2Params P)
-{
-  extern __shared__ __align__(128) unsigned char d2_smem[];
-  float *s_in = reinterpret_cast<float *>(d2_smem);                                         // [slot][stream][256]
-  float2 *s_v = reinterpret_cast<float2 *>(d2_smem + D2_SMEM_IN);                           // [buf][scale][258]
-  float *s_ring = reinterpret_cast<float *>(d2_smem + D2_SMEM_IN + D2_SMEM_V);              // [slot][plane][500]
-  unsigned short *s_list = reinterpret_cast<unsigned short *>(d2_smem + D2_SMEM_IN + D2_SMEM_V + D2_SMEM_RING);
-  __shared__ __align__(8) uint64_t s_full[D2_NS];
-  __shared__ int s_cnt[4];
-  __shared__ int s_kn, s_next;
-  __shared__ D2Keypoint s_kq[D2_KQ];
-
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int half = tid >> 7, cl = tid & 127;              // vertical role: columns cl, cl+128, scales 4*half..+3
-  const int hs_ = lane & 7, cgl = lane >> 3;              // horizontal role: scale hs_, column group cg
-  const int cg = 4 * warp + cgl;
-  const float thresh = P.thresh;
-
-  int item = blockIdx.x;
-  unsigned int req = 0;
-  if (tid == 0) req = gridDim.x + atomicAdd(P.sched, 1u);
-
-  while (item < P.numItems) {
-    // ------------------------------------------------------------------ item set-up
-    const uint4 it = __ldg(P.items + item);
-    const int level = it.x & 0xff, img = it.x >> 8;
-    const int x0 = (int)it.y, ry0 = (int)it.z, hs = (int)it.w;
-    const D2Level &L = P.lev[level];
-    const int w = L.w, h = L.h;
-    const CUtensorMap *map = P.maps + (size_t)img * CS_MAX_LEVELS + level;
-    SiftPoint *pts = P.pts + (size_t)img * P.ptsStride;
-    unsigned int *counters = P.counters + (size_t)img * CS_CNT_STRIDE;
-    const int nsteps = hs + 2;                            // DoG rows ry0-1+k (stream A), ry0+hs-1+k (stream B), k < nsteps
-    const int nrows = 8 + nsteps;                         // input rows per stream: ry0-5+i (A), i < nrows
-
-    __syncthreads();     // previous item's last extrema pass and keypoint flush are complete
-    if (tid == 0) {
-      for (int i = 0; i < D2_NS; i++) mbarrier_init(&s_full[i], 1);
-      mbarrier_init_fence();
-      s_cnt[0] = s_cnt[1] = s_cnt[2] = s_cnt[3] = 0;
-      s_kn = 0;
-      s_next = (int)req;                                  // requested during the previous item
-      req = gridDim.x + atomicAdd(P.sched, 1u);
-    }
-    __syncthreads();     // barriers initialised, next item index published
-    if (tid == 0) {
-      tensormap_acquire(map);
-      for (int i = 0; i < D2_NS; i++) {                   // prologue rows: all in flight at once
-        mbarrier_expect_tx(&s_full[i], 2 * D2_IW * 4);
-        tma_load_2d(s_in + (2 * i) * D2_IW, map, x0 - 4, min(max(ry0 - 5 + i, 0), h - 1), &s_full[i]);
-        tma_load_2d(s_in + (2 * i + 1) * D2_IW, map, x0 - 4, min(max(ry0 + hs - 5 + i, 0), h - 1), &s_full[i]);
-      }
-    }
-    // columns this thread reads from a staged row (clamped to the image: cudaSiftD.cu:1764-1767)
-    const int ci0 = min(max(x0 - 4 + cl, 0), w - 1) - (x0 - 4);
-    const int ci1 = min(max(x0 - 4 + cl + 128, 0), w - 1) - (x0 - 4);
-    // horizontal role
-    const bool hact = cg < 31 && x0 + 8 * cg <= w - 1;    // this lane's 8 DoG columns start inside the image
-    const unsigned hmask = __ballot_sync(0xffffffffu, hact);
-    float kh[5], kv[4][5];                                // taps: this lane's scale (horizontal), this half's 4 scales (vertical)
-#pragma unroll
-    for (int j = 0; j < 5; j++) kh[j] = L.taps.k[hs_][j];
-#pragma unroll
-    for (int s = 0; s < 4; s++)
-#pragma unroll
-      for (int j = 0; j < 5; j++) kv[s][j] = L.taps.k[4 * half + s][j];
-    unsigned colok = 0;                                   // which of the 8 DoG columns may hold an extremum
-#pragma unroll
-    for (int d = 0; d < 8; d++) {
-      const int dc = 8 * cg + d;
-      if (dc >= 1 && dc <= D2_TESTED && x0 + dc <= w - 2) colok |= 1u << d;
-    }
-
-    f32x2 W0[9], W1[9];
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-      mbarrier_wait(&s_full[i], 0);
-      const float *ra = s_in + (2 * i) * D2_IW, *rb = ra + D2_IW;
-      W0[i] = pk2(ra[ci0], rb[ci0]);
-      W1[i] = pk2(ra[ci1], rb[ci1]);
-    }
-    W0[8] = 0ull; W1[8] = 0ull;
-    __syncthreads();                                      // every thread has read the prologue rows
-    if (tid == 0) {
-      for (int i = 0; i < D2_NS; i++) {
-        if (8 + i < nrows) {
-          mbarrier_expect_tx(&s_full[i], 2 * D2_IW * 4);
-          tma_load_2d(s_in + (2 * i) * D2_IW, map, x0 - 4, min(max(ry0 + 3 + i, 0), h - 1), &s_full[i]);
-          tma_load_2d(s_in + (2 * i + 1) * D2_IW, map, x0 - 4, min(max(ry0 + hs + 3 + i, 0), h - 1), &s_full[i]);
-        }
-      }
-    }
-
-    int ph = 8;                                           // window slot of the newest row: (8 + k) % 9
-    for (int k = 0; k <= nsteps; k++) {
-      const bool compute = k < nsteps;
-      const int q = k & 3;
-      if (compute) {
-        // ---------------------------------------------------------------- vertical pass
-        const int slot = k & (D2_NS - 1);
-        mbarrier_wait(&s_full[slot], ((8 + k) >> 3) & 1);
-        const float *ra = s_in + (2 * slot) * D2_IW, *rb = ra + D2_IW;
-        const f32x2 n0 = pk2(ra[ci0], rb[ci0]), n1 = pk2(ra[ci1], rb[ci1]);
-        float2 *vdst = s_v + (k & 1) * D2_VBUF2 + (4 * half) * D2_VROW2 + cl;
-#define D2_CASE(p) case p: d2_vertical<p>(W0, W1, n0, n1, kv, vdst); break;
-        switch (ph) {
-          D2_CASE(0) D2_CASE(1) D2_CASE(2) D2_CASE(3) D2_CASE(4) D2_CASE(5) D2_CASE(6) D2_CASE(7) D2_CASE(8)
-        }
-#undef D2_CASE
-        ph = (ph == 8) ? 0 : ph + 1;
-      }
-      __syncthreads();
-      if (tid == 0) {
-        s_cnt[(k + 1) & 3] = 0;                           // list of step k+1 (last read during step k-1)
-        const int slot = k & (D2_NS - 1);
-        if (compute && 16 + k < nrows) {                  // the slot just consumed: refill with the row 8 steps ahead
-          mbarrier_expect_tx(&s_full[slot], 2 * D2_IW * 4);
-          tma_load_2d(s_in + (2 * slot) * D2_IW, map, x0 - 4, min(max(ry0 + 11 + k, 0), h - 1), &s_full[slot]);
-          tma_load_2d(s_in + (2 * slot + 1) * D2_IW, map, x0 - 4, min(max(ry0 + hs + 11 + k, 0), h - 1), &s_full[slot]);
-        }
-      }
-      if (compute && hact) {
-        // -------------------------------------------------------------- horizontal pass + DoG
-        const float4 *src = reinterpret_cast<const float4 *>(s_v + (k & 1) * D2_VBUF2 + hs_ * D2_VROW2 + 8 * cg);
-        f32x2 V[16];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          const float4 t4 = src[j];
-          V[2 * j] = pk2(t4.x, t4.y);
-          V[2 * j + 1] = pk2(t4.z, t4.w);
-        }
-        f32x2 dg[8];
-#pragma unroll
-        for (int d = 0; d < 8; d++) {
-          const f32x2 o = d2_sym9(kh, V[d + 4], add2(V[d + 3], V[d + 5]), add2(V[d + 2], V[d + 6]),
-                                   add2(V[d + 1], V[d + 7]), add2(V[d], V[d + 8]));
-          const float2 of = upk(o);
-          const float plo = __shfl_up_sync(hmask, of.x, 1), phi = __shfl_up_sync(hmask, of.y, 1);
-          dg[d] = sub2(o, pk2(plo, phi));                 // blur[s] - blur[s-1]: DoG plane s-1 (cudaSiftD.cu:1790)
-        }
-        if (hs_ >= 1) {
-          float4 *dst = reinterpret_cast<float4 *>(s_ring + q * D2_RSLOTF + (hs_ - 1) * D2_RROWF + 16 * cg);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            const float2 a = upk(dg[2 * j]), b = upk(dg[2 * j + 1]);
-            dst[j] = make_float4(a.x, a.y, b.x, b.y);
-          }
-        }
-        if (hs_ >= 2 && hs_ <= 6 && k >= 1 && k <= hs) {  // planes 1..5, rows that are tested
-          float m = 0.0f;
-#pragma unroll
-          for (int d = 0; d < 8; d++) {
-            const float2 a = upk(dg[d]);
-            m = fmaxf(m, fmaxf(fabsf(a.x), fabsf(a.y)));
-          }
-          if (m > thresh) {
-            const bool okA = ry0 - 1 + k <= h - 2, okB = ry0 + hs - 1 + k <= h - 2;
-            unsigned bits = 0;
-#pragma unroll
-            for (int d = 0; d < 8; d++) {
-              const float2 a = upk(dg[d]);
-              if (okA && fabsf(a.x) > thresh) bits |= 1u << d;
-              if (okB && fabsf(a.y) > thresh) bits |= 0x100u << d;
-            }
-            bits &= colok | (colok << 8);
-            if (bits) {
-              int at = atomicAdd(&s_cnt[q], __popc(bits));
-              while (bits) {
-                const int b = __ffs(bits) - 1;
-                bits &= bits - 1;
-                if (at < D2_LCAP) s_list[q * 512 + at] = (unsigned short)((8 * cg + (b & 7)) | ((hs_ - 1) << 8) | ((b >> 3) << 11));
-                at++;
-              }
-            }
-          }
-        }
-      }
-      if (k >= 2) {
-        // -------------------------------------------------------------- extrema of step j = k - 2
-        const int j = k - 2, qj = j & 3;
-        int n = s_cnt[qj];
-        const bool scan = n > D2_LCAP;                    // list overflow: test every pixel of the row pair
-        if (scan) n = 2 * CS_NUM_SCALES * D2_TESTED;
-        const float *rm = s_ring + ((j + 3) & 3) * D2_RSLOTF, *r0 = s_ring + qj * D2_RSLOTF, *rp = s_ring + ((j + 1) & 3) * D2_RSLOTF;
-        for (int i = tid; i < n; i += D2_THREADS) {
-          int dc, p, hf;
-          if (!scan) {
-            const int e = s_list[qj * 512 + i];
-            dc = e & 255; p = (e >> 8) & 7; hf = e >> 11;
-          } else {
-            hf = i / (CS_NUM_SCALES * D2_TESTED);
-            const int r = i - hf * (CS_NUM_SCALES * D2_TESTED);
-            p = r / D2_TESTED;
-            dc = 1 + r - p * D2_TESTED;
-            p += 1;
-            const int gy_ = (hf ? ry0 + hs - 1 : ry0 - 1) + j;
-            if (j < 1 || j > hs || gy_ > h - 2 || x0 + dc > w - 2) continue;
-          }
-          const int o = p * D2_RROWF + 2 * dc + hf;
-          const float c = r0[o];
-          if (!(fabsf(c) > thresh)) continue;
-          float v[3][3][3];
-#pragma unroll
-          for (int pp = 0; pp < 3; pp++)
-#pragma unroll
-            for (int dx = 0; dx < 3; dx++) {
-              const int oo = o + (pp - 1) * D2_RROWF + 2 * (dx - 1);
-              v[pp][0][dx] = rm[oo];
-              v[pp][1][dx] = r0[oo];
-              v[pp][2][dx] = rp[oo];
-            }
-          bool mx = true, mn = true;
-#pragma unroll
-          for (int pp = 0; pp < 3; pp++)
-#pragma unroll
-            for (int dy = 0; dy < 3; dy++)
-#pragma unroll
-              for (int dx = 0; dx < 3; dx++)
-                if (pp != 1 || dy != 1 || dx != 1) { mx = mx && (c > v[pp][dy][dx]); mn = mn && (c < v[pp][dy][dx]); }
-          if (c > 0.0f ? mx : mn) {
-            const int gx = x0 + dc, gy = (hf ? ry0 + hs - 1 : ry0 - 1) + j;
-            const unsigned int tag = (unsigned)gx | ((unsigned)gy << 13) | ((unsigned)(p - 1) << 26) | ((unsigned)level << 29);
-            if (P.cells) {                                // extrema per 30x8 block and scale (reference cap, cudaSiftD.cu:1371)
-              const int cell = P.cellBase[level] + ((gy >> 3) * P.cellsX[level] + gx / 30) * CS_NUM_SCALES + (p - 1);
-              // no return value -> RED: the count is not on this thread's critical path; the fix-up kernel finds the
-              // cells that went past the limit by scanning the counters
-              atomicAdd(P.cells + (size_t)img * P.cellWords + (cell >> 2), 1u << (8 * (cell & 3)));
-            }
-            d2_refine(v, gx, gy, p - 1, L.subsampling, L.lowestScale, P.edgeLimit, P.factor, tag, s_kq, &s_kn, pts,
-                      &counters[0], P.maxPts);
-          }
-        }
-      }
-    }
-    __syncthreads();
-    {
-      const int nkq = min(s_kn, D2_KQ);
-      if (tid < nkq) d2_store_keypoint(pts, P.maxPts, atomicAdd(&counters[0], 1u), s_kq[tid]);
-    }
-    item = s_next;
-  }
-}
-
-// ================================================================================================
-// detect3: the same marching detector, warp-specialised.  One CTA of 16 warps per SM:
-//   warps 12-15 (producers): vertical pass of all 8 scales (thread = columns c and c+128, 9-row register
-//                           window, 40 taps in registers) and the TMA row ring -- the serial critical path, kept short
-//   warps 0-3 / 4-7 / 8-11 (consumer groups 0 / 1 / 2): horizontal pass + DoG + candidate flags of the steps
-//                           k = g mod 3 (2 x 16 column groups), then the extrema tests of row k-4; each group has
-//                           three steps of time for one step of work
-// The producers run ahead of the consumers through three vertical-result buffers (buffer = group); hand-over is by
-// named barriers (bar.arrive / bar.sync) instead of CTA-wide barriers:
-//   FULL[g]  producers -> group g: v[g] written        EMPTY[g] group g -> producers: v[g] is in registers
-//   DONE[g]  group g -> producers: the DoG row and the candidate list of its step are written (the extrema tests of
-//            an older row follow, off the producers' critical path)
-//   LATE[g]  group g -> producers: its previous step is complete, tests included (signalled at the start of the next step)
-//            The producers check DONE of step m-3 and LATE of step m-4 just before they signal FULL of step m.  Hence,
-//            when a group passes FULL of step k, every DoG row <= k-3 is written and every step <= k-4 of every group
-//            is complete: it may test the extrema of row k-4 (rows k-5..k-3) and overwrite ring slot k mod 8 (last
-//            read for rows k-9..k-7 in steps k-5, k-4 and -- by this same group -- k-3).
-// ================================================================================================
-// timing experiments (phase attribution, scripts/expbuild.sh -DD3_EXP=mask; results are wrong when set):
-// 1 no extrema tests, 2 no threshold flags / candidate lists, 4 no DoG ring stores, 8 no horizontal arithmetic and
-// shuffles (the loads stay), 16 no vertical arithmetic in the producers
-#ifndef D3_EXP
-#define D3_EXP 0
-#endif
-#ifndef D3_EXP_NOEXT
-#define D3_EXP_NOEXT (D3_EXP & 1)     // timing experiment only: no extrema tests
-#endif
 #define D3_THREADS 512
 #define D3_PT 128
 #define D3_RS 8
@@ -461,17 +172,10 @@ struct D3Item {
   int cellBase, cellsX, capLimit;
 };
 
-// Extrema of step j (DoG rows ry0-1+j / ry0+hs-1+j) by the 128 producer threads; rows j-1, j, j+1 are complete.
-#ifndef D3_EXT_INLINE
-#define D3_EXT_INLINE 1    // 1 = inlined, 0 = out of line
-#endif
-#if D3_EXT_INLINE
-__device__ __forceinline__
-#else
-__device__ __noinline__
-#endif
-void d3_extrema(const D3Item &I, int j, int pt, const float *s_ring, const unsigned short *s_list,
-                                        const int *s_cnt, D2Keypoint *s_kq, int *s_kn)
+// Extrema of step j (DoG rows ry0-1+j / ry0+hs-1+j) by the 128 threads of a consumer group; rows j-1, j, j+1 are
+// complete.
+__device__ __forceinline__ void d3_extrema(const D3Item &I, int j, int pt, const float *s_ring,
+                                           const unsigned short *s_list, const int *s_cnt, D2Keypoint *s_kq, int *s_kn)
 {
   const int qj = j & (D3_RS - 1);
   int n = s_cnt[qj];
@@ -534,7 +238,9 @@ void d3_extrema(const D3Item &I, int j, int pt, const float *s_ring, const unsig
       const unsigned int tag = (unsigned)gx | ((unsigned)gy << 13) | ((unsigned)(p - 1) << 26) | ((unsigned)I.level << 29);
       if (I.cells) {                                // extrema per 30x8 block and scale (reference cap, cudaSiftD.cu:1371)
         const int cell = I.cellBase + ((gy >> 3) * I.cellsX + gx / 30) * CS_NUM_SCALES + (p - 1);
-        atomicAdd(I.cells + (cell >> 2), 1u << (8 * (cell & 3)));     // RED (see detect2_kernel)
+        // no return value -> RED: the count is not on this thread's critical path; the fix-up kernel finds the
+        // cells that went past the limit by scanning the counters
+        atomicAdd(I.cells + (cell >> 2), 1u << (8 * (cell & 3)));
       }
       d2_refine(v, gx, gy, p - 1, I.subsampling, I.lowestScale, I.edgeLimit, I.factor, tag, s_kq, s_kn, I.pts,
                 &I.counters[0], I.maxPts);
@@ -550,11 +256,6 @@ __device__ __forceinline__ void d3_vertical(f32x2 (&W0)[9], f32x2 (&W1)[9], f32x
 #define D3_WI(i) ((PH + 1 + (i)) % 9)
   W0[PH] = n0;
   W1[PH] = n1;
-  if (D3_EXP & 16) {
-#pragma unroll
-    for (int s = 0; s < CS_LAPLACE_S; s++) { vdst[s * D2_VROW2] = upk(W0[D3_WI(4)]); vdst[s * D2_VROW2 + 128] = upk(W1[D3_WI(4)]); }
-    return;
-  }
   {
     const f32x2 c = W0[D3_WI(4)];
     const f32x2 p1 = add2(W0[D3_WI(3)], W0[D3_WI(5)]), p2 = add2(W0[D3_WI(2)], W0[D3_WI(6)]);
@@ -754,14 +455,13 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
           f32x2 dg[8];
 #pragma unroll
           for (int d = 0; d < 8; d++) {
-            if (D3_EXP & 8) { dg[d] = add2(V[d + 4], V[d + 8]); continue; }
             const f32x2 o = d2_sym9(kh, V[d + 4], add2(V[d + 3], V[d + 5]), add2(V[d + 2], V[d + 6]),
                                     add2(V[d + 1], V[d + 7]), add2(V[d], V[d + 8]));
             const float2 of = upk(o);
             const float plo = __shfl_up_sync(0xffffffffu, of.x, 1), phi = __shfl_up_sync(0xffffffffu, of.y, 1);
             dg[d] = sub2(o, pk2(plo, phi));                 // blur[s] - blur[s-1]: DoG plane s-1 (cudaSiftD.cu:1790)
           }
-          if (!(D3_EXP & 4) && act && hs_ >= 1) {
+          if (act && hs_ >= 1) {
             float4 *dst = reinterpret_cast<float4 *>(rdst0 + q * D2_RSLOTF + 256 * pass);
 #pragma unroll
             for (int j = 0; j < 4; j++) {
@@ -775,7 +475,7 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
             const float2 a = upk(dg[d]);
             m = fmaxf(m, fmaxf(fabsf(a.x), fabsf(a.y)));
           }
-          if (!(D3_EXP & 2) && m > thresh && rowsTested && act) {
+          if (m > thresh && rowsTested && act) {
             unsigned bits = 0, colok = 0;
 #pragma unroll
             for (int d = 0; d < 8; d++) {
@@ -806,8 +506,8 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
           }
         }
         nb_arrive(NB_DONE + g, 2 * D3_PT);                       // row k and its candidate list are written
-        // rows k-5..k-3 are complete; the call (out of line: registers) only when the row has candidates at all
-        if (!D3_EXP_NOEXT && k >= 5 && s_cnt[(k - 4) & (D3_RS - 1)] != 0) d3_extrema(I, k - 4, tig, s_ring, s_list, s_cnt, s_kq, &s_kn);
+        // rows k-5..k-3 are complete; the tests run only when the row has candidates at all
+        if (k >= 5 && s_cnt[(k - 4) & (D3_RS - 1)] != 0) d3_extrema(I, k - 4, tig, s_ring, s_list, s_cnt, s_kq, &s_kn);
       }
     }
     __syncthreads();
@@ -837,7 +537,6 @@ int detect2_init_device()
 }
 
 static int g_d2_configured[64];
-int g_d2_variant = 2;     // tuning: 2 = warp-specialised detect3 (default); 0 / 1 = detect2 with 2 / 1 CTAs per SM
 
 int launch_detect2(const Detect2Params &p, int sms, cudaStream_t st)
 {
@@ -845,22 +544,11 @@ int launch_detect2(const Detect2Params &p, int sms, cudaStream_t st)
   int dev = 0;
   CS_CUDA(cudaGetDevice(&dev));
   if (dev < 64 && !g_d2_configured[dev]) {      // per device: cudaFuncSetAttribute applies to the current device only
-    CS_CUDA(cudaFuncSetAttribute(detect2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, D2_SMEM_BYTES));
-    CS_CUDA(cudaFuncSetAttribute(detect2_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, D2_SMEM_BYTES));
     CS_CUDA(cudaFuncSetAttribute(detect3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, D3_SMEM_BYTES));
     g_d2_configured[dev] = 1;
   }
-  if (g_d2_variant == 2) {
-    const int grid3 = p.numItems < sms ? p.numItems : sms;
-    detect3_kernel<<<grid3, D3_THREADS, D3_SMEM_BYTES, st>>>(p);
-    count_launch();
-    CS_CUDA(cudaGetLastError());
-    return 0;
-  }
-  const int per = g_d2_variant == 1 ? 1 : 2;
-  const int grid = p.numItems < per * sms ? p.numItems : per * sms;
-  if (g_d2_variant == 1) detect2_kernel<1><<<grid, D2_THREADS, D2_SMEM_BYTES, st>>>(p);
-  else detect2_kernel<2><<<grid, D2_THREADS, D2_SMEM_BYTES, st>>>(p);
+  const int grid = p.numItems < sms ? p.numItems : sms;
+  detect3_kernel<<<grid, D3_THREADS, D3_SMEM_BYTES, st>>>(p);
   count_launch();
   CS_CUDA(cudaGetLastError());
   return 0;

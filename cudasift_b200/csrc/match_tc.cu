@@ -99,7 +99,9 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
 struct TcPlan {
   int n1, n2v, n_mt, n_nt, total, U, runs, grid;
   // experiments (env CS_TC_DBG, results are wrong when set): 1 = B tiles are not reloaded, 2 = MMAs without
-  // the top-3 update
+  // the top-3 update.  The bit-2 branch in t3_gemm_kernel also keeps the top-3 update below the consumers' release
+  // of the B stage: without it, ptxas moves part of the update above that arrive.  Pin the order explicitly before
+  // this field goes.
   int dbg;
 };
 // slot of (cta, run, row-in-tile)

@@ -44,6 +44,6 @@ struct Pipeline2 {
 };
 
 void build_detector_items(const int *lw, const int *lh, int numLevels, int n, int hs, std::vector<uint4> &v);
-extern int g_d2_hs, g_pa_rows, g_cap32, g_cap_limit, g_d2_variant, g_sd_split;
+extern int g_d2_hs, g_pa_rows, g_cap32, g_cap_limit, g_sd_split;
 
 }  // namespace cs

@@ -36,8 +36,8 @@ unsigned long long cs_launch_count(void);
 /* Tuning hook (benchmarks and tests only).  Keys: "legacy" (1 = the round-1 per-image kernels for pipelines
  * created afterwards, 0 = the batched TMA pipeline), "cap32" (0 = do not reproduce the reference's cap of 32
  * extrema per 30x8 block and scale, cudaSiftD.cu:1371), "d2_hs" / "pa_rows" (rows per detector stream / per CTA
- * of the first pyramid kernel, 0 = automatic), "detect_variant" / "detect_skip" (legacy detector).
- * Returns 0, or CS_E_ARG for an unknown key. */
+ * of the first pyramid kernel, 0 = automatic), "sd_split" (0 = every ScaleDown of a batch in the chain kernel),
+ * "cap32_limit" (the cap's limit, 1..199; default 32).  Returns 0, or CS_E_ARG for an unknown key. */
 int cs_set_tuning(const char *key, int value);
 /* Number of launches one steady-state cs_extractor_submit_* / cs_match issues. */
 int cs_extract_launches_per_image(int numOctaves, int scaleUp);

@@ -11,7 +11,7 @@ cis = []
 for i in range(32):
     ci = cs.CudaImage().Allocate(w, h, pitch, False, None, imgs[i % 8]); ci.Download(); cis.append(ci)
 ptrs = [c.d_data for c in cis]
-keys = sys.argv[1:] or ["d2_variant=0", "d2_variant=1"]
+keys = sys.argv[1:] or ["d2_hs=0"]
 for spec in keys:
     for kv in spec.split(","):
         k, v = kv.split("="); cs.set_tuning(k, int(v))

@@ -1,4 +1,4 @@
-"""Kernel-variant check: records of detector variants must be identical (same set, bit for bit).
+"""Tuning-settings check: records extracted under different tuning settings must be identical (same set, bit for bit).
 usage: variant_check.py key=a key=b ...   (first is the baseline)"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -164,27 +164,6 @@ def test_extractor_pipeline_and_u8_upload(cs):
     ex.close()
 
 
-def test_detector_variants_identical(cs):
-    """Every compiled detector configuration (CTA size, columns per horizontal task, row pairs per
-    vertical task) produces the same keypoints, bit for bit: tiling must not influence the results."""
-    arr = synth_image(1000, 700, seed=21)
-    L = cs.lib()
-    try:
-        assert L.cs_set_tuning(b"detect_variant", 0) == 0
-        base = canon(_extract(cs, arr, thresh=2.0))
-        assert len(base) > 500
-        for v in range(1, 8):
-            assert L.cs_set_tuning(b"detect_variant", v) == 0
-            got = canon(_extract(cs, arr, thresh=2.0))
-            assert len(got) == len(base), v
-            for f in ("xpos", "ypos", "scale", "sharpness", "edgeness", "orientation", "subsampling"):
-                assert np.array_equal(got[f], base[f]), (v, f)
-            assert np.array_equal(got["data"], base["data"]), v
-    finally:
-        L.cs_set_tuning(b"detect_variant", 0)
-    assert L.cs_set_tuning(b"no_such_key", 1) < 0
-
-
 def test_dense_candidates_low_threshold(cs):
     """thresh close to 0 flags almost every pixel: the thread-per-item extrema path, the keypoint queue
     overflow path and the maxPts clamp are all exercised; counts agree with the oracle."""

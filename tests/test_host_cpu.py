@@ -88,6 +88,8 @@ def test_new_abi_symbols_present():
         assert hasattr(L, name), name
     assert L.cs_max_batch() == 32
     assert L.cs_set_tuning(b"cap32_limit", 32) == 0 and L.cs_set_tuning(b"legacy", 0) == 0
+    for key in (b"no_such_key", b"detect_variant", b"detect_skip", b"d2_variant"):   # no longer tuning keys
+        assert L.cs_set_tuning(key, 1) < 0, key
 
 
 def test_demo_png_decoder_matches_opencv(tmp_path):
