@@ -15,7 +15,7 @@ from . import build as _build
 
 __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData", "InitSiftData", "FreeSiftData",
            "AllocSiftTempMemory", "FreeSiftTempMemory", "ExtractSift", "MatchSiftData", "FindHomography", "Extractor",
-           "CudaSiftError", "extract_host", "match_host"]
+           "CudaSiftError", "extract_host", "match_host", "rank_records"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -96,6 +96,9 @@ def lib():
         "cs_extractor_device_points": (vp, [vp]),
         "cs_extractor_host_points": (vp, [vp]),
         "cs_extractor_host_image": (vp, [vp]),
+        "cs_extractor_create_ranked": (vp, [ip, ip, ip, ip, ip, ip, ip]),
+        "cs_extractor_candidates": (ip, [vp, ip]),
+        "cs_rank_records": (ip, [vp, ip, vp, ip]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -294,18 +297,48 @@ def match_host(s1, s2, mode=0):
     return s1, ms.value
 
 
+def rank_records(records, n):
+    """The ranking stage on host records: the min(n, len(records)) records with the largest |sharpness|, sorted by
+    (|sharpness| descending, subsampling, ypos, xpos, scale, orientation); ranked on the device."""
+    records = np.ascontiguousarray(records, SIFT_DTYPE)
+    n = int(n)
+    if n < 1:
+        raise ValueError("n must be >= 1")
+    if len(records) == 0:
+        return records.copy()
+    d_in, d_out = DeviceBuffer(records.nbytes), DeviceBuffer(min(n, len(records)) * SIFT_DTYPE.itemsize)
+    try:
+        d_in.upload(records)
+        k = _check(lib().cs_rank_records(d_in.ptr, len(records), d_out.ptr, n), "cs_rank_records")
+        return d_out.download(SIFT_DTYPE, k)
+    finally:
+        d_in.free()
+        d_out.free()
+
+
 def set_tuning(key, value):
     return _check(lib().cs_set_tuning(key.encode(), int(value)), "cs_set_tuning")
 
 
 class Extractor:
     """Pipelined extractor (one CUDA stream + arena + result buffers for up to `batch` images per submit);
-    see cudasift_b200.h."""
+    see cudasift_b200.h.  maxCandidates=None: plain extractor (slot = the first maxPts records found, in no set
+    order).  An integer >= maxPts: ranked extractor, each slot holds the maxPts records with the largest |sharpness|
+    out of up to maxCandidates found, in a fixed order (cs_extractor_create_ranked)."""
 
-    def __init__(self, width, height, numOctaves=5, maxPts=32768, scaleUp=False, batch=1):
-        self.w, self.h, self.maxPts, self.batch = width, height, maxPts, batch
-        self.handle = _check(lib().cs_extractor_create_batch(width, height, numOctaves, maxPts, int(scaleUp), batch),
-                             "cs_extractor_create_batch")
+    def __init__(self, width, height, numOctaves=5, maxPts=32768, scaleUp=False, batch=1, maxCandidates=None):
+        self.handle = None
+        self.w, self.h, self.maxPts, self.batch, self.maxCandidates = width, height, maxPts, batch, maxCandidates
+        if maxCandidates is None:
+            self.handle = _check(lib().cs_extractor_create_batch(width, height, numOctaves, maxPts, int(scaleUp), batch),
+                                 "cs_extractor_create_batch")
+        else:
+            self.handle = _check(lib().cs_extractor_create_ranked(width, height, numOctaves, maxPts, int(scaleUp), batch,
+                                                                  int(maxCandidates)), "cs_extractor_create_ranked")
+
+    def candidates(self, slot):
+        """Records found for image `slot` in the last wait; == maxCandidates: the candidate area overflowed."""
+        return lib().cs_extractor_candidates(self.handle, slot)
 
     # ---- batches: one launch per stage for n images ----
     def submit_device_batch(self, d_imgs, pitch, initBlur=1.0, thresh=3.0, lowestScale=0.0):

@@ -25,7 +25,7 @@ REF_DIR = os.path.join(ORACLE_DIR, "_ref")
 REF_LIB = os.path.join(REF_DIR, "libcudasift_ref.so")
 
 SOURCES = ["api.cu", "pipeline2.cu", "pyramid.cu", "pyramid2.cu", "detect.cu", "detect2.cu", "cap32.cu", "describe.cu",
-           "match.cu", "match_tc.cu", "homography.cu", "geom.cu"]
+           "match.cu", "match_tc.cu", "homography.cu", "geom.cu", "rank.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared"]
 

@@ -287,8 +287,8 @@ struct DeviceCtx {
   unsigned int *h_counters = nullptr;      // pinned
   unsigned long long matchStats[4] = {0, 0, 0, 0};
   // scratch for *_host entry points
-  void *scratch[4] = {nullptr, nullptr, nullptr, nullptr};
-  size_t scratchBytes[4] = {0, 0, 0, 0};
+  void *scratch[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // 4: cs_rank_records
+  size_t scratchBytes[5] = {0, 0, 0, 0, 0};
 
   int ensure(int d)
   {
@@ -948,7 +948,10 @@ struct cs_extractor {
   Pipeline pipe;         // legacy per-image kernels (B == 1)
   Pipeline2 pipe2;       // batched TMA pipeline
   float *d_img;          // B staging images
-  SiftPoint *d_pts;      // B x maxPts records
+  SiftPoint *d_pts;      // B x maxPts records (ranked: the output slots)
+  int maxCand;           // ranked extractors: candidate records per image (0: plain extractor)
+  SiftPoint *d_cand;     // ranked: B x maxCand records, written by the pipeline as d_pts is for a plain extractor
+  unsigned int *d_rank;  // ranked: B x rank_scratch_words(maxCand)
   float *h_img;          // pinned, B x w x h
   uint8_t *d_u8;         // device staging for 8-bit uploads (lazily allocated)
   SiftPoint *h_pts;      // pinned, B x maxPts
@@ -956,6 +959,7 @@ struct cs_extractor {
   bool hostResults;
   int lastN;
   int lastCounts[CS_MAX_BATCH];
+  int lastCand[CS_MAX_BATCH];   // records found per image (ranked: in the candidate area)
   // CUDA graph of one steady-state submit (memset + kernels + count D2H).  Per image only the input pointer
   // changes: legacy = first parameter of the LowPass node, batched = the tensor maps in the parameters of the
   // first pyramid kernel; both are patched with cudaGraphExecKernelNodeSetParams.
@@ -989,7 +993,15 @@ static int extractor_enqueue(cs_extractor *ex, int n, const float *const *d_imgs
     if (r < 0) return r;
     CS_CUDA(cudaMemcpyAsync(ex->h_counters, ex->pipe.d_counters, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, ex->stream));
   } else {
-    r = ex->pipe2.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_pts, ex->maxPts, ex->maxPts, ex->stream, ev, paOut);
+    if (ex->maxCand > 0) {
+      RankParams rp;
+      memset(&rp, 0, sizeof(rp));
+      rp.out = ex->d_pts; rp.outStride = ex->maxPts; rp.maxOut = ex->maxPts; rp.scratch = ex->d_rank;
+      r = ex->pipe2.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_cand, ex->maxCand, ex->maxCand, ex->stream,
+                            ev, paOut, &rp);
+    } else {
+      r = ex->pipe2.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_pts, ex->maxPts, ex->maxPts, ex->stream, ev, paOut);
+    }
     if (r < 0) return r;
     CS_CUDA(cudaMemcpyAsync(ex->h_counters, ex->pipe2.d_state, (size_t)n * CS_CNT_STRIDE * sizeof(unsigned int),
                             cudaMemcpyDeviceToHost, ex->stream));
@@ -1040,7 +1052,7 @@ static int extractor_capture(cs_extractor *ex, int n, const float *const *d_imgs
   return 0;
 }
 
-cs_extractor *cs_extractor_create_batch(int w, int h, int numOctaves, int maxPts, int scaleUp, int batch)
+static cs_extractor *extractor_create(int w, int h, int numOctaves, int maxPts, int scaleUp, int batch, int maxCand)
 {
   if (batch < 1 || batch > CS_MAX_BATCH) { set_error("cs_extractor_create_batch: batch %d out of range (1..%d)", batch, CS_MAX_BATCH); return nullptr; }
   cs_extractor *ex = new cs_extractor();
@@ -1056,6 +1068,14 @@ cs_extractor *cs_extractor_create_batch(int w, int h, int numOctaves, int maxPts
   else ok = ok && ex->pipe2.init(w, h, numOctaves, scaleUp != 0, batch, nullptr) == 0;
   ok = ok && cudaMalloc((void **)&ex->d_img, (size_t)batch * ex->pitch * h * sizeof(float)) == cudaSuccess;
   ok = ok && cudaMalloc((void **)&ex->d_pts, (size_t)batch * maxPts * sizeof(SiftPoint)) == cudaSuccess;
+  // the pipeline leaves some fields of a record unwritten (score, match*, empty[1..2]): make them zero, not stale memory
+  ok = ok && cudaMemset(ex->d_pts, 0, (size_t)batch * maxPts * sizeof(SiftPoint)) == cudaSuccess;
+  if (maxCand > 0) {
+    ex->maxCand = maxCand;
+    ok = ok && cudaMalloc((void **)&ex->d_cand, (size_t)batch * maxCand * sizeof(SiftPoint)) == cudaSuccess;
+    ok = ok && cudaMemset(ex->d_cand, 0, (size_t)batch * maxCand * sizeof(SiftPoint)) == cudaSuccess;
+    ok = ok && cudaMalloc((void **)&ex->d_rank, (size_t)batch * rank_scratch_words(maxCand) * sizeof(unsigned int)) == cudaSuccess;
+  }
   ok = ok && cudaMallocHost((void **)&ex->h_img, (size_t)batch * w * h * sizeof(float)) == cudaSuccess;
   ok = ok && cudaMallocHost((void **)&ex->h_pts, (size_t)batch * maxPts * sizeof(SiftPoint)) == cudaSuccess;
   ok = ok && cudaMallocHost((void **)&ex->h_counters, (size_t)batch * CS_CNT_STRIDE * sizeof(unsigned int)) == cudaSuccess;
@@ -1065,6 +1085,26 @@ cs_extractor *cs_extractor_create_batch(int w, int h, int numOctaves, int maxPts
     return nullptr;
   }
   return ex;
+}
+
+cs_extractor *cs_extractor_create_batch(int w, int h, int numOctaves, int maxPts, int scaleUp, int batch)
+{
+  return extractor_create(w, h, numOctaves, maxPts, scaleUp, batch, 0);
+}
+
+// Argument checks come before any CUDA call (they hold on a machine without a device).
+cs_extractor *cs_extractor_create_ranked(int w, int h, int numOctaves, int maxPts, int scaleUp, int batch, int maxCandidates)
+{
+  if (maxPts < 1 || maxCandidates < maxPts || maxCandidates > CS_RANK_MAX_IN) {
+    set_error("cs_extractor_create_ranked: invalid argument (CS_E_ARG): need 1 <= maxPts (%d) <= maxCandidates (%d) <= %d",
+              maxPts, maxCandidates, CS_RANK_MAX_IN);
+    return nullptr;
+  }
+  if (legacy_mode()) {
+    set_error("cs_extractor_create_ranked: invalid argument (CS_E_ARG): ranking runs on the batched pipeline only (legacy is set)");
+    return nullptr;
+  }
+  return extractor_create(w, h, numOctaves, maxPts, scaleUp, batch, maxCandidates);
 }
 
 cs_extractor *cs_extractor_create(int w, int h, int numOctaves, int maxPts, int scaleUp)
@@ -1082,6 +1122,8 @@ int cs_extractor_destroy(cs_extractor *ex)
   if (ex->d_img) cudaFree(ex->d_img);
   if (ex->d_u8) cudaFree(ex->d_u8);
   if (ex->d_pts) cudaFree(ex->d_pts);
+  if (ex->d_cand) cudaFree(ex->d_cand);
+  if (ex->d_rank) cudaFree(ex->d_rank);
   if (ex->h_img) cudaFreeHost(ex->h_img);
   if (ex->h_pts) cudaFreeHost(ex->h_pts);
   if (ex->h_counters) cudaFreeHost(ex->h_counters);
@@ -1183,7 +1225,15 @@ int cs_extractor_wait_batch(cs_extractor *ex, int *counts)
   int total = 0;
   bool copies = false;
   for (int i = 0; i < n; i++) {
-    const int c = count_from_counters(ex->h_counters + (size_t)i * CS_CNT_STRIDE, ex->maxPts);
+    const unsigned int *hc = ex->h_counters + (size_t)i * CS_CNT_STRIDE;
+    int c;
+    if (ex->maxCand > 0) {                       // ranked: [2] = records in the output slot
+      c = (int)(hc[2] < (unsigned)ex->maxPts ? hc[2] : (unsigned)ex->maxPts);
+      ex->lastCand[i] = count_from_counters(hc, ex->maxCand);
+    } else {
+      c = count_from_counters(hc, ex->maxPts);
+      ex->lastCand[i] = c;
+    }
     ex->lastCounts[i] = c;
     if (counts) counts[i] = c;
     total += c;
@@ -1203,15 +1253,16 @@ int cs_extractor_profile_batch(cs_extractor *ex, int n, const float *const *d_im
                                float lowestScale, float out_ms[5])
 {
   if (n < 1 || n > ex->B) { set_error("cs_extractor_profile: bad batch"); return CS_E_ARG; }
-  cudaEvent_t ev[5];
-  for (int i = 0; i < 5; i++) CS_CUDA(cudaEventCreate(&ev[i]));
+  const int ne = ex->maxCand > 0 ? 6 : 5;       // ranked: one more event, after the ranking stage
+  cudaEvent_t ev[6];
+  for (int i = 0; i < ne; i++) CS_CUDA(cudaEventCreate(&ev[i]));
   ex->lastN = n;
   int r = extractor_enqueue(ex, n, d_imgs, pitch, initBlur, thresh, lowestScale, ev, nullptr);
-  if (r < 0) { for (int i = 0; i < 5; i++) cudaEventDestroy(ev[i]); return r; }
+  if (r < 0) { for (int i = 0; i < ne; i++) cudaEventDestroy(ev[i]); return r; }
   CS_CUDA(cudaStreamSynchronize(ex->stream));
   for (int i = 0; i < 4; i++) cudaEventElapsedTime(&out_ms[i], ev[i], ev[i + 1]);
-  cudaEventElapsedTime(&out_ms[4], ev[0], ev[4]);
-  for (int i = 0; i < 5; i++) cudaEventDestroy(ev[i]);
+  cudaEventElapsedTime(&out_ms[4], ev[0], ev[ne - 1]);
+  for (int i = 0; i < ne; i++) cudaEventDestroy(ev[i]);
   ex->hostResults = false;
   return cs_extractor_wait_batch(ex, nullptr);
 }
@@ -1242,6 +1293,39 @@ int cs_extractor_read_level(cs_extractor *ex, int slot, int level, float *h_out)
 }
 
 int cs_extractor_count(cs_extractor *ex, int slot) { return (slot >= 0 && slot < CS_MAX_BATCH) ? ex->lastCounts[slot] : 0; }
+int cs_extractor_candidates(cs_extractor *ex, int slot) { return (slot >= 0 && slot < CS_MAX_BATCH) ? ex->lastCand[slot] : 0; }
+
+int cs_rank_records(const void *d_in, int n, void *d_out, int maxOut)
+{
+  if (n < 0 || n > CS_RANK_MAX_IN || maxOut < 1 || (n > 0 && (!d_in || !d_out)) ||
+      ((reinterpret_cast<uintptr_t>(d_in) | reinterpret_cast<uintptr_t>(d_out)) & 15) != 0) {
+    set_error("cs_rank_records: need 0 <= n (%d) <= %d, maxOut (%d) >= 1 and 16-byte aligned record arrays", n, CS_RANK_MAX_IN, maxOut);
+    return CS_E_ARG;
+  }
+  if (n == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  void *buf = nullptr;
+  const size_t words = CS_CNT_STRIDE + rank_scratch_words(n);   // counters | scratch
+  int r = c->get_scratch(4, words * sizeof(unsigned int), &buf);
+  if (r < 0) return r;
+  unsigned int *cnt = (unsigned int *)buf;
+  const unsigned int init[CS_CNT_STRIDE] = {(unsigned)n, (unsigned)n, 0u, 0u};
+  CS_CUDA(cudaMemcpyAsync(cnt, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
+  RankParams rp;
+  memset(&rp, 0, sizeof(rp));
+  rp.in = (const SiftPoint *)d_in; rp.maxIn = n;
+  rp.out = (SiftPoint *)d_out; rp.maxOut = maxOut;
+  rp.counters = cnt; rp.scratch = cnt + CS_CNT_STRIDE;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if ((r = launch_rank(rp, 1, sms, c->stream)) < 0) return r;
+  CS_CUDA(cudaMemcpyAsync(c->h_counters, cnt, CS_CNT_STRIDE * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+  CS_CUDA(cudaStreamSynchronize(c->stream));
+  return (int)c->h_counters[2];
+}
 
 // ---- device timers (CUDA events on the extractor's own stream) ----
 void *cs_event_create(void)

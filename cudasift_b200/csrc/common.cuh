@@ -172,6 +172,24 @@ int launch_tex_probe(cudaTextureObject_t tex, const float *xs, const float *ys, 
 
 int make_texture(cudaTextureObject_t *tex, const float *img, int w, int h, int pitch);
 
+// ---- ranking (rank.cu): per image the maxOut candidates with the largest |sharpness|, in key order ---------------
+#define CS_RANK_MAX_IN (1 << 18)    // largest candidate count per image
+#define CS_RANK_SCRATCH_PER_IN 9    // scratch words per candidate
+struct RankParams {
+  const SiftPoint *in; long long inStride;   // image i: candidates in + i * inStride, count read from its counters
+  SiftPoint *out; long long outStride;       // image i: min(maxOut, found) records in rank order
+  unsigned int *counters;                    // image i: counters + i * CS_CNT_STRIDE; [2] receives the output count
+  unsigned int *scratch;                     // image i: scratch + i * rank_scratch_words(maxIn)
+  int maxIn, maxOut;
+};
+// per image: [maxIn] primary keys | [7][maxIn] survivors' keys and candidate index | [maxIn] survivors' ranks
+// | survivor count (4 words)
+__host__ __device__ inline size_t rank_scratch_words(int maxIn)
+{
+  return (size_t)maxIn * CS_RANK_SCRATCH_PER_IN + 4;
+}
+int launch_rank(const RankParams &p, int batch, int sms, cudaStream_t st);
+
 // ---- matcher ------------------------------------------------------------------------
 struct MatchWorkspace;   // opaque, owned by the per-device context
 int match_exact(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st);

@@ -1,6 +1,6 @@
 // pipeline2.cu -- host side of the batched extraction pipeline: one stream-ordered sequence of
 //   [ScaleUp] -> pyr_lowpass_sd (TMA) -> pyr_chain -> detect2 (TMA, all octaves, all images) -> cap32 fix-up
-//   -> describe (all octaves, all images) [-> rescale]
+//   -> describe (all octaves, all images) [-> rescale] [-> rank (ranked extractors)]
 // for 1..CS_MAX_BATCH images of one size.  Replaces the reference's per-image loop (mainSift.cpp:65-69 around
 // cudaSiftH.cu:72-144); the drop-in ExtractSift is the batch-of-one case.
 #include "common.cuh"
@@ -254,7 +254,7 @@ int Pipeline2::fill_pyr_a(PyrAParams &pa, int n, const float *const *d_imgs, int
 
 int Pipeline2::enqueue(int n, const float *const *d_imgs, int pitch, double initBlur, float thresh, float lowestScale,
                        SiftPoint *d_pts, long long ptsStride, int maxPts, cudaStream_t st, cudaEvent_t *ev,
-                       PyrAParams *paOut)
+                       PyrAParams *paOut, const RankParams *rank)
 {
   int r;
   if (n < 1 || n > B) { set_error("batch of %d images on a pipeline built for %d", n, B); return CS_E_ARG; }
@@ -341,6 +341,13 @@ int Pipeline2::enqueue(int n, const float *const *d_imgs, int pitch, double init
     for (int b = 0; b < n; b++)
       if ((r = launch_rescale(d_pts + (size_t)b * ptsStride, d_counters + (size_t)b * CS_CNT_STRIDE, maxPts, 0.5f, st)) < 0) return r;
   if (ev) cudaEventRecord(ev[4], st);
+  if (rank) {
+    RankParams rp = *rank;
+    rp.in = d_pts; rp.inStride = ptsStride; rp.maxIn = maxPts; rp.counters = d_counters;
+    if ((r = launch_rank(rp, n, sms, st)) < 0) return r;
+    if ((r = debug_stage(st, "rank")) < 0) return r;
+    if (ev) cudaEventRecord(ev[5], st);
+  }
   return 0;
 }
 

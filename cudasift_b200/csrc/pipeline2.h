@@ -38,9 +38,11 @@ struct Pipeline2 {
   // d_pts + i * ptsStride and its counters to counters(i).  ev (optional): 5 events at the stage boundaries
   // (start, after the level-0/1 kernel, after the chain, after detect, after describe).  paOut (optional)
   // receives the parameters of the first kernel (its tensor maps are the only per-call state of a captured graph).
+  // rank (optional): d_pts is then the candidate area, and the ranking stage (rank.cu) writes each image's
+  // rank->maxOut strongest records to rank->out + i * rank->outStride (ev: one more event, after ranking).
   int enqueue(int n, const float *const *d_imgs, int pitch, double initBlur, float thresh, float lowestScale,
               SiftPoint *d_pts, long long ptsStride, int maxPts, cudaStream_t st, cudaEvent_t *ev = nullptr,
-              PyrAParams *paOut = nullptr);
+              PyrAParams *paOut = nullptr, const RankParams *rank = nullptr);
 };
 
 void build_detector_items(const int *lw, const int *lh, int numLevels, int n, int hs, std::vector<uint4> &v);

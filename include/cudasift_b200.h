@@ -153,7 +153,28 @@ int cs_extractor_count(cs_extractor *ex, int slot);
 void *cs_extractor_device_points_at(cs_extractor *ex, int slot);
 void *cs_extractor_host_points_at(cs_extractor *ex, int slot);
 float *cs_extractor_host_image_at(cs_extractor *ex, int slot);
-/* Stage times of one batch (see cs_extractor_profile); returns the sum of the counts. */
+/* ---- ranked batch extraction: a fixed feature budget per image, in a fixed order ----
+ * Each image's slot receives the min(maxPts, found) records with the largest |sharpness|, sorted by the rank key
+ * (|sharpness| descending, then subsampling, ypos, xpos, scale, orientation ascending; numpy:
+ * lexsort((orientation, scale, xpos, ypos, subsampling, -abs(sharpness)))).  They are, byte for byte, the first
+ * maxPts records of a plain extractor's output (maxPts = maxCandidates) sorted by that key, whatever order the
+ * detector's atomics left them in.  The pipeline writes up to maxCandidates records per image into a candidate area;
+ * the ranking stage selects on the device and only the output records cross PCIe after a host submit.
+ * Requires 1 <= maxPts <= maxCandidates <= 262144 and the batched pipeline (not cs_set_tuning("legacy", 1));
+ * otherwise returns NULL and cs_last_error() names the invalid argument (CS_E_ARG), before any CUDA call.
+ * maxPts == maxCandidates returns every record in the fixed order.  cs_extractor_wait_batch returns the ranked
+ * counts; cs_extractor_device_points_at / host_points_at address the output slots. */
+cs_extractor *cs_extractor_create_ranked(int width, int height, int numOctaves, int maxPts, int scaleUp, int batch,
+                                         int maxCandidates);
+/* Records found for image `slot` in the last wait (ranked: in the candidate area).  A value equal to maxCandidates
+ * means the candidate area overflowed: the output is still sorted, but it is a subset that may depend on atomic
+ * order rather than the strongest maxPts records. */
+int cs_extractor_candidates(cs_extractor *ex, int slot);
+/* The ranking stage on its own: d_out (device, must not overlap d_in) receives the min(n, maxOut) records of d_in
+ * (n device records) with the smallest rank key, in key order.  Synchronous; returns the number written. */
+int cs_rank_records(const void *d_in, int n, void *d_out, int maxOut);
+/* Stage times of one batch (see cs_extractor_profile); returns the sum of the counts.  For a ranked extractor the
+ * total (out_ms[4]) includes the ranking stage, which runs after describe: ranking = total - out_ms[0..3]. */
 int cs_extractor_profile_batch(cs_extractor *ex, int n, const float *const *d_imgs, int pitch, double initBlur,
                                float thresh, float lowestScale, float out_ms[5]);
 /* Host logic of the batched detector (no device needed; tests): its work list for n images -- per item 4 ints
