@@ -15,7 +15,7 @@ from . import build as _build
 
 __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData", "InitSiftData", "FreeSiftData",
            "AllocSiftTempMemory", "FreeSiftTempMemory", "ExtractSift", "MatchSiftData", "FindHomography", "Extractor",
-           "CudaSiftError", "extract_host", "match_host", "rank_records"]
+           "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -62,6 +62,8 @@ def lib():
         "cs_match": (ip, [vp, ip, vp, ip, vp, ip, c.POINTER(c.c_double)]),
         "cs_match_host": (ip, [vp, ip, vp, ip, ip, c.POINTER(c.c_double)]),
         "cs_match_stats": (ip, [c.POINTER(c.c_ulonglong)]),
+        "cs_match_mutual": (ip, [vp, ip, vp, ip, fp, fp, vp, ip, ip, c.POINTER(c.c_double)]),
+        "cs_match_mutual_host": (ip, [vp, ip, vp, ip, fp, fp, vp, ip, ip, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -250,6 +252,33 @@ def MatchSiftData(data1, data2, mode=0):
     return ms.value
 
 
+MATCH_FIELDS = ("score", "ambiguity", "match", "match_xpos", "match_ypos")
+
+
+def MatchSiftDataMutual(data1, data2, minScore=0.0, maxAmbiguity=float("inf"), mode=0):
+    """Both directions of MatchSiftData in one call, cross-checked (cs_match_mutual).  data1's match fields become
+    those of MatchSiftData(data1, data2), data2's those of MatchSiftData(data2, data1); the h_data of a set that has
+    one receives its five match fields.  Returns (pairs, ms): int32 [k, 2] rows (i, j) with data1 row i and data2
+    row j each other's match, score > minScore and ambiguity < maxAmbiguity, in increasing i."""
+    n1, n2 = data1.numPts, data2.numPts
+    room = min(n1, n2)
+    ms = ctypes.c_double(0.0)
+    d_pairs = DeviceBuffer(max(room, 1) * 8)
+    try:
+        k = _check(lib().cs_match_mutual(data1.d_data, n1, data2.d_data, n2, float(minScore), float(maxAmbiguity),
+                                         d_pairs.ptr if room else None, room, int(mode), ctypes.byref(ms)),
+                   "MatchSiftDataMutual")
+        pairs = d_pairs.download(np.int32, 2 * k).reshape(k, 2) if k else np.zeros((0, 2), np.int32)
+    finally:
+        d_pairs.free()
+    for d, n in ((data1, n1), (data2, n2)):
+        if d.h_data is not None and n:
+            recs = d._buf.download(SIFT_DTYPE, n)
+            for f in MATCH_FIELDS:
+                d.h_data[f][:n] = recs[f]
+    return pairs, ms.value
+
+
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):
     """matching.cu:1000-1087; returns (3x3 homography, numMatches, ms).  seed: srand() value."""
     H = np.zeros(9, np.float32)
@@ -295,6 +324,18 @@ def match_host(s1, s2, mode=0):
     ms = ctypes.c_double(0.0)
     _check(lib().cs_match_host(_ptr(s1), len(s1), _ptr(s2), len(s2), int(mode), ctypes.byref(ms)), "cs_match_host")
     return s1, ms.value
+
+
+def match_mutual_host(s1, s2, minScore=0.0, maxAmbiguity=float("inf"), mode=0):
+    """MatchSiftDataMutual on host record arrays; returns (updated copy of s1, updated copy of s2, pairs[k, 2] int32,
+    ms)."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE).copy()
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE).copy()
+    pairs = np.zeros((min(len(s1), len(s2)), 2), np.int32)
+    ms = ctypes.c_double(0.0)
+    k = _check(lib().cs_match_mutual_host(_ptr(s1), len(s1), _ptr(s2), len(s2), float(minScore), float(maxAmbiguity),
+                                          _ptr(pairs), len(pairs), int(mode), ctypes.byref(ms)), "cs_match_mutual_host")
+    return s1, s2, pairs[:k].copy(), ms.value
 
 
 def rank_records(records, n):

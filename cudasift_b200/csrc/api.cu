@@ -287,8 +287,8 @@ struct DeviceCtx {
   unsigned int *h_counters = nullptr;      // pinned
   unsigned long long matchStats[4] = {0, 0, 0, 0};
   // scratch for *_host entry points
-  void *scratch[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // 4: cs_rank_records
-  size_t scratchBytes[5] = {0, 0, 0, 0, 0};
+  void *scratch[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 4: cs_rank_records, 5: mutual pairs
+  size_t scratchBytes[6] = {0, 0, 0, 0, 0, 0};
 
   int ensure(int d)
   {
@@ -442,6 +442,74 @@ static int match_sync(SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, SiftPoin
   if (useTensor) match_tensor_stats(c->matchStats);
   if (ms) *ms = t;
   return 0;
+}
+
+// Argument checks of the mutual matcher.  They come before any CUDA call (they hold on a machine without a device).
+static int mutual_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs,
+                       int mode)
+{
+  const char *bad = nullptr;
+  if (n1 < 0 || n2 < 0) bad = "n1 and n2 must be >= 0";
+  else if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) bad = "a set with records needs a pointer";
+  else if (maxPairs < 0) bad = "maxPairs must be >= 0";
+  else if (maxPairs > 0 && !pairs) bad = "maxPairs > 0 needs a pairs buffer";
+  else if (mode < 0 || mode > 2) bad = "mode must be 0 (auto), 1 (exact) or 2 (tensor)";
+  else if (n1 > 0 && n2 > 0) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(s1), b = reinterpret_cast<uintptr_t>(s2);
+    if (a < b + (uintptr_t)n2 * sizeof(SiftPoint) && b < a + (uintptr_t)n1 * sizeof(SiftPoint))
+      bad = "the record ranges of set 1 and set 2 overlap (both are written)";
+  }
+  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
+  return 0;
+}
+
+// Mutual matching: set 1's five match fields as match_sync(s1, s2) writes them, set 2's as match_sync(s2, s1), then
+// the cross-checked pairs (at most maxPairs written to d_pairs).  h_s1 / h_s2 (optional) receive the five fields of
+// their set.  Returns the number of pairs.
+static int mutual_sync(SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, float minScore, float maxAmbiguity,
+                       int2 *d_pairs, int maxPairs, int mode, SiftPoint *h_s1, SiftPoint *h_s2, double *ms)
+{
+  int err = 0;
+  if (ms) *ms = 0.0;
+  if (!n1 || !n2) return 0;                                                // matching.cu:1095-1096
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  cudaEventRecord(e0, c->stream);
+  // match_sync's rule, which is symmetric in the two sizes; the tensor path needs 32 candidates in either direction
+  const bool useTensor = ((mode == 2) || (mode == 0 && n1 >= 256 && n2 >= 256)) && match_tensor_supported() &&
+                         n1 >= 32 && n2 >= 32;
+  int r;
+  if (useTensor) {
+    r = match_tensor_mutual(d_s1, n1, d_s2, n2, minScore, maxAmbiguity, d_pairs, maxPairs, c->stream);
+  } else {
+    r = match_exact(d_s1, n1, d_s2, n2, c->stream);
+    if (r >= 0) r = match_exact(d_s2, n2, d_s1, n1, c->stream);
+    if (r >= 0) r = launch_mutual_pairs(d_s1, n1, d_s2, n2, minScore, maxAmbiguity, d_pairs, maxPairs, c->stream);
+  }
+  const SiftPoint *dev[2] = {d_s1, d_s2};
+  SiftPoint *host[2] = {h_s1, h_s2};
+  const int cnt[2] = {n1, n2};
+  for (int k = 0; k < 2 && r >= 0; k++) {
+    if (!host[k]) continue;
+    cudaError_t ce = cudaMemcpy2DAsync(&host[k][0].score, sizeof(SiftPoint), &dev[k][0].score, sizeof(SiftPoint),
+                                       5 * sizeof(float), cnt[k], cudaMemcpyDeviceToHost, c->stream);
+    if (ce != cudaSuccess) { set_error("cs_match_mutual: result copy failed: %s", cudaGetErrorString(ce)); r = CS_E_CUDA; }
+  }
+  if (r >= 0) {
+    cudaEventRecord(e1, c->stream);
+    cudaError_t ce = cudaStreamSynchronize(c->stream);
+    if (ce != cudaSuccess) { set_error("cs_match_mutual: %s", cudaGetErrorString(ce)); r = CS_E_CUDA; }
+  }
+  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }
+  float t = 0; cudaEventElapsedTime(&t, e0, e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
+  if (useTensor) match_tensor_stats(c->matchStats);                        // both directions summed
+  c->matchStats[3] = useTensor ? 2 : 1;
+  if (ms) *ms = t;
+  return mutual_pairs_total();
 }
 
 }  // namespace cs
@@ -854,6 +922,45 @@ int cs_match_host(void *h_s1, int n1, const void *h_s2, int n2, int mode, double
   CS_CUDA(cudaMemcpyAsync(d1, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
   CS_CUDA(cudaMemcpyAsync(d2, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
   return match_sync((SiftPoint *)d1, n1, (SiftPoint *)d2, n2, (SiftPoint *)h_s1, mode, ms);
+}
+
+int cs_match_mutual(void *d_s1, int n1, void *d_s2, int n2, float minScore, float maxAmbiguity, int *d_pairs, int maxPairs,
+                    int mode, double *ms)
+{
+  if (ms) *ms = 0.0;
+  int r = mutual_args("cs_match_mutual", d_s1, n1, d_s2, n2, d_pairs, maxPairs, mode);
+  if (r < 0) return r;
+  if ((reinterpret_cast<uintptr_t>(d_pairs) & 7) != 0) {
+    set_error("cs_match_mutual: invalid argument (CS_E_ARG): d_pairs must be 8-byte aligned");
+    return CS_E_ARG;
+  }
+  return mutual_sync((SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, minScore, maxAmbiguity, (int2 *)d_pairs, maxPairs, mode,
+                     nullptr, nullptr, ms);
+}
+
+int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore, float maxAmbiguity, int *h_pairs,
+                         int maxPairs, int mode, double *ms)
+{
+  if (ms) *ms = 0.0;
+  int r = mutual_args("cs_match_mutual_host", h_s1, n1, h_s2, n2, h_pairs, maxPairs, mode);
+  if (r < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const int room = maxPairs < (n1 < n2 ? n1 : n2) ? maxPairs : (n1 < n2 ? n1 : n2);   // no more pairs can exist
+  void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
+  if ((r = c->get_scratch(2, (size_t)n1 * sizeof(SiftPoint), &d1)) < 0) return r;
+  if ((r = c->get_scratch(3, (size_t)n2 * sizeof(SiftPoint), &d2)) < 0) return r;
+  if ((r = c->get_scratch(5, (size_t)(room > 0 ? room : 1) * sizeof(int2), &dp)) < 0) return r;
+  CS_CUDA(cudaMemcpyAsync(d1, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
+  CS_CUDA(cudaMemcpyAsync(d2, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
+  const int total = mutual_sync((SiftPoint *)d1, n1, (SiftPoint *)d2, n2, minScore, maxAmbiguity, (int2 *)dp, room, mode,
+                                (SiftPoint *)h_s1, (SiftPoint *)h_s2, ms);
+  if (total < 0) return total;
+  const int k = total < room ? total : room;
+  if (k > 0) CS_CUDA(cudaMemcpy(h_pairs, dp, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
+  return total;
 }
 
 int cs_match_stats(unsigned long long out[4])

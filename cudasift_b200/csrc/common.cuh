@@ -197,6 +197,13 @@ int match_tensor(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_
                  unsigned long long stats[4]);
 bool match_tensor_supported();
 void match_tensor_stats(unsigned long long stats[4]);   // after a synchronize
+// mutual matching: both directions on the tensor path (32 or more rows in each set), then the pairs
+int match_tensor_mutual(SiftPoint *s1, int n1, SiftPoint *s2, int n2, float minScore, float maxAmbiguity, int2 *pairs,
+                        int maxPairs, cudaStream_t st);
+// cross-check of two finished directions (match_mutual.cu); the total is read by mutual_pairs_total() after a synchronize
+int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, float minScore, float maxAmbiguity,
+                        int2 *pairs, int maxPairs, cudaStream_t st);
+int mutual_pairs_total();
 
 inline int idivup(int a, int b) { return (a + b - 1) / b; }
 inline int ialignup(int a, int b) { return (a % b != 0) ? (a - a % b + b) : a; }

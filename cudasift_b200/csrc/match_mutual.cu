@@ -1,0 +1,117 @@
+// match_mutual.cu -- cross-check of a mutual match: the pairs (i, j) with
+//   s1[i].match == j >= 0,  s2[j].match == i,  s1[i].score > minScore,  s1[i].ambiguity < maxAmbiguity
+// (strict comparisons, as FindHomography, homography.cu:200), written as int2 {i, j} in increasing i.  Every j
+// appears at most once (it pairs only with i = s2[j].match).  The order is defined by value: two launches, no atomics.
+//   1. flags   one thread per row i: the keep test; a ballot word per 32 rows and a count per CTA of 1024 rows.
+//   2. write   every CTA sums the counts of the CTAs before it (its exclusive prefix), scans its own 32 ballot words
+//              and writes its pairs; the last CTA writes the total.  Pairs at positions >= maxPairs are not written.
+#include "common.cuh"
+
+namespace cs {
+
+#define MP_ROWS 1024          // rows per CTA (one per thread)
+
+__global__ void __launch_bounds__(MP_ROWS)
+mutual_flags_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__restrict__ s2, int n2, float minScore,
+                    float maxAmbiguity, unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts)
+{
+  const int i = blockIdx.x * MP_ROWS + threadIdx.x;
+  bool keep = false;
+  if (i < n1) {
+    const int j = s1[i].match;
+    if (j >= 0 && j < n2 && s1[i].score > minScore && s1[i].ambiguity < maxAmbiguity) keep = __ldg(&s2[j].match) == i;
+  }
+  const unsigned int bal = __ballot_sync(0xffffffffu, keep);
+  if ((threadIdx.x & 31) == 0 && i < n1) masks[i >> 5] = bal;
+  const int cnt = __syncthreads_count(keep);
+  if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
+}
+
+__global__ void __launch_bounds__(MP_ROWS)
+mutual_write_kernel(const SiftPoint *__restrict__ s1, int n1, const unsigned int *__restrict__ masks,
+                    const unsigned int *__restrict__ blockCounts, int2 *__restrict__ pairs, int maxPairs,
+                    unsigned int *__restrict__ total)
+{
+  __shared__ unsigned int s_w[32];
+  __shared__ unsigned int s_base;
+  const unsigned int FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  // exclusive prefix of this CTA: the counts of the CTAs before it
+  unsigned int part = 0;
+  for (int k = threadIdx.x; k < (int)blockIdx.x; k += MP_ROWS) part += blockCounts[k];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
+  if (lane == 0) s_w[w] = part;
+  __syncthreads();
+  if (w == 0) {
+    unsigned int v = s_w[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+    if (lane == 0) s_base = v;
+  }
+  __syncthreads();
+  const unsigned int base = s_base;
+  // positions inside the CTA: exclusive scan of the warps' ballot counts
+  const int i = blockIdx.x * MP_ROWS + threadIdx.x;
+  const unsigned int bal = (blockIdx.x * MP_ROWS + w * 32 < n1) ? masks[(blockIdx.x * MP_ROWS >> 5) + w] : 0u;
+  if (lane == 0) s_w[w] = __popc(bal);
+  __syncthreads();
+  if (w == 0) {
+    const unsigned int c = s_w[lane];
+    unsigned int inc = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned int t = __shfl_up_sync(FULL, inc, o);
+      if (lane >= o) inc += t;
+    }
+    s_w[lane] = inc - c;
+    if (lane == 31 && blockIdx.x == gridDim.x - 1) *total = base + inc;
+  }
+  __syncthreads();
+  if ((bal >> lane) & 1u) {
+    const unsigned int pos = base + s_w[w] + __popc(bal & ((1u << lane) - 1u));
+    if (pos < (unsigned int)maxPairs) pairs[pos] = make_int2(i, s1[i].match);
+  }
+}
+
+// Per-device scratch (like the matcher's workspace, single-threaded per device): ballot words, CTA counts, the total.
+struct MutualWorkspace {
+  unsigned int *d = nullptr;
+  size_t cap = 0;
+  unsigned int *h_total = nullptr;    // pinned
+};
+static MutualWorkspace g_wsm[16];
+
+int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, float minScore, float maxAmbiguity,
+                        int2 *pairs, int maxPairs, cudaStream_t st)
+{
+  int dev = 0;
+  cudaGetDevice(&dev);
+  MutualWorkspace &ws = g_wsm[dev & 15];
+  const int blocks = idivup(n1, MP_ROWS), words = idivup(n1, 32);
+  const size_t bytes = ((size_t)words + blocks + 1) * sizeof(unsigned int);
+  if (ws.cap < bytes) {
+    if (ws.d) cudaFree(ws.d);
+    ws.d = nullptr; ws.cap = 0;
+    CS_CUDA(cudaMalloc((void **)&ws.d, bytes));
+    ws.cap = bytes;
+  }
+  if (!ws.h_total) CS_CUDA(cudaMallocHost((void **)&ws.h_total, sizeof(unsigned int)));
+  unsigned int *masks = ws.d, *counts = ws.d + words, *total = counts + blocks;
+  mutual_flags_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, s2, n2, minScore, maxAmbiguity, masks, counts);
+  mutual_write_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, masks, counts, pairs, maxPairs, total);
+  count_launch(2);
+  CS_CUDA(cudaGetLastError());
+  CS_CUDA(cudaMemcpyAsync(ws.h_total, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  return 0;
+}
+
+int mutual_pairs_total()
+{
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const MutualWorkspace &ws = g_wsm[dev & 15];
+  return ws.h_total ? (int)*ws.h_total : 0;
+}
+
+}  // namespace cs

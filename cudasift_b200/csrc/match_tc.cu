@@ -16,6 +16,8 @@
 //                and keep, per (row, partition), the three largest 4-candidate group maxima.
 //   3. resolve   eight lanes per row: merge the segments, certify, exact k=0..127 FMA chains for the
 //                surviving candidates, the reference's per-partition update rule and 8-way merge.
+// Mutual matching (match_tensor_mutual) converts both sets once for both directions (t3_prep_pair_kernel), runs
+// steps 2 and 3 and the exact fallback per direction on unchanged kernels, then the cross-check (match_mutual.cu).
 #include "common.cuh"
 
 #include <cuda_fp16.h>
@@ -143,11 +145,47 @@ __device__ __forceinline__ size_t tc_slot(const TcPlan &pl, int cta, int run, in
 struct T3Buffers {
   __half *a16, *b16;          // packed hi/lo operand tiles
   float *normA;               // per row of set 1
-  float *bmax;                // [0] max norm of set 2 (float bits), [1] bad-input flag
+  float *bmax;                // [0] max norm of the candidates (float bits); single direction: [1] bad-input flag
   float *pm;                  // per (row, segment) top-3 tables
   int *fbRows;                // fallback row list
   unsigned int *counters;     // [0] fallback rows, [1] candidate groups re-scored, [2] chains
 };
+
+// Chunk c (8 values) of a row's descriptor, zeros for rows >= nvalid: the split halves, the chunk's sum of squares and
+// the out-of-range test.
+__device__ __forceinline__ void t3_split_chunk(const SiftPoint *__restrict__ pts, int row, int nvalid, int c,
+                                               __half (&hi)[8], __half (&lo)[8], float &sq, bool &bad)
+{
+  float v[8];
+  if (row < nvalid) {
+    const float4 *p = reinterpret_cast<const float4 *>(pts[row].data + 8 * c);
+    float4 a = __ldg(p), b = __ldg(p + 1);
+    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; i++) v[i] = 0.0f;
+  }
+  sq = 0.0f;
+  bad = false;
+#pragma unroll
+  for (int i = 0; i < 8; i++) {
+    sq = fmaf(v[i], v[i], sq);
+    bad = bad || !(fabsf(v[i]) < T3_LIMIT);     // also catches NaN/Inf
+    const float x = v[i] * T3_SCALE;            // exact
+    hi[i] = __float2half_rn(x);
+    lo[i] = __float2half_rn(x - __half2float(hi[i]));   // the difference is exact in FP32
+  }
+}
+// eight halves -> the 16 bytes of one core-matrix row
+__device__ __forceinline__ uint4 t3_pack8(const __half (&h)[8])
+{
+  uint4 p;
+  p.x = (uint32_t)__half_as_ushort(h[0]) | ((uint32_t)__half_as_ushort(h[1]) << 16);
+  p.y = (uint32_t)__half_as_ushort(h[2]) | ((uint32_t)__half_as_ushort(h[3]) << 16);
+  p.z = (uint32_t)__half_as_ushort(h[4]) | ((uint32_t)__half_as_ushort(h[5]) << 16);
+  p.w = (uint32_t)__half_as_ushort(h[6]) | ((uint32_t)__half_as_ushort(h[7]) << 16);
+  return p;
+}
 
 // block = 32 rows x 16 chunks; one launch converts both sets (CTAs [0, blocksA) take set 1)
 __global__ void __launch_bounds__(512)
@@ -165,36 +203,12 @@ t3_prep_kernel(const SiftPoint *__restrict__ ptsA, int nA, __half *__restrict__ 
   const int row = (isB ? (int)blockIdx.x - blocksA : (int)blockIdx.x) * 32 + lane;
   if (threadIdx.x == 0) s_bad = 0;
   __syncthreads();
-  float v[8];
-  if (row < nvalid) {
-    const float4 *p = reinterpret_cast<const float4 *>(pts[row].data + 8 * c);
-    float4 a = __ldg(p), b = __ldg(p + 1);
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; i++) v[i] = 0.0f;
-  }
-  float sq = 0.0f;
-  bool bad = false;
   __half hi[8], lo[8];
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    sq = fmaf(v[i], v[i], sq);
-    bad = bad || !(fabsf(v[i]) < T3_LIMIT);     // also catches NaN/Inf
-    const float x = v[i] * T3_SCALE;            // exact
-    hi[i] = __float2half_rn(x);
-    lo[i] = __float2half_rn(x - __half2float(hi[i]));   // the difference is exact in FP32
-  }
+  float sq;
+  bool bad;
+  t3_split_chunk(pts, row, nvalid, c, hi, lo, sq, bad);
   if (bad) s_bad = 1;
-  uint4 ph, pl;
-  ph.x = (uint32_t)__half_as_ushort(hi[0]) | ((uint32_t)__half_as_ushort(hi[1]) << 16);
-  ph.y = (uint32_t)__half_as_ushort(hi[2]) | ((uint32_t)__half_as_ushort(hi[3]) << 16);
-  ph.z = (uint32_t)__half_as_ushort(hi[4]) | ((uint32_t)__half_as_ushort(hi[5]) << 16);
-  ph.w = (uint32_t)__half_as_ushort(hi[6]) | ((uint32_t)__half_as_ushort(hi[7]) << 16);
-  pl.x = (uint32_t)__half_as_ushort(lo[0]) | ((uint32_t)__half_as_ushort(lo[1]) << 16);
-  pl.y = (uint32_t)__half_as_ushort(lo[2]) | ((uint32_t)__half_as_ushort(lo[3]) << 16);
-  pl.z = (uint32_t)__half_as_ushort(lo[4]) | ((uint32_t)__half_as_ushort(lo[5]) << 16);
-  pl.w = (uint32_t)__half_as_ushort(lo[6]) | ((uint32_t)__half_as_ushort(lo[7]) << 16);
+  const uint4 ph = t3_pack8(hi), pl = t3_pack8(lo);
   if (!isB) {
     const int tile = row / T3_MT, r = row - tile * T3_MT;
     uint8_t *base = reinterpret_cast<uint8_t *>(outA) + (size_t)tile * T3_A_BYTES + ((size_t)c * T3_MT + r) * 16;
@@ -220,6 +234,72 @@ t3_prep_kernel(const SiftPoint *__restrict__ ptsA, int nA, __half *__restrict__ 
       if (lane == 0) atomicMax(reinterpret_cast<int *>(bmax), __float_as_int(nrm));
     }
     if (lane == 0 && s_bad) atomicMax(reinterpret_cast<int *>(bmax) + 1, 1);
+  }
+}
+
+// ---- mutual matching: both sets converted once, for both of their roles ---------------------------------------
+// A set is the A operand of its own direction (all n rows, with per-row norms) and the B operand of the other one
+// (only rows < nv = 32*floor(n/32), quirk Q7, zeros beyond).  The two roles have the same tile layout, so `a` serves
+// both unless the tail rows [nv, n) lie in a tile that the B role reads (n % 32 != 0 and nv % 128 != 0); then `b`
+// receives a B-role copy of the first bTiles tiles with the tail zeroed.
+static_assert(T3_MT == T3_N && T3_A_PART == T3_B_PART, "A and B operand tiles share one layout");
+struct T3PrepSet {
+  const SiftPoint *pts;
+  int n, nv;
+  int blocks;             // CTAs of 32 rows: every A tile of the set
+  __half *a, *b;          // b == NULL: `a` is also the B operand
+  int bTiles;             // tiles of the B role: ceil(nv / 128)
+  float *norms;           // per row, A role
+  float *bmax;            // max norm over rows < nv (float bits): the error bound of the other direction
+};
+
+// block = 32 rows x 16 chunks; CTAs [0, s0.blocks) take set 1, the rest set 2
+__global__ void __launch_bounds__(512)
+t3_prep_pair_kernel(const T3PrepSet s0, const T3PrepSet s1, float *__restrict__ gate, float *__restrict__ nextFlags)
+{
+  __shared__ float s_sq[16][33];
+  __shared__ int s_bad;
+  if (blockIdx.x == 0 && threadIdx.x < 16) nextFlags[threadIdx.x] = 0.0f;   // the next call's flag area
+  const bool second = (int)blockIdx.x >= s0.blocks;
+  const T3PrepSet s = second ? s1 : s0;
+  const int blk = second ? (int)blockIdx.x - s0.blocks : (int)blockIdx.x;
+  const int lane = threadIdx.x & 31, c = threadIdx.x >> 5;
+  const int row = blk * 32 + lane;
+  // nv is a multiple of 32: the CTA's rows lie all below nv (candidates of the other direction) or none of them
+  const bool cand = blk * 32 < s.nv;
+  if (threadIdx.x == 0) s_bad = 0;
+  __syncthreads();
+  __half hi[8], lo[8];
+  float sq;
+  bool bad;
+  t3_split_chunk(s.pts, row, s.n, c, hi, lo, sq, bad);
+  if (bad) s_bad = 1;
+  const uint4 ph = t3_pack8(hi), pl = t3_pack8(lo);
+  const int tile = row / T3_MT, r = row - tile * T3_MT;
+  const size_t off = (size_t)tile * T3_A_BYTES + ((size_t)c * T3_MT + r) * 16;
+  uint8_t *a = reinterpret_cast<uint8_t *>(s.a) + off;
+  *reinterpret_cast<uint4 *>(a) = ph;
+  *reinterpret_cast<uint4 *>(a + T3_A_PART) = pl;
+  if (s.b && tile < s.bTiles) {
+    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+    uint8_t *b = reinterpret_cast<uint8_t *>(s.b) + off;
+    *reinterpret_cast<uint4 *>(b) = cand ? ph : z;
+    *reinterpret_cast<uint4 *>(b + T3_B_PART) = cand ? pl : z;
+  }
+  s_sq[c][lane] = sq;
+  __syncthreads();
+  if (c == 0) {
+    float t = 0.0f;
+#pragma unroll
+    for (int i = 0; i < 16; i++) t += s_sq[i][lane];
+    float nrm = sqrtf(t) * 1.0001f;
+    if (row < s.n) s.norms[row] = nrm;
+    if (cand) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) nrm = fmaxf(nrm, __shfl_xor_sync(0xffffffffu, nrm, o));
+      if (lane == 0) atomicMax(reinterpret_cast<int *>(s.bmax), __float_as_int(nrm));
+    }
+    if (lane == 0 && s_bad) atomicMax(reinterpret_cast<int *>(gate), 1);
   }
 }
 
@@ -565,7 +645,9 @@ struct T3Workspace {
   T3Buffers bf = {};
   size_t cap[8] = {};
   unsigned int *h_counters = nullptr;
-  float *flags = nullptr;         // 2 x 16 words: [0] max norm of set 2, [1] bad-input flag, [4..7] counters
+  // 2 x 16 words, used alternately: [0] max norm of the candidates, [1] bad-input flag, [4..6] counters; a mutual call
+  // adds [2] the max norm of the reverse direction's candidates and [8..10] its counters
+  float *flags = nullptr;
   unsigned long long calls = 0;
   bool dirty = false;             // a call returned with an error after it had started to use the current flag area
   bool configured = false;
@@ -573,17 +655,17 @@ struct T3Workspace {
 };
 static T3Workspace g_ws3[16];
 
-// stats: [0] candidate groups re-scored, [1] exact chains, [2] rows that fell back to the exact scan
-int match_tensor(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st, unsigned long long stats[4])
+static int t3_sms()
 {
-  stats[0] = stats[1] = stats[2] = 0;
-  const int n2v = (n2 / 32) * 32;                      // matching.cu:325 (quirk Q7)
-  if (n1 <= 0) return 0;
-  if (n2v == 0 || !match_tensor_supported()) return match_exact(s1, n1, s2, n2, st);
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  T3Workspace &ws = g_ws3[dev & 15];
+  return sms;
+}
+
+// persistent GEMM schedule: n1 rows against the first n2v candidates
+static TcPlan t3_plan(int n1, int n2v, int sms)
+{
   TcPlan pl;
   pl.n1 = n1; pl.n2v = n2v;
   pl.n_mt = idivup(n1, T3_MT); pl.n_nt = idivup(n2v, T3_N);
@@ -593,70 +675,189 @@ int match_tensor(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_
   pl.grid = idivup(pl.total, pl.U);
   pl.runs = idivup(pl.U, pl.n_nt) + 1;
   { const char *e = getenv("CS_TC_DBG"); pl.dbg = e ? atoi(e) : 0; }    // experiments, results are wrong when set
-  const size_t slots = (size_t)pl.grid * pl.runs * T3_MT;
-  const size_t rowsPad = (size_t)pl.n_mt * T3_MT;
+  return pl;
+}
+static size_t t3_slots(const TcPlan &pl) { return (size_t)pl.grid * pl.runs * T3_MT; }
+
+// Grows the workspace buffers to the given sizes and selects this call's flag area (*flags).  Flags and counters live
+// in two 64-byte areas used alternately: a call's prep kernel clears the other one (*nextFlags) for the next call,
+// which saves a memset node per call.
+static int t3_begin(T3Workspace &ws, size_t aBytes, size_t bBytes, size_t normRows, size_t slots, size_t fbRows,
+                    cudaStream_t st, float **flags, float **nextFlags)
+{
   T3Buffers &bf = ws.bf;
   int r;
-  if ((r = ensure((void **)&bf.a16, &ws.cap[0], (size_t)pl.n_mt * T3_A_BYTES)) < 0) return r;
-  if ((r = ensure((void **)&bf.b16, &ws.cap[1], (size_t)pl.n_nt * T3_B_BYTES)) < 0) return r;
-  if ((r = ensure((void **)&bf.normA, &ws.cap[2], rowsPad * sizeof(float))) < 0) return r;
+  if ((r = ensure((void **)&bf.a16, &ws.cap[0], aBytes)) < 0) return r;
+  if ((r = ensure((void **)&bf.b16, &ws.cap[1], bBytes)) < 0) return r;
+  if ((r = ensure((void **)&bf.normA, &ws.cap[2], normRows * sizeof(float))) < 0) return r;
   if ((r = ensure((void **)&bf.pm, &ws.cap[3], slots * T3_PM * sizeof(float))) < 0) return r;
-  if ((r = ensure((void **)&bf.fbRows, &ws.cap[4], rowsPad * sizeof(int))) < 0) return r;
-  // flags/counters: two 64-byte areas used alternately; a call's prep kernel clears the other one for the
-  // next call, which saves a memset node per call
+  if ((r = ensure((void **)&bf.fbRows, &ws.cap[4], fbRows * sizeof(int))) < 0) return r;
   if (!ws.flags) {
     size_t dummy = 0;
     if ((r = ensure((void **)&ws.flags, &dummy, 128)) < 0) return r;
     CS_CUDA(cudaMemsetAsync(ws.flags, 0, 128, st));
     CS_CUDA(cudaMallocHost((void **)&ws.h_counters, 64));
   }
-  bf.bmax = ws.flags + 16 * (ws.calls & 1);
-  float *nextFlags = ws.flags + 16 * ((ws.calls + 1) & 1);
+  *flags = ws.flags + 16 * (ws.calls & 1);
+  *nextFlags = ws.flags + 16 * ((ws.calls + 1) & 1);
   if (ws.dirty) CS_CUDA(cudaMemsetAsync(ws.flags, 0, 128, st));     // a previous call failed between its launches
   ws.dirty = true;                                                  // until this call's launches are all in
-  bf.counters = reinterpret_cast<unsigned int *>(bf.bmax) + 4;
   if (!ws.configured) {
     CS_CUDA(cudaFuncSetAttribute(t3_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T3_SMEM_BYTES));
     ws.configured = true;
   }
-  // CUDASIFT_MATCH_TIMING=1: CUDA events between the kernels, printed to stderr (warm caches, unlike ncu)
-  static int timing = -1;
-  static cudaEvent_t tev[6];
-  if (timing < 0) {
-    const char *e = getenv("CUDASIFT_MATCH_TIMING");
-    timing = (e && atoi(e)) ? 1 : 0;
-    if (timing) for (int i = 0; i < 6; i++) cudaEventCreate(&tev[i]);
-  }
-  if (timing) cudaEventRecord(tev[0], st);
-  const int blocksA = pl.n_mt * (T3_MT / 32), blocksB = pl.n_nt * (T3_N / 32);
-  if (timing) cudaEventRecord(tev[1], st);
-  t3_prep_kernel<<<blocksA + blocksB, 512, 0, st>>>(s1, n1, bf.a16, bf.normA, blocksA, s2, n2v, bf.b16, bf.bmax, nextFlags);
-  if (timing) cudaEventRecord(tev[2], st);
-  t3_gemm_kernel<<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf);
-  if (timing) cudaEventRecord(tev[3], st);
-  t3_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2);
-  if (timing) cudaEventRecord(tev[4], st);
-  count_launch(3);
-  CS_CUDA(cudaGetLastError());
-  // rows that could not be certified -- or, for inputs the split cannot bound (|x| >= 8, NaN, Inf), every row --
-  // go through the exact kernel; which of the two is decided on the device
-  if ((r = match_exact_fallback(s1, n1, s2, n2, bf.fbRows, bf.counters, reinterpret_cast<const unsigned int *>(bf.bmax) + 1, st)) < 0) return r;
-  if (timing) {
-    cudaEventRecord(tev[5], st);
-    cudaEventSynchronize(tev[5]);
-    float ms[5];
-    for (int i = 0; i < 5; i++) cudaEventElapsedTime(&ms[i], tev[i], tev[i + 1]);
-    fprintf(stderr, "match timing %dx%d [us]: memset %.1f prep %.1f gemm %.1f resolve %.1f exact-fallback %.1f\n", n1, n2,
-            ms[0] * 1e3f, ms[1] * 1e3f, ms[2] * 1e3f, ms[3] * 1e3f, ms[4] * 1e3f);
-  }
-  CS_CUDA(cudaMemcpyAsync(ws.h_counters, bf.bmax, 64, cudaMemcpyDeviceToHost, st));
-  ws.calls++;                           // the prep kernel of this call cleared the other flag area for the next one
-  ws.dirty = false;
-  ws.pendingStats = true;               // read by match_tensor_stats() after the caller's synchronize
   return 0;
 }
 
-// statistics of the last match_tensor on this device (call after the stream was synchronized)
+// One direction after the prep kernel: GEMM, resolve, then the exact kernel for the rows that could not be certified
+// -- or, for inputs the split cannot bound (*gate != 0: |x| >= 8, NaN, Inf), for every row; which of the two is
+// decided on the device.  ev (optional): three events, recorded after each launch.
+static int t3_direction(const TcPlan &pl, const T3Buffers &bf, SiftPoint *s1, int n1, const SiftPoint *s2, int n2,
+                        const unsigned int *gate, cudaStream_t st, cudaEvent_t *ev)
+{
+  t3_gemm_kernel<<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf);
+  if (ev) cudaEventRecord(ev[0], st);
+  t3_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2);
+  if (ev) cudaEventRecord(ev[1], st);
+  count_launch(2);
+  CS_CUDA(cudaGetLastError());
+  int r;
+  if ((r = match_exact_fallback(s1, n1, s2, n2, bf.fbRows, bf.counters, gate, st)) < 0) return r;
+  if (ev) cudaEventRecord(ev[2], st);
+  return 0;
+}
+
+// the call's counters to the host, read by match_tensor_stats() after the caller's synchronize
+static int t3_end(T3Workspace &ws, const float *flags, cudaStream_t st)
+{
+  CS_CUDA(cudaMemcpyAsync(ws.h_counters, flags, 64, cudaMemcpyDeviceToHost, st));
+  ws.calls++;                           // the prep kernel of this call cleared the other flag area for the next one
+  ws.dirty = false;
+  ws.pendingStats = true;
+  return 0;
+}
+
+// CUDASIFT_MATCH_TIMING=1: CUDA events between the kernels, printed to stderr (warm caches, unlike ncu)
+static cudaEvent_t *t3_timing_events()
+{
+  static int timing = -1;
+  static cudaEvent_t tev[9];
+  if (timing < 0) {
+    const char *e = getenv("CUDASIFT_MATCH_TIMING");
+    timing = (e && atoi(e)) ? 1 : 0;
+    if (timing) for (int i = 0; i < 9; i++) cudaEventCreate(&tev[i]);
+  }
+  return timing ? tev : nullptr;
+}
+static void t3_print_timing(const char *what, int n1, int n2, const cudaEvent_t *tev, const char *const *names, int n)
+{
+  cudaEventSynchronize(tev[n]);
+  fprintf(stderr, "%s timing %dx%d [us]:", what, n1, n2);
+  for (int i = 0; i < n; i++) {
+    float ms = 0.0f;
+    cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
+    fprintf(stderr, " %s %.1f", names[i], ms * 1e3f);
+  }
+  fprintf(stderr, "\n");
+}
+
+// stats: [0] candidate groups re-scored, [1] exact chains, [2] rows that fell back to the exact scan
+int match_tensor(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st, unsigned long long stats[4])
+{
+  stats[0] = stats[1] = stats[2] = 0;
+  const int n2v = (n2 / 32) * 32;                      // matching.cu:325 (quirk Q7)
+  if (n1 <= 0) return 0;
+  if (n2v == 0 || !match_tensor_supported()) return match_exact(s1, n1, s2, n2, st);
+  int dev = 0;
+  cudaGetDevice(&dev);
+  T3Workspace &ws = g_ws3[dev & 15];
+  const TcPlan pl = t3_plan(n1, n2v, t3_sms());
+  const size_t rowsPad = (size_t)pl.n_mt * T3_MT;
+  float *flags = nullptr, *nextFlags = nullptr;
+  int r;
+  if ((r = t3_begin(ws, (size_t)pl.n_mt * T3_A_BYTES, (size_t)pl.n_nt * T3_B_BYTES, rowsPad, t3_slots(pl), rowsPad, st,
+                    &flags, &nextFlags)) < 0)
+    return r;
+  T3Buffers bf = ws.bf;
+  bf.bmax = flags;
+  bf.counters = reinterpret_cast<unsigned int *>(flags) + 4;
+  cudaEvent_t *tev = t3_timing_events();
+  if (tev) { cudaEventRecord(tev[0], st); cudaEventRecord(tev[1], st); }
+  const int blocksA = pl.n_mt * (T3_MT / 32), blocksB = pl.n_nt * (T3_N / 32);
+  t3_prep_kernel<<<blocksA + blocksB, 512, 0, st>>>(s1, n1, bf.a16, bf.normA, blocksA, s2, n2v, bf.b16, bf.bmax, nextFlags);
+  count_launch();
+  if (tev) cudaEventRecord(tev[2], st);
+  if ((r = t3_direction(pl, bf, s1, n1, s2, n2, reinterpret_cast<const unsigned int *>(flags) + 1, st,
+                        tev ? tev + 3 : nullptr)) < 0)
+    return r;
+  if (tev) {
+    static const char *const names[] = {"memset", "prep", "gemm", "resolve", "exact-fallback"};
+    t3_print_timing("match", n1, n2, tev, names, 5);
+  }
+  return t3_end(ws, flags, st);
+}
+
+// Mutual match on the tensor path (needs n1v = 32*floor(n1/32) > 0 and n2v > 0): set 1's five match fields exactly as
+// match_tensor(s1, n1, s2, n2) writes them, set 2's exactly as match_tensor(s2, n2, s1, n1), then the cross-checked
+// pairs (launch_mutual_pairs).  One prep launch converts each set once for both of its roles (T3PrepSet); each
+// direction then runs the single-direction kernels on its own plan and its own view of the workspace.  The top-3
+// tables and the fallback row list are shared: the two directions are stream-ordered.
+int match_tensor_mutual(SiftPoint *s1, int n1, SiftPoint *s2, int n2, float minScore, float maxAmbiguity, int2 *pairs,
+                        int maxPairs, cudaStream_t st)
+{
+  const int n1v = (n1 / 32) * 32, n2v = (n2 / 32) * 32;
+  if (n1v == 0 || n2v == 0) { set_error("match_tensor_mutual: both sets need 32 rows or more"); return CS_E_ARG; }
+  int dev = 0;
+  cudaGetDevice(&dev);
+  T3Workspace &ws = g_ws3[dev & 15];
+  const int sms = t3_sms();
+  const TcPlan pf = t3_plan(n1, n2v, sms), pr = t3_plan(n2, n1v, sms);
+  // a set needs its own B-role copy when its tail rows [nv, n) lie in a tile that the B role reads
+  const bool copy1 = n1 != n1v && n1v % T3_N != 0, copy2 = n2 != n2v && n2v % T3_N != 0;
+  const size_t bBytes1 = copy1 ? (size_t)pr.n_nt * T3_B_BYTES : 0, bBytes2 = copy2 ? (size_t)pf.n_nt * T3_B_BYTES : 0;
+  const size_t pad1 = (size_t)pf.n_mt * T3_MT, pad2 = (size_t)pr.n_mt * T3_MT;
+  const size_t slots = t3_slots(pf) > t3_slots(pr) ? t3_slots(pf) : t3_slots(pr);
+  float *flags = nullptr, *nextFlags = nullptr;
+  int r;
+  if ((r = t3_begin(ws, (pad1 + pad2) / T3_MT * T3_A_BYTES, bBytes1 + bBytes2, pad1 + pad2, slots,
+                    pad1 > pad2 ? pad1 : pad2, st, &flags, &nextFlags)) < 0)
+    return r;
+  auto at = [](__half *p, size_t bytes) { return reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(p) + bytes); };
+  // workspace: A tiles of set 1 then of set 2, B-role copies likewise; flags [0] / [2] take the candidates' max norm
+  // of the forward / reverse direction, i.e. of set 2 / set 1
+  T3PrepSet p1, p2;
+  p1.pts = s1; p1.n = n1; p1.nv = n1v; p1.blocks = pf.n_mt * (T3_MT / 32);
+  p1.a = ws.bf.a16; p1.b = copy1 ? ws.bf.b16 : nullptr; p1.bTiles = pr.n_nt;
+  p1.norms = ws.bf.normA; p1.bmax = flags + 2;
+  p2.pts = s2; p2.n = n2; p2.nv = n2v; p2.blocks = pr.n_mt * (T3_MT / 32);
+  p2.a = at(ws.bf.a16, pad1 / T3_MT * T3_A_BYTES); p2.b = copy2 ? at(ws.bf.b16, bBytes1) : nullptr; p2.bTiles = pf.n_nt;
+  p2.norms = ws.bf.normA + pad1; p2.bmax = flags;
+  T3Buffers fw = ws.bf, rv = ws.bf;
+  fw.a16 = p1.a; fw.b16 = copy2 ? p2.b : p2.a; fw.normA = p1.norms;
+  fw.bmax = flags; fw.counters = reinterpret_cast<unsigned int *>(flags) + 4;
+  rv.a16 = p2.a; rv.b16 = copy1 ? p1.b : p1.a; rv.normA = p2.norms;
+  rv.bmax = flags + 2; rv.counters = reinterpret_cast<unsigned int *>(flags) + 8;
+  const unsigned int *gate = reinterpret_cast<const unsigned int *>(flags) + 1;   // shared: any bad value, either set
+  cudaEvent_t *tev = t3_timing_events();
+  if (tev) cudaEventRecord(tev[0], st);
+  t3_prep_pair_kernel<<<p1.blocks + p2.blocks, 512, 0, st>>>(p1, p2, flags + 1, nextFlags);
+  count_launch();
+  CS_CUDA(cudaGetLastError());
+  if (tev) cudaEventRecord(tev[1], st);
+  if ((r = t3_direction(pf, fw, s1, n1, s2, n2, gate, st, tev ? tev + 2 : nullptr)) < 0) return r;
+  if ((r = t3_direction(pr, rv, s2, n2, s1, n1, gate, st, tev ? tev + 5 : nullptr)) < 0) return r;
+  if ((r = launch_mutual_pairs(s1, n1, s2, n2, minScore, maxAmbiguity, pairs, maxPairs, st)) < 0) return r;
+  if (tev) {
+    cudaEventRecord(tev[8], st);
+    static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
+                                        "reverse-exact-fallback", "pairs"};
+    t3_print_timing("mutual", n1, n2, tev, names, 8);
+  }
+  return t3_end(ws, flags, st);
+}
+
+// statistics of the last match_tensor / match_tensor_mutual on this device (call after the stream was synchronized);
+// a mutual call reports both directions summed
 void match_tensor_stats(unsigned long long stats[4])
 {
   int dev = 0;
@@ -664,10 +865,11 @@ void match_tensor_stats(unsigned long long stats[4])
   T3Workspace &ws = g_ws3[dev & 15];
   if (!ws.pendingStats) return;
   ws.pendingStats = false;
-  if (ws.h_counters[1] != 0) { stats[0] = stats[1] = 0; stats[2] = ~0ull; return; }   // everything went the exact way
-  stats[0] = ws.h_counters[4 + 1];
-  stats[1] = ws.h_counters[4 + 2];
-  stats[2] = ws.h_counters[4 + 0];
+  const unsigned int *h = ws.h_counters;
+  if (h[1] != 0) { stats[0] = stats[1] = 0; stats[2] = ~0ull; return; }   // everything went the exact way
+  stats[0] = (unsigned long long)h[4 + 1] + h[8 + 1];                     // [8..10] stay zero in a single direction
+  stats[1] = (unsigned long long)h[4 + 2] + h[8 + 2];
+  stats[2] = (unsigned long long)h[4 + 0] + h[8 + 0];
 }
 
 }  // namespace cs

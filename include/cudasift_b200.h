@@ -80,8 +80,29 @@ int cs_match(void *d_s1, int n1, void *d_s2, int n2, void *h_s1, int mode, doubl
 int cs_match_host(void *h_s1, int n1, const void *h_s2, int n2, int mode, double *ms);
 /* Statistics of the last tensor-core match on this thread's device:
  * out[0]=candidate groups emitted, out[1]=groups re-scored, out[2]=(row,partition)
- * pairs that took the exact-scan fallback, out[3]=path used (1 or 2). */
+ * pairs that took the exact-scan fallback, out[3]=path used (1 or 2).  After a mutual
+ * match, out[0..2] are both directions summed. */
 int cs_match_stats(unsigned long long out[4]);
+
+/* Mutual (cross-checked) nearest-neighbour matching, both directions in one call.
+ * - Set 1's score/ambiguity/match/match_xpos/match_ypos are written exactly as cs_match(s1, n1, s2, n2) writes
+ *   them, and set 2's exactly as cs_match(s2, n2, s1, n1) does, bit for bit (including quirk Q7: the reverse
+ *   direction only visits the set-1 rows below 32*floor(n1/32)).  Descriptors and all other fields are untouched.
+ * - The pairs are the (i, j) with s1[i].match == j >= 0, s2[j].match == i, s1[i].score > minScore and
+ *   s1[i].ambiguity < maxAmbiguity (strict, as cs_find_homography), stored as int pairs {i, j} in increasing i.
+ *   Each j appears at most once, so there are at most min(n1, n2).  The order does not depend on atomics.
+ * - mode as for cs_match; auto (0) picks the tensor path when both sets have 256 records or more.  The two sets are
+ *   converted for the tensor cores once, for both directions.
+ * - n1 == 0 or n2 == 0 returns 0 and writes nothing.  *ms (may be NULL) gets the event time of the whole call.
+ * Returns the number of mutual pairs (only the first maxPairs are written to d_pairs, device, 8-byte aligned), or
+ * CS_E_*.  CS_E_ARG, before any CUDA call, for n < 0, a NULL set with n > 0, maxPairs < 0, NULL pairs with
+ * maxPairs > 0, mode not in {0, 1, 2} and overlapping set-1 and set-2 record ranges. */
+int cs_match_mutual(void *d_s1, int n1, void *d_s2, int n2, float minScore, float maxAmbiguity,
+                    int *d_pairs, int maxPairs, int mode, double *ms);
+/* Same with host record arrays and a host pairs buffer: copies both sets up, matches, and copies the five match
+ * fields of both sets and the first min(total, maxPairs) pairs back. */
+int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore, float maxAmbiguity,
+                         int *h_pairs, int maxPairs, int mode, double *ms);
 
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
