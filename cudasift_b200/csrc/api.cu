@@ -406,7 +406,11 @@ static int extract_sync(const float *d_img, int w, int h, int pitch, int numOcta
   return numPts;
 }
 
-static int match_sync(SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, SiftPoint *h_s1, int mode, double *ms)
+// Set 1's five match fields on the device, copied to h_s1 when given.  With mu also set 2's, as a match of set 2 against
+// set 1 writes them (copied to h_s2 when given), then the cross-checked pairs; the call then returns the number of
+// pairs.  fn prefixes the error messages.
+static int match_sync(const char *fn, SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, const MutualArgs *mu, int mode,
+                      SiftPoint *h_s1, SiftPoint *h_s2, double *ms)
 {
   int err = 0;
   if (ms) *ms = 0.0;
@@ -414,33 +418,54 @@ static int match_sync(SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, SiftPoin
   if (!d_s1 || !d_s2) return 0;                                            // matching.cu:1101-1102
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
+  // The tensor path: asked for (mode 2) or automatic for 256 x 256 and more.  A one-way call with fewer than 32
+  // candidates runs the exact kernel inside match_tensor and reports path 2; a mutual call takes the exact path unless
+  // both sets have 32 rows.
+  bool tensor = (mode == 2) || (mode == 0 && match_tensor_supported() && n1 >= 256 && n2 >= 256);
+  if (mu) tensor = tensor && match_tensor_supported() && n1 >= 32 && n2 >= 32;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   cudaEventRecord(e0, c->stream);
   int r;
-  bool useTensor = (mode == 2) || (mode == 0 && match_tensor_supported() && n1 >= 256 && n2 >= 256);
-  if (useTensor) {
-    r = match_tensor(d_s1, n1, d_s2, n2, c->stream, c->matchStats);
-    c->matchStats[3] = 2;
+  if (tensor) {
+    r = match_tensor(d_s1, n1, d_s2, n2, mu, c->stream);
   } else {
     r = match_exact(d_s1, n1, d_s2, n2, c->stream);
-    c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0; c->matchStats[3] = 1;
+    if (mu && r >= 0) r = match_exact(d_s2, n2, d_s1, n1, c->stream);
+    if (mu && r >= 0) r = launch_mutual_pairs(d_s1, n1, d_s2, n2, *mu, c->stream);
   }
-  if (r >= 0 && h_s1) {                                                    // matching.cu:1195-1199
-    cudaError_t ce = cudaMemcpy2DAsync(&h_s1[0].score, sizeof(SiftPoint), &d_s1[0].score, sizeof(SiftPoint),
-                                       5 * sizeof(float), n1, cudaMemcpyDeviceToHost, c->stream);
-    if (ce != cudaSuccess) { set_error("MatchSiftData: result copy failed: %s", cudaGetErrorString(ce)); r = CS_E_CUDA; }
+  const SiftPoint *dev[2] = {d_s1, d_s2};
+  SiftPoint *host[2] = {h_s1, h_s2};
+  const int cnt[2] = {n1, n2};
+  for (int k = 0; k < 2 && r >= 0; k++) {                                  // matching.cu:1195-1199
+    if (!host[k]) continue;
+    cudaError_t ce = cudaMemcpy2DAsync(&host[k][0].score, sizeof(SiftPoint), &dev[k][0].score, sizeof(SiftPoint),
+                                       5 * sizeof(float), cnt[k], cudaMemcpyDeviceToHost, c->stream);
+    if (ce != cudaSuccess) { set_error("%s: result copy failed: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
   }
   if (r >= 0) {
     cudaEventRecord(e1, c->stream);
     cudaError_t ce = cudaStreamSynchronize(c->stream);
-    if (ce != cudaSuccess) { set_error("MatchSiftData: %s", cudaGetErrorString(ce)); r = CS_E_CUDA; }
+    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
   }
   if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }     // no event leak on the error paths
   float t = 0; cudaEventElapsedTime(&t, e0, e1);
   cudaEventDestroy(e0); cudaEventDestroy(e1);
-  if (useTensor) match_tensor_stats(c->matchStats);
+  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
+  if (tensor) match_tensor_stats(c->matchStats);                           // a mutual call: both directions summed
+  c->matchStats[3] = tensor ? 2 : 1;
   if (ms) *ms = t;
+  return mu ? mutual_pairs_total() : 0;
+}
+
+// The two host sets to the context's match scratch (the caller's stream order makes them visible to the match).
+static int upload_sets(DeviceCtx *c, const void *h_s1, int n1, const void *h_s2, int n2, void **d1, void **d2)
+{
+  int r;
+  if ((r = c->get_scratch(2, (size_t)n1 * sizeof(SiftPoint), d1)) < 0) return r;
+  if ((r = c->get_scratch(3, (size_t)n2 * sizeof(SiftPoint), d2)) < 0) return r;
+  CS_CUDA(cudaMemcpyAsync(*d1, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
+  CS_CUDA(cudaMemcpyAsync(*d2, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
   return 0;
 }
 
@@ -461,55 +486,6 @@ static int mutual_args(const char *fn, const void *s1, int n1, const void *s2, i
   }
   if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
   return 0;
-}
-
-// Mutual matching: set 1's five match fields as match_sync(s1, s2) writes them, set 2's as match_sync(s2, s1), then
-// the cross-checked pairs (at most maxPairs written to d_pairs).  h_s1 / h_s2 (optional) receive the five fields of
-// their set.  Returns the number of pairs.
-static int mutual_sync(SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, float minScore, float maxAmbiguity,
-                       int2 *d_pairs, int maxPairs, int mode, SiftPoint *h_s1, SiftPoint *h_s2, double *ms)
-{
-  int err = 0;
-  if (ms) *ms = 0.0;
-  if (!n1 || !n2) return 0;                                                // matching.cu:1095-1096
-  DeviceCtx *c = current_ctx(&err);
-  if (!c) return err;
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  cudaEventRecord(e0, c->stream);
-  // match_sync's rule, which is symmetric in the two sizes; the tensor path needs 32 candidates in either direction
-  const bool useTensor = ((mode == 2) || (mode == 0 && n1 >= 256 && n2 >= 256)) && match_tensor_supported() &&
-                         n1 >= 32 && n2 >= 32;
-  int r;
-  if (useTensor) {
-    r = match_tensor_mutual(d_s1, n1, d_s2, n2, minScore, maxAmbiguity, d_pairs, maxPairs, c->stream);
-  } else {
-    r = match_exact(d_s1, n1, d_s2, n2, c->stream);
-    if (r >= 0) r = match_exact(d_s2, n2, d_s1, n1, c->stream);
-    if (r >= 0) r = launch_mutual_pairs(d_s1, n1, d_s2, n2, minScore, maxAmbiguity, d_pairs, maxPairs, c->stream);
-  }
-  const SiftPoint *dev[2] = {d_s1, d_s2};
-  SiftPoint *host[2] = {h_s1, h_s2};
-  const int cnt[2] = {n1, n2};
-  for (int k = 0; k < 2 && r >= 0; k++) {
-    if (!host[k]) continue;
-    cudaError_t ce = cudaMemcpy2DAsync(&host[k][0].score, sizeof(SiftPoint), &dev[k][0].score, sizeof(SiftPoint),
-                                       5 * sizeof(float), cnt[k], cudaMemcpyDeviceToHost, c->stream);
-    if (ce != cudaSuccess) { set_error("cs_match_mutual: result copy failed: %s", cudaGetErrorString(ce)); r = CS_E_CUDA; }
-  }
-  if (r >= 0) {
-    cudaEventRecord(e1, c->stream);
-    cudaError_t ce = cudaStreamSynchronize(c->stream);
-    if (ce != cudaSuccess) { set_error("cs_match_mutual: %s", cudaGetErrorString(ce)); r = CS_E_CUDA; }
-  }
-  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }
-  float t = 0; cudaEventElapsedTime(&t, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
-  if (useTensor) match_tensor_stats(c->matchStats);                        // both directions summed
-  c->matchStats[3] = useTensor ? 2 : 1;
-  if (ms) *ms = t;
-  return mutual_pairs_total();
 }
 
 }  // namespace cs
@@ -776,9 +752,10 @@ double MatchSiftData(SiftData &data1, SiftData &data2)
   ExitGuard g;
   double ms = 0.0;
 #ifdef MANAGEDMEM
-  int r = match_sync(data1.m_data, data1.numPts, data2.m_data, data2.numPts, NULL, 0, &ms);
+  int r = match_sync("MatchSiftData", data1.m_data, data1.numPts, data2.m_data, data2.numPts, NULL, 0, NULL, NULL, &ms);
 #else
-  int r = match_sync(data1.d_data, data1.numPts, data2.d_data, data2.numPts, data1.h_data, 0, &ms);
+  int r = match_sync("MatchSiftData", data1.d_data, data1.numPts, data2.d_data, data2.numPts, NULL, 0, data1.h_data, NULL,
+                     &ms);
 #endif
   die_if(r);
   if (verbose()) printf("MatchSiftData time =          %.2f ms\n", ms);
@@ -905,7 +882,8 @@ int cs_extract_host(const float *h_img, int w, int h, int numOctaves, double ini
 
 int cs_match(void *d_s1, int n1, void *d_s2, int n2, void *h_s1, int mode, double *ms)
 {
-  return match_sync((SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, (SiftPoint *)h_s1, mode, ms);
+  return match_sync("MatchSiftData", (SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, nullptr, mode, (SiftPoint *)h_s1, nullptr,
+                    ms);
 }
 
 int cs_match_host(void *h_s1, int n1, const void *h_s2, int n2, int mode, double *ms)
@@ -917,11 +895,8 @@ int cs_match_host(void *h_s1, int n1, const void *h_s2, int n2, int mode, double
   if (!c) return err;
   void *d1 = nullptr, *d2 = nullptr;
   int r;
-  if ((r = c->get_scratch(2, (size_t)n1 * sizeof(SiftPoint), &d1)) < 0) return r;
-  if ((r = c->get_scratch(3, (size_t)n2 * sizeof(SiftPoint), &d2)) < 0) return r;
-  CS_CUDA(cudaMemcpyAsync(d1, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
-  CS_CUDA(cudaMemcpyAsync(d2, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
-  return match_sync((SiftPoint *)d1, n1, (SiftPoint *)d2, n2, (SiftPoint *)h_s1, mode, ms);
+  if ((r = upload_sets(c, h_s1, n1, h_s2, n2, &d1, &d2)) < 0) return r;
+  return match_sync("MatchSiftData", (SiftPoint *)d1, n1, (SiftPoint *)d2, n2, nullptr, mode, (SiftPoint *)h_s1, nullptr, ms);
 }
 
 int cs_match_mutual(void *d_s1, int n1, void *d_s2, int n2, float minScore, float maxAmbiguity, int *d_pairs, int maxPairs,
@@ -934,8 +909,8 @@ int cs_match_mutual(void *d_s1, int n1, void *d_s2, int n2, float minScore, floa
     set_error("cs_match_mutual: invalid argument (CS_E_ARG): d_pairs must be 8-byte aligned");
     return CS_E_ARG;
   }
-  return mutual_sync((SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, minScore, maxAmbiguity, (int2 *)d_pairs, maxPairs, mode,
-                     nullptr, nullptr, ms);
+  const MutualArgs mu = {minScore, maxAmbiguity, (int2 *)d_pairs, maxPairs};
+  return match_sync("cs_match_mutual", (SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, &mu, mode, nullptr, nullptr, ms);
 }
 
 int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore, float maxAmbiguity, int *h_pairs,
@@ -950,13 +925,11 @@ int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore,
   if (!c) return err;
   const int room = maxPairs < (n1 < n2 ? n1 : n2) ? maxPairs : (n1 < n2 ? n1 : n2);   // no more pairs can exist
   void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
-  if ((r = c->get_scratch(2, (size_t)n1 * sizeof(SiftPoint), &d1)) < 0) return r;
-  if ((r = c->get_scratch(3, (size_t)n2 * sizeof(SiftPoint), &d2)) < 0) return r;
   if ((r = c->get_scratch(5, (size_t)(room > 0 ? room : 1) * sizeof(int2), &dp)) < 0) return r;
-  CS_CUDA(cudaMemcpyAsync(d1, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
-  CS_CUDA(cudaMemcpyAsync(d2, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
-  const int total = mutual_sync((SiftPoint *)d1, n1, (SiftPoint *)d2, n2, minScore, maxAmbiguity, (int2 *)dp, room, mode,
-                                (SiftPoint *)h_s1, (SiftPoint *)h_s2, ms);
+  if ((r = upload_sets(c, h_s1, n1, h_s2, n2, &d1, &d2)) < 0) return r;
+  const MutualArgs mu = {minScore, maxAmbiguity, (int2 *)dp, room};
+  const int total = match_sync("cs_match_mutual", (SiftPoint *)d1, n1, (SiftPoint *)d2, n2, &mu, mode, (SiftPoint *)h_s1,
+                               (SiftPoint *)h_s2, ms);
   if (total < 0) return total;
   const int k = total < room ? total : room;
   if (k > 0) CS_CUDA(cudaMemcpy(h_pairs, dp, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));

@@ -192,17 +192,19 @@ int launch_rank(const RankParams &p, int batch, int sms, cudaStream_t st);
 
 // ---- matcher ------------------------------------------------------------------------
 struct MatchWorkspace;   // opaque, owned by the per-device context
+// the cross-check of a mutual match: pairs with score > minScore and ambiguity < maxAmbiguity, at most maxPairs written
+struct MutualArgs {
+  float minScore, maxAmbiguity;
+  int2 *pairs;
+  int maxPairs;
+};
 int match_exact(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st);
-int match_tensor(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st,
-                 unsigned long long stats[4]);
+// tensor path: set 1 against set 2, or with mu (32 or more rows in each set) both directions and then the pairs
+int match_tensor(SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs *mu, cudaStream_t st);
 bool match_tensor_supported();
 void match_tensor_stats(unsigned long long stats[4]);   // after a synchronize
-// mutual matching: both directions on the tensor path (32 or more rows in each set), then the pairs
-int match_tensor_mutual(SiftPoint *s1, int n1, SiftPoint *s2, int n2, float minScore, float maxAmbiguity, int2 *pairs,
-                        int maxPairs, cudaStream_t st);
 // cross-check of two finished directions (match_mutual.cu); the total is read by mutual_pairs_total() after a synchronize
-int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, float minScore, float maxAmbiguity,
-                        int2 *pairs, int maxPairs, cudaStream_t st);
+int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu, cudaStream_t st);
 int mutual_pairs_total();
 
 inline int idivup(int a, int b) { return (a + b - 1) / b; }

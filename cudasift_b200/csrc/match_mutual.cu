@@ -82,8 +82,7 @@ struct MutualWorkspace {
 };
 static MutualWorkspace g_wsm[16];
 
-int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, float minScore, float maxAmbiguity,
-                        int2 *pairs, int maxPairs, cudaStream_t st)
+int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu, cudaStream_t st)
 {
   int dev = 0;
   cudaGetDevice(&dev);
@@ -98,8 +97,8 @@ int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2
   }
   if (!ws.h_total) CS_CUDA(cudaMallocHost((void **)&ws.h_total, sizeof(unsigned int)));
   unsigned int *masks = ws.d, *counts = ws.d + words, *total = counts + blocks;
-  mutual_flags_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, s2, n2, minScore, maxAmbiguity, masks, counts);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, masks, counts, pairs, maxPairs, total);
+  mutual_flags_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, masks, counts);
+  mutual_write_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, masks, counts, mu.pairs, mu.maxPairs, total);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
   CS_CUDA(cudaMemcpyAsync(ws.h_total, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));

@@ -16,8 +16,8 @@
 //                and keep, per (row, partition), the three largest 4-candidate group maxima.
 //   3. resolve   eight lanes per row: merge the segments, certify, exact k=0..127 FMA chains for the
 //                surviving candidates, the reference's per-partition update rule and 8-way merge.
-// Mutual matching (match_tensor_mutual) converts both sets once for both directions (t3_prep_pair_kernel), runs
-// steps 2 and 3 and the exact fallback per direction on unchanged kernels, then the cross-check (match_mutual.cu).
+// Mutual matching uses the same prep launch to convert each set once for both of its roles, runs steps 2 and 3 and
+// the exact fallback per direction, then the cross-check (match_mutual.cu).
 #include "common.cuh"
 
 #include <cuda_fp16.h>
@@ -100,11 +100,6 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
 // ------------------------------------------------------------------------------ workspace
 struct TcPlan {
   int n1, n2v, n_mt, n_nt, total, U, runs, grid;
-  // experiments (env CS_TC_DBG, results are wrong when set): 1 = B tiles are not reloaded, 2 = MMAs without
-  // the top-3 update.  The bit-2 branch in t3_gemm_kernel also keeps the top-3 update below the consumers' release
-  // of the B stage: without it, ptxas moves part of the update above that arrive.  Pin the order explicitly before
-  // this field goes.
-  int dbg;
 };
 // slot of (cta, run, row-in-tile)
 __device__ __forceinline__ size_t tc_slot(const TcPlan &pl, int cta, int run, int rowInTile)
@@ -145,7 +140,7 @@ __device__ __forceinline__ size_t tc_slot(const TcPlan &pl, int cta, int run, in
 struct T3Buffers {
   __half *a16, *b16;          // packed hi/lo operand tiles
   float *normA;               // per row of set 1
-  float *bmax;                // [0] max norm of the candidates (float bits); single direction: [1] bad-input flag
+  float *bmax;                // max norm of the candidates (float bits)
   float *pm;                  // per (row, segment) top-3 tables
   int *fbRows;                // fallback row list
   unsigned int *counters;     // [0] fallback rows, [1] candidate groups re-scored, [2] chains
@@ -187,61 +182,12 @@ __device__ __forceinline__ uint4 t3_pack8(const __half (&h)[8])
   return p;
 }
 
-// block = 32 rows x 16 chunks; one launch converts both sets (CTAs [0, blocksA) take set 1)
-__global__ void __launch_bounds__(512)
-t3_prep_kernel(const SiftPoint *__restrict__ ptsA, int nA, __half *__restrict__ outA, float *__restrict__ norms,
-               int blocksA, const SiftPoint *__restrict__ ptsB, int nB, __half *__restrict__ outB,
-               float *__restrict__ bmax, float *__restrict__ nextFlags)
-{
-  __shared__ float s_sq[16][33];
-  __shared__ int s_bad;
-  if (blockIdx.x == 0 && threadIdx.x < 16) nextFlags[threadIdx.x] = 0.0f;   // the next call's flag area
-  const int isB = (int)blockIdx.x >= blocksA;
-  const SiftPoint *__restrict__ pts = isB ? ptsB : ptsA;
-  const int nvalid = isB ? nB : nA;
-  const int lane = threadIdx.x & 31, c = threadIdx.x >> 5;
-  const int row = (isB ? (int)blockIdx.x - blocksA : (int)blockIdx.x) * 32 + lane;
-  if (threadIdx.x == 0) s_bad = 0;
-  __syncthreads();
-  __half hi[8], lo[8];
-  float sq;
-  bool bad;
-  t3_split_chunk(pts, row, nvalid, c, hi, lo, sq, bad);
-  if (bad) s_bad = 1;
-  const uint4 ph = t3_pack8(hi), pl = t3_pack8(lo);
-  if (!isB) {
-    const int tile = row / T3_MT, r = row - tile * T3_MT;
-    uint8_t *base = reinterpret_cast<uint8_t *>(outA) + (size_t)tile * T3_A_BYTES + ((size_t)c * T3_MT + r) * 16;
-    *reinterpret_cast<uint4 *>(base) = ph;
-    *reinterpret_cast<uint4 *>(base + T3_A_PART) = pl;
-  } else {
-    const int tile = row / T3_N, r = row - tile * T3_N;
-    uint8_t *base = reinterpret_cast<uint8_t *>(outB) + (size_t)tile * T3_B_BYTES + ((size_t)c * T3_N + r) * 16;
-    *reinterpret_cast<uint4 *>(base) = ph;
-    *reinterpret_cast<uint4 *>(base + T3_B_PART) = pl;
-  }
-  s_sq[c][lane] = sq;
-  __syncthreads();
-  if (c == 0) {
-    float t = 0.0f;
-#pragma unroll
-    for (int i = 0; i < 16; i++) t += s_sq[i][lane];
-    float nrm = sqrtf(t) * 1.0001f;
-    if (!isB && row < nvalid) norms[row] = nrm;
-    if (isB) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) nrm = fmaxf(nrm, __shfl_xor_sync(0xffffffffu, nrm, o));
-      if (lane == 0) atomicMax(reinterpret_cast<int *>(bmax), __float_as_int(nrm));
-    }
-    if (lane == 0 && s_bad) atomicMax(reinterpret_cast<int *>(bmax) + 1, 1);
-  }
-}
-
-// ---- mutual matching: both sets converted once, for both of their roles ---------------------------------------
-// A set is the A operand of its own direction (all n rows, with per-row norms) and the B operand of the other one
-// (only rows < nv = 32*floor(n/32), quirk Q7, zeros beyond).  The two roles have the same tile layout, so `a` serves
-// both unless the tail rows [nv, n) lie in a tile that the B role reads (n % 32 != 0 and nv % 128 != 0); then `b`
-// receives a B-role copy of the first bTiles tiles with the tail zeroed.
+// ---- prep: each set converted once, for both of its roles ---------------------------------------------------------
+// In a mutual match a set is the A operand of its own direction (all n rows, with per-row norms) and the B operand of
+// the other one (only rows < nv = 32*floor(n/32), quirk Q7, zeros beyond).  The two roles have the same tile layout, so
+// `a` serves both unless the tail rows [nv, n) lie in a tile that the B role reads (n % 32 != 0 and nv % 128 != 0);
+// then `b` receives a B-role copy of the first bTiles tiles with the tail zeroed.  A one-way match gives set 1 the A
+// role only (nv = 0) and set 2 the B role only (n = nv).
 static_assert(T3_MT == T3_N && T3_A_PART == T3_B_PART, "A and B operand tiles share one layout");
 struct T3PrepSet {
   const SiftPoint *pts;
@@ -255,7 +201,7 @@ struct T3PrepSet {
 
 // block = 32 rows x 16 chunks; CTAs [0, s0.blocks) take set 1, the rest set 2
 __global__ void __launch_bounds__(512)
-t3_prep_pair_kernel(const T3PrepSet s0, const T3PrepSet s1, float *__restrict__ gate, float *__restrict__ nextFlags)
+t3_prep_kernel(const T3PrepSet s0, const T3PrepSet s1, float *__restrict__ gate, float *__restrict__ nextFlags)
 {
   __shared__ float s_sq[16][33];
   __shared__ int s_bad;
@@ -340,7 +286,6 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
         }
         const int s = i % T3_STAGES, it = i / T3_STAGES;
         if (it > 0) mbar_wait(&bar_b_empty[s], (it - 1) & 1);
-        if ((pl.dbg & 1) && it > 0) { mbar_arrive(&bar_b_full[s]); continue; }   // experiment: no B traffic
         mbar_expect_tx(&bar_b_full[s], T3_B_BYTES);
         bulk_g2s(sB + s * T3_B_BYTES, reinterpret_cast<const uint8_t *>(bf.b16) + (size_t)nt * T3_B_BYTES, T3_B_BYTES, &bar_b_full[s]);
       }
@@ -393,23 +338,21 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
         mbar_arrive(&bar_b_empty[s]);
         if (lastOfRun) mbar_arrive(&bar_a_empty);
       }
-      if (!(pl.dbg & 2)) {                           // experiment (bit 1): MMAs without the top-3 update
-        // columns 8j + 2(lane % 4) + {0, 1}: the lane pair (lane, lane ^ 1) holds group 2j + hb of partition 2(j % 4) + hb
-        const int gbase = nt * (T3_N / 4) + hb;
+      // columns 8j + 2(lane % 4) + {0, 1}: the lane pair (lane, lane ^ 1) holds group 2j + hb of partition 2(j % 4) + hb
+      const int gbase = nt * (T3_N / 4) + hb;
 #pragma unroll
-        for (int j = 0; j < 16; j++) {
+      for (int j = 0; j < 16; j++) {
 #pragma unroll
-          for (int r = 0; r < 2; r++) {
-            float v = fmaxf(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]);
-            v = fmaxf(v, __shfl_xor_sync(FULL, v, 1));
-            const int q = j & 3, id = gbase + 2 * j;
-            const bool t = v > g1[r][q], u2 = v > g2[r][q];
-            g3[r][q] = fmaxf(g3[r][q], fminf(g2[r][q], v));
-            i2[r][q] = u2 ? (t ? i1[r][q] : id) : i2[r][q];
-            g2[r][q] = fmaxf(g2[r][q], fminf(g1[r][q], v));
-            i1[r][q] = t ? id : i1[r][q];
-            g1[r][q] = fmaxf(g1[r][q], v);
-          }
+        for (int r = 0; r < 2; r++) {
+          float v = fmaxf(acc[4 * j + 2 * r], acc[4 * j + 2 * r + 1]);
+          v = fmaxf(v, __shfl_xor_sync(FULL, v, 1));
+          const int q = j & 3, id = gbase + 2 * j;
+          const bool t = v > g1[r][q], u2 = v > g2[r][q];
+          g3[r][q] = fmaxf(g3[r][q], fminf(g2[r][q], v));
+          i2[r][q] = u2 ? (t ? i1[r][q] : id) : i2[r][q];
+          g2[r][q] = fmaxf(g2[r][q], fminf(g1[r][q], v));
+          i1[r][q] = t ? id : i1[r][q];
+          g1[r][q] = fmaxf(g1[r][q], v);
         }
       }
       if (lastOfRun && !(lane & 1)) {
@@ -674,7 +617,6 @@ static TcPlan t3_plan(int n1, int n2v, int sms)
   pl.U = idivup(pl.total, pl.grid);
   pl.grid = idivup(pl.total, pl.U);
   pl.runs = idivup(pl.U, pl.n_nt) + 1;
-  { const char *e = getenv("CS_TC_DBG"); pl.dbg = e ? atoi(e) : 0; }    // experiments, results are wrong when set
   return pl;
 }
 static size_t t3_slots(const TcPlan &pl) { return (size_t)pl.grid * pl.runs * T3_MT; }
@@ -761,102 +703,81 @@ static void t3_print_timing(const char *what, int n1, int n2, const cudaEvent_t 
   fprintf(stderr, "\n");
 }
 
-// stats: [0] candidate groups re-scored, [1] exact chains, [2] rows that fell back to the exact scan
-int match_tensor(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st, unsigned long long stats[4])
+// Set 1's five match fields; with mu (32 or more rows in each set) also set 2's, exactly as a one-way match of set 2
+// against set 1 writes them, then the cross-checked pairs (launch_mutual_pairs).  One prep launch converts each set once
+// for every role it has (T3PrepSet); each direction then runs on its own plan and its own view of the workspace.  The
+// top-3 tables and the fallback row list are shared: the two directions are stream-ordered.
+int match_tensor(SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs *mu, cudaStream_t st)
 {
-  stats[0] = stats[1] = stats[2] = 0;
-  const int n2v = (n2 / 32) * 32;                      // matching.cu:325 (quirk Q7)
-  if (n1 <= 0) return 0;
-  if (n2v == 0 || !match_tensor_supported()) return match_exact(s1, n1, s2, n2, st);
-  int dev = 0;
-  cudaGetDevice(&dev);
-  T3Workspace &ws = g_ws3[dev & 15];
-  const TcPlan pl = t3_plan(n1, n2v, t3_sms());
-  const size_t rowsPad = (size_t)pl.n_mt * T3_MT;
-  float *flags = nullptr, *nextFlags = nullptr;
-  int r;
-  if ((r = t3_begin(ws, (size_t)pl.n_mt * T3_A_BYTES, (size_t)pl.n_nt * T3_B_BYTES, rowsPad, t3_slots(pl), rowsPad, st,
-                    &flags, &nextFlags)) < 0)
-    return r;
-  T3Buffers bf = ws.bf;
-  bf.bmax = flags;
-  bf.counters = reinterpret_cast<unsigned int *>(flags) + 4;
-  cudaEvent_t *tev = t3_timing_events();
-  if (tev) { cudaEventRecord(tev[0], st); cudaEventRecord(tev[1], st); }
-  const int blocksA = pl.n_mt * (T3_MT / 32), blocksB = pl.n_nt * (T3_N / 32);
-  t3_prep_kernel<<<blocksA + blocksB, 512, 0, st>>>(s1, n1, bf.a16, bf.normA, blocksA, s2, n2v, bf.b16, bf.bmax, nextFlags);
-  count_launch();
-  if (tev) cudaEventRecord(tev[2], st);
-  if ((r = t3_direction(pl, bf, s1, n1, s2, n2, reinterpret_cast<const unsigned int *>(flags) + 1, st,
-                        tev ? tev + 3 : nullptr)) < 0)
-    return r;
-  if (tev) {
-    static const char *const names[] = {"memset", "prep", "gemm", "resolve", "exact-fallback"};
-    t3_print_timing("match", n1, n2, tev, names, 5);
+  const int n1v = (n1 / 32) * 32, n2v = (n2 / 32) * 32;   // matching.cu:325 (quirk Q7)
+  if (!mu) {
+    if (n1 <= 0) return 0;
+    if (n2v == 0 || !match_tensor_supported()) return match_exact(s1, n1, s2, n2, st);
+  } else if (n1v == 0 || n2v == 0) {
+    set_error("match_tensor: a mutual match needs 32 rows or more in each set");
+    return CS_E_ARG;
   }
-  return t3_end(ws, flags, st);
-}
-
-// Mutual match on the tensor path (needs n1v = 32*floor(n1/32) > 0 and n2v > 0): set 1's five match fields exactly as
-// match_tensor(s1, n1, s2, n2) writes them, set 2's exactly as match_tensor(s2, n2, s1, n1), then the cross-checked
-// pairs (launch_mutual_pairs).  One prep launch converts each set once for both of its roles (T3PrepSet); each
-// direction then runs the single-direction kernels on its own plan and its own view of the workspace.  The top-3
-// tables and the fallback row list are shared: the two directions are stream-ordered.
-int match_tensor_mutual(SiftPoint *s1, int n1, SiftPoint *s2, int n2, float minScore, float maxAmbiguity, int2 *pairs,
-                        int maxPairs, cudaStream_t st)
-{
-  const int n1v = (n1 / 32) * 32, n2v = (n2 / 32) * 32;
-  if (n1v == 0 || n2v == 0) { set_error("match_tensor_mutual: both sets need 32 rows or more"); return CS_E_ARG; }
   int dev = 0;
   cudaGetDevice(&dev);
   T3Workspace &ws = g_ws3[dev & 15];
   const int sms = t3_sms();
-  const TcPlan pf = t3_plan(n1, n2v, sms), pr = t3_plan(n2, n1v, sms);
-  // a set needs its own B-role copy when its tail rows [nv, n) lie in a tile that the B role reads
-  const bool copy1 = n1 != n1v && n1v % T3_N != 0, copy2 = n2 != n2v && n2v % T3_N != 0;
-  const size_t bBytes1 = copy1 ? (size_t)pr.n_nt * T3_B_BYTES : 0, bBytes2 = copy2 ? (size_t)pf.n_nt * T3_B_BYTES : 0;
-  const size_t pad1 = (size_t)pf.n_mt * T3_MT, pad2 = (size_t)pr.n_mt * T3_MT;
+  const TcPlan pf = t3_plan(n1, n2v, sms), pr = mu ? t3_plan(n2, n1v, sms) : TcPlan{};
+  // set 1 has the A role, set 2 the B role; in a mutual match each set has both.  Workspace: the sets' tiles one after
+  // the other in a16 (their norms likewise in normA, set 2's unread in a one-way match), the B-role copies in b16.
+  T3PrepSet p[2] = {{s1, n1, mu ? n1v : 0}, {s2, mu ? n2 : n2v, n2v}};
+  size_t aOff[2], bOff[2], nOff[2], aBytes = 0, bBytes = 0, rows = 0;
+  bool copy[2];
+  for (int k = 0; k < 2; k++) {
+    const int tiles = idivup(p[k].n, T3_MT);
+    p[k].blocks = tiles * (T3_MT / 32);
+    p[k].bTiles = idivup(p[k].nv, T3_N);
+    aOff[k] = aBytes; aBytes += (size_t)tiles * T3_A_BYTES;
+    nOff[k] = rows; rows += (size_t)tiles * T3_MT;
+    // a set needs its own B-role copy when its tail rows [nv, n) lie in a tile that the B role reads
+    copy[k] = p[k].n != p[k].nv && p[k].nv % T3_N != 0;
+    bOff[k] = bBytes; bBytes += copy[k] ? (size_t)p[k].bTiles * T3_B_BYTES : 0;
+  }
   const size_t slots = t3_slots(pf) > t3_slots(pr) ? t3_slots(pf) : t3_slots(pr);
   float *flags = nullptr, *nextFlags = nullptr;
   int r;
-  if ((r = t3_begin(ws, (pad1 + pad2) / T3_MT * T3_A_BYTES, bBytes1 + bBytes2, pad1 + pad2, slots,
-                    pad1 > pad2 ? pad1 : pad2, st, &flags, &nextFlags)) < 0)
+  if ((r = t3_begin(ws, aBytes, bBytes, rows, slots, (size_t)(pf.n_mt > pr.n_mt ? pf.n_mt : pr.n_mt) * T3_MT, st,
+                    &flags, &nextFlags)) < 0)
     return r;
   auto at = [](__half *p, size_t bytes) { return reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(p) + bytes); };
-  // workspace: A tiles of set 1 then of set 2, B-role copies likewise; flags [0] / [2] take the candidates' max norm
-  // of the forward / reverse direction, i.e. of set 2 / set 1
-  T3PrepSet p1, p2;
-  p1.pts = s1; p1.n = n1; p1.nv = n1v; p1.blocks = pf.n_mt * (T3_MT / 32);
-  p1.a = ws.bf.a16; p1.b = copy1 ? ws.bf.b16 : nullptr; p1.bTiles = pr.n_nt;
-  p1.norms = ws.bf.normA; p1.bmax = flags + 2;
-  p2.pts = s2; p2.n = n2; p2.nv = n2v; p2.blocks = pr.n_mt * (T3_MT / 32);
-  p2.a = at(ws.bf.a16, pad1 / T3_MT * T3_A_BYTES); p2.b = copy2 ? at(ws.bf.b16, bBytes1) : nullptr; p2.bTiles = pf.n_nt;
-  p2.norms = ws.bf.normA + pad1; p2.bmax = flags;
+  for (int k = 0; k < 2; k++) {
+    p[k].a = at(ws.bf.a16, aOff[k]);
+    p[k].b = copy[k] ? at(ws.bf.b16, bOff[k]) : nullptr;
+    p[k].norms = ws.bf.normA + nOff[k];
+  }
+  // flags [0] / [2] take the candidates' max norm of the forward / reverse direction, i.e. of set 2 / set 1
+  p[0].bmax = flags + 2; p[1].bmax = flags;
   T3Buffers fw = ws.bf, rv = ws.bf;
-  fw.a16 = p1.a; fw.b16 = copy2 ? p2.b : p2.a; fw.normA = p1.norms;
+  fw.a16 = p[0].a; fw.b16 = copy[1] ? p[1].b : p[1].a; fw.normA = p[0].norms;
   fw.bmax = flags; fw.counters = reinterpret_cast<unsigned int *>(flags) + 4;
-  rv.a16 = p2.a; rv.b16 = copy1 ? p1.b : p1.a; rv.normA = p2.norms;
+  rv.a16 = p[1].a; rv.b16 = copy[0] ? p[0].b : p[0].a; rv.normA = p[1].norms;
   rv.bmax = flags + 2; rv.counters = reinterpret_cast<unsigned int *>(flags) + 8;
   const unsigned int *gate = reinterpret_cast<const unsigned int *>(flags) + 1;   // shared: any bad value, either set
   cudaEvent_t *tev = t3_timing_events();
   if (tev) cudaEventRecord(tev[0], st);
-  t3_prep_pair_kernel<<<p1.blocks + p2.blocks, 512, 0, st>>>(p1, p2, flags + 1, nextFlags);
+  t3_prep_kernel<<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], flags + 1, nextFlags);
   count_launch();
   CS_CUDA(cudaGetLastError());
   if (tev) cudaEventRecord(tev[1], st);
   if ((r = t3_direction(pf, fw, s1, n1, s2, n2, gate, st, tev ? tev + 2 : nullptr)) < 0) return r;
-  if ((r = t3_direction(pr, rv, s2, n2, s1, n1, gate, st, tev ? tev + 5 : nullptr)) < 0) return r;
-  if ((r = launch_mutual_pairs(s1, n1, s2, n2, minScore, maxAmbiguity, pairs, maxPairs, st)) < 0) return r;
+  if (mu) {
+    if ((r = t3_direction(pr, rv, s2, n2, s1, n1, gate, st, tev ? tev + 5 : nullptr)) < 0) return r;
+    if ((r = launch_mutual_pairs(s1, n1, s2, n2, *mu, st)) < 0) return r;
+    if (tev) cudaEventRecord(tev[8], st);
+  }
   if (tev) {
-    cudaEventRecord(tev[8], st);
     static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
                                         "reverse-exact-fallback", "pairs"};
-    t3_print_timing("mutual", n1, n2, tev, names, 8);
+    t3_print_timing(mu ? "mutual" : "match", n1, n2, tev, names, mu ? 8 : 4);
   }
   return t3_end(ws, flags, st);
 }
 
-// statistics of the last match_tensor / match_tensor_mutual on this device (call after the stream was synchronized);
+// statistics of the last match_tensor on this device (call after the stream was synchronized);
 // a mutual call reports both directions summed
 void match_tensor_stats(unsigned long long stats[4])
 {
