@@ -15,7 +15,8 @@ from . import build as _build
 
 __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData", "InitSiftData", "FreeSiftData",
            "AllocSiftTempMemory", "FreeSiftTempMemory", "ExtractSift", "MatchSiftData", "FindHomography", "Extractor",
-           "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host"]
+           "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host",
+           "match_knn2", "MatchSiftDataRatio", "match_ratio_host"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -64,6 +65,9 @@ def lib():
         "cs_match_stats": (ip, [c.POINTER(c.c_ulonglong)]),
         "cs_match_mutual": (ip, [vp, ip, vp, ip, fp, fp, vp, ip, ip, c.POINTER(c.c_double)]),
         "cs_match_mutual_host": (ip, [vp, ip, vp, ip, fp, fp, vp, ip, ip, c.POINTER(c.c_double)]),
+        "cs_match_knn2": (ip, [vp, ip, vp, ip, vp, vp, ip, c.POINTER(c.c_double)]),
+        "cs_match_ratio": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, ip, ip, c.POINTER(c.c_double)]),
+        "cs_match_ratio_host": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, ip, ip, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -277,6 +281,61 @@ def MatchSiftDataMutual(data1, data2, minScore=0.0, maxAmbiguity=float("inf"), m
             for f in MATCH_FIELDS:
                 d.h_data[f][:n] = recs[f]
     return pairs, ms.value
+
+
+def match_knn2(s1, s2, mode=0):
+    """The two nearest neighbours of every row of s1 among all rows of s2 (cs_match_knn2), on host record arrays.
+    Returns (idx int32 [n1, 2], score float32 [n1, 2], ms): j1 is the lowest index with the largest positive score, j2
+    the lowest other index with the largest remaining one; a missing neighbour is (-1, 0.0).  The records are only read."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    n1, n2 = len(s1), len(s2)
+    idx, score = np.full((n1, 2), -1, np.int32), np.zeros((n1, 2), np.float32)
+    ms = ctypes.c_double(0.0)
+    if n1 == 0 or n2 == 0:                   # no neighbours: nothing to compute
+        return idx, score, ms.value
+    bufs = [DeviceBuffer(s1.nbytes), DeviceBuffer(s2.nbytes), DeviceBuffer(idx.nbytes), DeviceBuffer(score.nbytes)]
+    try:
+        bufs[0].upload(s1)
+        bufs[1].upload(s2)
+        _check(lib().cs_match_knn2(bufs[0].ptr, n1, bufs[1].ptr, n2, bufs[2].ptr, bufs[3].ptr, int(mode), ctypes.byref(ms)),
+               "cs_match_knn2")
+        idx = bufs[2].download(np.int32, 2 * n1).reshape(n1, 2)
+        score = bufs[3].download(np.float32, 2 * n1).reshape(n1, 2)
+    finally:
+        for b in bufs:
+            b.free()
+    return idx, score, ms.value
+
+
+def MatchSiftDataRatio(data1, data2, maxRatio=0.8, maxDistance=0.7, crossCheck=True, mode=0):
+    """Lowe's ratio test on the true two nearest neighbours (cs_match_ratio; the defaults are COLMAP's).  Returns
+    (pairs, ms): int32 [k, 2] rows (i, j), data1 row i matched to data2 row j, in increasing i.  The records are only
+    read."""
+    n1, n2 = data1.numPts, data2.numPts
+    room = min(n1, n2) if crossCheck else n1
+    ms = ctypes.c_double(0.0)
+    d_pairs = DeviceBuffer(max(room, 1) * 8)
+    try:
+        k = _check(lib().cs_match_ratio(data1.d_data, n1, data2.d_data, n2, float(maxRatio), float(maxDistance),
+                                        int(bool(crossCheck)), d_pairs.ptr if room else None, room, int(mode),
+                                        ctypes.byref(ms)), "MatchSiftDataRatio")
+        pairs = d_pairs.download(np.int32, 2 * k).reshape(k, 2) if k else np.zeros((0, 2), np.int32)
+    finally:
+        d_pairs.free()
+    return pairs, ms.value
+
+
+def match_ratio_host(s1, s2, maxRatio=0.8, maxDistance=0.7, crossCheck=True, mode=0):
+    """MatchSiftDataRatio on host record arrays (cs_match_ratio_host); returns (pairs[k, 2] int32, ms)."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    pairs = np.zeros((min(len(s1), len(s2)) if crossCheck else len(s1), 2), np.int32)
+    ms = ctypes.c_double(0.0)
+    k = _check(lib().cs_match_ratio_host(_ptr(s1), len(s1), _ptr(s2), len(s2), float(maxRatio), float(maxDistance),
+                                         int(bool(crossCheck)), _ptr(pairs), len(pairs), int(mode), ctypes.byref(ms)),
+               "cs_match_ratio_host")
+    return pairs[:k].copy(), ms.value
 
 
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):

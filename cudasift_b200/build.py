@@ -25,7 +25,7 @@ REF_DIR = os.path.join(ORACLE_DIR, "_ref")
 REF_LIB = os.path.join(REF_DIR, "libcudasift_ref.so")
 
 SOURCES = ["api.cu", "pipeline2.cu", "pyramid.cu", "pyramid2.cu", "detect.cu", "detect2.cu", "cap32.cu", "describe.cu",
-           "match.cu", "match_tc.cu", "match_mutual.cu", "homography.cu", "geom.cu", "rank.cu"]
+           "match.cu", "match_tc.cu", "match_mutual.cu", "match_knn.cu", "homography.cu", "geom.cu", "rank.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared"]
 
@@ -102,6 +102,24 @@ def build_oracle(force=False):
     return ORACLE_LIB
 
 
+KNN_ORACLE_SRC = os.path.join(ROOT, "tests", "knn_oracle.c")
+KNN_ORACLE_LIB = os.path.join(LIBDIR, "libknn_oracle.so")
+
+
+def build_knn_oracle(force=False):
+    """tests/knn_oracle.c: the CPU statement of the two-nearest-neighbour search (test infrastructure)."""
+    if not force and _newer(KNN_ORACLE_LIB, [KNN_ORACLE_SRC]):
+        return KNN_ORACLE_LIB
+    if shutil.which("gcc") is None:
+        if os.path.exists(KNN_ORACLE_LIB):
+            return KNN_ORACLE_LIB
+        raise RuntimeError("gcc not found and no prebuilt libknn_oracle.so")
+    os.makedirs(LIBDIR, exist_ok=True)
+    _run(["gcc", "-O2", "-mfma", "-ffp-contract=off", "-fPIC", "-shared", "-o", KNN_ORACLE_LIB, KNN_ORACLE_SRC, "-lm",
+          "-lpthread"])
+    return KNN_ORACLE_LIB
+
+
 def build_reference(force=False):
     """The unmodified reference in oracle/_ref/ (recipe: oracle/build_reference.py)."""
     sys.path.insert(0, ROOT)
@@ -133,6 +151,7 @@ def build_all(force=False, verbose=False):
     out = build_library(force, verbose), build_oracle(force), build_reference(force), build_demo(force)
     build_library(force, verbose, managed=True)
     build_demo(force, managed=True)
+    build_knn_oracle(force)
     return out
 
 

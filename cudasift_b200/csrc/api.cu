@@ -287,8 +287,9 @@ struct DeviceCtx {
   unsigned int *h_counters = nullptr;      // pinned
   unsigned long long matchStats[4] = {0, 0, 0, 0};
   // scratch for *_host entry points
-  void *scratch[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // 4: cs_rank_records, 5: mutual pairs
-  size_t scratchBytes[6] = {0, 0, 0, 0, 0, 0};
+  // 4: cs_rank_records, 5: mutual / ratio pairs, 6: the knn lists of cs_match_ratio
+  void *scratch[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  size_t scratchBytes[7] = {0, 0, 0, 0, 0, 0, 0};
 
   int ensure(int d)
   {
@@ -486,6 +487,100 @@ static int mutual_args(const char *fn, const void *s1, int n1, const void *s2, i
   }
   if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
   return 0;
+}
+
+// The two nearest neighbours of set 1's rows in set 2 (idx1 / score1, [n1][2]); with idx2 also those of set 2's rows in
+// set 1; with ra then the ratio-test pairs, cross-checked when idx2 is given, and the call returns their number.  The
+// records are only read.  Path rule: the tensor path when asked for (mode 2) or automatically for 256 x 256 and more.
+static int knn_sync(const char *fn, const SiftPoint *d_s1, int n1, const SiftPoint *d_s2, int n2, int *idx1, float *score1,
+                    int *idx2, float *score2, const RatioArgs *ra, int mode, double *ms)
+{
+  int err = 0;
+  if (ms) *ms = 0.0;
+  if (n1 <= 0 || n2 <= 0) return 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const bool tensor = match_tensor_supported() && (mode == 2 || (mode == 0 && n1 >= 256 && n2 >= 256));
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  cudaEventRecord(e0, c->stream);
+  int r;
+  if (tensor) {
+    r = match_knn_tensor(d_s1, n1, d_s2, n2, idx1, score1, idx2, score2, c->stream);
+  } else {
+    r = knn_exact(d_s1, n1, d_s2, n2, idx1, score1, c->stream);
+    if (idx2 && r >= 0) r = knn_exact(d_s2, n2, d_s1, n1, idx2, score2, c->stream);
+  }
+  if (ra && r >= 0) r = launch_ratio_pairs(idx1, score1, n1, idx2, score2, n2, *ra, c->stream);
+  if (r >= 0) {
+    cudaEventRecord(e1, c->stream);
+    cudaError_t ce = cudaStreamSynchronize(c->stream);
+    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
+  }
+  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }
+  float t = 0; cudaEventElapsedTime(&t, e0, e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
+  if (tensor) match_tensor_stats(c->matchStats);                           // both directions summed
+  c->matchStats[3] = tensor ? 2 : 1;
+  if (ms) *ms = t;
+  return ra ? mutual_pairs_total() : 0;
+}
+
+// [a, a + na) and [b, b + nb) share a byte
+static bool ranges_overlap(const void *a, size_t na, const void *b, size_t nb)
+{
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return na > 0 && nb > 0 && x < y + nb && y < x + na;
+}
+
+// Argument checks of the knn and ratio matchers, before any CUDA call.  out[k] (outBytes[k] bytes) are the output
+// buffers: 8-byte aligned, outside both record ranges and apart from each other.
+static int knn_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *const *out,
+                    const size_t *outBytes, int nout, int mode, const float *thresholds)
+{
+  const char *bad = nullptr;
+  const size_t r1 = n1 > 0 ? (size_t)n1 * sizeof(SiftPoint) : 0, r2 = n2 > 0 ? (size_t)n2 * sizeof(SiftPoint) : 0;
+  if (n1 < 0 || n2 < 0) bad = "n1 and n2 must be >= 0";
+  else if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) bad = "a set with records needs a pointer";
+  else if (mode < 0 || mode > 2) bad = "mode must be 0 (auto), 1 (exact) or 2 (tensor)";
+  else if (thresholds && (std::isnan(thresholds[0]) || std::isnan(thresholds[1]))) bad = "maxRatio and maxDistance must not be NaN";
+  for (int k = 0; k < nout && !bad; k++) {
+    if (outBytes[k] == 0) continue;
+    if ((reinterpret_cast<uintptr_t>(out[k]) & 7) != 0) bad = "output buffers must be 8-byte aligned";
+    else if (ranges_overlap(out[k], outBytes[k], s1, r1) || ranges_overlap(out[k], outBytes[k], s2, r2))
+      bad = "an output buffer overlaps a record range";
+    for (int m = 0; m < k && !bad; m++)
+      if (ranges_overlap(out[k], outBytes[k], out[m], outBytes[m])) bad = "the output buffers overlap";
+  }
+  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
+  return 0;
+}
+
+static int ratio_args(const char *fn, const void *s1, int n1, const void *s2, int n2, float maxRatio, float maxDistance,
+                      const void *pairs, int maxPairs, int mode)
+{
+  const char *bad = nullptr;
+  if (maxPairs < 0) bad = "maxPairs must be >= 0";
+  else if (maxPairs > 0 && !pairs) bad = "maxPairs > 0 needs a pairs buffer";
+  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
+  const void *out[1] = {pairs};
+  const size_t bytes[1] = {(size_t)maxPairs * 2 * sizeof(int)};
+  const float th[2] = {maxRatio, maxDistance};
+  return knn_args(fn, s1, n1, s2, n2, out, bytes, 1, mode, th);
+}
+
+// cs_match_ratio on device sets: the knn lists of both directions in the context's scratch.
+static int ratio_device(const char *fn, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, DeviceCtx *c,
+                        const RatioArgs &ra, bool crossCheck, int mode, double *ms)
+{
+  const size_t a = ialignup(2 * n1, 64), b = crossCheck ? ialignup(2 * n2, 64) : 0;
+  void *w = nullptr;
+  int r;
+  if ((r = c->get_scratch(6, (2 * a + 2 * b) * sizeof(int), &w)) < 0) return r;
+  int *idx1 = static_cast<int *>(w), *idx2 = crossCheck ? idx1 + 2 * a : nullptr;
+  float *sc1 = reinterpret_cast<float *>(idx1 + a), *sc2 = crossCheck ? reinterpret_cast<float *>(idx2 + b) : nullptr;
+  return knn_sync(fn, d1, n1, d2, n2, idx1, sc1, idx2, sc2, &ra, mode, ms);
 }
 
 }  // namespace cs
@@ -930,6 +1025,60 @@ int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore,
   const MutualArgs mu = {minScore, maxAmbiguity, (int2 *)dp, room};
   const int total = match_sync("cs_match_mutual", (SiftPoint *)d1, n1, (SiftPoint *)d2, n2, &mu, mode, (SiftPoint *)h_s1,
                                (SiftPoint *)h_s2, ms);
+  if (total < 0) return total;
+  const int k = total < room ? total : room;
+  if (k > 0) CS_CUDA(cudaMemcpy(h_pairs, dp, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
+  return total;
+}
+
+int cs_match_knn2(const void *d_s1, int n1, const void *d_s2, int n2, int *d_idx, float *d_score, int mode, double *ms)
+{
+  if (ms) *ms = 0.0;
+  const char *fn = "cs_match_knn2";
+  if (n1 > 0 && (!d_idx || !d_score)) {
+    set_error("%s: invalid argument (CS_E_ARG): n1 > 0 needs idx and score buffers", fn);
+    return CS_E_ARG;
+  }
+  const void *out[2] = {d_idx, d_score};
+  const size_t bytes[2] = {n1 > 0 ? (size_t)n1 * 2 * sizeof(int) : 0, n1 > 0 ? (size_t)n1 * 2 * sizeof(float) : 0};
+  int r = knn_args(fn, d_s1, n1, d_s2, n2, out, bytes, 2, mode, nullptr);
+  if (r < 0) return r;
+  return knn_sync(fn, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_idx, d_score, nullptr, nullptr, nullptr,
+                  mode, ms);
+}
+
+int cs_match_ratio(const void *d_s1, int n1, const void *d_s2, int n2, float maxRatio, float maxDistance, int crossCheck,
+                   int *d_pairs, int maxPairs, int mode, double *ms)
+{
+  if (ms) *ms = 0.0;
+  int r = ratio_args("cs_match_ratio", d_s1, n1, d_s2, n2, maxRatio, maxDistance, d_pairs, maxPairs, mode);
+  if (r < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const RatioArgs ra = {maxRatio, maxDistance, (int2 *)d_pairs, maxPairs};
+  return ratio_device("cs_match_ratio", (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, c, ra, crossCheck != 0,
+                      mode, ms);
+}
+
+int cs_match_ratio_host(const void *h_s1, int n1, const void *h_s2, int n2, float maxRatio, float maxDistance,
+                        int crossCheck, int *h_pairs, int maxPairs, int mode, double *ms)
+{
+  if (ms) *ms = 0.0;
+  int r = ratio_args("cs_match_ratio_host", h_s1, n1, h_s2, n2, maxRatio, maxDistance, h_pairs, maxPairs, mode);
+  if (r < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const int room = maxPairs < n1 ? maxPairs : n1;                      // at most one pair per row of set 1
+  void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
+  if ((r = c->get_scratch(5, (size_t)(room > 0 ? room : 1) * sizeof(int2), &dp)) < 0) return r;
+  if ((r = upload_sets(c, h_s1, n1, h_s2, n2, &d1, &d2)) < 0) return r;
+  const RatioArgs ra = {maxRatio, maxDistance, (int2 *)dp, room};
+  const int total = ratio_device("cs_match_ratio_host", (const SiftPoint *)d1, n1, (const SiftPoint *)d2, n2, c, ra,
+                                 crossCheck != 0, mode, ms);
   if (total < 0) return total;
   const int k = total < room ? total : room;
   if (k > 0) CS_CUDA(cudaMemcpy(h_pairs, dp, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));

@@ -206,6 +206,20 @@ void match_tensor_stats(unsigned long long stats[4]);   // after a synchronize
 // cross-check of two finished directions (match_mutual.cu); the total is read by mutual_pairs_total() after a synchronize
 int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu, cudaStream_t st);
 int mutual_pairs_total();
+// two nearest neighbours among all candidates (match_knn.cu states the order): idx / score are [n1][2], 8-byte aligned
+int knn_exact(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, cudaStream_t st);
+// tensor path of the same; with idx2 also set 2 against set 1 (match_tc.cu)
+int match_knn_tensor(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx1, float *score1, int *idx2,
+                     float *score2, cudaStream_t st);
+// Lowe's ratio test (COLMAP's rule) on finished knn lists, cross-checked when idx2 != nullptr; the total is read by
+// mutual_pairs_total() after a synchronize
+struct RatioArgs {
+  float maxRatio, maxDistance;
+  int2 *pairs;
+  int maxPairs;
+};
+int launch_ratio_pairs(const int *idx1, const float *score1, int n1, const int *idx2, const float *score2, int n2,
+                       const RatioArgs &ra, cudaStream_t st);
 
 inline int idivup(int a, int b) { return (a + b - 1) / b; }
 inline int ialignup(int a, int b) { return (a % b != 0) ? (a - a % b + b) : a; }

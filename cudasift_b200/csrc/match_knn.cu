@@ -1,0 +1,232 @@
+// match_knn.cu -- exact FP32 two-nearest-neighbour search (the exact path of cs_match_knn2 / cs_match_ratio).
+//
+// Semantics: score(i, j) is the reference's score, the sequential k = 0..127 FMA chain starting from 0 (the same value
+// MatchSiftData writes).  For every row i of set 1 all n2 candidates are visited (no quirk Q7 tail) and only scores
+// > 0 count.  The two neighbours are the first two candidates in the total order (score descending, index ascending):
+// j1 is the lowest index with the largest score, j2 the lowest index != j1 with the largest remaining score (it may
+// equal score1).  A missing neighbour is index -1 with score 0.  This is COLMAP's brute-force loop (strict '>' in
+// increasing j) with the second index kept as well.
+//
+// knn_exact_kernel is tiled like match_exact_kernel (32 rows x 32 candidates per step, 128 threads) and keeps top-2
+// state per (row, thread); the candidate range is split over gridDim.y slices so that a handful of rows does not scan
+// thousands of candidates in one CTA.  With more than one slice every slice writes its top two to a partial area and
+// knn_merge_kernel combines them.  The merge key is a total order, so the result does not depend on the slicing.
+#include "common.cuh"
+
+namespace cs {
+
+#define KX_ROWS 32          // rows of set 1 per CTA
+#define KX_COLS 32          // candidates of set 2 per step
+#define KX_LD 33            // row stride in float4 (+1 float4 padding: conflict-free LDS.128)
+#define KX_THREADS 128
+#define KX_MIN_STEPS 4      // candidate steps per slice at least (128 candidates)
+#define KX_MAX_SLICES 128
+
+// (s, j) comes before (t, k) in the neighbour order: larger score first, then the lower index.  The empty entry
+// (0, -1) comes after every positive score and before every other one, so non-positive scores never enter.
+__device__ __forceinline__ bool knn_before(float s, int j, float t, int k) { return s > t || (s == t && j < k); }
+
+struct Top2 {
+  float s1, s2;
+  int j1, j2;
+};
+__device__ __forceinline__ void top2_init(Top2 &t) { t.s1 = t.s2 = 0.0f; t.j1 = t.j2 = -1; }
+__device__ __forceinline__ void top2_insert(Top2 &t, float s, int j)
+{
+  if (knn_before(s, j, t.s1, t.j1)) { t.s2 = t.s1; t.j2 = t.j1; t.s1 = s; t.j1 = j; }
+  else if (knn_before(s, j, t.s2, t.j2)) { t.s2 = s; t.j2 = j; }
+}
+
+// rows == nullptr: rows [32*b, +32) of set 1, b grid-strided; otherwise entries [32*b, +32) of the row list (*nrows
+// entries).  gate != nullptr: *gate != 0 scans every row, else only the listed ones (the tensor path's fallback).
+// part == nullptr: one slice, the results go to idx / score; otherwise slice y writes part[(y * rowsCap + entry)].
+__global__ void __launch_bounds__(KX_THREADS)
+knn_exact_kernel(const SiftPoint *__restrict__ sift1, const SiftPoint *__restrict__ sift2, int n1, int n2,
+                 const int *__restrict__ rows, const unsigned int *__restrict__ nrows, const unsigned int *__restrict__ gate,
+                 int2 *__restrict__ idx, float2 *__restrict__ score, Top2 *__restrict__ part, int rowsCap)
+{
+  if (gate) {
+    if (*gate != 0) rows = nullptr;
+    else if (!rows) return;
+  }
+  __shared__ float4 s_a[KX_ROWS * KX_LD];
+  __shared__ float4 s_b[KX_COLS * KX_LD];
+  const int tid = threadIdx.x;
+  const int rq = tid & 15;       // rows rq and rq+16 of the CTA's 32
+  const int pt = tid >> 4;       // candidates 4*pt..4*pt+3 of each step
+  if (rows) n1 = min((int)*nrows, n1);
+  const int nblk = (n2 + KX_COLS - 1) / KX_COLS;
+  const int per = (nblk + gridDim.y - 1) / gridDim.y;
+  const int b0 = blockIdx.y * per, b1 = min(nblk, b0 + per);
+  for (int bp1 = blockIdx.x * KX_ROWS; bp1 < n1; bp1 += gridDim.x * KX_ROWS) {
+    __syncthreads();
+    for (int i = tid; i < KX_ROWS * 32; i += KX_THREADS) {
+      const int r = i >> 5, d = i & 31;
+      int p1 = min(bp1 + r, n1 - 1);
+      if (rows) p1 = rows[p1];
+      s_a[r * KX_LD + d] = reinterpret_cast<const float4 *>(sift1[p1].data)[d];
+    }
+    Top2 st[2];
+    top2_init(st[0]); top2_init(st[1]);
+    for (int b = b0; b < b1; b++) {
+      __syncthreads();
+      for (int i = tid; i < KX_COLS * 32; i += KX_THREADS) {
+        const int r = i >> 5, d = i & 31, p2 = b * KX_COLS + r;
+        s_b[r * KX_LD + d] = p2 < n2 ? __ldg(reinterpret_cast<const float4 *>(sift2[p2].data) + d)
+                                     : make_float4(0.0f, 0.0f, 0.0f, 0.0f);   // zeros score 0: never a neighbour
+      }
+      __syncthreads();
+      float acc[2][4];
+#pragma unroll
+      for (int i = 0; i < 2; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) acc[i][j] = 0.0f;
+#pragma unroll 4
+      for (int d = 0; d < 32; d++) {
+        const float4 a0 = s_a[rq * KX_LD + d], a1 = s_a[(rq + 16) * KX_LD + d];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+          const float4 bv = s_b[(4 * pt + j) * KX_LD + d];
+          acc[0][j] = __fmaf_rn(a0.x, bv.x, acc[0][j]);
+          acc[0][j] = __fmaf_rn(a0.y, bv.y, acc[0][j]);
+          acc[0][j] = __fmaf_rn(a0.z, bv.z, acc[0][j]);
+          acc[0][j] = __fmaf_rn(a0.w, bv.w, acc[0][j]);
+          acc[1][j] = __fmaf_rn(a1.x, bv.x, acc[1][j]);
+          acc[1][j] = __fmaf_rn(a1.y, bv.y, acc[1][j]);
+          acc[1][j] = __fmaf_rn(a1.z, bv.z, acc[1][j]);
+          acc[1][j] = __fmaf_rn(a1.w, bv.w, acc[1][j]);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int p2 = b * KX_COLS + 4 * pt + j;
+        top2_insert(st[0], acc[0][j], p2);
+        top2_insert(st[1], acc[1][j], p2);
+      }
+    }
+    __syncthreads();
+    // publish the (row, thread) states, then one thread per row merges its eight
+    Top2 *m = reinterpret_cast<Top2 *>(s_b);
+    m[pt * KX_ROWS + rq] = st[0];
+    m[pt * KX_ROWS + rq + 16] = st[1];
+    __syncthreads();
+    const int e = bp1 + tid;
+    if (tid < KX_ROWS && e < n1) {
+      Top2 t = m[tid];
+      for (int y = 1; y < 8; y++) {
+        const Top2 o = m[y * KX_ROWS + tid];
+        top2_insert(t, o.s1, o.j1);
+        top2_insert(t, o.s2, o.j2);
+      }
+      if (part) {
+        part[(size_t)blockIdx.y * rowsCap + e] = t;
+      } else {
+        const int row = rows ? rows[e] : e;
+        idx[row] = make_int2(t.j1, t.j2);
+        score[row] = make_float2(t.s1, t.s2);
+      }
+    }
+  }
+}
+
+// One thread per entry: the slices' top two, combined.  Same row selection as knn_exact_kernel.
+__global__ void __launch_bounds__(256)
+knn_merge_kernel(int n1, const int *__restrict__ rows, const unsigned int *__restrict__ nrows,
+                 const unsigned int *__restrict__ gate, const Top2 *__restrict__ part, int rowsCap, int slices,
+                 int2 *__restrict__ idx, float2 *__restrict__ score)
+{
+  if (gate) {
+    if (*gate != 0) rows = nullptr;
+    else if (!rows) return;
+  }
+  if (rows) n1 = min((int)*nrows, n1);
+  for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n1; e += gridDim.x * blockDim.x) {
+    Top2 t = part[e];
+    for (int y = 1; y < slices; y++) {
+      const Top2 o = part[(size_t)y * rowsCap + e];
+      top2_insert(t, o.s1, o.j1);
+      top2_insert(t, o.s2, o.j2);
+    }
+    const int row = rows ? rows[e] : e;
+    idx[row] = make_int2(t.j1, t.j2);
+    score[row] = make_float2(t.s1, t.s2);
+  }
+}
+
+// Per-device partial area of the sliced scan (single-threaded per device, like the matcher's workspace).
+struct KnnWorkspace {
+  Top2 *part = nullptr;
+  size_t cap = 0;
+};
+static KnnWorkspace g_wsk[16];
+
+static int knn_sms()
+{
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms;
+}
+
+// Slices of the candidate range: enough CTAs for two per SM when the rows alone do not provide them, and at least
+// KX_MIN_STEPS candidate steps per slice.
+static int knn_slices(int rowBlocks, int n2, int sms)
+{
+  const int steps = idivup(n2, KX_COLS);
+  int s = idivup(2 * sms, rowBlocks);
+  const int most = idivup(steps, KX_MIN_STEPS);
+  if (s > most) s = most;
+  if (s > KX_MAX_SLICES) s = KX_MAX_SLICES;
+  return s < 1 ? 1 : s;
+}
+
+static int knn_launch(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, const int *rows,
+                      const unsigned int *nrows, const unsigned int *gate, int rowBlocks, int slices, cudaStream_t st)
+{
+  int dev = 0;
+  cudaGetDevice(&dev);
+  KnnWorkspace &ws = g_wsk[dev & 15];
+  int2 *i2 = reinterpret_cast<int2 *>(idx);
+  float2 *f2 = reinterpret_cast<float2 *>(score);
+  Top2 *part = nullptr;
+  if (slices > 1) {
+    const size_t bytes = (size_t)slices * n1 * sizeof(Top2);
+    if (ws.cap < bytes) {
+      if (ws.part) cudaFree(ws.part);
+      ws.part = nullptr; ws.cap = 0;
+      CS_CUDA(cudaMalloc((void **)&ws.part, bytes));
+      ws.cap = bytes;
+    }
+    part = ws.part;
+  }
+  knn_exact_kernel<<<dim3(rowBlocks, slices), KX_THREADS, 0, st>>>(s1, s2, n1, n2, rows, nrows, gate, i2, f2, part, n1);
+  count_launch();
+  if (part) {
+    const int blocks = idivup(n1, 256) < 264 ? idivup(n1, 256) : 264;
+    knn_merge_kernel<<<blocks, 256, 0, st>>>(n1, rows, nrows, gate, part, n1, slices, i2, f2);
+    count_launch();
+  }
+  CS_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Every row of set 1 (mode 1 and small sets).
+int knn_exact(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, cudaStream_t st)
+{
+  if (n1 <= 0 || n2 <= 0) return 0;
+  const int rowBlocks = idivup(n1, KX_ROWS);
+  return knn_launch(s1, n1, s2, n2, idx, score, nullptr, nullptr, nullptr, rowBlocks,
+                    knn_slices(rowBlocks, n2, knn_sms()), st);
+}
+
+// Fallback of the tensor path, decided on the device: the listed rows (usually a few, so the slices are chosen for one
+// row block), or every row if *gate != 0 (grid-strided over at most 296 row blocks).
+int knn_exact_fallback(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, const int *rows,
+                       const unsigned int *nrows, const unsigned int *gate, cudaStream_t st)
+{
+  if (n1 <= 0 || n2 <= 0) return 0;
+  const int rowBlocks = idivup(n1, KX_ROWS) < 296 ? idivup(n1, KX_ROWS) : 296;
+  return knn_launch(s1, n1, s2, n2, idx, score, rows, nrows, gate, rowBlocks, knn_slices(1, n2, knn_sms()), st);
+}
+
+}  // namespace cs

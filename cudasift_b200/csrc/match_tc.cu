@@ -17,7 +17,9 @@
 //   3. resolve   eight lanes per row: merge the segments, certify, exact k=0..127 FMA chains for the
 //                surviving candidates, the reference's per-partition update rule and 8-way merge.
 // Mutual matching uses the same prep launch to convert each set once for both of its roles, runs steps 2 and 3 and
-// the exact fallback per direction, then the cross-check (match_mutual.cu).
+// the exact fallback per direction, then the cross-check (match_mutual.cu).  Two-nearest-neighbour matching
+// (match_knn_tensor) runs the same prep and GEMM over all candidates, then knn_resolve_kernel and the exact top-2
+// fallback (match_knn.cu).
 #include "common.cuh"
 
 #include <cuda_fp16.h>
@@ -558,6 +560,173 @@ t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ s
   if (threadIdx.x == 0 && s_chains) { atomicAdd(&bf.counters[1], s_chains >> 2); atomicAdd(&bf.counters[2], s_chains); }
 }
 
+// ---- knn resolve ---------------------------------------------------------------------------------
+// The true two nearest neighbours (match_knn.cu states the order) from the same top-3 tables, all n2 candidates.
+// Per partition the merged tables give G >= S >= Th and the groups I1, I2.  T is the second largest of the 16 values
+// {G[0..7], S[0..7]}: two distinct groups have approximate maxima >= T, so two distinct candidates have exact scores
+// >= T - eps, and score2 >= T - eps.  A candidate whose group is not re-scored lies in a group below T - delta
+// (delta = 2 eps): it is either a partition's third group or lower (<= Th, certified < T - delta) or an I1 / I2 group
+// below T - delta.  Its exact score is then < T - eps <= score2, strictly, so the top two of the re-scored candidates
+// (at most 8 x 2 groups x 4 = T3_TAB) are the row's top two, ties included.  T > 2 delta keeps both clearly positive.
+struct KnnResolveSmem {
+  float4 a[T3_RW][4][33];             // the rows' own descriptors
+  float sc[T3_RW][4][T3_TAB];         // exact scores
+  int p2[T3_RW][4][T3_TAB];           // their indices
+  int grp[T3_RW][4][16];              // candidate group list
+};
+
+// neighbour order: larger score first, then the lower index; the empty entry (0, -1) is passed by positive scores only
+__device__ __forceinline__ void knn_top2_insert(float &s1, int &j1, float &s2, int &j2, float s, int j)
+{
+  if (s > s1 || (s == s1 && j < j1)) { s2 = s1; j2 = j1; s1 = s; j1 = j; }
+  else if (s > s2 || (s == s2 && j < j2)) { s2 = s; j2 = j; }
+}
+
+__global__ void __launch_bounds__(32 * T3_RW)
+knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restrict__ sift1,
+                   const SiftPoint *__restrict__ sift2, int n2, int2 *__restrict__ idx, float2 *__restrict__ score)
+{
+  __shared__ KnnResolveSmem sm;
+  __shared__ unsigned int s_chains;
+  if (threadIdx.x == 0) s_chains = 0;
+  __syncthreads();
+  const unsigned int FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int sub = lane >> 3, p = lane & 7;                   // row within the warp; partition / candidate slot
+  const int row = (blockIdx.x * T3_RW + w) * 4 + sub;
+  const bool valid = row < pl.n1;
+  const int rrow = valid ? row : pl.n1 - 1;                   // clamped: padding lanes mirror the last row
+  const int mt = rrow / T3_MT, rowInTile = rrow - mt * T3_MT;
+#pragma unroll
+  for (int j = 0; j < 4; j++) sm.a[w][sub][p + 8 * j] = __ldg(reinterpret_cast<const float4 *>(sift1[rrow].data) + p + 8 * j);
+  const float bmax = __int_as_float(*reinterpret_cast<const int *>(bf.bmax));
+  const float normA = bf.normA[rrow];
+  // merged top-3 of partition p over the segments (as t3_resolve_kernel)
+  float G = 0.0f, S = 0.0f, Th = 0.0f;
+  int I1 = -1, I2 = -1;
+  {
+    const int u0 = mt * pl.n_nt, u1 = u0 + pl.n_nt - 1;
+    const int c0 = u0 / pl.U, c1 = u1 / pl.U;
+    auto insert = [&](float v, int id) {
+      const bool t = v > G, u2 = v > S;
+      Th = fmaxf(Th, fminf(S, v));
+      I2 = u2 ? (t ? I1 : id) : I2;
+      S = fmaxf(S, fminf(G, v));
+      I1 = t ? id : I1;
+      G = fmaxf(G, v);
+    };
+    constexpr int T3_SEG = 6;
+    float v[T3_SEG][3];
+    int id[T3_SEG][2];
+#pragma unroll
+    for (int k = 0; k < T3_SEG; k++) {
+      const int c = c0 + k;
+      if (c <= c1) {
+        const int run = mt - (c * pl.U) / pl.n_nt;
+        const float *q = bf.pm + tc_slot(pl, c, run, rowInTile) * T3_PM;
+        v[k][0] = q[p]; v[k][1] = q[8 + p]; v[k][2] = q[16 + p];
+        id[k][0] = __float_as_int(q[24 + p]); id[k][1] = __float_as_int(q[32 + p]);
+      } else {
+        v[k][0] = v[k][1] = v[k][2] = 0.0f; id[k][0] = id[k][1] = -1;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < T3_SEG; k++) { insert(v[k][0], id[k][0]); insert(v[k][1], id[k][1]); insert(v[k][2], -1); }
+    for (int c = c0 + T3_SEG; c <= c1; c++) {
+      const int run = mt - (c * pl.U) / pl.n_nt;
+      const float *q = bf.pm + tc_slot(pl, c, run, rowInTile) * T3_PM;
+      insert(q[p], __float_as_int(q[24 + p])); insert(q[8 + p], __float_as_int(q[32 + p])); insert(q[16 + p], -1);
+    }
+    G *= T3_UNSCALE; S *= T3_UNSCALE; Th *= T3_UNSCALE;
+  }
+  const float delta = 2.0f * (T3_C1 * normA * bmax + T3_C2 * (normA + bmax));
+  // T = second largest of {G[0..7], S[0..7]}
+  float m1 = 0.0f, m2 = 0.0f;
+#pragma unroll
+  for (int y = 0; y < 8; y++) {
+    const float gy = __shfl_sync(FULL, G, y, 8), sy = __shfl_sync(FULL, S, y, 8);
+    m2 = fmaxf(m2, fminf(m1, gy));
+    m1 = fmaxf(m1, gy);
+    m2 = fmaxf(m2, fminf(m1, sy));
+    m1 = fmaxf(m1, sy);
+  }
+  const float T = m2;
+  const bool rowOk = (T > 2.0f * delta) && (T < 3.0e38f);
+  const float low = T - delta;
+  const bool cert = Th <= 0.0f || Th < low;
+  const bool use1 = rowOk && I1 >= 0 && G >= low;
+  const bool use2 = rowOk && I2 >= 0 && S >= low;
+  const unsigned int certMask = (__ballot_sync(FULL, cert) >> (8 * sub)) & 0xffu;
+  const bool ok = valid && rowOk && certMask == 0xffu;
+  if (valid && !ok && p == 0) {
+    const unsigned at = atomicAdd(&bf.counters[0], 1u);
+    if (at < (unsigned)pl.n_mt * T3_MT) bf.fbRows[at] = row;
+  }
+  const unsigned int b1 = (__ballot_sync(FULL, ok && use1) >> (8 * sub)) & 0xffu;
+  const unsigned int b2 = (__ballot_sync(FULL, ok && use2) >> (8 * sub)) & 0xffu;
+  const int n1g = __popc(b1), ncand = 4 * (n1g + __popc(b2));
+  if (ok && use1) sm.grp[w][sub][__popc(b1 & ((1u << p) - 1))] = I1;
+  if (ok && use2) sm.grp[w][sub][n1g + __popc(b2 & ((1u << p) - 1))] = I2;
+  __syncwarp();
+  int maxc = ncand;
+#pragma unroll
+  for (int o = 16; o >= 8; o >>= 1) maxc = max(maxc, __shfl_xor_sync(FULL, maxc, o));
+  for (int c0 = 0; c0 < maxc; c0 += 8) {
+    const int c = c0 + p;
+    if (c < ncand) {
+      const int p2 = sm.grp[w][sub][c >> 2] * 4 + (c & 3);
+      float acc = 0.0f;                 // candidates past n2 (zero rows of the last tile) score 0: never a neighbour
+      if (p2 < n2) {
+        const float4 *bp = reinterpret_cast<const float4 *>(sift2[p2].data);
+        // the reference's score: sequential k = 0..127 FMA chain starting from 0, loads pipelined as in t3_resolve_kernel
+        float4 bv[8], bn[8];
+#pragma unroll
+        for (int j = 0; j < 8; j++) bv[j] = __ldg(bp + j);
+#pragma unroll
+        for (int blk = 0; blk < 4; blk++) {
+          if (blk < 3) {
+#pragma unroll
+            for (int j = 0; j < 8; j++) bn[j] = __ldg(bp + 8 * (blk + 1) + j);
+          }
+          float4 av[8];
+#pragma unroll
+          for (int j = 0; j < 8; j++) av[j] = sm.a[w][sub][8 * blk + j];
+#pragma unroll
+          for (int j = 0; j < 8; j++) {
+            acc = __fmaf_rn(av[j].x, bv[j].x, acc);
+            acc = __fmaf_rn(av[j].y, bv[j].y, acc);
+            acc = __fmaf_rn(av[j].z, bv[j].z, acc);
+            acc = __fmaf_rn(av[j].w, bv[j].w, acc);
+          }
+#pragma unroll
+          for (int j = 0; j < 8; j++) bv[j] = bn[j];
+        }
+      }
+      sm.sc[w][sub][c] = acc;
+      sm.p2[w][sub][c] = p2;
+    }
+  }
+  __syncwarp();
+  // lane p: top two of entries p, p + 8, ...; then a butterfly over the row's eight lanes (the order is total)
+  float s1 = 0.0f, s2 = 0.0f;
+  int j1 = -1, j2 = -1;
+  for (int e = p; e < ncand; e += 8) knn_top2_insert(s1, j1, s2, j2, sm.sc[w][sub][e], sm.p2[w][sub][e]);
+#pragma unroll
+  for (int o = 1; o < 8; o <<= 1) {
+    const float t1 = __shfl_xor_sync(FULL, s1, o, 8), t2 = __shfl_xor_sync(FULL, s2, o, 8);
+    const int k1 = __shfl_xor_sync(FULL, j1, o, 8), k2 = __shfl_xor_sync(FULL, j2, o, 8);
+    knn_top2_insert(s1, j1, s2, j2, t1, k1);
+    knn_top2_insert(s1, j1, s2, j2, t2, k2);
+  }
+  if (ok && p == 0) {
+    idx[row] = make_int2(j1, j2);
+    score[row] = make_float2(s1, s2);
+    atomicAdd(&s_chains, (unsigned)ncand);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_chains) { atomicAdd(&bf.counters[1], s_chains >> 2); atomicAdd(&bf.counters[2], s_chains); }
+}
+
 // exact SIMT scan of the rows the tensor path could not certify (match.cu)
 int match_exact_fallback(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *rows, const unsigned int *nrows,
                          const unsigned int *gate, cudaStream_t st);
@@ -773,6 +942,84 @@ int match_tensor(SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs 
     static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
                                         "reverse-exact-fallback", "pairs"};
     t3_print_timing(mu ? "mutual" : "match", n1, n2, tev, names, mu ? 8 : 4);
+  }
+  return t3_end(ws, flags, st);
+}
+
+// exact two-nearest-neighbour scan of the listed rows, or of every row if *gate != 0 (match_knn.cu)
+int knn_exact_fallback(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, const int *rows,
+                       const unsigned int *nrows, const unsigned int *gate, cudaStream_t st);
+
+// One knn direction after the prep kernel: GEMM, knn resolve, exact fallback.  ev (optional): three events.
+static int knn_direction(const TcPlan &pl, const T3Buffers &bf, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2,
+                         int *idx, float *score, const unsigned int *gate, cudaStream_t st, cudaEvent_t *ev)
+{
+  t3_gemm_kernel<<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf);
+  if (ev) cudaEventRecord(ev[0], st);
+  knn_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2, n2, reinterpret_cast<int2 *>(idx),
+                                                                  reinterpret_cast<float2 *>(score));
+  if (ev) cudaEventRecord(ev[1], st);
+  count_launch(2);
+  CS_CUDA(cudaGetLastError());
+  int r;
+  if ((r = knn_exact_fallback(s1, n1, s2, n2, idx, score, bf.fbRows, bf.counters, gate, st)) < 0) return r;
+  if (ev) cudaEventRecord(ev[2], st);
+  return 0;
+}
+
+// The two nearest neighbours of every row of set 1 among all n2 candidates (idx1 / score1, [n1][2]); with idx2 also
+// those of every row of set 2 among set 1's n1 rows.  The records are only read.  Same plan, workspace, flag areas and
+// bad-input gate as match_tensor; there is no Q7 tail, so each set is prepared with n == nv: its A tiles are also the
+// other direction's B operand (rows past n are zeros, score 0, and never enter the tables).
+int match_knn_tensor(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx1, float *score1, int *idx2,
+                     float *score2, cudaStream_t st)
+{
+  if (n1 <= 0 || n2 <= 0) return 0;
+  const bool both = idx2 != nullptr;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  T3Workspace &ws = g_ws3[dev & 15];
+  const int sms = t3_sms();
+  const TcPlan pf = t3_plan(n1, n2, sms), pr = both ? t3_plan(n2, n1, sms) : TcPlan{};
+  T3PrepSet p[2] = {{s1, n1, both ? n1 : 0}, {s2, n2, n2}};
+  size_t aOff[2], nOff[2], aBytes = 0, rows = 0;
+  for (int k = 0; k < 2; k++) {
+    const int tiles = idivup(p[k].n, T3_MT);
+    p[k].blocks = tiles * (T3_MT / 32);
+    p[k].bTiles = idivup(p[k].nv, T3_N);
+    aOff[k] = aBytes; aBytes += (size_t)tiles * T3_A_BYTES;
+    nOff[k] = rows; rows += (size_t)tiles * T3_MT;
+  }
+  const size_t slots = t3_slots(pf) > t3_slots(pr) ? t3_slots(pf) : t3_slots(pr);
+  float *flags = nullptr, *nextFlags = nullptr;
+  int r;
+  if ((r = t3_begin(ws, aBytes, 0, rows, slots, (size_t)(pf.n_mt > pr.n_mt ? pf.n_mt : pr.n_mt) * T3_MT, st, &flags,
+                    &nextFlags)) < 0)
+    return r;
+  for (int k = 0; k < 2; k++) {
+    p[k].a = reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(ws.bf.a16) + aOff[k]);
+    p[k].b = nullptr;
+    p[k].norms = ws.bf.normA + nOff[k];
+  }
+  p[0].bmax = flags + 2; p[1].bmax = flags;
+  T3Buffers fw = ws.bf, rv = ws.bf;
+  fw.a16 = p[0].a; fw.b16 = p[1].a; fw.normA = p[0].norms;
+  fw.bmax = flags; fw.counters = reinterpret_cast<unsigned int *>(flags) + 4;
+  rv.a16 = p[1].a; rv.b16 = p[0].a; rv.normA = p[1].norms;
+  rv.bmax = flags + 2; rv.counters = reinterpret_cast<unsigned int *>(flags) + 8;
+  const unsigned int *gate = reinterpret_cast<const unsigned int *>(flags) + 1;
+  cudaEvent_t *tev = t3_timing_events();
+  if (tev) cudaEventRecord(tev[0], st);
+  t3_prep_kernel<<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], flags + 1, nextFlags);
+  count_launch();
+  CS_CUDA(cudaGetLastError());
+  if (tev) cudaEventRecord(tev[1], st);
+  if ((r = knn_direction(pf, fw, s1, n1, s2, n2, idx1, score1, gate, st, tev ? tev + 2 : nullptr)) < 0) return r;
+  if (both && (r = knn_direction(pr, rv, s2, n2, s1, n1, idx2, score2, gate, st, tev ? tev + 5 : nullptr)) < 0) return r;
+  if (tev) {
+    static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
+                                        "reverse-exact-fallback"};
+    t3_print_timing("knn", n1, n2, tev, names, both ? 7 : 4);
   }
   return t3_end(ws, flags, st);
 }

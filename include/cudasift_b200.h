@@ -104,6 +104,31 @@ int cs_match_mutual(void *d_s1, int n1, void *d_s2, int n2, float minScore, floa
 int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore, float maxAmbiguity,
                          int *h_pairs, int maxPairs, int mode, double *ms);
 
+/* Two nearest neighbours: for every row i of set 1, among ALL n2 rows of set 2 (no quirk Q7 tail), with the reference's
+ * score (the sequential k = 0..127 FMA chain, the value MatchSiftData writes) and only scores > 0 counted:
+ *   j1 = the lowest index with the largest score, j2 = the lowest index != j1 with the largest remaining score (it may
+ *   equal score1); a missing neighbour is index -1 with score 0.0f.
+ * d_idx[i][0..1] = {j1, j2}, d_score[i][0..1] = {score1, score2} (device, [n1][2] each, 8-byte aligned).  The records
+ * are only read, so the sets may overlap (a set against itself).  mode: 0 = auto (tensor path on sm_90 when n1 and n2
+ * are >= 256), 1 = exact FP32 SIMT path, 2 = tensor path (any size); both give the same bits.  n1 == 0 or n2 == 0
+ * returns 0 and writes nothing.  Returns 0 or CS_E_*; CS_E_ARG, before any CUDA call, for n < 0, a NULL set with
+ * n > 0, NULL idx / score with n1 > 0, mode not in {0, 1, 2}, output buffers that are not 8-byte aligned or that
+ * overlap a record range or each other.  cs_match_stats reports the call. */
+int cs_match_knn2(const void *d_s1, int n1, const void *d_s2, int n2, int *d_idx, float *d_score, int mode, double *ms);
+/* Lowe's ratio test on the two nearest neighbours (COLMAP's max_ratio / max_distance / cross_check):
+ * d = acos(min(score, 1)) in double, and (i, j1) is kept when j1 >= 0, d1 <= maxDistance and d1 < maxRatio * d2
+ * (a missing second neighbour gives d2 = pi / 2).  crossCheck != 0: also set 2 against set 1, and (i, j) is kept only
+ * if row j of set 2 passes the same test and its j1 is i (the auto mode then needs 256 rows in both sets).  Pairs are
+ * int pairs {i, j} in increasing i (with crossCheck each j at most once); the order depends only on the values.
+ * Returns the number of pairs and writes the first maxPairs (device, 8-byte aligned), or CS_E_*: CS_E_ARG as for
+ * cs_match_knn2, and for maxPairs < 0, NULL pairs with maxPairs > 0 and a NaN maxRatio or maxDistance.  The knn lists
+ * live in per-device scratch.  With crossCheck, cs_match_stats reports both directions summed. */
+int cs_match_ratio(const void *d_s1, int n1, const void *d_s2, int n2, float maxRatio, float maxDistance, int crossCheck,
+                   int *d_pairs, int maxPairs, int mode, double *ms);
+/* Same with host record arrays and a host pairs buffer. */
+int cs_match_ratio_host(const void *h_s1, int n1, const void *h_s2, int n2, float maxRatio, float maxDistance,
+                        int crossCheck, int *h_pairs, int maxPairs, int mode, double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
