@@ -16,7 +16,8 @@ from . import build as _build
 __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData", "InitSiftData", "FreeSiftData",
            "AllocSiftTempMemory", "FreeSiftTempMemory", "ExtractSift", "MatchSiftData", "FindHomography", "Extractor",
            "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host",
-           "match_knn2", "MatchSiftDataRatio", "match_ratio_host"]
+           "match_knn2", "MatchSiftDataRatio", "match_ratio_host", "VerifyPairs", "verify_pairs_host", "verify_stats",
+           "GEOM_MODELS"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -68,6 +69,11 @@ def lib():
         "cs_match_knn2": (ip, [vp, ip, vp, ip, vp, vp, ip, c.POINTER(c.c_double)]),
         "cs_match_ratio": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, ip, ip, c.POINTER(c.c_double)]),
         "cs_match_ratio_host": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, ip, ip, c.POINTER(c.c_double)]),
+        "cs_verify_pairs": (ip, [vp, ip, vp, ip, vp, ip, ip, ip, fp, c.c_ulonglong, vp, vp, ip, c.POINTER(c.c_double)]),
+        "cs_verify_pairs_host": (ip, [vp, ip, vp, ip, vp, ip, ip, ip, fp, c.c_ulonglong, vp, vp, ip,
+                                      c.POINTER(c.c_double)]),
+        "cs_verify_stats": (ip, [c.POINTER(c.c_longlong)]),
+        "cs_verify_models": (ip, [vp, ip, vp, ip, vp, ip, ip, ip, fp, c.c_ulonglong, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -336,6 +342,66 @@ def match_ratio_host(s1, s2, maxRatio=0.8, maxDistance=0.7, crossCheck=True, mod
                                          int(bool(crossCheck)), _ptr(pairs), len(pairs), int(mode), ctypes.byref(ms)),
                "cs_match_ratio_host")
     return pairs[:k].copy(), ms.value
+
+
+GEOM_MODELS = {"homography": 1, "fundamental": 2}     # CS_GEOM_HOMOGRAPHY, CS_GEOM_FUNDAMENTAL
+
+
+def _geom_model(model):
+    if isinstance(model, str):
+        if model not in GEOM_MODELS:
+            raise ValueError("model must be 'homography' or 'fundamental', not %r" % model)
+        return GEOM_MODELS[model]
+    return int(model)
+
+
+def _pair_array(pairs):
+    return np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
+
+
+def VerifyPairs(data1, data2, pairs, model="fundamental", numLoops=4096, thresh=4.0, seed=0):
+    """RANSAC verification of a correspondence list on the device (cs_verify_pairs): pairs is the int32 [k, 2] array of
+    (data1 row, data2 row) that MatchSiftDataMutual and MatchSiftDataRatio return.  model: "fundamental" (7-point) or
+    "homography" (4-point); thresh in pixels (COLMAP's max_error = 4 by default; Sampson error for F, transfer error
+    for H).  Returns (model 3x3 float64 in pixel coordinates, inliers int32 [m, 2] in input order, ms)."""
+    pairs = _pair_array(pairs)
+    k = len(pairs)
+    out = np.zeros(9, np.float64)
+    ms = ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(k, 1) * 8), DeviceBuffer(max(k, 1) * 8)]
+    try:
+        if k:
+            bufs[0].upload(pairs)
+        m = _check(lib().cs_verify_pairs(data1.d_data, data1.numPts, data2.d_data, data2.numPts, bufs[0].ptr if k else None,
+                                         k, _geom_model(model), int(numLoops), float(thresh), int(seed), _ptr(out),
+                                         bufs[1].ptr if k else None, k, ctypes.byref(ms)), "VerifyPairs")
+        inliers = bufs[1].download(np.int32, 2 * m).reshape(m, 2) if m else np.zeros((0, 2), np.int32)
+    finally:
+        for b in bufs:
+            b.free()
+    return out.reshape(3, 3), inliers, ms.value
+
+
+def verify_pairs_host(s1, s2, pairs, model="fundamental", numLoops=4096, thresh=4.0, seed=0):
+    """VerifyPairs on host record arrays (cs_verify_pairs_host); returns (model 3x3 float64, inliers [m, 2] int32, ms)."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    pairs = _pair_array(pairs)
+    out = np.zeros(9, np.float64)
+    inliers = np.zeros((len(pairs), 2), np.int32)
+    ms = ctypes.c_double(0.0)
+    m = _check(lib().cs_verify_pairs_host(_ptr(s1), len(s1), _ptr(s2), len(s2), _ptr(pairs), len(pairs),
+                                          _geom_model(model), int(numLoops), float(thresh), int(seed), _ptr(out),
+                                          _ptr(inliers), len(inliers), ctypes.byref(ms)), "cs_verify_pairs_host")
+    return out.reshape(3, 3), inliers[:m].copy(), ms.value
+
+
+def verify_stats():
+    """The last verify call: [valid pairs, invalid pairs, non-degenerate samples, models scored, winning slot
+    (sample*3 + root, -1 if none), its inlier count, refit kept (0/1), final inlier count]."""
+    out = (ctypes.c_longlong * 8)()
+    _check(lib().cs_verify_stats(out), "cs_verify_stats")
+    return list(out)
 
 
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):

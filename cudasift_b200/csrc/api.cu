@@ -287,9 +287,11 @@ struct DeviceCtx {
   unsigned int *h_counters = nullptr;      // pinned
   unsigned long long matchStats[4] = {0, 0, 0, 0};
   // scratch for *_host entry points
-  // 4: cs_rank_records, 5: mutual / ratio pairs, 6: the knn lists of cs_match_ratio
-  void *scratch[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  size_t scratchBytes[7] = {0, 0, 0, 0, 0, 0, 0};
+  // 4: cs_rank_records, 5: mutual / ratio pairs, 6: the knn lists of cs_match_ratio, 7: cs_verify_pairs
+  void *scratch[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  size_t scratchBytes[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  void *h_verify = nullptr;                // pinned: the state a verify call copies back
+  long long verifyStats[8] = {0, 0, 0, 0, -1, 0, 0, 0};
 
   int ensure(int d)
   {
@@ -581,6 +583,64 @@ static int ratio_device(const char *fn, const SiftPoint *d1, int n1, const SiftP
   int *idx1 = static_cast<int *>(w), *idx2 = crossCheck ? idx1 + 2 * a : nullptr;
   float *sc1 = reinterpret_cast<float *>(idx1 + a), *sc2 = crossCheck ? reinterpret_cast<float *>(idx2 + b) : nullptr;
   return knn_sync(fn, d1, n1, d2, n2, idx1, sc1, idx2, sc2, &ra, mode, ms);
+}
+
+// Argument checks of the verifier, before any CUDA call.  The records are only read (they may overlap each other); the
+// pair and inlier buffers are 8-byte aligned, apart from each other and from both record ranges.
+static int verify_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                       int model, int numLoops, float thresh, const double *model_out, const void *inliers, int maxInliers)
+{
+  const char *bad = nullptr;
+  if (n1 < 0 || n2 < 0) bad = "n1 and n2 must be >= 0";
+  else if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) bad = "a set with records needs a pointer";
+  else if (numPairs < 0) bad = "numPairs must be >= 0";
+  else if (numPairs > 0 && !pairs) bad = "numPairs > 0 needs a pairs buffer";
+  else if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL) bad = "model must be 1 (homography) or 2 (fundamental)";
+  else if (numLoops < 1 || numLoops > 65536) bad = "numLoops must be in [1, 65536]";
+  else if (!std::isfinite(thresh) || thresh <= 0.0f) bad = "thresh must be finite and > 0";
+  else if (!model_out) bad = "model_out must not be NULL";
+  else if (maxInliers < 0) bad = "maxInliers must be >= 0";
+  else if (maxInliers > 0 && !inliers) bad = "maxInliers > 0 needs an inliers buffer";
+  if (!bad) {
+    const size_t r1 = n1 > 0 ? (size_t)n1 * sizeof(SiftPoint) : 0, r2 = n2 > 0 ? (size_t)n2 * sizeof(SiftPoint) : 0;
+    const void *out[2] = {pairs, inliers};
+    const size_t bytes[2] = {(size_t)numPairs * 2 * sizeof(int), (size_t)maxInliers * 2 * sizeof(int)};
+    for (int k = 0; k < 2 && !bad; k++) {
+      if (bytes[k] == 0) continue;
+      if ((reinterpret_cast<uintptr_t>(out[k]) & 7) != 0) bad = "pair and inlier buffers must be 8-byte aligned";
+      else if (ranges_overlap(out[k], bytes[k], s1, r1) || ranges_overlap(out[k], bytes[k], s2, r2))
+        bad = "a pair or inlier buffer overlaps a record range";
+    }
+    if (!bad && ranges_overlap(out[0], bytes[0], out[1], bytes[1])) bad = "the pair and inlier buffers overlap";
+  }
+  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
+  return 0;
+}
+
+// cs_verify_pairs on device sets and a device pair list: the launches, one copy of the state, one synchronize.
+static int verify_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
+                       const int *pairs, int numPairs, int model, int numLoops, float thresh, unsigned long long seed,
+                       double model_out[9], int *inliers, int maxInliers, double *ms)
+{
+  void *w = nullptr;
+  int r;
+  if ((r = c->get_scratch(7, verify_scratch_bytes(numPairs, numLoops), &w)) < 0) return r;
+  if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  cudaEventRecord(e0, c->stream);
+  r = launch_verify(d1, n1, d2, n2, pairs, numPairs, model, numLoops, thresh, seed, inliers, maxInliers, w, c->h_verify,
+                    true, c->stream);
+  if (r >= 0) {
+    cudaEventRecord(e1, c->stream);
+    cudaError_t ce = cudaStreamSynchronize(c->stream);
+    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
+  }
+  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }
+  float t = 0; cudaEventElapsedTime(&t, e0, e1);
+  cudaEventDestroy(e0); cudaEventDestroy(e1);
+  if (ms) *ms = t;
+  return verify_result(c->h_verify, numPairs, model_out, c->verifyStats);
 }
 
 }  // namespace cs
@@ -1092,6 +1152,84 @@ int cs_match_stats(unsigned long long out[4])
   if (!c) return err;
   for (int i = 0; i < 4; i++) out[i] = c->matchStats[i];
   return 0;
+}
+
+int cs_verify_pairs(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs, int model,
+                    int numLoops, float thresh, unsigned long long seed, double model_out[9], int *d_inliers,
+                    int maxInliers, double *ms)
+{
+  const char *fn = "cs_verify_pairs";
+  if (ms) *ms = 0.0;
+  int r = verify_args(fn, d_s1, n1, d_s2, n2, d_pairs, numPairs, model, numLoops, thresh, model_out, d_inliers, maxInliers);
+  if (r < 0) return r;
+  for (int k = 0; k < 9; k++) model_out[k] = 0.0;
+  if (numPairs == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  return verify_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, numLoops,
+                     thresh, seed, model_out, d_inliers, maxInliers, ms);
+}
+
+int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs, int model,
+                         int numLoops, float thresh, unsigned long long seed, double model_out[9], int *h_inliers,
+                         int maxInliers, double *ms)
+{
+  const char *fn = "cs_verify_pairs_host";
+  if (ms) *ms = 0.0;
+  int r = verify_args(fn, h_s1, n1, h_s2, n2, h_pairs, numPairs, model, numLoops, thresh, model_out, h_inliers, maxInliers);
+  if (r < 0) return r;
+  for (int k = 0; k < 9; k++) model_out[k] = 0.0;
+  if (numPairs == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const int room = maxInliers < numPairs ? maxInliers : numPairs;     // no more inliers can exist
+  void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
+  if ((r = c->get_scratch(5, (size_t)(numPairs + room) * sizeof(int2), &dp)) < 0) return r;
+  if ((r = upload_sets(c, h_s1, n1 > 0 ? n1 : 0, h_s2, n2 > 0 ? n2 : 0, &d1, &d2)) < 0) return r;
+  int *pairs = static_cast<int *>(dp), *inl = pairs + 2 * (size_t)numPairs;
+  CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice, c->stream));
+  const int total = verify_sync(fn, c, (const SiftPoint *)d1, n1, (const SiftPoint *)d2, n2, pairs, numPairs, model,
+                                numLoops, thresh, seed, model_out, inl, room, ms);
+  if (total < 0) return total;
+  const int k = total < room ? total : room;
+  if (k > 0) CS_CUDA(cudaMemcpy(h_inliers, inl, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
+  return total;
+}
+
+int cs_verify_stats(long long out[8])
+{
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  for (int i = 0; i < 8; i++) out[i] = c->verifyStats[i];
+  return 0;
+}
+
+int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs, int model,
+                     int numLoops, float thresh, unsigned long long seed, double *h_models, int *h_counts,
+                     double h_norm[5])
+{
+  const char *fn = "cs_verify_models";
+  double dummy[9];
+  int r = verify_args(fn, d_s1, n1, d_s2, n2, d_pairs, numPairs, model, numLoops, thresh, dummy, nullptr, 0);
+  if (r < 0) return r;
+  if (!h_models || !h_counts || !h_norm) {
+    set_error("%s: invalid argument (CS_E_ARG): NULL output array", fn);
+    return CS_E_ARG;
+  }
+  if (numPairs == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  void *w = nullptr;
+  if ((r = c->get_scratch(7, verify_scratch_bytes(numPairs, numLoops), &w)) < 0) return r;
+  if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
+  r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, numLoops, thresh,
+                    seed, nullptr, 0, w, c->h_verify, false, c->stream);
+  if (r < 0) return r;
+  return verify_models_to_host(w, c->h_verify, numPairs, numLoops, model, h_models, h_counts, h_norm, c->stream);
 }
 
 // ---- stage-level entry points ----

@@ -221,6 +221,19 @@ struct RatioArgs {
 int launch_ratio_pairs(const int *idx1, const float *score1, int n1, const int *idx2, const float *score2, int n2,
                        const RatioArgs &ra, cudaStream_t st);
 
+// ---- geometric verification (verify.cu) -------------------------------------------------------------------------
+size_t verify_scratch_bytes(int numPairs, int numLoops);   // device scratch of one call
+size_t verify_result_bytes();                              // the state copied to the host (pinned) at the end
+// steps 1-4, and with full also 5-8 (arg-max, refit, output); ends with the state copy to h_state on the stream
+int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *pairs, int numPairs, int model,
+                  int numLoops, float thresh, unsigned long long seed, int *inliers, int maxInliers, void *scratch,
+                  void *h_state, bool full, cudaStream_t st);
+// after a full launch and a synchronize: the inlier count, the pixel model and the statistics
+int verify_result(const void *h_state, int numPairs, double model_out[9], long long stats[8]);
+// after a launch without full: every slot's pixel model, count and the normalisation (synchronizes); returns numValid
+int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
+                          double *h_models, int *h_counts, double h_norm[5], cudaStream_t st);
+
 inline int idivup(int a, int b) { return (a + b - 1) / b; }
 inline int ialignup(int a, int b) { return (a % b != 0) ? (a - a % b + b) : a; }
 

@@ -1,0 +1,841 @@
+// verify.cu -- geometric verification of a correspondence list: RANSAC for a fundamental matrix (7-point minimal solver)
+// or a homography (4-point), sampled on the device with a counter-based generator, scored in FP32 on normalised
+// coordinates, refitted once.  The rules (validity, sampler, residuals, output order) are stated in cudasift_b200.h at
+// cs_verify_pairs; tests/verify_oracle.py restates them in float64.
+//
+// Eight launches, one host synchronisation (by the caller, after the result copy):
+//   1. flags     one thread per pair: valid (indices in range, four finite coordinates); a ballot word per 32 pairs and
+//                a count per CTA of 1024 pairs.
+//   2. compact   exclusive prefix (as mutual_write_kernel) -> the valid pairs' pixel coordinates (float4 x1 y1 x2 y2) and
+//                their input index, in input order; the last CTA writes the valid count.
+//   3. norm      one CTA: centroids c1, c2 and the common Hartley scale s in double, fixed-order reductions; writes the
+//                normalised FP32 coordinates and resets the arg-max key and the counters.
+//   4. hyp       one thread per sample: draws, the minimal solver in FP64, up to 3 models (slot sample*3 + root) stored
+//                unit-norm in normalised coordinates; an empty slot holds NaN.  Zeroes its slots' inlier counts.
+//   5. score     grid (model blocks, point chunks): point tiles in shared memory, one model per thread, integer counts.
+//   6. argmax    packed atomicMax of (count << 32 | ~slot): the highest count, then the lowest slot.
+//   7. refit     one CTA: the normal matrix of the best model's inliers (fixed-order double reduction), Jacobi, rank 2 for
+//                F, re-score, keep the refit unless it has fewer inliers; the final mask (ballot words, CTA counts), the
+//                pixel model and the statistics.
+//   8. write     exclusive prefix of the final mask -> the input pairs {i, j} of the inliers, in input order.
+#include <cmath>
+#include <math_constants.h>
+
+#include "common.cuh"
+
+namespace cs {
+
+#define VP_ROWS 1024          // pairs per CTA of the flags / compact / write kernels
+#define VP_HYP_T 128          // samples per CTA of the hypothesis kernel
+#define VP_SC_T 128           // models per CTA of the scoring kernel
+#define VP_TILE 1024          // points per shared-memory tile
+#define VP_CHUNK 1024         // points per scoring CTA (one tile: more CTAs than models alone would give)
+#define VP_REFIT_T 256
+#define VP_EPS 1e-9           // smallest pivot / collinearity cross product, normalised coordinates (entries of order 1)
+#define VP_MAX_DRAWS 64
+
+struct VerifyState {
+  double c1x, c1y, c2x, c2y, s;   // normalisation: u = s * (x - c)
+  double model[9];                // the returned model, pixel coordinates
+  unsigned long long best;        // packed arg-max key; 0 = no model
+  unsigned long long samples, models;
+  long long stats[8];
+  float thr2;                     // (s * thresh)^2
+  int numValid;
+  int total;                      // final inlier count
+};
+
+// ---- shared helpers (host and device) --------------------------------------------------------------------------------
+__host__ __device__ inline unsigned long long vp_splitmix64(unsigned long long z)
+{
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__host__ __device__ inline void vp_mul33(const double *a, const double *b, double *c)
+{
+  for (int r = 0; r < 3; r++)
+    for (int k = 0; k < 3; k++) c[3 * r + k] = a[3 * r] * b[k] + a[3 * r + 1] * b[3 + k] + a[3 * r + 2] * b[6 + k];
+}
+
+// a normalised-coordinate model to pixel coordinates and its output scale: H = T2^-1 Hn T1 with H[8] = 1,
+// F = T2^T Fn T1 with unit Frobenius norm and its largest-magnitude entry (the first of equals) positive
+__host__ __device__ inline void vp_denormalise(const double *m, int model, double c1x, double c1y, double c2x, double c2y,
+                                               double s, double *out)
+{
+  const double T1[9] = {s, 0, -s * c1x, 0, s, -s * c1y, 0, 0, 1};
+  double L[9], t[9];
+  if (model == CS_GEOM_HOMOGRAPHY) {
+    const double T2i[9] = {1.0 / s, 0, c2x, 0, 1.0 / s, c2y, 0, 0, 1};
+    for (int k = 0; k < 9; k++) L[k] = T2i[k];
+  } else {
+    const double T2t[9] = {s, 0, 0, 0, s, 0, -s * c2x, -s * c2y, 1};
+    for (int k = 0; k < 9; k++) L[k] = T2t[k];
+  }
+  vp_mul33(L, m, t);
+  vp_mul33(t, T1, out);
+  if (model == CS_GEOM_HOMOGRAPHY) {
+    const double d = out[8];
+    if (d != 0.0) for (int k = 0; k < 9; k++) out[k] /= d;
+  } else {
+    double n = 0.0;
+    int big = 0;
+    for (int k = 0; k < 9; k++) {
+      n += out[k] * out[k];
+      if (fabs(out[k]) > fabs(out[big])) big = k;
+    }
+    const double f = (out[big] < 0 ? -1.0 : 1.0) / sqrt(n);
+    if (n > 0.0) for (int k = 0; k < 9; k++) out[k] *= f;
+  }
+}
+
+// Symmetric eigen-decomposition by cyclic Jacobi: a becomes diagonal, the columns of v are the eigenvectors.
+template <int N>
+__host__ __device__ inline void vp_jacobi(double (&a)[N][N], double (&v)[N][N])
+{
+  double tot = 0.0;
+  for (int p = 0; p < N; p++)
+    for (int q = 0; q < N; q++) { v[p][q] = p == q ? 1.0 : 0.0; tot += a[p][q] * a[p][q]; }
+  for (int sweep = 0; sweep < 30; sweep++) {
+    double off = 0.0;
+    for (int p = 0; p < N; p++)
+      for (int q = p + 1; q < N; q++) off += a[p][q] * a[p][q];
+    if (!(off > 1e-32 * tot)) break;
+    for (int p = 0; p < N; p++)
+      for (int q = p + 1; q < N; q++) {
+        // after three sweeps an element too small to change either diagonal entry is set to zero (Numerical Recipes'
+        // rule), so that the sweeps end instead of running against rounding
+        const double g = 100.0 * fabs(a[p][q]);
+        if (sweep > 2 && fabs(a[p][p]) + g == fabs(a[p][p]) && fabs(a[q][q]) + g == fabs(a[q][q])) {
+          a[p][q] = a[q][p] = 0.0;
+          continue;
+        }
+        if (a[p][q] == 0.0) continue;
+        const double th = (a[q][q] - a[p][p]) / (2.0 * a[p][q]);
+        const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < N; k++) {
+          const double kp = a[k][p], kq = a[k][q];
+          a[k][p] = c * kp - s * kq; a[k][q] = s * kp + c * kq;
+        }
+        for (int k = 0; k < N; k++) {
+          const double pk = a[p][k], qk = a[q][k];
+          a[p][k] = c * pk - s * qk; a[q][k] = s * pk + c * qk;
+        }
+        for (int k = 0; k < N; k++) {
+          const double kp = v[k][p], kq = v[k][q];
+          v[k][p] = c * kp - s * kq; v[k][q] = s * kp + c * kq;
+        }
+      }
+  }
+}
+
+// ---- device routines ----------------------------------------------------------------------------------------------
+// Null space of an M x 9 system (M = 7 or 8): Gaussian elimination with partial pivoting on columns 0..M-1, then back
+// substitution for each free column f = M..8 (x_f = 1, the other free entries 0).  false when a pivot is below VP_EPS.
+template <int M>
+__device__ bool vp_nullspace(double (&A)[M][9], double (&N)[9 - M][9])
+{
+#pragma unroll
+  for (int c = 0; c < M; c++) {
+    int p = c;
+    double best = fabs(A[c][c]);
+#pragma unroll
+    for (int r = c + 1; r < M; r++)
+      if (fabs(A[r][c]) > best) { best = fabs(A[r][c]); p = r; }
+    if (!(best >= VP_EPS)) return false;
+#pragma unroll
+    for (int r = c + 1; r < M; r++)
+      if (r == p) {
+#pragma unroll
+        for (int j = 0; j < 9; j++) { const double t = A[c][j]; A[c][j] = A[r][j]; A[r][j] = t; }
+      }
+#pragma unroll
+    for (int r = c + 1; r < M; r++) {
+      const double f = A[r][c] / A[c][c];
+#pragma unroll
+      for (int j = c; j < 9; j++) A[r][j] -= f * A[c][j];
+    }
+  }
+#pragma unroll
+  for (int f = M; f < 9; f++) {
+    double *x = N[f - M];
+#pragma unroll
+    for (int j = M; j < 9; j++) x[j] = j == f ? 1.0 : 0.0;
+#pragma unroll
+    for (int r = M - 1; r >= 0; r--) {
+      double acc = 0.0;
+#pragma unroll
+      for (int j = r + 1; j < 9; j++) acc += A[r][j] * x[j];
+      x[r] = -acc / A[r][r];
+    }
+  }
+  return true;
+}
+
+__device__ inline double vp_det3(const double *m)
+{
+  return m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
+}
+
+// Real roots of c0 + c1 a + c2 a^2 + c3 a^3 (closed form, unpolished, unordered).  A coefficient below 1e-10 of the
+// largest counts as zero from the top (cubic -> quadratic -> linear).
+__device__ int vp_cubic_roots(const double *c, double *roots)
+{
+  double cm = 0.0;
+  for (int k = 0; k < 4; k++) cm = fmax(cm, fabs(c[k]));
+  if (!(cm > 0.0)) return 0;
+  int n = 0;
+  if (fabs(c[3]) > 1e-10 * cm) {
+    const double a = c[2] / c[3], b = c[1] / c[3], d = c[0] / c[3];
+    const double p = b - a * a / 3.0, q = 2.0 * a * a * a / 27.0 - a * b / 3.0 + d;
+    const double disc = 0.25 * q * q + p * p * p / 27.0;
+    if (disc > 0.0) {
+      const double sq = sqrt(disc);
+      roots[n++] = cbrt(-0.5 * q + sq) + cbrt(-0.5 * q - sq) - a / 3.0;
+    } else if (p == 0.0) {
+      roots[n++] = -a / 3.0;
+    } else {
+      const double r = sqrt(-p / 3.0);
+      const double arg = fmin(1.0, fmax(-1.0, 1.5 * q / p * sqrt(-3.0 / p)));
+      const double phi = acos(arg);
+      for (int k = 0; k < 3; k++) roots[n++] = 2.0 * r * cos(phi / 3.0 - 2.0 * M_PI * k / 3.0) - a / 3.0;
+    }
+  } else if (fabs(c[2]) > 1e-10 * cm) {
+    const double disc = c[1] * c[1] - 4.0 * c[2] * c[0];
+    if (disc >= 0.0) {
+      const double qq = -0.5 * (c[1] + (c[1] >= 0 ? 1.0 : -1.0) * sqrt(disc));
+      roots[n++] = qq / c[2];
+      if (qq != 0.0) roots[n++] = c[0] / qq;
+    }
+  } else if (fabs(c[1]) > 1e-10 * cm) {
+    roots[n++] = -c[0] / c[1];
+  }
+  return n;
+}
+
+__device__ inline bool vp_store_unit(double *slot, const double *m)
+{
+  double n = 0.0;
+  for (int k = 0; k < 9; k++) n += m[k] * m[k];
+  if (!(n > 0.0) || !isfinite(n)) return false;
+  const double f = 1.0 / sqrt(n);
+  for (int k = 0; k < 9; k++) slot[k] = m[k] * f;
+  return true;
+}
+
+// FP32 inlier tests on normalised coordinates p = {u1, v1, u2, v2}, against thr2 = (s * thresh)^2.  The explicit fmaf
+// chain pins the arithmetic: scoring, the refit's counts and the final mask see the same bits.
+__device__ __forceinline__ bool vp_inlier(const float *m, float4 p, float thr2, bool homography)
+{
+  if (homography) {                    // |(X, Y) / w - x2|^2 < thr2, multiplied through by w^2 (no division)
+    const float w = fmaf(m[6], p.x, fmaf(m[7], p.y, m[8]));
+    const float X = fmaf(m[0], p.x, fmaf(m[1], p.y, m[2]));
+    const float Y = fmaf(m[3], p.x, fmaf(m[4], p.y, m[5]));
+    const float dx = fmaf(-p.z, w, X), dy = fmaf(-p.w, w, Y);
+    return fmaf(dx, dx, dy * dy) < thr2 * (w * w);
+  }
+  const float a0 = fmaf(m[0], p.x, fmaf(m[1], p.y, m[2]));
+  const float a1 = fmaf(m[3], p.x, fmaf(m[4], p.y, m[5]));
+  const float a2 = fmaf(m[6], p.x, fmaf(m[7], p.y, m[8]));
+  const float b0 = fmaf(m[0], p.z, fmaf(m[3], p.w, m[6]));
+  const float b1 = fmaf(m[1], p.z, fmaf(m[4], p.w, m[7]));
+  const float num = fmaf(p.z, a0, fmaf(p.w, a1, a2));
+  const float den = fmaf(a0, a0, fmaf(a1, a1, fmaf(b0, b0, b1 * b1)));
+  return num * num < thr2 * den;
+}
+
+// This thread's exclusive position among the set bits of masks (one word per 32 rows, one count per CTA of VP_ROWS
+// rows), the bit itself in *bit; the last CTA's last warp writes the total to *total when given.
+__device__ unsigned int vp_scan(const unsigned int *__restrict__ masks, const unsigned int *__restrict__ blockCounts, int n,
+                                bool *bit, int *total)
+{
+  __shared__ unsigned int s_w[32];
+  __shared__ unsigned int s_base;
+  const unsigned int FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned int part = 0;
+  for (int k = threadIdx.x; k < (int)blockIdx.x; k += VP_ROWS) part += blockCounts[k];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
+  if (lane == 0) s_w[w] = part;
+  __syncthreads();
+  if (w == 0) {
+    unsigned int v = s_w[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
+    if (lane == 0) s_base = v;
+  }
+  __syncthreads();
+  const unsigned int base = s_base;
+  const unsigned int bal = (blockIdx.x * VP_ROWS + w * 32 < n) ? masks[(blockIdx.x * VP_ROWS >> 5) + w] : 0u;
+  __syncthreads();
+  if (lane == 0) s_w[w] = __popc(bal);
+  __syncthreads();
+  if (w == 0) {
+    const unsigned int c = s_w[lane];
+    unsigned int inc = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned int t = __shfl_up_sync(FULL, inc, o);
+      if (lane >= o) inc += t;
+    }
+    s_w[lane] = inc - c;
+    if (total && lane == 31 && blockIdx.x == gridDim.x - 1) *total = (int)(base + inc);
+  }
+  __syncthreads();
+  *bit = (bal >> lane) & 1u;
+  return base + s_w[w] + __popc(bal & ((1u << lane) - 1u));
+}
+
+// ---- kernels ----------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(VP_ROWS)
+vp_flags_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__restrict__ s2, int n2,
+                const int2 *__restrict__ pairs, int numPairs, unsigned int *__restrict__ masks,
+                unsigned int *__restrict__ blockCounts)
+{
+  const int k = blockIdx.x * VP_ROWS + threadIdx.x;
+  bool keep = false;
+  if (k < numPairs) {
+    const int2 p = pairs[k];
+    if (p.x >= 0 && p.x < n1 && p.y >= 0 && p.y < n2)
+      keep = isfinite(s1[p.x].xpos) && isfinite(s1[p.x].ypos) && isfinite(s2[p.y].xpos) && isfinite(s2[p.y].ypos);
+  }
+  const unsigned int bal = __ballot_sync(0xffffffffu, keep);
+  if ((threadIdx.x & 31) == 0 && k < numPairs) masks[k >> 5] = bal;
+  const int cnt = __syncthreads_count(keep);
+  if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
+}
+
+__global__ void __launch_bounds__(VP_ROWS)
+vp_compact_kernel(const SiftPoint *__restrict__ s1, const SiftPoint *__restrict__ s2, const int2 *__restrict__ pairs,
+                  int numPairs, const unsigned int *__restrict__ masks, const unsigned int *__restrict__ blockCounts,
+                  float4 *__restrict__ xy, int *__restrict__ orig, VerifyState *st)
+{
+  bool bit;
+  const unsigned int pos = vp_scan(masks, blockCounts, numPairs, &bit, &st->numValid);
+  if (bit) {
+    const int k = blockIdx.x * VP_ROWS + threadIdx.x;
+    const int2 p = pairs[k];
+    xy[pos] = make_float4(s1[p.x].xpos, s1[p.x].ypos, s2[p.y].xpos, s2[p.y].ypos);
+    orig[pos] = k;
+  }
+}
+
+// block-wide sum of 4 doubles in a fixed order (xor butterfly per warp, then warp 0 over the warp partials)
+__device__ void vp_block_sum4(double (&v)[4], double (*s_red)[4])
+{
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int j = 0; j < 4; j++)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+  if (lane == 0)
+    for (int j = 0; j < 4; j++) s_red[w][j] = v[j];
+  __syncthreads();
+  if (w == 0) {
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      double t = lane < (int)(blockDim.x >> 5) ? s_red[lane][j] : 0.0;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+      if (lane == 0) s_red[0][j] = t;
+    }
+  }
+  __syncthreads();
+  for (int j = 0; j < 4; j++) v[j] = s_red[0][j];
+  __syncthreads();
+}
+
+__global__ void __launch_bounds__(1024)
+vp_norm_kernel(const float4 *__restrict__ xy, float4 *__restrict__ un, float thresh, VerifyState *st)
+{
+  __shared__ double s_red[32][4];
+  const int n = st->numValid;
+  double v[4] = {0, 0, 0, 0};
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    const float4 p = xy[k];
+    v[0] += p.x; v[1] += p.y; v[2] += p.z; v[3] += p.w;
+  }
+  vp_block_sum4(v, s_red);
+  const double c1x = n ? v[0] / n : 0.0, c1y = n ? v[1] / n : 0.0, c2x = n ? v[2] / n : 0.0, c2y = n ? v[3] / n : 0.0;
+  double d[4] = {0, 0, 0, 0};
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    const float4 p = xy[k];
+    d[0] += sqrt((p.x - c1x) * (p.x - c1x) + (p.y - c1y) * (p.y - c1y));
+    d[1] += sqrt((p.z - c2x) * (p.z - c2x) + (p.w - c2y) * (p.w - c2y));
+  }
+  vp_block_sum4(d, s_red);
+  const double mean = n ? (d[0] + d[1]) / (2.0 * n) : 0.0;
+  const double s = mean > 0.0 ? sqrt(2.0) / mean : 0.0;
+  for (int k = threadIdx.x; k < n; k += blockDim.x) {
+    const float4 p = xy[k];
+    un[k] = make_float4((float)((p.x - c1x) * s), (float)((p.y - c1y) * s), (float)((p.z - c2x) * s),
+                        (float)((p.w - c2y) * s));
+  }
+  if (threadIdx.x == 0) {
+    st->c1x = c1x; st->c1y = c1y; st->c2x = c2x; st->c2y = c2y; st->s = s;
+    const double t = s * (double)thresh;
+    st->thr2 = (float)(t * t);
+    st->best = 0; st->samples = 0; st->models = 0;
+  }
+}
+
+// The k distinct indices of sample smp into the n valid pairs (the rule of cs_verify_pairs); false after 64 draws.
+template <int K>
+__device__ bool vp_draw(unsigned long long seed, int smp, int n, int (&idx)[K])
+{
+  int got = 0;
+  for (int d = 0; d < VP_MAX_DRAWS && got < K; d++) {
+    const unsigned long long x = vp_splitmix64(seed + 0x9E3779B97F4A7C15ull * (((unsigned long long)smp << 8) | (unsigned)d));
+    const int i = (int)(((x >> 32) * (unsigned long long)n) >> 32);
+    bool dup = false;
+#pragma unroll
+    for (int j = 0; j < K; j++) dup |= (j < got && idx[j] == i);
+    if (dup) continue;
+#pragma unroll
+    for (int j = 0; j < K; j++) if (j == got) idx[j] = i;
+    got++;
+  }
+  return got == K;
+}
+
+__device__ inline double vp_cross(double ax, double ay, double bx, double by, double cx, double cy)
+{
+  return (bx - ax) * (cy - ay) - (by - ay) * (cx - ax);
+}
+
+__global__ void __launch_bounds__(VP_HYP_T)
+vp_hyp_kernel(const float4 *__restrict__ xy, int numLoops, int model, unsigned long long seed, double *__restrict__ models,
+              unsigned int *__restrict__ counts, const VerifyState *st)
+{
+  const int smp = blockIdx.x * VP_HYP_T + threadIdx.x;
+  if (smp >= numLoops) return;
+  double *slot = models + (size_t)smp * 27;
+  for (int r = 0; r < 3; r++) { slot[9 * r] = CUDART_NAN; counts[3 * smp + r] = 0; }
+  const int n = st->numValid;
+  const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
+  if (!(s > 0.0)) return;
+  if (model == CS_GEOM_HOMOGRAPHY) {
+    int idx[4];
+    if (n < 4 || !vp_draw<4>(seed, smp, n, idx)) return;
+    double u[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const float4 p = xy[idx[i]];
+      u[i][0] = (p.x - c1x) * s; u[i][1] = (p.y - c1y) * s; u[i][2] = (p.z - c2x) * s; u[i][3] = (p.w - c2y) * s;
+    }
+    const int tri[4][3] = {{0, 1, 2}, {0, 1, 3}, {0, 2, 3}, {1, 2, 3}};
+#pragma unroll
+    for (int t = 0; t < 4; t++)
+#pragma unroll
+      for (int im = 0; im < 2; im++) {
+        const double *a = u[tri[t][0]] + 2 * im, *b = u[tri[t][1]] + 2 * im, *c = u[tri[t][2]] + 2 * im;
+        if (!(fabs(vp_cross(a[0], a[1], b[0], b[1], c[0], c[1])) >= VP_EPS)) return;
+      }
+    double A[8][9], N[1][9];
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+      const double x = u[i][0], y = u[i][1], X = u[i][2], Y = u[i][3];
+      const double r1[9] = {x, y, 1, 0, 0, 0, -X * x, -X * y, -X}, r2[9] = {0, 0, 0, x, y, 1, -Y * x, -Y * y, -Y};
+#pragma unroll
+      for (int j = 0; j < 9; j++) { A[2 * i][j] = r1[j]; A[2 * i + 1][j] = r2[j]; }
+    }
+    if (!vp_nullspace<8>(A, N)) return;
+    vp_store_unit(slot, N[0]);
+    return;
+  }
+  int idx[7];
+  if (n < 7 || !vp_draw<7>(seed, smp, n, idx)) return;
+  double A[7][9], N[2][9];
+#pragma unroll
+  for (int i = 0; i < 7; i++) {
+    const float4 p = xy[idx[i]];
+    const double x = (p.x - c1x) * s, y = (p.y - c1y) * s, X = (p.z - c2x) * s, Y = (p.w - c2y) * s;
+    const double r[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
+#pragma unroll
+    for (int j = 0; j < 9; j++) A[i][j] = r[j];
+  }
+  if (!vp_nullspace<7>(A, N)) return;
+  // det(a F1 + (1 - a) F2) = det(F2 + a (F1 - F2)) = c0 + c1 a + c2 a^2 + c3 a^3, from its values at a = 0, 1, -1, 2
+  double D[9], M[9], p[4];
+  for (int k = 0; k < 9; k++) D[k] = N[0][k] - N[1][k];
+  const double at[4] = {0.0, 1.0, -1.0, 2.0};
+  for (int q = 0; q < 4; q++) {
+    for (int k = 0; k < 9; k++) M[k] = N[1][k] + at[q] * D[k];
+    p[q] = vp_det3(M);
+  }
+  double c[4];
+  c[0] = p[0];
+  c[2] = 0.5 * (p[1] + p[2]) - p[0];
+  const double a = 0.5 * (p[1] - p[2]), b = p[3] - p[0] - 4.0 * c[2];
+  c[3] = (b - 2.0 * a) / 6.0;
+  c[1] = a - c[3];
+  // two Newton steps per root on the determinant itself (the interpolated cubic's derivative as the slope), then
+  // ascending order
+  double roots[3];
+  const int nr = vp_cubic_roots(c, roots);
+  for (int k = 0; k < nr; k++)
+    for (int it = 0; it < 2; it++) {
+      const double x = roots[k];
+      const double d = (3.0 * c[3] * x + 2.0 * c[2]) * x + c[1];
+      if (d == 0.0) break;
+      for (int j = 0; j < 9; j++) M[j] = N[1][j] + x * D[j];
+      const double y = x - vp_det3(M) / d;
+      if (isfinite(y)) roots[k] = y;
+    }
+  for (int i = 1; i < nr; i++)
+    for (int j = i; j > 0 && roots[j] < roots[j - 1]; j--) { const double t = roots[j]; roots[j] = roots[j - 1]; roots[j - 1] = t; }
+  int r = 0;
+  for (int k = 0; k < nr; k++) {
+    for (int j = 0; j < 9; j++) M[j] = roots[k] * N[0][j] + (1.0 - roots[k]) * N[1][j];
+    if (vp_store_unit(slot + 9 * r, M)) r++;
+  }
+}
+
+// one thread per slot (F) or per sample's slot 3s (H: its only model), VP_CHUNK points per CTA
+__global__ void __launch_bounds__(VP_SC_T)
+vp_score_kernel(const float4 *__restrict__ un, const double *__restrict__ models, int numSlots, int model,
+                unsigned int *__restrict__ counts, const VerifyState *st)
+{
+  __shared__ float4 s_p[VP_TILE];
+  const int n = st->numValid;
+  const int p0 = blockIdx.y * VP_CHUNK;
+  if (p0 >= n) return;
+  const int p1 = min(n, p0 + VP_CHUNK);
+  const int slot = (blockIdx.x * VP_SC_T + threadIdx.x) * (model == CS_GEOM_HOMOGRAPHY ? 3 : 1);
+  float m[9];
+  bool live = slot < numSlots && !isnan(models[(size_t)slot * 9]);
+  if (live)
+    for (int k = 0; k < 9; k++) m[k] = (float)models[(size_t)slot * 9 + k];
+  const float thr2 = st->thr2;
+  const bool homography = model == CS_GEOM_HOMOGRAPHY;
+  unsigned int cnt = 0;
+  for (int t0 = p0; t0 < p1; t0 += VP_TILE) {
+    const int tn = min(VP_TILE, p1 - t0);
+    __syncthreads();
+    for (int k = threadIdx.x; k < tn; k += VP_SC_T) s_p[k] = un[t0 + k];
+    __syncthreads();
+    if (live)
+      for (int k = 0; k < tn; k++) cnt += vp_inlier(m, s_p[k], thr2, homography);
+  }
+  if (live && cnt) atomicAdd(&counts[slot], cnt);
+}
+
+__global__ void __launch_bounds__(256)
+vp_argmax_kernel(const double *__restrict__ models, const unsigned int *__restrict__ counts, int numSlots, VerifyState *st)
+{
+  const int slot = blockIdx.x * 256 + threadIdx.x;
+  const bool live = slot < numSlots && !isnan(models[(size_t)slot * 9]);
+  unsigned long long key = live ? ((unsigned long long)counts[slot] << 32) | (unsigned int)~slot : 0ull;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
+    key = t > key ? t : key;
+  }
+  const unsigned int nm = __popc(__ballot_sync(0xffffffffu, live));
+  const unsigned int ns = __popc(__ballot_sync(0xffffffffu, live && slot % 3 == 0));
+  if ((threadIdx.x & 31) == 0) {
+    if (key) atomicMax(&st->best, key);
+    if (nm) atomicAdd(&st->models, (unsigned long long)nm);
+    if (ns) atomicAdd(&st->samples, (unsigned long long)ns);
+  }
+}
+
+// block-wide sum of an int (fixed order; the result in every thread)
+__device__ int vp_block_count(int v, int *s_cnt)
+{
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if (lane == 0) s_cnt[w] = v;
+  __syncthreads();
+  int t = 0;
+  for (int k = 0; k < VP_REFIT_T / 32; k++) t += s_cnt[k];
+  return t;
+}
+
+__global__ void __launch_bounds__(VP_REFIT_T)
+vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, const double *__restrict__ models, int model,
+                unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts, VerifyState *st)
+{
+  __shared__ double s_nm[VP_REFIT_T / 32][45];
+  __shared__ double s_m[2][9];         // [0] minimal model, [1] refit
+  __shared__ float s_f[9];
+  __shared__ int s_cnt[VP_REFIT_T / 32];
+  __shared__ int s_refit;
+  const int n = st->numValid;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const bool homography = model == CS_GEOM_HOMOGRAPHY;
+  const unsigned long long key = st->best;
+  const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
+  const float thr2 = st->thr2;
+  const int best = key ? (int)~(unsigned int)key : -1;
+  int cnt0 = 0, cntR = 0, kept = 0;
+  if (best >= 0) {
+    if (threadIdx.x < 9) { s_m[0][threadIdx.x] = models[(size_t)best * 9 + threadIdx.x]; s_f[threadIdx.x] = (float)s_m[0][threadIdx.x]; }
+    __syncthreads();
+    float m[9];
+    for (int k = 0; k < 9; k++) m[k] = s_f[k];
+    // the normal matrix (upper triangle, 45 entries) of the minimal model's inliers
+    double acc[45];
+#pragma unroll
+    for (int k = 0; k < 45; k++) acc[k] = 0.0;
+    int c = 0;
+    for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
+      if (!vp_inlier(m, un[k], thr2, homography)) continue;
+      c++;
+      const float4 p = xy[k];
+      const double x = (p.x - c1x) * s, y = (p.y - c1y) * s, X = (p.z - c2x) * s, Y = (p.w - c2y) * s;
+      // DLT: two rows per point; 8-point: one row (the zero second row adds exact zeros)
+      double r[2][9];
+      if (homography) {
+        const double r1[9] = {x, y, 1, 0, 0, 0, -X * x, -X * y, -X}, r2[9] = {0, 0, 0, x, y, 1, -Y * x, -Y * y, -Y};
+#pragma unroll
+        for (int j = 0; j < 9; j++) { r[0][j] = r1[j]; r[1][j] = r2[j]; }
+      } else {
+        const double r1[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
+#pragma unroll
+        for (int j = 0; j < 9; j++) { r[0][j] = r1[j]; r[1][j] = 0.0; }
+      }
+#pragma unroll
+      for (int q = 0; q < 2; q++) {
+        int e = 0;
+#pragma unroll
+        for (int i = 0; i < 9; i++)
+#pragma unroll
+          for (int j = i; j < 9; j++) acc[e++] += r[q][i] * r[q][j];
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 45; e++) {
+      double v = acc[e];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) s_nm[w][e] = v;
+    }
+    cnt0 = vp_block_count(c, s_cnt);
+    if (threadIdx.x == 0) {
+      s_refit = 0;
+      if (cnt0 >= (homography ? 4 : 8)) {
+        double A[9][9], V[9][9];
+        int e = 0;
+        for (int i = 0; i < 9; i++)
+          for (int j = i; j < 9; j++) {
+            double t = 0.0;
+            for (int q = 0; q < VP_REFIT_T / 32; q++) t += s_nm[q][e];
+            A[i][j] = A[j][i] = t;
+            e++;
+          }
+        vp_jacobi<9>(A, V);
+        int lo = 0;
+        for (int i = 1; i < 9; i++) if (A[i][i] < A[lo][lo]) lo = i;
+        double f[9];
+        for (int i = 0; i < 9; i++) f[i] = V[i][lo];
+        if (!homography) {             // rank 2: F (I - v v^T), v the right singular vector of the smallest singular value
+          double B[3][3], W[3][3];
+          for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) B[i][j] = f[i] * f[j] + f[3 + i] * f[3 + j] + f[6 + i] * f[6 + j];
+          vp_jacobi<3>(B, W);
+          int l3 = 0;
+          for (int i = 1; i < 3; i++) if (B[i][i] < B[l3][l3]) l3 = i;
+          const double vv[3] = {W[0][l3], W[1][l3], W[2][l3]};
+          for (int r = 0; r < 3; r++) {
+            const double fv = f[3 * r] * vv[0] + f[3 * r + 1] * vv[1] + f[3 * r + 2] * vv[2];
+            for (int j = 0; j < 3; j++) f[3 * r + j] -= fv * vv[j];
+          }
+        }
+        if (vp_store_unit(s_m[1], f)) s_refit = 1;
+      }
+    }
+    __syncthreads();
+    if (s_refit) {
+      for (int k = 0; k < 9; k++) m[k] = (float)s_m[1][k];
+      int cr = 0;
+      for (int k = threadIdx.x; k < n; k += VP_REFIT_T) cr += vp_inlier(m, un[k], thr2, homography);
+      cntR = vp_block_count(cr, s_cnt);
+      kept = cntR >= cnt0;
+    }
+    if (!kept)
+      for (int k = 0; k < 9; k++) m[k] = s_f[k];
+    // the final mask: ballot words per 32 points, then counts per VP_ROWS points
+    for (int k0 = 0; k0 < n; k0 += VP_REFIT_T) {
+      const int k = k0 + threadIdx.x;
+      const bool in = k < n && vp_inlier(m, un[k], thr2, homography);
+      const unsigned int bal = __ballot_sync(0xffffffffu, in);
+      if (lane == 0 && k < n) masks[k >> 5] = bal;
+    }
+  } else {
+    for (int k = threadIdx.x; k < (n + 31) / 32; k += VP_REFIT_T) masks[k] = 0u;
+  }
+  __syncthreads();
+  const int words = (n + 31) / 32;
+  int tot = 0;
+  for (int b = threadIdx.x; b * (VP_ROWS / 32) < words; b += VP_REFIT_T) {
+    unsigned int t = 0;
+    for (int q = b * (VP_ROWS / 32); q < min(words, (b + 1) * (VP_ROWS / 32)); q++) t += __popc(masks[q]);
+    blockCounts[b] = t;
+    tot += (int)t;
+  }
+  tot = vp_block_count(tot, s_cnt);
+  if (threadIdx.x == 0) {
+    double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    if (best >= 0) vp_denormalise(kept ? s_m[1] : s_m[0], model, c1x, c1y, c2x, c2y, s, out);
+    for (int k = 0; k < 9; k++) st->model[k] = out[k];
+    st->total = tot;
+    st->stats[0] = n;
+    st->stats[2] = (long long)st->samples;
+    st->stats[3] = (long long)st->models;
+    st->stats[4] = best;
+    st->stats[5] = cnt0;
+    st->stats[6] = kept;
+    st->stats[7] = tot;
+  }
+}
+
+__global__ void __launch_bounds__(VP_ROWS)
+vp_write_kernel(const int2 *__restrict__ pairs, const int *__restrict__ orig, const unsigned int *__restrict__ masks,
+                const unsigned int *__restrict__ blockCounts, int2 *__restrict__ inliers, int maxInliers,
+                const VerifyState *st)
+{
+  const int n = st->numValid;
+  if ((int)blockIdx.x * VP_ROWS >= n) return;       // the whole CTA: no thread reaches the scan's barriers
+  bool bit;
+  const unsigned int pos = vp_scan(masks, blockCounts, n, &bit, nullptr);
+  if (bit && pos < (unsigned int)maxInliers) inliers[pos] = pairs[orig[blockIdx.x * VP_ROWS + threadIdx.x]];
+}
+
+// ---- host side ------------------------------------------------------------------------------------------------------
+struct VerifyLayout {
+  size_t masks, counts, xy, un, orig, models, slotCounts, state, bytes;
+};
+
+static VerifyLayout verify_layout(int numPairs, int numLoops)
+{
+  VerifyLayout L;
+  size_t o = 0;
+  auto take = [&](size_t b) { const size_t at = o; o += (b + 255) & ~(size_t)255; return at; };
+  const size_t P = numPairs > 0 ? (size_t)numPairs : 1, S = 3 * (size_t)numLoops;
+  L.masks = take(((P + 31) / 32) * sizeof(unsigned int));
+  L.counts = take(((P + VP_ROWS - 1) / VP_ROWS) * sizeof(unsigned int));
+  L.xy = take(P * sizeof(float4));
+  L.un = take(P * sizeof(float4));
+  L.orig = take(P * sizeof(int));
+  L.models = take(S * 9 * sizeof(double));
+  L.slotCounts = take(S * sizeof(unsigned int));
+  L.state = take(sizeof(VerifyState));
+  L.bytes = o;
+  return L;
+}
+
+size_t verify_scratch_bytes(int numPairs, int numLoops) { return verify_layout(numPairs, numLoops).bytes; }
+size_t verify_result_bytes() { return sizeof(VerifyState); }
+
+// CUDASIFT_MATCH_TIMING=1: CUDA events between the kernels, printed to stderr
+static cudaEvent_t *vp_timing_events()
+{
+  static int timing = -1;
+  static cudaEvent_t tev[9];
+  if (timing < 0) {
+    const char *e = getenv("CUDASIFT_MATCH_TIMING");
+    timing = (e && atoi(e)) ? 1 : 0;
+    if (timing) for (int i = 0; i < 9; i++) cudaEventCreate(&tev[i]);
+  }
+  return timing ? tev : nullptr;
+}
+
+static void vp_timing_print(cudaEvent_t *tev, int numPairs, int numLoops, int model)
+{
+  static const char *names[8] = {"flags", "compact", "norm", "hyp", "score", "argmax", "refit", "write"};
+  cudaEventSynchronize(tev[8]);
+  fprintf(stderr, "verify timing model=%d pairs=%d loops=%d", model, numPairs, numLoops);
+  for (int i = 0; i < 8; i++) {
+    float t = 0; cudaEventElapsedTime(&t, tev[i], tev[i + 1]);
+    fprintf(stderr, " %s=%.4f", names[i], t);
+  }
+  fprintf(stderr, "\n");
+}
+
+// Steps 1-4 (and, with full, 5-8) on the stream; then the state is copied to h_state (pinned, verify_result_bytes()).
+// inliers may be null when maxInliers == 0.  full == false stops after scoring (the models and counts stay in scratch).
+int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *pairs, int numPairs, int model,
+                  int numLoops, float thresh, unsigned long long seed, int *inliers, int maxInliers, void *scratch,
+                  void *h_state, bool full, cudaStream_t st)
+{
+  const VerifyLayout L = verify_layout(numPairs, numLoops);
+  char *b = static_cast<char *>(scratch);
+  unsigned int *masks = reinterpret_cast<unsigned int *>(b + L.masks), *counts = reinterpret_cast<unsigned int *>(b + L.counts);
+  float4 *xy = reinterpret_cast<float4 *>(b + L.xy), *un = reinterpret_cast<float4 *>(b + L.un);
+  int *orig = reinterpret_cast<int *>(b + L.orig);
+  double *models = reinterpret_cast<double *>(b + L.models);
+  unsigned int *slotCounts = reinterpret_cast<unsigned int *>(b + L.slotCounts);
+  VerifyState *vs = reinterpret_cast<VerifyState *>(b + L.state);
+  const int2 *p2 = reinterpret_cast<const int2 *>(pairs);
+  const int blocks = idivup(numPairs, VP_ROWS), slots = 3 * numLoops;
+  cudaEvent_t *tev = full ? vp_timing_events() : nullptr;
+  if (tev) cudaEventRecord(tev[0], st);
+  vp_flags_kernel<<<blocks, VP_ROWS, 0, st>>>(s1, n1, s2, n2, p2, numPairs, masks, counts);
+  if (tev) cudaEventRecord(tev[1], st);
+  vp_compact_kernel<<<blocks, VP_ROWS, 0, st>>>(s1, s2, p2, numPairs, masks, counts, xy, orig, vs);
+  if (tev) cudaEventRecord(tev[2], st);
+  vp_norm_kernel<<<1, 1024, 0, st>>>(xy, un, thresh, vs);
+  if (tev) cudaEventRecord(tev[3], st);
+  vp_hyp_kernel<<<idivup(numLoops, VP_HYP_T), VP_HYP_T, 0, st>>>(xy, numLoops, model, seed, models, slotCounts, vs);
+  if (tev) cudaEventRecord(tev[4], st);
+  const int scoreThreads = model == CS_GEOM_HOMOGRAPHY ? numLoops : slots;
+  vp_score_kernel<<<dim3(idivup(scoreThreads, VP_SC_T), idivup(numPairs, VP_CHUNK)), VP_SC_T, 0, st>>>(un, models, slots,
+                                                                                                      model, slotCounts, vs);
+  count_launch(5);
+  if (full) {
+    if (tev) cudaEventRecord(tev[5], st);
+    vp_argmax_kernel<<<idivup(slots, 256), 256, 0, st>>>(models, slotCounts, slots, vs);
+    if (tev) cudaEventRecord(tev[6], st);
+    vp_refit_kernel<<<1, VP_REFIT_T, 0, st>>>(xy, un, models, model, masks, counts, vs);
+    if (tev) cudaEventRecord(tev[7], st);
+    vp_write_kernel<<<blocks, VP_ROWS, 0, st>>>(p2, orig, masks, counts, reinterpret_cast<int2 *>(inliers), maxInliers, vs);
+    if (tev) cudaEventRecord(tev[8], st);
+    count_launch(3);
+  }
+  CS_CUDA(cudaGetLastError());
+  CS_CUDA(cudaMemcpyAsync(h_state, vs, sizeof(VerifyState), cudaMemcpyDeviceToHost, st));
+  if (tev) vp_timing_print(tev, numPairs, numLoops, model);
+  return 0;
+}
+
+// After launch_verify and a synchronize: the count, the model and the statistics from the copied state.
+int verify_result(const void *h_state, int numPairs, double model_out[9], long long stats[8])
+{
+  const VerifyState *v = static_cast<const VerifyState *>(h_state);
+  for (int k = 0; k < 9; k++) model_out[k] = v->model[k];
+  for (int k = 0; k < 8; k++) stats[k] = v->stats[k];
+  stats[1] = (long long)numPairs - v->numValid;
+  return v->total;
+}
+
+// After launch_verify(full = false) and a synchronize: every slot's model in pixel coordinates (NaN-filled when empty),
+// every slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s}.  Returns the number of valid pairs.
+int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
+                          double *h_models, int *h_counts, double h_norm[5], cudaStream_t st)
+{
+  const VerifyLayout L = verify_layout(numPairs, numLoops);
+  const char *b = static_cast<const char *>(scratch);
+  const size_t S = 3 * (size_t)numLoops;
+  CS_CUDA(cudaMemcpyAsync(h_models, b + L.models, S * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CS_CUDA(cudaMemcpyAsync(h_counts, b + L.slotCounts, S * sizeof(int), cudaMemcpyDeviceToHost, st));
+  CS_CUDA(cudaStreamSynchronize(st));
+  const VerifyState *v = static_cast<const VerifyState *>(h_state);
+  h_norm[0] = v->c1x; h_norm[1] = v->c1y; h_norm[2] = v->c2x; h_norm[3] = v->c2y; h_norm[4] = v->s;
+  for (size_t k = 0; k < S; k++) {
+    double *m = h_models + 9 * k;
+    if (std::isnan(m[0])) { for (int j = 0; j < 9; j++) m[j] = NAN; continue; }
+    double out[9];
+    vp_denormalise(m, model, v->c1x, v->c1y, v->c2x, v->c2y, v->s, out);
+    for (int j = 0; j < 9; j++) m[j] = out[j];
+  }
+  return v->numValid;
+}
+
+}  // namespace cs

@@ -129,6 +129,52 @@ int cs_match_ratio(const void *d_s1, int n1, const void *d_s2, int n2, float max
 int cs_match_ratio_host(const void *h_s1, int n1, const void *h_s2, int n2, float maxRatio, float maxDistance,
                         int crossCheck, int *h_pairs, int maxPairs, int mode, double *ms);
 
+/* Geometric verification of a correspondence list (RANSAC on the device), for any int pair list {i, j} such as
+ * cs_match_mutual and cs_match_ratio write.  Pair k, {i, j} = d_pairs[2k..2k+1], is (s1[i].xpos, s1[i].ypos) <->
+ * (s2[j].xpos, s2[j].ypos).  A pair is invalid when i is outside [0, n1), j outside [0, n2) or one of its four coordinates
+ * is not finite; invalid pairs are never sampled and never inliers.  The records are only read.
+ * - model: CS_GEOM_HOMOGRAPHY (4-point minimal solver) or CS_GEOM_FUNDAMENTAL (7-point, up to 3 models per sample).
+ * - Sampling (counter-based, reproducible on a CPU): draw d of sample s is
+ *     x = splitmix64(seed + 0x9E3779B97F4A7C15 * ((s << 8) | d)),   idx = ((x >> 32) * numValid) >> 32   (uint64)
+ *   where idx indexes the valid pairs in input order and splitmix64(z) is the output of one splitmix64 step from state z:
+ *     z += 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9; z = (z ^ (z >> 27)) * 0x94D049BB133111EB;
+ *     return z ^ (z >> 31).
+ *   A draw that repeats an earlier index of the same sample is skipped (the next draw is d + 1); a sample that has not
+ *   found its 4 / 7 distinct indices after 64 draws is degenerate.
+ * - Residuals in pixels; a pair is an inlier when its residual is strictly below thresh:
+ *     homography: the transfer error |x2 - pi(H x1)|;
+ *     fundamental: the Sampson error, (x2^T F x1)^2 / ((F x1)_0^2 + (F x1)_1^2 + (F^T x2)_0^2 + (F^T x2)_1^2) < thresh^2.
+ *   Scoring runs in FP32 on coordinates normalised with per-image centroids and one common scale, against the threshold
+ *   scaled by the same factor, so these pixel definitions hold up to FP32 rounding.
+ * - The model with the most inliers wins (ties: the lowest slot sample*3 + root, roots in ascending order of the pencil
+ *   parameter a of det(a F1 + (1 - a) F2) = 0).  It is refitted once on its inliers (8-point for F, needs 8; DLT for H)
+ *   and the refit is kept unless it has fewer inliers.  A degenerate sample: fewer than k distinct draws, three of the
+ *   four points collinear in either image (H), or a pivot below 1e-9 in the elimination on normalised coordinates.
+ * - model_out: row-major 3x3, pixel coordinates; H scaled to H[2][2] = 1, F to unit Frobenius norm with its
+ *   largest-magnitude entry positive.  d_inliers: the inlier pairs {i, j} of that model in input order (int pairs,
+ *   device, 8-byte aligned); only the first maxInliers are written.
+ * Returns the total inlier count, or CS_E_*.  Fewer than 4 (H) / 7 (F) valid pairs, or no non-degenerate sample: 0 and
+ * a zero model.  numPairs == 0 returns 0 and a zero model before any CUDA call (cs_verify_stats keeps the previous
+ * call).  CS_E_ARG, before any CUDA call, for n < 0, a NULL set with n > 0, numPairs < 0, NULL pairs with
+ * numPairs > 0, model not in {1, 2}, numLoops outside [1, 65536], thresh not finite or <= 0, NULL model_out,
+ * maxInliers < 0, NULL inliers with maxInliers > 0, and pair or inlier buffers that are not 8-byte aligned or that
+ * overlap each other or a record range.  *ms (may be NULL) gets the event time of the call.
+ * One call issues 8 kernel launches and synchronises with the host once, at the end; its scratch lives in the
+ * per-device context. */
+#define CS_GEOM_HOMOGRAPHY  1
+#define CS_GEOM_FUNDAMENTAL 2
+int cs_verify_pairs(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs,
+                    int model, int numLoops, float thresh, unsigned long long seed,
+                    double model_out[9], int *d_inliers, int maxInliers, double *ms);
+/* Same with host record arrays, a host pair list and a host inlier buffer. */
+int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs,
+                         int model, int numLoops, float thresh, unsigned long long seed,
+                         double model_out[9], int *h_inliers, int maxInliers, double *ms);
+/* The last cs_verify_pairs* call on this thread's device: out[0] = valid pairs, [1] = invalid pairs, [2] =
+ * non-degenerate samples, [3] = models scored, [4] = the winning slot (sample*3 + root, -1 if none), [5] = its inlier
+ * count, [6] = 1 if the refit was kept, [7] = the final inlier count. */
+int cs_verify_stats(long long out[8]);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
@@ -154,6 +200,13 @@ int cs_dog_planes(const float *d_base, float *d_dog, int width, int height, int 
  * cudaSiftH.cu:186-205): out[i] = tex2D(img, xs[i], ys[i]); all pointers device. */
 int cs_tex_probe(const float *d_img, int width, int height, int pitch,
                  const float *d_xs, const float *d_ys, int n, float *d_out);
+/* Steps 1-4 of cs_verify_pairs (validation, normalisation, minimal solvers, scoring) with the same arguments and checks:
+ * h_models[3*numLoops][9] receives every slot's model in pixel coordinates with the output scaling of cs_verify_pairs
+ * (NaN-filled when the slot is empty), h_counts[3*numLoops] every slot's inlier count and h_norm the normalisation
+ * {c1x, c1y, c2x, c2y, s} (u = s * (x - c)).  Returns the number of valid pairs. */
+int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs, int model,
+                     int numLoops, float thresh, unsigned long long seed, double *h_models, int *h_counts,
+                     double h_norm[5]);
 
 /* ---- pipelined extractor (extension; the reference API is strictly synchronous) ----
  * One extractor = one CUDA stream + arena + SiftPoint array + pinned staging.  Several
