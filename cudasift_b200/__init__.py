@@ -82,6 +82,7 @@ def lib():
         "cs_laplace_taps": (ip, [ip, fp, vp]),
         "cs_dog_planes": (ip, [vp, vp, ip, ip, ip, ip, ip]),
         "cs_tex_probe": (ip, [vp, ip, ip, ip, vp, vp, ip, vp]),
+        "cs_describe_points": (ip, [vp, ip, ip, ip, vp, ip, ip, fp]),
         "cs_extractor_create": (vp, [ip, ip, ip, ip, ip]),
         "cs_extractor_destroy": (ip, [vp]),
         "cs_extractor_submit_device": (ip, [vp, vp, ip, c.c_double, fp, fp]),

@@ -12,6 +12,7 @@
 #include "pipeline2.h"
 
 #include <cmath>
+#include <cstddef>
 #include <cstdarg>
 #include <cstring>
 #include <chrono>
@@ -1305,6 +1306,55 @@ int cs_tex_probe(const float *d_img, int w, int h, int pitch, const float *d_xs,
   cudaStreamSynchronize(c->stream);
   cudaDestroyTextureObject(tex);
   return r;
+}
+
+int cs_describe_points(const float *d_img, int w, int h, int pitch, void *d_pts, int n, int maxPts,
+                       float finestSubsampling)
+{
+  if (!d_img || !d_pts || w < 1 || h < 1 || pitch < w || maxPts < 1 || n < 0 || n > maxPts) {
+    set_error("cs_describe_points: invalid argument (CS_E_ARG)");
+    return CS_E_ARG;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if (n == 0) return 0;
+  // describe_kernel picks the texture by log2(subsampling): refuse records it cannot index
+  std::vector<float> sub(n);
+  CS_CUDA(cudaMemcpy2D(sub.data(), sizeof(float), (const char *)d_pts + offsetof(SiftPoint, subsampling),
+                       sizeof(SiftPoint), sizeof(float), n, cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n; i++) {
+    int e = 0;
+    if (!(std::frexp(sub[i], &e) == 0.5f && e >= 1 && e <= CS_MAX_LEVELS)) {
+      set_error("cs_describe_points: record %d has subsampling %g, not 2^k with 0 <= k < %d", i, sub[i], CS_MAX_LEVELS);
+      return CS_E_ARG;
+    }
+  }
+  DescribeParams ds;
+  memset(&ds, 0, sizeof(ds));
+  cudaTextureObject_t tex = 0;
+  int r = make_texture(&tex, d_img, w, h, pitch);
+  if (r < 0) return r;
+  for (int i = 0; i < CS_MAX_LEVELS; i++) ds.tex[i] = tex;
+  unsigned int *d_cnt = nullptr;
+  const unsigned int cnt0[4] = {(unsigned)n, 0u, 0u, 0u};
+  cudaError_t e = cudaMalloc((void **)&d_cnt, sizeof(cnt0));
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_cnt, cnt0, sizeof(cnt0), cudaMemcpyHostToDevice, c->stream);
+  if (e == cudaSuccess) {
+    ds.numLevels = CS_MAX_LEVELS; ds.pts = (SiftPoint *)d_pts; ds.counters = d_cnt; ds.maxPts = maxPts;
+    ds.finestSubsampling = finestSubsampling;
+    int sms = 132, dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    r = launch_describe(ds, sms * 8, c->stream);
+    if (r == 0) e = cudaMemcpyAsync(c->h_counters, d_cnt, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream);
+    if (r == 0 && e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+  }
+  if (d_cnt) cudaFree(d_cnt);
+  cudaDestroyTextureObject(tex);
+  if (r < 0) return r;
+  CS_CUDA(e);
+  return count_from_counters(c->h_counters, maxPts);
 }
 
 // ---- pipelined extractor ----

@@ -200,6 +200,13 @@ int cs_dog_planes(const float *d_base, float *d_dog, int width, int height, int 
  * cudaSiftH.cu:186-205): out[i] = tex2D(img, xs[i], ys[i]); all pointers device. */
 int cs_tex_probe(const float *d_img, int width, int height, int pitch,
                  const float *d_xs, const float *d_ys, int n, float *d_out);
+/* The describe stage alone (orientations, secondaries, descriptors) on one level image: d_pts[0..n) are records as
+ * the detector leaves them (xpos, ypos, scale in level coordinates, subsampling = 2^k with 0 <= k < 8, capacity
+ * maxPts records), described in place by the extractor's kernel; secondaries go to slots n.. while they fit, and none
+ * for records with subsampling == finestSubsampling (reference quirk Q1).  Returns the record count by the
+ * extractor's rule, max(min(primaries, maxPts), min(slots claimed, maxPts)). */
+int cs_describe_points(const float *d_img, int width, int height, int pitch, void *d_pts, int n, int maxPts,
+                       float finestSubsampling);
 /* Steps 1-4 of cs_verify_pairs (validation, normalisation, minimal solvers, scoring) with the same arguments and checks:
  * h_models[3*numLoops][9] receives every slot's model in pixel coordinates with the output scaling of cs_verify_pairs
  * (NaN-filled when the slot is empty), h_counts[3*numLoops] every slot's inlier count and h_norm the normalisation

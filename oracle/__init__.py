@@ -54,6 +54,7 @@ def lib():
         L.oracle_tex2d.restype = fp
         L.oracle_orientations.argtypes = [vp, ip, ip, ip, vp, ip, ip, vp, ip]
         L.oracle_descriptors.argtypes = [vp, ip, ip, ip, vp, ip, ip, fp]
+        L.oracle_last_q22.restype = ip
         L.oracle_extract.argtypes = [vp, ip, ip, ip, ip, fp, fp, fp, ip, vp, ip, vp]
         L.oracle_extract.restype = ip
         L.oracle_match.argtypes = [vp, ip, vp, ip]
@@ -112,6 +113,28 @@ def tex2d(img, xs, ys):
     h, w = img.shape
     L = lib()
     return np.array([L.oracle_tex2d(_p(img), w, h, w, float(x), float(y)) for x, y in zip(xs, ys)], np.float32)
+
+
+def orientations(level, pts):
+    """oracle_orientations on one pyramid level: pts (records in level coordinates) with their orientations set and
+    the secondaries appended, as the reference's ComputeOrientations leaves them."""
+    level = np.ascontiguousarray(level, np.float32)
+    h, w = level.shape
+    out = np.zeros(2 * len(pts), SIFT_DTYPE)
+    out[:len(pts)] = pts
+    count = ctypes.c_int(len(pts))
+    lib().oracle_orientations(_p(level), w, h, w, _p(out), 0, len(pts), ctypes.byref(count), len(out))
+    return out[:count.value].copy()
+
+
+def descriptors(level, pts, subsampling=1.0):
+    """oracle_descriptors on one pyramid level: (records with descriptors, positions scaled by subsampling; the
+    number of angi == 8 votes, quirk Q22)."""
+    level = np.ascontiguousarray(level, np.float32)
+    h, w = level.shape
+    out = np.ascontiguousarray(pts, SIFT_DTYPE).copy()
+    lib().oracle_descriptors(_p(level), w, h, w, _p(out), 0, len(out), subsampling)
+    return out, int(lib().oracle_last_q22())
 
 
 def set_cap32(on):

@@ -412,6 +412,9 @@ static float fast_atan2(float y, float x)
   return r;
 }
 
+static int g_q22 = 0;
+int oracle_last_q22(void) { return g_q22; }   /* angi == 8 votes (quirk Q22) of the last oracle_descriptors call */
+
 static float warp_tree_sum(float *v)
 { /* the ShiftDown reduction of cudaSiftD.cu:392-393: lane 0 of a 32-lane butterfly */
   for (int d = 16; d > 0; d /= 2)
@@ -423,6 +426,7 @@ void oracle_descriptors(const float *img, int w, int h, int pitch, OracleSiftPoi
                         int first, int last, float subsampling)
 { /* cudaSiftD.cu:308-417 */
   float gauss[16];
+  g_q22 = 0;
   for (int t = 0; t < 16; t++) {
     float d = t - 7.5f;
     gauss[t] = exp2f(((d * d) * 0.0078125f) * -1.44269502f);   /* __expf(-(t-7.5)^2/128) */
@@ -457,6 +461,7 @@ void oracle_descriptors(const float *img, int w, int h, int pitch, OracleSiftPoi
         int hist = 8 * (4 * veri + hori);
         int p1 = angi + hist, p2 = angp + hist;
 #define VOTE(i, v) do { int ii = (i); if (ii >= 0 && ii < 128 + 48) buffer[ii] += (v); } while (0)
+        if (angi == 8) g_q22 += (tx >= 2) * ((y >= 2) + (y <= 13)) + (tx <= 13) * ((y >= 2) + (y <= 13));
         if (tx >= 2) {
           float grad1 = ihorf * grad;
           if (y >= 2) { float g2 = iverf * grad1; VOTE(p1, iangf * g2); VOTE(p2, angf * g2); }

@@ -69,6 +69,8 @@ void oracle_orientations(const float *img, int w, int h, int pitch, OracleSiftPo
 /* cudaSiftD.cu:308-417 (ExtractSiftDescriptorsCONSTNew) over pts[first..last). */
 void oracle_descriptors(const float *img, int w, int h, int pitch, OracleSiftPoint *pts,
                         int first, int last, float subsampling);
+/* Votes with angi == 8 (quirk Q22: into angle bin 0 of the next cell) in the last oracle_descriptors call. */
+int oracle_last_q22(void);
 
 /* cudaSiftH.cu:72-144 (ExtractSift, scaleUp optional).  img is w*h floats with row
  * stride `pitch`.  Returns numPts as the reference reports it (quirk Q1: the finest
