@@ -268,89 +268,52 @@ static inline int count_from_counters(const unsigned int *c, int maxPts)
 }
 
 // ------------------------------------------------------------------------------ device ctx
-struct PipeKey {
-  int w, h, oct, up; float *arena;
-  bool operator<(const PipeKey &o) const
-  {
-    if (w != o.w) return w < o.w;
-    if (h != o.h) return h < o.h;
-    if (oct != o.oct) return oct < o.oct;
-    if (up != o.up) return up < o.up;
-    return arena < o.arena;
+int DeviceCtx::ensure(int d)
+{
+  if (dev == d && stream) return 0;
+  dev = d;
+  CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d));
+  CS_CUDA(cudaStreamCreate(&stream));
+  CS_CUDA(cudaMallocHost((void **)&h_counters, 4 * sizeof(unsigned int)));
+  return 0;
+}
+Pipeline *DeviceCtx::get_pipe(int w, int h, int oct, bool up, float *arena, int *err)
+{
+  PipeKey k{w, h, oct, up ? 1 : 0, arena};
+  auto it = pipes.find(k);
+  if (it != pipes.end()) return it->second;
+  if (!arena && pipes.size() > 8) drop_pipes(nullptr, true);   // bound the internal-arena cache
+  Pipeline *p = new Pipeline();
+  int r = p->init(w, h, oct, up, arena);
+  if (r < 0) { p->destroy(); delete p; *err = r; return nullptr; }
+  pipes[k] = p;
+  return p;
+}
+Pipeline2 *DeviceCtx::get_pipe2(int w, int h, int oct, bool up, float *arena, int *err)
+{
+  PipeKey k{w, h, oct, up ? 1 : 0, arena};
+  auto it = pipes2.find(k);
+  if (it != pipes2.end()) return it->second;
+  if (!arena && pipes2.size() > 8) drop_pipes(nullptr, true);
+  Pipeline2 *p = new Pipeline2();
+  int r = p->init(w, h, oct, up, 1, arena);
+  if (r < 0) { p->destroy(); delete p; *err = r; return nullptr; }
+  pipes2[k] = p;
+  return p;
+}
+void DeviceCtx::drop_pipes(float *arena, bool internalOnly)
+{
+  for (auto it = pipes.begin(); it != pipes.end();) {
+    bool hit = internalOnly ? it->second->ownArena : (it->first.arena == arena);
+    if (hit) { it->second->destroy(); delete it->second; it = pipes.erase(it); }
+    else ++it;
   }
-};
-
-struct DeviceCtx {
-  int dev = -1;
-  cudaStream_t stream = nullptr;           // blocking stream: ordered after legacy default-stream work
-  std::map<PipeKey, Pipeline *> pipes;     // legacy per-image pipelines
-  std::map<PipeKey, Pipeline2 *> pipes2;   // batched pipeline, batch of one (the drop-in ExtractSift)
-  unsigned int *h_counters = nullptr;      // pinned
-  unsigned long long matchStats[4] = {0, 0, 0, 0};
-  // scratch for *_host entry points
-  // 4: cs_rank_records, 5: mutual / ratio pairs, 6: the knn lists of cs_match_ratio, 7: cs_verify_pairs
-  void *scratch[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  size_t scratchBytes[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  void *h_verify = nullptr;                // pinned: the state a verify call copies back
-  long long verifyStats[8] = {0, 0, 0, 0, -1, 0, 0, 0};
-
-  int ensure(int d)
-  {
-    if (dev == d && stream) return 0;
-    dev = d;
-    CS_CUDA(cudaStreamCreate(&stream));
-    CS_CUDA(cudaMallocHost((void **)&h_counters, 4 * sizeof(unsigned int)));
-    return 0;
+  for (auto it = pipes2.begin(); it != pipes2.end();) {
+    bool hit = internalOnly ? it->second->ownArena : (it->first.arena == arena);
+    if (hit) { it->second->destroy(); delete it->second; it = pipes2.erase(it); }
+    else ++it;
   }
-  int get_scratch(int slot, size_t bytes, void **out)
-  {
-    if (scratchBytes[slot] < bytes) {
-      if (scratch[slot]) cudaFree(scratch[slot]);
-      scratch[slot] = nullptr; scratchBytes[slot] = 0;
-      CS_CUDA(cudaMalloc(&scratch[slot], bytes));
-      scratchBytes[slot] = bytes;
-    }
-    *out = scratch[slot];
-    return 0;
-  }
-  Pipeline *get_pipe(int w, int h, int oct, bool up, float *arena, int *err)
-  {
-    PipeKey k{w, h, oct, up ? 1 : 0, arena};
-    auto it = pipes.find(k);
-    if (it != pipes.end()) return it->second;
-    if (!arena && pipes.size() > 8) drop_pipes(nullptr, true);   // bound the internal-arena cache
-    Pipeline *p = new Pipeline();
-    int r = p->init(w, h, oct, up, arena);
-    if (r < 0) { p->destroy(); delete p; *err = r; return nullptr; }
-    pipes[k] = p;
-    return p;
-  }
-  Pipeline2 *get_pipe2(int w, int h, int oct, bool up, float *arena, int *err)
-  {
-    PipeKey k{w, h, oct, up ? 1 : 0, arena};
-    auto it = pipes2.find(k);
-    if (it != pipes2.end()) return it->second;
-    if (!arena && pipes2.size() > 8) drop_pipes(nullptr, true);
-    Pipeline2 *p = new Pipeline2();
-    int r = p->init(w, h, oct, up, 1, arena);
-    if (r < 0) { p->destroy(); delete p; *err = r; return nullptr; }
-    pipes2[k] = p;
-    return p;
-  }
-  void drop_pipes(float *arena, bool internalOnly)
-  {
-    for (auto it = pipes.begin(); it != pipes.end();) {
-      bool hit = internalOnly ? it->second->ownArena : (it->first.arena == arena);
-      if (hit) { it->second->destroy(); delete it->second; it = pipes.erase(it); }
-      else ++it;
-    }
-    for (auto it = pipes2.begin(); it != pipes2.end();) {
-      bool hit = internalOnly ? it->second->ownArena : (it->first.arena == arena);
-      if (hit) { it->second->destroy(); delete it->second; it = pipes2.erase(it); }
-      else ++it;
-    }
-  }
-};
+}
 
 static std::mutex g_mutex;
 static std::map<int, DeviceCtx *> g_ctx;
@@ -410,9 +373,37 @@ static int extract_sync(const float *d_img, int w, int h, int pitch, int numOcta
   return numPts;
 }
 
+// Runs enqueue() on c's stream between two events, then synchronizes; *ms (when given) receives the time between the
+// events if all went well.  A failed synchronize is CS_E_CUDA, its message prefixed by fn.  Returns enqueue's result.
+template <class Enqueue>
+static int timed_sync(const char *fn, DeviceCtx *c, double *ms, Enqueue &&enqueue)
+{
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0); cudaEventCreate(&e1);
+  cudaEventRecord(e0, c->stream);
+  int r = enqueue();
+  if (r >= 0) {
+    cudaEventRecord(e1, c->stream);
+    cudaError_t ce = cudaStreamSynchronize(c->stream);
+    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
+  }
+  if (r >= 0 && ms) { float t = 0; cudaEventElapsedTime(&t, e0, e1); *ms = t; }
+  cudaEventDestroy(e0); cudaEventDestroy(e1);                              // on every path
+  return r;
+}
+
+// cs_match_stats after a finished match or knn call: the tensor path's counters (a two-way call: both directions
+// summed) and the path taken
+static void set_match_stats(DeviceCtx *c, bool tensor)
+{
+  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
+  if (tensor) match_tensor_stats(*c, c->matchStats);
+  c->matchStats[3] = tensor ? 2 : 1;
+}
+
 // Set 1's five match fields on the device, copied to h_s1 when given.  With mu also set 2's, as a match of set 2 against
 // set 1 writes them (copied to h_s2 when given), then the cross-checked pairs; the call then returns the number of
-// pairs.  fn prefixes the error messages.
+// pairs.  fn prefixes the error messages.  *ms covers the copies to the host.
 static int match_sync(const char *fn, SiftPoint *d_s1, int n1, SiftPoint *d_s2, int n2, const MutualArgs *mu, int mode,
                       SiftPoint *h_s1, SiftPoint *h_s2, double *ms)
 {
@@ -427,107 +418,66 @@ static int match_sync(const char *fn, SiftPoint *d_s1, int n1, SiftPoint *d_s2, 
   // both sets have 32 rows.
   bool tensor = (mode == 2) || (mode == 0 && match_tensor_supported() && n1 >= 256 && n2 >= 256);
   if (mu) tensor = tensor && match_tensor_supported() && n1 >= 32 && n2 >= 32;
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  cudaEventRecord(e0, c->stream);
-  int r;
-  if (tensor) {
-    r = match_tensor(d_s1, n1, d_s2, n2, mu, c->stream);
-  } else {
-    r = match_exact(d_s1, n1, d_s2, n2, c->stream);
-    if (mu && r >= 0) r = match_exact(d_s2, n2, d_s1, n1, c->stream);
-    if (mu && r >= 0) r = launch_mutual_pairs(d_s1, n1, d_s2, n2, *mu, c->stream);
-  }
-  const SiftPoint *dev[2] = {d_s1, d_s2};
-  SiftPoint *host[2] = {h_s1, h_s2};
-  const int cnt[2] = {n1, n2};
-  for (int k = 0; k < 2 && r >= 0; k++) {                                  // matching.cu:1195-1199
-    if (!host[k]) continue;
-    cudaError_t ce = cudaMemcpy2DAsync(&host[k][0].score, sizeof(SiftPoint), &dev[k][0].score, sizeof(SiftPoint),
-                                       5 * sizeof(float), cnt[k], cudaMemcpyDeviceToHost, c->stream);
-    if (ce != cudaSuccess) { set_error("%s: result copy failed: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
-  }
-  if (r >= 0) {
-    cudaEventRecord(e1, c->stream);
-    cudaError_t ce = cudaStreamSynchronize(c->stream);
-    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
-  }
-  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }     // no event leak on the error paths
-  float t = 0; cudaEventElapsedTime(&t, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
-  if (tensor) match_tensor_stats(c->matchStats);                           // a mutual call: both directions summed
-  c->matchStats[3] = tensor ? 2 : 1;
-  if (ms) *ms = t;
-  return mu ? mutual_pairs_total() : 0;
+  auto enqueue = [&]() -> int {
+    int r;
+    if (tensor) {
+      r = match_tensor(*c, d_s1, n1, d_s2, n2, mu);
+    } else {
+      r = match_exact(d_s1, n1, d_s2, n2, c->stream);
+      if (mu && r >= 0) r = match_exact(d_s2, n2, d_s1, n1, c->stream);
+      if (mu && r >= 0) r = launch_mutual_pairs(*c, d_s1, n1, d_s2, n2, *mu);
+    }
+    const SiftPoint *dev[2] = {d_s1, d_s2};
+    SiftPoint *host[2] = {h_s1, h_s2};
+    const int cnt[2] = {n1, n2};
+    for (int k = 0; k < 2 && r >= 0; k++) {                                // matching.cu:1195-1199
+      if (!host[k]) continue;
+      cudaError_t ce = cudaMemcpy2DAsync(&host[k][0].score, sizeof(SiftPoint), &dev[k][0].score, sizeof(SiftPoint),
+                                         5 * sizeof(float), cnt[k], cudaMemcpyDeviceToHost, c->stream);
+      if (ce != cudaSuccess) { set_error("%s: result copy failed: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
+    }
+    return r;
+  };
+  const int r = timed_sync(fn, c, ms, enqueue);
+  if (r < 0) return r;
+  set_match_stats(c, tensor);
+  return mu ? (int)*c->h_pairTotal : 0;
 }
 
-// The two host sets to the context's match scratch (the caller's stream order makes them visible to the match).
-static int upload_sets(DeviceCtx *c, const void *h_s1, int n1, const void *h_s2, int n2, void **d1, void **d2)
+// The two host sets to the context's set buffers (the caller's stream order makes them visible to the match).
+static int upload_sets(DeviceCtx *c, const void *h_s1, int n1, const void *h_s2, int n2)
 {
   int r;
-  if ((r = c->get_scratch(2, (size_t)n1 * sizeof(SiftPoint), d1)) < 0) return r;
-  if ((r = c->get_scratch(3, (size_t)n2 * sizeof(SiftPoint), d2)) < 0) return r;
-  CS_CUDA(cudaMemcpyAsync(*d1, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
-  CS_CUDA(cudaMemcpyAsync(*d2, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
+  if ((r = c->set1.grow((size_t)n1 * sizeof(SiftPoint))) < 0) return r;
+  if ((r = c->set2.grow((size_t)n2 * sizeof(SiftPoint))) < 0) return r;
+  CS_CUDA(cudaMemcpyAsync(c->set1.p, h_s1, (size_t)n1 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
+  CS_CUDA(cudaMemcpyAsync(c->set2.p, h_s2, (size_t)n2 * sizeof(SiftPoint), cudaMemcpyHostToDevice, c->stream));
   return 0;
 }
 
-// Argument checks of the mutual matcher.  They come before any CUDA call (they hold on a machine without a device).
-static int mutual_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs,
-                       int mode)
+// The shared path of the *_host entry points that return pairs: the sets uploaded, then run(d1, d2, buf) -- the device
+// variant, with the context's pair buffer of `entries` int2 as buf -- and min(total, room) pairs from buf + at copied
+// to h_out.  Returns run's total.
+template <class Run>
+static int host_pairs(DeviceCtx *c, const void *h_s1, int n1, const void *h_s2, int n2, size_t entries, size_t at,
+                      int room, int *h_out, Run &&run)
 {
-  const char *bad = nullptr;
-  if (n1 < 0 || n2 < 0) bad = "n1 and n2 must be >= 0";
-  else if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) bad = "a set with records needs a pointer";
-  else if (maxPairs < 0) bad = "maxPairs must be >= 0";
-  else if (maxPairs > 0 && !pairs) bad = "maxPairs > 0 needs a pairs buffer";
-  else if (mode < 0 || mode > 2) bad = "mode must be 0 (auto), 1 (exact) or 2 (tensor)";
-  else if (n1 > 0 && n2 > 0) {
-    const uintptr_t a = reinterpret_cast<uintptr_t>(s1), b = reinterpret_cast<uintptr_t>(s2);
-    if (a < b + (uintptr_t)n2 * sizeof(SiftPoint) && b < a + (uintptr_t)n1 * sizeof(SiftPoint))
-      bad = "the record ranges of set 1 and set 2 overlap (both are written)";
-  }
-  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
-  return 0;
+  int r;
+  if ((r = c->pairs.grow(entries * sizeof(int2))) < 0) return r;
+  if ((r = upload_sets(c, h_s1, n1, h_s2, n2)) < 0) return r;
+  int2 *buf = c->pairs.as<int2>();
+  const int total = run(c->set1.as<SiftPoint>(), c->set2.as<SiftPoint>(), buf);
+  if (total < 0) return total;
+  const int k = total < room ? total : room;
+  if (k > 0) CS_CUDA(cudaMemcpy(h_out, buf + at, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
+  return total;
 }
 
-// The two nearest neighbours of set 1's rows in set 2 (idx1 / score1, [n1][2]); with idx2 also those of set 2's rows in
-// set 1; with ra then the ratio-test pairs, cross-checked when idx2 is given, and the call returns their number.  The
-// records are only read.  Path rule: the tensor path when asked for (mode 2) or automatically for 256 x 256 and more.
-static int knn_sync(const char *fn, const SiftPoint *d_s1, int n1, const SiftPoint *d_s2, int n2, int *idx1, float *score1,
-                    int *idx2, float *score2, const RatioArgs *ra, int mode, double *ms)
+// ---- argument checks: they come before any CUDA call (they hold on a machine without a device) ----
+static int arg_error(const char *fn, const char *bad)
 {
-  int err = 0;
-  if (ms) *ms = 0.0;
-  if (n1 <= 0 || n2 <= 0) return 0;
-  DeviceCtx *c = current_ctx(&err);
-  if (!c) return err;
-  const bool tensor = match_tensor_supported() && (mode == 2 || (mode == 0 && n1 >= 256 && n2 >= 256));
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  cudaEventRecord(e0, c->stream);
-  int r;
-  if (tensor) {
-    r = match_knn_tensor(d_s1, n1, d_s2, n2, idx1, score1, idx2, score2, c->stream);
-  } else {
-    r = knn_exact(d_s1, n1, d_s2, n2, idx1, score1, c->stream);
-    if (idx2 && r >= 0) r = knn_exact(d_s2, n2, d_s1, n1, idx2, score2, c->stream);
-  }
-  if (ra && r >= 0) r = launch_ratio_pairs(idx1, score1, n1, idx2, score2, n2, *ra, c->stream);
-  if (r >= 0) {
-    cudaEventRecord(e1, c->stream);
-    cudaError_t ce = cudaStreamSynchronize(c->stream);
-    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
-  }
-  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }
-  float t = 0; cudaEventElapsedTime(&t, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  c->matchStats[0] = c->matchStats[1] = c->matchStats[2] = 0;
-  if (tensor) match_tensor_stats(c->matchStats);                           // both directions summed
-  c->matchStats[3] = tensor ? 2 : 1;
-  if (ms) *ms = t;
-  return ra ? mutual_pairs_total() : 0;
+  set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad);
+  return CS_E_ARG;
 }
 
 // [a, a + na) and [b, b + nb) share a byte
@@ -536,85 +486,131 @@ static bool ranges_overlap(const void *a, size_t na, const void *b, size_t nb)
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
   return na > 0 && nb > 0 && x < y + nb && y < x + na;
 }
+static size_t record_bytes(int n) { return n > 0 ? (size_t)n * sizeof(SiftPoint) : 0; }
 
-// Argument checks of the knn and ratio matchers, before any CUDA call.  out[k] (outBytes[k] bytes) are the output
-// buffers: 8-byte aligned, outside both record ranges and apart from each other.
-static int knn_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *const *out,
-                    const size_t *outBytes, int nout, int mode, const float *thresholds)
+// The two record sets and the path mode (0 auto, 1 exact, 2 tensor).
+static int check_sets(const char *fn, const void *s1, int n1, const void *s2, int n2, int mode)
 {
-  const char *bad = nullptr;
-  const size_t r1 = n1 > 0 ? (size_t)n1 * sizeof(SiftPoint) : 0, r2 = n2 > 0 ? (size_t)n2 * sizeof(SiftPoint) : 0;
-  if (n1 < 0 || n2 < 0) bad = "n1 and n2 must be >= 0";
-  else if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) bad = "a set with records needs a pointer";
-  else if (mode < 0 || mode > 2) bad = "mode must be 0 (auto), 1 (exact) or 2 (tensor)";
-  else if (thresholds && (std::isnan(thresholds[0]) || std::isnan(thresholds[1]))) bad = "maxRatio and maxDistance must not be NaN";
-  for (int k = 0; k < nout && !bad; k++) {
-    if (outBytes[k] == 0) continue;
-    if ((reinterpret_cast<uintptr_t>(out[k]) & 7) != 0) bad = "output buffers must be 8-byte aligned";
-    else if (ranges_overlap(out[k], outBytes[k], s1, r1) || ranges_overlap(out[k], outBytes[k], s2, r2))
-      bad = "an output buffer overlaps a record range";
-    for (int m = 0; m < k && !bad; m++)
-      if (ranges_overlap(out[k], outBytes[k], out[m], outBytes[m])) bad = "the output buffers overlap";
-  }
-  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
+  if (n1 < 0 || n2 < 0) return arg_error(fn, "n1 and n2 must be >= 0");
+  if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) return arg_error(fn, "a set with records needs a pointer");
+  if (mode < 0 || mode > 2) return arg_error(fn, "mode must be 0 (auto), 1 (exact) or 2 (tensor)");
   return 0;
+}
+
+// The other buffers of a call (buf[k], bytes[k] bytes, called name[k]): every non-empty one 8-byte aligned, outside
+// both record ranges and apart from the others.
+static int check_buffers(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *const *buf,
+                         const size_t *bytes, const char *const *name, int n)
+{
+  char bad[64] = "";
+  for (int k = 0; k < n && !bad[0]; k++) {
+    const void *b = buf[k];
+    const size_t nb = bytes[k];
+    if (nb == 0) continue;
+    if ((reinterpret_cast<uintptr_t>(b) & 7) != 0) snprintf(bad, sizeof(bad), "%s must be 8-byte aligned", name[k]);
+    else if (ranges_overlap(b, nb, s1, record_bytes(n1)) || ranges_overlap(b, nb, s2, record_bytes(n2)))
+      snprintf(bad, sizeof(bad), "%s overlaps a record range", name[k]);
+    for (int m = 0; m < k && !bad[0]; m++)
+      if (ranges_overlap(b, nb, buf[m], bytes[m])) snprintf(bad, sizeof(bad), "%s and %s overlap", name[m], name[k]);
+  }
+  return bad[0] ? arg_error(fn, bad) : 0;
+}
+
+// The pairs buffer of the mutual and ratio matchers: maxPairs int2.
+static int check_pairs(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs)
+{
+  if (maxPairs < 0) return arg_error(fn, "maxPairs must be >= 0");
+  if (maxPairs > 0 && !pairs) return arg_error(fn, "maxPairs > 0 needs a pairs buffer");
+  const size_t bytes = (size_t)maxPairs * sizeof(int2);
+  const char *name = "pairs";
+  return check_buffers(fn, s1, n1, s2, n2, &pairs, &bytes, &name, 1);
+}
+
+// The mutual matcher writes both record sets, so they must not overlap.
+static int mutual_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs,
+                       int mode)
+{
+  int r;
+  if ((r = check_sets(fn, s1, n1, s2, n2, mode)) < 0) return r;
+  if (ranges_overlap(s1, record_bytes(n1), s2, record_bytes(n2)))
+    return arg_error(fn, "the record ranges of set 1 and set 2 overlap (both are written)");
+  return check_pairs(fn, s1, n1, s2, n2, pairs, maxPairs);
 }
 
 static int ratio_args(const char *fn, const void *s1, int n1, const void *s2, int n2, float maxRatio, float maxDistance,
                       const void *pairs, int maxPairs, int mode)
 {
-  const char *bad = nullptr;
-  if (maxPairs < 0) bad = "maxPairs must be >= 0";
-  else if (maxPairs > 0 && !pairs) bad = "maxPairs > 0 needs a pairs buffer";
-  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
-  const void *out[1] = {pairs};
-  const size_t bytes[1] = {(size_t)maxPairs * 2 * sizeof(int)};
-  const float th[2] = {maxRatio, maxDistance};
-  return knn_args(fn, s1, n1, s2, n2, out, bytes, 1, mode, th);
+  int r;
+  if ((r = check_sets(fn, s1, n1, s2, n2, mode)) < 0) return r;
+  if (std::isnan(maxRatio) || std::isnan(maxDistance)) return arg_error(fn, "maxRatio and maxDistance must not be NaN");
+  return check_pairs(fn, s1, n1, s2, n2, pairs, maxPairs);
 }
 
-// cs_match_ratio on device sets: the knn lists of both directions in the context's scratch.
-static int ratio_device(const char *fn, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, DeviceCtx *c,
-                        const RatioArgs &ra, bool crossCheck, int mode, double *ms)
+// The records are only read (they may overlap each other); the pair and inlier buffers are checked as outputs.
+static int verify_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                       int model, int numLoops, float thresh, const double *model_out, const void *inliers,
+                       int maxInliers)
+{
+  int r;
+  if ((r = check_sets(fn, s1, n1, s2, n2, 0)) < 0) return r;              // mode 0: the verifier has one path
+  if (numPairs < 0) return arg_error(fn, "numPairs must be >= 0");
+  if (numPairs > 0 && !pairs) return arg_error(fn, "numPairs > 0 needs a pairs buffer");
+  if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL)
+    return arg_error(fn, "model must be 1 (homography) or 2 (fundamental)");
+  if (numLoops < 1 || numLoops > 65536) return arg_error(fn, "numLoops must be in [1, 65536]");
+  if (!std::isfinite(thresh) || thresh <= 0.0f) return arg_error(fn, "thresh must be finite and > 0");
+  if (!model_out) return arg_error(fn, "model_out must not be NULL");
+  if (maxInliers < 0) return arg_error(fn, "maxInliers must be >= 0");
+  if (maxInliers > 0 && !inliers) return arg_error(fn, "maxInliers > 0 needs an inliers buffer");
+  const void *buf[2] = {pairs, inliers};
+  const size_t bytes[2] = {(size_t)numPairs * sizeof(int2), (size_t)maxInliers * sizeof(int2)};
+  const char *const name[2] = {"pairs", "inliers"};
+  return check_buffers(fn, s1, n1, s2, n2, buf, bytes, name, 2);
+}
+
+// The two nearest neighbours of set 1's rows in set 2 (idx1 / score1, [n1][2]); with idx2 also those of set 2's rows in
+// set 1; with ra then the ratio-test pairs, cross-checked when idx2 is given, and the call returns their number.  The
+// records are only read; both sets are non-empty.  Path rule: the tensor path when asked for (mode 2) or automatically
+// for 256 x 256 and more.
+static int knn_sync(const char *fn, DeviceCtx *c, const SiftPoint *d_s1, int n1, const SiftPoint *d_s2, int n2,
+                    int *idx1, float *score1, int *idx2, float *score2, const RatioArgs *ra, int mode, double *ms)
+{
+  const bool tensor = match_tensor_supported() && (mode == 2 || (mode == 0 && n1 >= 256 && n2 >= 256));
+  auto enqueue = [&]() -> int {
+    int r;
+    if (tensor) {
+      r = match_knn_tensor(*c, d_s1, n1, d_s2, n2, idx1, score1, idx2, score2);
+    } else {
+      r = knn_exact(*c, d_s1, n1, d_s2, n2, idx1, score1);
+      if (idx2 && r >= 0) r = knn_exact(*c, d_s2, n2, d_s1, n1, idx2, score2);
+    }
+    if (ra && r >= 0) r = launch_ratio_pairs(*c, idx1, score1, n1, idx2, score2, n2, *ra);
+    return r;
+  };
+  const int r = timed_sync(fn, c, ms, enqueue);
+  if (r < 0) return r;
+  set_match_stats(c, tensor);
+  return ra ? (int)*c->h_pairTotal : 0;
+}
+
+// cs_match_ratio on device sets: the knn lists of both directions in the context's knnLists.
+static int ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
+                      const RatioArgs &ra, bool crossCheck, int mode, double *ms)
 {
   const size_t a = ialignup(2 * n1, 64), b = crossCheck ? ialignup(2 * n2, 64) : 0;
-  void *w = nullptr;
   int r;
-  if ((r = c->get_scratch(6, (2 * a + 2 * b) * sizeof(int), &w)) < 0) return r;
-  int *idx1 = static_cast<int *>(w), *idx2 = crossCheck ? idx1 + 2 * a : nullptr;
+  if ((r = c->knnLists.grow((2 * a + 2 * b) * sizeof(int))) < 0) return r;
+  int *idx1 = c->knnLists.as<int>(), *idx2 = crossCheck ? idx1 + 2 * a : nullptr;
   float *sc1 = reinterpret_cast<float *>(idx1 + a), *sc2 = crossCheck ? reinterpret_cast<float *>(idx2 + b) : nullptr;
-  return knn_sync(fn, d1, n1, d2, n2, idx1, sc1, idx2, sc2, &ra, mode, ms);
+  return knn_sync(fn, c, d1, n1, d2, n2, idx1, sc1, idx2, sc2, &ra, mode, ms);
 }
 
-// Argument checks of the verifier, before any CUDA call.  The records are only read (they may overlap each other); the
-// pair and inlier buffers are 8-byte aligned, apart from each other and from both record ranges.
-static int verify_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
-                       int model, int numLoops, float thresh, const double *model_out, const void *inliers, int maxInliers)
+// The verifier's scratch and the pinned copy of its state.
+static int verify_buffers(DeviceCtx *c, int numPairs, int numLoops)
 {
-  const char *bad = nullptr;
-  if (n1 < 0 || n2 < 0) bad = "n1 and n2 must be >= 0";
-  else if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) bad = "a set with records needs a pointer";
-  else if (numPairs < 0) bad = "numPairs must be >= 0";
-  else if (numPairs > 0 && !pairs) bad = "numPairs > 0 needs a pairs buffer";
-  else if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL) bad = "model must be 1 (homography) or 2 (fundamental)";
-  else if (numLoops < 1 || numLoops > 65536) bad = "numLoops must be in [1, 65536]";
-  else if (!std::isfinite(thresh) || thresh <= 0.0f) bad = "thresh must be finite and > 0";
-  else if (!model_out) bad = "model_out must not be NULL";
-  else if (maxInliers < 0) bad = "maxInliers must be >= 0";
-  else if (maxInliers > 0 && !inliers) bad = "maxInliers > 0 needs an inliers buffer";
-  if (!bad) {
-    const size_t r1 = n1 > 0 ? (size_t)n1 * sizeof(SiftPoint) : 0, r2 = n2 > 0 ? (size_t)n2 * sizeof(SiftPoint) : 0;
-    const void *out[2] = {pairs, inliers};
-    const size_t bytes[2] = {(size_t)numPairs * 2 * sizeof(int), (size_t)maxInliers * 2 * sizeof(int)};
-    for (int k = 0; k < 2 && !bad; k++) {
-      if (bytes[k] == 0) continue;
-      if ((reinterpret_cast<uintptr_t>(out[k]) & 7) != 0) bad = "pair and inlier buffers must be 8-byte aligned";
-      else if (ranges_overlap(out[k], bytes[k], s1, r1) || ranges_overlap(out[k], bytes[k], s2, r2))
-        bad = "a pair or inlier buffer overlaps a record range";
-    }
-    if (!bad && ranges_overlap(out[0], bytes[0], out[1], bytes[1])) bad = "the pair and inlier buffers overlap";
-  }
-  if (bad) { set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad); return CS_E_ARG; }
+  int r;
+  if ((r = c->verify.grow(verify_scratch_bytes(numPairs, numLoops))) < 0) return r;
+  if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
   return 0;
 }
 
@@ -623,24 +619,13 @@ static int verify_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1
                        const int *pairs, int numPairs, int model, int numLoops, float thresh, unsigned long long seed,
                        double model_out[9], int *inliers, int maxInliers, double *ms)
 {
-  void *w = nullptr;
   int r;
-  if ((r = c->get_scratch(7, verify_scratch_bytes(numPairs, numLoops), &w)) < 0) return r;
-  if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
-  cudaEvent_t e0, e1;
-  cudaEventCreate(&e0); cudaEventCreate(&e1);
-  cudaEventRecord(e0, c->stream);
-  r = launch_verify(d1, n1, d2, n2, pairs, numPairs, model, numLoops, thresh, seed, inliers, maxInliers, w, c->h_verify,
-                    true, c->stream);
-  if (r >= 0) {
-    cudaEventRecord(e1, c->stream);
-    cudaError_t ce = cudaStreamSynchronize(c->stream);
-    if (ce != cudaSuccess) { set_error("%s: %s", fn, cudaGetErrorString(ce)); r = CS_E_CUDA; }
-  }
-  if (r < 0) { cudaEventDestroy(e0); cudaEventDestroy(e1); return r; }
-  float t = 0; cudaEventElapsedTime(&t, e0, e1);
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
-  if (ms) *ms = t;
+  if ((r = verify_buffers(c, numPairs, numLoops)) < 0) return r;
+  auto enqueue = [&] {
+    return launch_verify(d1, n1, d2, n2, pairs, numPairs, model, numLoops, thresh, seed, inliers, maxInliers,
+                         c->verify.p, c->h_verify, true, c->stream);
+  };
+  if ((r = timed_sync(fn, c, ms, enqueue)) < 0) return r;
   return verify_result(c->h_verify, numPairs, model_out, c->verifyStats);
 }
 
@@ -1026,14 +1011,13 @@ int cs_extract_host(const float *h_img, int w, int h, int numOctaves, double ini
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   int pitch = ialignup(w, 128);
-  void *d_img = nullptr, *d_pts = nullptr;
   int r;
-  if ((r = c->get_scratch(0, (size_t)pitch * h * sizeof(float), &d_img)) < 0) return r;
-  if ((r = c->get_scratch(1, (size_t)maxPts * sizeof(SiftPoint), &d_pts)) < 0) return r;
-  CS_CUDA(cudaMemcpy2DAsync(d_img, (size_t)pitch * sizeof(float), h_img, (size_t)w * sizeof(float),
+  if ((r = c->image.grow((size_t)pitch * h * sizeof(float))) < 0) return r;
+  if ((r = c->points.grow((size_t)maxPts * sizeof(SiftPoint))) < 0) return r;
+  CS_CUDA(cudaMemcpy2DAsync(c->image.p, (size_t)pitch * sizeof(float), h_img, (size_t)w * sizeof(float),
                             (size_t)w * sizeof(float), h, cudaMemcpyHostToDevice, c->stream));
-  return extract_sync((const float *)d_img, w, h, pitch, numOctaves, initBlur, thresh, lowestScale, scaleUp != 0,
-                      nullptr, (SiftPoint *)d_pts, (SiftPoint *)h_pts, maxPts, NULL);
+  return extract_sync(c->image.as<const float>(), w, h, pitch, numOctaves, initBlur, thresh, lowestScale, scaleUp != 0,
+                      nullptr, c->points.as<SiftPoint>(), (SiftPoint *)h_pts, maxPts, NULL);
 }
 
 int cs_match(void *d_s1, int n1, void *d_s2, int n2, void *h_s1, int mode, double *ms)
@@ -1049,24 +1033,23 @@ int cs_match_host(void *h_s1, int n1, const void *h_s2, int n2, int mode, double
   if (n1 <= 0 || n2 <= 0) return 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  void *d1 = nullptr, *d2 = nullptr;
   int r;
-  if ((r = upload_sets(c, h_s1, n1, h_s2, n2, &d1, &d2)) < 0) return r;
-  return match_sync("MatchSiftData", (SiftPoint *)d1, n1, (SiftPoint *)d2, n2, nullptr, mode, (SiftPoint *)h_s1, nullptr, ms);
+  if ((r = upload_sets(c, h_s1, n1, h_s2, n2)) < 0) return r;
+  return match_sync("MatchSiftData", c->set1.as<SiftPoint>(), n1, c->set2.as<SiftPoint>(), n2, nullptr, mode,
+                    (SiftPoint *)h_s1, nullptr, ms);
 }
 
 int cs_match_mutual(void *d_s1, int n1, void *d_s2, int n2, float minScore, float maxAmbiguity, int *d_pairs, int maxPairs,
                     int mode, double *ms)
 {
+  const char *fn = "cs_match_mutual";
   if (ms) *ms = 0.0;
-  int r = mutual_args("cs_match_mutual", d_s1, n1, d_s2, n2, d_pairs, maxPairs, mode);
+  int r = mutual_args(fn, d_s1, n1, d_s2, n2, d_pairs, maxPairs, mode);
   if (r < 0) return r;
-  if ((reinterpret_cast<uintptr_t>(d_pairs) & 7) != 0) {
-    set_error("cs_match_mutual: invalid argument (CS_E_ARG): d_pairs must be 8-byte aligned");
-    return CS_E_ARG;
-  }
+  if ((reinterpret_cast<uintptr_t>(d_pairs) & 7) != 0)                 // also when maxPairs is 0
+    return arg_error(fn, "pairs must be 8-byte aligned");
   const MutualArgs mu = {minScore, maxAmbiguity, (int2 *)d_pairs, maxPairs};
-  return match_sync("cs_match_mutual", (SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, &mu, mode, nullptr, nullptr, ms);
+  return match_sync(fn, (SiftPoint *)d_s1, n1, (SiftPoint *)d_s2, n2, &mu, mode, nullptr, nullptr, ms);
 }
 
 int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore, float maxAmbiguity, int *h_pairs,
@@ -1080,32 +1063,31 @@ int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore,
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const int room = maxPairs < (n1 < n2 ? n1 : n2) ? maxPairs : (n1 < n2 ? n1 : n2);   // no more pairs can exist
-  void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
-  if ((r = c->get_scratch(5, (size_t)(room > 0 ? room : 1) * sizeof(int2), &dp)) < 0) return r;
-  if ((r = upload_sets(c, h_s1, n1, h_s2, n2, &d1, &d2)) < 0) return r;
-  const MutualArgs mu = {minScore, maxAmbiguity, (int2 *)dp, room};
-  const int total = match_sync("cs_match_mutual", (SiftPoint *)d1, n1, (SiftPoint *)d2, n2, &mu, mode, (SiftPoint *)h_s1,
-                               (SiftPoint *)h_s2, ms);
-  if (total < 0) return total;
-  const int k = total < room ? total : room;
-  if (k > 0) CS_CUDA(cudaMemcpy(h_pairs, dp, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
-  return total;
+  return host_pairs(c, h_s1, n1, h_s2, n2, room > 0 ? room : 1, 0, room, h_pairs,
+                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
+                      const MutualArgs mu = {minScore, maxAmbiguity, pairs, room};
+                      return match_sync("cs_match_mutual", d1, n1, d2, n2, &mu, mode, (SiftPoint *)h_s1,
+                                        (SiftPoint *)h_s2, ms);
+                    });
 }
 
 int cs_match_knn2(const void *d_s1, int n1, const void *d_s2, int n2, int *d_idx, float *d_score, int mode, double *ms)
 {
-  if (ms) *ms = 0.0;
   const char *fn = "cs_match_knn2";
-  if (n1 > 0 && (!d_idx || !d_score)) {
-    set_error("%s: invalid argument (CS_E_ARG): n1 > 0 needs idx and score buffers", fn);
-    return CS_E_ARG;
-  }
-  const void *out[2] = {d_idx, d_score};
-  const size_t bytes[2] = {n1 > 0 ? (size_t)n1 * 2 * sizeof(int) : 0, n1 > 0 ? (size_t)n1 * 2 * sizeof(float) : 0};
-  int r = knn_args(fn, d_s1, n1, d_s2, n2, out, bytes, 2, mode, nullptr);
+  if (ms) *ms = 0.0;
+  int r = check_sets(fn, d_s1, n1, d_s2, n2, mode);
   if (r < 0) return r;
-  return knn_sync(fn, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_idx, d_score, nullptr, nullptr, nullptr,
-                  mode, ms);
+  if (n1 > 0 && (!d_idx || !d_score)) return arg_error(fn, "n1 > 0 needs idx and score buffers");
+  const void *buf[2] = {d_idx, d_score};
+  const size_t bytes[2] = {(size_t)n1 * 2 * sizeof(int), (size_t)n1 * 2 * sizeof(float)};
+  const char *const name[2] = {"idx", "score"};
+  if ((r = check_buffers(fn, d_s1, n1, d_s2, n2, buf, bytes, name, 2)) < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  return knn_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_idx, d_score, nullptr, nullptr,
+                  nullptr, mode, ms);
 }
 
 int cs_match_ratio(const void *d_s1, int n1, const void *d_s2, int n2, float maxRatio, float maxDistance, int crossCheck,
@@ -1119,31 +1101,27 @@ int cs_match_ratio(const void *d_s1, int n1, const void *d_s2, int n2, float max
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const RatioArgs ra = {maxRatio, maxDistance, (int2 *)d_pairs, maxPairs};
-  return ratio_device("cs_match_ratio", (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, c, ra, crossCheck != 0,
-                      mode, ms);
+  return ratio_sync("cs_match_ratio", c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, ra, crossCheck != 0,
+                    mode, ms);
 }
 
 int cs_match_ratio_host(const void *h_s1, int n1, const void *h_s2, int n2, float maxRatio, float maxDistance,
                         int crossCheck, int *h_pairs, int maxPairs, int mode, double *ms)
 {
+  const char *fn = "cs_match_ratio_host";
   if (ms) *ms = 0.0;
-  int r = ratio_args("cs_match_ratio_host", h_s1, n1, h_s2, n2, maxRatio, maxDistance, h_pairs, maxPairs, mode);
+  int r = ratio_args(fn, h_s1, n1, h_s2, n2, maxRatio, maxDistance, h_pairs, maxPairs, mode);
   if (r < 0) return r;
   if (n1 == 0 || n2 == 0) return 0;
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const int room = maxPairs < n1 ? maxPairs : n1;                      // at most one pair per row of set 1
-  void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
-  if ((r = c->get_scratch(5, (size_t)(room > 0 ? room : 1) * sizeof(int2), &dp)) < 0) return r;
-  if ((r = upload_sets(c, h_s1, n1, h_s2, n2, &d1, &d2)) < 0) return r;
-  const RatioArgs ra = {maxRatio, maxDistance, (int2 *)dp, room};
-  const int total = ratio_device("cs_match_ratio_host", (const SiftPoint *)d1, n1, (const SiftPoint *)d2, n2, c, ra,
-                                 crossCheck != 0, mode, ms);
-  if (total < 0) return total;
-  const int k = total < room ? total : room;
-  if (k > 0) CS_CUDA(cudaMemcpy(h_pairs, dp, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
-  return total;
+  return host_pairs(c, h_s1, n1, h_s2, n2, room > 0 ? room : 1, 0, room, h_pairs,
+                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
+                      const RatioArgs ra = {maxRatio, maxDistance, pairs, room};
+                      return ratio_sync(fn, c, d1, n1, d2, n2, ra, crossCheck != 0, mode, ms);
+                    });
 }
 
 int cs_match_stats(unsigned long long out[4])
@@ -1186,17 +1164,15 @@ int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, con
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const int room = maxInliers < numPairs ? maxInliers : numPairs;     // no more inliers can exist
-  void *d1 = nullptr, *d2 = nullptr, *dp = nullptr;
-  if ((r = c->get_scratch(5, (size_t)(numPairs + room) * sizeof(int2), &dp)) < 0) return r;
-  if ((r = upload_sets(c, h_s1, n1 > 0 ? n1 : 0, h_s2, n2 > 0 ? n2 : 0, &d1, &d2)) < 0) return r;
-  int *pairs = static_cast<int *>(dp), *inl = pairs + 2 * (size_t)numPairs;
-  CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice, c->stream));
-  const int total = verify_sync(fn, c, (const SiftPoint *)d1, n1, (const SiftPoint *)d2, n2, pairs, numPairs, model,
-                                numLoops, thresh, seed, model_out, inl, room, ms);
-  if (total < 0) return total;
-  const int k = total < room ? total : room;
-  if (k > 0) CS_CUDA(cudaMemcpy(h_inliers, inl, (size_t)k * sizeof(int2), cudaMemcpyDeviceToHost));
-  return total;
+  // the pair buffer holds the input pairs, then room inliers
+  return host_pairs(c, h_s1, n1, h_s2, n2, (size_t)numPairs + room, numPairs, room, h_inliers,
+                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
+                      CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice,
+                                              c->stream));
+                      return verify_sync(fn, c, d1, n1, d2, n2, reinterpret_cast<int *>(pairs), numPairs, model,
+                                         numLoops, thresh, seed, model_out, reinterpret_cast<int *>(pairs + numPairs),
+                                         room, ms);
+                    });
 }
 
 int cs_verify_stats(long long out[8])
@@ -1216,21 +1192,17 @@ int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const i
   double dummy[9];
   int r = verify_args(fn, d_s1, n1, d_s2, n2, d_pairs, numPairs, model, numLoops, thresh, dummy, nullptr, 0);
   if (r < 0) return r;
-  if (!h_models || !h_counts || !h_norm) {
-    set_error("%s: invalid argument (CS_E_ARG): NULL output array", fn);
-    return CS_E_ARG;
-  }
+  if (!h_models || !h_counts || !h_norm) return arg_error(fn, "NULL output array");
   if (numPairs == 0) return 0;
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  void *w = nullptr;
-  if ((r = c->get_scratch(7, verify_scratch_bytes(numPairs, numLoops), &w)) < 0) return r;
-  if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
+  if ((r = verify_buffers(c, numPairs, numLoops)) < 0) return r;
   r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, numLoops, thresh,
-                    seed, nullptr, 0, w, c->h_verify, false, c->stream);
+                    seed, nullptr, 0, c->verify.p, c->h_verify, false, c->stream);
   if (r < 0) return r;
-  return verify_models_to_host(w, c->h_verify, numPairs, numLoops, model, h_models, h_counts, h_norm, c->stream);
+  return verify_models_to_host(c->verify.p, c->h_verify, numPairs, numLoops, model, h_models, h_counts, h_norm,
+                               c->stream);
 }
 
 // ---- stage-level entry points ----
@@ -1343,10 +1315,7 @@ int cs_describe_points(const float *d_img, int w, int h, int pitch, void *d_pts,
   if (e == cudaSuccess) {
     ds.numLevels = CS_MAX_LEVELS; ds.pts = (SiftPoint *)d_pts; ds.counters = d_cnt; ds.maxPts = maxPts;
     ds.finestSubsampling = finestSubsampling;
-    int sms = 132, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    r = launch_describe(ds, sms * 8, c->stream);
+    r = launch_describe(ds, c->sms * 8, c->stream);
     if (r == 0) e = cudaMemcpyAsync(c->h_counters, d_cnt, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream);
     if (r == 0 && e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   }
@@ -1723,11 +1692,10 @@ int cs_rank_records(const void *d_in, int n, void *d_out, int maxOut)
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  void *buf = nullptr;
   const size_t words = CS_CNT_STRIDE + rank_scratch_words(n);   // counters | scratch
-  int r = c->get_scratch(4, words * sizeof(unsigned int), &buf);
+  int r = c->rank.grow(words * sizeof(unsigned int));
   if (r < 0) return r;
-  unsigned int *cnt = (unsigned int *)buf;
+  unsigned int *cnt = c->rank.as<unsigned int>();
   const unsigned int init[CS_CNT_STRIDE] = {(unsigned)n, (unsigned)n, 0u, 0u};
   CS_CUDA(cudaMemcpyAsync(cnt, init, sizeof(init), cudaMemcpyHostToDevice, c->stream));
   RankParams rp;
@@ -1735,10 +1703,7 @@ int cs_rank_records(const void *d_in, int n, void *d_out, int maxOut)
   rp.in = (const SiftPoint *)d_in; rp.maxIn = n;
   rp.out = (SiftPoint *)d_out; rp.maxOut = maxOut;
   rp.counters = cnt; rp.scratch = cnt + CS_CNT_STRIDE;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if ((r = launch_rank(rp, 1, sms, c->stream)) < 0) return r;
+  if ((r = launch_rank(rp, 1, c->sms, c->stream)) < 0) return r;
   CS_CUDA(cudaMemcpyAsync(c->h_counters, cnt, CS_CNT_STRIDE * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
   CS_CUDA(cudaStreamSynchronize(c->stream));
   return (int)c->h_counters[2];

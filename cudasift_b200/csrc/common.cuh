@@ -5,6 +5,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
+#include <map>
 
 #include "../../include/cudaSift.h"
 #include "../../include/cudasift_b200.h"
@@ -190,8 +191,87 @@ __host__ __device__ inline size_t rank_scratch_words(int maxIn)
 }
 int launch_rank(const RankParams &p, int batch, int sms, cudaStream_t st);
 
+// ---- per-device context ---------------------------------------------------------------------------------------------
+// A device buffer that grows on demand: grow() keeps the allocation when it holds `bytes`, else replaces it (the
+// contents are not kept).
+struct GrowBuffer {
+  void *p = nullptr;
+  size_t cap = 0;
+  int grow(size_t bytes)
+  {
+    if (cap >= bytes) return 0;
+    if (p) cudaFree(p);
+    p = nullptr; cap = 0;
+    CS_CUDA(cudaMalloc(&p, bytes));
+    cap = bytes;
+    return 0;
+  }
+  template <class T> T *as() const { return static_cast<T *>(p); }
+};
+
+struct Pipeline;    // round-1 per-image extraction (api.cu)
+struct Pipeline2;   // batched extraction (pipeline2.h)
+struct PipeKey {
+  int w, h, oct, up; float *arena;
+  bool operator<(const PipeKey &o) const
+  {
+    if (w != o.w) return w < o.w;
+    if (h != o.h) return h < o.h;
+    if (oct != o.oct) return oct < o.oct;
+    if (up != o.up) return up < o.up;
+    return arena < o.arena;
+  }
+};
+
+// Everything a device keeps between calls, one per device index (api.cu: current_ctx()).  Calls use it on its stream:
+// like the reference (function-local static caches, cudaSiftH.cu:310,409) the library is single-threaded per device --
+// two host threads calling on the same device at the same time would share these buffers.
+struct DeviceCtx {
+  int dev = -1;
+  int sms = 0;                             // multiprocessor count
+  cudaStream_t stream = nullptr;           // blocking stream: ordered after legacy default-stream work
+  std::map<PipeKey, Pipeline *> pipes;     // legacy per-image pipelines
+  std::map<PipeKey, Pipeline2 *> pipes2;   // batched pipeline, batch of one (the drop-in ExtractSift)
+
+  // Device buffers grown on demand, and the entry points that use them.  A call may use several at once
+  // (cs_match_ratio: knnLists, pairScratch, the tc* tables and knnPartials), so each has its own member.
+  GrowBuffer image, points;   // cs_extract_host: the image, the records
+  // cs_match_host, cs_match_mutual_host, cs_match_ratio_host, cs_verify_pairs_host: the uploaded sets
+  GrowBuffer set1, set2;
+  // cs_match_mutual_host, cs_match_ratio_host: the pairs; cs_verify_pairs_host: the input pairs, then the inliers
+  GrowBuffer pairs;
+  GrowBuffer knnLists;        // cs_match_ratio(_host): both directions' neighbour lists
+  GrowBuffer pairScratch;     // cs_match_mutual(_host), cs_match_ratio(_host): ballot words, CTA counts, the total
+  GrowBuffer knnPartials;     // cs_match_knn2, cs_match_ratio(_host): the slices of the exact scan
+  GrowBuffer verify;          // cs_verify_pairs(_host), cs_verify_models
+  GrowBuffer rank;            // cs_rank_records: counters, scratch
+  // the tensor path (match_tc.cu) of cs_match(_host), cs_match_mutual(_host), cs_match_knn2, cs_match_ratio(_host):
+  // operand tiles, B-role copies, row norms, top-3 tables, fallback rows, and 2 x 16 words of flags used alternately
+  GrowBuffer tcA, tcB, tcNorms, tcTables, tcRows, tcFlags;
+  unsigned long long tcCalls = 0;          // selects the flag area
+  bool tcDirty = false;                    // a call returned with an error after it had started to use its flag area
+  bool tcConfigured = false;               // the GEMM kernel's shared-memory size is set
+  bool tcPendingStats = false;             // h_tcFlags holds the last call's counters, not yet read
+
+  // pinned host words
+  unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
+  unsigned int *h_tcFlags = nullptr;       // 16: the tensor path's flag area of the last call
+  unsigned int *h_pairTotal = nullptr;     // the pair total of the last mutual or ratio call
+  void *h_verify = nullptr;                // the state a verify call copies back
+
+  unsigned long long matchStats[4] = {0, 0, 0, 0};
+  long long verifyStats[8] = {0, 0, 0, 0, -1, 0, 0, 0};
+
+  int ensure(int d);
+  Pipeline *get_pipe(int w, int h, int oct, bool up, float *arena, int *err);
+  Pipeline2 *get_pipe2(int w, int h, int oct, bool up, float *arena, int *err);
+  void drop_pipes(float *arena, bool internalOnly);
+};
+
+// CUDASIFT_MATCH_TIMING=1: nine events for timing the kernels of a match or verify call, else null
+cudaEvent_t *match_timing_events();
+
 // ---- matcher ------------------------------------------------------------------------
-struct MatchWorkspace;   // opaque, owned by the per-device context
 // the cross-check of a mutual match: pairs with score > minScore and ambiguity < maxAmbiguity, at most maxPairs written
 struct MutualArgs {
   float minScore, maxAmbiguity;
@@ -199,27 +279,27 @@ struct MutualArgs {
   int maxPairs;
 };
 int match_exact(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cudaStream_t st);
+// The launchers below run on c.stream.
 // tensor path: set 1 against set 2, or with mu (32 or more rows in each set) both directions and then the pairs
-int match_tensor(SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs *mu, cudaStream_t st);
+int match_tensor(DeviceCtx &c, SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs *mu);
 bool match_tensor_supported();
-void match_tensor_stats(unsigned long long stats[4]);   // after a synchronize
-// cross-check of two finished directions (match_mutual.cu); the total is read by mutual_pairs_total() after a synchronize
-int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu, cudaStream_t st);
-int mutual_pairs_total();
+void match_tensor_stats(DeviceCtx &c, unsigned long long stats[4]);   // after a synchronize
+// cross-check of two finished directions (match_mutual.cu); the total reaches *c.h_pairTotal by the synchronize
+int launch_mutual_pairs(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu);
 // two nearest neighbours among all candidates (match_knn.cu states the order): idx / score are [n1][2], 8-byte aligned
-int knn_exact(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, cudaStream_t st);
+int knn_exact(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score);
 // tensor path of the same; with idx2 also set 2 against set 1 (match_tc.cu)
-int match_knn_tensor(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx1, float *score1, int *idx2,
-                     float *score2, cudaStream_t st);
-// Lowe's ratio test (COLMAP's rule) on finished knn lists, cross-checked when idx2 != nullptr; the total is read by
-// mutual_pairs_total() after a synchronize
+int match_knn_tensor(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx1, float *score1,
+                     int *idx2, float *score2);
+// Lowe's ratio test (COLMAP's rule) on finished knn lists, cross-checked when idx2 != nullptr; the total reaches
+// *c.h_pairTotal by the synchronize
 struct RatioArgs {
   float maxRatio, maxDistance;
   int2 *pairs;
   int maxPairs;
 };
-int launch_ratio_pairs(const int *idx1, const float *score1, int n1, const int *idx2, const float *score2, int n2,
-                       const RatioArgs &ra, cudaStream_t st);
+int launch_ratio_pairs(DeviceCtx &c, const int *idx1, const float *score1, int n1, const int *idx2, const float *score2,
+                       int n2, const RatioArgs &ra);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 size_t verify_scratch_bytes(int numPairs, int numLoops);   // device scratch of one call

@@ -153,21 +153,6 @@ knn_merge_kernel(int n1, const int *__restrict__ rows, const unsigned int *__res
   }
 }
 
-// Per-device partial area of the sliced scan (single-threaded per device, like the matcher's workspace).
-struct KnnWorkspace {
-  Top2 *part = nullptr;
-  size_t cap = 0;
-};
-static KnnWorkspace g_wsk[16];
-
-static int knn_sms()
-{
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
-}
-
 // Slices of the candidate range: enough CTAs for two per SM when the rows alone do not provide them, and at least
 // KX_MIN_STEPS candidate steps per slice.
 static int knn_slices(int rowBlocks, int n2, int sms)
@@ -180,30 +165,24 @@ static int knn_slices(int rowBlocks, int n2, int sms)
   return s < 1 ? 1 : s;
 }
 
-static int knn_launch(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, const int *rows,
-                      const unsigned int *nrows, const unsigned int *gate, int rowBlocks, int slices, cudaStream_t st)
+// More than one slice: the slices' partial results go to c.knnPartials.
+static int knn_launch(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score,
+                      const int *rows, const unsigned int *nrows, const unsigned int *gate, int rowBlocks, int slices)
 {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  KnnWorkspace &ws = g_wsk[dev & 15];
   int2 *i2 = reinterpret_cast<int2 *>(idx);
   float2 *f2 = reinterpret_cast<float2 *>(score);
   Top2 *part = nullptr;
   if (slices > 1) {
-    const size_t bytes = (size_t)slices * n1 * sizeof(Top2);
-    if (ws.cap < bytes) {
-      if (ws.part) cudaFree(ws.part);
-      ws.part = nullptr; ws.cap = 0;
-      CS_CUDA(cudaMalloc((void **)&ws.part, bytes));
-      ws.cap = bytes;
-    }
-    part = ws.part;
+    int r;
+    if ((r = c.knnPartials.grow((size_t)slices * n1 * sizeof(Top2))) < 0) return r;
+    part = c.knnPartials.as<Top2>();
   }
-  knn_exact_kernel<<<dim3(rowBlocks, slices), KX_THREADS, 0, st>>>(s1, s2, n1, n2, rows, nrows, gate, i2, f2, part, n1);
+  knn_exact_kernel<<<dim3(rowBlocks, slices), KX_THREADS, 0, c.stream>>>(s1, s2, n1, n2, rows, nrows, gate, i2, f2, part,
+                                                                         n1);
   count_launch();
   if (part) {
     const int blocks = idivup(n1, 256) < 264 ? idivup(n1, 256) : 264;
-    knn_merge_kernel<<<blocks, 256, 0, st>>>(n1, rows, nrows, gate, part, n1, slices, i2, f2);
+    knn_merge_kernel<<<blocks, 256, 0, c.stream>>>(n1, rows, nrows, gate, part, n1, slices, i2, f2);
     count_launch();
   }
   CS_CUDA(cudaGetLastError());
@@ -211,22 +190,22 @@ static int knn_launch(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, 
 }
 
 // Every row of set 1 (mode 1 and small sets).
-int knn_exact(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, cudaStream_t st)
+int knn_exact(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score)
 {
   if (n1 <= 0 || n2 <= 0) return 0;
   const int rowBlocks = idivup(n1, KX_ROWS);
-  return knn_launch(s1, n1, s2, n2, idx, score, nullptr, nullptr, nullptr, rowBlocks,
-                    knn_slices(rowBlocks, n2, knn_sms()), st);
+  const int slices = knn_slices(rowBlocks, n2, c.sms);
+  return knn_launch(c, s1, n1, s2, n2, idx, score, nullptr, nullptr, nullptr, rowBlocks, slices);
 }
 
 // Fallback of the tensor path, decided on the device: the listed rows (usually a few, so the slices are chosen for one
 // row block), or every row if *gate != 0 (grid-strided over at most 296 row blocks).
-int knn_exact_fallback(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, const int *rows,
-                       const unsigned int *nrows, const unsigned int *gate, cudaStream_t st)
+int knn_exact_fallback(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score,
+                       const int *rows, const unsigned int *nrows, const unsigned int *gate)
 {
   if (n1 <= 0 || n2 <= 0) return 0;
   const int rowBlocks = idivup(n1, KX_ROWS) < 296 ? idivup(n1, KX_ROWS) : 296;
-  return knn_launch(s1, n1, s2, n2, idx, score, rows, nrows, gate, rowBlocks, knn_slices(1, n2, knn_sms()), st);
+  return knn_launch(c, s1, n1, s2, n2, idx, score, rows, nrows, gate, rowBlocks, knn_slices(1, n2, c.sms));
 }
 
 }  // namespace cs

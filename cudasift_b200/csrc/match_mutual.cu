@@ -110,78 +110,50 @@ ratio_flags_kernel(const int2 *__restrict__ idx1, const float2 *__restrict__ sco
   if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
 }
 
-// Per-device scratch (like the matcher's workspace, single-threaded per device): ballot words, CTA counts, the total.
-struct MutualWorkspace {
-  unsigned int *d = nullptr;
-  size_t cap = 0;
-  unsigned int *h_total = nullptr;    // pinned
-};
-static MutualWorkspace g_wsm[16];
-
-// ballot words, CTA counts and the total of n1 rows
-static int pairs_scratch(int n1, unsigned int **masks, unsigned int **counts, unsigned int **total)
+// Ballot words, CTA counts and the total of n1 rows in c.pairScratch; the total is copied to *c.h_pairTotal after the
+// two launches.
+static int pairs_scratch(DeviceCtx &c, int n1, unsigned int **masks, unsigned int **counts, unsigned int **total)
 {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  MutualWorkspace &ws = g_wsm[dev & 15];
   const int blocks = idivup(n1, MP_ROWS), words = idivup(n1, 32);
-  const size_t bytes = ((size_t)words + blocks + 1) * sizeof(unsigned int);
-  if (ws.cap < bytes) {
-    if (ws.d) cudaFree(ws.d);
-    ws.d = nullptr; ws.cap = 0;
-    CS_CUDA(cudaMalloc((void **)&ws.d, bytes));
-    ws.cap = bytes;
-  }
-  if (!ws.h_total) CS_CUDA(cudaMallocHost((void **)&ws.h_total, sizeof(unsigned int)));
-  *masks = ws.d; *counts = ws.d + words; *total = *counts + blocks;
+  int r;
+  if ((r = c.pairScratch.grow(((size_t)words + blocks + 1) * sizeof(unsigned int))) < 0) return r;
+  if (!c.h_pairTotal) CS_CUDA(cudaMallocHost((void **)&c.h_pairTotal, sizeof(unsigned int)));
+  *masks = c.pairScratch.as<unsigned int>(); *counts = *masks + words; *total = *counts + blocks;
   return 0;
 }
 
-static int pairs_total_to_host(const unsigned int *total, cudaStream_t st)
+int launch_mutual_pairs(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu)
 {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  CS_CUDA(cudaMemcpyAsync(g_wsm[dev & 15].h_total, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+  unsigned int *masks, *counts, *total;
+  int r;
+  if ((r = pairs_scratch(c, n1, &masks, &counts, &total)) < 0) return r;
+  const int blocks = idivup(n1, MP_ROWS);
+  mutual_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, masks, counts);
+  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(&s1[0].match, (int)(sizeof(SiftPoint) / sizeof(int)), n1, masks,
+                                                        counts, mu.pairs, mu.maxPairs, total);
+  count_launch(2);
+  CS_CUDA(cudaGetLastError());
+  CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
   return 0;
 }
 
-int launch_mutual_pairs(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu, cudaStream_t st)
+int launch_ratio_pairs(DeviceCtx &c, const int *idx1, const float *score1, int n1, const int *idx2, const float *score2,
+                       int n2, const RatioArgs &ra)
 {
   unsigned int *masks, *counts, *total;
   int r;
-  if ((r = pairs_scratch(n1, &masks, &counts, &total)) < 0) return r;
+  if ((r = pairs_scratch(c, n1, &masks, &counts, &total)) < 0) return r;
   const int blocks = idivup(n1, MP_ROWS);
-  mutual_flags_kernel<<<blocks, MP_ROWS, 0, st>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, masks, counts);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, st>>>(&s1[0].match, (int)(sizeof(SiftPoint) / sizeof(int)), n1, masks, counts,
-                                                  mu.pairs, mu.maxPairs, total);
+  ratio_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(reinterpret_cast<const int2 *>(idx1),
+                                                       reinterpret_cast<const float2 *>(score1), n1,
+                                                       reinterpret_cast<const int2 *>(idx2),
+                                                       reinterpret_cast<const float2 *>(score2), n2, (double)ra.maxRatio,
+                                                       (double)ra.maxDistance, masks, counts);
+  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(idx1, 2, n1, masks, counts, ra.pairs, ra.maxPairs, total);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
-  return pairs_total_to_host(total, st);
-}
-
-int launch_ratio_pairs(const int *idx1, const float *score1, int n1, const int *idx2, const float *score2, int n2,
-                       const RatioArgs &ra, cudaStream_t st)
-{
-  unsigned int *masks, *counts, *total;
-  int r;
-  if ((r = pairs_scratch(n1, &masks, &counts, &total)) < 0) return r;
-  const int blocks = idivup(n1, MP_ROWS);
-  ratio_flags_kernel<<<blocks, MP_ROWS, 0, st>>>(reinterpret_cast<const int2 *>(idx1), reinterpret_cast<const float2 *>(score1),
-                                                 n1, reinterpret_cast<const int2 *>(idx2),
-                                                 reinterpret_cast<const float2 *>(score2), n2, (double)ra.maxRatio,
-                                                 (double)ra.maxDistance, masks, counts);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, st>>>(idx1, 2, n1, masks, counts, ra.pairs, ra.maxPairs, total);
-  count_launch(2);
-  CS_CUDA(cudaGetLastError());
-  return pairs_total_to_host(total, st);
-}
-
-int mutual_pairs_total()
-{
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const MutualWorkspace &ws = g_wsm[dev & 15];
-  return ws.h_total ? (int)*ws.h_total : 0;
+  CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
+  return 0;
 }
 
 }  // namespace cs

@@ -732,47 +732,12 @@ int match_exact_fallback(SiftPoint *s1, int n1, const SiftPoint *s2, int n2, con
                          const unsigned int *gate, cudaStream_t st);
 
 // ------------------------------------------------------------------------------ host
-static int ensure(void **p, size_t *cap, size_t bytes)
-{
-  if (*cap >= bytes) return 0;
-  if (*p) cudaFree(*p);
-  *p = nullptr; *cap = 0;
-  CS_CUDA(cudaMalloc(p, bytes));
-  *cap = bytes;
-  return 0;
-}
-
 bool match_tensor_supported()
 {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return false;
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   return major == 9;
-}
-
-// One workspace per device, used on the caller's stream: like the reference (function-local static caches,
-// cudaSiftH.cu:310,409) the matcher is single-threaded per device -- two host threads matching on the same device at
-// the same time would share the tables and the flag areas.
-struct T3Workspace {
-  T3Buffers bf = {};
-  size_t cap[8] = {};
-  unsigned int *h_counters = nullptr;
-  // 2 x 16 words, used alternately: [0] max norm of the candidates, [1] bad-input flag, [4..6] counters; a mutual call
-  // adds [2] the max norm of the reverse direction's candidates and [8..10] its counters
-  float *flags = nullptr;
-  unsigned long long calls = 0;
-  bool dirty = false;             // a call returned with an error after it had started to use the current flag area
-  bool configured = false;
-  bool pendingStats = false;
-};
-static T3Workspace g_ws3[16];
-
-static int t3_sms()
-{
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms;
 }
 
 // persistent GEMM schedule: n1 rows against the first n2v candidates
@@ -790,33 +755,82 @@ static TcPlan t3_plan(int n1, int n2v, int sms)
 }
 static size_t t3_slots(const TcPlan &pl) { return (size_t)pl.grid * pl.runs * T3_MT; }
 
-// Grows the workspace buffers to the given sizes and selects this call's flag area (*flags).  Flags and counters live
-// in two 64-byte areas used alternately: a call's prep kernel clears the other one (*nextFlags) for the next call,
-// which saves a memset node per call.
-static int t3_begin(T3Workspace &ws, size_t aBytes, size_t bBytes, size_t normRows, size_t slots, size_t fbRows,
-                    cudaStream_t st, float **flags, float **nextFlags)
+// A tensor-path call once its prep kernel is in: each direction's plan and view of the workspace, the bad-input gate
+// (shared: any bad value, either set), the call's flag area and the timing events (or null).
+struct T3Call {
+  TcPlan pf, pr;
+  T3Buffers fw, rv;
+  const unsigned int *gate;
+  const float *flags;
+  cudaEvent_t *tev;
+};
+
+// The part of a call that matching and knn share: grows the workspace, fills the prep sets, builds the forward view
+// (set 1 against set 2) and, with both, the reverse one, and launches the prep kernel.  n1v / n2v are the rows of each
+// set that are candidates of the other direction: 32*floor(n/32) in a match (quirk Q7), all of them in knn.  Set 1 has
+// the A role, set 2 the B role, and with both each set has both roles.  Workspace: the sets' tiles one after the other
+// in tcA (their norms likewise in tcNorms, set 2's unread in a one-way call), the B-role copies in tcB.  The top-3 tables
+// and the fallback row list are shared: the two directions are stream-ordered.  Flags and counters live in two 64-byte
+// areas used alternately: a call's prep kernel clears the other one for the next call, which saves a memset node.
+static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const SiftPoint *s2, int n2, int n2v, bool both,
+                    T3Call &t)
 {
-  T3Buffers &bf = ws.bf;
+  t.pf = t3_plan(n1, n2v, c.sms);
+  t.pr = both ? t3_plan(n2, n1v, c.sms) : TcPlan{};
+  T3PrepSet p[2] = {{s1, n1, both ? n1v : 0}, {s2, both ? n2 : n2v, n2v}};
+  size_t aOff[2], bOff[2], nOff[2], aBytes = 0, bBytes = 0, rows = 0;
+  bool copy[2];
+  for (int k = 0; k < 2; k++) {
+    const int tiles = idivup(p[k].n, T3_MT);
+    p[k].blocks = tiles * (T3_MT / 32);
+    p[k].bTiles = idivup(p[k].nv, T3_N);
+    aOff[k] = aBytes; aBytes += (size_t)tiles * T3_A_BYTES;
+    nOff[k] = rows; rows += (size_t)tiles * T3_MT;
+    // a set needs its own B-role copy when its tail rows [nv, n) lie in a tile that the B role reads (never in knn)
+    copy[k] = p[k].n != p[k].nv && p[k].nv % T3_N != 0;
+    bOff[k] = bBytes; bBytes += copy[k] ? (size_t)p[k].bTiles * T3_B_BYTES : 0;
+  }
+  const size_t slots = t3_slots(t.pf) > t3_slots(t.pr) ? t3_slots(t.pf) : t3_slots(t.pr);
+  const size_t fbRows = (size_t)(t.pf.n_mt > t.pr.n_mt ? t.pf.n_mt : t.pr.n_mt) * T3_MT;
+  const cudaStream_t st = c.stream;
   int r;
-  if ((r = ensure((void **)&bf.a16, &ws.cap[0], aBytes)) < 0) return r;
-  if ((r = ensure((void **)&bf.b16, &ws.cap[1], bBytes)) < 0) return r;
-  if ((r = ensure((void **)&bf.normA, &ws.cap[2], normRows * sizeof(float))) < 0) return r;
-  if ((r = ensure((void **)&bf.pm, &ws.cap[3], slots * T3_PM * sizeof(float))) < 0) return r;
-  if ((r = ensure((void **)&bf.fbRows, &ws.cap[4], fbRows * sizeof(int))) < 0) return r;
-  if (!ws.flags) {
-    size_t dummy = 0;
-    if ((r = ensure((void **)&ws.flags, &dummy, 128)) < 0) return r;
-    CS_CUDA(cudaMemsetAsync(ws.flags, 0, 128, st));
-    CS_CUDA(cudaMallocHost((void **)&ws.h_counters, 64));
+  if ((r = c.tcA.grow(aBytes)) < 0 || (r = c.tcB.grow(bBytes)) < 0 || (r = c.tcNorms.grow(rows * sizeof(float))) < 0 ||
+      (r = c.tcTables.grow(slots * T3_PM * sizeof(float))) < 0 || (r = c.tcRows.grow(fbRows * sizeof(int))) < 0)
+    return r;
+  if (!c.h_tcFlags) {
+    if ((r = c.tcFlags.grow(128)) < 0) return r;
+    CS_CUDA(cudaMemsetAsync(c.tcFlags.p, 0, 128, st));
+    CS_CUDA(cudaMallocHost((void **)&c.h_tcFlags, 64));
   }
-  *flags = ws.flags + 16 * (ws.calls & 1);
-  *nextFlags = ws.flags + 16 * ((ws.calls + 1) & 1);
-  if (ws.dirty) CS_CUDA(cudaMemsetAsync(ws.flags, 0, 128, st));     // a previous call failed between its launches
-  ws.dirty = true;                                                  // until this call's launches are all in
-  if (!ws.configured) {
+  float *flags = c.tcFlags.as<float>() + 16 * (c.tcCalls & 1);
+  float *nextFlags = c.tcFlags.as<float>() + 16 * ((c.tcCalls + 1) & 1);
+  if (c.tcDirty) CS_CUDA(cudaMemsetAsync(c.tcFlags.p, 0, 128, st));   // a previous call failed between its launches
+  c.tcDirty = true;                                                  // until this call's launches are all in
+  if (!c.tcConfigured) {
     CS_CUDA(cudaFuncSetAttribute(t3_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T3_SMEM_BYTES));
-    ws.configured = true;
+    c.tcConfigured = true;
   }
+  auto at = [](void *base, size_t bytes) { return reinterpret_cast<__half *>(static_cast<uint8_t *>(base) + bytes); };
+  for (int k = 0; k < 2; k++) {
+    p[k].a = at(c.tcA.p, aOff[k]);
+    p[k].b = copy[k] ? at(c.tcB.p, bOff[k]) : nullptr;
+    p[k].norms = c.tcNorms.as<float>() + nOff[k];
+  }
+  // flags [0] / [2] take the candidates' max norm of the forward / reverse direction, i.e. of set 2 / set 1; the
+  // counters of the two directions are flags [4..6] and [8..10]
+  p[0].bmax = flags + 2; p[1].bmax = flags;
+  unsigned int *counters = reinterpret_cast<unsigned int *>(flags);
+  t.fw = {p[0].a, copy[1] ? p[1].b : p[1].a, p[0].norms, flags, c.tcTables.as<float>(), c.tcRows.as<int>(), counters + 4};
+  t.rv = {p[1].a, copy[0] ? p[0].b : p[0].a, p[1].norms, flags + 2, c.tcTables.as<float>(), c.tcRows.as<int>(),
+          counters + 8};
+  t.gate = counters + 1;
+  t.flags = flags;
+  t.tev = match_timing_events();
+  if (t.tev) cudaEventRecord(t.tev[0], st);
+  t3_prep_kernel<<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], flags + 1, nextFlags);
+  count_launch();
+  CS_CUDA(cudaGetLastError());
+  if (t.tev) cudaEventRecord(t.tev[1], st);
   return 0;
 }
 
@@ -839,17 +853,17 @@ static int t3_direction(const TcPlan &pl, const T3Buffers &bf, SiftPoint *s1, in
 }
 
 // the call's counters to the host, read by match_tensor_stats() after the caller's synchronize
-static int t3_end(T3Workspace &ws, const float *flags, cudaStream_t st)
+static int t3_end(DeviceCtx &c, const float *flags)
 {
-  CS_CUDA(cudaMemcpyAsync(ws.h_counters, flags, 64, cudaMemcpyDeviceToHost, st));
-  ws.calls++;                           // the prep kernel of this call cleared the other flag area for the next one
-  ws.dirty = false;
-  ws.pendingStats = true;
+  CS_CUDA(cudaMemcpyAsync(c.h_tcFlags, flags, 64, cudaMemcpyDeviceToHost, c.stream));
+  c.tcCalls++;                          // the prep kernel of this call cleared the other flag area for the next one
+  c.tcDirty = false;
+  c.tcPendingStats = true;
   return 0;
 }
 
-// CUDASIFT_MATCH_TIMING=1: CUDA events between the kernels, printed to stderr (warm caches, unlike ncu)
-static cudaEvent_t *t3_timing_events()
+// CUDA events between the kernels, printed to stderr (warm caches, unlike ncu)
+cudaEvent_t *match_timing_events()
 {
   static int timing = -1;
   static cudaEvent_t tev[9];
@@ -860,8 +874,11 @@ static cudaEvent_t *t3_timing_events()
   }
   return timing ? tev : nullptr;
 }
-static void t3_print_timing(const char *what, int n1, int n2, const cudaEvent_t *tev, const char *const *names, int n)
+// the first n stages: a one-way call has 4, a two-way knn call 7, a mutual call 8
+static void t3_print_timing(const char *what, int n1, int n2, const cudaEvent_t *tev, int n)
 {
+  static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
+                                      "reverse-exact-fallback", "pairs"};
   cudaEventSynchronize(tev[n]);
   fprintf(stderr, "%s timing %dx%d [us]:", what, n1, n2);
   for (int i = 0; i < n; i++) {
@@ -874,86 +891,40 @@ static void t3_print_timing(const char *what, int n1, int n2, const cudaEvent_t 
 
 // Set 1's five match fields; with mu (32 or more rows in each set) also set 2's, exactly as a one-way match of set 2
 // against set 1 writes them, then the cross-checked pairs (launch_mutual_pairs).  One prep launch converts each set once
-// for every role it has (T3PrepSet); each direction then runs on its own plan and its own view of the workspace.  The
-// top-3 tables and the fallback row list are shared: the two directions are stream-ordered.
-int match_tensor(SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs *mu, cudaStream_t st)
+// for every role it has (T3PrepSet); each direction then runs on its own plan and its own view of the workspace.
+int match_tensor(DeviceCtx &c, SiftPoint *s1, int n1, SiftPoint *s2, int n2, const MutualArgs *mu)
 {
   const int n1v = (n1 / 32) * 32, n2v = (n2 / 32) * 32;   // matching.cu:325 (quirk Q7)
   if (!mu) {
     if (n1 <= 0) return 0;
-    if (n2v == 0 || !match_tensor_supported()) return match_exact(s1, n1, s2, n2, st);
+    if (n2v == 0 || !match_tensor_supported()) return match_exact(s1, n1, s2, n2, c.stream);
   } else if (n1v == 0 || n2v == 0) {
     set_error("match_tensor: a mutual match needs 32 rows or more in each set");
     return CS_E_ARG;
   }
-  int dev = 0;
-  cudaGetDevice(&dev);
-  T3Workspace &ws = g_ws3[dev & 15];
-  const int sms = t3_sms();
-  const TcPlan pf = t3_plan(n1, n2v, sms), pr = mu ? t3_plan(n2, n1v, sms) : TcPlan{};
-  // set 1 has the A role, set 2 the B role; in a mutual match each set has both.  Workspace: the sets' tiles one after
-  // the other in a16 (their norms likewise in normA, set 2's unread in a one-way match), the B-role copies in b16.
-  T3PrepSet p[2] = {{s1, n1, mu ? n1v : 0}, {s2, mu ? n2 : n2v, n2v}};
-  size_t aOff[2], bOff[2], nOff[2], aBytes = 0, bBytes = 0, rows = 0;
-  bool copy[2];
-  for (int k = 0; k < 2; k++) {
-    const int tiles = idivup(p[k].n, T3_MT);
-    p[k].blocks = tiles * (T3_MT / 32);
-    p[k].bTiles = idivup(p[k].nv, T3_N);
-    aOff[k] = aBytes; aBytes += (size_t)tiles * T3_A_BYTES;
-    nOff[k] = rows; rows += (size_t)tiles * T3_MT;
-    // a set needs its own B-role copy when its tail rows [nv, n) lie in a tile that the B role reads
-    copy[k] = p[k].n != p[k].nv && p[k].nv % T3_N != 0;
-    bOff[k] = bBytes; bBytes += copy[k] ? (size_t)p[k].bTiles * T3_B_BYTES : 0;
-  }
-  const size_t slots = t3_slots(pf) > t3_slots(pr) ? t3_slots(pf) : t3_slots(pr);
-  float *flags = nullptr, *nextFlags = nullptr;
+  T3Call t;
   int r;
-  if ((r = t3_begin(ws, aBytes, bBytes, rows, slots, (size_t)(pf.n_mt > pr.n_mt ? pf.n_mt : pr.n_mt) * T3_MT, st,
-                    &flags, &nextFlags)) < 0)
-    return r;
-  auto at = [](__half *p, size_t bytes) { return reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(p) + bytes); };
-  for (int k = 0; k < 2; k++) {
-    p[k].a = at(ws.bf.a16, aOff[k]);
-    p[k].b = copy[k] ? at(ws.bf.b16, bOff[k]) : nullptr;
-    p[k].norms = ws.bf.normA + nOff[k];
-  }
-  // flags [0] / [2] take the candidates' max norm of the forward / reverse direction, i.e. of set 2 / set 1
-  p[0].bmax = flags + 2; p[1].bmax = flags;
-  T3Buffers fw = ws.bf, rv = ws.bf;
-  fw.a16 = p[0].a; fw.b16 = copy[1] ? p[1].b : p[1].a; fw.normA = p[0].norms;
-  fw.bmax = flags; fw.counters = reinterpret_cast<unsigned int *>(flags) + 4;
-  rv.a16 = p[1].a; rv.b16 = copy[0] ? p[0].b : p[0].a; rv.normA = p[1].norms;
-  rv.bmax = flags + 2; rv.counters = reinterpret_cast<unsigned int *>(flags) + 8;
-  const unsigned int *gate = reinterpret_cast<const unsigned int *>(flags) + 1;   // shared: any bad value, either set
-  cudaEvent_t *tev = t3_timing_events();
-  if (tev) cudaEventRecord(tev[0], st);
-  t3_prep_kernel<<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], flags + 1, nextFlags);
-  count_launch();
-  CS_CUDA(cudaGetLastError());
-  if (tev) cudaEventRecord(tev[1], st);
-  if ((r = t3_direction(pf, fw, s1, n1, s2, n2, gate, st, tev ? tev + 2 : nullptr)) < 0) return r;
+  if ((r = t3_setup(c, s1, n1, n1v, s2, n2, n2v, mu != nullptr, t)) < 0) return r;
+  cudaEvent_t *tev = t.tev;
+  if ((r = t3_direction(t.pf, t.fw, s1, n1, s2, n2, t.gate, c.stream, tev ? tev + 2 : nullptr)) < 0) return r;
   if (mu) {
-    if ((r = t3_direction(pr, rv, s2, n2, s1, n1, gate, st, tev ? tev + 5 : nullptr)) < 0) return r;
-    if ((r = launch_mutual_pairs(s1, n1, s2, n2, *mu, st)) < 0) return r;
-    if (tev) cudaEventRecord(tev[8], st);
+    if ((r = t3_direction(t.pr, t.rv, s2, n2, s1, n1, t.gate, c.stream, tev ? tev + 5 : nullptr)) < 0) return r;
+    if ((r = launch_mutual_pairs(c, s1, n1, s2, n2, *mu)) < 0) return r;
+    if (tev) cudaEventRecord(tev[8], c.stream);
   }
-  if (tev) {
-    static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
-                                        "reverse-exact-fallback", "pairs"};
-    t3_print_timing(mu ? "mutual" : "match", n1, n2, tev, names, mu ? 8 : 4);
-  }
-  return t3_end(ws, flags, st);
+  if (tev) t3_print_timing(mu ? "mutual" : "match", n1, n2, tev, mu ? 8 : 4);
+  return t3_end(c, t.flags);
 }
 
 // exact two-nearest-neighbour scan of the listed rows, or of every row if *gate != 0 (match_knn.cu)
-int knn_exact_fallback(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score, const int *rows,
-                       const unsigned int *nrows, const unsigned int *gate, cudaStream_t st);
+int knn_exact_fallback(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score,
+                       const int *rows, const unsigned int *nrows, const unsigned int *gate);
 
 // One knn direction after the prep kernel: GEMM, knn resolve, exact fallback.  ev (optional): three events.
-static int knn_direction(const TcPlan &pl, const T3Buffers &bf, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2,
-                         int *idx, float *score, const unsigned int *gate, cudaStream_t st, cudaEvent_t *ev)
+static int knn_direction(DeviceCtx &c, const TcPlan &pl, const T3Buffers &bf, const SiftPoint *s1, int n1,
+                         const SiftPoint *s2, int n2, int *idx, float *score, const unsigned int *gate, cudaEvent_t *ev)
 {
+  const cudaStream_t st = c.stream;
   t3_gemm_kernel<<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf);
   if (ev) cudaEventRecord(ev[0], st);
   knn_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2, n2, reinterpret_cast<int2 *>(idx),
@@ -962,78 +933,38 @@ static int knn_direction(const TcPlan &pl, const T3Buffers &bf, const SiftPoint 
   count_launch(2);
   CS_CUDA(cudaGetLastError());
   int r;
-  if ((r = knn_exact_fallback(s1, n1, s2, n2, idx, score, bf.fbRows, bf.counters, gate, st)) < 0) return r;
+  if ((r = knn_exact_fallback(c, s1, n1, s2, n2, idx, score, bf.fbRows, bf.counters, gate)) < 0) return r;
   if (ev) cudaEventRecord(ev[2], st);
   return 0;
 }
 
 // The two nearest neighbours of every row of set 1 among all n2 candidates (idx1 / score1, [n1][2]); with idx2 also
-// those of every row of set 2 among set 1's n1 rows.  The records are only read.  Same plan, workspace, flag areas and
-// bad-input gate as match_tensor; there is no Q7 tail, so each set is prepared with n == nv: its A tiles are also the
-// other direction's B operand (rows past n are zeros, score 0, and never enter the tables).
-int match_knn_tensor(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx1, float *score1, int *idx2,
-                     float *score2, cudaStream_t st)
+// those of every row of set 2 among set 1's n1 rows.  The records are only read.  Same setup as match_tensor; there is
+// no Q7 tail, so each set's A tiles are also the other direction's B operand (rows past n are zeros, score 0, and never
+// enter the tables).
+int match_knn_tensor(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx1, float *score1,
+                     int *idx2, float *score2)
 {
   if (n1 <= 0 || n2 <= 0) return 0;
   const bool both = idx2 != nullptr;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  T3Workspace &ws = g_ws3[dev & 15];
-  const int sms = t3_sms();
-  const TcPlan pf = t3_plan(n1, n2, sms), pr = both ? t3_plan(n2, n1, sms) : TcPlan{};
-  T3PrepSet p[2] = {{s1, n1, both ? n1 : 0}, {s2, n2, n2}};
-  size_t aOff[2], nOff[2], aBytes = 0, rows = 0;
-  for (int k = 0; k < 2; k++) {
-    const int tiles = idivup(p[k].n, T3_MT);
-    p[k].blocks = tiles * (T3_MT / 32);
-    p[k].bTiles = idivup(p[k].nv, T3_N);
-    aOff[k] = aBytes; aBytes += (size_t)tiles * T3_A_BYTES;
-    nOff[k] = rows; rows += (size_t)tiles * T3_MT;
-  }
-  const size_t slots = t3_slots(pf) > t3_slots(pr) ? t3_slots(pf) : t3_slots(pr);
-  float *flags = nullptr, *nextFlags = nullptr;
+  T3Call t;
   int r;
-  if ((r = t3_begin(ws, aBytes, 0, rows, slots, (size_t)(pf.n_mt > pr.n_mt ? pf.n_mt : pr.n_mt) * T3_MT, st, &flags,
-                    &nextFlags)) < 0)
+  if ((r = t3_setup(c, s1, n1, n1, s2, n2, n2, both, t)) < 0) return r;
+  cudaEvent_t *tev = t.tev;
+  if ((r = knn_direction(c, t.pf, t.fw, s1, n1, s2, n2, idx1, score1, t.gate, tev ? tev + 2 : nullptr)) < 0) return r;
+  if (both && (r = knn_direction(c, t.pr, t.rv, s2, n2, s1, n1, idx2, score2, t.gate, tev ? tev + 5 : nullptr)) < 0)
     return r;
-  for (int k = 0; k < 2; k++) {
-    p[k].a = reinterpret_cast<__half *>(reinterpret_cast<uint8_t *>(ws.bf.a16) + aOff[k]);
-    p[k].b = nullptr;
-    p[k].norms = ws.bf.normA + nOff[k];
-  }
-  p[0].bmax = flags + 2; p[1].bmax = flags;
-  T3Buffers fw = ws.bf, rv = ws.bf;
-  fw.a16 = p[0].a; fw.b16 = p[1].a; fw.normA = p[0].norms;
-  fw.bmax = flags; fw.counters = reinterpret_cast<unsigned int *>(flags) + 4;
-  rv.a16 = p[1].a; rv.b16 = p[0].a; rv.normA = p[1].norms;
-  rv.bmax = flags + 2; rv.counters = reinterpret_cast<unsigned int *>(flags) + 8;
-  const unsigned int *gate = reinterpret_cast<const unsigned int *>(flags) + 1;
-  cudaEvent_t *tev = t3_timing_events();
-  if (tev) cudaEventRecord(tev[0], st);
-  t3_prep_kernel<<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], flags + 1, nextFlags);
-  count_launch();
-  CS_CUDA(cudaGetLastError());
-  if (tev) cudaEventRecord(tev[1], st);
-  if ((r = knn_direction(pf, fw, s1, n1, s2, n2, idx1, score1, gate, st, tev ? tev + 2 : nullptr)) < 0) return r;
-  if (both && (r = knn_direction(pr, rv, s2, n2, s1, n1, idx2, score2, gate, st, tev ? tev + 5 : nullptr)) < 0) return r;
-  if (tev) {
-    static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
-                                        "reverse-exact-fallback"};
-    t3_print_timing("knn", n1, n2, tev, names, both ? 7 : 4);
-  }
-  return t3_end(ws, flags, st);
+  if (tev) t3_print_timing("knn", n1, n2, tev, both ? 7 : 4);
+  return t3_end(c, t.flags);
 }
 
-// statistics of the last match_tensor on this device (call after the stream was synchronized);
-// a mutual call reports both directions summed
-void match_tensor_stats(unsigned long long stats[4])
+// statistics of the last tensor-path call on this context (call after the stream was synchronized);
+// a two-way call reports both directions summed
+void match_tensor_stats(DeviceCtx &c, unsigned long long stats[4])
 {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  T3Workspace &ws = g_ws3[dev & 15];
-  if (!ws.pendingStats) return;
-  ws.pendingStats = false;
-  const unsigned int *h = ws.h_counters;
+  if (!c.tcPendingStats) return;
+  c.tcPendingStats = false;
+  const unsigned int *h = c.h_tcFlags;
   if (h[1] != 0) { stats[0] = stats[1] = 0; stats[2] = ~0ull; return; }   // everything went the exact way
   stats[0] = (unsigned long long)h[4 + 1] + h[8 + 1];                     // [8..10] stay zero in a single direction
   stats[1] = (unsigned long long)h[4 + 2] + h[8 + 2];

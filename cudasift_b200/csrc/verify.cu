@@ -734,19 +734,7 @@ static VerifyLayout verify_layout(int numPairs, int numLoops)
 size_t verify_scratch_bytes(int numPairs, int numLoops) { return verify_layout(numPairs, numLoops).bytes; }
 size_t verify_result_bytes() { return sizeof(VerifyState); }
 
-// CUDASIFT_MATCH_TIMING=1: CUDA events between the kernels, printed to stderr
-static cudaEvent_t *vp_timing_events()
-{
-  static int timing = -1;
-  static cudaEvent_t tev[9];
-  if (timing < 0) {
-    const char *e = getenv("CUDASIFT_MATCH_TIMING");
-    timing = (e && atoi(e)) ? 1 : 0;
-    if (timing) for (int i = 0; i < 9; i++) cudaEventCreate(&tev[i]);
-  }
-  return timing ? tev : nullptr;
-}
-
+// CUDASIFT_MATCH_TIMING=1: the events between the kernels, printed to stderr
 static void vp_timing_print(cudaEvent_t *tev, int numPairs, int numLoops, int model)
 {
   static const char *names[8] = {"flags", "compact", "norm", "hyp", "score", "argmax", "refit", "write"};
@@ -775,7 +763,7 @@ int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cons
   VerifyState *vs = reinterpret_cast<VerifyState *>(b + L.state);
   const int2 *p2 = reinterpret_cast<const int2 *>(pairs);
   const int blocks = idivup(numPairs, VP_ROWS), slots = 3 * numLoops;
-  cudaEvent_t *tev = full ? vp_timing_events() : nullptr;
+  cudaEvent_t *tev = full ? match_timing_events() : nullptr;
   if (tev) cudaEventRecord(tev[0], st);
   vp_flags_kernel<<<blocks, VP_ROWS, 0, st>>>(s1, n1, s2, n2, p2, numPairs, masks, counts);
   if (tev) cudaEventRecord(tev[1], st);

@@ -45,6 +45,9 @@ def _bad_calls(base):
         ("same set twice", (s1, 4, s1, 4, 0.0, 1.0, pairs, 4, 0)),
         ("set 2 starts inside set 1", (s1, 4, s1 + 3 * REC, 4, 0.0, 1.0, pairs, 4, 0)),
         ("set 1 starts inside set 2", (s2 + REC, 2, s2, 2, 0.0, 1.0, pairs, 4, 0)),
+        ("pairs unaligned", (s1, 4, s2, 4, 0.0, 1.0, pairs + 4, 4, 0)),
+        ("pairs inside set 1", (s1, 4, s2, 4, 0.0, 1.0, s1 + 8, 4, 0)),
+        ("pairs run into set 2", (s1, 4, s2, 4, 0.0, 1.0, s2 - 8, 4, 0)),
     ]
 
 
