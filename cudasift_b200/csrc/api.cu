@@ -110,156 +110,6 @@ static size_t temp_floats(int width, int height, int numOctaves, bool scaleUp)
   return size + sizeTmp;
 }
 
-// ------------------------------------------------------------------------------ pipeline
-// One Pipeline = everything ExtractSift needs for one (width, height, octaves, scaleUp,
-// arena) combination: level pointers inside the arena, texture objects, counters.
-struct Pipeline {
-  int w0 = 0, h0 = 0, numOctaves = 0;
-  bool scaleUp = false;
-  float *arena = nullptr;
-  bool ownArena = false;
-  int numLevels = 0;
-  float *lev[CS_MAX_LEVELS] = {};
-  int lw[CS_MAX_LEVELS] = {}, lh[CS_MAX_LEVELS] = {}, lp[CS_MAX_LEVELS] = {};
-  float *upImg = nullptr;
-  cudaTextureObject_t tex[CS_MAX_LEVELS] = {};
-  unsigned int *d_counters = nullptr;   // [0] primaries found, [1] total incl. secondaries
-  uint2 *d_tiles = nullptr;             // detector tile list (level, x0, y0), all levels
-  int numTiles = 0;
-  float lapTaps[8 * 12 * 16];
-  Taps5 sdTaps;
-  int describeBlocks = 0;
-
-  int init(int w, int h, int octaves, bool up, float *arenaPtr);
-  void destroy();
-  // ev (optional): 5 events recorded at stage boundaries (start, after LowPass, after the
-  // ScaleDown chain, after detect, after describe) for per-kernel timing.
-  int enqueue(const float *d_img, int pitch, double initBlur, float thresh, float lowestScale,
-              SiftPoint *d_pts, int maxPts, cudaStream_t st, cudaEvent_t *ev = nullptr);
-};
-
-int Pipeline::init(int w, int h, int octaves, bool up, float *arenaPtr)
-{
-  if (w < 1 || h < 1 || octaves < 1 || octaves > 7) {   // quirk Q17: taps table holds octave <= 7
-    set_error("ExtractSift: invalid size %dx%d or numOctaves %d (1..7)", w, h, octaves);
-    return CS_E_ARG;
-  }
-  w0 = w; h0 = h; numOctaves = octaves; scaleUp = up;
-  if (arenaPtr) { arena = arenaPtr; ownArena = false; }
-  else {
-    size_t fl = temp_floats(w, h, octaves, up);
-    CS_CUDA(cudaMalloc((void **)&arena, fl * sizeof(float)));
-    ownArena = true;
-  }
-  int W = w * (up ? 2 : 1), H = h * (up ? 2 : 1);
-  float *cur = arena;
-  numLevels = octaves;
-  lw[0] = W; lh[0] = H; lp[0] = ialignup(W, 128);
-  for (int i = 0; i < octaves; i++) {
-    if (i > 0) { lw[i] = lw[i - 1] / 2; lh[i] = lh[i - 1] / 2; lp[i] = ialignup(lw[i], 128); }
-    lev[i] = cur;
-    cur += (size_t)lh[i] * lp[i];
-    if (lw[i] < 1 || lh[i] < 1) { numLevels = i; break; }
-  }
-  if (up) { upImg = cur; cur += (size_t)lh[0] * lp[0]; }
-  for (int i = 0; i < numLevels; i++) {
-    int r = make_texture(&tex[i], lev[i], lw[i], lh[i], lp[i]);
-    if (r < 0) return r;
-  }
-  CS_CUDA(cudaMalloc((void **)&d_counters, 4 * sizeof(unsigned int)));
-  {
-    // coarsest level first: its tiles carry the most extrema candidates, so the persistent CTAs
-    // finish on the light tiles of the finest level
-    std::vector<uint2> tl;
-    int nl = 0, idx[CS_MAX_LEVELS];
-    for (int i = 0; i < numLevels; i++) idx[i] = (lw[i] < 3 || lh[i] < 3) ? -1 : nl++;   // no interior pixel -> no extrema
-    for (int i = numLevels - 1; i >= 0; i--) {
-      if (idx[i] < 0) continue;
-      const int tx = idivup(lw[i] - 2, CS_DETECT_TILE_W), ty = idivup(lh[i] - 2, CS_DETECT_TILE_H);
-      for (int y = 0; y < ty; y++)
-        for (int x = 0; x < tx; x++)
-          tl.push_back(make_uint2((unsigned)idx[i] | ((unsigned)(x * CS_DETECT_TILE_W) << 8), (unsigned)(y * CS_DETECT_TILE_H)));
-    }
-    numTiles = (int)tl.size();
-    if (numTiles > 0) {
-      CS_CUDA(cudaMalloc((void **)&d_tiles, tl.size() * sizeof(uint2)));
-      CS_CUDA(cudaMemcpy(d_tiles, tl.data(), tl.size() * sizeof(uint2), cudaMemcpyHostToDevice));
-    }
-  }
-  memset(lapTaps, 0, sizeof(lapTaps));
-  laplace_taps(octaves, 0.0f, lapTaps);           // cudaSiftH.cu:110
-  scaledown_taps(0.5f, sdTaps.k);                 // cudaSiftH.cu:157
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  describeBlocks = sms * 8;
-  return 0;
-}
-
-void Pipeline::destroy()
-{
-  for (int i = 0; i < CS_MAX_LEVELS; i++)
-    if (tex[i]) { cudaDestroyTextureObject(tex[i]); tex[i] = 0; }
-  if (d_counters) { cudaFree(d_counters); d_counters = nullptr; }
-  if (d_tiles) { cudaFree(d_tiles); d_tiles = nullptr; }
-  if (ownArena && arena) cudaFree(arena);
-  arena = nullptr;
-}
-
-int Pipeline::enqueue(const float *d_img, int pitch, double initBlur, float thresh, float lowestScale,
-                      SiftPoint *d_pts, int maxPts, cudaStream_t st, cudaEvent_t *ev)
-{
-  int r;
-  CS_CUDA(cudaMemsetAsync(d_counters, 0, 4 * sizeof(unsigned int), st));   // cudaSiftH.cu:77
-  if (ev) cudaEventRecord(ev[0], st);
-  Taps9 lp9;
-  float sigma = (float)(initBlur > (double)0.001f ? initBlur : (double)0.001f);   // cudaSiftH.cu:112
-  lowpass_taps(sigma, lp9.k);
-  if (!scaleUp) {
-    if ((r = launch_lowpass(d_img, pitch, lev[0], lp[0], lw[0], lh[0], lp9, st)) < 0) return r;
-  } else {                                                                 // cudaSiftH.cu:119-123
-    if ((r = launch_scaleup(d_img, upImg, w0, h0, pitch, lp[0], st)) < 0) return r;
-    if ((r = launch_lowpass(upImg, lp[0], lev[0], lp[0], lw[0], lh[0], lp9, st)) < 0) return r;
-    lowestScale *= 2.0f;                                                   // cudaSiftH.cu:127
-  }
-  if (ev) cudaEventRecord(ev[1], st);
-  for (int i = 1; i < numLevels; i++)                                      // cudaSiftH.cu:153-157
-    if ((r = launch_scaledown(lev[i - 1], lev[i], lw[i - 1], lh[i - 1], lp[i - 1], lp[i], sdTaps, st)) < 0) return r;
-  if (ev) cudaEventRecord(ev[2], st);
-
-  DetectParams dp;
-  memset(&dp, 0, sizeof(dp));
-  int tiles = 0, nl = 0;
-  for (int i = 0; i < numLevels; i++) {
-    if (lw[i] < 3 || lh[i] < 3) continue;          // no interior pixel -> no extrema possible
-    DetectLevel &L = dp.lev[nl++];
-    L.img = lev[i]; L.w = lw[i]; L.h = lh[i]; L.pitch = lp[i];
-    tiles += idivup(lw[i] - 2, CS_DETECT_TILE_W) * idivup(lh[i] - 2, CS_DETECT_TILE_H);   // see Pipeline::init (d_tiles)
-    L.subsampling = (float)(1 << i);
-    L.lowestScale = lowestScale / L.subsampling;                           // cudaSiftH.cu:213
-    const float *k = lapTaps + (numOctaves - i) * 12 * 16;                 // octave index, :161,:1766
-    for (int s = 0; s < CS_LAPLACE_S; s++)
-      for (int j = 0; j < 5; j++) L.taps.set(s, j, k[16 * s + j]);
-  }
-  dp.numLevels = nl; dp.totalTiles = tiles; dp.tiles = d_tiles;
-  if (tiles != numTiles) { set_error("detector tile list out of sync"); return CS_E_ARG; }
-  dp.thresh = thresh; dp.edgeLimit = 10.0f; dp.factor = 1.0f / CS_NUM_SCALES;   // cudaSiftH.cu:213
-  dp.pts = d_pts; dp.counters = d_counters; dp.maxPts = maxPts;
-  if ((r = launch_detect(dp, st)) < 0) return r;
-  if (ev) cudaEventRecord(ev[3], st);
-
-  DescribeParams ds;
-  memset(&ds, 0, sizeof(ds));
-  for (int i = 0; i < numLevels; i++) ds.tex[i] = tex[i];
-  ds.numLevels = numLevels; ds.pts = d_pts; ds.counters = d_counters; ds.maxPts = maxPts;
-  ds.finestSubsampling = 1.0f;
-  if ((r = launch_describe(ds, describeBlocks, st)) < 0) return r;
-  if (scaleUp)                                                             // cudaSiftH.cu:130
-    if ((r = launch_rescale(d_pts, d_counters, maxPts, 0.5f, st)) < 0) return r;
-  if (ev) cudaEventRecord(ev[4], st);
-  return 0;
-}
-
 static inline int count_from_counters(const unsigned int *c, int maxPts)
 {
   unsigned int a = c[0] < (unsigned)maxPts ? c[0] : (unsigned)maxPts;
@@ -284,21 +134,9 @@ Pipeline *DeviceCtx::get_pipe(int w, int h, int oct, bool up, float *arena, int 
   if (it != pipes.end()) return it->second;
   if (!arena && pipes.size() > 8) drop_pipes(nullptr, true);   // bound the internal-arena cache
   Pipeline *p = new Pipeline();
-  int r = p->init(w, h, oct, up, arena);
-  if (r < 0) { p->destroy(); delete p; *err = r; return nullptr; }
-  pipes[k] = p;
-  return p;
-}
-Pipeline2 *DeviceCtx::get_pipe2(int w, int h, int oct, bool up, float *arena, int *err)
-{
-  PipeKey k{w, h, oct, up ? 1 : 0, arena};
-  auto it = pipes2.find(k);
-  if (it != pipes2.end()) return it->second;
-  if (!arena && pipes2.size() > 8) drop_pipes(nullptr, true);
-  Pipeline2 *p = new Pipeline2();
   int r = p->init(w, h, oct, up, 1, arena);
   if (r < 0) { p->destroy(); delete p; *err = r; return nullptr; }
-  pipes2[k] = p;
+  pipes[k] = p;
   return p;
 }
 void DeviceCtx::drop_pipes(float *arena, bool internalOnly)
@@ -306,11 +144,6 @@ void DeviceCtx::drop_pipes(float *arena, bool internalOnly)
   for (auto it = pipes.begin(); it != pipes.end();) {
     bool hit = internalOnly ? it->second->ownArena : (it->first.arena == arena);
     if (hit) { it->second->destroy(); delete it->second; it = pipes.erase(it); }
-    else ++it;
-  }
-  for (auto it = pipes2.begin(); it != pipes2.end();) {
-    bool hit = internalOnly ? it->second->ownArena : (it->first.arena == arena);
-    if (hit) { it->second->destroy(); delete it->second; it = pipes2.erase(it); }
     else ++it;
   }
 }
@@ -343,23 +176,23 @@ static int extract_sync(const float *d_img, int w, int h, int pitch, int numOcta
 {
   int err = 0;
   if (!d_img || !d_pts || maxPts < 1) { set_error("ExtractSift: missing image or SiftData"); return CS_E_ARG; }
+  if ((reinterpret_cast<uintptr_t>(d_tmp) & 15) != 0) {   // the level textures and tensor maps start in it
+    set_error("ExtractSift: tempMemory %p must be 16-byte aligned", (void *)d_tmp);
+    return CS_E_ARG;
+  }
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  const bool useLegacy = legacy_mode() || !tensor_map_compatible(d_img, pitch) ||
-                         (d_tmp && (reinterpret_cast<uintptr_t>(d_tmp) & 15) != 0);
-  Pipeline *p = nullptr;
-  Pipeline2 *p2 = nullptr;
-  if (useLegacy) p = c->get_pipe(w, h, numOctaves, scaleUp, d_tmp, &err);
-  else p2 = c->get_pipe2(w, h, numOctaves, scaleUp, d_tmp, &err);
-  if (!p && !p2) return err;
+  Pipeline *p = c->get_pipe(w, h, numOctaves, scaleUp, d_tmp, &err);
+  if (!p) return err;
+  // the round-1 kernels: asked for, or an image (or arena) TMA cannot address
+  const bool round1 = legacy_mode() || !p->tma || !tensor_map_compatible(d_img, pitch);
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (msKernel) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, c->stream); }
-  int r = p ? p->enqueue(d_img, pitch, initBlur, thresh, lowestScale, d_pts, maxPts, c->stream)
-            : p2->enqueue(1, &d_img, pitch, initBlur, thresh, lowestScale, d_pts, 0, maxPts, c->stream);
+  int r = round1 ? p->enqueue_round1(d_img, pitch, initBlur, thresh, lowestScale, d_pts, maxPts, c->stream)
+                 : p->enqueue(1, &d_img, pitch, initBlur, thresh, lowestScale, d_pts, 0, maxPts, c->stream);
   if (r < 0) { if (msKernel) { cudaEventDestroy(e0); cudaEventDestroy(e1); } return r; }
   if (msKernel) cudaEventRecord(e1, c->stream);
-  const unsigned int *d_cnt = p ? p->d_counters : p2->counters(0);
-  CS_CUDA(cudaMemcpyAsync(c->h_counters, d_cnt, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+  CS_CUDA(cudaMemcpyAsync(c->h_counters, p->counters(0), 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
   CS_CUDA(cudaStreamSynchronize(c->stream));
   int numPts = count_from_counters(c->h_counters, maxPts);                 // cudaSiftH.cu:115-116
   if (msKernel) {
@@ -1328,38 +1161,35 @@ int cs_describe_points(const float *d_img, int w, int h, int pitch, void *d_pts,
 
 // ---- pipelined extractor ----
 struct cs_extractor {
-  int w, h, numOctaves, maxPts, scaleUp, pitch, B;
-  cudaStream_t stream;
-  bool legacy;
-  Pipeline pipe;         // legacy per-image kernels (B == 1)
-  Pipeline2 pipe2;       // batched TMA pipeline
-  float *d_img;          // B staging images
-  SiftPoint *d_pts;      // B x maxPts records (ranked: the output slots)
-  int maxCand;           // ranked extractors: candidate records per image (0: plain extractor)
-  SiftPoint *d_cand;     // ranked: B x maxCand records, written by the pipeline as d_pts is for a plain extractor
-  unsigned int *d_rank;  // ranked: B x rank_scratch_words(maxCand)
-  float *h_img;          // pinned, B x w x h
-  uint8_t *d_u8;         // device staging for 8-bit uploads (lazily allocated)
-  SiftPoint *h_pts;      // pinned, B x maxPts
-  unsigned int *h_counters;   // pinned, B x CS_CNT_STRIDE
-  bool hostResults;
-  int lastN;
-  int lastCounts[CS_MAX_BATCH];
-  int lastCand[CS_MAX_BATCH];   // records found per image (ranked: in the candidate area)
-  // CUDA graph of one steady-state submit (memset + kernels + count D2H).  Per image only the input pointer
-  // changes: legacy = first parameter of the LowPass node, batched = the tensor maps in the parameters of the
-  // first pyramid kernel; both are patched with cudaGraphExecKernelNodeSetParams.
-  cudaGraphExec_t gexec;
-  cudaGraph_t graph;
-  cudaGraphNode_t gnode;
-  cudaKernelNodeParams gparams;
-  void *gargs[16];
-  const float *gsrc;
-  PyrAParams gpa;
-  int gn, gpitch, glaunches;
-  double gblur;
-  float gthresh, glowest;
-  int submits;
+  int w = 0, h = 0, numOctaves = 0, maxPts = 0, scaleUp = 0, pitch = 0, B = 0;
+  cudaStream_t stream = nullptr;
+  bool legacy = false;             // the round-1 per-image kernels (B == 1)
+  Pipeline pipe;
+  float *d_img = nullptr;          // B staging images
+  SiftPoint *d_pts = nullptr;      // B x maxPts records (ranked: the output slots)
+  int maxCand = 0;                 // ranked extractors: candidate records per image (0: plain extractor)
+  SiftPoint *d_cand = nullptr;     // ranked: B x maxCand records, written by the pipeline as d_pts is for a plain extractor
+  unsigned int *d_rank = nullptr;  // ranked: B x rank_scratch_words(maxCand)
+  float *h_img = nullptr;          // pinned, B x w x h
+  uint8_t *d_u8 = nullptr;         // device staging for 8-bit uploads (lazily allocated)
+  SiftPoint *h_pts = nullptr;      // pinned, B x maxPts
+  unsigned int *h_counters = nullptr;   // pinned, B x CS_CNT_STRIDE
+  bool hostResults = false;
+  int lastN = 0;
+  int lastCounts[CS_MAX_BATCH] = {};
+  int lastCand[CS_MAX_BATCH] = {};      // records found per image (ranked: in the candidate area)
+  // CUDA graph of one steady-state submit of the batched kernels (memset + kernels + count D2H).  Per submit only the
+  // input images change: the tensor maps in the parameters of the first pyramid kernel, patched with
+  // cudaGraphExecKernelNodeSetParams.
+  cudaGraphExec_t gexec = nullptr;
+  cudaGraph_t graph = nullptr;
+  cudaGraphNode_t gnode = nullptr;
+  cudaKernelNodeParams gparams = {};
+  PyrAParams gpa = {};
+  int gn = 0, gpitch = 0, glaunches = 0;
+  double gblur = 0.0;
+  float gthresh = 0.0f, glowest = 0.0f;
+  int submits = 0;
 };
 
 
@@ -1375,32 +1205,28 @@ static int extractor_enqueue(cs_extractor *ex, int n, const float *const *d_imgs
 {
   int r;
   if (ex->legacy) {
-    r = ex->pipe.enqueue(d_imgs[0], pitch, initBlur, thresh, lowestScale, ex->d_pts, ex->maxPts, ex->stream, ev);
-    if (r < 0) return r;
-    CS_CUDA(cudaMemcpyAsync(ex->h_counters, ex->pipe.d_counters, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, ex->stream));
+    r = ex->pipe.enqueue_round1(d_imgs[0], pitch, initBlur, thresh, lowestScale, ex->d_pts, ex->maxPts, ex->stream, ev);
+  } else if (ex->maxCand > 0) {
+    RankParams rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.out = ex->d_pts; rp.outStride = ex->maxPts; rp.maxOut = ex->maxPts; rp.scratch = ex->d_rank;
+    r = ex->pipe.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_cand, ex->maxCand, ex->maxCand, ex->stream,
+                         ev, paOut, &rp);
   } else {
-    if (ex->maxCand > 0) {
-      RankParams rp;
-      memset(&rp, 0, sizeof(rp));
-      rp.out = ex->d_pts; rp.outStride = ex->maxPts; rp.maxOut = ex->maxPts; rp.scratch = ex->d_rank;
-      r = ex->pipe2.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_cand, ex->maxCand, ex->maxCand, ex->stream,
-                            ev, paOut, &rp);
-    } else {
-      r = ex->pipe2.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_pts, ex->maxPts, ex->maxPts, ex->stream, ev, paOut);
-    }
-    if (r < 0) return r;
-    CS_CUDA(cudaMemcpyAsync(ex->h_counters, ex->pipe2.d_state, (size_t)n * CS_CNT_STRIDE * sizeof(unsigned int),
-                            cudaMemcpyDeviceToHost, ex->stream));
+    r = ex->pipe.enqueue(n, d_imgs, pitch, initBlur, thresh, lowestScale, ex->d_pts, ex->maxPts, ex->maxPts, ex->stream, ev, paOut);
   }
+  if (r < 0) return r;
+  CS_CUDA(cudaMemcpyAsync(ex->h_counters, ex->pipe.counters(0), (size_t)n * CS_CNT_STRIDE * sizeof(unsigned int),
+                          cudaMemcpyDeviceToHost, ex->stream));
   return 0;
 }
 
-// Capture one submit into a graph.  Leaves ex->gexec == NULL if anything is unsupported; the caller then
-// launches directly.
+// Capture one submit of the batched kernels into a graph.  Leaves ex->gexec == NULL if anything is unsupported (the
+// up-scaled and the round-1 pipelines are not captured); the caller then launches directly.
 static int extractor_capture(cs_extractor *ex, int n, const float *const *d_imgs, int pitch, double initBlur, float thresh,
                              float lowestScale)
 {
-  if (ex->scaleUp) return 0;
+  if (ex->scaleUp || ex->legacy) return 0;
   if (getenv("CUDASIFT_NO_GRAPH")) return 0;
   cudaGraph_t g = nullptr;
   if (cudaStreamBeginCapture(ex->stream, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -1420,13 +1246,7 @@ static int extractor_capture(cs_extractor *ex, int n, const float *const *d_imgs
     if (cudaGraphNodeGetType(nodes[i], &t) != cudaSuccess || t != cudaGraphNodeTypeKernel) continue;
     cudaKernelNodeParams kp;
     if (cudaGraphKernelNodeGetParams(nodes[i], &kp) != cudaSuccess || !kp.kernelParams) continue;
-    if (ex->legacy) {   // the kernel node that reads d_img (first kernel parameter == d_img): lowpass_kernel, 7 parameters
-      if (*reinterpret_cast<const float *const *>(kp.kernelParams[0]) == d_imgs[0] && kp.blockDim.x == 256) {
-        ex->gnode = nodes[i]; ex->gparams = kp;
-        for (int a = 0; a < 7; a++) ex->gargs[a] = kp.kernelParams[a];
-        found = true;
-      }
-    } else if (kp.func == cs::pyr_a_func()) {
+    if (kp.func == cs::pyr_a_func()) {
       ex->gnode = nodes[i]; ex->gparams = kp;
       found = true;
     }
@@ -1434,7 +1254,7 @@ static int extractor_capture(cs_extractor *ex, int n, const float *const *d_imgs
   cudaGraphExec_t ge = nullptr;
   if (!found || cudaGraphInstantiate(&ge, g, 0) != cudaSuccess) { cudaGetLastError(); cudaGraphDestroy(g); return 0; }
   ex->graph = g; ex->gexec = ge;
-  ex->gsrc = d_imgs[0]; ex->gn = n; ex->gpitch = pitch; ex->gblur = initBlur; ex->gthresh = thresh; ex->glowest = lowestScale;
+  ex->gn = n; ex->gpitch = pitch; ex->gblur = initBlur; ex->gthresh = thresh; ex->glowest = lowestScale;
   return 0;
 }
 
@@ -1442,16 +1262,12 @@ static cs_extractor *extractor_create(int w, int h, int numOctaves, int maxPts, 
 {
   if (batch < 1 || batch > CS_MAX_BATCH) { set_error("cs_extractor_create_batch: batch %d out of range (1..%d)", batch, CS_MAX_BATCH); return nullptr; }
   cs_extractor *ex = new cs_extractor();
-  memset((void *)ex, 0, sizeof(*ex));
-  new (&ex->pipe) Pipeline();
-  new (&ex->pipe2) Pipeline2();
   ex->w = w; ex->h = h; ex->numOctaves = numOctaves; ex->maxPts = maxPts; ex->scaleUp = scaleUp; ex->B = batch;
   ex->pitch = ialignup(w, 128);
   ex->legacy = legacy_mode();
   if (ex->legacy && batch != 1) { set_error("the legacy pipeline takes one image at a time"); delete ex; return nullptr; }
   bool ok = cudaStreamCreateWithFlags(&ex->stream, cudaStreamNonBlocking) == cudaSuccess;
-  if (ex->legacy) ok = ok && ex->pipe.init(w, h, numOctaves, scaleUp != 0, nullptr) == 0;
-  else ok = ok && ex->pipe2.init(w, h, numOctaves, scaleUp != 0, batch, nullptr) == 0;
+  ok = ok && ex->pipe.init(w, h, numOctaves, scaleUp != 0, batch, nullptr) == 0;
   ok = ok && cudaMalloc((void **)&ex->d_img, (size_t)batch * ex->pitch * h * sizeof(float)) == cudaSuccess;
   ok = ok && cudaMalloc((void **)&ex->d_pts, (size_t)batch * maxPts * sizeof(SiftPoint)) == cudaSuccess;
   // the pipeline leaves some fields of a record unwritten (score, match*, empty[1..2]): make them zero, not stale memory
@@ -1504,7 +1320,6 @@ int cs_extractor_destroy(cs_extractor *ex)
   if (ex->stream) cudaStreamSynchronize(ex->stream);
   extractor_drop_graph(ex);
   ex->pipe.destroy();
-  ex->pipe2.destroy();
   if (ex->d_img) cudaFree(ex->d_img);
   if (ex->d_u8) cudaFree(ex->d_u8);
   if (ex->d_pts) cudaFree(ex->d_pts);
@@ -1538,25 +1353,12 @@ int cs_extractor_submit_device_batch(cs_extractor *ex, int n, const float *const
   }
   if (!ex->gexec && ex->submits == 2) extractor_capture(ex, n, d_imgs, pitch, initBlur, thresh, lowestScale);
   if (ex->gexec) {
-    if (ex->legacy) {
-      if (d_imgs[0] != ex->gsrc) {
-        const float *src = d_imgs[0];
-        cudaKernelNodeParams kp = ex->gparams;
-        void *args[7];
-        for (int a = 0; a < 7; a++) args[a] = ex->gargs[a];
-        args[0] = (void *)&src;
-        kp.kernelParams = args;
-        CS_CUDA(cudaGraphExecKernelNodeSetParams(ex->gexec, ex->gnode, &kp));
-        ex->gsrc = d_imgs[0];
-      }
-    } else {
-      int r = ex->pipe2.fill_pyr_a(ex->gpa, n, d_imgs, pitch, initBlur);
-      if (r < 0) return r;
-      cudaKernelNodeParams kp = ex->gparams;
-      void *args[1] = {(void *)&ex->gpa};
-      kp.kernelParams = args;
-      CS_CUDA(cudaGraphExecKernelNodeSetParams(ex->gexec, ex->gnode, &kp));
-    }
+    int r = ex->pipe.fill_pyr_a(ex->gpa, n, d_imgs, pitch, initBlur);
+    if (r < 0) return r;
+    cudaKernelNodeParams kp = ex->gparams;
+    void *args[1] = {(void *)&ex->gpa};
+    kp.kernelParams = args;
+    CS_CUDA(cudaGraphExecKernelNodeSetParams(ex->gexec, ex->gnode, &kp));
     CS_CUDA(cudaGraphLaunch(ex->gexec, ex->stream));
     count_launch(ex->glaunches);
     return 0;
@@ -1664,14 +1466,9 @@ int cs_extractor_profile(cs_extractor *ex, const float *d_img, int pitch, double
 int cs_extractor_read_level(cs_extractor *ex, int slot, int level, float *h_out)
 {
   CS_CUDA(cudaStreamSynchronize(ex->stream));
-  const float *src; int lw, lh, lp;
-  if (ex->legacy) {
-    if (slot != 0 || level < 0 || level >= ex->pipe.numLevels) { set_error("cs_extractor_read_level: bad level"); return CS_E_ARG; }
-    src = ex->pipe.lev[level]; lw = ex->pipe.lw[level]; lh = ex->pipe.lh[level]; lp = ex->pipe.lp[level];
-  } else {
-    if (slot < 0 || slot >= ex->B || level < 0 || level >= ex->pipe2.numLevels) { set_error("cs_extractor_read_level: bad level"); return CS_E_ARG; }
-    src = ex->pipe2.level(slot, level); lw = ex->pipe2.lw[level]; lh = ex->pipe2.lh[level]; lp = ex->pipe2.lp[level];
-  }
+  if (slot < 0 || slot >= ex->B || level < 0 || level >= ex->pipe.numLevels) { set_error("cs_extractor_read_level: bad level"); return CS_E_ARG; }
+  const float *src = ex->pipe.level(slot, level);
+  const int lw = ex->pipe.lw[level], lh = ex->pipe.lh[level], lp = ex->pipe.lp[level];
   if (h_out)
     CS_CUDA(cudaMemcpy2D(h_out, (size_t)lw * sizeof(float), src, (size_t)lp * sizeof(float), (size_t)lw * sizeof(float), lh,
                          cudaMemcpyDeviceToHost));

@@ -209,8 +209,7 @@ struct GrowBuffer {
   template <class T> T *as() const { return static_cast<T *>(p); }
 };
 
-struct Pipeline;    // round-1 per-image extraction (api.cu)
-struct Pipeline2;   // batched extraction (pipeline2.h)
+struct Pipeline;    // extraction, batched and round-1 kernels (pipeline2.h)
 struct PipeKey {
   int w, h, oct, up; float *arena;
   bool operator<(const PipeKey &o) const
@@ -230,8 +229,7 @@ struct DeviceCtx {
   int dev = -1;
   int sms = 0;                             // multiprocessor count
   cudaStream_t stream = nullptr;           // blocking stream: ordered after legacy default-stream work
-  std::map<PipeKey, Pipeline *> pipes;     // legacy per-image pipelines
-  std::map<PipeKey, Pipeline2 *> pipes2;   // batched pipeline, batch of one (the drop-in ExtractSift)
+  std::map<PipeKey, Pipeline *> pipes;     // batch-of-one pipelines of the drop-in ExtractSift
 
   // Device buffers grown on demand, and the entry points that use them.  A call may use several at once
   // (cs_match_ratio: knnLists, pairScratch, the tc* tables and knnPartials), so each has its own member.
@@ -264,7 +262,6 @@ struct DeviceCtx {
 
   int ensure(int d);
   Pipeline *get_pipe(int w, int h, int oct, bool up, float *arena, int *err);
-  Pipeline2 *get_pipe2(int w, int h, int oct, bool up, float *arena, int *err);
   void drop_pipes(float *arena, bool internalOnly);
 };
 

@@ -522,7 +522,7 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
 }
 
 
-// once per device, outside any stream capture (Pipeline2::init)
+// once per device, outside any stream capture (Pipeline::init)
 static int g_d2_table[64];
 int detect2_init_device()
 {

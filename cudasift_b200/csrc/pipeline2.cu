@@ -1,8 +1,10 @@
-// pipeline2.cu -- host side of the batched extraction pipeline: one stream-ordered sequence of
+// pipeline2.cu -- host side of the extraction pipeline: one stream-ordered sequence of
 //   [ScaleUp] -> pyr_lowpass_sd (TMA) -> pyr_chain -> detect2 (TMA, all octaves, all images) -> cap32 fix-up
 //   -> describe (all octaves, all images) [-> rescale] [-> rank (ranked extractors)]
 // for 1..CS_MAX_BATCH images of one size.  Replaces the reference's per-image loop (mainSift.cpp:65-69 around
-// cudaSiftH.cu:72-144); the drop-in ExtractSift is the batch-of-one case.
+// cudaSiftH.cu:72-144); the drop-in ExtractSift is the batch-of-one case.  Over the same levels a batch of one also
+// runs the round-1 per-image kernels (LowPass, ScaleDown chain, detect, describe): CUDASIFT_LEGACY, and images TMA
+// cannot address.
 #include "common.cuh"
 #include "pipeline2.h"
 
@@ -92,8 +94,8 @@ static int debug_stage(cudaStream_t st, const char *name)
   return 0;
 }
 
-// ------------------------------------------------------------------------------ Pipeline2
-int Pipeline2::init(int w, int h, int octaves, bool up, int maxBatch, float *arenaPtr)
+// ------------------------------------------------------------------------------ Pipeline
+int Pipeline::init(int w, int h, int octaves, bool up, int maxBatch, float *arenaPtr)
 {
   if (w < 1 || h < 1 || octaves < 1 || octaves > 7) {   // quirk Q17: taps table holds octave <= 7
     set_error("ExtractSift: invalid size %dx%d or numOctaves %d (1..7)", w, h, octaves);
@@ -103,7 +105,6 @@ int Pipeline2::init(int w, int h, int octaves, bool up, int maxBatch, float *are
     set_error("batch size %d out of range (1..%d)", maxBatch, CS_MAX_BATCH);
     return CS_E_ARG;
   }
-  if (!encode_fn()) { set_error("cuTensorMapEncodeTiled is not available from this driver"); return CS_E_CUDA; }
   { int r0 = detect2_init_device(); if (r0 < 0) return r0; }
   w0 = w; h0 = h; numOctaves = octaves; scaleUp = up; B = maxBatch;
   const int W = w * (up ? 2 : 1), H = h * (up ? 2 : 1);
@@ -123,28 +124,27 @@ int Pipeline2::init(int w, int h, int octaves, bool up, int maxBatch, float *are
     CS_CUDA(cudaMalloc((void **)&arena, perImage * B * sizeof(float)));
     ownArena = true;
   }
-  if ((reinterpret_cast<uintptr_t>(arena) & 15) != 0) { set_error("temp memory must be 16-byte aligned"); return CS_E_ARG; }
+  // the batched kernels read the levels through tensor maps; on an arena TMA cannot address only enqueue_round1 runs
+  tma = encode_fn() != nullptr && (reinterpret_cast<uintptr_t>(arena) & 15) == 0;
 
-  // textures + tensor maps of every level of every image slot
-  std::vector<cudaTextureObject_t> texs((size_t)B * CS_MAX_LEVELS, 0);
+  // textures (+ tensor maps) of every level of every image slot
   std::vector<CUtensorMap> maps((size_t)B * CS_MAX_LEVELS);
   memset(maps.data(), 0, maps.size() * sizeof(CUtensorMap));
   h_tex.assign((size_t)B * CS_MAX_LEVELS, 0);
   upMaps.resize(B);
   for (int b = 0; b < B; b++) {
     for (int i = 0; i < numLevels; i++) {
-      int r = make_texture(&texs[(size_t)b * CS_MAX_LEVELS + i], level(b, i), lw[i], lh[i], lp[i]);
+      int r = make_texture(&h_tex[(size_t)b * CS_MAX_LEVELS + i], level(b, i), lw[i], lh[i], lp[i]);
       if (r < 0) return r;
-      h_tex[(size_t)b * CS_MAX_LEVELS + i] = texs[(size_t)b * CS_MAX_LEVELS + i];
-      if ((r = make_tensor_map_2d(&maps[(size_t)b * CS_MAX_LEVELS + i], level(b, i), lw[i], lh[i], lp[i], 256, 1)) < 0) return r;
+      if (tma && (r = make_tensor_map_2d(&maps[(size_t)b * CS_MAX_LEVELS + i], level(b, i), lw[i], lh[i], lp[i], 256, 1)) < 0) return r;
     }
-    if (up) {
+    if (tma && up) {
       int r = make_tensor_map_2d(&upMaps[b], arena + (size_t)b * perImage + upOff, lw[0], lh[0], lp[0], CS_PA_BOX, 1);
       if (r < 0) return r;
     }
   }
-  CS_CUDA(cudaMalloc((void **)&d_tex, texs.size() * sizeof(cudaTextureObject_t)));
-  CS_CUDA(cudaMemcpy(d_tex, texs.data(), texs.size() * sizeof(cudaTextureObject_t), cudaMemcpyHostToDevice));
+  CS_CUDA(cudaMalloc((void **)&d_tex, h_tex.size() * sizeof(cudaTextureObject_t)));
+  CS_CUDA(cudaMemcpy(d_tex, h_tex.data(), h_tex.size() * sizeof(cudaTextureObject_t), cudaMemcpyHostToDevice));
   CS_CUDA(cudaMalloc((void **)&d_maps, maps.size() * sizeof(CUtensorMap)));
   CS_CUDA(cudaMemcpy(d_maps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
 
@@ -158,6 +158,25 @@ int Pipeline2::init(int w, int h, int octaves, bool up, int maxBatch, float *are
   stateWords = (size_t)B * CS_CNT_STRIDE + 4 + (size_t)B * cellWords;
   CS_CUDA(cudaMalloc((void **)&d_state, stateWords * sizeof(unsigned int)));
 
+  if (B == 1) {
+    // the round-1 detector's tiles, coarsest level first: its tiles carry the most extrema candidates, so the
+    // persistent CTAs finish on the light tiles of the finest level
+    std::vector<uint2> tl;
+    int nl = 0, idx[CS_MAX_LEVELS];
+    for (int i = 0; i < numLevels; i++) idx[i] = (lw[i] < 3 || lh[i] < 3) ? -1 : nl++;   // no interior pixel -> no extrema
+    for (int i = numLevels - 1; i >= 0; i--) {
+      if (idx[i] < 0) continue;
+      const int tx = idivup(lw[i] - 2, CS_DETECT_TILE_W), ty = idivup(lh[i] - 2, CS_DETECT_TILE_H);
+      for (int y = 0; y < ty; y++)
+        for (int x = 0; x < tx; x++)
+          tl.push_back(make_uint2((unsigned)idx[i] | ((unsigned)(x * CS_DETECT_TILE_W) << 8), (unsigned)(y * CS_DETECT_TILE_H)));
+    }
+    numTiles = (int)tl.size();
+    if (numTiles > 0) {
+      CS_CUDA(cudaMalloc((void **)&d_tiles, tl.size() * sizeof(uint2)));
+      CS_CUDA(cudaMemcpy(d_tiles, tl.data(), tl.size() * sizeof(uint2), cudaMemcpyHostToDevice));
+    }
+  }
   memset(lapTaps, 0, sizeof(lapTaps));
   laplace_taps(octaves, 0.0f, lapTaps);           // cudaSiftH.cu:110
   scaledown_taps(0.5f, sdTaps.k);                 // cudaSiftH.cu:157
@@ -168,7 +187,7 @@ int Pipeline2::init(int w, int h, int octaves, bool up, int maxBatch, float *are
   return 0;
 }
 
-void Pipeline2::destroy()
+void Pipeline::destroy()
 {
   for (size_t i = 0; i < h_tex.size(); i++)
     if (h_tex[i]) cudaDestroyTextureObject(h_tex[i]);
@@ -176,6 +195,7 @@ void Pipeline2::destroy()
   if (d_tex) { cudaFree(d_tex); d_tex = nullptr; }
   if (d_maps) { cudaFree(d_maps); d_maps = nullptr; }
   if (d_state) { cudaFree(d_state); d_state = nullptr; }
+  if (d_tiles) { cudaFree(d_tiles); d_tiles = nullptr; }
   for (auto &it : items) if (it.second.d) cudaFree(it.second.d);
   items.clear();
   if (ownArena && arena) cudaFree(arena);
@@ -204,7 +224,7 @@ void build_detector_items(const int *lw, const int *lh, int numLevels, int n, in
   }
 }
 
-int Pipeline2::get_items(int n, int hs, const uint4 **d_items, int *count)
+int Pipeline::get_items(int n, int hs, const uint4 **d_items, int *count)
 {
   const int key = n * 1024 + hs;
   auto it = items.find(key);
@@ -225,7 +245,7 @@ int Pipeline2::get_items(int n, int hs, const uint4 **d_items, int *count)
   return 0;
 }
 
-int Pipeline2::fill_pyr_a(PyrAParams &pa, int n, const float *const *d_imgs, int pitch, double initBlur)
+int Pipeline::fill_pyr_a(PyrAParams &pa, int n, const float *const *d_imgs, int pitch, double initBlur)
 {
   memset(&pa, 0, sizeof(pa));
   for (int b = 0; b < n; b++) {
@@ -252,12 +272,16 @@ int Pipeline2::fill_pyr_a(PyrAParams &pa, int n, const float *const *d_imgs, int
   return 0;
 }
 
-int Pipeline2::enqueue(int n, const float *const *d_imgs, int pitch, double initBlur, float thresh, float lowestScale,
+int Pipeline::enqueue(int n, const float *const *d_imgs, int pitch, double initBlur, float thresh, float lowestScale,
                        SiftPoint *d_pts, long long ptsStride, int maxPts, cudaStream_t st, cudaEvent_t *ev,
                        PyrAParams *paOut, const RankParams *rank)
 {
   int r;
   if (n < 1 || n > B) { set_error("batch of %d images on a pipeline built for %d", n, B); return CS_E_ARG; }
+  if (!tma) {
+    set_error("the batched pipeline needs cuTensorMapEncodeTiled and a 16-byte aligned arena (arena %p)", (void *)arena);
+    return CS_E_ARG;
+  }
   CS_CUDA(cudaMemsetAsync(d_state, 0, stateWords * sizeof(unsigned int), st));   // cudaSiftH.cu:77
   if (ev) cudaEventRecord(ev[0], st);
   unsigned int *d_counters = d_state, *d_sched = d_state + (size_t)B * CS_CNT_STRIDE;
@@ -348,6 +372,63 @@ int Pipeline2::enqueue(int n, const float *const *d_imgs, int pitch, double init
     if ((r = debug_stage(st, "rank")) < 0) return r;
     if (ev) cudaEventRecord(ev[5], st);
   }
+  return 0;
+}
+
+int Pipeline::enqueue_round1(const float *d_img, int pitch, double initBlur, float thresh, float lowestScale,
+                             SiftPoint *d_pts, int maxPts, cudaStream_t st, cudaEvent_t *ev)
+{
+  int r;
+  if (B != 1) { set_error("the round-1 kernels take one image at a time (pipeline built for %d)", B); return CS_E_ARG; }
+  unsigned int *d_counters = counters(0);
+  CS_CUDA(cudaMemsetAsync(d_counters, 0, CS_CNT_STRIDE * sizeof(unsigned int), st));   // cudaSiftH.cu:77
+  if (ev) cudaEventRecord(ev[0], st);
+  Taps9 lp9;
+  float sigma = (float)(initBlur > (double)0.001f ? initBlur : (double)0.001f);   // cudaSiftH.cu:112
+  lowpass_taps(sigma, lp9.k);
+  if (!scaleUp) {
+    if ((r = launch_lowpass(d_img, pitch, level(0, 0), lp[0], lw[0], lh[0], lp9, st)) < 0) return r;
+  } else {                                                                 // cudaSiftH.cu:119-123
+    float *upImg = arena + upOff;
+    if ((r = launch_scaleup(d_img, upImg, w0, h0, pitch, lp[0], st)) < 0) return r;
+    if ((r = launch_lowpass(upImg, lp[0], level(0, 0), lp[0], lw[0], lh[0], lp9, st)) < 0) return r;
+    lowestScale *= 2.0f;                                                   // cudaSiftH.cu:127
+  }
+  if (ev) cudaEventRecord(ev[1], st);
+  for (int i = 1; i < numLevels; i++)                                      // cudaSiftH.cu:153-157
+    if ((r = launch_scaledown(level(0, i - 1), level(0, i), lw[i - 1], lh[i - 1], lp[i - 1], lp[i], sdTaps, st)) < 0) return r;
+  if (ev) cudaEventRecord(ev[2], st);
+
+  DetectParams dp;
+  memset(&dp, 0, sizeof(dp));
+  int tiles = 0, nl = 0;
+  for (int i = 0; i < numLevels; i++) {
+    if (lw[i] < 3 || lh[i] < 3) continue;          // no interior pixel -> no extrema possible
+    DetectLevel &L = dp.lev[nl++];
+    L.img = level(0, i); L.w = lw[i]; L.h = lh[i]; L.pitch = lp[i];
+    tiles += idivup(lw[i] - 2, CS_DETECT_TILE_W) * idivup(lh[i] - 2, CS_DETECT_TILE_H);   // see init (d_tiles)
+    L.subsampling = (float)(1 << i);
+    L.lowestScale = lowestScale / L.subsampling;                           // cudaSiftH.cu:213
+    const float *k = lapTaps + (numOctaves - i) * 12 * 16;                 // octave index, :161,:1766
+    for (int s = 0; s < CS_LAPLACE_S; s++)
+      for (int j = 0; j < 5; j++) L.taps.set(s, j, k[16 * s + j]);
+  }
+  dp.numLevels = nl; dp.totalTiles = tiles; dp.tiles = d_tiles;
+  if (tiles != numTiles) { set_error("detector tile list out of sync"); return CS_E_ARG; }
+  dp.thresh = thresh; dp.edgeLimit = 10.0f; dp.factor = 1.0f / CS_NUM_SCALES;   // cudaSiftH.cu:213
+  dp.pts = d_pts; dp.counters = d_counters; dp.maxPts = maxPts;
+  if ((r = launch_detect(dp, st)) < 0) return r;
+  if (ev) cudaEventRecord(ev[3], st);
+
+  DescribeParams ds;
+  memset(&ds, 0, sizeof(ds));
+  for (int i = 0; i < numLevels; i++) ds.tex[i] = h_tex[i];
+  ds.numLevels = numLevels; ds.pts = d_pts; ds.counters = d_counters; ds.maxPts = maxPts;
+  ds.finestSubsampling = 1.0f;
+  if ((r = launch_describe(ds, sms * 8, st)) < 0) return r;
+  if (scaleUp)                                                             // cudaSiftH.cu:130
+    if ((r = launch_rescale(d_pts, d_counters, maxPts, 0.5f, st)) < 0) return r;
+  if (ev) cudaEventRecord(ev[4], st);
   return 0;
 }
 

@@ -1,4 +1,6 @@
-// pipeline2.h -- host-side state of the batched extraction pipeline (pipeline2.cu).
+// pipeline2.h -- host-side state of the extraction pipeline (pipeline2.cu).  One Pipeline per (size, octaves, scaleUp,
+// arena) serves both kernel sets over one level layout: the batched TMA kernels (enqueue) and, for a batch of one,
+// the round-1 per-image kernels (enqueue_round1).
 #pragma once
 
 #include "common.cuh"
@@ -8,9 +10,10 @@
 
 namespace cs {
 
-struct Pipeline2 {
+struct Pipeline {
   int w0 = 0, h0 = 0, numOctaves = 0, numLevels = 0, B = 0, sms = 132;
   bool scaleUp = false;
+  bool tma = false;                    // tensor maps made (driver encoder present, arena 16-byte aligned): enqueue works
   float *arena = nullptr;              // B consecutive per-image blocks: levels 0..n-1 [+ the up-scaled input]
   bool ownArena = false;
   size_t perImage = 0, levOff[CS_MAX_LEVELS] = {}, upOff = 0;   // in floats
@@ -22,6 +25,8 @@ struct Pipeline2 {
   unsigned int *d_state = nullptr;           // counters | scheduler | cap cells (one memset)
   size_t stateWords = 0;
   int cellWords = 0, cellBase[CS_MAX_LEVELS] = {}, cellsX[CS_MAX_LEVELS] = {};
+  uint2 *d_tiles = nullptr;                  // B == 1: the round-1 detector's tiles (level | x0 << 8, y0)
+  int numTiles = 0;
   float lapTaps[8 * 12 * 16];
   Taps5 sdTaps;
   struct ItemList { uint4 *d; int n; };
@@ -43,6 +48,10 @@ struct Pipeline2 {
   int enqueue(int n, const float *const *d_imgs, int pitch, double initBlur, float thresh, float lowestScale,
               SiftPoint *d_pts, long long ptsStride, int maxPts, cudaStream_t st, cudaEvent_t *ev = nullptr,
               PyrAParams *paOut = nullptr, const RankParams *rank = nullptr);
+  // The same extraction of one image (B == 1) by the round-1 kernels, which need no TMA: any pitch, any image address.
+  // ev (optional): the same 5 events.
+  int enqueue_round1(const float *d_img, int pitch, double initBlur, float thresh, float lowestScale, SiftPoint *d_pts,
+                     int maxPts, cudaStream_t st, cudaEvent_t *ev = nullptr);
 };
 
 void build_detector_items(const int *lw, const int *lh, int numLevels, int n, int hs, std::vector<uint4> &v);
