@@ -35,7 +35,7 @@ def lib():
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("CUDASIFT_B200_LIB") or _build.LIB     # override: kernel experiments (scripts/expbuild.sh)
+    path = os.environ.get("CUDASIFT_B200_LIB") or _build.LIB     # override: a library built some other way
     if not os.path.exists(path):
         path = _build.build_library()
     L = ctypes.CDLL(path)

@@ -30,6 +30,13 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared"]
 
 
+def headers():
+    """Every header a translation unit may include: all of csrc/*.cuh and csrc/*.h plus the public headers.
+    An edit to any of them rebuilds every unit."""
+    return sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))) + [
+        os.path.join(ROOT, "include", h) for h in ("cudaSift.h", "cudaImage.h", "cudasift_b200.h")]
+
+
 def _newer(target, deps):
     if not os.path.exists(target):
         return False
@@ -62,8 +69,7 @@ def build_library(force=False, verbose=False, managed=False):
     from concurrent.futures import ThreadPoolExecutor
     lib = LIB_MANAGED if managed else LIB
     srcs = [os.path.join(CSRC, s) for s in SOURCES]
-    hdrs = [os.path.join(CSRC, h) for h in ("common.cuh", "tma.cuh", "pipeline2.h")] + [
-        os.path.join(ROOT, "include", h) for h in ("cudaSift.h", "cudaImage.h", "cudasift_b200.h")]
+    hdrs = headers()
     if not force and _newer(lib, srcs + hdrs):
         return lib
     nvcc = nvcc_path()

@@ -2,12 +2,13 @@
 // cudaSiftD.cu:1361-1380: `pos<MEMWID` keeps the first 32 in (column, row) order, `tx<totbits` refines them).
 //
 // The detector (detect2.cu) counts the extrema of every such cell in packed 8-bit counters (reductions without a
-// return value); this kernel scans the counters for cells past the limit.  That almost never happens (it needs > 13 % of a block's pixels to be 26-neighbour extrema
-// above the threshold), so the repair is a separate, tiny, usually empty kernel: per listed cell it recomputes the
-// cell's DoG planes from the octave base image with the detector's arithmetic, ranks the extrema in the reference's
-// order and deletes the keypoints of rank >= 32 from the image's list (those that survived refinement; the list is
-// unordered anyway, so a hole is filled with the last record).
+// return value); this kernel scans the counters for cells past the limit.  That almost never happens (it needs > 13 %
+// of a block's pixels to be 26-neighbour extrema above the threshold), so the repair is a separate, tiny, usually empty
+// kernel: per listed cell it recomputes the cell's DoG planes from the octave base image with the detector's arithmetic
+// (sift_arith.cuh), ranks the extrema in the reference's order and deletes the keypoints of rank >= 32 from the image's
+// list (those that survived refinement; the list is unordered anyway, so a hole is filled with the last record).
 #include "common.cuh"
+#include "sift_arith.cuh"
 
 namespace cs {
 
@@ -15,16 +16,6 @@ namespace cs {
 #define C32_W 32              // DoG columns: cell column -1 .. +30
 #define C32_H 10              // DoG rows: cell row -1 .. +8
 #define C32_VW (C32_W + 8)    // columns of vertical results
-
-__device__ __forceinline__ float c32_sym9(const float *k, float c, float p1, float p2, float p3, float p4)
-{ // cudaSiftD.cu:1769-1788 as in detect2.cu: FMUL(k1,p1); FFMA(k0,c); FFMA(k2,p2); FFMA(k3,p3); FFMA(k4,p4)
-  float s = __fmul_rn(k[1], p1);
-  s = __fmaf_rn(k[0], c, s);
-  s = __fmaf_rn(k[2], p2, s);
-  s = __fmaf_rn(k[3], p3, s);
-  s = __fmaf_rn(k[4], p4, s);
-  return s;
-}
 
 __global__ void __launch_bounds__(C32_THREADS)
 cap32_fixup_kernel(const __grid_constant__ Detect2Params P)
@@ -94,7 +85,7 @@ cap32_fixup_kernel(const __grid_constant__ Detect2Params P)
       float in[9];
 #pragma unroll
       for (int j = 0; j < 9; j++) in[j] = __ldg(base + (size_t)min(max(y - 4 + j, 0), h - 1) * pitch + x);
-      s_v[s][r][c] = c32_sym9(L.taps.k[scale + s], in[4], __fadd_rn(in[3], in[5]), __fadd_rn(in[2], in[6]),
+      s_v[s][r][c] = laplace9(L.taps.k[scale + s], in[4], __fadd_rn(in[3], in[5]), __fadd_rn(in[2], in[6]),
                               __fadd_rn(in[1], in[7]), __fadd_rn(in[0], in[8]));
     }
     __syncthreads();
@@ -102,7 +93,7 @@ cap32_fixup_kernel(const __grid_constant__ Detect2Params P)
     for (int i = tid; i < 4 * C32_H * C32_W; i += C32_THREADS) {
       const int s = i / (C32_H * C32_W), r = (i / C32_W) % C32_H, c = i % C32_W;
       const float *v = &s_v[s][r][c];
-      s_b[s][r][c] = c32_sym9(L.taps.k[scale + s], v[4], __fadd_rn(v[3], v[5]), __fadd_rn(v[2], v[6]),
+      s_b[s][r][c] = laplace9(L.taps.k[scale + s], v[4], __fadd_rn(v[3], v[5]), __fadd_rn(v[2], v[6]),
                               __fadd_rn(v[1], v[7]), __fadd_rn(v[0], v[8]));
     }
     __syncthreads();

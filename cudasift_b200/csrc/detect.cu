@@ -14,9 +14,8 @@
 // and no register shuffling is needed.  Taps are duplicated (k,k) in the kernel parameters and
 // consumed straight from uniform registers.
 //
-// Per-pixel arithmetic (which products are fused, order of the sums) is pinned to the
-// reference's SASS with explicit round-to-nearest operations, so DoG values and therefore the extrema decisions
-// are bit-identical to the reference's.
+// Per-pixel arithmetic and refinement come from sift_arith.cuh (pinned to the reference's SASS), so DoG
+// values and therefore the extrema decisions are bit-identical to the reference's.
 //
 // Scheduling: persistent CTAs (4 per SM) walk the tile list; the global loads of the next tile
 // are issued into registers while the current tile is still being blurred, and the slot
@@ -26,6 +25,7 @@
 // Deliberate difference (documented in DESIGN.md): the reference keeps at most 32
 // candidates per 30x8x1 block (cudaSiftD.cu:1371,1379); no such cap exists here.
 #include "common.cuh"
+#include "sift_arith.cuh"
 
 namespace cs {
 
@@ -47,18 +47,6 @@ namespace cs {
 #define DT_SMEM_BYTES ((DT_SM_IN + DT_SM_V + DT_SM_DOG) * 8)   // 56832 B -> 4 CTAs per SM
 
 // f32x2, pk/upk, fma2/mul2/add2/sub2: tma.cuh (lo = row r, hi = row r+8)
-
-// cudaSiftD.cu:1769-1772 / 1779-1788: sum = k0*c; sum += kj*(x[-j]+x[+j]), j=1..4.
-// SASS: FMUL(k1,p1); FFMA(k0,c); FFMA(k2,p2); FFMA(k3,p3); FFMA(k4,p4)  -- here on both halves at once.
-__device__ __forceinline__ f32x2 lap_sym9(const float2 *k, f32x2 c, f32x2 p1, f32x2 p2, f32x2 p3, f32x2 p4)
-{
-  f32x2 s = mul2(pk(k[1]), p1);
-  s = fma2(pk(k[0]), c, s);
-  s = fma2(pk(k[2]), p2, s);
-  s = fma2(pk(k[3]), p3, s);
-  s = fma2(pk(k[4]), p4, s);
-  return s;
-}
 
 // float index of DoG element (plane, row, col) in the swizzled pair layout
 __device__ __forceinline__ int dog_index(int plane, int row, int col)
@@ -155,7 +143,7 @@ __device__ __forceinline__ unsigned int dog_tile(int w, int h, int x0, int y0, c
           const f32x2 p3 = add2(in[rr + 1], in[rr + 7]), p4 = add2(in[rr], in[rr + 8]);
 #pragma unroll
           for (int s = 0; s < DT_PH; s++)
-            s_v[(s * DT_HP + DT_VR * vh + rr) * DT_VS + vc] = upk(lap_sym9(taps.k[DT_PH * ph + s], cc, p1, p2, p3, p4));
+            s_v[(s * DT_HP + DT_VR * vh + rr) * DT_VS + vc] = upk(laplace9(taps.k[DT_PH * ph + s], cc, p1, p2, p3, p4));
         }
       }
     }
@@ -176,7 +164,7 @@ __device__ __forceinline__ unsigned int dog_tile(int w, int h, int x0, int y0, c
         f32x2 o[DT_NC];
 #pragma unroll
         for (int d = 0; d < DT_NC; d++)
-          o[d] = lap_sym9(taps.k[sg], v[d + 4], add2(v[d + 3], v[d + 5]), add2(v[d + 2], v[d + 6]),
+          o[d] = laplace9(taps.k[sg], v[d + 4], add2(v[d + 3], v[d + 5]), add2(v[d + 2], v[d + 6]),
                           add2(v[d + 1], v[d + 7]), add2(v[d], v[d + 8]));
         if (sg > 0) {
           float4 *out = reinterpret_cast<float4 *>(s_dog) + ((sg - 1) * DT_HP + hr) * (DT_W / 2);
@@ -245,8 +233,8 @@ __device__ __forceinline__ void store_keypoint(const DetectParams &P, unsigned i
   q->subsampling = kp.subsampling;
 }
 
-// cudaSiftD.cu:1383-1429 on the shared-memory DoG planes.  pl = plane `scale` (the candidate sits in
-// plane scale+1 at tile position (r, d)).  An accepted keypoint is parked in the shared queue; its
+// cudaSiftD.cu:1383-1429 (sift_arith.cuh) on the shared-memory DoG planes.  pl = plane `scale` (the candidate
+// sits in plane scale+1 at tile position (r, d)).  An accepted keypoint is parked in the shared queue; its
 // slot in the output array is allocated (one global atomic) at the start of the next tile and the
 // record written in the middle of it, so the atomic's round trip is off the critical path.
 __device__ __noinline__ void refine(const float *pl, int r, int d, int gx, int gy, int scale,
@@ -261,47 +249,10 @@ __device__ __noinline__ void refine(const float *pl, int r, int d, int gx, int g
 #pragma unroll
       for (int p = 0; p < 3; p++) v[p][dy][dx] = pl[p * (DT_HP * DT_W * 2) + o];
     }
-  const float val = v[1][1][1];
-  float two = __fadd_rn(val, val);
-  float dxx = __fsub_rn(__fsub_rn(two, v[1][1][0]), v[1][1][2]);
-  float dyy = __fsub_rn(__fsub_rn(two, v[1][0][1]), v[1][2][1]);
-  float dxy = __fmul_rn(0.25f, __fsub_rn(__fsub_rn(__fadd_rn(v[1][2][2], v[1][0][0]), v[1][0][2]), v[1][2][0]));
-  float tra = __fadd_rn(dxx, dyy);
-  float det = __fmaf_rn(dxx, dyy, -__fmul_rn(dxy, dxy));
-  float tra2 = __fmul_rn(tra, tra);
-  if (!(tra2 < __fmul_rn(P.edgeLimit, det))) return;
-  float edge = __fdividef(tra2, det);
-  float dx = __fmul_rn(0.5f, __fsub_rn(v[1][1][2], v[1][1][0]));
-  float dy = __fmul_rn(0.5f, __fsub_rn(v[1][2][1], v[1][0][1]));
-  float ds = __fmul_rn(0.5f, __fsub_rn(v[0][1][1], v[2][1][1]));
-  float dss = __fsub_rn(__fsub_rn(two, v[2][1][1]), v[0][1][1]);
-  float dxs = __fmul_rn(0.25f, __fsub_rn(__fsub_rn(__fadd_rn(v[2][1][2], v[0][1][0]), v[0][1][2]), v[2][1][0]));
-  float dys = __fmul_rn(0.25f, __fsub_rn(__fsub_rn(__fadd_rn(v[2][2][1], v[0][0][1]), v[2][0][1]), v[0][2][1]));
-  float idxx = __fmaf_rn(dyy, dss, -__fmul_rn(dys, dys));
-  float idxy = __fmaf_rn(dys, dxs, -__fmul_rn(dxy, dss));
-  float idxs = __fmaf_rn(dxy, dys, -__fmul_rn(dyy, dxs));
-  float det3 = __fmaf_rn(idxs, dxs, __fmaf_rn(idxx, dxx, __fmul_rn(idxy, dxy)));
-  float idet = __fdividef(1.0f, det3);
-  float idyy = __fmaf_rn(dxx, dss, -__fmul_rn(dxs, dxs));
-  float idys = __fmaf_rn(dxy, dxs, -__fmul_rn(dxx, dys));
-  float idss = det;
-  float pdx = __fmul_rn(idet, __fmaf_rn(ds, idxs, __fmaf_rn(dx, idxx, __fmul_rn(dy, idxy))));
-  float pdy = __fmul_rn(idet, __fmaf_rn(ds, idys, __fmaf_rn(dy, idyy, __fmul_rn(dx, idxy))));
-  float pds = __fmul_rn(idet, __fmaf_rn(idss, ds, __fmaf_rn(dx, idxs, __fmul_rn(dy, idys))));
-  if (pdx < -0.5f || pdx > 0.5f || pdy < -0.5f || pdy > 0.5f || pds < -0.5f || pds > 0.5f) {
-    pdx = __fdividef(dx, dxx);
-    pdy = __fdividef(dy, dyy);
-    pds = __fdividef(ds, dss);
-  }
-  float dsum = __fmaf_rn(ds, pds, __fmaf_rn(dx, pdx, __fmul_rn(dy, pdy)));
-  float sc = __fmul_rn(powf(2.0f, __fdiv_rn((float)scale, (float)CS_NUM_SCALES)), exp2f(__fmul_rn(pds, P.factor)));
-  if (!(sc >= L.lowestScale)) return;
   Keypoint kp;
-  kp.x = __fadd_rn((float)gx, pdx);
-  kp.y = __fadd_rn((float)gy, pdy);
-  kp.scale = sc;
-  kp.sharpness = __fmaf_rn(dsum, 0.5f, val);
-  kp.edgeness = edge;
+  if (!refine_extremum(v, gx, gy, P.edgeLimit, P.factor, L.lowestScale,
+                       [&] { return powf(2.0f, __fdiv_rn((float)scale, (float)CS_NUM_SCALES)); }, kp))
+    return;
   kp.subsampling = L.subsampling;
   const int q = atomicAdd(s_kn, 1);
   if (q < DT_KQ) s_kq[q] = kp;

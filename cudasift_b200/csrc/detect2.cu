@@ -2,8 +2,8 @@
 // a whole BATCH of images in one launch (detect3_kernel).
 //
 // Behavioural spec: reference LaplaceMultiMem (cudaSiftD.cu:1753-1793, host :460-487) and
-// FindPointsMultiNew (cudaSiftD.cu:1292-1431, host :489-514).  Same per-pixel arithmetic as detect.cu
-// (pinned to the reference's SASS: which products are fused, the order of the sums), new dataflow:
+// FindPointsMultiNew (cudaSiftD.cu:1292-1431, host :489-514).  Per-pixel arithmetic and refinement from
+// sift_arith.cuh (pinned to the reference's SASS: which products are fused, the order of the sums), new dataflow:
 //
 //  * A work item is a column strip (256 staged columns -> 248 DoG columns -> 244 tested columns) times a
 //    range of rows of one octave of one image.  The CTA marches down the rows; nothing is recomputed
@@ -39,6 +39,7 @@
 // Shared memory per row pair and step: 128 (vertical STS) + 256 (horizontal LDS) + 128 (shuffles) + 112 (DoG
 // STS) wavefronts for 2 x 244 pixels x 8 scales = 1.3 wavefronts per pixel (detect.cu: 2.7).
 #include "common.cuh"
+#include "sift_arith.cuh"
 
 namespace cs {
 
@@ -54,26 +55,12 @@ namespace cs {
 #define D2_KQ 32             // keypoints parked per item before the slots are allocated
 #define D2_SMEM_IN (D2_NS * 2 * D2_IW * 4)            // 16384
 
-// cudaSiftD.cu:1769-1772 / 1779-1788: sum = k0*c; sum += kj*(x[-j]+x[+j]), j=1..4.
-// SASS: FMUL(k1,p1); FFMA(k0,c); FFMA(k2,p2); FFMA(k3,p3); FFMA(k4,p4)  -- here on both halves at once.
-// A tap is ONE register: pk2(k, k) feeds the same register to both scalar halves.
-__device__ __forceinline__ f32x2 d2_sym9(const float (&k)[5], f32x2 c, f32x2 p1, f32x2 p2, f32x2 p3, f32x2 p4)
-{
-  f32x2 s = mul2(pk2(k[1], k[1]), p1);
-  s = fma2(pk2(k[0], k[0]), c, s);
-  s = fma2(pk2(k[2], k[2]), p2, s);
-  s = fma2(pk2(k[3], k[3]), p3, s);
-  s = fma2(pk2(k[4], k[4]), p4, s);
-  return s;
-}
-
 struct D2Keypoint { float x, y, scale, sharpness, edgeness, subsampling; unsigned int tag; };
 
-// powf(2.0f, scale / 5) of cudaSiftD.cu:1413 for the five scales an extremum can have.  The table is filled on the
+// powf(2.0f, scale / 5) of cudaSiftD.cu:1417 for the five scales an extremum can have.  The table is filled on the
 // device by the same powf (d2_fill_pow_table, first launch per device), so the values are the ones the reference's
 // expression yields; it takes ~100 instructions out of the refinement of every extremum.
 __device__ float d2_pow_table[CS_NUM_SCALES];
-__device__ __forceinline__ float d2_pow_scale(int scale) { return d2_pow_table[scale]; }
 __global__ void d2_fill_pow_table()
 {
   if (threadIdx.x < CS_NUM_SCALES) d2_pow_table[threadIdx.x] = powf(2.0f, __fdiv_rn((float)threadIdx.x, (float)CS_NUM_SCALES));
@@ -92,52 +79,13 @@ __device__ __forceinline__ void d2_store_keypoint(SiftPoint *pts, int maxPts, un
   q->empty[0] = __uint_as_float(kp.tag);            // integer position of the extremum (cap32 bookkeeping)
 }
 
-// cudaSiftD.cu:1383-1429.  v[p][dy][dx]: the 3x3x3 DoG neighbourhood, candidate at [1][1][1].
+// cudaSiftD.cu:1383-1429 (sift_arith.cuh).  v[p][dy][dx]: the 3x3x3 DoG neighbourhood, candidate at [1][1][1].
 __device__ __forceinline__ void d2_refine(const float (&v)[3][3][3], int gx, int gy, int scale, float subsampling,
                                        float lowestScale, float edgeLimit, float factor, unsigned int tag,
                                        D2Keypoint *s_kq, int *s_kn, SiftPoint *pts, unsigned int *counter, int maxPts)
 {
-  const float val = v[1][1][1];
-  float two = __fadd_rn(val, val);
-  float dxx = __fsub_rn(__fsub_rn(two, v[1][1][0]), v[1][1][2]);
-  float dyy = __fsub_rn(__fsub_rn(two, v[1][0][1]), v[1][2][1]);
-  float dxy = __fmul_rn(0.25f, __fsub_rn(__fsub_rn(__fadd_rn(v[1][2][2], v[1][0][0]), v[1][0][2]), v[1][2][0]));
-  float tra = __fadd_rn(dxx, dyy);
-  float det = __fmaf_rn(dxx, dyy, -__fmul_rn(dxy, dxy));
-  float tra2 = __fmul_rn(tra, tra);
-  if (!(tra2 < __fmul_rn(edgeLimit, det))) return;
-  float edge = __fdividef(tra2, det);
-  float dx = __fmul_rn(0.5f, __fsub_rn(v[1][1][2], v[1][1][0]));
-  float dy = __fmul_rn(0.5f, __fsub_rn(v[1][2][1], v[1][0][1]));
-  float ds = __fmul_rn(0.5f, __fsub_rn(v[0][1][1], v[2][1][1]));
-  float dss = __fsub_rn(__fsub_rn(two, v[2][1][1]), v[0][1][1]);
-  float dxs = __fmul_rn(0.25f, __fsub_rn(__fsub_rn(__fadd_rn(v[2][1][2], v[0][1][0]), v[0][1][2]), v[2][1][0]));
-  float dys = __fmul_rn(0.25f, __fsub_rn(__fsub_rn(__fadd_rn(v[2][2][1], v[0][0][1]), v[2][0][1]), v[0][2][1]));
-  float idxx = __fmaf_rn(dyy, dss, -__fmul_rn(dys, dys));
-  float idxy = __fmaf_rn(dys, dxs, -__fmul_rn(dxy, dss));
-  float idxs = __fmaf_rn(dxy, dys, -__fmul_rn(dyy, dxs));
-  float det3 = __fmaf_rn(idxs, dxs, __fmaf_rn(idxx, dxx, __fmul_rn(idxy, dxy)));
-  float idet = __fdividef(1.0f, det3);
-  float idyy = __fmaf_rn(dxx, dss, -__fmul_rn(dxs, dxs));
-  float idys = __fmaf_rn(dxy, dxs, -__fmul_rn(dxx, dys));
-  float idss = det;
-  float pdx = __fmul_rn(idet, __fmaf_rn(ds, idxs, __fmaf_rn(dx, idxx, __fmul_rn(dy, idxy))));
-  float pdy = __fmul_rn(idet, __fmaf_rn(ds, idys, __fmaf_rn(dy, idyy, __fmul_rn(dx, idxy))));
-  float pds = __fmul_rn(idet, __fmaf_rn(idss, ds, __fmaf_rn(dx, idxs, __fmul_rn(dy, idys))));
-  if (pdx < -0.5f || pdx > 0.5f || pdy < -0.5f || pdy > 0.5f || pds < -0.5f || pds > 0.5f) {
-    pdx = __fdividef(dx, dxx);
-    pdy = __fdividef(dy, dyy);
-    pds = __fdividef(ds, dss);
-  }
-  float dsum = __fmaf_rn(ds, pds, __fmaf_rn(dx, pdx, __fmul_rn(dy, pdy)));
-  float sc = __fmul_rn(d2_pow_scale(scale), exp2f(__fmul_rn(pds, factor)));
-  if (!(sc >= lowestScale)) return;
   D2Keypoint kp;
-  kp.x = __fadd_rn((float)gx, pdx);
-  kp.y = __fadd_rn((float)gy, pdy);
-  kp.scale = sc;
-  kp.sharpness = __fmaf_rn(dsum, 0.5f, val);
-  kp.edgeness = edge;
+  if (!refine_extremum(v, gx, gy, edgeLimit, factor, lowestScale, [&] { return d2_pow_table[scale]; }, kp)) return;
   kp.subsampling = subsampling;
   kp.tag = tag;
   const int q = atomicAdd(s_kn, 1);
@@ -261,14 +209,14 @@ __device__ __forceinline__ void d3_vertical(f32x2 (&W0)[9], f32x2 (&W1)[9], f32x
     const f32x2 p1 = add2(W0[D3_WI(3)], W0[D3_WI(5)]), p2 = add2(W0[D3_WI(2)], W0[D3_WI(6)]);
     const f32x2 p3 = add2(W0[D3_WI(1)], W0[D3_WI(7)]), p4 = add2(W0[D3_WI(0)], W0[D3_WI(8)]);
 #pragma unroll
-    for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2] = upk(d2_sym9(kv[s], c, p1, p2, p3, p4));
+    for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2] = upk(laplace9(kv[s], c, p1, p2, p3, p4));
   }
   {
     const f32x2 c = W1[D3_WI(4)];
     const f32x2 p1 = add2(W1[D3_WI(3)], W1[D3_WI(5)]), p2 = add2(W1[D3_WI(2)], W1[D3_WI(6)]);
     const f32x2 p3 = add2(W1[D3_WI(1)], W1[D3_WI(7)]), p4 = add2(W1[D3_WI(0)], W1[D3_WI(8)]);
 #pragma unroll
-    for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2 + 128] = upk(d2_sym9(kv[s], c, p1, p2, p3, p4));
+    for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2 + 128] = upk(laplace9(kv[s], c, p1, p2, p3, p4));
   }
 #undef D3_WI
 }
@@ -455,8 +403,8 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
           f32x2 dg[8];
 #pragma unroll
           for (int d = 0; d < 8; d++) {
-            const f32x2 o = d2_sym9(kh, V[d + 4], add2(V[d + 3], V[d + 5]), add2(V[d + 2], V[d + 6]),
-                                    add2(V[d + 1], V[d + 7]), add2(V[d], V[d + 8]));
+            const f32x2 o = laplace9(kh, V[d + 4], add2(V[d + 3], V[d + 5]), add2(V[d + 2], V[d + 6]),
+                                     add2(V[d + 1], V[d + 7]), add2(V[d], V[d + 8]));
             const float2 of = upk(o);
             const float plo = __shfl_up_sync(0xffffffffu, of.x, 1), phi = __shfl_up_sync(0xffffffffu, of.y, 1);
             dg[d] = sub2(o, pk2(plo, phi));                 // blur[s] - blur[s-1]: DoG plane s-1 (cudaSiftD.cu:1790)

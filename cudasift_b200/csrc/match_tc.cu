@@ -29,33 +29,7 @@ namespace cs {
 #define TC_KCH 16           // 16-byte chunks (8 halves) per descriptor
 
 // ------------------------------------------------------------------------------ PTX helpers
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count)
-{
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes)
-{
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar)
-{
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity)
-{
-  uint32_t addr = smem_u32(bar), ok;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-  } while (!ok);
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
-{
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
+// (mbarrier and bulk-copy wrappers: tma.cuh)
 // GMMA shared-memory descriptor, K-major, no swizzle ("interleaved" core matrices of
 // 8 rows x 16 bytes).  lbo = byte distance between the two K chunks of one K=16 step,
 // sbo = byte distance between consecutive 8-row groups (PTX ISA, "Matrix Descriptor Format").
@@ -266,10 +240,9 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
 
   if (threadIdx.x == 0) {
     // the empty barriers take one arrival per consumer warp (8): each warp's wgmma.wait_group covers its own reads
-    mbar_init(&bar_a_full, 1); mbar_init(&bar_a_empty, 8);
-    for (int s = 0; s < T3_STAGES; s++) { mbar_init(&bar_b_full[s], 1); mbar_init(&bar_b_empty[s], 8); }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    mbarrier_init(&bar_a_full, 1); mbarrier_init(&bar_a_empty, 8);
+    for (int s = 0; s < T3_STAGES; s++) { mbarrier_init(&bar_b_full[s], 1); mbarrier_init(&bar_b_empty[s], 8); }
+    mbarrier_init_fence();
   }
   __syncthreads();
 
@@ -281,14 +254,14 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
         const int mt = u / pl.n_nt, nt = u - mt * pl.n_nt;
         if (mt != prevMt) {
           // every MMA of the previous run must have read the A tile before it is overwritten
-          if (runIdx > 0) mbar_wait(&bar_a_empty, (runIdx - 1) & 1);
-          mbar_expect_tx(&bar_a_full, T3_A_BYTES);
+          if (runIdx > 0) mbarrier_wait(&bar_a_empty, (runIdx - 1) & 1);
+          mbarrier_expect_tx(&bar_a_full, T3_A_BYTES);
           bulk_g2s(sA, reinterpret_cast<const uint8_t *>(bf.a16) + (size_t)mt * T3_A_BYTES, T3_A_BYTES, &bar_a_full);
           prevMt = mt; runIdx++;
         }
         const int s = i % T3_STAGES, it = i / T3_STAGES;
-        if (it > 0) mbar_wait(&bar_b_empty[s], (it - 1) & 1);
-        mbar_expect_tx(&bar_b_full[s], T3_B_BYTES);
+        if (it > 0) mbarrier_wait(&bar_b_empty[s], (it - 1) & 1);
+        mbarrier_expect_tx(&bar_b_full[s], T3_B_BYTES);
         bulk_g2s(sB + s * T3_B_BYTES, reinterpret_cast<const uint8_t *>(bf.b16) + (size_t)nt * T3_B_BYTES, T3_B_BYTES, &bar_b_full[s]);
       }
     }
@@ -298,7 +271,7 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
     const int g = (warp - 4) >> 2, wi = warp & 3;
     const int hb = (lane >> 1) & 1;       // this lane's 4-candidate groups are those of the partitions of parity hb
     const int rowInTile = g * T3_M + 16 * wi + (lane >> 2);   // and +8 (accumulator fragment rows)
-    const uint32_t aBase = smem_u32(sA) + g * T3_M * 16, bBase = smem_u32(sB);
+    const uint32_t aBase = smem_addr(sA) + g * T3_M * 16, bBase = smem_addr(sB);
     float acc[64];
 #pragma unroll
     for (int e = 0; e < 64; e++) acc[e] = 0.0f;
@@ -311,7 +284,7 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
       const int mt = u / pl.n_nt, nt = u - mt * pl.n_nt;
       if (mt != prevMt) {
         slot = tc_slot(pl, cta, runIdx, rowInTile);
-        mbar_wait(&bar_a_full, runIdx & 1);
+        mbarrier_wait(&bar_a_full, runIdx & 1);
         prevMt = mt; runIdx++;
 #pragma unroll
         for (int r = 0; r < 2; r++)
@@ -319,7 +292,7 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
           for (int q = 0; q < 4; q++) { g1[r][q] = 0.0f; g2[r][q] = 0.0f; g3[r][q] = 0.0f; i1[r][q] = -1; i2[r][q] = -1; }
       }
       const int s = i % T3_STAGES, it = i / T3_STAGES;
-      mbar_wait(&bar_b_full[s], it & 1);
+      mbarrier_wait(&bar_b_full[s], it & 1);
       const uint32_t bS = bBase + s * T3_B_BYTES;
       wg_fence();
 #pragma unroll
@@ -337,8 +310,8 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
       wg_wait0(acc);
       const bool lastOfRun = (u + 1 == u_end) || ((u + 1) / pl.n_nt != mt);
       if (lane == 0) {
-        mbar_arrive(&bar_b_empty[s]);
-        if (lastOfRun) mbar_arrive(&bar_a_empty);
+        mbarrier_arrive(&bar_b_empty[s]);
+        if (lastOfRun) mbarrier_arrive(&bar_a_empty);
       }
       // columns 8j + 2(lane % 4) + {0, 1}: the lane pair (lane, lane ^ 1) holds group 2j + hb of partition 2(j % 4) + hb
       const int gbase = nt * (T3_N / 4) + hb;

@@ -3,15 +3,12 @@
 // Behavioural spec: reference cudaSiftD.cu:1986-2037 (LowPassBlock), :84-168 (ScaleDown),
 // :170-190 (ScaleUp) and their host launchers cudaSiftH.cu:308-351, 406-435.
 // These are new kernels (shared-memory tiles, 128-bit shared/global accesses); what is
-// kept from the reference is the arithmetic of every output pixel: the order of the
-// additions and which products are fused into FMAs was read off the reference's
-// SASS and is pinned here with __fmul_rn/__fmaf_rn/__fadd_rn so that the pyramid is
-// bit-identical to the reference's (and to oracle/sift_oracle.c).
+// kept from the reference is the arithmetic of every output pixel (sift_arith.cuh), so
+// that the pyramid is bit-identical to the reference's (and to oracle/sift_oracle.c).
 #include "common.cuh"
+#include "sift_arith.cuh"
 
 namespace cs {
-
-__device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
 
 // ---------------------------------------------------------------------------------------
 // LowPass: 9-tap separable Gaussian, horizontal then vertical, clamp-to-edge.
@@ -22,18 +19,6 @@ __device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v,
 #define LP_R 4
 #define LP_IW (LP_W + 2 * LP_R)   // 136
 #define LP_IH (LP_H + 2 * LP_R)   // 40
-
-// k[4] is the centre tap.  SASS of LowPassBlock: FMUL(k3,p1); FFMA(k4,c); FFMA(k2,p2);
-// FFMA(k1,p3); FFMA(k0,p4) for both passes.
-__device__ __forceinline__ float lp_sym9(const Taps9 &t, float c, float p1, float p2, float p3, float p4)
-{
-  float s = __fmul_rn(t.k[3], p1);
-  s = __fmaf_rn(t.k[4], c, s);
-  s = __fmaf_rn(t.k[2], p2, s);
-  s = __fmaf_rn(t.k[1], p3, s);
-  s = __fmaf_rn(t.k[0], p4, s);
-  return s;
-}
 
 __global__ void __launch_bounds__(256, 4)      // 510 CTAs at 1080p fit one wave (132 x 4)
 lowpass_kernel(const float *__restrict__ src, int srcPitch, float *__restrict__ dst, int dstPitch,
@@ -92,8 +77,8 @@ lowpass_kernel(const float *__restrict__ src, int srcPitch, float *__restrict__ 
     float o[4];
 #pragma unroll
     for (int d = 0; d < 4; d++)
-      o[d] = lp_sym9(taps, v[d + 4], __fadd_rn(v[d + 5], v[d + 3]), __fadd_rn(v[d + 6], v[d + 2]),
-                     __fadd_rn(v[d + 7], v[d + 1]), __fadd_rn(v[d + 8], v[d]));
+      o[d] = lowpass9(taps.k, v[d + 4], __fadd_rn(v[d + 5], v[d + 3]), __fadd_rn(v[d + 6], v[d + 2]),
+                      __fadd_rn(v[d + 7], v[d + 1]), __fadd_rn(v[d + 8], v[d]));
     *reinterpret_cast<float4 *>(&s_h[r][4 * seg]) = make_float4(o[0], o[1], o[2], o[3]);
   }
   __syncthreads();
@@ -109,9 +94,9 @@ lowpass_kernel(const float *__restrict__ src, int srcPitch, float *__restrict__ 
     for (int d = 0; d < 4; d++) {
       const int gy = y0 + 4 * rg + d;
       float4 o;
-#define LPV(f)                                                                                   \
-  lp_sym9(taps, v[d + 4].f, __fadd_rn(v[d + 3].f, v[d + 5].f), __fadd_rn(v[d + 2].f, v[d + 6].f), \
-          __fadd_rn(v[d + 1].f, v[d + 7].f), __fadd_rn(v[d].f, v[d + 8].f))
+#define LPV(f)                                                                                      \
+  lowpass9(taps.k, v[d + 4].f, __fadd_rn(v[d + 3].f, v[d + 5].f), __fadd_rn(v[d + 2].f, v[d + 6].f), \
+           __fadd_rn(v[d + 1].f, v[d + 7].f), __fadd_rn(v[d].f, v[d + 8].f))
       o.x = LPV(x); o.y = LPV(y); o.z = LPV(z); o.w = LPV(w);
 #undef LPV
       if (gy < h) {
@@ -178,31 +163,22 @@ scaledown_kernel(const float *__restrict__ src, float *__restrict__ dst, int w, 
   }
   __syncthreads();
 
-  // horizontal: cudaSiftD.cu:121  k0*(a0+a4) + k1*(a1+a3) + k2*a2
-  //   SASS: FMUL(k1,(a1+a3)); FFMA(k0,(a0+a4)); FFMA(k2,a2)
+  // horizontal 5-tap
   for (int t = tid; t < SD_IH * SD_W; t += 256) {
     int r = t / SD_W, x = t - r * SD_W;
     const float2 *p = reinterpret_cast<const float2 *>(&s_in[r][2 * x]);
     float2 a01 = p[0], a23 = p[1], a45 = p[2];
-    float s = __fmul_rn(taps.k[1], __fadd_rn(a01.y, a23.y));
-    s = __fmaf_rn(taps.k[0], __fadd_rn(a01.x, a45.x), s);
-    s = __fmaf_rn(taps.k[2], a23.x, s);
-    s_h[r][x] = s;
+    s_h[r][x] = scaledown_h(taps.k, a01.x, a01.y, a23.x, a23.y, a45.x);
   }
   __syncthreads();
 
-  // vertical: cudaSiftD.cu:123  k2*c + k0*(r0+r4) + k1*(r1+r3)
-  //   SASS: FMUL(k0,(r0+r4)); FFMA(k2,c); FFMA(k1,(r1+r3))
+  // vertical 5-tap
   for (int t = tid; t < SD_H * SD_W; t += 256) {
     int y = t / SD_W, x = t - y * SD_W;
     int gx = ox0 + x, gy = oy0 + y;
     if (gx < w2 && gy < h2) {
-      float r0 = s_h[2 * y][x], r1 = s_h[2 * y + 1][x], r2 = s_h[2 * y + 2][x];
-      float r3 = s_h[2 * y + 3][x], r4 = s_h[2 * y + 4][x];
-      float s = __fmul_rn(taps.k[0], __fadd_rn(r0, r4));
-      s = __fmaf_rn(taps.k[2], r2, s);
-      s = __fmaf_rn(taps.k[1], __fadd_rn(r1, r3), s);
-      dst[(size_t)gy * newpitch + gx] = s;
+      dst[(size_t)gy * newpitch + gx] =
+          scaledown_v(taps.k, s_h[2 * y][x], s_h[2 * y + 1][x], s_h[2 * y + 2][x], s_h[2 * y + 3][x], s_h[2 * y + 4][x]);
     }
   }
 }

@@ -1,7 +1,7 @@
 // pyramid2.cu -- fused, batched Gaussian pyramid: (A) LowPass + first ScaleDown in one marching kernel fed by
 // TMA, (B) the remaining ScaleDowns in one launch.  Behavioural spec: reference LowPassBlock
 // (cudaSiftD.cu:1986-2037, host cudaSiftH.cu:406-435) and ScaleDown (cudaSiftD.cu:84-168, host :308-338);
-// per-pixel arithmetic as in pyramid.cu (pinned to the reference's SASS), so every level is bit-identical
+// per-pixel arithmetic from sift_arith.cuh (pinned to the reference's SASS), so every level is bit-identical
 // to the reference's.
 //
 // Kernel A: a WARP owns a strip of 120 columns x R rows of the full-resolution level and marches down the rows; warps
@@ -15,37 +15,9 @@
 // for that tile in shared memory (85x85 -> 41x41 -> 19x19 -> 8x8), writing the part of every level it owns: the
 // four dependent launches of the reference (cudaSiftH.cu:153-157) become two.
 #include "common.cuh"
+#include "sift_arith.cuh"
 
 namespace cs {
-
-__device__ __forceinline__ int clampi2(int v, int lo, int hi) { return min(max(v, lo), hi); }
-
-// k[4] is the centre tap.  SASS of LowPassBlock: FMUL(k3,p1); FFMA(k4,c); FFMA(k2,p2); FFMA(k1,p3); FFMA(k0,p4).
-__device__ __forceinline__ float pa_sym9(const Taps9 &t, float c, float p1, float p2, float p3, float p4)
-{
-  float s = __fmul_rn(t.k[3], p1);
-  s = __fmaf_rn(t.k[4], c, s);
-  s = __fmaf_rn(t.k[2], p2, s);
-  s = __fmaf_rn(t.k[1], p3, s);
-  s = __fmaf_rn(t.k[0], p4, s);
-  return s;
-}
-// ScaleDown horizontal (cudaSiftD.cu:121): FMUL(k1,(a1+a3)); FFMA(k0,(a0+a4)); FFMA(k2,a2)
-__device__ __forceinline__ float sd_h(const Taps5 &t, float a0, float a1, float a2, float a3, float a4)
-{
-  float s = __fmul_rn(t.k[1], __fadd_rn(a1, a3));
-  s = __fmaf_rn(t.k[0], __fadd_rn(a0, a4), s);
-  s = __fmaf_rn(t.k[2], a2, s);
-  return s;
-}
-// ScaleDown vertical (cudaSiftD.cu:123): FMUL(k0,(r0+r4)); FFMA(k2,c); FFMA(k1,(r1+r3))
-__device__ __forceinline__ float sd_v(const Taps5 &t, float r0, float r1, float r2, float r3, float r4)
-{
-  float s = __fmul_rn(t.k[0], __fadd_rn(r0, r4));
-  s = __fmaf_rn(t.k[2], r2, s);
-  s = __fmaf_rn(t.k[1], __fadd_rn(r1, r3), s);
-  return s;
-}
 
 #define PA_THREADS 32      // one warp per CTA: a strip is private to its warp, so the march needs no CTA barrier
 #define PA_IW CS_PA_BOX    // staged input columns x0-8 .. x0+127 (one TMA box row)
@@ -91,24 +63,20 @@ __device__ __forceinline__ void pa_step(const PaCtx &C, PaRun &R, f32x2 (&W)[9][
   if (EDGE) {
     if (C.cb - 4 < 0 || C.cb + 7 > C.w - 1) {                // cudaSiftD.cu:2005-2008: clamped column reads
 #pragma unroll
-      for (int i = 0; i < 12; i++) v[i] = rowp[clampi2(C.cb - 4 + i, 0, C.w - 1) - (C.x0 - 8)];
+      for (int i = 0; i < 12; i++) v[i] = rowp[clampi(C.cb - 4 + i, 0, C.w - 1) - (C.x0 - 8)];
     }
   }
   float o[4];
 #pragma unroll
   for (int d = 0; d < 4; d++)
-#ifdef PA_SKEL   // diagnostic build (scripts/expbuild.sh -DPA_SKEL): the march without its arithmetic = the memory-side ceiling
-    o[d] = v[d + 4];
-#else
-    o[d] = pa_sym9(lp, v[d + 4], __fadd_rn(v[d + 5], v[d + 3]), __fadd_rn(v[d + 6], v[d + 2]),
-                   __fadd_rn(v[d + 7], v[d + 1]), __fadd_rn(v[d + 8], v[d]));
-#endif
+    o[d] = lowpass9(lp.k, v[d + 4], __fadd_rn(v[d + 5], v[d + 3]), __fadd_rn(v[d + 6], v[d + 2]),
+                    __fadd_rn(v[d + 7], v[d + 1]), __fadd_rn(v[d + 8], v[d]));
   W[PH][0] = pk2(o[0], o[1]);
   W[PH][1] = pk2(o[2], o[3]);
   __syncwarp();                                              // every lane has consumed the slot
   if (lane == 0 && R.seq + PA_NS <= C.seqEnd) {              // refill it with the row 9 steps ahead
     mbarrier_expect_tx(&s_full[PH], PA_IW * 4);
-    tma_load_2d(rowp, map, C.x0 - 8, clampi2(C.ia + R.seq + PA_NS, 0, C.h - 1), &s_full[PH]);
+    tma_load_2d(rowp, map, C.x0 - 8, clampi(C.ia + R.seq + PA_NS, 0, C.h - 1), &s_full[PH]);
   }
   R.seq++;
   if (!MAIN) return;
@@ -116,18 +84,11 @@ __device__ __forceinline__ void pa_step(const PaCtx &C, PaRun &R, f32x2 (&W)[9][
   const int y = R.y;
   float4 o4;
   {
-    // window order: oldest = slot PH+1 (row y-4) ... newest = slot PH (row y+4); same sums as pa_sym9, two columns at once
+    // window order: oldest = slot PH+1 (row y-4) ... newest = slot PH (row y+4); two columns at once
 #define PAW(i, hh) W[(PH + 1 + (i)) % 9][hh]
-#define PAV(hh)                                                                                             \
-  fma2(pk2(lp.k[0], lp.k[0]), add2(PAW(0, hh), PAW(8, hh)),                                                  \
-       fma2(pk2(lp.k[1], lp.k[1]), add2(PAW(1, hh), PAW(7, hh)),                                             \
-            fma2(pk2(lp.k[2], lp.k[2]), add2(PAW(2, hh), PAW(6, hh)),                                        \
-                 fma2(pk2(lp.k[4], lp.k[4]), PAW(4, hh), mul2(pk2(lp.k[3], lp.k[3]), add2(PAW(3, hh), PAW(5, hh)))))))
-#ifdef PA_SKEL
-    const float2 lo = upk(PAW(4, 0)), hi = upk(PAW(4, 1));
-#else
+#define PAV(hh) \
+  lowpass9(lp.k, PAW(0, hh), PAW(1, hh), PAW(2, hh), PAW(3, hh), PAW(4, hh), PAW(5, hh), PAW(6, hh), PAW(7, hh), PAW(8, hh))
     const float2 lo = upk(PAV(0)), hi = upk(PAV(1));
-#endif
 #undef PAV
 #undef PAW
     o4 = make_float4(lo.x, lo.y, hi.x, hi.y);
@@ -155,15 +116,12 @@ __device__ __forceinline__ void pa_step(const PaCtx &C, PaRun &R, f32x2 (&W)[9][
     *reinterpret_cast<float4 *>(s_l0 + 4 * lane) = o4;       // s_l0[i] = column x0-4+i
     __syncwarp();
 #pragma unroll
-    for (int i = 0; i < 7; i++) a[i] = s_l0[clampi2(clampi2(C.cb - 2 + i, 0, C.w - 1) - (C.x0 - 4), 0, 4 * PA_THREADS - 1)];
+    for (int i = 0; i < 7; i++) a[i] = s_l0[clampi(clampi(C.cb - 2 + i, 0, C.w - 1) - (C.x0 - 4), 0, 4 * PA_THREADS - 1)];
   }
   float2 *h2 = s_h2 + lane;                                  // [row & 7][lane] and again at [8 + (row & 7)][lane]: a private
   {                                                          // column, stored twice so that any 5 consecutive rows are contiguous
-#ifdef PA_SKEL
-    const float2 hv = make_float2(a[2] + a[0] + a[6], a[4]);
-#else
-    const float2 hv = make_float2(sd_h(sdk, a[0], a[1], a[2], a[3], a[4]), sd_h(sdk, a[2], a[3], a[4], a[5], a[6]));
-#endif
+    const float2 hv = make_float2(scaledown_h(sdk.k, a[0], a[1], a[2], a[3], a[4]),
+                                  scaledown_h(sdk.k, a[2], a[3], a[4], a[5], a[6]));
     float2 *hw = h2 + (y & 7) * PA_THREADS;
     hw[0] = hv;
     hw[8 * PA_THREADS] = hv;
@@ -176,11 +134,9 @@ __device__ __forceinline__ void pa_step(const PaCtx &C, PaRun &R, f32x2 (&W)[9][
       for (int j = 0; j < 5; j++) q[j] = pk(h2[(((y + 4) & 7) + j) * PA_THREADS]);
     } else {
 #pragma unroll
-      for (int j = 0; j < 5; j++) q[j] = pk(h2[(clampi2(2 * R.nextY1 - 2 + j, 0, C.h - 1) & 7) * PA_THREADS]);
+      for (int j = 0; j < 5; j++) q[j] = pk(h2[(clampi(2 * R.nextY1 - 2 + j, 0, C.h - 1) & 7) * PA_THREADS]);
     }
-    // sd_v on both columns: FMUL(k0,(r0+r4)); FFMA(k2,c); FFMA(k1,(r1+r3))
-    const f32x2 s = fma2(pk2(sdk.k[1], sdk.k[1]), add2(q[1], q[3]),
-                         fma2(pk2(sdk.k[2], sdk.k[2]), q[2], mul2(pk2(sdk.k[0], sdk.k[0]), add2(q[0], q[4]))));
+    const f32x2 s = scaledown_v(sdk.k, q[0], q[1], q[2], q[3], q[4]);     // both columns at once
     if (C.own) {
       const float2 r = upk(s);
       if (!EDGE || C.x1 + 1 < C.w1) *reinterpret_cast<float2 *>(R.out1) = r;
@@ -252,7 +208,7 @@ pyr_lowpass_sd_kernel(const __grid_constant__ PyrAParams P)
     mbarrier_init_fence();
     for (int i = 0; i < PA_NS; i++) {                         // the maps are kernel parameters: no descriptor fence needed
       mbarrier_expect_tx(&s_full[i], PA_IW * 4);
-      tma_load_2d(s_in + i * PA_SLOT, map, C.x0 - 8, clampi2(C.ia + i, 0, C.h - 1), &s_full[i]);
+      tma_load_2d(s_in + i * PA_SLOT, map, C.x0 - 8, clampi(C.ia + i, 0, C.h - 1), &s_full[i]);
     }
   }
   __syncwarp();
@@ -298,12 +254,12 @@ __device__ __forceinline__ void pb_scaledown(const float *src, int sx0, int sy0,
     float a[5];
     if (CLAMP) {
 #pragma unroll
-      for (int j = 0; j < 5; j++) a[j] = row[clampi2(clampi2(2 * (dx0 + c) - 2 + j, 0, sw - 1) - sx0, 0, NIN - 1)];
+      for (int j = 0; j < 5; j++) a[j] = row[clampi(clampi(2 * (dx0 + c) - 2 + j, 0, sw - 1) - sx0, 0, NIN - 1)];
     } else {
 #pragma unroll
       for (int j = 0; j < 5; j++) a[j] = row[2 * c + j];
     }
-    tmp[i] = sd_h(k, a[0], a[1], a[2], a[3], a[4]);
+    tmp[i] = scaledown_h(k.k, a[0], a[1], a[2], a[3], a[4]);
   }
   __syncthreads();
   for (int i = threadIdx.x; i < NOUT * NOUT; i += PB_THREADS) {
@@ -311,12 +267,12 @@ __device__ __forceinline__ void pb_scaledown(const float *src, int sx0, int sy0,
     float q[5];
     if (CLAMP) {
 #pragma unroll
-      for (int j = 0; j < 5; j++) q[j] = tmp[clampi2(clampi2(2 * (dy0 + r) - 2 + j, 0, sh - 1) - sy0, 0, NIN - 1) * NOUT + c];
+      for (int j = 0; j < 5; j++) q[j] = tmp[clampi(clampi(2 * (dy0 + r) - 2 + j, 0, sh - 1) - sy0, 0, NIN - 1) * NOUT + c];
     } else {
 #pragma unroll
       for (int j = 0; j < 5; j++) q[j] = tmp[(2 * r + j) * NOUT + c];
     }
-    dst[i] = sd_v(k, q[0], q[1], q[2], q[3], q[4]);
+    dst[i] = scaledown_v(k.k, q[0], q[1], q[2], q[3], q[4]);
   }
   __syncthreads();
 }
@@ -347,7 +303,7 @@ __device__ __forceinline__ void pb_chain(const PyrBParams &P, int img, float *bu
     const int sx0 = ox[STEPS], sy0 = oy[STEPS];
     for (int i = threadIdx.x; i < NS * NS; i += PB_THREADS) {
       const int r = i / NS, c = i - r * NS;
-      if (CLAMP) bufA[i] = __ldg(src + (size_t)clampi2(sy0 + r, 0, P.h[0] - 1) * P.pitch[0] + clampi2(sx0 + c, 0, P.w[0] - 1));
+      if (CLAMP) bufA[i] = __ldg(src + (size_t)clampi(sy0 + r, 0, P.h[0] - 1) * P.pitch[0] + clampi(sx0 + c, 0, P.w[0] - 1));
       else bufA[i] = __ldg(src + (size_t)(sy0 + r) * P.pitch[0] + sx0 + c);
     }
   }

@@ -1,5 +1,5 @@
-// tma.cuh -- mbarrier + TMA (cp.async.bulk.tensor) helpers and FP32-pair (f32x2) arithmetic shared by
-// the pyramid and detector kernels (sm_90a).
+// tma.cuh -- mbarrier, TMA (cp.async.bulk.tensor) and bulk-copy (cp.async.bulk) helpers shared by the pyramid,
+// detector and tensor-core matcher kernels, and the FP32-pair (f32x2) arithmetic of the pyramid and detector (sm_90a).
 #pragma once
 
 #include <cuda.h>   // CUtensorMap (type only: the encoder is resolved at run time, see make_tensor_map_2d)
@@ -17,6 +17,10 @@ __device__ __forceinline__ void mbarrier_init(uint64_t *bar, uint32_t count)
 __device__ __forceinline__ void mbarrier_expect_tx(uint64_t *bar, uint32_t bytes)
 {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_addr(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbarrier_arrive(uint64_t *bar)
+{
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_addr(bar)) : "memory");
 }
 __device__ __forceinline__ void mbarrier_wait(uint64_t *bar, uint32_t parity)
 {
@@ -37,6 +41,13 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, i
 {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
                ::"r"(smem_addr(dst)), "l"((unsigned long long)map), "r"(x), "r"(y), "r"(smem_addr(bar)) : "memory");
+}
+// `bytes` contiguous bytes from global into shared memory (both 16-byte aligned, bytes a multiple of 16); completion
+// is signalled on `bar` as transaction count.
+__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar)
+{
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_addr(dst)), "l"(src), "r"(bytes), "r"(smem_addr(bar)) : "memory");
 }
 // Tensor maps that live in global memory (written by the host before the launch): make them visible to
 // the TMA unit's descriptor cache before first use.
