@@ -17,7 +17,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "AllocSiftTempMemory", "FreeSiftTempMemory", "ExtractSift", "MatchSiftData", "FindHomography", "Extractor",
            "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host",
            "match_knn2", "MatchSiftDataRatio", "match_ratio_host", "VerifyPairs", "verify_pairs_host", "verify_stats",
-           "GEOM_MODELS"]
+           "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -73,6 +73,10 @@ def lib():
         "cs_verify_pairs_host": (ip, [vp, ip, vp, ip, vp, ip, ip, ip, fp, c.c_ulonglong, vp, vp, ip,
                                       c.POINTER(c.c_double)]),
         "cs_verify_stats": (ip, [c.POINTER(c.c_longlong)]),
+        "cs_match_knn2_guided": (ip, [vp, ip, vp, ip, ip, vp, fp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_match_guided": (ip, [vp, ip, vp, ip, ip, vp, fp, fp, fp, ip, vp, ip, c.POINTER(c.c_double)]),
+        "cs_match_guided_host": (ip, [vp, ip, vp, ip, ip, vp, fp, fp, fp, ip, vp, ip, c.POINTER(c.c_double)]),
+        "cs_match_guided_stats": (ip, [c.POINTER(c.c_ulonglong)]),
         "cs_verify_models": (ip, [vp, ip, vp, ip, vp, ip, ip, ip, fp, c.c_ulonglong, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
@@ -402,6 +406,78 @@ def verify_stats():
     (sample*3 + root, -1 if none), its inlier count, refit kept (0/1), final inlier count]."""
     out = (ctypes.c_longlong * 8)()
     _check(lib().cs_verify_stats(out), "cs_verify_stats")
+    return list(out)
+
+
+def _guided_model(M):
+    return np.ascontiguousarray(np.asarray(M, np.float64).reshape(9))
+
+
+def match_knn2_guided(s1, s2, model, M, thresh=4.0):
+    """Guided two nearest neighbours (cs_match_knn2_guided) on host record arrays: match_knn2, with row i of s1 only
+    considering the rows j of s2 that the model M (3x3, set-1 pixels to set-2 pixels, as VerifyPairs returns it)
+    admits within thresh pixels (Sampson error for "fundamental", forward transfer error for "homography").  Returns
+    (idx int32 [n1, 2], score float32 [n1, 2], ms)."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    n1, n2 = len(s1), len(s2)
+    m = _guided_model(M)
+    idx, score = np.full((n1, 2), -1, np.int32), np.zeros((n1, 2), np.float32)
+    ms = ctypes.c_double(0.0)
+    if n1 == 0 or n2 == 0:
+        _check(lib().cs_match_knn2_guided(None, 0, None, 0, _geom_model(model), _ptr(m), float(thresh), None, None,
+                                          None), "cs_match_knn2_guided")
+        return idx, score, ms.value
+    bufs = [DeviceBuffer(s1.nbytes), DeviceBuffer(s2.nbytes), DeviceBuffer(idx.nbytes), DeviceBuffer(score.nbytes)]
+    try:
+        bufs[0].upload(s1)
+        bufs[1].upload(s2)
+        _check(lib().cs_match_knn2_guided(bufs[0].ptr, n1, bufs[1].ptr, n2, _geom_model(model), _ptr(m), float(thresh),
+                                          bufs[2].ptr, bufs[3].ptr, ctypes.byref(ms)), "cs_match_knn2_guided")
+        idx = bufs[2].download(np.int32, 2 * n1).reshape(n1, 2)
+        score = bufs[3].download(np.float32, 2 * n1).reshape(n1, 2)
+    finally:
+        for b in bufs:
+            b.free()
+    return idx, score, ms.value
+
+
+def MatchSiftDataGuided(data1, data2, model, M, thresh=4.0, maxRatio=0.8, maxDistance=0.7, crossCheck=True):
+    """Guided matching (cs_match_guided, COLMAP's guided_matching): MatchSiftDataRatio restricted to the pairs the model
+    M admits within thresh pixels; model and M as VerifyPairs returns them.  Returns (pairs int32 [k, 2], ms)."""
+    n1, n2 = data1.numPts, data2.numPts
+    m = _guided_model(M)
+    room = min(n1, n2) if crossCheck else n1
+    ms = ctypes.c_double(0.0)
+    d_pairs = DeviceBuffer(max(room, 1) * 8)
+    try:
+        k = _check(lib().cs_match_guided(data1.d_data, n1, data2.d_data, n2, _geom_model(model), _ptr(m), float(thresh),
+                                         float(maxRatio), float(maxDistance), int(bool(crossCheck)),
+                                         d_pairs.ptr if room else None, room, ctypes.byref(ms)), "MatchSiftDataGuided")
+        pairs = d_pairs.download(np.int32, 2 * k).reshape(k, 2) if k else np.zeros((0, 2), np.int32)
+    finally:
+        d_pairs.free()
+    return pairs, ms.value
+
+
+def match_guided_host(s1, s2, model, M, thresh=4.0, maxRatio=0.8, maxDistance=0.7, crossCheck=True):
+    """MatchSiftDataGuided on host record arrays (cs_match_guided_host); returns (pairs[k, 2] int32, ms)."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    m = _guided_model(M)
+    pairs = np.zeros((min(len(s1), len(s2)) if crossCheck else len(s1), 2), np.int32)
+    ms = ctypes.c_double(0.0)
+    k = _check(lib().cs_match_guided_host(_ptr(s1), len(s1), _ptr(s2), len(s2), _geom_model(model), _ptr(m),
+                                          float(thresh), float(maxRatio), float(maxDistance), int(bool(crossCheck)),
+                                          _ptr(pairs), len(pairs), ctypes.byref(ms)), "cs_match_guided_host")
+    return pairs[:k].copy(), ms.value
+
+
+def guided_stats():
+    """The last guided call: [predicate evaluations, admissible pairs (exact chains run), rows of set 1 with an
+    admissible candidate, the same for set 2 in a cross-checked call (else 0)]."""
+    out = (ctypes.c_ulonglong * 4)()
+    _check(lib().cs_match_guided_stats(out), "cs_match_guided_stats")
     return list(out)
 
 

@@ -25,7 +25,8 @@ REF_DIR = os.path.join(ORACLE_DIR, "_ref")
 REF_LIB = os.path.join(REF_DIR, "libcudasift_ref.so")
 
 SOURCES = ["api.cu", "pipeline2.cu", "pyramid.cu", "pyramid2.cu", "detect.cu", "detect2.cu", "cap32.cu", "describe.cu",
-           "match.cu", "match_tc.cu", "match_mutual.cu", "match_knn.cu", "homography.cu", "geom.cu", "rank.cu", "verify.cu"]
+           "match.cu", "match_tc.cu", "match_mutual.cu", "match_knn.cu", "match_guided.cu", "homography.cu", "geom.cu",
+           "rank.cu", "verify.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared"]
 
@@ -126,6 +127,24 @@ def build_knn_oracle(force=False):
     return KNN_ORACLE_LIB
 
 
+GUIDED_ORACLE_SRC = os.path.join(ROOT, "tests", "guided_oracle.c")
+GUIDED_ORACLE_LIB = os.path.join(LIBDIR, "libguided_oracle.so")
+
+
+def build_guided_oracle(force=False):
+    """tests/guided_oracle.c: the CPU statement of guided matching (test infrastructure)."""
+    if not force and _newer(GUIDED_ORACLE_LIB, [GUIDED_ORACLE_SRC]):
+        return GUIDED_ORACLE_LIB
+    if shutil.which("gcc") is None:
+        if os.path.exists(GUIDED_ORACLE_LIB):
+            return GUIDED_ORACLE_LIB
+        raise RuntimeError("gcc not found and no prebuilt libguided_oracle.so")
+    os.makedirs(LIBDIR, exist_ok=True)
+    _run(["gcc", "-O2", "-mfma", "-ffp-contract=off", "-fPIC", "-shared", "-o", GUIDED_ORACLE_LIB, GUIDED_ORACLE_SRC,
+          "-lm", "-lpthread"])
+    return GUIDED_ORACLE_LIB
+
+
 def build_reference(force=False):
     """The unmodified reference in oracle/_ref/ (recipe: oracle/build_reference.py)."""
     sys.path.insert(0, ROOT)
@@ -158,6 +177,7 @@ def build_all(force=False, verbose=False):
     build_library(force, verbose, managed=True)
     build_demo(force, managed=True)
     build_knn_oracle(force)
+    build_guided_oracle(force)
     return out
 
 

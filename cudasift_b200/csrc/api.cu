@@ -426,16 +426,74 @@ static int knn_sync(const char *fn, DeviceCtx *c, const SiftPoint *d_s1, int n1,
   return ra ? (int)*c->h_pairTotal : 0;
 }
 
-// cs_match_ratio on device sets: the knn lists of both directions in the context's knnLists.
-static int ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
-                      const RatioArgs &ra, bool crossCheck, int mode, double *ms)
+// The knn lists of a ratio call in the context's knnLists: set 1's rows, and with crossCheck set 2's (else null).
+struct KnnLists {
+  int *idx1, *idx2;
+  float *sc1, *sc2;
+};
+static int knn_lists(DeviceCtx *c, int n1, int n2, bool crossCheck, KnnLists *l)
 {
   const size_t a = ialignup(2 * n1, 64), b = crossCheck ? ialignup(2 * n2, 64) : 0;
   int r;
   if ((r = c->knnLists.grow((2 * a + 2 * b) * sizeof(int))) < 0) return r;
-  int *idx1 = c->knnLists.as<int>(), *idx2 = crossCheck ? idx1 + 2 * a : nullptr;
-  float *sc1 = reinterpret_cast<float *>(idx1 + a), *sc2 = crossCheck ? reinterpret_cast<float *>(idx2 + b) : nullptr;
-  return knn_sync(fn, c, d1, n1, d2, n2, idx1, sc1, idx2, sc2, &ra, mode, ms);
+  l->idx1 = c->knnLists.as<int>();
+  l->idx2 = crossCheck ? l->idx1 + 2 * a : nullptr;
+  l->sc1 = reinterpret_cast<float *>(l->idx1 + a);
+  l->sc2 = crossCheck ? reinterpret_cast<float *>(l->idx2 + b) : nullptr;
+  return 0;
+}
+
+// cs_match_ratio on device sets.
+static int ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
+                      const RatioArgs &ra, bool crossCheck, int mode, double *ms)
+{
+  KnnLists l;
+  const int r = knn_lists(c, n1, n2, crossCheck, &l);
+  if (r < 0) return r;
+  return knn_sync(fn, c, d1, n1, d2, n2, l.idx1, l.sc1, l.idx2, l.sc2, &ra, mode, ms);
+}
+
+// The model and threshold of a guided call (the records and buffers are checked as for cs_match_knn2 / cs_match_ratio).
+static int guided_args(const char *fn, int model, const double *model_in, float thresh)
+{
+  if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL)
+    return arg_error(fn, "model must be 1 (homography) or 2 (fundamental)");
+  if (!model_in) return arg_error(fn, "model_in must not be NULL");
+  double s = 0.0;
+  for (int k = 0; k < 9; k++) {
+    if (!std::isfinite(model_in[k])) return arg_error(fn, "model_in must be finite");
+    s += model_in[k] * model_in[k];
+  }
+  if (!(s > 0.0 && std::isfinite(s))) return arg_error(fn, "model_in must not be all zero (and its norm must be finite)");
+  if (!std::isfinite(thresh) || thresh <= 0.0f) return arg_error(fn, "thresh must be finite and > 0");
+  return 0;
+}
+
+// cs_match_knn2_guided / cs_match_guided on device sets: the guided lists of set 1 (and with idx2 of set 2), with ra
+// then the ratio-test pairs, and the call returns their number; one synchronize.
+static int guided_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
+                       const GuidedModel &gm, int *idx1, float *sc1, int *idx2, float *sc2, const RatioArgs *ra,
+                       double *ms)
+{
+  auto enqueue = [&]() -> int {
+    int r = launch_guided_knn(*c, d1, n1, d2, n2, gm, idx1, sc1, idx2, sc2);
+    if (ra && r >= 0) r = launch_ratio_pairs(*c, idx1, sc1, n1, idx2, sc2, n2, *ra);
+    return r;
+  };
+  const int r = timed_sync(fn, c, ms, enqueue);
+  if (r < 0) return r;
+  for (int k = 0; k < 4; k++) c->guidedStats[k] = c->h_guidedStats[k];
+  return ra ? (int)*c->h_pairTotal : 0;
+}
+
+// cs_match_guided on device sets: the lists in the context's knnLists, as for cs_match_ratio.
+static int guided_ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
+                             const GuidedModel &gm, const RatioArgs &ra, bool crossCheck, double *ms)
+{
+  KnnLists l;
+  const int r = knn_lists(c, n1, n2, crossCheck, &l);
+  if (r < 0) return r;
+  return guided_sync(fn, c, d1, n1, d2, n2, gm, l.idx1, l.sc1, l.idx2, l.sc2, &ra, ms);
 }
 
 // The verifier's scratch and the pinned copy of its state.
@@ -904,17 +962,24 @@ int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore,
                     });
 }
 
+// The idx / score buffers of a knn call: [n1][2] each.
+static int knn_out_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const int *idx,
+                        const float *score)
+{
+  if (n1 > 0 && (!idx || !score)) return arg_error(fn, "n1 > 0 needs idx and score buffers");
+  const void *buf[2] = {idx, score};
+  const size_t bytes[2] = {(size_t)n1 * 2 * sizeof(int), (size_t)n1 * 2 * sizeof(float)};
+  const char *const name[2] = {"idx", "score"};
+  return check_buffers(fn, s1, n1, s2, n2, buf, bytes, name, 2);
+}
+
 int cs_match_knn2(const void *d_s1, int n1, const void *d_s2, int n2, int *d_idx, float *d_score, int mode, double *ms)
 {
   const char *fn = "cs_match_knn2";
   if (ms) *ms = 0.0;
   int r = check_sets(fn, d_s1, n1, d_s2, n2, mode);
   if (r < 0) return r;
-  if (n1 > 0 && (!d_idx || !d_score)) return arg_error(fn, "n1 > 0 needs idx and score buffers");
-  const void *buf[2] = {d_idx, d_score};
-  const size_t bytes[2] = {(size_t)n1 * 2 * sizeof(int), (size_t)n1 * 2 * sizeof(float)};
-  const char *const name[2] = {"idx", "score"};
-  if ((r = check_buffers(fn, d_s1, n1, d_s2, n2, buf, bytes, name, 2)) < 0) return r;
+  if ((r = knn_out_args(fn, d_s1, n1, d_s2, n2, d_idx, d_score)) < 0) return r;
   if (n1 == 0 || n2 == 0) return 0;
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
@@ -955,6 +1020,72 @@ int cs_match_ratio_host(const void *h_s1, int n1, const void *h_s2, int n2, floa
                       const RatioArgs ra = {maxRatio, maxDistance, pairs, room};
                       return ratio_sync(fn, c, d1, n1, d2, n2, ra, crossCheck != 0, mode, ms);
                     });
+}
+
+int cs_match_knn2_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],
+                         float thresh, int *d_idx, float *d_score, double *ms)
+{
+  const char *fn = "cs_match_knn2_guided";
+  if (ms) *ms = 0.0;
+  int r = check_sets(fn, d_s1, n1, d_s2, n2, 0);                            // mode 0: one path
+  if (r < 0) return r;
+  if ((r = guided_args(fn, model, model_in, thresh)) < 0) return r;
+  if ((r = knn_out_args(fn, d_s1, n1, d_s2, n2, d_idx, d_score)) < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  return guided_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2,
+                     guided_model(model, model_in, thresh), d_idx, d_score, nullptr, nullptr, nullptr, ms);
+}
+
+int cs_match_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],
+                    float thresh, float maxRatio, float maxDistance, int crossCheck, int *d_pairs, int maxPairs,
+                    double *ms)
+{
+  const char *fn = "cs_match_guided";
+  if (ms) *ms = 0.0;
+  int r = ratio_args(fn, d_s1, n1, d_s2, n2, maxRatio, maxDistance, d_pairs, maxPairs, 0);
+  if (r < 0) return r;
+  if ((r = guided_args(fn, model, model_in, thresh)) < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const RatioArgs ra = {maxRatio, maxDistance, (int2 *)d_pairs, maxPairs};
+  return guided_ratio_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2,
+                           guided_model(model, model_in, thresh), ra, crossCheck != 0, ms);
+}
+
+int cs_match_guided_host(const void *h_s1, int n1, const void *h_s2, int n2, int model, const double model_in[9],
+                         float thresh, float maxRatio, float maxDistance, int crossCheck, int *h_pairs, int maxPairs,
+                         double *ms)
+{
+  const char *fn = "cs_match_guided_host";
+  if (ms) *ms = 0.0;
+  int r = ratio_args(fn, h_s1, n1, h_s2, n2, maxRatio, maxDistance, h_pairs, maxPairs, 0);
+  if (r < 0) return r;
+  if ((r = guided_args(fn, model, model_in, thresh)) < 0) return r;
+  if (n1 == 0 || n2 == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const GuidedModel gm = guided_model(model, model_in, thresh);
+  const int room = maxPairs < n1 ? maxPairs : n1;                      // at most one pair per row of set 1
+  return host_pairs(c, h_s1, n1, h_s2, n2, room > 0 ? room : 1, 0, room, h_pairs,
+                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
+                      const RatioArgs ra = {maxRatio, maxDistance, pairs, room};
+                      return guided_ratio_sync(fn, c, d1, n1, d2, n2, gm, ra, crossCheck != 0, ms);
+                    });
+}
+
+int cs_match_guided_stats(unsigned long long out[4])
+{
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  for (int i = 0; i < 4; i++) out[i] = c->guidedStats[i];
+  return 0;
 }
 
 int cs_match_stats(unsigned long long out[4])

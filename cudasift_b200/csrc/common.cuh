@@ -243,6 +243,8 @@ struct DeviceCtx {
   GrowBuffer knnPartials;     // cs_match_knn2, cs_match_ratio(_host): the slices of the exact scan
   GrowBuffer verify;          // cs_verify_pairs(_host), cs_verify_models
   GrowBuffer rank;            // cs_rank_records: counters, scratch
+  // cs_match_knn2_guided, cs_match_guided(_host): coefficient records, cell grids and the sorted candidate copies
+  GrowBuffer guided;
   // the tensor path (match_tc.cu) of cs_match(_host), cs_match_mutual(_host), cs_match_knn2, cs_match_ratio(_host):
   // operand tiles, B-role copies, row norms, top-3 tables, fallback rows, and 2 x 16 words of flags used alternately
   GrowBuffer tcA, tcB, tcNorms, tcTables, tcRows, tcFlags;
@@ -256,8 +258,10 @@ struct DeviceCtx {
   unsigned int *h_tcFlags = nullptr;       // 16: the tensor path's flag area of the last call
   unsigned int *h_pairTotal = nullptr;     // the pair total of the last mutual or ratio call
   void *h_verify = nullptr;                // the state a verify call copies back
+  unsigned long long *h_guidedStats = nullptr;   // 4: the counters of the last guided call
 
   unsigned long long matchStats[4] = {0, 0, 0, 0};
+  unsigned long long guidedStats[4] = {0, 0, 0, 0};
   long long verifyStats[8] = {0, 0, 0, 0, -1, 0, 0, 0};
 
   int ensure(int d);
@@ -297,6 +301,35 @@ struct RatioArgs {
 };
 int launch_ratio_pairs(DeviceCtx &c, const int *idx1, const float *score1, int n1, const int *idx2, const float *score2,
                        int n2, const RatioArgs &ra);
+
+// The neighbour order of the exact knn searches (match_knn.cu, match_guided.cu): (s, j) comes before (t, k) when the
+// score is larger, then the index lower.  The empty entry (0, -1) comes after every positive score and before every
+// other one, so non-positive scores never enter.
+__device__ __forceinline__ bool knn_before(float s, int j, float t, int k) { return s > t || (s == t && j < k); }
+
+struct Top2 {
+  float s1, s2;
+  int j1, j2;
+};
+__device__ __forceinline__ void top2_init(Top2 &t) { t.s1 = t.s2 = 0.0f; t.j1 = t.j2 = -1; }
+__device__ __forceinline__ void top2_insert(Top2 &t, float s, int j)
+{
+  if (knn_before(s, j, t.s1, t.j1)) { t.s2 = t.s1; t.j2 = t.j1; t.s1 = s; t.j1 = j; }
+  else if (knn_before(s, j, t.s2, t.j2)) { t.s2 = s; t.j2 = j; }
+}
+
+// ---- guided matching (match_guided.cu) ------------------------------------------------------------------------------
+// The model as the predicate uses it: entries of the unit-Frobenius model rounded to float, t2 = fl(thresh * thresh).
+struct GuidedModel {
+  int model;          // CS_GEOM_HOMOGRAPHY or CS_GEOM_FUNDAMENTAL
+  float f[9];
+  float t2;
+};
+GuidedModel guided_model(int model, const double in[9], float thresh);
+// The two nearest admissible neighbours of set 1's rows in set 2 (idx1 / score1, [n1][2]); with idx2 also those of
+// set 2's rows in set 1.  Uses c.guided; the statistics reach c.h_guidedStats by the caller's synchronize.
+int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const GuidedModel &gm,
+                      int *idx1, float *score1, int *idx2, float *score2);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 size_t verify_scratch_bytes(int numPairs, int numLoops);   // device scratch of one call

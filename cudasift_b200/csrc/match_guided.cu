@@ -1,0 +1,602 @@
+// match_guided.cu -- guided matching: the two nearest neighbours of every row among the candidates a homography or a
+// fundamental matrix admits (cs_match_knn2_guided, cs_match_guided).
+//
+// Semantics: those of knn_exact (match_knn.cu: the reference's sequential 128-step FMA chain, scores > 0, the order
+// (score descending, index ascending)), restricted to the pairs (i, j) with admissible(i, j).  The predicate is the
+// FP32 statement of include/cudasift_b200.h: every operation one rounding (__fmul_rn / __fadd_rn / __fsub_rn), set-1
+// coefficients {l0, l1, l2, a} (F) or {px, py, pw} (H) and set-2 coefficients {u, v, b}, computed once per point.
+// Both directions evaluate the same function on the same operands, so admissibility never depends on the direction.
+//
+// Every score is exact, so there is nothing to certify: the work is to visit few candidates.  Per direction:
+//   1. prep     (both sets, one launch) the coefficient records, the index position of every candidate, the bounding
+//               box of those positions, max a over set 1 and max b over set 2.
+//   2. index    a cell grid over the box (cell size from the box and the count, on the device), a counting sort of
+//               the candidates into it (histogram, scan, scatter) with two sorted copies of the coefficient records:
+//               column-major and row-major, so that a cell column or a cell row is one contiguous range.
+//   3. knn      one warp per row: the cells the row's admissible region can reach (a disc for H, a strip for F, see
+//               DESIGN.md section 4 for the bounds), the predicate on their candidates, the exact chain on the
+//               admissible ones (queued so that all 32 lanes run chains together), a butterfly merge of the lanes'
+//               top two.  The order is total, so the atomic order inside a cell does not matter.
+// A row for which the bounds do not hold (coordinates beyond 1e12, |pw| < 1e-12, an extreme threshold) scans every
+// candidate: that is correct, only slower.
+#include <cfloat>
+#include <cmath>
+
+#include "common.cuh"
+
+namespace cs {
+
+#define GD_PER_CELL 2.0       // candidates per cell the grid aims at
+#define GD_MAX_SIDE 2048      // cells per grid side at most
+#define GD_SLACK 1e-6         // relative slack of the culling bounds (about 16 FP32 roundings)
+#define GD_SAFE_POS 1e12f     // the bounds hold for |xpos|, |ypos| up to this
+#define GD_SAFE_PW 1e-12f     // ... and, for H, |pw| of set-1 points at least this
+#define GD_WARPS 8            // rows per CTA of the knn kernel (one warp each)
+
+// One point of either set: its predicate coefficients (NaN when its position is not finite), its position, and its
+// index position as a candidate (NaN: not indexed, because it can never be admissible or its direction is not built).
+struct GPoint {
+  float4 coef;
+  float2 pos, key;
+};
+
+// Zeroed before every call.  Direction 0: set 1's rows against set 2's candidates; direction 1: the reverse.
+struct GHdr {
+  unsigned int bb[2][4];        // ordered keys: ~min x, ~min y, max x, max y of the index positions
+  unsigned int count[2];        // indexed candidates
+  unsigned int maxA, maxB;      // float bits: max a over set 1's indexed points, max b over set 2's
+  unsigned int unsafe[2];       // an indexed candidate outside the range where the bounds hold
+  unsigned long long stats[4];  // cs_match_guided_stats
+};
+
+struct GGrid {
+  float x0, y0, x1, y1, inv;    // the box and 1 / cell size
+  double cs;                    // 1 / inv
+  int gx, gy;
+};
+
+// One direction of a call, as the knn kernel sees it.
+struct GDir {
+  const SiftPoint *rowSift, *candSift;
+  const GPoint *rowPts;
+  int nRows, dir, capCells;
+  const float4 *coefC, *coefR;  // sorted candidate coefficients, column-major and row-major cell order
+  const int *idxC, *idxR;
+  const unsigned int *startC, *startR;   // [cells + 1]
+  int2 *idx;
+  float2 *score;
+};
+
+// float -> unsigned key with the order of the floats (finite values only)
+__device__ __forceinline__ unsigned int fkey(float f)
+{
+  const unsigned int u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float fdec(unsigned int k)
+{
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// (a0 * x + a1 * y) + a2, three roundings
+__device__ __forceinline__ float dot3(float a0, float a1, float a2, float x, float y)
+{
+  return __fadd_rn(__fadd_rn(__fmul_rn(a0, x), __fmul_rn(a1, y)), a2);
+}
+
+// The contract's predicate: c1 = set-1 coefficients, c2 = set-2 coefficients {u, v, b}.
+__device__ __forceinline__ bool admissible(int model, float4 c1, float4 c2, float t2)
+{
+  if (model == CS_GEOM_FUNDAMENTAL) {
+    const float num = dot3(c1.x, c1.y, c1.z, c2.x, c2.y);
+    return __fmul_rn(num, num) < __fmul_rn(t2, __fadd_rn(c1.w, c2.z));
+  }
+  const float dx = __fsub_rn(__fmul_rn(c2.x, c1.z), c1.x), dy = __fsub_rn(__fmul_rn(c2.y, c1.z), c1.y);
+  return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) < __fmul_rn(t2, __fmul_rn(c1.z, c1.z));
+}
+
+// The cell grid of a direction, the same in every thread that asks.  At most max(GD_MAX_SIDE^2, capCells) cells:
+// cells beyond the cap merge into the last column / row.
+__device__ GGrid grid_of(const GHdr &h, int dir, int capCells)
+{
+  GGrid g;
+  if (h.count[dir] == 0) {
+    g.x0 = g.y0 = g.x1 = g.y1 = 0.0f; g.inv = 1.0f; g.cs = 1.0; g.gx = g.gy = 1;
+    return g;
+  }
+  g.x0 = fdec(~h.bb[dir][0]); g.y0 = fdec(~h.bb[dir][1]);
+  g.x1 = fdec(h.bb[dir][2]); g.y1 = fdec(h.bb[dir][3]);
+  const double n = (double)h.count[dir];
+  const double wx = (double)g.x1 - g.x0, wy = (double)g.y1 - g.y0, w = fmax(wx, wy);
+  double cs = fmax(sqrt(wx * wy * GD_PER_CELL / n), w * GD_PER_CELL / n);
+  cs = fmax(cs, w / (GD_MAX_SIDE - 1));
+  if (!(cs > 0.0)) cs = 1.0;                                 // one position (or none)
+  g.inv = fmaxf((float)(1.0 / cs), 1e-37f);
+  g.cs = 1.0 / (double)g.inv;
+  g.gx = (int)fmin(wx / g.cs, GD_MAX_SIDE - 1.0) + 1;
+  g.gy = (int)fmin(wy / g.cs, GD_MAX_SIDE - 1.0) + 1;
+  while ((long long)g.gx * g.gy > capCells) {
+    if (g.gx >= g.gy) g.gx = (g.gx + 1) / 2;
+    else g.gy = (g.gy + 1) / 2;
+  }
+  return g;
+}
+
+// The cell coordinate of p: floor((p - p0) * inv) clamped to [0, g).  Monotone in p, which the bounds rely on.
+__device__ __forceinline__ int cell_of(float p, float p0, float inv, int g)
+{
+  return (int)fminf(fmaxf(__fmul_rn(__fsub_rn(p, p0), inv), 0.0f), (float)(g - 1));
+}
+
+// ---- 1. prep ------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256)
+guided_prep_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__restrict__ s2, int n2, GuidedModel gm,
+                   int dirs, GPoint *__restrict__ pts, GHdr *__restrict__ h)
+{
+  const float *f = gm.f;
+  const float nan = __int_as_float(0x7fffffff);
+  const int n = n1 + n2, lane = threadIdx.x & 31;
+  for (int base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
+    const int t = base + threadIdx.x;
+    bool indexed = false, safe = true;
+    float maxA = 0.0f, maxB = 0.0f;
+    const int dir = t < n1 ? 1 : 0;                          // the direction in which the point is a candidate
+    GPoint g;
+    g.key = make_float2(nan, nan);
+    if (t < n) {
+      const SiftPoint &s = dir ? s1[t] : s2[t - n1];
+      const float x = s.xpos, y = s.ypos;
+      g.pos = make_float2(x, y);
+      g.coef = make_float4(nan, nan, nan, nan);
+      g.key = make_float2(x, y);
+      indexed = isfinite(x) && isfinite(y) && (dir == 0 || dirs == 2);
+      safe = fabsf(x) <= GD_SAFE_POS && fabsf(y) <= GD_SAFE_POS;
+      if (isfinite(x) && isfinite(y)) {
+        if (dir == 1 && gm.model == CS_GEOM_FUNDAMENTAL) {
+          const float l0 = dot3(f[0], f[1], f[2], x, y), l1 = dot3(f[3], f[4], f[5], x, y);
+          const float l2 = dot3(f[6], f[7], f[8], x, y);
+          const float a = __fadd_rn(__fmul_rn(l0, l0), __fmul_rn(l1, l1));
+          g.coef = make_float4(l0, l1, l2, a);
+          if (indexed && !isnan(a)) maxA = a;
+        } else if (dir == 1) {
+          const float px = dot3(f[0], f[1], f[2], x, y), py = dot3(f[3], f[4], f[5], x, y);
+          const float pw = dot3(f[6], f[7], f[8], x, y);
+          g.coef = make_float4(px, py, pw, 0.0f);
+          // pw == 0 or a non-finite coefficient admits nothing; the predicted point is the index position
+          indexed = indexed && pw != 0.0f && isfinite(px) && isfinite(py) && isfinite(pw);
+          safe = safe && fabsf(pw) >= GD_SAFE_PW;
+          g.key = make_float2(fminf(fmaxf(__fdiv_rn(px, pw), -FLT_MAX), FLT_MAX),
+                              fminf(fmaxf(__fdiv_rn(py, pw), -FLT_MAX), FLT_MAX));
+        } else {
+          float b = 0.0f;
+          if (gm.model == CS_GEOM_FUNDAMENTAL) {
+            const float m0 = dot3(f[0], f[3], f[6], x, y), m1 = dot3(f[1], f[4], f[7], x, y);
+            b = __fadd_rn(__fmul_rn(m0, m0), __fmul_rn(m1, m1));
+            if (indexed && !isnan(b)) maxB = b;
+          }
+          g.coef = make_float4(x, y, b, 0.0f);
+        }
+      }
+      if (!indexed) g.key = make_float2(nan, nan);
+      pts[t] = g;
+    }
+    // warp-reduced atomics, per direction
+    const unsigned int FULL = 0xffffffffu;
+    for (int d = 0; d < 2; d++) {
+      const bool mine = indexed && dir == d;
+      const unsigned int cnt = __reduce_add_sync(FULL, mine ? 1u : 0u);
+      const unsigned int k0 = __reduce_max_sync(FULL, mine ? ~fkey(g.key.x) : 0u);
+      const unsigned int k1 = __reduce_max_sync(FULL, mine ? ~fkey(g.key.y) : 0u);
+      const unsigned int k2 = __reduce_max_sync(FULL, mine ? fkey(g.key.x) : 0u);
+      const unsigned int k3 = __reduce_max_sync(FULL, mine ? fkey(g.key.y) : 0u);
+      const unsigned int bad = __reduce_or_sync(FULL, (mine && !safe) ? 1u : 0u);
+      if (lane == 0 && cnt) {
+        atomicAdd(&h->count[d], cnt);
+        atomicMax(&h->bb[d][0], k0); atomicMax(&h->bb[d][1], k1);
+        atomicMax(&h->bb[d][2], k2); atomicMax(&h->bb[d][3], k3);
+        if (bad) atomicOr(&h->unsafe[d], 1u);
+      }
+    }
+    const unsigned int ma = __reduce_max_sync(FULL, __float_as_uint(maxA));   // non-negative floats: bit order
+    const unsigned int mb = __reduce_max_sync(FULL, __float_as_uint(maxB));
+    if (lane == 0 && ma) atomicMax(&h->maxA, ma);
+    if (lane == 0 && mb) atomicMax(&h->maxB, mb);
+  }
+}
+
+// ---- 2. index -----------------------------------------------------------------------------------------------------
+// Per indexed point: its cell (cx * gy + cy) and its slot inside the cell.
+__global__ void __launch_bounds__(256)
+guided_hist_kernel(const GPoint *__restrict__ pts, int n1, int n, const GHdr *__restrict__ h, unsigned int *counts0,
+                   unsigned int *counts1, int cap0, int cap1, int2 *__restrict__ cellSlot)
+{
+  __shared__ GGrid sg[2];
+  if (threadIdx.x < 2) sg[threadIdx.x] = grid_of(*h, threadIdx.x, threadIdx.x ? cap1 : cap0);
+  __syncthreads();
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+    const float2 k = pts[t].key;
+    if (isnan(k.x)) { cellSlot[t] = make_int2(-1, 0); continue; }
+    const int d = t < n1 ? 1 : 0;
+    const GGrid &g = sg[d];
+    const int cell = cell_of(k.x, g.x0, g.inv, g.gx) * g.gy + cell_of(k.y, g.y0, g.inv, g.gy);
+    cellSlot[t] = make_int2(cell, (int)atomicAdd((d ? counts1 : counts0) + cell, 1u));
+  }
+}
+
+// Exclusive scans of the cell counts: CTA 2 * dir + order, order 0 column-major (cell cx * gy + cy), order 1
+// row-major (cy * gx + cx).  start[cells] = the count.
+__global__ void __launch_bounds__(1024)
+guided_scan_kernel(const GHdr *__restrict__ h, const unsigned int *counts0, const unsigned int *counts1, int cap0,
+                   int cap1, unsigned int *start0C, unsigned int *start0R, unsigned int *start1C, unsigned int *start1R)
+{
+  __shared__ unsigned int s_w[32];
+  const int dir = blockIdx.x >> 1, order = blockIdx.x & 1;
+  const GGrid g = grid_of(*h, dir, dir ? cap1 : cap0);
+  const unsigned int *cnt = dir ? counts1 : counts0;
+  unsigned int *out = dir ? (order ? start1R : start1C) : (order ? start0R : start0C);
+  const int cells = g.gx * g.gy, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned int carry = 0;
+  for (int e0 = 0; e0 < cells; e0 += 1024) {
+    const int e = e0 + threadIdx.x;
+    unsigned int v = 0;
+    if (e < cells) v = cnt[order ? (e % g.gx) * g.gy + e / g.gx : e];
+    unsigned int inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned int t = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += t;
+    }
+    if (lane == 31) s_w[w] = inc;
+    __syncthreads();
+    if (w == 0) {
+      const unsigned int c = s_w[lane];
+      unsigned int wi = c;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned int t = __shfl_up_sync(0xffffffffu, wi, o);
+        if (lane >= o) wi += t;
+      }
+      s_w[lane] = wi - c;
+    }
+    __syncthreads();
+    if (e < cells) out[e] = carry + s_w[w] + inc - v;
+    const unsigned int chunk = __shfl_sync(0xffffffffu, s_w[31] + inc, 31);   // valid in warp 31
+    __syncthreads();
+    if (threadIdx.x == 1023) s_w[0] = chunk;
+    __syncthreads();
+    carry += s_w[0];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[cells] = carry;
+}
+
+__global__ void __launch_bounds__(256)
+guided_scatter_kernel(const GPoint *__restrict__ pts, int n1, int n, const GHdr *__restrict__ h,
+                      const int2 *__restrict__ cellSlot, int cap0, int cap1, const unsigned int *start0C,
+                      const unsigned int *start0R, const unsigned int *start1C, const unsigned int *start1R,
+                      float4 *coef0C, int *idx0C, float4 *coef0R, int *idx0R, float4 *coef1C, int *idx1C,
+                      float4 *coef1R, int *idx1R)
+{
+  __shared__ int sgx[2], sgy[2];
+  if (threadIdx.x < 2) {
+    const GGrid g = grid_of(*h, threadIdx.x, threadIdx.x ? cap1 : cap0);
+    sgx[threadIdx.x] = g.gx; sgy[threadIdx.x] = g.gy;
+  }
+  __syncthreads();
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+    const int2 cl = cellSlot[t];
+    if (cl.x < 0) continue;
+    const int d = t < n1 ? 1 : 0, gx = sgx[d], gy = sgy[d];
+    const int cx = cl.x / gy, cy = cl.x - cx * gy;
+    const unsigned int pc = (d ? start1C : start0C)[cl.x] + cl.y, pr = (d ? start1R : start0R)[cy * gx + cx] + cl.y;
+    const float4 c = pts[t].coef;
+    const int i = d ? t : t - n1;
+    (d ? coef1C : coef0C)[pc] = c; (d ? idx1C : idx0C)[pc] = i;
+    (d ? coef1R : coef0R)[pr] = c; (d ? idx1R : idx0R)[pr] = i;
+  }
+}
+
+// ---- 3. knn -------------------------------------------------------------------------------------------------------
+// The reference's score: the sequential k = 0..127 FMA chain from 0, as knn_exact_kernel computes it.
+__device__ __forceinline__ float chain_score(const float4 *a, const float4 *__restrict__ b)
+{
+  float acc = 0.0f;
+#pragma unroll 8
+  for (int d = 0; d < 32; d++) {
+    const float4 av = a[d], bv = __ldg(b + d);
+    acc = __fmaf_rn(av.x, bv.x, acc);
+    acc = __fmaf_rn(av.y, bv.y, acc);
+    acc = __fmaf_rn(av.z, bv.z, acc);
+    acc = __fmaf_rn(av.w, bv.w, acc);
+  }
+  return acc;
+}
+
+// What a row visits: nothing, every candidate, the cell box [c0, c1] x [r0, r1] (H), or the strip
+// |L0 X + L1 Y + L2| <= W (F) walked by cell columns (|L1| >= |L0|) or by cell rows.
+enum { GK_NONE, GK_ALL, GK_BOX, GK_COLS, GK_ROWS };
+struct Region {
+  int kind, c0, c1, r0, r1;
+  double L0, L1, L2, W;
+};
+
+__device__ __forceinline__ double fabs_max(float a, float b) { return fmax(fabs((double)a), fabs((double)b)); }
+
+__device__ Region row_region(const GDir &d, const GPoint &rp, const GuidedModel &gm, const GGrid &g, double kmax,
+                             bool cull)
+{
+  Region R;
+  R.kind = GK_ALL;
+  const float *f = gm.f;
+  const double E = GD_SLACK, x = rp.pos.x, y = rp.pos.y;
+  const double ucand = fabs_max(g.x0, g.x1) + fabs_max(g.y0, g.y1);   // |X| + |Y| of every candidate, at most
+  bool safe = cull && fabs(x) <= GD_SAFE_POS && fabs(y) <= GD_SAFE_POS;
+  if (gm.model == CS_GEOM_HOMOGRAPHY) {
+    double cx = x, cy = y;
+    if (d.dir == 0) {
+      const float px = rp.coef.x, py = rp.coef.y, pw = rp.coef.z;
+      if (!(pw != 0.0f && isfinite(px) && isfinite(py) && isfinite(pw))) { R.kind = GK_NONE; return R; }
+      safe = safe && fabsf(pw) >= GD_SAFE_PW;
+      cx = (double)px / pw; cy = (double)py / pw;
+    }
+    if (!safe) return R;
+    const double rad = sqrt((double)gm.t2) * (1.0 + E) + E * (1.0 + fabs(cx) + fabs(cy) + ucand);
+    const double xl = cx - rad, xh = cx + rad, yl = cy - rad, yh = cy + rad;
+    if (!(isfinite(xl) && isfinite(xh) && isfinite(yl) && isfinite(yh))) return R;
+    if (xh < g.x0 || xl > g.x1 || yh < g.y0 || yl > g.y1) { R.kind = GK_NONE; return R; }
+    R.kind = GK_BOX;
+    R.c0 = cell_of(__double2float_rd(xl), g.x0, g.inv, g.gx); R.c1 = cell_of(__double2float_ru(xh), g.x0, g.inv, g.gx);
+    R.r0 = cell_of(__double2float_rd(yl), g.y0, g.inv, g.gy); R.r1 = cell_of(__double2float_ru(yh), g.y0, g.inv, g.gy);
+    return R;
+  }
+  if (!safe) return R;
+  // The row's line in the candidates' image, in double: F x1 (direction 0) or F^T x2 (direction 1).  The FP32 num
+  // differs from x2^T F x1 by at most about 6 roundings of |x2|^T |F| |x1|; g bounds that row's |F| |x1| or
+  // |F|^T |x2|, and the candidates' |X|, |Y| are at most those of the box.
+  double own, g0, g1, g2;                                     // own: the row's a (direction 0) or b (direction 1)
+  const int s = d.dir == 0 ? 1 : 3, o = d.dir == 0 ? 3 : 1;   // strides of f along and across the line's entries
+  R.L0 = (double)f[0] * x + (double)f[s] * y + f[2 * s];
+  R.L1 = (double)f[o] * x + (double)f[o + s] * y + f[o + 2 * s];
+  R.L2 = (double)f[2 * o] * x + (double)f[2 * o + s] * y + f[2 * o + 2 * s];
+  g0 = fabs((double)f[0] * x) + fabs((double)f[s] * y) + fabs((double)f[2 * s]);
+  g1 = fabs((double)f[o] * x) + fabs((double)f[o + s] * y) + fabs((double)f[o + 2 * s]);
+  g2 = fabs((double)f[2 * o] * x) + fabs((double)f[2 * o + s] * y) + fabs((double)f[2 * o + 2 * s]);
+  own = d.dir == 0 ? rp.coef.w : rp.coef.z;
+  const double slack = E * (g0 * fabs_max(g.x0, g.x1) + g1 * fabs_max(g.y0, g.y1) + g2) + 1e-30;
+  R.W = sqrt((double)gm.t2 * (own + kmax)) * (1.0 + E) + slack;
+  if (!(isfinite(R.W) && fmax(fabs(R.L0), fabs(R.L1)) > 0.0)) return R;
+  R.kind = fabs(R.L1) >= fabs(R.L0) ? GK_COLS : GK_ROWS;
+  return R;
+}
+
+// Cell line k of a strip (a column for GK_COLS, a row for GK_ROWS): the cells [lo, hi] across it that the strip
+// can reach, or false.  a0 / a1 / n: the line's axis; b0 / b1 / m: the other axis.  A candidate in line k has its
+// coordinate along the axis in [ua, ub] (the slack covers the rounding of cell_of).
+__device__ __forceinline__ bool strip_cells(int k, int n, float a0, float a1, float b0, float b1, int m, double cs,
+                                            float inv, double P, double Q, double R2, double W, int &lo, int &hi)
+{
+  // the strip: |P * s + Q * o + R2| <= W, s along the axis, o across it, |Q| >= |P|
+  const double dl = GD_SLACK * (1.0 + fabs((double)a0) + (k + 1) * cs);
+  const double ua = k == 0 ? (double)a0 : fmax((double)a0 + k * cs - dl, (double)a0);
+  const double ub = k == n - 1 ? (double)a1 : fmin((double)a0 + (k + 1) * cs + dl, (double)a1);
+  if (ua > ub) return false;
+  const double va = -(P * ua + R2) / Q, vb = -(P * ub + R2) / Q, wv = W / fabs(Q);
+  double vl = fmin(va, vb) - wv, vh = fmax(va, vb) + wv;
+  vl -= 1e-9 * (1.0 + fabs(vl));
+  vh += 1e-9 * (1.0 + fabs(vh));
+  if (!(vh >= b0 && vl <= b1)) return false;
+  lo = cell_of(__double2float_rd(vl), b0, inv, m);
+  hi = cell_of(__double2float_ru(vh), b0, inv, m);
+  return true;
+}
+
+__global__ void __launch_bounds__(GD_WARPS * 32)
+guided_knn_kernel(GDir d, GuidedModel gm, const GHdr *__restrict__ h, bool cull, unsigned long long *stats)
+{
+  __shared__ float4 s_row[GD_WARPS][32];
+  __shared__ int s_q[GD_WARPS][64];
+  const unsigned int FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const GGrid g = grid_of(*h, d.dir, d.capCells);
+  const unsigned int nc = h->count[d.dir];
+  cull = cull && !h->unsafe[d.dir];
+  const double kmax = __uint_as_float(d.dir == 0 ? h->maxB : h->maxA);
+  unsigned long long evals = 0, hits = 0, rowsHit = 0;
+  for (int r = blockIdx.x * GD_WARPS + w; r < d.nRows; r += gridDim.x * GD_WARPS) {
+    const GPoint rp = d.rowPts[r];
+    Top2 t;
+    top2_init(t);
+    unsigned int rowHits = 0;
+    Region R;
+    R.kind = GK_NONE;
+    if (nc > 0 && isfinite(rp.pos.x) && isfinite(rp.pos.y)) R = row_region(d, rp, gm, g, kmax, cull);
+    if (R.kind != GK_NONE) {
+      s_row[w][lane] = reinterpret_cast<const float4 *>(d.rowSift[r].data)[lane];
+      __syncwarp();
+      const bool rowOrder = R.kind == GK_ROWS;
+      const float4 *coef = rowOrder ? d.coefR : d.coefC;
+      const int *cidx = rowOrder ? d.idxR : d.idxC;
+      const int lines = R.kind == GK_ALL ? 1 : R.kind == GK_BOX ? R.c1 - R.c0 + 1 : R.kind == GK_COLS ? g.gx : g.gy;
+      int qn = 0;
+      for (int base = 0; base < lines; base += 32) {
+        // this lane's line: a contiguous range [s, s + len) of the sorted candidates
+        const int k = base + lane;
+        unsigned int s = 0, len = 0;
+        if (k < lines) {
+          int lo = 0, hi = -1, line = k, across = 0;
+          if (R.kind == GK_ALL) { s = 0; len = nc; }
+          else if (R.kind == GK_BOX) { line = R.c0 + k; lo = R.r0; hi = R.r1; across = g.gy; }
+          else if (R.kind == GK_COLS) {
+            if (!strip_cells(k, g.gx, g.x0, g.x1, g.y0, g.y1, g.gy, g.cs, g.inv, R.L0, R.L1, R.L2, R.W, lo, hi)) hi = -1;
+            across = g.gy;
+          } else {
+            if (!strip_cells(k, g.gy, g.y0, g.y1, g.x0, g.x1, g.gx, g.cs, g.inv, R.L1, R.L0, R.L2, R.W, lo, hi)) hi = -1;
+            across = g.gx;
+          }
+          if (R.kind != GK_ALL && hi >= lo) {
+            const unsigned int *st = rowOrder ? d.startR : d.startC;
+            s = st[line * across + lo];
+            len = st[line * across + hi + 1] - s;
+          }
+        }
+        unsigned int inc = len;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const unsigned int v = __shfl_up_sync(FULL, inc, o);
+          if (lane >= o) inc += v;
+        }
+        const unsigned int excl = inc - len, total = __shfl_sync(FULL, inc, 31);
+        evals += total;
+        for (unsigned int k0 = 0; k0 < total; k0 += 32) {
+          const unsigned int e = k0 + lane;
+          int src = 0;                                           // the lane whose range holds e
+#pragma unroll
+          for (int step = 16; step > 0; step >>= 1)
+            if (__shfl_sync(FULL, excl, src + step) <= e) src += step;
+          const unsigned int p = __shfl_sync(FULL, s, src) + (e - __shfl_sync(FULL, excl, src));
+          bool ok = false;
+          int j = -1;
+          if (e < total) {
+            const float4 cc = coef[p];
+            ok = d.dir == 0 ? admissible(gm.model, rp.coef, cc, gm.t2) : admissible(gm.model, cc, rp.coef, gm.t2);
+            j = cidx[p];
+          }
+          const unsigned int bal = __ballot_sync(FULL, ok);
+          if (ok) s_q[w][qn + __popc(bal & ((1u << lane) - 1u))] = j;
+          qn += __popc(bal);
+          rowHits += __popc(bal);
+          __syncwarp();
+          if (qn >= 32) {                                        // every lane runs one chain
+            const int jj = s_q[w][lane];
+            top2_insert(t, chain_score(s_row[w], reinterpret_cast<const float4 *>(d.candSift[jj].data)), jj);
+            __syncwarp();
+            if (lane < qn - 32) s_q[w][lane] = s_q[w][lane + 32];
+            qn -= 32;
+            __syncwarp();
+          }
+        }
+      }
+      if (lane < qn) {
+        const int jj = s_q[w][lane];
+        top2_insert(t, chain_score(s_row[w], reinterpret_cast<const float4 *>(d.candSift[jj].data)), jj);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {                         // butterfly: disjoint halves at every step
+        Top2 u;
+        u.s1 = __shfl_xor_sync(FULL, t.s1, o); u.j1 = __shfl_xor_sync(FULL, t.j1, o);
+        u.s2 = __shfl_xor_sync(FULL, t.s2, o); u.j2 = __shfl_xor_sync(FULL, t.j2, o);
+        top2_insert(t, u.s1, u.j1);
+        top2_insert(t, u.s2, u.j2);
+      }
+      __syncwarp();                                              // s_row and s_q are reused by the next row
+    }
+    hits += rowHits;
+    rowsHit += rowHits > 0;
+    if (lane == 0) {
+      d.idx[r] = make_int2(t.j1, t.j2);
+      d.score[r] = make_float2(t.s1, t.s2);
+    }
+  }
+  if (lane == 0 && (evals || rowsHit)) {
+    atomicAdd(&stats[0], evals);
+    atomicAdd(&stats[1], hits);
+    atomicAdd(&stats[2 + d.dir], rowsHit);
+  }
+}
+
+// ---- host -----------------------------------------------------------------------------------------------------------
+GuidedModel guided_model(int model, const double in[9], float thresh)
+{
+  GuidedModel gm;
+  gm.model = model;
+  double s = 0.0;
+  for (int k = 0; k < 9; k++) s += in[k] * in[k];
+  s = std::sqrt(s);
+  for (int k = 0; k < 9; k++) gm.f[k] = (float)(in[k] / s);
+  gm.t2 = thresh * thresh;
+  return gm;
+}
+
+// Bytes of a, rounded up to 256.
+static size_t gd_align(size_t a) { return (a + 255) & ~(size_t)255; }
+
+int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const GuidedModel &gm,
+                      int *idx1, float *score1, int *idx2, float *score2)
+{
+  const int dirs = idx2 ? 2 : 1, n = n1 + n2;
+  const int cap0 = 2 * n2 + 64, cap1 = dirs == 2 ? 2 * n1 + 64 : 1;
+  // layout: header and cell counts first (one memset), then the rest
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += gd_align(bytes); return o; };
+  const size_t oHdr = take(sizeof(GHdr)), oCnt0 = take(4 * (size_t)cap0), oCnt1 = take(4 * (size_t)cap1);
+  const size_t zeroBytes = off;
+  const size_t oPts = take(sizeof(GPoint) * (size_t)n), oCell = take(sizeof(int2) * (size_t)n);
+  const size_t oS0C = take(4 * ((size_t)cap0 + 1)), oS0R = take(4 * ((size_t)cap0 + 1));
+  const size_t oS1C = take(4 * ((size_t)cap1 + 1)), oS1R = take(4 * ((size_t)cap1 + 1));
+  const size_t oC0C = take(16 * (size_t)n2), oI0C = take(4 * (size_t)n2), oC0R = take(16 * (size_t)n2),
+               oI0R = take(4 * (size_t)n2);
+  const size_t m1 = dirs == 2 ? n1 : 1;
+  const size_t oC1C = take(16 * m1), oI1C = take(4 * m1), oC1R = take(16 * m1), oI1R = take(4 * m1);
+  int r;
+  if ((r = c.guided.grow(off)) < 0) return r;
+  if (!c.h_guidedStats) CS_CUDA(cudaMallocHost((void **)&c.h_guidedStats, 4 * sizeof(unsigned long long)));
+  char *b = c.guided.as<char>();
+  GHdr *h = reinterpret_cast<GHdr *>(b + oHdr);
+  unsigned int *cnt0 = reinterpret_cast<unsigned int *>(b + oCnt0), *cnt1 = reinterpret_cast<unsigned int *>(b + oCnt1);
+  GPoint *pts = reinterpret_cast<GPoint *>(b + oPts);
+  int2 *cell = reinterpret_cast<int2 *>(b + oCell);
+  auto u32 = [&](size_t o) { return reinterpret_cast<unsigned int *>(b + o); };
+  auto f4 = [&](size_t o) { return reinterpret_cast<float4 *>(b + o); };
+  auto i32 = [&](size_t o) { return reinterpret_cast<int *>(b + o); };
+  cudaStream_t st = c.stream;
+  cudaEvent_t *tev = match_timing_events();
+  if (tev) cudaEventRecord(tev[0], st);
+  CS_CUDA(cudaMemsetAsync(b, 0, zeroBytes, st));
+  const int blocks = idivup(n, 256) < 4 * c.sms ? idivup(n, 256) : 4 * c.sms;
+  guided_prep_kernel<<<blocks, 256, 0, st>>>(s1, n1, s2, n2, gm, dirs, pts, h);
+  if (tev) cudaEventRecord(tev[1], st);
+  guided_hist_kernel<<<blocks, 256, 0, st>>>(pts, n1, n, h, cnt0, cnt1, cap0, cap1, cell);
+  guided_scan_kernel<<<2 * dirs, 1024, 0, st>>>(h, cnt0, cnt1, cap0, cap1, u32(oS0C), u32(oS0R), u32(oS1C), u32(oS1R));
+  guided_scatter_kernel<<<blocks, 256, 0, st>>>(pts, n1, n, h, cell, cap0, cap1, u32(oS0C), u32(oS0R), u32(oS1C),
+                                                u32(oS1R), f4(oC0C), i32(oI0C), f4(oC0R), i32(oI0R), f4(oC1C),
+                                                i32(oI1C), f4(oC1R), i32(oI1R));
+  count_launch(4);
+  CS_CUDA(cudaGetLastError());
+  if (tev) cudaEventRecord(tev[2], st);
+  // the bounds of DESIGN.md section 4 hold for thresholds whose square is a normal float well inside the range
+  const bool cull = gm.t2 >= 1e-6f && gm.t2 <= 1e12f;
+  for (int dir = 0; dir < dirs; dir++) {
+    GDir d;
+    d.dir = dir;
+    d.rowSift = dir ? s2 : s1;
+    d.candSift = dir ? s1 : s2;
+    d.rowPts = dir ? pts + n1 : pts;
+    d.nRows = dir ? n2 : n1;
+    d.capCells = dir ? cap1 : cap0;
+    d.coefC = f4(dir ? oC1C : oC0C); d.idxC = i32(dir ? oI1C : oI0C);
+    d.coefR = f4(dir ? oC1R : oC0R); d.idxR = i32(dir ? oI1R : oI0R);
+    d.startC = u32(dir ? oS1C : oS0C); d.startR = u32(dir ? oS1R : oS0R);
+    d.idx = reinterpret_cast<int2 *>(dir ? idx2 : idx1);
+    d.score = reinterpret_cast<float2 *>(dir ? score2 : score1);
+    const int rowBlocks = idivup(d.nRows, GD_WARPS) < 16 * c.sms ? idivup(d.nRows, GD_WARPS) : 16 * c.sms;
+    guided_knn_kernel<<<rowBlocks, GD_WARPS * 32, 0, st>>>(d, gm, h, cull, h->stats);
+    count_launch();
+    CS_CUDA(cudaGetLastError());
+    if (tev) cudaEventRecord(tev[3 + dir], st);
+  }
+  CS_CUDA(cudaMemcpyAsync(c.h_guidedStats, h->stats, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (tev) {
+    static const char *const names[] = {"prep", "index", "knn", "reverse-knn"};
+    cudaEventSynchronize(tev[2 + dirs]);
+    fprintf(stderr, "guided timing %dx%d [us]:", n1, n2);
+    for (int i = 0; i < 2 + dirs; i++) {
+      float ms = 0.0f;
+      cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
+      fprintf(stderr, " %s %.1f", names[i], 1000.0f * ms);
+    }
+    fprintf(stderr, "\n");
+  }
+  return 0;
+}
+
+}  // namespace cs

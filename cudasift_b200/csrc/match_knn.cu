@@ -22,21 +22,6 @@ namespace cs {
 #define KX_MIN_STEPS 4      // candidate steps per slice at least (128 candidates)
 #define KX_MAX_SLICES 128
 
-// (s, j) comes before (t, k) in the neighbour order: larger score first, then the lower index.  The empty entry
-// (0, -1) comes after every positive score and before every other one, so non-positive scores never enter.
-__device__ __forceinline__ bool knn_before(float s, int j, float t, int k) { return s > t || (s == t && j < k); }
-
-struct Top2 {
-  float s1, s2;
-  int j1, j2;
-};
-__device__ __forceinline__ void top2_init(Top2 &t) { t.s1 = t.s2 = 0.0f; t.j1 = t.j2 = -1; }
-__device__ __forceinline__ void top2_insert(Top2 &t, float s, int j)
-{
-  if (knn_before(s, j, t.s1, t.j1)) { t.s2 = t.s1; t.j2 = t.j1; t.s1 = s; t.j1 = j; }
-  else if (knn_before(s, j, t.s2, t.j2)) { t.s2 = s; t.j2 = j; }
-}
-
 // rows == nullptr: rows [32*b, +32) of set 1, b grid-strided; otherwise entries [32*b, +32) of the row list (*nrows
 // entries).  gate != nullptr: *gate != 0 scans every row, else only the listed ones (the tensor path's fallback).
 // part == nullptr: one slice, the results go to idx / score; otherwise slice y writes part[(y * rowsCap + entry)].

@@ -175,6 +175,42 @@ int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, con
  * count, [6] = 1 if the refit was kept, [7] = the final inlier count. */
 int cs_verify_stats(long long out[8]);
 
+/* Guided matching (COLMAP's guided_matching): the two nearest neighbours and the ratio test restricted to the pairs a
+ * model admits.  cs_match_knn2_guided has the semantics of cs_match_knn2 (the reference's score, only scores > 0, the
+ * order score descending then index ascending, a missing neighbour is (-1, 0.0f)), except that row i of set 1 only
+ * considers the j with admissible(i, j).  cs_match_guided is cs_match_ratio on those lists (same rule, cross-check
+ * and pair order) and returns the pair count; with crossCheck, row j of set 2 considers the i with admissible(i, j),
+ * the same function of (i, j) evaluated on the same operands in the same order.
+ * - model: CS_GEOM_HOMOGRAPHY or CS_GEOM_FUNDAMENTAL; model_in: row-major 3x3 mapping set-1 pixels to set-2 pixels (what
+ *   cs_verify_pairs writes).  It is scaled to unit Frobenius norm in double (the sum of squares in index order) and
+ *   each entry rounded to float, f0..f8; t2 = fl(thresh * thresh).
+ * - The predicate, every operation one IEEE FP32 rounding in the stated order, no contraction; (x, y) = set-1 xpos,
+ *   ypos and (u, v) = set-2 xpos, ypos:
+ *     F: l0 = (f0*x + f1*y) + f2, l1 = (f3*x + f4*y) + f5, l2 = (f6*x + f7*y) + f8, a = l0*l0 + l1*l1;
+ *        m0 = (f0*u + f3*v) + f6, m1 = (f1*u + f4*v) + f7, b = m0*m0 + m1*m1; num = (l0*u + l1*v) + l2;
+ *        admissible iff num*num < t2 * (a + b)  (the Sampson error below thresh).
+ *     H: px = (f0*x + f1*y) + f2, py = (f3*x + f4*y) + f5, pw = (f6*x + f7*y) + f8; dx = u*pw - px, dy = v*pw - py;
+ *        admissible iff dx*dx + dy*dy < t2 * (pw*pw)  (the forward transfer error below thresh; pw == 0 admits
+ *        nothing).
+ *   A record with a non-finite xpos or ypos is admissible with nothing.  cs_verify_pairs scores on normalised
+ *   coordinates, so a pair within about 1e-4 px of thresh can be an inlier there and not admissible here.
+ * - CS_E_ARG, before any CUDA call: the argument rules of cs_match_knn2 / cs_match_ratio except mode (there is one
+ *   path), a model outside {1, 2}, a NULL model_in, a non-finite or all-zero model_in (or one whose norm is not
+ *   finite), and thresh not finite or <= 0.  n1 == 0 or n2 == 0 returns 0 and writes nothing.  The records are only
+ *   read.  The call synchronises once, at the end; the lists of cs_match_guided live in per-device scratch. */
+int cs_match_knn2_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],
+                         float thresh, int *d_idx, float *d_score, double *ms);
+int cs_match_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],
+                    float thresh, float maxRatio, float maxDistance, int crossCheck, int *d_pairs, int maxPairs,
+                    double *ms);
+/* Same with host record arrays and a host pairs buffer. */
+int cs_match_guided_host(const void *h_s1, int n1, const void *h_s2, int n2, int model, const double model_in[9],
+                         float thresh, float maxRatio, float maxDistance, int crossCheck, int *h_pairs, int maxPairs,
+                         double *ms);
+/* the last guided call on this thread's device: [0] predicate evaluations, [1] admissible pairs (= exact chains run),
+ * [2] rows of set 1 with at least one admissible candidate, [3] the same for set 2 in a cross-checked call, else 0 */
+int cs_match_guided_stats(unsigned long long out[4]);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
