@@ -17,7 +17,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "AllocSiftTempMemory", "FreeSiftTempMemory", "ExtractSift", "MatchSiftData", "FindHomography", "Extractor",
            "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host",
            "match_knn2", "MatchSiftDataRatio", "match_ratio_host", "VerifyPairs", "verify_pairs_host", "verify_stats",
-           "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats"]
+           "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
+           "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -78,6 +79,12 @@ def lib():
         "cs_match_guided_host": (ip, [vp, ip, vp, ip, ip, vp, fp, fp, fp, ip, vp, ip, c.POINTER(c.c_double)]),
         "cs_match_guided_stats": (ip, [c.POINTER(c.c_ulonglong)]),
         "cs_verify_models": (ip, [vp, ip, vp, ip, vp, ip, ip, ip, fp, c.c_ulonglong, vp, vp, vp]),
+        "cs_verify_essential": (ip, [vp, ip, vp, ip, vp, ip, vp, vp, ip, fp, c.c_ulonglong, vp, vp, vp, vp, ip,
+                                     c.POINTER(c.c_double)]),
+        "cs_verify_essential_host": (ip, [vp, ip, vp, ip, vp, ip, vp, vp, ip, fp, c.c_ulonglong, vp, vp, vp, vp, ip,
+                                          c.POINTER(c.c_double)]),
+        "cs_verify_essential_stats": (ip, [c.POINTER(c.c_longlong)]),
+        "cs_verify_essential_models": (ip, [vp, ip, vp, ip, vp, ip, vp, vp, ip, fp, c.c_ulonglong, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -407,6 +414,73 @@ def verify_stats():
     out = (ctypes.c_longlong * 8)()
     _check(lib().cs_verify_stats(out), "cs_verify_stats")
     return list(out)
+
+
+def _intrinsics(K):
+    return np.ascontiguousarray(np.asarray(K, np.float64).reshape(9))
+
+
+def VerifyEssential(data1, data2, pairs, K1, K2, numLoops=4096, thresh=4.0, seed=0):
+    """Calibrated verification on the device (cs_verify_essential): RANSAC for the essential matrix with the 5-point
+    solver, then the relative pose.  pairs as for VerifyPairs; K1, K2 the 3x3 pinhole intrinsics of the two images
+    (skew allowed); thresh in pixels (the Sampson error of F = K2^-T E K1^-1, as VerifyPairs' "fundamental").
+    Returns (E 3x3, R 3x3, t [3], inliers int32 [m, 2] in input order, ms): E at unit Frobenius norm, X2 = R X1 + t
+    with |t| = 1."""
+    pairs = _pair_array(pairs)
+    k = len(pairs)
+    E, R, t = np.zeros(9), np.zeros(9), np.zeros(3)
+    k1, k2 = _intrinsics(K1), _intrinsics(K2)
+    ms = ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(k, 1) * 8), DeviceBuffer(max(k, 1) * 8)]
+    try:
+        if k:
+            bufs[0].upload(pairs)
+        m = _check(lib().cs_verify_essential(data1.d_data, data1.numPts, data2.d_data, data2.numPts,
+                                             bufs[0].ptr if k else None, k, _ptr(k1), _ptr(k2), int(numLoops),
+                                             float(thresh), int(seed), _ptr(E), _ptr(R), _ptr(t),
+                                             bufs[1].ptr if k else None, k, ctypes.byref(ms)), "VerifyEssential")
+        inliers = bufs[1].download(np.int32, 2 * m).reshape(m, 2) if m else np.zeros((0, 2), np.int32)
+    finally:
+        for b in bufs:
+            b.free()
+    return E.reshape(3, 3), R.reshape(3, 3), t, inliers, ms.value
+
+
+def verify_essential_host(s1, s2, pairs, K1, K2, numLoops=4096, thresh=4.0, seed=0):
+    """VerifyEssential on host record arrays (cs_verify_essential_host); returns (E, R, t, inliers [m, 2] int32, ms)."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    pairs = _pair_array(pairs)
+    E, R, t = np.zeros(9), np.zeros(9), np.zeros(3)
+    k1, k2 = _intrinsics(K1), _intrinsics(K2)
+    inliers = np.zeros((len(pairs), 2), np.int32)
+    ms = ctypes.c_double(0.0)
+    m = _check(lib().cs_verify_essential_host(_ptr(s1), len(s1), _ptr(s2), len(s2), _ptr(pairs), len(pairs), _ptr(k1),
+                                              _ptr(k2), int(numLoops), float(thresh), int(seed), _ptr(E), _ptr(R),
+                                              _ptr(t), _ptr(inliers), len(inliers), ctypes.byref(ms)),
+               "cs_verify_essential_host")
+    return E.reshape(3, 3), R.reshape(3, 3), t, inliers[:m].copy(), ms.value
+
+
+def essential_stats():
+    """The last essential call: the eight fields of verify_stats (winning slot sample*10 + root), then the final
+    inliers in front of the chosen pose and the runner-up pose candidate's count."""
+    out = (ctypes.c_longlong * 10)()
+    _check(lib().cs_verify_essential_stats(out), "cs_verify_essential_stats")
+    return list(out)
+
+
+def essential_to_fundamental(E, K1, K2):
+    """F = K2^-T E K1^-1 at unit Frobenius norm with its largest-magnitude entry positive: the pixel model of an
+    essential matrix, for MatchSiftDataGuided(..., "fundamental", F)."""
+    E = np.asarray(E, np.float64).reshape(3, 3)
+    K1, K2 = np.asarray(K1, np.float64).reshape(3, 3), np.asarray(K2, np.float64).reshape(3, 3)
+    F = np.linalg.inv(K2).T @ E @ np.linalg.inv(K1)
+    n = np.linalg.norm(F)
+    if not n > 0:
+        return np.zeros((3, 3))
+    flat = F.reshape(-1)
+    return F * (np.copysign(1.0, flat[int(np.argmax(np.abs(flat)))]) / n)
 
 
 def _guided_model(M):

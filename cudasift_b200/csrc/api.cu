@@ -496,11 +496,39 @@ static int guided_ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, 
   return guided_sync(fn, c, d1, n1, d2, n2, gm, l.idx1, l.sc1, l.idx2, l.sc2, &ra, ms);
 }
 
-// The verifier's scratch and the pinned copy of its state.
-static int verify_buffers(DeviceCtx *c, int numPairs, int numLoops)
+// The intrinsics of an essential call: a finite row-major pinhole K (skew allowed) with K[3] = K[6] = K[7] = 0,
+// K[8] = 1, K[0] > 0 and K[4] > 0.
+static int check_intrinsics(const char *fn, const double *K, const char *name)
+{
+  char msg[96];
+  snprintf(msg, sizeof msg, "%s must be a finite pinhole matrix (K[3] = K[6] = K[7] = 0, K[8] = 1, K[0] > 0, K[4] > 0)",
+           name);
+  if (!K) return arg_error(fn, msg);
+  for (int k = 0; k < 9; k++)
+    if (!std::isfinite(K[k])) return arg_error(fn, msg);
+  if (K[3] != 0.0 || K[6] != 0.0 || K[7] != 0.0 || K[8] != 1.0 || !(K[0] > 0.0) || !(K[4] > 0.0)) return arg_error(fn, msg);
+  return 0;
+}
+
+// The arguments of cs_verify_essential*: those of cs_verify_pairs except model, the intrinsics and the three outputs.
+static int essential_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                          const double *K1, const double *K2, int numLoops, float thresh, const double *E,
+                          const double *R, const double *t, const void *inliers, int maxInliers)
 {
   int r;
-  if ((r = c->verify.grow(verify_scratch_bytes(numPairs, numLoops))) < 0) return r;
+  if (!E || !R || !t) return arg_error(fn, "E_out, R_out and t_out must not be NULL");
+  if ((r = verify_args(fn, s1, n1, s2, n2, pairs, numPairs, CS_GEOM_FUNDAMENTAL, numLoops, thresh, E, inliers,
+                       maxInliers)) < 0)
+    return r;
+  if ((r = check_intrinsics(fn, K1, "K1")) < 0) return r;
+  return check_intrinsics(fn, K2, "K2");
+}
+
+// The verifier's scratch and the pinned copy of its state.
+static int verify_buffers(DeviceCtx *c, int numPairs, int numLoops, int model)
+{
+  int r;
+  if ((r = c->verify.grow(verify_scratch_bytes(numPairs, numLoops, model))) < 0) return r;
   if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
   return 0;
 }
@@ -511,13 +539,36 @@ static int verify_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1
                        double model_out[9], int *inliers, int maxInliers, double *ms)
 {
   int r;
-  if ((r = verify_buffers(c, numPairs, numLoops)) < 0) return r;
+  if ((r = verify_buffers(c, numPairs, numLoops, model)) < 0) return r;
   auto enqueue = [&] {
-    return launch_verify(d1, n1, d2, n2, pairs, numPairs, model, numLoops, thresh, seed, inliers, maxInliers,
+    return launch_verify(d1, n1, d2, n2, pairs, numPairs, model, nullptr, numLoops, thresh, seed, inliers, maxInliers,
                          c->verify.p, c->h_verify, true, c->stream);
   };
   if ((r = timed_sync(fn, c, ms, enqueue)) < 0) return r;
   return verify_result(c->h_verify, numPairs, model_out, c->verifyStats);
+}
+
+// cs_verify_essential on device sets and a device pair list: as verify_sync, with the pose.
+static int essential_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
+                          const int *pairs, int numPairs, const VerifyCalib &cal, int numLoops, float thresh,
+                          unsigned long long seed, double E[9], double R[9], double t[3], int *inliers, int maxInliers,
+                          double *ms)
+{
+  int r;
+  if ((r = verify_buffers(c, numPairs, numLoops, VERIFY_ESSENTIAL)) < 0) return r;
+  auto enqueue = [&] {
+    return launch_verify(d1, n1, d2, n2, pairs, numPairs, VERIFY_ESSENTIAL, &cal, numLoops, thresh, seed, inliers,
+                         maxInliers, c->verify.p, c->h_verify, true, c->stream);
+  };
+  if ((r = timed_sync(fn, c, ms, enqueue)) < 0) return r;
+  return verify_essential_result(c->h_verify, numPairs, E, R, t, c->essentialStats);
+}
+
+static VerifyCalib verify_calib(const double K1[9], const double K2[9])
+{
+  VerifyCalib cal;
+  for (int k = 0; k < 9; k++) { cal.K1[k] = K1[k]; cal.K2[k] = K2[k]; }
+  return cal;
 }
 
 }  // namespace cs
@@ -1161,12 +1212,96 @@ int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const i
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  if ((r = verify_buffers(c, numPairs, numLoops)) < 0) return r;
-  r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, numLoops, thresh,
-                    seed, nullptr, 0, c->verify.p, c->h_verify, false, c->stream);
+  if ((r = verify_buffers(c, numPairs, numLoops, model)) < 0) return r;
+  r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, nullptr, numLoops,
+                    thresh, seed, nullptr, 0, c->verify.p, c->h_verify, false, c->stream);
   if (r < 0) return r;
-  return verify_models_to_host(c->verify.p, c->h_verify, numPairs, numLoops, model, h_models, h_counts, h_norm,
+  return verify_models_to_host(c->verify.p, c->h_verify, numPairs, numLoops, model, nullptr, h_models, h_counts, h_norm,
                                c->stream);
+}
+
+static void essential_zero(double E[9], double R[9], double t[3])
+{
+  for (int k = 0; k < 9; k++) E[k] = R[k] = 0.0;
+  for (int k = 0; k < 3; k++) t[k] = 0.0;
+}
+
+int cs_verify_essential(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs,
+                        const double K1[9], const double K2[9], int numLoops, float thresh, unsigned long long seed,
+                        double E_out[9], double R_out[9], double t_out[3], int *d_inliers, int maxInliers, double *ms)
+{
+  const char *fn = "cs_verify_essential";
+  if (ms) *ms = 0.0;
+  int r = essential_args(fn, d_s1, n1, d_s2, n2, d_pairs, numPairs, K1, K2, numLoops, thresh, E_out, R_out, t_out,
+                         d_inliers, maxInliers);
+  if (r < 0) return r;
+  essential_zero(E_out, R_out, t_out);
+  if (numPairs == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  return essential_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs,
+                        verify_calib(K1, K2), numLoops, thresh, seed, E_out, R_out, t_out, d_inliers, maxInliers, ms);
+}
+
+int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs,
+                             const double K1[9], const double K2[9], int numLoops, float thresh,
+                             unsigned long long seed, double E_out[9], double R_out[9], double t_out[3],
+                             int *h_inliers, int maxInliers, double *ms)
+{
+  const char *fn = "cs_verify_essential_host";
+  if (ms) *ms = 0.0;
+  int r = essential_args(fn, h_s1, n1, h_s2, n2, h_pairs, numPairs, K1, K2, numLoops, thresh, E_out, R_out, t_out,
+                         h_inliers, maxInliers);
+  if (r < 0) return r;
+  essential_zero(E_out, R_out, t_out);
+  if (numPairs == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const VerifyCalib cal = verify_calib(K1, K2);
+  const int room = maxInliers < numPairs ? maxInliers : numPairs;     // no more inliers can exist
+  // the pair buffer holds the input pairs, then room inliers
+  return host_pairs(c, h_s1, n1, h_s2, n2, (size_t)numPairs + room, numPairs, room, h_inliers,
+                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
+                      CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice,
+                                              c->stream));
+                      return essential_sync(fn, c, d1, n1, d2, n2, reinterpret_cast<int *>(pairs), numPairs, cal,
+                                            numLoops, thresh, seed, E_out, R_out, t_out,
+                                            reinterpret_cast<int *>(pairs + numPairs), room, ms);
+                    });
+}
+
+int cs_verify_essential_stats(long long out[10])
+{
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  for (int i = 0; i < 10; i++) out[i] = c->essentialStats[i];
+  return 0;
+}
+
+int cs_verify_essential_models(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs,
+                               const double K1[9], const double K2[9], int numLoops, float thresh,
+                               unsigned long long seed, double *h_models, int *h_counts, double h_norm[5])
+{
+  const char *fn = "cs_verify_essential_models";
+  double dummy[12];
+  int r = essential_args(fn, d_s1, n1, d_s2, n2, d_pairs, numPairs, K1, K2, numLoops, thresh, dummy, dummy, dummy,
+                         nullptr, 0);
+  if (r < 0) return r;
+  if (!h_models || !h_counts || !h_norm) return arg_error(fn, "NULL output array");
+  if (numPairs == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const VerifyCalib cal = verify_calib(K1, K2);
+  if ((r = verify_buffers(c, numPairs, numLoops, VERIFY_ESSENTIAL)) < 0) return r;
+  r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, VERIFY_ESSENTIAL, &cal,
+                    numLoops, thresh, seed, nullptr, 0, c->verify.p, c->h_verify, false, c->stream);
+  if (r < 0) return r;
+  return verify_models_to_host(c->verify.p, c->h_verify, numPairs, numLoops, VERIFY_ESSENTIAL, &cal, h_models, h_counts,
+                               h_norm, c->stream);
 }
 
 // ---- stage-level entry points ----

@@ -241,7 +241,7 @@ struct DeviceCtx {
   GrowBuffer knnLists;        // cs_match_ratio(_host): both directions' neighbour lists
   GrowBuffer pairScratch;     // cs_match_mutual(_host), cs_match_ratio(_host): ballot words, CTA counts, the total
   GrowBuffer knnPartials;     // cs_match_knn2, cs_match_ratio(_host): the slices of the exact scan
-  GrowBuffer verify;          // cs_verify_pairs(_host), cs_verify_models
+  GrowBuffer verify;          // cs_verify_pairs(_host), cs_verify_models, cs_verify_essential(_host, _models)
   GrowBuffer rank;            // cs_rank_records: counters, scratch
   // cs_match_knn2_guided, cs_match_guided(_host): coefficient records, cell grids and the sorted candidate copies
   GrowBuffer guided;
@@ -263,6 +263,7 @@ struct DeviceCtx {
   unsigned long long matchStats[4] = {0, 0, 0, 0};
   unsigned long long guidedStats[4] = {0, 0, 0, 0};
   long long verifyStats[8] = {0, 0, 0, 0, -1, 0, 0, 0};
+  long long essentialStats[10] = {0, 0, 0, 0, -1, 0, 0, 0, 0, 0};
 
   int ensure(int d);
   Pipeline *get_pipe(int w, int h, int oct, bool up, float *arena, int *err);
@@ -332,17 +333,28 @@ int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint
                       int *idx1, float *score1, int *idx2, float *score2);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
-size_t verify_scratch_bytes(int numPairs, int numLoops);   // device scratch of one call
+// The model id launch_verify uses for cs_verify_essential (not a model value of the public cs_verify_pairs).
+#define VERIFY_ESSENTIAL 3
+// The intrinsics of an essential call (row-major, checked by the caller).
+struct VerifyCalib {
+  double K1[9], K2[9];
+};
+size_t verify_scratch_bytes(int numPairs, int numLoops, int model);   // device scratch of one call
 size_t verify_result_bytes();                              // the state copied to the host (pinned) at the end
-// steps 1-4, and with full also 5-8 (arg-max, refit, output); ends with the state copy to h_state on the stream
+// steps 1-4, and with full also 5-8 (arg-max, refit, output); ends with the state copy to h_state on the stream.
+// cal is read for VERIFY_ESSENTIAL only.
 int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *pairs, int numPairs, int model,
-                  int numLoops, float thresh, unsigned long long seed, int *inliers, int maxInliers, void *scratch,
-                  void *h_state, bool full, cudaStream_t st);
+                  const VerifyCalib *cal, int numLoops, float thresh, unsigned long long seed, int *inliers,
+                  int maxInliers, void *scratch, void *h_state, bool full, cudaStream_t st);
 // after a full launch and a synchronize: the inlier count, the pixel model and the statistics
 int verify_result(const void *h_state, int numPairs, double model_out[9], long long stats[8]);
-// after a launch without full: every slot's pixel model, count and the normalisation (synchronizes); returns numValid
+// the same after a full VERIFY_ESSENTIAL launch: E, R, t and the ten statistics of cs_verify_essential_stats
+int verify_essential_result(const void *h_state, int numPairs, double E[9], double R[9], double t[3],
+                            long long stats[10]);
+// after a launch without full: every slot's pixel model (E for VERIFY_ESSENTIAL), count and the normalisation
+// (synchronizes); returns numValid
 int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
-                          double *h_models, int *h_counts, double h_norm[5], cudaStream_t st);
+                          const VerifyCalib *cal, double *h_models, int *h_counts, double h_norm[5], cudaStream_t st);
 
 inline int idivup(int a, int b) { return (a + b - 1) / b; }
 inline int ialignup(int a, int b) { return (a % b != 0) ? (a - a % b + b) : a; }

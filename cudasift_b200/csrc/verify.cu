@@ -43,6 +43,9 @@ struct VerifyState {
   float thr2;                     // (s * thresh)^2
   int numValid;
   int total;                      // final inlier count
+  // cs_verify_essential: model holds E; the chosen pose; [0] its points in front, [1] the runner-up candidate's count
+  double R[9], t[3];
+  long long pose[2];
 };
 
 // ---- shared helpers (host and device) --------------------------------------------------------------------------------
@@ -133,10 +136,10 @@ __host__ __device__ inline void vp_jacobi(double (&a)[N][N], double (&v)[N][N])
 }
 
 // ---- device routines ----------------------------------------------------------------------------------------------
-// Null space of an M x 9 system (M = 7 or 8): Gaussian elimination with partial pivoting on columns 0..M-1, then back
+// Null space of an M x 9 system (M = 5, 7 or 8): Gaussian elimination with partial pivoting on columns 0..M-1, then back
 // substitution for each free column f = M..8 (x_f = 1, the other free entries 0).  false when a pivot is below VP_EPS.
 template <int M>
-__device__ bool vp_nullspace(double (&A)[M][9], double (&N)[9 - M][9])
+__host__ __device__ bool vp_nullspace(double (&A)[M][9], double (&N)[9 - M][9])
 {
 #pragma unroll
   for (int c = 0; c < M; c++) {
@@ -524,8 +527,10 @@ vp_score_kernel(const float4 *__restrict__ un, const double *__restrict__ models
   if (live && cnt) atomicAdd(&counts[slot], cnt);
 }
 
+// perSample: slots per sample (3 for F and H, 10 for E); a sample counts when its first slot is live
 __global__ void __launch_bounds__(256)
-vp_argmax_kernel(const double *__restrict__ models, const unsigned int *__restrict__ counts, int numSlots, VerifyState *st)
+vp_argmax_kernel(const double *__restrict__ models, const unsigned int *__restrict__ counts, int numSlots, int perSample,
+                 VerifyState *st)
 {
   const int slot = blockIdx.x * 256 + threadIdx.x;
   const bool live = slot < numSlots && !isnan(models[(size_t)slot * 9]);
@@ -536,7 +541,7 @@ vp_argmax_kernel(const double *__restrict__ models, const unsigned int *__restri
     key = t > key ? t : key;
   }
   const unsigned int nm = __popc(__ballot_sync(0xffffffffu, live));
-  const unsigned int ns = __popc(__ballot_sync(0xffffffffu, live && slot % 3 == 0));
+  const unsigned int ns = __popc(__ballot_sync(0xffffffffu, live && slot % perSample == 0));
   if ((threadIdx.x & 31) == 0) {
     if (key) atomicMax(&st->best, key);
     if (nm) atomicAdd(&st->models, (unsigned long long)nm);
@@ -558,6 +563,65 @@ __device__ int vp_block_count(int v, int *s_cnt)
   return t;
 }
 
+// The final mask of a refit CTA: ballot words per 32 points of the FP32 test with m (all clear when m is null), then
+// counts per VP_ROWS points; returns the total in every thread.
+__device__ int vp_final_mask(const float *m, const float4 *__restrict__ un, int n, float thr2, bool homography,
+                             unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts, int *s_cnt)
+{
+  const int lane = threadIdx.x & 31;
+  if (m) {
+    for (int k0 = 0; k0 < n; k0 += VP_REFIT_T) {
+      const int k = k0 + threadIdx.x;
+      const bool in = k < n && vp_inlier(m, un[k], thr2, homography);
+      const unsigned int bal = __ballot_sync(0xffffffffu, in);
+      if (lane == 0 && k < n) masks[k >> 5] = bal;
+    }
+  } else {
+    for (int k = threadIdx.x; k < (n + 31) / 32; k += VP_REFIT_T) masks[k] = 0u;
+  }
+  __syncthreads();
+  const int words = (n + 31) / 32;
+  int tot = 0;
+  for (int b = threadIdx.x; b * (VP_ROWS / 32) < words; b += VP_REFIT_T) {
+    unsigned int t = 0;
+    for (int q = b * (VP_ROWS / 32); q < min(words, (b + 1) * (VP_ROWS / 32)); q++) t += __popc(masks[q]);
+    blockCounts[b] = t;
+    tot += (int)t;
+  }
+  return vp_block_count(tot, s_cnt);
+}
+
+// The 45 upper-triangle entries of one thread's normal-matrix partial sums, summed over each warp into s_nm[warp].
+__device__ __forceinline__ void vp_warp_normal(const double (&acc)[45], double (*s_nm)[45])
+{
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int e = 0; e < 45; e++) {
+    double v = acc[e];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) s_nm[w][e] = v;
+  }
+}
+
+// The symmetric 9x9 normal matrix from the warps' sums (in warp order), and its smallest eigenvector (Jacobi).
+__device__ void vp_smallest_eigvec(const double (*s_nm)[45], double (&f)[9])
+{
+  double A[9][9], V[9][9];
+  int e = 0;
+  for (int i = 0; i < 9; i++)
+    for (int j = i; j < 9; j++) {
+      double t = 0.0;
+      for (int q = 0; q < VP_REFIT_T / 32; q++) t += s_nm[q][e];
+      A[i][j] = A[j][i] = t;
+      e++;
+    }
+  vp_jacobi<9>(A, V);
+  int lo = 0;
+  for (int i = 1; i < 9; i++) if (A[i][i] < A[lo][lo]) lo = i;
+  for (int i = 0; i < 9; i++) f[i] = V[i][lo];
+}
+
 __global__ void __launch_bounds__(VP_REFIT_T)
 vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, const double *__restrict__ models, int model,
                 unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts, VerifyState *st)
@@ -568,17 +632,16 @@ vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, co
   __shared__ int s_cnt[VP_REFIT_T / 32];
   __shared__ int s_refit;
   const int n = st->numValid;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const bool homography = model == CS_GEOM_HOMOGRAPHY;
   const unsigned long long key = st->best;
   const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
   const float thr2 = st->thr2;
   const int best = key ? (int)~(unsigned int)key : -1;
   int cnt0 = 0, cntR = 0, kept = 0;
+  float m[9];
   if (best >= 0) {
     if (threadIdx.x < 9) { s_m[0][threadIdx.x] = models[(size_t)best * 9 + threadIdx.x]; s_f[threadIdx.x] = (float)s_m[0][threadIdx.x]; }
     __syncthreads();
-    float m[9];
     for (int k = 0; k < 9; k++) m[k] = s_f[k];
     // the normal matrix (upper triangle, 45 entries) of the minimal model's inliers
     double acc[45];
@@ -610,31 +673,13 @@ vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, co
           for (int j = i; j < 9; j++) acc[e++] += r[q][i] * r[q][j];
       }
     }
-#pragma unroll
-    for (int e = 0; e < 45; e++) {
-      double v = acc[e];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-      if (lane == 0) s_nm[w][e] = v;
-    }
+    vp_warp_normal(acc, s_nm);
     cnt0 = vp_block_count(c, s_cnt);
     if (threadIdx.x == 0) {
       s_refit = 0;
       if (cnt0 >= (homography ? 4 : 8)) {
-        double A[9][9], V[9][9];
-        int e = 0;
-        for (int i = 0; i < 9; i++)
-          for (int j = i; j < 9; j++) {
-            double t = 0.0;
-            for (int q = 0; q < VP_REFIT_T / 32; q++) t += s_nm[q][e];
-            A[i][j] = A[j][i] = t;
-            e++;
-          }
-        vp_jacobi<9>(A, V);
-        int lo = 0;
-        for (int i = 1; i < 9; i++) if (A[i][i] < A[lo][lo]) lo = i;
         double f[9];
-        for (int i = 0; i < 9; i++) f[i] = V[i][lo];
+        vp_smallest_eigvec(s_nm, f);
         if (!homography) {             // rank 2: F (I - v v^T), v the right singular vector of the smallest singular value
           double B[3][3], W[3][3];
           for (int i = 0; i < 3; i++)
@@ -661,26 +706,8 @@ vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, co
     }
     if (!kept)
       for (int k = 0; k < 9; k++) m[k] = s_f[k];
-    // the final mask: ballot words per 32 points, then counts per VP_ROWS points
-    for (int k0 = 0; k0 < n; k0 += VP_REFIT_T) {
-      const int k = k0 + threadIdx.x;
-      const bool in = k < n && vp_inlier(m, un[k], thr2, homography);
-      const unsigned int bal = __ballot_sync(0xffffffffu, in);
-      if (lane == 0 && k < n) masks[k >> 5] = bal;
-    }
-  } else {
-    for (int k = threadIdx.x; k < (n + 31) / 32; k += VP_REFIT_T) masks[k] = 0u;
   }
-  __syncthreads();
-  const int words = (n + 31) / 32;
-  int tot = 0;
-  for (int b = threadIdx.x; b * (VP_ROWS / 32) < words; b += VP_REFIT_T) {
-    unsigned int t = 0;
-    for (int q = b * (VP_ROWS / 32); q < min(words, (b + 1) * (VP_ROWS / 32)); q++) t += __popc(masks[q]);
-    blockCounts[b] = t;
-    tot += (int)t;
-  }
-  tot = vp_block_count(tot, s_cnt);
+  const int tot = vp_final_mask(best >= 0 ? m : nullptr, un, n, thr2, homography, masks, blockCounts, s_cnt);
   if (threadIdx.x == 0) {
     double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     if (best >= 0) vp_denormalise(kept ? s_m[1] : s_m[0], model, c1x, c1y, c2x, c2y, s, out);
@@ -708,17 +735,597 @@ vp_write_kernel(const int2 *__restrict__ pairs, const int *__restrict__ orig, co
   if (bit && pos < (unsigned int)maxInliers) inliers[pos] = pairs[orig[blockIdx.x * VP_ROWS + threadIdx.x]];
 }
 
+// ---- the calibrated path (cs_verify_essential) -------------------------------------------------------------------------
+// Steps 1-3 and 5, 6, 8 are the kernels above (scoring with the F test on Fn = T2^-T K2^-T E K1^-1 T1^-1); step 4 is
+// vp_hyp5_kernel (10 slots per sample) and step 7 vp_refit_e_kernel.  The rules are stated in cudasift_b200.h at
+// cs_verify_essential.
+#define VP_E_SLOTS 10            // models per sample of the 5-point solver
+#define VP_E_PIVOT 1e-12         // Gauss-Jordan pivot, relative to the largest |entry| of the 10x20 matrix
+#define VP_E_LEAD 1e-12          // leading coefficients of the degree-10 polynomial at or below this (relative) are dropped
+#define VP_E_REM 1e-14           // a Sturm remainder at or below this (relative to its dividend) ends the sequence
+#define VP_E_WIDTH 1e-10         // root refinement: bisection down to this width (relative to max(1, |end|))
+#define VP_E_STACK 64            // isolation intervals pending at once
+#define VP_E_PARALLEL 1e-12      // cheirality: rays whose sin^2(angle) is at or below this are not in front
+
+// calibrated coordinates x^ = K^-1 (x, y, 1) of an upper-triangular K: y^ = (y - K[5]) / K[4], x^ = (x - K[2] - K[1] y^) / K[0]
+__host__ __device__ inline void vp_calibrate(const double *K, double x, double y, double &cx, double &cy)
+{
+  cy = (y - K[5]) / K[4];
+  cx = (x - K[2] - K[1] * cy) / K[0];
+}
+
+// G = K^-1 T^-1 (normalised coordinates -> calibrated) and its inverse TK = T K, T the normalisation u = s (x - c)
+__host__ __device__ inline void vp_calib_maps(const double *K, double cx, double cy, double s, double *G, double *TK)
+{
+  const double Ki[9] = {1.0 / K[0], -K[1] / (K[0] * K[4]), (K[1] * K[5] - K[2] * K[4]) / (K[0] * K[4]),
+                        0, 1.0 / K[4], -K[5] / K[4], 0, 0, 1};
+  const double Ti[9] = {1.0 / s, 0, cx, 0, 1.0 / s, cy, 0, 0, 1};
+  const double T[9] = {s, 0, -s * cx, 0, s, -s * cy, 0, 0, 1};
+  vp_mul33(Ki, Ti, G);
+  vp_mul33(T, K, TK);
+}
+
+// out = A^T M B: Fn = G2^T E G1, and back E = TK2^T Fn TK1
+__host__ __device__ inline void vp_sandwich(const double *A, const double *M, const double *B, double *out)
+{
+  double At[9], t[9];
+  for (int r = 0; r < 3; r++)
+    for (int c = 0; c < 3; c++) At[3 * r + c] = A[3 * c + r];
+  vp_mul33(At, M, t);
+  vp_mul33(t, B, out);
+}
+
+// F's output scaling: unit Frobenius norm, the largest-magnitude entry (the first of equals) positive; false for zero
+__host__ __device__ inline bool vp_unit_sign(double *m)
+{
+  double n = 0.0;
+  int big = 0;
+  for (int k = 0; k < 9; k++) {
+    n += m[k] * m[k];
+    if (fabs(m[k]) > fabs(m[big])) big = k;
+  }
+  if (!(n > 0.0) || !isfinite(n)) return false;
+  const double f = (m[big] < 0 ? -1.0 : 1.0) / sqrt(n);
+  for (int k = 0; k < 9; k++) m[k] *= f;
+  return true;
+}
+
+// Polynomials of degree <= 3 in (x, y, z): 20 coefficients in Nister's monomial order
+//   x^3 y^3 x^2y xy^2 x^2z x^2 y^2z y^2 xyz xy | xz^2 xz x yz^2 yz y z^3 z^2 z 1
+__host__ __device__ constexpr int vp_mono(int a, int b, int c)      // the slot of x^a y^b z^c
+{
+  return a == 3 ? 0 : b == 3 ? 1 : (a == 2 && b == 1) ? 2 : (a == 1 && b == 2) ? 3 : (a == 2 && c == 1) ? 4
+       : a == 2 ? 5 : (b == 2 && c == 1) ? 6 : b == 2 ? 7 : (a == 1 && b == 1 && c == 1) ? 8 : (a == 1 && b == 1) ? 9
+       : (a == 1 && c == 2) ? 10 : (a == 1 && c == 1) ? 11 : a == 1 ? 12 : (b == 1 && c == 2) ? 13
+       : (b == 1 && c == 1) ? 14 : b == 1 ? 15 : c == 3 ? 16 : c == 2 ? 17 : c == 1 ? 18 : 19;
+}
+__host__ __device__ constexpr int vp_mono_exp(int k)                // the exponents of slot k, a << 4 | b << 2 | c
+{
+  return k == 0 ? 0x30 : k == 1 ? 0x0C : k == 2 ? 0x24 : k == 3 ? 0x18 : k == 4 ? 0x21 : k == 5 ? 0x20 : k == 6 ? 0x09
+       : k == 7 ? 0x08 : k == 8 ? 0x15 : k == 9 ? 0x14 : k == 10 ? 0x12 : k == 11 ? 0x11 : k == 12 ? 0x10
+       : k == 13 ? 0x06 : k == 14 ? 0x05 : k == 15 ? 0x04 : k == 16 ? 0x03 : k == 17 ? 0x02 : k == 18 ? 0x01 : 0x00;
+}
+__host__ __device__ constexpr int vp_mono_deg(int e) { return (e >> 4) + ((e >> 2) & 3) + (e & 3); }
+
+// r += sign * p * q for p of degree <= DP and q of degree <= DQ, DP + DQ <= 3
+template <int DP, int DQ>
+__host__ __device__ __forceinline__ void vp_pmul(const double *p, const double *q, double sign, double *r)
+{
+#pragma unroll
+  for (int i = 0; i < 20; i++) {
+    if (vp_mono_deg(vp_mono_exp(i)) > DP) continue;
+#pragma unroll
+    for (int j = 0; j < 20; j++) {
+      if (vp_mono_deg(vp_mono_exp(j)) > DQ) continue;
+      const int a = vp_mono_exp(i), b = vp_mono_exp(j);
+      r[vp_mono((a >> 4) + (b >> 4), ((a >> 2) & 3) + ((b >> 2) & 3), (a & 3) + (b & 3))] += sign * (p[i] * q[j]);
+    }
+  }
+}
+
+// out[0..na+nb] = a * b, coefficients in ascending powers
+__host__ __device__ inline void vp_upoly_mul(const double *a, int na, const double *b, int nb, double *out)
+{
+  for (int k = 0; k <= na + nb; k++) out[k] = 0.0;
+  for (int i = 0; i <= na; i++)
+    for (int j = 0; j <= nb; j++) out[i + j] += a[i] * b[j];
+}
+
+__host__ __device__ inline double vp_horner(const double *c, int n, double x)
+{
+  double v = c[n];
+  for (int k = n - 1; k >= 0; k--) v = v * x + c[k];
+  return v;
+}
+
+// sign changes of the Sturm sequence at x (zeros skipped)
+__host__ __device__ inline int vp_sturm_changes(const double (*S)[11], const int *deg, int ns, double x)
+{
+  int changes = 0;
+  double prev = 0.0;
+  for (int k = 0; k < ns; k++) {
+    const double v = vp_horner(S[k], deg[k], x);
+    if (v == 0.0) continue;
+    if (prev != 0.0 && (v > 0.0) != (prev > 0.0)) changes++;
+    prev = v;
+  }
+  return changes;
+}
+
+// The distinct real roots of c[0] + c[1] z + ... + c[n] z^n (n <= 10), ascending; returns their number.  Leading
+// coefficients at or below VP_E_LEAD of the largest |c| are dropped.  Sturm sequence of the monic p: S0 = p,
+// S1 = p' / n, S(k+1) = -rem(S(k-1), S(k)) scaled by 1 / |its leading coefficient|, ending when a remainder's largest
+// |coefficient| is at or below VP_E_REM of its dividend's (leading remainder coefficients at or below VP_E_REM of that
+// largest one are dropped).  Isolation: (-B, B], B = 1 + 2 max_k |a(n-k)|^(1/k) of the monic p (Fujiwara), bisected
+// at midpoints, left half first, halves without a root dropped; an interval is refined as one root when it holds one
+// root, is narrower than VP_E_WIDTH * max(1, |lo|, |hi|), or more than VP_E_STACK - 2 other intervals are pending
+// (the stack then has no room for two halves).  Refinement: bisection to that width, on the sign of p
+// when p changes sign across the interval, else on the Sturm count (the left half while it holds a root); then up to
+// three Newton steps from the midpoint, each kept only while it stays inside the interval.
+__host__ __device__ inline int vp_real_roots(const double *c, int n, double *roots)
+{
+  double cm = 0.0;
+  for (int k = 0; k <= n; k++) cm = fmax(cm, fabs(c[k]));
+  if (!(cm > 0.0) || !isfinite(cm)) return 0;
+  while (n > 0 && !(fabs(c[n]) > VP_E_LEAD * cm)) n--;
+  if (n == 0) return 0;
+  double S[11][11];
+  int deg[11];
+  for (int k = 0; k <= n; k++) S[0][k] = c[k] / c[n];
+  for (int k = 0; k < n; k++) S[1][k] = (k + 1) * S[0][k + 1] / n;
+  deg[0] = n; deg[1] = n - 1;
+  int ns = 2;
+  while (deg[ns - 1] > 0) {
+    const double *a = S[ns - 2], *b = S[ns - 1];
+    const int da = deg[ns - 2], db = deg[ns - 1];
+    double r[11], am = 0.0;
+    for (int k = 0; k <= da; k++) { r[k] = a[k]; am = fmax(am, fabs(a[k])); }
+    for (int k = da - db; k >= 0; k--) {
+      const double q = r[db + k] / b[db];
+      for (int j = 0; j <= db; j++) r[j + k] -= q * b[j];
+    }
+    double rm = 0.0;
+    for (int k = 0; k < db; k++) rm = fmax(rm, fabs(r[k]));
+    if (!(rm > VP_E_REM * am)) break;
+    int dr = db - 1;
+    while (dr > 0 && !(fabs(r[dr]) > VP_E_REM * rm)) dr--;
+    const double f = -1.0 / fabs(r[dr]);
+    for (int k = 0; k <= dr; k++) S[ns][k] = r[k] * f;
+    deg[ns++] = dr;
+  }
+  double B = 0.0;                      // Fujiwara's bound 2 max |a(n-k)|^(1/k), plus 1
+  for (int k = 1; k <= n; k++) B = fmax(B, pow(fabs(S[0][n - k]), 1.0 / k));
+  B = 2.0 * B + 1.0;
+  struct Iv { double lo, hi; int vlo, vhi; };
+  Iv stack[VP_E_STACK];
+  int top = 0, nr = 0;
+  stack[top++] = {-B, B, vp_sturm_changes(S, deg, ns, -B), vp_sturm_changes(S, deg, ns, B)};
+  while (top > 0 && nr < n) {
+    Iv iv = stack[--top];
+    const int cnt = iv.vlo - iv.vhi;
+    if (cnt <= 0) continue;
+    const double tol = VP_E_WIDTH * fmax(1.0, fmax(fabs(iv.lo), fabs(iv.hi)));
+    if (cnt > 1 && iv.hi - iv.lo > tol && top + 2 <= VP_E_STACK) {
+      const double mid = 0.5 * (iv.lo + iv.hi);
+      const int vm = vp_sturm_changes(S, deg, ns, mid);
+      if (vm > iv.vhi) stack[top++] = {mid, iv.hi, vm, iv.vhi};      // only halves that hold a root are kept
+      if (iv.vlo > vm) stack[top++] = {iv.lo, mid, iv.vlo, vm};
+      continue;
+    }
+    double lo = iv.lo, hi = iv.hi, plo = vp_horner(S[0], n, lo);
+    int vlo = iv.vlo;
+    const double phi = vp_horner(S[0], n, hi);
+    const bool change = plo != 0.0 && phi != 0.0 && (plo > 0.0) != (phi > 0.0);
+    for (int it = 0; it < 200 && hi - lo > VP_E_WIDTH * fmax(1.0, fmax(fabs(lo), fabs(hi))); it++) {
+      const double mid = 0.5 * (lo + hi);
+      if (change) {
+        const double pm = vp_horner(S[0], n, mid);
+        if (pm == 0.0) { lo = hi = mid; break; }
+        if ((pm > 0.0) == (plo > 0.0)) { lo = mid; plo = pm; } else { hi = mid; }
+      } else {
+        const int vm = vp_sturm_changes(S, deg, ns, mid);
+        if (vlo - vm >= 1) hi = mid; else { lo = mid; vlo = vm; }
+      }
+    }
+    double x = 0.5 * (lo + hi);
+    for (int it = 0; it < 3; it++) {
+      double p = S[0][n], d = 0.0;
+      for (int k = n - 1; k >= 0; k--) { d = d * x + p; p = p * x + S[0][k]; }
+      if (d == 0.0) break;
+      const double y = x - p / d;
+      if (!(y >= lo && y <= hi)) break;
+      x = y;
+    }
+    roots[nr++] = x;
+  }
+  return nr;
+}
+
+// The solver's basis of the null space: modified Gram-Schmidt of N0..N3 in order (q0..q3), then the fixed orthogonal
+// mix X, Y, Z, W = (q0 - q1 + q2 - q3, q0 + q1 - q2 - q3, q0 - q1 - q2 + q3, q0 + q1 + q2 + q3) / 2, so that no
+// chart coordinate is one entry of E (E22, the coordinate of N3, vanishes for small rotations).  false when a vector
+// vanishes.
+__host__ __device__ inline bool vp_e_basis(double (&N)[4][9])
+{
+  for (int i = 0; i < 4; i++) {
+    for (int j = 0; j < i; j++) {
+      double d = 0.0;
+      for (int k = 0; k < 9; k++) d += N[i][k] * N[j][k];
+      for (int k = 0; k < 9; k++) N[i][k] -= d * N[j][k];
+    }
+    double n = 0.0;
+    for (int k = 0; k < 9; k++) n += N[i][k] * N[i][k];
+    if (!(n > 0.0)) return false;
+    const double f = 1.0 / sqrt(n);
+    for (int k = 0; k < 9; k++) N[i][k] *= f;
+  }
+  for (int k = 0; k < 9; k++) {
+    const double q0 = N[0][k], q1 = N[1][k], q2 = N[2][k], q3 = N[3][k];
+    N[0][k] = 0.5 * (q0 - q1 + q2 - q3);
+    N[1][k] = 0.5 * (q0 + q1 - q2 - q3);
+    N[2][k] = 0.5 * (q0 - q1 - q2 + q3);
+    N[3][k] = 0.5 * (q0 + q1 + q2 + q3);
+  }
+  return true;
+}
+
+// Nister's 5-point solver on the basis N (vp_e_basis) of the null space: E = x N0 + y N1 + z N2 + N3.  Row 0 of
+// the 10 x 20 system is det E = 0, rows 1 + 3i + j entry (i, j) of 2 E E^T E - tr(E E^T) E = 0.  Gauss-Jordan with
+// partial pivoting (the first of equal magnitudes) reduces its first ten columns to the identity; a pivot at or below
+// VP_E_PIVOT of the largest |entry| makes the sample degenerate.  Rows 4 - z row 5, 6 - z row 7 and 8 - z row 9 are
+// [x y 1] times cubic, cubic, quartic polynomials in z; the determinant of that 3 x 3 polynomial matrix (cofactor
+// expansion along its first row) is the degree-10 polynomial, its real roots ascending (vp_real_roots).  For each root,
+// (x, y, 1) is the cross product of two rows of the evaluated matrix -- the pair (0,1), (0,2), (1,2) whose third
+// component has the largest magnitude, the first of equals -- divided by that component (the root is skipped when it
+// is 0).  Returns the number of solutions in E[].
+__host__ __device__ inline int vp_five_point(const double (&N)[4][9], double (*E)[9])
+{
+  double P[9][20];                     // the entries of E, degree-1 polynomials
+  for (int k = 0; k < 9; k++) {
+    for (int j = 0; j < 20; j++) P[k][j] = 0.0;
+    P[k][vp_mono(1, 0, 0)] = N[0][k]; P[k][vp_mono(0, 1, 0)] = N[1][k];
+    P[k][vp_mono(0, 0, 1)] = N[2][k]; P[k][vp_mono(0, 0, 0)] = N[3][k];
+  }
+  double C[10][20];
+  for (int r = 0; r < 10; r++)
+    for (int j = 0; j < 20; j++) C[r][j] = 0.0;
+  {                                    // det E, cofactors along row 0
+    double cof[20];
+    const int cols[3][2] = {{1, 2}, {0, 2}, {0, 1}};
+    const double sg[3] = {1.0, -1.0, 1.0};
+    for (int c = 0; c < 3; c++) {
+      for (int j = 0; j < 20; j++) cof[j] = 0.0;
+      const int a = cols[c][0], b = cols[c][1];
+      vp_pmul<1, 1>(P[3 + a], P[6 + b], 1.0, cof);
+      vp_pmul<1, 1>(P[3 + b], P[6 + a], -1.0, cof);
+      vp_pmul<2, 1>(cof, P[c], sg[c], C[0]);
+    }
+  }
+  {                                    // 2 E E^T E - tr(E E^T) E
+    double Q[3][3][20];
+    for (int i = 0; i < 3; i++)
+      for (int l = i; l < 3; l++) {
+        for (int j = 0; j < 20; j++) Q[i][l][j] = 0.0;
+        for (int k = 0; k < 3; k++) vp_pmul<1, 1>(P[3 * i + k], P[3 * l + k], 2.0, Q[i][l]);
+      }
+    double tr[20];
+    for (int j = 0; j < 20; j++) tr[j] = 0.5 * (Q[0][0][j] + Q[1][1][j] + Q[2][2][j]);
+    for (int i = 0; i < 3; i++) {
+      for (int l = 0; l < i; l++)
+        for (int j = 0; j < 20; j++) Q[i][l][j] = Q[l][i][j];
+      for (int j = 0; j < 20; j++) Q[i][i][j] -= tr[j];
+    }
+    for (int i = 0; i < 3; i++)
+      for (int j = 0; j < 3; j++)
+        for (int l = 0; l < 3; l++) vp_pmul<2, 1>(Q[i][l], P[3 * l + j], 1.0, C[1 + 3 * i + j]);
+  }
+  double amax = 0.0;
+  for (int r = 0; r < 10; r++)
+    for (int j = 0; j < 20; j++) amax = fmax(amax, fabs(C[r][j]));
+  if (!(amax > 0.0) || !isfinite(amax)) return 0;
+#pragma unroll 1
+  for (int c = 0; c < 10; c++) {
+    int p = c;
+    for (int r = c + 1; r < 10; r++)
+      if (fabs(C[r][c]) > fabs(C[p][c])) p = r;
+    if (!(fabs(C[p][c]) > VP_E_PIVOT * amax)) return 0;
+    if (p != c)
+      for (int j = c; j < 20; j++) { const double t = C[c][j]; C[c][j] = C[p][j]; C[p][j] = t; }
+    const double inv = 1.0 / C[c][c];
+    for (int j = c + 1; j < 20; j++) C[c][j] *= inv;
+    C[c][c] = 1.0;
+    for (int r = 0; r < 10; r++) {
+      if (r == c) continue;
+      const double f = C[r][c];
+      for (int j = c + 1; j < 20; j++) C[r][j] -= f * C[c][j];
+      C[r][c] = 0.0;
+    }
+  }
+  // row a - z row b over the last ten columns: x (xz^2 xz x), y (yz^2 yz y) and 1 (z^3 z^2 z 1), ascending in z
+  double Bx[3][4], By[3][4], B1[3][5];
+  for (int q = 0; q < 3; q++) {
+    const double *a = C[4 + 2 * q] + 10, *b = C[5 + 2 * q] + 10;
+    Bx[q][0] = a[2]; Bx[q][1] = a[1] - b[2]; Bx[q][2] = a[0] - b[1]; Bx[q][3] = -b[0];
+    By[q][0] = a[5]; By[q][1] = a[4] - b[5]; By[q][2] = a[3] - b[4]; By[q][3] = -b[3];
+    B1[q][0] = a[9]; B1[q][1] = a[8] - b[9]; B1[q][2] = a[7] - b[8]; B1[q][3] = a[6] - b[7]; B1[q][4] = -b[6];
+  }
+  double t1[8], t2[8], m1[8], m2[8], m3[7], d[11], e[11];
+  vp_upoly_mul(By[1], 3, B1[2], 4, t1);          // ly m1 - l1 my
+  vp_upoly_mul(B1[1], 4, By[2], 3, t2);
+  for (int k = 0; k < 8; k++) m1[k] = t1[k] - t2[k];
+  vp_upoly_mul(Bx[1], 3, B1[2], 4, t1);          // lx m1 - l1 mx
+  vp_upoly_mul(B1[1], 4, Bx[2], 3, t2);
+  for (int k = 0; k < 8; k++) m2[k] = t1[k] - t2[k];
+  vp_upoly_mul(Bx[1], 3, By[2], 3, t1);          // lx my - ly mx
+  vp_upoly_mul(By[1], 3, Bx[2], 3, t2);
+  for (int k = 0; k < 7; k++) m3[k] = t1[k] - t2[k];
+  vp_upoly_mul(Bx[0], 3, m1, 7, d);
+  vp_upoly_mul(By[0], 3, m2, 7, e);
+  for (int k = 0; k < 11; k++) d[k] -= e[k];
+  vp_upoly_mul(B1[0], 4, m3, 6, e);
+  for (int k = 0; k < 11; k++) d[k] += e[k];
+  double z[10];
+  const int nz = vp_real_roots(d, 10, z);
+  int ns = 0;
+  for (int k = 0; k < nz; k++) {
+    double M[3][3];
+    for (int q = 0; q < 3; q++) {
+      M[q][0] = vp_horner(Bx[q], 3, z[k]); M[q][1] = vp_horner(By[q], 3, z[k]); M[q][2] = vp_horner(B1[q], 4, z[k]);
+    }
+    const int pr[3][2] = {{0, 1}, {0, 2}, {1, 2}};
+    double v[3] = {0.0, 0.0, 0.0};
+    for (int q = 0; q < 3; q++) {
+      const double *a = M[pr[q][0]], *b = M[pr[q][1]];
+      const double w[3] = {a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]};
+      if (fabs(w[2]) > fabs(v[2])) { v[0] = w[0]; v[1] = w[1]; v[2] = w[2]; }
+    }
+    if (!(v[2] != 0.0)) continue;
+    const double x = v[0] / v[2], y = v[1] / v[2];
+    for (int j = 0; j < 9; j++) E[ns][j] = x * N[0][j] + y * N[1][j] + z[k] * N[2][j] + N[3][j];
+    ns++;
+  }
+  return ns;
+}
+
+// one thread per sample: 5 draws, calibrated rows, the null space, the 5-point solver; slot sample*10 + r holds the
+// r-th solution as Fn = G2^T E G1 (unit norm), NaN when empty
+__global__ void __launch_bounds__(VP_HYP_T)
+vp_hyp5_kernel(const float4 *__restrict__ xy, int numLoops, unsigned long long seed, VerifyCalib cal,
+               double *__restrict__ models, unsigned int *__restrict__ counts, const VerifyState *st)
+{
+  const int smp = blockIdx.x * VP_HYP_T + threadIdx.x;
+  if (smp >= numLoops) return;
+  double *slot = models + (size_t)smp * 9 * VP_E_SLOTS;
+  for (int r = 0; r < VP_E_SLOTS; r++) { slot[9 * r] = CUDART_NAN; counts[VP_E_SLOTS * smp + r] = 0; }
+  const int n = st->numValid;
+  const double s = st->s;
+  if (!(s > 0.0)) return;
+  int idx[5];
+  if (n < 5 || !vp_draw<5>(seed, smp, n, idx)) return;
+  double A[5][9], N[4][9];
+#pragma unroll
+  for (int i = 0; i < 5; i++) {
+    const float4 p = xy[idx[i]];
+    double x, y, X, Y;
+    vp_calibrate(cal.K1, p.x, p.y, x, y);
+    vp_calibrate(cal.K2, p.z, p.w, X, Y);
+    const double r[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
+#pragma unroll
+    for (int j = 0; j < 9; j++) A[i][j] = r[j];
+  }
+  if (!vp_nullspace<5>(A, N) || !vp_e_basis(N)) return;
+  double E[VP_E_SLOTS][9];
+  const int ne = vp_five_point(N, E);
+  double G1[9], G2[9], TK[9];
+  vp_calib_maps(cal.K1, st->c1x, st->c1y, s, G1, TK);
+  vp_calib_maps(cal.K2, st->c2x, st->c2y, s, G2, TK);
+  int r = 0;
+  for (int k = 0; k < ne; k++) {
+    double fn[9];
+    vp_sandwich(G2, E[k], G1, fn);
+    if (vp_store_unit(slot + 9 * r, fn)) r++;
+  }
+}
+
+// The nearest essential matrix through the eigenvectors of E^T E (Jacobi; descending eigenvalues, the lower index first
+// on ties): v1, v2 of the two largest, sigma_i = sqrt(lambda_i), u_i = E v_i / sigma_i, Ep = u1 v1^T + u2 v2^T and
+// the right-handed bases u3 = u1 x u2, v3 = v1 x v2 (u[i], v[i] the vectors).  false when sigma2 is not > 0.
+__host__ __device__ inline bool vp_essential_project(const double *E, double *Ep, double (&u)[3][3], double (&v)[3][3])
+{
+  double B[3][3], W[3][3];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) B[i][j] = E[i] * E[j] + E[3 + i] * E[3 + j] + E[6 + i] * E[6 + j];
+  vp_jacobi<3>(B, W);
+  int o[3] = {0, 1, 2};
+  for (int i = 1; i < 3; i++)
+    for (int j = i; j > 0 && B[o[j]][o[j]] > B[o[j - 1]][o[j - 1]]; j--) { const int t = o[j]; o[j] = o[j - 1]; o[j - 1] = t; }
+  for (int a = 0; a < 2; a++) {
+    const double sg = sqrt(fmax(B[o[a]][o[a]], 0.0));
+    if (!(sg > 0.0) || !isfinite(sg)) return false;
+    for (int i = 0; i < 3; i++) v[a][i] = W[i][o[a]];
+    for (int i = 0; i < 3; i++) u[a][i] = (E[3 * i] * v[a][0] + E[3 * i + 1] * v[a][1] + E[3 * i + 2] * v[a][2]) / sg;
+  }
+  u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];
+  u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
+  u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+  v[2][0] = v[0][1] * v[1][2] - v[0][2] * v[1][1];
+  v[2][1] = v[0][2] * v[1][0] - v[0][0] * v[1][2];
+  v[2][2] = v[0][0] * v[1][1] - v[0][1] * v[1][0];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) Ep[3 * i + j] = u[0][i] * v[0][j] + u[1][i] * v[1][j];
+  return true;
+}
+
+// (R, t) in front for the calibrated pair (x1, y1) <-> (x2, y2): the least-squares depths of l2 x^2 = l1 R x^1 + t
+// are both positive, and the rays are not parallel (sin^2 of their angle above VP_E_PARALLEL)
+__host__ __device__ __forceinline__ bool vp_in_front(const double *R, const double *t, double x1, double y1, double x2, double y2)
+{
+  const double a[3] = {R[0] * x1 + R[1] * y1 + R[2], R[3] * x1 + R[4] * y1 + R[5], R[6] * x1 + R[7] * y1 + R[8]};
+  const double b[3] = {x2, y2, 1.0};
+  const double aa = a[0] * a[0] + a[1] * a[1] + a[2] * a[2], bb = b[0] * b[0] + b[1] * b[1] + b[2] * b[2];
+  const double ab = a[0] * b[0] + a[1] * b[1] + a[2] * b[2];
+  const double at = a[0] * t[0] + a[1] * t[1] + a[2] * t[2], bt = b[0] * t[0] + b[1] * t[1] + b[2] * t[2];
+  if (!(aa * bb - ab * ab > VP_E_PARALLEL * aa * bb)) return false;
+  return ab * bt - at * bb > 0.0 && aa * bt - ab * at > 0.0;      // l1, l2 times the positive determinant
+}
+
+// Step 7 of an essential call, one CTA: the winning Fn's inliers, the 8-point normal matrix on calibrated coordinates
+// scaled by lambda = s * (K1[0] K1[4] K2[0] K2[4])^(1/4) (not centred), its smallest eigenvector E' and E = S E' S with
+// S = diag(lambda, lambda, 1), projected to the essential manifold; re-scored as Fn, kept unless it has fewer inliers;
+// the final mask; then the four poses of the final E and the in-front counts over the final inliers.
+__global__ void __launch_bounds__(VP_REFIT_T)
+vp_refit_e_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, const double *__restrict__ models,
+                  VerifyCalib cal, unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts,
+                  VerifyState *st)
+{
+  __shared__ double s_nm[VP_REFIT_T / 32][45];
+  __shared__ double s_m[2][9];         // Fn of [0] the minimal model, [1] the refit
+  __shared__ double s_ep[9];           // the refit's projected E
+  __shared__ double s_R[4][9], s_t[4][3];
+  __shared__ float s_f[9];
+  __shared__ int s_cnt[VP_REFIT_T / 32];
+  __shared__ int s_refit, s_pose;
+  const int n = st->numValid;
+  const unsigned long long key = st->best;
+  const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
+  const float thr2 = st->thr2;
+  const int best = key ? (int)~(unsigned int)key : -1;
+  int cnt0 = 0, cntR = 0, kept = 0;
+  float m[9];
+  if (best >= 0) {
+    if (threadIdx.x < 9) { s_m[0][threadIdx.x] = models[(size_t)best * 9 + threadIdx.x]; s_f[threadIdx.x] = (float)s_m[0][threadIdx.x]; }
+    __syncthreads();
+    for (int k = 0; k < 9; k++) m[k] = s_f[k];
+    const double lam = s * sqrt(sqrt(cal.K1[0] * cal.K1[4]) * sqrt(cal.K2[0] * cal.K2[4]));
+    double acc[45];
+#pragma unroll
+    for (int k = 0; k < 45; k++) acc[k] = 0.0;
+    int c = 0;
+    for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
+      if (!vp_inlier(m, un[k], thr2, false)) continue;
+      c++;
+      const float4 p = xy[k];
+      double x, y, X, Y;
+      vp_calibrate(cal.K1, p.x, p.y, x, y);
+      vp_calibrate(cal.K2, p.z, p.w, X, Y);
+      x *= lam; y *= lam; X *= lam; Y *= lam;
+      const double r[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
+      int e = 0;
+#pragma unroll
+      for (int i = 0; i < 9; i++)
+#pragma unroll
+        for (int j = i; j < 9; j++) acc[e++] += r[i] * r[j];
+    }
+    vp_warp_normal(acc, s_nm);
+    cnt0 = vp_block_count(c, s_cnt);
+    if (threadIdx.x == 0) {
+      s_refit = 0;
+      if (cnt0 >= 8) {
+        double f[9], E[9], u[3][3], v[3][3];
+        vp_smallest_eigvec(s_nm, f);
+        for (int i = 0; i < 3; i++)
+          for (int j = 0; j < 3; j++) E[3 * i + j] = f[3 * i + j] * (i < 2 ? lam : 1.0) * (j < 2 ? lam : 1.0);
+        if (vp_essential_project(E, s_ep, u, v)) {
+          double G1[9], G2[9], TK[9], fn[9];
+          vp_calib_maps(cal.K1, c1x, c1y, s, G1, TK);
+          vp_calib_maps(cal.K2, c2x, c2y, s, G2, TK);
+          vp_sandwich(G2, s_ep, G1, fn);
+          if (vp_store_unit(s_m[1], fn)) s_refit = 1;
+        }
+      }
+    }
+    __syncthreads();
+    if (s_refit) {
+      for (int k = 0; k < 9; k++) m[k] = (float)s_m[1][k];
+      int cr = 0;
+      for (int k = threadIdx.x; k < n; k += VP_REFIT_T) cr += vp_inlier(m, un[k], thr2, false);
+      cntR = vp_block_count(cr, s_cnt);
+      kept = cntR >= cnt0;
+    }
+    if (!kept)
+      for (int k = 0; k < 9; k++) m[k] = s_f[k];
+  }
+  const int tot = vp_final_mask(best >= 0 ? m : nullptr, un, n, thr2, false, masks, blockCounts, s_cnt);
+  // the final E and its four poses (R_a = U W V^T, R_b = U W^T V^T; t = +u3, -u3): candidates 0..3 =
+  // (R_a, +), (R_a, -), (R_b, +), (R_b, -)
+  if (threadIdx.x == 0) {
+    s_pose = 0;
+    double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    if (best >= 0) {
+      double E[9], Ep[9], u[3][3], v[3][3];
+      if (kept) {
+        for (int k = 0; k < 9; k++) E[k] = s_ep[k];
+      } else {
+        double G[9], TK1[9], TK2[9];
+        vp_calib_maps(cal.K1, c1x, c1y, s, G, TK1);
+        vp_calib_maps(cal.K2, c2x, c2y, s, G, TK2);
+        vp_sandwich(TK2, s_m[0], TK1, E);
+      }
+      if (vp_essential_project(E, Ep, u, v) && vp_unit_sign(Ep)) {
+        for (int k = 0; k < 9; k++) out[k] = Ep[k];
+        const double tn = 1.0 / sqrt(u[2][0] * u[2][0] + u[2][1] * u[2][1] + u[2][2] * u[2][2]);
+        for (int i = 0; i < 3; i++)
+          for (int j = 0; j < 3; j++) {
+            const double a = u[1][i] * v[0][j] - u[0][i] * v[1][j], b = u[0][i] * v[1][j] - u[1][i] * v[0][j];
+            const double w = u[2][i] * v[2][j];
+            s_R[0][3 * i + j] = s_R[1][3 * i + j] = a + w;
+            s_R[2][3 * i + j] = s_R[3][3 * i + j] = b + w;
+          }
+        for (int i = 0; i < 3; i++) {
+          s_t[0][i] = s_t[2][i] = u[2][i] * tn;
+          s_t[1][i] = s_t[3][i] = -u[2][i] * tn;
+        }
+        s_pose = 1;
+      }
+    }
+    for (int k = 0; k < 9; k++) st->model[k] = out[k];
+  }
+  __syncthreads();
+  int front[4] = {0, 0, 0, 0};
+  if (s_pose) {
+    for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
+      if (!((masks[k >> 5] >> (k & 31)) & 1u)) continue;
+      const float4 p = xy[k];
+      double x, y, X, Y;
+      vp_calibrate(cal.K1, p.x, p.y, x, y);
+      vp_calibrate(cal.K2, p.z, p.w, X, Y);
+      for (int q = 0; q < 4; q++) front[q] += vp_in_front(s_R[q], s_t[q], x, y, X, Y);
+    }
+    for (int q = 0; q < 4; q++) front[q] = vp_block_count(front[q], s_cnt);
+  }
+  if (threadIdx.x == 0) {
+    int pick = 0, runner = 0;
+    for (int q = 1; q < 4; q++) if (front[q] > front[pick]) pick = q;
+    for (int q = 0; q < 4; q++) if (q != pick) runner = max(runner, front[q]);
+    for (int k = 0; k < 9; k++) st->R[k] = s_pose ? s_R[pick][k] : 0.0;
+    for (int k = 0; k < 3; k++) st->t[k] = s_pose ? s_t[pick][k] : 0.0;
+    st->pose[0] = front[pick];
+    st->pose[1] = runner;
+    st->total = tot;
+    st->stats[0] = n;
+    st->stats[2] = (long long)st->samples;
+    st->stats[3] = (long long)st->models;
+    st->stats[4] = best;
+    st->stats[5] = cnt0;
+    st->stats[6] = kept;
+    st->stats[7] = tot;
+  }
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------
 struct VerifyLayout {
   size_t masks, counts, xy, un, orig, models, slotCounts, state, bytes;
 };
 
-static VerifyLayout verify_layout(int numPairs, int numLoops)
+// model slots per sample: up to 3 roots of the 7-point cubic (F; H uses the first), up to 10 of the 5-point solver (E)
+static int vp_slots_per_sample(int model) { return model == VERIFY_ESSENTIAL ? VP_E_SLOTS : 3; }
+
+static VerifyLayout verify_layout(int numPairs, int numLoops, int model)
 {
   VerifyLayout L;
   size_t o = 0;
   auto take = [&](size_t b) { const size_t at = o; o += (b + 255) & ~(size_t)255; return at; };
-  const size_t P = numPairs > 0 ? (size_t)numPairs : 1, S = 3 * (size_t)numLoops;
+  const size_t P = numPairs > 0 ? (size_t)numPairs : 1, S = vp_slots_per_sample(model) * (size_t)numLoops;
   L.masks = take(((P + 31) / 32) * sizeof(unsigned int));
   L.counts = take(((P + VP_ROWS - 1) / VP_ROWS) * sizeof(unsigned int));
   L.xy = take(P * sizeof(float4));
@@ -731,7 +1338,7 @@ static VerifyLayout verify_layout(int numPairs, int numLoops)
   return L;
 }
 
-size_t verify_scratch_bytes(int numPairs, int numLoops) { return verify_layout(numPairs, numLoops).bytes; }
+size_t verify_scratch_bytes(int numPairs, int numLoops, int model) { return verify_layout(numPairs, numLoops, model).bytes; }
 size_t verify_result_bytes() { return sizeof(VerifyState); }
 
 // CUDASIFT_MATCH_TIMING=1: the events between the kernels, printed to stderr
@@ -750,10 +1357,10 @@ static void vp_timing_print(cudaEvent_t *tev, int numPairs, int numLoops, int mo
 // Steps 1-4 (and, with full, 5-8) on the stream; then the state is copied to h_state (pinned, verify_result_bytes()).
 // inliers may be null when maxInliers == 0.  full == false stops after scoring (the models and counts stay in scratch).
 int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *pairs, int numPairs, int model,
-                  int numLoops, float thresh, unsigned long long seed, int *inliers, int maxInliers, void *scratch,
-                  void *h_state, bool full, cudaStream_t st)
+                  const VerifyCalib *cal, int numLoops, float thresh, unsigned long long seed, int *inliers,
+                  int maxInliers, void *scratch, void *h_state, bool full, cudaStream_t st)
 {
-  const VerifyLayout L = verify_layout(numPairs, numLoops);
+  const VerifyLayout L = verify_layout(numPairs, numLoops, model);
   char *b = static_cast<char *>(scratch);
   unsigned int *masks = reinterpret_cast<unsigned int *>(b + L.masks), *counts = reinterpret_cast<unsigned int *>(b + L.counts);
   float4 *xy = reinterpret_cast<float4 *>(b + L.xy), *un = reinterpret_cast<float4 *>(b + L.un);
@@ -762,7 +1369,9 @@ int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cons
   unsigned int *slotCounts = reinterpret_cast<unsigned int *>(b + L.slotCounts);
   VerifyState *vs = reinterpret_cast<VerifyState *>(b + L.state);
   const int2 *p2 = reinterpret_cast<const int2 *>(pairs);
-  const int blocks = idivup(numPairs, VP_ROWS), slots = 3 * numLoops;
+  const bool essential = model == VERIFY_ESSENTIAL;
+  const int perSample = vp_slots_per_sample(model);
+  const int blocks = idivup(numPairs, VP_ROWS), slots = perSample * numLoops;
   cudaEvent_t *tev = full ? match_timing_events() : nullptr;
   if (tev) cudaEventRecord(tev[0], st);
   vp_flags_kernel<<<blocks, VP_ROWS, 0, st>>>(s1, n1, s2, n2, p2, numPairs, masks, counts);
@@ -771,17 +1380,25 @@ int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, cons
   if (tev) cudaEventRecord(tev[2], st);
   vp_norm_kernel<<<1, 1024, 0, st>>>(xy, un, thresh, vs);
   if (tev) cudaEventRecord(tev[3], st);
-  vp_hyp_kernel<<<idivup(numLoops, VP_HYP_T), VP_HYP_T, 0, st>>>(xy, numLoops, model, seed, models, slotCounts, vs);
+  if (essential)
+    vp_hyp5_kernel<<<idivup(numLoops, VP_HYP_T), VP_HYP_T, 0, st>>>(xy, numLoops, seed, *cal, models, slotCounts, vs);
+  else
+    vp_hyp_kernel<<<idivup(numLoops, VP_HYP_T), VP_HYP_T, 0, st>>>(xy, numLoops, model, seed, models, slotCounts, vs);
   if (tev) cudaEventRecord(tev[4], st);
+  const int scoreModel = essential ? CS_GEOM_FUNDAMENTAL : model;      // E is scored as its Fn
   const int scoreThreads = model == CS_GEOM_HOMOGRAPHY ? numLoops : slots;
   vp_score_kernel<<<dim3(idivup(scoreThreads, VP_SC_T), idivup(numPairs, VP_CHUNK)), VP_SC_T, 0, st>>>(un, models, slots,
-                                                                                                      model, slotCounts, vs);
+                                                                                                      scoreModel, slotCounts,
+                                                                                                      vs);
   count_launch(5);
   if (full) {
     if (tev) cudaEventRecord(tev[5], st);
-    vp_argmax_kernel<<<idivup(slots, 256), 256, 0, st>>>(models, slotCounts, slots, vs);
+    vp_argmax_kernel<<<idivup(slots, 256), 256, 0, st>>>(models, slotCounts, slots, perSample, vs);
     if (tev) cudaEventRecord(tev[6], st);
-    vp_refit_kernel<<<1, VP_REFIT_T, 0, st>>>(xy, un, models, model, masks, counts, vs);
+    if (essential)
+      vp_refit_e_kernel<<<1, VP_REFIT_T, 0, st>>>(xy, un, models, *cal, masks, counts, vs);
+    else
+      vp_refit_kernel<<<1, VP_REFIT_T, 0, st>>>(xy, un, models, model, masks, counts, vs);
     if (tev) cudaEventRecord(tev[7], st);
     vp_write_kernel<<<blocks, VP_ROWS, 0, st>>>(p2, orig, masks, counts, reinterpret_cast<int2 *>(inliers), maxInliers, vs);
     if (tev) cudaEventRecord(tev[8], st);
@@ -803,14 +1420,26 @@ int verify_result(const void *h_state, int numPairs, double model_out[9], long l
   return v->total;
 }
 
-// After launch_verify(full = false) and a synchronize: every slot's model in pixel coordinates (NaN-filled when empty),
-// every slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s}.  Returns the number of valid pairs.
-int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
-                          double *h_models, int *h_counts, double h_norm[5], cudaStream_t st)
+// The same after an essential launch: E (in model), the pose and the ten statistics.
+int verify_essential_result(const void *h_state, int numPairs, double E[9], double R[9], double t[3], long long stats[10])
 {
-  const VerifyLayout L = verify_layout(numPairs, numLoops);
+  const VerifyState *v = static_cast<const VerifyState *>(h_state);
+  for (int k = 0; k < 9; k++) R[k] = v->R[k];
+  for (int k = 0; k < 3; k++) t[k] = v->t[k];
+  stats[8] = v->pose[0];
+  stats[9] = v->pose[1];
+  return verify_result(h_state, numPairs, E, stats);
+}
+
+// After launch_verify(full = false) and a synchronize: every slot's model in pixel coordinates (NaN-filled when empty),
+// every slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s}.  Returns the number of valid pairs.  An
+// essential slot's Fn becomes E = (T2 K2)^T Fn (T1 K1) with F's output scaling.
+int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
+                          const VerifyCalib *cal, double *h_models, int *h_counts, double h_norm[5], cudaStream_t st)
+{
+  const VerifyLayout L = verify_layout(numPairs, numLoops, model);
   const char *b = static_cast<const char *>(scratch);
-  const size_t S = 3 * (size_t)numLoops;
+  const size_t S = vp_slots_per_sample(model) * (size_t)numLoops;
   CS_CUDA(cudaMemcpyAsync(h_models, b + L.models, S * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaMemcpyAsync(h_counts, b + L.slotCounts, S * sizeof(int), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaStreamSynchronize(st));
@@ -820,7 +1449,15 @@ int verify_models_to_host(const void *scratch, const void *h_state, int numPairs
     double *m = h_models + 9 * k;
     if (std::isnan(m[0])) { for (int j = 0; j < 9; j++) m[j] = NAN; continue; }
     double out[9];
-    vp_denormalise(m, model, v->c1x, v->c1y, v->c2x, v->c2y, v->s, out);
+    if (model == VERIFY_ESSENTIAL) {
+      double G[9], TK1[9], TK2[9];
+      vp_calib_maps(cal->K1, v->c1x, v->c1y, v->s, G, TK1);
+      vp_calib_maps(cal->K2, v->c2x, v->c2y, v->s, G, TK2);
+      vp_sandwich(TK2, m, TK1, out);
+      vp_unit_sign(out);
+    } else {
+      vp_denormalise(m, model, v->c1x, v->c1y, v->c2x, v->c2y, v->s, out);
+    }
     for (int j = 0; j < 9; j++) m[j] = out[j];
   }
   return v->numValid;

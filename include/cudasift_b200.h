@@ -175,6 +175,74 @@ int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, con
  * count, [6] = 1 if the refit was kept, [7] = the final inlier count. */
 int cs_verify_stats(long long out[8]);
 
+/* Calibrated two-view verification (RANSAC for the essential matrix, 5-point minimal solver) and the relative pose:
+ * findEssentialMat + recoverPose on the device.  Validity, the pair format, the sampler (5 distinct draws per
+ * sample), the order of d_inliers, synchronisation, scratch and the argument checks are those of cs_verify_pairs.
+ * - K1, K2: row-major pinhole intrinsics of image 1 and image 2, skew allowed: all entries finite, K[3] = K[6] = K[7] =
+ *   0, K[8] = 1, K[0] > 0, K[4] > 0.  Calibrated coordinates, in double from the float record coordinates:
+ *     y^ = (y - K[5]) / K[4],   x^ = (x - K[2] - K[1] * y^) / K[0].
+ * - Minimal solver (Nister), FP64 on the calibrated coordinates of the 5 drawn pairs: rows {X x, X y, X, Y x, Y y, Y,
+ *   x, y, 1} ((x, y) image 1, (X, Y) image 2), their null space by the elimination of cs_verify_pairs (pivot 1e-9;
+ *   N0..N3 for the free columns 5..8).  Basis: modified Gram-Schmidt of N0, N1, N2, N3 in that order (each vector minus
+ *   its projections on the earlier unit vectors, then divided by its norm; a zero norm makes the sample degenerate),
+ *   giving q0..q3, then X = (q0 - q1 + q2 - q3) / 2, Y = (q0 + q1 - q2 - q3) / 2, Z = (q0 - q1 - q2 + q3) / 2,
+ *   W = (q0 + q1 + q2 + q3) / 2, and E = x X + y Y + z Z + W.  The ten cubics det E = 0 and
+ *   2 E E^T E - tr(E E^T) E = 0 (entry (i, j) is row 1 + 3i + j) in the 20 monomials x^3 y^3 x^2y xy^2 x^2z x^2 y^2z y^2
+ *   xyz xy xz^2 xz x yz^2 yz y z^3 z^2 z 1; Gauss-Jordan with partial pivoting on the first ten columns (the first row
+ *   of equal magnitude; a pivot at or below 1e-12 of the largest |entry| makes the sample degenerate).  Rows 4 - z*5,
+ *   6 - z*7, 8 - z*9 are [x y 1] times polynomials in z; the determinant of that 3x3 matrix (cofactors along its
+ *   first row) has degree 10.  Its leading coefficients at or below 1e-12 of the largest |coefficient| are dropped.
+ *   Distinct real roots by a Sturm sequence of the monic polynomial p of degree n: S0 = p, S1 = p' / n,
+ *   S(k+1) = -rem(S(k-1), S(k)) divided by the magnitude of its leading coefficient.  The sequence ends at a remainder
+ *   whose largest |coefficient| is at or below 1e-14 of its dividend's largest; a remainder's leading coefficients at
+ *   or below 1e-14 of its own largest |coefficient| are dropped.  Isolation on (-B, B] with Fujiwara's bound
+ *   B = 1 + 2 max_k |a(n-k)|^(1/k) (a the monic coefficients, k = 1..n), by bisection at midpoints, left half first,
+ *   halves without a root dropped; an interval is refined as one root when it holds one root, when it is narrower than
+ *   1e-10 * max(1, |lo|, |hi|), or when more than 62 other intervals are pending (room for 64).  Refinement: bisection
+ *   to a width of 1e-10 * max(1, |lo|, |hi|) (on the sign of the polynomial when it changes sign across the interval,
+ *   else on the Sturm count, keeping the left half while it holds a root), then up to 3 Newton steps from the
+ *   midpoint, each kept only while it stays inside the interval.  Roots ascending in z.  (x, y, 1) is the cross product
+ *   of two rows of the evaluated 3x3 matrix, the pair (0,1), (0,2), (1,2) with the largest |third component| (the first
+ *   of equals), divided by that component; a root where it is 0 is skipped.  Slot sample*10 + r holds the r-th
+ *   remaining solution; a sample is degenerate when it has fewer than 5 distinct draws or a pivot fails.
+ * - Residual: the Sampson error in pixels of F = K2^-T E K1^-1, exactly as cs_verify_pairs with CS_GEOM_FUNDAMENTAL
+ *   (FP32 on normalised coordinates, the model Fn = T2^-T F T1^-1 at unit norm), so thresh means the same and the F
+ *   of a result can go to cs_match_guided(..., CS_GEOM_FUNDAMENTAL, ...).  Ties: the lowest slot.
+ * - Refit, once, with at least 8 inliers of the winning model: the 8-point normal matrix on calibrated coordinates of
+ *   both images scaled by lambda = s * (K1[0] K1[4] K2[0] K2[4])^(1/4) (s the normalisation scale; not centred), its
+ *   smallest eigenvector E' (Jacobi), E = S E' S with S = diag(lambda, lambda, 1), projected to the essential manifold
+ *   (below).  Kept unless it has fewer inliers.
+ * - Projection: the eigenvectors of E^T E (Jacobi), descending (the lower index first on ties); v1, v2 those of the
+ *   two largest eigenvalues, sigma_i their square roots (> 0, else no projection), u_i = E v_i / sigma_i;
+ *   Ep = u1 v1^T + u2 v2^T, U = (u1, u2, u1 x u2), V = (v1, v2, v1 x v2).
+ * - Outputs: E_out is the projection of the final E (the refit, or the winner (T2 K2)^T Fn (T1 K1)) at unit Frobenius
+ *   norm, its largest-magnitude entry positive.  Pose candidates, in this order: (U W V^T, +u3), (U W V^T, -u3),
+ *   (U W^T V^T, +u3), (U W^T V^T, -u3), W = [0 -1 0; 1 0 0; 0 0 1]; each is a rotation (det +1) and a unit
+ *   translation with E_out proportional to [t]x R, mapping camera-1 points to camera 2 (X2 = R X1 + t).  A final inlier
+ *   is in front of a candidate when the least-squares depths of l2 x^2 = l1 R x^1 + t are both > 0, computed in double
+ *   as l1 ~ (a.b)(b.t) - (a.t)(b.b), l2 ~ (a.a)(b.t) - (a.b)(a.t) with a = R x^1, b = x^2, and its rays are not parallel:
+ *   (a.a)(b.b) - (a.b)^2 > 1e-12 (a.a)(b.b).  R_out, t_out: the candidate with the most inliers in front (the first
+ *   of equals).  A planar scene admits two physically valid poses; the one returned is then one of them.
+ * Returns the total inlier count, or CS_E_*.  Fewer than 5 valid pairs or no non-degenerate sample: 0 and zero E, R,
+ * t.  numPairs == 0 returns 0 and zero E, R, t before any CUDA call.  A final E that cannot be projected leaves E, R, t
+ * zero.  CS_E_ARG, before any CUDA call, as cs_verify_pairs (model aside), and for NULL or invalid K1 or K2 and NULL
+ * E_out, R_out or t_out.  One call issues 8 kernel launches (flags, compact, norm, 5-point hypotheses, score, arg-max,
+ * E refit with the pose, write) and synchronises once, at the end.  The hypothesis kernel uses an 8 KB stack per thread:
+ * the first call of a process makes the CUDA driver reserve local memory for every thread that can be resident (about
+ * 1.8 GB measured on an H100), which it keeps for the life of the context. */
+int cs_verify_essential(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs,
+                        const double K1[9], const double K2[9], int numLoops, float thresh, unsigned long long seed,
+                        double E_out[9], double R_out[9], double t_out[3], int *d_inliers, int maxInliers, double *ms);
+/* Same with host record arrays, a host pair list and a host inlier buffer. */
+int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs,
+                             const double K1[9], const double K2[9], int numLoops, float thresh,
+                             unsigned long long seed, double E_out[9], double R_out[9], double t_out[3],
+                             int *h_inliers, int maxInliers, double *ms);
+/* The last cs_verify_essential* call on this thread's device: [0..7] as cs_verify_stats (the winning slot is
+ * sample*10 + root), [8] = the final inliers in front of the chosen pose, [9] = the runner-up candidate's count.
+ * cs_verify_stats keeps describing cs_verify_pairs* calls. */
+int cs_verify_essential_stats(long long out[10]);
+
 /* Guided matching (COLMAP's guided_matching): the two nearest neighbours and the ratio test restricted to the pairs a
  * model admits.  cs_match_knn2_guided has the semantics of cs_match_knn2 (the reference's score, only scores > 0, the
  * order score descending then index ascending, a missing neighbour is (-1, 0.0f)), except that row i of set 1 only
@@ -250,6 +318,12 @@ int cs_describe_points(const float *d_img, int width, int height, int pitch, voi
 int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs, int model,
                      int numLoops, float thresh, unsigned long long seed, double *h_models, int *h_counts,
                      double h_norm[5]);
+/* The same for cs_verify_essential: h_models[10*numLoops][9] receives every slot's E = (T2 K2)^T Fn (T1 K1) at unit
+ * Frobenius norm with its largest-magnitude entry positive (NaN-filled when empty), h_counts[10*numLoops] and h_norm
+ * as above. */
+int cs_verify_essential_models(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs,
+                               const double K1[9], const double K2[9], int numLoops, float thresh,
+                               unsigned long long seed, double *h_models, int *h_counts, double h_norm[5]);
 
 /* ---- pipelined extractor (extension; the reference API is strictly synchronous) ----
  * One extractor = one CUDA stream + arena + SiftPoint array + pinned staging.  Several
