@@ -18,7 +18,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "CudaSiftError", "extract_host", "match_host", "rank_records", "MatchSiftDataMutual", "match_mutual_host",
            "match_knn2", "MatchSiftDataRatio", "match_ratio_host", "VerifyPairs", "verify_pairs_host", "verify_stats",
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
-           "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental"]
+           "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
+           "VerifyPairsBatch", "VerifyEssentialBatch"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -85,6 +86,8 @@ def lib():
                                           c.POINTER(c.c_double)]),
         "cs_verify_essential_stats": (ip, [c.POINTER(c.c_longlong)]),
         "cs_verify_essential_models": (ip, [vp, ip, vp, ip, vp, ip, vp, vp, ip, fp, c.c_ulonglong, vp, vp, vp]),
+        "cs_verify_pairs_batch": (ip, [vp, ip, ip, ip, fp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_verify_essential_batch": (ip, [vp, ip, vp, vp, ip, fp, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -418,6 +421,91 @@ def verify_stats():
 
 def _intrinsics(K):
     return np.ascontiguousarray(np.asarray(K, np.float64).reshape(9))
+
+
+class VerifyJob(ctypes.Structure):
+    """cs_verify_job: one image pair of a batched verification (device records, pairs and inlier buffer)."""
+    _fields_ = [("s1", ctypes.c_void_p), ("n1", ctypes.c_int), ("s2", ctypes.c_void_p), ("n2", ctypes.c_int),
+                ("pairs", ctypes.c_void_p), ("numPairs", ctypes.c_int), ("seed", ctypes.c_ulonglong),
+                ("inliers", ctypes.c_void_p), ("maxInliers", ctypes.c_int)]
+
+
+class _BatchJobs:
+    """The job table of a batch call for [(data1, data2, pairs) or (data1, data2, pairs, seed)]: every pair list in one
+    device buffer and every inlier list in another, each job's pointers into them (room for all its pairs)."""
+
+    def __init__(self, jobs):
+        parsed = []
+        for j in jobs:
+            if len(j) not in (3, 4):
+                raise ValueError("a job is (data1, data2, pairs) or (data1, data2, pairs, seed)")
+            parsed.append((j[0], j[1], _pair_array(j[2]), int(j[3]) if len(j) == 4 else 0))
+        self.sizes = [len(p[2]) for p in parsed]
+        self.offsets = np.concatenate([[0], np.cumsum(self.sizes, dtype=np.int64)]).astype(np.int64)
+        total = int(self.offsets[-1])
+        self.bufs = [DeviceBuffer(max(total, 1) * 8), DeviceBuffer(max(total, 1) * 8)]
+        if total:
+            self.bufs[0].upload(np.concatenate([p[2] for p in parsed]))
+        self.table = (VerifyJob * max(len(parsed), 1))()
+        for q, (d1, d2, pairs, seed) in enumerate(parsed):
+            k, o = self.sizes[q], 8 * int(self.offsets[q])
+            self.table[q] = VerifyJob(d1.d_data, d1.numPts, d2.d_data, d2.numPts, self.bufs[0].ptr + o if k else None, k,
+                                      seed, self.bufs[1].ptr + o if k else None, k)
+        self.count = len(parsed)
+
+    def ptr(self):
+        return ctypes.addressof(self.table) if self.count else None
+
+    def inliers(self, counts):
+        """Each job's inlier list, int32 [m, 2], from the shared inlier buffer."""
+        total = int(self.offsets[-1])
+        flat = self.bufs[1].download(np.int32, 2 * total).reshape(-1, 2) if total else np.zeros((0, 2), np.int32)
+        return [flat[self.offsets[q]:self.offsets[q] + int(counts[q])].copy() for q in range(self.count)]
+
+    def free(self):
+        for b in self.bufs:
+            b.free()
+
+
+def VerifyPairsBatch(jobs, model="fundamental", numLoops=4096, thresh=4.0):
+    """VerifyPairs over many image pairs in one call (cs_verify_pairs_batch): jobs is a list of (data1, data2, pairs)
+    or (data1, data2, pairs, seed), the seed 0 when not given; model, numLoops and thresh are common.  Job p's results
+    equal VerifyPairs(data1, data2, pairs, model, numLoops, thresh, seed) bit for bit.  Returns (models [J, 3, 3]
+    float64, inliers: a list of int32 [m, 2], stats int64 [J, 8] as verify_stats, ms)."""
+    code = _geom_model(model)
+    J = len(jobs)
+    models, counts, stats = np.zeros((J, 9)), np.zeros(J, np.int32), np.zeros((J, 8), np.int64)
+    ms = ctypes.c_double(0.0)
+    b = _BatchJobs(jobs)
+    try:
+        _check(lib().cs_verify_pairs_batch(b.ptr(), J, code, int(numLoops), float(thresh), _ptr(models), _ptr(counts),
+                                           _ptr(stats), ctypes.byref(ms)), "VerifyPairsBatch")
+        inliers = b.inliers(counts)
+    finally:
+        b.free()
+    return models.reshape(J, 3, 3), inliers, stats, ms.value
+
+
+def VerifyEssentialBatch(jobs, K1s, K2s, numLoops=4096, thresh=4.0):
+    """VerifyEssential over many image pairs in one call (cs_verify_essential_batch): jobs as for VerifyPairsBatch,
+    K1s and K2s the intrinsics per job ([J, 3, 3], or one 3x3 for all jobs).  Job p's results equal
+    VerifyEssential(data1, data2, pairs, K1s[p], K2s[p], numLoops, thresh, seed) bit for bit.  Returns (E [J, 3, 3],
+    R [J, 3, 3], t [J, 3], inliers: a list of int32 [m, 2], stats int64 [J, 10] as essential_stats, ms)."""
+    J = len(jobs)
+    k1 = np.ascontiguousarray(np.broadcast_to(np.asarray(K1s, np.float64).reshape(-1, 9), (J, 9)))
+    k2 = np.ascontiguousarray(np.broadcast_to(np.asarray(K2s, np.float64).reshape(-1, 9), (J, 9)))
+    E, R, t = np.zeros((J, 9)), np.zeros((J, 9)), np.zeros((J, 3))
+    counts, stats = np.zeros(J, np.int32), np.zeros((J, 10), np.int64)
+    ms = ctypes.c_double(0.0)
+    b = _BatchJobs(jobs)
+    try:
+        _check(lib().cs_verify_essential_batch(b.ptr(), J, _ptr(k1), _ptr(k2), int(numLoops), float(thresh), _ptr(E),
+                                               _ptr(R), _ptr(t), _ptr(counts), _ptr(stats), ctypes.byref(ms)),
+               "VerifyEssentialBatch")
+        inliers = b.inliers(counts)
+    finally:
+        b.free()
+    return E.reshape(J, 3, 3), R.reshape(J, 3, 3), t, inliers, stats, ms.value
 
 
 def VerifyEssential(data1, data2, pairs, K1, K2, numLoops=4096, thresh=4.0, seed=0):

@@ -11,6 +11,8 @@
 #include "common.cuh"
 #include "pipeline2.h"
 
+#include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstddef>
 #include <cstdarg>
@@ -524,28 +526,52 @@ static int essential_args(const char *fn, const void *s1, int n1, const void *s2
   return check_intrinsics(fn, K2, "K2");
 }
 
-// The verifier's scratch and the pinned copy of its state.
-static int verify_buffers(DeviceCtx *c, int numPairs, int numLoops, int model)
+// The verifier's scratch and the pinned area of its states and job table, for a batch (or a single call: one job).
+static int verify_buffers(DeviceCtx *c, const cs_verify_job *jobs, int numJobs, int numLoops, int model)
 {
   int r;
-  if ((r = c->verify.grow(verify_scratch_bytes(numPairs, numLoops, model))) < 0) return r;
-  if (!c->h_verify) CS_CUDA(cudaMallocHost(&c->h_verify, verify_result_bytes()));
+  if ((r = c->verify.grow(verify_scratch_bytes(jobs, numJobs, numLoops, model))) < 0) return r;
+  const size_t hb = verify_host_bytes(numJobs);
+  if (c->h_verifyBytes < hb) {                 // every verify call ends in a synchronize: no copy is pending here
+    if (c->h_verify) cudaFreeHost(c->h_verify);
+    c->h_verify = nullptr;
+    c->h_verifyBytes = 0;
+    CS_CUDA(cudaMallocHost(&c->h_verify, hb));
+    c->h_verifyBytes = hb;
+  }
   return 0;
 }
 
-// cs_verify_pairs on device sets and a device pair list: the launches, one copy of the state, one synchronize.
+static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, const int *pairs, int numPairs,
+                                unsigned long long seed, int *inliers, int maxInliers)
+{
+  cs_verify_job j;
+  j.s1 = d1; j.n1 = n1; j.s2 = d2; j.n2 = n2; j.pairs = pairs; j.numPairs = numPairs;
+  j.seed = seed; j.inliers = inliers; j.maxInliers = maxInliers;
+  return j;
+}
+
+// The launches of a batch (cal: per job, essential only), one synchronize.
+static int verify_batch_sync(const char *fn, DeviceCtx *c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal,
+                             int model, int numLoops, float thresh, double *ms)
+{
+  int r;
+  if ((r = verify_buffers(c, jobs, numJobs, numLoops, model)) < 0) return r;
+  auto enqueue = [&] {
+    return launch_verify(jobs, numJobs, cal, model, numLoops, thresh, c->verify.p, c->h_verify, true, c->stream);
+  };
+  return timed_sync(fn, c, ms, enqueue);
+}
+
+// cs_verify_pairs on device sets and a device pair list: a batch of one job.
 static int verify_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
                        const int *pairs, int numPairs, int model, int numLoops, float thresh, unsigned long long seed,
                        double model_out[9], int *inliers, int maxInliers, double *ms)
 {
-  int r;
-  if ((r = verify_buffers(c, numPairs, numLoops, model)) < 0) return r;
-  auto enqueue = [&] {
-    return launch_verify(d1, n1, d2, n2, pairs, numPairs, model, nullptr, numLoops, thresh, seed, inliers, maxInliers,
-                         c->verify.p, c->h_verify, true, c->stream);
-  };
-  if ((r = timed_sync(fn, c, ms, enqueue)) < 0) return r;
-  return verify_result(c->h_verify, numPairs, model_out, c->verifyStats);
+  const cs_verify_job job = verify_job(d1, n1, d2, n2, pairs, numPairs, seed, inliers, maxInliers);
+  const int r = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms);
+  if (r < 0) return r;
+  return verify_result(c->h_verify, 0, numPairs, model_out, c->verifyStats);
 }
 
 // cs_verify_essential on device sets and a device pair list: as verify_sync, with the pose.
@@ -554,14 +580,87 @@ static int essential_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int
                           unsigned long long seed, double E[9], double R[9], double t[3], int *inliers, int maxInliers,
                           double *ms)
 {
+  const cs_verify_job job = verify_job(d1, n1, d2, n2, pairs, numPairs, seed, inliers, maxInliers);
+  const int r = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms);
+  if (r < 0) return r;
+  return verify_essential_result(c->h_verify, 0, numPairs, E, R, t, c->essentialStats);
+}
+
+// cs_verify_models / cs_verify_essential_models: steps 1-4 of one job, then its slots to the host.
+static int verify_models_sync(DeviceCtx *c, const cs_verify_job &job, const VerifyCalib *cal, int model, int numLoops,
+                              float thresh, double *h_models, int *h_counts, double h_norm[5])
+{
   int r;
-  if ((r = verify_buffers(c, numPairs, numLoops, VERIFY_ESSENTIAL)) < 0) return r;
-  auto enqueue = [&] {
-    return launch_verify(d1, n1, d2, n2, pairs, numPairs, VERIFY_ESSENTIAL, &cal, numLoops, thresh, seed, inliers,
-                         maxInliers, c->verify.p, c->h_verify, true, c->stream);
+  if ((r = verify_buffers(c, &job, 1, numLoops, model)) < 0) return r;
+  if ((r = launch_verify(&job, 1, cal, model, numLoops, thresh, c->verify.p, c->h_verify, false, c->stream)) < 0) return r;
+  return verify_models_to_host(c->verify.p, c->h_verify, job, numLoops, model, cal, h_models, h_counts, h_norm,
+                               c->stream);
+}
+
+// The arguments of cs_verify_pairs_batch (cal_args false) and cs_verify_essential_batch: the common ones, then every
+// job's as its single call checks them (named jobs[p]), the total pair count, then the inlier buffers against every
+// other job's buffers and records (sorted ranges, O(J log J)).
+static int verify_batch_args(const char *fn, const cs_verify_job *jobs, int numJobs, int model, int numLoops,
+                             float thresh, const double *K1s, const double *K2s, bool essential)
+{
+  int r;
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs a jobs array");
+  if (essential && numJobs > 0 && (!K1s || !K2s)) return arg_error(fn, "K1s and K2s must not be NULL");
+  long long total = 0;
+  const double dummy = 0.0;
+  for (int p = 0; p < numJobs; p++) {
+    const cs_verify_job &j = jobs[p];
+    char name[96];
+    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
+    if ((r = verify_args(name, j.s1, j.n1, j.s2, j.n2, j.pairs, j.numPairs, model, numLoops, thresh, &dummy, j.inliers,
+                         j.maxInliers)) < 0)
+      return r;
+    if (essential && ((r = check_intrinsics(name, K1s + 9 * (size_t)p, "K1s[p]")) < 0 ||
+                      (r = check_intrinsics(name, K2s + 9 * (size_t)p, "K2s[p]")) < 0))
+      return r;
+    total += j.numPairs;
+    if (total > INT_MAX) {
+      char bad[96];
+      snprintf(bad, sizeof bad, "the total numPairs exceeds INT_MAX at jobs[%d]", p);
+      return arg_error(fn, bad);
+    }
+  }
+  // every non-empty range; a writable one (an inlier buffer) may overlap no other range of another job (its own job's
+  // were checked above).  Sorted by start, an overlap is an earlier range that ends after a later one starts.
+  struct Range { uintptr_t lo, hi; int job, kind; };        // kind 0 inliers, 1 pairs, 2 s1, 3 s2
+  static const char *const kinds[4] = {"inliers", "pairs", "s1", "s2"};
+  std::vector<Range> rs;
+  rs.reserve(4 * (size_t)numJobs);
+  auto add = [&](const void *b, size_t bytes, int job, int kind) {
+    if (bytes) rs.push_back({reinterpret_cast<uintptr_t>(b), reinterpret_cast<uintptr_t>(b) + bytes, job, kind});
   };
-  if ((r = timed_sync(fn, c, ms, enqueue)) < 0) return r;
-  return verify_essential_result(c->h_verify, numPairs, E, R, t, c->essentialStats);
+  for (int p = 0; p < numJobs; p++) {
+    const cs_verify_job &j = jobs[p];
+    add(j.inliers, (size_t)j.maxInliers * sizeof(int2), p, 0);
+    add(j.pairs, (size_t)j.numPairs * sizeof(int2), p, 1);
+    add(j.s1, record_bytes(j.n1), p, 2);
+    add(j.s2, record_bytes(j.n2), p, 3);
+  }
+  std::sort(rs.begin(), rs.end(), [](const Range &a, const Range &b) {
+    return a.lo != b.lo ? a.lo < b.lo : a.kind != b.kind ? a.kind < b.kind : a.job < b.job;
+  });
+  const Range *anyEnd = nullptr, *outEnd = nullptr;       // the earlier ranges (and inlier buffers) that end last
+  for (const Range &x : rs) {
+    const Range *hit = nullptr;
+    if (x.kind == 0 && anyEnd && anyEnd->hi > x.lo) hit = anyEnd;
+    else if (outEnd && outEnd->hi > x.lo) hit = outEnd;
+    if (hit) {
+      const Range &a = hit->job <= x.job ? *hit : x, &b = hit->job <= x.job ? x : *hit;
+      char bad[128];
+      snprintf(bad, sizeof bad, "jobs[%d].%s and jobs[%d].%s overlap (an inlier buffer overlaps another range)", a.job,
+               kinds[a.kind], b.job, kinds[b.kind]);
+      return arg_error(fn, bad);
+    }
+    if (!anyEnd || x.hi > anyEnd->hi) anyEnd = &x;
+    if (x.kind == 0 && (!outEnd || x.hi > outEnd->hi)) outEnd = &x;
+  }
+  return 0;
 }
 
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
@@ -1212,12 +1311,9 @@ int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const i
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  if ((r = verify_buffers(c, numPairs, numLoops, model)) < 0) return r;
-  r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, nullptr, numLoops,
-                    thresh, seed, nullptr, 0, c->verify.p, c->h_verify, false, c->stream);
-  if (r < 0) return r;
-  return verify_models_to_host(c->verify.p, c->h_verify, numPairs, numLoops, model, nullptr, h_models, h_counts, h_norm,
-                               c->stream);
+  const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
+                                       nullptr, 0);
+  return verify_models_sync(c, job, nullptr, model, numLoops, thresh, h_models, h_counts, h_norm);
 }
 
 static void essential_zero(double E[9], double R[9], double t[3])
@@ -1296,12 +1392,76 @@ int cs_verify_essential_models(const void *d_s1, int n1, const void *d_s2, int n
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const VerifyCalib cal = verify_calib(K1, K2);
-  if ((r = verify_buffers(c, numPairs, numLoops, VERIFY_ESSENTIAL)) < 0) return r;
-  r = launch_verify((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, VERIFY_ESSENTIAL, &cal,
-                    numLoops, thresh, seed, nullptr, 0, c->verify.p, c->h_verify, false, c->stream);
+  const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
+                                       nullptr, 0);
+  return verify_models_sync(c, job, &cal, VERIFY_ESSENTIAL, numLoops, thresh, h_models, h_counts, h_norm);
+}
+
+int cs_verify_pairs_batch(const cs_verify_job *jobs, int numJobs, int model, int numLoops, float thresh,
+                          double *models_out, int *counts_out, long long *stats_out, double *ms)
+{
+  const char *fn = "cs_verify_pairs_batch";
+  if (ms) *ms = 0.0;
+  int r = verify_batch_args(fn, jobs, numJobs, model, numLoops, thresh, nullptr, nullptr, false);
   if (r < 0) return r;
-  return verify_models_to_host(c->verify.p, c->h_verify, numPairs, numLoops, VERIFY_ESSENTIAL, &cal, h_models, h_counts,
-                               h_norm, c->stream);
+  if (numJobs > 0 && (!models_out || !counts_out)) return arg_error(fn, "models_out and counts_out must not be NULL");
+  bool any = false;
+  for (int p = 0; p < numJobs; p++) {
+    for (int k = 0; k < 9; k++) models_out[9 * (size_t)p + k] = 0.0;
+    counts_out[p] = 0;
+    if (stats_out)
+      for (int k = 0; k < 8; k++) stats_out[8 * (size_t)p + k] = 0;
+    any |= jobs[p].numPairs > 0;
+  }
+  if (!any) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = verify_batch_sync(fn, c, jobs, numJobs, nullptr, model, numLoops, thresh, ms)) < 0) return r;
+  for (int p = 0, q = 0; p < numJobs; p++) {
+    if (jobs[p].numPairs == 0) continue;
+    long long st[8];
+    counts_out[p] = verify_result(c->h_verify, q++, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
+    if (stats_out)
+      for (int k = 0; k < 8; k++) stats_out[8 * (size_t)p + k] = st[k];
+  }
+  return 0;
+}
+
+int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const double *K1s, const double *K2s,
+                              int numLoops, float thresh, double *E_out, double *R_out, double *t_out,
+                              int *counts_out, long long *stats_out, double *ms)
+{
+  const char *fn = "cs_verify_essential_batch";
+  if (ms) *ms = 0.0;
+  int r = verify_batch_args(fn, jobs, numJobs, CS_GEOM_FUNDAMENTAL, numLoops, thresh, K1s, K2s, true);
+  if (r < 0) return r;
+  if (numJobs > 0 && (!E_out || !R_out || !t_out || !counts_out))
+    return arg_error(fn, "E_out, R_out, t_out and counts_out must not be NULL");
+  bool any = false;
+  std::vector<VerifyCalib> cal((size_t)numJobs);
+  for (int p = 0; p < numJobs; p++) {
+    essential_zero(E_out + 9 * (size_t)p, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p);
+    counts_out[p] = 0;
+    if (stats_out)
+      for (int k = 0; k < 10; k++) stats_out[10 * (size_t)p + k] = 0;
+    cal[p] = verify_calib(K1s + 9 * (size_t)p, K2s + 9 * (size_t)p);
+    any |= jobs[p].numPairs > 0;
+  }
+  if (!any) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = verify_batch_sync(fn, c, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh, ms)) < 0) return r;
+  for (int p = 0, q = 0; p < numJobs; p++) {
+    if (jobs[p].numPairs == 0) continue;
+    long long st[10];
+    counts_out[p] = verify_essential_result(c->h_verify, q++, jobs[p].numPairs, E_out + 9 * (size_t)p,
+                                            R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
+    if (stats_out)
+      for (int k = 0; k < 10; k++) stats_out[10 * (size_t)p + k] = st[k];
+  }
+  return 0;
 }
 
 // ---- stage-level entry points ----

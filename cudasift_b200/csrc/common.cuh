@@ -241,7 +241,7 @@ struct DeviceCtx {
   GrowBuffer knnLists;        // cs_match_ratio(_host): both directions' neighbour lists
   GrowBuffer pairScratch;     // cs_match_mutual(_host), cs_match_ratio(_host): ballot words, CTA counts, the total
   GrowBuffer knnPartials;     // cs_match_knn2, cs_match_ratio(_host): the slices of the exact scan
-  GrowBuffer verify;          // cs_verify_pairs(_host), cs_verify_models, cs_verify_essential(_host, _models)
+  GrowBuffer verify;          // cs_verify_pairs(_host, _batch), cs_verify_models, cs_verify_essential(_host, _models, _batch)
   GrowBuffer rank;            // cs_rank_records: counters, scratch
   // cs_match_knn2_guided, cs_match_guided(_host): coefficient records, cell grids and the sorted candidate copies
   GrowBuffer guided;
@@ -257,7 +257,8 @@ struct DeviceCtx {
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
   unsigned int *h_tcFlags = nullptr;       // 16: the tensor path's flag area of the last call
   unsigned int *h_pairTotal = nullptr;     // the pair total of the last mutual or ratio call
-  void *h_verify = nullptr;                // the state a verify call copies back
+  void *h_verify = nullptr;                // the states a verify call copies back, and its job table
+  size_t h_verifyBytes = 0;
   unsigned long long *h_guidedStats = nullptr;   // 4: the counters of the last guided call
 
   unsigned long long matchStats[4] = {0, 0, 0, 0};
@@ -339,21 +340,22 @@ int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint
 struct VerifyCalib {
   double K1[9], K2[9];
 };
-size_t verify_scratch_bytes(int numPairs, int numLoops, int model);   // device scratch of one call
-size_t verify_result_bytes();                              // the state copied to the host (pinned) at the end
-// steps 1-4, and with full also 5-8 (arg-max, refit, output); ends with the state copy to h_state on the stream.
-// cal is read for VERIFY_ESSENTIAL only.
-int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *pairs, int numPairs, int model,
-                  const VerifyCalib *cal, int numLoops, float thresh, unsigned long long seed, int *inliers,
-                  int maxInliers, void *scratch, void *h_state, bool full, cudaStream_t st);
-// after a full launch and a synchronize: the inlier count, the pixel model and the statistics
-int verify_result(const void *h_state, int numPairs, double model_out[9], long long stats[8]);
+// A batch of jobs (one for a single call) runs in waves: its non-empty jobs in order, verify_jobs_per_wave() at a time.
+int verify_jobs_per_wave(int numLoops, int model);
+size_t verify_scratch_bytes(const cs_verify_job *jobs, int numJobs, int numLoops, int model);   // device scratch
+size_t verify_host_bytes(int numJobs);                     // the pinned area: the states copied back, the job table
+// Per wave steps 1-4, and with full also 5-8 (arg-max, refit, output), then the wave's state copy to h_pinned, all on
+// the stream.  cal (numJobs entries) is read for VERIFY_ESSENTIAL only.
+int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model, int numLoops, float thresh,
+                  void *scratch, void *h_pinned, bool full, cudaStream_t st);
+// after a full launch and a synchronize: the q-th non-empty job's inlier count, pixel model and statistics
+int verify_result(const void *h_pinned, int q, int numPairs, double model_out[9], long long stats[8]);
 // the same after a full VERIFY_ESSENTIAL launch: E, R, t and the ten statistics of cs_verify_essential_stats
-int verify_essential_result(const void *h_state, int numPairs, double E[9], double R[9], double t[3],
+int verify_essential_result(const void *h_pinned, int q, int numPairs, double E[9], double R[9], double t[3],
                             long long stats[10]);
-// after a launch without full: every slot's pixel model (E for VERIFY_ESSENTIAL), count and the normalisation
-// (synchronizes); returns numValid
-int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
+// after a launch of one job without full: every slot's pixel model (E for VERIFY_ESSENTIAL), count and the
+// normalisation (synchronizes); returns numValid
+int verify_models_to_host(const void *scratch, const void *h_pinned, const cs_verify_job &job, int numLoops, int model,
                           const VerifyCalib *cal, double *h_models, int *h_counts, double h_norm[5], cudaStream_t st);
 
 inline int idivup(int a, int b) { return (a + b - 1) / b; }

@@ -18,7 +18,17 @@
 //                F, re-score, keep the refit unless it has fewer inliers; the final mask (ballot words, CTA counts), the
 //                pixel model and the statistics.
 //   8. write     exclusive prefix of the final mask -> the input pairs {i, j} of the inliers, in input order.
+//
+// Every launch verifies a wave of jobs (cs_verify_pairs_batch; a single call is a wave of one job).  A device table
+// (VerifyJob) gives each job its records, pairs, seed, inlier buffer and intrinsics, and the first CTA of its range in
+// the row kernels (1, 2, 8: one CTA per VP_ROWS pairs, each job on CTAs of its own) and among the point chunks of the
+// scoring kernel (grid y: the model blocks).  A CTA finds its job by binary search over those bases, built on the host.
+// Norm and refit run one CTA per job, hyp and argmax a fixed number of CTAs per job.  Per job, every kernel does what
+// it does for a single call, in the same CTA shapes and reduction orders, so a job's results do not depend on the
+// other jobs of its wave.
+#include <algorithm>
 #include <cmath>
+#include <vector>
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -47,6 +57,30 @@ struct VerifyState {
   double R[9], t[3];
   long long pose[2];
 };
+
+// One job of a wave, as the kernels read it.  Its pair scratch (masks, CTA counts, coordinates, input indices) starts
+// at CTA rowBase of the wave's row space, its model slots at job * slots per job.
+struct VerifyJob {
+  const SiftPoint *s1, *s2;
+  const int2 *pairs;
+  int2 *inliers;
+  unsigned long long seed;
+  int n1, n2, numPairs, maxInliers;
+  int rowBase;                    // its first CTA of the flags / compact / write kernels
+  int scoreBase;                  // its first CTA of the scoring kernel
+  VerifyCalib cal;                // read by the essential kernels only
+};
+
+// The job whose CTA range holds cta: the last j with jobs[j].*base <= cta (bases ascending, every range non-empty).
+__device__ __forceinline__ int vp_job_of(const VerifyJob *jobs, int numJobs, int cta, int VerifyJob::*base)
+{
+  int lo = 0, hi = numJobs - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (jobs[mid].*base <= cta) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
 
 // ---- shared helpers (host and device) --------------------------------------------------------------------------------
 __host__ __device__ inline unsigned long long vp_splitmix64(unsigned long long z)
@@ -251,16 +285,17 @@ __device__ __forceinline__ bool vp_inlier(const float *m, float4 p, float thr2, 
 }
 
 // This thread's exclusive position among the set bits of masks (one word per 32 rows, one count per CTA of VP_ROWS
-// rows), the bit itself in *bit; the last CTA's last warp writes the total to *total when given.
+// rows), the bit itself in *bit, in CTA b of the job's nb; the job's last CTA's last warp writes the total to *total
+// when given.
 __device__ unsigned int vp_scan(const unsigned int *__restrict__ masks, const unsigned int *__restrict__ blockCounts, int n,
-                                bool *bit, int *total)
+                                int b, int nb, bool *bit, int *total)
 {
   __shared__ unsigned int s_w[32];
   __shared__ unsigned int s_base;
   const unsigned int FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   unsigned int part = 0;
-  for (int k = threadIdx.x; k < (int)blockIdx.x; k += VP_ROWS) part += blockCounts[k];
+  for (int k = threadIdx.x; k < b; k += VP_ROWS) part += blockCounts[k];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
   if (lane == 0) s_w[w] = part;
@@ -273,7 +308,7 @@ __device__ unsigned int vp_scan(const unsigned int *__restrict__ masks, const un
   }
   __syncthreads();
   const unsigned int base = s_base;
-  const unsigned int bal = (blockIdx.x * VP_ROWS + w * 32 < n) ? masks[(blockIdx.x * VP_ROWS >> 5) + w] : 0u;
+  const unsigned int bal = (b * VP_ROWS + w * 32 < n) ? masks[(b * VP_ROWS >> 5) + w] : 0u;
   __syncthreads();
   if (lane == 0) s_w[w] = __popc(bal);
   __syncthreads();
@@ -286,7 +321,7 @@ __device__ unsigned int vp_scan(const unsigned int *__restrict__ masks, const un
       if (lane >= o) inc += t;
     }
     s_w[lane] = inc - c;
-    if (total && lane == 31 && blockIdx.x == gridDim.x - 1) *total = (int)(base + inc);
+    if (total && lane == 31 && b == nb - 1) *total = (int)(base + inc);
   }
   __syncthreads();
   *bit = (bal >> lane) & 1u;
@@ -294,36 +329,73 @@ __device__ unsigned int vp_scan(const unsigned int *__restrict__ masks, const un
 }
 
 // ---- kernels ----------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(VP_ROWS)
-vp_flags_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__restrict__ s2, int n2,
-                const int2 *__restrict__ pairs, int numPairs, unsigned int *__restrict__ masks,
-                unsigned int *__restrict__ blockCounts)
+// The scratch of a wave: per row CTA VP_ROWS / 32 mask words, one count and VP_ROWS coordinates and input indices;
+// per job `slots` model slots, their counts and one state.
+struct VerifyWave {
+  const VerifyJob *jobs;
+  int numJobs, slots;
+  unsigned int *masks, *counts;
+  float4 *xy, *un;
+  int *orig;
+  double *models;
+  unsigned int *slotCounts;
+  VerifyState *st;
+};
+
+// One job's part of a wave's scratch.
+struct VerifyJobScratch {
+  unsigned int *masks, *counts;
+  float4 *xy, *un;
+  int *orig;
+  double *models;
+  unsigned int *slotCounts;
+  VerifyState *st;
+};
+
+__device__ __forceinline__ VerifyJobScratch vp_job_scratch(const VerifyWave &w, int j)
 {
-  const int k = blockIdx.x * VP_ROWS + threadIdx.x;
+  const size_t r = (size_t)w.jobs[j].rowBase;
+  return {w.masks + r * (VP_ROWS / 32), w.counts + r, w.xy + r * VP_ROWS, w.un + r * VP_ROWS, w.orig + r * VP_ROWS,
+          w.models + (size_t)j * w.slots * 9, w.slotCounts + (size_t)j * w.slots, w.st + j};
+}
+
+__global__ void __launch_bounds__(VP_ROWS)
+vp_flags_kernel(VerifyWave w)
+{
+  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::rowBase);
+  const VerifyJob &job = w.jobs[j];
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const SiftPoint *__restrict__ s1 = job.s1, *__restrict__ s2 = job.s2;
+  const int n1 = job.n1, n2 = job.n2, numPairs = job.numPairs;
+  const int b = blockIdx.x - job.rowBase;
+  const int k = b * VP_ROWS + threadIdx.x;
   bool keep = false;
   if (k < numPairs) {
-    const int2 p = pairs[k];
+    const int2 p = job.pairs[k];
     if (p.x >= 0 && p.x < n1 && p.y >= 0 && p.y < n2)
       keep = isfinite(s1[p.x].xpos) && isfinite(s1[p.x].ypos) && isfinite(s2[p.y].xpos) && isfinite(s2[p.y].ypos);
   }
   const unsigned int bal = __ballot_sync(0xffffffffu, keep);
-  if ((threadIdx.x & 31) == 0 && k < numPairs) masks[k >> 5] = bal;
+  if ((threadIdx.x & 31) == 0 && k < numPairs) js.masks[k >> 5] = bal;
   const int cnt = __syncthreads_count(keep);
-  if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
+  if (threadIdx.x == 0) js.counts[b] = (unsigned int)cnt;
 }
 
 __global__ void __launch_bounds__(VP_ROWS)
-vp_compact_kernel(const SiftPoint *__restrict__ s1, const SiftPoint *__restrict__ s2, const int2 *__restrict__ pairs,
-                  int numPairs, const unsigned int *__restrict__ masks, const unsigned int *__restrict__ blockCounts,
-                  float4 *__restrict__ xy, int *__restrict__ orig, VerifyState *st)
+vp_compact_kernel(VerifyWave w)
 {
+  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::rowBase);
+  const VerifyJob &job = w.jobs[j];
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const int b = blockIdx.x - job.rowBase;
   bool bit;
-  const unsigned int pos = vp_scan(masks, blockCounts, numPairs, &bit, &st->numValid);
+  const unsigned int pos = vp_scan(js.masks, js.counts, job.numPairs, b, (job.numPairs + VP_ROWS - 1) / VP_ROWS, &bit,
+                                   &js.st->numValid);
   if (bit) {
-    const int k = blockIdx.x * VP_ROWS + threadIdx.x;
-    const int2 p = pairs[k];
-    xy[pos] = make_float4(s1[p.x].xpos, s1[p.x].ypos, s2[p.y].xpos, s2[p.y].ypos);
-    orig[pos] = k;
+    const int k = b * VP_ROWS + threadIdx.x;
+    const int2 p = job.pairs[k];
+    js.xy[pos] = make_float4(job.s1[p.x].xpos, job.s1[p.x].ypos, job.s2[p.y].xpos, job.s2[p.y].ypos);
+    js.orig[pos] = k;
   }
 }
 
@@ -352,10 +424,15 @@ __device__ void vp_block_sum4(double (&v)[4], double (*s_red)[4])
   __syncthreads();
 }
 
+// one CTA per job
 __global__ void __launch_bounds__(1024)
-vp_norm_kernel(const float4 *__restrict__ xy, float4 *__restrict__ un, float thresh, VerifyState *st)
+vp_norm_kernel(VerifyWave w, float thresh)
 {
   __shared__ double s_red[32][4];
+  const VerifyJobScratch js = vp_job_scratch(w, blockIdx.x);
+  const float4 *__restrict__ xy = js.xy;
+  float4 *__restrict__ un = js.un;
+  VerifyState *st = js.st;
   const int n = st->numValid;
   double v[4] = {0, 0, 0, 0};
   for (int k = threadIdx.x; k < n; k += blockDim.x) {
@@ -410,14 +487,19 @@ __device__ inline double vp_cross(double ax, double ay, double bx, double by, do
   return (bx - ax) * (cy - ay) - (by - ay) * (cx - ax);
 }
 
+// idivup(numLoops, VP_HYP_T) CTAs per job
 __global__ void __launch_bounds__(VP_HYP_T)
-vp_hyp_kernel(const float4 *__restrict__ xy, int numLoops, int model, unsigned long long seed, double *__restrict__ models,
-              unsigned int *__restrict__ counts, const VerifyState *st)
+vp_hyp_kernel(VerifyWave w, int numLoops, int model)
 {
-  const int smp = blockIdx.x * VP_HYP_T + threadIdx.x;
+  const int per = (numLoops + VP_HYP_T - 1) / VP_HYP_T, j = blockIdx.x / per;
+  const int smp = (blockIdx.x - j * per) * VP_HYP_T + threadIdx.x;
   if (smp >= numLoops) return;
-  double *slot = models + (size_t)smp * 27;
-  for (int r = 0; r < 3; r++) { slot[9 * r] = CUDART_NAN; counts[3 * smp + r] = 0; }
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const float4 *__restrict__ xy = js.xy;
+  const VerifyState *st = js.st;
+  const unsigned long long seed = w.jobs[j].seed;
+  double *slot = js.models + (size_t)smp * 27;
+  for (int r = 0; r < 3; r++) { slot[9 * r] = CUDART_NAN; js.slotCounts[3 * smp + r] = 0; }
   const int n = st->numValid;
   const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
   if (!(s > 0.0)) return;
@@ -498,22 +580,27 @@ vp_hyp_kernel(const float4 *__restrict__ xy, int numLoops, int model, unsigned l
   }
 }
 
-// one thread per slot (F) or per sample's slot 3s (H: its only model), VP_CHUNK points per CTA
+// one thread per slot (F) or per sample's slot 3s (H: its only model), VP_CHUNK points per CTA; grid (point chunks of
+// all jobs, model blocks): a job's chunks are the idivup(numPairs, VP_CHUNK) CTAs from its scoreBase on
 __global__ void __launch_bounds__(VP_SC_T)
-vp_score_kernel(const float4 *__restrict__ un, const double *__restrict__ models, int numSlots, int model,
-                unsigned int *__restrict__ counts, const VerifyState *st)
+vp_score_kernel(VerifyWave w, int model)
 {
   __shared__ float4 s_p[VP_TILE];
-  const int n = st->numValid;
-  const int p0 = blockIdx.y * VP_CHUNK;
+  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::scoreBase);
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const float4 *__restrict__ un = js.un;
+  const double *__restrict__ models = js.models;
+  const int numSlots = w.slots;
+  const int n = js.st->numValid;
+  const int p0 = (blockIdx.x - w.jobs[j].scoreBase) * VP_CHUNK;
   if (p0 >= n) return;
   const int p1 = min(n, p0 + VP_CHUNK);
-  const int slot = (blockIdx.x * VP_SC_T + threadIdx.x) * (model == CS_GEOM_HOMOGRAPHY ? 3 : 1);
+  const int slot = (blockIdx.y * VP_SC_T + threadIdx.x) * (model == CS_GEOM_HOMOGRAPHY ? 3 : 1);
   float m[9];
   bool live = slot < numSlots && !isnan(models[(size_t)slot * 9]);
   if (live)
     for (int k = 0; k < 9; k++) m[k] = (float)models[(size_t)slot * 9 + k];
-  const float thr2 = st->thr2;
+  const float thr2 = js.st->thr2;
   const bool homography = model == CS_GEOM_HOMOGRAPHY;
   unsigned int cnt = 0;
   for (int t0 = p0; t0 < p1; t0 += VP_TILE) {
@@ -524,15 +611,20 @@ vp_score_kernel(const float4 *__restrict__ un, const double *__restrict__ models
     if (live)
       for (int k = 0; k < tn; k++) cnt += vp_inlier(m, s_p[k], thr2, homography);
   }
-  if (live && cnt) atomicAdd(&counts[slot], cnt);
+  if (live && cnt) atomicAdd(&js.slotCounts[slot], cnt);
 }
 
-// perSample: slots per sample (3 for F and H, 10 for E); a sample counts when its first slot is live
+// perSample: slots per sample (3 for F and H, 10 for E); a sample counts when its first slot is live.
+// idivup(slots, 256) CTAs per job, so that no warp holds two jobs' slots.
 __global__ void __launch_bounds__(256)
-vp_argmax_kernel(const double *__restrict__ models, const unsigned int *__restrict__ counts, int numSlots, int perSample,
-                 VerifyState *st)
+vp_argmax_kernel(VerifyWave w, int perSample)
 {
-  const int slot = blockIdx.x * 256 + threadIdx.x;
+  const int numSlots = w.slots, per = (numSlots + 255) / 256, j = blockIdx.x / per;
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const double *__restrict__ models = js.models;
+  const unsigned int *__restrict__ counts = js.slotCounts;
+  VerifyState *st = js.st;
+  const int slot = (blockIdx.x - j * per) * 256 + threadIdx.x;
   const bool live = slot < numSlots && !isnan(models[(size_t)slot * 9]);
   unsigned long long key = live ? ((unsigned long long)counts[slot] << 32) | (unsigned int)~slot : 0ull;
 #pragma unroll
@@ -622,10 +714,15 @@ __device__ void vp_smallest_eigvec(const double (*s_nm)[45], double (&f)[9])
   for (int i = 0; i < 9; i++) f[i] = V[i][lo];
 }
 
+// one CTA per job
 __global__ void __launch_bounds__(VP_REFIT_T)
-vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, const double *__restrict__ models, int model,
-                unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts, VerifyState *st)
+vp_refit_kernel(VerifyWave w, int model)
 {
+  const VerifyJobScratch js = vp_job_scratch(w, blockIdx.x);
+  const float4 *__restrict__ xy = js.xy, *__restrict__ un = js.un;
+  const double *__restrict__ models = js.models;
+  unsigned int *__restrict__ masks = js.masks, *__restrict__ blockCounts = js.counts;
+  VerifyState *st = js.st;
   __shared__ double s_nm[VP_REFIT_T / 32][45];
   __shared__ double s_m[2][9];         // [0] minimal model, [1] refit
   __shared__ float s_f[9];
@@ -724,15 +821,17 @@ vp_refit_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, co
 }
 
 __global__ void __launch_bounds__(VP_ROWS)
-vp_write_kernel(const int2 *__restrict__ pairs, const int *__restrict__ orig, const unsigned int *__restrict__ masks,
-                const unsigned int *__restrict__ blockCounts, int2 *__restrict__ inliers, int maxInliers,
-                const VerifyState *st)
+vp_write_kernel(VerifyWave w)
 {
-  const int n = st->numValid;
-  if ((int)blockIdx.x * VP_ROWS >= n) return;       // the whole CTA: no thread reaches the scan's barriers
+  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::rowBase);
+  const VerifyJob &job = w.jobs[j];
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const int b = blockIdx.x - job.rowBase;
+  const int n = js.st->numValid;
+  if (b * VP_ROWS >= n) return;                     // the whole CTA: no thread reaches the scan's barriers
   bool bit;
-  const unsigned int pos = vp_scan(masks, blockCounts, n, &bit, nullptr);
-  if (bit && pos < (unsigned int)maxInliers) inliers[pos] = pairs[orig[blockIdx.x * VP_ROWS + threadIdx.x]];
+  const unsigned int pos = vp_scan(js.masks, js.counts, n, b, 0, &bit, nullptr);
+  if (bit && pos < (unsigned int)job.maxInliers) job.inliers[pos] = job.pairs[js.orig[b * VP_ROWS + threadIdx.x]];
 }
 
 // ---- the calibrated path (cs_verify_essential) -------------------------------------------------------------------------
@@ -1088,15 +1187,20 @@ __host__ __device__ inline int vp_five_point(const double (&N)[4][9], double (*E
 }
 
 // one thread per sample: 5 draws, calibrated rows, the null space, the 5-point solver; slot sample*10 + r holds the
-// r-th solution as Fn = G2^T E G1 (unit norm), NaN when empty
+// r-th solution as Fn = G2^T E G1 (unit norm), NaN when empty; idivup(numLoops, VP_HYP_T) CTAs per job
 __global__ void __launch_bounds__(VP_HYP_T)
-vp_hyp5_kernel(const float4 *__restrict__ xy, int numLoops, unsigned long long seed, VerifyCalib cal,
-               double *__restrict__ models, unsigned int *__restrict__ counts, const VerifyState *st)
+vp_hyp5_kernel(VerifyWave w, int numLoops)
 {
-  const int smp = blockIdx.x * VP_HYP_T + threadIdx.x;
+  const int per = (numLoops + VP_HYP_T - 1) / VP_HYP_T, j = blockIdx.x / per;
+  const int smp = (blockIdx.x - j * per) * VP_HYP_T + threadIdx.x;
   if (smp >= numLoops) return;
-  double *slot = models + (size_t)smp * 9 * VP_E_SLOTS;
-  for (int r = 0; r < VP_E_SLOTS; r++) { slot[9 * r] = CUDART_NAN; counts[VP_E_SLOTS * smp + r] = 0; }
+  const VerifyJobScratch js = vp_job_scratch(w, j);
+  const float4 *__restrict__ xy = js.xy;
+  const VerifyState *st = js.st;
+  const unsigned long long seed = w.jobs[j].seed;
+  const VerifyCalib &cal = w.jobs[j].cal;
+  double *slot = js.models + (size_t)smp * 9 * VP_E_SLOTS;
+  for (int r = 0; r < VP_E_SLOTS; r++) { slot[9 * r] = CUDART_NAN; js.slotCounts[VP_E_SLOTS * smp + r] = 0; }
   const int n = st->numValid;
   const double s = st->s;
   if (!(s > 0.0)) return;
@@ -1173,11 +1277,16 @@ __host__ __device__ __forceinline__ bool vp_in_front(const double *R, const doub
 // scaled by lambda = s * (K1[0] K1[4] K2[0] K2[4])^(1/4) (not centred), its smallest eigenvector E' and E = S E' S with
 // S = diag(lambda, lambda, 1), projected to the essential manifold; re-scored as Fn, kept unless it has fewer inliers;
 // the final mask; then the four poses of the final E and the in-front counts over the final inliers.
+// One CTA per job.
 __global__ void __launch_bounds__(VP_REFIT_T)
-vp_refit_e_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, const double *__restrict__ models,
-                  VerifyCalib cal, unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts,
-                  VerifyState *st)
+vp_refit_e_kernel(VerifyWave w)
 {
+  const VerifyJobScratch js = vp_job_scratch(w, blockIdx.x);
+  const float4 *__restrict__ xy = js.xy, *__restrict__ un = js.un;
+  const double *__restrict__ models = js.models;
+  unsigned int *__restrict__ masks = js.masks, *__restrict__ blockCounts = js.counts;
+  VerifyState *st = js.st;
+  const VerifyCalib &cal = w.jobs[blockIdx.x].cal;
   __shared__ double s_nm[VP_REFIT_T / 32][45];
   __shared__ double s_m[2][9];         // Fn of [0] the minimal model, [1] the refit
   __shared__ double s_ep[9];           // the refit's projected E
@@ -1313,33 +1422,73 @@ vp_refit_e_kernel(const float4 *__restrict__ xy, const float4 *__restrict__ un, 
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-struct VerifyLayout {
-  size_t masks, counts, xy, un, orig, models, slotCounts, state, bytes;
-};
-
 // model slots per sample: up to 3 roots of the 7-point cubic (F; H uses the first), up to 10 of the 5-point solver (E)
 static int vp_slots_per_sample(int model) { return model == VERIFY_ESSENTIAL ? VP_E_SLOTS : 3; }
 
-static VerifyLayout verify_layout(int numPairs, int numLoops, int model)
+#define VP_WAVE_BYTES ((size_t)256 << 20)    // model-slot scratch of a wave: 9 doubles and one count per slot
+
+int verify_jobs_per_wave(int numLoops, int model)
+{
+  const size_t perJob = (size_t)vp_slots_per_sample(model) * numLoops * (9 * sizeof(double) + sizeof(unsigned int));
+  const size_t k = VP_WAVE_BYTES / perJob;
+  return k < 1 ? 1 : k > 65536 ? 65536 : (int)k;
+}
+
+// The waves of a batch: its non-empty jobs in input order (live[q] is the input index of the q-th), cut into runs of
+// perWave jobs (the last run may be shorter); rows is the largest number of row CTAs of a wave.
+struct VerifyPlan {
+  std::vector<int> live;
+  int perWave = 1;
+  size_t rows = 0;
+};
+
+static VerifyPlan verify_plan(const cs_verify_job *jobs, int numJobs, int numLoops, int model)
+{
+  VerifyPlan p;
+  p.perWave = verify_jobs_per_wave(numLoops, model);
+  for (int k = 0; k < numJobs; k++)
+    if (jobs[k].numPairs > 0) p.live.push_back(k);
+  for (size_t q0 = 0; q0 < p.live.size(); q0 += p.perWave) {
+    size_t rows = 0;
+    for (size_t q = q0; q < std::min(p.live.size(), q0 + p.perWave); q++) rows += idivup(jobs[p.live[q]].numPairs, VP_ROWS);
+    p.rows = std::max(p.rows, rows);
+  }
+  return p;
+}
+
+struct VerifyLayout {
+  size_t jobs, masks, counts, xy, un, orig, models, slotCounts, state, bytes;
+};
+
+// The device table of the batch's non-empty jobs, then the scratch of one wave (reused by the next).
+static VerifyLayout verify_layout(const VerifyPlan &p, int numLoops, int model)
 {
   VerifyLayout L;
   size_t o = 0;
   auto take = [&](size_t b) { const size_t at = o; o += (b + 255) & ~(size_t)255; return at; };
-  const size_t P = numPairs > 0 ? (size_t)numPairs : 1, S = vp_slots_per_sample(model) * (size_t)numLoops;
-  L.masks = take(((P + 31) / 32) * sizeof(unsigned int));
-  L.counts = take(((P + VP_ROWS - 1) / VP_ROWS) * sizeof(unsigned int));
+  const size_t live = std::max(p.live.size(), (size_t)1), J = std::min(live, (size_t)p.perWave);
+  const size_t P = std::max(p.rows, (size_t)1) * VP_ROWS, S = vp_slots_per_sample(model) * (size_t)numLoops * J;
+  L.jobs = take(live * sizeof(VerifyJob));
+  L.masks = take(P / 32 * sizeof(unsigned int));
+  L.counts = take(P / VP_ROWS * sizeof(unsigned int));
   L.xy = take(P * sizeof(float4));
   L.un = take(P * sizeof(float4));
   L.orig = take(P * sizeof(int));
   L.models = take(S * 9 * sizeof(double));
   L.slotCounts = take(S * sizeof(unsigned int));
-  L.state = take(sizeof(VerifyState));
+  L.state = take(J * sizeof(VerifyState));
   L.bytes = o;
   return L;
 }
 
-size_t verify_scratch_bytes(int numPairs, int numLoops, int model) { return verify_layout(numPairs, numLoops, model).bytes; }
-size_t verify_result_bytes() { return sizeof(VerifyState); }
+size_t verify_scratch_bytes(const cs_verify_job *jobs, int numJobs, int numLoops, int model)
+{
+  return verify_layout(verify_plan(jobs, numJobs, numLoops, model), numLoops, model).bytes;
+}
+
+// The pinned host area of a batch: one state per job (the q-th non-empty job's at q), then the job table.
+static size_t vp_host_states_bytes(int numJobs) { return ((size_t)std::max(numJobs, 1) * sizeof(VerifyState) + 255) & ~(size_t)255; }
+size_t verify_host_bytes(int numJobs) { return vp_host_states_bytes(numJobs) + (size_t)std::max(numJobs, 1) * sizeof(VerifyJob); }
 
 // CUDASIFT_MATCH_TIMING=1: the events between the kernels, printed to stderr
 static void vp_timing_print(cudaEvent_t *tev, int numPairs, int numLoops, int model)
@@ -1354,66 +1503,103 @@ static void vp_timing_print(cudaEvent_t *tev, int numPairs, int numLoops, int mo
   fprintf(stderr, "\n");
 }
 
-// Steps 1-4 (and, with full, 5-8) on the stream; then the state is copied to h_state (pinned, verify_result_bytes()).
-// inliers may be null when maxInliers == 0.  full == false stops after scoring (the models and counts stay in scratch).
-int launch_verify(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const int *pairs, int numPairs, int model,
-                  const VerifyCalib *cal, int numLoops, float thresh, unsigned long long seed, int *inliers,
-                  int maxInliers, void *scratch, void *h_state, bool full, cudaStream_t st)
+// Per wave: steps 1-4 (and, with full, 5-8) on the stream, then the wave's states copied to the pinned area.
+// full == false stops after scoring (the models and counts of the last wave stay in scratch).
+int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model, int numLoops, float thresh,
+                  void *scratch, void *h_pinned, bool full, cudaStream_t st)
 {
-  const VerifyLayout L = verify_layout(numPairs, numLoops, model);
+  const VerifyPlan plan = verify_plan(jobs, numJobs, numLoops, model);
+  const int live = (int)plan.live.size();
+  if (live == 0) return 0;
+  const VerifyLayout L = verify_layout(plan, numLoops, model);
   char *b = static_cast<char *>(scratch);
-  unsigned int *masks = reinterpret_cast<unsigned int *>(b + L.masks), *counts = reinterpret_cast<unsigned int *>(b + L.counts);
-  float4 *xy = reinterpret_cast<float4 *>(b + L.xy), *un = reinterpret_cast<float4 *>(b + L.un);
-  int *orig = reinterpret_cast<int *>(b + L.orig);
-  double *models = reinterpret_cast<double *>(b + L.models);
-  unsigned int *slotCounts = reinterpret_cast<unsigned int *>(b + L.slotCounts);
-  VerifyState *vs = reinterpret_cast<VerifyState *>(b + L.state);
-  const int2 *p2 = reinterpret_cast<const int2 *>(pairs);
+  VerifyState *h_states = static_cast<VerifyState *>(h_pinned);
+  VerifyJob *h_jobs = reinterpret_cast<VerifyJob *>(static_cast<char *>(h_pinned) + vp_host_states_bytes(numJobs));
   const bool essential = model == VERIFY_ESSENTIAL;
-  const int perSample = vp_slots_per_sample(model);
-  const int blocks = idivup(numPairs, VP_ROWS), slots = perSample * numLoops;
-  cudaEvent_t *tev = full ? match_timing_events() : nullptr;
-  if (tev) cudaEventRecord(tev[0], st);
-  vp_flags_kernel<<<blocks, VP_ROWS, 0, st>>>(s1, n1, s2, n2, p2, numPairs, masks, counts);
-  if (tev) cudaEventRecord(tev[1], st);
-  vp_compact_kernel<<<blocks, VP_ROWS, 0, st>>>(s1, s2, p2, numPairs, masks, counts, xy, orig, vs);
-  if (tev) cudaEventRecord(tev[2], st);
-  vp_norm_kernel<<<1, 1024, 0, st>>>(xy, un, thresh, vs);
-  if (tev) cudaEventRecord(tev[3], st);
-  if (essential)
-    vp_hyp5_kernel<<<idivup(numLoops, VP_HYP_T), VP_HYP_T, 0, st>>>(xy, numLoops, seed, *cal, models, slotCounts, vs);
-  else
-    vp_hyp_kernel<<<idivup(numLoops, VP_HYP_T), VP_HYP_T, 0, st>>>(xy, numLoops, model, seed, models, slotCounts, vs);
-  if (tev) cudaEventRecord(tev[4], st);
-  const int scoreModel = essential ? CS_GEOM_FUNDAMENTAL : model;      // E is scored as its Fn
-  const int scoreThreads = model == CS_GEOM_HOMOGRAPHY ? numLoops : slots;
-  vp_score_kernel<<<dim3(idivup(scoreThreads, VP_SC_T), idivup(numPairs, VP_CHUNK)), VP_SC_T, 0, st>>>(un, models, slots,
-                                                                                                      scoreModel, slotCounts,
-                                                                                                      vs);
-  count_launch(5);
-  if (full) {
-    if (tev) cudaEventRecord(tev[5], st);
-    vp_argmax_kernel<<<idivup(slots, 256), 256, 0, st>>>(models, slotCounts, slots, perSample, vs);
-    if (tev) cudaEventRecord(tev[6], st);
-    if (essential)
-      vp_refit_e_kernel<<<1, VP_REFIT_T, 0, st>>>(xy, un, models, *cal, masks, counts, vs);
-    else
-      vp_refit_kernel<<<1, VP_REFIT_T, 0, st>>>(xy, un, models, model, masks, counts, vs);
-    if (tev) cudaEventRecord(tev[7], st);
-    vp_write_kernel<<<blocks, VP_ROWS, 0, st>>>(p2, orig, masks, counts, reinterpret_cast<int2 *>(inliers), maxInliers, vs);
-    if (tev) cudaEventRecord(tev[8], st);
-    count_launch(3);
+  const int perSample = vp_slots_per_sample(model), slots = perSample * numLoops;
+  // the table; the row and score bases count from the first job of each wave
+  int rowBase = 0, scoreBase = 0;
+  for (int q = 0; q < live; q++) {
+    if (q % plan.perWave == 0) rowBase = scoreBase = 0;
+    const cs_verify_job &a = jobs[plan.live[q]];
+    VerifyJob &t = h_jobs[q];
+    t.s1 = static_cast<const SiftPoint *>(a.s1);
+    t.s2 = static_cast<const SiftPoint *>(a.s2);
+    t.pairs = reinterpret_cast<const int2 *>(a.pairs);
+    t.inliers = reinterpret_cast<int2 *>(a.inliers);
+    t.seed = a.seed;
+    t.n1 = a.n1; t.n2 = a.n2; t.numPairs = a.numPairs; t.maxInliers = a.maxInliers;
+    t.rowBase = rowBase;
+    t.scoreBase = scoreBase;
+    t.cal = cal ? cal[plan.live[q]] : VerifyCalib{};
+    rowBase += idivup(a.numPairs, VP_ROWS);
+    scoreBase += idivup(a.numPairs, VP_CHUNK);
   }
-  CS_CUDA(cudaGetLastError());
-  CS_CUDA(cudaMemcpyAsync(h_state, vs, sizeof(VerifyState), cudaMemcpyDeviceToHost, st));
-  if (tev) vp_timing_print(tev, numPairs, numLoops, model);
+  VerifyJob *d_jobs = reinterpret_cast<VerifyJob *>(b + L.jobs);
+  CS_CUDA(cudaMemcpyAsync(d_jobs, h_jobs, (size_t)live * sizeof(VerifyJob), cudaMemcpyHostToDevice, st));
+  VerifyWave w;
+  w.slots = slots;
+  w.masks = reinterpret_cast<unsigned int *>(b + L.masks);
+  w.counts = reinterpret_cast<unsigned int *>(b + L.counts);
+  w.xy = reinterpret_cast<float4 *>(b + L.xy);
+  w.un = reinterpret_cast<float4 *>(b + L.un);
+  w.orig = reinterpret_cast<int *>(b + L.orig);
+  w.models = reinterpret_cast<double *>(b + L.models);
+  w.slotCounts = reinterpret_cast<unsigned int *>(b + L.slotCounts);
+  w.st = reinterpret_cast<VerifyState *>(b + L.state);
+  const int hypPerJob = idivup(numLoops, VP_HYP_T), argPerJob = idivup(slots, 256);
+  const int scoreModel = essential ? CS_GEOM_FUNDAMENTAL : model;      // E is scored as its Fn
+  const int modelBlocks = idivup(model == CS_GEOM_HOMOGRAPHY ? numLoops : slots, VP_SC_T);
+  cudaEvent_t *tev = full ? match_timing_events() : nullptr;
+  for (int q0 = 0; q0 < live; q0 += plan.perWave) {
+    const int nj = std::min(plan.perWave, live - q0);
+    const VerifyJob &last = h_jobs[q0 + nj - 1];
+    const int rows = last.rowBase + idivup(last.numPairs, VP_ROWS);
+    const int chunks = last.scoreBase + idivup(last.numPairs, VP_CHUNK);
+    w.jobs = d_jobs + q0;
+    w.numJobs = nj;
+    if (tev) cudaEventRecord(tev[0], st);
+    vp_flags_kernel<<<rows, VP_ROWS, 0, st>>>(w);
+    if (tev) cudaEventRecord(tev[1], st);
+    vp_compact_kernel<<<rows, VP_ROWS, 0, st>>>(w);
+    if (tev) cudaEventRecord(tev[2], st);
+    vp_norm_kernel<<<nj, 1024, 0, st>>>(w, thresh);
+    if (tev) cudaEventRecord(tev[3], st);
+    if (essential)
+      vp_hyp5_kernel<<<nj * hypPerJob, VP_HYP_T, 0, st>>>(w, numLoops);
+    else
+      vp_hyp_kernel<<<nj * hypPerJob, VP_HYP_T, 0, st>>>(w, numLoops, model);
+    if (tev) cudaEventRecord(tev[4], st);
+    vp_score_kernel<<<dim3(chunks, modelBlocks), VP_SC_T, 0, st>>>(w, scoreModel);
+    count_launch(5);
+    if (full) {
+      if (tev) cudaEventRecord(tev[5], st);
+      vp_argmax_kernel<<<nj * argPerJob, 256, 0, st>>>(w, perSample);
+      if (tev) cudaEventRecord(tev[6], st);
+      if (essential)
+        vp_refit_e_kernel<<<nj, VP_REFIT_T, 0, st>>>(w);
+      else
+        vp_refit_kernel<<<nj, VP_REFIT_T, 0, st>>>(w, model);
+      if (tev) cudaEventRecord(tev[7], st);
+      vp_write_kernel<<<rows, VP_ROWS, 0, st>>>(w);
+      if (tev) cudaEventRecord(tev[8], st);
+      count_launch(3);
+    }
+    CS_CUDA(cudaGetLastError());
+    CS_CUDA(cudaMemcpyAsync(h_states + q0, w.st, (size_t)nj * sizeof(VerifyState), cudaMemcpyDeviceToHost, st));
+    if (tev) {
+      int pairs = 0;
+      for (int q = q0; q < q0 + nj; q++) pairs += h_jobs[q].numPairs;
+      vp_timing_print(tev, pairs, numLoops, model);
+    }
+  }
   return 0;
 }
 
-// After launch_verify and a synchronize: the count, the model and the statistics from the copied state.
-int verify_result(const void *h_state, int numPairs, double model_out[9], long long stats[8])
+// After launch_verify and a synchronize: the q-th non-empty job's count, model and statistics from its copied state.
+int verify_result(const void *h_pinned, int q, int numPairs, double model_out[9], long long stats[8])
 {
-  const VerifyState *v = static_cast<const VerifyState *>(h_state);
+  const VerifyState *v = static_cast<const VerifyState *>(h_pinned) + q;
   for (int k = 0; k < 9; k++) model_out[k] = v->model[k];
   for (int k = 0; k < 8; k++) stats[k] = v->stats[k];
   stats[1] = (long long)numPairs - v->numValid;
@@ -1421,29 +1607,30 @@ int verify_result(const void *h_state, int numPairs, double model_out[9], long l
 }
 
 // The same after an essential launch: E (in model), the pose and the ten statistics.
-int verify_essential_result(const void *h_state, int numPairs, double E[9], double R[9], double t[3], long long stats[10])
+int verify_essential_result(const void *h_pinned, int q, int numPairs, double E[9], double R[9], double t[3],
+                            long long stats[10])
 {
-  const VerifyState *v = static_cast<const VerifyState *>(h_state);
+  const VerifyState *v = static_cast<const VerifyState *>(h_pinned) + q;
   for (int k = 0; k < 9; k++) R[k] = v->R[k];
   for (int k = 0; k < 3; k++) t[k] = v->t[k];
   stats[8] = v->pose[0];
   stats[9] = v->pose[1];
-  return verify_result(h_state, numPairs, E, stats);
+  return verify_result(h_pinned, q, numPairs, E, stats);
 }
 
-// After launch_verify(full = false) and a synchronize: every slot's model in pixel coordinates (NaN-filled when empty),
-// every slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s}.  Returns the number of valid pairs.  An
-// essential slot's Fn becomes E = (T2 K2)^T Fn (T1 K1) with F's output scaling.
-int verify_models_to_host(const void *scratch, const void *h_state, int numPairs, int numLoops, int model,
+// After launch_verify(full = false) of one job and a synchronize: every slot's model in pixel coordinates (NaN-filled
+// when empty), every slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s}.  Returns the number of valid
+// pairs.  An essential slot's Fn becomes E = (T2 K2)^T Fn (T1 K1) with F's output scaling.
+int verify_models_to_host(const void *scratch, const void *h_pinned, const cs_verify_job &job, int numLoops, int model,
                           const VerifyCalib *cal, double *h_models, int *h_counts, double h_norm[5], cudaStream_t st)
 {
-  const VerifyLayout L = verify_layout(numPairs, numLoops, model);
+  const VerifyLayout L = verify_layout(verify_plan(&job, 1, numLoops, model), numLoops, model);
   const char *b = static_cast<const char *>(scratch);
   const size_t S = vp_slots_per_sample(model) * (size_t)numLoops;
   CS_CUDA(cudaMemcpyAsync(h_models, b + L.models, S * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaMemcpyAsync(h_counts, b + L.slotCounts, S * sizeof(int), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaStreamSynchronize(st));
-  const VerifyState *v = static_cast<const VerifyState *>(h_state);
+  const VerifyState *v = static_cast<const VerifyState *>(h_pinned);
   h_norm[0] = v->c1x; h_norm[1] = v->c1y; h_norm[2] = v->c2x; h_norm[3] = v->c2y; h_norm[4] = v->s;
   for (size_t k = 0; k < S; k++) {
     double *m = h_models + 9 * k;

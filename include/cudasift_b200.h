@@ -243,6 +243,46 @@ int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2,
  * cs_verify_stats keeps describing cs_verify_pairs* calls. */
 int cs_verify_essential_stats(long long out[10]);
 
+/* Batched verification: J independent jobs in one call, for example every matched pair of an image collection.  A job
+ * is one image pair's record sets, pair list and seed; model, numLoops and thresh are common to all jobs. */
+typedef struct cs_verify_job {
+  const void *s1; int n1;          /* device SiftPoint records, as cs_verify_pairs */
+  const void *s2; int n2;
+  const int *pairs; int numPairs;  /* device int pairs {i, j}, 8-byte aligned */
+  unsigned long long seed;
+  int *inliers; int maxInliers;    /* device, 8-byte aligned; NULL allowed when maxInliers == 0 */
+} cs_verify_job;
+/* - Equivalence: for job p, models_out[p] (E_out[p], R_out[p], t_out[p]), counts_out[p], the first maxInliers inlier
+ *   pairs and stats_out[p] equal, bit for bit, what a call on that job's fields alone returns:
+ *   cs_verify_pairs(s1, n1, s2, n2, pairs, numPairs, model, numLoops, thresh, seed, ...) and then cs_verify_stats for
+ *   cs_verify_pairs_batch; cs_verify_essential with K1s[p], K2s[p] and then cs_verify_essential_stats for
+ *   cs_verify_essential_batch.  Every other rule is the single call's: validity, sampler, residuals, ties, refit,
+ *   projection, pose and inlier order.  Jobs do not interact: permuting the jobs permutes the results.
+ * - Empty jobs: a job with numPairs == 0 gets a zero model (zero E, R and t), count 0 and zero statistics, and launches
+ *   nothing.  numJobs == 0 returns 0 before any CUDA call (the outputs may then be NULL).
+ * - CS_E_ARG, before any CUDA call, with the first offending job index (jobs[p]) in cs_last_error(): every per-job rule
+ *   of cs_verify_pairs / cs_verify_essential (its sets, pair and inlier buffers; model, numLoops and thresh), numJobs
+ *   outside [0, 65536], NULL jobs with numJobs > 0, NULL models_out / E_out / R_out / t_out or counts_out, NULL or
+ *   invalid K1s / K2s, a total of numPairs over all jobs above INT_MAX, and an inlier buffer that overlaps another
+ *   job's inlier buffer, pair list or record range.  Record sets and pair lists are only read, so jobs may share them
+ *   (one image's records in many pairs, a set paired with itself).  The overlap test sorts the ranges: O(J log J).
+ * - Launches: the non-empty jobs, in order, run in waves.  A wave is the longest run of consecutive non-empty jobs
+ *   (empty jobs skipped) whose model-slot scratch, slots per sample x numLoops x 76 bytes per job (3 slots per sample
+ *   for F and H, 10 for E), fits 256 MiB; it holds at least one job.  Each wave issues the 8 launches of a single
+ *   call, so a batch issues 8 x waves launches (cs_launch_count) with waves = ceil(non-empty jobs / max(1,
+ *   floor(256 MiB / (slots per sample x numLoops x 76 B)))).  The call synchronises with the host once, at the end;
+ *   its scratch lives in the per-device context.  *ms (may be NULL) gets the event time of the call.
+ * - cs_verify_stats and cs_verify_essential_stats keep describing single calls; batch statistics come back only
+ *   through stats_out (NULL: not written).
+ * models_out[J][9], counts_out[J]; stats_out[J][8] may be NULL.  Returns 0 or CS_E_*. */
+int cs_verify_pairs_batch(const cs_verify_job *jobs, int numJobs, int model, int numLoops, float thresh,
+                          double *models_out, int *counts_out, long long *stats_out, double *ms);
+/* K1s, K2s: [J][9] intrinsics per job; E_out[J][9], R_out[J][9], t_out[J][3], counts_out[J];
+ * stats_out[J][10] may be NULL. */
+int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const double *K1s, const double *K2s,
+                              int numLoops, float thresh, double *E_out, double *R_out, double *t_out,
+                              int *counts_out, long long *stats_out, double *ms);
+
 /* Guided matching (COLMAP's guided_matching): the two nearest neighbours and the ratio test restricted to the pairs a
  * model admits.  cs_match_knn2_guided has the semantics of cs_match_knn2 (the reference's score, only scores > 0, the
  * order score descending then index ascending, a missing neighbour is (-1, 0.0f)), except that row i of set 1 only
