@@ -374,41 +374,55 @@ def _pair_array(pairs):
     return np.ascontiguousarray(np.asarray(pairs, np.int32).reshape(-1, 2))
 
 
+def _verify_device(pairs, call):
+    """The shared path of VerifyPairs and VerifyEssential: the pairs in one device buffer, room for as many inliers in
+    another; call(d_pairs, k, d_inliers) makes the library call and returns the inlier count.  Returns the inliers,
+    int32 [m, 2]."""
+    k = len(pairs)
+    bufs = [DeviceBuffer(max(k, 1) * 8), DeviceBuffer(max(k, 1) * 8)]
+    try:
+        if k:
+            bufs[0].upload(pairs)
+        m = call(bufs[0].ptr if k else None, k, bufs[1].ptr if k else None)
+        return bufs[1].download(np.int32, 2 * m).reshape(m, 2) if m else np.zeros((0, 2), np.int32)
+    finally:
+        for b in bufs:
+            b.free()
+
+
+def _verify_host(s1, s2, pairs, call):
+    """The shared path of verify_pairs_host and verify_essential_host: contiguous records and pairs, room for every pair
+    as an inlier; call(s1, s2, pairs, inliers) makes the library call and returns the inlier count.  Returns the
+    inliers, int32 [m, 2]."""
+    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
+    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
+    pairs = _pair_array(pairs)
+    inliers = np.zeros((len(pairs), 2), np.int32)
+    m = call(s1, s2, pairs, inliers)
+    return inliers[:m].copy()
+
+
 def VerifyPairs(data1, data2, pairs, model="fundamental", numLoops=4096, thresh=4.0, seed=0):
     """RANSAC verification of a correspondence list on the device (cs_verify_pairs): pairs is the int32 [k, 2] array of
     (data1 row, data2 row) that MatchSiftDataMutual and MatchSiftDataRatio return.  model: "fundamental" (7-point) or
     "homography" (4-point); thresh in pixels (COLMAP's max_error = 4 by default; Sampson error for F, transfer error
     for H).  Returns (model 3x3 float64 in pixel coordinates, inliers int32 [m, 2] in input order, ms)."""
-    pairs = _pair_array(pairs)
-    k = len(pairs)
     out = np.zeros(9, np.float64)
     ms = ctypes.c_double(0.0)
-    bufs = [DeviceBuffer(max(k, 1) * 8), DeviceBuffer(max(k, 1) * 8)]
-    try:
-        if k:
-            bufs[0].upload(pairs)
-        m = _check(lib().cs_verify_pairs(data1.d_data, data1.numPts, data2.d_data, data2.numPts, bufs[0].ptr if k else None,
-                                         k, _geom_model(model), int(numLoops), float(thresh), int(seed), _ptr(out),
-                                         bufs[1].ptr if k else None, k, ctypes.byref(ms)), "VerifyPairs")
-        inliers = bufs[1].download(np.int32, 2 * m).reshape(m, 2) if m else np.zeros((0, 2), np.int32)
-    finally:
-        for b in bufs:
-            b.free()
+    inliers = _verify_device(_pair_array(pairs), lambda d_pairs, k, d_inliers: _check(lib().cs_verify_pairs(
+        data1.d_data, data1.numPts, data2.d_data, data2.numPts, d_pairs, k, _geom_model(model), int(numLoops),
+        float(thresh), int(seed), _ptr(out), d_inliers, k, ctypes.byref(ms)), "VerifyPairs"))
     return out.reshape(3, 3), inliers, ms.value
 
 
 def verify_pairs_host(s1, s2, pairs, model="fundamental", numLoops=4096, thresh=4.0, seed=0):
     """VerifyPairs on host record arrays (cs_verify_pairs_host); returns (model 3x3 float64, inliers [m, 2] int32, ms)."""
-    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
-    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
-    pairs = _pair_array(pairs)
     out = np.zeros(9, np.float64)
-    inliers = np.zeros((len(pairs), 2), np.int32)
     ms = ctypes.c_double(0.0)
-    m = _check(lib().cs_verify_pairs_host(_ptr(s1), len(s1), _ptr(s2), len(s2), _ptr(pairs), len(pairs),
-                                          _geom_model(model), int(numLoops), float(thresh), int(seed), _ptr(out),
-                                          _ptr(inliers), len(inliers), ctypes.byref(ms)), "cs_verify_pairs_host")
-    return out.reshape(3, 3), inliers[:m].copy(), ms.value
+    inliers = _verify_host(s1, s2, pairs, lambda s1, s2, pairs, inliers: _check(lib().cs_verify_pairs_host(
+        _ptr(s1), len(s1), _ptr(s2), len(s2), _ptr(pairs), len(pairs), _geom_model(model), int(numLoops),
+        float(thresh), int(seed), _ptr(out), _ptr(inliers), len(inliers), ctypes.byref(ms)), "cs_verify_pairs_host"))
+    return out.reshape(3, 3), inliers, ms.value
 
 
 def verify_stats():
@@ -514,40 +528,25 @@ def VerifyEssential(data1, data2, pairs, K1, K2, numLoops=4096, thresh=4.0, seed
     (skew allowed); thresh in pixels (the Sampson error of F = K2^-T E K1^-1, as VerifyPairs' "fundamental").
     Returns (E 3x3, R 3x3, t [3], inliers int32 [m, 2] in input order, ms): E at unit Frobenius norm, X2 = R X1 + t
     with |t| = 1."""
-    pairs = _pair_array(pairs)
-    k = len(pairs)
     E, R, t = np.zeros(9), np.zeros(9), np.zeros(3)
     k1, k2 = _intrinsics(K1), _intrinsics(K2)
     ms = ctypes.c_double(0.0)
-    bufs = [DeviceBuffer(max(k, 1) * 8), DeviceBuffer(max(k, 1) * 8)]
-    try:
-        if k:
-            bufs[0].upload(pairs)
-        m = _check(lib().cs_verify_essential(data1.d_data, data1.numPts, data2.d_data, data2.numPts,
-                                             bufs[0].ptr if k else None, k, _ptr(k1), _ptr(k2), int(numLoops),
-                                             float(thresh), int(seed), _ptr(E), _ptr(R), _ptr(t),
-                                             bufs[1].ptr if k else None, k, ctypes.byref(ms)), "VerifyEssential")
-        inliers = bufs[1].download(np.int32, 2 * m).reshape(m, 2) if m else np.zeros((0, 2), np.int32)
-    finally:
-        for b in bufs:
-            b.free()
+    inliers = _verify_device(_pair_array(pairs), lambda d_pairs, k, d_inliers: _check(lib().cs_verify_essential(
+        data1.d_data, data1.numPts, data2.d_data, data2.numPts, d_pairs, k, _ptr(k1), _ptr(k2), int(numLoops),
+        float(thresh), int(seed), _ptr(E), _ptr(R), _ptr(t), d_inliers, k, ctypes.byref(ms)), "VerifyEssential"))
     return E.reshape(3, 3), R.reshape(3, 3), t, inliers, ms.value
 
 
 def verify_essential_host(s1, s2, pairs, K1, K2, numLoops=4096, thresh=4.0, seed=0):
     """VerifyEssential on host record arrays (cs_verify_essential_host); returns (E, R, t, inliers [m, 2] int32, ms)."""
-    s1 = np.ascontiguousarray(s1, SIFT_DTYPE)
-    s2 = np.ascontiguousarray(s2, SIFT_DTYPE)
-    pairs = _pair_array(pairs)
     E, R, t = np.zeros(9), np.zeros(9), np.zeros(3)
     k1, k2 = _intrinsics(K1), _intrinsics(K2)
-    inliers = np.zeros((len(pairs), 2), np.int32)
     ms = ctypes.c_double(0.0)
-    m = _check(lib().cs_verify_essential_host(_ptr(s1), len(s1), _ptr(s2), len(s2), _ptr(pairs), len(pairs), _ptr(k1),
-                                              _ptr(k2), int(numLoops), float(thresh), int(seed), _ptr(E), _ptr(R),
-                                              _ptr(t), _ptr(inliers), len(inliers), ctypes.byref(ms)),
-               "cs_verify_essential_host")
-    return E.reshape(3, 3), R.reshape(3, 3), t, inliers[:m].copy(), ms.value
+    inliers = _verify_host(s1, s2, pairs, lambda s1, s2, pairs, inliers: _check(lib().cs_verify_essential_host(
+        _ptr(s1), len(s1), _ptr(s2), len(s2), _ptr(pairs), len(pairs), _ptr(k1), _ptr(k2), int(numLoops),
+        float(thresh), int(seed), _ptr(E), _ptr(R), _ptr(t), _ptr(inliers), len(inliers), ctypes.byref(ms)),
+        "cs_verify_essential_host"))
+    return E.reshape(3, 3), R.reshape(3, 3), t, inliers, ms.value
 
 
 def essential_stats():

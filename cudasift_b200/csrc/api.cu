@@ -563,27 +563,54 @@ static int verify_batch_sync(const char *fn, DeviceCtx *c, const cs_verify_job *
   return timed_sync(fn, c, ms, enqueue);
 }
 
-// cs_verify_pairs on device sets and a device pair list: a batch of one job.
-static int verify_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
-                       const int *pairs, int numPairs, int model, int numLoops, float thresh, unsigned long long seed,
-                       double model_out[9], int *inliers, int maxInliers, double *ms)
+// The shared path of cs_verify_pairs_host and cs_verify_essential_host: the sets and the input pairs uploaded, then
+// run(job) -- the single call as a job on them, its inliers after the pairs in the context's pair buffer -- and the
+// inliers copied to h_inliers.  Returns run's total.
+template <class Run>
+static int verify_host_pairs(DeviceCtx *c, const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs,
+                             int numPairs, unsigned long long seed, int *h_inliers, int maxInliers, Run &&run)
 {
-  const cs_verify_job job = verify_job(d1, n1, d2, n2, pairs, numPairs, seed, inliers, maxInliers);
-  const int r = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms);
-  if (r < 0) return r;
-  return verify_result(c->h_verify, 0, numPairs, model_out, c->verifyStats);
+  const int room = maxInliers < numPairs ? maxInliers : numPairs;     // no more inliers can exist
+  // the pair buffer holds the input pairs, then room inliers
+  return host_pairs(c, h_s1, n1, h_s2, n2, (size_t)numPairs + room, numPairs, room, h_inliers,
+                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
+                      CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice,
+                                              c->stream));
+                      return run(verify_job(d1, n1, d2, n2, reinterpret_cast<int *>(pairs), numPairs, seed,
+                                            reinterpret_cast<int *>(pairs + numPairs), room));
+                    });
 }
 
-// cs_verify_essential on device sets and a device pair list: as verify_sync, with the pose.
-static int essential_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
-                          const int *pairs, int numPairs, const VerifyCalib &cal, int numLoops, float thresh,
-                          unsigned long long seed, double E[9], double R[9], double t[3], int *inliers, int maxInliers,
-                          double *ms)
+// The body of cs_verify_pairs_batch and cs_verify_essential_batch after their argument checks: every job's outputs
+// zeroed (zero(p), the count and numStats statistics), the launches when a job has pairs, then every non-empty job's
+// count and statistics from result(q, p, stats), job p being the q-th non-empty one.
+template <class Zero, class Result>
+static int verify_batch_body(const char *fn, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model,
+                             int numLoops, float thresh, int *counts_out, long long *stats_out, int numStats, double *ms,
+                             Zero &&zero, Result &&result)
 {
-  const cs_verify_job job = verify_job(d1, n1, d2, n2, pairs, numPairs, seed, inliers, maxInliers);
-  const int r = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms);
-  if (r < 0) return r;
-  return verify_essential_result(c->h_verify, 0, numPairs, E, R, t, c->essentialStats);
+  bool any = false;
+  for (int p = 0; p < numJobs; p++) {
+    zero(p);
+    counts_out[p] = 0;
+    if (stats_out)
+      for (int k = 0; k < numStats; k++) stats_out[numStats * (size_t)p + k] = 0;
+    any |= jobs[p].numPairs > 0;
+  }
+  if (!any) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  int r;
+  if ((r = verify_batch_sync(fn, c, jobs, numJobs, cal, model, numLoops, thresh, ms)) < 0) return r;
+  for (int p = 0, q = 0; p < numJobs; p++) {
+    if (jobs[p].numPairs == 0) continue;
+    long long st[10];
+    counts_out[p] = result(c->h_verify, q++, p, st);
+    if (stats_out)
+      for (int k = 0; k < numStats; k++) stats_out[numStats * (size_t)p + k] = st[k];
+  }
+  return 0;
 }
 
 // cs_verify_models / cs_verify_essential_models: steps 1-4 of one job, then its slots to the host.
@@ -1260,8 +1287,10 @@ int cs_verify_pairs(const void *d_s1, int n1, const void *d_s2, int n2, const in
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  return verify_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, model, numLoops,
-                     thresh, seed, model_out, d_inliers, maxInliers, ms);
+  const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
+                                       d_inliers, maxInliers);
+  if ((r = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms)) < 0) return r;
+  return verify_result(c->h_verify, 0, numPairs, model_out, c->verifyStats);
 }
 
 int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs, int model,
@@ -1277,16 +1306,11 @@ int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, con
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  const int room = maxInliers < numPairs ? maxInliers : numPairs;     // no more inliers can exist
-  // the pair buffer holds the input pairs, then room inliers
-  return host_pairs(c, h_s1, n1, h_s2, n2, (size_t)numPairs + room, numPairs, room, h_inliers,
-                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
-                      CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice,
-                                              c->stream));
-                      return verify_sync(fn, c, d1, n1, d2, n2, reinterpret_cast<int *>(pairs), numPairs, model,
-                                         numLoops, thresh, seed, model_out, reinterpret_cast<int *>(pairs + numPairs),
-                                         room, ms);
-                    });
+  return verify_host_pairs(c, h_s1, n1, h_s2, n2, h_pairs, numPairs, seed, h_inliers, maxInliers,
+                           [&](const cs_verify_job &job) {
+                             const int q = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms);
+                             return q < 0 ? q : verify_result(c->h_verify, 0, numPairs, model_out, c->verifyStats);
+                           });
 }
 
 int cs_verify_stats(long long out[8])
@@ -1336,8 +1360,11 @@ int cs_verify_essential(const void *d_s1, int n1, const void *d_s2, int n2, cons
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  return essential_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs,
-                        verify_calib(K1, K2), numLoops, thresh, seed, E_out, R_out, t_out, d_inliers, maxInliers, ms);
+  const VerifyCalib cal = verify_calib(K1, K2);
+  const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
+                                       d_inliers, maxInliers);
+  if ((r = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms)) < 0) return r;
+  return verify_essential_result(c->h_verify, 0, numPairs, E_out, R_out, t_out, c->essentialStats);
 }
 
 int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs,
@@ -1356,16 +1383,12 @@ int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2,
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const VerifyCalib cal = verify_calib(K1, K2);
-  const int room = maxInliers < numPairs ? maxInliers : numPairs;     // no more inliers can exist
-  // the pair buffer holds the input pairs, then room inliers
-  return host_pairs(c, h_s1, n1, h_s2, n2, (size_t)numPairs + room, numPairs, room, h_inliers,
-                    [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
-                      CS_CUDA(cudaMemcpyAsync(pairs, h_pairs, (size_t)numPairs * sizeof(int2), cudaMemcpyHostToDevice,
-                                              c->stream));
-                      return essential_sync(fn, c, d1, n1, d2, n2, reinterpret_cast<int *>(pairs), numPairs, cal,
-                                            numLoops, thresh, seed, E_out, R_out, t_out,
-                                            reinterpret_cast<int *>(pairs + numPairs), room, ms);
-                    });
+  return verify_host_pairs(c, h_s1, n1, h_s2, n2, h_pairs, numPairs, seed, h_inliers, maxInliers,
+                           [&](const cs_verify_job &job) {
+                             const int q = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms);
+                             return q < 0 ? q : verify_essential_result(c->h_verify, 0, numPairs, E_out, R_out, t_out,
+                                                                        c->essentialStats);
+                           });
 }
 
 int cs_verify_essential_stats(long long out[10])
@@ -1405,27 +1428,11 @@ int cs_verify_pairs_batch(const cs_verify_job *jobs, int numJobs, int model, int
   int r = verify_batch_args(fn, jobs, numJobs, model, numLoops, thresh, nullptr, nullptr, false);
   if (r < 0) return r;
   if (numJobs > 0 && (!models_out || !counts_out)) return arg_error(fn, "models_out and counts_out must not be NULL");
-  bool any = false;
-  for (int p = 0; p < numJobs; p++) {
-    for (int k = 0; k < 9; k++) models_out[9 * (size_t)p + k] = 0.0;
-    counts_out[p] = 0;
-    if (stats_out)
-      for (int k = 0; k < 8; k++) stats_out[8 * (size_t)p + k] = 0;
-    any |= jobs[p].numPairs > 0;
-  }
-  if (!any) return 0;
-  int err = 0;
-  DeviceCtx *c = current_ctx(&err);
-  if (!c) return err;
-  if ((r = verify_batch_sync(fn, c, jobs, numJobs, nullptr, model, numLoops, thresh, ms)) < 0) return r;
-  for (int p = 0, q = 0; p < numJobs; p++) {
-    if (jobs[p].numPairs == 0) continue;
-    long long st[8];
-    counts_out[p] = verify_result(c->h_verify, q++, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
-    if (stats_out)
-      for (int k = 0; k < 8; k++) stats_out[8 * (size_t)p + k] = st[k];
-  }
-  return 0;
+  return verify_batch_body(fn, jobs, numJobs, nullptr, model, numLoops, thresh, counts_out, stats_out, 8, ms,
+                           [&](int p) { for (int k = 0; k < 9; k++) models_out[9 * (size_t)p + k] = 0.0; },
+                           [&](const void *h, int q, int p, long long *st) {
+                             return verify_result(h, q, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
+                           });
 }
 
 int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const double *K1s, const double *K2s,
@@ -1438,30 +1445,14 @@ int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const doub
   if (r < 0) return r;
   if (numJobs > 0 && (!E_out || !R_out || !t_out || !counts_out))
     return arg_error(fn, "E_out, R_out, t_out and counts_out must not be NULL");
-  bool any = false;
   std::vector<VerifyCalib> cal((size_t)numJobs);
-  for (int p = 0; p < numJobs; p++) {
-    essential_zero(E_out + 9 * (size_t)p, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p);
-    counts_out[p] = 0;
-    if (stats_out)
-      for (int k = 0; k < 10; k++) stats_out[10 * (size_t)p + k] = 0;
-    cal[p] = verify_calib(K1s + 9 * (size_t)p, K2s + 9 * (size_t)p);
-    any |= jobs[p].numPairs > 0;
-  }
-  if (!any) return 0;
-  int err = 0;
-  DeviceCtx *c = current_ctx(&err);
-  if (!c) return err;
-  if ((r = verify_batch_sync(fn, c, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh, ms)) < 0) return r;
-  for (int p = 0, q = 0; p < numJobs; p++) {
-    if (jobs[p].numPairs == 0) continue;
-    long long st[10];
-    counts_out[p] = verify_essential_result(c->h_verify, q++, jobs[p].numPairs, E_out + 9 * (size_t)p,
-                                            R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
-    if (stats_out)
-      for (int k = 0; k < 10; k++) stats_out[10 * (size_t)p + k] = st[k];
-  }
-  return 0;
+  for (int p = 0; p < numJobs; p++) cal[p] = verify_calib(K1s + 9 * (size_t)p, K2s + 9 * (size_t)p);
+  return verify_batch_body(fn, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh, counts_out, stats_out, 10,
+                           ms, [&](int p) { essential_zero(E_out + 9 * (size_t)p, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p); },
+                           [&](const void *h, int q, int p, long long *st) {
+                             return verify_essential_result(h, q, jobs[p].numPairs, E_out + 9 * (size_t)p,
+                                                            R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
+                           });
 }
 
 // ---- stage-level entry points ----

@@ -97,8 +97,23 @@ __host__ __device__ inline void vp_mul33(const double *a, const double *b, doubl
     for (int k = 0; k < 3; k++) c[3 * r + k] = a[3 * r] * b[k] + a[3 * r + 1] * b[3 + k] + a[3 * r + 2] * b[6 + k];
 }
 
+// F's output scaling: unit Frobenius norm, the largest-magnitude entry (the first of equals) positive; false for zero
+__host__ __device__ inline bool vp_unit_sign(double *m)
+{
+  double n = 0.0;
+  int big = 0;
+  for (int k = 0; k < 9; k++) {
+    n += m[k] * m[k];
+    if (fabs(m[k]) > fabs(m[big])) big = k;
+  }
+  if (!(n > 0.0) || !isfinite(n)) return false;
+  const double f = (m[big] < 0 ? -1.0 : 1.0) / sqrt(n);
+  for (int k = 0; k < 9; k++) m[k] *= f;
+  return true;
+}
+
 // a normalised-coordinate model to pixel coordinates and its output scale: H = T2^-1 Hn T1 with H[8] = 1,
-// F = T2^T Fn T1 with unit Frobenius norm and its largest-magnitude entry (the first of equals) positive
+// F = T2^T Fn T1 with F's output scaling (vp_unit_sign)
 __host__ __device__ inline void vp_denormalise(const double *m, int model, double c1x, double c1y, double c2x, double c2y,
                                                double s, double *out)
 {
@@ -117,14 +132,7 @@ __host__ __device__ inline void vp_denormalise(const double *m, int model, doubl
     const double d = out[8];
     if (d != 0.0) for (int k = 0; k < 9; k++) out[k] /= d;
   } else {
-    double n = 0.0;
-    int big = 0;
-    for (int k = 0; k < 9; k++) {
-      n += out[k] * out[k];
-      if (fabs(out[k]) > fabs(out[big])) big = k;
-    }
-    const double f = (out[big] < 0 ? -1.0 : 1.0) / sqrt(n);
-    if (n > 0.0) for (int k = 0; k < 9; k++) out[k] *= f;
+    vp_unit_sign(out);
   }
 }
 
@@ -463,10 +471,12 @@ vp_norm_kernel(VerifyWave w, float thresh)
   }
 }
 
-// The k distinct indices of sample smp into the n valid pairs (the rule of cs_verify_pairs); false after 64 draws.
+// The k distinct indices of sample smp into the n valid pairs (the rule of cs_verify_pairs); false when n < K or after
+// 64 draws.
 template <int K>
 __device__ bool vp_draw(unsigned long long seed, int smp, int n, int (&idx)[K])
 {
+  if (n < K) return false;
   int got = 0;
   for (int d = 0; d < VP_MAX_DRAWS && got < K; d++) {
     const unsigned long long x = vp_splitmix64(seed + 0x9E3779B97F4A7C15ull * (((unsigned long long)smp << 8) | (unsigned)d));
@@ -487,25 +497,40 @@ __device__ inline double vp_cross(double ax, double ay, double bx, double by, do
   return (bx - ax) * (cy - ay) - (by - ay) * (cx - ax);
 }
 
-// idivup(numLoops, VP_HYP_T) CTAs per job
+// One thread's sample in a hypothesis kernel: its job, that job's scratch, the sample's first slot and index.
+struct VerifySample {
+  const VerifyJob *job;
+  VerifyJobScratch js;
+  double *slot;
+  int smp;
+};
+
+// The prologue of the hypothesis kernels (idivup(numLoops, VP_HYP_T) CTAs per job, one thread per sample): the sample's
+// job, its PER slots NaN-filled with zero counts, then the scale check and the K draws of the sample into idx.  false
+// when the thread has no sample or the sample has no draw.
+template <int PER, int K>
+__device__ __forceinline__ bool vp_hyp_prologue(const VerifyWave &w, int numLoops, VerifySample &h, int (&idx)[K])
+{
+  const int per = (numLoops + VP_HYP_T - 1) / VP_HYP_T, j = blockIdx.x / per;
+  h.smp = (blockIdx.x - j * per) * VP_HYP_T + threadIdx.x;
+  if (h.smp >= numLoops) return false;
+  h.job = w.jobs + j;
+  h.js = vp_job_scratch(w, j);
+  h.slot = h.js.models + (size_t)h.smp * 9 * PER;
+  for (int r = 0; r < PER; r++) { h.slot[9 * r] = CUDART_NAN; h.js.slotCounts[PER * h.smp + r] = 0; }
+  return h.js.st->s > 0.0 && vp_draw<K>(h.job->seed, h.smp, h.js.st->numValid, idx);
+}
+
 __global__ void __launch_bounds__(VP_HYP_T)
 vp_hyp_kernel(VerifyWave w, int numLoops, int model)
 {
-  const int per = (numLoops + VP_HYP_T - 1) / VP_HYP_T, j = blockIdx.x / per;
-  const int smp = (blockIdx.x - j * per) * VP_HYP_T + threadIdx.x;
-  if (smp >= numLoops) return;
-  const VerifyJobScratch js = vp_job_scratch(w, j);
-  const float4 *__restrict__ xy = js.xy;
-  const VerifyState *st = js.st;
-  const unsigned long long seed = w.jobs[j].seed;
-  double *slot = js.models + (size_t)smp * 27;
-  for (int r = 0; r < 3; r++) { slot[9 * r] = CUDART_NAN; js.slotCounts[3 * smp + r] = 0; }
-  const int n = st->numValid;
-  const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
-  if (!(s > 0.0)) return;
+  VerifySample h;
   if (model == CS_GEOM_HOMOGRAPHY) {
     int idx[4];
-    if (n < 4 || !vp_draw<4>(seed, smp, n, idx)) return;
+    if (!vp_hyp_prologue<3>(w, numLoops, h, idx)) return;
+    const float4 *__restrict__ xy = h.js.xy;
+    const VerifyState *st = h.js.st;
+    const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
     double u[4][4];
 #pragma unroll
     for (int i = 0; i < 4; i++) {
@@ -529,11 +554,14 @@ vp_hyp_kernel(VerifyWave w, int numLoops, int model)
       for (int j = 0; j < 9; j++) { A[2 * i][j] = r1[j]; A[2 * i + 1][j] = r2[j]; }
     }
     if (!vp_nullspace<8>(A, N)) return;
-    vp_store_unit(slot, N[0]);
+    vp_store_unit(h.slot, N[0]);
     return;
   }
   int idx[7];
-  if (n < 7 || !vp_draw<7>(seed, smp, n, idx)) return;
+  if (!vp_hyp_prologue<3>(w, numLoops, h, idx)) return;
+  const float4 *__restrict__ xy = h.js.xy;
+  const VerifyState *st = h.js.st;
+  const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
   double A[7][9], N[2][9];
 #pragma unroll
   for (int i = 0; i < 7; i++) {
@@ -576,7 +604,7 @@ vp_hyp_kernel(VerifyWave w, int numLoops, int model)
   int r = 0;
   for (int k = 0; k < nr; k++) {
     for (int j = 0; j < 9; j++) M[j] = roots[k] * N[0][j] + (1.0 - roots[k]) * N[1][j];
-    if (vp_store_unit(slot + 9 * r, M)) r++;
+    if (vp_store_unit(h.slot + 9 * r, M)) r++;
   }
 }
 
@@ -714,112 +742,6 @@ __device__ void vp_smallest_eigvec(const double (*s_nm)[45], double (&f)[9])
   for (int i = 0; i < 9; i++) f[i] = V[i][lo];
 }
 
-// one CTA per job
-__global__ void __launch_bounds__(VP_REFIT_T)
-vp_refit_kernel(VerifyWave w, int model)
-{
-  const VerifyJobScratch js = vp_job_scratch(w, blockIdx.x);
-  const float4 *__restrict__ xy = js.xy, *__restrict__ un = js.un;
-  const double *__restrict__ models = js.models;
-  unsigned int *__restrict__ masks = js.masks, *__restrict__ blockCounts = js.counts;
-  VerifyState *st = js.st;
-  __shared__ double s_nm[VP_REFIT_T / 32][45];
-  __shared__ double s_m[2][9];         // [0] minimal model, [1] refit
-  __shared__ float s_f[9];
-  __shared__ int s_cnt[VP_REFIT_T / 32];
-  __shared__ int s_refit;
-  const int n = st->numValid;
-  const bool homography = model == CS_GEOM_HOMOGRAPHY;
-  const unsigned long long key = st->best;
-  const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
-  const float thr2 = st->thr2;
-  const int best = key ? (int)~(unsigned int)key : -1;
-  int cnt0 = 0, cntR = 0, kept = 0;
-  float m[9];
-  if (best >= 0) {
-    if (threadIdx.x < 9) { s_m[0][threadIdx.x] = models[(size_t)best * 9 + threadIdx.x]; s_f[threadIdx.x] = (float)s_m[0][threadIdx.x]; }
-    __syncthreads();
-    for (int k = 0; k < 9; k++) m[k] = s_f[k];
-    // the normal matrix (upper triangle, 45 entries) of the minimal model's inliers
-    double acc[45];
-#pragma unroll
-    for (int k = 0; k < 45; k++) acc[k] = 0.0;
-    int c = 0;
-    for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
-      if (!vp_inlier(m, un[k], thr2, homography)) continue;
-      c++;
-      const float4 p = xy[k];
-      const double x = (p.x - c1x) * s, y = (p.y - c1y) * s, X = (p.z - c2x) * s, Y = (p.w - c2y) * s;
-      // DLT: two rows per point; 8-point: one row (the zero second row adds exact zeros)
-      double r[2][9];
-      if (homography) {
-        const double r1[9] = {x, y, 1, 0, 0, 0, -X * x, -X * y, -X}, r2[9] = {0, 0, 0, x, y, 1, -Y * x, -Y * y, -Y};
-#pragma unroll
-        for (int j = 0; j < 9; j++) { r[0][j] = r1[j]; r[1][j] = r2[j]; }
-      } else {
-        const double r1[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
-#pragma unroll
-        for (int j = 0; j < 9; j++) { r[0][j] = r1[j]; r[1][j] = 0.0; }
-      }
-#pragma unroll
-      for (int q = 0; q < 2; q++) {
-        int e = 0;
-#pragma unroll
-        for (int i = 0; i < 9; i++)
-#pragma unroll
-          for (int j = i; j < 9; j++) acc[e++] += r[q][i] * r[q][j];
-      }
-    }
-    vp_warp_normal(acc, s_nm);
-    cnt0 = vp_block_count(c, s_cnt);
-    if (threadIdx.x == 0) {
-      s_refit = 0;
-      if (cnt0 >= (homography ? 4 : 8)) {
-        double f[9];
-        vp_smallest_eigvec(s_nm, f);
-        if (!homography) {             // rank 2: F (I - v v^T), v the right singular vector of the smallest singular value
-          double B[3][3], W[3][3];
-          for (int i = 0; i < 3; i++)
-            for (int j = 0; j < 3; j++) B[i][j] = f[i] * f[j] + f[3 + i] * f[3 + j] + f[6 + i] * f[6 + j];
-          vp_jacobi<3>(B, W);
-          int l3 = 0;
-          for (int i = 1; i < 3; i++) if (B[i][i] < B[l3][l3]) l3 = i;
-          const double vv[3] = {W[0][l3], W[1][l3], W[2][l3]};
-          for (int r = 0; r < 3; r++) {
-            const double fv = f[3 * r] * vv[0] + f[3 * r + 1] * vv[1] + f[3 * r + 2] * vv[2];
-            for (int j = 0; j < 3; j++) f[3 * r + j] -= fv * vv[j];
-          }
-        }
-        if (vp_store_unit(s_m[1], f)) s_refit = 1;
-      }
-    }
-    __syncthreads();
-    if (s_refit) {
-      for (int k = 0; k < 9; k++) m[k] = (float)s_m[1][k];
-      int cr = 0;
-      for (int k = threadIdx.x; k < n; k += VP_REFIT_T) cr += vp_inlier(m, un[k], thr2, homography);
-      cntR = vp_block_count(cr, s_cnt);
-      kept = cntR >= cnt0;
-    }
-    if (!kept)
-      for (int k = 0; k < 9; k++) m[k] = s_f[k];
-  }
-  const int tot = vp_final_mask(best >= 0 ? m : nullptr, un, n, thr2, homography, masks, blockCounts, s_cnt);
-  if (threadIdx.x == 0) {
-    double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    if (best >= 0) vp_denormalise(kept ? s_m[1] : s_m[0], model, c1x, c1y, c2x, c2y, s, out);
-    for (int k = 0; k < 9; k++) st->model[k] = out[k];
-    st->total = tot;
-    st->stats[0] = n;
-    st->stats[2] = (long long)st->samples;
-    st->stats[3] = (long long)st->models;
-    st->stats[4] = best;
-    st->stats[5] = cnt0;
-    st->stats[6] = kept;
-    st->stats[7] = tot;
-  }
-}
-
 __global__ void __launch_bounds__(VP_ROWS)
 vp_write_kernel(VerifyWave w)
 {
@@ -836,8 +758,8 @@ vp_write_kernel(VerifyWave w)
 
 // ---- the calibrated path (cs_verify_essential) -------------------------------------------------------------------------
 // Steps 1-3 and 5, 6, 8 are the kernels above (scoring with the F test on Fn = T2^-T K2^-T E K1^-1 T1^-1); step 4 is
-// vp_hyp5_kernel (10 slots per sample) and step 7 vp_refit_e_kernel.  The rules are stated in cudasift_b200.h at
-// cs_verify_essential.
+// vp_hyp5_kernel (10 slots per sample) and step 7 vp_refit_kernel<true>.  The rules are stated in
+// cudasift_b200.h at cs_verify_essential.
 #define VP_E_SLOTS 10            // models per sample of the 5-point solver
 #define VP_E_PIVOT 1e-12         // Gauss-Jordan pivot, relative to the largest |entry| of the 10x20 matrix
 #define VP_E_LEAD 1e-12          // leading coefficients of the degree-10 polynomial at or below this (relative) are dropped
@@ -853,14 +775,19 @@ __host__ __device__ inline void vp_calibrate(const double *K, double x, double y
   cx = (x - K[2] - K[1] * cy) / K[0];
 }
 
-// G = K^-1 T^-1 (normalised coordinates -> calibrated) and its inverse TK = T K, T the normalisation u = s (x - c)
-__host__ __device__ inline void vp_calib_maps(const double *K, double cx, double cy, double s, double *G, double *TK)
+// G = K^-1 T^-1: normalised coordinates -> calibrated, T the normalisation u = s (x - c)
+__host__ __device__ inline void vp_norm_to_calib(const double *K, double cx, double cy, double s, double *G)
 {
   const double Ki[9] = {1.0 / K[0], -K[1] / (K[0] * K[4]), (K[1] * K[5] - K[2] * K[4]) / (K[0] * K[4]),
                         0, 1.0 / K[4], -K[5] / K[4], 0, 0, 1};
   const double Ti[9] = {1.0 / s, 0, cx, 0, 1.0 / s, cy, 0, 0, 1};
-  const double T[9] = {s, 0, -s * cx, 0, s, -s * cy, 0, 0, 1};
   vp_mul33(Ki, Ti, G);
+}
+
+// TK = T K, the inverse of G
+__host__ __device__ inline void vp_calib_to_norm(const double *K, double cx, double cy, double s, double *TK)
+{
+  const double T[9] = {s, 0, -s * cx, 0, s, -s * cy, 0, 0, 1};
   vp_mul33(T, K, TK);
 }
 
@@ -874,19 +801,13 @@ __host__ __device__ inline void vp_sandwich(const double *A, const double *M, co
   vp_mul33(t, B, out);
 }
 
-// F's output scaling: unit Frobenius norm, the largest-magnitude entry (the first of equals) positive; false for zero
-__host__ __device__ inline bool vp_unit_sign(double *m)
+// E = (T2 K2)^T Fn (T1 K1): the essential matrix of a stored Fn, under the job's normalisation v
+__host__ __device__ inline void vp_fn_to_e(const VerifyCalib &cal, const VerifyState &v, const double *fn, double *E)
 {
-  double n = 0.0;
-  int big = 0;
-  for (int k = 0; k < 9; k++) {
-    n += m[k] * m[k];
-    if (fabs(m[k]) > fabs(m[big])) big = k;
-  }
-  if (!(n > 0.0) || !isfinite(n)) return false;
-  const double f = (m[big] < 0 ? -1.0 : 1.0) / sqrt(n);
-  for (int k = 0; k < 9; k++) m[k] *= f;
-  return true;
+  double TK1[9], TK2[9];
+  vp_calib_to_norm(cal.K1, v.c1x, v.c1y, v.s, TK1);
+  vp_calib_to_norm(cal.K2, v.c2x, v.c2y, v.s, TK2);
+  vp_sandwich(TK2, fn, TK1, E);
 }
 
 // Polynomials of degree <= 3 in (x, y, z): 20 coefficients in Nister's monomial order
@@ -1187,25 +1108,17 @@ __host__ __device__ inline int vp_five_point(const double (&N)[4][9], double (*E
 }
 
 // one thread per sample: 5 draws, calibrated rows, the null space, the 5-point solver; slot sample*10 + r holds the
-// r-th solution as Fn = G2^T E G1 (unit norm), NaN when empty; idivup(numLoops, VP_HYP_T) CTAs per job
+// r-th solution as Fn = G2^T E G1 (unit norm), NaN when empty
 __global__ void __launch_bounds__(VP_HYP_T)
 vp_hyp5_kernel(VerifyWave w, int numLoops)
 {
-  const int per = (numLoops + VP_HYP_T - 1) / VP_HYP_T, j = blockIdx.x / per;
-  const int smp = (blockIdx.x - j * per) * VP_HYP_T + threadIdx.x;
-  if (smp >= numLoops) return;
-  const VerifyJobScratch js = vp_job_scratch(w, j);
-  const float4 *__restrict__ xy = js.xy;
-  const VerifyState *st = js.st;
-  const unsigned long long seed = w.jobs[j].seed;
-  const VerifyCalib &cal = w.jobs[j].cal;
-  double *slot = js.models + (size_t)smp * 9 * VP_E_SLOTS;
-  for (int r = 0; r < VP_E_SLOTS; r++) { slot[9 * r] = CUDART_NAN; js.slotCounts[VP_E_SLOTS * smp + r] = 0; }
-  const int n = st->numValid;
-  const double s = st->s;
-  if (!(s > 0.0)) return;
+  VerifySample h;
   int idx[5];
-  if (n < 5 || !vp_draw<5>(seed, smp, n, idx)) return;
+  if (!vp_hyp_prologue<VP_E_SLOTS>(w, numLoops, h, idx)) return;
+  const float4 *__restrict__ xy = h.js.xy;
+  const VerifyState *st = h.js.st;
+  const VerifyCalib &cal = h.job->cal;
+  const double s = st->s;
   double A[5][9], N[4][9];
 #pragma unroll
   for (int i = 0; i < 5; i++) {
@@ -1220,14 +1133,14 @@ vp_hyp5_kernel(VerifyWave w, int numLoops)
   if (!vp_nullspace<5>(A, N) || !vp_e_basis(N)) return;
   double E[VP_E_SLOTS][9];
   const int ne = vp_five_point(N, E);
-  double G1[9], G2[9], TK[9];
-  vp_calib_maps(cal.K1, st->c1x, st->c1y, s, G1, TK);
-  vp_calib_maps(cal.K2, st->c2x, st->c2y, s, G2, TK);
+  double G1[9], G2[9];
+  vp_norm_to_calib(cal.K1, st->c1x, st->c1y, s, G1);
+  vp_norm_to_calib(cal.K2, st->c2x, st->c2y, s, G2);
   int r = 0;
   for (int k = 0; k < ne; k++) {
     double fn[9];
     vp_sandwich(G2, E[k], G1, fn);
-    if (vp_store_unit(slot + 9 * r, fn)) r++;
+    if (vp_store_unit(h.slot + 9 * r, fn)) r++;
   }
 }
 
@@ -1273,14 +1186,42 @@ __host__ __device__ __forceinline__ bool vp_in_front(const double *R, const doub
   return ab * bt - at * bb > 0.0 && aa * bt - ab * at > 0.0;      // l1, l2 times the positive determinant
 }
 
-// Step 7 of an essential call, one CTA: the winning Fn's inliers, the 8-point normal matrix on calibrated coordinates
-// scaled by lambda = s * (K1[0] K1[4] K2[0] K2[4])^(1/4) (not centred), its smallest eigenvector E' and E = S E' S with
-// S = diag(lambda, lambda, 1), projected to the essential manifold; re-scored as Fn, kept unless it has fewer inliers;
-// the final mask; then the four poses of the final E and the in-front counts over the final inliers.
-// One CTA per job.
-__global__ void __launch_bounds__(VP_REFIT_T)
-vp_refit_e_kernel(VerifyWave w)
+// ---- step 7: the refit ---------------------------------------------------------------------------------------------
+// rank 2 for F: F (I - v v^T), v the right singular vector of the smallest singular value
+__device__ inline void vp_rank2(double (&f)[9])
 {
+  double B[3][3], W[3][3];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) B[i][j] = f[i] * f[j] + f[3 + i] * f[3 + j] + f[6 + i] * f[6 + j];
+  vp_jacobi<3>(B, W);
+  int l3 = 0;
+  for (int i = 1; i < 3; i++) if (B[i][i] < B[l3][l3]) l3 = i;
+  const double vv[3] = {W[0][l3], W[1][l3], W[2][l3]};
+  for (int r = 0; r < 3; r++) {
+    const double fv = f[3 * r] * vv[0] + f[3 * r + 1] * vv[1] + f[3 * r + 2] * vv[2];
+    for (int j = 0; j < 3; j++) f[3 * r + j] -= fv * vv[j];
+  }
+}
+
+// One CTA per job; model is CS_GEOM_HOMOGRAPHY or CS_GEOM_FUNDAMENTAL, or with ESSENTIAL the essential call.  E is an
+// instantiation of its own rather than a run-time case, so that F and H keep their register count: at 128 registers
+// two CTAs fit an SM and a wave's refits run side by side; E needs more.
+//   1. the winning slot's model and its FP32 inliers;
+//   2. the normal matrix of their rows (45 upper-triangle entries, fixed-order double reduction): the two DLT rows (H)
+//      or the 8-point row (F) on normalised coordinates; for E the 8-point row on calibrated coordinates scaled by
+//      lam = s * (K1[0] K1[4] K2[0] K2[4])^(1/4), not centred;
+//   3. with at least 4 (H) or 8 (F, E) inliers, its smallest eigenvector f (Jacobi);
+//   4. post-processed at unit norm: H as it is; F at rank 2; E = S f S with S = diag(lam, lam, 1), projected to the
+//      essential manifold and stored as Fn;
+//   5. re-scored, and kept unless it has fewer inliers than the minimal model;
+//   6. the final mask (vp_final_mask);
+//   7. the output model (pixel coordinates, or E and the pose) and the statistics.
+template <bool ESSENTIAL>
+__global__ void __launch_bounds__(VP_REFIT_T)
+vp_refit_kernel(VerifyWave w, int model)
+{
+  constexpr bool essential = ESSENTIAL;
+  const bool homography = !essential && model == CS_GEOM_HOMOGRAPHY;
   const VerifyJobScratch js = vp_job_scratch(w, blockIdx.x);
   const float4 *__restrict__ xy = js.xy, *__restrict__ un = js.un;
   const double *__restrict__ models = js.models;
@@ -1288,12 +1229,10 @@ vp_refit_e_kernel(VerifyWave w)
   VerifyState *st = js.st;
   const VerifyCalib &cal = w.jobs[blockIdx.x].cal;
   __shared__ double s_nm[VP_REFIT_T / 32][45];
-  __shared__ double s_m[2][9];         // Fn of [0] the minimal model, [1] the refit
-  __shared__ double s_ep[9];           // the refit's projected E
-  __shared__ double s_R[4][9], s_t[4][3];
+  __shared__ double s_m[essential ? 3 : 2][9];     // [0] minimal model, [1] refit (E: both as Fn), [2] E: projected E
   __shared__ float s_f[9];
   __shared__ int s_cnt[VP_REFIT_T / 32];
-  __shared__ int s_refit, s_pose;
+  __shared__ int s_refit;
   const int n = st->numValid;
   const unsigned long long key = st->best;
   const double s = st->s, c1x = st->c1x, c1y = st->c1y, c2x = st->c2x, c2y = st->c2y;
@@ -1305,41 +1244,66 @@ vp_refit_e_kernel(VerifyWave w)
     if (threadIdx.x < 9) { s_m[0][threadIdx.x] = models[(size_t)best * 9 + threadIdx.x]; s_f[threadIdx.x] = (float)s_m[0][threadIdx.x]; }
     __syncthreads();
     for (int k = 0; k < 9; k++) m[k] = s_f[k];
-    const double lam = s * sqrt(sqrt(cal.K1[0] * cal.K1[4]) * sqrt(cal.K2[0] * cal.K2[4]));
+    const double lam = essential ? s * sqrt(sqrt(cal.K1[0] * cal.K1[4]) * sqrt(cal.K2[0] * cal.K2[4])) : 0.0;
     double acc[45];
 #pragma unroll
     for (int k = 0; k < 45; k++) acc[k] = 0.0;
     int c = 0;
     for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
-      if (!vp_inlier(m, un[k], thr2, false)) continue;
+      if (!vp_inlier(m, un[k], thr2, homography)) continue;
       c++;
       const float4 p = xy[k];
-      double x, y, X, Y;
-      vp_calibrate(cal.K1, p.x, p.y, x, y);
-      vp_calibrate(cal.K2, p.z, p.w, X, Y);
-      x *= lam; y *= lam; X *= lam; Y *= lam;
-      const double r[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
-      int e = 0;
+      double r[2][9];                  // F's zero second row adds exact zeros
+      if constexpr (essential) {
+        double x, y, X, Y;
+        vp_calibrate(cal.K1, p.x, p.y, x, y);
+        vp_calibrate(cal.K2, p.z, p.w, X, Y);
+        x *= lam; y *= lam; X *= lam; Y *= lam;
+        const double r1[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
 #pragma unroll
-      for (int i = 0; i < 9; i++)
+        for (int j = 0; j < 9; j++) r[0][j] = r1[j];
+      } else {
+        const double x = (p.x - c1x) * s, y = (p.y - c1y) * s, X = (p.z - c2x) * s, Y = (p.w - c2y) * s;
+        if (homography) {
+          const double r1[9] = {x, y, 1, 0, 0, 0, -X * x, -X * y, -X}, r2[9] = {0, 0, 0, x, y, 1, -Y * x, -Y * y, -Y};
 #pragma unroll
-        for (int j = i; j < 9; j++) acc[e++] += r[i] * r[j];
+          for (int j = 0; j < 9; j++) { r[0][j] = r1[j]; r[1][j] = r2[j]; }
+        } else {
+          const double r1[9] = {X * x, X * y, X, Y * x, Y * y, Y, x, y, 1};
+#pragma unroll
+          for (int j = 0; j < 9; j++) { r[0][j] = r1[j]; r[1][j] = 0.0; }
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < (essential ? 1 : 2); q++) {
+        int e = 0;
+#pragma unroll
+        for (int i = 0; i < 9; i++)
+#pragma unroll
+          for (int j = i; j < 9; j++) acc[e++] += r[q][i] * r[q][j];
+      }
     }
     vp_warp_normal(acc, s_nm);
     cnt0 = vp_block_count(c, s_cnt);
     if (threadIdx.x == 0) {
       s_refit = 0;
-      if (cnt0 >= 8) {
-        double f[9], E[9], u[3][3], v[3][3];
+      if (cnt0 >= (homography ? 4 : 8)) {
+        double f[9];
         vp_smallest_eigvec(s_nm, f);
-        for (int i = 0; i < 3; i++)
-          for (int j = 0; j < 3; j++) E[3 * i + j] = f[3 * i + j] * (i < 2 ? lam : 1.0) * (j < 2 ? lam : 1.0);
-        if (vp_essential_project(E, s_ep, u, v)) {
-          double G1[9], G2[9], TK[9], fn[9];
-          vp_calib_maps(cal.K1, c1x, c1y, s, G1, TK);
-          vp_calib_maps(cal.K2, c2x, c2y, s, G2, TK);
-          vp_sandwich(G2, s_ep, G1, fn);
-          if (vp_store_unit(s_m[1], fn)) s_refit = 1;
+        if constexpr (essential) {
+          double E[9], u[3][3], v[3][3];
+          for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) E[3 * i + j] = f[3 * i + j] * (i < 2 ? lam : 1.0) * (j < 2 ? lam : 1.0);
+          if (vp_essential_project(E, s_m[2], u, v)) {
+            double G1[9], G2[9], fn[9];
+            vp_norm_to_calib(cal.K1, c1x, c1y, s, G1);
+            vp_norm_to_calib(cal.K2, c2x, c2y, s, G2);
+            vp_sandwich(G2, s_m[2], G1, fn);
+            if (vp_store_unit(s_m[1], fn)) s_refit = 1;
+          }
+        } else {
+          if (!homography) vp_rank2(f);
+          if (vp_store_unit(s_m[1], f)) s_refit = 1;
         }
       }
     }
@@ -1347,69 +1311,77 @@ vp_refit_e_kernel(VerifyWave w)
     if (s_refit) {
       for (int k = 0; k < 9; k++) m[k] = (float)s_m[1][k];
       int cr = 0;
-      for (int k = threadIdx.x; k < n; k += VP_REFIT_T) cr += vp_inlier(m, un[k], thr2, false);
+      for (int k = threadIdx.x; k < n; k += VP_REFIT_T) cr += vp_inlier(m, un[k], thr2, homography);
       cntR = vp_block_count(cr, s_cnt);
       kept = cntR >= cnt0;
     }
     if (!kept)
       for (int k = 0; k < 9; k++) m[k] = s_f[k];
   }
-  const int tot = vp_final_mask(best >= 0 ? m : nullptr, un, n, thr2, false, masks, blockCounts, s_cnt);
-  // the final E and its four poses (R_a = U W V^T, R_b = U W^T V^T; t = +u3, -u3): candidates 0..3 =
-  // (R_a, +), (R_a, -), (R_b, +), (R_b, -)
-  if (threadIdx.x == 0) {
-    s_pose = 0;
-    double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    if (best >= 0) {
-      double E[9], Ep[9], u[3][3], v[3][3];
-      if (kept) {
-        for (int k = 0; k < 9; k++) E[k] = s_ep[k];
-      } else {
-        double G[9], TK1[9], TK2[9];
-        vp_calib_maps(cal.K1, c1x, c1y, s, G, TK1);
-        vp_calib_maps(cal.K2, c2x, c2y, s, G, TK2);
-        vp_sandwich(TK2, s_m[0], TK1, E);
-      }
-      if (vp_essential_project(E, Ep, u, v) && vp_unit_sign(Ep)) {
-        for (int k = 0; k < 9; k++) out[k] = Ep[k];
-        const double tn = 1.0 / sqrt(u[2][0] * u[2][0] + u[2][1] * u[2][1] + u[2][2] * u[2][2]);
-        for (int i = 0; i < 3; i++)
-          for (int j = 0; j < 3; j++) {
-            const double a = u[1][i] * v[0][j] - u[0][i] * v[1][j], b = u[0][i] * v[1][j] - u[1][i] * v[0][j];
-            const double w = u[2][i] * v[2][j];
-            s_R[0][3 * i + j] = s_R[1][3 * i + j] = a + w;
-            s_R[2][3 * i + j] = s_R[3][3 * i + j] = b + w;
-          }
-        for (int i = 0; i < 3; i++) {
-          s_t[0][i] = s_t[2][i] = u[2][i] * tn;
-          s_t[1][i] = s_t[3][i] = -u[2][i] * tn;
+  const int tot = vp_final_mask(best >= 0 ? m : nullptr, un, n, thr2, homography, masks, blockCounts, s_cnt);
+  if constexpr (essential) {
+    // The final E (the kept refit's projected E, else the one recovered from the winning Fn) projected again with F's
+    // output scaling; its four poses R_a = U W V^T, R_b = U W^T V^T and t = +u3, -u3: candidates 0..3 = (R_a, +),
+    // (R_a, -), (R_b, +), (R_b, -); the pose with the most final inliers in front (the first of equals).
+    __shared__ double s_R[4][9], s_t[4][3];
+    __shared__ int s_pose;
+    if (threadIdx.x == 0) {
+      s_pose = 0;
+      double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+      if (best >= 0) {
+        double E[9], Ep[9], u[3][3], v[3][3];
+        if (kept) {
+          for (int k = 0; k < 9; k++) E[k] = s_m[2][k];
+        } else {
+          vp_fn_to_e(cal, *st, s_m[0], E);
         }
-        s_pose = 1;
+        if (vp_essential_project(E, Ep, u, v) && vp_unit_sign(Ep)) {
+          for (int k = 0; k < 9; k++) out[k] = Ep[k];
+          const double tn = 1.0 / sqrt(u[2][0] * u[2][0] + u[2][1] * u[2][1] + u[2][2] * u[2][2]);
+          for (int i = 0; i < 3; i++)
+            for (int j = 0; j < 3; j++) {
+              const double a = u[1][i] * v[0][j] - u[0][i] * v[1][j], b = u[0][i] * v[1][j] - u[1][i] * v[0][j];
+              const double w = u[2][i] * v[2][j];
+              s_R[0][3 * i + j] = s_R[1][3 * i + j] = a + w;
+              s_R[2][3 * i + j] = s_R[3][3 * i + j] = b + w;
+            }
+          for (int i = 0; i < 3; i++) {
+            s_t[0][i] = s_t[2][i] = u[2][i] * tn;
+            s_t[1][i] = s_t[3][i] = -u[2][i] * tn;
+          }
+          s_pose = 1;
+        }
       }
+      for (int k = 0; k < 9; k++) st->model[k] = out[k];
     }
+    __syncthreads();
+    int front[4] = {0, 0, 0, 0};
+    if (s_pose) {
+      for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
+        if (!((masks[k >> 5] >> (k & 31)) & 1u)) continue;
+        const float4 p = xy[k];
+        double x, y, X, Y;
+        vp_calibrate(cal.K1, p.x, p.y, x, y);
+        vp_calibrate(cal.K2, p.z, p.w, X, Y);
+        for (int q = 0; q < 4; q++) front[q] += vp_in_front(s_R[q], s_t[q], x, y, X, Y);
+      }
+      for (int q = 0; q < 4; q++) front[q] = vp_block_count(front[q], s_cnt);
+    }
+    if (threadIdx.x == 0) {
+      int pick = 0, runner = 0;
+      for (int q = 1; q < 4; q++) if (front[q] > front[pick]) pick = q;
+      for (int q = 0; q < 4; q++) if (q != pick) runner = max(runner, front[q]);
+      for (int k = 0; k < 9; k++) st->R[k] = s_pose ? s_R[pick][k] : 0.0;
+      for (int k = 0; k < 3; k++) st->t[k] = s_pose ? s_t[pick][k] : 0.0;
+      st->pose[0] = front[pick];
+      st->pose[1] = runner;
+    }
+  } else if (threadIdx.x == 0) {
+    double out[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    if (best >= 0) vp_denormalise(kept ? s_m[1] : s_m[0], model, c1x, c1y, c2x, c2y, s, out);
     for (int k = 0; k < 9; k++) st->model[k] = out[k];
   }
-  __syncthreads();
-  int front[4] = {0, 0, 0, 0};
-  if (s_pose) {
-    for (int k = threadIdx.x; k < n; k += VP_REFIT_T) {
-      if (!((masks[k >> 5] >> (k & 31)) & 1u)) continue;
-      const float4 p = xy[k];
-      double x, y, X, Y;
-      vp_calibrate(cal.K1, p.x, p.y, x, y);
-      vp_calibrate(cal.K2, p.z, p.w, X, Y);
-      for (int q = 0; q < 4; q++) front[q] += vp_in_front(s_R[q], s_t[q], x, y, X, Y);
-    }
-    for (int q = 0; q < 4; q++) front[q] = vp_block_count(front[q], s_cnt);
-  }
   if (threadIdx.x == 0) {
-    int pick = 0, runner = 0;
-    for (int q = 1; q < 4; q++) if (front[q] > front[pick]) pick = q;
-    for (int q = 0; q < 4; q++) if (q != pick) runner = max(runner, front[q]);
-    for (int k = 0; k < 9; k++) st->R[k] = s_pose ? s_R[pick][k] : 0.0;
-    for (int k = 0; k < 3; k++) st->t[k] = s_pose ? s_t[pick][k] : 0.0;
-    st->pose[0] = front[pick];
-    st->pose[1] = runner;
     st->total = tot;
     st->stats[0] = n;
     st->stats[2] = (long long)st->samples;
@@ -1577,9 +1549,9 @@ int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal
       vp_argmax_kernel<<<nj * argPerJob, 256, 0, st>>>(w, perSample);
       if (tev) cudaEventRecord(tev[6], st);
       if (essential)
-        vp_refit_e_kernel<<<nj, VP_REFIT_T, 0, st>>>(w);
+        vp_refit_kernel<true><<<nj, VP_REFIT_T, 0, st>>>(w, model);
       else
-        vp_refit_kernel<<<nj, VP_REFIT_T, 0, st>>>(w, model);
+        vp_refit_kernel<false><<<nj, VP_REFIT_T, 0, st>>>(w, model);
       if (tev) cudaEventRecord(tev[7], st);
       vp_write_kernel<<<rows, VP_ROWS, 0, st>>>(w);
       if (tev) cudaEventRecord(tev[8], st);
@@ -1637,10 +1609,7 @@ int verify_models_to_host(const void *scratch, const void *h_pinned, const cs_ve
     if (std::isnan(m[0])) { for (int j = 0; j < 9; j++) m[j] = NAN; continue; }
     double out[9];
     if (model == VERIFY_ESSENTIAL) {
-      double G[9], TK1[9], TK2[9];
-      vp_calib_maps(cal->K1, v->c1x, v->c1y, v->s, G, TK1);
-      vp_calib_maps(cal->K2, v->c2x, v->c2y, v->s, G, TK2);
-      vp_sandwich(TK2, m, TK1, out);
+      vp_fn_to_e(*cal, *v, m, out);
       vp_unit_sign(out);
     } else {
       vp_denormalise(m, model, v->c1x, v->c1y, v->c2x, v->c2y, v->s, out);
