@@ -19,7 +19,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "match_knn2", "MatchSiftDataRatio", "match_ratio_host", "VerifyPairs", "verify_pairs_host", "verify_stats",
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
-           "VerifyPairsBatch", "VerifyEssentialBatch"]
+           "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -88,6 +88,7 @@ def lib():
         "cs_verify_essential_models": (ip, [vp, ip, vp, ip, vp, ip, vp, vp, ip, fp, c.c_ulonglong, vp, vp, vp]),
         "cs_verify_pairs_batch": (ip, [vp, ip, ip, ip, fp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_verify_essential_batch": (ip, [vp, ip, vp, vp, ip, fp, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_match_ratio_batch": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -345,6 +346,49 @@ def MatchSiftDataRatio(data1, data2, maxRatio=0.8, maxDistance=0.7, crossCheck=T
     finally:
         d_pairs.free()
     return pairs, ms.value
+
+
+class MatchSet(ctypes.Structure):
+    """cs_match_set: one image's device records in a batched ratio match."""
+    _fields_ = [("pts", ctypes.c_void_p), ("n", ctypes.c_int)]
+
+
+class MatchJob(ctypes.Structure):
+    """cs_match_job: two set indices and the job's device pair buffer."""
+    _fields_ = [("set1", ctypes.c_int), ("set2", ctypes.c_int), ("pairs", ctypes.c_void_p), ("maxPairs", ctypes.c_int)]
+
+
+def MatchSiftDataRatioBatch(datas, jobs, maxRatio=0.8, maxDistance=0.7, crossCheck=True):
+    """MatchSiftDataRatio over many image pairs in one call (cs_match_ratio_batch): datas is a list of SiftData, jobs a
+    list of (a, b) indices into it.  Job p's pairs equal MatchSiftDataRatio(datas[a], datas[b], maxRatio, maxDistance,
+    crossCheck) bit for bit.  Every pair list lives in one device buffer, room for each job's largest count.  Returns
+    (pairs: a list of int32 [k, 2], stats uint64 [J, 4] as match_stats after a mode-2 call, ms)."""
+    sets = (MatchSet * max(len(datas), 1))()
+    for s, d in enumerate(datas):
+        sets[s] = MatchSet(d.d_data, d.numPts)
+    rooms = []
+    for a, b in jobs:
+        n1, n2 = datas[a].numPts, datas[b].numPts
+        rooms.append(min(n1, n2) if crossCheck else n1)
+    offsets = np.concatenate([[0], np.cumsum(rooms, dtype=np.int64)]).astype(np.int64)
+    total = int(offsets[-1])
+    J = len(jobs)
+    counts, stats = np.zeros(J, np.int32), np.zeros((J, 4), np.uint64)
+    ms = ctypes.c_double(0.0)
+    buf = DeviceBuffer(max(total, 1) * 8)
+    try:
+        table = (MatchJob * max(J, 1))()
+        for q, (a, b) in enumerate(jobs):
+            table[q] = MatchJob(int(a), int(b), buf.ptr + 8 * int(offsets[q]) if rooms[q] else None, rooms[q])
+        _check(lib().cs_match_ratio_batch(ctypes.addressof(sets) if datas else None, len(datas),
+                                          ctypes.addressof(table) if J else None, J, float(maxRatio),
+                                          float(maxDistance), int(bool(crossCheck)), _ptr(counts), _ptr(stats),
+                                          ctypes.byref(ms)), "MatchSiftDataRatioBatch")
+        flat = buf.download(np.int32, 2 * total).reshape(-1, 2) if total else np.zeros((0, 2), np.int32)
+    finally:
+        buf.free()
+    pairs = [flat[offsets[q]:offsets[q] + int(counts[q])].copy() for q in range(J)]
+    return pairs, stats, ms.value
 
 
 def match_ratio_host(s1, s2, maxRatio=0.8, maxDistance=0.7, crossCheck=True, mode=0):

@@ -351,6 +351,36 @@ static int check_buffers(const char *fn, const void *s1, int n1, const void *s2,
   return bad[0] ? arg_error(fn, bad) : 0;
 }
 
+// The buffers of a batch call: [lo, hi) of table entry `owner`, its kind, and whether the call writes it.  A written
+// range may share no byte with any other range: overlap_sweep sorts them by start (O(n log n)), and an overlap is then an
+// earlier range that ends after a later one starts.  report(x, y) makes the error of the first overlap found.
+struct SweepRange {
+  uintptr_t lo, hi;
+  int owner, kind;
+  bool out;
+};
+static void sweep_add(std::vector<SweepRange> &rs, const void *b, size_t bytes, int owner, int kind, bool out)
+{
+  if (bytes) rs.push_back({reinterpret_cast<uintptr_t>(b), reinterpret_cast<uintptr_t>(b) + bytes, owner, kind, out});
+}
+template <class Report>
+static int overlap_sweep(std::vector<SweepRange> &rs, Report &&report)
+{
+  std::sort(rs.begin(), rs.end(), [](const SweepRange &a, const SweepRange &b) {
+    return a.lo != b.lo ? a.lo < b.lo : a.kind != b.kind ? a.kind < b.kind : a.owner < b.owner;
+  });
+  const SweepRange *anyEnd = nullptr, *outEnd = nullptr;  // the earlier ranges (and written ones) that end last
+  for (const SweepRange &x : rs) {
+    const SweepRange *hit = nullptr;
+    if (x.out && anyEnd && anyEnd->hi > x.lo) hit = anyEnd;
+    else if (outEnd && outEnd->hi > x.lo) hit = outEnd;
+    if (hit) return report(*hit, x);
+    if (!anyEnd || x.hi > anyEnd->hi) anyEnd = &x;
+    if (x.out && (!outEnd || x.hi > outEnd->hi)) outEnd = &x;
+  }
+  return 0;
+}
+
 // The pairs buffer of the mutual and ratio matchers: maxPairs int2.
 static int check_pairs(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs)
 {
@@ -653,41 +683,67 @@ static int verify_batch_args(const char *fn, const cs_verify_job *jobs, int numJ
       return arg_error(fn, bad);
     }
   }
-  // every non-empty range; a writable one (an inlier buffer) may overlap no other range of another job (its own job's
-  // were checked above).  Sorted by start, an overlap is an earlier range that ends after a later one starts.
-  struct Range { uintptr_t lo, hi; int job, kind; };        // kind 0 inliers, 1 pairs, 2 s1, 3 s2
+  // every non-empty range; a writable one (an inlier buffer, kind 0) may overlap no other range of another job (its own
+  // job's were checked above)
   static const char *const kinds[4] = {"inliers", "pairs", "s1", "s2"};
-  std::vector<Range> rs;
+  std::vector<SweepRange> rs;
   rs.reserve(4 * (size_t)numJobs);
-  auto add = [&](const void *b, size_t bytes, int job, int kind) {
-    if (bytes) rs.push_back({reinterpret_cast<uintptr_t>(b), reinterpret_cast<uintptr_t>(b) + bytes, job, kind});
-  };
   for (int p = 0; p < numJobs; p++) {
     const cs_verify_job &j = jobs[p];
-    add(j.inliers, (size_t)j.maxInliers * sizeof(int2), p, 0);
-    add(j.pairs, (size_t)j.numPairs * sizeof(int2), p, 1);
-    add(j.s1, record_bytes(j.n1), p, 2);
-    add(j.s2, record_bytes(j.n2), p, 3);
+    sweep_add(rs, j.inliers, (size_t)j.maxInliers * sizeof(int2), p, 0, true);
+    sweep_add(rs, j.pairs, (size_t)j.numPairs * sizeof(int2), p, 1, false);
+    sweep_add(rs, j.s1, record_bytes(j.n1), p, 2, false);
+    sweep_add(rs, j.s2, record_bytes(j.n2), p, 3, false);
   }
-  std::sort(rs.begin(), rs.end(), [](const Range &a, const Range &b) {
-    return a.lo != b.lo ? a.lo < b.lo : a.kind != b.kind ? a.kind < b.kind : a.job < b.job;
+  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
+    const SweepRange &a = x.owner <= y.owner ? x : y, &b = x.owner <= y.owner ? y : x;
+    char bad[128];
+    snprintf(bad, sizeof bad, "jobs[%d].%s and jobs[%d].%s overlap (an inlier buffer overlaps another range)", a.owner,
+             kinds[a.kind], b.owner, kinds[b.kind]);
+    return arg_error(fn, bad);
   });
-  const Range *anyEnd = nullptr, *outEnd = nullptr;       // the earlier ranges (and inlier buffers) that end last
-  for (const Range &x : rs) {
-    const Range *hit = nullptr;
-    if (x.kind == 0 && anyEnd && anyEnd->hi > x.lo) hit = anyEnd;
-    else if (outEnd && outEnd->hi > x.lo) hit = outEnd;
-    if (hit) {
-      const Range &a = hit->job <= x.job ? *hit : x, &b = hit->job <= x.job ? x : *hit;
-      char bad[128];
-      snprintf(bad, sizeof bad, "jobs[%d].%s and jobs[%d].%s overlap (an inlier buffer overlaps another range)", a.job,
-               kinds[a.kind], b.job, kinds[b.kind]);
-      return arg_error(fn, bad);
-    }
-    if (!anyEnd || x.hi > anyEnd->hi) anyEnd = &x;
-    if (x.kind == 0 && (!outEnd || x.hi > outEnd->hi)) outEnd = &x;
+}
+
+// The arguments of cs_match_ratio_batch: the common ones, every set (named sets[s]) and job (jobs[p]), then the pair
+// buffers against each other and against every set's records (overlap_sweep).
+static int ratio_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                            float maxRatio, float maxDistance, const int *counts_out)
+{
+  if (numSets < 0 || numSets > 65536) return arg_error(fn, "numSets must be in [0, 65536]");
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numSets > 0 && !sets) return arg_error(fn, "numSets > 0 needs a sets array");
+  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs a jobs array");
+  if (numJobs > 0 && !counts_out) return arg_error(fn, "counts_out must not be NULL");
+  if (std::isnan(maxRatio) || std::isnan(maxDistance)) return arg_error(fn, "maxRatio and maxDistance must not be NaN");
+  char bad[128] = "";
+  for (int s = 0; s < numSets && !bad[0]; s++) {
+    if (sets[s].n < 0) snprintf(bad, sizeof bad, "sets[%d]: n must be >= 0", s);
+    else if (sets[s].n > 0 && !sets[s].pts) snprintf(bad, sizeof bad, "sets[%d]: a set with records needs a pointer", s);
   }
-  return 0;
+  for (int p = 0; p < numJobs && !bad[0]; p++) {
+    const cs_match_job &j = jobs[p];
+    if (j.set1 < 0 || j.set1 >= numSets || j.set2 < 0 || j.set2 >= numSets)
+      snprintf(bad, sizeof bad, "jobs[%d]: set1 and set2 must be in [0, numSets)", p);
+    else if (j.maxPairs < 0) snprintf(bad, sizeof bad, "jobs[%d]: maxPairs must be >= 0", p);
+    else if (j.maxPairs > 0 && !j.pairs) snprintf(bad, sizeof bad, "jobs[%d]: maxPairs > 0 needs a pairs buffer", p);
+    else if (j.maxPairs > 0 && (reinterpret_cast<uintptr_t>(j.pairs) & 7) != 0)
+      snprintf(bad, sizeof bad, "jobs[%d]: pairs must be 8-byte aligned", p);
+  }
+  if (bad[0]) return arg_error(fn, bad);
+  // the pair buffers (kind 0, written) against each other and every set's records (kind 1, read)
+  std::vector<SweepRange> rs;
+  rs.reserve((size_t)numSets + numJobs);
+  for (int p = 0; p < numJobs; p++) sweep_add(rs, jobs[p].pairs, (size_t)jobs[p].maxPairs * sizeof(int2), p, 0, true);
+  for (int s = 0; s < numSets; s++) sweep_add(rs, sets[s].pts, record_bytes(sets[s].n), s, 1, false);
+  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
+    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
+    const SweepRange &b = &a == &x ? y : x;
+    char msg[128];
+    snprintf(msg, sizeof msg, "%s[%d].%s and %s[%d].%s overlap (a pair buffer overlaps another range)",
+             a.kind ? "sets" : "jobs", a.owner, a.kind ? "pts" : "pairs", b.kind ? "sets" : "jobs", b.owner,
+             b.kind ? "pts" : "pairs");
+    return arg_error(fn, msg);
+  });
 }
 
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
@@ -1453,6 +1509,48 @@ int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const doub
                              return verify_essential_result(h, q, jobs[p].numPairs, E_out + 9 * (size_t)p,
                                                             R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
                            });
+}
+
+int cs_match_ratio_batch(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs, float maxRatio,
+                         float maxDistance, int crossCheck, int *counts_out, unsigned long long *stats_out, double *ms)
+{
+  const char *fn = "cs_match_ratio_batch";
+  if (ms) *ms = 0.0;
+  int r = ratio_batch_args(fn, sets, numSets, jobs, numJobs, maxRatio, maxDistance, counts_out);
+  if (r < 0) return r;
+  bool any = false;
+  for (int p = 0; p < numJobs; p++) {
+    counts_out[p] = 0;
+    if (stats_out)
+      for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = 0;
+    any |= sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0;
+  }
+  if (!any) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  std::vector<RatioBatchOut> out((size_t)numJobs);
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return ratio_batch_enqueue(*c, sets, numSets, jobs, numJobs, maxRatio, maxDistance, crossCheck != 0, out.data());
+       })) < 0)
+    return r;
+  for (int p = 0; p < numJobs; p++) {
+    const RatioBatchOut &o = out[p];
+    if (!o.total) continue;                                               // an empty job
+    counts_out[p] = (int)*o.total;
+    if (!stats_out) continue;
+    unsigned long long *st = stats_out + 4 * (size_t)p;
+    if (*o.bad1 || *o.bad2) {                                             // as match_tensor_stats: all exact
+      st[0] = st[1] = 0; st[2] = ~0ull;
+    } else {
+      for (int k = 0; k < 2; k++) {
+        if (!o.counters[k]) continue;
+        st[0] += o.counters[k][1]; st[1] += o.counters[k][2]; st[2] += o.counters[k][0];
+      }
+    }
+    st[3] = 2;
+  }
+  return 0;
 }
 
 // ---- stage-level entry points ----

@@ -252,6 +252,12 @@ struct DeviceCtx {
   bool tcDirty = false;                    // a call returned with an error after it had started to use its flag area
   bool tcConfigured = false;               // the GEMM kernel's shared-memory size is set
   bool tcPendingStats = false;             // h_tcFlags holds the last call's counters, not yet read
+  // cs_match_ratio_batch (besides tcA, tcNorms and tcTables): a wave's set, direction and job tables; its neighbour
+  // lists and fallback entries; its flags, counters and totals (cleared per wave), then the pair scratch
+  GrowBuffer mbTables, mbLists, mbState;
+  bool mbConfigured = false;               // the batch GEMM's shared-memory size is set
+  void *h_mb = nullptr;                    // pinned: every wave's tables (uploaded) and state (copied back)
+  size_t h_mbBytes = 0;
 
   // pinned host words
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
@@ -303,6 +309,68 @@ struct RatioArgs {
 };
 int launch_ratio_pairs(DeviceCtx &c, const int *idx1, const float *score1, int n1, const int *idx2, const float *score2,
                        int n2, const RatioArgs &ra);
+
+// The entry e of a table sorted by a start field (first CTA, first unit) with a[e].*start <= x < a[e + 1].*start;
+// every entry spans at least one.
+template <class T>
+__device__ __forceinline__ int table_find(const T *__restrict__ a, int n, int T::*start, int x)
+{
+  int lo = 0, hi = n - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (a[mid].*start <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// One pair list of the flags / write kernels (match_mutual.cu): the keep test of rows [0, n1) of set 1, then pairs
+// {i, jv[i * jstride]} at positions < maxPairs and the total.  A single call passes one by value; a batch passes a
+// table in device memory, job k owning the CTAs from cta0 on.
+struct PairJob {
+  const int *jv; int jstride;
+  int n1, n2;
+  const int2 *idx1; const float2 *score1;     // ratio: the knn lists of set 1
+  const int2 *idx2; const float2 *score2;     // and of set 2 (cross-check), or null
+  unsigned int *masks, *blockCounts;          // ceil(n1 / 32) ballot words, ceil(n1 / 1024) CTA counts
+  int2 *pairs; int maxPairs;
+  unsigned int *total;
+  int cta0;
+};
+
+// ---- batched ratio matching (cs_match_ratio_batch) ------------------------------------------------------------------
+// A direction of a wave: the n1 rows of set 1 against the n2 candidates of set 2, with its operand tiles, its units of
+// the wave's GEMM, its top-3 table tiles, its resolve CTAs and its neighbour lists.  Built on the host (match_tc.cu).
+struct MbDir {
+  const SiftPoint *s1, *s2;
+  int n1, n2;
+  const float *norms;                 // set 1's row norms
+  const float *bmax;                  // set 2's max norm (float bits)
+  const unsigned int *bad1, *bad2;    // the sets' bad-input flags: either one gates the direction
+  int2 *idx; float2 *score;           // [n1] neighbour lists
+  unsigned int *counters;             // [0] fallback rows, [1] groups re-scored, [2] chains
+  int aTile0, bTile0;                 // set 1's / set 2's first operand tile
+  int n_nt;                           // candidate tiles
+  int u0;                             // first GEMM unit (n_mt x n_nt of them)
+  int gt0;                            // first table tile (n_mt of them)
+  int cta0;                           // first resolve CTA (ceil(n1 / 16) of them)
+};
+// Where the results of job p of a batch land in pinned memory after the call's synchronize: its pair total and, per
+// direction (the second null without the cross-check), the counters and the two sets' bad-input flags.
+struct RatioBatchOut {
+  const unsigned int *total;
+  const unsigned int *counters[2];
+  const unsigned int *bad1, *bad2;
+};
+// Every non-empty job of a batch (argument-checked) in waves on c.stream, without a synchronize; out[p] is filled for
+// the non-empty jobs.
+int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                        float maxRatio, float maxDistance, bool crossCheck, RatioBatchOut *out);
+// the exact top-2 scan of the rows the wave's resolve listed ({direction, row} entries, *numEntries of them)
+int launch_knn_list_fallback(DeviceCtx &c, const MbDir *dirs, const int2 *entries, const unsigned int *numEntries,
+                             int cap);
+// the ratio flags and pair writes of a wave's jobs (numCtas = the CTAs of all jobs)
+int launch_ratio_pairs_batch(DeviceCtx &c, const PairJob *jobs, int numJobs, int numCtas, float maxRatio,
+                             float maxDistance);
 
 // The neighbour order of the exact knn searches (match_knn.cu, match_guided.cu): (s, j) comes before (t, k) when the
 // score is larger, then the index lower.  The empty entry (0, -1) comes after every positive score and before every

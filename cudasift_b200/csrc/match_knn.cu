@@ -183,6 +183,69 @@ int knn_exact(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, in
   return knn_launch(c, s1, n1, s2, n2, idx, score, nullptr, nullptr, nullptr, rowBlocks, slices);
 }
 
+// Fallback of a batch wave: the {direction, row} entries its resolve listed (*numEntries, at most cap), each row of its
+// own direction's set 1 against all n2 candidates of that direction's set 2.  Rows of one wave belong to different sets,
+// so there is no candidate tile to share as in knn_exact_kernel: one warp per entry, the row in shared memory, each lane
+// two candidates at a time with their own FMA chains, then the lanes' top two merged by a butterfly (the order is
+// total, so the result does not depend on which lane saw which candidate).  Grid-strided: the work is the listed rows
+// times their candidates, whatever the number of directions.
+#define KL_WARPS 8
+__global__ void __launch_bounds__(32 * KL_WARPS)
+knn_list_kernel(const MbDir *__restrict__ dirs, const int2 *__restrict__ entries, const unsigned int *__restrict__ numEntries,
+                int cap)
+{
+  __shared__ float4 s_a[KL_WARPS][32];
+  const unsigned int FULL = 0xffffffffu;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int n = min((int)*numEntries, cap);
+  for (int e = blockIdx.x * KL_WARPS + w; e < n; e += gridDim.x * KL_WARPS) {
+    const int2 en = entries[e];
+    const MbDir &D = dirs[en.x];
+    const SiftPoint *__restrict__ s2 = D.s2;
+    const int n2 = D.n2;
+    __syncwarp();
+    s_a[w][lane] = __ldg(reinterpret_cast<const float4 *>(D.s1[en.y].data) + lane);
+    __syncwarp();
+    Top2 t;
+    top2_init(t);
+    for (int j = lane; j < n2; j += 64) {
+      const int k = j + 32;
+      const float4 *b0 = reinterpret_cast<const float4 *>(s2[j].data);
+      const float4 *b1 = reinterpret_cast<const float4 *>(s2[k < n2 ? k : j].data);
+      float acc0 = 0.0f, acc1 = 0.0f;       // the reference's score: sequential k = 0..127 FMA chain from 0
+#pragma unroll 8
+      for (int d = 0; d < 32; d++) {
+        const float4 a = s_a[w][d], x = __ldg(b0 + d), y = __ldg(b1 + d);
+        acc0 = __fmaf_rn(a.x, x.x, acc0); acc1 = __fmaf_rn(a.x, y.x, acc1);
+        acc0 = __fmaf_rn(a.y, x.y, acc0); acc1 = __fmaf_rn(a.y, y.y, acc1);
+        acc0 = __fmaf_rn(a.z, x.z, acc0); acc1 = __fmaf_rn(a.z, y.z, acc1);
+        acc0 = __fmaf_rn(a.w, x.w, acc0); acc1 = __fmaf_rn(a.w, y.w, acc1);
+      }
+      top2_insert(t, acc0, j);
+      if (k < n2) top2_insert(t, acc1, k);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float t1 = __shfl_xor_sync(FULL, t.s1, o), t2 = __shfl_xor_sync(FULL, t.s2, o);
+      const int k1 = __shfl_xor_sync(FULL, t.j1, o), k2 = __shfl_xor_sync(FULL, t.j2, o);
+      top2_insert(t, t1, k1);
+      top2_insert(t, t2, k2);
+    }
+    if (lane == 0) {
+      D.idx[en.y] = make_int2(t.j1, t.j2);
+      D.score[en.y] = make_float2(t.s1, t.s2);
+    }
+  }
+}
+
+int launch_knn_list_fallback(DeviceCtx &c, const MbDir *dirs, const int2 *entries, const unsigned int *numEntries, int cap)
+{
+  knn_list_kernel<<<4 * c.sms, 32 * KL_WARPS, 0, c.stream>>>(dirs, entries, numEntries, cap);
+  count_launch();
+  CS_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // Fallback of the tensor path, decided on the device: the listed rows (usually a few, so the slices are chosen for one
 // row block), or every row if *gate != 0 (grid-strided over at most 296 row blocks).
 int knn_exact_fallback(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score,

@@ -30,18 +30,32 @@ mutual_flags_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *_
   if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
 }
 
+// The pair list of this CTA and the CTA's index in it: the one of a call, or job k of a batch table (jobs != nullptr).
+__device__ __forceinline__ PairJob pair_job(const PairJob &one, const PairJob *__restrict__ jobs, int numJobs, int &blk)
+{
+  if (!jobs) { blk = blockIdx.x; return one; }
+  const PairJob j = jobs[table_find(jobs, numJobs, &PairJob::cta0, (int)blockIdx.x)];
+  blk = (int)blockIdx.x - j.cta0;
+  return j;
+}
+
+// Positions by value: within its pair list, every CTA sums the counts of the CTAs before it; the last writes the total.
 __global__ void __launch_bounds__(MP_ROWS)
-mutual_write_kernel(const int *__restrict__ jv, int jstride, int n1, const unsigned int *__restrict__ masks,
-                    const unsigned int *__restrict__ blockCounts, int2 *__restrict__ pairs, int maxPairs,
-                    unsigned int *__restrict__ total)
+mutual_write_kernel(const PairJob one, const PairJob *__restrict__ jobs, int numJobs)
 {
   __shared__ unsigned int s_w[32];
   __shared__ unsigned int s_base;
+  int blk;
+  const PairJob pj = pair_job(one, jobs, numJobs, blk);
+  const int *__restrict__ jv = pj.jv;
+  const int jstride = pj.jstride, n1 = pj.n1, maxPairs = pj.maxPairs;
+  const unsigned int *__restrict__ masks = pj.masks, *__restrict__ blockCounts = pj.blockCounts;
+  int2 *__restrict__ pairs = pj.pairs;
   const unsigned int FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   // exclusive prefix of this CTA: the counts of the CTAs before it
   unsigned int part = 0;
-  for (int k = threadIdx.x; k < (int)blockIdx.x; k += MP_ROWS) part += blockCounts[k];
+  for (int k = threadIdx.x; k < blk; k += MP_ROWS) part += blockCounts[k];
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
   if (lane == 0) s_w[w] = part;
@@ -55,8 +69,8 @@ mutual_write_kernel(const int *__restrict__ jv, int jstride, int n1, const unsig
   __syncthreads();
   const unsigned int base = s_base;
   // positions inside the CTA: exclusive scan of the warps' ballot counts
-  const int i = blockIdx.x * MP_ROWS + threadIdx.x;
-  const unsigned int bal = (blockIdx.x * MP_ROWS + w * 32 < n1) ? masks[(blockIdx.x * MP_ROWS >> 5) + w] : 0u;
+  const int i = blk * MP_ROWS + threadIdx.x;
+  const unsigned int bal = (blk * MP_ROWS + w * 32 < n1) ? masks[(blk * MP_ROWS >> 5) + w] : 0u;
   if (lane == 0) s_w[w] = __popc(bal);
   __syncthreads();
   if (w == 0) {
@@ -68,7 +82,7 @@ mutual_write_kernel(const int *__restrict__ jv, int jstride, int n1, const unsig
       if (lane >= o) inc += t;
     }
     s_w[lane] = inc - c;
-    if (lane == 31 && blockIdx.x == gridDim.x - 1) *total = base + inc;
+    if (lane == 31 && blk == (n1 - 1) / MP_ROWS) *pj.total = base + inc;
   }
   __syncthreads();
   if ((bal >> lane) & 1u) {
@@ -91,11 +105,14 @@ __device__ __forceinline__ bool ratio_keep(const int2 *__restrict__ idx, const f
 
 // one thread per row i of set 1; idx2 != nullptr: cross-check, row j1 of set 2 must pass as well and name i
 __global__ void __launch_bounds__(MP_ROWS)
-ratio_flags_kernel(const int2 *__restrict__ idx1, const float2 *__restrict__ score1, int n1, const int2 *__restrict__ idx2,
-                   const float2 *__restrict__ score2, int n2, double maxRatio, double maxDistance,
-                   unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts)
+ratio_flags_kernel(const PairJob one, const PairJob *__restrict__ jobs, int numJobs, double maxRatio, double maxDistance)
 {
-  const int i = blockIdx.x * MP_ROWS + threadIdx.x;
+  int blk;
+  const PairJob pj = pair_job(one, jobs, numJobs, blk);
+  const int2 *__restrict__ idx1 = pj.idx1, *__restrict__ idx2 = pj.idx2;
+  const float2 *__restrict__ score1 = pj.score1, *__restrict__ score2 = pj.score2;
+  const int n1 = pj.n1, n2 = pj.n2;
+  const int i = blk * MP_ROWS + threadIdx.x;
   bool keep = false;
   if (i < n1 && ratio_keep(idx1, score1, i, maxRatio, maxDistance)) {
     keep = true;
@@ -105,54 +122,70 @@ ratio_flags_kernel(const int2 *__restrict__ idx1, const float2 *__restrict__ sco
     }
   }
   const unsigned int bal = __ballot_sync(0xffffffffu, keep);
-  if ((threadIdx.x & 31) == 0 && i < n1) masks[i >> 5] = bal;
+  if ((threadIdx.x & 31) == 0 && i < n1) pj.masks[i >> 5] = bal;
   const int cnt = __syncthreads_count(keep);
-  if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
+  if (threadIdx.x == 0) pj.blockCounts[blk] = (unsigned int)cnt;
 }
 
 // Ballot words, CTA counts and the total of n1 rows in c.pairScratch; the total is copied to *c.h_pairTotal after the
 // two launches.
-static int pairs_scratch(DeviceCtx &c, int n1, unsigned int **masks, unsigned int **counts, unsigned int **total)
+static int pairs_scratch(DeviceCtx &c, int n1, PairJob &pj)
 {
   const int blocks = idivup(n1, MP_ROWS), words = idivup(n1, 32);
   int r;
   if ((r = c.pairScratch.grow(((size_t)words + blocks + 1) * sizeof(unsigned int))) < 0) return r;
   if (!c.h_pairTotal) CS_CUDA(cudaMallocHost((void **)&c.h_pairTotal, sizeof(unsigned int)));
-  *masks = c.pairScratch.as<unsigned int>(); *counts = *masks + words; *total = *counts + blocks;
+  pj.n1 = n1;
+  pj.masks = c.pairScratch.as<unsigned int>(); pj.blockCounts = pj.masks + words; pj.total = pj.blockCounts + blocks;
+  pj.cta0 = 0;
   return 0;
 }
 
 int launch_mutual_pairs(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const MutualArgs &mu)
 {
-  unsigned int *masks, *counts, *total;
+  PairJob pj = {};
   int r;
-  if ((r = pairs_scratch(c, n1, &masks, &counts, &total)) < 0) return r;
+  if ((r = pairs_scratch(c, n1, pj)) < 0) return r;
+  pj.jv = &s1[0].match; pj.jstride = (int)(sizeof(SiftPoint) / sizeof(int));
+  pj.pairs = mu.pairs; pj.maxPairs = mu.maxPairs;
   const int blocks = idivup(n1, MP_ROWS);
-  mutual_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, masks, counts);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(&s1[0].match, (int)(sizeof(SiftPoint) / sizeof(int)), n1, masks,
-                                                        counts, mu.pairs, mu.maxPairs, total);
+  mutual_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, pj.masks,
+                                                        pj.blockCounts);
+  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(pj, nullptr, 0);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
-  CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
+  CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, pj.total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
   return 0;
 }
 
 int launch_ratio_pairs(DeviceCtx &c, const int *idx1, const float *score1, int n1, const int *idx2, const float *score2,
                        int n2, const RatioArgs &ra)
 {
-  unsigned int *masks, *counts, *total;
+  PairJob pj = {};
   int r;
-  if ((r = pairs_scratch(c, n1, &masks, &counts, &total)) < 0) return r;
+  if ((r = pairs_scratch(c, n1, pj)) < 0) return r;
+  pj.jv = idx1; pj.jstride = 2; pj.n2 = n2;
+  pj.idx1 = reinterpret_cast<const int2 *>(idx1); pj.score1 = reinterpret_cast<const float2 *>(score1);
+  pj.idx2 = reinterpret_cast<const int2 *>(idx2); pj.score2 = reinterpret_cast<const float2 *>(score2);
+  pj.pairs = ra.pairs; pj.maxPairs = ra.maxPairs;
   const int blocks = idivup(n1, MP_ROWS);
-  ratio_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(reinterpret_cast<const int2 *>(idx1),
-                                                       reinterpret_cast<const float2 *>(score1), n1,
-                                                       reinterpret_cast<const int2 *>(idx2),
-                                                       reinterpret_cast<const float2 *>(score2), n2, (double)ra.maxRatio,
-                                                       (double)ra.maxDistance, masks, counts);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(idx1, 2, n1, masks, counts, ra.pairs, ra.maxPairs, total);
+  ratio_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(pj, nullptr, 0, (double)ra.maxRatio, (double)ra.maxDistance);
+  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(pj, nullptr, 0);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
-  CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
+  CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, pj.total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
+  return 0;
+}
+
+// A batch wave: the ratio test and the pair writes of every job of the table, each job's CTAs from its cta0 on.
+int launch_ratio_pairs_batch(DeviceCtx &c, const PairJob *jobs, int numJobs, int numCtas, float maxRatio,
+                             float maxDistance)
+{
+  const PairJob none = {};
+  ratio_flags_kernel<<<numCtas, MP_ROWS, 0, c.stream>>>(none, jobs, numJobs, (double)maxRatio, (double)maxDistance);
+  mutual_write_kernel<<<numCtas, MP_ROWS, 0, c.stream>>>(none, jobs, numJobs);
+  count_launch(2);
+  CS_CUDA(cudaGetLastError());
   return 0;
 }
 

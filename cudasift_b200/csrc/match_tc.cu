@@ -24,6 +24,9 @@
 
 #include <cuda_fp16.h>
 
+#include <algorithm>
+#include <vector>
+
 namespace cs {
 
 #define TC_KCH 16           // 16-byte chunks (8 halves) per descriptor
@@ -74,13 +77,17 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
 }
 
 // ------------------------------------------------------------------------------ workspace
+// The GEMM's units (A tile, B tile) are numbered in row-tile order, and CTA c takes units [c U, (c + 1) U).  In a batch
+// wave the units of its directions follow each other (MbDir::u0) and U, total and grid cover all of them.
 struct TcPlan {
-  int n1, n2v, n_mt, n_nt, total, U, runs, grid;
+  int n1, n2v, n_mt, n_nt, total, U, grid;
 };
-// slot of (cta, run, row-in-tile)
-__device__ __forceinline__ size_t tc_slot(const TcPlan &pl, int cta, int run, int rowInTile)
+// The top-3 tables hold one entry per (A tile, segment): the units of row tile t (numbered over all directions of a
+// wave) that CTA c runs.  Along the units both t and c only grow and one of them steps at every new segment, so t + c
+// numbers the segments without gaps or repeats: slot (t + c) * 128 + row-in-tile, (tiles + grid) * 128 slots.
+__device__ __forceinline__ size_t tc_slot(int tile, int cta, int rowInTile)
 {
-  return ((size_t)cta * pl.runs + run) * 128 + rowInTile;   // 128 = rows per CTA tile (T3_MT)
+  return (size_t)(tile + cta) * 128 + rowInTile;           // 128 = rows per CTA tile (T3_MT)
 }
 
 // ------------------------------------------------------------------------------ single-pass matcher
@@ -173,18 +180,31 @@ struct T3PrepSet {
   int bTiles;             // tiles of the B role: ceil(nv / 128)
   float *norms;           // per row, A role
   float *bmax;            // max norm over rows < nv (float bits): the error bound of the other direction
+  float *bad;             // batch: the set's bad-input flag
+  int blk0;               // batch: its first CTA
 };
 
-// block = 32 rows x 16 chunks; CTAs [0, s0.blocks) take set 1, the rest set 2
+// block = 32 rows x 16 chunks.  A call: CTAs [0, s0.blocks) take set 1, the rest set 2, a bad value raises *gate.  A
+// batch wave (TABLE): the table's sets, each from its blk0 on, each with its own flag.
+template <bool TABLE>
 __global__ void __launch_bounds__(512)
-t3_prep_kernel(const T3PrepSet s0, const T3PrepSet s1, float *__restrict__ gate, float *__restrict__ nextFlags)
+t3_prep_kernel(const T3PrepSet s0, const T3PrepSet s1, const T3PrepSet *__restrict__ sets, int numSets,
+               float *__restrict__ gate, float *__restrict__ nextFlags)
 {
   __shared__ float s_sq[16][33];
   __shared__ int s_bad;
-  if (blockIdx.x == 0 && threadIdx.x < 16) nextFlags[threadIdx.x] = 0.0f;   // the next call's flag area
-  const bool second = (int)blockIdx.x >= s0.blocks;
-  const T3PrepSet s = second ? s1 : s0;
-  const int blk = second ? (int)blockIdx.x - s0.blocks : (int)blockIdx.x;
+  T3PrepSet s;
+  int blk;
+  if (TABLE) {
+    s = sets[table_find(sets, numSets, &T3PrepSet::blk0, (int)blockIdx.x)];
+    blk = (int)blockIdx.x - s.blk0;
+    gate = s.bad;
+  } else {
+    if (blockIdx.x == 0 && threadIdx.x < 16) nextFlags[threadIdx.x] = 0.0f;   // the next call's flag area
+    const bool second = (int)blockIdx.x >= s0.blocks;
+    s = second ? s1 : s0;
+    blk = second ? (int)blockIdx.x - s0.blocks : (int)blockIdx.x;
+  }
   const int lane = threadIdx.x & 31, c = threadIdx.x >> 5;
   const int row = blk * 32 + lane;
   // nv is a multiple of 32: the CTA's rows lie all below nv (candidates of the other direction) or none of them
@@ -225,8 +245,35 @@ t3_prep_kernel(const T3PrepSet s0, const T3PrepSet s1, float *__restrict__ gate,
   }
 }
 
+// Unit u of the GEMM: its table tile, its A and B operand tiles (in a16 / b16), its candidate tile nt in the direction,
+// and whether it is the last unit of its row tile.  A call has one direction, its tiles in row-tile order; a batch wave
+// (TABLE) has a table of directions, d the one of the previous unit (the units only grow).
+struct T3Unit {
+  int gt, aTile, bTile, nt;
+  bool last;
+};
+template <bool TABLE>
+__device__ __forceinline__ T3Unit t3_unit(const TcPlan &pl, const MbDir *__restrict__ dirs, int numDirs, int &d, int u)
+{
+  T3Unit r;
+  if (TABLE) {
+    while (d + 1 < numDirs && dirs[d + 1].u0 <= u) d++;
+    const int n_nt = dirs[d].n_nt, l = u - dirs[d].u0, mt = l / n_nt;
+    r.nt = l - mt * n_nt;
+    r.gt = dirs[d].gt0 + mt; r.aTile = dirs[d].aTile0 + mt; r.bTile = dirs[d].bTile0 + r.nt;
+    r.last = r.nt == n_nt - 1;
+  } else {
+    const int mt = u / pl.n_nt;
+    r.nt = u - mt * pl.n_nt;
+    r.gt = r.aTile = mt; r.bTile = r.nt;
+    r.last = (u + 1) / pl.n_nt != mt;
+  }
+  return r;
+}
+
+template <bool TABLE>
 __global__ void __launch_bounds__(T3_THREADS, 1)
-t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
+t3_gemm_kernel(const TcPlan pl, const T3Buffers bf, const MbDir *__restrict__ dirs, int numDirs)
 {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -249,20 +296,23 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
   if (warp == 0) {
     // ============================ producer: bulk copies of whole operand tiles ============================
     if (lane == 0) {
-      int runIdx = 0, prevMt = -1;
+      int runIdx = 0, prevGt = -1;
+      int d = TABLE ? table_find(dirs, numDirs, &MbDir::u0, u_begin) : 0;
       for (int u = u_begin, i = 0; u < u_end; u++, i++) {
-        const int mt = u / pl.n_nt, nt = u - mt * pl.n_nt;
-        if (mt != prevMt) {
+        const T3Unit un = t3_unit<TABLE>(pl, dirs, numDirs, d, u);
+        if (un.gt != prevGt) {
           // every MMA of the previous run must have read the A tile before it is overwritten
           if (runIdx > 0) mbarrier_wait(&bar_a_empty, (runIdx - 1) & 1);
           mbarrier_expect_tx(&bar_a_full, T3_A_BYTES);
-          bulk_g2s(sA, reinterpret_cast<const uint8_t *>(bf.a16) + (size_t)mt * T3_A_BYTES, T3_A_BYTES, &bar_a_full);
-          prevMt = mt; runIdx++;
+          bulk_g2s(sA, reinterpret_cast<const uint8_t *>(bf.a16) + (size_t)un.aTile * T3_A_BYTES, T3_A_BYTES,
+                   &bar_a_full);
+          prevGt = un.gt; runIdx++;
         }
         const int s = i % T3_STAGES, it = i / T3_STAGES;
         if (it > 0) mbarrier_wait(&bar_b_empty[s], (it - 1) & 1);
         mbarrier_expect_tx(&bar_b_full[s], T3_B_BYTES);
-        bulk_g2s(sB + s * T3_B_BYTES, reinterpret_cast<const uint8_t *>(bf.b16) + (size_t)nt * T3_B_BYTES, T3_B_BYTES, &bar_b_full[s]);
+        bulk_g2s(sB + s * T3_B_BYTES, reinterpret_cast<const uint8_t *>(bf.b16) + (size_t)un.bTile * T3_B_BYTES,
+                 T3_B_BYTES, &bar_b_full[s]);
       }
     }
   } else if (warp >= 4) {
@@ -278,14 +328,15 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
     // [fragment row][partition 2q + hb]
     float g1[2][4], g2[2][4], g3[2][4];
     int i1[2][4], i2[2][4];
-    int prevMt = -1, runIdx = 0;
+    int prevGt = -1, runIdx = 0;
+    int d = TABLE ? table_find(dirs, numDirs, &MbDir::u0, u_begin) : 0;
     size_t slot = 0;
     for (int u = u_begin, i = 0; u < u_end; u++, i++) {
-      const int mt = u / pl.n_nt, nt = u - mt * pl.n_nt;
-      if (mt != prevMt) {
-        slot = tc_slot(pl, cta, runIdx, rowInTile);
+      const T3Unit un = t3_unit<TABLE>(pl, dirs, numDirs, d, u);
+      if (un.gt != prevGt) {
+        slot = tc_slot(un.gt, cta, rowInTile);
         mbarrier_wait(&bar_a_full, runIdx & 1);
-        prevMt = mt; runIdx++;
+        prevGt = un.gt; runIdx++;
 #pragma unroll
         for (int r = 0; r < 2; r++)
 #pragma unroll
@@ -308,13 +359,13 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf)
       }
       wg_commit();
       wg_wait0(acc);
-      const bool lastOfRun = (u + 1 == u_end) || ((u + 1) / pl.n_nt != mt);
+      const bool lastOfRun = (u + 1 == u_end) || un.last;
       if (lane == 0) {
         mbarrier_arrive(&bar_b_empty[s]);
         if (lastOfRun) mbarrier_arrive(&bar_a_empty);
       }
       // columns 8j + 2(lane % 4) + {0, 1}: the lane pair (lane, lane ^ 1) holds group 2j + hb of partition 2(j % 4) + hb
-      const int gbase = nt * (T3_N / 4) + hb;
+      const int gbase = un.nt * (T3_N / 4) + hb;
 #pragma unroll
       for (int j = 0; j < 16; j++) {
 #pragma unroll
@@ -386,6 +437,7 @@ t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ s
   float G = 0.0f, S = 0.0f, Th = 0.0f;
   int I1 = -1, I2 = -1;
   {
+    const int gt = mt;
     const int u0 = mt * pl.n_nt, u1 = u0 + pl.n_nt - 1;
     const int c0 = u0 / pl.U, c1 = u1 / pl.U;
     auto insert = [&](float v, int id) {
@@ -403,8 +455,7 @@ t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ s
     for (int k = 0; k < T3_SEG; k++) {
       const int c = c0 + k;
       if (c <= c1) {
-        const int run = mt - (c * pl.U) / pl.n_nt;
-        const float *q = bf.pm + tc_slot(pl, c, run, rowInTile) * T3_PM;
+        const float *q = bf.pm + tc_slot(gt, c, rowInTile) * T3_PM;
         v[k][0] = q[p]; v[k][1] = q[8 + p]; v[k][2] = q[16 + p];
         id[k][0] = __float_as_int(q[24 + p]); id[k][1] = __float_as_int(q[32 + p]);
       } else {
@@ -414,8 +465,7 @@ t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ s
 #pragma unroll
     for (int k = 0; k < T3_SEG; k++) { insert(v[k][0], id[k][0]); insert(v[k][1], id[k][1]); insert(v[k][2], -1); }
     for (int c = c0 + T3_SEG; c <= c1; c++) {
-      const int run = mt - (c * pl.U) / pl.n_nt;
-      const float *q = bf.pm + tc_slot(pl, c, run, rowInTile) * T3_PM;
+      const float *q = bf.pm + tc_slot(gt, c, rowInTile) * T3_PM;
       insert(q[p], __float_as_int(q[24 + p])); insert(q[8 + p], __float_as_int(q[32 + p])); insert(q[16 + p], -1);
     }
     G *= T3_UNSCALE; S *= T3_UNSCALE; Th *= T3_UNSCALE;
@@ -555,9 +605,15 @@ __device__ __forceinline__ void knn_top2_insert(float &s1, int &j1, float &s2, i
   else if (s > s2 || (s == s2 && j < j2)) { s2 = s; j2 = j; }
 }
 
+// A call resolves one direction (pl, bf and the arguments).  A batch wave (TABLE) resolves every direction of the table,
+// each with ceil(n1 / 16) CTAs from its cta0 on; its rows go to the fallback as {direction, row} entries (cap of them),
+// all of them when either set raised its bad-input flag.
+template <bool TABLE>
 __global__ void __launch_bounds__(32 * T3_RW)
 knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restrict__ sift1,
-                   const SiftPoint *__restrict__ sift2, int n2, int2 *__restrict__ idx, float2 *__restrict__ score)
+                   const SiftPoint *__restrict__ sift2, int n2, int2 *__restrict__ idx, float2 *__restrict__ score,
+                   const MbDir *__restrict__ dirs, int numDirs, int2 *__restrict__ entries,
+                   unsigned int *__restrict__ numEntries, int cap)
 {
   __shared__ KnnResolveSmem sm;
   __shared__ unsigned int s_chains;
@@ -566,19 +622,39 @@ knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restr
   const unsigned int FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int sub = lane >> 3, p = lane & 7;                   // row within the warp; partition / candidate slot
-  const int row = (blockIdx.x * T3_RW + w) * 4 + sub;
-  const bool valid = row < pl.n1;
-  const int rrow = valid ? row : pl.n1 - 1;                   // clamped: padding lanes mirror the last row
+  int blk = blockIdx.x, n1 = pl.n1, n_nt = pl.n_nt, tileU0 = 0, gt0 = 0, dir = 0;
+  const float *normAs = bf.normA, *bmaxp = bf.bmax;
+  unsigned int *counters = bf.counters;
+  if (TABLE) {
+    dir = table_find(dirs, numDirs, &MbDir::cta0, (int)blockIdx.x);
+    const MbDir &D = dirs[dir];
+    blk -= D.cta0; n1 = D.n1; n2 = D.n2; n_nt = D.n_nt; tileU0 = D.u0; gt0 = D.gt0;
+    sift1 = D.s1; sift2 = D.s2; idx = D.idx; score = D.score;
+    normAs = D.norms; bmaxp = D.bmax; counters = D.counters;
+    if (*D.bad1 | *D.bad2) {                                  // gated: every row takes the exact way
+      const int row = (blk * T3_RW + w) * 4 + sub;
+      if (row < n1 && p == 0) {
+        atomicAdd(&counters[0], 1u);
+        const unsigned e = atomicAdd(numEntries, 1u);
+        if (e < (unsigned)cap) entries[e] = make_int2(dir, row);
+      }
+      return;
+    }
+  }
+  const int row = (blk * T3_RW + w) * 4 + sub;
+  const bool valid = row < n1;
+  const int rrow = valid ? row : n1 - 1;                      // clamped: padding lanes mirror the last row
   const int mt = rrow / T3_MT, rowInTile = rrow - mt * T3_MT;
 #pragma unroll
   for (int j = 0; j < 4; j++) sm.a[w][sub][p + 8 * j] = __ldg(reinterpret_cast<const float4 *>(sift1[rrow].data) + p + 8 * j);
-  const float bmax = __int_as_float(*reinterpret_cast<const int *>(bf.bmax));
-  const float normA = bf.normA[rrow];
+  const float bmax = __int_as_float(*reinterpret_cast<const int *>(bmaxp));
+  const float normA = normAs[rrow];
   // merged top-3 of partition p over the segments (as t3_resolve_kernel)
   float G = 0.0f, S = 0.0f, Th = 0.0f;
   int I1 = -1, I2 = -1;
   {
-    const int u0 = mt * pl.n_nt, u1 = u0 + pl.n_nt - 1;
+    const int gt = gt0 + mt;
+    const int u0 = tileU0 + mt * n_nt, u1 = u0 + n_nt - 1;
     const int c0 = u0 / pl.U, c1 = u1 / pl.U;
     auto insert = [&](float v, int id) {
       const bool t = v > G, u2 = v > S;
@@ -595,8 +671,7 @@ knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restr
     for (int k = 0; k < T3_SEG; k++) {
       const int c = c0 + k;
       if (c <= c1) {
-        const int run = mt - (c * pl.U) / pl.n_nt;
-        const float *q = bf.pm + tc_slot(pl, c, run, rowInTile) * T3_PM;
+        const float *q = bf.pm + tc_slot(gt, c, rowInTile) * T3_PM;
         v[k][0] = q[p]; v[k][1] = q[8 + p]; v[k][2] = q[16 + p];
         id[k][0] = __float_as_int(q[24 + p]); id[k][1] = __float_as_int(q[32 + p]);
       } else {
@@ -606,8 +681,7 @@ knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restr
 #pragma unroll
     for (int k = 0; k < T3_SEG; k++) { insert(v[k][0], id[k][0]); insert(v[k][1], id[k][1]); insert(v[k][2], -1); }
     for (int c = c0 + T3_SEG; c <= c1; c++) {
-      const int run = mt - (c * pl.U) / pl.n_nt;
-      const float *q = bf.pm + tc_slot(pl, c, run, rowInTile) * T3_PM;
+      const float *q = bf.pm + tc_slot(gt, c, rowInTile) * T3_PM;
       insert(q[p], __float_as_int(q[24 + p])); insert(q[8 + p], __float_as_int(q[32 + p])); insert(q[16 + p], -1);
     }
     G *= T3_UNSCALE; S *= T3_UNSCALE; Th *= T3_UNSCALE;
@@ -632,8 +706,13 @@ knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restr
   const unsigned int certMask = (__ballot_sync(FULL, cert) >> (8 * sub)) & 0xffu;
   const bool ok = valid && rowOk && certMask == 0xffu;
   if (valid && !ok && p == 0) {
-    const unsigned at = atomicAdd(&bf.counters[0], 1u);
-    if (at < (unsigned)pl.n_mt * T3_MT) bf.fbRows[at] = row;
+    const unsigned at = atomicAdd(&counters[0], 1u);
+    if (TABLE) {
+      const unsigned e = atomicAdd(numEntries, 1u);
+      if (e < (unsigned)cap) entries[e] = make_int2(dir, row);
+    } else if (at < (unsigned)pl.n_mt * T3_MT) {
+      bf.fbRows[at] = row;
+    }
   }
   const unsigned int b1 = (__ballot_sync(FULL, ok && use1) >> (8 * sub)) & 0xffu;
   const unsigned int b2 = (__ballot_sync(FULL, ok && use2) >> (8 * sub)) & 0xffu;
@@ -697,7 +776,7 @@ knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restr
     atomicAdd(&s_chains, (unsigned)ncand);
   }
   __syncthreads();
-  if (threadIdx.x == 0 && s_chains) { atomicAdd(&bf.counters[1], s_chains >> 2); atomicAdd(&bf.counters[2], s_chains); }
+  if (threadIdx.x == 0 && s_chains) { atomicAdd(&counters[1], s_chains >> 2); atomicAdd(&counters[2], s_chains); }
 }
 
 // exact SIMT scan of the rows the tensor path could not certify (match.cu)
@@ -713,20 +792,26 @@ bool match_tensor_supported()
   return major == 9;
 }
 
-// persistent GEMM schedule: n1 rows against the first n2v candidates
+// persistent GEMM schedule of `total` units: at most one CTA per SM, U units each
+static void t3_schedule(TcPlan &pl, int sms)
+{
+  pl.grid = pl.total < sms ? pl.total : sms;
+  pl.U = idivup(pl.total, pl.grid);
+  pl.grid = idivup(pl.total, pl.U);
+}
+// n1 rows against the first n2v candidates
 static TcPlan t3_plan(int n1, int n2v, int sms)
 {
   TcPlan pl;
   pl.n1 = n1; pl.n2v = n2v;
   pl.n_mt = idivup(n1, T3_MT); pl.n_nt = idivup(n2v, T3_N);
   pl.total = pl.n_mt * pl.n_nt;
-  pl.grid = pl.total < sms ? pl.total : sms;
-  pl.U = idivup(pl.total, pl.grid);
-  pl.grid = idivup(pl.total, pl.U);
-  pl.runs = idivup(pl.U, pl.n_nt) + 1;
+  t3_schedule(pl, sms);
   return pl;
 }
-static size_t t3_slots(const TcPlan &pl) { return (size_t)pl.grid * pl.runs * T3_MT; }
+// top-3 table slots of `tiles` row tiles run by `grid` CTAs (tc_slot)
+static size_t t3_slots(int tiles, int grid) { return ((size_t)tiles + grid) * T3_MT; }
+static size_t t3_slots(const TcPlan &pl) { return t3_slots(pl.n_mt, pl.grid); }
 
 // A tensor-path call once its prep kernel is in: each direction's plan and view of the workspace, the bad-input gate
 // (shared: any bad value, either set), the call's flag area and the timing events (or null).
@@ -780,7 +865,7 @@ static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const Si
   if (c.tcDirty) CS_CUDA(cudaMemsetAsync(c.tcFlags.p, 0, 128, st));   // a previous call failed between its launches
   c.tcDirty = true;                                                  // until this call's launches are all in
   if (!c.tcConfigured) {
-    CS_CUDA(cudaFuncSetAttribute(t3_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, T3_SMEM_BYTES));
+    CS_CUDA(cudaFuncSetAttribute(t3_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3_SMEM_BYTES));
     c.tcConfigured = true;
   }
   auto at = [](void *base, size_t bytes) { return reinterpret_cast<__half *>(static_cast<uint8_t *>(base) + bytes); };
@@ -800,7 +885,7 @@ static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const Si
   t.flags = flags;
   t.tev = match_timing_events();
   if (t.tev) cudaEventRecord(t.tev[0], st);
-  t3_prep_kernel<<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], flags + 1, nextFlags);
+  t3_prep_kernel<false><<<p[0].blocks + p[1].blocks, 512, 0, st>>>(p[0], p[1], nullptr, 0, flags + 1, nextFlags);
   count_launch();
   CS_CUDA(cudaGetLastError());
   if (t.tev) cudaEventRecord(t.tev[1], st);
@@ -813,7 +898,7 @@ static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const Si
 static int t3_direction(const TcPlan &pl, const T3Buffers &bf, SiftPoint *s1, int n1, const SiftPoint *s2, int n2,
                         const unsigned int *gate, cudaStream_t st, cudaEvent_t *ev)
 {
-  t3_gemm_kernel<<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf);
+  t3_gemm_kernel<false><<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf, nullptr, 0);
   if (ev) cudaEventRecord(ev[0], st);
   t3_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2);
   if (ev) cudaEventRecord(ev[1], st);
@@ -898,10 +983,12 @@ static int knn_direction(DeviceCtx &c, const TcPlan &pl, const T3Buffers &bf, co
                          const SiftPoint *s2, int n2, int *idx, float *score, const unsigned int *gate, cudaEvent_t *ev)
 {
   const cudaStream_t st = c.stream;
-  t3_gemm_kernel<<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf);
+  t3_gemm_kernel<false><<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf, nullptr, 0);
   if (ev) cudaEventRecord(ev[0], st);
-  knn_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2, n2, reinterpret_cast<int2 *>(idx),
-                                                                  reinterpret_cast<float2 *>(score));
+  knn_resolve_kernel<false><<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2, n2,
+                                                                         reinterpret_cast<int2 *>(idx),
+                                                                         reinterpret_cast<float2 *>(score), nullptr, 0,
+                                                                         nullptr, nullptr, 0);
   if (ev) cudaEventRecord(ev[1], st);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
@@ -942,6 +1029,233 @@ void match_tensor_stats(DeviceCtx &c, unsigned long long stats[4])
   stats[0] = (unsigned long long)h[4 + 1] + h[8 + 1];                     // [8..10] stay zero in a single direction
   stats[1] = (unsigned long long)h[4 + 2] + h[8 + 2];
   stats[2] = (unsigned long long)h[4 + 0] + h[8 + 0];
+}
+
+// ------------------------------------------------------------------------------ batched ratio matching
+// A wave (cs_match_ratio_batch states the rule): consecutive non-empty jobs whose scratch -- per distinct set its
+// operand tiles and norms, per direction its top-3 tables, neighbour lists and fallback entries -- fits MB_BUDGET.
+// Every wave runs the same six launches: prep, GEMM, knn resolve, list fallback, ratio flags, pair writes.
+#define MB_BUDGET ((size_t)256 << 20)
+static size_t mb_set_bytes(int n) { return (size_t)idivup(n, T3_MT) * T3_MT * (T3_A_BYTES / T3_MT + sizeof(float)); }
+static size_t mb_dir_bytes(int n1)
+{
+  return (size_t)idivup(n1, T3_MT) * T3_MT * T3_PM * sizeof(float) + (size_t)n1 * (sizeof(int2) + sizeof(float2) + sizeof(int2));
+}
+
+struct MbWave {
+  std::vector<int> jobs;            // the jobs, in order
+  std::vector<int> sets;            // the distinct sets, in order of first use
+  int dirs = 0, tiles = 0, dirTiles = 0, rows = 0, words = 0, pairCtas = 0, units = 0, resolveCtas = 0, prepCtas = 0;
+  size_t bytes = 0;                 // the rule's scratch
+  size_t tabBytes = 0, zeroWords = 0, pinOff = 0;
+};
+
+static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+static std::vector<MbWave> mb_waves(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                                    bool cross)
+{
+  std::vector<MbWave> waves;
+  std::vector<int> mark((size_t)numSets, -1);             // the last wave that converts the set
+  for (int p = 0; p < numJobs; p++) {
+    const int a = jobs[p].set1, b = jobs[p].set2, na = sets[a].n, nb = sets[b].n;
+    if (na == 0 || nb == 0) continue;
+    auto cost = [&](int w) {
+      size_t x = mb_dir_bytes(na) + (cross ? mb_dir_bytes(nb) : 0);
+      if (mark[a] != w) x += mb_set_bytes(na);
+      if (b != a && mark[b] != w) x += mb_set_bytes(nb);
+      return x;
+    };
+    int w = (int)waves.size() - 1;
+    if (w < 0 || waves[w].bytes + cost(w) > MB_BUDGET) { waves.emplace_back(); w++; }
+    MbWave &v = waves[w];
+    v.bytes += cost(w);
+    for (int s : {a, b})
+      if (mark[s] != w) {
+        mark[s] = w;
+        v.sets.push_back(s);
+        v.tiles += idivup(sets[s].n, T3_MT);
+        v.prepCtas += idivup(sets[s].n, T3_MT) * (T3_MT / 32);
+      }
+    v.jobs.push_back(p);
+    for (int k = 0; k < (cross ? 2 : 1); k++) {
+      const int n1 = k ? nb : na, n2 = k ? na : nb;
+      v.dirs++;
+      v.dirTiles += idivup(n1, T3_MT);
+      v.units += idivup(n1, T3_MT) * idivup(n2, T3_N);
+      v.resolveCtas += idivup(n1, 4 * T3_RW);
+      v.rows += n1;
+    }
+    v.words += idivup(na, 32);
+    v.pairCtas += idivup(na, 1024);                        // MP_ROWS (match_mutual.cu)
+  }
+  size_t pin = 0;
+  for (MbWave &v : waves) {
+    const size_t S = v.sets.size(), D = v.dirs, J = v.jobs.size();
+    v.tabBytes = align16(S * sizeof(T3PrepSet)) + align16(D * sizeof(MbDir)) + align16(J * sizeof(PairJob));
+    v.zeroWords = (2 * S + 4 * D + J + 1 + 3) & ~(size_t)3;
+    v.pinOff = pin;
+    pin += v.tabBytes + v.zeroWords * sizeof(unsigned int);
+  }
+  return waves;
+}
+
+// The device tables of a wave in pinned memory, with pointers into the context's buffers; out[p] for its jobs.
+// Device state: [2 s] set s's max norm, [2 s + 1] its bad-input flag; [2 S + 4 d] direction d's counters; then each
+// job's pair total and the fallback entry count (all cleared per wave); then the ballot words and CTA counts.
+static void mb_fill(DeviceCtx &c, const MbWave &v, const cs_match_set *sets, const cs_match_job *jobs, bool cross,
+                    std::vector<int> &slot, RatioBatchOut *out)
+{
+  const int S = (int)v.sets.size(), D = v.dirs, J = (int)v.jobs.size();
+  uint8_t *hp = static_cast<uint8_t *>(c.h_mb) + v.pinOff;
+  T3PrepSet *hs = reinterpret_cast<T3PrepSet *>(hp);
+  MbDir *hd = reinterpret_cast<MbDir *>(hp + align16(S * sizeof(T3PrepSet)));
+  PairJob *hj = reinterpret_cast<PairJob *>(hp + align16(S * sizeof(T3PrepSet)) + align16(D * sizeof(MbDir)));
+  const unsigned int *hstate = reinterpret_cast<const unsigned int *>(hp + v.tabBytes);
+  unsigned int *st = c.mbState.as<unsigned int>();
+  unsigned int *masks = st + v.zeroWords, *counts = masks + v.words;
+  int2 *idx = c.mbLists.as<int2>();
+  float2 *score = reinterpret_cast<float2 *>(idx + v.rows);
+  int tile = 0, blk = 0;
+  for (int k = 0; k < S; k++) {
+    const cs_match_set &m = sets[v.sets[k]];
+    slot[v.sets[k]] = k;
+    T3PrepSet &p = hs[k];
+    p = T3PrepSet{};
+    p.pts = static_cast<const SiftPoint *>(m.pts);
+    p.n = p.nv = m.n;
+    p.blocks = idivup(m.n, T3_MT) * (T3_MT / 32);
+    p.a = reinterpret_cast<__half *>(c.tcA.as<uint8_t>() + (size_t)tile * T3_A_BYTES);
+    p.b = nullptr;
+    p.norms = c.tcNorms.as<float>() + (size_t)tile * T3_MT;
+    p.bmax = reinterpret_cast<float *>(st + 2 * k);
+    p.bad = reinterpret_cast<float *>(st + 2 * k + 1);
+    p.blk0 = blk;
+    tile += idivup(m.n, T3_MT);
+    blk += p.blocks;
+  }
+  int d = 0, u0 = 0, gt0 = 0, cta0 = 0, list0 = 0, word0 = 0, pcta0 = 0;
+  for (int q = 0; q < J; q++) {
+    const int pj = v.jobs[q];
+    const cs_match_job &j = jobs[pj];
+    const int a = slot[j.set1], b = slot[j.set2];
+    int dd[2] = {-1, -1};
+    for (int k = 0; k < (cross ? 2 : 1); k++, d++) {
+      const int x = k ? b : a, y = k ? a : b;            // rows of set x against set y
+      MbDir &r = hd[d];
+      r.s1 = hs[x].pts; r.s2 = hs[y].pts; r.n1 = hs[x].n; r.n2 = hs[y].n;
+      r.norms = hs[x].norms;
+      r.bmax = hs[y].bmax;
+      r.bad1 = reinterpret_cast<const unsigned int *>(hs[x].bad);
+      r.bad2 = reinterpret_cast<const unsigned int *>(hs[y].bad);
+      r.idx = idx + list0; r.score = score + list0;
+      r.counters = st + 2 * S + 4 * d;
+      r.aTile0 = hs[x].blk0 / (T3_MT / 32); r.bTile0 = hs[y].blk0 / (T3_MT / 32);
+      r.n_nt = idivup(r.n2, T3_N);
+      r.u0 = u0; r.gt0 = gt0; r.cta0 = cta0;
+      u0 += idivup(r.n1, T3_MT) * r.n_nt; gt0 += idivup(r.n1, T3_MT); cta0 += idivup(r.n1, 4 * T3_RW);
+      list0 += r.n1;
+      dd[k] = d;
+    }
+    const MbDir &f = hd[dd[0]];
+    PairJob &pjob = hj[q];
+    pjob.jv = reinterpret_cast<const int *>(f.idx); pjob.jstride = 2;
+    pjob.n1 = f.n1; pjob.n2 = f.n2;
+    pjob.idx1 = f.idx; pjob.score1 = f.score;
+    pjob.idx2 = cross ? hd[dd[1]].idx : nullptr; pjob.score2 = cross ? hd[dd[1]].score : nullptr;
+    pjob.masks = masks + word0; pjob.blockCounts = counts + pcta0;
+    pjob.pairs = reinterpret_cast<int2 *>(j.pairs); pjob.maxPairs = j.maxPairs;
+    pjob.total = st + 2 * S + 4 * D + q;
+    pjob.cta0 = pcta0;
+    word0 += idivup(f.n1, 32); pcta0 += idivup(f.n1, 1024);
+    RatioBatchOut &o = out[pj];
+    o.total = hstate + 2 * S + 4 * D + q;
+    o.counters[0] = hstate + 2 * S + 4 * dd[0];
+    o.counters[1] = cross ? hstate + 2 * S + 4 * dd[1] : nullptr;
+    o.bad1 = hstate + 2 * a + 1; o.bad2 = hstate + 2 * b + 1;
+  }
+}
+
+int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                        float maxRatio, float maxDistance, bool cross, RatioBatchOut *out)
+{
+  const std::vector<MbWave> waves = mb_waves(sets, numSets, jobs, numJobs, cross);
+  if (waves.empty()) return 0;
+  size_t tiles = 0, slots = 0, rows = 0, state = 0, tab = 0, pin = 0;
+  for (const MbWave &v : waves) {
+    tiles = std::max(tiles, (size_t)v.tiles);
+    slots = std::max(slots, t3_slots(v.dirTiles, c.sms));
+    rows = std::max(rows, (size_t)v.rows);
+    state = std::max(state, v.zeroWords + v.words + v.pairCtas);
+    tab = std::max(tab, v.tabBytes);
+    pin = v.pinOff + v.tabBytes + v.zeroWords * sizeof(unsigned int);
+  }
+  const cudaStream_t st = c.stream;
+  int r;
+  if ((r = c.tcA.grow(tiles * T3_A_BYTES)) < 0 || (r = c.tcNorms.grow(tiles * T3_MT * sizeof(float))) < 0 ||
+      (r = c.tcTables.grow(slots * T3_PM * sizeof(float))) < 0 || (r = c.mbTables.grow(tab)) < 0 ||
+      (r = c.mbLists.grow(rows * (sizeof(int2) + sizeof(float2) + sizeof(int2)))) < 0 ||
+      (r = c.mbState.grow(state * sizeof(unsigned int))) < 0)
+    return r;
+  if (c.h_mbBytes < pin) {                  // every batch call ends in a synchronize: no copy is pending here
+    if (c.h_mb) cudaFreeHost(c.h_mb);
+    c.h_mb = nullptr;
+    c.h_mbBytes = 0;
+    CS_CUDA(cudaMallocHost(&c.h_mb, pin));
+    c.h_mbBytes = pin;
+  }
+  if (!c.mbConfigured) {
+    CS_CUDA(cudaFuncSetAttribute(t3_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3_SMEM_BYTES));
+    c.mbConfigured = true;
+  }
+  std::vector<int> slot((size_t)numSets, -1);
+  cudaEvent_t *tev = match_timing_events();
+  for (const MbWave &v : waves) {
+    mb_fill(c, v, sets, jobs, cross, slot, out);
+    const int S = (int)v.sets.size(), D = v.dirs, J = (int)v.jobs.size();
+    uint8_t *hp = static_cast<uint8_t *>(c.h_mb) + v.pinOff;
+    uint8_t *dt = c.mbTables.as<uint8_t>();
+    const T3PrepSet *ds = reinterpret_cast<const T3PrepSet *>(dt);
+    const MbDir *dd = reinterpret_cast<const MbDir *>(dt + align16(S * sizeof(T3PrepSet)));
+    const PairJob *dj = reinterpret_cast<const PairJob *>(dt + align16(S * sizeof(T3PrepSet)) + align16(D * sizeof(MbDir)));
+    unsigned int *state = c.mbState.as<unsigned int>();
+    int2 *entries = c.mbLists.as<int2>() + 2 * (size_t)v.rows;
+    unsigned int *numEntries = state + 2 * S + 4 * D + J;
+    TcPlan pl{};
+    pl.total = v.units;
+    t3_schedule(pl, c.sms);
+    const T3Buffers bf = {c.tcA.as<__half>(), c.tcA.as<__half>(), nullptr, nullptr, c.tcTables.as<float>(), nullptr,
+                          nullptr};
+    CS_CUDA(cudaMemsetAsync(state, 0, v.zeroWords * sizeof(unsigned int), st));
+    CS_CUDA(cudaMemcpyAsync(dt, hp, v.tabBytes, cudaMemcpyHostToDevice, st));
+    if (tev) cudaEventRecord(tev[0], st);
+    t3_prep_kernel<true><<<v.prepCtas, 512, 0, st>>>(T3PrepSet{}, T3PrepSet{}, ds, S, nullptr, nullptr);
+    if (tev) cudaEventRecord(tev[1], st);
+    t3_gemm_kernel<true><<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf, dd, D);
+    if (tev) cudaEventRecord(tev[2], st);
+    knn_resolve_kernel<true><<<v.resolveCtas, 32 * T3_RW, 0, st>>>(pl, bf, nullptr, nullptr, 0, nullptr, nullptr, dd, D,
+                                                                   entries, numEntries, v.rows);
+    if (tev) cudaEventRecord(tev[3], st);
+    count_launch(3);
+    CS_CUDA(cudaGetLastError());
+    if ((r = launch_knn_list_fallback(c, dd, entries, numEntries, v.rows)) < 0) return r;
+    if (tev) cudaEventRecord(tev[4], st);
+    if ((r = launch_ratio_pairs_batch(c, dj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
+    if (tev) cudaEventRecord(tev[5], st);
+    CS_CUDA(cudaMemcpyAsync(hp + v.tabBytes, state, v.zeroWords * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    if (tev) {
+      static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "pairs"};
+      cudaEventSynchronize(tev[5]);
+      fprintf(stderr, "ratio-batch timing %d jobs %d directions %d units [us]:", J, D, v.units);
+      for (int i = 0; i < 5; i++) {
+        float ms = 0.0f;
+        cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
+        fprintf(stderr, " %s %.1f", names[i], ms * 1e3f);
+      }
+      fprintf(stderr, "\n");
+    }
+  }
+  return 0;
 }
 
 }  // namespace cs

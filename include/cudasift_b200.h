@@ -283,6 +283,46 @@ int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const doub
                               int numLoops, float thresh, double *E_out, double *R_out, double *t_out,
                               int *counts_out, long long *stats_out, double *ms);
 
+/* Batched ratio matching: J independent jobs of cs_match_ratio in one call, for example every image pair of a
+ * collection.  A set is one image's records; a job names two sets and its own pair buffer.  maxRatio, maxDistance and
+ * crossCheck are common to all jobs. */
+typedef struct cs_match_set {
+  const void *pts; int n;          /* device SiftPoint records, only read */
+} cs_match_set;
+typedef struct cs_match_job {
+  int set1, set2;                  /* indices into sets */
+  int *pairs; int maxPairs;        /* device int pairs {i, j}, 8-byte aligned; NULL allowed when maxPairs == 0 */
+} cs_match_job;
+/* - Equivalence: for job p with A = sets[set1] and B = sets[set2], counts_out[p] and the first min(count, maxPairs)
+ *   pairs equal, bit for bit, what cs_match_ratio(A.pts, A.n, B.pts, B.n, maxRatio, maxDistance, crossCheck, pairs,
+ *   maxPairs, mode, ...) returns and writes, in every mode.  stats_out[p][0..2] equal cs_match_stats()[0..2] after that
+ *   call in mode 2 (the groups re-scored, the exact chains and the fallback rows, both directions summed with
+ *   crossCheck; the all-exact marker {0, 0, 2^64 - 1} when a value of A or B is not finite or |x| >= 8), and
+ *   stats_out[p][3] = 2.  Every job runs the tensor path at any size; the exact kernels serve the rows it cannot
+ *   certify.  Jobs do not interact: permuting the jobs permutes the results, and two calls give the same bytes.
+ * - Sets are shared: any number of jobs may name a set, in either role, a set may be paired with itself and sets may
+ *   overlap each other.  A job with an empty set gets count 0 and zero statistics, and launches nothing.  numJobs == 0,
+ *   or only empty jobs, returns 0 before any CUDA call.
+ * - CS_E_ARG, before any CUDA call, naming the first offending jobs[p] or sets[s] in cs_last_error(): numSets or
+ *   numJobs outside [0, 65536], NULL sets or jobs with a positive count, NULL counts_out with numJobs > 0, a set with
+ *   n < 0 or a NULL pts with n > 0, set1 or set2 outside [0, numSets), maxPairs < 0, NULL pairs with maxPairs > 0, a
+ *   pair buffer that is not 8-byte aligned, a NaN maxRatio or maxDistance, and a pair buffer that overlaps another
+ *   job's pair buffer or any set's records (one sweep over sorted ranges, O((J + S) log(J + S))).
+ * - Waves: the non-empty jobs, in order, run in waves.  A wave is the longest run of consecutive non-empty jobs whose
+ *   scratch fits 256 MiB; it holds at least one job.  The scratch of a wave counts, once per distinct set it uses,
+ *   516 bytes per row of the set rounded up to a multiple of 128 rows (split-FP16 operand tiles and norms; a set is
+ *   converted once per wave whatever the number of its jobs), and per direction (one per job, two with crossCheck: the
+ *   rows of set 1 against set 2 and the rows of set 2 against set 1) 160 bytes per row of its first set rounded up to
+ *   128 rows (top-3 tables) plus 24 bytes per row (neighbour lists, fallback entries).  A call also reserves 20 KiB of
+ *   tables per SM and a few words per row for the pair scratch.
+ * - Launches: each wave issues 6 kernel launches, whatever its number of jobs and crossCheck (convert, GEMM, resolve,
+ *   exact fallback, ratio test, pair writes), so a batch issues 6 x waves (cs_launch_count).  The call synchronises
+ *   with the host once, at the end; its scratch lives in the per-device context.  *ms (may be NULL) gets the event
+ *   time of the call.  cs_match_stats keeps describing single calls.
+ * counts_out[J]; stats_out[J][4] may be NULL.  Returns 0 or CS_E_*. */
+int cs_match_ratio_batch(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs, float maxRatio,
+                         float maxDistance, int crossCheck, int *counts_out, unsigned long long *stats_out, double *ms);
+
 /* Guided matching (COLMAP's guided_matching): the two nearest neighbours and the ratio test restricted to the pairs a
  * model admits.  cs_match_knn2_guided has the semantics of cs_match_knn2 (the reference's score, only scores > 0, the
  * order score descending then index ascending, a missing neighbour is (-1, 0.0f)), except that row i of set 1 only
