@@ -340,6 +340,8 @@ struct PairJob {
 // ---- batched ratio matching (cs_match_ratio_batch) ------------------------------------------------------------------
 // A direction of a wave: the n1 rows of set 1 against the n2 candidates of set 2, with its operand tiles, its units of
 // the wave's GEMM, its top-3 table tiles, its resolve CTAs and its neighbour lists.  Built on the host (match_tc.cu).
+// A single call's resolve takes one by value: its rows, candidates, norms, max norm, counters and, for the top-2 rule,
+// its lists; the table fields stay zero.
 struct MbDir {
   const SiftPoint *s1, *s2;
   int n1, n2;

@@ -15,16 +15,18 @@
 //                registers; three MMAs per K step: hi*hi + hi*lo + lo*hi) with both operands in shared memory,
 //                and keep, per (row, partition), the three largest 4-candidate group maxima.
 //   3. resolve   eight lanes per row: merge the segments, certify, exact k=0..127 FMA chains for the
-//                surviving candidates, the reference's per-partition update rule and 8-way merge.
+//                surviving candidates, then the rule: the reference's per-partition update rule and 8-way merge, or
+//                the two nearest neighbours.  One kernel, t3_resolve_kernel<KNN, TABLE>, serves both rules.
 // Mutual matching uses the same prep launch to convert each set once for both of its roles, runs steps 2 and 3 and
 // the exact fallback per direction, then the cross-check (match_mutual.cu).  Two-nearest-neighbour matching
-// (match_knn_tensor) runs the same prep and GEMM over all candidates, then knn_resolve_kernel and the exact top-2
-// fallback (match_knn.cu).
+// (match_knn_tensor) runs the same prep and GEMM over all candidates, then the resolve's top-2 rule and the exact top-2
+// fallback (match_knn.cu); a batch wave of ratio matching runs them over a table of directions.
 #include "common.cuh"
 
 #include <cuda_fp16.h>
 
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 
 namespace cs {
@@ -80,7 +82,7 @@ __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc,
 // The GEMM's units (A tile, B tile) are numbered in row-tile order, and CTA c takes units [c U, (c + 1) U).  In a batch
 // wave the units of its directions follow each other (MbDir::u0) and U, total and grid cover all of them.
 struct TcPlan {
-  int n1, n2v, n_mt, n_nt, total, U, grid;
+  int n_mt, n_nt, total, U, grid;
 };
 // The top-3 tables hold one entry per (A tile, segment): the units of row tile t (numbered over all directions of a
 // wave) that CTA c runs.  Along the units both t and c only grow and one of them steps at every new segment, so t + c
@@ -122,11 +124,8 @@ __device__ __forceinline__ size_t tc_slot(int tile, int cta, int rowInTile)
 
 struct T3Buffers {
   __half *a16, *b16;          // packed hi/lo operand tiles
-  float *normA;               // per row of set 1
-  float *bmax;                // max norm of the candidates (float bits)
   float *pm;                  // per (row, segment) top-3 tables
   int *fbRows;                // fallback row list
-  unsigned int *counters;     // [0] fallback rows, [1] candidate groups re-scored, [2] chains
 };
 
 // Chunk c (8 values) of a row's descriptor, zeros for rows >= nvalid: the split halves, the chunk's sum of squares and
@@ -398,47 +397,90 @@ t3_gemm_kernel(const TcPlan pl, const T3Buffers bf, const MbDir *__restrict__ di
 }
 
 // ---- resolve ---------------------------------------------------------------------------------
-// Eight lanes per row (four rows per warp): merge the segments' top-3 tables (lane = partition),
-// decide which partitions can matter, re-score their first (and, within delta, second) groups
-// exactly (lane = candidate, eight per round), then the reference's per-partition rule
-// (matching.cu:354-359, stated order-independently) and 8-way merge (:378-390).
+// Eight lanes per row (four rows per warp): merge the segments' top-3 tables (lane = partition), decide which partitions
+// can matter, re-score their first (and, within delta, second) groups exactly (lane = candidate, eight per round), then
+// the rule's final step.  Two rules share every step but the threshold pool, the certification and the final step:
+// - the reference rule (MatchSiftData): the reference's per-partition rule (matching.cu:354-359, stated
+//   order-independently) and 8-way merge (:378-390) into set 1's five match fields;
+// - KNN: the true two nearest neighbours (match_knn.cu states the order) among all n2 candidates.  Per partition the
+//   merged tables give G >= S >= Th and the groups I1, I2.  T is the second largest of the 16 values {G[0..7], S[0..7]}:
+//   two distinct groups have approximate maxima >= T, so two distinct candidates have exact scores >= T - eps, and
+//   score2 >= T - eps.  A candidate whose group is not re-scored lies in a group below T - delta (delta = 2 eps): it is
+//   either a partition's third group or lower (<= Th, certified < T - delta) or an I1 / I2 group below T - delta.  Its
+//   exact score is then < T - eps <= score2, strictly, so the top two of the re-scored candidates (at most 8 x 2 groups
+//   x 4 = T3_TAB) are the row's top two, ties included.  T > 2 delta keeps both clearly positive.
 #define T3_RW 4                       // warps per CTA (16 rows)
 #define T3_TAB 64                     // exact scores a row can collect (8 partitions x 2 groups x 4)
 
-struct T3ResolveSmem {
+struct T3ResolveXy {
+  float2 xy[T3_RW][4][T3_TAB];        // the candidates' positions (match_xpos / match_ypos)
+};
+struct T3ResolveNoXy {};
+// Only the reference rule carries positions: the top-2 rule keeps the smaller footprint and its resident CTAs.
+template <bool KNN>
+struct T3ResolveSmem : std::conditional_t<KNN, T3ResolveNoXy, T3ResolveXy> {
   float4 a[T3_RW][4][33];             // the rows' own descriptors (+1: the four rows of a warp hit different banks)
   float sc[T3_RW][4][T3_TAB];         // exact scores
   int p2[T3_RW][4][T3_TAB];           // their indices
-  float2 xy[T3_RW][4][T3_TAB];        // their positions (match_xpos / match_ypos)
   int grp[T3_RW][4][16];              // candidate group list
 };
 
-__global__ void __launch_bounds__(32 * T3_RW)
-t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ sift1, const SiftPoint *__restrict__ sift2)
+// neighbour order: larger score first, then the lower index; the empty entry (0, -1) is passed by positive scores only
+__device__ __forceinline__ void knn_top2_insert(float &s1, int &j1, float &s2, int &j2, float s, int j)
 {
-  __shared__ T3ResolveSmem sm;
+  if (s > s1 || (s == s1 && j < j1)) { s2 = s1; j2 = j1; s1 = s; j1 = j; }
+  else if (s > s2 || (s == s2 && j < j2)) { s2 = s; j2 = j; }
+}
+
+// A call resolves one direction, `one`, and lists its uncertified rows in bf.fbRows.  A batch wave (TABLE, top-2 rule)
+// resolves every direction of the table, each with ceil(n1 / 16) CTAs from its cta0 on; its rows go to the fallback as
+// {direction, row} entries (cap of them), all of them when either set raised its bad-input flag.
+template <bool KNN, bool TABLE>
+__global__ void __launch_bounds__(32 * T3_RW)
+t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, const MbDir one, const MbDir *__restrict__ dirs, int numDirs,
+                  int2 *__restrict__ entries, unsigned int *__restrict__ numEntries, int cap)
+{
+  static_assert(KNN || !TABLE, "a batch wave runs the top-2 rule");
+  __shared__ T3ResolveSmem<KNN> sm;
   __shared__ unsigned int s_chains;      // one global atomic per CTA: same-address atomics serialise in L2
   if (threadIdx.x == 0) s_chains = 0;
   __syncthreads();
   const unsigned int FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int sub = lane >> 3, p = lane & 7;                   // row within the warp; partition / candidate slot
-  const int row = (blockIdx.x * T3_RW + w) * 4 + sub;
-  const bool valid = row < pl.n1;
-  const int rrow = valid ? row : pl.n1 - 1;                   // clamped: padding lanes mirror the last row
+  int blk = blockIdx.x, dir = 0;
+  MbDir D = one;
+  if (TABLE) {
+    dir = table_find(dirs, numDirs, &MbDir::cta0, (int)blockIdx.x);
+    D = dirs[dir];
+    blk -= D.cta0;
+  }
+  const int row = (blk * T3_RW + w) * 4 + sub;
+  const bool valid = row < D.n1;
+  if constexpr (TABLE) {
+    if (*D.bad1 | *D.bad2) {                                  // gated: every row takes the exact way
+      if (valid && p == 0) {
+        atomicAdd(&D.counters[0], 1u);
+        const unsigned e = atomicAdd(numEntries, 1u);
+        if (e < (unsigned)cap) entries[e] = make_int2(dir, row);
+      }
+      return;
+    }
+  }
+  const int rrow = valid ? row : D.n1 - 1;                    // clamped: padding lanes mirror the last row
   const int mt = rrow / T3_MT, rowInTile = rrow - mt * T3_MT;
   // the row's descriptor (each lane four float4), needed by every chain
 #pragma unroll
-  for (int j = 0; j < 4; j++) sm.a[w][sub][p + 8 * j] = __ldg(reinterpret_cast<const float4 *>(sift1[rrow].data) + p + 8 * j);
-  const float bmax = __int_as_float(*reinterpret_cast<const int *>(bf.bmax));
-  const float normA = bf.normA[rrow];
+  for (int j = 0; j < 4; j++) sm.a[w][sub][p + 8 * j] = __ldg(reinterpret_cast<const float4 *>(D.s1[rrow].data) + p + 8 * j);
+  const float bmax = __int_as_float(*reinterpret_cast<const int *>(D.bmax));
+  const float normA = D.norms[rrow];
   // merged top-3 of partition p.  The segments' tables are fetched together (independent loads, one
   // round trip) and inserted afterwards; T3_SEG bounds the unrolled part, more segments take the loop.
   float G = 0.0f, S = 0.0f, Th = 0.0f;
   int I1 = -1, I2 = -1;
   {
-    const int gt = mt;
-    const int u0 = mt * pl.n_nt, u1 = u0 + pl.n_nt - 1;
+    const int gt = D.gt0 + mt;
+    const int u0 = D.u0 + mt * D.n_nt, u1 = u0 + D.n_nt - 1;
     const int c0 = u0 / pl.U, c1 = u1 / pl.U;
     auto insert = [&](float v, int id) {
       const bool t = v > G, u2 = v > S;
@@ -471,28 +513,55 @@ t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ s
     G *= T3_UNSCALE; S *= T3_UNSCALE; Th *= T3_UNSCALE;
   }
   const float delta = 2.0f * (T3_C1 * normA * bmax + T3_C2 * (normA + bmax));
-  // L = second largest element of the pool {G[0..7], S[0]} (S[0] bounds partition 0's second best, quirk Q9)
-  float m1 = __shfl_sync(FULL, S, 0, 8), m2 = 0.0f;
+  // m2 = the second largest element of the rule's pool
+  float m1 = 0.0f, m2 = 0.0f;
+  if constexpr (KNN) {
+    // T: {G[0..7], S[0..7]}
 #pragma unroll
-  for (int y = 0; y < 8; y++) {
-    const float gy = __shfl_sync(FULL, G, y, 8);
-    m2 = fmaxf(m2, fminf(m1, gy));
-    m1 = fmaxf(m1, gy);
+    for (int y = 0; y < 8; y++) {
+      const float gy = __shfl_sync(FULL, G, y, 8), sy = __shfl_sync(FULL, S, y, 8);
+      m2 = fmaxf(m2, fminf(m1, gy));
+      m1 = fmaxf(m1, gy);
+      m2 = fmaxf(m2, fminf(m1, sy));
+      m1 = fmaxf(m1, sy);
+    }
+  } else {
+    // L: {G[0..7], S[0]} (S[0] bounds partition 0's second best, quirk Q9)
+    m1 = __shfl_sync(FULL, S, 0, 8);
+#pragma unroll
+    for (int y = 0; y < 8; y++) {
+      const float gy = __shfl_sync(FULL, G, y, 8);
+      m2 = fmaxf(m2, fminf(m1, gy));
+      m1 = fmaxf(m1, gy);
+    }
   }
-  const float L = m2;
-  const bool rowOk = (L > 2.0f * delta) && (L < 3.0e38f);       // the deciding elements are clearly positive
-  const bool rel = rowOk && (G >= L - delta);
-  const float low = (p == 0 ? fminf(L, G) : G) - delta;        // partition 0 also supplies its second best
-  const bool cert = !rel || Th <= 0.0f || Th < low;
-  const bool use1 = rel && I1 >= 0;
-  const bool use2 = rel && I2 >= 0 && S >= low;
+  const bool rowOk = (m2 > 2.0f * delta) && (m2 < 3.0e38f);    // the deciding elements are clearly positive
+  bool cert, use1, use2;
+  if constexpr (KNN) {
+    const float low = m2 - delta;
+    cert = Th <= 0.0f || Th < low;
+    use1 = rowOk && I1 >= 0 && G >= low;
+    use2 = rowOk && I2 >= 0 && S >= low;
+  } else {
+    const float L = m2;
+    const bool rel = rowOk && (G >= L - delta);
+    const float low = (p == 0 ? fminf(L, G) : G) - delta;      // partition 0 also supplies its second best
+    cert = !rel || Th <= 0.0f || Th < low;
+    use1 = rel && I1 >= 0;
+    use2 = rel && I2 >= 0 && S >= low;
+  }
   const unsigned int certMask = (__ballot_sync(FULL, cert) >> (8 * sub)) & 0xffu;
   const bool ok = valid && rowOk && certMask == 0xffu;
   if (valid && !ok && p == 0) {
-    // every row lists itself at most once, so the index stays below n1 when the counter started at zero; the clamp
-    // keeps a stale counter (a previous call that failed half-way) from writing past the list
-    const unsigned at = atomicAdd(&bf.counters[0], 1u);
-    if (at < (unsigned)pl.n_mt * T3_MT) bf.fbRows[at] = row;
+    const unsigned at = atomicAdd(&D.counters[0], 1u);
+    if (TABLE) {
+      const unsigned e = atomicAdd(numEntries, 1u);
+      if (e < (unsigned)cap) entries[e] = make_int2(dir, row);
+    } else if (at < (unsigned)pl.n_mt * T3_MT) {
+      // every row lists itself at most once, so the index stays below n1 when the counter started at zero; the clamp
+      // keeps a stale counter (a previous call that failed half-way) from writing past the list
+      bf.fbRows[at] = row;
+    }
   }
   // candidate group list (first groups, then second groups)
   const unsigned int b1 = (__ballot_sync(FULL, ok && use1) >> (8 * sub)) & 0xffu;
@@ -508,229 +577,15 @@ t3_resolve_kernel(const TcPlan pl, const T3Buffers bf, SiftPoint *__restrict__ s
     const int c = c0 + p;
     if (c < ncand) {
       const int p2 = sm.grp[w][sub][c >> 2] * 4 + (c & 3);
-      const float4 *bp = reinterpret_cast<const float4 *>(sift2[p2].data);
-      const float2 xy = make_float2(sift2[p2].xpos, sift2[p2].ypos);
-      // the reference's score: sequential k = 0..127 FMA chain starting from 0 (matching.cu:338-351).
-      // Software pipeline: the next eight float4 of the candidate are in flight while eight are consumed.
+      // candidates past n2 (zero rows of the last tile, top-2 rule) score 0: never a neighbour.  In the reference rule
+      // the B operand is zero from n2v = 32*floor(n2/32) on, so such groups never enter the tables.
       float acc = 0.0f;
-      float4 bv[8], bn[8];
-#pragma unroll
-      for (int j = 0; j < 8; j++) bv[j] = __ldg(bp + j);
-#pragma unroll
-      for (int blk = 0; blk < 4; blk++) {
-        if (blk < 3) {
-#pragma unroll
-          for (int j = 0; j < 8; j++) bn[j] = __ldg(bp + 8 * (blk + 1) + j);
-        }
-        float4 av[8];
-#pragma unroll
-        for (int j = 0; j < 8; j++) av[j] = sm.a[w][sub][8 * blk + j];
-#pragma unroll
-        for (int j = 0; j < 8; j++) {
-          acc = __fmaf_rn(av[j].x, bv[j].x, acc);
-          acc = __fmaf_rn(av[j].y, bv[j].y, acc);
-          acc = __fmaf_rn(av[j].z, bv[j].z, acc);
-          acc = __fmaf_rn(av[j].w, bv[j].w, acc);
-        }
-#pragma unroll
-        for (int j = 0; j < 8; j++) bv[j] = bn[j];
-      }
-      sm.sc[w][sub][c] = acc;
-      sm.p2[w][sub][c] = p2;
-      sm.xy[w][sub][c] = xy;
-    }
-  }
-  __syncwarp();
-  // per-partition rule: lane p scans its row's table for partition p ((p2 >> 2) & 7)
-  float pmx = 0.0f, psec = 0.0f;
-  int pidx = -1, pent = -1;
-  for (int e = 0; e < maxc; e++) {
-    if (e < ncand) {
-      const int p2 = sm.p2[w][sub][e];
-      const float sc = sm.sc[w][sub][e];
-      if (((p2 >> 2) & 7) == p && sc > 0.0f) {       // a non-positive score cannot match (matching.cu:317-321)
-        if (sc > pmx) { psec = pmx; pmx = sc; pidx = p2; pent = e; }
-        else {
-          if (sc == pmx && p2 < pidx) { pidx = p2; pent = e; }
-          psec = fmaxf(psec, sc);
-        }
-      }
-    }
-  }
-  // 8-way merge, matching.cu:378-390
-  float mx = __shfl_sync(FULL, pmx, 0, 8), sec = __shfl_sync(FULL, psec, 0, 8);
-  int idx = __shfl_sync(FULL, pidx, 0, 8), ent = __shfl_sync(FULL, pent, 0, 8);
-#pragma unroll
-  for (int y = 0; y < 8; y++) {
-    const float my = __shfl_sync(FULL, pmx, y, 8);
-    const int iy = __shfl_sync(FULL, pidx, y, 8), ey = __shfl_sync(FULL, pent, y, 8);
-    if (idx != iy) {
-      if (my > mx) { sec = fmaxf(mx, sec); mx = my; idx = iy; ent = ey; }
-      else if (my > sec) sec = my;
-    }
-  }
-  if (ok && p == 0) {
-    SiftPoint *o = sift1 + row;
-    const float2 xy = ent >= 0 ? sm.xy[w][sub][ent] : make_float2(0.0f, 0.0f);
-    o->score = mx;
-    o->match = idx;
-    o->match_xpos = xy.x;
-    o->match_ypos = xy.y;
-    o->ambiguity = __fdiv_rn(sec, __fadd_rn(mx, 1e-6f));
-    atomicAdd(&s_chains, (unsigned)ncand);
-  }
-  __syncthreads();
-  if (threadIdx.x == 0 && s_chains) { atomicAdd(&bf.counters[1], s_chains >> 2); atomicAdd(&bf.counters[2], s_chains); }
-}
-
-// ---- knn resolve ---------------------------------------------------------------------------------
-// The true two nearest neighbours (match_knn.cu states the order) from the same top-3 tables, all n2 candidates.
-// Per partition the merged tables give G >= S >= Th and the groups I1, I2.  T is the second largest of the 16 values
-// {G[0..7], S[0..7]}: two distinct groups have approximate maxima >= T, so two distinct candidates have exact scores
-// >= T - eps, and score2 >= T - eps.  A candidate whose group is not re-scored lies in a group below T - delta
-// (delta = 2 eps): it is either a partition's third group or lower (<= Th, certified < T - delta) or an I1 / I2 group
-// below T - delta.  Its exact score is then < T - eps <= score2, strictly, so the top two of the re-scored candidates
-// (at most 8 x 2 groups x 4 = T3_TAB) are the row's top two, ties included.  T > 2 delta keeps both clearly positive.
-struct KnnResolveSmem {
-  float4 a[T3_RW][4][33];             // the rows' own descriptors
-  float sc[T3_RW][4][T3_TAB];         // exact scores
-  int p2[T3_RW][4][T3_TAB];           // their indices
-  int grp[T3_RW][4][16];              // candidate group list
-};
-
-// neighbour order: larger score first, then the lower index; the empty entry (0, -1) is passed by positive scores only
-__device__ __forceinline__ void knn_top2_insert(float &s1, int &j1, float &s2, int &j2, float s, int j)
-{
-  if (s > s1 || (s == s1 && j < j1)) { s2 = s1; j2 = j1; s1 = s; j1 = j; }
-  else if (s > s2 || (s == s2 && j < j2)) { s2 = s; j2 = j; }
-}
-
-// A call resolves one direction (pl, bf and the arguments).  A batch wave (TABLE) resolves every direction of the table,
-// each with ceil(n1 / 16) CTAs from its cta0 on; its rows go to the fallback as {direction, row} entries (cap of them),
-// all of them when either set raised its bad-input flag.
-template <bool TABLE>
-__global__ void __launch_bounds__(32 * T3_RW)
-knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restrict__ sift1,
-                   const SiftPoint *__restrict__ sift2, int n2, int2 *__restrict__ idx, float2 *__restrict__ score,
-                   const MbDir *__restrict__ dirs, int numDirs, int2 *__restrict__ entries,
-                   unsigned int *__restrict__ numEntries, int cap)
-{
-  __shared__ KnnResolveSmem sm;
-  __shared__ unsigned int s_chains;
-  if (threadIdx.x == 0) s_chains = 0;
-  __syncthreads();
-  const unsigned int FULL = 0xffffffffu;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int sub = lane >> 3, p = lane & 7;                   // row within the warp; partition / candidate slot
-  int blk = blockIdx.x, n1 = pl.n1, n_nt = pl.n_nt, tileU0 = 0, gt0 = 0, dir = 0;
-  const float *normAs = bf.normA, *bmaxp = bf.bmax;
-  unsigned int *counters = bf.counters;
-  if (TABLE) {
-    dir = table_find(dirs, numDirs, &MbDir::cta0, (int)blockIdx.x);
-    const MbDir &D = dirs[dir];
-    blk -= D.cta0; n1 = D.n1; n2 = D.n2; n_nt = D.n_nt; tileU0 = D.u0; gt0 = D.gt0;
-    sift1 = D.s1; sift2 = D.s2; idx = D.idx; score = D.score;
-    normAs = D.norms; bmaxp = D.bmax; counters = D.counters;
-    if (*D.bad1 | *D.bad2) {                                  // gated: every row takes the exact way
-      const int row = (blk * T3_RW + w) * 4 + sub;
-      if (row < n1 && p == 0) {
-        atomicAdd(&counters[0], 1u);
-        const unsigned e = atomicAdd(numEntries, 1u);
-        if (e < (unsigned)cap) entries[e] = make_int2(dir, row);
-      }
-      return;
-    }
-  }
-  const int row = (blk * T3_RW + w) * 4 + sub;
-  const bool valid = row < n1;
-  const int rrow = valid ? row : n1 - 1;                      // clamped: padding lanes mirror the last row
-  const int mt = rrow / T3_MT, rowInTile = rrow - mt * T3_MT;
-#pragma unroll
-  for (int j = 0; j < 4; j++) sm.a[w][sub][p + 8 * j] = __ldg(reinterpret_cast<const float4 *>(sift1[rrow].data) + p + 8 * j);
-  const float bmax = __int_as_float(*reinterpret_cast<const int *>(bmaxp));
-  const float normA = normAs[rrow];
-  // merged top-3 of partition p over the segments (as t3_resolve_kernel)
-  float G = 0.0f, S = 0.0f, Th = 0.0f;
-  int I1 = -1, I2 = -1;
-  {
-    const int gt = gt0 + mt;
-    const int u0 = tileU0 + mt * n_nt, u1 = u0 + n_nt - 1;
-    const int c0 = u0 / pl.U, c1 = u1 / pl.U;
-    auto insert = [&](float v, int id) {
-      const bool t = v > G, u2 = v > S;
-      Th = fmaxf(Th, fminf(S, v));
-      I2 = u2 ? (t ? I1 : id) : I2;
-      S = fmaxf(S, fminf(G, v));
-      I1 = t ? id : I1;
-      G = fmaxf(G, v);
-    };
-    constexpr int T3_SEG = 6;
-    float v[T3_SEG][3];
-    int id[T3_SEG][2];
-#pragma unroll
-    for (int k = 0; k < T3_SEG; k++) {
-      const int c = c0 + k;
-      if (c <= c1) {
-        const float *q = bf.pm + tc_slot(gt, c, rowInTile) * T3_PM;
-        v[k][0] = q[p]; v[k][1] = q[8 + p]; v[k][2] = q[16 + p];
-        id[k][0] = __float_as_int(q[24 + p]); id[k][1] = __float_as_int(q[32 + p]);
-      } else {
-        v[k][0] = v[k][1] = v[k][2] = 0.0f; id[k][0] = id[k][1] = -1;
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < T3_SEG; k++) { insert(v[k][0], id[k][0]); insert(v[k][1], id[k][1]); insert(v[k][2], -1); }
-    for (int c = c0 + T3_SEG; c <= c1; c++) {
-      const float *q = bf.pm + tc_slot(gt, c, rowInTile) * T3_PM;
-      insert(q[p], __float_as_int(q[24 + p])); insert(q[8 + p], __float_as_int(q[32 + p])); insert(q[16 + p], -1);
-    }
-    G *= T3_UNSCALE; S *= T3_UNSCALE; Th *= T3_UNSCALE;
-  }
-  const float delta = 2.0f * (T3_C1 * normA * bmax + T3_C2 * (normA + bmax));
-  // T = second largest of {G[0..7], S[0..7]}
-  float m1 = 0.0f, m2 = 0.0f;
-#pragma unroll
-  for (int y = 0; y < 8; y++) {
-    const float gy = __shfl_sync(FULL, G, y, 8), sy = __shfl_sync(FULL, S, y, 8);
-    m2 = fmaxf(m2, fminf(m1, gy));
-    m1 = fmaxf(m1, gy);
-    m2 = fmaxf(m2, fminf(m1, sy));
-    m1 = fmaxf(m1, sy);
-  }
-  const float T = m2;
-  const bool rowOk = (T > 2.0f * delta) && (T < 3.0e38f);
-  const float low = T - delta;
-  const bool cert = Th <= 0.0f || Th < low;
-  const bool use1 = rowOk && I1 >= 0 && G >= low;
-  const bool use2 = rowOk && I2 >= 0 && S >= low;
-  const unsigned int certMask = (__ballot_sync(FULL, cert) >> (8 * sub)) & 0xffu;
-  const bool ok = valid && rowOk && certMask == 0xffu;
-  if (valid && !ok && p == 0) {
-    const unsigned at = atomicAdd(&counters[0], 1u);
-    if (TABLE) {
-      const unsigned e = atomicAdd(numEntries, 1u);
-      if (e < (unsigned)cap) entries[e] = make_int2(dir, row);
-    } else if (at < (unsigned)pl.n_mt * T3_MT) {
-      bf.fbRows[at] = row;
-    }
-  }
-  const unsigned int b1 = (__ballot_sync(FULL, ok && use1) >> (8 * sub)) & 0xffu;
-  const unsigned int b2 = (__ballot_sync(FULL, ok && use2) >> (8 * sub)) & 0xffu;
-  const int n1g = __popc(b1), ncand = 4 * (n1g + __popc(b2));
-  if (ok && use1) sm.grp[w][sub][__popc(b1 & ((1u << p) - 1))] = I1;
-  if (ok && use2) sm.grp[w][sub][n1g + __popc(b2 & ((1u << p) - 1))] = I2;
-  __syncwarp();
-  int maxc = ncand;
-#pragma unroll
-  for (int o = 16; o >= 8; o >>= 1) maxc = max(maxc, __shfl_xor_sync(FULL, maxc, o));
-  for (int c0 = 0; c0 < maxc; c0 += 8) {
-    const int c = c0 + p;
-    if (c < ncand) {
-      const int p2 = sm.grp[w][sub][c >> 2] * 4 + (c & 3);
-      float acc = 0.0f;                 // candidates past n2 (zero rows of the last tile) score 0: never a neighbour
-      if (p2 < n2) {
-        const float4 *bp = reinterpret_cast<const float4 *>(sift2[p2].data);
-        // the reference's score: sequential k = 0..127 FMA chain starting from 0, loads pipelined as in t3_resolve_kernel
+      float2 xy = make_float2(0.0f, 0.0f);
+      if (p2 < D.n2) {
+        const float4 *bp = reinterpret_cast<const float4 *>(D.s2[p2].data);
+        if constexpr (!KNN) xy = make_float2(D.s2[p2].xpos, D.s2[p2].ypos);
+        // the reference's score: sequential k = 0..127 FMA chain starting from 0 (matching.cu:338-351).
+        // Software pipeline: the next eight float4 of the candidate are in flight while eight are consumed.
         float4 bv[8], bn[8];
 #pragma unroll
         for (int j = 0; j < 8; j++) bv[j] = __ldg(bp + j);
@@ -756,27 +611,68 @@ knn_resolve_kernel(const TcPlan pl, const T3Buffers bf, const SiftPoint *__restr
       }
       sm.sc[w][sub][c] = acc;
       sm.p2[w][sub][c] = p2;
+      if constexpr (!KNN) sm.xy[w][sub][c] = xy;
     }
   }
   __syncwarp();
-  // lane p: top two of entries p, p + 8, ...; then a butterfly over the row's eight lanes (the order is total)
-  float s1 = 0.0f, s2 = 0.0f;
-  int j1 = -1, j2 = -1;
-  for (int e = p; e < ncand; e += 8) knn_top2_insert(s1, j1, s2, j2, sm.sc[w][sub][e], sm.p2[w][sub][e]);
+  if constexpr (KNN) {
+    // lane p: top two of entries p, p + 8, ...; then a butterfly over the row's eight lanes (the order is total)
+    float s1 = 0.0f, s2 = 0.0f;
+    int j1 = -1, j2 = -1;
+    for (int e = p; e < ncand; e += 8) knn_top2_insert(s1, j1, s2, j2, sm.sc[w][sub][e], sm.p2[w][sub][e]);
 #pragma unroll
-  for (int o = 1; o < 8; o <<= 1) {
-    const float t1 = __shfl_xor_sync(FULL, s1, o, 8), t2 = __shfl_xor_sync(FULL, s2, o, 8);
-    const int k1 = __shfl_xor_sync(FULL, j1, o, 8), k2 = __shfl_xor_sync(FULL, j2, o, 8);
-    knn_top2_insert(s1, j1, s2, j2, t1, k1);
-    knn_top2_insert(s1, j1, s2, j2, t2, k2);
+    for (int o = 1; o < 8; o <<= 1) {
+      const float t1 = __shfl_xor_sync(FULL, s1, o, 8), t2 = __shfl_xor_sync(FULL, s2, o, 8);
+      const int k1 = __shfl_xor_sync(FULL, j1, o, 8), k2 = __shfl_xor_sync(FULL, j2, o, 8);
+      knn_top2_insert(s1, j1, s2, j2, t1, k1);
+      knn_top2_insert(s1, j1, s2, j2, t2, k2);
+    }
+    if (ok && p == 0) {
+      D.idx[row] = make_int2(j1, j2);
+      D.score[row] = make_float2(s1, s2);
+    }
+  } else {
+    // per-partition rule: lane p scans its row's table for partition p ((p2 >> 2) & 7)
+    float pmx = 0.0f, psec = 0.0f;
+    int pidx = -1, pent = -1;
+    for (int e = 0; e < maxc; e++) {
+      if (e < ncand) {
+        const int p2 = sm.p2[w][sub][e];
+        const float sc = sm.sc[w][sub][e];
+        if (((p2 >> 2) & 7) == p && sc > 0.0f) {       // a non-positive score cannot match (matching.cu:317-321)
+          if (sc > pmx) { psec = pmx; pmx = sc; pidx = p2; pent = e; }
+          else {
+            if (sc == pmx && p2 < pidx) { pidx = p2; pent = e; }
+            psec = fmaxf(psec, sc);
+          }
+        }
+      }
+    }
+    // 8-way merge, matching.cu:378-390
+    float mx = __shfl_sync(FULL, pmx, 0, 8), sec = __shfl_sync(FULL, psec, 0, 8);
+    int idx = __shfl_sync(FULL, pidx, 0, 8), ent = __shfl_sync(FULL, pent, 0, 8);
+#pragma unroll
+    for (int y = 0; y < 8; y++) {
+      const float my = __shfl_sync(FULL, pmx, y, 8);
+      const int iy = __shfl_sync(FULL, pidx, y, 8), ey = __shfl_sync(FULL, pent, y, 8);
+      if (idx != iy) {
+        if (my > mx) { sec = fmaxf(mx, sec); mx = my; idx = iy; ent = ey; }
+        else if (my > sec) sec = my;
+      }
+    }
+    if (ok && p == 0) {
+      SiftPoint *o = const_cast<SiftPoint *>(D.s1) + row;     // a match writes set 1's match fields in place
+      const float2 xy = ent >= 0 ? sm.xy[w][sub][ent] : make_float2(0.0f, 0.0f);
+      o->score = mx;
+      o->match = idx;
+      o->match_xpos = xy.x;
+      o->match_ypos = xy.y;
+      o->ambiguity = __fdiv_rn(sec, __fadd_rn(mx, 1e-6f));
+    }
   }
-  if (ok && p == 0) {
-    idx[row] = make_int2(j1, j2);
-    score[row] = make_float2(s1, s2);
-    atomicAdd(&s_chains, (unsigned)ncand);
-  }
+  if (ok && p == 0) atomicAdd(&s_chains, (unsigned)ncand);
   __syncthreads();
-  if (threadIdx.x == 0 && s_chains) { atomicAdd(&counters[1], s_chains >> 2); atomicAdd(&counters[2], s_chains); }
+  if (threadIdx.x == 0 && s_chains) { atomicAdd(&D.counters[1], s_chains >> 2); atomicAdd(&D.counters[2], s_chains); }
 }
 
 // exact SIMT scan of the rows the tensor path could not certify (match.cu)
@@ -803,7 +699,6 @@ static void t3_schedule(TcPlan &pl, int sms)
 static TcPlan t3_plan(int n1, int n2v, int sms)
 {
   TcPlan pl;
-  pl.n1 = n1; pl.n2v = n2v;
   pl.n_mt = idivup(n1, T3_MT); pl.n_nt = idivup(n2v, T3_N);
   pl.total = pl.n_mt * pl.n_nt;
   t3_schedule(pl, sms);
@@ -813,11 +708,13 @@ static TcPlan t3_plan(int n1, int n2v, int sms)
 static size_t t3_slots(int tiles, int grid) { return ((size_t)tiles + grid) * T3_MT; }
 static size_t t3_slots(const TcPlan &pl) { return t3_slots(pl.n_mt, pl.grid); }
 
-// A tensor-path call once its prep kernel is in: each direction's plan and view of the workspace, the bad-input gate
-// (shared: any bad value, either set), the call's flag area and the timing events (or null).
+// A tensor-path call once its prep kernel is in: each direction's plan, view of the workspace and resolve view (its
+// rows, candidates, norms, counters; a knn call adds the neighbour lists), the bad-input gate (shared: any bad value,
+// either set), the call's flag area and the timing events (or null).
 struct T3Call {
   TcPlan pf, pr;
   T3Buffers fw, rv;
+  MbDir df, dr;
   const unsigned int *gate;
   const float *flags;
   cudaEvent_t *tev;
@@ -878,9 +775,17 @@ static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const Si
   // counters of the two directions are flags [4..6] and [8..10]
   p[0].bmax = flags + 2; p[1].bmax = flags;
   unsigned int *counters = reinterpret_cast<unsigned int *>(flags);
-  t.fw = {p[0].a, copy[1] ? p[1].b : p[1].a, p[0].norms, flags, c.tcTables.as<float>(), c.tcRows.as<int>(), counters + 4};
-  t.rv = {p[1].a, copy[0] ? p[0].b : p[0].a, p[1].norms, flags + 2, c.tcTables.as<float>(), c.tcRows.as<int>(),
-          counters + 8};
+  t.fw = {p[0].a, copy[1] ? p[1].b : p[1].a, c.tcTables.as<float>(), c.tcRows.as<int>()};
+  t.rv = {p[1].a, copy[0] ? p[0].b : p[0].a, c.tcTables.as<float>(), c.tcRows.as<int>()};
+  auto view = [](const SiftPoint *a, int na, const SiftPoint *b, int nb, const float *norms, const float *bmax,
+                 unsigned int *cnt, int n_nt) {
+    MbDir d{};
+    d.s1 = a; d.s2 = b; d.n1 = na; d.n2 = nb;
+    d.norms = norms; d.bmax = bmax; d.counters = cnt; d.n_nt = n_nt;
+    return d;
+  };
+  t.df = view(s1, n1, s2, n2, p[0].norms, flags, counters + 4, t.pf.n_nt);
+  t.dr = view(s2, n2, s1, n1, p[1].norms, flags + 2, counters + 8, t.pr.n_nt);
   t.gate = counters + 1;
   t.flags = flags;
   t.tev = match_timing_events();
@@ -892,20 +797,30 @@ static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const Si
   return 0;
 }
 
-// One direction after the prep kernel: GEMM, resolve, then the exact kernel for the rows that could not be certified
-// -- or, for inputs the split cannot bound (*gate != 0: |x| >= 8, NaN, Inf), for every row; which of the two is
-// decided on the device.  ev (optional): three events, recorded after each launch.
-static int t3_direction(const TcPlan &pl, const T3Buffers &bf, SiftPoint *s1, int n1, const SiftPoint *s2, int n2,
-                        const unsigned int *gate, cudaStream_t st, cudaEvent_t *ev)
+// exact two-nearest-neighbour scan of the listed rows, or of every row if *gate != 0 (match_knn.cu)
+int knn_exact_fallback(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score,
+                       const int *rows, const unsigned int *nrows, const unsigned int *gate);
+
+// One direction after the prep kernel: GEMM, resolve, then the rule's exact kernel for the rows that could not be
+// certified -- or, for inputs the split cannot bound (*gate != 0: |x| >= 8, NaN, Inf), for every row; which of the two
+// is decided on the device.  KNN: the two nearest neighbours into d.idx / d.score; else the reference rule into set 1's
+// match fields.  ev (optional): three events, recorded after each launch.
+template <bool KNN>
+static int t3_direction(DeviceCtx &c, const TcPlan &pl, const T3Buffers &bf, const MbDir &d, const unsigned int *gate,
+                        cudaEvent_t *ev)
 {
+  const cudaStream_t st = c.stream;
   t3_gemm_kernel<false><<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf, nullptr, 0);
   if (ev) cudaEventRecord(ev[0], st);
-  t3_resolve_kernel<<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2);
+  t3_resolve_kernel<KNN, false><<<idivup(d.n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, d, nullptr, 0, nullptr, nullptr, 0);
   if (ev) cudaEventRecord(ev[1], st);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
-  int r;
-  if ((r = match_exact_fallback(s1, n1, s2, n2, bf.fbRows, bf.counters, gate, st)) < 0) return r;
+  const int r = KNN ? knn_exact_fallback(c, d.s1, d.n1, d.s2, d.n2, reinterpret_cast<int *>(d.idx),
+                                         reinterpret_cast<float *>(d.score), bf.fbRows, d.counters, gate)
+                    : match_exact_fallback(const_cast<SiftPoint *>(d.s1), d.n1, d.s2, d.n2, bf.fbRows, d.counters, gate,
+                                           st);
+  if (r < 0) return r;
   if (ev) cudaEventRecord(ev[2], st);
   return 0;
 }
@@ -964,38 +879,14 @@ int match_tensor(DeviceCtx &c, SiftPoint *s1, int n1, SiftPoint *s2, int n2, con
   int r;
   if ((r = t3_setup(c, s1, n1, n1v, s2, n2, n2v, mu != nullptr, t)) < 0) return r;
   cudaEvent_t *tev = t.tev;
-  if ((r = t3_direction(t.pf, t.fw, s1, n1, s2, n2, t.gate, c.stream, tev ? tev + 2 : nullptr)) < 0) return r;
+  if ((r = t3_direction<false>(c, t.pf, t.fw, t.df, t.gate, tev ? tev + 2 : nullptr)) < 0) return r;
   if (mu) {
-    if ((r = t3_direction(t.pr, t.rv, s2, n2, s1, n1, t.gate, c.stream, tev ? tev + 5 : nullptr)) < 0) return r;
+    if ((r = t3_direction<false>(c, t.pr, t.rv, t.dr, t.gate, tev ? tev + 5 : nullptr)) < 0) return r;
     if ((r = launch_mutual_pairs(c, s1, n1, s2, n2, *mu)) < 0) return r;
     if (tev) cudaEventRecord(tev[8], c.stream);
   }
   if (tev) t3_print_timing(mu ? "mutual" : "match", n1, n2, tev, mu ? 8 : 4);
   return t3_end(c, t.flags);
-}
-
-// exact two-nearest-neighbour scan of the listed rows, or of every row if *gate != 0 (match_knn.cu)
-int knn_exact_fallback(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int *idx, float *score,
-                       const int *rows, const unsigned int *nrows, const unsigned int *gate);
-
-// One knn direction after the prep kernel: GEMM, knn resolve, exact fallback.  ev (optional): three events.
-static int knn_direction(DeviceCtx &c, const TcPlan &pl, const T3Buffers &bf, const SiftPoint *s1, int n1,
-                         const SiftPoint *s2, int n2, int *idx, float *score, const unsigned int *gate, cudaEvent_t *ev)
-{
-  const cudaStream_t st = c.stream;
-  t3_gemm_kernel<false><<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf, nullptr, 0);
-  if (ev) cudaEventRecord(ev[0], st);
-  knn_resolve_kernel<false><<<idivup(n1, 4 * T3_RW), 32 * T3_RW, 0, st>>>(pl, bf, s1, s2, n2,
-                                                                         reinterpret_cast<int2 *>(idx),
-                                                                         reinterpret_cast<float2 *>(score), nullptr, 0,
-                                                                         nullptr, nullptr, 0);
-  if (ev) cudaEventRecord(ev[1], st);
-  count_launch(2);
-  CS_CUDA(cudaGetLastError());
-  int r;
-  if ((r = knn_exact_fallback(c, s1, n1, s2, n2, idx, score, bf.fbRows, bf.counters, gate)) < 0) return r;
-  if (ev) cudaEventRecord(ev[2], st);
-  return 0;
 }
 
 // The two nearest neighbours of every row of set 1 among all n2 candidates (idx1 / score1, [n1][2]); with idx2 also
@@ -1011,9 +902,10 @@ int match_knn_tensor(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint 
   int r;
   if ((r = t3_setup(c, s1, n1, n1, s2, n2, n2, both, t)) < 0) return r;
   cudaEvent_t *tev = t.tev;
-  if ((r = knn_direction(c, t.pf, t.fw, s1, n1, s2, n2, idx1, score1, t.gate, tev ? tev + 2 : nullptr)) < 0) return r;
-  if (both && (r = knn_direction(c, t.pr, t.rv, s2, n2, s1, n1, idx2, score2, t.gate, tev ? tev + 5 : nullptr)) < 0)
-    return r;
+  t.df.idx = reinterpret_cast<int2 *>(idx1); t.df.score = reinterpret_cast<float2 *>(score1);
+  t.dr.idx = reinterpret_cast<int2 *>(idx2); t.dr.score = reinterpret_cast<float2 *>(score2);
+  if ((r = t3_direction<true>(c, t.pf, t.fw, t.df, t.gate, tev ? tev + 2 : nullptr)) < 0) return r;
+  if (both && (r = t3_direction<true>(c, t.pr, t.rv, t.dr, t.gate, tev ? tev + 5 : nullptr)) < 0) return r;
   if (tev) t3_print_timing("knn", n1, n2, tev, both ? 7 : 4);
   return t3_end(c, t.flags);
 }
@@ -1224,8 +1116,7 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
     TcPlan pl{};
     pl.total = v.units;
     t3_schedule(pl, c.sms);
-    const T3Buffers bf = {c.tcA.as<__half>(), c.tcA.as<__half>(), nullptr, nullptr, c.tcTables.as<float>(), nullptr,
-                          nullptr};
+    const T3Buffers bf = {c.tcA.as<__half>(), c.tcA.as<__half>(), c.tcTables.as<float>(), nullptr};
     CS_CUDA(cudaMemsetAsync(state, 0, v.zeroWords * sizeof(unsigned int), st));
     CS_CUDA(cudaMemcpyAsync(dt, hp, v.tabBytes, cudaMemcpyHostToDevice, st));
     if (tev) cudaEventRecord(tev[0], st);
@@ -1233,8 +1124,8 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
     if (tev) cudaEventRecord(tev[1], st);
     t3_gemm_kernel<true><<<pl.grid, T3_THREADS, T3_SMEM_BYTES, st>>>(pl, bf, dd, D);
     if (tev) cudaEventRecord(tev[2], st);
-    knn_resolve_kernel<true><<<v.resolveCtas, 32 * T3_RW, 0, st>>>(pl, bf, nullptr, nullptr, 0, nullptr, nullptr, dd, D,
-                                                                   entries, numEntries, v.rows);
+    t3_resolve_kernel<true, true><<<v.resolveCtas, 32 * T3_RW, 0, st>>>(pl, bf, MbDir{}, dd, D, entries, numEntries,
+                                                                        v.rows);
     if (tev) cudaEventRecord(tev[3], st);
     count_launch(3);
     CS_CUDA(cudaGetLastError());

@@ -1,7 +1,7 @@
 """CPU checks of two-nearest-neighbour matching (cs_match_knn2, cs_match_ratio, cs_match_ratio_host): the entry points
 exist, they reject bad arguments before any CUDA call, the Python wrappers pass their arguments through, the CPU
 statement (tests/knn_oracle.c) equals a brute-force numpy chain, and a numpy restatement of the tensor path's top-2
-certification rule (knn_resolve_kernel in csrc/match_tc.cu) reproduces the oracle on every row it certifies."""
+certification rule (the top-2 rule of t3_resolve_kernel in csrc/match_tc.cu) reproduces the oracle on every row it certifies."""
 import ctypes
 import os
 import re

@@ -1,5 +1,5 @@
 """CPU restatement (numpy) of the tensor matcher's decision logic (csrc/match_tc.cu: epilogue top-3
-tracking + t3_resolve_kernel), checked against the oracle's exact MatchSiftData.  It pins the argument
+tracking + t3_resolve_kernel's reference rule), checked against the oracle's exact MatchSiftData.  It pins the argument
 that makes one approximate GEMM pass sufficient: with |approx - exact| <= eps and delta = 2*eps,
 
   * per (row, partition) the three largest 4-candidate group maxima g1 >= g2 >= g3 and the ids of the
