@@ -19,7 +19,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "match_knn2", "MatchSiftDataRatio", "match_ratio_host", "VerifyPairs", "verify_pairs_host", "verify_stats",
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
-           "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch"]
+           "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
+           "MatchSiftDataGuidedBatch"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -89,6 +90,7 @@ def lib():
         "cs_verify_pairs_batch": (ip, [vp, ip, ip, ip, fp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_verify_essential_batch": (ip, [vp, ip, vp, vp, ip, fp, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_match_ratio_batch": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
+        "cs_match_guided_batch": (ip, [vp, ip, vp, ip, vp, vp, fp, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -358,11 +360,10 @@ class MatchJob(ctypes.Structure):
     _fields_ = [("set1", ctypes.c_int), ("set2", ctypes.c_int), ("pairs", ctypes.c_void_p), ("maxPairs", ctypes.c_int)]
 
 
-def MatchSiftDataRatioBatch(datas, jobs, maxRatio=0.8, maxDistance=0.7, crossCheck=True):
-    """MatchSiftDataRatio over many image pairs in one call (cs_match_ratio_batch): datas is a list of SiftData, jobs a
-    list of (a, b) indices into it.  Job p's pairs equal MatchSiftDataRatio(datas[a], datas[b], maxRatio, maxDistance,
-    crossCheck) bit for bit.  Every pair list lives in one device buffer, room for each job's largest count.  Returns
-    (pairs: a list of int32 [k, 2], stats uint64 [J, 4] as match_stats after a mode-2 call, ms)."""
+def _match_batch(datas, jobs, crossCheck, call):
+    """The set and job tables of a batched match over SiftData datas and (a, b) jobs, every pair list in one device
+    buffer with room for each job's largest count; call(sets, numSets, jobs, numJobs, counts, stats, ms) runs the
+    batch.  Returns (pairs: a list of int32 [k, 2], stats uint64 [J, 4], ms)."""
     sets = (MatchSet * max(len(datas), 1))()
     for s, d in enumerate(datas):
         sets[s] = MatchSet(d.d_data, d.numPts)
@@ -380,15 +381,24 @@ def MatchSiftDataRatioBatch(datas, jobs, maxRatio=0.8, maxDistance=0.7, crossChe
         table = (MatchJob * max(J, 1))()
         for q, (a, b) in enumerate(jobs):
             table[q] = MatchJob(int(a), int(b), buf.ptr + 8 * int(offsets[q]) if rooms[q] else None, rooms[q])
-        _check(lib().cs_match_ratio_batch(ctypes.addressof(sets) if datas else None, len(datas),
-                                          ctypes.addressof(table) if J else None, J, float(maxRatio),
-                                          float(maxDistance), int(bool(crossCheck)), _ptr(counts), _ptr(stats),
-                                          ctypes.byref(ms)), "MatchSiftDataRatioBatch")
+        call(ctypes.addressof(sets) if datas else None, len(datas), ctypes.addressof(table) if J else None, J,
+             _ptr(counts), _ptr(stats), ctypes.byref(ms))
         flat = buf.download(np.int32, 2 * total).reshape(-1, 2) if total else np.zeros((0, 2), np.int32)
     finally:
         buf.free()
     pairs = [flat[offsets[q]:offsets[q] + int(counts[q])].copy() for q in range(J)]
     return pairs, stats, ms.value
+
+
+def MatchSiftDataRatioBatch(datas, jobs, maxRatio=0.8, maxDistance=0.7, crossCheck=True):
+    """MatchSiftDataRatio over many image pairs in one call (cs_match_ratio_batch): datas is a list of SiftData, jobs a
+    list of (a, b) indices into it.  Job p's pairs equal MatchSiftDataRatio(datas[a], datas[b], maxRatio, maxDistance,
+    crossCheck) bit for bit.  Every pair list lives in one device buffer, room for each job's largest count.  Returns
+    (pairs: a list of int32 [k, 2], stats uint64 [J, 4] as match_stats after a mode-2 call, ms)."""
+    def call(sets, S, table, J, counts, stats, ms):
+        _check(lib().cs_match_ratio_batch(sets, S, table, J, float(maxRatio), float(maxDistance), int(bool(crossCheck)),
+                                          counts, stats, ms), "MatchSiftDataRatioBatch")
+    return _match_batch(datas, jobs, crossCheck, call)
 
 
 def match_ratio_host(s1, s2, maxRatio=0.8, maxDistance=0.7, crossCheck=True, mode=0):
@@ -684,6 +694,26 @@ def guided_stats():
     out = (ctypes.c_ulonglong * 4)()
     _check(lib().cs_match_guided_stats(out), "cs_match_guided_stats")
     return list(out)
+
+
+def MatchSiftDataGuidedBatch(datas, jobs, model, Ms, thresh=4.0, maxRatio=0.8, maxDistance=0.7, crossCheck=True):
+    """MatchSiftDataGuided over many image pairs in one call (cs_match_guided_batch): datas and jobs as for
+    MatchSiftDataRatioBatch; model one name or code for every job, or a list with one per job; Ms [J, 3, 3], for example
+    the models VerifyPairsBatch returns (leave out the jobs whose verification failed: a zero model is an error).  Job
+    p's pairs equal MatchSiftDataGuided(datas[a], datas[b], model[p], Ms[p], thresh, maxRatio, maxDistance, crossCheck)
+    bit for bit.  Returns (pairs: a list of int32 [k, 2], stats uint64 [J, 4] as guided_stats after that call, ms)."""
+    J = len(jobs)
+    names = list(model) if isinstance(model, (list, tuple, np.ndarray)) else [model] * J
+    if len(names) != J:
+        raise ValueError("model: one for every job, or a list of %d, not %d" % (J, len(names)))
+    codes = np.array([_geom_model(m) for m in names], np.int32)
+    m = np.ascontiguousarray(np.asarray(Ms, np.float64).reshape(J, 9))
+
+    def call(sets, S, table, J, counts, stats, ms):
+        _check(lib().cs_match_guided_batch(sets, S, table, J, _ptr(codes), _ptr(m), float(thresh), float(maxRatio),
+                                           float(maxDistance), int(bool(crossCheck)), counts, stats, ms),
+               "MatchSiftDataGuidedBatch")
+    return _match_batch(datas, jobs, crossCheck, call)
 
 
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):

@@ -746,6 +746,23 @@ static int ratio_batch_args(const char *fn, const cs_match_set *sets, int numSet
   });
 }
 
+// The arguments of cs_match_guided_batch: those of cs_match_ratio_batch, then every job's model as the single call
+// checks it (named jobs[p]).
+static int guided_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs,
+                             int numJobs, const int *models, const double *models_in, float thresh, float maxRatio,
+                             float maxDistance, const int *counts_out)
+{
+  int r;
+  if ((r = ratio_batch_args(fn, sets, numSets, jobs, numJobs, maxRatio, maxDistance, counts_out)) < 0) return r;
+  if (numJobs > 0 && (!models || !models_in)) return arg_error(fn, "models and models_in must not be NULL");
+  for (int p = 0; p < numJobs; p++) {
+    char name[96];
+    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
+    if ((r = guided_args(name, models[p], models_in + 9 * (size_t)p, thresh)) < 0) return r;
+  }
+  return 0;
+}
+
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
 {
   VerifyCalib cal;
@@ -1549,6 +1566,41 @@ int cs_match_ratio_batch(const cs_match_set *sets, int numSets, const cs_match_j
       }
     }
     st[3] = 2;
+  }
+  return 0;
+}
+
+int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                          const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
+                          int crossCheck, int *counts_out, unsigned long long *stats_out, double *ms)
+{
+  const char *fn = "cs_match_guided_batch";
+  if (ms) *ms = 0.0;
+  int r = guided_batch_args(fn, sets, numSets, jobs, numJobs, models, models_in, thresh, maxRatio, maxDistance,
+                            counts_out);
+  if (r < 0) return r;
+  bool any = false;
+  for (int p = 0; p < numJobs; p++) {
+    counts_out[p] = 0;
+    if (stats_out)
+      for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = 0;
+    any |= sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0;
+  }
+  if (!any) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  std::vector<GuidedBatchOut> out((size_t)numJobs, GuidedBatchOut{nullptr, nullptr});
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return guided_batch_enqueue(*c, sets, jobs, numJobs, models, models_in, thresh, maxRatio, maxDistance,
+                                     crossCheck != 0, out.data());
+       })) < 0)
+    return r;
+  for (int p = 0; p < numJobs; p++) {
+    if (!out[p].total) continue;                                          // an empty job
+    counts_out[p] = (int)*out[p].total;
+    if (stats_out)
+      for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = out[p].stats[k];
   }
   return 0;
 }

@@ -243,8 +243,11 @@ struct DeviceCtx {
   GrowBuffer knnPartials;     // cs_match_knn2, cs_match_ratio(_host): the slices of the exact scan
   GrowBuffer verify;          // cs_verify_pairs(_host, _batch), cs_verify_models, cs_verify_essential(_host, _models, _batch)
   GrowBuffer rank;            // cs_rank_records: counters, scratch
-  // cs_match_knn2_guided, cs_match_guided(_host): coefficient records, cell grids and the sorted candidate copies
+  // cs_match_knn2_guided, cs_match_guided(_host, _batch): coefficient records, cell grids and the sorted candidate
+  // copies; a batch wave's tables, headers, knn lists and pair scratch as well
   GrowBuffer guided;
+  void *h_guidedBatch = nullptr;           // pinned: every cs_match_guided_batch wave's tables and copied-back state
+  size_t h_guidedBatchBytes = 0;
   // the tensor path (match_tc.cu) of cs_match(_host), cs_match_mutual(_host), cs_match_knn2, cs_match_ratio(_host):
   // operand tiles, B-role copies, row norms, top-3 tables, fallback rows, and 2 x 16 words of flags used alternately
   GrowBuffer tcA, tcB, tcNorms, tcTables, tcRows, tcFlags;
@@ -402,6 +405,21 @@ GuidedModel guided_model(int model, const double in[9], float thresh);
 // set 2's rows in set 1.  Uses c.guided; the statistics reach c.h_guidedStats by the caller's synchronize.
 int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const GuidedModel &gm,
                       int *idx1, float *score1, int *idx2, float *score2);
+// Batched guided matching (cs_match_guided_batch, whose header comment states the wave rule).  A job's wave scratch:
+// its index, knn lists and pair scratch (every piece rounded up to 256 bytes) and GD_JOB_STATE_BYTES for its header and
+// pair total.
+#define GD_WAVE_BYTES ((size_t)256 << 20)
+#define GD_JOB_STATE_BYTES 256
+size_t guided_job_bytes(int n1, int n2, bool cross);
+// Where job p's results land in pinned memory after the call's synchronize (null for an empty job).
+struct GuidedBatchOut {
+  const unsigned int *total;
+  const unsigned long long *stats;
+};
+// Every non-empty job of a batch (argument-checked) in waves on c.stream, without a synchronize.
+int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs,
+                         const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
+                         bool cross, GuidedBatchOut *out);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id launch_verify uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

@@ -19,8 +19,16 @@
 //               top two.  The order is total, so the atomic order inside a cell does not matter.
 // A row for which the bounds do not hold (coordinates beyond 1e12, |pw| < 1e-12, an extreme threshold) scans every
 // candidate: that is correct, only slower.
+//
+// Batches (cs_match_guided_batch): every kernel takes one entry by value (a single call) or, instantiated with TABLE,
+// a device table of entries in which a CTA finds its own by its index (table_find over CTA bases the host summed).
+// Each job has its own slice of everything, so a row's result depends only on its job: see DESIGN.md section 4.
+// TABLE is a template argument, not a null test, so that the single call's kernels keep reading their entry from the
+// parameter bank instead of holding it in registers.
+#include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <vector>
 
 #include "common.cuh"
 
@@ -55,7 +63,26 @@ struct GGrid {
   int gx, gy;
 };
 
-// One direction of a call, as the knn kernel sees it.
+// One call or batch job as prep, hist, scan and scatter see it: its sets, model and header, its points, cell/slot
+// array, cell counts (cap0 / cap1 cells at most per direction), exclusive starts and sorted candidate copies per
+// direction (0: set 2's candidates, 1: set 1's, built when dirs == 2).  In a batch table job q owns the point CTAs
+// (ceil((n1 + n2) / 256)) from cta0 on and the scan CTAs (2 * dirs) from scan0 on.
+struct GJob {
+  const SiftPoint *s1, *s2;
+  int n1, n2, dirs, cap0, cap1;
+  GuidedModel gm;
+  GHdr *h;
+  GPoint *pts;
+  int2 *cellSlot;
+  unsigned int *counts0, *counts1;
+  unsigned int *start0C, *start0R, *start1C, *start1R;
+  float4 *coef0C, *coef0R, *coef1C, *coef1R;
+  int *idx0C, *idx0R, *idx1C, *idx1R;
+  int cta0, scan0;
+};
+
+// One direction of a call or batch job, as the knn kernel sees it.  In a batch table the entry owns the CTAs
+// (ceil(nRows / GD_WARPS)) from cta0 on.
 struct GDir {
   const SiftPoint *rowSift, *candSift;
   const GPoint *rowPts;
@@ -65,7 +92,22 @@ struct GDir {
   const unsigned int *startC, *startR;   // [cells + 1]
   int2 *idx;
   float2 *score;
+  GuidedModel gm;
+  GHdr *h;                      // the job's header; the statistics are summed into h->stats
+  int cull;                     // the threshold allows the culling bounds
+  int cta0;
 };
+
+// The entry of this CTA and the CTA's index within it (blk): `one` in a single call, else the table's entry whose CTA
+// range (from its `start` field on) holds blockIdx.x.
+template <bool TABLE, class T>
+__device__ __forceinline__ T gd_entry(const T &one, const T *__restrict__ tab, int n, int T::*start, int &blk)
+{
+  if (!TABLE) { blk = blockIdx.x; return one; }
+  const T e = tab[table_find(tab, n, start, (int)blockIdx.x)];
+  blk = (int)blockIdx.x - e.*start;
+  return e;
+}
 
 // float -> unsigned key with the order of the floats (finite values only)
 __device__ __forceinline__ unsigned int fkey(float f)
@@ -129,14 +171,25 @@ __device__ __forceinline__ int cell_of(float p, float p0, float inv, int g)
 }
 
 // ---- 1. prep ------------------------------------------------------------------------------------------------------
+// The CTAs of a point-parallel kernel in a call (the grid) or a batch job (one per 256 points).
+template <bool TABLE>
+__device__ __forceinline__ int gd_point_ctas(int n) { return TABLE ? (n + 255) >> 8 : (int)gridDim.x; }
+
+template <bool TABLE>
 __global__ void __launch_bounds__(256)
-guided_prep_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__restrict__ s2, int n2, GuidedModel gm,
-                   int dirs, GPoint *__restrict__ pts, GHdr *__restrict__ h)
+guided_prep_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
 {
+  int blk;
+  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::cta0, blk);
+  const SiftPoint *__restrict__ s1 = jb.s1, *__restrict__ s2 = jb.s2;
+  const int n1 = jb.n1, dirs = jb.dirs;
+  const GuidedModel &gm = jb.gm;
+  GPoint *__restrict__ pts = jb.pts;
+  GHdr *__restrict__ h = jb.h;
   const float *f = gm.f;
   const float nan = __int_as_float(0x7fffffff);
-  const int n = n1 + n2, lane = threadIdx.x & 31;
-  for (int base = blockIdx.x * blockDim.x; base < n; base += gridDim.x * blockDim.x) {
+  const int n = n1 + jb.n2, lane = threadIdx.x & 31;
+  for (int base = blk * blockDim.x; base < n; base += gd_point_ctas<TABLE>(n) * blockDim.x) {
     const int t = base + threadIdx.x;
     bool indexed = false, safe = true;
     float maxA = 0.0f, maxB = 0.0f;
@@ -206,14 +259,21 @@ guided_prep_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__
 
 // ---- 2. index -----------------------------------------------------------------------------------------------------
 // Per indexed point: its cell (cx * gy + cy) and its slot inside the cell.
+template <bool TABLE>
 __global__ void __launch_bounds__(256)
-guided_hist_kernel(const GPoint *__restrict__ pts, int n1, int n, const GHdr *__restrict__ h, unsigned int *counts0,
-                   unsigned int *counts1, int cap0, int cap1, int2 *__restrict__ cellSlot)
+guided_hist_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
 {
   __shared__ GGrid sg[2];
-  if (threadIdx.x < 2) sg[threadIdx.x] = grid_of(*h, threadIdx.x, threadIdx.x ? cap1 : cap0);
+  int blk;
+  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::cta0, blk);
+  const GPoint *__restrict__ pts = jb.pts;
+  const GHdr *__restrict__ h = jb.h;
+  unsigned int *counts0 = jb.counts0, *counts1 = jb.counts1;
+  int2 *__restrict__ cellSlot = jb.cellSlot;
+  const int n1 = jb.n1, n = n1 + jb.n2;
+  if (threadIdx.x < 2) sg[threadIdx.x] = grid_of(*h, threadIdx.x, threadIdx.x ? jb.cap1 : jb.cap0);
   __syncthreads();
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+  for (int t = blk * blockDim.x + threadIdx.x; t < n; t += gd_point_ctas<TABLE>(n) * blockDim.x) {
     const float2 k = pts[t].key;
     if (isnan(k.x)) { cellSlot[t] = make_int2(-1, 0); continue; }
     const int d = t < n1 ? 1 : 0;
@@ -225,15 +285,17 @@ guided_hist_kernel(const GPoint *__restrict__ pts, int n1, int n, const GHdr *__
 
 // Exclusive scans of the cell counts: CTA 2 * dir + order, order 0 column-major (cell cx * gy + cy), order 1
 // row-major (cy * gx + cx).  start[cells] = the count.
+template <bool TABLE>
 __global__ void __launch_bounds__(1024)
-guided_scan_kernel(const GHdr *__restrict__ h, const unsigned int *counts0, const unsigned int *counts1, int cap0,
-                   int cap1, unsigned int *start0C, unsigned int *start0R, unsigned int *start1C, unsigned int *start1R)
+guided_scan_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
 {
   __shared__ unsigned int s_w[32];
-  const int dir = blockIdx.x >> 1, order = blockIdx.x & 1;
-  const GGrid g = grid_of(*h, dir, dir ? cap1 : cap0);
-  const unsigned int *cnt = dir ? counts1 : counts0;
-  unsigned int *out = dir ? (order ? start1R : start1C) : (order ? start0R : start0C);
+  int blk;
+  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::scan0, blk);
+  const int dir = blk >> 1, order = blk & 1;
+  const GGrid g = grid_of(*jb.h, dir, dir ? jb.cap1 : jb.cap0);
+  const unsigned int *cnt = dir ? jb.counts1 : jb.counts0;
+  unsigned int *out = dir ? (order ? jb.start1R : jb.start1C) : (order ? jb.start0R : jb.start0C);
   const int cells = g.gx * g.gy, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   unsigned int carry = 0;
   for (int e0 = 0; e0 < cells; e0 += 1024) {
@@ -270,29 +332,32 @@ guided_scan_kernel(const GHdr *__restrict__ h, const unsigned int *counts0, cons
   if (threadIdx.x == 0) out[cells] = carry;
 }
 
+template <bool TABLE>
 __global__ void __launch_bounds__(256)
-guided_scatter_kernel(const GPoint *__restrict__ pts, int n1, int n, const GHdr *__restrict__ h,
-                      const int2 *__restrict__ cellSlot, int cap0, int cap1, const unsigned int *start0C,
-                      const unsigned int *start0R, const unsigned int *start1C, const unsigned int *start1R,
-                      float4 *coef0C, int *idx0C, float4 *coef0R, int *idx0R, float4 *coef1C, int *idx1C,
-                      float4 *coef1R, int *idx1R)
+guided_scatter_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
 {
   __shared__ int sgx[2], sgy[2];
+  int blk;
+  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::cta0, blk);
+  const GPoint *__restrict__ pts = jb.pts;
+  const int2 *__restrict__ cellSlot = jb.cellSlot;
+  const int n1 = jb.n1, n = n1 + jb.n2;
   if (threadIdx.x < 2) {
-    const GGrid g = grid_of(*h, threadIdx.x, threadIdx.x ? cap1 : cap0);
+    const GGrid g = grid_of(*jb.h, threadIdx.x, threadIdx.x ? jb.cap1 : jb.cap0);
     sgx[threadIdx.x] = g.gx; sgy[threadIdx.x] = g.gy;
   }
   __syncthreads();
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+  for (int t = blk * blockDim.x + threadIdx.x; t < n; t += gd_point_ctas<TABLE>(n) * blockDim.x) {
     const int2 cl = cellSlot[t];
     if (cl.x < 0) continue;
     const int d = t < n1 ? 1 : 0, gx = sgx[d], gy = sgy[d];
     const int cx = cl.x / gy, cy = cl.x - cx * gy;
-    const unsigned int pc = (d ? start1C : start0C)[cl.x] + cl.y, pr = (d ? start1R : start0R)[cy * gx + cx] + cl.y;
+    const unsigned int pc = (d ? jb.start1C : jb.start0C)[cl.x] + cl.y;
+    const unsigned int pr = (d ? jb.start1R : jb.start0R)[cy * gx + cx] + cl.y;
     const float4 c = pts[t].coef;
     const int i = d ? t : t - n1;
-    (d ? coef1C : coef0C)[pc] = c; (d ? idx1C : idx0C)[pc] = i;
-    (d ? coef1R : coef0R)[pr] = c; (d ? idx1R : idx0R)[pr] = i;
+    (d ? jb.coef1C : jb.coef0C)[pc] = c; (d ? jb.idx1C : jb.idx0C)[pc] = i;
+    (d ? jb.coef1R : jb.coef0R)[pr] = c; (d ? jb.idx1R : jb.idx0R)[pr] = i;
   }
 }
 
@@ -390,19 +455,23 @@ __device__ __forceinline__ bool strip_cells(int k, int n, float a0, float a1, fl
   return true;
 }
 
-__global__ void __launch_bounds__(GD_WARPS * 32)
-guided_knn_kernel(GDir d, GuidedModel gm, const GHdr *__restrict__ h, bool cull, unsigned long long *stats)
+// The rows of direction d that CTA blk of ctas runs (a call grid-strides, a batch gives every direction one CTA per
+// GD_WARPS rows).  d is the kernel's parameter or the table's entry in global memory, read in place: a copy would
+// index gm.f from local memory.
+__device__ __forceinline__ void guided_knn_rows(const GDir &d, int blk, int ctas)
 {
   __shared__ float4 s_row[GD_WARPS][32];
   __shared__ int s_q[GD_WARPS][64];
+  const GuidedModel &gm = d.gm;
+  const GHdr *__restrict__ h = d.h;
   const unsigned int FULL = 0xffffffffu;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const GGrid g = grid_of(*h, d.dir, d.capCells);
   const unsigned int nc = h->count[d.dir];
-  cull = cull && !h->unsafe[d.dir];
+  const bool cull = d.cull && !h->unsafe[d.dir];
   const double kmax = __uint_as_float(d.dir == 0 ? h->maxB : h->maxA);
   unsigned long long evals = 0, hits = 0, rowsHit = 0;
-  for (int r = blockIdx.x * GD_WARPS + w; r < d.nRows; r += gridDim.x * GD_WARPS) {
+  for (int r = blk * GD_WARPS + w; r < d.nRows; r += ctas * GD_WARPS) {
     const GPoint rp = d.rowPts[r];
     Top2 t;
     top2_init(t);
@@ -498,10 +567,22 @@ guided_knn_kernel(GDir d, GuidedModel gm, const GHdr *__restrict__ h, bool cull,
     }
   }
   if (lane == 0 && (evals || rowsHit)) {
-    atomicAdd(&stats[0], evals);
-    atomicAdd(&stats[1], hits);
-    atomicAdd(&stats[2 + d.dir], rowsHit);
+    atomicAdd(&d.h->stats[0], evals);
+    atomicAdd(&d.h->stats[1], hits);
+    atomicAdd(&d.h->stats[2 + d.dir], rowsHit);
   }
+}
+
+template <bool TABLE>
+__global__ void __launch_bounds__(GD_WARPS * 32)
+guided_knn_kernel(const GDir one, const GDir *__restrict__ dirs, int numDirs)
+{
+  if (!TABLE) {
+    guided_knn_rows(one, blockIdx.x, gridDim.x);
+    return;
+  }
+  const GDir &d = dirs[table_find(dirs, numDirs, &GDir::cta0, (int)blockIdx.x)];
+  guided_knn_rows(d, (int)blockIdx.x - d.cta0, (d.nRows + GD_WARPS - 1) / GD_WARPS);
 }
 
 // ---- host -----------------------------------------------------------------------------------------------------------
@@ -520,66 +601,110 @@ GuidedModel guided_model(int model, const double in[9], float thresh)
 // Bytes of a, rounded up to 256.
 static size_t gd_align(size_t a) { return (a + 255) & ~(size_t)255; }
 
+// The scratch of one call or batch job (its header aside), every piece 256-byte aligned: the cell counts, zeroed before
+// the call (offsets from the zeroed base), then the rest (offsets from the other base).  own: a batch job, which also
+// holds its knn lists and pair scratch; a single call uses the context's knnLists and pairScratch.
+struct GLayout {
+  int cap0, cap1;
+  size_t cnt0, cnt1, zeroBytes;
+  size_t pts, cell, s0C, s0R, s1C, s1R, c0C, i0C, c0R, i0R, c1C, i1C, c1R, i1R;
+  size_t idx1, sc1, idx2, sc2, masks, ctaCounts, bytes;
+};
+static GLayout gd_layout(int n1, int n2, int dirs, bool own)
+{
+  GLayout L;
+  const size_t n = (size_t)n1 + n2, m1 = dirs == 2 ? n1 : 1;
+  L.cap0 = 2 * n2 + 64;
+  L.cap1 = dirs == 2 ? 2 * n1 + 64 : 1;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { const size_t o = off; off += gd_align(bytes); return o; };
+  L.cnt0 = take(4 * (size_t)L.cap0); L.cnt1 = take(4 * (size_t)L.cap1);
+  L.zeroBytes = off;
+  off = 0;
+  L.pts = take(sizeof(GPoint) * n); L.cell = take(sizeof(int2) * n);
+  L.s0C = take(4 * ((size_t)L.cap0 + 1)); L.s0R = take(4 * ((size_t)L.cap0 + 1));
+  L.s1C = take(4 * ((size_t)L.cap1 + 1)); L.s1R = take(4 * ((size_t)L.cap1 + 1));
+  L.c0C = take(16 * (size_t)n2); L.i0C = take(4 * (size_t)n2); L.c0R = take(16 * (size_t)n2); L.i0R = take(4 * (size_t)n2);
+  L.c1C = take(16 * m1); L.i1C = take(4 * m1); L.c1R = take(16 * m1); L.i1R = take(4 * m1);
+  const size_t l2 = own && dirs == 2 ? (size_t)n2 : 0;
+  L.idx1 = take(own ? 8 * (size_t)n1 : 0); L.sc1 = take(own ? 8 * (size_t)n1 : 0);
+  L.idx2 = take(8 * l2); L.sc2 = take(8 * l2);
+  // the flags / write kernels' ballot words and counts of 1024-row CTAs (match_mutual.cu)
+  L.masks = take(own ? 4 * (size_t)idivup(n1, 32) : 0); L.ctaCounts = take(own ? 4 * (size_t)idivup(n1, 1024) : 0);
+  L.bytes = off;
+  return L;
+}
+
+// The entry of a call or job: header h, cell counts from z, the rest from b.
+static GJob gd_job(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int dirs, const GuidedModel &gm, GHdr *h,
+                   char *z, char *b, const GLayout &L)
+{
+  GJob j = {};
+  j.s1 = s1; j.n1 = n1; j.s2 = s2; j.n2 = n2; j.dirs = dirs; j.cap0 = L.cap0; j.cap1 = L.cap1;
+  j.gm = gm; j.h = h;
+  j.counts0 = reinterpret_cast<unsigned int *>(z + L.cnt0); j.counts1 = reinterpret_cast<unsigned int *>(z + L.cnt1);
+  auto u32 = [&](size_t o) { return reinterpret_cast<unsigned int *>(b + o); };
+  auto f4 = [&](size_t o) { return reinterpret_cast<float4 *>(b + o); };
+  auto i32 = [&](size_t o) { return reinterpret_cast<int *>(b + o); };
+  j.pts = reinterpret_cast<GPoint *>(b + L.pts); j.cellSlot = reinterpret_cast<int2 *>(b + L.cell);
+  j.start0C = u32(L.s0C); j.start0R = u32(L.s0R); j.start1C = u32(L.s1C); j.start1R = u32(L.s1R);
+  j.coef0C = f4(L.c0C); j.idx0C = i32(L.i0C); j.coef0R = f4(L.c0R); j.idx0R = i32(L.i0R);
+  j.coef1C = f4(L.c1C); j.idx1C = i32(L.i1C); j.coef1R = f4(L.c1R); j.idx1R = i32(L.i1R);
+  return j;
+}
+
+// Direction dir of a call or job (0: set 1's rows against set 2, 1: the reverse), its lists at idx / score.
+static GDir gd_dir(const GJob &j, int dir, int2 *idx, float2 *score, int cta0)
+{
+  GDir d;
+  d.dir = dir;
+  d.rowSift = dir ? j.s2 : j.s1;
+  d.candSift = dir ? j.s1 : j.s2;
+  d.rowPts = dir ? j.pts + j.n1 : j.pts;
+  d.nRows = dir ? j.n2 : j.n1;
+  d.capCells = dir ? j.cap1 : j.cap0;
+  d.coefC = dir ? j.coef1C : j.coef0C; d.idxC = dir ? j.idx1C : j.idx0C;
+  d.coefR = dir ? j.coef1R : j.coef0R; d.idxR = dir ? j.idx1R : j.idx0R;
+  d.startC = dir ? j.start1C : j.start0C; d.startR = dir ? j.start1R : j.start0R;
+  d.idx = idx; d.score = score;
+  d.gm = j.gm; d.h = j.h;
+  // the bounds of DESIGN.md section 4 hold for thresholds whose square is a normal float well inside the range
+  d.cull = j.gm.t2 >= 1e-6f && j.gm.t2 <= 1e12f;
+  d.cta0 = cta0;
+  return d;
+}
+
 int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const GuidedModel &gm,
                       int *idx1, float *score1, int *idx2, float *score2)
 {
   const int dirs = idx2 ? 2 : 1, n = n1 + n2;
-  const int cap0 = 2 * n2 + 64, cap1 = dirs == 2 ? 2 * n1 + 64 : 1;
   // layout: header and cell counts first (one memset), then the rest
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += gd_align(bytes); return o; };
-  const size_t oHdr = take(sizeof(GHdr)), oCnt0 = take(4 * (size_t)cap0), oCnt1 = take(4 * (size_t)cap1);
-  const size_t zeroBytes = off;
-  const size_t oPts = take(sizeof(GPoint) * (size_t)n), oCell = take(sizeof(int2) * (size_t)n);
-  const size_t oS0C = take(4 * ((size_t)cap0 + 1)), oS0R = take(4 * ((size_t)cap0 + 1));
-  const size_t oS1C = take(4 * ((size_t)cap1 + 1)), oS1R = take(4 * ((size_t)cap1 + 1));
-  const size_t oC0C = take(16 * (size_t)n2), oI0C = take(4 * (size_t)n2), oC0R = take(16 * (size_t)n2),
-               oI0R = take(4 * (size_t)n2);
-  const size_t m1 = dirs == 2 ? n1 : 1;
-  const size_t oC1C = take(16 * m1), oI1C = take(4 * m1), oC1R = take(16 * m1), oI1R = take(4 * m1);
+  const GLayout L = gd_layout(n1, n2, dirs, false);
+  const size_t zeroBytes = gd_align(sizeof(GHdr)) + L.zeroBytes;
   int r;
-  if ((r = c.guided.grow(off)) < 0) return r;
+  if ((r = c.guided.grow(zeroBytes + L.bytes)) < 0) return r;
   if (!c.h_guidedStats) CS_CUDA(cudaMallocHost((void **)&c.h_guidedStats, 4 * sizeof(unsigned long long)));
   char *b = c.guided.as<char>();
-  GHdr *h = reinterpret_cast<GHdr *>(b + oHdr);
-  unsigned int *cnt0 = reinterpret_cast<unsigned int *>(b + oCnt0), *cnt1 = reinterpret_cast<unsigned int *>(b + oCnt1);
-  GPoint *pts = reinterpret_cast<GPoint *>(b + oPts);
-  int2 *cell = reinterpret_cast<int2 *>(b + oCell);
-  auto u32 = [&](size_t o) { return reinterpret_cast<unsigned int *>(b + o); };
-  auto f4 = [&](size_t o) { return reinterpret_cast<float4 *>(b + o); };
-  auto i32 = [&](size_t o) { return reinterpret_cast<int *>(b + o); };
+  GHdr *h = reinterpret_cast<GHdr *>(b);
+  const GJob j = gd_job(s1, n1, s2, n2, dirs, gm, h, b + gd_align(sizeof(GHdr)), b + zeroBytes, L);
   cudaStream_t st = c.stream;
   cudaEvent_t *tev = match_timing_events();
   if (tev) cudaEventRecord(tev[0], st);
   CS_CUDA(cudaMemsetAsync(b, 0, zeroBytes, st));
   const int blocks = idivup(n, 256) < 4 * c.sms ? idivup(n, 256) : 4 * c.sms;
-  guided_prep_kernel<<<blocks, 256, 0, st>>>(s1, n1, s2, n2, gm, dirs, pts, h);
+  guided_prep_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
   if (tev) cudaEventRecord(tev[1], st);
-  guided_hist_kernel<<<blocks, 256, 0, st>>>(pts, n1, n, h, cnt0, cnt1, cap0, cap1, cell);
-  guided_scan_kernel<<<2 * dirs, 1024, 0, st>>>(h, cnt0, cnt1, cap0, cap1, u32(oS0C), u32(oS0R), u32(oS1C), u32(oS1R));
-  guided_scatter_kernel<<<blocks, 256, 0, st>>>(pts, n1, n, h, cell, cap0, cap1, u32(oS0C), u32(oS0R), u32(oS1C),
-                                                u32(oS1R), f4(oC0C), i32(oI0C), f4(oC0R), i32(oI0R), f4(oC1C),
-                                                i32(oI1C), f4(oC1R), i32(oI1R));
+  guided_hist_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
+  guided_scan_kernel<false><<<2 * dirs, 1024, 0, st>>>(j, nullptr, 0);
+  guided_scatter_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
   count_launch(4);
   CS_CUDA(cudaGetLastError());
   if (tev) cudaEventRecord(tev[2], st);
-  // the bounds of DESIGN.md section 4 hold for thresholds whose square is a normal float well inside the range
-  const bool cull = gm.t2 >= 1e-6f && gm.t2 <= 1e12f;
   for (int dir = 0; dir < dirs; dir++) {
-    GDir d;
-    d.dir = dir;
-    d.rowSift = dir ? s2 : s1;
-    d.candSift = dir ? s1 : s2;
-    d.rowPts = dir ? pts + n1 : pts;
-    d.nRows = dir ? n2 : n1;
-    d.capCells = dir ? cap1 : cap0;
-    d.coefC = f4(dir ? oC1C : oC0C); d.idxC = i32(dir ? oI1C : oI0C);
-    d.coefR = f4(dir ? oC1R : oC0R); d.idxR = i32(dir ? oI1R : oI0R);
-    d.startC = u32(dir ? oS1C : oS0C); d.startR = u32(dir ? oS1R : oS0R);
-    d.idx = reinterpret_cast<int2 *>(dir ? idx2 : idx1);
-    d.score = reinterpret_cast<float2 *>(dir ? score2 : score1);
+    const GDir d = gd_dir(j, dir, reinterpret_cast<int2 *>(dir ? idx2 : idx1),
+                          reinterpret_cast<float2 *>(dir ? score2 : score1), 0);
     const int rowBlocks = idivup(d.nRows, GD_WARPS) < 16 * c.sms ? idivup(d.nRows, GD_WARPS) : 16 * c.sms;
-    guided_knn_kernel<<<rowBlocks, GD_WARPS * 32, 0, st>>>(d, gm, h, cull, h->stats);
+    guided_knn_kernel<false><<<rowBlocks, GD_WARPS * 32, 0, st>>>(d, nullptr, 0);
     count_launch();
     CS_CUDA(cudaGetLastError());
     if (tev) cudaEventRecord(tev[3 + dir], st);
@@ -595,6 +720,150 @@ int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint
       fprintf(stderr, " %s %.1f", names[i], 1000.0f * ms);
     }
     fprintf(stderr, "\n");
+  }
+  return 0;
+}
+
+// ---- batches --------------------------------------------------------------------------------------------------------
+size_t guided_job_bytes(int n1, int n2, bool cross)
+{
+  const GLayout L = gd_layout(n1, n2, cross ? 2 : 1, true);
+  return L.zeroBytes + L.bytes + GD_JOB_STATE_BYTES;
+}
+
+static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+// A wave (the header states the rule): the non-empty jobs ne[q0, q1) and what its launches need.  Device scratch
+// (c.guided): the tables; then, zeroed per wave, the headers and pair totals (copied back) and every job's cell
+// counts; then the rest of every job.  Pinned (c.h_guidedBatch from pinOff): the tables, then the copied-back state.
+struct GdWave {
+  int q0 = 0, q1 = 0, pointCtas = 0, knnCtas = 0, pairCtas = 0, dirs = 0;
+  size_t bytes = 0, tabBytes = 0, stateBytes = 0, zeroBytes = 0, restBytes = 0, pinOff = 0;
+};
+
+int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs,
+                         const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
+                         bool cross, GuidedBatchOut *out)
+{
+  const int D = cross ? 2 : 1;
+  std::vector<int> ne;
+  for (int p = 0; p < numJobs; p++)
+    if (sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0) ne.push_back(p);
+  if (ne.empty()) return 0;
+  std::vector<GdWave> waves;
+  size_t dev = 0, pin = 0;
+  for (int q = 0; q < (int)ne.size(); q++) {
+    const cs_match_job &jb = jobs[ne[q]];
+    const int n1 = sets[jb.set1].n, n2 = sets[jb.set2].n;
+    const size_t cost = guided_job_bytes(n1, n2, cross);
+    if (waves.empty() || waves.back().bytes + cost > GD_WAVE_BYTES) {
+      waves.emplace_back();
+      waves.back().q0 = q;
+    }
+    GdWave &v = waves.back();
+    const GLayout L = gd_layout(n1, n2, D, true);
+    v.q1 = q + 1;
+    v.bytes += cost;
+    v.zeroBytes += L.zeroBytes;
+    v.restBytes += L.bytes;
+    v.pointCtas += idivup(n1 + n2, 256);
+    v.knnCtas += idivup(n1, GD_WARPS) + (cross ? idivup(n2, GD_WARPS) : 0);
+    v.pairCtas += idivup(n1, 1024);
+  }
+  for (GdWave &v : waves) {
+    const size_t J = v.q1 - v.q0;
+    v.dirs = (int)J * D;
+    v.tabBytes = align16(J * sizeof(GJob)) + align16(v.dirs * sizeof(GDir)) + align16(J * sizeof(PairJob));
+    v.stateBytes = align16(J * sizeof(GHdr)) + align16(J * sizeof(unsigned int));
+    v.pinOff = pin;
+    pin += v.tabBytes + v.stateBytes;
+    dev = std::max(dev, gd_align(v.tabBytes) + gd_align(v.stateBytes) + v.zeroBytes + v.restBytes);
+  }
+  int r;
+  if ((r = c.guided.grow(dev)) < 0) return r;
+  if (c.h_guidedBatchBytes < pin) {          // every batch call ends in a synchronize: no copy is pending here
+    if (c.h_guidedBatch) cudaFreeHost(c.h_guidedBatch);
+    c.h_guidedBatch = nullptr;
+    c.h_guidedBatchBytes = 0;
+    CS_CUDA(cudaMallocHost(&c.h_guidedBatch, pin));
+    c.h_guidedBatchBytes = pin;
+  }
+  const cudaStream_t st = c.stream;
+  cudaEvent_t *tev = match_timing_events();
+  for (const GdWave &v : waves) {
+    const int J = v.q1 - v.q0;
+    char *hp = static_cast<char *>(c.h_guidedBatch) + v.pinOff;
+    GJob *hj = reinterpret_cast<GJob *>(hp);
+    GDir *hd = reinterpret_cast<GDir *>(hp + align16(J * sizeof(GJob)));
+    PairJob *hpj = reinterpret_cast<PairJob *>(hp + align16(J * sizeof(GJob)) + align16(v.dirs * sizeof(GDir)));
+    const char *hstate = hp + v.tabBytes;
+    char *dt = c.guided.as<char>(), *ds = dt + gd_align(v.tabBytes);
+    GHdr *hdrs = reinterpret_cast<GHdr *>(ds);
+    unsigned int *totals = reinterpret_cast<unsigned int *>(ds + align16(J * sizeof(GHdr)));
+    char *z = ds + gd_align(v.stateBytes), *b = z + v.zeroBytes;
+    int pointCta = 0, knnCta = 0, pairCta = 0;
+    for (int k = 0; k < J; k++) {
+      const int p = ne[v.q0 + k];
+      const cs_match_job &jb = jobs[p];
+      const int n1 = sets[jb.set1].n, n2 = sets[jb.set2].n;
+      const GLayout L = gd_layout(n1, n2, D, true);
+      GJob &j = hj[k];
+      j = gd_job(static_cast<const SiftPoint *>(sets[jb.set1].pts), n1, static_cast<const SiftPoint *>(sets[jb.set2].pts),
+                 n2, D, guided_model(models[p], models_in + 9 * (size_t)p, thresh), hdrs + k, z, b, L);
+      j.cta0 = pointCta; j.scan0 = 2 * D * k;
+      pointCta += idivup(n1 + n2, 256);
+      int2 *idx1 = reinterpret_cast<int2 *>(b + L.idx1), *idx2 = cross ? reinterpret_cast<int2 *>(b + L.idx2) : nullptr;
+      float2 *sc1 = reinterpret_cast<float2 *>(b + L.sc1), *sc2 = cross ? reinterpret_cast<float2 *>(b + L.sc2) : nullptr;
+      for (int dir = 0; dir < D; dir++) {
+        hd[D * k + dir] = gd_dir(j, dir, dir ? idx2 : idx1, dir ? sc2 : sc1, knnCta);
+        knnCta += idivup(dir ? n2 : n1, GD_WARPS);
+      }
+      PairJob &pj = hpj[k];
+      pj = PairJob{};
+      pj.jv = reinterpret_cast<const int *>(idx1); pj.jstride = 2;
+      pj.n1 = n1; pj.n2 = n2;
+      pj.idx1 = idx1; pj.score1 = sc1; pj.idx2 = idx2; pj.score2 = sc2;
+      pj.masks = reinterpret_cast<unsigned int *>(b + L.masks);
+      pj.blockCounts = reinterpret_cast<unsigned int *>(b + L.ctaCounts);
+      pj.pairs = reinterpret_cast<int2 *>(jb.pairs); pj.maxPairs = jb.maxPairs;
+      pj.total = totals + k;
+      pj.cta0 = pairCta;
+      pairCta += idivup(n1, 1024);
+      out[p].stats = reinterpret_cast<const GHdr *>(hstate)[k].stats;
+      out[p].total = reinterpret_cast<const unsigned int *>(hstate + align16(J * sizeof(GHdr))) + k;
+      z += L.zeroBytes;
+      b += L.bytes;
+    }
+    const GJob *dj = reinterpret_cast<const GJob *>(dt);
+    const GDir *dd = reinterpret_cast<const GDir *>(dt + align16(J * sizeof(GJob)));
+    const PairJob *dpj = reinterpret_cast<const PairJob *>(dt + align16(J * sizeof(GJob)) + align16(v.dirs * sizeof(GDir)));
+    CS_CUDA(cudaMemsetAsync(ds, 0, gd_align(v.stateBytes) + v.zeroBytes, st));
+    CS_CUDA(cudaMemcpyAsync(dt, hp, v.tabBytes, cudaMemcpyHostToDevice, st));
+    if (tev) cudaEventRecord(tev[0], st);
+    guided_prep_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
+    if (tev) cudaEventRecord(tev[1], st);
+    guided_hist_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
+    guided_scan_kernel<true><<<2 * D * J, 1024, 0, st>>>(GJob{}, dj, J);
+    guided_scatter_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
+    if (tev) cudaEventRecord(tev[2], st);
+    guided_knn_kernel<true><<<v.knnCtas, GD_WARPS * 32, 0, st>>>(GDir{}, dd, v.dirs);
+    if (tev) cudaEventRecord(tev[3], st);
+    count_launch(5);
+    CS_CUDA(cudaGetLastError());
+    if ((r = launch_ratio_pairs_batch(c, dpj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
+    if (tev) cudaEventRecord(tev[4], st);
+    CS_CUDA(cudaMemcpyAsync(hp + v.tabBytes, ds, v.stateBytes, cudaMemcpyDeviceToHost, st));
+    if (tev) {
+      static const char *const names[] = {"prep", "index", "knn", "pairs"};
+      cudaEventSynchronize(tev[4]);
+      fprintf(stderr, "guided-batch timing %d jobs %d directions %d rows [us]:", J, v.dirs, 8 * v.knnCtas);
+      for (int i = 0; i < 4; i++) {
+        float ms = 0.0f;
+        cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
+        fprintf(stderr, " %s %.1f", names[i], 1000.0f * ms);
+      }
+      fprintf(stderr, "\n");
+    }
   }
   return 0;
 }

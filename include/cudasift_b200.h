@@ -359,6 +359,40 @@ int cs_match_guided_host(const void *h_s1, int n1, const void *h_s2, int n2, int
  * [2] rows of set 1 with at least one admissible candidate, [3] the same for set 2 in a cross-checked call, else 0 */
 int cs_match_guided_stats(unsigned long long out[4]);
 
+/* Batched guided matching: J independent jobs of cs_match_guided in one call, for example every verified image pair of
+ * a collection.  Sets and jobs are those of cs_match_ratio_batch; each job has its own model.  thresh, maxRatio,
+ * maxDistance and crossCheck are common to all jobs.
+ * - models[p]: CS_GEOM_HOMOGRAPHY or CS_GEOM_FUNDAMENTAL; models_in[p]: row-major 3x3 mapping set-1 pixels to set-2
+ *   pixels, laid out as cs_verify_pairs_batch's models_out, so that output can be passed in unchanged (for a calibrated
+ *   pair, the F of its essential matrix).
+ * - Equivalence: for job p with A = sets[set1] and B = sets[set2], counts_out[p] and the first min(count, maxPairs)
+ *   pairs equal, bit for bit, what cs_match_guided(A.pts, A.n, B.pts, B.n, models[p], models_in + 9 p, thresh,
+ *   maxRatio, maxDistance, crossCheck, pairs, maxPairs, ...) returns and writes, and stats_out[p] equals
+ *   cs_match_guided_stats() after that call.  Jobs do not interact: permuting the jobs permutes the results, and two
+ *   calls give the same bytes.
+ * - Sets are shared: any number of jobs may name a set, in either role, a set may be paired with itself and sets may
+ *   overlap each other.  A job with an empty set gets count 0 and zero statistics, and launches nothing.  numJobs == 0,
+ *   or only empty jobs, returns 0 before any CUDA call.
+ * - CS_E_ARG, before any CUDA call, naming the first offending jobs[p] or sets[s] in cs_last_error(): every rule of
+ *   cs_match_ratio_batch, NULL models or models_in with numJobs > 0, and per job every model rule of cs_match_guided
+ *   (a model outside {1, 2}, a non-finite or all-zero models_in[p] or one whose norm is not finite, thresh not finite
+ *   or <= 0).  A zero model is an error: leave out the jobs whose verification failed.
+ * - Waves: the non-empty jobs, in order, run in waves.  A wave is the longest run of consecutive non-empty jobs whose
+ *   scratch fits 256 MiB; it holds at least one job.  With c = crossCheck, m = c ? n1 : 1, cap0 = 2 n2 + 64 and
+ *   cap1 = c ? 2 n1 + 64 : 1, the scratch of a job of n1 x n2 rows is 256 bytes (header and pair total) plus these
+ *   pieces, each rounded up to a multiple of 256 bytes: 4 cap0 and 4 cap1 (cell counts), 32 (n1 + n2) (points),
+ *   8 (n1 + n2) (cells), 4 (cap0 + 1) twice and 4 (cap1 + 1) twice (cell starts), 16 n2, 4 n2, 16 n2, 4 n2, 16 m,
+ *   4 m, 16 m and 4 m (sorted candidate copies), 8 n1 twice and with c 8 n2 twice (knn lists), 4 ceil(n1 / 32) and
+ *   4 ceil(n1 / 1024) (pair scratch).
+ * - Launches: each wave issues 7 kernel launches, whatever its number of jobs and crossCheck (prep, histogram, scan,
+ *   scatter, knn over every direction of every job, ratio test, pair writes), so a batch issues 7 x waves
+ *   (cs_launch_count).  The call synchronises with the host once, at the end; its scratch lives in the per-device
+ *   context.  *ms (may be NULL) gets the event time of the call.  cs_match_guided_stats keeps describing single calls.
+ * models[J], models_in[J][9], counts_out[J]; stats_out[J][4] may be NULL.  Returns 0 or CS_E_*. */
+int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                          const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
+                          int crossCheck, int *counts_out, unsigned long long *stats_out, double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
