@@ -20,7 +20,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
-           "MatchSiftDataGuidedBatch"]
+           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -91,6 +91,7 @@ def lib():
         "cs_verify_essential_batch": (ip, [vp, ip, vp, vp, ip, fp, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_match_ratio_batch": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_match_guided_batch": (ip, [vp, ip, vp, ip, vp, vp, fp, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
+        "cs_build_tracks": (ip, [vp, ip, vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -714,6 +715,50 @@ def MatchSiftDataGuidedBatch(datas, jobs, model, Ms, thresh=4.0, maxRatio=0.8, m
                                            float(maxDistance), int(bool(crossCheck)), counts, stats, ms),
                "MatchSiftDataGuidedBatch")
     return _match_batch(datas, jobs, crossCheck, call)
+
+
+class TrackList(ctypes.Structure):
+    """cs_track_list: the device pair list of one image pair, for BuildTracks."""
+    _fields_ = [("image1", ctypes.c_int), ("image2", ctypes.c_int), ("pairs", ctypes.c_void_p),
+                ("numPairs", ctypes.c_int)]
+
+
+def BuildTracks(imageSizes, lists, minLength=2, dropConflicting=True):
+    """Feature tracks over many image pairs in one call (cs_build_tracks): imageSizes[a] is the feature count of image
+    a, lists a sequence of (a, b, pairs) with pairs int32 [k, 2] of {feature of a, feature of b}, for example
+    zip(jobs, pairs) from MatchSiftDataGuidedBatch or MatchSiftDataRatioBatch.  The lists go up in one device buffer;
+    the outputs are sized from the pair count (no track has fewer than minLength of the at most 2 k features the
+    pairs touch), so one call returns them whole.  Returns (offsets int32 [T + 1], members int32 [M, 2] of {image,
+    feature}, trackOf int32 [N], stats int64 [8] as the header describes them, ms)."""
+    sizes = np.ascontiguousarray(np.asarray(imageSizes, np.int64).reshape(-1).astype(np.int32))
+    parsed = [(int(a), int(b), _pair_array(p)) for a, b, p in lists]
+    counts = [len(p) for _, _, p in parsed]
+    offs = np.concatenate([[0], np.cumsum(counts, dtype=np.int64)]).astype(np.int64)
+    P, N = int(offs[-1]), int(sizes.sum(dtype=np.int64))
+    maxMembers = min(N, 2 * P)
+    maxTracks = maxMembers // max(int(minLength), 2)
+    table = (TrackList * max(len(parsed), 1))()
+    stats, ms = np.zeros(8, np.int64), ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(P, 1) * 8), DeviceBuffer(max(N, 1) * 4), DeviceBuffer((maxTracks + 1) * 4),
+            DeviceBuffer(max(maxMembers, 1) * 8)]
+    try:
+        if P:
+            bufs[0].upload(np.concatenate([p for _, _, p in parsed]))
+        for q, (a, b, p) in enumerate(parsed):
+            table[q] = TrackList(a, b, bufs[0].ptr + 8 * int(offs[q]) if counts[q] else None, counts[q])
+        T = _check(lib().cs_build_tracks(_ptr(sizes), len(sizes), ctypes.addressof(table) if parsed else None,
+                                         len(parsed), int(minLength), int(bool(dropConflicting)),
+                                         bufs[1].ptr if N else None, bufs[2].ptr, maxTracks,
+                                         bufs[3].ptr if maxMembers else None, maxMembers, _ptr(stats),
+                                         ctypes.byref(ms)), "BuildTracks")
+        M = int(stats[7])
+        offsets = bufs[2].download(np.int32, T + 1)
+        members = bufs[3].download(np.int32, 2 * M).reshape(M, 2) if M else np.zeros((0, 2), np.int32)
+        trackOf = bufs[1].download(np.int32, N) if N else np.zeros(0, np.int32)
+    finally:
+        for buf in bufs:
+            buf.free()
+    return offsets, members, trackOf, stats, ms.value
 
 
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):

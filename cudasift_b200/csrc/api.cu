@@ -763,6 +763,65 @@ static int guided_batch_args(const char *fn, const cs_match_set *sets, int numSe
   return 0;
 }
 
+// The arguments of cs_build_tracks: the counts and tables, every image (imageSizes[a]) and list (lists[p]), the
+// outputs, then the output buffers against each other and every pair list (overlap_sweep).  *N and *P receive the
+// feature and pair totals.
+static int tracks_args(const char *fn, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
+                       int minLength, const int *trackOf, const int *offsets, int maxTracks, const int *members,
+                       int maxMembers, int *N, int *P)
+{
+  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
+  if (numLists < 0 || numLists > (1 << 24)) return arg_error(fn, "numLists must be in [0, 2^24]");
+  if (numImages > 0 && !imageSizes) return arg_error(fn, "numImages > 0 needs an imageSizes array");
+  if (numLists > 0 && !lists) return arg_error(fn, "numLists > 0 needs a lists array");
+  char bad[128] = "";
+  long long n = 0, pairs = 0;
+  for (int a = 0; a < numImages && !bad[0]; a++) {
+    if (imageSizes[a] < 0) snprintf(bad, sizeof bad, "imageSizes[%d] must be >= 0", a);
+    else if ((n += imageSizes[a]) > INT_MAX) snprintf(bad, sizeof bad, "imageSizes[%d]: the sizes pass INT_MAX", a);
+  }
+  for (int p = 0; p < numLists && !bad[0]; p++) {
+    const cs_track_list &l = lists[p];
+    if (l.image1 < 0 || l.image1 >= numImages || l.image2 < 0 || l.image2 >= numImages)
+      snprintf(bad, sizeof bad, "lists[%d]: image1 and image2 must be in [0, numImages)", p);
+    else if (l.numPairs < 0) snprintf(bad, sizeof bad, "lists[%d]: numPairs must be >= 0", p);
+    else if (l.numPairs > 0 && !l.pairs) snprintf(bad, sizeof bad, "lists[%d]: numPairs > 0 needs a pairs buffer", p);
+    else if (l.numPairs > 0 && (reinterpret_cast<uintptr_t>(l.pairs) & 7) != 0)
+      snprintf(bad, sizeof bad, "lists[%d]: pairs must be 8-byte aligned", p);
+    else if ((pairs += l.numPairs) > INT_MAX) snprintf(bad, sizeof bad, "lists[%d]: the pair counts pass INT_MAX", p);
+  }
+  if (bad[0]) return arg_error(fn, bad);
+  if (minLength < 2) return arg_error(fn, "minLength must be >= 2");
+  if (maxTracks < 0 || maxMembers < 0) return arg_error(fn, "maxTracks and maxMembers must be >= 0");
+  if (maxTracks > 0 && !offsets) return arg_error(fn, "maxTracks > 0 needs d_offsets");
+  if (maxMembers > 0 && !members) return arg_error(fn, "maxMembers > 0 needs d_members");
+  if ((reinterpret_cast<uintptr_t>(trackOf) & 3) != 0 || (reinterpret_cast<uintptr_t>(offsets) & 3) != 0)
+    return arg_error(fn, "d_trackOf and d_offsets must be 4-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(members) & 7) != 0) return arg_error(fn, "d_members must be 8-byte aligned");
+  // the outputs (kind 0, written; owners 0 d_trackOf, 1 d_offsets, 2 d_members) against each other and every pair
+  // list (kind 1, read)
+  std::vector<SweepRange> rs;
+  rs.reserve((size_t)numLists + 3);
+  if (trackOf) sweep_add(rs, trackOf, (size_t)n * sizeof(int), 0, 0, true);
+  if (offsets) sweep_add(rs, offsets, ((size_t)maxTracks + 1) * sizeof(int), 1, 0, true);
+  sweep_add(rs, members, (size_t)maxMembers * sizeof(int2), 2, 0, true);
+  for (int p = 0; p < numLists; p++) sweep_add(rs, lists[p].pairs, (size_t)lists[p].numPairs * sizeof(int2), p, 1, false);
+  const int r = overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
+    static const char *const outs[3] = {"d_trackOf", "d_offsets", "d_members"};
+    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
+    const SweepRange &b = &a == &x ? y : x;
+    char msg[128], nb[32];
+    if (b.kind) snprintf(nb, sizeof nb, "lists[%d].pairs", b.owner);
+    else snprintf(nb, sizeof nb, "%s", outs[b.owner]);
+    snprintf(msg, sizeof msg, "%s and %s overlap (an output overlaps another range)", outs[a.owner], nb);
+    return arg_error(fn, msg);
+  });
+  if (r < 0) return r;
+  *N = (int)n;
+  *P = (int)pairs;
+  return 0;
+}
+
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
 {
   VerifyCalib cal;
@@ -1603,6 +1662,40 @@ int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_
       for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = out[p].stats[k];
   }
   return 0;
+}
+
+int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *lists, int numLists, int minLength,
+                    int dropConflicting, int *d_trackOf, int *d_offsets, int maxTracks, int *d_members, int maxMembers,
+                    long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_build_tracks";
+  if (ms) *ms = 0.0;
+  int N = 0, P = 0;
+  int r = tracks_args(fn, imageSizes, numImages, lists, numLists, minLength, d_trackOf, d_offsets, maxTracks, d_members,
+                      maxMembers, &N, &P);
+  if (r < 0) return r;
+  if (stats_out)
+    for (int k = 0; k < 8; k++) stats_out[k] = 0;
+  const bool fillTrackOf = d_trackOf && N > 0;
+  if (P == 0 && !fillTrackOf && !d_offsets) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if (P == 0) {                                                           // no pairs: no track, no launch
+    if (fillTrackOf) CS_CUDA(cudaMemsetAsync(d_trackOf, 0xff, (size_t)N * sizeof(int), c->stream));
+    if (d_offsets) CS_CUDA(cudaMemsetAsync(d_offsets, 0, sizeof(int), c->stream));
+    CS_CUDA(cudaStreamSynchronize(c->stream));
+    return 0;
+  }
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return tracks_enqueue(*c, imageSizes, numImages, lists, numLists, minLength, dropConflicting != 0, d_trackOf,
+                               d_offsets, maxTracks, d_members, maxMembers);
+       })) < 0)
+    return r;
+  const unsigned long long *st = static_cast<const unsigned long long *>(c->h_tracks);
+  if (stats_out)
+    for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
+  return (int)st[6];
 }
 
 // ---- stage-level entry points ----

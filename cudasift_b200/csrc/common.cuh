@@ -261,6 +261,10 @@ struct DeviceCtx {
   bool mbConfigured = false;               // the batch GEMM's shared-memory size is set
   void *h_mb = nullptr;                    // pinned: every wave's tables (uploaded) and state (copied back)
   size_t h_mbBytes = 0;
+  // cs_build_tracks: the statistics, image bases, list table, per-tile totals, per-feature arrays and sort storage
+  GrowBuffer tracks;
+  void *h_tracks = nullptr;                // pinned: the statistics (copied back), then the bases and list table
+  size_t h_tracksBytes = 0;
 
   // pinned host words
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
@@ -420,6 +424,12 @@ struct GuidedBatchOut {
 int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs,
                          const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
                          bool cross, GuidedBatchOut *out);
+
+// ---- feature tracks (tracks.cu) ---------------------------------------------------------------------------------
+// The kernels of cs_build_tracks (argument-checked, at least one pair in all) on c.stream, without a synchronize; the
+// eight statistics reach c.h_tracks (unsigned long long) by the caller's synchronize.
+int tracks_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
+                   int minLength, bool drop, int *trackOf, int *offsets, int maxTracks, int *members, int maxMembers);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id launch_verify uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

@@ -393,6 +393,61 @@ int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_
                           const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
                           int crossCheck, int *counts_out, unsigned long long *stats_out, double *ms);
 
+/* Feature tracks: the connected components of the features that the pair lists of many image pairs join, for example
+ * every job of cs_match_guided_batch or cs_match_ratio_batch, in one call (COLMAP's correspondence graph and track
+ * building; OpenMVG's tracks builder).  A list uses the pair convention of cs_match_job, so a batch job's buffer can be
+ * passed unchanged with numPairs = min(counts_out[p], maxPairs). */
+typedef struct cs_track_list {
+  int image1, image2;              /* indices into imageSizes */
+  const int *pairs; int numPairs;  /* device int pairs {i, j}, 8-byte aligned: feature i of image1 <-> feature j of image2 */
+} cs_track_list;
+/* - Features: feature f of image a is valid when 0 <= f < imageSizes[a]; its global id is g = imageSizes[0] + ... +
+ *   imageSizes[a - 1] + f, and N is the sum of all sizes.
+ * - Pairs: pair {i, j} of lists[p] is valid when i is a valid feature of image1 and j a valid feature of image2; it
+ *   joins (image1, i) and (image2, j).  An invalid pair is ignored and counted.  image1 == image2, repeated lists and
+ *   repeated pairs are allowed.
+ * - Components: a feature is matched when it is an endpoint of at least one valid pair; the components are the
+ *   connected components of the matched features.  A component conflicts when it holds two distinct features of the
+ *   same image.  It is a track when it has at least minLength features (minLength >= 2) and does not conflict, or
+ *   dropConflicting == 0.
+ * - Order, defined by value: tracks in ascending order of their smallest global id; the members of a track in
+ *   ascending global id, which is ascending (image, feature).  d_members receives int pairs {image, feature},
+ *   d_offsets[k] is the number of members before track k, d_trackOf[g] is the track index of feature g or -1.  The
+ *   output depends only on the set of valid pairs: permuting the lists, permuting the pairs of a list, swapping a
+ *   list's two images together with its pair columns, or adding duplicates leave every byte unchanged, and two calls
+ *   give the same bytes.
+ * - Returns the track count T, or CS_E_*.  With M the total member count: d_offsets (room for maxTracks + 1 ints, 4-byte
+ *   aligned) receives its first min(T, maxTracks) + 1 entries; it may be NULL when maxTracks == 0, and then nothing is
+ *   written to it.  d_members (room for maxMembers int pairs, 8-byte aligned) receives the first min(M, maxMembers)
+ *   members.  d_trackOf (N ints, 4-byte aligned) may be NULL; otherwise all N entries are written, track indices
+ *   >= maxTracks included.
+ * - stats_out (may be NULL): [0] valid pairs, [1] invalid pairs, [2] matched features, [3] components, [4] components
+ *   of at least minLength features that conflict (whatever dropConflicting is), [5] components below minLength, [6] T,
+ *   [7] M.
+ * - CS_E_ARG, before any CUDA call, naming the first offending lists[p] or imageSizes[a] in cs_last_error(): numImages
+ *   or numLists outside [0, 2^24], NULL imageSizes or lists with a positive count, imageSizes[a] < 0, N above INT_MAX
+ *   (named at the image where the sum passes it), image1 or image2 outside [0, numImages), numPairs < 0, NULL pairs
+ *   with numPairs > 0, pairs not 8-byte aligned, the total of numPairs above INT_MAX, minLength < 2, maxTracks < 0,
+ *   maxMembers < 0, NULL d_offsets with maxTracks > 0, NULL d_members with maxMembers > 0, misaligned output buffers,
+ *   and output buffers that overlap each other or any pair list (one sweep over sorted ranges, O(L log L)).  Pair lists
+ *   are only read and may overlap each other.
+ * - No pairs at all (numLists == 0, or every numPairs 0): returns 0 with zero statistics; d_trackOf (when not NULL) is
+ *   filled with -1 and d_offsets[0] (when not NULL) set to 0 by memsets, with no kernel launch; with N == 0 or
+ *   d_trackOf NULL, and d_offsets NULL, the call makes no CUDA call.  Lists with pairs but no valid pair: returns 0,
+ *   d_trackOf all -1, statistics [1] set.
+ * - Launches: a call with pairs issues 8 kernel launches (cs_launch_count), whatever numLists and the pair counts:
+ *   init, hook (every pair of every list), compress, run bounds, tile reduce, tile scan, track heads, members.  Between
+ *   compress and run bounds, cub::DeviceRadixSort sorts the N (label, global id) pairs over ceil(log2 N) key bits; its
+ *   launches (a few, by CUB's own plan) are not counted.  The call synchronises with the host once, at the end; *ms
+ *   (may be NULL) gets its event time.
+ * - Scratch, in the per-device context: 26 bytes per feature (the sort's four buffers, track index and first member
+ *   per label, two flag bytes), 8 bytes per 2048 features, 4 bytes per image, 32 bytes per list with pairs, and the
+ *   sort's temporary storage; there is no term per pair or per matched feature.  The pair lists are read in place.
+ * imageSizes[numImages], lists[numLists] on the host. */
+int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *lists, int numLists, int minLength,
+                    int dropConflicting, int *d_trackOf, int *d_offsets, int maxTracks, int *d_members, int maxMembers,
+                    long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
