@@ -1802,13 +1802,14 @@ int cs_describe_points(const float *d_img, int w, int h, int pitch, void *d_pts,
   if (r < 0) return r;
   for (int i = 0; i < CS_MAX_LEVELS; i++) ds.tex[i] = tex;
   unsigned int *d_cnt = nullptr;
-  const unsigned int cnt0[4] = {(unsigned)n, 0u, 0u, 0u};
+  const unsigned int cnt0[CS_CNT_STRIDE + 1] = {(unsigned)n, 0u, 0u, 0u, 0u};   // counters | queue word
   cudaError_t e = cudaMalloc((void **)&d_cnt, sizeof(cnt0));
   if (e == cudaSuccess) e = cudaMemcpyAsync(d_cnt, cnt0, sizeof(cnt0), cudaMemcpyHostToDevice, c->stream);
   if (e == cudaSuccess) {
-    ds.numLevels = CS_MAX_LEVELS; ds.pts = (SiftPoint *)d_pts; ds.counters = d_cnt; ds.maxPts = maxPts;
+    ds.numLevels = CS_MAX_LEVELS; ds.numImages = 1; ds.pts = (SiftPoint *)d_pts; ds.counters = d_cnt; ds.maxPts = maxPts;
     ds.finestSubsampling = finestSubsampling;
-    r = launch_describe(ds, c->sms * 8, c->stream);
+    ds.queue = d_cnt + CS_CNT_STRIDE;
+    r = launch_describe(ds, c->stream);
     if (r == 0) e = cudaMemcpyAsync(c->h_counters, d_cnt, 2 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream);
     if (r == 0 && e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   }

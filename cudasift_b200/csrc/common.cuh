@@ -158,14 +158,16 @@ struct DescribeParams {
   cudaTextureObject_t tex[CS_MAX_LEVELS];   // indexed by log2(subsampling); used when texArr == NULL
   const cudaTextureObject_t *texArr;        // batch: [image * CS_MAX_LEVELS + level] (device memory)
   int numLevels;
+  int numImages;                            // 1..CS_MAX_BATCH
   SiftPoint *pts;                           // image i: pts + i * ptsStride
   long long ptsStride;
   unsigned int *counters;                   // image i: counters + i * cntStride
   int cntStride;
   int maxPts;
   float finestSubsampling;  // secondaries of this level are dropped (reference quirk Q1)
+  unsigned int *queue;      // keypoint queue counter of all images (zero before the launch)
 };
-int launch_describe(const DescribeParams &p, int gridBlocks, cudaStream_t st, int batch = 1);
+int launch_describe(const DescribeParams &p, cudaStream_t st);
 int launch_rescale(SiftPoint *pts, const unsigned int *counters, int maxPts, float f,
                    cudaStream_t st);
 int launch_tex_probe(cudaTextureObject_t tex, const float *xs, const float *ys, int n,

@@ -15,11 +15,16 @@
 // Image samples go through the texture unit exactly as in the reference (bilinear,
 // clamp, unnormalised coordinates, cudaSiftH.cu:186-205), so the 1.8 fixed-point
 // interpolation weights are the hardware's own.
+//
+// Scheduling: the keypoints of all images of a launch form one queue (image 0's, then image 1's, ...), and one
+// resident wave of CTAs claims them from a counter.  A keypoint's chain of barriers is latency-bound, so what sets
+// the stage's time is how many chains are in flight per SM and that no CTA idles while another image still has work.
 #include "common.cuh"
 
 namespace cs {
 
 #define DS_THREADS 128
+#define DS_MIN_CTAS 10      // resident CTAs per SM the register budget is set for (at most 48 registers a thread)
 
 // cudaSiftD.cu:295-306, as scheduled in the reference's SASS.
 __device__ __forceinline__ float fast_atan2(float y, float x)
@@ -37,7 +42,7 @@ __device__ __forceinline__ float fast_atan2(float y, float x)
   return r;
 }
 
-__global__ void __launch_bounds__(DS_THREADS)
+__global__ void __launch_bounds__(DS_THREADS, DS_MIN_CTAS)
 describe_kernel(const __grid_constant__ DescribeParams P)
 {
   __shared__ float s_gauss11[11];
@@ -51,22 +56,37 @@ describe_kernel(const __grid_constant__ DescribeParams P)
   __shared__ int s_angi[16 * 17];
   __shared__ float s_hp[32][33];       // orientation: private 32-bin histograms of warp 0's lanes
   __shared__ float s_pb[128][9];       // descriptor: private angle bins (+ Q22 overflow slot) per (cell, row)
-  __shared__ float s_sums[4];
+  __shared__ float s_sums[2][4];       // the two norms of a descriptor: separate words, so no barrier between them
   __shared__ float s_ori[2];
   __shared__ int s_slot[2];
   __shared__ int s_nori;
+  __shared__ int s_next;               // the keypoint this CTA takes after the current one
 
-  const int tx = threadIdx.x;
+  const int tx = threadIdx.x, lane = tx & 31;
   if (tx < 16) s_gauss16[tx] = __expf(-(tx - 7.5f) * (tx - 7.5f) / 128.0f);   // cudaSiftD.cu:318
   for (int i = tx; i < 32 * 33; i += DS_THREADS) (&s_hp[0][0])[i] = 0.0f;
 
-  const int img = blockIdx.y;
-  SiftPoint *const pts = P.pts + (size_t)img * P.ptsStride;
-  unsigned int *const counters = P.counters + (size_t)img * P.cntStride;
-  const unsigned int found = counters[0];
-  const int numPrim = (int)min(found, (unsigned)P.maxPts);
+  // The queue: image i owns the batch-wide indices [end_{i-1}, end_i), end_i = sum over j <= i of
+  // min(found_j, maxPts).  Every warp keeps end_lane in a register (lanes past the last image hold the total).
+  unsigned int end = 0;
+  if (lane < P.numImages) end = min(P.counters[(size_t)lane * P.cntStride], (unsigned)P.maxPts);
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int t = __shfl_up_sync(0xffffffffu, end, o);
+    if (lane >= o) end += t;
+  }
+  const int total = (int)__shfl_sync(0xffffffffu, end, 31);
+  // claims run one keypoint ahead: the claim made during keypoint i is read while keypoint i + 1 runs
+  unsigned int req = 0;
+  if (tx == 0) req = gridDim.x + atomicAdd(P.queue, 1u);
 
-  for (int pt = blockIdx.x; pt < numPrim; pt += gridDim.x) {
+  for (int g = blockIdx.x; g < total;) {
+    const int img = __popc(__ballot_sync(0xffffffffu, end <= (unsigned)g));   // images that end at or before g
+    const unsigned int first = img ? __shfl_sync(0xffffffffu, end, (img - 1) & 31) : 0u;
+    const int numPrim = (int)(__shfl_sync(0xffffffffu, end, img) - first);
+    const int pt = g - (int)first;
+    SiftPoint *const pts = P.pts + (size_t)img * P.ptsStride;
+    unsigned int *const counters = P.counters + (size_t)img * P.cntStride;
     SiftPoint *sp = pts + pt;
     const float px = sp->xpos, py = sp->ypos, pscale = sp->scale, psub = sp->subsampling;
     const int level = ((__float_as_int(psub) >> 23) & 0xff) - 127;   // subsampling = 2^level
@@ -140,6 +160,8 @@ describe_kernel(const __grid_constant__ DescribeParams P)
       const float val1 = __shfl_sync(0xffffffffu, sm, (i1 + 1) & 31), val2 = __shfl_sync(0xffffffffu, sm, (i1 + 31) & 31);
       const float v1 = __shfl_sync(0xffffffffu, sm, (i2 + 1) & 31), v2 = __shfl_sync(0xffffffffu, sm, (i2 + 31) & 31);
       if (tx == 0) {   // :1034-1053
+        s_next = (int)req;
+        req = gridDim.x + atomicAdd(P.queue, 1u);
         float peak = __fadd_rn((float)i1, __fdiv_rn(__fmul_rn(0.5f, __fsub_rn(val1, val2)),
                                                     __fsub_rn(__fsub_rn(__fadd_rn(maxval1, maxval1), val1), val2)));
         s_ori[0] = __fmul_rn(11.25f, (peak < 0.0f ? __fadd_rn(peak, 32.0f) : peak));
@@ -165,6 +187,8 @@ describe_kernel(const __grid_constant__ DescribeParams P)
     }
     __syncthreads();
     const int nori = s_nori;
+    // read before any thread can pass the next keypoint's first two barriers, after which thread 0 rewrites it
+    const int gnext = s_next;
 
     // ------------------------------------------------------------------ descriptors
     for (int k = 0; k < nori; k++) {
@@ -210,27 +234,45 @@ describe_kernel(const __grid_constant__ DescribeParams P)
       {  // deterministic accumulation.  Thread (cell, k): the k-th sample row of the cell's 8x8
          // window, summed over x into 8 private angle bins (+ slot 8 for quirk Q22: angi == 8
          // votes into angle bin 0 of the NEXT cell in flat order, cudaSiftD.cu:353-384).
+        // The bins live in registers: each vote is a predicated add at a compile-time index, x ascending as before.
+        // The loop has no branch: a (row, x) outside the 16x16 window votes +0.0f, which leaves every bin as it is
+        // (a bin starts at +0, and a round-to-nearest sum that starts at +0 is never -0).
         const int cell = tx >> 3, kr = tx & 7;
         const int cy = cell >> 2, cx = cell & 3;
-        float *pb = s_pb[tx];
+        const int y = 4 * cy - 2 + kr;
+        const bool rowIn = (unsigned)y <= 15u;
+        const int row = min(max(y, 0), 15) * 17;
+        const int lower = kr < 4;                             // sample votes into its lower cell: ((y + 2) >> 2) - 1 != cy
+        float pb[9];
 #pragma unroll
         for (int a = 0; a < 9; a++) pb[a] = 0.0f;
-        const int y = 4 * cy - 2 + kr;
-        if (y >= 0 && y <= 15) {
-          const int lower = (((y + 2) >> 2) - 1 != cy);       // sample votes into its lower cell
-          const int xlo = max(0, 4 * cx - 2), xhi = min(15, 4 * cx + 5);
-          for (int x = xlo; x <= xhi; x++) {
-            const int right = (((x + 2) >> 2) - 1 != cx);     // ... into its right cell
-            const int sidx = y * 17 + x;
-            const int angi = s_angi[sidx];
-            const int angp = (angi < 7 ? angi + 1 : 0);
-            const float af = s_angf[sidx];
-            const float g2 = s_g2[2 * right + lower][sidx];
-            const int a1 = min(angi, 8);
-            pb[a1] = __fadd_rn(pb[a1], __fmul_rn(__fsub_rn(1.0f, af), g2));
-            pb[angp] = __fadd_rn(pb[angp], __fmul_rn(af, g2));
-          }
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+          const int x = 4 * cx - 2 + j;                       // inside the window for j = 2..5 whatever cx is
+          const bool edge = j < 2 || j > 5;
+          const bool in = rowIn && (!edge || (unsigned)x <= 15u);
+          const int sidx = row + (edge ? min(max(x, 0), 15) : x);
+          const int angi = s_angi[sidx];
+          const float af = s_angf[sidx];
+          const float g2 = s_g2[(j < 4 ? 2 : 0) + lower][sidx];   // j < 4: ... into its right cell, ((x + 2) >> 2) - 1 != cx
+          const float v1 = in ? __fmul_rn(__fsub_rn(1.0f, af), g2) : 0.0f;
+          const float v2 = in ? __fmul_rn(af, g2) : 0.0f;
+          const int a1 = min(angi, 8);
+          // v1 goes to bin a1, v2 to bin angp = (angi < 7 ? angi + 1 : 0): bin a >= 1 when a1 == a - 1, bin 0 when
+          // a1 >= 7.  a1 != angp, so no bin takes two votes of one sample.
+          bool eq[9];
+#pragma unroll
+          for (int a = 0; a < 9; a++) eq[a] = (a1 == a);
+#pragma unroll
+          for (int a = 0; a < 9; a++)
+            if (eq[a]) pb[a] = __fadd_rn(pb[a], v1);
+          if (a1 >= 7) pb[0] = __fadd_rn(pb[0], v2);
+#pragma unroll
+          for (int a = 1; a < 8; a++)
+            if (eq[a - 1]) pb[a] = __fadd_rn(pb[a], v2);
         }
+#pragma unroll
+        for (int a = 0; a < 9; a++) s_pb[tx][a] = pb[a];
       }
       __syncthreads();
       float v;
@@ -249,17 +291,16 @@ describe_kernel(const __grid_constant__ DescribeParams P)
       float sum = __fmul_rn(v, v);
 #pragma unroll
       for (int i = 16; i > 0; i /= 2) sum = __fadd_rn(sum, __shfl_down_sync(0xffffffffu, sum, i));
-      if ((tx & 31) == 0) s_sums[tx >> 5] = sum;
+      if ((tx & 31) == 0) s_sums[0][tx >> 5] = sum;
       __syncthreads();
-      float tsum1 = __fadd_rn(__fadd_rn(__fadd_rn(s_sums[0], s_sums[1]), s_sums[2]), s_sums[3]);
+      float tsum1 = __fadd_rn(__fadd_rn(__fadd_rn(s_sums[0][0], s_sums[0][1]), s_sums[0][2]), s_sums[0][3]);
       float t1 = fminf(__fmul_rn(v, rsqrtf(tsum1)), 0.2f);
       sum = __fmul_rn(t1, t1);
 #pragma unroll
       for (int i = 16; i > 0; i /= 2) sum = __fadd_rn(sum, __shfl_down_sync(0xffffffffu, sum, i));
+      if ((tx & 31) == 0) s_sums[1][tx >> 5] = sum;
       __syncthreads();
-      if ((tx & 31) == 0) s_sums[tx >> 5] = sum;
-      __syncthreads();
-      float tsum2 = __fadd_rn(__fadd_rn(__fadd_rn(s_sums[0], s_sums[1]), s_sums[2]), s_sums[3]);
+      float tsum2 = __fadd_rn(__fadd_rn(__fadd_rn(s_sums[1][0], s_sums[1][1]), s_sums[1][2]), s_sums[1][3]);
       SiftPoint *out = pts + s_slot[k];
       out->data[tx] = __fmul_rn(t1, rsqrtf(tsum2));
       if (tx == 0) {
@@ -273,14 +314,35 @@ describe_kernel(const __grid_constant__ DescribeParams P)
           out->subsampling = psub;
         }
       }
-      __syncthreads();
+      // No barrier here: every shared word read since the last one is next written only after a later barrier
+      // (the next orientation's first one, or the next keypoint's second one).
     }
+    g = gnext;
   }
 }
 
-int launch_describe(const DescribeParams &p, int gridBlocks, cudaStream_t st, int batch)
+// One resident wave: as many CTAs as the device holds at once (queried once per device).  A CTA whose first claim
+// is past the end of the queue exits at once.
+static int describe_grid()
 {
-  describe_kernel<<<dim3(gridBlocks, batch), DS_THREADS, 0, st>>>(p);
+  static int gridOf[64];
+  int dev = 0;
+  CS_CUDA(cudaGetDevice(&dev));
+  dev &= 63;
+  if (gridOf[dev] == 0) {
+    int sms = 0, perSm = 0;
+    CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    CS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, describe_kernel, DS_THREADS, 0));
+    gridOf[dev] = (perSm > 0 ? perSm : 1) * sms;
+  }
+  return gridOf[dev];
+}
+
+int launch_describe(const DescribeParams &p, cudaStream_t st)
+{
+  const int grid = describe_grid();
+  if (grid < 0) return grid;
+  describe_kernel<<<grid, DS_THREADS, 0, st>>>(p);
   count_launch();
   CS_CUDA(cudaGetLastError());
   return 0;

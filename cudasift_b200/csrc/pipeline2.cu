@@ -354,12 +354,11 @@ int Pipeline::enqueue(int n, const float *const *d_imgs, int pitch, double initB
   DescribeParams ds;
   memset(&ds, 0, sizeof(ds));
   ds.texArr = d_tex;
-  ds.numLevels = numLevels; ds.pts = d_pts; ds.ptsStride = ptsStride; ds.counters = d_counters;
+  ds.numLevels = numLevels; ds.numImages = n; ds.pts = d_pts; ds.ptsStride = ptsStride; ds.counters = d_counters;
   ds.cntStride = CS_CNT_STRIDE; ds.maxPts = maxPts;
   ds.finestSubsampling = 1.0f;
-  int gx = (sms * 12) / n;
-  if (gx < 96) gx = 96;
-  if ((r = launch_describe(ds, gx, st, n)) < 0) return r;
+  ds.queue = d_sched + 1;
+  if ((r = launch_describe(ds, st)) < 0) return r;
   if ((r = debug_stage(st, "describe")) < 0) return r;
   if (scaleUp)                                                             // cudaSiftH.cu:130
     for (int b = 0; b < n; b++)
@@ -380,8 +379,9 @@ int Pipeline::enqueue_round1(const float *d_img, int pitch, double initBlur, flo
 {
   int r;
   if (B != 1) { set_error("the round-1 kernels take one image at a time (pipeline built for %d)", B); return CS_E_ARG; }
-  unsigned int *d_counters = counters(0);
-  CS_CUDA(cudaMemsetAsync(d_counters, 0, CS_CNT_STRIDE * sizeof(unsigned int), st));   // cudaSiftH.cu:77
+  unsigned int *d_counters = counters(0), *d_sched = d_state + CS_CNT_STRIDE;
+  // the counters (cudaSiftH.cu:77) and the scheduler words that follow them (describe's queue word)
+  CS_CUDA(cudaMemsetAsync(d_counters, 0, (CS_CNT_STRIDE + 4) * sizeof(unsigned int), st));
   if (ev) cudaEventRecord(ev[0], st);
   Taps9 lp9;
   float sigma = (float)(initBlur > (double)0.001f ? initBlur : (double)0.001f);   // cudaSiftH.cu:112
@@ -423,9 +423,10 @@ int Pipeline::enqueue_round1(const float *d_img, int pitch, double initBlur, flo
   DescribeParams ds;
   memset(&ds, 0, sizeof(ds));
   for (int i = 0; i < numLevels; i++) ds.tex[i] = h_tex[i];
-  ds.numLevels = numLevels; ds.pts = d_pts; ds.counters = d_counters; ds.maxPts = maxPts;
+  ds.numLevels = numLevels; ds.numImages = 1; ds.pts = d_pts; ds.counters = d_counters; ds.maxPts = maxPts;
   ds.finestSubsampling = 1.0f;
-  if ((r = launch_describe(ds, sms * 8, st)) < 0) return r;
+  ds.queue = d_sched + 1;
+  if ((r = launch_describe(ds, st)) < 0) return r;
   if (scaleUp)                                                             // cudaSiftH.cu:130
     if ((r = launch_rescale(d_pts, d_counters, maxPts, 0.5f, st)) < 0) return r;
   if (ev) cudaEventRecord(ev[4], st);
