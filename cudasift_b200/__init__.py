@@ -20,7 +20,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
-           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks"]
+           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -92,6 +92,8 @@ def lib():
         "cs_match_ratio_batch": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_match_guided_batch": (ip, [vp, ip, vp, ip, vp, vp, fp, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_build_tracks": (ip, [vp, ip, vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, c.POINTER(c.c_double)]),
+        "cs_triangulate_tracks": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, c.c_ulonglong,
+                                       vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -759,6 +761,54 @@ def BuildTracks(imageSizes, lists, minLength=2, dropConflicting=True):
         for buf in bufs:
             buf.free()
     return offsets, members, trackOf, stats, ms.value
+
+
+def _per_image(x, shape, n, what):
+    """x as float64 [n, *shape]: one array per image, or one for every image."""
+    x = np.asarray(x, np.float64)
+    if x.shape == shape:
+        x = np.broadcast_to(x, (n,) + shape)
+    if x.shape != (n,) + shape:
+        raise ValueError("%s: shape %s or (%d, %s), not %s" % (what, shape, n, ", ".join(map(str, shape)), x.shape))
+    return np.ascontiguousarray(x)
+
+
+def TriangulateTracks(datas, Ks, Rs, ts, offsets, members, numTrials=256, maxError=4.0, minTriAngle=1.5, seed=0):
+    """A 3-D point per feature track with known cameras, in one call (cs_triangulate_tracks): RANSAC over two-view DLT
+    points, inliers by reprojection error below maxError pixels, one multi-view refit.  datas[a] holds image a's
+    records; Ks, Rs ([3, 3] each) and ts ([3]) are per image or one for every image, camera a mapping a world point X to
+    R_a X + t_a; offsets and members are BuildTracks' outputs.  Returns (points float64 [T, 3] (NaN without a point),
+    counts int32 [T], errors float32 [M], inlier bool [M], stats int64 [8] as the header describes them, ms)."""
+    S = len(datas)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1).astype(np.int32))
+    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1, 2).astype(np.int32))
+    T, M = max(len(off) - 1, 0), len(mem)
+    sets = (MatchSet * max(S, 1))(*[MatchSet(d.d_data, d.numPts) for d in datas])
+    points, counts = np.full((T, 3), np.nan), np.zeros(T, np.int32)
+    errors, inlier = np.full(M, np.nan, np.float32), np.zeros(M, bool)
+    stats, ms = np.zeros(8, np.int64), ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(off.nbytes, 4)), DeviceBuffer(max(mem.nbytes, 8)), DeviceBuffer(max(points.nbytes, 8)),
+            DeviceBuffer(max(counts.nbytes, 4)), DeviceBuffer(max(errors.nbytes, 4)), DeviceBuffer(max(M, 1))]
+    try:
+        if T:
+            bufs[0].upload(off)
+        if M:
+            bufs[1].upload(mem)
+        _check(lib().cs_triangulate_tracks(sets if S else None, S, _ptr(K), _ptr(R), _ptr(t), bufs[0].ptr, T,
+                                           bufs[1].ptr, M, int(numTrials), float(maxError), float(minTriAngle),
+                                           int(seed), bufs[2].ptr, bufs[3].ptr, bufs[4].ptr, bufs[5].ptr, _ptr(stats),
+                                           ctypes.byref(ms)), "TriangulateTracks")
+        if T:
+            points = bufs[2].download(np.float64, 3 * T).reshape(T, 3)
+            counts = bufs[3].download(np.int32, T)
+        if M:
+            errors = bufs[4].download(np.float32, M)
+            inlier = bufs[5].download(np.uint8, M).astype(bool)
+    finally:
+        for buf in bufs:
+            buf.free()
+    return points, counts, errors, inlier, stats, ms.value
 
 
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):

@@ -822,6 +822,89 @@ static int tracks_args(const char *fn, const int *imageSizes, int numImages, con
   return 0;
 }
 
+// The arguments of cs_triangulate_tracks: the counts and tables, every set (sets[a]) and camera (Ks[a], Rs[a], ts[a]),
+// the parameters, the buffers, then the outputs against each other, the tracks and every set's records (overlap_sweep).
+static int triangulate_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                            const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
+                            int numTrials, double maxError, double minTriAngle, const double *points, const int *counts,
+                            const float *errors, const unsigned char *inlier)
+{
+  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
+  if (numTracks < 0) return arg_error(fn, "numTracks must be >= 0");
+  if (numMembers < 0) return arg_error(fn, "numMembers must be >= 0");
+  if (numImages > 0 && (!sets || !Ks || !Rs || !ts)) return arg_error(fn, "numImages > 0 needs sets, Ks, Rs and ts");
+  char bad[128] = "";
+  for (int a = 0; a < numImages && !bad[0]; a++) {
+    if (sets[a].n < 0) snprintf(bad, sizeof bad, "sets[%d]: n must be >= 0", a);
+    else if (sets[a].n > 0 && !sets[a].pts) snprintf(bad, sizeof bad, "sets[%d]: a set with records needs a pointer", a);
+  }
+  if (bad[0]) return arg_error(fn, bad);
+  for (int a = 0; a < numImages; a++) {
+    snprintf(bad, sizeof bad, "Ks[%d]", a);
+    const int r = check_intrinsics(fn, Ks + 9 * (size_t)a, bad);
+    if (r < 0) return r;
+    const double *R = Rs + 9 * (size_t)a, *t = ts + 3 * (size_t)a;
+    bool ok = true;
+    for (int k = 0; k < 9; k++) ok = ok && std::isfinite(R[k]);
+    for (int i = 0; i < 3 && ok; i++)
+      for (int j = 0; j < 3; j++) {
+        const double d = R[3 * i] * R[3 * j] + R[3 * i + 1] * R[3 * j + 1] + R[3 * i + 2] * R[3 * j + 2];
+        ok = ok && std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-6;
+      }
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
+                       R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (!ok || !(det > 0.0)) {
+      snprintf(bad, sizeof bad, "Rs[%d] must be a finite rotation (R R^T = I within 1e-6, det R > 0)", a);
+      return arg_error(fn, bad);
+    }
+    if (!std::isfinite(t[0]) || !std::isfinite(t[1]) || !std::isfinite(t[2])) {
+      snprintf(bad, sizeof bad, "ts[%d] must be finite", a);
+      return arg_error(fn, bad);
+    }
+  }
+  if (numTrials < 1 || numTrials > (1 << 20)) return arg_error(fn, "numTrials must be in [1, 2^20]");
+  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
+  if (!std::isfinite(minTriAngle) || !(minTriAngle >= 0.0) || !(minTriAngle < 180.0))
+    return arg_error(fn, "minTriAngle must be finite and in [0, 180)");
+  if (numTracks > 0 && !offsets) return arg_error(fn, "numTracks > 0 needs d_offsets");
+  if (numTracks > 0 && (!points || !counts)) return arg_error(fn, "numTracks > 0 needs d_points and d_counts");
+  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
+  if ((reinterpret_cast<uintptr_t>(offsets) & 3) != 0 || (reinterpret_cast<uintptr_t>(counts) & 3) != 0 ||
+      (reinterpret_cast<uintptr_t>(errors) & 3) != 0)
+    return arg_error(fn, "d_offsets, d_counts and d_errors must be 4-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(members) & 7) != 0 || (reinterpret_cast<uintptr_t>(points) & 7) != 0)
+    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
+  // the outputs (kind 0, written; owners 0 d_points, 1 d_counts, 2 d_errors, 3 d_inlier), the tracks (kind 1, read;
+  // owners 0 d_offsets, 1 d_members) and every set's records (kind 2, read)
+  std::vector<SweepRange> rs;
+  rs.reserve((size_t)numImages + 6);
+  if (numTracks > 0) {
+    sweep_add(rs, points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
+    sweep_add(rs, counts, (size_t)numTracks * sizeof(int), 1, 0, true);
+    sweep_add(rs, offsets, ((size_t)numTracks + 1) * sizeof(int), 0, 1, false);
+  }
+  if (errors) sweep_add(rs, errors, (size_t)numMembers * sizeof(float), 2, 0, true);
+  if (inlier) sweep_add(rs, inlier, (size_t)numMembers, 3, 0, true);
+  sweep_add(rs, members, (size_t)numMembers * sizeof(int2), 1, 1, false);
+  for (int a = 0; a < numImages; a++) sweep_add(rs, sets[a].pts, record_bytes(sets[a].n), a, 2, false);
+  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
+    static const char *const outs[4] = {"d_points", "d_counts", "d_errors", "d_inlier"};
+    static const char *const ins[2] = {"d_offsets", "d_members"};
+    auto name = [&](const SweepRange &z, char *buf, size_t n) {
+      if (z.kind == 0) snprintf(buf, n, "%s", outs[z.owner]);
+      else if (z.kind == 1) snprintf(buf, n, "%s", ins[z.owner]);
+      else snprintf(buf, n, "sets[%d].pts", z.owner);
+    };
+    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
+    const SweepRange &b = &a == &x ? y : x;
+    char na[32], nb[32], msg[128];
+    name(a, na, sizeof na);
+    name(b, nb, sizeof nb);
+    snprintf(msg, sizeof msg, "%s and %s overlap (an output overlaps another range)", na, nb);
+    return arg_error(fn, msg);
+  });
+}
+
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
 {
   VerifyCalib cal;
@@ -1696,6 +1779,33 @@ int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *l
   if (stats_out)
     for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
   return (int)st[6];
+}
+
+int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
+                          const int *d_offsets, int numTracks, const int *d_members, int numMembers, int numTrials,
+                          double maxError, double minTriAngle, unsigned long long seed, double *d_points, int *d_counts,
+                          float *d_errors, unsigned char *d_inlier, long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_triangulate_tracks";
+  if (ms) *ms = 0.0;
+  int r = triangulate_args(fn, sets, numImages, Ks, Rs, ts, d_offsets, numTracks, d_members, numMembers, numTrials,
+                           maxError, minTriAngle, d_points, d_counts, d_errors, d_inlier);
+  if (r < 0) return r;
+  if (stats_out)
+    for (int k = 0; k < 8; k++) stats_out[k] = 0;
+  if (numTracks == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return triangulate_enqueue(*c, sets, numImages, Ks, Rs, ts, d_offsets, numTracks, d_members, numMembers,
+                                    numTrials, maxError, minTriAngle, seed, d_points, d_counts, d_errors, d_inlier);
+       })) < 0)
+    return r;
+  const unsigned long long *st = static_cast<const unsigned long long *>(c->h_tri);
+  if (stats_out)
+    for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
+  return (int)st[5];
 }
 
 // ---- stage-level entry points ----

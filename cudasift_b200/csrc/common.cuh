@@ -267,6 +267,10 @@ struct DeviceCtx {
   GrowBuffer tracks;
   void *h_tracks = nullptr;                // pinned: the statistics (copied back), then the bases and list table
   size_t h_tracksBytes = 0;
+  // cs_triangulate_tracks: the statistics and queue word, the camera table and the spilled members
+  GrowBuffer tri;
+  void *h_tri = nullptr;                   // pinned: the statistics (copied back), then the camera table
+  size_t h_triBytes = 0;
 
   // pinned host words
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
@@ -432,6 +436,14 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
 // eight statistics reach c.h_tracks (unsigned long long) by the caller's synchronize.
 int tracks_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
                    int minLength, bool drop, int *trackOf, int *offsets, int maxTracks, int *members, int maxMembers);
+
+// ---- triangulation (triangulate.cu) -----------------------------------------------------------------------------
+// The launch of cs_triangulate_tracks (argument-checked, numTracks > 0) on c.stream, without a synchronize; the eight
+// statistics reach c.h_tri (unsigned long long) by the caller's synchronize.
+int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                        const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
+                        int numTrials, double maxError, double minTriAngle, unsigned long long seed, double *points,
+                        int *counts, float *errors, unsigned char *inlier);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id launch_verify uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

@@ -448,6 +448,66 @@ int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *l
                     int dropConflicting, int *d_trackOf, int *d_offsets, int maxTracks, int *d_members, int maxMembers,
                     long long stats_out[8], double *ms);
 
+/* Triangulation of feature tracks with known cameras (COLMAP's point_triangulator, without bundle adjustment): per
+ * track, RANSAC over two-view DLT points, the inliers by reprojection error, one multi-view DLT refit.  The tracks of
+ * cs_build_tracks can be passed unchanged: d_offsets, d_members and numMembers = its stats_out[7].
+ * - Images and cameras: sets[a] holds image a's records (the indexing of cs_build_tracks' imageSizes).  Camera a maps
+ *   a world point X to Xc = R_a X + t_a (the convention of cs_verify_essential's pose); its centre is C_a = -R_a^T t_a.
+ *   K_a follows cs_verify_essential's rule, and the calibrated coordinates of a record are its formula, in double from
+ *   the float xpos, ypos: y^ = (y - K[5]) / K[4], x^ = (x - K[2] - K[1] * y^) / K[0].  Ks, Rs, ts: row-major
+ *   [numImages][9], [numImages][9], [numImages][3] on the host.
+ * - Tracks: track k's members are d_members[offsets[k] .. offsets[k+1]) (int pairs {image, feature}).  A track is
+ *   malformed when offsets[k] < 0, offsets[k+1] < offsets[k] or offsets[k+1] > numMembers (checked on the device): it
+ *   gets no point, is counted, and nothing of its members is read or written.  A member {a, f} is valid when
+ *   0 <= a < numImages, 0 <= f < sets[a].n and its xpos and ypos are finite.  V is the number of valid members of a
+ *   track; ranks 0 .. V-1 index them in member order.
+ * - Hypotheses: when V (V - 1) / 2 <= numTrials, every pair of ranks p < q, in lexicographic order, h = 0, 1, ...;
+ *   otherwise numTrials samples h = s = 0 .. numTrials-1, drawn with x = splitmix64(seed + 0x9E3779B97F4A7C15 *
+ *   ((k << 24) | (s << 4) | d)) and rank = ((x >> 32) * V) >> 32 for d = 0, 1, ... (64-bit unsigned arithmetic,
+ *   splitmix64 as in cs_verify_pairs): p is the first draw and q the next draw different from it; a sample without
+ *   two distinct ranks after 16 draws is degenerate and is not evaluated.  V < 2: no hypothesis.
+ * - Hypothesis h is the two-view DLT in calibrated coordinates: the rows x^ P[2] - P[0] and y^ P[2] - P[1] of member
+ *   p, then of member q (P = [R | t] of the member's image, P[i] its row i), summed into the 4x4 normal matrix, whose
+ *   eigenvector of the smallest eigenvalue (cyclic Jacobi, the lowest index on ties) is dehomogenised.  It is
+ *   admissible when the two members are of different images, the eigenvector's w is nonzero and the point X is
+ *   finite, its depth (R X + t)_2 is > 0 in both cameras, and, with a = X - C_p, b = X - C_q, a.b <= cosMin *
+ *   sqrt((a.a) (b.b)), cosMin = cos(minTriAngle * pi / 180) (the triangulation angle is at least minTriAngle degrees).
+ * - Inlier: a valid member whose depth d = (R X + t)_2 is > 0 and whose squared pixel reprojection error is strictly
+ *   below maxError^2, evaluated in double as (u0 - x d)^2 + (u1 - y d)^2 < maxError^2 d^2 with (u0, u1, d) = K (R X + t)
+ *   and (x, y) the record's position.
+ * - Winner: the admissible hypothesis with the most inliers, the lowest h on ties.  When it has at least 2 inliers,
+ *   one refit: the normal matrix of the rows of all its inliers (in rank order), solved as above; it is kept unless it
+ *   is not finite (w = 0 or X not finite) or has fewer inliers.  No depth or angle test applies to the refit.  A track
+ *   has a point when a winner exists and the final point's inlier count is >= 2.
+ * - Outputs: d_points[k] = the final point, d_counts[k] = its inlier count; a track without a point (malformed
+ *   included) gets NaN, NaN, NaN and 0.  For every member of a well-formed track, when the buffer is given:
+ *   d_errors = (float)sqrt(e2), e2 the squared pixel error under the final point, +inf when its depth is <= 0, NaN for
+ *   an invalid member or a track without a point; d_inlier = 1 for a final inlier, else 0.
+ * - Returns the number of tracks with a point, or CS_E_*.  stats_out (may be NULL): [0] well-formed tracks, [1]
+ *   malformed tracks, [2] invalid members, [3] hypotheses evaluated (non-degenerate samples), [4] admissible
+ *   hypotheses, [5] tracks with a point, [6] refits kept, [7] the sum of the final inlier counts.
+ * - Determinism: the outputs are a function of the arguments; two calls give the same bytes, whatever the device's
+ *   scheduling (except for a member that two well-formed tracks share, possible only with decreasing offsets: its
+ *   outputs come from either track).  They agree with a float64 statement of these rules to rounding, not bit for bit: the device contracts
+ *   products into fused multiply-adds, and the refit's sums run in a fixed per-lane order.
+ * - CS_E_ARG, before any CUDA call, naming the offending sets[a], camera a (Ks[a], Rs[a], ts[a]) or buffer in
+ *   cs_last_error(): numImages outside [0, 2^24], numTracks < 0, numMembers < 0, NULL sets, Ks, Rs or ts with
+ *   numImages > 0, NULL d_offsets or d_points or d_counts with numTracks > 0, NULL d_members with numMembers > 0, a set
+ *   with n < 0 or a NULL pts with n > 0, K not valid by cs_verify_essential's rule, R not finite, not orthonormal
+ *   (|R R^T - I| above 1e-6 in an entry) or with det R <= 0, t not finite, numTrials outside [1, 2^20], maxError not
+ *   finite or <= 0, minTriAngle not finite or outside [0, 180), d_offsets or d_counts or d_errors not 4-byte aligned,
+ *   d_members or d_points not 8-byte aligned, and an output (d_points [numTracks][3] doubles, d_counts, d_errors,
+ *   d_inlier) that overlaps another output, d_offsets (numTracks + 1 ints), d_members or any set's records (one sweep
+ *   over sorted ranges).  numTracks == 0 returns 0 with zero statistics and makes no CUDA call.
+ * - Launches: 1 kernel launch (cs_launch_count), whatever numTracks and the track lengths: a warp per track, claimed
+ *   from a queue by one resident wave of CTAs.  The call synchronises with the host once, at the end; *ms (may be
+ *   NULL) gets its event time.  Scratch, in the per-device context: 256 bytes, 280 bytes per image (the camera table)
+ *   and 16 bytes per member (valid members past the 128 a warp stages in shared memory). */
+int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
+                          const int *d_offsets, int numTracks, const int *d_members, int numMembers, int numTrials,
+                          double maxError, double minTriAngle, unsigned long long seed, double *d_points, int *d_counts,
+                          float *d_errors, unsigned char *d_inlier, long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
