@@ -125,8 +125,12 @@ int DeviceCtx::ensure(int d)
   if (dev == d && stream) return 0;
   dev = d;
   CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, d));
+  // the stream last: a context that has one has every pinned word
+  if (!h_counters) CS_CUDA(cudaMallocHost((void **)&h_counters, 4 * sizeof(unsigned int)));
+  if (!h_tcFlags) CS_CUDA(cudaMallocHost((void **)&h_tcFlags, 16 * sizeof(unsigned int)));
+  if (!h_pairTotal) CS_CUDA(cudaMallocHost((void **)&h_pairTotal, sizeof(unsigned int)));
+  if (!h_guidedStats) CS_CUDA(cudaMallocHost((void **)&h_guidedStats, 4 * sizeof(unsigned long long)));
   CS_CUDA(cudaStreamCreate(&stream));
-  CS_CUDA(cudaMallocHost((void **)&h_counters, 4 * sizeof(unsigned int)));
   return 0;
 }
 Pipeline *DeviceCtx::get_pipe(int w, int h, int oct, bool up, float *arena, int *err)
@@ -225,6 +229,35 @@ static int timed_sync(const char *fn, DeviceCtx *c, double *ms, Enqueue &&enqueu
   if (r >= 0 && ms) { float t = 0; cudaEventElapsedTime(&t, e0, e1); *ms = t; }
   cudaEventDestroy(e0); cudaEventDestroy(e1);                              // on every path
   return r;
+}
+
+// CUDA events between the kernels, printed to stderr (warm caches, unlike ncu)
+cudaEvent_t *match_timing_events()
+{
+  static int timing = -1;
+  static cudaEvent_t tev[9];
+  if (timing < 0) {
+    const char *e = getenv("CUDASIFT_MATCH_TIMING");
+    timing = (e && atoi(e)) ? 1 : 0;
+    if (timing) for (int i = 0; i < 9; i++) cudaEventCreate(&tev[i]);
+  }
+  return timing ? tev : nullptr;
+}
+
+void report_stage_times(const cudaEvent_t *tev, const char *const *names, int n, const char *header, ...)
+{
+  cudaEventSynchronize(tev[n]);
+  va_list ap;
+  va_start(ap, header);
+  vfprintf(stderr, header, ap);
+  va_end(ap);
+  fprintf(stderr, " [us]:");
+  for (int i = 0; i < n; i++) {
+    float ms = 0.0f;
+    cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
+    fprintf(stderr, " %s %.1f", names[i], ms * 1e3f);
+  }
+  fprintf(stderr, "\n");
 }
 
 // cs_match_stats after a finished match or knn call: the tensor path's counters (a two-way call: both directions
@@ -561,15 +594,7 @@ static int verify_buffers(DeviceCtx *c, const cs_verify_job *jobs, int numJobs, 
 {
   int r;
   if ((r = c->verify.grow(verify_scratch_bytes(jobs, numJobs, numLoops, model))) < 0) return r;
-  const size_t hb = verify_host_bytes(numJobs);
-  if (c->h_verifyBytes < hb) {                 // every verify call ends in a synchronize: no copy is pending here
-    if (c->h_verify) cudaFreeHost(c->h_verify);
-    c->h_verify = nullptr;
-    c->h_verifyBytes = 0;
-    CS_CUDA(cudaMallocHost(&c->h_verify, hb));
-    c->h_verifyBytes = hb;
-  }
-  return 0;
+  return c->h_verify.grow(verify_host_bytes(numJobs));
 }
 
 static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, const int *pairs, int numPairs,
@@ -581,16 +606,20 @@ static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2
   return j;
 }
 
-// The launches of a batch (cal: per job, essential only), one synchronize.
-static int verify_batch_sync(const char *fn, DeviceCtx *c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal,
-                             int model, int numLoops, float thresh, double *ms)
+// The launches of a batch (cal: per job, essential only), without a synchronize.
+static int verify_enqueue(DeviceCtx *c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model,
+                          int numLoops, float thresh)
 {
   int r;
   if ((r = verify_buffers(c, jobs, numJobs, numLoops, model)) < 0) return r;
-  auto enqueue = [&] {
-    return launch_verify(jobs, numJobs, cal, model, numLoops, thresh, c->verify.p, c->h_verify, true, c->stream);
-  };
-  return timed_sync(fn, c, ms, enqueue);
+  return launch_verify(jobs, numJobs, cal, model, numLoops, thresh, c->verify.p, c->h_verify.p, true, c->stream);
+}
+
+// The same, one synchronize.
+static int verify_batch_sync(const char *fn, DeviceCtx *c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal,
+                             int model, int numLoops, float thresh, double *ms)
+{
+  return timed_sync(fn, c, ms, [&] { return verify_enqueue(c, jobs, numJobs, cal, model, numLoops, thresh); });
 }
 
 // The shared path of cs_verify_pairs_host and cs_verify_essential_host: the sets and the input pairs uploaded, then
@@ -611,13 +640,12 @@ static int verify_host_pairs(DeviceCtx *c, const void *h_s1, int n1, const void 
                     });
 }
 
-// The body of cs_verify_pairs_batch and cs_verify_essential_batch after their argument checks: every job's outputs
-// zeroed (zero(p), the count and numStats statistics), the launches when a job has pairs, then every non-empty job's
-// count and statistics from result(q, p, stats), job p being the q-th non-empty one.
-template <class Zero, class Result>
-static int verify_batch_body(const char *fn, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model,
-                             int numLoops, float thresh, int *counts_out, long long *stats_out, int numStats, double *ms,
-                             Zero &&zero, Result &&result)
+// The body of a batch entry point after its argument checks: every job's outputs zeroed (zero(p), the count and
+// numStats statistics); when some job has work (work(p)), enqueue(c) and one synchronize; then the count and statistics
+// of every job with work from result(c, p, q, st), job p being the q-th with work and st numStats zeros on entry.
+template <class Stat, class Zero, class Work, class Enqueue, class Result>
+static int batch_body(const char *fn, int numJobs, int *counts_out, Stat *stats_out, int numStats, double *ms,
+                      Zero &&zero, Work &&work, Enqueue &&enqueue, Result &&result)
 {
   bool any = false;
   for (int p = 0; p < numJobs; p++) {
@@ -625,18 +653,18 @@ static int verify_batch_body(const char *fn, const cs_verify_job *jobs, int numJ
     counts_out[p] = 0;
     if (stats_out)
       for (int k = 0; k < numStats; k++) stats_out[numStats * (size_t)p + k] = 0;
-    any |= jobs[p].numPairs > 0;
+    any |= work(p);
   }
   if (!any) return 0;
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   int r;
-  if ((r = verify_batch_sync(fn, c, jobs, numJobs, cal, model, numLoops, thresh, ms)) < 0) return r;
+  if ((r = timed_sync(fn, c, ms, [&] { return enqueue(c); })) < 0) return r;
   for (int p = 0, q = 0; p < numJobs; p++) {
-    if (jobs[p].numPairs == 0) continue;
-    long long st[10];
-    counts_out[p] = result(c->h_verify, q++, p, st);
+    if (!work(p)) continue;
+    Stat st[10] = {};
+    counts_out[p] = result(c, p, q++, st);
     if (stats_out)
       for (int k = 0; k < numStats; k++) stats_out[numStats * (size_t)p + k] = st[k];
   }
@@ -649,8 +677,9 @@ static int verify_models_sync(DeviceCtx *c, const cs_verify_job &job, const Veri
 {
   int r;
   if ((r = verify_buffers(c, &job, 1, numLoops, model)) < 0) return r;
-  if ((r = launch_verify(&job, 1, cal, model, numLoops, thresh, c->verify.p, c->h_verify, false, c->stream)) < 0) return r;
-  return verify_models_to_host(c->verify.p, c->h_verify, job, numLoops, model, cal, h_models, h_counts, h_norm,
+  if ((r = launch_verify(&job, 1, cal, model, numLoops, thresh, c->verify.p, c->h_verify.p, false, c->stream)) < 0)
+    return r;
+  return verify_models_to_host(c->verify.p, c->h_verify.p, job, numLoops, model, cal, h_models, h_counts, h_norm,
                                c->stream);
 }
 
@@ -1505,7 +1534,7 @@ int cs_verify_pairs(const void *d_s1, int n1, const void *d_s2, int n2, const in
   const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
                                        d_inliers, maxInliers);
   if ((r = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms)) < 0) return r;
-  return verify_result(c->h_verify, 0, numPairs, model_out, c->verifyStats);
+  return verify_result(c->h_verify.p, 0, numPairs, model_out, c->verifyStats);
 }
 
 int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs, int model,
@@ -1524,7 +1553,7 @@ int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, con
   return verify_host_pairs(c, h_s1, n1, h_s2, n2, h_pairs, numPairs, seed, h_inliers, maxInliers,
                            [&](const cs_verify_job &job) {
                              const int q = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms);
-                             return q < 0 ? q : verify_result(c->h_verify, 0, numPairs, model_out, c->verifyStats);
+                             return q < 0 ? q : verify_result(c->h_verify.p, 0, numPairs, model_out, c->verifyStats);
                            });
 }
 
@@ -1579,7 +1608,7 @@ int cs_verify_essential(const void *d_s1, int n1, const void *d_s2, int n2, cons
   const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
                                        d_inliers, maxInliers);
   if ((r = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms)) < 0) return r;
-  return verify_essential_result(c->h_verify, 0, numPairs, E_out, R_out, t_out, c->essentialStats);
+  return verify_essential_result(c->h_verify.p, 0, numPairs, E_out, R_out, t_out, c->essentialStats);
 }
 
 int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs,
@@ -1601,7 +1630,7 @@ int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2,
   return verify_host_pairs(c, h_s1, n1, h_s2, n2, h_pairs, numPairs, seed, h_inliers, maxInliers,
                            [&](const cs_verify_job &job) {
                              const int q = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms);
-                             return q < 0 ? q : verify_essential_result(c->h_verify, 0, numPairs, E_out, R_out, t_out,
+                             return q < 0 ? q : verify_essential_result(c->h_verify.p, 0, numPairs, E_out, R_out, t_out,
                                                                         c->essentialStats);
                            });
 }
@@ -1643,11 +1672,13 @@ int cs_verify_pairs_batch(const cs_verify_job *jobs, int numJobs, int model, int
   int r = verify_batch_args(fn, jobs, numJobs, model, numLoops, thresh, nullptr, nullptr, false);
   if (r < 0) return r;
   if (numJobs > 0 && (!models_out || !counts_out)) return arg_error(fn, "models_out and counts_out must not be NULL");
-  return verify_batch_body(fn, jobs, numJobs, nullptr, model, numLoops, thresh, counts_out, stats_out, 8, ms,
-                           [&](int p) { for (int k = 0; k < 9; k++) models_out[9 * (size_t)p + k] = 0.0; },
-                           [&](const void *h, int q, int p, long long *st) {
-                             return verify_result(h, q, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
-                           });
+  return batch_body(fn, numJobs, counts_out, stats_out, 8, ms,
+                    [&](int p) { for (int k = 0; k < 9; k++) models_out[9 * (size_t)p + k] = 0.0; },
+                    [&](int p) { return jobs[p].numPairs > 0; },
+                    [&](DeviceCtx *c) { return verify_enqueue(c, jobs, numJobs, nullptr, model, numLoops, thresh); },
+                    [&](DeviceCtx *c, int p, int q, long long *st) {
+                      return verify_result(c->h_verify.p, q, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
+                    });
 }
 
 int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const double *K1s, const double *K2s,
@@ -1662,12 +1693,16 @@ int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const doub
     return arg_error(fn, "E_out, R_out, t_out and counts_out must not be NULL");
   std::vector<VerifyCalib> cal((size_t)numJobs);
   for (int p = 0; p < numJobs; p++) cal[p] = verify_calib(K1s + 9 * (size_t)p, K2s + 9 * (size_t)p);
-  return verify_batch_body(fn, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh, counts_out, stats_out, 10,
-                           ms, [&](int p) { essential_zero(E_out + 9 * (size_t)p, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p); },
-                           [&](const void *h, int q, int p, long long *st) {
-                             return verify_essential_result(h, q, jobs[p].numPairs, E_out + 9 * (size_t)p,
-                                                            R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
-                           });
+  return batch_body(fn, numJobs, counts_out, stats_out, 10, ms,
+                    [&](int p) { essential_zero(E_out + 9 * (size_t)p, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p); },
+                    [&](int p) { return jobs[p].numPairs > 0; },
+                    [&](DeviceCtx *c) {
+                      return verify_enqueue(c, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh);
+                    },
+                    [&](DeviceCtx *c, int p, int q, long long *st) {
+                      return verify_essential_result(c->h_verify.p, q, jobs[p].numPairs, E_out + 9 * (size_t)p,
+                                                     R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
+                    });
 }
 
 int cs_match_ratio_batch(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs, float maxRatio,
@@ -1677,39 +1712,26 @@ int cs_match_ratio_batch(const cs_match_set *sets, int numSets, const cs_match_j
   if (ms) *ms = 0.0;
   int r = ratio_batch_args(fn, sets, numSets, jobs, numJobs, maxRatio, maxDistance, counts_out);
   if (r < 0) return r;
-  bool any = false;
-  for (int p = 0; p < numJobs; p++) {
-    counts_out[p] = 0;
-    if (stats_out)
-      for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = 0;
-    any |= sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0;
-  }
-  if (!any) return 0;
-  int err = 0;
-  DeviceCtx *c = current_ctx(&err);
-  if (!c) return err;
   std::vector<RatioBatchOut> out((size_t)numJobs);
-  if ((r = timed_sync(fn, c, ms, [&] {
-         return ratio_batch_enqueue(*c, sets, numSets, jobs, numJobs, maxRatio, maxDistance, crossCheck != 0, out.data());
-       })) < 0)
-    return r;
-  for (int p = 0; p < numJobs; p++) {
-    const RatioBatchOut &o = out[p];
-    if (!o.total) continue;                                               // an empty job
-    counts_out[p] = (int)*o.total;
-    if (!stats_out) continue;
-    unsigned long long *st = stats_out + 4 * (size_t)p;
-    if (*o.bad1 || *o.bad2) {                                             // as match_tensor_stats: all exact
-      st[0] = st[1] = 0; st[2] = ~0ull;
-    } else {
-      for (int k = 0; k < 2; k++) {
-        if (!o.counters[k]) continue;
-        st[0] += o.counters[k][1]; st[1] += o.counters[k][2]; st[2] += o.counters[k][0];
-      }
-    }
-    st[3] = 2;
-  }
-  return 0;
+  return batch_body(fn, numJobs, counts_out, stats_out, 4, ms, [](int) {},
+                    [&](int p) { return sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0; },
+                    [&](DeviceCtx *c) {
+                      return ratio_batch_enqueue(*c, sets, numSets, jobs, numJobs, maxRatio, maxDistance, crossCheck != 0,
+                                                 out.data());
+                    },
+                    [&](DeviceCtx *, int p, int, unsigned long long *st) {
+                      const RatioBatchOut &o = out[p];
+                      if (*o.bad1 || *o.bad2) {                             // as match_tensor_stats: all exact
+                        st[0] = st[1] = 0; st[2] = ~0ull;
+                      } else {
+                        for (int k = 0; k < 2; k++) {
+                          if (!o.counters[k]) continue;
+                          st[0] += o.counters[k][1]; st[1] += o.counters[k][2]; st[2] += o.counters[k][0];
+                        }
+                      }
+                      st[3] = 2;
+                      return (int)*o.total;
+                    });
 }
 
 int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
@@ -1721,30 +1743,17 @@ int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_
   int r = guided_batch_args(fn, sets, numSets, jobs, numJobs, models, models_in, thresh, maxRatio, maxDistance,
                             counts_out);
   if (r < 0) return r;
-  bool any = false;
-  for (int p = 0; p < numJobs; p++) {
-    counts_out[p] = 0;
-    if (stats_out)
-      for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = 0;
-    any |= sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0;
-  }
-  if (!any) return 0;
-  int err = 0;
-  DeviceCtx *c = current_ctx(&err);
-  if (!c) return err;
   std::vector<GuidedBatchOut> out((size_t)numJobs, GuidedBatchOut{nullptr, nullptr});
-  if ((r = timed_sync(fn, c, ms, [&] {
-         return guided_batch_enqueue(*c, sets, jobs, numJobs, models, models_in, thresh, maxRatio, maxDistance,
-                                     crossCheck != 0, out.data());
-       })) < 0)
-    return r;
-  for (int p = 0; p < numJobs; p++) {
-    if (!out[p].total) continue;                                          // an empty job
-    counts_out[p] = (int)*out[p].total;
-    if (stats_out)
-      for (int k = 0; k < 4; k++) stats_out[4 * (size_t)p + k] = out[p].stats[k];
-  }
-  return 0;
+  return batch_body(fn, numJobs, counts_out, stats_out, 4, ms, [](int) {},
+                    [&](int p) { return sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0; },
+                    [&](DeviceCtx *c) {
+                      return guided_batch_enqueue(*c, sets, jobs, numJobs, models, models_in, thresh, maxRatio,
+                                                  maxDistance, crossCheck != 0, out.data());
+                    },
+                    [&](DeviceCtx *, int p, int, unsigned long long *st) {
+                      for (int k = 0; k < 4; k++) st[k] = out[p].stats[k];
+                      return (int)*out[p].total;
+                    });
 }
 
 int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *lists, int numLists, int minLength,
@@ -1775,7 +1784,7 @@ int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *l
                                d_offsets, maxTracks, d_members, maxMembers);
        })) < 0)
     return r;
-  const unsigned long long *st = static_cast<const unsigned long long *>(c->h_tracks);
+  const unsigned long long *st = c->h_tracks.as<const unsigned long long>();
   if (stats_out)
     for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
   return (int)st[6];
@@ -1802,7 +1811,7 @@ int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double 
                                     numTrials, maxError, minTriAngle, seed, d_points, d_counts, d_errors, d_inlier);
        })) < 0)
     return r;
-  const unsigned long long *st = static_cast<const unsigned long long *>(c->h_tri);
+  const unsigned long long *st = c->h_tri.as<const unsigned long long>();
   if (stats_out)
     for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
   return (int)st[5];

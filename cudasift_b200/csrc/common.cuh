@@ -210,6 +210,35 @@ struct GrowBuffer {
   }
   template <class T> T *as() const { return static_cast<T *>(p); }
 };
+// The same in pinned host memory.  Every call that copies into or out of one ends in a synchronize, so no copy is
+// pending when the next call grows it.
+struct PinnedBuffer {
+  void *p = nullptr;
+  size_t cap = 0;
+  int grow(size_t bytes)
+  {
+    if (cap >= bytes) return 0;
+    if (p) cudaFreeHost(p);
+    p = nullptr; cap = 0;
+    CS_CUDA(cudaMallocHost(&p, bytes));
+    cap = bytes;
+    return 0;
+  }
+  template <class T> T *as() const { return static_cast<T *>(p); }
+};
+
+// Consecutive pieces of one allocation: take(n) returns the next piece's offset and moves on by n rounded up to align
+// (a power of two); bytes is the size of the pieces taken so far.
+struct Layout {
+  size_t align, bytes = 0;
+  explicit Layout(size_t a) : align(a) {}
+  size_t take(size_t n)
+  {
+    const size_t at = bytes;
+    bytes += (n + align - 1) & ~(align - 1);
+    return at;
+  }
+};
 
 struct Pipeline;    // extraction, batched and round-1 kernels (pipeline2.h)
 struct PipeKey {
@@ -248,8 +277,7 @@ struct DeviceCtx {
   // cs_match_knn2_guided, cs_match_guided(_host, _batch): coefficient records, cell grids and the sorted candidate
   // copies; a batch wave's tables, headers, knn lists and pair scratch as well
   GrowBuffer guided;
-  void *h_guidedBatch = nullptr;           // pinned: every cs_match_guided_batch wave's tables and copied-back state
-  size_t h_guidedBatchBytes = 0;
+  PinnedBuffer h_guidedBatch;              // every cs_match_guided_batch wave's tables and copied-back state
   // the tensor path (match_tc.cu) of cs_match(_host), cs_match_mutual(_host), cs_match_knn2, cs_match_ratio(_host):
   // operand tiles, B-role copies, row norms, top-3 tables, fallback rows, and 2 x 16 words of flags used alternately
   GrowBuffer tcA, tcB, tcNorms, tcTables, tcRows, tcFlags;
@@ -261,23 +289,20 @@ struct DeviceCtx {
   // lists and fallback entries; its flags, counters and totals (cleared per wave), then the pair scratch
   GrowBuffer mbTables, mbLists, mbState;
   bool mbConfigured = false;               // the batch GEMM's shared-memory size is set
-  void *h_mb = nullptr;                    // pinned: every wave's tables (uploaded) and state (copied back)
-  size_t h_mbBytes = 0;
+  PinnedBuffer h_mb;                       // every wave's tables (uploaded) and state (copied back)
   // cs_build_tracks: the statistics, image bases, list table, per-tile totals, per-feature arrays and sort storage
   GrowBuffer tracks;
-  void *h_tracks = nullptr;                // pinned: the statistics (copied back), then the bases and list table
-  size_t h_tracksBytes = 0;
+  PinnedBuffer h_tracks;                   // the statistics (copied back), then the bases and list table
   // cs_triangulate_tracks: the statistics and queue word, the camera table and the spilled members
   GrowBuffer tri;
-  void *h_tri = nullptr;                   // pinned: the statistics (copied back), then the camera table
-  size_t h_triBytes = 0;
+  PinnedBuffer h_tri;                      // the statistics (copied back), then the camera table
+  // cs_verify_*: the states a call copies back, and its job table
+  PinnedBuffer h_verify;
 
-  // pinned host words
+  // pinned host words, allocated by ensure()
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
   unsigned int *h_tcFlags = nullptr;       // 16: the tensor path's flag area of the last call
   unsigned int *h_pairTotal = nullptr;     // the pair total of the last mutual or ratio call
-  void *h_verify = nullptr;                // the states a verify call copies back, and its job table
-  size_t h_verifyBytes = 0;
   unsigned long long *h_guidedStats = nullptr;   // 4: the counters of the last guided call
 
   unsigned long long matchStats[4] = {0, 0, 0, 0};
@@ -292,6 +317,10 @@ struct DeviceCtx {
 
 // CUDASIFT_MATCH_TIMING=1: nine events for timing the kernels of a match or verify call, else null
 cudaEvent_t *match_timing_events();
+// After the stages' launches: "<header> [us]: name t name t ..." on stderr, stage i timed from tev[i] to tev[i + 1]
+// (waits for tev[n]).  header is a printf format.
+void report_stage_times(const cudaEvent_t *tev, const char *const *names, int n, const char *header, ...)
+    __attribute__((format(printf, 4, 5)));
 
 // ---- matcher ------------------------------------------------------------------------
 // the cross-check of a mutual match: pairs with score > minScore and ambiguity < maxAmbiguity, at most maxPairs written

@@ -598,9 +598,6 @@ GuidedModel guided_model(int model, const double in[9], float thresh)
   return gm;
 }
 
-// Bytes of a, rounded up to 256.
-static size_t gd_align(size_t a) { return (a + 255) & ~(size_t)255; }
-
 // The scratch of one call or batch job (its header aside), every piece 256-byte aligned: the cell counts, zeroed before
 // the call (offsets from the zeroed base), then the rest (offsets from the other base).  own: a batch job, which also
 // holds its knn lists and pair scratch; a single call uses the context's knnLists and pairScratch.
@@ -616,22 +613,21 @@ static GLayout gd_layout(int n1, int n2, int dirs, bool own)
   const size_t n = (size_t)n1 + n2, m1 = dirs == 2 ? n1 : 1;
   L.cap0 = 2 * n2 + 64;
   L.cap1 = dirs == 2 ? 2 * n1 + 64 : 1;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { const size_t o = off; off += gd_align(bytes); return o; };
-  L.cnt0 = take(4 * (size_t)L.cap0); L.cnt1 = take(4 * (size_t)L.cap1);
-  L.zeroBytes = off;
-  off = 0;
-  L.pts = take(sizeof(GPoint) * n); L.cell = take(sizeof(int2) * n);
-  L.s0C = take(4 * ((size_t)L.cap0 + 1)); L.s0R = take(4 * ((size_t)L.cap0 + 1));
-  L.s1C = take(4 * ((size_t)L.cap1 + 1)); L.s1R = take(4 * ((size_t)L.cap1 + 1));
-  L.c0C = take(16 * (size_t)n2); L.i0C = take(4 * (size_t)n2); L.c0R = take(16 * (size_t)n2); L.i0R = take(4 * (size_t)n2);
-  L.c1C = take(16 * m1); L.i1C = take(4 * m1); L.c1R = take(16 * m1); L.i1R = take(4 * m1);
+  Layout z(256), b(256);
+  L.cnt0 = z.take(4 * (size_t)L.cap0); L.cnt1 = z.take(4 * (size_t)L.cap1);
+  L.zeroBytes = z.bytes;
+  L.pts = b.take(sizeof(GPoint) * n); L.cell = b.take(sizeof(int2) * n);
+  L.s0C = b.take(4 * ((size_t)L.cap0 + 1)); L.s0R = b.take(4 * ((size_t)L.cap0 + 1));
+  L.s1C = b.take(4 * ((size_t)L.cap1 + 1)); L.s1R = b.take(4 * ((size_t)L.cap1 + 1));
+  L.c0C = b.take(16 * (size_t)n2); L.i0C = b.take(4 * (size_t)n2);
+  L.c0R = b.take(16 * (size_t)n2); L.i0R = b.take(4 * (size_t)n2);
+  L.c1C = b.take(16 * m1); L.i1C = b.take(4 * m1); L.c1R = b.take(16 * m1); L.i1R = b.take(4 * m1);
   const size_t l2 = own && dirs == 2 ? (size_t)n2 : 0;
-  L.idx1 = take(own ? 8 * (size_t)n1 : 0); L.sc1 = take(own ? 8 * (size_t)n1 : 0);
-  L.idx2 = take(8 * l2); L.sc2 = take(8 * l2);
+  L.idx1 = b.take(own ? 8 * (size_t)n1 : 0); L.sc1 = b.take(own ? 8 * (size_t)n1 : 0);
+  L.idx2 = b.take(8 * l2); L.sc2 = b.take(8 * l2);
   // the flags / write kernels' ballot words and counts of 1024-row CTAs (match_mutual.cu)
-  L.masks = take(own ? 4 * (size_t)idivup(n1, 32) : 0); L.ctaCounts = take(own ? 4 * (size_t)idivup(n1, 1024) : 0);
-  L.bytes = off;
+  L.masks = b.take(own ? 4 * (size_t)idivup(n1, 32) : 0); L.ctaCounts = b.take(own ? 4 * (size_t)idivup(n1, 1024) : 0);
+  L.bytes = b.bytes;
   return L;
 }
 
@@ -680,17 +676,17 @@ int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint
   const int dirs = idx2 ? 2 : 1, n = n1 + n2;
   // layout: header and cell counts first (one memset), then the rest
   const GLayout L = gd_layout(n1, n2, dirs, false);
-  const size_t zeroBytes = gd_align(sizeof(GHdr)) + L.zeroBytes;
+  Layout dev(256);
+  const size_t hdrAt = dev.take(sizeof(GHdr)), zeroAt = dev.take(L.zeroBytes), restAt = dev.take(L.bytes);
   int r;
-  if ((r = c.guided.grow(zeroBytes + L.bytes)) < 0) return r;
-  if (!c.h_guidedStats) CS_CUDA(cudaMallocHost((void **)&c.h_guidedStats, 4 * sizeof(unsigned long long)));
+  if ((r = c.guided.grow(dev.bytes)) < 0) return r;
   char *b = c.guided.as<char>();
-  GHdr *h = reinterpret_cast<GHdr *>(b);
-  const GJob j = gd_job(s1, n1, s2, n2, dirs, gm, h, b + gd_align(sizeof(GHdr)), b + zeroBytes, L);
+  GHdr *h = reinterpret_cast<GHdr *>(b + hdrAt);
+  const GJob j = gd_job(s1, n1, s2, n2, dirs, gm, h, b + zeroAt, b + restAt, L);
   cudaStream_t st = c.stream;
   cudaEvent_t *tev = match_timing_events();
   if (tev) cudaEventRecord(tev[0], st);
-  CS_CUDA(cudaMemsetAsync(b, 0, zeroBytes, st));
+  CS_CUDA(cudaMemsetAsync(b, 0, restAt, st));
   const int blocks = idivup(n, 256) < 4 * c.sms ? idivup(n, 256) : 4 * c.sms;
   guided_prep_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
   if (tev) cudaEventRecord(tev[1], st);
@@ -710,17 +706,8 @@ int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint
     if (tev) cudaEventRecord(tev[3 + dir], st);
   }
   CS_CUDA(cudaMemcpyAsync(c.h_guidedStats, h->stats, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  if (tev) {
-    static const char *const names[] = {"prep", "index", "knn", "reverse-knn"};
-    cudaEventSynchronize(tev[2 + dirs]);
-    fprintf(stderr, "guided timing %dx%d [us]:", n1, n2);
-    for (int i = 0; i < 2 + dirs; i++) {
-      float ms = 0.0f;
-      cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
-      fprintf(stderr, " %s %.1f", names[i], 1000.0f * ms);
-    }
-    fprintf(stderr, "\n");
-  }
+  static const char *const stages[] = {"prep", "index", "knn", "reverse-knn"};
+  if (tev) report_stage_times(tev, stages, 2 + dirs, "guided timing %dx%d", n1, n2);
   return 0;
 }
 
@@ -731,14 +718,17 @@ size_t guided_job_bytes(int n1, int n2, bool cross)
   return L.zeroBytes + L.bytes + GD_JOB_STATE_BYTES;
 }
 
-static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
-
-// A wave (the header states the rule): the non-empty jobs ne[q0, q1) and what its launches need.  Device scratch
-// (c.guided): the tables; then, zeroed per wave, the headers and pair totals (copied back) and every job's cell
-// counts; then the rest of every job.  Pinned (c.h_guidedBatch from pinOff): the tables, then the copied-back state.
+// A wave (the header states the rule): the non-empty jobs ne[q0, q1) and what its launches need.
 struct GdWave {
   int q0 = 0, q1 = 0, pointCtas = 0, knnCtas = 0, pairCtas = 0, dirs = 0;
-  size_t bytes = 0, tabBytes = 0, stateBytes = 0, zeroBytes = 0, restBytes = 0, pinOff = 0;
+  size_t bytes = 0, zeroBytes = 0, restBytes = 0;
+  // The tables (jobs at 0, directions at dirsAt, pair jobs at pairJobsAt) and the state (headers at 0, pair totals at
+  // totalsAt), each piece at a multiple of 16 bytes.  Pinned (c.h_guidedBatch from pinOff): the tables, then from
+  // tabBytes the copied-back state.  Device scratch (c.guided), every piece at a multiple of 256 bytes: the tables;
+  // from stateDev, zeroed per wave, the state and every job's cell counts (from zeroDev); from restDev the rest of
+  // every job.
+  size_t dirsAt = 0, pairJobsAt = 0, tabBytes = 0, totalsAt = 0, stateBytes = 0, pinOff = 0;
+  size_t stateDev = 0, zeroDev = 0, restDev = 0;
 };
 
 int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs,
@@ -773,34 +763,38 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
   for (GdWave &v : waves) {
     const size_t J = v.q1 - v.q0;
     v.dirs = (int)J * D;
-    v.tabBytes = align16(J * sizeof(GJob)) + align16(v.dirs * sizeof(GDir)) + align16(J * sizeof(PairJob));
-    v.stateBytes = align16(J * sizeof(GHdr)) + align16(J * sizeof(unsigned int));
+    Layout tab(16), state(16), scratch(256);
+    tab.take(J * sizeof(GJob));
+    v.dirsAt = tab.take(v.dirs * sizeof(GDir));
+    v.pairJobsAt = tab.take(J * sizeof(PairJob));
+    v.tabBytes = tab.bytes;
+    state.take(J * sizeof(GHdr));
+    v.totalsAt = state.take(J * sizeof(unsigned int));
+    v.stateBytes = state.bytes;
     v.pinOff = pin;
     pin += v.tabBytes + v.stateBytes;
-    dev = std::max(dev, gd_align(v.tabBytes) + gd_align(v.stateBytes) + v.zeroBytes + v.restBytes);
+    scratch.take(v.tabBytes);
+    v.stateDev = scratch.take(v.stateBytes);
+    v.zeroDev = scratch.take(v.zeroBytes);
+    v.restDev = scratch.take(v.restBytes);
+    dev = std::max(dev, scratch.bytes);
   }
   int r;
   if ((r = c.guided.grow(dev)) < 0) return r;
-  if (c.h_guidedBatchBytes < pin) {          // every batch call ends in a synchronize: no copy is pending here
-    if (c.h_guidedBatch) cudaFreeHost(c.h_guidedBatch);
-    c.h_guidedBatch = nullptr;
-    c.h_guidedBatchBytes = 0;
-    CS_CUDA(cudaMallocHost(&c.h_guidedBatch, pin));
-    c.h_guidedBatchBytes = pin;
-  }
+  if ((r = c.h_guidedBatch.grow(pin)) < 0) return r;
   const cudaStream_t st = c.stream;
   cudaEvent_t *tev = match_timing_events();
   for (const GdWave &v : waves) {
     const int J = v.q1 - v.q0;
-    char *hp = static_cast<char *>(c.h_guidedBatch) + v.pinOff;
+    char *hp = c.h_guidedBatch.as<char>() + v.pinOff;
     GJob *hj = reinterpret_cast<GJob *>(hp);
-    GDir *hd = reinterpret_cast<GDir *>(hp + align16(J * sizeof(GJob)));
-    PairJob *hpj = reinterpret_cast<PairJob *>(hp + align16(J * sizeof(GJob)) + align16(v.dirs * sizeof(GDir)));
+    GDir *hd = reinterpret_cast<GDir *>(hp + v.dirsAt);
+    PairJob *hpj = reinterpret_cast<PairJob *>(hp + v.pairJobsAt);
     const char *hstate = hp + v.tabBytes;
-    char *dt = c.guided.as<char>(), *ds = dt + gd_align(v.tabBytes);
+    char *dt = c.guided.as<char>(), *ds = dt + v.stateDev;
     GHdr *hdrs = reinterpret_cast<GHdr *>(ds);
-    unsigned int *totals = reinterpret_cast<unsigned int *>(ds + align16(J * sizeof(GHdr)));
-    char *z = ds + gd_align(v.stateBytes), *b = z + v.zeroBytes;
+    unsigned int *totals = reinterpret_cast<unsigned int *>(ds + v.totalsAt);
+    char *z = dt + v.zeroDev, *b = dt + v.restDev;
     int pointCta = 0, knnCta = 0, pairCta = 0;
     for (int k = 0; k < J; k++) {
       const int p = ne[v.q0 + k];
@@ -830,14 +824,14 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
       pj.cta0 = pairCta;
       pairCta += idivup(n1, 1024);
       out[p].stats = reinterpret_cast<const GHdr *>(hstate)[k].stats;
-      out[p].total = reinterpret_cast<const unsigned int *>(hstate + align16(J * sizeof(GHdr))) + k;
+      out[p].total = reinterpret_cast<const unsigned int *>(hstate + v.totalsAt) + k;
       z += L.zeroBytes;
       b += L.bytes;
     }
     const GJob *dj = reinterpret_cast<const GJob *>(dt);
-    const GDir *dd = reinterpret_cast<const GDir *>(dt + align16(J * sizeof(GJob)));
-    const PairJob *dpj = reinterpret_cast<const PairJob *>(dt + align16(J * sizeof(GJob)) + align16(v.dirs * sizeof(GDir)));
-    CS_CUDA(cudaMemsetAsync(ds, 0, gd_align(v.stateBytes) + v.zeroBytes, st));
+    const GDir *dd = reinterpret_cast<const GDir *>(dt + v.dirsAt);
+    const PairJob *dpj = reinterpret_cast<const PairJob *>(dt + v.pairJobsAt);
+    CS_CUDA(cudaMemsetAsync(ds, 0, v.restDev - v.stateDev, st));
     CS_CUDA(cudaMemcpyAsync(dt, hp, v.tabBytes, cudaMemcpyHostToDevice, st));
     if (tev) cudaEventRecord(tev[0], st);
     guided_prep_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
@@ -853,17 +847,9 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
     if ((r = launch_ratio_pairs_batch(c, dpj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
     if (tev) cudaEventRecord(tev[4], st);
     CS_CUDA(cudaMemcpyAsync(hp + v.tabBytes, ds, v.stateBytes, cudaMemcpyDeviceToHost, st));
-    if (tev) {
-      static const char *const names[] = {"prep", "index", "knn", "pairs"};
-      cudaEventSynchronize(tev[4]);
-      fprintf(stderr, "guided-batch timing %d jobs %d directions %d rows [us]:", J, v.dirs, 8 * v.knnCtas);
-      for (int i = 0; i < 4; i++) {
-        float ms = 0.0f;
-        cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
-        fprintf(stderr, " %s %.1f", names[i], 1000.0f * ms);
-      }
-      fprintf(stderr, "\n");
-    }
+    static const char *const stages[] = {"prep", "index", "knn", "pairs"};
+    if (tev)
+      report_stage_times(tev, stages, 4, "guided-batch timing %d jobs %d directions %d rows", J, v.dirs, 8 * v.knnCtas);
   }
   return 0;
 }

@@ -134,7 +134,6 @@ static int pairs_scratch(DeviceCtx &c, int n1, PairJob &pj)
   const int blocks = idivup(n1, MP_ROWS), words = idivup(n1, 32);
   int r;
   if ((r = c.pairScratch.grow(((size_t)words + blocks + 1) * sizeof(unsigned int))) < 0) return r;
-  if (!c.h_pairTotal) CS_CUDA(cudaMallocHost((void **)&c.h_pairTotal, sizeof(unsigned int)));
   pj.n1 = n1;
   pj.masks = c.pairScratch.as<unsigned int>(); pj.blockCounts = pj.masks + words; pj.total = pj.blockCounts + blocks;
   pj.cta0 = 0;

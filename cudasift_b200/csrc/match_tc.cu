@@ -752,10 +752,9 @@ static int t3_setup(DeviceCtx &c, const SiftPoint *s1, int n1, int n1v, const Si
   if ((r = c.tcA.grow(aBytes)) < 0 || (r = c.tcB.grow(bBytes)) < 0 || (r = c.tcNorms.grow(rows * sizeof(float))) < 0 ||
       (r = c.tcTables.grow(slots * T3_PM * sizeof(float))) < 0 || (r = c.tcRows.grow(fbRows * sizeof(int))) < 0)
     return r;
-  if (!c.h_tcFlags) {
+  if (!c.tcFlags.p) {
     if ((r = c.tcFlags.grow(128)) < 0) return r;
     CS_CUDA(cudaMemsetAsync(c.tcFlags.p, 0, 128, st));
-    CS_CUDA(cudaMallocHost((void **)&c.h_tcFlags, 64));
   }
   float *flags = c.tcFlags.as<float>() + 16 * (c.tcCalls & 1);
   float *nextFlags = c.tcFlags.as<float>() + 16 * ((c.tcCalls + 1) & 1);
@@ -835,32 +834,9 @@ static int t3_end(DeviceCtx &c, const float *flags)
   return 0;
 }
 
-// CUDA events between the kernels, printed to stderr (warm caches, unlike ncu)
-cudaEvent_t *match_timing_events()
-{
-  static int timing = -1;
-  static cudaEvent_t tev[9];
-  if (timing < 0) {
-    const char *e = getenv("CUDASIFT_MATCH_TIMING");
-    timing = (e && atoi(e)) ? 1 : 0;
-    if (timing) for (int i = 0; i < 9; i++) cudaEventCreate(&tev[i]);
-  }
-  return timing ? tev : nullptr;
-}
-// the first n stages: a one-way call has 4, a two-way knn call 7, a mutual call 8
-static void t3_print_timing(const char *what, int n1, int n2, const cudaEvent_t *tev, int n)
-{
-  static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
-                                      "reverse-exact-fallback", "pairs"};
-  cudaEventSynchronize(tev[n]);
-  fprintf(stderr, "%s timing %dx%d [us]:", what, n1, n2);
-  for (int i = 0; i < n; i++) {
-    float ms = 0.0f;
-    cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
-    fprintf(stderr, " %s %.1f", names[i], ms * 1e3f);
-  }
-  fprintf(stderr, "\n");
-}
+// the stages of a tensor-path call; a one-way call has the first 4, a two-way knn call 7, a mutual call 8
+static const char *const t3_stages[] = {"prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve",
+                                        "reverse-exact-fallback", "pairs"};
 
 // Set 1's five match fields; with mu (32 or more rows in each set) also set 2's, exactly as a one-way match of set 2
 // against set 1 writes them, then the cross-checked pairs (launch_mutual_pairs).  One prep launch converts each set once
@@ -885,7 +861,7 @@ int match_tensor(DeviceCtx &c, SiftPoint *s1, int n1, SiftPoint *s2, int n2, con
     if ((r = launch_mutual_pairs(c, s1, n1, s2, n2, *mu)) < 0) return r;
     if (tev) cudaEventRecord(tev[8], c.stream);
   }
-  if (tev) t3_print_timing(mu ? "mutual" : "match", n1, n2, tev, mu ? 8 : 4);
+  if (tev) report_stage_times(tev, t3_stages, mu ? 8 : 4, "%s timing %dx%d", mu ? "mutual" : "match", n1, n2);
   return t3_end(c, t.flags);
 }
 
@@ -906,7 +882,7 @@ int match_knn_tensor(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint 
   t.dr.idx = reinterpret_cast<int2 *>(idx2); t.dr.score = reinterpret_cast<float2 *>(score2);
   if ((r = t3_direction<true>(c, t.pf, t.fw, t.df, t.gate, tev ? tev + 2 : nullptr)) < 0) return r;
   if (both && (r = t3_direction<true>(c, t.pr, t.rv, t.dr, t.gate, tev ? tev + 5 : nullptr)) < 0) return r;
-  if (tev) t3_print_timing("knn", n1, n2, tev, both ? 7 : 4);
+  if (tev) report_stage_times(tev, t3_stages, both ? 7 : 4, "knn timing %dx%d", n1, n2);
   return t3_end(c, t.flags);
 }
 
@@ -939,10 +915,11 @@ struct MbWave {
   std::vector<int> sets;            // the distinct sets, in order of first use
   int dirs = 0, tiles = 0, dirTiles = 0, rows = 0, words = 0, pairCtas = 0, units = 0, resolveCtas = 0, prepCtas = 0;
   size_t bytes = 0;                 // the rule's scratch
-  size_t tabBytes = 0, zeroWords = 0, pinOff = 0;
+  size_t zeroWords = 0;
+  // The wave's pinBytes in c.h_mb, from pinOff: the tables (sets at 0, directions at dirsAt, jobs at jobsAt; uploaded
+  // to c.mbTables), then from stateAt the state's zeroWords (copied back).  Every piece starts at a multiple of 16 bytes.
+  size_t pinOff = 0, pinBytes = 0, dirsAt = 0, jobsAt = 0, stateAt = 0;
 };
-
-static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
 static std::vector<MbWave> mb_waves(const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
                                     bool cross)
@@ -984,10 +961,15 @@ static std::vector<MbWave> mb_waves(const cs_match_set *sets, int numSets, const
   size_t pin = 0;
   for (MbWave &v : waves) {
     const size_t S = v.sets.size(), D = v.dirs, J = v.jobs.size();
-    v.tabBytes = align16(S * sizeof(T3PrepSet)) + align16(D * sizeof(MbDir)) + align16(J * sizeof(PairJob));
     v.zeroWords = (2 * S + 4 * D + J + 1 + 3) & ~(size_t)3;
+    Layout L(16);
+    L.take(S * sizeof(T3PrepSet));
+    v.dirsAt = L.take(D * sizeof(MbDir));
+    v.jobsAt = L.take(J * sizeof(PairJob));
+    v.stateAt = L.take(v.zeroWords * sizeof(unsigned int));
     v.pinOff = pin;
-    pin += v.tabBytes + v.zeroWords * sizeof(unsigned int);
+    v.pinBytes = L.bytes;
+    pin += v.pinBytes;
   }
   return waves;
 }
@@ -999,11 +981,11 @@ static void mb_fill(DeviceCtx &c, const MbWave &v, const cs_match_set *sets, con
                     std::vector<int> &slot, RatioBatchOut *out)
 {
   const int S = (int)v.sets.size(), D = v.dirs, J = (int)v.jobs.size();
-  uint8_t *hp = static_cast<uint8_t *>(c.h_mb) + v.pinOff;
+  uint8_t *hp = c.h_mb.as<uint8_t>() + v.pinOff;
   T3PrepSet *hs = reinterpret_cast<T3PrepSet *>(hp);
-  MbDir *hd = reinterpret_cast<MbDir *>(hp + align16(S * sizeof(T3PrepSet)));
-  PairJob *hj = reinterpret_cast<PairJob *>(hp + align16(S * sizeof(T3PrepSet)) + align16(D * sizeof(MbDir)));
-  const unsigned int *hstate = reinterpret_cast<const unsigned int *>(hp + v.tabBytes);
+  MbDir *hd = reinterpret_cast<MbDir *>(hp + v.dirsAt);
+  PairJob *hj = reinterpret_cast<PairJob *>(hp + v.jobsAt);
+  const unsigned int *hstate = reinterpret_cast<const unsigned int *>(hp + v.stateAt);
   unsigned int *st = c.mbState.as<unsigned int>();
   unsigned int *masks = st + v.zeroWords, *counts = masks + v.words;
   int2 *idx = c.mbLists.as<int2>();
@@ -1079,8 +1061,8 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
     slots = std::max(slots, t3_slots(v.dirTiles, c.sms));
     rows = std::max(rows, (size_t)v.rows);
     state = std::max(state, v.zeroWords + v.words + v.pairCtas);
-    tab = std::max(tab, v.tabBytes);
-    pin = v.pinOff + v.tabBytes + v.zeroWords * sizeof(unsigned int);
+    tab = std::max(tab, v.stateAt);
+    pin = v.pinOff + v.pinBytes;
   }
   const cudaStream_t st = c.stream;
   int r;
@@ -1089,13 +1071,7 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
       (r = c.mbLists.grow(rows * (sizeof(int2) + sizeof(float2) + sizeof(int2)))) < 0 ||
       (r = c.mbState.grow(state * sizeof(unsigned int))) < 0)
     return r;
-  if (c.h_mbBytes < pin) {                  // every batch call ends in a synchronize: no copy is pending here
-    if (c.h_mb) cudaFreeHost(c.h_mb);
-    c.h_mb = nullptr;
-    c.h_mbBytes = 0;
-    CS_CUDA(cudaMallocHost(&c.h_mb, pin));
-    c.h_mbBytes = pin;
-  }
+  if ((r = c.h_mb.grow(pin)) < 0) return r;
   if (!c.mbConfigured) {
     CS_CUDA(cudaFuncSetAttribute(t3_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, T3_SMEM_BYTES));
     c.mbConfigured = true;
@@ -1105,11 +1081,11 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
   for (const MbWave &v : waves) {
     mb_fill(c, v, sets, jobs, cross, slot, out);
     const int S = (int)v.sets.size(), D = v.dirs, J = (int)v.jobs.size();
-    uint8_t *hp = static_cast<uint8_t *>(c.h_mb) + v.pinOff;
+    uint8_t *hp = c.h_mb.as<uint8_t>() + v.pinOff;
     uint8_t *dt = c.mbTables.as<uint8_t>();
     const T3PrepSet *ds = reinterpret_cast<const T3PrepSet *>(dt);
-    const MbDir *dd = reinterpret_cast<const MbDir *>(dt + align16(S * sizeof(T3PrepSet)));
-    const PairJob *dj = reinterpret_cast<const PairJob *>(dt + align16(S * sizeof(T3PrepSet)) + align16(D * sizeof(MbDir)));
+    const MbDir *dd = reinterpret_cast<const MbDir *>(dt + v.dirsAt);
+    const PairJob *dj = reinterpret_cast<const PairJob *>(dt + v.jobsAt);
     unsigned int *state = c.mbState.as<unsigned int>();
     int2 *entries = c.mbLists.as<int2>() + 2 * (size_t)v.rows;
     unsigned int *numEntries = state + 2 * S + 4 * D + J;
@@ -1118,7 +1094,7 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
     t3_schedule(pl, c.sms);
     const T3Buffers bf = {c.tcA.as<__half>(), c.tcA.as<__half>(), c.tcTables.as<float>(), nullptr};
     CS_CUDA(cudaMemsetAsync(state, 0, v.zeroWords * sizeof(unsigned int), st));
-    CS_CUDA(cudaMemcpyAsync(dt, hp, v.tabBytes, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(dt, hp, v.stateAt, cudaMemcpyHostToDevice, st));
     if (tev) cudaEventRecord(tev[0], st);
     t3_prep_kernel<true><<<v.prepCtas, 512, 0, st>>>(T3PrepSet{}, T3PrepSet{}, ds, S, nullptr, nullptr);
     if (tev) cudaEventRecord(tev[1], st);
@@ -1133,18 +1109,9 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
     if (tev) cudaEventRecord(tev[4], st);
     if ((r = launch_ratio_pairs_batch(c, dj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
     if (tev) cudaEventRecord(tev[5], st);
-    CS_CUDA(cudaMemcpyAsync(hp + v.tabBytes, state, v.zeroWords * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-    if (tev) {
-      static const char *const names[] = {"prep", "gemm", "resolve", "exact-fallback", "pairs"};
-      cudaEventSynchronize(tev[5]);
-      fprintf(stderr, "ratio-batch timing %d jobs %d directions %d units [us]:", J, D, v.units);
-      for (int i = 0; i < 5; i++) {
-        float ms = 0.0f;
-        cudaEventElapsedTime(&ms, tev[i], tev[i + 1]);
-        fprintf(stderr, " %s %.1f", names[i], ms * 1e3f);
-      }
-      fprintf(stderr, "\n");
-    }
+    CS_CUDA(cudaMemcpyAsync(hp + v.stateAt, state, v.zeroWords * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
+    static const char *const stages[] = {"prep", "gemm", "resolve", "exact-fallback", "pairs"};
+    if (tev) report_stage_times(tev, stages, 5, "ratio-batch timing %d jobs %d directions %d units", J, D, v.units);
   }
   return 0;
 }

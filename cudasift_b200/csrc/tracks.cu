@@ -270,8 +270,6 @@ __global__ void __launch_bounds__(TK_THREADS) tracks_members_kernel(TkBufs b, co
   }
 }
 
-size_t round256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int grid_of(long long n, int per) { return (int)((n + per - 1) / per > 0 ? (n + per - 1) / per : 1); }
 
 }  // namespace
@@ -281,8 +279,8 @@ int grid_of(long long n, int per) { return (int)((n + per - 1) / per > 0 ? (n + 
 // size is computed (tempBytes from cub).
 static size_t tracks_layout(char *base, int N, int numImages, int numTables, TkBufs *b, size_t tempBytes)
 {
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char *p = base ? base + off : nullptr; off += round256(bytes); return p; };
+  Layout L(256);
+  auto take = [&](size_t bytes) { const size_t at = L.take(bytes); return base ? base + at : nullptr; };
   b->stats = reinterpret_cast<unsigned long long *>(take(8 * sizeof(unsigned long long)));
   b->bases = reinterpret_cast<const int *>(take((size_t)numImages * sizeof(int)));
   b->lists = reinterpret_cast<const TkList *>(take((size_t)numTables * sizeof(TkList)));
@@ -295,7 +293,7 @@ static size_t tracks_layout(char *base, int N, int numImages, int numTables, TkB
   b->conf = reinterpret_cast<unsigned char *>(take((size_t)N));
   b->sortTemp = take(tempBytes);
   b->sortBytes = tempBytes;
-  return off;
+  return L.bytes;
 }
 
 int tracks_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
@@ -331,15 +329,8 @@ int tracks_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const cs_
   // the bases and the list table go up in one copy from pinned memory (the previous call ended in a synchronize)
   const size_t tableOff = reinterpret_cast<const char *>(b.lists) - reinterpret_cast<const char *>(b.bases);
   const size_t up = tableOff + (size_t)numTables * sizeof(TkList);
-  const size_t pin = 8 * sizeof(unsigned long long) + up;
-  if (c.h_tracksBytes < pin) {
-    if (c.h_tracks) cudaFreeHost(c.h_tracks);
-    c.h_tracks = nullptr;
-    c.h_tracksBytes = 0;
-    CS_CUDA(cudaMallocHost(&c.h_tracks, pin));
-    c.h_tracksBytes = pin;
-  }
-  char *h = static_cast<char *>(c.h_tracks) + 8 * sizeof(unsigned long long);
+  if ((r = c.h_tracks.grow(8 * sizeof(unsigned long long) + up)) < 0) return r;
+  char *h = c.h_tracks.as<char>() + 8 * sizeof(unsigned long long);
   if (numImages) memcpy(h, bases.data(), (size_t)numImages * sizeof(int));
   if (numTables) memcpy(h + tableOff, table.data(), (size_t)numTables * sizeof(TkList));
   CS_CUDA(cudaMemcpyAsync(const_cast<int *>(b.bases), h, up, cudaMemcpyHostToDevice, c.stream));
@@ -365,7 +356,7 @@ int tracks_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const cs_
                                                    reinterpret_cast<int2 *>(members), maxMembers);
   count_launch(5);
   CS_CUDA(cudaGetLastError());
-  CS_CUDA(cudaMemcpyAsync(c.h_tracks, b.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CS_CUDA(cudaMemcpyAsync(c.h_tracks.p, b.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   return 0;
 }
 

@@ -362,8 +362,6 @@ int triangulate_grid()
   return gridOf[dev];
 }
 
-size_t round256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 }  // namespace
 
 int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
@@ -371,24 +369,18 @@ int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, c
                         int numTrials, double maxError, double minTriAngle, unsigned long long seed, double *points,
                         int *counts, float *errors, unsigned char *inlier)
 {
-  // scratch: the statistics and the queue word (256 bytes), the camera table, the spilled members
-  const size_t camBytes = round256((size_t)numImages * sizeof(TrCam));
-  const size_t bytes = 256 + camBytes + (size_t)numMembers * sizeof(TrEntry);
-  int r = c.tri.grow(bytes);
+  // scratch: the statistics and the queue word, the camera table, the spilled members
+  Layout L(256);
+  const size_t statsAt = L.take(8 * sizeof(unsigned long long) + sizeof(unsigned int));
+  const size_t camAt = L.take((size_t)numImages * sizeof(TrCam)), spillAt = L.bytes;
+  int r = c.tri.grow(spillAt + (size_t)numMembers * sizeof(TrEntry));
   if (r < 0) return r;
   char *base = c.tri.as<char>();
 
   // the camera table is built in pinned memory after the statistics' landing area (the previous call ended in a
   // synchronize) and goes up in one copy
-  const size_t pin = 256 + camBytes;
-  if (c.h_triBytes < pin) {
-    if (c.h_tri) cudaFreeHost(c.h_tri);
-    c.h_tri = nullptr;
-    c.h_triBytes = 0;
-    CS_CUDA(cudaMallocHost(&c.h_tri, pin));
-    c.h_triBytes = pin;
-  }
-  TrCam *cams = reinterpret_cast<TrCam *>(static_cast<char *>(c.h_tri) + 256);
+  if ((r = c.h_tri.grow(spillAt)) < 0) return r;
+  TrCam *cams = reinterpret_cast<TrCam *>(c.h_tri.as<char>() + camAt);
   for (int a = 0; a < numImages; a++) {
     TrCam &m = cams[a];
     const double *K = Ks + 9 * (size_t)a, *R = Rs + 9 * (size_t)a, *t = ts + 3 * (size_t)a;
@@ -407,10 +399,10 @@ int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, c
   }
 
   TrParams prm;
-  prm.stats = reinterpret_cast<unsigned long long *>(base);
-  prm.queue = reinterpret_cast<unsigned int *>(base + 8 * sizeof(unsigned long long));
-  prm.cams = reinterpret_cast<const TrCam *>(base + 256);
-  prm.spill = reinterpret_cast<TrEntry *>(base + 256 + camBytes);
+  prm.stats = reinterpret_cast<unsigned long long *>(base + statsAt);
+  prm.queue = reinterpret_cast<unsigned int *>(prm.stats + 8);
+  prm.cams = reinterpret_cast<const TrCam *>(base + camAt);
+  prm.spill = reinterpret_cast<TrEntry *>(base + spillAt);
   prm.offsets = offsets;
   prm.members = reinterpret_cast<const int2 *>(members);
   prm.points = points;
@@ -429,12 +421,12 @@ int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, c
   if (wave < 0) return wave;
   const int grid = std::min(wave, idivup(numTracks, TR_WARPS));
   const cudaStream_t st = c.stream;
-  CS_CUDA(cudaMemsetAsync(base, 0, 256, st));
-  if (numImages) CS_CUDA(cudaMemcpyAsync(base + 256, cams, (size_t)numImages * sizeof(TrCam), cudaMemcpyHostToDevice, st));
+  CS_CUDA(cudaMemsetAsync(base + statsAt, 0, camAt - statsAt, st));
+  if (numImages) CS_CUDA(cudaMemcpyAsync(base + camAt, cams, (size_t)numImages * sizeof(TrCam), cudaMemcpyHostToDevice, st));
   triangulate_kernel<<<grid, TR_THREADS, 0, st>>>(prm);
   count_launch();
   CS_CUDA(cudaGetLastError());
-  CS_CUDA(cudaMemcpyAsync(c.h_tri, prm.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CS_CUDA(cudaMemcpyAsync(c.h_tri.p, prm.stats, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   return 0;
 }
 

@@ -1381,20 +1381,19 @@ struct VerifyLayout {
 static VerifyLayout verify_layout(const VerifyPlan &p, int numLoops, int model)
 {
   VerifyLayout L;
-  size_t o = 0;
-  auto take = [&](size_t b) { const size_t at = o; o += (b + 255) & ~(size_t)255; return at; };
+  Layout o(256);
   const size_t live = std::max(p.live.size(), (size_t)1), J = std::min(live, (size_t)p.perWave);
   const size_t P = std::max(p.rows, (size_t)1) * VP_ROWS, S = vp_slots_per_sample(model) * (size_t)numLoops * J;
-  L.jobs = take(live * sizeof(VerifyJob));
-  L.masks = take(P / 32 * sizeof(unsigned int));
-  L.counts = take(P / VP_ROWS * sizeof(unsigned int));
-  L.xy = take(P * sizeof(float4));
-  L.un = take(P * sizeof(float4));
-  L.orig = take(P * sizeof(int));
-  L.models = take(S * 9 * sizeof(double));
-  L.slotCounts = take(S * sizeof(unsigned int));
-  L.state = take(J * sizeof(VerifyState));
-  L.bytes = o;
+  L.jobs = o.take(live * sizeof(VerifyJob));
+  L.masks = o.take(P / 32 * sizeof(unsigned int));
+  L.counts = o.take(P / VP_ROWS * sizeof(unsigned int));
+  L.xy = o.take(P * sizeof(float4));
+  L.un = o.take(P * sizeof(float4));
+  L.orig = o.take(P * sizeof(int));
+  L.models = o.take(S * 9 * sizeof(double));
+  L.slotCounts = o.take(S * sizeof(unsigned int));
+  L.state = o.take(J * sizeof(VerifyState));
+  L.bytes = o.bytes;
   return L;
 }
 
@@ -1403,22 +1402,15 @@ size_t verify_scratch_bytes(const cs_verify_job *jobs, int numJobs, int numLoops
   return verify_layout(verify_plan(jobs, numJobs, numLoops, model), numLoops, model).bytes;
 }
 
-// The pinned host area of a batch: one state per job (the q-th non-empty job's at q), then the job table.
-static size_t vp_host_states_bytes(int numJobs) { return ((size_t)std::max(numJobs, 1) * sizeof(VerifyState) + 255) & ~(size_t)255; }
-size_t verify_host_bytes(int numJobs) { return vp_host_states_bytes(numJobs) + (size_t)std::max(numJobs, 1) * sizeof(VerifyJob); }
-
-// CUDASIFT_MATCH_TIMING=1: the events between the kernels, printed to stderr
-static void vp_timing_print(cudaEvent_t *tev, int numPairs, int numLoops, int model)
+// The pinned host area of a batch: one state per job (the q-th non-empty job's at q), then from the returned offset the
+// job table.
+static size_t vp_host_jobs_at(int numJobs)
 {
-  static const char *names[8] = {"flags", "compact", "norm", "hyp", "score", "argmax", "refit", "write"};
-  cudaEventSynchronize(tev[8]);
-  fprintf(stderr, "verify timing model=%d pairs=%d loops=%d", model, numPairs, numLoops);
-  for (int i = 0; i < 8; i++) {
-    float t = 0; cudaEventElapsedTime(&t, tev[i], tev[i + 1]);
-    fprintf(stderr, " %s=%.4f", names[i], t);
-  }
-  fprintf(stderr, "\n");
+  Layout L(256);
+  L.take((size_t)std::max(numJobs, 1) * sizeof(VerifyState));
+  return L.bytes;
 }
+size_t verify_host_bytes(int numJobs) { return vp_host_jobs_at(numJobs) + (size_t)std::max(numJobs, 1) * sizeof(VerifyJob); }
 
 // Per wave: steps 1-4 (and, with full, 5-8) on the stream, then the wave's states copied to the pinned area.
 // full == false stops after scoring (the models and counts of the last wave stay in scratch).
@@ -1431,7 +1423,7 @@ int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal
   const VerifyLayout L = verify_layout(plan, numLoops, model);
   char *b = static_cast<char *>(scratch);
   VerifyState *h_states = static_cast<VerifyState *>(h_pinned);
-  VerifyJob *h_jobs = reinterpret_cast<VerifyJob *>(static_cast<char *>(h_pinned) + vp_host_states_bytes(numJobs));
+  VerifyJob *h_jobs = reinterpret_cast<VerifyJob *>(static_cast<char *>(h_pinned) + vp_host_jobs_at(numJobs));
   const bool essential = model == VERIFY_ESSENTIAL;
   const int perSample = vp_slots_per_sample(model), slots = perSample * numLoops;
   // the table; the row and score bases count from the first job of each wave
@@ -1505,9 +1497,10 @@ int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal
     CS_CUDA(cudaGetLastError());
     CS_CUDA(cudaMemcpyAsync(h_states + q0, w.st, (size_t)nj * sizeof(VerifyState), cudaMemcpyDeviceToHost, st));
     if (tev) {
+      static const char *const stages[] = {"flags", "compact", "norm", "hyp", "score", "argmax", "refit", "write"};
       int pairs = 0;
       for (int q = q0; q < q0 + nj; q++) pairs += h_jobs[q].numPairs;
-      vp_timing_print(tev, pairs, numLoops, model);
+      report_stage_times(tev, stages, 8, "verify timing model=%d pairs=%d loops=%d", model, pairs, numLoops);
     }
   }
   return 0;

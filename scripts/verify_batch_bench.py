@@ -15,7 +15,6 @@ import argparse
 import ctypes
 import json
 import os
-import re
 import subprocess
 import sys
 
@@ -156,8 +155,8 @@ def parse_split(text):
         if line.startswith("call"):
             rows = []
         elif line.startswith("verify timing"):
-            rows.append({k: 1000.0 * float(v) for k, v in re.findall(r"(\w+)=([0-9.]+)", line)
-                         if k not in ("model", "pairs", "loops")})
+            toks = line.split("[us]:")[1].split()
+            rows.append({toks[i]: float(toks[i + 1]) for i in range(0, len(toks), 2)})
         elif line.startswith("setting "):
             split = {k: round(sum(r[k] for r in rows), 1) for k in rows[0]} if rows else {}
             split["waves"] = len(rows)

@@ -13,7 +13,6 @@ import argparse
 import ctypes
 import json
 import os
-import re
 import subprocess
 import sys
 import time
@@ -65,8 +64,8 @@ def parse_split(text):
     out, rows = {}, []
     for line in text.splitlines():
         if line.startswith("verify timing"):
-            rows.append({k: 1000.0 * float(v) for k, v in re.findall(r"(\w+)=([0-9.]+)", line)
-                         if k not in ("model", "pairs", "loops")})
+            toks = line.split("[us]:")[1].split()
+            rows.append({toks[i]: float(toks[i + 1]) for i in range(0, len(toks), 2)})
         elif line.startswith("input "):
             keep = rows[len(rows) // 2:]
             out[line[6:].strip()] = {k: round(float(np.median([r[k] for r in keep])), 1) for k in keep[0]} if keep else {}
