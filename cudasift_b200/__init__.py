@@ -20,7 +20,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
-           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks"]
+           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -94,6 +94,8 @@ def lib():
         "cs_build_tracks": (ip, [vp, ip, vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_triangulate_tracks": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, c.c_ulonglong,
                                        vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
         "cs_improve_homography": (ip, [vp, ip, vp, ip, fp, fp, fp, c.POINTER(c.c_int)]),
         "cs_lowpass": (ip, [vp, vp, ip, ip, ip, fp]),
@@ -809,6 +811,64 @@ def TriangulateTracks(datas, Ks, Rs, ts, offsets, members, numTrials=256, maxErr
         for buf in bufs:
             buf.free()
     return points, counts, errors, inlier, stats, ms.value
+
+
+class PoseJob(ctypes.Structure):
+    """cs_pose_job: one image to register, its point indices and its per-feature outputs (device pointers)."""
+    _fields_ = [("pts", ctypes.c_void_p), ("n", ctypes.c_int), ("pointOf", ctypes.c_void_p),
+                ("seed", ctypes.c_ulonglong), ("errors", ctypes.c_void_p), ("inlier", ctypes.c_void_p)]
+
+
+def AbsolutePoseBatch(datas, pointOfs, points, Ks, numLoops=1024, maxError=4.0, seeds=None):
+    """The pose of many images against known 3-D points, in one call (cs_absolute_pose_batch): RANSAC over P3P poses,
+    inliers by reprojection error below maxError pixels, one Levenberg-Marquardt refinement.  datas[p] holds image p's
+    records and pointOfs[p] (int, one per record) the point of each feature or < 0, for example
+    trackOf[base_p : base_p + n_p] of BuildTracks; points [P, 3], for example TriangulateTracks' points; Ks [3, 3] per
+    image or one for every image; seeds one per job (default 0, 1, ...).  The point indices and the points go up once
+    each.  Returns (R float64 [J, 3, 3], t [J, 3] with X_c = R X + t (zero without a pose), counts int32 [J], errors: a
+    list of float32 [n_p], inlier: a list of bool [n_p], stats int64 [J, 8] as the header describes them, ms)."""
+    J = len(datas)
+    if len(pointOfs) != J:
+        raise ValueError("pointOfs: one per image, %d, not %d" % (J, len(pointOfs)))
+    K = _per_image(Ks, (3, 3), J, "Ks")
+    P = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+    seeds = np.arange(J, dtype=np.uint64) if seeds is None else np.asarray(seeds, np.uint64).reshape(-1)
+    if len(seeds) != J:
+        raise ValueError("seeds: one per image, %d, not %d" % (J, len(seeds)))
+    ns = [int(d.numPts) for d in datas]
+    idx = [np.asarray(po, np.int64).reshape(-1) for po in pointOfs]
+    for p in range(J):
+        if len(idx[p]) != ns[p]:
+            raise ValueError("pointOfs[%d]: %d entries for %d records" % (p, len(idx[p]), ns[p]))
+    offs = np.concatenate([[0], np.cumsum(ns, dtype=np.int64)]).astype(np.int64)
+    N = int(offs[-1])
+    flat = np.ascontiguousarray(np.concatenate(idx).astype(np.int32)) if N else np.zeros(0, np.int32)
+    R, t = np.zeros((J, 3, 3)), np.zeros((J, 3))
+    counts, stats, ms = np.zeros(J, np.int32), np.zeros((J, 8), np.int64), ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(P.nbytes, 8)), DeviceBuffer(max(4 * N, 4)), DeviceBuffer(max(4 * N, 4)),
+            DeviceBuffer(max(N, 1))]
+    try:
+        if len(P):
+            bufs[0].upload(P)
+        if N:
+            bufs[1].upload(flat)
+        table = (PoseJob * max(J, 1))()
+        for p in range(J):
+            o = int(offs[p])
+            table[p] = PoseJob(datas[p].d_data if ns[p] else None, ns[p], bufs[1].ptr + 4 * o if ns[p] else None,
+                               int(seeds[p]), bufs[2].ptr + 4 * o if ns[p] else None, bufs[3].ptr + o if ns[p] else None)
+        _check(lib().cs_absolute_pose_batch(bufs[0].ptr if len(P) else None, len(P),
+                                            ctypes.addressof(table) if J else None, J, _ptr(K), int(numLoops),
+                                            float(maxError), _ptr(R), _ptr(t), _ptr(counts), _ptr(stats),
+                                            ctypes.byref(ms)), "AbsolutePoseBatch")
+        err = bufs[2].download(np.float32, N) if N else np.zeros(0, np.float32)
+        inl = bufs[3].download(np.uint8, N).astype(bool) if N else np.zeros(0, bool)
+    finally:
+        for buf in bufs:
+            buf.free()
+    errors = [err[offs[p]:offs[p + 1]].copy() for p in range(J)]
+    inlier = [inl[offs[p]:offs[p + 1]].copy() for p in range(J)]
+    return R, t, counts, errors, inlier, stats, ms.value
 
 
 def FindHomography(data, numLoops=1000, minScore=0.85, maxAmbiguity=0.95, thresh=5.0, seed=None):

@@ -934,6 +934,59 @@ static int triangulate_args(const char *fn, const cs_match_set *sets, int numIma
   });
 }
 
+// The arguments of cs_absolute_pose_batch: the counts and tables, every job (named jobs[p]) and its K, the parameters,
+// the outputs, then every per-feature output against the other outputs, every record range, every pointOf and the
+// points (overlap_sweep).
+static int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
+                     const double *Ks, int numLoops, double maxError)
+{
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numJobs > 0 && (!jobs || !Ks)) return arg_error(fn, "numJobs > 0 needs jobs and Ks");
+  if (numPoints < 0) return arg_error(fn, "numPoints must be >= 0");
+  if (numPoints > 0 && !points) return arg_error(fn, "numPoints > 0 needs d_points");
+  if ((reinterpret_cast<uintptr_t>(points) & 7) != 0) return arg_error(fn, "d_points must be 8-byte aligned");
+  char bad[128] = "";
+  for (int p = 0; p < numJobs && !bad[0]; p++) {
+    const cs_pose_job &j = jobs[p];
+    if (j.n < 0) snprintf(bad, sizeof bad, "jobs[%d]: n must be >= 0", p);
+    else if (j.n > 0 && (!j.pts || !j.pointOf)) snprintf(bad, sizeof bad, "jobs[%d]: n > 0 needs pts and pointOf", p);
+    else if ((reinterpret_cast<uintptr_t>(j.pointOf) & 3) != 0 || (reinterpret_cast<uintptr_t>(j.errors) & 3) != 0)
+      snprintf(bad, sizeof bad, "jobs[%d]: pointOf and errors must be 4-byte aligned", p);
+  }
+  if (bad[0]) return arg_error(fn, bad);
+  for (int p = 0; p < numJobs; p++) {
+    char name[96];
+    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
+    const int r = check_intrinsics(name, Ks + 9 * (size_t)p, "Ks[p]");
+    if (r < 0) return r;
+  }
+  if (numLoops < 1 || numLoops > 65536) return arg_error(fn, "numLoops must be in [1, 65536]");
+  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
+  // the per-feature outputs (kind 0 errors, 1 inlier: written), the records (2), pointOf (3) and d_points (4)
+  static const char *const kinds[5] = {"errors", "inlier", "pts", "pointOf", "d_points"};
+  std::vector<SweepRange> rs;
+  rs.reserve(4 * (size_t)numJobs + 1);
+  for (int p = 0; p < numJobs; p++) {
+    const cs_pose_job &j = jobs[p];
+    if (j.n <= 0) continue;
+    if (j.errors) sweep_add(rs, j.errors, (size_t)j.n * sizeof(float), p, 0, true);
+    if (j.inlier) sweep_add(rs, j.inlier, (size_t)j.n, p, 1, true);
+    sweep_add(rs, j.pts, record_bytes(j.n), p, 2, false);
+    sweep_add(rs, j.pointOf, (size_t)j.n * sizeof(int), p, 3, false);
+  }
+  sweep_add(rs, points, (size_t)numPoints * 3 * sizeof(double), 0, 4, false);
+  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
+    const SweepRange &a = x.out && (!y.out || x.owner <= y.owner) ? x : y;
+    const SweepRange &b = &a == &x ? y : x;
+    char na[48], nb[48], msg[160];
+    snprintf(na, sizeof na, "jobs[%d].%s", a.owner, kinds[a.kind]);
+    if (b.kind == 4) snprintf(nb, sizeof nb, "d_points");
+    else snprintf(nb, sizeof nb, "jobs[%d].%s", b.owner, kinds[b.kind]);
+    snprintf(msg, sizeof msg, "%s and %s overlap (a per-feature output overlaps another range)", na, nb);
+    return arg_error(fn, msg);
+  });
+}
+
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
 {
   VerifyCalib cal;
@@ -1815,6 +1868,47 @@ int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double 
   if (stats_out)
     for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
   return (int)st[5];
+}
+
+int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,
+                           const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
+                           int *counts_out, long long *stats_out, double *ms)
+{
+  const char *fn = "cs_absolute_pose_batch";
+  if (ms) *ms = 0.0;
+  int r = pose_args(fn, d_points, numPoints, jobs, numJobs, Ks, numLoops, maxError);
+  if (r < 0) return r;
+  if (numJobs > 0 && (!R_out || !t_out || !counts_out)) return arg_error(fn, "R_out, t_out and counts_out must not be NULL");
+  r = batch_body(fn, numJobs, counts_out, stats_out, 8, ms,
+                 [&](int p) {
+                   for (int k = 0; k < 9; k++) R_out[9 * (size_t)p + k] = 0.0;
+                   for (int k = 0; k < 3; k++) t_out[3 * (size_t)p + k] = 0.0;
+                 },
+                 [&](int p) { return jobs[p].n > 0; },
+                 [&](DeviceCtx *c) { return pose_enqueue(*c, d_points, numPoints, jobs, numJobs, Ks, numLoops, maxError, true); },
+                 [&](DeviceCtx *c, int p, int q, long long *st) {
+                   return pose_result(*c, q, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
+                 });
+  if (r < 0) return r;
+  int posed = 0;
+  for (int p = 0; p < numJobs; p++) posed += counts_out[p] > 0;
+  return posed;
+}
+
+int cs_absolute_pose_models(const double *d_points, int numPoints, const cs_pose_job *job, const double K[9],
+                            int numLoops, double maxError, double *h_R, double *h_t, int *h_counts)
+{
+  const char *fn = "cs_absolute_pose_models";
+  int r = pose_args(fn, d_points, numPoints, job, job ? 1 : 0, K, numLoops, maxError);
+  if (r < 0) return r;
+  if (!job) return arg_error(fn, "job must not be NULL");
+  if (!h_R || !h_t || !h_counts) return arg_error(fn, "NULL output array");
+  if (job->n == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = pose_enqueue(*c, d_points, numPoints, job, 1, K, numLoops, maxError, false)) < 0) return r;
+  return pose_models_to_host(*c, *job, numLoops, h_R, h_t, h_counts);
 }
 
 // ---- stage-level entry points ----

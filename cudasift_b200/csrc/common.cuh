@@ -296,6 +296,10 @@ struct DeviceCtx {
   // cs_triangulate_tracks: the statistics and queue word, the camera table and the spilled members
   GrowBuffer tri;
   PinnedBuffer h_tri;                      // the statistics (copied back), then the camera table
+  // cs_absolute_pose_batch, cs_absolute_pose_models: the job table, then a wave's correspondences, slots, slot counts
+  // and job states
+  GrowBuffer pose;
+  PinnedBuffer h_pose;                     // every job's state (copied back), then the job table
   // cs_verify_*: the states a call copies back, and its job table
   PinnedBuffer h_verify;
 
@@ -473,6 +477,20 @@ int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, c
                         const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
                         int numTrials, double maxError, double minTriAngle, unsigned long long seed, double *points,
                         int *counts, float *errors, unsigned char *inlier);
+
+// ---- absolute pose (pose.cu) ------------------------------------------------------------------------------------
+// cs_absolute_pose_batch's non-empty jobs per wave: floor(256 MiB / (4 numLoops x 100 B)), clamped to [1, 65536].
+int pose_jobs_per_wave(int numLoops);
+// The waves of an argument-checked batch on c.stream, without a synchronize: with full the five launches per wave, else
+// the first three (gather, hypotheses, scoring; the slots of the last wave stay in c.pose).  The q-th non-empty job's
+// state reaches c.h_pose by the caller's synchronize.
+int pose_enqueue(DeviceCtx &c, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
+                 const double *Ks, int numLoops, double maxError, bool full);
+// after a full enqueue and a synchronize: the q-th non-empty job's pose, statistics and count
+int pose_result(const DeviceCtx &c, int q, double R[9], double t[3], long long stats[8]);
+// after an enqueue of one job without full: every slot's R, t (NaN-filled when empty) and count (synchronizes);
+// returns the job's number of valid correspondences
+int pose_models_to_host(DeviceCtx &c, const cs_pose_job &job, int numLoops, double *h_R, double *h_t, int *h_counts);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id launch_verify uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

@@ -138,29 +138,7 @@ __device__ __forceinline__ bool tr_solve(const double (&s)[10], double (&X)[3])
   return isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]);
 }
 
-// u = P (X, 1): the homogeneous pixel, u[2] the depth.  The explicit fma chain pins the arithmetic, so scoring, the
-// refit's count and the member outputs see the same bits.
-__device__ __forceinline__ void tr_project(const double *P, const double (&X)[3], double (&u)[3])
-{
-#pragma unroll
-  for (int i = 0; i < 3; i++) u[i] = fma(P[4 * i], X[0], fma(P[4 * i + 1], X[1], fma(P[4 * i + 2], X[2], P[4 * i + 3])));
-}
-
-// The squared pixel error times the squared depth: (u0 - x u2)^2 + (u1 - y u2)^2.
-__device__ __forceinline__ double tr_err2z2(const double (&u)[3], float x, float y)
-{
-  const double dx = fma(-(double)x, u[2], u[0]), dy = fma(-(double)y, u[2], u[1]);
-  return fma(dx, dx, dy * dy);
-}
-
-// An inlier: depth > 0 and the squared pixel error strictly below maxError^2 (multiplied through by depth^2).
-__device__ __forceinline__ bool tr_inlier(const double *P, const double (&X)[3], float x, float y, double thr2)
-{
-  double u[3];
-  tr_project(P, X, u);
-  return u[2] > 0.0 && tr_err2z2(u, x, y) < thr2 * (u[2] * u[2]);
-}
-
+// tr_project, tr_err2z2 and tr_inlier (the reprojection inlier rule) are in vp_math.cuh.
 __device__ __forceinline__ double tr_depth(const TrCam &c, const double (&X)[3])
 {
   return c.Rt[8] * X[0] + c.Rt[9] * X[1] + c.Rt[10] * X[2] + c.Rt[11];

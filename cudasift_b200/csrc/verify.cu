@@ -43,7 +43,6 @@ namespace cs {
 #define VP_CHUNK 1024         // points per scoring CTA (one tile: more CTAs than models alone would give)
 #define VP_REFIT_T 256
 #define VP_EPS 1e-9           // smallest pivot / collinearity cross product, normalised coordinates (entries of order 1)
-#define VP_MAX_DRAWS 64
 
 struct VerifyState {
   double c1x, c1y, c2x, c2y, s;   // normalisation: u = s * (x - c)
@@ -83,7 +82,7 @@ __device__ __forceinline__ int vp_job_of(const VerifyJob *jobs, int numJobs, int
   return lo;
 }
 
-// ---- shared helpers (host and device); vp_splitmix64, vp_jacobi and vp_calibrate are in vp_math.cuh -----------------
+// ---- shared helpers (host and device); vp_splitmix64, vp_jacobi, vp_calibrate and vp_draw are in vp_math.cuh --------
 __host__ __device__ inline void vp_mul33(const double *a, const double *b, double *c)
 {
   for (int r = 0; r < 3; r++)
@@ -421,27 +420,6 @@ vp_norm_kernel(VerifyWave w, float thresh)
     st->thr2 = (float)(t * t);
     st->best = 0; st->samples = 0; st->models = 0;
   }
-}
-
-// The k distinct indices of sample smp into the n valid pairs (the rule of cs_verify_pairs); false when n < K or after
-// 64 draws.
-template <int K>
-__device__ bool vp_draw(unsigned long long seed, int smp, int n, int (&idx)[K])
-{
-  if (n < K) return false;
-  int got = 0;
-  for (int d = 0; d < VP_MAX_DRAWS && got < K; d++) {
-    const unsigned long long x = vp_splitmix64(seed + 0x9E3779B97F4A7C15ull * (((unsigned long long)smp << 8) | (unsigned)d));
-    const int i = (int)(((x >> 32) * (unsigned long long)n) >> 32);
-    bool dup = false;
-#pragma unroll
-    for (int j = 0; j < K; j++) dup |= (j < got && idx[j] == i);
-    if (dup) continue;
-#pragma unroll
-    for (int j = 0; j < K; j++) if (j == got) idx[j] = i;
-    got++;
-  }
-  return got == K;
 }
 
 __device__ inline double vp_cross(double ax, double ay, double bx, double by, double cx, double cy)

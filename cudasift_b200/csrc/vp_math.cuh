@@ -1,6 +1,7 @@
-// vp_math.cuh -- the FP64 helpers that geometric verification (verify.cu) and triangulation (triangulate.cu) share:
-// the counter-based sampler, the cyclic Jacobi eigen-decomposition and the calibrated coordinates of a pinhole K.
-// tests/verify_oracle.py and tests/triangulate_oracle.py restate them in float64.
+// vp_math.cuh -- the FP64 helpers that geometric verification (verify.cu), triangulation (triangulate.cu) and
+// absolute pose (pose.cu) share: the counter-based generator and sampler, the cyclic Jacobi eigen-decomposition, the
+// calibrated coordinates of a pinhole K and the reprojection inlier rule.  tests/verify_oracle.py and
+// tests/triangulate_oracle.py restate them in float64.
 #pragma once
 
 #include <cmath>
@@ -61,6 +62,53 @@ __host__ __device__ inline void vp_calibrate(const double *K, double x, double y
 {
   cy = (y - K[5]) / K[4];
   cx = (x - K[2] - K[1] * cy) / K[0];
+}
+
+#define VP_MAX_DRAWS 64
+
+// The k distinct indices of sample smp into the n valid items (the rule of cs_verify_pairs); false when n < K or after
+// 64 draws.
+template <int K>
+__device__ bool vp_draw(unsigned long long seed, int smp, int n, int (&idx)[K])
+{
+  if (n < K) return false;
+  int got = 0;
+  for (int d = 0; d < VP_MAX_DRAWS && got < K; d++) {
+    const unsigned long long x = vp_splitmix64(seed + 0x9E3779B97F4A7C15ull * (((unsigned long long)smp << 8) | (unsigned)d));
+    const int i = (int)(((x >> 32) * (unsigned long long)n) >> 32);
+    bool dup = false;
+#pragma unroll
+    for (int j = 0; j < K; j++) dup |= (j < got && idx[j] == i);
+    if (dup) continue;
+#pragma unroll
+    for (int j = 0; j < K; j++) if (j == got) idx[j] = i;
+    got++;
+  }
+  return got == K;
+}
+
+// The reprojection inlier rule of triangulation and absolute pose.  u = P (X, 1) with P = K [R | t] row-major 3 x 4:
+// the homogeneous pixel, u[2] the depth.  The explicit fma chain pins the arithmetic, so scoring, refits and the
+// per-feature outputs see the same bits.
+__device__ __forceinline__ void tr_project(const double *P, const double (&X)[3], double (&u)[3])
+{
+#pragma unroll
+  for (int i = 0; i < 3; i++) u[i] = fma(P[4 * i], X[0], fma(P[4 * i + 1], X[1], fma(P[4 * i + 2], X[2], P[4 * i + 3])));
+}
+
+// The squared pixel error times the squared depth: (u0 - x u2)^2 + (u1 - y u2)^2.
+__device__ __forceinline__ double tr_err2z2(const double (&u)[3], float x, float y)
+{
+  const double dx = fma(-(double)x, u[2], u[0]), dy = fma(-(double)y, u[2], u[1]);
+  return fma(dx, dx, dy * dy);
+}
+
+// An inlier: depth > 0 and the squared pixel error strictly below maxError^2 (multiplied through by depth^2).
+__device__ __forceinline__ bool tr_inlier(const double *P, const double (&X)[3], float x, float y, double thr2)
+{
+  double u[3];
+  tr_project(P, X, u);
+  return u[2] > 0.0 && tr_err2z2(u, x, y) < thr2 * (u[2] * u[2]);
 }
 
 }  // namespace cs

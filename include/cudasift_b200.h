@@ -508,6 +508,95 @@ int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double 
                           double maxError, double minTriAngle, unsigned long long seed, double *d_points, int *d_counts,
                           float *d_errors, unsigned char *d_inlier, long long stats_out[8], double *ms);
 
+/* Camera registration against known 3-D points (COLMAP's image_registrator, OpenCV's solvePnPRansac), many images in
+ * one call: per job, RANSAC over Lambda Twist P3P poses (Persson & Nordberg, ECCV 2018) in FP64, the inliers by the
+ * reprojection rule of cs_triangulate_tracks, then one Levenberg-Marquardt refinement.  cs_build_tracks' d_trackOf
+ * (offset by the image's global base) and cs_triangulate_tracks' d_points go in unchanged, and R, t come out in the
+ * convention cs_triangulate_tracks takes. */
+typedef struct cs_pose_job {
+  const void *pts; int n;          /* device SiftPoint records of the image to register */
+  const int *pointOf;              /* device int[n]: the 3-D point of feature f, or < 0 for none */
+  unsigned long long seed;
+  float *errors;                   /* device float[n] or NULL: pixel error of every feature under the final pose */
+  unsigned char *inlier;           /* device byte[n] or NULL: 1 for a final inlier */
+} cs_pose_job;
+/* - Correspondences: feature f of job p is valid when 0 <= pointOf[f] < numPoints, the three coordinates of that
+ *   point are finite and the record's xpos and ypos are finite (so triangulation's NaN rows, "no point", are skipped).
+ *   V is the number of valid correspondences; ranks 0 .. V-1 index them in feature order.  Features may share a point.
+ *   A feature with pointOf[f] >= 0 that is not valid is counted as invalid.
+ * - K (Ks[p], row-major) follows cs_verify_essential's rule.  The bearing of a correspondence is (x^, y^, 1) divided by
+ *   sqrt(x^ x^ + y^ y^ + 1), computed in double, with x^, y^ the calibrated coordinates of cs_verify_essential.
+ * - Sampler: cs_verify_pairs' rule with 3 distinct draws over the V ranks: draw d of sample s is
+ *   ((x >> 32) * V) >> 32 with x = splitmix64(seed + 0x9E3779B97F4A7C15 * ((s << 8) | d)), repeats skipped, at most
+ *   64 draws; samples s = 0 .. numLoops-1.  Y_k, X_k (k = 0, 1, 2) are the bearings and world points in draw order.
+ * - Minimal solver (FP64): d12 = X0 - X1, d13 = X0 - X2, d23 = X1 - X2, aij = |dij|^2, n = d12 x d13;
+ *   cij = Yi . Yj, sij = 1 - cij^2, bij = -2 cij.  The sample is degenerate when |n|^2 <= 1e-10 a12 a13 (collinear
+ *   world points) or some sij <= 1e-10 (near-parallel bearings).  With blob = c12 c23 c13 - 1:
+ *     p3 = a13 (a23 s13 - a13 s23),
+ *     p2 = 2 blob a23 a13 + a13 (2 a12 + a13) s23 + a23 (a23 - a12) s13,
+ *     p1 = a23 (a13 - a23) s12 - a12^2 s23 - 2 a12 (blob a23 + a13 s23),
+ *     p0 = a12 (a12 s23 - a23 s12);
+ *   p3 == 0 is degenerate.  g is the largest real root of g^3 + (p2/p3) g^2 + (p1/p3) g + p0/p3: the closed form
+ *   (Cardano when the discriminant q^2/4 + p^3/27 of the depressed cubic is >= 0, else 2 sqrt(-p/3) cos(acos(...)/3)),
+ *   then 2 Newton steps, each taken when the derivative is nonzero and the result finite.  D0 = D1 - g D2 is
+ *     [a23 (1 - g),  a23 b12 / 2,          -a23 b13 g / 2;
+ *      .,            a23 - a12 + a13 g,    b23 (a13 g - a12) / 2;
+ *      .,            .,                    g (a13 - a23) - a12]  (symmetric; a non-finite entry is degenerate),
+ *   decomposed by the cyclic Jacobi of the verifiers (vp_jacobi<3>, not the closed form with the known zero
+ *   eigenvalue).  e0, e1 are its eigenvalues of largest and second largest magnitude (the lower index first on ties),
+ *   u0, u1 their eigenvectors; e0 == 0 is degenerate; v = sqrt(max(0, -e1 / e0)).  For s = +v, then s = -v:
+ *   w2 = 1 / (s u1[0] - u0[0]), w0 = (u0[1] - s u1[1]) w2, w1 = (u0[2] - s u1[2]) w2 (so l1 = w0 l2 + w1 l3), and the
+ *   quadratic tau^2 + B tau + C = 0 with qa = 1 / ((a13 - a12) w1^2 - a12 b13 w1 - a12),
+ *   B = (a13 b12 w1 - a12 b13 w0 - 2 w0 w1 (a12 - a13)) qa, C = ((a13 - a12) w0^2 + a13 b12 w0 + a13) qa.  When
+ *   B^2 - 4 C >= 0: tau1 = (-B + sqrt) / 2 if B < 0 else (-B - sqrt) / 2, tau2 = C / tau1 (NaN when tau1 == 0); for
+ *   tau1, then tau2, when tau > 0 and dd = a23 / (tau (b23 + tau) + 1) > 0: l2 = sqrt(dd), l3 = tau l2,
+ *   l1 = w0 l2 + w1 l3, kept when l1 > 0.  Each kept (l1, l2, l3) takes up to 5 Newton steps on the three equations
+ *   li^2 + lj^2 + bij li lj = aij (the 3x3 Jacobian inverted by its adjugate; a step is taken only when its
+ *   determinant is nonzero and the result is finite and lowers |r12| + |r13| + |r23|, else the steps stop), and is
+ *   dropped unless all three are finite and > 0.  Alignment: with Ck = lk Yk, R = [C0 - C1, C0 - C2, (C0 - C1) x
+ *   (C0 - C2)] [d12, d13, n]^-1 (the inverse's rows (d13 x n, n x d12, d12 x d13) / (d12 . (d13 x n))),
+ *   t = C0 - R X0; a pose with a non-finite entry is dropped.  Slot sample*4 + r holds the r-th remaining pose; a
+ *   degenerate sample is one with fewer than 3 distinct draws or one that trips a test above.
+ * - Inlier (FP64, exactly cs_triangulate_tracks' test and fma chain): depth d = (R X + t)_2 > 0 and
+ *   (u0 - x d)^2 + (u1 - y d)^2 < maxError^2 d^2, (u0, u1, d) = K (R X + t), through P = K [R | t].
+ * - Winner: the slot with the most inliers, the lowest slot on ties.
+ * - Refinement, once, when the winner has at least 3 inliers: Levenberg-Marquardt on the sum of squared pixel
+ *   residuals (K0 a + K1 b + K2 - x, K4 b + K5 - y), (a, b) = (Xc0, Xc1) / Xc2, Xc = R X + t, over the winner's
+ *   inliers in rank order.  Update R <- exp([w]x) R, t <- exp([w]x) t + delta (Rodrigues, I + A [w]x + B [w]x^2 with
+ *   A = sin th / th, B = 2 sin^2(th / 2) / th^2, A = 1, B = 1/2 at th = 0), so the Jacobian row of a residual with
+ *   gradient gr = d(pixel) / d(Xc) is (Xc x gr, gr): gr_x = (K0, K1, -(K0 a + K1 b)) / Xc2, gr_y = (0, K4, -K4 b) / Xc2.
+ *   The 28 sums per residual, x then y of each correspondence: H = J^T J (21, upper triangle row by row), g = J^T r
+ *   (6), the cost r^T r.  The step solves (H + lambda diag(H)) step = -g by Cholesky (a pivot not > 0 or not finite
+ *   rejects the step); lambda starts at 1e-3, x10 on a rejected step, /10 on an accepted one.  A step is accepted when
+ *   every residual point stays in front (Xc2 > 0) and the cost decreases.  At most 20 iterations; it stops after an
+ *   accepted step whose largest |component| is <= 1e-12 or whose cost decrease is <= 1e-12 of the previous cost.  The
+ *   refined pose is kept unless it is not finite or has fewer inliers than the winner.
+ * - Outputs: R_out[p] (row-major), t_out[p] with X_c = R X + t; counts_out[p] the final inlier count.  A job without
+ *   a pose (V < 3, no pose scored, or a final count < 3) gets zero R and t and count 0.  Per feature, when the buffer
+ *   is given: errors[f] = (float)sqrt(e2), e2 the squared pixel error under the final pose, +inf when its depth is
+ *   <= 0, NaN for a feature that is not a valid correspondence or in a job without a pose; inlier[f] = 1 for a final
+ *   inlier, else 0.  stats_out[p] (may be NULL): [0] valid correspondences, [1] invalid ones, [2] non-degenerate
+ *   samples, [3] poses scored, [4] the winning slot (-1 if none), [5] its count, [6] 1 when the refinement was kept,
+ *   [7] the final count (counts_out[p]).
+ * - Returns the number of jobs with a pose, or CS_E_*.
+ * - Batch: jobs do not interact; permuting the jobs permutes the results, a job's results are bit-identical alone or
+ *   in any batch, and two calls give the same bytes.  Empty jobs (n == 0) get zero outputs and statistics and launch
+ *   nothing; numJobs == 0 returns 0 before any CUDA call.  Sums of the refinement run per lane of a warp and combine
+ *   by a fixed butterfly, so they agree with a float64 statement of these rules to rounding, not bit for bit.
+ * - CS_E_ARG, before any CUDA call, naming the offending jobs[p] in cs_last_error(): numJobs outside [0, 65536], NULL
+ *   jobs or Ks with numJobs > 0, numPoints < 0, NULL d_points with numPoints > 0, d_points not 8-byte aligned, n < 0,
+ *   NULL pts or pointOf with n > 0, pointOf or errors not 4-byte aligned, an invalid Ks[p], numLoops outside
+ *   [1, 65536], maxError not finite or <= 0, NULL R_out, t_out or counts_out with numJobs > 0, and a per-feature
+ *   output that overlaps another output, any record range, any pointOf or d_points (one sweep over sorted ranges).
+ * - Waves: the non-empty jobs, in order, run in waves of floor(256 MiB / (4 x numLoops x 100 B)) jobs (clamped to
+ *   [1, 65536]; a slot is 12 doubles and a count).  Each wave issues 5 kernel launches (gather, hypotheses, score,
+ *   arg-max, refine), so a batch issues 5 x waves (cs_launch_count).  The call synchronises with the host once, at
+ *   the end; its scratch lives in the per-device context.  *ms (may be NULL) gets the event time of the call.
+ * d_points [numPoints][3]; Ks [J][9]; R_out [J][9], t_out [J][3], counts_out [J]; stats_out [J][8] or NULL. */
+int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,
+                           const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
+                           int *counts_out, long long *stats_out, double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
@@ -553,6 +642,12 @@ int cs_verify_models(const void *d_s1, int n1, const void *d_s2, int n2, const i
 int cs_verify_essential_models(const void *d_s1, int n1, const void *d_s2, int n2, const int *d_pairs, int numPairs,
                                const double K1[9], const double K2[9], int numLoops, float thresh,
                                unsigned long long seed, double *h_models, int *h_counts, double h_norm[5]);
+/* The steps of cs_absolute_pose_batch up to scoring for one job, with its argument checks (K the job's intrinsics):
+ * h_R[4*numLoops][9], h_t[4*numLoops][3] receive every slot's pose (NaN-filled when the slot is empty) and
+ * h_counts[4*numLoops] every slot's inlier count.  Returns V, the job's number of valid correspondences (0 for n == 0,
+ * with no CUDA call and the outputs untouched). */
+int cs_absolute_pose_models(const double *d_points, int numPoints, const cs_pose_job *job, const double K[9],
+                            int numLoops, double maxError, double *h_R, double *h_t, int *h_counts);
 
 /* ---- pipelined extractor (extension; the reference API is strictly synchronous) ----
  * One extractor = one CUDA stream + arena + SiftPoint array + pinned staging.  Several
