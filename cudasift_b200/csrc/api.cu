@@ -589,14 +589,6 @@ static int essential_args(const char *fn, const void *s1, int n1, const void *s2
   return check_intrinsics(fn, K2, "K2");
 }
 
-// The verifier's scratch and the pinned area of its states and job table, for a batch (or a single call: one job).
-static int verify_buffers(DeviceCtx *c, const cs_verify_job *jobs, int numJobs, int numLoops, int model)
-{
-  int r;
-  if ((r = c->verify.grow(verify_scratch_bytes(jobs, numJobs, numLoops, model))) < 0) return r;
-  return c->h_verify.grow(verify_host_bytes(numJobs));
-}
-
 static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, const int *pairs, int numPairs,
                                 unsigned long long seed, int *inliers, int maxInliers)
 {
@@ -606,20 +598,11 @@ static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2
   return j;
 }
 
-// The launches of a batch (cal: per job, essential only), without a synchronize.
-static int verify_enqueue(DeviceCtx *c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model,
-                          int numLoops, float thresh)
-{
-  int r;
-  if ((r = verify_buffers(c, jobs, numJobs, numLoops, model)) < 0) return r;
-  return launch_verify(jobs, numJobs, cal, model, numLoops, thresh, c->verify.p, c->h_verify.p, true, c->stream);
-}
-
-// The same, one synchronize.
+// The launches of a batch (cal: per job, essential only) and one synchronize.
 static int verify_batch_sync(const char *fn, DeviceCtx *c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal,
                              int model, int numLoops, float thresh, double *ms)
 {
-  return timed_sync(fn, c, ms, [&] { return verify_enqueue(c, jobs, numJobs, cal, model, numLoops, thresh); });
+  return timed_sync(fn, c, ms, [&] { return verify_enqueue(*c, jobs, numJobs, cal, model, numLoops, thresh, true); });
 }
 
 // The shared path of cs_verify_pairs_host and cs_verify_essential_host: the sets and the input pairs uploaded, then
@@ -676,11 +659,8 @@ static int verify_models_sync(DeviceCtx *c, const cs_verify_job &job, const Veri
                               float thresh, double *h_models, int *h_counts, double h_norm[5])
 {
   int r;
-  if ((r = verify_buffers(c, &job, 1, numLoops, model)) < 0) return r;
-  if ((r = launch_verify(&job, 1, cal, model, numLoops, thresh, c->verify.p, c->h_verify.p, false, c->stream)) < 0)
-    return r;
-  return verify_models_to_host(c->verify.p, c->h_verify.p, job, numLoops, model, cal, h_models, h_counts, h_norm,
-                               c->stream);
+  if ((r = verify_enqueue(*c, &job, 1, cal, model, numLoops, thresh, false)) < 0) return r;
+  return verify_models_to_host(*c, job, numLoops, model, cal, h_models, h_counts, h_norm);
 }
 
 // The arguments of cs_verify_pairs_batch (cal_args false) and cs_verify_essential_batch: the common ones, then every
@@ -1587,7 +1567,7 @@ int cs_verify_pairs(const void *d_s1, int n1, const void *d_s2, int n2, const in
   const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
                                        d_inliers, maxInliers);
   if ((r = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms)) < 0) return r;
-  return verify_result(c->h_verify.p, 0, numPairs, model_out, c->verifyStats);
+  return verify_result(*c, 0, numPairs, model_out, c->verifyStats);
 }
 
 int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs, int model,
@@ -1606,7 +1586,7 @@ int cs_verify_pairs_host(const void *h_s1, int n1, const void *h_s2, int n2, con
   return verify_host_pairs(c, h_s1, n1, h_s2, n2, h_pairs, numPairs, seed, h_inliers, maxInliers,
                            [&](const cs_verify_job &job) {
                              const int q = verify_batch_sync(fn, c, &job, 1, nullptr, model, numLoops, thresh, ms);
-                             return q < 0 ? q : verify_result(c->h_verify.p, 0, numPairs, model_out, c->verifyStats);
+                             return q < 0 ? q : verify_result(*c, 0, numPairs, model_out, c->verifyStats);
                            });
 }
 
@@ -1661,7 +1641,7 @@ int cs_verify_essential(const void *d_s1, int n1, const void *d_s2, int n2, cons
   const cs_verify_job job = verify_job((const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2, d_pairs, numPairs, seed,
                                        d_inliers, maxInliers);
   if ((r = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms)) < 0) return r;
-  return verify_essential_result(c->h_verify.p, 0, numPairs, E_out, R_out, t_out, c->essentialStats);
+  return verify_essential_result(*c, 0, numPairs, E_out, R_out, t_out, c->essentialStats);
 }
 
 int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2, const int *h_pairs, int numPairs,
@@ -1683,7 +1663,7 @@ int cs_verify_essential_host(const void *h_s1, int n1, const void *h_s2, int n2,
   return verify_host_pairs(c, h_s1, n1, h_s2, n2, h_pairs, numPairs, seed, h_inliers, maxInliers,
                            [&](const cs_verify_job &job) {
                              const int q = verify_batch_sync(fn, c, &job, 1, &cal, VERIFY_ESSENTIAL, numLoops, thresh, ms);
-                             return q < 0 ? q : verify_essential_result(c->h_verify.p, 0, numPairs, E_out, R_out, t_out,
+                             return q < 0 ? q : verify_essential_result(*c, 0, numPairs, E_out, R_out, t_out,
                                                                         c->essentialStats);
                            });
 }
@@ -1728,9 +1708,9 @@ int cs_verify_pairs_batch(const cs_verify_job *jobs, int numJobs, int model, int
   return batch_body(fn, numJobs, counts_out, stats_out, 8, ms,
                     [&](int p) { for (int k = 0; k < 9; k++) models_out[9 * (size_t)p + k] = 0.0; },
                     [&](int p) { return jobs[p].numPairs > 0; },
-                    [&](DeviceCtx *c) { return verify_enqueue(c, jobs, numJobs, nullptr, model, numLoops, thresh); },
+                    [&](DeviceCtx *c) { return verify_enqueue(*c, jobs, numJobs, nullptr, model, numLoops, thresh, true); },
                     [&](DeviceCtx *c, int p, int q, long long *st) {
-                      return verify_result(c->h_verify.p, q, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
+                      return verify_result(*c, q, jobs[p].numPairs, models_out + 9 * (size_t)p, st);
                     });
 }
 
@@ -1750,10 +1730,10 @@ int cs_verify_essential_batch(const cs_verify_job *jobs, int numJobs, const doub
                     [&](int p) { essential_zero(E_out + 9 * (size_t)p, R_out + 9 * (size_t)p, t_out + 3 * (size_t)p); },
                     [&](int p) { return jobs[p].numPairs > 0; },
                     [&](DeviceCtx *c) {
-                      return verify_enqueue(c, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh);
+                      return verify_enqueue(*c, jobs, numJobs, cal.data(), VERIFY_ESSENTIAL, numLoops, thresh, true);
                     },
                     [&](DeviceCtx *c, int p, int q, long long *st) {
-                      return verify_essential_result(c->h_verify.p, q, jobs[p].numPairs, E_out + 9 * (size_t)p,
+                      return verify_essential_result(*c, q, jobs[p].numPairs, E_out + 9 * (size_t)p,
                                                      R_out + 9 * (size_t)p, t_out + 3 * (size_t)p, st);
                     });
 }

@@ -5,7 +5,9 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstdint>
+#include <algorithm>
 #include <map>
+#include <vector>
 
 #include "../../include/cudaSift.h"
 #include "../../include/cudasift_b200.h"
@@ -239,6 +241,51 @@ struct Layout {
     return at;
   }
 };
+
+// ---- the waves of a batched RANSAC call (verify.cu, pose.cu) --------------------------------------------------------
+// A wave holds floor(256 MiB / slotBytes) jobs, slotBytes being one job's model slots and their counts, clamped to
+// [1, 65536].
+constexpr size_t RANSAC_WAVE_BYTES = (size_t)256 << 20;
+inline int ransac_jobs_per_wave(size_t slotBytes)
+{
+  const size_t k = RANSAC_WAVE_BYTES / slotBytes;
+  return k < 1 ? 1 : k > 65536 ? 65536 : (int)k;
+}
+
+// The waves of a batch: its non-empty jobs (extent > 0) in input order (live[q] is the input index of the q-th), cut
+// into runs of perWave jobs (the last run may be shorter); extent is the largest sum of the per-job extents of a wave.
+struct WavePlan {
+  std::vector<int> live;
+  int perWave = 1;
+  size_t extent = 0;
+};
+template <class Job, class Extent>
+WavePlan wave_plan(const Job *jobs, int numJobs, size_t slotBytes, Extent &&extent)
+{
+  WavePlan p;
+  p.perWave = ransac_jobs_per_wave(slotBytes);
+  for (int k = 0; k < numJobs; k++)
+    if (extent(jobs[k]) > 0) p.live.push_back(k);
+  for (size_t q0 = 0; q0 < p.live.size(); q0 += p.perWave) {
+    size_t n = 0;
+    for (size_t q = q0; q < std::min(p.live.size(), q0 + p.perWave); q++) n += extent(jobs[p.live[q]]);
+    p.extent = std::max(p.extent, n);
+  }
+  return p;
+}
+
+// The pinned area of a batch, grown in h: one State per non-empty job (the q-th's at q), then the job table.
+template <class State, class Job>
+int pinned_states_and_jobs(PinnedBuffer &h, int live, State *&states, Job *&jobs)
+{
+  Layout L(256);
+  L.take((size_t)std::max(live, 1) * sizeof(State));
+  int r;
+  if ((r = h.grow(L.bytes + (size_t)live * sizeof(Job))) < 0) return r;
+  states = h.as<State>();
+  jobs = reinterpret_cast<Job *>(h.as<char>() + L.bytes);
+  return 0;
+}
 
 struct Pipeline;    // extraction, batched and round-1 kernels (pipeline2.h)
 struct PipeKey {
@@ -479,8 +526,6 @@ int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, c
                         int *counts, float *errors, unsigned char *inlier);
 
 // ---- absolute pose (pose.cu) ------------------------------------------------------------------------------------
-// cs_absolute_pose_batch's non-empty jobs per wave: floor(256 MiB / (4 numLoops x 100 B)), clamped to [1, 65536].
-int pose_jobs_per_wave(int numLoops);
 // The waves of an argument-checked batch on c.stream, without a synchronize: with full the five launches per wave, else
 // the first three (gather, hypotheses, scoring; the slots of the last wave stay in c.pose).  The q-th non-empty job's
 // state reaches c.h_pose by the caller's synchronize.
@@ -493,29 +538,27 @@ int pose_result(const DeviceCtx &c, int q, double R[9], double t[3], long long s
 int pose_models_to_host(DeviceCtx &c, const cs_pose_job &job, int numLoops, double *h_R, double *h_t, int *h_counts);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
-// The model id launch_verify uses for cs_verify_essential (not a model value of the public cs_verify_pairs).
+// The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).
 #define VERIFY_ESSENTIAL 3
 // The intrinsics of an essential call (row-major, checked by the caller).
 struct VerifyCalib {
   double K1[9], K2[9];
 };
-// A batch of jobs (one for a single call) runs in waves: its non-empty jobs in order, verify_jobs_per_wave() at a time.
-int verify_jobs_per_wave(int numLoops, int model);
-size_t verify_scratch_bytes(const cs_verify_job *jobs, int numJobs, int numLoops, int model);   // device scratch
-size_t verify_host_bytes(int numJobs);                     // the pinned area: the states copied back, the job table
-// Per wave steps 1-4, and with full also 5-8 (arg-max, refit, output), then the wave's state copy to h_pinned, all on
-// the stream.  cal (numJobs entries) is read for VERIFY_ESSENTIAL only.
-int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model, int numLoops, float thresh,
-                  void *scratch, void *h_pinned, bool full, cudaStream_t st);
-// after a full launch and a synchronize: the q-th non-empty job's inlier count, pixel model and statistics
-int verify_result(const void *h_pinned, int q, int numPairs, double model_out[9], long long stats[8]);
-// the same after a full VERIFY_ESSENTIAL launch: E, R, t and the ten statistics of cs_verify_essential_stats
-int verify_essential_result(const void *h_pinned, int q, int numPairs, double E[9], double R[9], double t[3],
+// The waves of an argument-checked batch (one job for a single call) on c.stream, without a synchronize: per wave steps
+// 1-4, and with full also 5-8 (arg-max, refit, output; without full the slots of the last wave stay in c.verify).  The
+// q-th non-empty job's state reaches c.h_verify by the caller's synchronize.  cal (numJobs entries) is read for
+// VERIFY_ESSENTIAL only.
+int verify_enqueue(DeviceCtx &c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model, int numLoops,
+                   float thresh, bool full);
+// after a full enqueue and a synchronize: the q-th non-empty job's inlier count, pixel model and statistics
+int verify_result(const DeviceCtx &c, int q, int numPairs, double model_out[9], long long stats[8]);
+// the same after a full VERIFY_ESSENTIAL enqueue: E, R, t and the ten statistics of cs_verify_essential_stats
+int verify_essential_result(const DeviceCtx &c, int q, int numPairs, double E[9], double R[9], double t[3],
                             long long stats[10]);
-// after a launch of one job without full: every slot's pixel model (E for VERIFY_ESSENTIAL), count and the
+// after an enqueue of one job without full: every slot's pixel model (E for VERIFY_ESSENTIAL), count and the
 // normalisation (synchronizes); returns numValid
-int verify_models_to_host(const void *scratch, const void *h_pinned, const cs_verify_job &job, int numLoops, int model,
-                          const VerifyCalib *cal, double *h_models, int *h_counts, double h_norm[5], cudaStream_t st);
+int verify_models_to_host(DeviceCtx &c, const cs_verify_job &job, int numLoops, int model, const VerifyCalib *cal,
+                          double *h_models, int *h_counts, double h_norm[5]);
 
 inline int idivup(int a, int b) { return (a + b - 1) / b; }
 inline int ialignup(int a, int b) { return (a % b != 0) ? (a - a % b + b) : a; }

@@ -41,7 +41,6 @@ constexpr double PS_EPS = 1e-10;     // degeneracy thresholds: collinear world p
 constexpr int PS_GN_STEPS = 5;
 constexpr int PS_LM_ITERS = 20;
 constexpr double PS_LM_LAMBDA0 = 1e-3, PS_LM_STEP_TOL = 1e-12, PS_LM_COST_TOL = 1e-12;
-constexpr size_t PS_WAVE_BYTES = (size_t)256 << 20;
 
 // A valid correspondence: its world point, bearing, pixel and feature index.
 struct PoseCorr {
@@ -308,13 +307,9 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pose_gather_kernel(PoseWave w)
 
 __global__ void __launch_bounds__(PS_HYP_T) pose_hyp_kernel(PoseWave w)
 {
-  const int per = (w.numLoops + PS_HYP_T - 1) / PS_HYP_T, j = blockIdx.x / per;
-  const int smp = (blockIdx.x - j * per) * PS_HYP_T + threadIdx.x;
-  if (smp >= w.numLoops) return;
-  const size_t S = (size_t)PS_SLOTS * w.numLoops;
-  double *slot = w.slots + ((size_t)j * S + (size_t)PS_SLOTS * smp) * PS_SLOT_DOUBLES;
-  unsigned int *cnt = w.slotCounts + (size_t)j * S + PS_SLOTS * smp;
-  for (int r = 0; r < PS_SLOTS; r++) { slot[PS_SLOT_DOUBLES * r] = CUDART_NAN; cnt[r] = 0; }
+  int j, smp;
+  double *slot;
+  if (!vp_hyp_sample<PS_HYP_T, PS_SLOTS, PS_SLOT_DOUBLES>(w.numLoops, w.slots, w.slotCounts, j, smp, slot)) return;
   const PoseJobDev &job = w.jobs[j];
   int idx[3];
   if (!vp_draw<3>(job.seed, smp, w.st[j].V, idx)) return;
@@ -374,17 +369,7 @@ __global__ void __launch_bounds__(256) pose_argmax_kernel(PoseWave w)
   const int S = PS_SLOTS * w.numLoops, per = (S + 255) / 256, j = blockIdx.x / per;
   const int slot = (blockIdx.x - j * per) * 256 + threadIdx.x;
   const bool live = slot < S && !isnan(w.slots[((size_t)j * S + slot) * PS_SLOT_DOUBLES]);
-  unsigned long long key = live ? ((unsigned long long)w.slotCounts[(size_t)j * S + slot] << 32) | (unsigned int)~slot : 0ull;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
-    key = t > key ? t : key;
-  }
-  const unsigned int nl = __popc(__ballot_sync(0xffffffffu, live));
-  if ((threadIdx.x & 31) == 0) {
-    if (key) atomicMax(&w.st[j].best, key);
-    if (nl) atomicAdd(&w.st[j].poses, (unsigned long long)nl);
-  }
+  vp_argmax_warp(live, w.slotCounts + (size_t)j * S + slot, slot, &w.st[j].best, &w.st[j].poses);
 }
 
 constexpr int PS_SUMS = 28;          // H (21, upper triangle row by row), g (6), the cost
@@ -591,26 +576,11 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pose_refine_kernel(PoseWave w)
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------
-// The waves of a batch: its non-empty jobs in input order (live[q] is the input index of the q-th), cut into runs of
-// perWave jobs; corr is the largest record count of a wave.
-struct PosePlan {
-  std::vector<int> live;
-  int perWave = 1;
-  size_t corr = 0;
-};
-
-PosePlan pose_plan(const cs_pose_job *jobs, int numJobs, int numLoops)
+// The waves of a batch, a job's extent being its correspondence count.
+WavePlan pose_plan(const cs_pose_job *jobs, int numJobs, int numLoops)
 {
-  PosePlan p;
-  p.perWave = pose_jobs_per_wave(numLoops);
-  for (int k = 0; k < numJobs; k++)
-    if (jobs[k].n > 0) p.live.push_back(k);
-  for (size_t q0 = 0; q0 < p.live.size(); q0 += p.perWave) {
-    size_t n = 0;
-    for (size_t q = q0; q < std::min(p.live.size(), q0 + p.perWave); q++) n += jobs[p.live[q]].n;
-    p.corr = std::max(p.corr, n);
-  }
-  return p;
+  const size_t slotBytes = (size_t)PS_SLOTS * numLoops * (PS_SLOT_DOUBLES * sizeof(double) + sizeof(unsigned int));
+  return wave_plan(jobs, numJobs, slotBytes, [](const cs_pose_job &a) { return (size_t)a.n; });
 }
 
 struct PoseLayout {
@@ -618,14 +588,14 @@ struct PoseLayout {
 };
 
 // The device table of the batch's non-empty jobs, then the scratch of one wave (reused by the next).
-PoseLayout pose_layout(const PosePlan &p, int numLoops)
+PoseLayout pose_layout(const WavePlan &p, int numLoops)
 {
   PoseLayout L;
   Layout o(256);
   const size_t live = std::max(p.live.size(), (size_t)1), J = std::min(live, (size_t)p.perWave);
   const size_t S = (size_t)PS_SLOTS * numLoops * J;
   L.jobs = o.take(live * sizeof(PoseJobDev));
-  L.corr = o.take(std::max(p.corr, (size_t)1) * sizeof(PoseCorr));
+  L.corr = o.take(std::max(p.extent, (size_t)1) * sizeof(PoseCorr));
   L.slots = o.take(S * PS_SLOT_DOUBLES * sizeof(double));
   L.slotCounts = o.take(S * sizeof(unsigned int));
   L.state = o.take(J * sizeof(PoseState));
@@ -633,37 +603,21 @@ PoseLayout pose_layout(const PosePlan &p, int numLoops)
   return L;
 }
 
-// The pinned area: one state per non-empty job, then from the returned offset the job table.
-size_t pose_host_jobs_at(int numJobs)
-{
-  Layout L(256);
-  L.take((size_t)std::max(numJobs, 1) * sizeof(PoseState));
-  return L.bytes;
-}
-
 }  // namespace
-
-int pose_jobs_per_wave(int numLoops)
-{
-  const size_t perJob = (size_t)PS_SLOTS * numLoops * (PS_SLOT_DOUBLES * sizeof(double) + sizeof(unsigned int));
-  const size_t k = PS_WAVE_BYTES / perJob;
-  return k < 1 ? 1 : k > 65536 ? 65536 : (int)k;
-}
 
 int pose_enqueue(DeviceCtx &c, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
                  const double *Ks, int numLoops, double maxError, bool full)
 {
-  const PosePlan plan = pose_plan(jobs, numJobs, numLoops);
+  const WavePlan plan = pose_plan(jobs, numJobs, numLoops);
   const int live = (int)plan.live.size();
   if (live == 0) return 0;
   const PoseLayout L = pose_layout(plan, numLoops);
   int r;
   if ((r = c.pose.grow(L.bytes)) < 0) return r;
-  const size_t jobsAt = pose_host_jobs_at(live);
-  if ((r = c.h_pose.grow(jobsAt + (size_t)live * sizeof(PoseJobDev))) < 0) return r;
+  PoseState *h_states;
+  PoseJobDev *h_jobs;
+  if ((r = pinned_states_and_jobs(c.h_pose, live, h_states, h_jobs)) < 0) return r;
   char *b = c.pose.as<char>();
-  PoseState *h_states = c.h_pose.as<PoseState>();
-  PoseJobDev *h_jobs = reinterpret_cast<PoseJobDev *>(c.h_pose.as<char>() + jobsAt);
   // the table; the correspondence and score bases count from the first job of each wave
   int corrBase = 0, scoreBase = 0;
   for (int q = 0; q < live; q++) {

@@ -71,17 +71,6 @@ struct VerifyJob {
   VerifyCalib cal;                // read by the essential kernels only
 };
 
-// The job whose CTA range holds cta: the last j with jobs[j].*base <= cta (bases ascending, every range non-empty).
-__device__ __forceinline__ int vp_job_of(const VerifyJob *jobs, int numJobs, int cta, int VerifyJob::*base)
-{
-  int lo = 0, hi = numJobs - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (jobs[mid].*base <= cta) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
 // ---- shared helpers (host and device); vp_splitmix64, vp_jacobi, vp_calibrate and vp_draw are in vp_math.cuh --------
 __host__ __device__ inline void vp_mul33(const double *a, const double *b, double *c)
 {
@@ -321,7 +310,7 @@ __device__ __forceinline__ VerifyJobScratch vp_job_scratch(const VerifyWave &w, 
 __global__ void __launch_bounds__(VP_ROWS)
 vp_flags_kernel(VerifyWave w)
 {
-  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::rowBase);
+  const int j = table_find(w.jobs, w.numJobs, &VerifyJob::rowBase, (int)blockIdx.x);
   const VerifyJob &job = w.jobs[j];
   const VerifyJobScratch js = vp_job_scratch(w, j);
   const SiftPoint *__restrict__ s1 = job.s1, *__restrict__ s2 = job.s2;
@@ -343,7 +332,7 @@ vp_flags_kernel(VerifyWave w)
 __global__ void __launch_bounds__(VP_ROWS)
 vp_compact_kernel(VerifyWave w)
 {
-  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::rowBase);
+  const int j = table_find(w.jobs, w.numJobs, &VerifyJob::rowBase, (int)blockIdx.x);
   const VerifyJob &job = w.jobs[j];
   const VerifyJobScratch js = vp_job_scratch(w, j);
   const int b = blockIdx.x - job.rowBase;
@@ -435,19 +424,15 @@ struct VerifySample {
   int smp;
 };
 
-// The prologue of the hypothesis kernels (idivup(numLoops, VP_HYP_T) CTAs per job, one thread per sample): the sample's
-// job, its PER slots NaN-filled with zero counts, then the scale check and the K draws of the sample into idx.  false
-// when the thread has no sample or the sample has no draw.
+// The prologue of the hypothesis kernels: vp_hyp_sample (PER slots of 9 doubles per sample), then the scale check and
+// the K draws of the sample into idx.  false when the thread has no sample or the sample has no draw.
 template <int PER, int K>
 __device__ __forceinline__ bool vp_hyp_prologue(const VerifyWave &w, int numLoops, VerifySample &h, int (&idx)[K])
 {
-  const int per = (numLoops + VP_HYP_T - 1) / VP_HYP_T, j = blockIdx.x / per;
-  h.smp = (blockIdx.x - j * per) * VP_HYP_T + threadIdx.x;
-  if (h.smp >= numLoops) return false;
+  int j;
+  if (!vp_hyp_sample<VP_HYP_T, PER, 9>(numLoops, w.models, w.slotCounts, j, h.smp, h.slot)) return false;
   h.job = w.jobs + j;
   h.js = vp_job_scratch(w, j);
-  h.slot = h.js.models + (size_t)h.smp * 9 * PER;
-  for (int r = 0; r < PER; r++) { h.slot[9 * r] = CUDART_NAN; h.js.slotCounts[PER * h.smp + r] = 0; }
   return h.js.st->s > 0.0 && vp_draw<K>(h.job->seed, h.smp, h.js.st->numValid, idx);
 }
 
@@ -544,7 +529,7 @@ __global__ void __launch_bounds__(VP_SC_T)
 vp_score_kernel(VerifyWave w, int model)
 {
   __shared__ float4 s_p[VP_TILE];
-  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::scoreBase);
+  const int j = table_find(w.jobs, w.numJobs, &VerifyJob::scoreBase, (int)blockIdx.x);
   const VerifyJobScratch js = vp_job_scratch(w, j);
   const float4 *__restrict__ un = js.un;
   const double *__restrict__ models = js.models;
@@ -584,19 +569,9 @@ vp_argmax_kernel(VerifyWave w, int perSample)
   VerifyState *st = js.st;
   const int slot = (blockIdx.x - j * per) * 256 + threadIdx.x;
   const bool live = slot < numSlots && !isnan(models[(size_t)slot * 9]);
-  unsigned long long key = live ? ((unsigned long long)counts[slot] << 32) | (unsigned int)~slot : 0ull;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
-    key = t > key ? t : key;
-  }
-  const unsigned int nm = __popc(__ballot_sync(0xffffffffu, live));
+  vp_argmax_warp(live, counts + slot, slot, &st->best, &st->models);
   const unsigned int ns = __popc(__ballot_sync(0xffffffffu, live && slot % perSample == 0));
-  if ((threadIdx.x & 31) == 0) {
-    if (key) atomicMax(&st->best, key);
-    if (nm) atomicAdd(&st->models, (unsigned long long)nm);
-    if (ns) atomicAdd(&st->samples, (unsigned long long)ns);
-  }
+  if ((threadIdx.x & 31) == 0 && ns) atomicAdd(&st->samples, (unsigned long long)ns);
 }
 
 // block-wide sum of an int (fixed order; the result in every thread)
@@ -675,7 +650,7 @@ __device__ void vp_smallest_eigvec(const double (*s_nm)[45], double (&f)[9])
 __global__ void __launch_bounds__(VP_ROWS)
 vp_write_kernel(VerifyWave w)
 {
-  const int j = vp_job_of(w.jobs, w.numJobs, blockIdx.x, &VerifyJob::rowBase);
+  const int j = table_find(w.jobs, w.numJobs, &VerifyJob::rowBase, (int)blockIdx.x);
   const VerifyJob &job = w.jobs[j];
   const VerifyJobScratch js = vp_job_scratch(w, j);
   const int b = blockIdx.x - job.rowBase;
@@ -1320,35 +1295,11 @@ vp_refit_kernel(VerifyWave w, int model)
 // model slots per sample: up to 3 roots of the 7-point cubic (F; H uses the first), up to 10 of the 5-point solver (E)
 static int vp_slots_per_sample(int model) { return model == VERIFY_ESSENTIAL ? VP_E_SLOTS : 3; }
 
-#define VP_WAVE_BYTES ((size_t)256 << 20)    // model-slot scratch of a wave: 9 doubles and one count per slot
-
-int verify_jobs_per_wave(int numLoops, int model)
+// The waves of a batch, a job's extent being its row CTAs; a slot is 9 doubles and a count.
+static WavePlan verify_plan(const cs_verify_job *jobs, int numJobs, int numLoops, int model)
 {
-  const size_t perJob = (size_t)vp_slots_per_sample(model) * numLoops * (9 * sizeof(double) + sizeof(unsigned int));
-  const size_t k = VP_WAVE_BYTES / perJob;
-  return k < 1 ? 1 : k > 65536 ? 65536 : (int)k;
-}
-
-// The waves of a batch: its non-empty jobs in input order (live[q] is the input index of the q-th), cut into runs of
-// perWave jobs (the last run may be shorter); rows is the largest number of row CTAs of a wave.
-struct VerifyPlan {
-  std::vector<int> live;
-  int perWave = 1;
-  size_t rows = 0;
-};
-
-static VerifyPlan verify_plan(const cs_verify_job *jobs, int numJobs, int numLoops, int model)
-{
-  VerifyPlan p;
-  p.perWave = verify_jobs_per_wave(numLoops, model);
-  for (int k = 0; k < numJobs; k++)
-    if (jobs[k].numPairs > 0) p.live.push_back(k);
-  for (size_t q0 = 0; q0 < p.live.size(); q0 += p.perWave) {
-    size_t rows = 0;
-    for (size_t q = q0; q < std::min(p.live.size(), q0 + p.perWave); q++) rows += idivup(jobs[p.live[q]].numPairs, VP_ROWS);
-    p.rows = std::max(p.rows, rows);
-  }
-  return p;
+  const size_t slotBytes = (size_t)vp_slots_per_sample(model) * numLoops * (9 * sizeof(double) + sizeof(unsigned int));
+  return wave_plan(jobs, numJobs, slotBytes, [](const cs_verify_job &a) { return (size_t)idivup(a.numPairs, VP_ROWS); });
 }
 
 struct VerifyLayout {
@@ -1356,12 +1307,12 @@ struct VerifyLayout {
 };
 
 // The device table of the batch's non-empty jobs, then the scratch of one wave (reused by the next).
-static VerifyLayout verify_layout(const VerifyPlan &p, int numLoops, int model)
+static VerifyLayout verify_layout(const WavePlan &p, int numLoops, int model)
 {
   VerifyLayout L;
   Layout o(256);
   const size_t live = std::max(p.live.size(), (size_t)1), J = std::min(live, (size_t)p.perWave);
-  const size_t P = std::max(p.rows, (size_t)1) * VP_ROWS, S = vp_slots_per_sample(model) * (size_t)numLoops * J;
+  const size_t P = std::max(p.extent, (size_t)1) * VP_ROWS, S = vp_slots_per_sample(model) * (size_t)numLoops * J;
   L.jobs = o.take(live * sizeof(VerifyJob));
   L.masks = o.take(P / 32 * sizeof(unsigned int));
   L.counts = o.take(P / VP_ROWS * sizeof(unsigned int));
@@ -1375,33 +1326,22 @@ static VerifyLayout verify_layout(const VerifyPlan &p, int numLoops, int model)
   return L;
 }
 
-size_t verify_scratch_bytes(const cs_verify_job *jobs, int numJobs, int numLoops, int model)
-{
-  return verify_layout(verify_plan(jobs, numJobs, numLoops, model), numLoops, model).bytes;
-}
-
-// The pinned host area of a batch: one state per job (the q-th non-empty job's at q), then from the returned offset the
-// job table.
-static size_t vp_host_jobs_at(int numJobs)
-{
-  Layout L(256);
-  L.take((size_t)std::max(numJobs, 1) * sizeof(VerifyState));
-  return L.bytes;
-}
-size_t verify_host_bytes(int numJobs) { return vp_host_jobs_at(numJobs) + (size_t)std::max(numJobs, 1) * sizeof(VerifyJob); }
-
 // Per wave: steps 1-4 (and, with full, 5-8) on the stream, then the wave's states copied to the pinned area.
 // full == false stops after scoring (the models and counts of the last wave stay in scratch).
-int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model, int numLoops, float thresh,
-                  void *scratch, void *h_pinned, bool full, cudaStream_t st)
+int verify_enqueue(DeviceCtx &c, const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal, int model, int numLoops,
+                   float thresh, bool full)
 {
-  const VerifyPlan plan = verify_plan(jobs, numJobs, numLoops, model);
+  const WavePlan plan = verify_plan(jobs, numJobs, numLoops, model);
   const int live = (int)plan.live.size();
   if (live == 0) return 0;
   const VerifyLayout L = verify_layout(plan, numLoops, model);
-  char *b = static_cast<char *>(scratch);
-  VerifyState *h_states = static_cast<VerifyState *>(h_pinned);
-  VerifyJob *h_jobs = reinterpret_cast<VerifyJob *>(static_cast<char *>(h_pinned) + vp_host_jobs_at(numJobs));
+  int r;
+  if ((r = c.verify.grow(L.bytes)) < 0) return r;
+  VerifyState *h_states;
+  VerifyJob *h_jobs;
+  if ((r = pinned_states_and_jobs(c.h_verify, live, h_states, h_jobs)) < 0) return r;
+  char *b = c.verify.as<char>();
+  const cudaStream_t st = c.stream;
   const bool essential = model == VERIFY_ESSENTIAL;
   const int perSample = vp_slots_per_sample(model), slots = perSample * numLoops;
   // the table; the row and score bases count from the first job of each wave
@@ -1484,10 +1424,10 @@ int launch_verify(const cs_verify_job *jobs, int numJobs, const VerifyCalib *cal
   return 0;
 }
 
-// After launch_verify and a synchronize: the q-th non-empty job's count, model and statistics from its copied state.
-int verify_result(const void *h_pinned, int q, int numPairs, double model_out[9], long long stats[8])
+// After verify_enqueue and a synchronize: the q-th non-empty job's count, model and statistics from its copied state.
+int verify_result(const DeviceCtx &c, int q, int numPairs, double model_out[9], long long stats[8])
 {
-  const VerifyState *v = static_cast<const VerifyState *>(h_pinned) + q;
+  const VerifyState *v = c.h_verify.as<const VerifyState>() + q;
   for (int k = 0; k < 9; k++) model_out[k] = v->model[k];
   for (int k = 0; k < 8; k++) stats[k] = v->stats[k];
   stats[1] = (long long)numPairs - v->numValid;
@@ -1495,30 +1435,30 @@ int verify_result(const void *h_pinned, int q, int numPairs, double model_out[9]
 }
 
 // The same after an essential launch: E (in model), the pose and the ten statistics.
-int verify_essential_result(const void *h_pinned, int q, int numPairs, double E[9], double R[9], double t[3],
+int verify_essential_result(const DeviceCtx &c, int q, int numPairs, double E[9], double R[9], double t[3],
                             long long stats[10])
 {
-  const VerifyState *v = static_cast<const VerifyState *>(h_pinned) + q;
+  const VerifyState *v = c.h_verify.as<const VerifyState>() + q;
   for (int k = 0; k < 9; k++) R[k] = v->R[k];
   for (int k = 0; k < 3; k++) t[k] = v->t[k];
   stats[8] = v->pose[0];
   stats[9] = v->pose[1];
-  return verify_result(h_pinned, q, numPairs, E, stats);
+  return verify_result(c, q, numPairs, E, stats);
 }
 
-// After launch_verify(full = false) of one job and a synchronize: every slot's model in pixel coordinates (NaN-filled
-// when empty), every slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s}.  Returns the number of valid
-// pairs.  An essential slot's Fn becomes E = (T2 K2)^T Fn (T1 K1) with F's output scaling.
-int verify_models_to_host(const void *scratch, const void *h_pinned, const cs_verify_job &job, int numLoops, int model,
-                          const VerifyCalib *cal, double *h_models, int *h_counts, double h_norm[5], cudaStream_t st)
+// After verify_enqueue(full = false) of one job: every slot's model in pixel coordinates (NaN-filled when empty), every
+// slot's inlier count and the normalisation {c1x, c1y, c2x, c2y, s} (synchronizes).  Returns the number of valid pairs.
+// An essential slot's Fn becomes E = (T2 K2)^T Fn (T1 K1) with F's output scaling.
+int verify_models_to_host(DeviceCtx &c, const cs_verify_job &job, int numLoops, int model, const VerifyCalib *cal,
+                          double *h_models, int *h_counts, double h_norm[5])
 {
   const VerifyLayout L = verify_layout(verify_plan(&job, 1, numLoops, model), numLoops, model);
-  const char *b = static_cast<const char *>(scratch);
+  const char *b = c.verify.as<const char>();
   const size_t S = vp_slots_per_sample(model) * (size_t)numLoops;
-  CS_CUDA(cudaMemcpyAsync(h_models, b + L.models, S * 9 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CS_CUDA(cudaMemcpyAsync(h_counts, b + L.slotCounts, S * sizeof(int), cudaMemcpyDeviceToHost, st));
-  CS_CUDA(cudaStreamSynchronize(st));
-  const VerifyState *v = static_cast<const VerifyState *>(h_pinned);
+  CS_CUDA(cudaMemcpyAsync(h_models, b + L.models, S * 9 * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+  CS_CUDA(cudaMemcpyAsync(h_counts, b + L.slotCounts, S * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+  CS_CUDA(cudaStreamSynchronize(c.stream));
+  const VerifyState *v = c.h_verify.as<const VerifyState>();
   h_norm[0] = v->c1x; h_norm[1] = v->c1y; h_norm[2] = v->c2x; h_norm[3] = v->c2y; h_norm[4] = v->s;
   for (size_t k = 0; k < S; k++) {
     double *m = h_models + 9 * k;

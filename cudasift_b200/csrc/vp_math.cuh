@@ -1,10 +1,12 @@
 // vp_math.cuh -- the FP64 helpers that geometric verification (verify.cu), triangulation (triangulate.cu) and
 // absolute pose (pose.cu) share: the counter-based generator and sampler, the cyclic Jacobi eigen-decomposition, the
-// calibrated coordinates of a pinhole K and the reprojection inlier rule.  tests/verify_oracle.py and
-// tests/triangulate_oracle.py restate them in float64.
+// calibrated coordinates of a pinhole K and the reprojection inlier rule; and the hypothesis prologue and slot arg-max
+// of the two batched RANSAC calls (verify.cu, pose.cu).  tests/verify_oracle.py and tests/triangulate_oracle.py restate
+// the rules in float64.
 #pragma once
 
 #include <cmath>
+#include <math_constants.h>
 
 namespace cs {
 
@@ -85,6 +87,43 @@ __device__ bool vp_draw(unsigned long long seed, int smp, int n, int (&idx)[K])
     got++;
   }
   return got == K;
+}
+
+// The prologue of a RANSAC hypothesis kernel (idivup(numLoops, T) CTAs of T threads per job, one thread per sample):
+// the thread's job j and sample smp, then the sample's PER slots of D doubles NaN-filled (an empty slot) with zero
+// counts.  slots and counts are a wave's arrays, PER numLoops slots per job; slot is the sample's first.  false when the
+// thread has no sample.
+template <int T, int PER, int D>
+__device__ __forceinline__ bool vp_hyp_sample(int numLoops, double *slots, unsigned int *counts, int &j, int &smp,
+                                              double *&slot)
+{
+  const int per = (numLoops + T - 1) / T;
+  j = blockIdx.x / per;
+  smp = (blockIdx.x - j * per) * T + threadIdx.x;
+  if (smp >= numLoops) return false;
+  const size_t first = (size_t)j * PER * numLoops + (size_t)PER * smp;
+  slot = slots + first * D;
+  for (int r = 0; r < PER; r++) { slot[D * r] = CUDART_NAN; counts[first + r] = 0; }
+  return true;
+}
+
+// The packed arg-max of a warp's slots, all of one job: key = count << 32 | ~slot for a live slot (the most inliers,
+// then the lowest slot), 0 otherwise; a butterfly, then lane 0's atomicMax of the key into *best and its addition of the
+// warp's live slots to *numLive.  count is read for a live slot only.
+__device__ __forceinline__ void vp_argmax_warp(bool live, const unsigned int *count, int slot, unsigned long long *best,
+                                               unsigned long long *numLive)
+{
+  unsigned long long key = live ? ((unsigned long long)*count << 32) | (unsigned int)~slot : 0ull;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
+    key = t > key ? t : key;
+  }
+  const unsigned int nl = __popc(__ballot_sync(0xffffffffu, live));
+  if ((threadIdx.x & 31) == 0) {
+    if (key) atomicMax(best, key);
+    if (nl) atomicAdd(numLive, (unsigned long long)nl);
+  }
 }
 
 // The reprojection inlier rule of triangulation and absolute pose.  u = P (X, 1) with P = K [R | t] row-major 3 x 4:
