@@ -20,7 +20,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "GEOM_MODELS", "match_knn2_guided", "MatchSiftDataGuided", "match_guided_host", "guided_stats",
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
-           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch"]
+           "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
+           "BundleAdjust"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -94,6 +95,8 @@ def lib():
         "cs_build_tracks": (ip, [vp, ip, vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_triangulate_tracks": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, c.c_ulonglong,
                                        vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_bundle_adjust": (ip, [vp, ip, vp, vp, vp, vp, vp, ip, vp, ip, vp, vp, ip, ip, c.c_double, c.c_double,
+                                  vp, vp, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -811,6 +814,68 @@ def TriangulateTracks(datas, Ks, Rs, ts, offsets, members, numTrials=256, maxErr
         for buf in bufs:
             buf.free()
     return points, counts, errors, inlier, stats, ms.value
+
+
+def BundleAdjust(datas, Ks, Rs, ts, offsets, members, points, use=None, fixed=None, maxIterations=50,
+                 maxLinearIterations=100, linearTol=1e-6, maxError=4.0):
+    """Bundle adjustment of every camera and track point in one call (cs_bundle_adjust): Levenberg-Marquardt with the
+    points eliminated by the Schur complement and the camera system solved by preconditioned CG on the device.  datas,
+    Ks, Rs, ts, offsets and members as for TriangulateTracks; points [T, 3] its points (NaN: no point); use (bool [M],
+    for example TriangulateTracks' inlier) selects the members to adjust on, None every valid one.  fixed (uint8 per
+    image: 0 free, 1 held, 2..4 t[fixed - 2] held); None is COLMAP's gauge: image 0 held and image 1's largest |t|
+    component held.  Returns (R [S, 3, 3], t [S, 3], points [T, 3], errors float32 [M], inlier bool [M] under the final
+    parameters, cost (initial, final), trace float64 [iterations run, 4] of {candidate cost, lambda, CG iterations,
+    accepted}, stats int64 [8] as the header describes them, ms)."""
+    S = len(datas)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1).astype(np.int32))
+    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1, 2).astype(np.int32))
+    T, M = max(len(off) - 1, 0), len(mem)
+    pts = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+    if len(pts) != T:
+        raise ValueError("points: one per track, %d, not %d" % (T, len(pts)))
+    if fixed is None:
+        fixed = np.zeros(S, np.uint8)
+        if S > 0:
+            fixed[0] = 1
+        if S > 1:
+            fixed[1] = 2 + int(np.argmax(np.abs(t[1])))
+    fix = np.ascontiguousarray(np.asarray(fixed).reshape(-1).astype(np.uint8))
+    if len(fix) != S:
+        raise ValueError("fixed: one per image, %d, not %d" % (S, len(fix)))
+    u = None if use is None else np.ascontiguousarray(np.asarray(use).reshape(-1).astype(np.uint8))
+    if u is not None and len(u) != M:
+        raise ValueError("use: one per member, %d, not %d" % (M, len(u)))
+    sets = (MatchSet * max(S, 1))(*[MatchSet(d.d_data, d.numPts) for d in datas])
+    R_out, t_out = np.zeros((S, 3, 3)), np.zeros((S, 3))
+    errors, inlier = np.full(M, np.nan, np.float32), np.zeros(M, bool)
+    cost, trace = np.zeros(2), np.zeros((max(int(maxIterations), 0), 4))
+    stats, ms = np.zeros(8, np.int64), ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(off.nbytes, 4)), DeviceBuffer(max(mem.nbytes, 8)), DeviceBuffer(max(pts.nbytes, 8)),
+            DeviceBuffer(max(4 * M, 4)), DeviceBuffer(max(M, 1)), DeviceBuffer(max(M, 1))]
+    try:
+        if T:
+            bufs[0].upload(off)
+            bufs[2].upload(pts)
+        if M:
+            bufs[1].upload(mem)
+            if u is not None:
+                bufs[5].upload(u)
+        _check(lib().cs_bundle_adjust(sets if S else None, S, _ptr(K), _ptr(R), _ptr(t), _ptr(fix) if S else None,
+                                          bufs[0].ptr, T, bufs[1].ptr, M, bufs[5].ptr if u is not None else None,
+                                          bufs[2].ptr, int(maxIterations), int(maxLinearIterations), float(linearTol),
+                                          float(maxError), _ptr(R_out), _ptr(t_out), bufs[3].ptr, bufs[4].ptr,
+                                          _ptr(cost), _ptr(trace) if len(trace) else None, _ptr(stats),
+                                          ctypes.byref(ms)), "BundleAdjust")
+        if T:
+            pts = bufs[2].download(np.float64, 3 * T).reshape(T, 3)
+        if M and T:
+            errors = bufs[3].download(np.float32, M)
+            inlier = bufs[4].download(np.uint8, M).astype(bool)
+    finally:
+        for buf in bufs:
+            buf.free()
+    return R_out, t_out, pts, errors, inlier, (cost[0], cost[1]), trace[:int(stats[6])].copy(), stats, ms.value
 
 
 class PoseJob(ctypes.Structure):

@@ -831,12 +831,10 @@ static int tracks_args(const char *fn, const int *imageSizes, int numImages, con
   return 0;
 }
 
-// The arguments of cs_triangulate_tracks: the counts and tables, every set (sets[a]) and camera (Ks[a], Rs[a], ts[a]),
-// the parameters, the buffers, then the outputs against each other, the tracks and every set's records (overlap_sweep).
-static int triangulate_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
-                            const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
-                            int numTrials, double maxError, double minTriAngle, const double *points, const int *counts,
-                            const float *errors, const unsigned char *inlier)
+// The images of cs_triangulate_tracks and cs_bundle_adjust: the counts, every set (sets[a]) and camera (Ks[a], Rs[a],
+// ts[a]).
+static int camera_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                       const double *ts, int numTracks, int numMembers)
 {
   if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
   if (numTracks < 0) return arg_error(fn, "numTracks must be >= 0");
@@ -871,6 +869,18 @@ static int triangulate_args(const char *fn, const cs_match_set *sets, int numIma
       return arg_error(fn, bad);
     }
   }
+  return 0;
+}
+
+// The arguments of cs_triangulate_tracks: the images (camera_args), the parameters, the buffers, then the outputs
+// against each other, the tracks and every set's records (overlap_sweep).
+static int triangulate_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                            const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
+                            int numTrials, double maxError, double minTriAngle, const double *points, const int *counts,
+                            const float *errors, const unsigned char *inlier)
+{
+  const int r = camera_args(fn, sets, numImages, Ks, Rs, ts, numTracks, numMembers);
+  if (r < 0) return r;
   if (numTrials < 1 || numTrials > (1 << 20)) return arg_error(fn, "numTrials must be in [1, 2^20]");
   if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
   if (!std::isfinite(minTriAngle) || !(minTriAngle >= 0.0) || !(minTriAngle < 180.0))
@@ -899,6 +909,67 @@ static int triangulate_args(const char *fn, const cs_match_set *sets, int numIma
   return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
     static const char *const outs[4] = {"d_points", "d_counts", "d_errors", "d_inlier"};
     static const char *const ins[2] = {"d_offsets", "d_members"};
+    auto name = [&](const SweepRange &z, char *buf, size_t n) {
+      if (z.kind == 0) snprintf(buf, n, "%s", outs[z.owner]);
+      else if (z.kind == 1) snprintf(buf, n, "%s", ins[z.owner]);
+      else snprintf(buf, n, "sets[%d].pts", z.owner);
+    };
+    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
+    const SweepRange &b = &a == &x ? y : x;
+    char na[32], nb[32], msg[128];
+    name(a, na, sizeof na);
+    name(b, nb, sizeof nb);
+    snprintf(msg, sizeof msg, "%s and %s overlap (an output overlaps another range)", na, nb);
+    return arg_error(fn, msg);
+  });
+}
+
+// The arguments of cs_bundle_adjust: the images (camera_args), the gauge codes, the parameters, the buffers, then the
+// outputs against each other, the tracks, d_use and every set's records (overlap_sweep).
+static int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                       const double *ts, const unsigned char *fixed, const int *offsets, int numTracks,
+                       const int *members, int numMembers, const unsigned char *use, const double *points,
+                       int maxIterations, int maxLinearIterations, double linearTol, double maxError,
+                       const double *R_out, const double *t_out, const float *errors, const unsigned char *inlier,
+                       const double *cost_out)
+{
+  int r = camera_args(fn, sets, numImages, Ks, Rs, ts, numTracks, numMembers);
+  if (r < 0) return r;
+  char bad[128];
+  for (int a = 0; fixed && a < numImages; a++)
+    if (fixed[a] > 4) {
+      snprintf(bad, sizeof bad, "fixed[%d] must be 0 (free), 1 (held) or 2..4 (t[fixed - 2] held)", a);
+      return arg_error(fn, bad);
+    }
+  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
+  if (maxLinearIterations < 1 || maxLinearIterations > 10000)
+    return arg_error(fn, "maxLinearIterations must be in [1, 10000]");
+  if (!(linearTol > 0.0) || !(linearTol < 1.0)) return arg_error(fn, "linearTol must be in (0, 1)");
+  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
+  if (numImages > 0 && (!R_out || !t_out)) return arg_error(fn, "numImages > 0 needs R_out and t_out");
+  if (!cost_out) return arg_error(fn, "cost_out must not be NULL");
+  if (numTracks > 0 && (!offsets || !points)) return arg_error(fn, "numTracks > 0 needs d_offsets and d_points");
+  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
+  if ((reinterpret_cast<uintptr_t>(offsets) & 3) != 0 || (reinterpret_cast<uintptr_t>(errors) & 3) != 0)
+    return arg_error(fn, "d_offsets and d_errors must be 4-byte aligned");
+  if ((reinterpret_cast<uintptr_t>(members) & 7) != 0 || (reinterpret_cast<uintptr_t>(points) & 7) != 0)
+    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
+  // the outputs (kind 0, written; owners 0 d_points, 1 d_errors, 2 d_inlier), the inputs (kind 1, read; owners
+  // 0 d_offsets, 1 d_members, 2 d_use) and every set's records (kind 2, read)
+  std::vector<SweepRange> rs;
+  rs.reserve((size_t)numImages + 6);
+  if (numTracks > 0) {
+    sweep_add(rs, points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
+    sweep_add(rs, offsets, ((size_t)numTracks + 1) * sizeof(int), 0, 1, false);
+  }
+  if (errors) sweep_add(rs, errors, (size_t)numMembers * sizeof(float), 1, 0, true);
+  if (inlier) sweep_add(rs, inlier, (size_t)numMembers, 2, 0, true);
+  sweep_add(rs, members, (size_t)numMembers * sizeof(int2), 1, 1, false);
+  if (use) sweep_add(rs, use, (size_t)numMembers, 2, 1, false);
+  for (int a = 0; a < numImages; a++) sweep_add(rs, sets[a].pts, record_bytes(sets[a].n), a, 2, false);
+  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
+    static const char *const outs[3] = {"d_points", "d_errors", "d_inlier"};
+    static const char *const ins[3] = {"d_offsets", "d_members", "d_use"};
     auto name = [&](const SweepRange &z, char *buf, size_t n) {
       if (z.kind == 0) snprintf(buf, n, "%s", outs[z.owner]);
       else if (z.kind == 1) snprintf(buf, n, "%s", ins[z.owner]);
@@ -1848,6 +1919,41 @@ int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double 
   if (stats_out)
     for (int k = 0; k < 8; k++) stats_out[k] = (long long)st[k];
   return (int)st[5];
+}
+
+int cs_bundle_adjust(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
+                     const unsigned char *fixed, const int *d_offsets, int numTracks, const int *d_members,
+                     int numMembers, const unsigned char *d_use, double *d_points, int maxIterations,
+                     int maxLinearIterations, double linearTol, double maxError, double *R_out, double *t_out,
+                     float *d_errors, unsigned char *d_inlier, double cost_out[2], double *trace_out,
+                     long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_bundle_adjust";
+  if (ms) *ms = 0.0;
+  int r = bundle_args(fn, sets, numImages, Ks, Rs, ts, fixed, d_offsets, numTracks, d_members, numMembers, d_use,
+                      d_points, maxIterations, maxLinearIterations, linearTol, maxError, R_out, t_out, d_errors,
+                      d_inlier, cost_out);
+  if (r < 0) return r;
+  if (numTracks == 0) {
+    if (R_out != Rs) memmove(R_out, Rs, (size_t)numImages * 9 * sizeof(double));
+    if (t_out != ts) memmove(t_out, ts, (size_t)numImages * 3 * sizeof(double));
+    cost_out[0] = cost_out[1] = 0.0;
+    if (trace_out)
+      for (int k = 0; k < 4 * maxIterations; k++) trace_out[k] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 8; k++) stats_out[k] = 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return bundle_enqueue(*c, sets, numImages, Ks, Rs, ts, fixed, d_offsets, numTracks, d_members, numMembers,
+                               d_use, d_points, maxIterations, maxLinearIterations, linearTol, maxError, d_errors,
+                               d_inlier);
+       })) < 0)
+    return r;
+  return bundle_result(*c, numImages, maxIterations, R_out, t_out, cost_out, trace_out, stats_out);
 }
 
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,

@@ -347,6 +347,10 @@ struct DeviceCtx {
   // and job states
   GrowBuffer pose;
   PinnedBuffer h_pose;                     // every job's state (copied back), then the job table
+  // cs_bundle_adjust: the result words, the trace, the camera, point and observation tables, the camera pieces and
+  // partials, the sort storage
+  GrowBuffer bundle;
+  PinnedBuffer h_bundle;                   // the result words and the trace (copied back), then the camera table
   // cs_verify_*: the states a call copies back, and its job table
   PinnedBuffer h_verify;
 
@@ -536,6 +540,18 @@ int pose_result(const DeviceCtx &c, int q, double R[9], double t[3], long long s
 // after an enqueue of one job without full: every slot's R, t (NaN-filled when empty) and count (synchronizes);
 // returns the job's number of valid correspondences
 int pose_models_to_host(DeviceCtx &c, const cs_pose_job &job, int numLoops, double *h_R, double *h_t, int *h_counts);
+
+// ---- bundle adjustment (bundle.cu) -----------------------------------------------------------------------------
+// The launches of cs_bundle_adjust (argument-checked, numTracks > 0) on c.stream, without a synchronize; the results
+// reach c.h_bundle by the caller's synchronize, and bundle_result reads them.
+int bundle_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                   const double *ts, const unsigned char *fixed, const int *offsets, int numTracks, const int *members,
+                   int numMembers, const unsigned char *use, double *points, int maxIterations, int maxLinearIterations,
+                   double linearTol, double maxError, float *errors, unsigned char *inlier);
+// after the synchronize: the final R, t of every image, the costs, the trace (may be NULL) and the statistics; returns
+// the number of accepted steps
+int bundle_result(const DeviceCtx &c, int numImages, int maxIterations, double *R_out, double *t_out, double cost[2],
+                  double *trace, long long stats[8]);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

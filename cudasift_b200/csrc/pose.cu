@@ -444,24 +444,12 @@ __device__ bool ps_lm_solve(const double (&s)[PS_SUMS], double lam, double (&x)[
   return true;
 }
 
-// R' = exp([w]x) R, t' = exp([w]x) t + delta (Rodrigues: I + A [w]x + B [w]x^2, A = sin th / th, B = 2 sin^2(th/2) / th^2)
+// R' = exp([w]x) R, t' = exp([w]x) t + delta (vp_rodrigues)
 __device__ void ps_update(const double (&R)[9], const double (&t)[3], const double (&x)[6], double (&R1)[9],
                           double (&t1)[3])
 {
-  const double th2 = x[0] * x[0] + x[1] * x[1] + x[2] * x[2], th = sqrt(th2);
-  double A = 1.0, B = 0.5;
-  if (th2 != 0.0) {
-    const double sh = sin(0.5 * th);
-    A = sin(th) / th;
-    B = 2.0 * sh * sh / th2;
-  }
-  const double W[9] = {0.0, -x[2], x[1], x[2], 0.0, -x[0], -x[1], x[0], 0.0};
   double Q[9];
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) {
-      const double W2 = W[3 * i] * W[j] + W[3 * i + 1] * W[3 + j] + W[3 * i + 2] * W[6 + j];
-      Q[3 * i + j] = (i == j ? 1.0 : 0.0) + A * W[3 * i + j] + B * W2;
-    }
+  vp_rodrigues(x, Q);
   for (int i = 0; i < 3; i++) {
     for (int j = 0; j < 3; j++) R1[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
     t1[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + x[3 + i];

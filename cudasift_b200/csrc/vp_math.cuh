@@ -1,8 +1,8 @@
 // vp_math.cuh -- the FP64 helpers that geometric verification (verify.cu), triangulation (triangulate.cu) and
 // absolute pose (pose.cu) share: the counter-based generator and sampler, the cyclic Jacobi eigen-decomposition, the
-// calibrated coordinates of a pinhole K and the reprojection inlier rule; and the hypothesis prologue and slot arg-max
-// of the two batched RANSAC calls (verify.cu, pose.cu).  tests/verify_oracle.py and tests/triangulate_oracle.py restate
-// the rules in float64.
+// calibrated coordinates of a pinhole K, the Rodrigues rotation and the reprojection inlier rule; and the hypothesis
+// prologue and slot arg-max of the two batched RANSAC calls (verify.cu, pose.cu).  tests/verify_oracle.py and
+// tests/triangulate_oracle.py restate the rules in float64.
 #pragma once
 
 #include <cmath>
@@ -124,6 +124,25 @@ __device__ __forceinline__ void vp_argmax_warp(bool live, const unsigned int *co
     if (key) atomicMax(best, key);
     if (nl) atomicAdd(numLive, (unsigned long long)nl);
   }
+}
+
+// The Rodrigues rotation exp([w]x) = I + A [w]x + B [w]x^2, A = sin th / th, B = 2 sin^2(th / 2) / th^2 (A = 1, B = 1/2
+// at th = 0): the update of absolute pose's refinement and of bundle adjustment.
+__device__ __forceinline__ void vp_rodrigues(const double *w, double (&Q)[9])
+{
+  const double th2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2], th = sqrt(th2);
+  double A = 1.0, B = 0.5;
+  if (th2 != 0.0) {
+    const double sh = sin(0.5 * th);
+    A = sin(th) / th;
+    B = 2.0 * sh * sh / th2;
+  }
+  const double W[9] = {0.0, -w[2], w[1], w[2], 0.0, -w[0], -w[1], w[0], 0.0};
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) {
+      const double W2 = W[3 * i] * W[j] + W[3 * i + 1] * W[3 + j] + W[3 * i + 2] * W[6 + j];
+      Q[3 * i + j] = (i == j ? 1.0 : 0.0) + A * W[3 * i + j] + B * W2;
+    }
 }
 
 // The reprojection inlier rule of triangulation and absolute pose.  u = P (X, 1) with P = K [R | t] row-major 3 x 4:

@@ -597,6 +597,74 @@ int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_
                            const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
                            int *counts_out, long long *stats_out, double *ms);
 
+/* Bundle adjustment (Triggs et al. 2000; COLMAP's bundle_adjuster): Levenberg-Marquardt over every camera pose and
+ * track point at once, the points eliminated by the Schur complement and the reduced camera system solved by
+ * preconditioned conjugate gradients (Agarwal et al., ECCV 2010; Wu et al., CVPR 2011).  It takes what
+ * cs_triangulate_tracks takes and returns (sets, Ks, Rs, ts, d_offsets, d_members) and the points it wrote.
+ * - Observations: tracks, malformed tracks and valid members follow cs_triangulate_tracks.  A member of a well-formed
+ *   track is used when it is valid, d_use is NULL or d_use[m] != 0, the track's point is finite, and the point's depth
+ *   (R X + t)_2 is > 0 at the input parameters.  A track whose point has at least 2 used observations takes part;
+ *   otherwise its observations are dropped and its point is left unchanged, byte for byte.  Observation o runs over the
+ *   used observations of the participating tracks, in track order, then member order.
+ * - Cameras: fixed[a] (host bytes; NULL = every image free) is 0 (free: 6 parameters), 1 (held), or 2, 3, 4 (free but
+ *   for component fixed[a] - 2 of t, held: COLMAP's scale gauge).  An image with no used observation is held.  K is not
+ *   adjusted.  Held images and held components come back bit for bit.
+ * - Residual (cs_absolute_pose_batch's): r = (K0 a + K1 b + K2 - x, K4 b + K5 - y), (a, b) = (Xc0, Xc1) / Xc2,
+ *   Xc = R X + t.  Update R <- exp([w]x) R (the Rodrigues rule of cs_absolute_pose_batch), t <- t + delta,
+ *   X <- X + dX; with gr_x = (K0, K1, -(K0 a + K1 b)) / Xc2, gr_y = (0, K4, -K4 b) / Xc2 the Jacobian rows are
+ *   ((R X) x gr, gr) for the camera (w, delta) and gr^T R for the point.  The cost is the sum of r^T r over the used
+ *   observations.
+ * - LM: H + lambda D, D = diag(H) clamped to [1e-6, 1e32]; lambda starts at 1e-3, /10 after an accepted step, x10
+ *   after a rejected one.  A step is accepted when the linear solve succeeded, every used observation stays in front
+ *   (Xc2 > 0) and the cost decreases.  The loop stops after maxIterations iterations (accepted or rejected), after an
+ *   accepted step with previous cost - new cost <= 1e-10 previous cost, or when lambda exceeds 1e16 after a rejection.
+ *   maxIterations = 0, or no used observation, evaluates only.
+ * - Linear solve of [U* W; W^T V*] [dc; dp] = -[g_c; g_p] (U, V the camera and point blocks of J^T J, W = J_c^T J_p):
+ *   every V*_k by Cholesky, then S dc = b~ with S = U* - W V*^-1 W^T and b~ = -g_c + W V*^-1 g_p, restricted to the
+ *   free components (a held component's row and column are the identity's, its b~ entry 0).  Preconditioned CG from
+ *   dc = 0: the preconditioner is S's 6 x 6 diagonal block per camera (U*_a - sum over the used observations o of image
+ *   a of W_o V*_k^-1 W_ak^T, W_ak the sum of W over track k's observations in image a) by Cholesky; with z = M^-1 r,
+ *   p = z + beta p, alpha = r.z / p.S p, beta = r.z(new) / r.z(old).  CG stops before an iteration when
+ *   r.r <= linearTol^2 b~.b~ (so with no free camera parameter it runs none: structure only), after
+ *   maxLinearIterations iterations, or when p.S p is not > 0.  Then dp_k = V*_k^-1 (-g_k - sum_o J_p^T J_c dc_a).  A
+ *   Cholesky pivot that is not > 0 or not finite anywhere rejects the step without evaluating it.
+ * - Outputs: R_out [numImages][9], t_out [numImages][3] (may alias Rs, ts exactly); d_points adjusted in place;
+ *   for every member of a well-formed track, when the buffer is given, under the final parameters: d_errors and
+ *   d_inlier by cs_triangulate_tracks' output rule with maxError (NaN and 0 for an invalid member or a non-finite
+ *   point).  cost_out = {initial, final}.  trace_out (may be NULL) [maxIterations][4]: per iteration {the candidate's
+ *   cost (NaN when the solve failed), lambda, CG iterations, 1 if accepted}; rows past the last iteration are 0.
+ *   stats_out (may be NULL): [0] well-formed tracks, [1] malformed tracks, [2] invalid members, [3] used observations,
+ *   [4] points adjusted, [5] free camera parameters, [6] LM iterations, [7] CG iterations in all.
+ * - Returns the number of accepted steps, or CS_E_*.
+ * - Determinism: every sum has a fixed order that depends on the data only, and no scratch word is rewritten before
+ *   every CTA has read it, so two calls give the same bytes whatever the number of images.  Per
+ *   point: its observations in order.  Per camera: its observations in order o, cut at multiples of 256 of the
+ *   camera-sorted list; a piece is summed by a warp (lane l takes l, l + 32, ..., then an xor butterfly) and the pieces
+ *   in ascending order.  Totals over tracks (the cost): tiles of 256 tracks (warp butterflies, then the 8 warps in
+ *   order); over cameras (the CG dot products): tiles of 32 cameras (a butterfly); the tile partials lane-strided in
+ *   ascending order, then a butterfly.  The results agree with a float64 statement of these rules to rounding.
+ * - CS_E_ARG, before any CUDA call, naming the offending sets[a], camera a or buffer in cs_last_error(): every check of
+ *   cs_triangulate_tracks but numTrials and minTriAngle (d_counts is not an argument), a fixed[a] outside 0..4,
+ *   maxIterations outside [0, 1000], maxLinearIterations outside [1, 10000], linearTol not in (0, 1), NULL R_out or
+ *   t_out or cost_out with numImages > 0, and an output (d_points, d_errors, d_inlier) that overlaps another output,
+ *   d_offsets, d_members, d_use or any set's records (one sweep over sorted ranges).  numTracks == 0 returns 0
+ *   with R_out = Rs, t_out = ts, zero costs, trace and statistics, and makes no CUDA call.  numImages == 0 with
+ *   numTracks > 0 runs on the device like any call: every member is invalid, but the tracks (d_offsets) are device
+ *   memory, and the well-formed tracks' member outputs (NaN and 0) and the statistics are written from them.
+ * - Launches: 3 kernel launches (cs_launch_count) whatever the sizes and iteration counts: the count and fill kernels
+ *   and one cooperative kernel (a resident wave, SMs x occupancy CTAs of 256 threads) that runs the whole LM loop with
+ *   grid barriers between its phases; a cub scan and sort (not counted) run between them.  The call synchronises with
+ *   the host once, at the end; *ms (may be NULL) gets its event time.  Scratch, in the per-device context: 1 392
+ *   bytes per image (its state and camera pieces), 176 per track, 200 per member (the observation, J_c, J_p and r,
+ *   the sort keys), 432 per 256 members, 36 per LM iteration, plus the cub scan and sort storage; pinned, 944 bytes
+ *   per image and 32 per LM iteration. */
+int cs_bundle_adjust(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
+                     const unsigned char *fixed, const int *d_offsets, int numTracks, const int *d_members,
+                     int numMembers, const unsigned char *d_use, double *d_points, int maxIterations,
+                     int maxLinearIterations, double linearTol, double maxError, double *R_out, double *t_out,
+                     float *d_errors, unsigned char *d_inlier, double cost_out[2], double *trace_out,
+                     long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
