@@ -9,10 +9,10 @@
 // per-device state instead of function-local statics (quirk Q12); quiet unless
 // CUDASIFT_VERBOSE is set (quirk Q13).
 #include "common.cuh"
+#include "args.h"
 #include "pipeline2.h"
 
 #include <algorithm>
-#include <climits>
 #include <cmath>
 #include <cstddef>
 #include <cstdarg>
@@ -341,131 +341,6 @@ static int host_pairs(DeviceCtx *c, const void *h_s1, int n1, const void *h_s2, 
   return total;
 }
 
-// ---- argument checks: they come before any CUDA call (they hold on a machine without a device) ----
-static int arg_error(const char *fn, const char *bad)
-{
-  set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad);
-  return CS_E_ARG;
-}
-
-// [a, a + na) and [b, b + nb) share a byte
-static bool ranges_overlap(const void *a, size_t na, const void *b, size_t nb)
-{
-  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
-  return na > 0 && nb > 0 && x < y + nb && y < x + na;
-}
-static size_t record_bytes(int n) { return n > 0 ? (size_t)n * sizeof(SiftPoint) : 0; }
-
-// The two record sets and the path mode (0 auto, 1 exact, 2 tensor).
-static int check_sets(const char *fn, const void *s1, int n1, const void *s2, int n2, int mode)
-{
-  if (n1 < 0 || n2 < 0) return arg_error(fn, "n1 and n2 must be >= 0");
-  if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) return arg_error(fn, "a set with records needs a pointer");
-  if (mode < 0 || mode > 2) return arg_error(fn, "mode must be 0 (auto), 1 (exact) or 2 (tensor)");
-  return 0;
-}
-
-// The other buffers of a call (buf[k], bytes[k] bytes, called name[k]): every non-empty one 8-byte aligned, outside
-// both record ranges and apart from the others.
-static int check_buffers(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *const *buf,
-                         const size_t *bytes, const char *const *name, int n)
-{
-  char bad[64] = "";
-  for (int k = 0; k < n && !bad[0]; k++) {
-    const void *b = buf[k];
-    const size_t nb = bytes[k];
-    if (nb == 0) continue;
-    if ((reinterpret_cast<uintptr_t>(b) & 7) != 0) snprintf(bad, sizeof(bad), "%s must be 8-byte aligned", name[k]);
-    else if (ranges_overlap(b, nb, s1, record_bytes(n1)) || ranges_overlap(b, nb, s2, record_bytes(n2)))
-      snprintf(bad, sizeof(bad), "%s overlaps a record range", name[k]);
-    for (int m = 0; m < k && !bad[0]; m++)
-      if (ranges_overlap(b, nb, buf[m], bytes[m])) snprintf(bad, sizeof(bad), "%s and %s overlap", name[m], name[k]);
-  }
-  return bad[0] ? arg_error(fn, bad) : 0;
-}
-
-// The buffers of a batch call: [lo, hi) of table entry `owner`, its kind, and whether the call writes it.  A written
-// range may share no byte with any other range: overlap_sweep sorts them by start (O(n log n)), and an overlap is then an
-// earlier range that ends after a later one starts.  report(x, y) makes the error of the first overlap found.
-struct SweepRange {
-  uintptr_t lo, hi;
-  int owner, kind;
-  bool out;
-};
-static void sweep_add(std::vector<SweepRange> &rs, const void *b, size_t bytes, int owner, int kind, bool out)
-{
-  if (bytes) rs.push_back({reinterpret_cast<uintptr_t>(b), reinterpret_cast<uintptr_t>(b) + bytes, owner, kind, out});
-}
-template <class Report>
-static int overlap_sweep(std::vector<SweepRange> &rs, Report &&report)
-{
-  std::sort(rs.begin(), rs.end(), [](const SweepRange &a, const SweepRange &b) {
-    return a.lo != b.lo ? a.lo < b.lo : a.kind != b.kind ? a.kind < b.kind : a.owner < b.owner;
-  });
-  const SweepRange *anyEnd = nullptr, *outEnd = nullptr;  // the earlier ranges (and written ones) that end last
-  for (const SweepRange &x : rs) {
-    const SweepRange *hit = nullptr;
-    if (x.out && anyEnd && anyEnd->hi > x.lo) hit = anyEnd;
-    else if (outEnd && outEnd->hi > x.lo) hit = outEnd;
-    if (hit) return report(*hit, x);
-    if (!anyEnd || x.hi > anyEnd->hi) anyEnd = &x;
-    if (x.out && (!outEnd || x.hi > outEnd->hi)) outEnd = &x;
-  }
-  return 0;
-}
-
-// The pairs buffer of the mutual and ratio matchers: maxPairs int2.
-static int check_pairs(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs)
-{
-  if (maxPairs < 0) return arg_error(fn, "maxPairs must be >= 0");
-  if (maxPairs > 0 && !pairs) return arg_error(fn, "maxPairs > 0 needs a pairs buffer");
-  const size_t bytes = (size_t)maxPairs * sizeof(int2);
-  const char *name = "pairs";
-  return check_buffers(fn, s1, n1, s2, n2, &pairs, &bytes, &name, 1);
-}
-
-// The mutual matcher writes both record sets, so they must not overlap.
-static int mutual_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs,
-                       int mode)
-{
-  int r;
-  if ((r = check_sets(fn, s1, n1, s2, n2, mode)) < 0) return r;
-  if (ranges_overlap(s1, record_bytes(n1), s2, record_bytes(n2)))
-    return arg_error(fn, "the record ranges of set 1 and set 2 overlap (both are written)");
-  return check_pairs(fn, s1, n1, s2, n2, pairs, maxPairs);
-}
-
-static int ratio_args(const char *fn, const void *s1, int n1, const void *s2, int n2, float maxRatio, float maxDistance,
-                      const void *pairs, int maxPairs, int mode)
-{
-  int r;
-  if ((r = check_sets(fn, s1, n1, s2, n2, mode)) < 0) return r;
-  if (std::isnan(maxRatio) || std::isnan(maxDistance)) return arg_error(fn, "maxRatio and maxDistance must not be NaN");
-  return check_pairs(fn, s1, n1, s2, n2, pairs, maxPairs);
-}
-
-// The records are only read (they may overlap each other); the pair and inlier buffers are checked as outputs.
-static int verify_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
-                       int model, int numLoops, float thresh, const double *model_out, const void *inliers,
-                       int maxInliers)
-{
-  int r;
-  if ((r = check_sets(fn, s1, n1, s2, n2, 0)) < 0) return r;              // mode 0: the verifier has one path
-  if (numPairs < 0) return arg_error(fn, "numPairs must be >= 0");
-  if (numPairs > 0 && !pairs) return arg_error(fn, "numPairs > 0 needs a pairs buffer");
-  if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL)
-    return arg_error(fn, "model must be 1 (homography) or 2 (fundamental)");
-  if (numLoops < 1 || numLoops > 65536) return arg_error(fn, "numLoops must be in [1, 65536]");
-  if (!std::isfinite(thresh) || thresh <= 0.0f) return arg_error(fn, "thresh must be finite and > 0");
-  if (!model_out) return arg_error(fn, "model_out must not be NULL");
-  if (maxInliers < 0) return arg_error(fn, "maxInliers must be >= 0");
-  if (maxInliers > 0 && !inliers) return arg_error(fn, "maxInliers > 0 needs an inliers buffer");
-  const void *buf[2] = {pairs, inliers};
-  const size_t bytes[2] = {(size_t)numPairs * sizeof(int2), (size_t)maxInliers * sizeof(int2)};
-  const char *const name[2] = {"pairs", "inliers"};
-  return check_buffers(fn, s1, n1, s2, n2, buf, bytes, name, 2);
-}
-
 // The two nearest neighbours of set 1's rows in set 2 (idx1 / score1, [n1][2]); with idx2 also those of set 2's rows in
 // set 1; with ra then the ratio-test pairs, cross-checked when idx2 is given, and the call returns their number.  The
 // records are only read; both sets are non-empty.  Path rule: the tensor path when asked for (mode 2) or automatically
@@ -518,22 +393,6 @@ static int ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1,
   return knn_sync(fn, c, d1, n1, d2, n2, l.idx1, l.sc1, l.idx2, l.sc2, &ra, mode, ms);
 }
 
-// The model and threshold of a guided call (the records and buffers are checked as for cs_match_knn2 / cs_match_ratio).
-static int guided_args(const char *fn, int model, const double *model_in, float thresh)
-{
-  if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL)
-    return arg_error(fn, "model must be 1 (homography) or 2 (fundamental)");
-  if (!model_in) return arg_error(fn, "model_in must not be NULL");
-  double s = 0.0;
-  for (int k = 0; k < 9; k++) {
-    if (!std::isfinite(model_in[k])) return arg_error(fn, "model_in must be finite");
-    s += model_in[k] * model_in[k];
-  }
-  if (!(s > 0.0 && std::isfinite(s))) return arg_error(fn, "model_in must not be all zero (and its norm must be finite)");
-  if (!std::isfinite(thresh) || thresh <= 0.0f) return arg_error(fn, "thresh must be finite and > 0");
-  return 0;
-}
-
 // cs_match_knn2_guided / cs_match_guided on device sets: the guided lists of set 1 (and with idx2 of set 2), with ra
 // then the ratio-test pairs, and the call returns their number; one synchronize.
 static int guided_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
@@ -559,34 +418,6 @@ static int guided_ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, 
   const int r = knn_lists(c, n1, n2, crossCheck, &l);
   if (r < 0) return r;
   return guided_sync(fn, c, d1, n1, d2, n2, gm, l.idx1, l.sc1, l.idx2, l.sc2, &ra, ms);
-}
-
-// The intrinsics of an essential call: a finite row-major pinhole K (skew allowed) with K[3] = K[6] = K[7] = 0,
-// K[8] = 1, K[0] > 0 and K[4] > 0.
-static int check_intrinsics(const char *fn, const double *K, const char *name)
-{
-  char msg[96];
-  snprintf(msg, sizeof msg, "%s must be a finite pinhole matrix (K[3] = K[6] = K[7] = 0, K[8] = 1, K[0] > 0, K[4] > 0)",
-           name);
-  if (!K) return arg_error(fn, msg);
-  for (int k = 0; k < 9; k++)
-    if (!std::isfinite(K[k])) return arg_error(fn, msg);
-  if (K[3] != 0.0 || K[6] != 0.0 || K[7] != 0.0 || K[8] != 1.0 || !(K[0] > 0.0) || !(K[4] > 0.0)) return arg_error(fn, msg);
-  return 0;
-}
-
-// The arguments of cs_verify_essential*: those of cs_verify_pairs except model, the intrinsics and the three outputs.
-static int essential_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
-                          const double *K1, const double *K2, int numLoops, float thresh, const double *E,
-                          const double *R, const double *t, const void *inliers, int maxInliers)
-{
-  int r;
-  if (!E || !R || !t) return arg_error(fn, "E_out, R_out and t_out must not be NULL");
-  if ((r = verify_args(fn, s1, n1, s2, n2, pairs, numPairs, CS_GEOM_FUNDAMENTAL, numLoops, thresh, E, inliers,
-                       maxInliers)) < 0)
-    return r;
-  if ((r = check_intrinsics(fn, K1, "K1")) < 0) return r;
-  return check_intrinsics(fn, K2, "K2");
 }
 
 static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, const int *pairs, int numPairs,
@@ -661,381 +492,6 @@ static int verify_models_sync(DeviceCtx *c, const cs_verify_job &job, const Veri
   int r;
   if ((r = verify_enqueue(*c, &job, 1, cal, model, numLoops, thresh, false)) < 0) return r;
   return verify_models_to_host(*c, job, numLoops, model, cal, h_models, h_counts, h_norm);
-}
-
-// The arguments of cs_verify_pairs_batch (cal_args false) and cs_verify_essential_batch: the common ones, then every
-// job's as its single call checks them (named jobs[p]), the total pair count, then the inlier buffers against every
-// other job's buffers and records (sorted ranges, O(J log J)).
-static int verify_batch_args(const char *fn, const cs_verify_job *jobs, int numJobs, int model, int numLoops,
-                             float thresh, const double *K1s, const double *K2s, bool essential)
-{
-  int r;
-  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
-  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs a jobs array");
-  if (essential && numJobs > 0 && (!K1s || !K2s)) return arg_error(fn, "K1s and K2s must not be NULL");
-  long long total = 0;
-  const double dummy = 0.0;
-  for (int p = 0; p < numJobs; p++) {
-    const cs_verify_job &j = jobs[p];
-    char name[96];
-    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
-    if ((r = verify_args(name, j.s1, j.n1, j.s2, j.n2, j.pairs, j.numPairs, model, numLoops, thresh, &dummy, j.inliers,
-                         j.maxInliers)) < 0)
-      return r;
-    if (essential && ((r = check_intrinsics(name, K1s + 9 * (size_t)p, "K1s[p]")) < 0 ||
-                      (r = check_intrinsics(name, K2s + 9 * (size_t)p, "K2s[p]")) < 0))
-      return r;
-    total += j.numPairs;
-    if (total > INT_MAX) {
-      char bad[96];
-      snprintf(bad, sizeof bad, "the total numPairs exceeds INT_MAX at jobs[%d]", p);
-      return arg_error(fn, bad);
-    }
-  }
-  // every non-empty range; a writable one (an inlier buffer, kind 0) may overlap no other range of another job (its own
-  // job's were checked above)
-  static const char *const kinds[4] = {"inliers", "pairs", "s1", "s2"};
-  std::vector<SweepRange> rs;
-  rs.reserve(4 * (size_t)numJobs);
-  for (int p = 0; p < numJobs; p++) {
-    const cs_verify_job &j = jobs[p];
-    sweep_add(rs, j.inliers, (size_t)j.maxInliers * sizeof(int2), p, 0, true);
-    sweep_add(rs, j.pairs, (size_t)j.numPairs * sizeof(int2), p, 1, false);
-    sweep_add(rs, j.s1, record_bytes(j.n1), p, 2, false);
-    sweep_add(rs, j.s2, record_bytes(j.n2), p, 3, false);
-  }
-  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
-    const SweepRange &a = x.owner <= y.owner ? x : y, &b = x.owner <= y.owner ? y : x;
-    char bad[128];
-    snprintf(bad, sizeof bad, "jobs[%d].%s and jobs[%d].%s overlap (an inlier buffer overlaps another range)", a.owner,
-             kinds[a.kind], b.owner, kinds[b.kind]);
-    return arg_error(fn, bad);
-  });
-}
-
-// The arguments of cs_match_ratio_batch: the common ones, every set (named sets[s]) and job (jobs[p]), then the pair
-// buffers against each other and against every set's records (overlap_sweep).
-static int ratio_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
-                            float maxRatio, float maxDistance, const int *counts_out)
-{
-  if (numSets < 0 || numSets > 65536) return arg_error(fn, "numSets must be in [0, 65536]");
-  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
-  if (numSets > 0 && !sets) return arg_error(fn, "numSets > 0 needs a sets array");
-  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs a jobs array");
-  if (numJobs > 0 && !counts_out) return arg_error(fn, "counts_out must not be NULL");
-  if (std::isnan(maxRatio) || std::isnan(maxDistance)) return arg_error(fn, "maxRatio and maxDistance must not be NaN");
-  char bad[128] = "";
-  for (int s = 0; s < numSets && !bad[0]; s++) {
-    if (sets[s].n < 0) snprintf(bad, sizeof bad, "sets[%d]: n must be >= 0", s);
-    else if (sets[s].n > 0 && !sets[s].pts) snprintf(bad, sizeof bad, "sets[%d]: a set with records needs a pointer", s);
-  }
-  for (int p = 0; p < numJobs && !bad[0]; p++) {
-    const cs_match_job &j = jobs[p];
-    if (j.set1 < 0 || j.set1 >= numSets || j.set2 < 0 || j.set2 >= numSets)
-      snprintf(bad, sizeof bad, "jobs[%d]: set1 and set2 must be in [0, numSets)", p);
-    else if (j.maxPairs < 0) snprintf(bad, sizeof bad, "jobs[%d]: maxPairs must be >= 0", p);
-    else if (j.maxPairs > 0 && !j.pairs) snprintf(bad, sizeof bad, "jobs[%d]: maxPairs > 0 needs a pairs buffer", p);
-    else if (j.maxPairs > 0 && (reinterpret_cast<uintptr_t>(j.pairs) & 7) != 0)
-      snprintf(bad, sizeof bad, "jobs[%d]: pairs must be 8-byte aligned", p);
-  }
-  if (bad[0]) return arg_error(fn, bad);
-  // the pair buffers (kind 0, written) against each other and every set's records (kind 1, read)
-  std::vector<SweepRange> rs;
-  rs.reserve((size_t)numSets + numJobs);
-  for (int p = 0; p < numJobs; p++) sweep_add(rs, jobs[p].pairs, (size_t)jobs[p].maxPairs * sizeof(int2), p, 0, true);
-  for (int s = 0; s < numSets; s++) sweep_add(rs, sets[s].pts, record_bytes(sets[s].n), s, 1, false);
-  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
-    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
-    const SweepRange &b = &a == &x ? y : x;
-    char msg[128];
-    snprintf(msg, sizeof msg, "%s[%d].%s and %s[%d].%s overlap (a pair buffer overlaps another range)",
-             a.kind ? "sets" : "jobs", a.owner, a.kind ? "pts" : "pairs", b.kind ? "sets" : "jobs", b.owner,
-             b.kind ? "pts" : "pairs");
-    return arg_error(fn, msg);
-  });
-}
-
-// The arguments of cs_match_guided_batch: those of cs_match_ratio_batch, then every job's model as the single call
-// checks it (named jobs[p]).
-static int guided_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs,
-                             int numJobs, const int *models, const double *models_in, float thresh, float maxRatio,
-                             float maxDistance, const int *counts_out)
-{
-  int r;
-  if ((r = ratio_batch_args(fn, sets, numSets, jobs, numJobs, maxRatio, maxDistance, counts_out)) < 0) return r;
-  if (numJobs > 0 && (!models || !models_in)) return arg_error(fn, "models and models_in must not be NULL");
-  for (int p = 0; p < numJobs; p++) {
-    char name[96];
-    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
-    if ((r = guided_args(name, models[p], models_in + 9 * (size_t)p, thresh)) < 0) return r;
-  }
-  return 0;
-}
-
-// The arguments of cs_build_tracks: the counts and tables, every image (imageSizes[a]) and list (lists[p]), the
-// outputs, then the output buffers against each other and every pair list (overlap_sweep).  *N and *P receive the
-// feature and pair totals.
-static int tracks_args(const char *fn, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
-                       int minLength, const int *trackOf, const int *offsets, int maxTracks, const int *members,
-                       int maxMembers, int *N, int *P)
-{
-  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
-  if (numLists < 0 || numLists > (1 << 24)) return arg_error(fn, "numLists must be in [0, 2^24]");
-  if (numImages > 0 && !imageSizes) return arg_error(fn, "numImages > 0 needs an imageSizes array");
-  if (numLists > 0 && !lists) return arg_error(fn, "numLists > 0 needs a lists array");
-  char bad[128] = "";
-  long long n = 0, pairs = 0;
-  for (int a = 0; a < numImages && !bad[0]; a++) {
-    if (imageSizes[a] < 0) snprintf(bad, sizeof bad, "imageSizes[%d] must be >= 0", a);
-    else if ((n += imageSizes[a]) > INT_MAX) snprintf(bad, sizeof bad, "imageSizes[%d]: the sizes pass INT_MAX", a);
-  }
-  for (int p = 0; p < numLists && !bad[0]; p++) {
-    const cs_track_list &l = lists[p];
-    if (l.image1 < 0 || l.image1 >= numImages || l.image2 < 0 || l.image2 >= numImages)
-      snprintf(bad, sizeof bad, "lists[%d]: image1 and image2 must be in [0, numImages)", p);
-    else if (l.numPairs < 0) snprintf(bad, sizeof bad, "lists[%d]: numPairs must be >= 0", p);
-    else if (l.numPairs > 0 && !l.pairs) snprintf(bad, sizeof bad, "lists[%d]: numPairs > 0 needs a pairs buffer", p);
-    else if (l.numPairs > 0 && (reinterpret_cast<uintptr_t>(l.pairs) & 7) != 0)
-      snprintf(bad, sizeof bad, "lists[%d]: pairs must be 8-byte aligned", p);
-    else if ((pairs += l.numPairs) > INT_MAX) snprintf(bad, sizeof bad, "lists[%d]: the pair counts pass INT_MAX", p);
-  }
-  if (bad[0]) return arg_error(fn, bad);
-  if (minLength < 2) return arg_error(fn, "minLength must be >= 2");
-  if (maxTracks < 0 || maxMembers < 0) return arg_error(fn, "maxTracks and maxMembers must be >= 0");
-  if (maxTracks > 0 && !offsets) return arg_error(fn, "maxTracks > 0 needs d_offsets");
-  if (maxMembers > 0 && !members) return arg_error(fn, "maxMembers > 0 needs d_members");
-  if ((reinterpret_cast<uintptr_t>(trackOf) & 3) != 0 || (reinterpret_cast<uintptr_t>(offsets) & 3) != 0)
-    return arg_error(fn, "d_trackOf and d_offsets must be 4-byte aligned");
-  if ((reinterpret_cast<uintptr_t>(members) & 7) != 0) return arg_error(fn, "d_members must be 8-byte aligned");
-  // the outputs (kind 0, written; owners 0 d_trackOf, 1 d_offsets, 2 d_members) against each other and every pair
-  // list (kind 1, read)
-  std::vector<SweepRange> rs;
-  rs.reserve((size_t)numLists + 3);
-  if (trackOf) sweep_add(rs, trackOf, (size_t)n * sizeof(int), 0, 0, true);
-  if (offsets) sweep_add(rs, offsets, ((size_t)maxTracks + 1) * sizeof(int), 1, 0, true);
-  sweep_add(rs, members, (size_t)maxMembers * sizeof(int2), 2, 0, true);
-  for (int p = 0; p < numLists; p++) sweep_add(rs, lists[p].pairs, (size_t)lists[p].numPairs * sizeof(int2), p, 1, false);
-  const int r = overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
-    static const char *const outs[3] = {"d_trackOf", "d_offsets", "d_members"};
-    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
-    const SweepRange &b = &a == &x ? y : x;
-    char msg[128], nb[32];
-    if (b.kind) snprintf(nb, sizeof nb, "lists[%d].pairs", b.owner);
-    else snprintf(nb, sizeof nb, "%s", outs[b.owner]);
-    snprintf(msg, sizeof msg, "%s and %s overlap (an output overlaps another range)", outs[a.owner], nb);
-    return arg_error(fn, msg);
-  });
-  if (r < 0) return r;
-  *N = (int)n;
-  *P = (int)pairs;
-  return 0;
-}
-
-// The images of cs_triangulate_tracks and cs_bundle_adjust: the counts, every set (sets[a]) and camera (Ks[a], Rs[a],
-// ts[a]).
-static int camera_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
-                       const double *ts, int numTracks, int numMembers)
-{
-  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
-  if (numTracks < 0) return arg_error(fn, "numTracks must be >= 0");
-  if (numMembers < 0) return arg_error(fn, "numMembers must be >= 0");
-  if (numImages > 0 && (!sets || !Ks || !Rs || !ts)) return arg_error(fn, "numImages > 0 needs sets, Ks, Rs and ts");
-  char bad[128] = "";
-  for (int a = 0; a < numImages && !bad[0]; a++) {
-    if (sets[a].n < 0) snprintf(bad, sizeof bad, "sets[%d]: n must be >= 0", a);
-    else if (sets[a].n > 0 && !sets[a].pts) snprintf(bad, sizeof bad, "sets[%d]: a set with records needs a pointer", a);
-  }
-  if (bad[0]) return arg_error(fn, bad);
-  for (int a = 0; a < numImages; a++) {
-    snprintf(bad, sizeof bad, "Ks[%d]", a);
-    const int r = check_intrinsics(fn, Ks + 9 * (size_t)a, bad);
-    if (r < 0) return r;
-    const double *R = Rs + 9 * (size_t)a, *t = ts + 3 * (size_t)a;
-    bool ok = true;
-    for (int k = 0; k < 9; k++) ok = ok && std::isfinite(R[k]);
-    for (int i = 0; i < 3 && ok; i++)
-      for (int j = 0; j < 3; j++) {
-        const double d = R[3 * i] * R[3 * j] + R[3 * i + 1] * R[3 * j + 1] + R[3 * i + 2] * R[3 * j + 2];
-        ok = ok && std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-6;
-      }
-    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
-                       R[2] * (R[3] * R[7] - R[4] * R[6]);
-    if (!ok || !(det > 0.0)) {
-      snprintf(bad, sizeof bad, "Rs[%d] must be a finite rotation (R R^T = I within 1e-6, det R > 0)", a);
-      return arg_error(fn, bad);
-    }
-    if (!std::isfinite(t[0]) || !std::isfinite(t[1]) || !std::isfinite(t[2])) {
-      snprintf(bad, sizeof bad, "ts[%d] must be finite", a);
-      return arg_error(fn, bad);
-    }
-  }
-  return 0;
-}
-
-// The arguments of cs_triangulate_tracks: the images (camera_args), the parameters, the buffers, then the outputs
-// against each other, the tracks and every set's records (overlap_sweep).
-static int triangulate_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
-                            const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
-                            int numTrials, double maxError, double minTriAngle, const double *points, const int *counts,
-                            const float *errors, const unsigned char *inlier)
-{
-  const int r = camera_args(fn, sets, numImages, Ks, Rs, ts, numTracks, numMembers);
-  if (r < 0) return r;
-  if (numTrials < 1 || numTrials > (1 << 20)) return arg_error(fn, "numTrials must be in [1, 2^20]");
-  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
-  if (!std::isfinite(minTriAngle) || !(minTriAngle >= 0.0) || !(minTriAngle < 180.0))
-    return arg_error(fn, "minTriAngle must be finite and in [0, 180)");
-  if (numTracks > 0 && !offsets) return arg_error(fn, "numTracks > 0 needs d_offsets");
-  if (numTracks > 0 && (!points || !counts)) return arg_error(fn, "numTracks > 0 needs d_points and d_counts");
-  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
-  if ((reinterpret_cast<uintptr_t>(offsets) & 3) != 0 || (reinterpret_cast<uintptr_t>(counts) & 3) != 0 ||
-      (reinterpret_cast<uintptr_t>(errors) & 3) != 0)
-    return arg_error(fn, "d_offsets, d_counts and d_errors must be 4-byte aligned");
-  if ((reinterpret_cast<uintptr_t>(members) & 7) != 0 || (reinterpret_cast<uintptr_t>(points) & 7) != 0)
-    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
-  // the outputs (kind 0, written; owners 0 d_points, 1 d_counts, 2 d_errors, 3 d_inlier), the tracks (kind 1, read;
-  // owners 0 d_offsets, 1 d_members) and every set's records (kind 2, read)
-  std::vector<SweepRange> rs;
-  rs.reserve((size_t)numImages + 6);
-  if (numTracks > 0) {
-    sweep_add(rs, points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
-    sweep_add(rs, counts, (size_t)numTracks * sizeof(int), 1, 0, true);
-    sweep_add(rs, offsets, ((size_t)numTracks + 1) * sizeof(int), 0, 1, false);
-  }
-  if (errors) sweep_add(rs, errors, (size_t)numMembers * sizeof(float), 2, 0, true);
-  if (inlier) sweep_add(rs, inlier, (size_t)numMembers, 3, 0, true);
-  sweep_add(rs, members, (size_t)numMembers * sizeof(int2), 1, 1, false);
-  for (int a = 0; a < numImages; a++) sweep_add(rs, sets[a].pts, record_bytes(sets[a].n), a, 2, false);
-  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
-    static const char *const outs[4] = {"d_points", "d_counts", "d_errors", "d_inlier"};
-    static const char *const ins[2] = {"d_offsets", "d_members"};
-    auto name = [&](const SweepRange &z, char *buf, size_t n) {
-      if (z.kind == 0) snprintf(buf, n, "%s", outs[z.owner]);
-      else if (z.kind == 1) snprintf(buf, n, "%s", ins[z.owner]);
-      else snprintf(buf, n, "sets[%d].pts", z.owner);
-    };
-    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
-    const SweepRange &b = &a == &x ? y : x;
-    char na[32], nb[32], msg[128];
-    name(a, na, sizeof na);
-    name(b, nb, sizeof nb);
-    snprintf(msg, sizeof msg, "%s and %s overlap (an output overlaps another range)", na, nb);
-    return arg_error(fn, msg);
-  });
-}
-
-// The arguments of cs_bundle_adjust: the images (camera_args), the gauge codes, the parameters, the buffers, then the
-// outputs against each other, the tracks, d_use and every set's records (overlap_sweep).
-static int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
-                       const double *ts, const unsigned char *fixed, const int *offsets, int numTracks,
-                       const int *members, int numMembers, const unsigned char *use, const double *points,
-                       int maxIterations, int maxLinearIterations, double linearTol, double maxError,
-                       const double *R_out, const double *t_out, const float *errors, const unsigned char *inlier,
-                       const double *cost_out)
-{
-  int r = camera_args(fn, sets, numImages, Ks, Rs, ts, numTracks, numMembers);
-  if (r < 0) return r;
-  char bad[128];
-  for (int a = 0; fixed && a < numImages; a++)
-    if (fixed[a] > 4) {
-      snprintf(bad, sizeof bad, "fixed[%d] must be 0 (free), 1 (held) or 2..4 (t[fixed - 2] held)", a);
-      return arg_error(fn, bad);
-    }
-  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
-  if (maxLinearIterations < 1 || maxLinearIterations > 10000)
-    return arg_error(fn, "maxLinearIterations must be in [1, 10000]");
-  if (!(linearTol > 0.0) || !(linearTol < 1.0)) return arg_error(fn, "linearTol must be in (0, 1)");
-  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
-  if (numImages > 0 && (!R_out || !t_out)) return arg_error(fn, "numImages > 0 needs R_out and t_out");
-  if (!cost_out) return arg_error(fn, "cost_out must not be NULL");
-  if (numTracks > 0 && (!offsets || !points)) return arg_error(fn, "numTracks > 0 needs d_offsets and d_points");
-  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
-  if ((reinterpret_cast<uintptr_t>(offsets) & 3) != 0 || (reinterpret_cast<uintptr_t>(errors) & 3) != 0)
-    return arg_error(fn, "d_offsets and d_errors must be 4-byte aligned");
-  if ((reinterpret_cast<uintptr_t>(members) & 7) != 0 || (reinterpret_cast<uintptr_t>(points) & 7) != 0)
-    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
-  // the outputs (kind 0, written; owners 0 d_points, 1 d_errors, 2 d_inlier), the inputs (kind 1, read; owners
-  // 0 d_offsets, 1 d_members, 2 d_use) and every set's records (kind 2, read)
-  std::vector<SweepRange> rs;
-  rs.reserve((size_t)numImages + 6);
-  if (numTracks > 0) {
-    sweep_add(rs, points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
-    sweep_add(rs, offsets, ((size_t)numTracks + 1) * sizeof(int), 0, 1, false);
-  }
-  if (errors) sweep_add(rs, errors, (size_t)numMembers * sizeof(float), 1, 0, true);
-  if (inlier) sweep_add(rs, inlier, (size_t)numMembers, 2, 0, true);
-  sweep_add(rs, members, (size_t)numMembers * sizeof(int2), 1, 1, false);
-  if (use) sweep_add(rs, use, (size_t)numMembers, 2, 1, false);
-  for (int a = 0; a < numImages; a++) sweep_add(rs, sets[a].pts, record_bytes(sets[a].n), a, 2, false);
-  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
-    static const char *const outs[3] = {"d_points", "d_errors", "d_inlier"};
-    static const char *const ins[3] = {"d_offsets", "d_members", "d_use"};
-    auto name = [&](const SweepRange &z, char *buf, size_t n) {
-      if (z.kind == 0) snprintf(buf, n, "%s", outs[z.owner]);
-      else if (z.kind == 1) snprintf(buf, n, "%s", ins[z.owner]);
-      else snprintf(buf, n, "sets[%d].pts", z.owner);
-    };
-    const SweepRange &a = x.kind < y.kind || (x.kind == y.kind && x.owner <= y.owner) ? x : y;
-    const SweepRange &b = &a == &x ? y : x;
-    char na[32], nb[32], msg[128];
-    name(a, na, sizeof na);
-    name(b, nb, sizeof nb);
-    snprintf(msg, sizeof msg, "%s and %s overlap (an output overlaps another range)", na, nb);
-    return arg_error(fn, msg);
-  });
-}
-
-// The arguments of cs_absolute_pose_batch: the counts and tables, every job (named jobs[p]) and its K, the parameters,
-// the outputs, then every per-feature output against the other outputs, every record range, every pointOf and the
-// points (overlap_sweep).
-static int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
-                     const double *Ks, int numLoops, double maxError)
-{
-  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
-  if (numJobs > 0 && (!jobs || !Ks)) return arg_error(fn, "numJobs > 0 needs jobs and Ks");
-  if (numPoints < 0) return arg_error(fn, "numPoints must be >= 0");
-  if (numPoints > 0 && !points) return arg_error(fn, "numPoints > 0 needs d_points");
-  if ((reinterpret_cast<uintptr_t>(points) & 7) != 0) return arg_error(fn, "d_points must be 8-byte aligned");
-  char bad[128] = "";
-  for (int p = 0; p < numJobs && !bad[0]; p++) {
-    const cs_pose_job &j = jobs[p];
-    if (j.n < 0) snprintf(bad, sizeof bad, "jobs[%d]: n must be >= 0", p);
-    else if (j.n > 0 && (!j.pts || !j.pointOf)) snprintf(bad, sizeof bad, "jobs[%d]: n > 0 needs pts and pointOf", p);
-    else if ((reinterpret_cast<uintptr_t>(j.pointOf) & 3) != 0 || (reinterpret_cast<uintptr_t>(j.errors) & 3) != 0)
-      snprintf(bad, sizeof bad, "jobs[%d]: pointOf and errors must be 4-byte aligned", p);
-  }
-  if (bad[0]) return arg_error(fn, bad);
-  for (int p = 0; p < numJobs; p++) {
-    char name[96];
-    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
-    const int r = check_intrinsics(name, Ks + 9 * (size_t)p, "Ks[p]");
-    if (r < 0) return r;
-  }
-  if (numLoops < 1 || numLoops > 65536) return arg_error(fn, "numLoops must be in [1, 65536]");
-  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
-  // the per-feature outputs (kind 0 errors, 1 inlier: written), the records (2), pointOf (3) and d_points (4)
-  static const char *const kinds[5] = {"errors", "inlier", "pts", "pointOf", "d_points"};
-  std::vector<SweepRange> rs;
-  rs.reserve(4 * (size_t)numJobs + 1);
-  for (int p = 0; p < numJobs; p++) {
-    const cs_pose_job &j = jobs[p];
-    if (j.n <= 0) continue;
-    if (j.errors) sweep_add(rs, j.errors, (size_t)j.n * sizeof(float), p, 0, true);
-    if (j.inlier) sweep_add(rs, j.inlier, (size_t)j.n, p, 1, true);
-    sweep_add(rs, j.pts, record_bytes(j.n), p, 2, false);
-    sweep_add(rs, j.pointOf, (size_t)j.n * sizeof(int), p, 3, false);
-  }
-  sweep_add(rs, points, (size_t)numPoints * 3 * sizeof(double), 0, 4, false);
-  return overlap_sweep(rs, [&](const SweepRange &x, const SweepRange &y) {
-    const SweepRange &a = x.out && (!y.out || x.owner <= y.owner) ? x : y;
-    const SweepRange &b = &a == &x ? y : x;
-    char na[48], nb[48], msg[160];
-    snprintf(na, sizeof na, "jobs[%d].%s", a.owner, kinds[a.kind]);
-    if (b.kind == 4) snprintf(nb, sizeof nb, "d_points");
-    else snprintf(nb, sizeof nb, "jobs[%d].%s", b.owner, kinds[b.kind]);
-    snprintf(msg, sizeof msg, "%s and %s overlap (a per-feature output overlaps another range)", na, nb);
-    return arg_error(fn, msg);
-  });
 }
 
 static VerifyCalib verify_calib(const double K1[9], const double K2[9])
@@ -1485,17 +941,6 @@ int cs_match_mutual_host(void *h_s1, int n1, void *h_s2, int n2, float minScore,
                       return match_sync("cs_match_mutual", d1, n1, d2, n2, &mu, mode, (SiftPoint *)h_s1,
                                         (SiftPoint *)h_s2, ms);
                     });
-}
-
-// The idx / score buffers of a knn call: [n1][2] each.
-static int knn_out_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const int *idx,
-                        const float *score)
-{
-  if (n1 > 0 && (!idx || !score)) return arg_error(fn, "n1 > 0 needs idx and score buffers");
-  const void *buf[2] = {idx, score};
-  const size_t bytes[2] = {(size_t)n1 * 2 * sizeof(int), (size_t)n1 * 2 * sizeof(float)};
-  const char *const name[2] = {"idx", "score"};
-  return check_buffers(fn, s1, n1, s2, n2, buf, bytes, name, 2);
 }
 
 int cs_match_knn2(const void *d_s1, int n1, const void *d_s2, int n2, int *d_idx, float *d_score, int mode, double *ms)

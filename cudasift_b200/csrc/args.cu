@@ -1,0 +1,494 @@
+// args.cu -- the argument checks of the C ABI (args.h).  Alignment rules differ between calls and stay with each call;
+// every call that takes buffers declares them to one range checker, ArgRanges.
+#include "args.h"
+#include "common.cuh"
+
+#include <algorithm>
+#include <climits>
+#include <cmath>
+#include <cstdarg>
+#include <memory>
+
+namespace cs {
+
+int arg_error(const char *fn, const char *fmt, ...)
+{
+  char bad[256];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(bad, sizeof bad, fmt, ap);
+  va_end(ap);
+  set_error("%s: invalid argument (CS_E_ARG): %s", fn, bad);
+  return CS_E_ARG;
+}
+
+static bool misaligned(const void *p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) != 0; }
+static size_t record_bytes(int n) { return n > 0 ? (size_t)n * sizeof(SiftPoint) : 0; }
+
+// The byte ranges of one call: each has a kind (names[kind] is a printf pattern that takes the owner, such as
+// "jobs[%d].inliers" or "d_points") and an owner (a table entry, or 0), and is exclusive when it may share no byte with
+// any other range (it is written, or must stand alone).
+// A single call's ranges (at most 4) stay in `local`, so the per-job checks of a batch allocate nothing; a batch
+// call's move to `heap`, sized for the `most` it may add.
+struct ArgRanges {
+  struct Range {
+    uintptr_t lo, hi;
+    int kind, owner;
+    bool exclusive;
+  };
+  const char *const *names;
+  Range local[4], *rs = local;
+  std::unique_ptr<Range[]> heap;
+  size_t n = 0, cap = 4;
+
+  ArgRanges(const char *const *names_, size_t most) : names(names_)
+  {
+    if (most > cap) grow(most);
+  }
+  void grow(size_t want)
+  {
+    Range *p = new Range[want];
+    std::copy(rs, rs + n, p);
+    heap.reset(p);
+    rs = p;
+    cap = want;
+  }
+  void add(const void *p, size_t bytes, int kind, int owner, bool exclusive)
+  {
+    if (!bytes) return;
+    if (n == cap) grow(2 * cap);
+    const uintptr_t lo = reinterpret_cast<uintptr_t>(p);
+    rs[n++] = {lo, lo + bytes, kind, owner, exclusive};
+  }
+  // The ranges sorted by (start, kind, owner) and swept once (O(n log n)): a range that starts before an earlier one
+  // ends overlaps it.  The first conflict found is reported as "<A> and <B> overlap", A the range of the lower
+  // (kind, owner).
+  int check(const char *fn)
+  {
+    std::sort(rs, rs + n, [](const Range &a, const Range &b) {
+      return a.lo != b.lo ? a.lo < b.lo : a.kind != b.kind ? a.kind < b.kind : a.owner < b.owner;
+    });
+    const Range *anyEnd = nullptr, *exclEnd = nullptr;   // the earlier ranges (and exclusive ones) that end last
+    for (const Range *x_ = rs; x_ != rs + n; x_++) {
+      const Range &x = *x_;
+      const Range *hit = nullptr;
+      if (x.exclusive && anyEnd && anyEnd->hi > x.lo) hit = anyEnd;
+      else if (exclEnd && exclEnd->hi > x.lo) hit = exclEnd;
+      if (hit) {
+        const bool xFirst = x.kind != hit->kind ? x.kind < hit->kind : x.owner < hit->owner;
+        const Range &a = xFirst ? x : *hit, &b = xFirst ? *hit : x;
+        char na[48], nb[48];
+        snprintf(na, sizeof na, names[a.kind], a.owner);
+        snprintf(nb, sizeof nb, names[b.kind], b.owner);
+        return arg_error(fn, "%s and %s overlap", na, nb);
+      }
+      if (!anyEnd || x.hi > anyEnd->hi) anyEnd = &x;
+      if (x.exclusive && (!exclEnd || x.hi > exclEnd->hi)) exclEnd = &x;
+    }
+    return 0;
+  }
+};
+
+int check_sets(const char *fn, const void *s1, int n1, const void *s2, int n2, int mode)
+{
+  if (n1 < 0 || n2 < 0) return arg_error(fn, "n1 and n2 must be >= 0");
+  if ((n1 > 0 && !s1) || (n2 > 0 && !s2)) return arg_error(fn, "a set with records needs a pointer");
+  if (mode < 0 || mode > 2) return arg_error(fn, "mode must be 0 (auto), 1 (exact) or 2 (tensor)");
+  return 0;
+}
+
+// The buffers of a single call: buf[k] of bytes[k] bytes, named names[k], then the records of set 1 and set 2 (named
+// names[n] and names[n + 1]).  Every non-empty buffer is 8-byte aligned and shares no byte with another buffer or a
+// record range; the record ranges may overlap each other unless the call writes them.
+static int call_buffers(const char *fn, const void *s1, int n1, const void *s2, int n2, bool setsWritten,
+                        const void *const *buf, const size_t *bytes, const char *const *names, int n)
+{
+  for (int k = 0; k < n; k++)
+    if (bytes[k] && misaligned(buf[k], 8)) return arg_error(fn, "%s must be 8-byte aligned", names[k]);
+  ArgRanges rs(names, n + 2);
+  for (int k = 0; k < n; k++) rs.add(buf[k], bytes[k], k, 0, true);
+  rs.add(s1, record_bytes(n1), n, 0, setsWritten);
+  rs.add(s2, record_bytes(n2), n + 1, 0, setsWritten);
+  return rs.check(fn);
+}
+
+// The pairs buffer of the mutual and ratio matchers: maxPairs int2.
+static int check_pairs(const char *fn, const void *s1, int n1, const void *s2, int n2, bool setsWritten,
+                       const void *pairs, int maxPairs)
+{
+  if (maxPairs < 0) return arg_error(fn, "maxPairs must be >= 0");
+  if (maxPairs > 0 && !pairs) return arg_error(fn, "maxPairs > 0 needs a pairs buffer");
+  static const char *const names[3] = {"pairs", "s1", "s2"};
+  const size_t bytes = (size_t)maxPairs * sizeof(int2);
+  return call_buffers(fn, s1, n1, s2, n2, setsWritten, &pairs, &bytes, names, 1);
+}
+
+int mutual_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs,
+                int mode)
+{
+  const int r = check_sets(fn, s1, n1, s2, n2, mode);
+  return r < 0 ? r : check_pairs(fn, s1, n1, s2, n2, true, pairs, maxPairs);
+}
+
+int ratio_args(const char *fn, const void *s1, int n1, const void *s2, int n2, float maxRatio, float maxDistance,
+               const void *pairs, int maxPairs, int mode)
+{
+  int r;
+  if ((r = check_sets(fn, s1, n1, s2, n2, mode)) < 0) return r;
+  if (std::isnan(maxRatio) || std::isnan(maxDistance)) return arg_error(fn, "maxRatio and maxDistance must not be NaN");
+  return check_pairs(fn, s1, n1, s2, n2, false, pairs, maxPairs);
+}
+
+int verify_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                int model, int numLoops, float thresh, const double *model_out, const void *inliers, int maxInliers)
+{
+  int r;
+  if ((r = check_sets(fn, s1, n1, s2, n2, 0)) < 0) return r;              // mode 0: the verifier has one path
+  if (numPairs < 0) return arg_error(fn, "numPairs must be >= 0");
+  if (numPairs > 0 && !pairs) return arg_error(fn, "numPairs > 0 needs a pairs buffer");
+  if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL)
+    return arg_error(fn, "model must be 1 (homography) or 2 (fundamental)");
+  if (numLoops < 1 || numLoops > 65536) return arg_error(fn, "numLoops must be in [1, 65536]");
+  if (!std::isfinite(thresh) || thresh <= 0.0f) return arg_error(fn, "thresh must be finite and > 0");
+  if (!model_out) return arg_error(fn, "model_out must not be NULL");
+  if (maxInliers < 0) return arg_error(fn, "maxInliers must be >= 0");
+  if (maxInliers > 0 && !inliers) return arg_error(fn, "maxInliers > 0 needs an inliers buffer");
+  static const char *const names[4] = {"pairs", "inliers", "s1", "s2"};
+  const void *buf[2] = {pairs, inliers};
+  const size_t bytes[2] = {(size_t)numPairs * sizeof(int2), (size_t)maxInliers * sizeof(int2)};
+  return call_buffers(fn, s1, n1, s2, n2, false, buf, bytes, names, 2);
+}
+
+int knn_out_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const int *idx, const float *score)
+{
+  if (n1 > 0 && (!idx || !score)) return arg_error(fn, "n1 > 0 needs idx and score buffers");
+  static const char *const names[4] = {"idx", "score", "s1", "s2"};
+  const void *buf[2] = {idx, score};
+  const size_t bytes[2] = {(size_t)n1 * 2 * sizeof(int), (size_t)n1 * 2 * sizeof(float)};
+  return call_buffers(fn, s1, n1, s2, n2, false, buf, bytes, names, 2);
+}
+
+int guided_args(const char *fn, int model, const double *model_in, float thresh)
+{
+  if (model != CS_GEOM_HOMOGRAPHY && model != CS_GEOM_FUNDAMENTAL)
+    return arg_error(fn, "model must be 1 (homography) or 2 (fundamental)");
+  if (!model_in) return arg_error(fn, "model_in must not be NULL");
+  double s = 0.0;
+  for (int k = 0; k < 9; k++) {
+    if (!std::isfinite(model_in[k])) return arg_error(fn, "model_in must be finite");
+    s += model_in[k] * model_in[k];
+  }
+  if (!(s > 0.0 && std::isfinite(s))) return arg_error(fn, "model_in must not be all zero (and its norm must be finite)");
+  if (!std::isfinite(thresh) || thresh <= 0.0f) return arg_error(fn, "thresh must be finite and > 0");
+  return 0;
+}
+
+// Intrinsics: a finite row-major pinhole K (skew allowed) with K[3] = K[6] = K[7] = 0, K[8] = 1, K[0] > 0 and K[4] > 0.
+static int check_intrinsics(const char *fn, const double *K, const char *name)
+{
+  bool ok = K != nullptr;
+  for (int k = 0; k < 9 && ok; k++) ok = std::isfinite(K[k]);
+  if (!ok || K[3] != 0.0 || K[6] != 0.0 || K[7] != 0.0 || K[8] != 1.0 || !(K[0] > 0.0) || !(K[4] > 0.0))
+    return arg_error(fn, "%s must be a finite pinhole matrix (K[3] = K[6] = K[7] = 0, K[8] = 1, K[0] > 0, K[4] > 0)",
+                     name);
+  return 0;
+}
+
+int essential_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                   const double *K1, const double *K2, int numLoops, float thresh, const double *E, const double *R,
+                   const double *t, const void *inliers, int maxInliers)
+{
+  int r;
+  if (!E || !R || !t) return arg_error(fn, "E_out, R_out and t_out must not be NULL");
+  if ((r = verify_args(fn, s1, n1, s2, n2, pairs, numPairs, CS_GEOM_FUNDAMENTAL, numLoops, thresh, E, inliers,
+                       maxInliers)) < 0)
+    return r;
+  if ((r = check_intrinsics(fn, K1, "K1")) < 0) return r;
+  return check_intrinsics(fn, K2, "K2");
+}
+
+// The common arguments, every job's as its single call checks them (named "<fn>: jobs[p]"), the total pair count, then
+// the inlier buffers against every other job's buffers and records.
+int verify_batch_args(const char *fn, const cs_verify_job *jobs, int numJobs, int model, int numLoops, float thresh,
+                      const double *K1s, const double *K2s, bool essential)
+{
+  int r;
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs a jobs array");
+  if (essential && numJobs > 0 && (!K1s || !K2s)) return arg_error(fn, "K1s and K2s must not be NULL");
+  long long total = 0;
+  const double dummy = 0.0;
+  for (int p = 0; p < numJobs; p++) {
+    const cs_verify_job &j = jobs[p];
+    char name[96];
+    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
+    if ((r = verify_args(name, j.s1, j.n1, j.s2, j.n2, j.pairs, j.numPairs, model, numLoops, thresh, &dummy, j.inliers,
+                         j.maxInliers)) < 0)
+      return r;
+    if (essential && ((r = check_intrinsics(name, K1s + 9 * (size_t)p, "K1s[p]")) < 0 ||
+                      (r = check_intrinsics(name, K2s + 9 * (size_t)p, "K2s[p]")) < 0))
+      return r;
+    if ((total += j.numPairs) > INT_MAX) return arg_error(fn, "the total numPairs exceeds INT_MAX at jobs[%d]", p);
+  }
+  // an inlier buffer (written) may overlap no other range; a job's own were checked above
+  static const char *const names[4] = {"jobs[%d].inliers", "jobs[%d].pairs", "jobs[%d].s1", "jobs[%d].s2"};
+  ArgRanges rs(names, 4 * (size_t)numJobs);
+  for (int p = 0; p < numJobs; p++) {
+    const cs_verify_job &j = jobs[p];
+    rs.add(j.inliers, (size_t)j.maxInliers * sizeof(int2), 0, p, true);
+    rs.add(j.pairs, (size_t)j.numPairs * sizeof(int2), 1, p, false);
+    rs.add(j.s1, record_bytes(j.n1), 2, p, false);
+    rs.add(j.s2, record_bytes(j.n2), 3, p, false);
+  }
+  return rs.check(fn);
+}
+
+// Every set of a cs_match_set table (named sets[s]).
+static int check_set_table(const char *fn, const cs_match_set *sets, int numSets)
+{
+  for (int s = 0; s < numSets; s++) {
+    if (sets[s].n < 0) return arg_error(fn, "sets[%d]: n must be >= 0", s);
+    if (sets[s].n > 0 && !sets[s].pts) return arg_error(fn, "sets[%d]: a set with records needs a pointer", s);
+  }
+  return 0;
+}
+
+// The common arguments, every set (named sets[s]) and job (jobs[p]), then the pair buffers against each other and
+// against every set's records.
+int ratio_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                     float maxRatio, float maxDistance, const int *counts_out)
+{
+  if (numSets < 0 || numSets > 65536) return arg_error(fn, "numSets must be in [0, 65536]");
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numSets > 0 && !sets) return arg_error(fn, "numSets > 0 needs a sets array");
+  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs a jobs array");
+  if (numJobs > 0 && !counts_out) return arg_error(fn, "counts_out must not be NULL");
+  if (std::isnan(maxRatio) || std::isnan(maxDistance)) return arg_error(fn, "maxRatio and maxDistance must not be NaN");
+  const int r = check_set_table(fn, sets, numSets);
+  if (r < 0) return r;
+  for (int p = 0; p < numJobs; p++) {
+    const cs_match_job &j = jobs[p];
+    if (j.set1 < 0 || j.set1 >= numSets || j.set2 < 0 || j.set2 >= numSets)
+      return arg_error(fn, "jobs[%d]: set1 and set2 must be in [0, numSets)", p);
+    if (j.maxPairs < 0) return arg_error(fn, "jobs[%d]: maxPairs must be >= 0", p);
+    if (j.maxPairs > 0 && !j.pairs) return arg_error(fn, "jobs[%d]: maxPairs > 0 needs a pairs buffer", p);
+    if (j.maxPairs > 0 && misaligned(j.pairs, 8)) return arg_error(fn, "jobs[%d]: pairs must be 8-byte aligned", p);
+  }
+  static const char *const names[2] = {"jobs[%d].pairs", "sets[%d].pts"};
+  ArgRanges rs(names, (size_t)numSets + numJobs);
+  for (int p = 0; p < numJobs; p++) rs.add(jobs[p].pairs, (size_t)jobs[p].maxPairs * sizeof(int2), 0, p, true);
+  for (int s = 0; s < numSets; s++) rs.add(sets[s].pts, record_bytes(sets[s].n), 1, s, false);
+  return rs.check(fn);
+}
+
+// Those of cs_match_ratio_batch, then every job's model as the single call checks it (named jobs[p]).
+int guided_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                      const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
+                      const int *counts_out)
+{
+  int r;
+  if ((r = ratio_batch_args(fn, sets, numSets, jobs, numJobs, maxRatio, maxDistance, counts_out)) < 0) return r;
+  if (numJobs > 0 && (!models || !models_in)) return arg_error(fn, "models and models_in must not be NULL");
+  for (int p = 0; p < numJobs; p++) {
+    char name[96];
+    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
+    if ((r = guided_args(name, models[p], models_in + 9 * (size_t)p, thresh)) < 0) return r;
+  }
+  return 0;
+}
+
+// The counts and tables, every image (imageSizes[a]) and list (lists[p]), the outputs, then the outputs against each
+// other and every pair list.
+int tracks_args(const char *fn, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
+                int minLength, const int *trackOf, const int *offsets, int maxTracks, const int *members,
+                int maxMembers, int *N, int *P)
+{
+  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
+  if (numLists < 0 || numLists > (1 << 24)) return arg_error(fn, "numLists must be in [0, 2^24]");
+  if (numImages > 0 && !imageSizes) return arg_error(fn, "numImages > 0 needs an imageSizes array");
+  if (numLists > 0 && !lists) return arg_error(fn, "numLists > 0 needs a lists array");
+  long long n = 0, pairs = 0;
+  for (int a = 0; a < numImages; a++) {
+    if (imageSizes[a] < 0) return arg_error(fn, "imageSizes[%d] must be >= 0", a);
+    if ((n += imageSizes[a]) > INT_MAX) return arg_error(fn, "imageSizes[%d]: the sizes pass INT_MAX", a);
+  }
+  for (int p = 0; p < numLists; p++) {
+    const cs_track_list &l = lists[p];
+    if (l.image1 < 0 || l.image1 >= numImages || l.image2 < 0 || l.image2 >= numImages)
+      return arg_error(fn, "lists[%d]: image1 and image2 must be in [0, numImages)", p);
+    if (l.numPairs < 0) return arg_error(fn, "lists[%d]: numPairs must be >= 0", p);
+    if (l.numPairs > 0 && !l.pairs) return arg_error(fn, "lists[%d]: numPairs > 0 needs a pairs buffer", p);
+    if (l.numPairs > 0 && misaligned(l.pairs, 8)) return arg_error(fn, "lists[%d]: pairs must be 8-byte aligned", p);
+    if ((pairs += l.numPairs) > INT_MAX) return arg_error(fn, "lists[%d]: the pair counts pass INT_MAX", p);
+  }
+  if (minLength < 2) return arg_error(fn, "minLength must be >= 2");
+  if (maxTracks < 0 || maxMembers < 0) return arg_error(fn, "maxTracks and maxMembers must be >= 0");
+  if (maxTracks > 0 && !offsets) return arg_error(fn, "maxTracks > 0 needs d_offsets");
+  if (maxMembers > 0 && !members) return arg_error(fn, "maxMembers > 0 needs d_members");
+  if (misaligned(trackOf, 4) || misaligned(offsets, 4))
+    return arg_error(fn, "d_trackOf and d_offsets must be 4-byte aligned");
+  if (misaligned(members, 8)) return arg_error(fn, "d_members must be 8-byte aligned");
+  // the outputs (written) and the pair lists (read)
+  static const char *const names[4] = {"d_trackOf", "d_offsets", "d_members", "lists[%d].pairs"};
+  ArgRanges rs(names, (size_t)numLists + 3);
+  if (trackOf) rs.add(trackOf, (size_t)n * sizeof(int), 0, 0, true);
+  if (offsets) rs.add(offsets, ((size_t)maxTracks + 1) * sizeof(int), 1, 0, true);
+  rs.add(members, (size_t)maxMembers * sizeof(int2), 2, 0, true);
+  for (int p = 0; p < numLists; p++) rs.add(lists[p].pairs, (size_t)lists[p].numPairs * sizeof(int2), 3, p, false);
+  *N = (int)n;
+  *P = (int)pairs;
+  return rs.check(fn);
+}
+
+// The images of cs_triangulate_tracks and cs_bundle_adjust: the counts, every set (sets[a]) and camera (Ks[a], Rs[a],
+// ts[a]).
+static int camera_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                       const double *ts, int numTracks, int numMembers)
+{
+  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
+  if (numTracks < 0) return arg_error(fn, "numTracks must be >= 0");
+  if (numMembers < 0) return arg_error(fn, "numMembers must be >= 0");
+  if (numImages > 0 && (!sets || !Ks || !Rs || !ts)) return arg_error(fn, "numImages > 0 needs sets, Ks, Rs and ts");
+  int r = check_set_table(fn, sets, numImages);
+  if (r < 0) return r;
+  for (int a = 0; a < numImages; a++) {
+    char name[32];
+    snprintf(name, sizeof name, "Ks[%d]", a);
+    if ((r = check_intrinsics(fn, Ks + 9 * (size_t)a, name)) < 0) return r;
+    const double *R = Rs + 9 * (size_t)a, *t = ts + 3 * (size_t)a;
+    bool ok = true;
+    for (int k = 0; k < 9; k++) ok = ok && std::isfinite(R[k]);
+    for (int i = 0; i < 3 && ok; i++)
+      for (int j = 0; j < 3; j++) {
+        const double d = R[3 * i] * R[3 * j] + R[3 * i + 1] * R[3 * j + 1] + R[3 * i + 2] * R[3 * j + 2];
+        ok = ok && std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-6;
+      }
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
+                       R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (!ok || !(det > 0.0))
+      return arg_error(fn, "Rs[%d] must be a finite rotation (R R^T = I within 1e-6, det R > 0)", a);
+    if (!std::isfinite(t[0]) || !std::isfinite(t[1]) || !std::isfinite(t[2]))
+      return arg_error(fn, "ts[%d] must be finite", a);
+  }
+  return 0;
+}
+
+// The images (camera_args), the parameters, the buffers, then the outputs against each other, the tracks and every
+// set's records.
+int triangulate_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                     const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
+                     int numTrials, double maxError, double minTriAngle, const double *points, const int *counts,
+                     const float *errors, const unsigned char *inlier)
+{
+  const int r = camera_args(fn, sets, numImages, Ks, Rs, ts, numTracks, numMembers);
+  if (r < 0) return r;
+  if (numTrials < 1 || numTrials > (1 << 20)) return arg_error(fn, "numTrials must be in [1, 2^20]");
+  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
+  if (!std::isfinite(minTriAngle) || !(minTriAngle >= 0.0) || !(minTriAngle < 180.0))
+    return arg_error(fn, "minTriAngle must be finite and in [0, 180)");
+  if (numTracks > 0 && !offsets) return arg_error(fn, "numTracks > 0 needs d_offsets");
+  if (numTracks > 0 && (!points || !counts)) return arg_error(fn, "numTracks > 0 needs d_points and d_counts");
+  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
+  if (misaligned(offsets, 4) || misaligned(counts, 4) || misaligned(errors, 4))
+    return arg_error(fn, "d_offsets, d_counts and d_errors must be 4-byte aligned");
+  if (misaligned(members, 8) || misaligned(points, 8))
+    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
+  // the outputs (written), the tracks and the records (read)
+  static const char *const names[7] = {"d_points", "d_counts", "d_errors", "d_inlier", "d_offsets", "d_members",
+                                       "sets[%d].pts"};
+  ArgRanges rs(names, (size_t)numImages + 6);
+  if (numTracks > 0) {
+    rs.add(points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
+    rs.add(counts, (size_t)numTracks * sizeof(int), 1, 0, true);
+    rs.add(offsets, ((size_t)numTracks + 1) * sizeof(int), 4, 0, false);
+  }
+  if (errors) rs.add(errors, (size_t)numMembers * sizeof(float), 2, 0, true);
+  if (inlier) rs.add(inlier, (size_t)numMembers, 3, 0, true);
+  rs.add(members, (size_t)numMembers * sizeof(int2), 5, 0, false);
+  for (int a = 0; a < numImages; a++) rs.add(sets[a].pts, record_bytes(sets[a].n), 6, a, false);
+  return rs.check(fn);
+}
+
+// The images (camera_args), the gauge codes, the parameters, the buffers, then the outputs against each other, the
+// tracks, d_use and every set's records.
+int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                const double *ts, const unsigned char *fixed, const int *offsets, int numTracks, const int *members,
+                int numMembers, const unsigned char *use, const double *points, int maxIterations,
+                int maxLinearIterations, double linearTol, double maxError, const double *R_out, const double *t_out,
+                const float *errors, const unsigned char *inlier, const double *cost_out)
+{
+  const int r = camera_args(fn, sets, numImages, Ks, Rs, ts, numTracks, numMembers);
+  if (r < 0) return r;
+  for (int a = 0; fixed && a < numImages; a++)
+    if (fixed[a] > 4) return arg_error(fn, "fixed[%d] must be 0 (free), 1 (held) or 2..4 (t[fixed - 2] held)", a);
+  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
+  if (maxLinearIterations < 1 || maxLinearIterations > 10000)
+    return arg_error(fn, "maxLinearIterations must be in [1, 10000]");
+  if (!(linearTol > 0.0) || !(linearTol < 1.0)) return arg_error(fn, "linearTol must be in (0, 1)");
+  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
+  if (numImages > 0 && (!R_out || !t_out)) return arg_error(fn, "numImages > 0 needs R_out and t_out");
+  if (!cost_out) return arg_error(fn, "cost_out must not be NULL");
+  if (numTracks > 0 && (!offsets || !points)) return arg_error(fn, "numTracks > 0 needs d_offsets and d_points");
+  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
+  if (misaligned(offsets, 4) || misaligned(errors, 4))
+    return arg_error(fn, "d_offsets and d_errors must be 4-byte aligned");
+  if (misaligned(members, 8) || misaligned(points, 8))
+    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
+  // the outputs (written), the inputs and the records (read)
+  static const char *const names[7] = {"d_points", "d_errors", "d_inlier", "d_offsets", "d_members", "d_use",
+                                       "sets[%d].pts"};
+  ArgRanges rs(names, (size_t)numImages + 6);
+  if (numTracks > 0) {
+    rs.add(points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
+    rs.add(offsets, ((size_t)numTracks + 1) * sizeof(int), 3, 0, false);
+  }
+  if (errors) rs.add(errors, (size_t)numMembers * sizeof(float), 1, 0, true);
+  if (inlier) rs.add(inlier, (size_t)numMembers, 2, 0, true);
+  rs.add(members, (size_t)numMembers * sizeof(int2), 4, 0, false);
+  if (use) rs.add(use, (size_t)numMembers, 5, 0, false);
+  for (int a = 0; a < numImages; a++) rs.add(sets[a].pts, record_bytes(sets[a].n), 6, a, false);
+  return rs.check(fn);
+}
+
+// The counts and tables, every job (named jobs[p]) and its K, the parameters, then every per-feature output against
+// the other outputs, every record range, every pointOf and the points.  Jobs with n <= 0 have no ranges.
+int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
+              const double *Ks, int numLoops, double maxError)
+{
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numJobs > 0 && (!jobs || !Ks)) return arg_error(fn, "numJobs > 0 needs jobs and Ks");
+  if (numPoints < 0) return arg_error(fn, "numPoints must be >= 0");
+  if (numPoints > 0 && !points) return arg_error(fn, "numPoints > 0 needs d_points");
+  if (misaligned(points, 8)) return arg_error(fn, "d_points must be 8-byte aligned");
+  for (int p = 0; p < numJobs; p++) {
+    const cs_pose_job &j = jobs[p];
+    if (j.n < 0) return arg_error(fn, "jobs[%d]: n must be >= 0", p);
+    if (j.n > 0 && (!j.pts || !j.pointOf)) return arg_error(fn, "jobs[%d]: n > 0 needs pts and pointOf", p);
+    if (misaligned(j.pointOf, 4) || misaligned(j.errors, 4))
+      return arg_error(fn, "jobs[%d]: pointOf and errors must be 4-byte aligned", p);
+  }
+  for (int p = 0; p < numJobs; p++) {
+    char name[96];
+    snprintf(name, sizeof name, "%s: jobs[%d]", fn, p);
+    const int r = check_intrinsics(name, Ks + 9 * (size_t)p, "Ks[p]");
+    if (r < 0) return r;
+  }
+  if (numLoops < 1 || numLoops > 65536) return arg_error(fn, "numLoops must be in [1, 65536]");
+  if (!std::isfinite(maxError) || !(maxError > 0.0)) return arg_error(fn, "maxError must be finite and > 0");
+  // the per-feature outputs (written), the records, pointOf and the points (read)
+  static const char *const names[5] = {"jobs[%d].errors", "jobs[%d].inlier", "jobs[%d].pts", "jobs[%d].pointOf",
+                                       "d_points"};
+  ArgRanges rs(names, 4 * (size_t)numJobs + 1);
+  for (int p = 0; p < numJobs; p++) {
+    const cs_pose_job &j = jobs[p];
+    if (j.n <= 0) continue;
+    if (j.errors) rs.add(j.errors, (size_t)j.n * sizeof(float), 0, p, true);
+    if (j.inlier) rs.add(j.inlier, (size_t)j.n, 1, p, true);
+    rs.add(j.pts, record_bytes(j.n), 2, p, false);
+    rs.add(j.pointOf, (size_t)j.n * sizeof(int), 3, p, false);
+  }
+  rs.add(points, (size_t)numPoints * 3 * sizeof(double), 4, 0, false);
+  return rs.check(fn);
+}
+
+}  // namespace cs

@@ -1,0 +1,58 @@
+// args.h -- the argument checks of the C ABI's matching, verification, tracks, triangulation, bundle adjustment and
+// absolute pose calls (args.cu).  Each returns 0, or CS_E_ARG with cs_last_error() naming the offending argument; none
+// makes a CUDA call, so they hold on a machine without a device.
+#pragma once
+
+#include "../../include/cudasift_b200.h"
+
+namespace cs {
+
+// CS_E_ARG, with "<fn>: invalid argument (CS_E_ARG): <fmt ...>" as the last error.
+int arg_error(const char *fn, const char *fmt, ...) __attribute__((format(printf, 2, 3)));
+
+// The two record sets and the path mode (0 auto, 1 exact, 2 tensor).
+int check_sets(const char *fn, const void *s1, int n1, const void *s2, int n2, int mode);
+// cs_match_mutual*: the sets, and a pairs buffer of maxPairs int2.  Both sets are written, so they must not overlap.
+int mutual_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int maxPairs,
+                int mode);
+// cs_match_ratio* and cs_match_guided*: the sets, the ratio parameters and a pairs buffer of maxPairs int2.
+int ratio_args(const char *fn, const void *s1, int n1, const void *s2, int n2, float maxRatio, float maxDistance,
+               const void *pairs, int maxPairs, int mode);
+// cs_verify_pairs* and cs_verify_models: the records are only read (they may overlap each other); the pair and inlier
+// buffers may overlap nothing.
+int verify_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                int model, int numLoops, float thresh, const double *model_out, const void *inliers, int maxInliers);
+// The idx / score buffers of a knn call: [n1][2] each.
+int knn_out_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const int *idx, const float *score);
+// The model and threshold of a guided call (the records and buffers are checked as for cs_match_knn2 / cs_match_ratio).
+int guided_args(const char *fn, int model, const double *model_in, float thresh);
+// cs_verify_essential*: those of cs_verify_pairs except model, the intrinsics and the three outputs.
+int essential_args(const char *fn, const void *s1, int n1, const void *s2, int n2, const void *pairs, int numPairs,
+                   const double *K1, const double *K2, int numLoops, float thresh, const double *E, const double *R,
+                   const double *t, const void *inliers, int maxInliers);
+// The batch calls: cs_verify_pairs_batch (essential false) and cs_verify_essential_batch, cs_match_ratio_batch,
+// cs_match_guided_batch, cs_build_tracks (*N and *P receive the feature and pair totals), cs_triangulate_tracks,
+// cs_bundle_adjust, and cs_absolute_pose_batch and cs_absolute_pose_models.
+int verify_batch_args(const char *fn, const cs_verify_job *jobs, int numJobs, int model, int numLoops, float thresh,
+                      const double *K1s, const double *K2s, bool essential);
+int ratio_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                     float maxRatio, float maxDistance, const int *counts_out);
+int guided_batch_args(const char *fn, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                      const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
+                      const int *counts_out);
+int tracks_args(const char *fn, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
+                int minLength, const int *trackOf, const int *offsets, int maxTracks, const int *members,
+                int maxMembers, int *N, int *P);
+int triangulate_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                     const double *ts, const int *offsets, int numTracks, const int *members, int numMembers,
+                     int numTrials, double maxError, double minTriAngle, const double *points, const int *counts,
+                     const float *errors, const unsigned char *inlier);
+int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                const double *ts, const unsigned char *fixed, const int *offsets, int numTracks, const int *members,
+                int numMembers, const unsigned char *use, const double *points, int maxIterations,
+                int maxLinearIterations, double linearTol, double maxError, const double *R_out, const double *t_out,
+                const float *errors, const unsigned char *inlier, const double *cost_out);
+int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
+              const double *Ks, int numLoops, double maxError);
+
+}  // namespace cs
