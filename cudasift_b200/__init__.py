@@ -21,7 +21,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
            "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
-           "BundleAdjust"]
+           "BundleAdjust", "TrainVocabulary", "AssignWords", "RetrievePairs"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -93,6 +93,9 @@ def lib():
         "cs_match_ratio_batch": (ip, [vp, ip, vp, ip, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_match_guided_batch": (ip, [vp, ip, vp, ip, vp, vp, fp, fp, fp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_build_tracks": (ip, [vp, ip, vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, c.POINTER(c.c_double)]),
+        "cs_vocab_assign": (ip, [vp, ip, vp, ip, vp, vp, c.POINTER(c.c_double)]),
+        "cs_vocab_train": (ip, [vp, ip, ip, ip, c.c_ulonglong, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_retrieve_pairs": (ip, [vp, ip, vp, ip, ip, vp, vp, vp, vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_triangulate_tracks": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, c.c_ulonglong,
                                        vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_bundle_adjust": (ip, [vp, ip, vp, vp, vp, vp, vp, ip, vp, ip, vp, vp, ip, ip, c.c_double, c.c_double,
@@ -766,6 +769,78 @@ def BuildTracks(imageSizes, lists, minLength=2, dropConflicting=True):
         for buf in bufs:
             buf.free()
     return offsets, members, trackOf, stats, ms.value
+
+
+def _set_table(datas):
+    return (MatchSet * max(len(datas), 1))(*[MatchSet(d.d_data, d.numPts) for d in datas])
+
+
+def TrainVocabulary(datas, numWords, maxIterations=10, seed=0):
+    """A visual vocabulary of numWords unit-length words by spherical k-means over every feature of datas, in one call
+    (cs_vocab_train).  Returns (vocab: a SiftData of numWords records whose descriptors are the words, trace float64
+    [iterations run, 4] of {changed assignments, words without members, fallback rows, mean best score}, stats int64
+    [4] as the header describes them, ms)."""
+    vocab = InitSiftData(SiftData(), int(numWords))
+    trace = np.zeros((max(int(maxIterations), 0), 4))
+    stats, ms = np.zeros(4, np.int64), ctypes.c_double(0.0)
+    try:
+        _check(lib().cs_vocab_train(_set_table(datas) if datas else None, len(datas), int(numWords),
+                                    int(maxIterations), int(seed), vocab.d_data, _ptr(trace) if len(trace) else None,
+                                    _ptr(stats), ctypes.byref(ms)), "TrainVocabulary")
+    except Exception:
+        FreeSiftData(vocab)
+        raise
+    vocab.numPts = int(numWords)
+    return vocab, trace[:int(stats[0])].copy(), stats, ms.value
+
+
+def AssignWords(datas, vocab):
+    """The word of every feature of datas in one call (cs_vocab_assign): j1 of match_knn2 against vocab's records, or
+    -1.  Returns (wordOf int32 [sum of numPts], feature g = numPts of the earlier sets + i as in BuildTracks, stats
+    uint64 [5] as the header describes them, ms)."""
+    N = sum(int(d.numPts) for d in datas)
+    stats, ms = np.zeros(5, np.uint64), ctypes.c_double(0.0)
+    wordOf = np.zeros(N, np.int32)
+    buf = DeviceBuffer(max(N, 1) * 4)
+    try:
+        _check(lib().cs_vocab_assign(_set_table(datas) if datas else None, len(datas), vocab.d_data, int(vocab.numPts),
+                                     buf.ptr if N else None, _ptr(stats), ctypes.byref(ms)), "AssignWords")
+        if N:
+            wordOf = buf.download(np.int32, N)
+    finally:
+        buf.free()
+    return wordOf, stats, ms.value
+
+
+def RetrievePairs(imageSizes, wordOf, numWords, topK=50):
+    """Every image's topK neighbours by tf-idf and the deduplicated pair table in one call (cs_retrieve_pairs):
+    imageSizes[a] is image a's feature count and wordOf (int32 [sum of the sizes]) AssignWords' output.  Returns
+    (neighbours int32 [N, topK] (-1: none), scores float64 [N, topK] (cosine of the fixed-point tf-idf vectors), pairs
+    int32 [P, 2] of {a < b} in ascending order, ready as MatchSiftDataRatioBatch's jobs, stats int64 [7], ms)."""
+    sizes = np.ascontiguousarray(np.asarray(imageSizes, np.int64).reshape(-1).astype(np.int32))
+    words = np.ascontiguousarray(np.asarray(wordOf, np.int32).reshape(-1))
+    I, N, K = len(sizes), int(sizes.sum(dtype=np.int64)), int(topK)
+    if len(words) != N:
+        raise ValueError("wordOf: one per feature, %d, not %d" % (N, len(words)))
+    maxPairs = I * K
+    neighbours, scores = np.full((I, K), -1, np.int32), np.zeros((I, K))
+    stats, ms = np.zeros(7, np.int64), ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(N, 1) * 4), DeviceBuffer(max(I * K, 1) * 4), DeviceBuffer(max(I * K, 1) * 8),
+            DeviceBuffer(max(maxPairs, 1) * 8)]
+    try:
+        if N:
+            bufs[0].upload(words)
+        P = _check(lib().cs_retrieve_pairs(_ptr(sizes) if I else None, I, bufs[0].ptr, int(numWords), K, bufs[1].ptr,
+                                           bufs[2].ptr, None, bufs[3].ptr, maxPairs, _ptr(stats), ctypes.byref(ms)),
+                   "RetrievePairs")
+        if N and I:
+            neighbours = bufs[1].download(np.int32, I * K).reshape(I, K)
+            scores = bufs[2].download(np.float64, I * K).reshape(I, K)
+        pairs = bufs[3].download(np.int32, 2 * P).reshape(P, 2) if P else np.zeros((0, 2), np.int32)
+    finally:
+        for buf in bufs:
+            buf.free()
+    return neighbours, scores, pairs, stats, ms.value
 
 
 def _per_image(x, shape, n, what):

@@ -1339,6 +1339,82 @@ int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *l
   return (int)st[6];
 }
 
+int cs_vocab_assign(const cs_match_set *sets, int numSets, const void *d_vocab, int numWords, int *d_wordOf,
+                    unsigned long long stats_out[5], double *ms)
+{
+  const char *fn = "cs_vocab_assign";
+  if (ms) *ms = 0.0;
+  int M = 0;
+  int r = vocab_assign_args(fn, sets, numSets, d_vocab, numWords, d_wordOf, &M);
+  if (r < 0) return r;
+  if (stats_out)
+    for (int k = 0; k < 5; k++) stats_out[k] = 0;
+  if (M == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  VocabAssign va;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return vocab_assign_enqueue(*c, sets, numSets, d_vocab, numWords, d_wordOf, nullptr, va);
+       })) < 0)
+    return r;
+  if (stats_out) vocab_assign_stats(va, stats_out);
+  return 0;
+}
+
+int cs_vocab_train(const cs_match_set *sets, int numSets, int numWords, int maxIterations, unsigned long long seed,
+                   void *d_vocab, double *trace_out, long long stats_out[4], double *ms)
+{
+  const char *fn = "cs_vocab_train";
+  if (ms) *ms = 0.0;
+  int M = 0;
+  int r = vocab_train_args(fn, sets, numSets, numWords, maxIterations, d_vocab, &M);
+  if (r < 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  std::vector<double> trace((size_t)4 * maxIterations);
+  long long st[4] = {0, 0, 0, 0};
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return vocab_train(*c, sets, numSets, numWords, maxIterations, seed, static_cast<SiftPoint *>(d_vocab),
+                            trace.data(), st);
+       })) < 0)
+    return r;
+  if (trace_out) std::copy(trace.begin(), trace.end(), trace_out);
+  if (stats_out)
+    for (int k = 0; k < 4; k++) stats_out[k] = st[k];
+  return (int)st[0];
+}
+
+int cs_retrieve_pairs(const int *imageSizes, int numImages, const int *d_wordOf, int numWords, int topK,
+                      int *d_neighbours, double *d_scores, double *d_idf, int *d_pairs, int maxPairs,
+                      long long stats_out[7], double *ms)
+{
+  const char *fn = "cs_retrieve_pairs";
+  if (ms) *ms = 0.0;
+  int N = 0;
+  int r = retrieve_args(fn, imageSizes, numImages, d_wordOf, numWords, topK, d_neighbours, d_scores, d_idf, d_pairs,
+                        maxPairs, &N);
+  if (r < 0) return r;
+  if (stats_out)
+    for (int k = 0; k < 7; k++) stats_out[k] = 0;
+  if (N == 0) return 0;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return retrieve_enqueue(*c, imageSizes, numImages, d_wordOf, numWords, topK, d_neighbours, d_scores, d_idf,
+                                 d_pairs, maxPairs);
+       })) < 0)
+    return r;
+  const unsigned long long *st = c->h_retrieve.as<const unsigned long long>();
+  if (stats_out) {
+    for (int k = 0; k < 7; k++) stats_out[k] = (long long)st[k];
+    stats_out[4] = c->retrieveWaves;
+  }
+  return (int)st[5];
+}
+
 int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
                           const int *d_offsets, int numTracks, const int *d_members, int numMembers, int numTrials,
                           double maxError, double minTriAngle, unsigned long long seed, double *d_points, int *d_counts,

@@ -450,6 +450,89 @@ int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const d
   return rs.check(fn);
 }
 
+// The set table of the vocabulary calls and the feature total *M (at most INT_MAX).
+static int vocab_sets(const char *fn, const cs_match_set *sets, int numSets, int numWords, int *M)
+{
+  if (numSets < 0 || numSets > 65536) return arg_error(fn, "numSets must be in [0, 65536]");
+  if (numSets > 0 && !sets) return arg_error(fn, "numSets > 0 needs a sets array");
+  if (numWords < 1 || numWords > (1 << 18)) return arg_error(fn, "numWords must be in [1, 2^18]");
+  int r;
+  if ((r = check_set_table(fn, sets, numSets)) < 0) return r;
+  long long n = 0;
+  for (int s = 0; s < numSets; s++)
+    if ((n += sets[s].n) > INT_MAX) return arg_error(fn, "sets[%d]: the set sizes pass INT_MAX", s);
+  *M = (int)n;
+  return 0;
+}
+
+int vocab_assign_args(const char *fn, const cs_match_set *sets, int numSets, const void *vocab, int numWords,
+                      const int *wordOf, int *M)
+{
+  int r;
+  if ((r = vocab_sets(fn, sets, numSets, numWords, M)) < 0) return r;
+  if (!vocab) return arg_error(fn, "d_vocab must not be NULL");
+  if (misaligned(vocab, 16)) return arg_error(fn, "d_vocab must be 16-byte aligned");
+  if (*M > 0 && !wordOf) return arg_error(fn, "sets with features need d_wordOf");
+  if (misaligned(wordOf, 4)) return arg_error(fn, "d_wordOf must be 4-byte aligned");
+  // the output (written), the vocabulary and the records (read)
+  static const char *const names[3] = {"d_wordOf", "d_vocab", "sets[%d].pts"};
+  ArgRanges rs(names, (size_t)numSets + 2);
+  rs.add(wordOf, (size_t)*M * sizeof(int), 0, 0, true);
+  rs.add(vocab, record_bytes(numWords), 1, 0, false);
+  for (int s = 0; s < numSets; s++) rs.add(sets[s].pts, record_bytes(sets[s].n), 2, s, false);
+  return rs.check(fn);
+}
+
+int vocab_train_args(const char *fn, const cs_match_set *sets, int numSets, int numWords, int maxIterations,
+                     const void *vocab, int *M)
+{
+  int r;
+  if ((r = vocab_sets(fn, sets, numSets, numWords, M)) < 0) return r;
+  if (numWords > *M) return arg_error(fn, "numWords must not exceed the feature count (%d)", *M);
+  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
+  if (!vocab) return arg_error(fn, "d_vocab must not be NULL");
+  if (misaligned(vocab, 16)) return arg_error(fn, "d_vocab must be 16-byte aligned");
+  static const char *const names[2] = {"d_vocab", "sets[%d].pts"};
+  ArgRanges rs(names, (size_t)numSets + 1);
+  rs.add(vocab, record_bytes(numWords), 0, 0, true);
+  for (int s = 0; s < numSets; s++) rs.add(sets[s].pts, record_bytes(sets[s].n), 1, s, false);
+  return rs.check(fn);
+}
+
+int retrieve_args(const char *fn, const int *imageSizes, int numImages, const int *wordOf, int numWords, int topK,
+                  const int *neighbours, const double *scores, const double *idf, const int *pairs, int maxPairs,
+                  int *N)
+{
+  if (numImages < 0 || numImages > 65536) return arg_error(fn, "numImages must be in [0, 65536]");
+  if (numImages > 0 && !imageSizes) return arg_error(fn, "numImages > 0 needs an imageSizes array");
+  long long n = 0;
+  for (int a = 0; a < numImages; a++) {
+    if (imageSizes[a] < 0) return arg_error(fn, "imageSizes[%d] must be >= 0", a);
+    if ((n += imageSizes[a]) > INT_MAX) return arg_error(fn, "imageSizes[%d]: the sizes pass INT_MAX", a);
+  }
+  if (numWords < 1 || numWords > (1 << 18)) return arg_error(fn, "numWords must be in [1, 2^18]");
+  if (topK < 1 || topK > 1024) return arg_error(fn, "topK must be in [1, 1024]");
+  if (maxPairs < 0) return arg_error(fn, "maxPairs must be >= 0");
+  if (n > 0 && !wordOf) return arg_error(fn, "images with features need d_wordOf");
+  if (numImages > 0 && (!neighbours || !scores)) return arg_error(fn, "numImages > 0 needs d_neighbours and d_scores");
+  if (maxPairs > 0 && !pairs) return arg_error(fn, "maxPairs > 0 needs d_pairs");
+  if (misaligned(wordOf, 4) || misaligned(neighbours, 4))
+    return arg_error(fn, "d_wordOf and d_neighbours must be 4-byte aligned");
+  if (misaligned(scores, 8) || misaligned(idf, 8) || misaligned(pairs, 8))
+    return arg_error(fn, "d_scores, d_idf and d_pairs must be 8-byte aligned");
+  // the outputs (written) and the words (read)
+  static const char *const names[5] = {"d_wordOf", "d_neighbours", "d_scores", "d_idf", "d_pairs"};
+  ArgRanges rs(names, 5);
+  const size_t lists = (size_t)numImages * topK;
+  rs.add(wordOf, (size_t)n * sizeof(int), 0, 0, false);
+  rs.add(neighbours, lists * sizeof(int), 1, 0, true);
+  rs.add(scores, lists * sizeof(double), 2, 0, true);
+  if (idf) rs.add(idf, (size_t)numWords * sizeof(double), 3, 0, true);
+  rs.add(pairs, (size_t)maxPairs * sizeof(int2), 4, 0, true);
+  *N = (int)n;
+  return rs.check(fn);
+}
+
 // The counts and tables, every job (named jobs[p]) and its K, the parameters, then every per-feature output against
 // the other outputs, every record range, every pointOf and the points.  Jobs with n <= 0 have no ranges.
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,

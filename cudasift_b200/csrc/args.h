@@ -54,5 +54,13 @@ int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const d
                 const float *errors, const unsigned char *inlier, const double *cost_out);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
+// cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.
+int vocab_assign_args(const char *fn, const cs_match_set *sets, int numSets, const void *vocab, int numWords,
+                      const int *wordOf, int *M);
+int vocab_train_args(const char *fn, const cs_match_set *sets, int numSets, int numWords, int maxIterations,
+                     const void *vocab, int *M);
+int retrieve_args(const char *fn, const int *imageSizes, int numImages, const int *wordOf, int numWords, int topK,
+                  const int *neighbours, const double *scores, const double *idf, const int *pairs, int maxPairs,
+                  int *N);
 
 }  // namespace cs

@@ -6,6 +6,7 @@
 #include <cstdlib>
 #include <cstdint>
 #include <algorithm>
+#include <functional>
 #include <map>
 #include <vector>
 
@@ -353,6 +354,15 @@ struct DeviceCtx {
   PinnedBuffer h_bundle;                   // the result words and the trace (copied back), then the camera table
   // cs_verify_*: the states a call copies back, and its job table
   PinnedBuffer h_verify;
+  // cs_vocab_train: the set table and start draws, the assignments, best scores, sort pairs, word bounds, tile
+  // partials and sort storage (cs_vocab_assign uses the batch buffers of cs_match_ratio_batch only)
+  GrowBuffer vocab;
+  PinnedBuffer h_vocab;                    // the set table and draws (uploaded), the partials and empty-word counts
+  // cs_retrieve_pairs: the statistics, image table, keys, postings, inverted file, word and image bounds, idf, the
+  // query accumulators of a wave, the candidate pair keys and the cub storage
+  GrowBuffer retrieve;
+  PinnedBuffer h_retrieve;                 // the statistics (copied back), then the image table
+  int retrieveWaves = 0;                   // the waves of the last cs_retrieve_pairs call
 
   // pinned host words, allocated by ensure()
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
@@ -464,6 +474,23 @@ struct RatioBatchOut {
 // the non-empty jobs.
 int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
                         float maxRatio, float maxDistance, bool crossCheck, RatioBatchOut *out);
+// A wave of knn directions once its four shared launches are in: its jobs (input indices, in order), its pair-job
+// table (device) and pair CTAs, and its neighbour lists: the rows of its directions one after the other, rows in all.
+struct KnnWave {
+  const std::vector<int> &jobs;
+  const PairJob *pairJobs;
+  int numJobs, pairCtas;
+  const int2 *idx;
+  const float2 *score;
+  int rows;
+};
+using KnnWaveFinish = std::function<int(const KnnWave &)>;
+// The waves of ratio_batch_enqueue with the last step of each wave left to finish (launched on c.stream after the
+// exact fallback; name heads the stage timing and lastStage names the step).  ratio_batch_enqueue is this with the
+// ratio flags and pair writes.
+int knn_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                      bool crossCheck, RatioBatchOut *out, const char *name, const char *lastStage,
+                      const KnnWaveFinish &finish);
 // the exact top-2 scan of the rows the wave's resolve listed ({direction, row} entries, *numEntries of them)
 int launch_knn_list_fallback(DeviceCtx &c, const MbDir *dirs, const int2 *entries, const unsigned int *numEntries,
                              int cap);
@@ -520,6 +547,35 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
 // eight statistics reach c.h_tracks (unsigned long long) by the caller's synchronize.
 int tracks_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const cs_track_list *lists, int numLists,
                    int minLength, bool drop, int *trackOf, int *offsets, int maxTracks, int *members, int maxMembers);
+
+// ---- vocabulary and retrieval (vocab.cu) ------------------------------------------------------------------------
+// One assignment call: the sets with the vocabulary appended, the jobs (a, vocabulary), each set's first global id,
+// where each job's counters land (RatioBatchOut) and the waves run.
+struct VocabAssign {
+  std::vector<cs_match_set> sets;
+  std::vector<cs_match_job> jobs;
+  std::vector<int> base;
+  std::vector<RatioBatchOut> out;
+  int waves = 0;
+};
+// The waves of cs_vocab_assign (argument-checked) on c.stream, without a synchronize: wordOf[base_a + i] = j1 of row i
+// of set a, and with best its score.
+int vocab_assign_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const void *vocab, int numWords,
+                         int *wordOf, float *best, VocabAssign &va);
+// after the synchronize: groups re-scored, exact chains, fallback rows, gated sets, waves
+void vocab_assign_stats(const VocabAssign &va, unsigned long long st[5]);
+// The start draws of cs_vocab_train (host): the first numWords distinct indices of the counter-based generator.
+std::vector<int> vocab_start_draws(unsigned long long seed, int M, int numWords);
+// cs_vocab_train (argument-checked), synchronizing once per iteration; trace [maxIterations][4] is written whole.
+// Returns the iterations run.
+int vocab_train(DeviceCtx &c, const cs_match_set *sets, int numSets, int numWords, int maxIterations,
+                unsigned long long seed, SiftPoint *vocab, double *trace, long long stats[4]);
+// cs_retrieve_pairs (argument-checked, some feature) on c.stream, without a synchronize; the seven statistics reach
+// c.h_retrieve (unsigned long long) by the caller's synchronize, the wave count c.retrieveWaves.
+constexpr size_t RT_WAVE_BYTES = (size_t)256 << 20;
+int retrieve_queries_per_wave(int numImages);
+int retrieve_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const int *wordOf, int numWords, int topK,
+                     int *neighbours, double *scores, double *idf, int *pairs, int maxPairs);
 
 // ---- triangulation (triangulate.cu) -----------------------------------------------------------------------------
 // The launch of cs_triangulate_tracks (argument-checked, numTracks > 0) on c.stream, without a synchronize; the eight

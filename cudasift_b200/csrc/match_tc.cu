@@ -899,10 +899,11 @@ void match_tensor_stats(DeviceCtx &c, unsigned long long stats[4])
   stats[2] = (unsigned long long)h[4 + 0] + h[8 + 0];
 }
 
-// ------------------------------------------------------------------------------ batched ratio matching
+// ------------------------------------------------------------------------------ batched knn directions
 // A wave (cs_match_ratio_batch states the rule): consecutive non-empty jobs whose scratch -- per distinct set its
 // operand tiles and norms, per direction its top-3 tables, neighbour lists and fallback entries -- fits MB_BUDGET.
-// Every wave runs the same six launches: prep, GEMM, knn resolve, list fallback, ratio flags, pair writes.
+// Every wave runs the same four launches (prep, GEMM, knn resolve, list fallback), then the caller's last step:
+// ratio flags and pair writes for cs_match_ratio_batch, the word copy for cs_vocab_assign.
 #define MB_BUDGET ((size_t)256 << 20)
 static size_t mb_set_bytes(int n) { return (size_t)idivup(n, T3_MT) * T3_MT * (T3_A_BYTES / T3_MT + sizeof(float)); }
 static size_t mb_dir_bytes(int n1)
@@ -1053,6 +1054,15 @@ static void mb_fill(DeviceCtx &c, const MbWave &v, const cs_match_set *sets, con
 int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
                         float maxRatio, float maxDistance, bool cross, RatioBatchOut *out)
 {
+  return knn_batch_enqueue(c, sets, numSets, jobs, numJobs, cross, out, "ratio-batch", "pairs", [&](const KnnWave &w) {
+    return launch_ratio_pairs_batch(c, w.pairJobs, w.numJobs, w.pairCtas, maxRatio, maxDistance);
+  });
+}
+
+int knn_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, const cs_match_job *jobs, int numJobs,
+                      bool cross, RatioBatchOut *out, const char *name, const char *lastStage,
+                      const KnnWaveFinish &finish)
+{
   const std::vector<MbWave> waves = mb_waves(sets, numSets, jobs, numJobs, cross);
   if (waves.empty()) return 0;
   size_t tiles = 0, slots = 0, rows = 0, state = 0, tab = 0, pin = 0;
@@ -1107,11 +1117,13 @@ int ratio_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, int numSets, con
     CS_CUDA(cudaGetLastError());
     if ((r = launch_knn_list_fallback(c, dd, entries, numEntries, v.rows)) < 0) return r;
     if (tev) cudaEventRecord(tev[4], st);
-    if ((r = launch_ratio_pairs_batch(c, dj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
+    const KnnWave w = {v.jobs, dj, J, v.pairCtas, c.mbLists.as<int2>(),
+                       reinterpret_cast<const float2 *>(c.mbLists.as<int2>() + v.rows), v.rows};
+    if ((r = finish(w)) < 0) return r;
     if (tev) cudaEventRecord(tev[5], st);
     CS_CUDA(cudaMemcpyAsync(hp + v.stateAt, state, v.zeroWords * sizeof(unsigned int), cudaMemcpyDeviceToHost, st));
-    static const char *const stages[] = {"prep", "gemm", "resolve", "exact-fallback", "pairs"};
-    if (tev) report_stage_times(tev, stages, 5, "ratio-batch timing %d jobs %d directions %d units", J, D, v.units);
+    const char *const stages[] = {"prep", "gemm", "resolve", "exact-fallback", lastStage};
+    if (tev) report_stage_times(tev, stages, 5, "%s timing %d jobs %d directions %d units", name, J, D, v.units);
   }
   return 0;
 }

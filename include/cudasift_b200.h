@@ -448,6 +448,90 @@ int cs_build_tracks(const int *imageSizes, int numImages, const cs_track_list *l
                     int dropConflicting, int *d_trackOf, int *d_offsets, int maxTracks, int *d_members, int maxMembers,
                     long long stats_out[8], double *ms);
 
+/* Image retrieval: a visual vocabulary (Sivic & Zisserman 2003; spherical k-means, Dhillon & Modha 2001), the word of
+ * every feature, and each image's top-k neighbours by tf-idf as the pair list to match (COLMAP's vocabulary-tree
+ * matching, without the tree).
+ * - Vocabulary: a device array of numWords SiftPoint records whose data[128] holds the words; every other field is 0.
+ *   It is a cs_match_set {d_vocab, numWords}: it can go wherever records go and be saved with the memcpy calls.
+ * - Word of a descriptor x: j1 of cs_match_knn2(x, vocab), the lowest index with the largest positive reference score
+ *   (the sequential FMA chain), or -1 when no score is positive (an all-zero descriptor).  This is the contract.
+ *
+ * cs_vocab_assign: d_wordOf[base_a + i] = the word of row i of sets[a], base_a = n_0 + ... + n_{a-1} (the global
+ * feature id of cs_build_tracks, so d_wordOf lines up with d_trackOf).
+ * - Equivalence: bit for bit cs_match_knn2(sets[a], vocab)'s j1 for every set, in every mode, rows of the exact
+ *   fallback and sets caught by the bad-input gate (a value of the set or the vocabulary not finite or |x| >= 8)
+ *   included.
+ * - Waves: those of cs_match_ratio_batch with crossCheck 0 over the jobs (a, vocabulary), a = 0 .. numSets - 1 (the
+ *   vocabulary is one set converted once per wave).  Each wave issues 5 kernel launches (convert, GEMM, resolve, exact
+ *   fallback, word copy), so a call issues 5 x waves (cs_launch_count).
+ * - stats_out (may be NULL) [5]: the totals over the sets of cs_match_stats' [0] groups re-scored, [1] exact chains and
+ *   [2] fallback rows (every row of a gated set), [3] the sets caught by the gate, [4] the waves.
+ * - CS_E_ARG, before any CUDA call, naming the offending sets[s] or buffer: numSets outside [0, 65536], NULL sets with
+ *   numSets > 0, a set with n < 0 or a NULL pts with n > 0, a feature total above INT_MAX, numWords outside [1, 2^18],
+ *   NULL or not 16-byte aligned d_vocab, NULL d_wordOf with features, d_wordOf not 4-byte aligned, and d_wordOf
+ *   overlapping the vocabulary or any set's records.  A call without features returns 0 and makes no CUDA call.  The
+ *   call synchronises once, at the end; *ms (may be NULL) gets its event time.  Returns 0 or CS_E_*. */
+int cs_vocab_assign(const cs_match_set *sets, int numSets, const void *d_vocab, int numWords, int *d_wordOf,
+                    unsigned long long stats_out[5], double *ms);
+
+/* cs_vocab_train: Lloyd iterations of spherical k-means over every feature of the sets, M descriptors in global order;
+ * writes numWords records to d_vocab.
+ * - Start: word k is the descriptor of the k-th distinct index of the draws idx = ((splitmix64(seed +
+ *   0x9E3779B97F4A7C15 * counter) >> 32) * M) >> 32, counter = 0, 1, 2, ... (uint64; splitmix64 as cs_verify_pairs),
+ *   a repeated index skipped.  Identical start descriptors are allowed: the tie rule empties all but the lowest copy.
+ * - Iteration t: (1) every descriptor's word by cs_vocab_assign; (2) the assignments that changed since iteration
+ *   t - 1 are counted (all of them at t = 0), and none stops the loop; (3) otherwise, per word with members: s =
+ *   the members' descriptors summed per component in float64 in ascending global id, norm = the 128 squares summed in
+ *   float64 in ascending component (no fused multiply-add), word = float32(s / sqrt(norm)).  A word without members, or
+ *   with norm 0, keeps its descriptor.  maxIterations = 0 returns the start words.
+ * - trace_out (may be NULL) [maxIterations][4], float64, per iteration run: the changed assignments, the words without
+ *   members (at a stop: those of the previous iteration, whose assignment it repeats), the fallback rows of the
+ *   assignment, and the mean best score over the assigned descriptors: per tile of 1024 features thread t (of 256) sums
+ *   the scores of tile + 4t .. 4t + 3 in order from 0, then x[t] += x[t + s] for s = 128, 64, .., 1, then the tiles in
+ *   ascending order, divided by the assigned count (0 without one).  Rows past the last iteration are 0.
+ * - stats_out (may be NULL) [4]: iterations run, 1 if the loop stopped on no change, M, kernel launches.
+ * - Launches: 1 (start words), then per iteration the 5 x waves of the assignment and 1 compare, and unless it stops 2
+ *   more (run bounds, word update); a stable cub::DeviceRadixSort of (word + 1, global id) pairs between them is not
+ *   counted.  The call synchronises with the host once per iteration.  Two calls with the same inputs give the same
+ *   bytes.
+ * - CS_E_ARG, before any CUDA call: the set checks of cs_vocab_assign, numWords outside [1, 2^18] or above M,
+ *   maxIterations outside [0, 1000], NULL or not 16-byte aligned d_vocab, and d_vocab overlapping any set's records.
+ * Returns the iterations run, or CS_E_*. */
+int cs_vocab_train(const cs_match_set *sets, int numSets, int numWords, int maxIterations, unsigned long long seed,
+                   void *d_vocab, double *trace_out, long long stats_out[4], double *ms);
+
+/* cs_retrieve_pairs: every image's top-k neighbours by tf-idf and the deduplicated pair table.  imageSizes (host) and
+ * d_wordOf (device, N = the sum of the sizes, in the global order of cs_vocab_assign) give each feature's image and
+ * word.
+ * - Counts: tf_a(w) = the features of image a with word w; words outside [0, numWords) are ignored.  df_w = the images
+ *   with tf > 0; N' = the images with at least one word.
+ * - Weights: idf_w = log(N' / df_w) in float64 on the device (0 for df_w = 0), written to d_idf (may be NULL);
+ *   x = tf idf, v_a(w) = x / sqrt(sum of x^2 over the image's words in ascending w, float64, no fused multiply-add) (0
+ *   when that sum is 0); q_a(w) = rint(v_a(w) 2^22) (round half to even), an int32.
+ * - Score: score(a, b) = sum_w q_a(w) q_b(w), exact in int64 (below 2^45 by Cauchy-Schwarz), so the order of the
+ *   64-bit atomics that form it reaches no output.  Similarity = score 2^-44 as a double (exact).
+ * - d_neighbours [numImages][topK] int, d_scores [numImages][topK] double: the images b != a with score > 0, by score
+ *   descending then b ascending, padded with -1 and 0.
+ * - d_pairs: {min(a, b), max(a, b)} of every listed neighbour, deduplicated, in ascending (first, second), int pairs
+ *   as cs_match_job's; the first min(count, maxPairs) are written.  Returns the full count, or CS_E_*.
+ * - Waves: the queries run in consecutive ranges of max(1, floor(256 MiB / (8 numImages))) images (their int64
+ *   accumulators).
+ * - stats_out (may be NULL) [7]: [0] N', [1] postings (distinct (image, word)), [2] sum of df_w^2, [3] score updates
+ *   (sum over w of the squared count of postings with q != 0: those with q = 0 add nothing and are skipped), [4] waves,
+ *   [5] the full pair count, [6] ignored features.
+ * - Launches: 6 + 2 x waves (keys, postings, idf, weights, word bounds; per wave scatter and top-k select; pair
+ *   writes).  cub sorts, run-length encoding and unique passes between them are not counted.  The call synchronises
+ *   once, at the end; *ms (may be NULL) gets its event time.
+ * - CS_E_ARG, before any CUDA call, naming the offending imageSizes[a] or buffer: numImages outside [0, 65536], NULL
+ *   imageSizes with numImages > 0, imageSizes[a] < 0, N above INT_MAX, numWords outside [1, 2^18], topK outside
+ *   [1, 1024], maxPairs < 0, NULL d_wordOf with N > 0, NULL d_neighbours or d_scores with numImages > 0, NULL d_pairs
+ *   with maxPairs > 0, misaligned buffers (d_wordOf, d_neighbours 4 bytes; d_scores, d_idf, d_pairs 8), and an output
+ *   overlapping another output or d_wordOf.  N == 0 returns 0 with zero statistics, writes nothing and makes no CUDA
+ *   call. */
+int cs_retrieve_pairs(const int *imageSizes, int numImages, const int *d_wordOf, int numWords, int topK,
+                      int *d_neighbours, double *d_scores, double *d_idf, int *d_pairs, int maxPairs,
+                      long long stats_out[7], double *ms);
+
 /* Triangulation of feature tracks with known cameras (COLMAP's point_triangulator, without bundle adjustment): per
  * track, RANSAC over two-view DLT points, the inliers by reprojection error, one multi-view DLT refit.  The tracks of
  * cs_build_tracks can be passed unchanged: d_offsets, d_members and numMembers = its stats_out[7].
