@@ -853,6 +853,13 @@ def _per_image(x, shape, n, what):
     return np.ascontiguousarray(x)
 
 
+def _tracks(offsets, members):
+    """BuildTracks' offsets and members as contiguous int32 arrays, with the track and member counts."""
+    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1).astype(np.int32))
+    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1, 2).astype(np.int32))
+    return off, mem, max(len(off) - 1, 0), len(mem)
+
+
 def TriangulateTracks(datas, Ks, Rs, ts, offsets, members, numTrials=256, maxError=4.0, minTriAngle=1.5, seed=0):
     """A 3-D point per feature track with known cameras, in one call (cs_triangulate_tracks): RANSAC over two-view DLT
     points, inliers by reprojection error below maxError pixels, one multi-view refit.  datas[a] holds image a's
@@ -861,10 +868,8 @@ def TriangulateTracks(datas, Ks, Rs, ts, offsets, members, numTrials=256, maxErr
     counts int32 [T], errors float32 [M], inlier bool [M], stats int64 [8] as the header describes them, ms)."""
     S = len(datas)
     K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
-    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1).astype(np.int32))
-    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1, 2).astype(np.int32))
-    T, M = max(len(off) - 1, 0), len(mem)
-    sets = (MatchSet * max(S, 1))(*[MatchSet(d.d_data, d.numPts) for d in datas])
+    off, mem, T, M = _tracks(offsets, members)
+    sets = _set_table(datas)
     points, counts = np.full((T, 3), np.nan), np.zeros(T, np.int32)
     errors, inlier = np.full(M, np.nan, np.float32), np.zeros(M, bool)
     stats, ms = np.zeros(8, np.int64), ctypes.c_double(0.0)
@@ -903,9 +908,7 @@ def BundleAdjust(datas, Ks, Rs, ts, offsets, members, points, use=None, fixed=No
     accepted}, stats int64 [8] as the header describes them, ms)."""
     S = len(datas)
     K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
-    off = np.ascontiguousarray(np.asarray(offsets, np.int64).reshape(-1).astype(np.int32))
-    mem = np.ascontiguousarray(np.asarray(members, np.int64).reshape(-1, 2).astype(np.int32))
-    T, M = max(len(off) - 1, 0), len(mem)
+    off, mem, T, M = _tracks(offsets, members)
     pts = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
     if len(pts) != T:
         raise ValueError("points: one per track, %d, not %d" % (T, len(pts)))
@@ -921,7 +924,7 @@ def BundleAdjust(datas, Ks, Rs, ts, offsets, members, points, use=None, fixed=No
     u = None if use is None else np.ascontiguousarray(np.asarray(use).reshape(-1).astype(np.uint8))
     if u is not None and len(u) != M:
         raise ValueError("use: one per member, %d, not %d" % (M, len(u)))
-    sets = (MatchSet * max(S, 1))(*[MatchSet(d.d_data, d.numPts) for d in datas])
+    sets = _set_table(datas)
     R_out, t_out = np.zeros((S, 3, 3)), np.zeros((S, 3))
     errors, inlier = np.full(M, np.nan, np.float32), np.zeros(M, bool)
     cost, trace = np.zeros(2), np.zeros((max(int(maxIterations), 0), 4))

@@ -160,17 +160,6 @@ __device__ __forceinline__ double ba_damp(double d, double lam) { return d + lam
 // The free components of a camera with fixed code f: 0 all six, 1 none, 2..4 all but t[f - 2] (bits 0-2 w, 3-5 t).
 __device__ __forceinline__ int ba_free_mask(int f) { return f == 0 ? 0x3f : f == 1 ? 0 : 0x3f & ~(1 << (f + 1)); }
 
-// Member validity (cs_triangulate_tracks' rule): a known image, a feature inside its set, a finite position.
-__device__ __forceinline__ bool ba_member(const BaCam *cams, int numImages, int2 af, float &x, float &y)
-{
-  if ((unsigned)af.x >= (unsigned)numImages) return false;
-  const BaCam &c = cams[af.x];
-  if ((unsigned)af.y >= (unsigned)c.n) return false;
-  x = c.pts[af.y].xpos;
-  y = c.pts[af.y].ypos;
-  return isfinite(x) && isfinite(y);
-}
-
 __device__ __forceinline__ double ba_depth(const double *R, const double *t, const double (&X)[3])
 {
   return R[6] * X[0] + R[7] * X[1] + R[8] * X[2] + t[2];
@@ -221,7 +210,7 @@ __device__ __forceinline__ int ba_used(const BaParams &p, int k, int &invalid, F
   for (int m = lo; m < hi; m++) {
     float x, y;
     const int2 af = p.members[m];
-    if (!ba_member(p.cams, p.numImages, af, x, y)) { invalid++; continue; }
+    if (!tr_member(p.cams, p.numImages, af, x, y)) { invalid++; continue; }
     if (!finite || (p.use && !p.use[m])) continue;
     const BaCam &c = p.cams[af.x];
     if (!(ba_depth(c.R, c.t, X) > 0.0)) continue;
@@ -289,10 +278,7 @@ __device__ __forceinline__ void ba_totals(const double *part, int n, int stride,
     for (int i = (int)threadIdx.x; i < n; i += 32)
 #pragma unroll
       for (int j = 0; j < K; j++) v[j] += part[(size_t)i * stride + j];
-#pragma unroll
-    for (int o = 16; o; o >>= 1)
-#pragma unroll
-      for (int j = 0; j < K; j++) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+    vp_warp_sum(v);
     if (threadIdx.x == 0)
 #pragma unroll
       for (int j = 0; j < K; j++) s_tot[j] = v[j];
@@ -308,10 +294,7 @@ template <int K>
 __device__ __forceinline__ void ba_cta_partial(double (&v)[K], double *out)
 {
   __shared__ double s_w[BA_WARPS][K];
-#pragma unroll
-  for (int o = 16; o; o >>= 1)
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+  vp_warp_sum(v);
   if ((threadIdx.x & 31) == 0)
 #pragma unroll
     for (int j = 0; j < K; j++) s_w[threadIdx.x >> 5][j] = v[j];
@@ -330,10 +313,7 @@ __device__ __forceinline__ void ba_cta_partial(double (&v)[K], double *out)
 template <int K>
 __device__ __forceinline__ void ba_warp_partial(double (&v)[K], double *out)
 {
-#pragma unroll
-  for (int o = 16; o; o >>= 1)
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+  vp_warp_sum(v);
   if ((threadIdx.x & 31) == 0)
 #pragma unroll
     for (int j = 0; j < K; j++) out[j] = v[j];
@@ -361,10 +341,7 @@ __device__ __forceinline__ void ba_pieces(const BaParams &p, int N, F &&f)
 #pragma unroll
         for (int j = 0; j < NV; j++) acc[j] += v[j];
       }
-#pragma unroll
-      for (int o = 16; o; o >>= 1)
-#pragma unroll
-        for (int j = 0; j < NV; j++) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+      vp_warp_sum(acc);
       if (lane == 0)
 #pragma unroll
         for (int j = 0; j < NV; j++) p.pieces[(size_t)(t + a) * BA_PV + OFF + j] = acc[j];
@@ -713,14 +690,9 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams p)
           continue;
         }
         double Q[9];
-        vp_rodrigues(c.x, Q);
+        vp_rotate(c.x, c.R, c.Rc, Q);
 #pragma unroll
-        for (int i = 0; i < 3; i++) {
-#pragma unroll
-          for (int j = 0; j < 3; j++)
-            c.Rc[3 * i + j] = Q[3 * i] * c.R[j] + Q[3 * i + 1] * c.R[3 + j] + Q[3 * i + 2] * c.R[6 + j];
-          c.tc[i] = ((c.mask >> (3 + i)) & 1) ? c.t[i] + c.x[3 + i] : c.t[i];
-        }
+        for (int i = 0; i < 3; i++) c.tc[i] = ((c.mask >> (3 + i)) & 1) ? c.t[i] + c.x[3 + i] : c.t[i];
       }
       grid.sync();
       // I. the candidate's cost and its observations behind a camera
@@ -804,13 +776,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams p)
       float x, y, err = CUDART_NAN_F;
       unsigned char in = 0;
       const int2 af = p.members[m];
-      if (ba_member(p.cams, C, af, x, y) && has) {
-        double u[3];
-        tr_project(p.cams[af.x].P, X, u);
-        const double e2z2 = tr_err2z2(u, x, y);
-        in = u[2] > 0.0 && e2z2 < p.thr2 * (u[2] * u[2]);
-        err = u[2] > 0.0 ? (float)sqrt(e2z2 / (u[2] * u[2])) : CUDART_INF_F;
-      }
+      if (tr_member(p.cams, C, af, x, y) && has) tr_reproject(p.cams[af.x].P, X, x, y, p.thr2, err, in);
       if (p.errors) p.errors[m] = err;
       if (p.inlier) p.inlier[m] = in;
     }
@@ -824,26 +790,17 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams p)
   }
 }
 
-// One resident wave of the cooperative kernel (queried once per device); CS_E_CUDA without cooperative launch.
-int bundle_grid(int *grid)
+// One resident wave of the cooperative kernel; CS_E_CUDA without cooperative launch.
+int bundle_grid()
 {
-  static int gridOf[64];
-  int dev = 0;
+  int dev = 0, coop = 0;
   CS_CUDA(cudaGetDevice(&dev));
-  const int d = dev & 63;
-  if (gridOf[d] == 0) {
-    int sms = 0, perSm = 0, coop = 0;
-    CS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    if (!coop) {
-      set_error("cs_bundle_adjust: device %d does not support cooperative launches", dev);
-      return CS_E_CUDA;
-    }
-    CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    CS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, bundle_kernel, BA_THREADS, 0));
-    gridOf[d] = (perSm > 0 ? perSm : 1) * sms;
+  CS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  if (!coop) {
+    set_error("cs_bundle_adjust: device %d does not support cooperative launches", dev);
+    return CS_E_CUDA;
   }
-  *grid = gridOf[d];
-  return 0;
+  return resident_grid<bundle_kernel, BA_THREADS>();
 }
 
 }  // namespace
@@ -929,8 +886,8 @@ int bundle_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const 
   prm.maxIterations = maxIterations;
   prm.maxLinear = maxLinearIterations;
 
-  int wave = 0;
-  if ((r = bundle_grid(&wave)) < 0) return r;
+  const int wave = bundle_grid();
+  if (wave < 0) return wave;
   const cudaStream_t st = c.stream;
   CS_CUDA(cudaMemsetAsync(base, 0, zeroEnd, st));
   if (C) CS_CUDA(cudaMemcpyAsync(prm.cams, cams, (size_t)C * sizeof(BaCam), cudaMemcpyHostToDevice, st));

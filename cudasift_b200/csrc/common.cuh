@@ -51,6 +51,24 @@ extern thread_local bool g_exit_on_error;
 extern unsigned long long g_launches;   // kernels launched by this library
 inline void count_launch(int n = 1) { g_launches += n; }
 
+// One resident wave of Kernel at Threads per CTA and no dynamic shared memory: the CTAs an SM holds at once (at least
+// one) times the SM count, queried once per device; CS_E_CUDA when a query fails.
+template <auto Kernel, int Threads>
+int resident_grid()
+{
+  static int gridOf[64];
+  int dev = 0;
+  CS_CUDA(cudaGetDevice(&dev));
+  dev &= 63;
+  if (gridOf[dev] == 0) {
+    int sms = 0, perSm = 0;
+    CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    CS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, Kernel, Threads, 0));
+    gridOf[dev] = (perSm > 0 ? perSm : 1) * sms;
+  }
+  return gridOf[dev];
+}
+
 // ---- filter taps (host) ----------------------------------------------------------
 void scaledown_taps(float variance, float k[5]);                  // cudaSiftH.cu:315-324
 void lowpass_taps(float sigma, float k[9]);                       // cudaSiftH.cu:408-419

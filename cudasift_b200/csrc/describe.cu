@@ -321,26 +321,10 @@ describe_kernel(const __grid_constant__ DescribeParams P)
   }
 }
 
-// One resident wave: as many CTAs as the device holds at once (queried once per device).  A CTA whose first claim
-// is past the end of the queue exits at once.
-static int describe_grid()
-{
-  static int gridOf[64];
-  int dev = 0;
-  CS_CUDA(cudaGetDevice(&dev));
-  dev &= 63;
-  if (gridOf[dev] == 0) {
-    int sms = 0, perSm = 0;
-    CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    CS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, describe_kernel, DS_THREADS, 0));
-    gridOf[dev] = (perSm > 0 ? perSm : 1) * sms;
-  }
-  return gridOf[dev];
-}
-
+// One resident wave (resident_grid); a CTA whose first claim is past the end of the queue exits at once.
 int launch_describe(const DescribeParams &p, cudaStream_t st)
 {
-  const int grid = describe_grid();
+  const int grid = resident_grid<describe_kernel, DS_THREADS>();
   if (grid < 0) return grid;
   describe_kernel<<<grid, DS_THREADS, 0, st>>>(p);
   count_launch();

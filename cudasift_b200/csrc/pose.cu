@@ -404,10 +404,7 @@ __device__ bool ps_lm_terms(const PoseCorr *corr, int V, const double *K, const 
       s[27] += res[q] * res[q];
     }
   }
-#pragma unroll
-  for (int o = 16; o; o >>= 1)
-#pragma unroll
-    for (int i = 0; i < PS_SUMS; i++) s[i] += __shfl_xor_sync(0xffffffffu, s[i], o);
+  vp_warp_sum(s);
   return __all_sync(0xffffffffu, front);
 }
 
@@ -444,16 +441,13 @@ __device__ bool ps_lm_solve(const double (&s)[PS_SUMS], double lam, double (&x)[
   return true;
 }
 
-// R' = exp([w]x) R, t' = exp([w]x) t + delta (vp_rodrigues)
+// R' = exp([w]x) R, t' = exp([w]x) t + delta (vp_rotate)
 __device__ void ps_update(const double (&R)[9], const double (&t)[3], const double (&x)[6], double (&R1)[9],
                           double (&t1)[3])
 {
   double Q[9];
-  vp_rodrigues(x, Q);
-  for (int i = 0; i < 3; i++) {
-    for (int j = 0; j < 3; j++) R1[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
-    t1[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + x[3 + i];
-  }
+  vp_rotate(x, R, R1, Q);
+  for (int i = 0; i < 3; i++) t1[i] = Q[3 * i] * t[0] + Q[3 * i + 1] * t[1] + Q[3 * i + 2] * t[2] + x[3 + i];
 }
 
 __device__ int ps_count(const PoseCorr *corr, int V, const double (&P)[12], double thr2)
@@ -551,11 +545,7 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pose_refine_kernel(PoseWave w)
       unsigned char in = 0;
       if (has) {
         const double X[3] = {c.X[0], c.X[1], c.X[2]};
-        double u[3];
-        tr_project(P, X, u);
-        const double e2z2 = tr_err2z2(u, c.x, c.y);
-        in = u[2] > 0.0 && e2z2 < w.thr2 * (u[2] * u[2]);
-        err = u[2] > 0.0 ? (float)sqrt(e2z2 / (u[2] * u[2])) : CUDART_INF_F;
+        tr_reproject(P, X, c.x, c.y, w.thr2, err, in);
       }
       if (job.errors) job.errors[c.pos] = err;
       if (job.inlier) job.inlier[c.pos] = in;

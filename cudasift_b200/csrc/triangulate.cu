@@ -138,7 +138,8 @@ __device__ __forceinline__ bool tr_solve(const double (&s)[10], double (&X)[3])
   return isfinite(X[0]) && isfinite(X[1]) && isfinite(X[2]);
 }
 
-// tr_project, tr_err2z2 and tr_inlier (the reprojection inlier rule) are in vp_math.cuh.
+// tr_member (the member rule), tr_inlier (the reprojection inlier rule) and tr_reproject (the member outputs) are in
+// vp_math.cuh.
 __device__ __forceinline__ double tr_depth(const TrCam &c, const double (&X)[3])
 {
   return c.Rt[8] * X[0] + c.Rt[9] * X[1] + c.Rt[10] * X[2] + c.Rt[11];
@@ -174,15 +175,8 @@ __global__ void __launch_bounds__(TR_THREADS) triangulate_kernel(TrParams p)
         TrEntry e{0.0f, 0.0f, 0, m};
         if (m < hi) {
           const int2 af = p.members[m];
-          if ((unsigned)af.x < (unsigned)p.numImages) {
-            const TrCam &c = p.cams[af.x];
-            if ((unsigned)af.y < (unsigned)c.n) {
-              e.x = c.pts[af.y].xpos;
-              e.y = c.pts[af.y].ypos;
-              e.a = af.x;
-              ok = isfinite(e.x) && isfinite(e.y);
-            }
-          }
+          ok = tr_member(p.cams, p.numImages, af, e.x, e.y);
+          if (ok) e.a = af.x;
           if (!ok) {
             invalid++;
             if (p.errors) p.errors[m] = CUDART_NAN_F;
@@ -239,12 +233,7 @@ __global__ void __launch_bounds__(TR_THREADS) triangulate_kernel(TrParams p)
       }
 
       // 3. the winner
-      unsigned long long best = key;
-#pragma unroll
-      for (int o = 16; o; o >>= 1) {
-        const unsigned long long y = __shfl_xor_sync(full, best, o);
-        best = y > best ? y : best;
-      }
+      const unsigned long long best = vp_warp_max(key);
       const int src = (int)((0xffffffffu - (unsigned)best) & 31u);
 #pragma unroll
       for (int i = 0; i < 3; i++) X[i] = __shfl_sync(full, X[i], src);
@@ -259,10 +248,7 @@ __global__ void __launch_bounds__(TR_THREADS) triangulate_kernel(TrParams p)
           const TrCam &c = p.cams[e.a];
           if (tr_inlier(c.P, X, e.x, e.y, p.thr2)) tr_add_rows(c, e.x, e.y, s);
         }
-#pragma unroll
-        for (int o = 16; o; o >>= 1)
-#pragma unroll
-          for (int i = 0; i < 10; i++) s[i] += __shfl_xor_sync(full, s[i], o);
+        vp_warp_sum(s);
         const bool finite = tr_solve(s, Y);
         int cnt = 0;
         if (finite)
@@ -303,13 +289,7 @@ __global__ void __launch_bounds__(TR_THREADS) triangulate_kernel(TrParams p)
           const TrEntry e = tr_entry(s_e, p.spill, lo, r);
           float err = CUDART_NAN_F;
           unsigned char in = 0;
-          if (has) {
-            double u[3];
-            tr_project(p.cams[e.a].P, X, u);
-            const double e2z2 = tr_err2z2(u, e.x, e.y);
-            in = u[2] > 0.0 && e2z2 < p.thr2 * (u[2] * u[2]);
-            err = u[2] > 0.0 ? (float)sqrt(e2z2 / (u[2] * u[2])) : CUDART_INF_F;
-          }
+          if (has) tr_reproject(p.cams[e.a].P, X, e.x, e.y, p.thr2, err, in);
           if (p.errors) p.errors[e.pos] = err;
           if (p.inlier) p.inlier[e.pos] = in;
         }
@@ -322,22 +302,6 @@ __global__ void __launch_bounds__(TR_THREADS) triangulate_kernel(TrParams p)
 
   __syncthreads();
   if (threadIdx.x < 8 && s_st[threadIdx.x]) atomicAdd(&p.stats[threadIdx.x], s_st[threadIdx.x]);
-}
-
-// One resident wave: as many CTAs as the device holds at once (queried once per device).
-int triangulate_grid()
-{
-  static int gridOf[64];
-  int dev = 0;
-  CS_CUDA(cudaGetDevice(&dev));
-  dev &= 63;
-  if (gridOf[dev] == 0) {
-    int sms = 0, perSm = 0;
-    CS_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    CS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSm, triangulate_kernel, TR_THREADS, 0));
-    gridOf[dev] = (perSm > 0 ? perSm : 1) * sms;
-  }
-  return gridOf[dev];
 }
 
 }  // namespace
@@ -395,7 +359,7 @@ int triangulate_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, c
   prm.numMembers = numMembers;
   prm.numTrials = numTrials;
 
-  const int wave = triangulate_grid();
+  const int wave = resident_grid<triangulate_kernel, TR_THREADS>();
   if (wave < 0) return wave;
   const int grid = std::min(wave, idivup(numTracks, TR_WARPS));
   const cudaStream_t st = c.stream;

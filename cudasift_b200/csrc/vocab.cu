@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "vp_math.cuh"
 
 namespace cs {
 
@@ -35,13 +36,6 @@ __device__ __forceinline__ const float *vb_desc(const VbSet *__restrict__ sets, 
 }
 
 constexpr unsigned long long GOLDEN = 0x9E3779B97F4A7C15ull;
-unsigned long long splitmix64(unsigned long long z)
-{
-  z += GOLDEN;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
 
 int key_bits(unsigned long long maxKey)
 {
@@ -208,14 +202,14 @@ static_assert(offsetof(SiftPoint, data) == 64 && sizeof(SiftPoint) == 144 * 4, "
 
 }  // namespace
 
-// The start indices: the k-th distinct idx = ((splitmix64(seed + GOLDEN * counter) >> 32) * M) >> 32 over counter = 0,
+// The start indices: the k-th distinct idx = ((vp_splitmix64(seed + GOLDEN * counter) >> 32) * M) >> 32 over counter = 0,
 // 1, 2, ... (uint64 arithmetic).
 std::vector<int> vocab_start_draws(unsigned long long seed, int M, int numWords)
 {
   std::vector<int> draws;
   std::vector<unsigned char> seen((size_t)M, 0);
   for (unsigned long long ctr = 0; (int)draws.size() < numWords; ctr++) {
-    const unsigned long long x = splitmix64(seed + GOLDEN * ctr);
+    const unsigned long long x = vp_splitmix64(seed + GOLDEN * ctr);
     const int idx = (int)(((x >> 32) * (unsigned long long)M) >> 32);
     if (!seen[idx]) { seen[idx] = 1; draws.push_back(idx); }
   }

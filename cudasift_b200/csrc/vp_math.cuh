@@ -1,7 +1,9 @@
-// vp_math.cuh -- the FP64 helpers that geometric verification (verify.cu), triangulation (triangulate.cu) and
-// absolute pose (pose.cu) share: the counter-based generator and sampler, the cyclic Jacobi eigen-decomposition, the
-// calibrated coordinates of a pinhole K, the Rodrigues rotation and the reprojection inlier rule; and the hypothesis
-// prologue and slot arg-max of the two batched RANSAC calls (verify.cu, pose.cu).  tests/verify_oracle.py and
+// vp_math.cuh -- the FP64 helpers that geometric verification (verify.cu), triangulation (triangulate.cu), absolute
+// pose (pose.cu), bundle adjustment (bundle.cu) and the vocabulary's start draws (vocab.cu) share: the counter-based
+// generator and sampler, the cyclic Jacobi eigen-decomposition, the calibrated coordinates of a pinhole K, the fixed
+// xor butterflies (a sum over K doubles, a max over a u64 key), the Rodrigues rotation and the left rotation update,
+// the member rule of a track, and the reprojection inlier rule and per-observation output; and the hypothesis prologue
+// and slot arg-max of the two batched RANSAC calls (verify.cu, pose.cu).  tests/verify_oracle.py and
 // tests/triangulate_oracle.py restate the rules in float64.
 #pragma once
 
@@ -107,18 +109,36 @@ __device__ __forceinline__ bool vp_hyp_sample(int numLoops, double *slots, unsig
   return true;
 }
 
+// The K sums of a full warp's v, left in every lane: a fixed xor butterfly (a + b and b + a round alike, so every lane
+// holds the same bits, and the order depends on nothing but the lanes' values).
+template <int K>
+__device__ __forceinline__ void vp_warp_sum(double (&v)[K])
+{
+#pragma unroll
+  for (int o = 16; o; o >>= 1)
+#pragma unroll
+    for (int j = 0; j < K; j++) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
+}
+
+// The largest key of a full warp, in every lane (a xor butterfly).
+__device__ __forceinline__ unsigned long long vp_warp_max(unsigned long long key)
+{
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
+    key = t > key ? t : key;
+  }
+  return key;
+}
+
 // The packed arg-max of a warp's slots, all of one job: key = count << 32 | ~slot for a live slot (the most inliers,
 // then the lowest slot), 0 otherwise; a butterfly, then lane 0's atomicMax of the key into *best and its addition of the
 // warp's live slots to *numLive.  count is read for a live slot only.
 __device__ __forceinline__ void vp_argmax_warp(bool live, const unsigned int *count, int slot, unsigned long long *best,
                                                unsigned long long *numLive)
 {
-  unsigned long long key = live ? ((unsigned long long)*count << 32) | (unsigned int)~slot : 0ull;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
-    key = t > key ? t : key;
-  }
+  const unsigned long long key =
+      vp_warp_max(live ? ((unsigned long long)*count << 32) | (unsigned int)~slot : 0ull);
   const unsigned int nl = __popc(__ballot_sync(0xffffffffu, live));
   if ((threadIdx.x & 31) == 0) {
     if (key) atomicMax(best, key);
@@ -145,6 +165,30 @@ __device__ __forceinline__ void vp_rodrigues(const double *w, double (&Q)[9])
     }
 }
 
+// The left rotation update R1 = Q R with Q = exp([w]x) (vp_rodrigues), Q kept for the translation update, which
+// differs between absolute pose and bundle adjustment.
+__device__ __forceinline__ void vp_rotate(const double *w, const double *R, double *R1, double (&Q)[9])
+{
+  vp_rodrigues(w, Q);
+#pragma unroll
+  for (int i = 0; i < 3; i++)
+#pragma unroll
+    for (int j = 0; j < 3; j++) R1[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
+}
+
+// A valid member (a, f) of a track, the rule of triangulation and bundle adjustment: a known image, a feature inside
+// its set, a finite position (x, y).  Cam is the call's camera table entry, with the set's pts and n.
+template <class Cam>
+__device__ __forceinline__ bool tr_member(const Cam *cams, int numImages, int2 af, float &x, float &y)
+{
+  if ((unsigned)af.x >= (unsigned)numImages) return false;
+  const Cam &c = cams[af.x];
+  if ((unsigned)af.y >= (unsigned)c.n) return false;
+  x = c.pts[af.y].xpos;
+  y = c.pts[af.y].ypos;
+  return isfinite(x) && isfinite(y);
+}
+
 // The reprojection inlier rule of triangulation and absolute pose.  u = P (X, 1) with P = K [R | t] row-major 3 x 4:
 // the homogeneous pixel, u[2] the depth.  The explicit fma chain pins the arithmetic, so scoring, refits and the
 // per-feature outputs see the same bits.
@@ -167,6 +211,18 @@ __device__ __forceinline__ bool tr_inlier(const double *P, const double (&X)[3],
   double u[3];
   tr_project(P, X, u);
   return u[2] > 0.0 && tr_err2z2(u, x, y) < thr2 * (u[2] * u[2]);
+}
+
+// The per-observation output of triangulation, absolute pose and bundle adjustment: the inlier byte of tr_inlier's
+// rule and the pixel error (inf behind the camera).
+__device__ __forceinline__ void tr_reproject(const double *P, const double (&X)[3], float x, float y, double thr2,
+                                             float &err, unsigned char &in)
+{
+  double u[3];
+  tr_project(P, X, u);
+  const double e2z2 = tr_err2z2(u, x, y);
+  in = u[2] > 0.0 && e2z2 < thr2 * (u[2] * u[2]);
+  err = u[2] > 0.0 ? (float)sqrt(e2z2 / (u[2] * u[2])) : CUDART_INF_F;
 }
 
 }  // namespace cs
