@@ -129,7 +129,6 @@ int DeviceCtx::ensure(int d)
   if (!h_counters) CS_CUDA(cudaMallocHost((void **)&h_counters, 4 * sizeof(unsigned int)));
   if (!h_tcFlags) CS_CUDA(cudaMallocHost((void **)&h_tcFlags, 16 * sizeof(unsigned int)));
   if (!h_pairTotal) CS_CUDA(cudaMallocHost((void **)&h_pairTotal, sizeof(unsigned int)));
-  if (!h_guidedStats) CS_CUDA(cudaMallocHost((void **)&h_guidedStats, 4 * sizeof(unsigned long long)));
   CS_CUDA(cudaStreamCreate(&stream));
   return 0;
 }
@@ -393,31 +392,24 @@ static int ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1,
   return knn_sync(fn, c, d1, n1, d2, n2, l.idx1, l.sc1, l.idx2, l.sc2, &ra, mode, ms);
 }
 
-// cs_match_knn2_guided / cs_match_guided on device sets: the guided lists of set 1 (and with idx2 of set 2), with ra
-// then the ratio-test pairs, and the call returns their number; one synchronize.
-static int guided_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
-                       const GuidedModel &gm, int *idx1, float *sc1, int *idx2, float *sc2, const RatioArgs *ra,
-                       double *ms)
+// cs_match_knn2_guided / cs_match_guided on non-empty device sets: one job of guided_enqueue over the sets {d1, d2}.
+// With ra its ratio-test pairs (cross-checked with crossCheck), and the call returns their number; without ra set 1's
+// lists go to idx / score.  One synchronize; the job's statistics become cs_match_guided_stats.
+static int guided_sync(const char *fn, DeviceCtx *c, const void *d1, int n1, const void *d2, int n2, int model,
+                       const double *model_in, float thresh, const RatioArgs *ra, bool crossCheck, int *idx,
+                       float *score, double *ms)
 {
-  auto enqueue = [&]() -> int {
-    int r = launch_guided_knn(*c, d1, n1, d2, n2, gm, idx1, sc1, idx2, sc2);
-    if (ra && r >= 0) r = launch_ratio_pairs(*c, idx1, sc1, n1, idx2, sc2, n2, *ra);
-    return r;
-  };
-  const int r = timed_sync(fn, c, ms, enqueue);
+  const cs_match_set sets[2] = {{d1, n1}, {d2, n2}};
+  const cs_match_job job = {0, 1, ra ? reinterpret_cast<int *>(ra->pairs) : nullptr, ra ? ra->maxPairs : 0};
+  const GuidedSingle single = {idx, score};
+  GuidedBatchOut out = {nullptr, nullptr};
+  const int r = timed_sync(fn, c, ms, [&]() {
+    return guided_enqueue(*c, sets, &job, 1, &model, model_in, thresh, ra ? ra->maxRatio : 0.0f,
+                          ra ? ra->maxDistance : 0.0f, crossCheck, &out, &single);
+  });
   if (r < 0) return r;
-  for (int k = 0; k < 4; k++) c->guidedStats[k] = c->h_guidedStats[k];
-  return ra ? (int)*c->h_pairTotal : 0;
-}
-
-// cs_match_guided on device sets: the lists in the context's knnLists, as for cs_match_ratio.
-static int guided_ratio_sync(const char *fn, DeviceCtx *c, const SiftPoint *d1, int n1, const SiftPoint *d2, int n2,
-                             const GuidedModel &gm, const RatioArgs &ra, bool crossCheck, double *ms)
-{
-  KnnLists l;
-  const int r = knn_lists(c, n1, n2, crossCheck, &l);
-  if (r < 0) return r;
-  return guided_sync(fn, c, d1, n1, d2, n2, gm, l.idx1, l.sc1, l.idx2, l.sc2, &ra, ms);
+  for (int k = 0; k < 4; k++) c->guidedStats[k] = out.stats[k];
+  return ra ? (int)*out.total : 0;
 }
 
 static cs_verify_job verify_job(const SiftPoint *d1, int n1, const SiftPoint *d2, int n2, const int *pairs, int numPairs,
@@ -1005,8 +997,7 @@ int cs_match_knn2_guided(const void *d_s1, int n1, const void *d_s2, int n2, int
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  return guided_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2,
-                     guided_model(model, model_in, thresh), d_idx, d_score, nullptr, nullptr, nullptr, ms);
+  return guided_sync(fn, c, d_s1, n1, d_s2, n2, model, model_in, thresh, nullptr, false, d_idx, d_score, ms);
 }
 
 int cs_match_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],
@@ -1023,8 +1014,7 @@ int cs_match_guided(const void *d_s1, int n1, const void *d_s2, int n2, int mode
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   const RatioArgs ra = {maxRatio, maxDistance, (int2 *)d_pairs, maxPairs};
-  return guided_ratio_sync(fn, c, (const SiftPoint *)d_s1, n1, (const SiftPoint *)d_s2, n2,
-                           guided_model(model, model_in, thresh), ra, crossCheck != 0, ms);
+  return guided_sync(fn, c, d_s1, n1, d_s2, n2, model, model_in, thresh, &ra, crossCheck != 0, nullptr, nullptr, ms);
 }
 
 int cs_match_guided_host(const void *h_s1, int n1, const void *h_s2, int n2, int model, const double model_in[9],
@@ -1040,12 +1030,12 @@ int cs_match_guided_host(const void *h_s1, int n1, const void *h_s2, int n2, int
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
-  const GuidedModel gm = guided_model(model, model_in, thresh);
   const int room = maxPairs < n1 ? maxPairs : n1;                      // at most one pair per row of set 1
   return host_pairs(c, h_s1, n1, h_s2, n2, room > 0 ? room : 1, 0, room, h_pairs,
                     [&](SiftPoint *d1, SiftPoint *d2, int2 *pairs) {
                       const RatioArgs ra = {maxRatio, maxDistance, pairs, room};
-                      return guided_ratio_sync(fn, c, d1, n1, d2, n2, gm, ra, crossCheck != 0, ms);
+                      return guided_sync(fn, c, d1, n1, d2, n2, model, model_in, thresh, &ra, crossCheck != 0,
+                                         nullptr, nullptr, ms);
                     });
 }
 
@@ -1296,8 +1286,8 @@ int cs_match_guided_batch(const cs_match_set *sets, int numSets, const cs_match_
   return batch_body(fn, numJobs, counts_out, stats_out, 4, ms, [](int) {},
                     [&](int p) { return sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0; },
                     [&](DeviceCtx *c) {
-                      return guided_batch_enqueue(*c, sets, jobs, numJobs, models, models_in, thresh, maxRatio,
-                                                  maxDistance, crossCheck != 0, out.data());
+                      return guided_enqueue(*c, sets, jobs, numJobs, models, models_in, thresh, maxRatio, maxDistance,
+                                            crossCheck != 0, out.data(), nullptr);
                     },
                     [&](DeviceCtx *, int p, int, unsigned long long *st) {
                       for (int k = 0; k < 4; k++) st[k] = out[p].stats[k];

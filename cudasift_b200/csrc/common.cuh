@@ -261,13 +261,16 @@ struct Layout {
   }
 };
 
+// The scratch budget of one wave of a batched call: RANSAC model slots (verify.cu, pose.cu), ratio and guided matching
+// (match_tc.cu, match_guided.cu) and retrieval query accumulators (vocab.cu).  The header states each call's rule.
+constexpr size_t WAVE_BYTES = (size_t)256 << 20;
+
 // ---- the waves of a batched RANSAC call (verify.cu, pose.cu) --------------------------------------------------------
-// A wave holds floor(256 MiB / slotBytes) jobs, slotBytes being one job's model slots and their counts, clamped to
+// A wave holds floor(WAVE_BYTES / slotBytes) jobs, slotBytes being one job's model slots and their counts, clamped to
 // [1, 65536].
-constexpr size_t RANSAC_WAVE_BYTES = (size_t)256 << 20;
 inline int ransac_jobs_per_wave(size_t slotBytes)
 {
-  const size_t k = RANSAC_WAVE_BYTES / slotBytes;
+  const size_t k = WAVE_BYTES / slotBytes;
   return k < 1 ? 1 : k > 65536 ? 65536 : (int)k;
 }
 
@@ -340,10 +343,10 @@ struct DeviceCtx {
   GrowBuffer knnPartials;     // cs_match_knn2, cs_match_ratio(_host): the slices of the exact scan
   GrowBuffer verify;          // cs_verify_pairs(_host, _batch), cs_verify_models, cs_verify_essential(_host, _models, _batch)
   GrowBuffer rank;            // cs_rank_records: counters, scratch
-  // cs_match_knn2_guided, cs_match_guided(_host, _batch): coefficient records, cell grids and the sorted candidate
-  // copies; a batch wave's tables, headers, knn lists and pair scratch as well
+  // cs_match_knn2_guided, cs_match_guided(_host, _batch): a wave's tables and headers, and per job its coefficient
+  // records, cell grids, sorted candidate copies, knn lists and pair scratch
   GrowBuffer guided;
-  PinnedBuffer h_guidedBatch;              // every cs_match_guided_batch wave's tables and copied-back state
+  PinnedBuffer h_guidedBatch;              // every guided wave's tables (uploaded) and state (copied back)
   // the tensor path (match_tc.cu) of cs_match(_host), cs_match_mutual(_host), cs_match_knn2, cs_match_ratio(_host):
   // operand tiles, B-role copies, row norms, top-3 tables, fallback rows, and 2 x 16 words of flags used alternately
   GrowBuffer tcA, tcB, tcNorms, tcTables, tcRows, tcFlags;
@@ -386,7 +389,6 @@ struct DeviceCtx {
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
   unsigned int *h_tcFlags = nullptr;       // 16: the tensor path's flag area of the last call
   unsigned int *h_pairTotal = nullptr;     // the pair total of the last mutual or ratio call
-  unsigned long long *h_guidedStats = nullptr;   // 4: the counters of the last guided call
 
   unsigned long long matchStats[4] = {0, 0, 0, 0};
   unsigned long long guidedStats[4] = {0, 0, 0, 0};
@@ -533,32 +535,22 @@ __device__ __forceinline__ void top2_insert(Top2 &t, float s, int j)
 }
 
 // ---- guided matching (match_guided.cu) ------------------------------------------------------------------------------
-// The model as the predicate uses it: entries of the unit-Frobenius model rounded to float, t2 = fl(thresh * thresh).
-struct GuidedModel {
-  int model;          // CS_GEOM_HOMOGRAPHY or CS_GEOM_FUNDAMENTAL
-  float f[9];
-  float t2;
-};
-GuidedModel guided_model(int model, const double in[9], float thresh);
-// The two nearest admissible neighbours of set 1's rows in set 2 (idx1 / score1, [n1][2]); with idx2 also those of
-// set 2's rows in set 1.  Uses c.guided; the statistics reach c.h_guidedStats by the caller's synchronize.
-int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const GuidedModel &gm,
-                      int *idx1, float *score1, int *idx2, float *score2);
-// Batched guided matching (cs_match_guided_batch, whose header comment states the wave rule).  A job's wave scratch:
-// its index, knn lists and pair scratch (every piece rounded up to 256 bytes) and GD_JOB_STATE_BYTES for its header and
-// pair total.
-#define GD_WAVE_BYTES ((size_t)256 << 20)
-#define GD_JOB_STATE_BYTES 256
-size_t guided_job_bytes(int n1, int n2, bool cross);
 // Where job p's results land in pinned memory after the call's synchronize (null for an empty job).
 struct GuidedBatchOut {
   const unsigned int *total;
   const unsigned long long *stats;
 };
-// Every non-empty job of a batch (argument-checked) in waves on c.stream, without a synchronize.
-int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs,
-                         const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
-                         bool cross, GuidedBatchOut *out);
+// What a single call (one job) adds: its stage timing is reported as "guided timing n1xn2", and with idx
+// (cs_match_knn2_guided, one direction) set 1's lists go to idx / score ([n1][2]) and no pair launches are issued.
+struct GuidedSingle {
+  int *idx;
+  float *score;
+};
+// Every non-empty job (argument-checked) in waves on c.stream (cs_match_guided_batch, whose header comment states the
+// wave rule), without a synchronize; single is null for a batch.
+int guided_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs, const int *models,
+                   const double *models_in, float thresh, float maxRatio, float maxDistance, bool cross,
+                   GuidedBatchOut *out, const GuidedSingle *single);
 
 // ---- feature tracks (tracks.cu) ---------------------------------------------------------------------------------
 // The kernels of cs_build_tracks (argument-checked, at least one pair in all) on c.stream, without a synchronize; the
@@ -590,7 +582,6 @@ int vocab_train(DeviceCtx &c, const cs_match_set *sets, int numSets, int numWord
                 unsigned long long seed, SiftPoint *vocab, double *trace, long long stats[4]);
 // cs_retrieve_pairs (argument-checked, some feature) on c.stream, without a synchronize; the seven statistics reach
 // c.h_retrieve (unsigned long long) by the caller's synchronize, the wave count c.retrieveWaves.
-constexpr size_t RT_WAVE_BYTES = (size_t)256 << 20;
 int retrieve_queries_per_wave(int numImages);
 int retrieve_enqueue(DeviceCtx &c, const int *imageSizes, int numImages, const int *wordOf, int numWords, int topK,
                      int *neighbours, double *scores, double *idf, int *pairs, int maxPairs);

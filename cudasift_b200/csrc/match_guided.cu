@@ -20,11 +20,9 @@
 // A row for which the bounds do not hold (coordinates beyond 1e12, |pw| < 1e-12, an extreme threshold) scans every
 // candidate: that is correct, only slower.
 //
-// Batches (cs_match_guided_batch): every kernel takes one entry by value (a single call) or, instantiated with TABLE,
-// a device table of entries in which a CTA finds its own by its index (table_find over CTA bases the host summed).
-// Each job has its own slice of everything, so a row's result depends only on its job: see DESIGN.md section 4.
-// TABLE is a template argument, not a null test, so that the single call's kernels keep reading their entry from the
-// parameter bank instead of holding it in registers.
+// Every call runs as waves of jobs (guided_enqueue; a single call is one job): every kernel takes a device table of
+// entries in which a CTA finds its own by its index (table_find over CTA bases the host summed).  Each job has its own
+// slice of everything, so a row's result depends only on its job: see DESIGN.md section 4.
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
@@ -40,6 +38,13 @@ namespace cs {
 #define GD_SAFE_POS 1e12f     // the bounds hold for |xpos|, |ypos| up to this
 #define GD_SAFE_PW 1e-12f     // ... and, for H, |pw| of set-1 points at least this
 #define GD_WARPS 8            // rows per CTA of the knn kernel (one warp each)
+
+// The model as the predicate uses it: entries of the unit-Frobenius model rounded to float, t2 = fl(thresh * thresh).
+struct GuidedModel {
+  int model;          // CS_GEOM_HOMOGRAPHY or CS_GEOM_FUNDAMENTAL
+  float f[9];
+  float t2;
+};
 
 // One point of either set: its predicate coefficients (NaN when its position is not finite), its position, and its
 // index position as a candidate (NaN: not indexed, because it can never be admissible or its direction is not built).
@@ -63,10 +68,10 @@ struct GGrid {
   int gx, gy;
 };
 
-// One call or batch job as prep, hist, scan and scatter see it: its sets, model and header, its points, cell/slot
-// array, cell counts (cap0 / cap1 cells at most per direction), exclusive starts and sorted candidate copies per
-// direction (0: set 2's candidates, 1: set 1's, built when dirs == 2).  In a batch table job q owns the point CTAs
-// (ceil((n1 + n2) / 256)) from cta0 on and the scan CTAs (2 * dirs) from scan0 on.
+// One job as prep, hist, scan and scatter see it: its sets, model and header, its points, cell/slot array, cell counts
+// (cap0 / cap1 cells at most per direction), exclusive starts and sorted candidate copies per direction (0: set 2's
+// candidates, 1: set 1's, built when dirs == 2).  Job q owns the point CTAs (ceil((n1 + n2) / 256)) from cta0 on and
+// the scan CTAs (2 * dirs) from scan0 on.
 struct GJob {
   const SiftPoint *s1, *s2;
   int n1, n2, dirs, cap0, cap1;
@@ -81,8 +86,7 @@ struct GJob {
   int cta0, scan0;
 };
 
-// One direction of a call or batch job, as the knn kernel sees it.  In a batch table the entry owns the CTAs
-// (ceil(nRows / GD_WARPS)) from cta0 on.
+// One direction of a job, as the knn kernel sees it.  The entry owns the CTAs (ceil(nRows / GD_WARPS)) from cta0 on.
 struct GDir {
   const SiftPoint *rowSift, *candSift;
   const GPoint *rowPts;
@@ -98,12 +102,11 @@ struct GDir {
   int cta0;
 };
 
-// The entry of this CTA and the CTA's index within it (blk): `one` in a single call, else the table's entry whose CTA
-// range (from its `start` field on) holds blockIdx.x.
-template <bool TABLE, class T>
-__device__ __forceinline__ T gd_entry(const T &one, const T *__restrict__ tab, int n, int T::*start, int &blk)
+// The entry of this CTA and the CTA's index within it (blk): the table's entry whose CTA range (from its `start` field
+// on) holds blockIdx.x.
+template <class T>
+__device__ __forceinline__ T gd_entry(const T *__restrict__ tab, int n, int T::*start, int &blk)
 {
-  if (!TABLE) { blk = blockIdx.x; return one; }
   const T e = tab[table_find(tab, n, start, (int)blockIdx.x)];
   blk = (int)blockIdx.x - e.*start;
   return e;
@@ -171,16 +174,11 @@ __device__ __forceinline__ int cell_of(float p, float p0, float inv, int g)
 }
 
 // ---- 1. prep ------------------------------------------------------------------------------------------------------
-// The CTAs of a point-parallel kernel in a call (the grid) or a batch job (one per 256 points).
-template <bool TABLE>
-__device__ __forceinline__ int gd_point_ctas(int n) { return TABLE ? (n + 255) >> 8 : (int)gridDim.x; }
-
-template <bool TABLE>
 __global__ void __launch_bounds__(256)
-guided_prep_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
+guided_prep_kernel(const GJob *__restrict__ jobs, int numJobs)
 {
   int blk;
-  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::cta0, blk);
+  const GJob jb = gd_entry(jobs, numJobs, &GJob::cta0, blk);
   const SiftPoint *__restrict__ s1 = jb.s1, *__restrict__ s2 = jb.s2;
   const int n1 = jb.n1, dirs = jb.dirs;
   const GuidedModel &gm = jb.gm;
@@ -189,7 +187,7 @@ guided_prep_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
   const float *f = gm.f;
   const float nan = __int_as_float(0x7fffffff);
   const int n = n1 + jb.n2, lane = threadIdx.x & 31;
-  for (int base = blk * blockDim.x; base < n; base += gd_point_ctas<TABLE>(n) * blockDim.x) {
+  for (int base = blk * blockDim.x; base < n; base += ((n + 255) >> 8) * blockDim.x) {
     const int t = base + threadIdx.x;
     bool indexed = false, safe = true;
     float maxA = 0.0f, maxB = 0.0f;
@@ -259,13 +257,12 @@ guided_prep_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
 
 // ---- 2. index -----------------------------------------------------------------------------------------------------
 // Per indexed point: its cell (cx * gy + cy) and its slot inside the cell.
-template <bool TABLE>
 __global__ void __launch_bounds__(256)
-guided_hist_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
+guided_hist_kernel(const GJob *__restrict__ jobs, int numJobs)
 {
   __shared__ GGrid sg[2];
   int blk;
-  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::cta0, blk);
+  const GJob jb = gd_entry(jobs, numJobs, &GJob::cta0, blk);
   const GPoint *__restrict__ pts = jb.pts;
   const GHdr *__restrict__ h = jb.h;
   unsigned int *counts0 = jb.counts0, *counts1 = jb.counts1;
@@ -273,7 +270,7 @@ guided_hist_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
   const int n1 = jb.n1, n = n1 + jb.n2;
   if (threadIdx.x < 2) sg[threadIdx.x] = grid_of(*h, threadIdx.x, threadIdx.x ? jb.cap1 : jb.cap0);
   __syncthreads();
-  for (int t = blk * blockDim.x + threadIdx.x; t < n; t += gd_point_ctas<TABLE>(n) * blockDim.x) {
+  for (int t = blk * blockDim.x + threadIdx.x; t < n; t += ((n + 255) >> 8) * blockDim.x) {
     const float2 k = pts[t].key;
     if (isnan(k.x)) { cellSlot[t] = make_int2(-1, 0); continue; }
     const int d = t < n1 ? 1 : 0;
@@ -285,13 +282,12 @@ guided_hist_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
 
 // Exclusive scans of the cell counts: CTA 2 * dir + order, order 0 column-major (cell cx * gy + cy), order 1
 // row-major (cy * gx + cx).  start[cells] = the count.
-template <bool TABLE>
 __global__ void __launch_bounds__(1024)
-guided_scan_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
+guided_scan_kernel(const GJob *__restrict__ jobs, int numJobs)
 {
   __shared__ unsigned int s_w[32];
   int blk;
-  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::scan0, blk);
+  const GJob jb = gd_entry(jobs, numJobs, &GJob::scan0, blk);
   const int dir = blk >> 1, order = blk & 1;
   const GGrid g = grid_of(*jb.h, dir, dir ? jb.cap1 : jb.cap0);
   const unsigned int *cnt = dir ? jb.counts1 : jb.counts0;
@@ -332,13 +328,12 @@ guided_scan_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
   if (threadIdx.x == 0) out[cells] = carry;
 }
 
-template <bool TABLE>
 __global__ void __launch_bounds__(256)
-guided_scatter_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs)
+guided_scatter_kernel(const GJob *__restrict__ jobs, int numJobs)
 {
   __shared__ int sgx[2], sgy[2];
   int blk;
-  const GJob jb = gd_entry<TABLE>(one, jobs, numJobs, &GJob::cta0, blk);
+  const GJob jb = gd_entry(jobs, numJobs, &GJob::cta0, blk);
   const GPoint *__restrict__ pts = jb.pts;
   const int2 *__restrict__ cellSlot = jb.cellSlot;
   const int n1 = jb.n1, n = n1 + jb.n2;
@@ -347,7 +342,7 @@ guided_scatter_kernel(const GJob one, const GJob *__restrict__ jobs, int numJobs
     sgx[threadIdx.x] = g.gx; sgy[threadIdx.x] = g.gy;
   }
   __syncthreads();
-  for (int t = blk * blockDim.x + threadIdx.x; t < n; t += gd_point_ctas<TABLE>(n) * blockDim.x) {
+  for (int t = blk * blockDim.x + threadIdx.x; t < n; t += ((n + 255) >> 8) * blockDim.x) {
     const int2 cl = cellSlot[t];
     if (cl.x < 0) continue;
     const int d = t < n1 ? 1 : 0, gx = sgx[d], gy = sgy[d];
@@ -455,11 +450,13 @@ __device__ __forceinline__ bool strip_cells(int k, int n, float a0, float a1, fl
   return true;
 }
 
-// The rows of direction d that CTA blk of ctas runs (a call grid-strides, a batch gives every direction one CTA per
-// GD_WARPS rows).  d is the kernel's parameter or the table's entry in global memory, read in place: a copy would
-// index gm.f from local memory.
-__device__ __forceinline__ void guided_knn_rows(const GDir &d, int blk, int ctas)
+// Every direction of the table has one CTA per GD_WARPS rows.  d is the table's entry in global memory, read in place:
+// a copy would index gm.f from local memory.
+__global__ void __launch_bounds__(GD_WARPS * 32)
+guided_knn_kernel(const GDir *__restrict__ dirs, int numDirs)
 {
+  const GDir &d = dirs[table_find(dirs, numDirs, &GDir::cta0, (int)blockIdx.x)];
+  const int blk = (int)blockIdx.x - d.cta0, ctas = (d.nRows + GD_WARPS - 1) / GD_WARPS;
   __shared__ float4 s_row[GD_WARPS][32];
   __shared__ int s_q[GD_WARPS][64];
   const GuidedModel &gm = d.gm;
@@ -573,20 +570,8 @@ __device__ __forceinline__ void guided_knn_rows(const GDir &d, int blk, int ctas
   }
 }
 
-template <bool TABLE>
-__global__ void __launch_bounds__(GD_WARPS * 32)
-guided_knn_kernel(const GDir one, const GDir *__restrict__ dirs, int numDirs)
-{
-  if (!TABLE) {
-    guided_knn_rows(one, blockIdx.x, gridDim.x);
-    return;
-  }
-  const GDir &d = dirs[table_find(dirs, numDirs, &GDir::cta0, (int)blockIdx.x)];
-  guided_knn_rows(d, (int)blockIdx.x - d.cta0, (d.nRows + GD_WARPS - 1) / GD_WARPS);
-}
-
 // ---- host -----------------------------------------------------------------------------------------------------------
-GuidedModel guided_model(int model, const double in[9], float thresh)
+static GuidedModel guided_model(int model, const double in[9], float thresh)
 {
   GuidedModel gm;
   gm.model = model;
@@ -598,16 +583,15 @@ GuidedModel guided_model(int model, const double in[9], float thresh)
   return gm;
 }
 
-// The scratch of one call or batch job (its header aside), every piece 256-byte aligned: the cell counts, zeroed before
-// the call (offsets from the zeroed base), then the rest (offsets from the other base).  own: a batch job, which also
-// holds its knn lists and pair scratch; a single call uses the context's knnLists and pairScratch.
+// The scratch of one job (its header aside), every piece 256-byte aligned: the cell counts, zeroed before the wave
+// (offsets from the zeroed base), then the rest, its knn lists and pair scratch included (offsets from the other base).
 struct GLayout {
   int cap0, cap1;
   size_t cnt0, cnt1, zeroBytes;
   size_t pts, cell, s0C, s0R, s1C, s1R, c0C, i0C, c0R, i0R, c1C, i1C, c1R, i1R;
   size_t idx1, sc1, idx2, sc2, masks, ctaCounts, bytes;
 };
-static GLayout gd_layout(int n1, int n2, int dirs, bool own)
+static GLayout gd_layout(int n1, int n2, int dirs)
 {
   GLayout L;
   const size_t n = (size_t)n1 + n2, m1 = dirs == 2 ? n1 : 1;
@@ -622,16 +606,16 @@ static GLayout gd_layout(int n1, int n2, int dirs, bool own)
   L.c0C = b.take(16 * (size_t)n2); L.i0C = b.take(4 * (size_t)n2);
   L.c0R = b.take(16 * (size_t)n2); L.i0R = b.take(4 * (size_t)n2);
   L.c1C = b.take(16 * m1); L.i1C = b.take(4 * m1); L.c1R = b.take(16 * m1); L.i1R = b.take(4 * m1);
-  const size_t l2 = own && dirs == 2 ? (size_t)n2 : 0;
-  L.idx1 = b.take(own ? 8 * (size_t)n1 : 0); L.sc1 = b.take(own ? 8 * (size_t)n1 : 0);
+  const size_t l2 = dirs == 2 ? (size_t)n2 : 0;
+  L.idx1 = b.take(8 * (size_t)n1); L.sc1 = b.take(8 * (size_t)n1);
   L.idx2 = b.take(8 * l2); L.sc2 = b.take(8 * l2);
   // the flags / write kernels' ballot words and counts of 1024-row CTAs (match_mutual.cu)
-  L.masks = b.take(own ? 4 * (size_t)idivup(n1, 32) : 0); L.ctaCounts = b.take(own ? 4 * (size_t)idivup(n1, 1024) : 0);
+  L.masks = b.take(4 * (size_t)idivup(n1, 32)); L.ctaCounts = b.take(4 * (size_t)idivup(n1, 1024));
   L.bytes = b.bytes;
   return L;
 }
 
-// The entry of a call or job: header h, cell counts from z, the rest from b.
+// The entry of a job: header h, cell counts from z, the rest from b.
 static GJob gd_job(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int dirs, const GuidedModel &gm, GHdr *h,
                    char *z, char *b, const GLayout &L)
 {
@@ -649,7 +633,7 @@ static GJob gd_job(const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, int
   return j;
 }
 
-// Direction dir of a call or job (0: set 1's rows against set 2, 1: the reverse), its lists at idx / score.
+// Direction dir of a job (0: set 1's rows against set 2, 1: the reverse), its lists at idx / score.
 static GDir gd_dir(const GJob &j, int dir, int2 *idx, float2 *score, int cta0)
 {
   GDir d;
@@ -670,53 +654,8 @@ static GDir gd_dir(const GJob &j, int dir, int2 *idx, float2 *score, int cta0)
   return d;
 }
 
-int launch_guided_knn(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoint *s2, int n2, const GuidedModel &gm,
-                      int *idx1, float *score1, int *idx2, float *score2)
-{
-  const int dirs = idx2 ? 2 : 1, n = n1 + n2;
-  // layout: header and cell counts first (one memset), then the rest
-  const GLayout L = gd_layout(n1, n2, dirs, false);
-  Layout dev(256);
-  const size_t hdrAt = dev.take(sizeof(GHdr)), zeroAt = dev.take(L.zeroBytes), restAt = dev.take(L.bytes);
-  int r;
-  if ((r = c.guided.grow(dev.bytes)) < 0) return r;
-  char *b = c.guided.as<char>();
-  GHdr *h = reinterpret_cast<GHdr *>(b + hdrAt);
-  const GJob j = gd_job(s1, n1, s2, n2, dirs, gm, h, b + zeroAt, b + restAt, L);
-  cudaStream_t st = c.stream;
-  cudaEvent_t *tev = match_timing_events();
-  if (tev) cudaEventRecord(tev[0], st);
-  CS_CUDA(cudaMemsetAsync(b, 0, restAt, st));
-  const int blocks = idivup(n, 256) < 4 * c.sms ? idivup(n, 256) : 4 * c.sms;
-  guided_prep_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
-  if (tev) cudaEventRecord(tev[1], st);
-  guided_hist_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
-  guided_scan_kernel<false><<<2 * dirs, 1024, 0, st>>>(j, nullptr, 0);
-  guided_scatter_kernel<false><<<blocks, 256, 0, st>>>(j, nullptr, 0);
-  count_launch(4);
-  CS_CUDA(cudaGetLastError());
-  if (tev) cudaEventRecord(tev[2], st);
-  for (int dir = 0; dir < dirs; dir++) {
-    const GDir d = gd_dir(j, dir, reinterpret_cast<int2 *>(dir ? idx2 : idx1),
-                          reinterpret_cast<float2 *>(dir ? score2 : score1), 0);
-    const int rowBlocks = idivup(d.nRows, GD_WARPS) < 16 * c.sms ? idivup(d.nRows, GD_WARPS) : 16 * c.sms;
-    guided_knn_kernel<false><<<rowBlocks, GD_WARPS * 32, 0, st>>>(d, nullptr, 0);
-    count_launch();
-    CS_CUDA(cudaGetLastError());
-    if (tev) cudaEventRecord(tev[3 + dir], st);
-  }
-  CS_CUDA(cudaMemcpyAsync(c.h_guidedStats, h->stats, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  static const char *const stages[] = {"prep", "index", "knn", "reverse-knn"};
-  if (tev) report_stage_times(tev, stages, 2 + dirs, "guided timing %dx%d", n1, n2);
-  return 0;
-}
-
-// ---- batches --------------------------------------------------------------------------------------------------------
-size_t guided_job_bytes(int n1, int n2, bool cross)
-{
-  const GLayout L = gd_layout(n1, n2, cross ? 2 : 1, true);
-  return L.zeroBytes + L.bytes + GD_JOB_STATE_BYTES;
-}
+// A job's wave scratch: its layout and GD_JOB_STATE_BYTES for its header and pair total (the header states the rule).
+#define GD_JOB_STATE_BYTES 256
 
 // A wave (the header states the rule): the non-empty jobs ne[q0, q1) and what its launches need.
 struct GdWave {
@@ -731,11 +670,12 @@ struct GdWave {
   size_t stateDev = 0, zeroDev = 0, restDev = 0;
 };
 
-int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs,
-                         const int *models, const double *models_in, float thresh, float maxRatio, float maxDistance,
-                         bool cross, GuidedBatchOut *out)
+int guided_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *jobs, int numJobs, const int *models,
+                   const double *models_in, float thresh, float maxRatio, float maxDistance, bool cross,
+                   GuidedBatchOut *out, const GuidedSingle *single)
 {
   const int D = cross ? 2 : 1;
+  const bool knnOnly = single && single->idx;
   std::vector<int> ne;
   for (int p = 0; p < numJobs; p++)
     if (sets[jobs[p].set1].n > 0 && sets[jobs[p].set2].n > 0) ne.push_back(p);
@@ -745,13 +685,13 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
   for (int q = 0; q < (int)ne.size(); q++) {
     const cs_match_job &jb = jobs[ne[q]];
     const int n1 = sets[jb.set1].n, n2 = sets[jb.set2].n;
-    const size_t cost = guided_job_bytes(n1, n2, cross);
-    if (waves.empty() || waves.back().bytes + cost > GD_WAVE_BYTES) {
+    const GLayout L = gd_layout(n1, n2, D);
+    const size_t cost = L.zeroBytes + L.bytes + GD_JOB_STATE_BYTES;
+    if (waves.empty() || waves.back().bytes + cost > WAVE_BYTES) {
       waves.emplace_back();
       waves.back().q0 = q;
     }
     GdWave &v = waves.back();
-    const GLayout L = gd_layout(n1, n2, D, true);
     v.q1 = q + 1;
     v.bytes += cost;
     v.zeroBytes += L.zeroBytes;
@@ -800,14 +740,16 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
       const int p = ne[v.q0 + k];
       const cs_match_job &jb = jobs[p];
       const int n1 = sets[jb.set1].n, n2 = sets[jb.set2].n;
-      const GLayout L = gd_layout(n1, n2, D, true);
+      const GLayout L = gd_layout(n1, n2, D);
       GJob &j = hj[k];
       j = gd_job(static_cast<const SiftPoint *>(sets[jb.set1].pts), n1, static_cast<const SiftPoint *>(sets[jb.set2].pts),
                  n2, D, guided_model(models[p], models_in + 9 * (size_t)p, thresh), hdrs + k, z, b, L);
       j.cta0 = pointCta; j.scan0 = 2 * D * k;
       pointCta += idivup(n1 + n2, 256);
-      int2 *idx1 = reinterpret_cast<int2 *>(b + L.idx1), *idx2 = cross ? reinterpret_cast<int2 *>(b + L.idx2) : nullptr;
-      float2 *sc1 = reinterpret_cast<float2 *>(b + L.sc1), *sc2 = cross ? reinterpret_cast<float2 *>(b + L.sc2) : nullptr;
+      int2 *idx1 = knnOnly ? reinterpret_cast<int2 *>(single->idx) : reinterpret_cast<int2 *>(b + L.idx1);
+      float2 *sc1 = knnOnly ? reinterpret_cast<float2 *>(single->score) : reinterpret_cast<float2 *>(b + L.sc1);
+      int2 *idx2 = cross ? reinterpret_cast<int2 *>(b + L.idx2) : nullptr;
+      float2 *sc2 = cross ? reinterpret_cast<float2 *>(b + L.sc2) : nullptr;
       for (int dir = 0; dir < D; dir++) {
         hd[D * k + dir] = gd_dir(j, dir, dir ? idx2 : idx1, dir ? sc2 : sc1, knnCta);
         knnCta += idivup(dir ? n2 : n1, GD_WARPS);
@@ -834,21 +776,25 @@ int guided_batch_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_
     CS_CUDA(cudaMemsetAsync(ds, 0, v.restDev - v.stateDev, st));
     CS_CUDA(cudaMemcpyAsync(dt, hp, v.tabBytes, cudaMemcpyHostToDevice, st));
     if (tev) cudaEventRecord(tev[0], st);
-    guided_prep_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
+    guided_prep_kernel<<<v.pointCtas, 256, 0, st>>>(dj, J);
     if (tev) cudaEventRecord(tev[1], st);
-    guided_hist_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
-    guided_scan_kernel<true><<<2 * D * J, 1024, 0, st>>>(GJob{}, dj, J);
-    guided_scatter_kernel<true><<<v.pointCtas, 256, 0, st>>>(GJob{}, dj, J);
+    guided_hist_kernel<<<v.pointCtas, 256, 0, st>>>(dj, J);
+    guided_scan_kernel<<<2 * D * J, 1024, 0, st>>>(dj, J);
+    guided_scatter_kernel<<<v.pointCtas, 256, 0, st>>>(dj, J);
     if (tev) cudaEventRecord(tev[2], st);
-    guided_knn_kernel<true><<<v.knnCtas, GD_WARPS * 32, 0, st>>>(GDir{}, dd, v.dirs);
+    guided_knn_kernel<<<v.knnCtas, GD_WARPS * 32, 0, st>>>(dd, v.dirs);
     if (tev) cudaEventRecord(tev[3], st);
     count_launch(5);
     CS_CUDA(cudaGetLastError());
-    if ((r = launch_ratio_pairs_batch(c, dpj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
-    if (tev) cudaEventRecord(tev[4], st);
+    if (!knnOnly) {
+      if ((r = launch_ratio_pairs_batch(c, dpj, J, v.pairCtas, maxRatio, maxDistance)) < 0) return r;
+      if (tev) cudaEventRecord(tev[4], st);
+    }
     CS_CUDA(cudaMemcpyAsync(hp + v.tabBytes, ds, v.stateBytes, cudaMemcpyDeviceToHost, st));
     static const char *const stages[] = {"prep", "index", "knn", "pairs"};
-    if (tev)
+    if (tev && single)
+      report_stage_times(tev, stages, knnOnly ? 3 : 4, "guided timing %dx%d", hj[0].n1, hj[0].n2);
+    else if (tev)
       report_stage_times(tev, stages, 4, "guided-batch timing %d jobs %d directions %d rows", J, v.dirs, 8 * v.knnCtas);
   }
   return 0;

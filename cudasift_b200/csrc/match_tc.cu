@@ -901,10 +901,9 @@ void match_tensor_stats(DeviceCtx &c, unsigned long long stats[4])
 
 // ------------------------------------------------------------------------------ batched knn directions
 // A wave (cs_match_ratio_batch states the rule): consecutive non-empty jobs whose scratch -- per distinct set its
-// operand tiles and norms, per direction its top-3 tables, neighbour lists and fallback entries -- fits MB_BUDGET.
+// operand tiles and norms, per direction its top-3 tables, neighbour lists and fallback entries -- fits WAVE_BYTES.
 // Every wave runs the same four launches (prep, GEMM, knn resolve, list fallback), then the caller's last step:
 // ratio flags and pair writes for cs_match_ratio_batch, the word copy for cs_vocab_assign.
-#define MB_BUDGET ((size_t)256 << 20)
 static size_t mb_set_bytes(int n) { return (size_t)idivup(n, T3_MT) * T3_MT * (T3_A_BYTES / T3_MT + sizeof(float)); }
 static size_t mb_dir_bytes(int n1)
 {
@@ -937,7 +936,7 @@ static std::vector<MbWave> mb_waves(const cs_match_set *sets, int numSets, const
       return x;
     };
     int w = (int)waves.size() - 1;
-    if (w < 0 || waves[w].bytes + cost(w) > MB_BUDGET) { waves.emplace_back(); w++; }
+    if (w < 0 || waves[w].bytes + cost(w) > WAVE_BYTES) { waves.emplace_back(); w++; }
     MbWave &v = waves[w];
     v.bytes += cost(w);
     for (int s : {a, b})

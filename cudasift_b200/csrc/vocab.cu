@@ -573,7 +573,7 @@ __global__ void rt_pairs_kernel(const unsigned int *__restrict__ uniq, const int
 
 int retrieve_queries_per_wave(int numImages)
 {
-  const size_t k = RT_WAVE_BYTES / ((size_t)numImages * sizeof(unsigned long long));
+  const size_t k = WAVE_BYTES / ((size_t)numImages * sizeof(unsigned long long));
   return k < 1 ? 1 : k > (size_t)numImages ? numImages : (int)k;
 }
 

@@ -345,7 +345,10 @@ int cs_match_ratio_batch(const cs_match_set *sets, int numSets, const cs_match_j
  * - CS_E_ARG, before any CUDA call: the argument rules of cs_match_knn2 / cs_match_ratio except mode (there is one
  *   path), a model outside {1, 2}, a NULL model_in, a non-finite or all-zero model_in (or one whose norm is not
  *   finite), and thresh not finite or <= 0.  n1 == 0 or n2 == 0 returns 0 and writes nothing.  The records are only
- *   read.  The call synchronises once, at the end; the lists of cs_match_guided live in per-device scratch. */
+ *   read.  A cs_match_guided call issues 7 kernel launches with or without crossCheck (prep, histogram, scan, scatter,
+ *   knn over every direction, ratio test, pair writes), a cs_match_knn2_guided call 5 (no ratio test or pair writes)
+ *   (cs_launch_count).  The call synchronises once, at the end; the lists of cs_match_guided live in per-device
+ *   scratch. */
 int cs_match_knn2_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],
                          float thresh, int *d_idx, float *d_score, double *ms);
 int cs_match_guided(const void *d_s1, int n1, const void *d_s2, int n2, int model, const double model_in[9],

@@ -2,7 +2,7 @@
 (tests/guided_oracle.c) on planted two-view sets, forward motion, candidates on the admissible boundary and
 degenerate positions; the reverse direction through the cross-checked pairs; the two limits (a model that admits
 everything, one that admits nothing); monotonicity after verification on two shifted views; the culling statistics;
-reproducibility and interleaving with the other matchers."""
+reproducibility and interleaving with the other matchers; the launch counts of single calls."""
 import functools
 
 import numpy as np
@@ -245,3 +245,17 @@ def test_reproducible_host_equals_device_and_interleaving(cs):
     finally:
         cs.FreeSiftData(d1)
         cs.FreeSiftData(d2)
+
+
+def test_single_call_launches(cs):
+    """A single call runs as one job of the batch waves: 7 launches for cs_match_guided with or without the cross-check
+    (both directions' knn in one launch), 5 for cs_match_knn2_guided (no ratio test or pair writes)."""
+    s1, s2, F = planted(1000, 1200, False, 11)
+    L = cs.lib()
+    for cross in (False, True):
+        before = L.cs_launch_count()
+        pairs, _ = cs.match_guided_host(s1, s2, "fundamental", F, 4.0, crossCheck=cross)
+        assert L.cs_launch_count() - before == 7 and len(pairs) > 0, cross
+    before = L.cs_launch_count()
+    cs.match_knn2_guided(s1, s2, "fundamental", F, 4.0)
+    assert L.cs_launch_count() - before == 5

@@ -17,7 +17,7 @@ for _p in (ROOT, os.path.join(ROOT, "tests"), os.path.join(ROOT, "scripts")):
 pytestmark = pytest.mark.gpu
 
 T3 = ["prep", "gemm", "resolve", "exact-fallback", "reverse-gemm", "reverse-resolve", "reverse-exact-fallback", "pairs"]
-GUIDED = ["prep", "index", "knn", "reverse-knn"]
+GUIDED = ["prep", "index", "knn", "pairs"]
 RATIO_BATCH = ["prep", "gemm", "resolve", "exact-fallback", "pairs"]
 GUIDED_BATCH = ["prep", "index", "knn", "pairs"]
 VERIFY = ["flags", "compact", "norm", "hyp", "score", "argmax", "refit", "write"]
