@@ -21,7 +21,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "VerifyEssential", "verify_essential_host", "essential_stats", "essential_to_fundamental", "VerifyJob",
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
            "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
-           "BundleAdjust", "TrainVocabulary", "AssignWords", "RetrievePairs"]
+           "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
+           "RetrievePairs"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -100,6 +101,10 @@ def lib():
                                        vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_bundle_adjust": (ip, [vp, ip, vp, vp, vp, vp, vp, ip, vp, ip, vp, vp, ip, ip, c.c_double, c.c_double,
                                   vp, vp, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_bundle_adjust_intrinsics": (ip, [vp, ip, vp, vp, vp, ip, c.c_double, vp, vp, vp, vp, ip, vp, ip, vp, vp,
+                                             ip, ip, c.c_double, c.c_double, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                             c.POINTER(c.c_double)]),
+        "cs_undistort_records": (ip, [vp, ip, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -908,6 +913,22 @@ def BundleAdjust(datas, Ks, Rs, ts, offsets, members, points, use=None, fixed=No
     accepted}, stats int64 [8] as the header describes them, ms)."""
     S = len(datas)
     K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+
+    def call(args):
+        return lib().cs_bundle_adjust(args[0], S, _ptr(K), _ptr(R), _ptr(t), *args[1:])
+    R_out, t_out, rest = _bundle_call(call, datas, R, t, offsets, members, points, use, fixed, maxIterations,
+                                      maxLinearIterations, linearTol, maxError, "BundleAdjust")
+    return (R_out, t_out) + rest
+
+
+def _bundle_call(call, datas, R, t, offsets, members, points, use, fixed, maxIterations, maxLinearIterations,
+                 linearTol, maxError, what):
+    """The common arguments of BundleAdjust and BundleAdjustIntrinsics: call(args) makes the C call with args =
+    (sets, fixed, d_offsets, numTracks, d_members, numMembers, d_use, d_points, maxIterations, maxLinearIterations,
+    linearTol, maxError, R_out, t_out, d_errors, d_inlier, cost_out, trace_out, stats_out, ms) (the intrinsics' call
+    puts its K_out and dist_out before R_out).  Returns (R_out, t_out, (points, errors, inlier, cost, trace, stats,
+    ms))."""
+    S = len(datas)
     off, mem, T, M = _tracks(offsets, members)
     pts = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
     if len(pts) != T:
@@ -939,12 +960,11 @@ def BundleAdjust(datas, Ks, Rs, ts, offsets, members, points, use=None, fixed=No
             bufs[1].upload(mem)
             if u is not None:
                 bufs[5].upload(u)
-        _check(lib().cs_bundle_adjust(sets if S else None, S, _ptr(K), _ptr(R), _ptr(t), _ptr(fix) if S else None,
-                                          bufs[0].ptr, T, bufs[1].ptr, M, bufs[5].ptr if u is not None else None,
-                                          bufs[2].ptr, int(maxIterations), int(maxLinearIterations), float(linearTol),
-                                          float(maxError), _ptr(R_out), _ptr(t_out), bufs[3].ptr, bufs[4].ptr,
-                                          _ptr(cost), _ptr(trace) if len(trace) else None, _ptr(stats),
-                                          ctypes.byref(ms)), "BundleAdjust")
+        _check(call((sets if S else None, _ptr(fix) if S else None, bufs[0].ptr, T, bufs[1].ptr, M,
+                     bufs[5].ptr if u is not None else None, bufs[2].ptr, int(maxIterations),
+                     int(maxLinearIterations), float(linearTol), float(maxError), _ptr(R_out), _ptr(t_out),
+                     bufs[3].ptr, bufs[4].ptr, _ptr(cost), _ptr(trace) if len(trace) else None, _ptr(stats),
+                     ctypes.byref(ms))), what)
         if T:
             pts = bufs[2].download(np.float64, 3 * T).reshape(T, 3)
         if M and T:
@@ -953,7 +973,68 @@ def BundleAdjust(datas, Ks, Rs, ts, offsets, members, points, use=None, fixed=No
     finally:
         for buf in bufs:
             buf.free()
-    return R_out, t_out, pts, errors, inlier, (cost[0], cost[1]), trace[:int(stats[6])].copy(), stats, ms.value
+    return R_out, t_out, (pts, errors, inlier, (cost[0], cost[1]), trace[:int(stats[6])].copy(), stats, ms.value)
+
+
+LOSSES = {"trivial": 0, "soft_l1": 1, "cauchy": 2}
+
+
+def BundleAdjustIntrinsics(datas, Ks, Rs, ts, offsets, members, points, dists=None, refine=3, loss="trivial",
+                           lossScale=1.0, use=None, fixed=None, maxIterations=50, maxLinearIterations=100,
+                           linearTol=1e-6, maxError=4.0):
+    """Self-calibrating bundle adjustment in one call (cs_bundle_adjust_intrinsics): BundleAdjust with each image's
+    focal length and radial distortion (k1, k2) refined and a robust loss.  dists ([2] per image or one for every image;
+    None: zero) start the distortion; refine is one mask for every image or one per image (bit 0 focal, 1 k1, 2 k2;
+    the default 3, focal and k1, is COLMAP's mapper default); loss is "trivial", "soft_l1" or "cauchy" with scale
+    lossScale pixels.  The other arguments as BundleAdjust.  Returns (K [S, 3, 3], dists [S, 2], R [S, 3, 3], t [S, 3],
+    points [T, 3], errors float32 [M], inlier bool [M] under the final parameters, cost (initial, final), trace,
+    stats int64 [8], ms)."""
+    S = len(datas)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    dist = np.zeros((S, 2)) if dists is None else _per_image(dists, (2,), S, "dists")
+    ref = np.asarray(refine).reshape(-1)
+    if ref.size == 1:
+        ref = np.full(S, int(ref[0]))
+    if len(ref) != S:
+        raise ValueError("refine: one mask, or one per image, %d, not %d" % (S, len(ref)))
+    if (ref < 0).any() or (ref > 7).any():
+        raise ValueError("refine: masks of bits 0 (focal), 1 (k1) and 2 (k2)")
+    ref = np.ascontiguousarray(ref.astype(np.uint8))
+    if loss not in LOSSES:
+        raise ValueError("loss: one of %s, not %r" % (", ".join(LOSSES), loss))
+    K_out, dist_out = np.zeros((S, 3, 3)), np.zeros((S, 2))
+
+    def call(args):
+        return lib().cs_bundle_adjust_intrinsics(args[0], S, _ptr(K), _ptr(dist) if S else None,
+                                                 _ptr(ref) if S else None, LOSSES[loss], float(lossScale), _ptr(R),
+                                                 _ptr(t), *args[1:12], _ptr(K_out), _ptr(dist_out), *args[12:])
+    R_out, t_out, rest = _bundle_call(call, datas, R, t, offsets, members, points, use, fixed, maxIterations,
+                                      maxLinearIterations, linearTol, maxError, "BundleAdjustIntrinsics")
+    return (K_out, dist_out, R_out, t_out) + rest
+
+
+def UndistortRecords(datas, Ks, dists):
+    """The records of every image with their positions undistorted under Ks and dists (cs_undistort_records), in new
+    device SiftData (the caller frees them); every other field is copied, orientation and scale are not corrected.  A
+    record whose inverse does not exist gets NaN positions (an invalid track member).  Ks [3, 3] and dists [2] per image
+    or one for every image."""
+    S = len(datas)
+    K, dist = _per_image(Ks, (3, 3), S, "Ks"), _per_image(dists, (2,), S, "dists")
+    outs = []
+    try:
+        for d in datas:
+            o = InitSiftData(SiftData(), max(int(d.numPts), 1))
+            o.numPts = int(d.numPts)
+            outs.append(o)
+        ptrs = (ctypes.c_void_p * max(S, 1))(*[o.d_data for o in outs])
+        ms = ctypes.c_double(0.0)
+        _check(lib().cs_undistort_records(_set_table(datas) if S else None, S, _ptr(K), _ptr(dist),
+                                          ptrs if S else None, ctypes.byref(ms)), "UndistortRecords")
+    except BaseException:
+        for o in outs:
+            FreeSiftData(o)
+        raise
+    return outs
 
 
 class PoseJob(ctypes.Structure):

@@ -1432,20 +1432,29 @@ int cs_triangulate_tracks(const cs_match_set *sets, int numImages, const double 
   return (int)st[5];
 }
 
-int cs_bundle_adjust(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
-                     const unsigned char *fixed, const int *d_offsets, int numTracks, const int *d_members,
-                     int numMembers, const unsigned char *d_use, double *d_points, int maxIterations,
-                     int maxLinearIterations, double linearTol, double maxError, double *R_out, double *t_out,
-                     float *d_errors, unsigned char *d_inlier, double cost_out[2], double *trace_out,
-                     long long stats_out[8], double *ms)
+// K_out = Ks and dist_out = dists (zero for NULL dists), each when given.
+static void bundle_intrinsics_unchanged(int numImages, const double *Ks, const double *dists, double *K_out,
+                                        double *dist_out)
 {
-  const char *fn = "cs_bundle_adjust";
-  if (ms) *ms = 0.0;
-  int r = bundle_args(fn, sets, numImages, Ks, Rs, ts, fixed, d_offsets, numTracks, d_members, numMembers, d_use,
-                      d_points, maxIterations, maxLinearIterations, linearTol, maxError, R_out, t_out, d_errors,
-                      d_inlier, cost_out);
-  if (r < 0) return r;
+  if (K_out && K_out != Ks) memmove(K_out, Ks, (size_t)numImages * 9 * sizeof(double));
+  if (dist_out && dist_out != dists) {
+    if (dists) memmove(dist_out, dists, (size_t)numImages * 2 * sizeof(double));
+    else memset(dist_out, 0, (size_t)numImages * 2 * sizeof(double));
+  }
+}
+
+// cs_bundle_adjust and cs_bundle_adjust_intrinsics past their argument checks (fn names the call).
+static int bundle_adjust_checked(const char *fn, const cs_match_set *sets, int numImages, const double *Ks,
+                                 const double *dists, const unsigned char *refine, int loss, double lossScale,
+                                 const double *Rs, const double *ts, const unsigned char *fixed, const int *d_offsets,
+                                 int numTracks, const int *d_members, int numMembers, const unsigned char *d_use,
+                                 double *d_points, int maxIterations, int maxLinearIterations, double linearTol,
+                                 double maxError, double *K_out, double *dist_out, double *R_out, double *t_out,
+                                 float *d_errors, unsigned char *d_inlier, double cost_out[2], double *trace_out,
+                                 long long stats_out[8], double *ms)
+{
   if (numTracks == 0) {
+    bundle_intrinsics_unchanged(numImages, Ks, dists, K_out, dist_out);
     if (R_out != Rs) memmove(R_out, Rs, (size_t)numImages * 9 * sizeof(double));
     if (t_out != ts) memmove(t_out, ts, (size_t)numImages * 3 * sizeof(double));
     cost_out[0] = cost_out[1] = 0.0;
@@ -1458,13 +1467,76 @@ int cs_bundle_adjust(const cs_match_set *sets, int numImages, const double *Ks, 
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
+  int r;
   if ((r = timed_sync(fn, c, ms, [&] {
-         return bundle_enqueue(*c, sets, numImages, Ks, Rs, ts, fixed, d_offsets, numTracks, d_members, numMembers,
-                               d_use, d_points, maxIterations, maxLinearIterations, linearTol, maxError, d_errors,
-                               d_inlier);
+         return bundle_enqueue(*c, sets, numImages, Ks, dists, refine, loss, lossScale, Rs, ts, fixed, d_offsets,
+                               numTracks, d_members, numMembers, d_use, d_points, maxIterations, maxLinearIterations,
+                               linearTol, maxError, d_errors, d_inlier);
        })) < 0)
     return r;
-  return bundle_result(*c, numImages, maxIterations, R_out, t_out, cost_out, trace_out, stats_out);
+  // K and k come back from the device only when the call ran the 9-parameter block; else they are the input's
+  const int nc = bundle_camera_block(numImages, dists, refine);
+  if (nc == 6) bundle_intrinsics_unchanged(numImages, Ks, dists, K_out, dist_out);
+  return bundle_result(*c, nc, numImages, maxIterations, K_out, dist_out, R_out, t_out, cost_out, trace_out,
+                       stats_out);
+}
+
+int cs_bundle_adjust(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs, const double *ts,
+                     const unsigned char *fixed, const int *d_offsets, int numTracks, const int *d_members,
+                     int numMembers, const unsigned char *d_use, double *d_points, int maxIterations,
+                     int maxLinearIterations, double linearTol, double maxError, double *R_out, double *t_out,
+                     float *d_errors, unsigned char *d_inlier, double cost_out[2], double *trace_out,
+                     long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_bundle_adjust";
+  if (ms) *ms = 0.0;
+  const int r = bundle_args(fn, sets, numImages, Ks, Rs, ts, fixed, d_offsets, numTracks, d_members, numMembers,
+                            d_use, d_points, maxIterations, maxLinearIterations, linearTol, maxError, R_out, t_out,
+                            d_errors, d_inlier, cost_out);
+  if (r < 0) return r;
+  return bundle_adjust_checked(fn, sets, numImages, Ks, nullptr, nullptr, 0, 1.0, Rs, ts, fixed, d_offsets, numTracks,
+                               d_members, numMembers, d_use, d_points, maxIterations, maxLinearIterations, linearTol,
+                               maxError, nullptr, nullptr, R_out, t_out, d_errors, d_inlier, cost_out, trace_out,
+                               stats_out, ms);
+}
+
+int cs_bundle_adjust_intrinsics(const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                                const unsigned char *refine, int loss, double lossScale, const double *Rs,
+                                const double *ts, const unsigned char *fixed, const int *d_offsets, int numTracks,
+                                const int *d_members, int numMembers, const unsigned char *d_use, double *d_points,
+                                int maxIterations, int maxLinearIterations, double linearTol, double maxError,
+                                double *K_out, double *dist_out, double *R_out, double *t_out, float *d_errors,
+                                unsigned char *d_inlier, double cost_out[2], double *trace_out, long long stats_out[8],
+                                double *ms)
+{
+  const char *fn = "cs_bundle_adjust_intrinsics";
+  if (ms) *ms = 0.0;
+  int r = bundle_args(fn, sets, numImages, Ks, Rs, ts, fixed, d_offsets, numTracks, d_members, numMembers, d_use,
+                      d_points, maxIterations, maxLinearIterations, linearTol, maxError, R_out, t_out, d_errors,
+                      d_inlier, cost_out);
+  if (r < 0) return r;
+  r = bundle_intrinsics_args(fn, numImages, Ks, dists, refine, loss, lossScale, Rs, ts, K_out, dist_out, R_out, t_out);
+  if (r < 0) return r;
+  return bundle_adjust_checked(fn, sets, numImages, Ks, dists, refine, loss, lossScale, Rs, ts, fixed, d_offsets,
+                               numTracks, d_members, numMembers, d_use, d_points, maxIterations, maxLinearIterations,
+                               linearTol, maxError, K_out, dist_out, R_out, t_out, d_errors, d_inlier, cost_out,
+                               trace_out, stats_out, ms);
+}
+
+int cs_undistort_records(const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                         void *const *d_out, double *ms)
+{
+  const char *fn = "cs_undistort_records";
+  if (ms) *ms = 0.0;
+  long long total = 0;
+  int r = undistort_args(fn, sets, numImages, Ks, dists, d_out, &total);
+  if (r < 0 || total == 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = timed_sync(fn, c, ms, [&] { return undistort_enqueue(*c, sets, numImages, Ks, dists, d_out); })) < 0)
+    return r;
+  return 0;
 }
 
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,

@@ -450,6 +450,65 @@ int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const d
   return rs.check(fn);
 }
 
+// The intrinsic arguments of cs_bundle_adjust_intrinsics, then its host arrays: an output may equal its own input
+// exactly (K_out == Ks, dist_out == dists, R_out == Rs, t_out == ts); otherwise no output shares a byte with another
+// output or with any of the four inputs.
+int bundle_intrinsics_args(const char *fn, int numImages, const double *Ks, const double *dists,
+                           const unsigned char *refine, int loss, double lossScale, const double *Rs, const double *ts,
+                           const double *K_out, const double *dist_out, const double *R_out, const double *t_out)
+{
+  for (int a = 0; refine && a < numImages; a++)
+    if (refine[a] > 7) return arg_error(fn, "refine[%d] must be a mask of bits 0 (focal), 1 (k1) and 2 (k2)", a);
+  if (loss < 0 || loss > 2) return arg_error(fn, "loss must be 0 (trivial), 1 (soft-L1) or 2 (Cauchy)");
+  if (!std::isfinite(lossScale) || !(lossScale > 0.0)) return arg_error(fn, "lossScale must be finite and > 0");
+  for (int a = 0; dists && a < numImages; a++)
+    if (!std::isfinite(dists[2 * (size_t)a]) || !std::isfinite(dists[2 * (size_t)a + 1]))
+      return arg_error(fn, "dists[%d] must be finite", a);
+  if (numImages <= 0) return 0;
+  static const char *const names[8] = {"K_out", "dist_out", "R_out", "t_out", "Ks", "dists", "Rs", "ts"};
+  const double *outs[4] = {K_out, dist_out, R_out, t_out}, *ins[4] = {Ks, dists, Rs, ts};
+  const size_t per[4] = {9, 2, 9, 3};
+  ArgRanges rs(names, 8);
+  for (int k = 0; k < 4; k++) {
+    const size_t bytes = (size_t)numImages * per[k] * sizeof(double);
+    if (outs[k]) rs.add(outs[k], bytes, k, 0, true);
+    if (ins[k] && ins[k] != outs[k]) rs.add(ins[k], bytes, 4 + k, 0, false);
+  }
+  return rs.check(fn);
+}
+
+// The images, the intrinsics and the outputs of cs_undistort_records: d_out[a] is 4-byte aligned and either is
+// sets[a].pts exactly (in place) or shares no byte with another output or any set's records.
+int undistort_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                   void *const *d_out, long long *total)
+{
+  if (numImages < 0 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [0, 2^24]");
+  if (numImages > 0 && (!sets || !Ks || !d_out)) return arg_error(fn, "numImages > 0 needs sets, Ks and d_out");
+  int r = check_set_table(fn, sets, numImages);
+  if (r < 0) return r;
+  long long n = 0;
+  for (int a = 0; a < numImages; a++) {
+    char name[32];
+    snprintf(name, sizeof name, "Ks[%d]", a);
+    if ((r = check_intrinsics(fn, Ks + 9 * (size_t)a, name)) < 0) return r;
+    if (dists && (!std::isfinite(dists[2 * (size_t)a]) || !std::isfinite(dists[2 * (size_t)a + 1])))
+      return arg_error(fn, "dists[%d] must be finite", a);
+    if (sets[a].n > 0 && !d_out[a]) return arg_error(fn, "d_out[%d]: a set with records needs an output", a);
+    if (sets[a].n > 0 && misaligned(d_out[a], 4)) return arg_error(fn, "d_out[%d] must be 4-byte aligned", a);
+    n += sets[a].n;
+  }
+  // the outputs (written; an in-place set is its own output) and the records (read)
+  static const char *const names[2] = {"d_out[%d]", "sets[%d].pts"};
+  ArgRanges rs(names, 2 * (size_t)numImages);
+  for (int a = 0; a < numImages; a++) {
+    const size_t bytes = record_bytes(sets[a].n);
+    rs.add(d_out[a], bytes, 0, a, true);
+    if (d_out[a] != sets[a].pts) rs.add(sets[a].pts, bytes, 1, a, false);
+  }
+  *total = n;
+  return rs.check(fn);
+}
+
 // The set table of the vocabulary calls and the feature total *M (at most INT_MAX).
 static int vocab_sets(const char *fn, const cs_match_set *sets, int numSets, int numWords, int *M)
 {

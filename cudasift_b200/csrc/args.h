@@ -52,6 +52,13 @@ int bundle_args(const char *fn, const cs_match_set *sets, int numImages, const d
                 int numMembers, const unsigned char *use, const double *points, int maxIterations,
                 int maxLinearIterations, double linearTol, double maxError, const double *R_out, const double *t_out,
                 const float *errors, const unsigned char *inlier, const double *cost_out);
+// cs_bundle_adjust_intrinsics past bundle_args: refine, loss, lossScale, dists and the host output aliasing rule.
+int bundle_intrinsics_args(const char *fn, int numImages, const double *Ks, const double *dists,
+                           const unsigned char *refine, int loss, double lossScale, const double *Rs, const double *ts,
+                           const double *K_out, const double *dist_out, const double *R_out, const double *t_out);
+// cs_undistort_records; *total receives the record total.
+int undistort_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                   void *const *d_out, long long *total);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

@@ -607,16 +607,23 @@ int pose_result(const DeviceCtx &c, int q, double R[9], double t[3], long long s
 int pose_models_to_host(DeviceCtx &c, const cs_pose_job &job, int numLoops, double *h_R, double *h_t, int *h_counts);
 
 // ---- bundle adjustment (bundle.cu) -----------------------------------------------------------------------------
-// The launches of cs_bundle_adjust (argument-checked, numTracks > 0) on c.stream, without a synchronize; the results
-// reach c.h_bundle by the caller's synchronize, and bundle_result reads them.
-int bundle_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
-                   const double *ts, const unsigned char *fixed, const int *offsets, int numTracks, const int *members,
-                   int numMembers, const unsigned char *use, double *points, int maxIterations, int maxLinearIterations,
+// The camera block of a call: 9 when an image refines an intrinsic or has a nonzero distortion coefficient, else 6.
+int bundle_camera_block(int numImages, const double *dists, const unsigned char *refine);
+// The launches of cs_bundle_adjust_intrinsics (argument-checked, numTracks > 0) on c.stream, without a synchronize;
+// the results reach c.h_bundle by the caller's synchronize, and bundle_result reads them.
+int bundle_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                   const unsigned char *refine, int loss, double lossScale, const double *Rs, const double *ts,
+                   const unsigned char *fixed, const int *offsets, int numTracks, const int *members, int numMembers,
+                   const unsigned char *use, double *points, int maxIterations, int maxLinearIterations,
                    double linearTol, double maxError, float *errors, unsigned char *inlier);
-// after the synchronize: the final R, t of every image, the costs, the trace (may be NULL) and the statistics; returns
-// the number of accepted steps
-int bundle_result(const DeviceCtx &c, int numImages, int maxIterations, double *R_out, double *t_out, double cost[2],
-                  double *trace, long long stats[8]);
+// after the synchronize, for the camera block nc the call ran: the final K, (k1, k2) (nc == 9 only; either may be
+// NULL), R, t of every image, the costs, the trace (may be NULL) and the statistics; returns the number of accepted
+// steps
+int bundle_result(const DeviceCtx &c, int nc, int numImages, int maxIterations, double *K_out, double *dist_out,
+                  double *R_out, double *t_out, double cost[2], double *trace, long long stats[8]);
+// The launch of cs_undistort_records (argument-checked, at least one record) on c.stream, without a synchronize.
+int undistort_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                      void *const *d_out);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

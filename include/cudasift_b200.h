@@ -752,6 +752,75 @@ int cs_bundle_adjust(const cs_match_set *sets, int numImages, const double *Ks, 
                      float *d_errors, unsigned char *d_inlier, double cost_out[2], double *trace_out,
                      long long stats_out[8], double *ms);
 
+/* Self-calibrating bundle adjustment (COLMAP's RADIAL camera, generalised to the full upper-triangular K): everything
+ * cs_bundle_adjust does, with per-image focal length and radial distortion refined and a robust loss.  cs_bundle_adjust
+ * is this call with dists = NULL, refine = NULL, loss = 0, K_out = dist_out = NULL.
+ * - Camera model, per image: K (K0 = fx, K1 = skew, K2 = cx, K4 = fy, K5 = cy) and k = (k1, k2) = dists[a] (NULL: all
+ *   zero).  With Xc = R X + t: (a, b) = (Xc0, Xc1) / Xc2, rho2 = a^2 + b^2, D = 1 + k1 rho2 + k2 rho2^2,
+ *   (a', b') = D (a, b), r = (K0 a' + K1 b' + K2 - x, K4 b' + K5 - y).  With k = 0 this is cs_bundle_adjust's residual.
+ * - Refined intrinsics: refine[a] (host bytes; NULL = none) has bit 0 the focal f = K0, bit 1 k1, bit 2 k2.  Update
+ *   f <- f + df with K1 / K0 and K4 / K0 held (K0c = K0 + df, K1c = K1 (K0c / K0), K4c = K4 (K0c / K0)),
+ *   k1 <- k1 + dk1, k2 <- k2 + dk2.  The principal point is not refined.  Intrinsics are held exactly as pose
+ *   components are: fixed governs the pose, refine the intrinsics, an image with no used observation holds everything,
+ *   and held values come back bit for bit.
+ * - Jacobian: with Dp = 2 (k1 + 2 k2 rho2), d(a', b') / d(a, b) = [D + Dp a^2, Dp a b; Dp a b, D + Dp b^2] = Dd and
+ *   d(u, v) / d(a, b) = [K0 K1; 0 K4] Dd, the rows gr = d(u, v) / d(Xc) give the pose and point rows as in
+ *   cs_bundle_adjust; d(u, v) / df = (K0 a' + K1 b', K4 b') / K0, d(u, v) / dk1 = (K0 a + K1 b, K4 b) rho2, and
+ *   d(u, v) / dk2 = that times rho2.
+ * - Loss on s = r^T r of each used observation, scale c = lossScale > 0 pixels, applied as c^2 rho(s / c^2):
+ *   loss 0 trivial rho(s) = s; 1 soft-L1 rho(s) = 2 (sqrt(1 + s) - 1), computed as 2 s / (sqrt(1 + s) + 1); 2 Cauchy
+ *   rho(s) = log(1 + s) (log1p).  The cost is the sum over the used observations (no 1/2).  Linearisation follows
+ *   Ceres's corrector: for these losses rho'' <= 0, so it reduces to scaling the observation's r and both Jacobian
+ *   blocks by sqrt(rho'(s / c^2)) (1 / sqrt(sqrt(1 + u)) soft-L1, 1 / sqrt(1 + u) Cauchy, u = s / c^2), taken at each
+ *   relinearisation; the candidate's cost uses the same rho.
+ * - Camera block: NC = 6 (w, delta) when no image refines an intrinsic and every k is 0 (0.0 or -0.0), else NC = 9
+ *   (w, delta, f, k1, k2) for every image.  NC = 6 with the trivial loss is cs_bundle_adjust's kernel, byte for byte.
+ *   Everything of cs_bundle_adjust that is per camera grows to NC: U, g_c, the Schur term, the preconditioner block and
+ *   its Cholesky, CG's vectors.  LM additionally rejects a step after which a refined focal is not > 0.
+ * - Outputs as cs_bundle_adjust's, plus K_out [numImages][9] (the final K, row-major, K[6..8] = (0, 0, 1)) and
+ *   dist_out [numImages][2] (final k1, k2); either may be NULL, and K_out may equal Ks, dist_out dists, R_out Rs and
+ *   t_out ts exactly.  With NC = 6 they are the input's (zeros for NULL dists).  stats_out[5] counts the free
+ *   intrinsic parameters too.  Member outputs under the final parameters: with NC = 6 cs_bundle_adjust's rule; with
+ *   NC = 9 err = (float)sqrt(r^T r) of the residual above (inf when Xc2 <= 0), inlier when Xc2 > 0 and
+ *   r^T r < maxError^2.
+ * - Determinism, launches and the fixed summation orders are cs_bundle_adjust's: 3 kernel launches, no floating-point
+ *   atomics, two calls give the same bytes.  Scratch with NC = 9: 2 400 bytes per image (1 536 of state, 864 of camera
+ *   pieces), 176 per track, 248 per member (the observation, J_c, J_p and r, the sort keys), 864 per 256 members,
+ *   36 per LM iteration, plus the cub storage; pinned, 1 536 bytes per image and 32 per LM iteration.
+ * - CS_E_ARG, before any CUDA call: every check of cs_bundle_adjust (naming cs_bundle_adjust_intrinsics), a refine[a]
+ *   > 7, loss outside 0..2, lossScale not finite or not > 0, a non-finite dists[a], and a host output (K_out, dist_out,
+ *   R_out, t_out) that overlaps another output or an input (Ks, dists, Rs, ts) other than exactly its own.
+ *   numTracks == 0 returns 0 with the inputs copied to the outputs and makes no CUDA call.
+ * dists [numImages][2] or NULL; refine [numImages] or NULL. */
+int cs_bundle_adjust_intrinsics(const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                                const unsigned char *refine, int loss, double lossScale, const double *Rs,
+                                const double *ts, const unsigned char *fixed, const int *d_offsets, int numTracks,
+                                const int *d_members, int numMembers, const unsigned char *d_use, double *d_points,
+                                int maxIterations, int maxLinearIterations, double linearTol, double maxError,
+                                double *K_out, double *dist_out, double *R_out, double *t_out, float *d_errors,
+                                unsigned char *d_inlier, double cost_out[2], double *trace_out, long long stats_out[8],
+                                double *ms);
+
+/* Undistortion of records under cs_bundle_adjust_intrinsics' radial model, so that triangulation and absolute pose
+ * (pinhole) can use a refined camera: every record of sets[a] goes to d_out[a] (device, sets[a].n records) with its
+ * position corrected under Ks[a] and dists[a] (NULL: all zero) and every other field copied byte for byte.  Orientation
+ * and scale are not corrected.
+ * - Rule (float64): b = (y - K5) / K4, a = (x - K2 - K1 b) / K0, r_d = sqrt(a^2 + b^2).  Radial distortion keeps the
+ *   direction, so r_u solves r_u (1 + k1 r_u^2 + k2 r_u^4) = r_d: Newton's method from r_u = r_d, at most 20
+ *   iterations; an iteration with derivative d = 1 + 3 k1 r_u^2 + 5 k2 r_u^4 not > 0 fails, else it takes
+ *   r_u -= (r_u (1 + k1 r_u^2 + k2 r_u^4) - r_d) / d and converges when that step's |step| <= 1e-12 r_d.  The output
+ *   position is (K0 a s + K1 b s + K2, K4 b s + K5) with s = r_u / r_d (1 when r_d = 0), rounded to float.  A record
+ *   gets NaN positions when the solve fails or does not converge, or when d <= 0 at the final r_u; NaN makes it an
+ *   invalid member for every track stage.  A non-finite input position gives NaN.
+ * - d_out[a] may equal sets[a].pts exactly (in place); otherwise it overlaps no other output and no set's records.
+ * - Returns 0 or CS_E_*.  One kernel launch (a thread per record); the call synchronises once, *ms (may be NULL) gets
+ *   its event time; no records make no CUDA call.  CS_E_ARG, before any CUDA call, naming the argument: numImages
+ *   outside [0, 2^24], NULL sets, Ks or d_out with numImages > 0, a set with records and no pointer, an invalid Ks[a]
+ *   (cs_verify_essential's rule), a non-finite dists[a], NULL or not 4-byte aligned d_out[a] for a set with records,
+ *   and an overlap (one sweep over sorted ranges). */
+int cs_undistort_records(const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
+                         void *const *d_out, double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,

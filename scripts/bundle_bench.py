@@ -12,7 +12,10 @@ The median of the call's event time over `--reps` calls after warm-up; the card'
 same run.  Phases inside the cooperative kernel are invisible to a profiler, so the time is split by differences of
 calls: maxIterations = 0 (setup and evaluation), 1 LM iteration with 1 CG iteration, and 1 LM iteration with
 --cg CG iterations (linearTol 1e-30 so that all of them run).  --host adds scipy.optimize.least_squares (TRF, LSMR,
-jac_sparsity) on (a) and (b) over the same observations, parameters and gauge.  Writes one JSON line (and --out FILE)."""
+jac_sparsity) on (a) and (b) over the same observations, parameters and gauge.  --refine MASK and --loss NAME add, for
+every workload in the same run, the same measurements of BundleAdjustIntrinsics (cs_bundle_adjust_intrinsics) with that
+refine mask (bit 0 focal, 1 k1, 2 k2), loss and --loss-scale, from the same start and k = 0, under the key
+"<workload>_intrinsics".  Writes one JSON line (and --out FILE)."""
 import argparse
 import json
 import os
@@ -63,18 +66,26 @@ def workload(cs, name):
     return [Data(cs, xy) for xy in s["xy"]], s, lambda: None
 
 
-def run_gpu(name, reps, cg):
+def run_gpu(name, reps, cg, intrinsics=None):
+    """intrinsics None: BundleAdjust; else (refine, loss, lossScale) of BundleAdjustIntrinsics."""
     import cudasift_b200 as cs
     cs.InitCuda(0)
     datas, s, free = workload(cs, name)
     args = (datas, s["K"], s["R0"], s["t0"], s["offsets"], s["members"], s["X0"])
     use = dict(use=s["use"])
+    if intrinsics:
+        use.update(refine=intrinsics[0], loss=intrinsics[1], lossScale=intrinsics[2])
+
+    def call(**kw):
+        if intrinsics:
+            return cs.BundleAdjustIntrinsics(*args, **kw)[2:]       # from R on: BundleAdjust's tuple
+        return cs.BundleAdjust(*args, **kw)
 
     def timed(**kw):
         kw.update(use)
         for _ in range(2):
-            out = cs.BundleAdjust(*args, **kw)
-        ms = [cs.BundleAdjust(*args, **kw)[-1] for _ in range(reps)]
+            out = call(**kw)
+        ms = [call(**kw)[-1] for _ in range(reps)]
         return out, float(np.median(ms))
     full, ms_full = timed(maxIterations=20, maxLinearIterations=50, linearTol=1e-2)
     _, ms_eval = timed(maxIterations=0)
@@ -131,6 +142,9 @@ def main():
     ap.add_argument("--workloads", default="abc")
     ap.add_argument("--cg", type=int, default=21)
     ap.add_argument("--host", action="store_true")
+    ap.add_argument("--refine", type=int, default=None)
+    ap.add_argument("--loss", default=None, choices=["trivial", "soft_l1", "cauchy"])
+    ap.add_argument("--loss-scale", type=float, default=2.0)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     res = dict(card=card())
@@ -138,6 +152,10 @@ def main():
         s, res[w] = run_gpu(w, a.reps, a.cg)
         if a.host and w in "ab":
             res[w].update(host_arm(s))
+        if a.refine is not None or a.loss is not None:
+            mode = (3 if a.refine is None else a.refine, a.loss or "trivial", a.loss_scale)
+            _, res[w + "_intrinsics"] = run_gpu(w, a.reps, a.cg, mode)
+            res[w + "_intrinsics"].update(refine=mode[0], loss=mode[1], loss_scale=mode[2])
     line = json.dumps(res)
     print(line)
     if a.out:
