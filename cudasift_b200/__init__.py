@@ -22,7 +22,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
            "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
-           "RetrievePairs"]
+           "RetrievePairs", "RotationAveraging", "GlobalPositioning"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -105,6 +105,10 @@ def lib():
                                              ip, ip, c.c_double, c.c_double, vp, vp, vp, vp, vp, vp, vp, vp, vp,
                                              c.POINTER(c.c_double)]),
         "cs_undistort_records": (ip, [vp, ip, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_global_positioning": (ip, [vp, ip, vp, vp, vp, ip, vp, ip, vp, ip, c.c_ulonglong, ip, c.c_double, ip, ip,
+                                       c.c_double, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_rotation_averaging": (ip, [ip, vp, ip, vp, vp, ip, ip, ip, c.c_double, c.c_double, c.c_double, vp, vp, vp,
+                                       vp, vp, vp, vp]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1035,6 +1039,81 @@ def UndistortRecords(datas, Ks, dists):
             FreeSiftData(o)
         raise
     return outs
+
+
+def RotationAveraging(numImages, edges, Rrel, weights, refImage=0, maxIterations=50, maxLinearIterations=200,
+                      linearTol=1e-8, sigmaDeg=5.0, maxAngleDeg=5.0):
+    """Every image's absolute rotation from the relative rotations of verified pairs (cs_rotation_averaging): a maximum
+    spanning tree by weight for the start, then IRLS under the Geman-McClure loss at sigmaDeg degrees (0: the squared
+    loss), each iteration a Laplacian system solved by CG on the device.  edges [E, 2] are image pairs {i, j}, Rrel
+    [E, 3, 3] VerifyEssentialBatch's R for them (X_j = R X_i + t) and weights [E] (for example its inlier counts), all
+    > 0.  Returns (R [N, 3, 3] (NaN for an image not joined to refImage), residual angles in degrees [E] (NaN for an
+    edge outside refImage's component), inlier bool [E] (angle < maxAngleDeg), cost (start, final), trace float64
+    [iterations run, 3] of {cost, CG iterations, largest step}, stats int64 [6] as the header describes them,
+    ms (spanning tree on the host, device))."""
+    N = int(numImages)
+    ed = np.ascontiguousarray(np.asarray(edges, np.int64).reshape(-1, 2).astype(np.int32))
+    E = len(ed)
+    Q = np.ascontiguousarray(np.asarray(Rrel, np.float64).reshape(-1, 9))
+    w = np.ascontiguousarray(np.asarray(weights, np.float64).reshape(-1))
+    if len(Q) != E or len(w) != E:
+        raise ValueError("Rrel and weights: one per edge, %d, not %d and %d" % (E, len(Q), len(w)))
+    R = np.zeros((max(N, 0), 9))
+    residuals, inlier = np.full(E, np.nan), np.zeros(E, np.uint8)
+    cost, trace = np.zeros(2), np.zeros((max(int(maxIterations), 0), 3))
+    stats, ms = np.zeros(6, np.int64), np.zeros(2)
+    p = (lambda a: _ptr(a) if a.size else None)
+    _check(lib().cs_rotation_averaging(N, p(ed), E, p(Q), p(w), int(refImage), int(maxIterations),
+                                       int(maxLinearIterations), float(linearTol), float(sigmaDeg),
+                                       float(maxAngleDeg), p(R), p(residuals), p(inlier), _ptr(cost), p(trace),
+                                       _ptr(stats), _ptr(ms)), "RotationAveraging")
+    return (R.reshape(-1, 3, 3), residuals, inlier.astype(bool), (cost[0], cost[1]), trace[:int(stats[3])].copy(),
+            stats, (ms[0], ms[1]))
+
+
+def GlobalPositioning(datas, Ks, Rs, offsets, members, use=None, refImage=0, seed=0, loss="trivial", lossScale=1.0,
+                      maxIterations=100, maxLinearIterations=100, linearTol=1e-6):
+    """Every camera centre and track point from known rotations, in one call (cs_global_positioning): GLOMAP's BATA
+    residual v - s (X - c) on every used observation, from random starts, by Levenberg-Marquardt on the device.  datas,
+    Ks, offsets and members as for BundleAdjust; Rs [S, 3, 3] RotationAveraging's rotations (NaN: the image takes no
+    part); use (bool [M]) selects members, None every valid one; loss "trivial", "soft_l1" or "cauchy" with scale
+    lossScale (on unit rays).  Returns (t [S, 3] (NaN without a used observation), points [T, 3] (NaN for a track with
+    fewer than 2), cost (start, final), trace float64 [iterations run, 4] as BundleAdjust's, stats int64 [8] as the
+    header describes them, ms), at the header's scale: the RMS distance of the positioned centres from refImage's."""
+    S = len(datas)
+    K = _per_image(Ks, (3, 3), S, "Ks")
+    R = _per_image(Rs, (3, 3), S, "Rs")
+    off, mem, T, M = _tracks(offsets, members)
+    u = None if use is None else np.ascontiguousarray(np.asarray(use).reshape(-1).astype(np.uint8))
+    if u is not None and len(u) != M:
+        raise ValueError("use: one per member, %d, not %d" % (M, len(u)))
+    if loss not in LOSSES:
+        raise ValueError("loss: one of %s, not %r" % (", ".join(LOSSES), loss))
+    t = np.zeros((S, 3))
+    points = np.full((T, 3), np.nan)
+    cost, trace = np.zeros(2), np.zeros((max(int(maxIterations), 0), 4))
+    stats, ms = np.zeros(8, np.int64), ctypes.c_double(0.0)
+    bufs = [DeviceBuffer(max(off.nbytes, 4)), DeviceBuffer(max(mem.nbytes, 8)), DeviceBuffer(max(points.nbytes, 8)),
+            DeviceBuffer(max(M, 1))]
+    try:
+        if T:
+            bufs[0].upload(off)
+        if M:
+            bufs[1].upload(mem)
+            if u is not None:
+                bufs[3].upload(u)
+        _check(lib().cs_global_positioning(_set_table(datas) if S else None, S, _ptr(K), _ptr(R), bufs[0].ptr, T,
+                                           bufs[1].ptr, M, bufs[3].ptr if u is not None else None, int(refImage),
+                                           int(seed), LOSSES[loss], float(lossScale), int(maxIterations),
+                                           int(maxLinearIterations), float(linearTol), _ptr(t), bufs[2].ptr,
+                                           _ptr(cost), _ptr(trace) if len(trace) else None, _ptr(stats),
+                                           ctypes.byref(ms)), "GlobalPositioning")
+        if T:
+            points = bufs[2].download(np.float64, 3 * T).reshape(T, 3)
+    finally:
+        for buf in bufs:
+            buf.free()
+    return t, points, (cost[0], cost[1]), trace[:int(stats[6])].copy(), stats, ms.value
 
 
 class PoseJob(ctypes.Structure):

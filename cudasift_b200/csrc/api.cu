@@ -1539,6 +1539,73 @@ int cs_undistort_records(const cs_match_set *sets, int numImages, const double *
   return 0;
 }
 
+int cs_rotation_averaging(int numImages, const int *edges, int numEdges, const double *Rrel, const double *weights,
+                          int refImage, int maxIterations, int maxLinearIterations, double linearTol, double sigmaDeg,
+                          double maxAngleDeg, double *R_out, double *residuals_out, unsigned char *inlier_out,
+                          double cost_out[2], double *trace_out, long long stats_out[6], double ms_out[2])
+{
+  const char *fn = "cs_rotation_averaging";
+  if (ms_out) ms_out[0] = ms_out[1] = 0.0;
+  int r = rotavg_args(fn, numImages, edges, numEdges, Rrel, weights, refImage, maxIterations, maxLinearIterations,
+                      linearTol, sigmaDeg, maxAngleDeg, R_out, residuals_out, inlier_out, cost_out, trace_out);
+  if (r < 0) return r;
+  if (numEdges == 0) {
+    for (int a = 0; a < numImages; a++)
+      for (int k = 0; k < 9; k++) R_out[9 * (size_t)a + k] = a == refImage ? (k % 4 == 0 ? 1.0 : 0.0) : NAN;
+    cost_out[0] = cost_out[1] = 0.0;
+    if (trace_out)
+      for (int k = 0; k < 3 * maxIterations; k++) trace_out[k] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 6; k++) stats_out[k] = k == 2 ? 1 : 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const auto t0 = std::chrono::steady_clock::now();
+  if ((r = rotavg_prepare(*c, numImages, edges, numEdges, Rrel, weights, refImage, maxIterations)) < 0) return r;
+  if (ms_out) ms_out[0] = ms_since(t0);
+  if ((r = timed_sync(fn, c, ms_out ? ms_out + 1 : nullptr, [&] {
+         return rotavg_enqueue(*c, numImages, numEdges, maxIterations, maxLinearIterations, linearTol, sigmaDeg);
+       })) < 0)
+    return r;
+  return rotavg_result(*c, numImages, numEdges, maxIterations, maxAngleDeg, R_out, residuals_out, inlier_out, cost_out,
+                       trace_out, stats_out);
+}
+
+int cs_global_positioning(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                          const int *d_offsets, int numTracks, const int *d_members, int numMembers,
+                          const unsigned char *d_use, int refImage, unsigned long long seed, int loss, double lossScale,
+                          int maxIterations, int maxLinearIterations, double linearTol, double *t_out,
+                          double *d_points, double cost_out[2], double *trace_out, long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_global_positioning";
+  if (ms) *ms = 0.0;
+  int r = globalpos_args(fn, sets, numImages, Ks, Rs, d_offsets, numTracks, d_members, numMembers, d_use, refImage,
+                         loss, lossScale, maxIterations, maxLinearIterations, linearTol, t_out, d_points, cost_out,
+                         trace_out);
+  if (r < 0) return r;
+  if (numTracks == 0) {
+    for (int k = 0; k < 3 * numImages; k++) t_out[k] = NAN;
+    cost_out[0] = cost_out[1] = 0.0;
+    if (trace_out)
+      for (int k = 0; k < 4 * maxIterations; k++) trace_out[k] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 8; k++) stats_out[k] = 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return globalpos_enqueue(*c, sets, numImages, Ks, Rs, d_offsets, numTracks, d_members, numMembers, d_use,
+                                  refImage, seed, loss, lossScale, maxIterations, maxLinearIterations, linearTol,
+                                  d_points);
+       })) < 0)
+    return r;
+  return globalpos_result(*c, numImages, Rs, maxIterations, t_out, cost_out, trace_out, stats_out);
+}
+
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,
                            const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
                            int *counts_out, long long *stats_out, double *ms)

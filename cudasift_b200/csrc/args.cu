@@ -509,6 +509,128 @@ int undistort_args(const char *fn, const cs_match_set *sets, int numImages, cons
   return rs.check(fn);
 }
 
+// The parameters of cs_rotation_averaging, its host arrays (the outputs R_out, residuals_out, inlier_out, cost_out and
+// trace_out share no byte with each other or with the inputs edges, Rrel and weights), then every edge.
+int rotavg_args(const char *fn, int numImages, const int *edges, int numEdges, const double *Rrel,
+                const double *weights, int refImage, int maxIterations, int maxLinearIterations, double linearTol,
+                double sigmaDeg, double maxAngleDeg, const double *R_out, const double *residuals,
+                const unsigned char *inlier, const double *cost_out, const double *trace_out)
+{
+  if (numImages < 1 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [1, 2^24]");
+  if (numEdges < 0 || numEdges > (1 << 26)) return arg_error(fn, "numEdges must be in [0, 2^26]");
+  if (refImage < 0 || refImage >= numImages) return arg_error(fn, "refImage must be in [0, numImages)");
+  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
+  if (maxLinearIterations < 1 || maxLinearIterations > 10000)
+    return arg_error(fn, "maxLinearIterations must be in [1, 10000]");
+  if (!(linearTol > 0.0) || !(linearTol < 1.0)) return arg_error(fn, "linearTol must be in (0, 1)");
+  if (!(sigmaDeg >= 0.0) || !(sigmaDeg <= 180.0)) return arg_error(fn, "sigmaDeg must be in [0, 180]");
+  if (!(maxAngleDeg > 0.0) || !(maxAngleDeg <= 180.0)) return arg_error(fn, "maxAngleDeg must be in (0, 180]");
+  if (numEdges > 0 && (!edges || !Rrel || !weights)) return arg_error(fn, "numEdges > 0 needs edges, Rrel and weights");
+  if (!R_out || !cost_out) return arg_error(fn, "R_out and cost_out must not be NULL");
+  static const char *const names[8] = {"R_out", "residuals_out", "inlier_out", "cost_out", "trace_out", "edges",
+                                        "Rrel", "weights"};
+  ArgRanges rs(names, 8);
+  const size_t E = (size_t)numEdges;
+  rs.add(R_out, (size_t)numImages * 9 * sizeof(double), 0, 0, true);
+  if (residuals) rs.add(residuals, E * sizeof(double), 1, 0, true);
+  if (inlier) rs.add(inlier, E, 2, 0, true);
+  rs.add(cost_out, 2 * sizeof(double), 3, 0, true);
+  if (trace_out) rs.add(trace_out, (size_t)maxIterations * 3 * sizeof(double), 4, 0, true);
+  if (numEdges > 0) {
+    rs.add(edges, E * 2 * sizeof(int), 5, 0, false);
+    rs.add(Rrel, E * 9 * sizeof(double), 6, 0, false);
+    rs.add(weights, E * sizeof(double), 7, 0, false);
+  }
+  int r = rs.check(fn);
+  if (r < 0) return r;
+  for (int e = 0; e < numEdges; e++) {
+    const int i = edges[2 * e], j = edges[2 * e + 1];
+    if (i < 0 || i >= numImages || j < 0 || j >= numImages)
+      return arg_error(fn, "edges[%d] = {%d, %d}: an image index outside [0, numImages)", e, i, j);
+    if (i == j) return arg_error(fn, "edges[%d] joins image %d to itself", e, i);
+    const double *R = Rrel + 9 * (size_t)e;
+    bool ok = true;
+    for (int k = 0; k < 9; k++) ok = ok && std::isfinite(R[k]);
+    for (int a = 0; a < 3 && ok; a++)
+      for (int b = 0; b < 3; b++) {
+        const double d = R[a] * R[b] + R[3 + a] * R[3 + b] + R[6 + a] * R[6 + b];
+        ok = ok && std::fabs(d - (a == b ? 1.0 : 0.0)) <= 1e-6;
+      }
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
+                       R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (!ok || !(std::fabs(det - 1.0) <= 1e-6))
+      return arg_error(fn, "Rrel[%d] must be a finite rotation (R^T R = I and det R = 1, within 1e-6)", e);
+    if (!std::isfinite(weights[e]) || !(weights[e] > 0.0)) return arg_error(fn, "weights[%d] must be finite and > 0", e);
+  }
+  return 0;
+}
+
+// The images of cs_global_positioning (sets, Ks; Rs[a] a rotation, or all nine entries NaN: not positioned), the
+// parameters, then two sweeps: the device ranges (d_points written; d_offsets, d_members, d_use and the records read)
+// and the host ranges (t_out, cost_out, trace_out written; Ks and Rs read).
+int globalpos_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                   const int *offsets, int numTracks, const int *members, int numMembers, const unsigned char *use,
+                   int refImage, int loss, double lossScale, int maxIterations, int maxLinearIterations,
+                   double linearTol, const double *t_out, const double *points, const double *cost_out,
+                   const double *trace_out)
+{
+  if (numImages < 1 || numImages > (1 << 24)) return arg_error(fn, "numImages must be in [1, 2^24]");
+  if (numTracks < 0) return arg_error(fn, "numTracks must be >= 0");
+  if (numMembers < 0) return arg_error(fn, "numMembers must be >= 0");
+  if (!sets || !Ks || !Rs) return arg_error(fn, "sets, Ks and Rs must not be NULL");
+  if (refImage < 0 || refImage >= numImages) return arg_error(fn, "refImage must be in [0, numImages)");
+  if (loss < 0 || loss > 2) return arg_error(fn, "loss must be 0 (trivial), 1 (soft-L1) or 2 (Cauchy)");
+  if (!std::isfinite(lossScale) || !(lossScale > 0.0)) return arg_error(fn, "lossScale must be finite and > 0");
+  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
+  if (maxLinearIterations < 1 || maxLinearIterations > 10000)
+    return arg_error(fn, "maxLinearIterations must be in [1, 10000]");
+  if (!(linearTol > 0.0) || !(linearTol < 1.0)) return arg_error(fn, "linearTol must be in (0, 1)");
+  if (!t_out || !cost_out) return arg_error(fn, "t_out and cost_out must not be NULL");
+  if (numTracks > 0 && (!offsets || !points)) return arg_error(fn, "numTracks > 0 needs d_offsets and d_points");
+  if (numMembers > 0 && !members) return arg_error(fn, "numMembers > 0 needs d_members");
+  if (misaligned(offsets, 4)) return arg_error(fn, "d_offsets must be 4-byte aligned");
+  if (misaligned(members, 8) || misaligned(points, 8))
+    return arg_error(fn, "d_members and d_points must be 8-byte aligned");
+  int r = check_set_table(fn, sets, numImages);
+  if (r < 0) return r;
+  for (int a = 0; a < numImages; a++) {
+    char name[32];
+    snprintf(name, sizeof name, "Ks[%d]", a);
+    if ((r = check_intrinsics(fn, Ks + 9 * (size_t)a, name)) < 0) return r;
+    const double *R = Rs + 9 * (size_t)a;
+    bool nan = true, ok = true;
+    for (int k = 0; k < 9; k++) { nan = nan && std::isnan(R[k]); ok = ok && std::isfinite(R[k]); }
+    if (nan) continue;
+    for (int i = 0; i < 3 && ok; i++)
+      for (int j = 0; j < 3; j++) {
+        const double d = R[3 * i] * R[3 * j] + R[3 * i + 1] * R[3 * j + 1] + R[3 * i + 2] * R[3 * j + 2];
+        ok = ok && std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-6;
+      }
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
+                       R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (!ok || !(det > 0.0))
+      return arg_error(fn, "Rs[%d] must be a rotation (R R^T = I within 1e-6, det R > 0) or all NaN", a);
+  }
+  static const char *const dnames[5] = {"d_points", "d_offsets", "d_members", "d_use", "sets[%d].pts"};
+  ArgRanges rs(dnames, (size_t)numImages + 4);
+  if (numTracks > 0) {
+    rs.add(points, (size_t)numTracks * 3 * sizeof(double), 0, 0, true);
+    rs.add(offsets, ((size_t)numTracks + 1) * sizeof(int), 1, 0, false);
+  }
+  rs.add(members, (size_t)numMembers * sizeof(int2), 2, 0, false);
+  if (use) rs.add(use, (size_t)numMembers, 3, 0, false);
+  for (int a = 0; a < numImages; a++) rs.add(sets[a].pts, record_bytes(sets[a].n), 4, a, false);
+  if ((r = rs.check(fn)) < 0) return r;
+  static const char *const hnames[5] = {"t_out", "cost_out", "trace_out", "Ks", "Rs"};
+  ArgRanges hs(hnames, 5);
+  hs.add(t_out, (size_t)numImages * 3 * sizeof(double), 0, 0, true);
+  hs.add(cost_out, 2 * sizeof(double), 1, 0, true);
+  if (trace_out) hs.add(trace_out, (size_t)maxIterations * 4 * sizeof(double), 2, 0, true);
+  hs.add(Ks, (size_t)numImages * 9 * sizeof(double), 3, 0, false);
+  hs.add(Rs, (size_t)numImages * 9 * sizeof(double), 4, 0, false);
+  return hs.check(fn);
+}
+
 // The set table of the vocabulary calls and the feature total *M (at most INT_MAX).
 static int vocab_sets(const char *fn, const cs_match_set *sets, int numSets, int numWords, int *M)
 {

@@ -59,6 +59,17 @@ int bundle_intrinsics_args(const char *fn, int numImages, const double *Ks, cons
 // cs_undistort_records; *total receives the record total.
 int undistort_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
                    void *const *d_out, long long *total);
+// cs_rotation_averaging: the graph, its relative rotations and weights, the parameters and the host outputs.
+int rotavg_args(const char *fn, int numImages, const int *edges, int numEdges, const double *Rrel,
+                const double *weights, int refImage, int maxIterations, int maxLinearIterations, double linearTol,
+                double sigmaDeg, double maxAngleDeg, const double *R_out, const double *residuals,
+                const unsigned char *inlier, const double *cost_out, const double *trace_out);
+// cs_global_positioning: the images (Rs[a] a rotation or all NaN), the tracks, the parameters and both range sweeps.
+int globalpos_args(const char *fn, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                   const int *offsets, int numTracks, const int *members, int numMembers, const unsigned char *use,
+                   int refImage, int loss, double lossScale, int maxIterations, int maxLinearIterations,
+                   double linearTol, const double *t_out, const double *points, const double *cost_out,
+                   const double *trace_out);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

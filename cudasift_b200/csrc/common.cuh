@@ -373,6 +373,13 @@ struct DeviceCtx {
   // partials, the sort storage
   GrowBuffer bundle;
   PinnedBuffer h_bundle;                   // the result words and the trace (copied back), then the camera table
+  // cs_rotation_averaging: the result words, the trace, the image and edge tables, the final angles, the incidence
+  // sort, the image pieces and partials, the sort storage
+  GrowBuffer rotavg;
+  // cs_global_positioning: the result words, the trace, the camera, point and observation tables, the pieces, the sorts
+  GrowBuffer globalpos;
+  PinnedBuffer h_globalpos;                // the result words and the trace (copied back), then the camera table
+  PinnedBuffer h_rotavg;                   // the same words, tables and incidences on the host (uploaded, copied back)
   // cs_verify_*: the states a call copies back, and its job table
   PinnedBuffer h_verify;
   // cs_vocab_train: the set table and start draws, the assignments, best scores, sort pairs, word bounds, tile
@@ -624,6 +631,33 @@ int bundle_result(const DeviceCtx &c, int nc, int numImages, int maxIterations, 
 // The launch of cs_undistort_records (argument-checked, at least one record) on c.stream, without a synchronize.
 int undistort_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
                       void *const *d_out);
+
+// ---- rotation averaging (rotavg.cu) -------------------------------------------------------------------------------
+// The host part of cs_rotation_averaging (argument-checked, numEdges > 0): the spanning tree, the start rotations and
+// the image, edge and incidence tables in c.h_rotavg.
+int rotavg_prepare(DeviceCtx &c, int numImages, const int *edges, int numEdges, const double *Rrel,
+                   const double *weights, int refImage, int maxIterations);
+// After rotavg_prepare: the sort and the cooperative launch on c.stream, without a synchronize; the results reach
+// c.h_rotavg by the caller's synchronize, and rotavg_result reads them.
+int rotavg_enqueue(DeviceCtx &c, int numImages, int numEdges, int maxIterations, int maxLinearIterations,
+                   double linearTol, double sigmaDeg);
+// after the synchronize: R_out, the residual angles and inlier bytes (either may be NULL), the costs, the trace (may be
+// NULL) and the statistics (may be NULL); returns the IRLS iterations run
+int rotavg_result(const DeviceCtx &c, int numImages, int numEdges, int maxIterations, double maxAngleDeg,
+                  double *R_out, double *residuals, unsigned char *inlier, double cost[2], double *trace,
+                  long long stats[6]);
+
+// ---- global positioning (globalpos.cu) -------------------------------------------------------------------------------
+// The launches of cs_global_positioning (argument-checked, numTracks > 0) on c.stream, without a synchronize; the results
+// reach c.h_globalpos by the caller's synchronize, and globalpos_result reads them.
+int globalpos_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                      const int *offsets, int numTracks, const int *members, int numMembers, const unsigned char *use,
+                      int refImage, unsigned long long seed, int loss, double lossScale, int maxIterations,
+                      int maxLinearIterations, double linearTol, double *points);
+// after the synchronize: t_out, the costs, the trace (may be NULL) and the statistics (may be NULL); returns the
+// accepted steps
+int globalpos_result(const DeviceCtx &c, int numImages, const double *Rs, int maxIterations, double *t_out,
+                     double cost[2], double *trace, long long stats[8]);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

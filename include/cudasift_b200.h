@@ -821,6 +821,123 @@ int cs_bundle_adjust_intrinsics(const cs_match_set *sets, int numImages, const d
 int cs_undistort_records(const cs_match_set *sets, int numImages, const double *Ks, const double *dists,
                          void *const *d_out, double *ms);
 
+/* Rotation averaging (Chatterjee and Govindu, ICCV 2013 / TPAMI 2018; the first stage of global structure from
+ * motion, as in Theia, OpenMVG and GLOMAP): every image's absolute rotation from the relative rotations of the verified
+ * image pairs, in one call.  The inputs are host arrays laid out as cs_verify_essential_batch returns them.
+ * - Graph: edge e joins images i = edges[2e] and j = edges[2e + 1] with the relative rotation Q_e = Rrel[e] (row-major,
+ *   X_j = Q_e X_i + t, so R_j ~ Q_e R_i) and a weight w0_e = weights[e] > 0 (for example the inlier count).  R maps
+ *   world to camera coordinates, as everywhere in this API.
+ * - Start (on the host): a maximum spanning tree by weight, Kruskal's algorithm over the edges sorted by weight
+ *   descending, ties to the lower edge index.  R_ref = I for refImage; then a breadth-first walk from refImage, each
+ *   image's tree edges in ascending edge index, gives an unvisited neighbour R_j = Q_e R_i (from i) or R_i = Q_e^T R_j
+ *   (from j).  The images the walk visits are reached; the others get NaN rotations.  An edge is active when its images
+ *   are reached (both are, or neither).
+ * - Residual of an active edge: D_e = R_j^T Q_e R_i (the discrepancy in the world frame) and rho_e = log D_e, the
+ *   rotation vector: c = (tr D - 1) / 2, v the axial vector of (D - D^T) / 2, s = |v|, theta_e = atan2(s, c); for
+ *   c > 0 rho = v theta / s (v when s = 0), else rho = theta a, a the unit axis from (D + D^T) / 2 = c I + (1 - c) a a^T
+ *   through its largest diagonal entry (the first on ties) and signed so that a.v >= 0.
+ * - Loss: sigma = sigmaDeg pi / 180 radians; with sigmaDeg = 0 the squared loss, cost_e = w0_e theta_e^2 and IRLS weight
+ *   w_e = w0_e; else Geman-McClure, q = sigma^2 / (theta_e^2 + sigma^2), cost_e = w0_e theta_e^2 q and w_e = w0_e q^2
+ *   (rho'(theta) / (2 theta)).  The cost is the sum over the active edges.
+ * - Linearisation: a free image's tangent x_i is in the world frame and moves it by R_i <- R_i exp([x_i]x), computed as
+ *   the left update exp([R_i x_i]x) R_i (vp_rotate).  Then D_e <- exp(-[x_j]x) D_e exp([x_i]x), and to first order
+ *   rho_e(x) = rho_e + Jr^-1(rho_e) x_i - Jl^-1(rho_e) x_j (the right and left Jacobians of SO(3)).  Since
+ *   Jr^-T(rho) rho = Jl^-T(rho) rho = rho, the cost's gradient is exactly that of the linear model rho_e + x_i - x_j:
+ *   the model has the exact first-order cost, and its Hessian, the weighted graph Laplacian (x) I3, differs from
+ *   Gauss-Newton's by O(|rho|).  Each iteration minimises sum_e w_e |rho_e + x_i - x_j|^2 over the free images (reached,
+ *   not refImage; x_ref = 0): L x = b with (L x)_a = sum over a's active edges of w_e (x_a - x_other) and
+ *   b_a = sum over a's edges of +w_e rho_e (a = j) or -w_e rho_e (a = i).
+ * - Solve: Jacobi-preconditioned CG from x = 0, z = r / diag(L), as cs_bundle_adjust's CG (p = z + beta p,
+ *   alpha = r.z / p.L p, beta = r.z(new) / r.z(old)); it stops before an iteration when r.r <= linearTol^2 b.b, after
+ *   maxLinearIterations iterations, or when p.L p is not > 0.  Every free image then takes its update.
+ * - Loop: the iteration above (weights and residuals at the current rotations), at most maxIterations times; it stops
+ *   after an iteration whose largest |x_a| is <= 1e-12.  maxIterations = 0 evaluates the start only.
+ * - Outputs: R_out [numImages][9] (NaN for an image not reached).  residuals_out [numEdges] (may be NULL): theta_e in
+ *   degrees under the final rotations, NaN for an inactive edge; inlier_out [numEdges] (may be NULL): 1 when that angle
+ *   is < maxAngleDeg (the filter for positioning and guided matching).  cost_out = {at the start, final}.  trace_out
+ *   (may be NULL) [maxIterations][3]: per iteration {the cost at its start, CG iterations, largest |x_a|}; rows past
+ *   the last iteration are 0.  stats_out (may be NULL): [0] active edges, [1] tree edges used (images reached - 1),
+ *   [2] images reached, [3] iterations, [4] CG iterations in all, [5] inlier edges.  ms_out (may be NULL): {the host's
+ *   spanning tree and tables, the device part (event time)} in milliseconds.  Returns the iterations run, or CS_E_*.
+ * - Determinism: every sum has a fixed order that depends on the data only and no floating-point atomics are used, so
+ *   two calls give the same bytes.  Per image: its incidences (image, 2 e + side) sorted by image (a stable radix sort,
+ *   so in edge order), cut at multiples of 256 of that list, a piece summed by a warp (lane l takes l, l + 32, ...,
+ *   then an xor butterfly) and the pieces in ascending order.  Totals over edges (the cost): tiles of 256 edges (warp
+ *   butterflies, then the 8 warps in order); over images (the CG dot products): tiles of 32 images (a butterfly); the
+ *   tile partials lane-strided in ascending order, then a butterfly.  The largest step is a max (exact).
+ * - Launches: 1 kernel launch (cs_launch_count) whatever the sizes and iteration counts: one cooperative kernel (a
+ *   resident wave, SMs x occupancy CTAs of 256 threads) runs the whole loop with grid barriers between its phases, after
+ *   a cub sort of the incidences (not counted).  The call synchronises with the host once.  Scratch, in the per-device
+ *   context: 216 bytes per image (its state), 32 per image and per 256 incidences (the pieces), 168 per edge (its state,
+ *   final angle and the four sort arrays), 24 per iteration, plus the sort storage; pinned, the same tables.
+ * - CS_E_ARG, before any CUDA call, naming the argument: numImages outside [1, 2^24], numEdges outside [0, 2^26],
+ *   refImage outside [0, numImages), maxIterations outside [0, 1000], maxLinearIterations outside [1, 10000], linearTol
+ *   not in (0, 1), sigmaDeg not in [0, 180], maxAngleDeg not in (0, 180], NULL edges, Rrel or weights with
+ *   numEdges > 0, NULL R_out or cost_out, edges[e] with an image outside [0, numImages) or joining an image to itself,
+ *   an Rrel[e] that is not finite or not a rotation (|R^T R - I| entries or |det R - 1| above 1e-6), weights[e] not
+ *   finite or not > 0, and an output (R_out, residuals_out, inlier_out, cost_out, trace_out) that overlaps another
+ *   output or an input (one sweep over sorted ranges, before any edge is read).  numEdges == 0 returns 0 with R = I
+ *   for refImage and NaN for every other image, zero costs and trace, stats {0, 0, 1, 0, 0, 0}, and makes no CUDA
+ *   call. */
+int cs_rotation_averaging(int numImages, const int *edges, int numEdges, const double *Rrel, const double *weights,
+                          int refImage, int maxIterations, int maxLinearIterations, double linearTol, double sigmaDeg,
+                          double maxAngleDeg, double *R_out, double *residuals_out, unsigned char *inlier_out,
+                          double cost_out[2], double *trace_out, long long stats_out[6], double ms_out[2]);
+
+/* Global positioning (GLOMAP's BATA residual on points; Zhuang et al., CVPR 2018): every camera centre and track point
+ * at once, from the rotations of cs_rotation_averaging, from random starts, with one robust least-squares problem over
+ * all observations.  It takes cs_bundle_adjust's images and tracks (sets, Ks, d_offsets, d_members, d_use) and returns
+ * the t that cs_triangulate_tracks and cs_bundle_adjust take.
+ * - Images: Rs[a] is a rotation, or all nine entries NaN (cs_rotation_averaging's output for an image it did not
+ *   reach): such an image takes no part.  refImage's centre is held at 0.
+ * - Observations: tracks, malformed tracks and valid members follow cs_bundle_adjust (the tr_member rule).  A member is
+ *   used when it is valid, its image has a rotation, and d_use is NULL or d_use[m] != 0; a track with at least 2 used
+ *   members takes part, and observation o runs over their used members in track order, then member order.
+ * - Residual of observation o (image a, track k): v_o = R_a^T K_a^-1 (x, y, 1) normalised, in float64;
+ *   r_o = v_o - s_o (X_k - c_a).  Unknowns: the centres c_a of the images with a used observation (but refImage), the
+ *   points X_k of the participating tracks, and one scale s_o per observation, kept >= 1e-6 (s <- max(s + ds, 1e-6)).
+ * - Loss on |r_o|^2 as cs_bundle_adjust_intrinsics' (loss 0 trivial, 1 soft-L1, 2 Cauchy, scale c = lossScale, cost
+ *   c^2 rho(|r|^2 / c^2), no 1/2), linearised by its corrector: r and every Jacobian block scaled by sqrt(rho').
+ * - Start: c_a and X_k drawn uniform in [-1, 1)^3: component j of item i of kind q (0 centres, 1 points) is
+ *   2 u - 1, u = (splitmix64(seed + 0x9E3779B97F4A7C15 ((q 2^32 + i) 3 + j)) >> 11) 2^-53; c_ref = 0; every s = 1.
+ *   Two calls with one seed give the same bytes.
+ * - LM: cs_bundle_adjust's rules (H + lambda D, D = diag(H) clamped to [1e-6, 1e32], taken before any elimination;
+ *   lambda from 1e-3, /10 on accept, x10 on reject; accept when the solve succeeded and the cost decreased; stop after
+ *   maxIterations, after an accepted step with previous - new <= 1e-10 previous, or when lambda exceeds 1e16).
+ * - Linear solve: with w2 = rho', d = X - c and h = w2 |d|^2 damped, each s_o is eliminated from its own 7 x 7 block,
+ *   leaving per observation P_o = w2 s^2 (I - w2 d d^T / h) on (X, c) as [P, -P; -P, P] and the right-hand side
+ *   beta_o = w2 s (r - w2 d (d.r) / h) on X (-beta_o on c).  Points: V*_k = sum P_o + lambda clamp(sum w2 s^2) I by
+ *   Cholesky, b_X = sum beta_o.  Cameras: U*_a likewise over a's observations; S = U* - W V*^-1 W^T,
+ *   b~_a = -sum beta_o + sum P_o V*_k^-1 b_X,k.  Block-Jacobi PCG from dc = 0 with 3 x 3 blocks
+ *   U*_a - sum_o P_o V*_k^-1 (sum of P over track k's observations in image a), cs_bundle_adjust's CG and stop rules.
+ *   Then dX_k = V*_k^-1 (b_X,k + sum_o P_o dc_a) and ds_o = w2 (d.r - s d.(dX - dc)) / h.  A pivot not > 0 anywhere
+ *   rejects the step.
+ * - Gauge: the scale is held by the damping during the loop.  After it, c and X are divided by
+ *   scale = sqrt(mean |c_a|^2) over the images with a used observation (refImage's 0 included; summed in tiles of 32
+ *   images, then the tile partials), or 1 when that is not > 0.
+ * - Outputs: t_out [numImages][3] = -R_a c_a / scale, NaN for an image with no used observation or with NaN R.
+ *   d_points [numTracks][3] = X_k / scale, NaN for a track that does not take part.  cost_out = {start, final};
+ *   trace_out (may be NULL) [maxIterations][4] as cs_bundle_adjust's; stats_out (may be NULL): [0] well-formed tracks,
+ *   [1] malformed tracks, [2] invalid members, [3] used observations, [4] tracks positioned, [5] images with a used
+ *   observation, [6] LM iterations, [7] CG iterations.  Returns the accepted steps, or CS_E_*.
+ * - Determinism and launches: cs_bundle_adjust's: 3 kernel launches whatever the sizes (count, fill, one cooperative
+ *   kernel), fixed summation orders (per point its observations in order; per camera tiles of 256 sorted observations
+ *   and pieces in ascending order; totals over tiles of 256 tracks or 32 cameras), no floating-point atomics.  Scratch:
+ *   416 bytes per image (state) plus 152 per image and per 256 members (pieces), 176 per track, 200 per member, 36 per
+ *   LM iteration, plus the cub storage; pinned, 416 bytes per image and 32 per LM iteration.
+ * - CS_E_ARG, before any CUDA call, naming the argument: numImages outside [1, 2^24], numTracks or numMembers < 0, NULL
+ *   sets, Ks or Rs, refImage outside [0, numImages), loss outside 0..2, lossScale not finite or not > 0, maxIterations
+ *   outside [0, 1000], maxLinearIterations outside [1, 10000], linearTol not in (0, 1), NULL t_out or cost_out, NULL
+ *   d_offsets or d_points with tracks, NULL d_members with members, misaligned buffers, a set with records and no
+ *   pointer, an invalid Ks[a] (cs_verify_essential's rule), an Rs[a] neither a rotation nor all NaN, d_points
+ *   overlapping d_offsets, d_members, d_use or any set's records, and t_out, cost_out or trace_out overlapping each
+ *   other, Ks or Rs.  numTracks == 0 returns 0 with NaN t, zero costs, trace and statistics, and makes no CUDA call. */
+int cs_global_positioning(const cs_match_set *sets, int numImages, const double *Ks, const double *Rs,
+                          const int *d_offsets, int numTracks, const int *d_members, int numMembers,
+                          const unsigned char *d_use, int refImage, unsigned long long seed, int loss, double lossScale,
+                          int maxIterations, int maxLinearIterations, double linearTol, double *t_out,
+                          double *d_points, double cost_out[2], double *trace_out, long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
