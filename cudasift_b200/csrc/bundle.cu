@@ -14,16 +14,12 @@
 // distortion coefficient is 0, else 9 (w, delta, f, k1, k2); bundle_kernel also per loss (trivial, or robust with
 // soft-L1 or Cauchy chosen at run time).  Every NC-sized piece below is a template of NC, so the <6, false>
 // instantiation is the kernel of the squared pixel loss with K held.
-// Every floating-point sum has a fixed order that depends on the data only, not on the grid or on scheduling:
-//   - per point: a thread sums its observations in observation order;
-//   - per camera: the sorted observations are cut into tiles of BA_TILE; a warp sums a camera's piece of a tile
-//     lane-strided, then by a fixed xor butterfly, and one lane per camera adds its pieces in ascending tile order;
-//   - totals over points (the cost): a CTA sums a tile of 256 tracks by butterflies and its warps in order; over
-//     cameras (the CG dot products): a warp sums a tile of 32 cameras by a butterfly; the tile partials are then added
-//     by warp 0 of every CTA, lane-strided in ascending order and by a butterfly.
-// No floating-point atomics.  Every branch around a grid barrier (the CG stop, the accept, the LM stop) is taken on
-// values that every CTA computes from the same words, written before the barrier, by the same instructions in the same
-// order, so every CTA takes the same path; every loop is bounded by maxIterations or maxLinearIterations.
+// Every floating-point sum has a fixed order that depends on the data only (coop.cuh): per point, a thread sums its
+// observations in observation order; per camera, the pieces of the sorted observations' tiles; totals over tiles of 256
+// tracks (the cost) or 32 cameras (the CG dot products).  No floating-point atomics.  Every branch around a grid barrier
+// (the CG stop, the accept, the LM stop) is taken on values that every CTA computes from the same words, written before
+// the barrier, by the same instructions in the same order, so every CTA takes the same path; every loop is bounded by
+// maxIterations or maxLinearIterations.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -32,7 +28,7 @@
 #include <math_constants.h>
 
 #include "common.cuh"
-#include "vp_math.cuh"
+#include "coop.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -42,7 +38,6 @@ namespace {
 
 constexpr int BA_THREADS = 256;
 constexpr int BA_WARPS = BA_THREADS / 32;
-constexpr int BA_TILE = 256;         // sorted observations per camera tile
 // Slots per camera tile partial.  p.S p has a slot of its own: CG phase G writes r.r and r.z with no grid barrier after
 // the totals of p.S p are read, so they may not share a slot.
 constexpr int BA_CP = 3;
@@ -134,58 +129,6 @@ struct BaParams {
 
 // ---- small dense helpers (row-major full matrices in registers) ----------------------------------------------------
 
-// Cholesky of the symmetric A (N x N); false when a pivot is not > 0 or not finite.  L is lower, packed row by row.
-template <int N>
-__device__ __forceinline__ bool ba_chol(const double (&A)[N][N], double *L)
-{
-  double F[N][N];
-#pragma unroll
-  for (int j = 0; j < N; j++) {
-    double d = A[j][j];
-#pragma unroll
-    for (int q = 0; q < j; q++) d -= F[j][q] * F[j][q];
-    if (!(d > 0.0) || !isfinite(d)) return false;
-    F[j][j] = sqrt(d);
-#pragma unroll
-    for (int i = j + 1; i < N; i++) {
-      double e = A[i][j];
-#pragma unroll
-      for (int q = 0; q < j; q++) e -= F[i][q] * F[j][q];
-      F[i][j] = e / F[j][j];
-    }
-  }
-  int k = 0;
-#pragma unroll
-  for (int i = 0; i < N; i++)
-#pragma unroll
-    for (int j = 0; j <= i; j++) L[k++] = F[i][j];
-  return true;
-}
-
-// x = A^-1 b from the packed factor of ba_chol (forward, then backward substitution)
-template <int N>
-__device__ __forceinline__ void ba_chol_solve(const double *L, const double (&b)[N], double (&x)[N])
-{
-  double z[N];
-#pragma unroll
-  for (int i = 0; i < N; i++) {
-    double e = b[i];
-#pragma unroll
-    for (int q = 0; q < i; q++) e -= L[i * (i + 1) / 2 + q] * z[q];
-    z[i] = e / L[i * (i + 1) / 2 + i];
-  }
-#pragma unroll
-  for (int i = N - 1; i >= 0; i--) {
-    double e = z[i];
-#pragma unroll
-    for (int q = i + 1; q < N; q++) e -= L[q * (q + 1) / 2 + i] * x[q];
-    x[i] = e / L[i * (i + 1) / 2 + i];
-  }
-}
-
-// the damped diagonal entry d + lambda clamp(d, 1e-6, 1e32)
-__device__ __forceinline__ double ba_damp(double d, double lam) { return d + lam * fmin(fmax(d, 1e-6), 1e32); }
-
 // The free components of a camera with fixed code f: 0 all six, 1 none, 2..4 all but t[f - 2] (bits 0-2 w, 3-5 t).
 __device__ __forceinline__ int ba_free_mask(int f) { return f == 0 ? 0x3f : f == 1 ? 0 : 0x3f & ~(1 << (f + 1)); }
 
@@ -268,19 +211,6 @@ __device__ __forceinline__ double ba_linearise_radial(const double *K, const dou
   return z;
 }
 
-// c^2 rho(s / c^2) of the robust loss (1 soft-L1, 2 Cauchy); *w = sqrt(rho'(s / c^2)), the corrector's scale.
-__device__ __forceinline__ double ba_loss(int loss, double c2, double s, double *w)
-{
-  const double u = s / c2;
-  if (loss == 1) {
-    const double q = sqrt(1.0 + u);
-    if (w) *w = sqrt(1.0 / q);
-    return c2 * (2.0 * u / (q + 1.0));
-  }
-  if (w) *w = sqrt(1.0 / (1.0 + u));
-  return c2 * log1p(u);
-}
-
 // The observation's residual at a camera's current or candidate parameters (J as ba_linearise).
 template <int NC>
 __device__ __forceinline__ double ba_observe(const BaCam<NC> &c, bool cand, const double (&X)[3], float x, float y,
@@ -321,24 +251,9 @@ __device__ __forceinline__ int ba_used(const BaParams<NC> &p, int k, int &invali
 template <int NC>
 __global__ void __launch_bounds__(BA_THREADS) bundle_count_kernel(BaParams<NC> p)
 {
-  const int k = blockIdx.x * BA_THREADS + threadIdx.x;
-  if (k == 0) p.cnt[p.numTracks] = 0;
-  if (k >= p.numTracks) return;
-  int invalid = 0;
-  const int used = ba_used(p, k, invalid, [](int, int, float, float, int) {});
-  unsigned long long *st = p.res->stats;
-  if (used < 0) {
-    atomicAdd(&st[1], 1ull);
-    p.cnt[k] = 0;
-    return;
-  }
-  atomicAdd(&st[0], 1ull);
-  if (invalid) atomicAdd(&st[2], (unsigned long long)invalid);
-  p.cnt[k] = used >= 2 ? used : 0;
-  if (used >= 2) {
-    atomicAdd(&st[3], (unsigned long long)used);
-    atomicAdd(&st[4], 1ull);
-  }
+  co_count(p, blockIdx.x * BA_THREADS + threadIdx.x, [&](int k, int &invalid) {
+    return ba_used(p, k, invalid, [](int, int, float, float, int) {});
+  });
 }
 
 template <int NC>
@@ -363,106 +278,6 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_fill_kernel(BaParams<NC> p)
 }
 
 // ---- the cooperative kernel ---------------------------------------------------------------------------------------
-
-// The K sums of n tile partials (part[tile * stride + j]): warp 0 adds them lane-strided in ascending order, then by a
-// fixed xor butterfly; every thread of the CTA receives them.  Every CTA reads the partials after the barrier that
-// follows their writes, so a slot read here must not be written again before the next grid barrier.
-template <int K>
-__device__ __forceinline__ void ba_totals(const double *part, int n, int stride, double (&out)[K])
-{
-  __shared__ double s_tot[K];
-  if (threadIdx.x < 32) {
-    double v[K];
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] = 0.0;
-    for (int i = (int)threadIdx.x; i < n; i += 32)
-#pragma unroll
-      for (int j = 0; j < K; j++) v[j] += part[(size_t)i * stride + j];
-    vp_warp_sum(v);
-    if (threadIdx.x == 0)
-#pragma unroll
-      for (int j = 0; j < K; j++) s_tot[j] = v[j];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < K; j++) out[j] = s_tot[j];
-  __syncthreads();                                           // s_tot is read before the next call writes it
-}
-
-// A CTA's tile partial of K values (one per thread): warp butterflies, then thread 0 adds the warps in order.
-template <int K>
-__device__ __forceinline__ void ba_cta_partial(double (&v)[K], double *out)
-{
-  __shared__ double s_w[BA_WARPS][K];
-  vp_warp_sum(v);
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int j = 0; j < K; j++) s_w[threadIdx.x >> 5][j] = v[j];
-  __syncthreads();
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int j = 0; j < K; j++) {
-      double s = s_w[0][j];
-      for (int w = 1; w < BA_WARPS; w++) s += s_w[w][j];
-      out[j] = s;
-    }
-  __syncthreads();
-}
-
-// A warp's tile partial of K values (one per lane, a lane per camera): a butterfly, lane 0 writes.
-template <int K>
-__device__ __forceinline__ void ba_warp_partial(double (&v)[K], double *out)
-{
-  vp_warp_sum(v);
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int j = 0; j < K; j++) out[j] = v[j];
-}
-
-// The camera pieces of NV values per observation (f(o, a, v)) at offset OFF: a warp per tile of BA_TILE sorted
-// observations, each camera's piece summed lane-strided and by a butterfly, stored at piece index tile + camera
-// (unique: a camera's tiles follow the previous camera's last one).
-template <int NV, int OFF, int NC, class F>
-__device__ __forceinline__ void ba_pieces(const BaParams<NC> &p, int N, F &&f)
-{
-  constexpr int PV = BaSize<NC>::PV;
-  const int lane = threadIdx.x & 31;
-  const int numWarps = (int)gridDim.x * BA_WARPS, numTiles = (N + BA_TILE - 1) / BA_TILE;
-  for (int t = (int)((blockIdx.x * BA_THREADS + threadIdx.x) >> 5); t < numTiles; t += numWarps) {
-    const int t1 = min(N, (t + 1) * BA_TILE);
-    for (int s = t * BA_TILE; s < t1;) {
-      const int a = p.keysS[s];
-      const int e = min(t1, p.cams[a].end);
-      double acc[NV];
-#pragma unroll
-      for (int j = 0; j < NV; j++) acc[j] = 0.0;
-      for (int i = s + lane; i < e; i += 32) {
-        double v[NV];
-        f(p.order[i], a, v);
-#pragma unroll
-        for (int j = 0; j < NV; j++) acc[j] += v[j];
-      }
-      vp_warp_sum(acc);
-      if (lane == 0)
-#pragma unroll
-        for (int j = 0; j < NV; j++) p.pieces[(size_t)(t + a) * PV + OFF + j] = acc[j];
-      s = e;
-    }
-  }
-}
-
-// The sum of camera c's pieces (NV values at OFF) in ascending tile order.
-template <int NV, int OFF, int NC>
-__device__ __forceinline__ void ba_gather(const BaParams<NC> &p, int a, const BaCam<NC> &c, double (&v)[NV])
-{
-  constexpr int PV = BaSize<NC>::PV;
-#pragma unroll
-  for (int j = 0; j < NV; j++) v[j] = 0.0;
-  if (c.end > c.start)
-    for (int t = c.start / BA_TILE; t <= (c.end - 1) / BA_TILE; t++)
-#pragma unroll
-      for (int j = 0; j < NV; j++) v[j] += p.pieces[(size_t)(t + a) * PV + OFF + j];
-}
 
 // J_c^T (J_p y) of observation o (NC values)
 template <int NC>
@@ -491,24 +306,6 @@ __device__ __forceinline__ void ba_wtx(const double *J, const double *x, double 
 template <int N>
 __device__ __forceinline__ int ba_up(int i, int j) { return i * N - i * (i - 1) / 2 + (j - i); }
 
-// Per participating track (a thread each, tiles of 256 tracks per CTA): f(k, s, e) returns K values for the tile
-// partials at part (or nothing with K == 0).
-template <int K, int NC, class F>
-__device__ __forceinline__ void ba_per_point(const BaParams<NC> &p, double *part, F &&f)
-{
-  for (int base = (int)blockIdx.x * BA_THREADS; base < p.numTracks; base += (int)gridDim.x * BA_THREADS) {
-    const int k = base + (int)threadIdx.x;
-    double v[K > 0 ? K : 1];
-#pragma unroll
-    for (int j = 0; j < (K > 0 ? K : 1); j++) v[j] = 0.0;
-    if (k < p.numTracks) {
-      const int s = p.start[k], e = p.start[k + 1];
-      if (e > s) f(k, s, e, v);
-    }
-    if constexpr (K > 0) ba_cta_partial<K>(v, part + (size_t)(base / BA_THREADS) * K);
-  }
-}
-
 // Linearise every observation of track k at the current parameters (or the candidate ones); returns its cost.  Under a
 // robust loss the observation's r and Jacobian rows are scaled by sqrt(rho'), the cost is c^2 rho(s / c^2).
 template <int NC, bool ROBUST>
@@ -525,8 +322,9 @@ __device__ __forceinline__ double ba_relinearise(const BaParams<NC> &p, int k, i
     double *J = p.J + (size_t)o * JD;
     ba_observe<NC>(c, cand, X, ob.x, ob.y, r, J);
     if constexpr (ROBUST) {
-      double w;
-      cost += ba_loss(p.loss, p.c2, r[0] * r[0] + r[1] * r[1], &w);
+      double w2;
+      cost += vp_loss(p.loss, p.c2, r[0] * r[0] + r[1] * r[1], &w2);
+      const double w = sqrt(w2);
 #pragma unroll
       for (int j = 0; j < JD; j++) J[j] *= w;
     } else {
@@ -539,7 +337,7 @@ __device__ __forceinline__ double ba_relinearise(const BaParams<NC> &p, int k, i
 template <int NC, bool ROBUST>
 __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
 {
-  constexpr int NU = BaSize<NC>::NU, JD = BaSize<NC>::JD, PJ = 2 * NC;   // PJ: J_p's first entry
+  constexpr int NU = BaSize<NC>::NU, JD = BaSize<NC>::JD, PV = BaSize<NC>::PV, PJ = 2 * NC;   // PJ: J_p's first entry
   cg::grid_group grid = cg::this_grid();
   const int tid = (int)(blockIdx.x * BA_THREADS + threadIdx.x), nthreads = (int)gridDim.x * BA_THREADS;
   const int lane = (int)threadIdx.x & 31;
@@ -548,11 +346,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
   const int camTiles = (C + 31) / 32, ptTiles = (p.numTracks + BA_THREADS - 1) / BA_THREADS;
 
   // 0. every camera's sorted range, its free components; the linearisation at the input and its cost
-  for (int i = tid; i < N; i += nthreads) {
-    const int a = p.keysS[i];
-    if (i == 0 || p.keysS[i - 1] != a) p.cams[a].start = i;
-    if (i == N - 1 || p.keysS[i + 1] != a) p.cams[a].end = i + 1;
-  }
+  co_ranges(p.keysS, N, p.cams, tid, nthreads);
   grid.sync();
   for (int a = tid; a < C; a += nthreads) {
     BaCam<NC> &c = p.cams[a];
@@ -562,14 +356,14 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
       c.mask = c.end > c.start ? ba_free_mask(c.fixed) | (c.refine << 6) : 0;
     if (c.mask) atomicAdd(&p.res->stats[5], (unsigned long long)__popc(c.mask));
   }
-  ba_per_point<1>(p, p.ptPart, [&](int k, int s, int e, double *v) {
+  co_per_track<1, BA_THREADS>(p.start, p.numTracks, p.ptPart, [&](int k, int s, int e, double *v) {
     v[0] = ba_relinearise<NC, ROBUST>(p, k, s, e, false);
   });
   grid.sync();
   double cost;
   {
     double t[1];
-    ba_totals<1>(p.ptPart, ptTiles, 1, t);
+    co_totals<1>(p.ptPart, ptTiles, 1, t);
     cost = t[0];
   }
   const double cost0 = cost;
@@ -579,7 +373,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
   for (int it = 0; it < p.maxIterations && N > 0; it++) {
     lmIters++;
     // A. per point: V* (damped) by Cholesky, g_p = J_p^T r, q = V*^-1 g_p
-    ba_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+    co_per_track<0, BA_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
       double V[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}}, g[3] = {0, 0, 0};
       for (int o = s; o < e; o++) {
         const double *J = p.J + (size_t)o * JD;
@@ -596,14 +390,14 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
       }
 #pragma unroll
       for (int i = 0; i < 3; i++) {
-        V[i][i] = ba_damp(V[i][i], lam);
+        V[i][i] += vp_damping(V[i][i], lam);
 #pragma unroll
         for (int j = 0; j < i; j++) V[i][j] = V[j][i];
       }
       BaPt &pt = p.pts[k];
-      if (!ba_chol<3>(V, pt.L)) { atomicOr(&p.flags[it], 1u); return; }
+      if (!vp_chol<3>(V, pt.L)) { atomicOr(&p.flags[it], 1u); return; }
       double q[3];
-      ba_chol_solve<3>(pt.L, g, q);
+      vp_chol_solve<3>(pt.L, g, q);
 #pragma unroll
       for (int i = 0; i < 3; i++) { pt.g[i] = g[i]; pt.q[i] = q[i]; }
     });
@@ -612,7 +406,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
 
     // B. the camera pieces: U, g_c, W q and the Schur term W_o V*^-1 W_ak^T (W_ak: the track's observations in image a)
     if (!fail) {
-      ba_pieces<NU, 0>(p, N, [&](int o, int, double *v) {
+      co_pieces<NU, 0, PV, BA_THREADS>(p.keysS, p.order, p.pieces, N, p.cams, [&](int o, int, double *v) {
         const double *J = p.J + (size_t)o * JD;
         int n = 0;
 #pragma unroll
@@ -620,14 +414,14 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
 #pragma unroll
           for (int j = i; j < NC; j++) v[n++] = J[i] * J[j] + J[NC + i] * J[NC + j];
       });
-      ba_pieces<2 * NC, NU>(p, N, [&](int o, int, double *v) {
+      co_pieces<2 * NC, NU, PV, BA_THREADS>(p.keysS, p.order, p.pieces, N, p.cams, [&](int o, int, double *v) {
         const double *J = p.J + (size_t)o * JD;
         const double *q = p.pts[p.obs[o].k].q;
 #pragma unroll
         for (int i = 0; i < NC; i++) v[i] = J[i] * J[PJ + 6] + J[NC + i] * J[PJ + 7];
         ba_wy<NC>(J, q, v + NC);
       });
-      ba_pieces<NU, NU + 2 * NC>(p, N, [&](int o, int a, double *v) {
+      co_pieces<NU, NU + 2 * NC, PV, BA_THREADS>(p.keysS, p.order, p.pieces, N, p.cams, [&](int o, int a, double *v) {
         const double *J = p.J + (size_t)o * JD;
         const int k = p.obs[o].k;
         double Wo[NC][3], Wa[NC][3], Y[NC][3];
@@ -648,7 +442,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
         }
         const double *L = p.pts[k].L;
 #pragma unroll
-        for (int i = 0; i < NC; i++) ba_chol_solve<3>(L, Wa[i], Y[i]);
+        for (int i = 0; i < NC; i++) vp_chol_solve<3>(L, Wa[i], Y[i]);
         int n = 0;
 #pragma unroll
         for (int i = 0; i < NC; i++)
@@ -667,9 +461,9 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
         if (a < C) {
           BaCam<NC> &c = p.cams[a];
           double U[NU], G[2 * NC], T[NU];
-          ba_gather<NU, 0>(p, a, c, U);
-          ba_gather<2 * NC, NU>(p, a, c, G);
-          ba_gather<NU, NU + 2 * NC>(p, a, c, T);
+          co_gather<NU, 0, PV>(p.pieces, a, c, U);
+          co_gather<2 * NC, NU, PV>(p.pieces, a, c, G);
+          co_gather<NU, NU + 2 * NC, PV>(p.pieces, a, c, T);
           double Us[NC][NC], M[NC][NC];
 #pragma unroll
           for (int i = 0; i < NC; i++)
@@ -677,7 +471,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
             for (int j = i; j < NC; j++) {
               const bool fr = ((c.mask >> i) & 1) && ((c.mask >> j) & 1);
               double u = U[ba_up<NC>(i, j)];
-              if (i == j) u = ba_damp(u, lam);
+              if (i == j) u += vp_damping(u, lam);
               Us[i][j] = Us[j][i] = fr ? u : (i == j ? 1.0 : 0.0);
               M[i][j] = M[j][i] = fr ? u - T[ba_up<NC>(i, j)] : (i == j ? 1.0 : 0.0);
             }
@@ -685,13 +479,13 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
           for (int i = 0; i < NC; i++)
 #pragma unroll
             for (int j = i; j < NC; j++) c.U[ba_up<NC>(i, j)] = Us[i][j];
-          if (!ba_chol<NC>(M, c.L)) {
+          if (!vp_chol<NC>(M, c.L)) {
             atomicOr(&p.flags[it], 1u);
           } else {
             double r[NC], z[NC];
 #pragma unroll
             for (int i = 0; i < NC; i++) r[i] = ((c.mask >> i) & 1) ? -G[i] + G[NC + i] : 0.0;
-            ba_chol_solve<NC>(c.L, r, z);
+            vp_chol_solve<NC>(c.L, r, z);
 #pragma unroll
             for (int i = 0; i < NC; i++) {
               c.x[i] = 0.0; c.r[i] = r[i]; c.z[i] = z[i]; c.p[i] = 0.0;
@@ -700,7 +494,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
             }
           }
         }
-        ba_warp_partial<2>(d, p.camPart + BA_CP * (size_t)w);
+        co_warp_partial<2>(d, p.camPart + BA_CP * (size_t)w);
       }
     grid.sync();
     fail = *(volatile unsigned int *)&p.flags[it];
@@ -709,12 +503,12 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
     int cgIt = 0;
     if (!fail) {
       double t2[2];
-      ba_totals<2>(p.camPart, camTiles, BA_CP, t2);
+      co_totals<2>(p.camPart, camTiles, BA_CP, t2);
       const double thr = p.tol2 * t2[0];
       double rr = t2[0], rz = t2[1], beta = 0.0;
       while (cgIt < p.maxLinear && !(rr <= thr)) {
         // D. per point: y = V*^-1 W^T p, with p = z + beta p_old of each camera
-        ba_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+        co_per_track<0, BA_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
           double h[3] = {0.0, 0.0, 0.0};
           for (int o = s; o < e; o++) {
             const BaCam<NC> &c = p.cams[p.obs[o].a];
@@ -725,13 +519,13 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
           }
           BaPt &pt = p.pts[k];
           double y[3];
-          ba_chol_solve<3>(pt.L, h, y);
+          vp_chol_solve<3>(pt.L, h, y);
 #pragma unroll
           for (int i = 0; i < 3; i++) pt.y[i] = y[i];
         });
         grid.sync();
         // E. the camera pieces of W y
-        ba_pieces<NC, 0>(p, N, [&](int o, int, double *v) {
+        co_pieces<NC, 0, PV, BA_THREADS>(p.keysS, p.order, p.pieces, N, p.cams, [&](int o, int, double *v) {
           ba_wy<NC>(p.J + (size_t)o * JD, p.pts[p.obs[o].k].y, v);
         });
         grid.sync();
@@ -742,7 +536,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
           if (a < C) {
             BaCam<NC> &c = p.cams[a];
             double Wy[NC], pn[NC];
-            ba_gather<NC, 0>(p, a, c, Wy);
+            co_gather<NC, 0, PV>(p.pieces, a, c, Wy);
 #pragma unroll
             for (int i = 0; i < NC; i++) pn[i] = fma(beta, c.p[i], c.z[i]);
 #pragma unroll
@@ -756,11 +550,11 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
               d[0] += pn[i] * q;
             }
           }
-          ba_warp_partial<1>(d, p.camPart + BA_CP * (size_t)w + 2);
+          co_warp_partial<1>(d, p.camPart + BA_CP * (size_t)w + 2);
         }
         grid.sync();
         double pq[1];
-        ba_totals<1>(p.camPart + 2, camTiles, BA_CP, pq);
+        co_totals<1>(p.camPart + 2, camTiles, BA_CP, pq);
         if (!(pq[0] > 0.0)) break;
         const double alpha = rz / pq[0];
         // G. per camera: x += alpha p, r -= alpha q, z = M^-1 r; the partials of r.r and r.z
@@ -776,7 +570,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
               r[i] = fma(-alpha, c.q[i], c.r[i]);
               c.r[i] = r[i];
             }
-            ba_chol_solve<NC>(c.L, r, z);
+            vp_chol_solve<NC>(c.L, r, z);
 #pragma unroll
             for (int i = 0; i < NC; i++) {
               c.z[i] = z[i];
@@ -784,11 +578,11 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
               d[1] += r[i] * z[i];
             }
           }
-          ba_warp_partial<2>(d, p.camPart + BA_CP * (size_t)w);
+          co_warp_partial<2>(d, p.camPart + BA_CP * (size_t)w);
         }
         cgIt++;
         grid.sync();
-        ba_totals<2>(p.camPart, camTiles, BA_CP, t2);
+        co_totals<2>(p.camPart, camTiles, BA_CP, t2);
         rr = t2[0];
         beta = t2[1] / rz;
         rz = t2[1];
@@ -800,13 +594,13 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
     double cand[2] = {CUDART_NAN, 0.0};
     bool badFocal = false;
     if (!fail) {
-      ba_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+      co_per_track<0, BA_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
         BaPt &pt = p.pts[k];
         double h[3] = {0.0, 0.0, 0.0}, dp[3];
         for (int o = s; o < e; o++) ba_wtx<NC>(p.J + (size_t)o * JD, p.cams[p.obs[o].a].x, h);
 #pragma unroll
         for (int i = 0; i < 3; i++) h[i] = -pt.g[i] - h[i];
-        ba_chol_solve<3>(pt.L, h, dp);
+        vp_chol_solve<3>(pt.L, h, dp);
 #pragma unroll
         for (int i = 0; i < 3; i++) pt.Xc[i] = pt.X[i] + dp[i];
       });
@@ -841,7 +635,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
       grid.sync();
       if constexpr (NC == 9) badFocal = (*(volatile unsigned int *)&p.flags[it] & 2u) != 0;
       // I. the candidate's cost and its observations behind a camera
-      ba_per_point<2>(p, p.ptPart, [&](int k, int s, int e, double *v) {
+      co_per_track<2, BA_THREADS>(p.start, p.numTracks, p.ptPart, [&](int k, int s, int e, double *v) {
         const BaPt &pt = p.pts[k];
         const double X[3] = {pt.Xc[0], pt.Xc[1], pt.Xc[2]};
         for (int o = s; o < e; o++) {
@@ -850,14 +644,14 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
           double r[2];
           const double z = ba_observe<NC>(c, true, X, ob.x, ob.y, r, nullptr);
           if constexpr (ROBUST)
-            v[0] += ba_loss(p.loss, p.c2, r[0] * r[0] + r[1] * r[1], nullptr);
+            v[0] += vp_loss(p.loss, p.c2, r[0] * r[0] + r[1] * r[1], nullptr);
           else
             v[0] += r[0] * r[0] + r[1] * r[1];
           if (!(z > 0.0)) v[1] += 1.0;
         }
       });
       grid.sync();
-      ba_totals<2>(p.ptPart, ptTiles, 2, cand);
+      co_totals<2>(p.ptPart, ptTiles, 2, cand);
     }
 
     // J. accept or reject
@@ -887,7 +681,7 @@ __global__ void __launch_bounds__(BA_THREADS) bundle_kernel(BaParams<NC> p)
           c.k[1] = c.kc[1];
         }
       }
-      ba_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+      co_per_track<0, BA_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
         ba_relinearise<NC, ROBUST>(p, k, s, e, true);
         BaPt &pt = p.pts[k];
 #pragma unroll
@@ -1019,20 +813,6 @@ __global__ void __launch_bounds__(UD_THREADS) undistort_kernel(const UdImage *im
   dst->ypos = yo;
 }
 
-// One resident wave of the cooperative kernel; CS_E_CUDA without cooperative launch.
-template <int NC, bool ROBUST>
-int bundle_grid()
-{
-  int dev = 0, coop = 0;
-  CS_CUDA(cudaGetDevice(&dev));
-  CS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) {
-    set_error("cs_bundle_adjust: device %d does not support cooperative launches", dev);
-    return CS_E_CUDA;
-  }
-  return resident_grid<bundle_kernel<NC, ROBUST>, BA_THREADS>();
-}
-
 // The pinned layout: the result words, the trace, then the camera table of NC; returns the table's offset.
 template <int NC>
 size_t bundle_host_layout(int numImages, int maxIterations, size_t *bytes)
@@ -1054,9 +834,8 @@ int bundle_run(DeviceCtx &c, const cs_match_set *sets, int numImages, const doub
 {
   constexpr int JD = BaSize<NC>::JD, PV = BaSize<NC>::PV;
   const int M = numMembers, T = numTracks, C = numImages;
-  const int tiles = (M + BA_TILE - 1) / BA_TILE;
-  int bits = 1;
-  while (bits < 31 && (1ll << bits) <= (long long)C) bits++;        // every key, the sentinel C included, is < 2^bits
+  const int tiles = idivup(M, CO_TILE);
+  const int bits = radix_bits(C);                                  // every key, the sentinel C included
   size_t scanBytes = 0, sortBytes = 0;
   CS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scanBytes, (int *)nullptr, (int *)nullptr, T + 1, c.stream));
   CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sortBytes, (int *)nullptr, (int *)nullptr, (int *)nullptr,
@@ -1133,7 +912,7 @@ int bundle_run(DeviceCtx &c, const cs_match_set *sets, int numImages, const doub
   prm.loss = loss;
   prm.c2 = lossScale * lossScale;
 
-  const int wave = bundle_grid<NC, ROBUST>();
+  const int wave = coop_grid<bundle_kernel<NC, ROBUST>, BA_THREADS>("cs_bundle_adjust");
   if (wave < 0) return wave;
   const cudaStream_t st = c.stream;
   CS_CUDA(cudaMemsetAsync(base, 0, zeroEnd, st));

@@ -69,6 +69,29 @@ int resident_grid()
   return gridOf[dev];
 }
 
+// resident_grid for a cooperative kernel, after the check that the device supports cooperative launches: CS_E_CUDA,
+// with call's name in the message, when it does not.
+template <auto Kernel, int Threads>
+int coop_grid(const char *call)
+{
+  int dev = 0, coop = 0;
+  CS_CUDA(cudaGetDevice(&dev));
+  CS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  if (!coop) {
+    set_error("%s: device %d does not support cooperative launches", call, dev);
+    return CS_E_CUDA;
+  }
+  return resident_grid<Kernel, Threads>();
+}
+
+// The key bits of a radix sort whose keys are at most maxKey: the smallest bits (1 to 31) with maxKey < 2^bits.
+inline int radix_bits(long long maxKey)
+{
+  int bits = 1;
+  while (bits < 31 && (1ll << bits) <= maxKey) bits++;
+  return bits;
+}
+
 // ---- filter taps (host) ----------------------------------------------------------
 void scaledown_taps(float variance, float k[5]);                  // cudaSiftH.cu:315-324
 void lowpass_taps(float sigma, float k[9]);                       // cudaSiftH.cu:408-419

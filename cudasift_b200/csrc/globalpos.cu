@@ -10,10 +10,9 @@
 //   3. (cub stable radix sort of (image, observation)) gp_kernel: one cooperative launch runs the whole LM loop
 // The camera block is 3 wide and the per-observation scale is eliminated inside its own 7 x 7 block, so this is a
 // kernel of its own rather than an instantiation of bundle_kernel.  Every floating-point sum has a fixed order that
-// depends on the data only: per point, a thread over its observations in order; per camera, tiles of GP_TILE sorted
-// observations, a warp per tile (lane-strided, then a butterfly) and the pieces in ascending tile order; totals over
-// tiles of 256 tracks or 32 cameras, the tile partials lane-strided by warp 0 and a butterfly.  No floating-point
-// atomics; every branch around a grid barrier is taken on values every CTA computes from the same words.
+// depends on the data only (coop.cuh): per point, a thread over its observations in order; per camera, the pieces of the
+// sorted observations' tiles; totals over tiles of 256 tracks or 32 cameras.  No floating-point atomics; every branch
+// around a grid barrier is taken on values every CTA computes from the same words.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -22,7 +21,7 @@
 #include <math_constants.h>
 
 #include "common.cuh"
-#include "vp_math.cuh"
+#include "coop.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -31,8 +30,6 @@ namespace cs {
 namespace {
 
 constexpr int GP_THREADS = 256;
-constexpr int GP_WARPS = GP_THREADS / 32;
-constexpr int GP_TILE = 256;         // sorted observations per camera tile
 constexpr int GP_PV = 19;            // a camera piece: sum P (6), sum w^2 s^2, sum beta (3), sum P q (3), Schur term (6)
 constexpr int GP_CP = 3;             // camera tile partial slots: r.r (b~.b~), r.z, p.S p
 constexpr double GP_SMIN = 1e-6;     // the lower bound of every scale s
@@ -97,27 +94,11 @@ struct GpParams {
 
 // ---- small helpers ----------------------------------------------------------------------------------------------
 
-// Cholesky of a symmetric 3 x 3 (packed upper, row by row) into L (lower, row by row); false on a pivot not > 0.
-__device__ __forceinline__ bool gp_chol(const double *A, double *L)
+// a packed symmetric 3 x 3 (upper, row by row) as a full matrix
+__device__ __forceinline__ void gp_full(const double *A, double (&F)[3][3])
 {
-  const double a00 = A[0], a01 = A[1], a02 = A[2], a11 = A[3], a12 = A[4], a22 = A[5];
-  if (!(a00 > 0.0) || !isfinite(a00)) return false;
-  const double l00 = sqrt(a00), l10 = a01 / l00, l20 = a02 / l00;
-  const double d1 = a11 - l10 * l10;
-  if (!(d1 > 0.0) || !isfinite(d1)) return false;
-  const double l11 = sqrt(d1), l21 = (a12 - l20 * l10) / l11;
-  const double d2 = a22 - l20 * l20 - l21 * l21;
-  if (!(d2 > 0.0) || !isfinite(d2)) return false;
-  L[0] = l00; L[1] = l10; L[2] = l11; L[3] = l20; L[4] = l21; L[5] = sqrt(d2);
-  return true;
-}
-
-__device__ __forceinline__ void gp_solve(const double *L, const double *b, double *x)
-{
-  const double z0 = b[0] / L[0], z1 = (b[1] - L[1] * z0) / L[2], z2 = (b[2] - L[3] * z0 - L[4] * z1) / L[5];
-  x[2] = z2 / L[5];
-  x[1] = (z1 - L[4] * x[2]) / L[2];
-  x[0] = (z0 - L[1] * x[1] - L[3] * x[2]) / L[0];
+  F[0][0] = A[0]; F[0][1] = F[1][0] = A[1]; F[0][2] = F[2][0] = A[2];
+  F[1][1] = A[3]; F[1][2] = F[2][1] = A[4]; F[2][2] = A[5];
 }
 
 // y = A x for a packed symmetric 3 x 3 A
@@ -126,25 +107,6 @@ __device__ __forceinline__ void gp_symv(const double *A, const double *x, double
   y[0] = A[0] * x[0] + A[1] * x[1] + A[2] * x[2];
   y[1] = A[1] * x[0] + A[3] * x[1] + A[4] * x[2];
   y[2] = A[2] * x[0] + A[4] * x[1] + A[5] * x[2];
-}
-
-__device__ __forceinline__ double gp_damp(double d, double lam) { return d + lam * fmin(fmax(d, 1e-6), 1e32); }
-
-// c^2 rho(s / c^2) (0 trivial, 1 soft-L1, 2 Cauchy) and *w2 = rho'(s / c^2): cs_bundle_adjust_intrinsics' loss.
-__device__ __forceinline__ double gp_loss(int loss, double c2, double s, double *w2)
-{
-  if (loss == 0) {
-    if (w2) *w2 = 1.0;
-    return s;
-  }
-  const double u = s / c2;
-  if (loss == 1) {
-    const double q = sqrt(1.0 + u);
-    if (w2) *w2 = 1.0 / q;
-    return c2 * (2.0 * u / (q + 1.0));
-  }
-  if (w2) *w2 = 1.0 / (1.0 + u);
-  return c2 * log1p(u);
 }
 
 // The start draw: component j of item i of kind (0 centres, 1 points), uniform in [-1, 1).
@@ -176,24 +138,9 @@ __device__ __forceinline__ int gp_used(const GpParams &p, int k, int &invalid, F
 
 __global__ void __launch_bounds__(GP_THREADS) gp_count_kernel(GpParams p)
 {
-  const int k = blockIdx.x * GP_THREADS + threadIdx.x;
-  if (k == 0) p.cnt[p.numTracks] = 0;
-  if (k >= p.numTracks) return;
-  int invalid = 0;
-  const int used = gp_used(p, k, invalid, [](int, int, float, float, int) {});
-  unsigned long long *st = p.res->stats;
-  if (used < 0) {
-    atomicAdd(&st[1], 1ull);
-    p.cnt[k] = 0;
-    return;
-  }
-  atomicAdd(&st[0], 1ull);
-  if (invalid) atomicAdd(&st[2], (unsigned long long)invalid);
-  p.cnt[k] = used >= 2 ? used : 0;
-  if (used >= 2) {
-    atomicAdd(&st[3], (unsigned long long)used);
-    atomicAdd(&st[4], 1ull);
-  }
+  co_count(p, blockIdx.x * GP_THREADS + threadIdx.x, [&](int k, int &invalid) {
+    return gp_used(p, k, invalid, [](int, int, float, float, int) {});
+  });
 }
 
 __global__ void __launch_bounds__(GP_THREADS) gp_fill_kernel(GpParams p)
@@ -229,100 +176,6 @@ __global__ void __launch_bounds__(GP_THREADS) gp_fill_kernel(GpParams p)
 
 // ---- the cooperative kernel ---------------------------------------------------------------------------------------
 
-template <int K>
-__device__ __forceinline__ void gp_totals(const double *part, int n, int stride, double (&out)[K])
-{
-  __shared__ double s_tot[K];
-  if (threadIdx.x < 32) {
-    double v[K];
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] = 0.0;
-    for (int i = (int)threadIdx.x; i < n; i += 32)
-#pragma unroll
-      for (int j = 0; j < K; j++) v[j] += part[(size_t)i * stride + j];
-    vp_warp_sum(v);
-    if (threadIdx.x == 0)
-#pragma unroll
-      for (int j = 0; j < K; j++) s_tot[j] = v[j];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < K; j++) out[j] = s_tot[j];
-  __syncthreads();
-}
-
-// Per participating track (a thread each, tiles of 256 tracks per CTA): f(k, s, e, v) gives K values for the partials.
-template <int K, class F>
-__device__ __forceinline__ void gp_per_point(const GpParams &p, double *part, F &&f)
-{
-  __shared__ double s_w[GP_WARPS][K > 0 ? K : 1];
-  for (int base = (int)blockIdx.x * GP_THREADS; base < p.numTracks; base += (int)gridDim.x * GP_THREADS) {
-    const int k = base + (int)threadIdx.x;
-    double v[K > 0 ? K : 1];
-#pragma unroll
-    for (int j = 0; j < (K > 0 ? K : 1); j++) v[j] = 0.0;
-    if (k < p.numTracks) {
-      const int s = p.start[k], e = p.start[k + 1];
-      if (e > s) f(k, s, e, v);
-    }
-    if constexpr (K > 0) {
-      vp_warp_sum(v);
-      if ((threadIdx.x & 31) == 0)
-#pragma unroll
-        for (int j = 0; j < K; j++) s_w[threadIdx.x >> 5][j] = v[j];
-      __syncthreads();
-      if (threadIdx.x == 0)
-#pragma unroll
-        for (int j = 0; j < K; j++) {
-          double t = s_w[0][j];
-          for (int w = 1; w < GP_WARPS; w++) t += s_w[w][j];
-          part[(size_t)(base / GP_THREADS) * K + j] = t;
-        }
-      __syncthreads();
-    }
-  }
-}
-
-// The camera pieces of NV values per observation (f(o, a, v)) at OFF: a warp per tile of sorted observations.
-template <int NV, int OFF, class F>
-__device__ __forceinline__ void gp_pieces(const GpParams &p, int N, F &&f)
-{
-  const int lane = threadIdx.x & 31;
-  const int numWarps = (int)gridDim.x * GP_WARPS, numTiles = (N + GP_TILE - 1) / GP_TILE;
-  for (int t = (int)((blockIdx.x * GP_THREADS + threadIdx.x) >> 5); t < numTiles; t += numWarps) {
-    const int t1 = min(N, (t + 1) * GP_TILE);
-    for (int s = t * GP_TILE; s < t1;) {
-      const int a = p.keysS[s];
-      const int e = min(t1, p.cams[a].end);
-      double acc[NV];
-#pragma unroll
-      for (int j = 0; j < NV; j++) acc[j] = 0.0;
-      for (int i = s + lane; i < e; i += 32) {
-        double v[NV];
-        f(p.order[i], a, v);
-#pragma unroll
-        for (int j = 0; j < NV; j++) acc[j] += v[j];
-      }
-      vp_warp_sum(acc);
-      if (lane == 0)
-#pragma unroll
-        for (int j = 0; j < NV; j++) p.pieces[(size_t)(t + a) * GP_PV + OFF + j] = acc[j];
-      s = e;
-    }
-  }
-}
-
-template <int NV, int OFF>
-__device__ __forceinline__ void gp_gather(const GpParams &p, int a, const GpCam &c, double (&v)[NV])
-{
-#pragma unroll
-  for (int j = 0; j < NV; j++) v[j] = 0.0;
-  if (c.end > c.start)
-    for (int t = c.start / GP_TILE; t <= (c.end - 1) / GP_TILE; t++)
-#pragma unroll
-      for (int j = 0; j < NV; j++) v[j] += p.pieces[(size_t)(t + a) * GP_PV + OFF + j];
-}
-
 // The observations of track k at the current (or candidate) parameters: d, r and rho' stored (unless cand); the cost.
 __device__ __forceinline__ double gp_relinearise(const GpParams &p, int k, int s, int e, bool cand, bool store)
 {
@@ -338,8 +191,9 @@ __device__ __forceinline__ double gp_relinearise(const GpParams &p, int k, int s
       d[q] = (cand ? pt.Xc[q] : pt.X[q]) - (cand ? c.cc[q] : c.c[q]);
       r[q] = ob.v[q] - sc * d[q];
     }
-    double w2;
-    cost += gp_loss(p.loss, p.c2, r[0] * r[0] + r[1] * r[1] + r[2] * r[2], &w2);
+    const double s2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
+    double w2 = 1.0;
+    cost += p.loss ? vp_loss(p.loss, p.c2, s2, &w2) : s2;
     if (store) {
 #pragma unroll
       for (int q = 0; q < 3; q++) { ob.d[q] = d[q]; ob.r[q] = r[q]; }
@@ -358,11 +212,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
   const int camTiles = (C + 31) / 32, ptTiles = (p.numTracks + GP_THREADS - 1) / GP_THREADS;
 
   // 0. every camera's sorted range and its start centre; every point's start; the linearisation and cost at the start
-  for (int i = tid; i < N; i += nthreads) {
-    const int a = p.keysS[i];
-    if (i == 0 || p.keysS[i - 1] != a) p.cams[a].start = i;
-    if (i == N - 1 || p.keysS[i + 1] != a) p.cams[a].end = i + 1;
-  }
+  co_ranges(p.keysS, N, p.cams, tid, nthreads);
   for (int a = tid; a < C; a += nthreads) {
     GpCam &c = p.cams[a];
 #pragma unroll
@@ -377,12 +227,12 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
     c.free = c.end > c.start && a != p.refImage;
     if (c.end > c.start) atomicAdd(&p.res->stats[5], 1ull);
   }
-  gp_per_point<1>(p, p.ptPart, [&](int k, int s, int e, double *v) { v[0] = gp_relinearise(p, k, s, e, false, true); });
+  co_per_track<1, GP_THREADS>(p.start, p.numTracks, p.ptPart, [&](int k, int s, int e, double *v) { v[0] = gp_relinearise(p, k, s, e, false, true); });
   grid.sync();
   double cost;
   {
     double t[1];
-    gp_totals<1>(p.ptPart, ptTiles, 1, t);
+    co_totals<1>(p.ptPart, ptTiles, 1, t);
     cost = t[0];
   }
   const double cost0 = cost;
@@ -392,12 +242,12 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
   for (int it = 0; it < p.maxIterations && N > 0; it++) {
     lmIters++;
     // A. per observation: s eliminated in its 7 x 7 block (h, P, beta); per point: V* by Cholesky, b_X, q = V*^-1 b_X
-    gp_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+    co_per_track<0, GP_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
       double V[6] = {0, 0, 0, 0, 0, 0}, b[3] = {0, 0, 0}, dg = 0.0;
       for (int o = s; o < e; o++) {
         GpObs &ob = p.obs[o];
         const double w2 = ob.w2, sv = ob.s, *d = ob.d, *r = ob.r;
-        const double h = gp_damp(w2 * (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), lam);
+        const double dd2 = w2 * (d[0] * d[0] + d[1] * d[1] + d[2] * d[2]), h = dd2 + vp_damping(dd2, lam);
         const double a2 = w2 * sv * sv, f = w2 / h, dr = d[0] * r[0] + d[1] * r[1] + d[2] * r[2];
         int n = 0;
 #pragma unroll
@@ -413,12 +263,14 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
         for (int i = 0; i < 3; i++) b[i] += ob.beta[i];
         dg += a2;
       }
-      const double dd = lam * fmin(fmax(dg, 1e-6), 1e32);
+      const double dd = vp_damping(dg, lam);
       V[0] += dd; V[3] += dd; V[5] += dd;
       GpPt &pt = p.pts[k];
-      if (!gp_chol(V, pt.L)) { atomicOr(&p.flags[it], 1u); return; }
+      double Vf[3][3];
+      gp_full(V, Vf);
+      if (!vp_chol<3>(Vf, pt.L)) { atomicOr(&p.flags[it], 1u); return; }
       double q[3];
-      gp_solve(pt.L, b, q);
+      vp_chol_solve<3>(pt.L, b, q);
 #pragma unroll
       for (int i = 0; i < 3; i++) { pt.b[i] = b[i]; pt.q[i] = q[i]; }
     });
@@ -427,7 +279,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
 
     // B. the camera pieces: sum P, sum w^2 s^2, sum beta, sum P q and the Schur term P_o V*^-1 W_ak
     if (!fail)
-      gp_pieces<GP_PV, 0>(p, N, [&](int o, int a, double *v) {
+      co_pieces<GP_PV, 0, GP_PV, GP_THREADS>(p.keysS, p.order, p.pieces, N, p.cams, [&](int o, int a, double *v) {
         const GpObs &ob = p.obs[o];
         const GpPt &pt = p.pts[ob.k];
 #pragma unroll
@@ -446,11 +298,12 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
         for (int j = 0; j < 3; j++) {
           const double w[3] = {Wa[j == 0 ? 0 : j == 1 ? 1 : 2], Wa[j == 0 ? 1 : j == 1 ? 3 : 4],
                                Wa[j == 0 ? 2 : j == 1 ? 4 : 5]};
-          gp_solve(pt.L, w, col);
+          vp_chol_solve<3>(pt.L, w, col);
 #pragma unroll
           for (int i = 0; i < 3; i++) Y[i][j] = col[i];
         }
-        const double Pf[3][3] = {{ob.P[0], ob.P[1], ob.P[2]}, {ob.P[1], ob.P[3], ob.P[4]}, {ob.P[2], ob.P[4], ob.P[5]}};
+        double Pf[3][3];
+        gp_full(ob.P, Pf);
         int n = 13;
 #pragma unroll
         for (int i = 0; i < 3; i++)
@@ -467,8 +320,8 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
         if (a < C) {
           GpCam &c = p.cams[a];
           double G[GP_PV];
-          gp_gather<GP_PV, 0>(p, a, c, G);
-          const double dd = lam * fmin(fmax(G[6], 1e-6), 1e32);
+          co_gather<GP_PV, 0, GP_PV>(p.pieces, a, c, G);
+          const double dd = vp_damping(G[6], lam);
           double U[6], M[6];
 #pragma unroll
           for (int j = 0; j < 6; j++) {
@@ -477,13 +330,15 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
             M[j] = c.free ? U[j] - G[13 + j] : U[j];
             c.U[j] = U[j];
           }
-          if (!gp_chol(M, c.L)) {
+          double Mf[3][3];
+          gp_full(M, Mf);
+          if (!vp_chol<3>(Mf, c.L)) {
             atomicOr(&p.flags[it], 1u);
           } else {
             double r[3], z[3];
 #pragma unroll
             for (int i = 0; i < 3; i++) r[i] = c.free ? -G[7 + i] + G[10 + i] : 0.0;
-            gp_solve(c.L, r, z);
+            vp_chol_solve<3>(c.L, r, z);
 #pragma unroll
             for (int i = 0; i < 3; i++) {
               c.x[i] = 0.0; c.r[i] = r[i]; c.z[i] = z[i]; c.p[i] = 0.0;
@@ -492,8 +347,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
             }
           }
         }
-        vp_warp_sum(d);
-        if (lane == 0) { p.camPart[GP_CP * (size_t)w] = d[0]; p.camPart[GP_CP * (size_t)w + 1] = d[1]; }
+        co_warp_partial<2>(d, p.camPart + GP_CP * (size_t)w);
       }
     grid.sync();
     fail = *(volatile unsigned int *)&p.flags[it];
@@ -502,11 +356,11 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
     int cgIt = 0;
     if (!fail) {
       double t2[2];
-      gp_totals<2>(p.camPart, camTiles, GP_CP, t2);
+      co_totals<2>(p.camPart, camTiles, GP_CP, t2);
       const double thr = p.tol2 * t2[0];
       double rr = t2[0], rz = t2[1], beta = 0.0;
       while (cgIt < p.maxLinear && !(rr <= thr)) {
-        gp_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+        co_per_track<0, GP_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
           double h[3] = {0.0, 0.0, 0.0};
           for (int o = s; o < e; o++) {
             const GpObs &ob = p.obs[o];
@@ -517,10 +371,10 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
 #pragma unroll
             for (int i = 0; i < 3; i++) h[i] += t[i];
           }
-          gp_solve(p.pts[k].L, h, p.pts[k].y);
+          vp_chol_solve<3>(p.pts[k].L, h, p.pts[k].y);
         });
         grid.sync();
-        gp_pieces<3, 0>(p, N, [&](int o, int, double *v) { gp_symv(p.obs[o].P, p.pts[p.obs[o].k].y, v); });
+        co_pieces<3, 0, GP_PV, GP_THREADS>(p.keysS, p.order, p.pieces, N, p.cams, [&](int o, int, double *v) { gp_symv(p.obs[o].P, p.pts[p.obs[o].k].y, v); });
         grid.sync();
         for (int w = warpG; w < camTiles; w += numWarps) {
           const int a = w * 32 + lane;
@@ -528,7 +382,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
           if (a < C) {
             GpCam &c = p.cams[a];
             double Wy[3], pn[3], Up[3];
-            gp_gather<3, 0>(p, a, c, Wy);
+            co_gather<3, 0, GP_PV>(p.pieces, a, c, Wy);
 #pragma unroll
             for (int i = 0; i < 3; i++) pn[i] = fma(beta, c.p[i], c.z[i]);
             gp_symv(c.U, pn, Up);
@@ -540,12 +394,11 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
               d[0] += pn[i] * q;
             }
           }
-          vp_warp_sum(d);
-          if (lane == 0) p.camPart[GP_CP * (size_t)w + 2] = d[0];
+          co_warp_partial<1>(d, p.camPart + GP_CP * (size_t)w + 2);
         }
         grid.sync();
         double pq[1];
-        gp_totals<1>(p.camPart + 2, camTiles, GP_CP, pq);
+        co_totals<1>(p.camPart + 2, camTiles, GP_CP, pq);
         if (!(pq[0] > 0.0)) break;
         const double alpha = rz / pq[0];
         for (int w = warpG; w < camTiles; w += numWarps) {
@@ -560,7 +413,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
               r[i] = fma(-alpha, c.q[i], c.r[i]);
               c.r[i] = r[i];
             }
-            gp_solve(c.L, r, z);
+            vp_chol_solve<3>(c.L, r, z);
 #pragma unroll
             for (int i = 0; i < 3; i++) {
               c.z[i] = z[i];
@@ -568,12 +421,11 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
               d[1] += r[i] * z[i];
             }
           }
-          vp_warp_sum(d);
-          if (lane == 0) { p.camPart[GP_CP * (size_t)w] = d[0]; p.camPart[GP_CP * (size_t)w + 1] = d[1]; }
+          co_warp_partial<2>(d, p.camPart + GP_CP * (size_t)w);
         }
         cgIt++;
         grid.sync();
-        gp_totals<2>(p.camPart, camTiles, GP_CP, t2);
+        co_totals<2>(p.camPart, camTiles, GP_CP, t2);
         rr = t2[0];
         beta = t2[1] / rz;
         rz = t2[1];
@@ -589,7 +441,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
 #pragma unroll
         for (int i = 0; i < 3; i++) c.cc[i] = c.free ? c.c[i] + c.x[i] : c.c[i];
       }
-      gp_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+      co_per_track<0, GP_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
         GpPt &pt = p.pts[k];
         double h[3] = {pt.b[0], pt.b[1], pt.b[2]}, dX[3];
         for (int o = s; o < e; o++) {
@@ -599,7 +451,7 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
 #pragma unroll
           for (int i = 0; i < 3; i++) h[i] += t[i];
         }
-        gp_solve(pt.L, h, dX);
+        vp_chol_solve<3>(pt.L, h, dX);
 #pragma unroll
         for (int i = 0; i < 3; i++) pt.Xc[i] = pt.X[i] + dX[i];
         for (int o = s; o < e; o++) {
@@ -615,9 +467,9 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
         }
       });
       grid.sync();
-      gp_per_point<1>(p, p.ptPart, [&](int k, int s, int e, double *v) { v[0] = gp_relinearise(p, k, s, e, true, false); });
+      co_per_track<1, GP_THREADS>(p.start, p.numTracks, p.ptPart, [&](int k, int s, int e, double *v) { v[0] = gp_relinearise(p, k, s, e, true, false); });
       grid.sync();
-      gp_totals<1>(p.ptPart, ptTiles, 1, cand);
+      co_totals<1>(p.ptPart, ptTiles, 1, cand);
     }
 
     // J. accept or reject
@@ -637,14 +489,14 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
       for (int a = tid; a < C; a += nthreads)
 #pragma unroll
         for (int i = 0; i < 3; i++) p.cams[a].c[i] = p.cams[a].cc[i];
-      gp_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) {
+      co_per_track<0, GP_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) {
         GpPt &pt = p.pts[k];
 #pragma unroll
         for (int i = 0; i < 3; i++) pt.X[i] = pt.Xc[i];
         for (int o = s; o < e; o++) p.obs[o].s = p.obs[o].sc;
       });
       grid.sync();
-      gp_per_point<0>(p, nullptr, [&](int k, int s, int e, double *) { gp_relinearise(p, k, s, e, false, true); });
+      co_per_track<0, GP_THREADS>(p.start, p.numTracks, nullptr, [&](int k, int s, int e, double *) { gp_relinearise(p, k, s, e, false, true); });
       grid.sync();
       if (stop) break;
     } else {
@@ -662,12 +514,11 @@ __global__ void __launch_bounds__(GP_THREADS) gp_kernel(GpParams p)
       d[0] = c[0] * c[0] + c[1] * c[1] + c[2] * c[2];
       d[1] = 1.0;
     }
-    vp_warp_sum(d);
-    if (lane == 0) { p.camPart[GP_CP * (size_t)w] = d[0]; p.camPart[GP_CP * (size_t)w + 1] = d[1]; }
+    co_warp_partial<2>(d, p.camPart + GP_CP * (size_t)w);
   }
   grid.sync();
   double t2[2];
-  gp_totals<2>(p.camPart, camTiles, GP_CP, t2);
+  co_totals<2>(p.camPart, camTiles, GP_CP, t2);
   const double rms = t2[1] > 0.0 ? sqrt(t2[0] / t2[1]) : 0.0;
   const double scale = rms > 0.0 && isfinite(rms) ? rms : 1.0;
   for (int k = tid; k < p.numTracks; k += nthreads) {
@@ -703,9 +554,8 @@ int globalpos_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, con
                       int maxLinearIterations, double linearTol, double *points)
 {
   const int M = numMembers, T = numTracks, C = numImages;
-  const int tiles = (M + GP_TILE - 1) / GP_TILE;
-  int bits = 1;
-  while (bits < 31 && (1ll << bits) <= (long long)C) bits++;
+  const int tiles = idivup(M, CO_TILE);
+  const int bits = radix_bits(C);                                  // every key, the sentinel C included
   size_t scanBytes = 0, sortBytes = 0;
   CS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scanBytes, (int *)nullptr, (int *)nullptr, T + 1, c.stream));
   CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sortBytes, (int *)nullptr, (int *)nullptr, (int *)nullptr,
@@ -773,14 +623,7 @@ int globalpos_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, con
   prm.loss = loss;
   prm.refImage = refImage;
 
-  int dev = 0, coop = 0;
-  CS_CUDA(cudaGetDevice(&dev));
-  CS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) {
-    set_error("cs_global_positioning: device %d does not support cooperative launches", dev);
-    return CS_E_CUDA;
-  }
-  const int wave = resident_grid<gp_kernel, GP_THREADS>();
+  const int wave = coop_grid<gp_kernel, GP_THREADS>("cs_global_positioning");
   if (wave < 0) return wave;
   const cudaStream_t st = c.stream;
   CS_CUDA(cudaMemsetAsync(base, 0, zeroEnd, st));

@@ -5,12 +5,9 @@
 // The spanning tree and the start rotations are host work (rotavg_prepare).  One counted launch follows:
 //   (cub stable radix sort of the incidences (image, 2 e + side): every image's edges in edge order)
 //   rotavg_kernel: one cooperative launch runs the whole IRLS loop, phases separated by grid barriers
-// Every floating-point sum has a fixed order that depends on the data only, not on the grid or on scheduling:
-//   - per image: the sorted incidences are cut into tiles of RA_TILE; a warp sums an image's piece of a tile
-//     lane-strided, then by a fixed xor butterfly, and one lane per image adds its pieces in ascending tile order;
-//   - totals over edges (the cost): a CTA sums a tile of 256 edges by butterflies and its warps in order; over images
-//     (the CG dot products): a warp sums a tile of 32 images by a butterfly; the tile partials are then added by warp 0
-//     of every CTA, lane-strided in ascending order and by a butterfly.  The largest step is a max, exact in any order.
+// Every floating-point sum has a fixed order that depends on the data only (coop.cuh): per image, the pieces of the
+// sorted incidences' tiles; totals over tiles of 256 edges (the cost) or 32 images (the CG dot products).  The largest
+// step is a max, exact in any order.
 // No floating-point atomics.  Every branch around a grid barrier (the CG stop, the IRLS stop) is taken on values that
 // every CTA computes from the same words, written before the barrier, by the same instructions in the same order, so
 // every CTA takes the same path; every loop is bounded by maxIterations or maxLinearIterations.
@@ -24,7 +21,7 @@
 #include <math_constants.h>
 
 #include "common.cuh"
-#include "vp_math.cuh"
+#include "coop.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -33,8 +30,6 @@ namespace cs {
 namespace {
 
 constexpr int RA_THREADS = 256;
-constexpr int RA_WARPS = RA_THREADS / 32;
-constexpr int RA_TILE = 256;         // sorted incidences per image tile
 constexpr int RA_PV = 4;             // an image piece: the sum of w, then three more (b, or the neighbours' w p)
 // Slots per image tile partial: r.r (or b.b), r.z and p.q; p.q has a slot of its own, as in bundle.cu.
 constexpr int RA_NP = 3;
@@ -134,30 +129,6 @@ __device__ __forceinline__ double ra_edge(const RaParams &p, int e)
   return g.w0 * (t2 * q);
 }
 
-// The K sums of n tile partials (part[tile * stride + j]): warp 0 adds them lane-strided in ascending order, then by a
-// fixed xor butterfly; every thread of the CTA receives them.
-template <int K>
-__device__ __forceinline__ void ra_totals(const double *part, int n, int stride, double (&out)[K])
-{
-  __shared__ double s_tot[K];
-  if (threadIdx.x < 32) {
-    double v[K];
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] = 0.0;
-    for (int i = (int)threadIdx.x; i < n; i += 32)
-#pragma unroll
-      for (int j = 0; j < K; j++) v[j] += part[(size_t)i * stride + j];
-    vp_warp_sum(v);
-    if (threadIdx.x == 0)
-#pragma unroll
-      for (int j = 0; j < K; j++) s_tot[j] = v[j];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < K; j++) out[j] = s_tot[j];
-  __syncthreads();
-}
-
 // The largest of n non-negative tile maxima, in every thread of the CTA (a max of non-negative doubles is the max of
 // their bit patterns).
 __device__ __forceinline__ double ra_max_total(const double *part, int n)
@@ -175,68 +146,6 @@ __device__ __forceinline__ double ra_max_total(const double *part, int n)
   return out;
 }
 
-// The image pieces of NV values per incidence (f(code, image, v), code = 2 e + side) at offset OFF: a warp per tile of
-// RA_TILE sorted incidences, each image's piece summed lane-strided and by a butterfly, stored at piece index
-// tile + image (unique: an image's tiles follow the previous image's last one).
-template <int NV, int OFF, class F>
-__device__ __forceinline__ void ra_pieces(const RaParams &p, F &&f)
-{
-  const int lane = threadIdx.x & 31, n = 2 * p.numEdges;
-  const int numWarps = (int)gridDim.x * RA_WARPS, numTiles = (n + RA_TILE - 1) / RA_TILE;
-  for (int t = (int)((blockIdx.x * RA_THREADS + threadIdx.x) >> 5); t < numTiles; t += numWarps) {
-    const int t1 = min(n, (t + 1) * RA_TILE);
-    for (int s = t * RA_TILE; s < t1;) {
-      const int a = p.keysS[s];
-      const int e = min(t1, p.nodes[a].end);
-      double acc[NV];
-#pragma unroll
-      for (int j = 0; j < NV; j++) acc[j] = 0.0;
-      for (int i = s + lane; i < e; i += 32) {
-        double v[NV];
-        f(p.order[i], v);
-#pragma unroll
-        for (int j = 0; j < NV; j++) acc[j] += v[j];
-      }
-      vp_warp_sum(acc);
-      if (lane == 0)
-#pragma unroll
-        for (int j = 0; j < NV; j++) p.pieces[(size_t)(t + a) * RA_PV + OFF + j] = acc[j];
-      s = e;
-    }
-  }
-}
-
-// The sum of image a's pieces (NV values at OFF) in ascending tile order.
-template <int NV, int OFF>
-__device__ __forceinline__ void ra_gather(const RaParams &p, int a, const RaNode &c, double (&v)[NV])
-{
-#pragma unroll
-  for (int j = 0; j < NV; j++) v[j] = 0.0;
-  if (c.end > c.start)
-    for (int t = c.start / RA_TILE; t <= (c.end - 1) / RA_TILE; t++)
-#pragma unroll
-      for (int j = 0; j < NV; j++) v[j] += p.pieces[(size_t)(t + a) * RA_PV + OFF + j];
-}
-
-// Every edge's residual and weight at the current rotations; the cost's tile partials (tiles of 256 edges per CTA).
-__device__ __forceinline__ void ra_residuals(const RaParams &p)
-{
-  __shared__ double s_w[RA_WARPS];
-  for (int base = (int)blockIdx.x * RA_THREADS; base < p.numEdges; base += (int)gridDim.x * RA_THREADS) {
-    const int e = base + (int)threadIdx.x;
-    double v[1] = {e < p.numEdges ? ra_edge(p, e) : 0.0};
-    vp_warp_sum(v);
-    if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v[0];
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double s = s_w[0];
-      for (int w = 1; w < RA_WARPS; w++) s += s_w[w];
-      p.edgePart[base / RA_THREADS] = s;
-    }
-    __syncthreads();
-  }
-}
-
 __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
 {
   cg::grid_group grid = cg::this_grid();
@@ -246,17 +155,13 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
   const int nodeTiles = (C + 31) / 32, edgeTiles = (p.numEdges + RA_THREADS - 1) / RA_THREADS;
 
   // 0. every image's sorted incidences; the residuals at the start rotations and their cost
-  for (int i = tid; i < n; i += nthreads) {
-    const int a = p.keysS[i];
-    if (i == 0 || p.keysS[i - 1] != a) p.nodes[a].start = i;
-    if (i == n - 1 || p.keysS[i + 1] != a) p.nodes[a].end = i + 1;
-  }
-  ra_residuals(p);
+  co_ranges(p.keysS, n, p.nodes, tid, nthreads);
+  co_per_item<1, RA_THREADS>(p.numEdges, p.edgePart, [&](int e, double *v) { v[0] = ra_edge(p, e); });
   grid.sync();
   double cost;
   {
     double t[1];
-    ra_totals<1>(p.edgePart, edgeTiles, 1, t);
+    co_totals<1>(p.edgePart, edgeTiles, 1, t);
     cost = t[0];
   }
   const double cost0 = cost;
@@ -265,7 +170,7 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
   for (int it = 0; it < p.maxIterations; it++) {
     iters++;
     // A. the image pieces: the Laplacian diagonal sum w and b = sum over its edges of -w rho (as i) or +w rho (as j)
-    ra_pieces<4, 0>(p, [&](int code, double *v) {
+    co_pieces<4, 0, RA_PV, RA_THREADS>(p.keysS, p.order, p.pieces, n, p.nodes, [&](int code, int, double *v) {
       const RaEdge &g = p.edges[code >> 1];
       const double sg = (code & 1) ? g.w : -g.w;
       v[0] = g.w;
@@ -281,7 +186,7 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
       if (a < C) {
         RaNode &c = p.nodes[a];
         double G[4];
-        ra_gather<4, 0>(p, a, c, G);
+        co_gather<4, 0, RA_PV>(p.pieces, a, c, G);
         c.diag = G[0];
         const double inv = c.free && G[0] > 0.0 ? 1.0 / G[0] : 0.0;
 #pragma unroll
@@ -292,8 +197,7 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
           d[1] += r * z;
         }
       }
-      vp_warp_sum(d);
-      if (lane == 0) { p.nodePart[RA_NP * (size_t)w] = d[0]; p.nodePart[RA_NP * (size_t)w + 1] = d[1]; }
+      co_warp_partial<2>(d, p.nodePart + RA_NP * (size_t)w);
     }
     grid.sync();
 
@@ -301,12 +205,12 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
     int cgIt = 0;
     {
       double t2[2];
-      ra_totals<2>(p.nodePart, nodeTiles, RA_NP, t2);
+      co_totals<2>(p.nodePart, nodeTiles, RA_NP, t2);
       const double thr = p.tol2 * t2[0];
       double rr = t2[0], rz = t2[1], beta = 0.0;
       while (cgIt < p.maxLinear && !(rr <= thr)) {
         // C. the image pieces of sum over its edges of w p_other, p = z + beta p_old of the other image
-        ra_pieces<3, 1>(p, [&](int code, double *v) {
+        co_pieces<3, 1, RA_PV, RA_THREADS>(p.keysS, p.order, p.pieces, n, p.nodes, [&](int code, int, double *v) {
           const RaEdge &g = p.edges[code >> 1];
           const RaNode &o = p.nodes[(code & 1) ? g.i : g.j];
 #pragma unroll
@@ -320,7 +224,7 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
           if (a < C) {
             RaNode &c = p.nodes[a];
             double Wp[3];
-            ra_gather<3, 1>(p, a, c, Wp);
+            co_gather<3, 1, RA_PV>(p.pieces, a, c, Wp);
 #pragma unroll
             for (int k = 0; k < 3; k++) {
               const double pn = fma(beta, c.p[k], c.z[k]);
@@ -330,12 +234,11 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
               d[0] += pn * q;
             }
           }
-          vp_warp_sum(d);
-          if (lane == 0) p.nodePart[RA_NP * (size_t)w + 2] = d[0];
+          co_warp_partial<1>(d, p.nodePart + RA_NP * (size_t)w + 2);
         }
         grid.sync();
         double pq[1];
-        ra_totals<1>(p.nodePart + 2, nodeTiles, RA_NP, pq);
+        co_totals<1>(p.nodePart + 2, nodeTiles, RA_NP, pq);
         if (!(pq[0] > 0.0)) break;
         const double alpha = rz / pq[0];
         // E. per image: x += alpha p, r -= alpha q, z = r / diag; the partials of r.r and r.z
@@ -355,12 +258,11 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
               d[1] += r * z;
             }
           }
-          vp_warp_sum(d);
-          if (lane == 0) { p.nodePart[RA_NP * (size_t)w] = d[0]; p.nodePart[RA_NP * (size_t)w + 1] = d[1]; }
+          co_warp_partial<2>(d, p.nodePart + RA_NP * (size_t)w);
         }
         cgIt++;
         grid.sync();
-        ra_totals<2>(p.nodePart, nodeTiles, RA_NP, t2);
+        co_totals<2>(p.nodePart, nodeTiles, RA_NP, t2);
         rr = t2[0];
         beta = t2[1] / rz;
         rz = t2[1];
@@ -390,7 +292,7 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
     const double step = ra_max_total(p.maxPart, nodeTiles);
 
     // H. the residuals at the new rotations; the trace row
-    ra_residuals(p);
+    co_per_item<1, RA_THREADS>(p.numEdges, p.edgePart, [&](int e, double *v) { v[0] = ra_edge(p, e); });
     grid.sync();
     if (tid == 0) {
       double *tr = p.trace + 3 * (size_t)it;
@@ -400,7 +302,7 @@ __global__ void __launch_bounds__(RA_THREADS) rotavg_kernel(RaParams p)
     }
     {
       double t[1];
-      ra_totals<1>(p.edgePart, edgeTiles, 1, t);
+      co_totals<1>(p.edgePart, edgeTiles, 1, t);
       cost = t[0];
     }
     if (step <= RA_STOP) break;
@@ -524,9 +426,8 @@ int rotavg_enqueue(DeviceCtx &c, int numImages, int numEdges, int maxIterations,
                    double linearTol, double sigmaDeg)
 {
   const int C = numImages, E = numEdges, n = 2 * E;
-  const int tiles = idivup(n, RA_TILE);
-  int bits = 1;
-  while (bits < 31 && (1ll << bits) < (long long)C) bits++;          // every key is < C <= 2^bits
+  const int tiles = idivup(n, CO_TILE);
+  const int bits = radix_bits(C - 1);                              // every key is < C
   size_t sortBytes = 0;
   CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sortBytes, (int *)nullptr, (int *)nullptr, (int *)nullptr,
                                           (int *)nullptr, n, 0, bits, c.stream));
@@ -569,14 +470,7 @@ int rotavg_enqueue(DeviceCtx &c, int numImages, int numEdges, int maxIterations,
   prm.maxIterations = maxIterations;
   prm.maxLinear = maxLinearIterations;
 
-  int dev = 0, coop = 0;
-  CS_CUDA(cudaGetDevice(&dev));
-  CS_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) {
-    set_error("cs_rotation_averaging: device %d does not support cooperative launches", dev);
-    return CS_E_CUDA;
-  }
-  const int wave = resident_grid<rotavg_kernel, RA_THREADS>();
+  const int wave = coop_grid<rotavg_kernel, RA_THREADS>("cs_rotation_averaging");
   if (wave < 0) return wave;
   const cudaStream_t st = c.stream;
   CS_CUDA(cudaMemsetAsync(base, 0, zeroEnd, st));

@@ -2,9 +2,10 @@
 // pose (pose.cu), bundle adjustment (bundle.cu) and the vocabulary's start draws (vocab.cu) share: the counter-based
 // generator and sampler, the cyclic Jacobi eigen-decomposition, the calibrated coordinates of a pinhole K, the fixed
 // xor butterflies (a sum over K doubles, a max over a u64 key), the Rodrigues rotation and the left rotation update,
-// the member rule of a track, and the reprojection inlier rule and per-observation output; and the hypothesis prologue
-// and slot arg-max of the two batched RANSAC calls (verify.cu, pose.cu).  tests/verify_oracle.py and
-// tests/triangulate_oracle.py restate the rules in float64.
+// the member rule of a track, and the reprojection inlier rule and per-observation output; the small Cholesky and its
+// solve, the Levenberg-Marquardt damping term and the robust losses of bundle adjustment and global positioning
+// (globalpos.cu); and the hypothesis prologue and slot arg-max of the two batched RANSAC calls (verify.cu, pose.cu).
+// tests/verify_oracle.py and tests/triangulate_oracle.py restate the rules in float64.
 #pragma once
 
 #include <cmath>
@@ -174,6 +175,74 @@ __device__ __forceinline__ void vp_rotate(const double *w, const double *R, doub
   for (int i = 0; i < 3; i++)
 #pragma unroll
     for (int j = 0; j < 3; j++) R1[3 * i + j] = Q[3 * i] * R[j] + Q[3 * i + 1] * R[3 + j] + Q[3 * i + 2] * R[6 + j];
+}
+
+// Cholesky of the symmetric A (N x N, its lower triangle read); false when a pivot is not > 0 or not finite.  L is
+// lower, packed row by row.
+template <int N>
+__device__ __forceinline__ bool vp_chol(const double (&A)[N][N], double *L)
+{
+  double F[N][N];
+#pragma unroll
+  for (int j = 0; j < N; j++) {
+    double d = A[j][j];
+#pragma unroll
+    for (int q = 0; q < j; q++) d -= F[j][q] * F[j][q];
+    if (!(d > 0.0) || !isfinite(d)) return false;
+    F[j][j] = sqrt(d);
+#pragma unroll
+    for (int i = j + 1; i < N; i++) {
+      double e = A[i][j];
+#pragma unroll
+      for (int q = 0; q < j; q++) e -= F[i][q] * F[j][q];
+      F[i][j] = e / F[j][j];
+    }
+  }
+  int k = 0;
+#pragma unroll
+  for (int i = 0; i < N; i++)
+#pragma unroll
+    for (int j = 0; j <= i; j++) L[k++] = F[i][j];
+  return true;
+}
+
+// x = A^-1 b from the packed factor of vp_chol (forward, then backward substitution)
+template <int N>
+__device__ __forceinline__ void vp_chol_solve(const double *L, const double (&b)[N], double (&x)[N])
+{
+  double z[N];
+#pragma unroll
+  for (int i = 0; i < N; i++) {
+    double e = b[i];
+#pragma unroll
+    for (int q = 0; q < i; q++) e -= L[i * (i + 1) / 2 + q] * z[q];
+    z[i] = e / L[i * (i + 1) / 2 + i];
+  }
+#pragma unroll
+  for (int i = N - 1; i >= 0; i--) {
+    double e = z[i];
+#pragma unroll
+    for (int q = i + 1; q < N; q++) e -= L[q * (q + 1) / 2 + i] * x[q];
+    x[i] = e / L[i * (i + 1) / 2 + i];
+  }
+}
+
+// The Levenberg-Marquardt damping lambda clamp(d, 1e-6, 1e32) added to a diagonal entry d of bundle adjustment and
+// global positioning (to the scale block and the point and camera diagonals there, each by its own d).
+__device__ __forceinline__ double vp_damping(double d, double lam) { return lam * fmin(fmax(d, 1e-6), 1e32); }
+
+// The robust losses of cs_bundle_adjust_intrinsics and cs_global_positioning (1 soft-L1, 2 Cauchy) at s of scale c2:
+// c^2 rho(s / c^2), and *w2 = rho'(s / c^2) when w2 is given.
+__device__ __forceinline__ double vp_loss(int loss, double c2, double s, double *w2)
+{
+  const double u = s / c2;
+  if (loss == 1) {
+    const double q = sqrt(1.0 + u);
+    if (w2) *w2 = 1.0 / q;
+    return c2 * (2.0 * u / (q + 1.0));
+  }
+  if (w2) *w2 = 1.0 / (1.0 + u);
+  return c2 * log1p(u);
 }
 
 // A valid member (a, f) of a track, the rule of triangulation and bundle adjustment: a known image, a feature inside
