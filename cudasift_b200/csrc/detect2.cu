@@ -13,10 +13,12 @@
 //  * Input rows arrive by TMA (cp.async.bulk.tensor.2d, one 256x1 box per row and stream, row index clamped
 //    by the issuing thread, columns clamped by the reading thread) into an 8-deep ring -> no address
 //    arithmetic and no global loads in the loop.
-//  * Warp-specialised, one CTA of 16 warps per SM:
-//      warps 12-15 (producers): vertical pass of all 8 scales (thread = columns c and c+128, 9-row register
-//                              window, 40 taps in registers) and the TMA row ring -- the serial critical path, kept
-//                              short; results go to shared memory once (STS.64)
+//  * Warp-specialised, one CTA of 20 warps per SM (five warpgroups):
+//      warps 12-19 (producers, two warpgroups): vertical pass of all 8 scales (thread = one staged column: warps 12-15
+//                              take columns 0-127, warps 16-19 columns 128-255; 9-row register window, 40 taps in
+//                              registers) and the TMA row ring (one lane issues it) -- a serial path, kept short so
+//                              that the consumer groups, not the producers, set the pace; results go to shared memory
+//                              once (STS.64)
 //      warps 0-3 / 4-7 / 8-11 (consumer groups 0 / 1 / 2): horizontal pass + DoG + candidate flags of the steps
 //                              k = g mod 3 (2 x 16 column groups), then the extrema tests of row k-4; each group has
 //                              three steps of time for one step of work.  Lane = (scale, 8 columns): 8 conflict-free
@@ -26,7 +28,9 @@
 //    four steps later, when the rows above and below exist.
 //
 // The producers run ahead of the consumers through three vertical-result buffers (buffer = group); hand-over is by
-// named barriers (bar.arrive / bar.sync) instead of CTA-wide barriers:
+// named barriers (bar.arrive / bar.sync) instead of CTA-wide barriers.  Each of them counts the 256 producer threads
+// and the 128 threads of one group, so it completes only when every thread of both producer warpgroups has arrived:
+// the producers pass them together, and every statement below about "the producers" holds for all 256.
 //   FULL[g]  producers -> group g: v[g] written        EMPTY[g] group g -> producers: v[g] is in registers
 //   DONE[g]  group g -> producers: the DoG row and the candidate list of its step are written (the extrema tests of
 //            an older row follow, off the producers' critical path)
@@ -93,8 +97,12 @@ __device__ __forceinline__ void d2_refine(const float (&v)[3][3][3], int gx, int
   else d2_store_keypoint(pts, maxPts, atomicAdd(counter, 1u), kp);
 }
 
-#define D3_THREADS 512
-#define D3_PT 128
+#define D3_GT 128                                        // threads per consumer group (one warpgroup)
+#define D3_PT 256                                        // producer threads (two warpgroups), one staged column each
+// 640 threads leave 96 registers per thread.  Both roles fit without a setmaxnreg rebalance: in the sm_90a SASS the
+// consumer code peaks at 94 registers and the one-column producer code at 60, with no spills.
+#define D3_THREADS (3 * D3_GT + D3_PT)
+#define D3_HAND (D3_GT + D3_PT)                          // threads on a FULL / EMPTY / DONE / LATE barrier
 #define D3_RS 8
 #define D3_SMEM_RING (D3_RS * D2_RSLOTF * 4)            // 112000
 #define D3_SMEM_LIST (D3_RS * 512 * 2)                  // 8192
@@ -132,7 +140,7 @@ __device__ __forceinline__ void d3_extrema(const D3Item &I, int j, int pt, const
   if (scan) n = 2 * CS_NUM_SCALES * D2_TESTED;
   const float *rm = s_ring + ((j + D3_RS - 1) & (D3_RS - 1)) * D2_RSLOTF, *r0 = s_ring + qj * D2_RSLOTF,
               *rp = s_ring + ((j + 1) & (D3_RS - 1)) * D2_RSLOTF;
-  for (int i = pt; i < n; i += D3_PT) {
+  for (int i = pt; i < n; i += D3_GT) {
     int dc, p, hf;
     if (!scan) {
       const int e = s_list[qj * 512 + i];
@@ -196,28 +204,17 @@ __device__ __forceinline__ void d3_extrema(const D3Item &I, int j, int pt, const
   }
 }
 
-// vertical pass of one step, all 8 scales of both columns
+// vertical pass of one step, all 8 scales of the thread's column
 template <int PH>
-__device__ __forceinline__ void d3_vertical(f32x2 (&W0)[9], f32x2 (&W1)[9], f32x2 n0, f32x2 n1,
-                                            const float (&kv)[CS_LAPLACE_S][5], float2 *vdst)
+__device__ __forceinline__ void d3_vertical(f32x2 (&W)[9], f32x2 n, const float (&kv)[CS_LAPLACE_S][5], float2 *vdst)
 {
 #define D3_WI(i) ((PH + 1 + (i)) % 9)
-  W0[PH] = n0;
-  W1[PH] = n1;
-  {
-    const f32x2 c = W0[D3_WI(4)];
-    const f32x2 p1 = add2(W0[D3_WI(3)], W0[D3_WI(5)]), p2 = add2(W0[D3_WI(2)], W0[D3_WI(6)]);
-    const f32x2 p3 = add2(W0[D3_WI(1)], W0[D3_WI(7)]), p4 = add2(W0[D3_WI(0)], W0[D3_WI(8)]);
+  W[PH] = n;
+  const f32x2 c = W[D3_WI(4)];
+  const f32x2 p1 = add2(W[D3_WI(3)], W[D3_WI(5)]), p2 = add2(W[D3_WI(2)], W[D3_WI(6)]);
+  const f32x2 p3 = add2(W[D3_WI(1)], W[D3_WI(7)]), p4 = add2(W[D3_WI(0)], W[D3_WI(8)]);
 #pragma unroll
-    for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2] = upk(laplace9(kv[s], c, p1, p2, p3, p4));
-  }
-  {
-    const f32x2 c = W1[D3_WI(4)];
-    const f32x2 p1 = add2(W1[D3_WI(3)], W1[D3_WI(5)]), p2 = add2(W1[D3_WI(2)], W1[D3_WI(6)]);
-    const f32x2 p3 = add2(W1[D3_WI(1)], W1[D3_WI(7)]), p4 = add2(W1[D3_WI(0)], W1[D3_WI(8)]);
-#pragma unroll
-    for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2 + 128] = upk(laplace9(kv[s], c, p1, p2, p3, p4));
-  }
+  for (int s = 0; s < CS_LAPLACE_S; s++) vdst[s * D2_VROW2] = upk(laplace9(kv[s], c, p1, p2, p3, p4));
 #undef D3_WI
 }
 
@@ -235,8 +232,8 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
   __shared__ D2Keypoint s_kq[D2_KQ];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool producer = warp >= 12;       // the highest warp ids: the issue arbiter favours them, and they are the critical path
-  const int pt = tid - 384;               // producer thread index (0..127)
+  const bool producer = warp >= 12;       // the highest warp ids: the issue arbiter favours them
+  const int pt = tid - 3 * D3_GT;         // producer thread index (0..255) = staged column
 
   int item = blockIdx.x;
   unsigned int req = 0;
@@ -273,23 +270,21 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
           tma_load_2d(s_in + (2 * i + 1) * D2_IW, map, x0 - 4, min(max(ry0 + hs - 5 + i, 0), h - 1), &s_full[i]);
         }
       }
-      // columns this thread reads from a staged row (clamped to the image: cudaSiftD.cu:1764-1767)
-      const int ci0 = min(max(x0 - 4 + pt, 0), w - 1) - (x0 - 4);
-      const int ci1 = min(max(x0 - 4 + pt + 128, 0), w - 1) - (x0 - 4);
+      // the column this thread reads from a staged row (clamped to the image: cudaSiftD.cu:1764-1767)
+      const int ci = min(max(x0 - 4 + pt, 0), w - 1) - (x0 - 4);
       float kv[CS_LAPLACE_S][5];
 #pragma unroll
       for (int s = 0; s < CS_LAPLACE_S; s++)
 #pragma unroll
         for (int j = 0; j < 5; j++) kv[s][j] = L.taps.k[s][j];
-      f32x2 W0[9], W1[9];
+      f32x2 W[9];
 #pragma unroll
       for (int i = 0; i < 8; i++) {
         mbarrier_wait(&s_full[i], 0);
         const float *ra = s_in + (2 * i) * D2_IW, *rb = ra + D2_IW;
-        W0[i] = pk2(ra[ci0], rb[ci0]);
-        W1[i] = pk2(ra[ci1], rb[ci1]);
+        W[i] = pk2(ra[ci], rb[ci]);
       }
-      W0[8] = 0ull; W1[8] = 0ull;
+      W[8] = 0ull;
       nb_sync(NB_PINT, D3_PT);                            // every producer has read the prologue rows
       if (pt == 0) {
         for (int i = 0; i < D2_NS; i++)
@@ -300,38 +295,37 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
           }
       }
       // rows of step 0 (software pipelining: the rows of step m+1 are fetched at the end of step m)
-      f32x2 n0, n1;
+      f32x2 n;
       {
         mbarrier_wait(&s_full[0], 1);
-        n0 = pk2(s_in[ci0], s_in[D2_IW + ci0]);
-        n1 = pk2(s_in[ci1], s_in[D2_IW + ci1]);
+        n = pk2(s_in[ci], s_in[D2_IW + ci]);
       }
       // step m: window slot of the newest row = (8 + m) % 9 -> unrolled by 9 so that the slots are compile-time.
-      // The EMPTY hand-over (all 128 producers take part) doubles as the producers' own barrier: past it, every
-      // producer has finished step m-1, so the input slots read up to then may be refilled.
+      // The EMPTY hand-over doubles as the producers' own barrier: it completes only when all 256 producer threads
+      // (both warpgroups) have arrived, so past it every producer has finished step m-1, and the input slots read up to
+      // then may be refilled.
 #define D3_PSTEP(p)                                                                                           \
   {                                                                                                           \
     const int m = m0 + (p);                                                                                   \
     if (m >= nsteps + 3) break;                                                                               \
-    f32x2 x0n = 0ull, x1n = 0ull;                                                                             \
+    f32x2 xn = 0ull;                                                                                          \
     if (m < nsteps) {                                                                                         \
-      if (m >= D3_NB) nb_sync(NB_EMPTY + (p) % D3_NB, 2 * D3_PT);                                             \
+      if (m >= D3_NB) nb_sync(NB_EMPTY + (p) % D3_NB, D3_HAND);                                               \
       if (m + 1 < nsteps) {                  /* rows of step m+1: their latency hides behind this step's math */ \
         const int slot = (m + 1) & (D2_NS - 1);                                                               \
         mbarrier_wait(&s_full[slot], ((9 + m) >> 3) & 1);                                                     \
         const float *ra = s_in + (2 * slot) * D2_IW, *rb = ra + D2_IW;                                        \
-        x0n = pk2(ra[ci0], rb[ci0]);                                                                          \
-        x1n = pk2(ra[ci1], rb[ci1]);                                                                          \
+        xn = pk2(ra[ci], rb[ci]);                                                                             \
       }                                                                                                       \
-      d3_vertical<(8 + (p)) % 9>(W0, W1, n0, n1, kv, s_v + ((p) % D3_NB) * D2_VBUF2 + pt);                    \
-      n0 = x0n; n1 = x1n;                                                                                     \
+      d3_vertical<(8 + (p)) % 9>(W, n, kv, s_v + ((p) % D3_NB) * D2_VBUF2 + pt);                              \
+      n = xn;                                                                                                 \
     }                                                                                                         \
     /* DONE: the group's previous step (m-3) has written its DoG row and candidate list.  LATE: step m-4 (another */ \
     /* group) is complete including its extrema tests (rows m-9..m-7, list of row m-8) */                     \
-    if (m >= D3_NB) nb_sync(NB_DONE + (p) % D3_NB, 2 * D3_PT);                                                \
-    if (m >= D3_NB + 1) nb_sync(NB_LATE + ((p) + 2) % D3_NB, 2 * D3_PT);                                      \
+    if (m >= D3_NB) nb_sync(NB_DONE + (p) % D3_NB, D3_HAND);                                                  \
+    if (m >= D3_NB + 1) nb_sync(NB_LATE + ((p) + 2) % D3_NB, D3_HAND);                                        \
     if (pt == 0 && m >= 8) s_cnt[m & (D3_RS - 1)] = 0;           /* list of row m-8: used again by step m */    \
-    nb_arrive(NB_FULL + (p) % D3_NB, 2 * D3_PT);               /* in the drain steps: only releases the tests */ \
+    nb_arrive(NB_FULL + (p) % D3_NB, D3_HAND);                 /* in the drain steps: only releases the tests */ \
     if (pt == 0 && m >= D3_NB && m < nsteps) {                                                                \
       /* past EMPTY of this step every producer has finished step m-1: refill the slots read up to then */     \
       for (int r = (m == D3_NB ? 0 : m - 1); r < m; r++)                                                      \
@@ -371,6 +365,17 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
       I.cellBase = P.cellBase[level]; I.cellsX = P.cellsX[level]; I.capLimit = P.capLimit;
       const bool testable = hs_ >= 2 && hs_ <= 6;               // DoG planes 1..5
       const int tig = tid & 127;                                // thread index within the group
+      // columns of the lane's 8 that are tested (bits d and 8 + d for the two streams), per pass: fixed for the item
+      unsigned colok[2];
+#pragma unroll
+      for (int pass = 0; pass < 2; pass++) {
+        colok[pass] = 0;
+#pragma unroll
+        for (int d = 0; d < 8; d++) {
+          const int dc = 8 * (16 * pass + 4 * wg + cgl) + d;
+          if (dc >= 1 && dc <= D2_TESTED && x0 + dc <= w - 2) colok[pass] |= 0x101u << d;
+        }
+      }
       for (int k = g; k < nsteps + 3; k += D3_NB) {
         const int q = k & (D3_RS - 1);
         // LATE: this group's previous step (k-3) is complete, extrema tests included.  It is signalled here, after the
@@ -378,15 +383,15 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
         // which is before they can signal FULL of step k+3, so two arrivals never pile up on the barrier.
         const bool late = k >= D3_NB && k - D3_NB <= nsteps - 2;
         if (k >= nsteps) {                                      // drain: only the extrema of the last rows
-          nb_sync(NB_FULL + g, 2 * D3_PT);
-          if (late) nb_arrive(NB_LATE + g, 2 * D3_PT);
+          nb_sync(NB_FULL + g, D3_HAND);
+          if (late) nb_arrive(NB_LATE + g, D3_HAND);
           if (k - 4 <= hs && s_cnt[(k - 4) & (D3_RS - 1)] != 0) d3_extrema(I, k - 4, tig, s_ring, s_list, s_cnt, s_kq, &s_kn);
           continue;
         }
         const bool rowsTested = testable && k >= 1 && k <= hs;
-        const bool okA = ry0 - 1 + k <= h - 2, okB = ry0 + hs - 1 + k <= h - 2;
-        nb_sync(NB_FULL + g, 2 * D3_PT);
-        if (late) nb_arrive(NB_LATE + g, 2 * D3_PT);
+        const unsigned rowok = (ry0 - 1 + k <= h - 2 ? 0xffu : 0u) | (ry0 + hs - 1 + k <= h - 2 ? 0xff00u : 0u);
+        nb_sync(NB_FULL + g, D3_HAND);
+        if (late) nb_arrive(NB_LATE + g, D3_HAND);
 #pragma unroll
         for (int pass = 0; pass < 2; pass++) {
           const int cg = 16 * pass + 4 * wg + cgl;
@@ -399,7 +404,7 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
             V[2 * j] = pk2(t4.x, t4.y);
             V[2 * j + 1] = pk2(t4.z, t4.w);
           }
-          if (pass == 1 && k + D3_NB < nsteps) nb_arrive(NB_EMPTY + g, 2 * D3_PT);   // v[g] is in registers
+          if (pass == 1 && k + D3_NB < nsteps) nb_arrive(NB_EMPTY + g, D3_HAND);   // v[g] is in registers
           f32x2 dg[8];
 #pragma unroll
           for (int d = 0; d < 8; d++) {
@@ -424,12 +429,10 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
             m = fmaxf(m, fmaxf(fabsf(a.x), fabsf(a.y)));
           }
           if (m > thresh && rowsTested && act) {
-            unsigned bits = 0, colok = 0;
+            unsigned bits = 0;
 #pragma unroll
             for (int d = 0; d < 8; d++) {
               const float2 a = upk(dg[d]);
-              const int dc = 8 * cg + d;
-              if (dc >= 1 && dc <= D2_TESTED && x0 + dc <= w - 2) colok |= 0x101u << d;
               // a necessary condition that is already in registers: an extremum beats its left and right neighbours
               // (columns 1..6 of the lane's 8; the two outer columns are decided by the full test)
               bool ex = true, ey = true;
@@ -438,10 +441,10 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
                 ex = a.x > 0.0f ? (a.x > l.x && a.x > r.x) : (a.x < l.x && a.x < r.x);
                 ey = a.y > 0.0f ? (a.y > l.y && a.y > r.y) : (a.y < l.y && a.y < r.y);
               }
-              if (okA && ex && fabsf(a.x) > thresh) bits |= 1u << d;
-              if (okB && ey && fabsf(a.y) > thresh) bits |= 0x100u << d;
+              if (ex && fabsf(a.x) > thresh) bits |= 1u << d;
+              if (ey && fabsf(a.y) > thresh) bits |= 0x100u << d;
             }
-            bits &= colok;
+            bits &= colok[pass] & rowok;
             if (bits) {
               int at = atomicAdd(&s_cnt[q], __popc(bits));
               while (bits) {
@@ -453,7 +456,7 @@ detect3_kernel(const __grid_constant__ Detect2Params P)
             }
           }
         }
-        nb_arrive(NB_DONE + g, 2 * D3_PT);                       // row k and its candidate list are written
+        nb_arrive(NB_DONE + g, D3_HAND);                       // row k and its candidate list are written
         // rows k-5..k-3 are complete; the tests run only when the row has candidates at all
         if (k >= 5 && s_cnt[(k - 4) & (D3_RS - 1)] != 0) d3_extrema(I, k - 4, tig, s_ring, s_list, s_cnt, s_kq, &s_kn);
       }
