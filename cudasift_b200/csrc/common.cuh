@@ -480,15 +480,15 @@ __device__ __forceinline__ int table_find(const T *__restrict__ a, int n, int T:
   return lo;
 }
 
-// One pair list of the flags / write kernels (match_mutual.cu): the keep test of rows [0, n1) of set 1, then pairs
-// {i, jv[i * jstride]} at positions < maxPairs and the total.  A single call passes one by value; a batch passes a
-// table in device memory, job k owning the CTAs from cta0 on.
+// One pair list of the flags / write kernels (match_mutual.cu; an ordered list of ordered_list.cuh): the keep test of
+// rows [0, n1) of set 1, then pairs {i, jv[i * jstride]} at positions < maxPairs and the total.  A single call passes
+// one by value; a batch passes a table in device memory, job k owning the CTAs from cta0 on.
 struct PairJob {
   const int *jv; int jstride;
   int n1, n2;
   const int2 *idx1; const float2 *score1;     // ratio: the knn lists of set 1
   const int2 *idx2; const float2 *score2;     // and of set 2 (cross-check), or null
-  unsigned int *masks, *blockCounts;          // ceil(n1 / 32) ballot words, ceil(n1 / 1024) CTA counts
+  unsigned int *masks, *blockCounts;          // list_words(n1) ballot words, list_ctas(n1) CTA counts
   int2 *pairs; int maxPairs;
   unsigned int *total;
   int cta0;

@@ -29,6 +29,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "ordered_list.cuh"
 
 namespace cs {
 
@@ -609,8 +610,8 @@ static GLayout gd_layout(int n1, int n2, int dirs)
   const size_t l2 = dirs == 2 ? (size_t)n2 : 0;
   L.idx1 = b.take(8 * (size_t)n1); L.sc1 = b.take(8 * (size_t)n1);
   L.idx2 = b.take(8 * l2); L.sc2 = b.take(8 * l2);
-  // the flags / write kernels' ballot words and counts of 1024-row CTAs (match_mutual.cu)
-  L.masks = b.take(4 * (size_t)idivup(n1, 32)); L.ctaCounts = b.take(4 * (size_t)idivup(n1, 1024));
+  // the pair list's ballot words and CTA counts (ordered_list.cuh)
+  L.masks = b.take(4 * (size_t)list_words(n1)); L.ctaCounts = b.take(4 * (size_t)list_ctas(n1));
   L.bytes = b.bytes;
   return L;
 }
@@ -698,7 +699,7 @@ int guided_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *j
     v.restBytes += L.bytes;
     v.pointCtas += idivup(n1 + n2, 256);
     v.knnCtas += idivup(n1, GD_WARPS) + (cross ? idivup(n2, GD_WARPS) : 0);
-    v.pairCtas += idivup(n1, 1024);
+    v.pairCtas += list_ctas(n1);
   }
   for (GdWave &v : waves) {
     const size_t J = v.q1 - v.q0;
@@ -764,7 +765,7 @@ int guided_enqueue(DeviceCtx &c, const cs_match_set *sets, const cs_match_job *j
       pj.pairs = reinterpret_cast<int2 *>(jb.pairs); pj.maxPairs = jb.maxPairs;
       pj.total = totals + k;
       pj.cta0 = pairCta;
-      pairCta += idivup(n1, 1024);
+      pairCta += list_ctas(n1);
       out[p].stats = reinterpret_cast<const GHdr *>(hstate)[k].stats;
       out[p].total = reinterpret_cast<const unsigned int *>(hstate + v.totalsAt) + k;
       z += L.zeroBytes;

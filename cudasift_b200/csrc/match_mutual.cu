@@ -1,33 +1,28 @@
-// match_mutual.cu -- the pair lists of a mutual match and of a ratio match.
+// match_mutual.cu -- the pair lists of a mutual match and of a ratio match, built as the ordered lists of
+// ordered_list.cuh (flag, then scan and write; no atomics, so the order follows from the values).
 // Mutual: the pairs (i, j) with
 //   s1[i].match == j >= 0,  s2[j].match == i,  s1[i].score > minScore,  s1[i].ambiguity < maxAmbiguity
 // (strict comparisons, as FindHomography, homography.cu:200), written as int2 {i, j} in increasing i.  Every j
-// appears at most once (it pairs only with i = s2[j].match).  The order is defined by value: two launches, no atomics.
-//   1. flags   one thread per row i: the keep test; a ballot word per 32 rows and a count per CTA of 1024 rows.
-//   2. write   every CTA sums the counts of the CTAs before it (its exclusive prefix), scans its own 32 ballot words
-//              and writes its pairs; the last CTA writes the total.  Pairs at positions >= maxPairs are not written.
+// appears at most once (it pairs only with i = s2[j].match).  Two launches: mutual_flags_kernel, then
+// mutual_write_kernel, which writes the pairs at positions < maxPairs and the total.
 // Ratio (cs_match_ratio): the same two launches on the two-nearest-neighbour lists; ratio_flags_kernel applies Lowe's
 // ratio test (COLMAP's rule, on angles) and the optional cross-check, and the write kernel reads j = idx[i][0].
 #include "common.cuh"
+#include "ordered_list.cuh"
 
 namespace cs {
 
-#define MP_ROWS 1024          // rows per CTA (one per thread)
-
-__global__ void __launch_bounds__(MP_ROWS)
+__global__ void __launch_bounds__(LIST_ROWS)
 mutual_flags_kernel(const SiftPoint *__restrict__ s1, int n1, const SiftPoint *__restrict__ s2, int n2, float minScore,
                     float maxAmbiguity, unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts)
 {
-  const int i = blockIdx.x * MP_ROWS + threadIdx.x;
+  const int i = blockIdx.x * LIST_ROWS + threadIdx.x;
   bool keep = false;
   if (i < n1) {
     const int j = s1[i].match;
     if (j >= 0 && j < n2 && s1[i].score > minScore && s1[i].ambiguity < maxAmbiguity) keep = __ldg(&s2[j].match) == i;
   }
-  const unsigned int bal = __ballot_sync(0xffffffffu, keep);
-  if ((threadIdx.x & 31) == 0 && i < n1) masks[i >> 5] = bal;
-  const int cnt = __syncthreads_count(keep);
-  if (threadIdx.x == 0) blockCounts[blockIdx.x] = (unsigned int)cnt;
+  list_flag(keep, i, n1, masks, blockCounts, blockIdx.x);
 }
 
 // The pair list of this CTA and the CTA's index in it: the one of a call, or job k of a batch table (jobs != nullptr).
@@ -39,56 +34,16 @@ __device__ __forceinline__ PairJob pair_job(const PairJob &one, const PairJob *_
   return j;
 }
 
-// Positions by value: within its pair list, every CTA sums the counts of the CTAs before it; the last writes the total.
-__global__ void __launch_bounds__(MP_ROWS)
+// The pairs {i, jv[i * jstride]} of the kept rows at their positions within the CTA's pair list, and the total.
+__global__ void __launch_bounds__(LIST_ROWS)
 mutual_write_kernel(const PairJob one, const PairJob *__restrict__ jobs, int numJobs)
 {
-  __shared__ unsigned int s_w[32];
-  __shared__ unsigned int s_base;
   int blk;
   const PairJob pj = pair_job(one, jobs, numJobs, blk);
-  const int *__restrict__ jv = pj.jv;
-  const int jstride = pj.jstride, n1 = pj.n1, maxPairs = pj.maxPairs;
-  const unsigned int *__restrict__ masks = pj.masks, *__restrict__ blockCounts = pj.blockCounts;
-  int2 *__restrict__ pairs = pj.pairs;
-  const unsigned int FULL = 0xffffffffu;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  // exclusive prefix of this CTA: the counts of the CTAs before it
-  unsigned int part = 0;
-  for (int k = threadIdx.x; k < blk; k += MP_ROWS) part += blockCounts[k];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
-  if (lane == 0) s_w[w] = part;
-  __syncthreads();
-  if (w == 0) {
-    unsigned int v = s_w[lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    if (lane == 0) s_base = v;
-  }
-  __syncthreads();
-  const unsigned int base = s_base;
-  // positions inside the CTA: exclusive scan of the warps' ballot counts
-  const int i = blk * MP_ROWS + threadIdx.x;
-  const unsigned int bal = (blk * MP_ROWS + w * 32 < n1) ? masks[(blk * MP_ROWS >> 5) + w] : 0u;
-  if (lane == 0) s_w[w] = __popc(bal);
-  __syncthreads();
-  if (w == 0) {
-    const unsigned int c = s_w[lane];
-    unsigned int inc = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int t = __shfl_up_sync(FULL, inc, o);
-      if (lane >= o) inc += t;
-    }
-    s_w[lane] = inc - c;
-    if (lane == 31 && blk == (n1 - 1) / MP_ROWS) *pj.total = base + inc;
-  }
-  __syncthreads();
-  if ((bal >> lane) & 1u) {
-    const unsigned int pos = base + s_w[w] + __popc(bal & ((1u << lane) - 1u));
-    if (pos < (unsigned int)maxPairs) pairs[pos] = make_int2(i, jv[(size_t)i * jstride]);
-  }
+  bool bit;
+  const unsigned int pos = list_position(pj.masks, pj.blockCounts, pj.n1, blk, &bit, pj.total);
+  const int i = blk * LIST_ROWS + threadIdx.x;
+  if (bit && pos < (unsigned int)pj.maxPairs) pj.pairs[pos] = make_int2(i, pj.jv[(size_t)i * pj.jstride]);
 }
 
 // COLMAP's one-way test on row i's two neighbours, in double: d = acos(min(score, 1)), keep when j1 >= 0,
@@ -104,7 +59,7 @@ __device__ __forceinline__ bool ratio_keep(const int2 *__restrict__ idx, const f
 }
 
 // one thread per row i of set 1; idx2 != nullptr: cross-check, row j1 of set 2 must pass as well and name i
-__global__ void __launch_bounds__(MP_ROWS)
+__global__ void __launch_bounds__(LIST_ROWS)
 ratio_flags_kernel(const PairJob one, const PairJob *__restrict__ jobs, int numJobs, double maxRatio, double maxDistance)
 {
   int blk;
@@ -112,7 +67,7 @@ ratio_flags_kernel(const PairJob one, const PairJob *__restrict__ jobs, int numJ
   const int2 *__restrict__ idx1 = pj.idx1, *__restrict__ idx2 = pj.idx2;
   const float2 *__restrict__ score1 = pj.score1, *__restrict__ score2 = pj.score2;
   const int n1 = pj.n1, n2 = pj.n2;
-  const int i = blk * MP_ROWS + threadIdx.x;
+  const int i = blk * LIST_ROWS + threadIdx.x;
   bool keep = false;
   if (i < n1 && ratio_keep(idx1, score1, i, maxRatio, maxDistance)) {
     keep = true;
@@ -121,17 +76,14 @@ ratio_flags_kernel(const PairJob one, const PairJob *__restrict__ jobs, int numJ
       keep = j < n2 && idx2[j].x == i && ratio_keep(idx2, score2, j, maxRatio, maxDistance);
     }
   }
-  const unsigned int bal = __ballot_sync(0xffffffffu, keep);
-  if ((threadIdx.x & 31) == 0 && i < n1) pj.masks[i >> 5] = bal;
-  const int cnt = __syncthreads_count(keep);
-  if (threadIdx.x == 0) pj.blockCounts[blk] = (unsigned int)cnt;
+  list_flag(keep, i, n1, pj.masks, pj.blockCounts, blk);
 }
 
 // Ballot words, CTA counts and the total of n1 rows in c.pairScratch; the total is copied to *c.h_pairTotal after the
 // two launches.
 static int pairs_scratch(DeviceCtx &c, int n1, PairJob &pj)
 {
-  const int blocks = idivup(n1, MP_ROWS), words = idivup(n1, 32);
+  const int blocks = list_ctas(n1), words = list_words(n1);
   int r;
   if ((r = c.pairScratch.grow(((size_t)words + blocks + 1) * sizeof(unsigned int))) < 0) return r;
   pj.n1 = n1;
@@ -147,10 +99,10 @@ int launch_mutual_pairs(DeviceCtx &c, const SiftPoint *s1, int n1, const SiftPoi
   if ((r = pairs_scratch(c, n1, pj)) < 0) return r;
   pj.jv = &s1[0].match; pj.jstride = (int)(sizeof(SiftPoint) / sizeof(int));
   pj.pairs = mu.pairs; pj.maxPairs = mu.maxPairs;
-  const int blocks = idivup(n1, MP_ROWS);
-  mutual_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, pj.masks,
-                                                        pj.blockCounts);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(pj, nullptr, 0);
+  const int blocks = list_ctas(n1);
+  mutual_flags_kernel<<<blocks, LIST_ROWS, 0, c.stream>>>(s1, n1, s2, n2, mu.minScore, mu.maxAmbiguity, pj.masks,
+                                                          pj.blockCounts);
+  mutual_write_kernel<<<blocks, LIST_ROWS, 0, c.stream>>>(pj, nullptr, 0);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
   CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, pj.total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
@@ -167,9 +119,9 @@ int launch_ratio_pairs(DeviceCtx &c, const int *idx1, const float *score1, int n
   pj.idx1 = reinterpret_cast<const int2 *>(idx1); pj.score1 = reinterpret_cast<const float2 *>(score1);
   pj.idx2 = reinterpret_cast<const int2 *>(idx2); pj.score2 = reinterpret_cast<const float2 *>(score2);
   pj.pairs = ra.pairs; pj.maxPairs = ra.maxPairs;
-  const int blocks = idivup(n1, MP_ROWS);
-  ratio_flags_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(pj, nullptr, 0, (double)ra.maxRatio, (double)ra.maxDistance);
-  mutual_write_kernel<<<blocks, MP_ROWS, 0, c.stream>>>(pj, nullptr, 0);
+  const int blocks = list_ctas(n1);
+  ratio_flags_kernel<<<blocks, LIST_ROWS, 0, c.stream>>>(pj, nullptr, 0, (double)ra.maxRatio, (double)ra.maxDistance);
+  mutual_write_kernel<<<blocks, LIST_ROWS, 0, c.stream>>>(pj, nullptr, 0);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
   CS_CUDA(cudaMemcpyAsync(c.h_pairTotal, pj.total, sizeof(unsigned int), cudaMemcpyDeviceToHost, c.stream));
@@ -181,8 +133,8 @@ int launch_ratio_pairs_batch(DeviceCtx &c, const PairJob *jobs, int numJobs, int
                              float maxDistance)
 {
   const PairJob none = {};
-  ratio_flags_kernel<<<numCtas, MP_ROWS, 0, c.stream>>>(none, jobs, numJobs, (double)maxRatio, (double)maxDistance);
-  mutual_write_kernel<<<numCtas, MP_ROWS, 0, c.stream>>>(none, jobs, numJobs);
+  ratio_flags_kernel<<<numCtas, LIST_ROWS, 0, c.stream>>>(none, jobs, numJobs, (double)maxRatio, (double)maxDistance);
+  mutual_write_kernel<<<numCtas, LIST_ROWS, 0, c.stream>>>(none, jobs, numJobs);
   count_launch(2);
   CS_CUDA(cudaGetLastError());
   return 0;

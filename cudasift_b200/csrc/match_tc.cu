@@ -22,6 +22,7 @@
 // (match_knn_tensor) runs the same prep and GEMM over all candidates, then the resolve's top-2 rule and the exact top-2
 // fallback (match_knn.cu); a batch wave of ratio matching runs them over a table of directions.
 #include "common.cuh"
+#include "ordered_list.cuh"
 
 #include <cuda_fp16.h>
 
@@ -955,8 +956,8 @@ static std::vector<MbWave> mb_waves(const cs_match_set *sets, int numSets, const
       v.resolveCtas += idivup(n1, 4 * T3_RW);
       v.rows += n1;
     }
-    v.words += idivup(na, 32);
-    v.pairCtas += idivup(na, 1024);                        // MP_ROWS (match_mutual.cu)
+    v.words += list_words(na);
+    v.pairCtas += list_ctas(na);
   }
   size_t pin = 0;
   for (MbWave &v : waves) {
@@ -1041,7 +1042,7 @@ static void mb_fill(DeviceCtx &c, const MbWave &v, const cs_match_set *sets, con
     pjob.pairs = reinterpret_cast<int2 *>(j.pairs); pjob.maxPairs = j.maxPairs;
     pjob.total = st + 2 * S + 4 * D + q;
     pjob.cta0 = pcta0;
-    word0 += idivup(f.n1, 32); pcta0 += idivup(f.n1, 1024);
+    word0 += list_words(f.n1); pcta0 += list_ctas(f.n1);
     RatioBatchOut &o = out[pj];
     o.total = hstate + 2 * S + 4 * D + q;
     o.counters[0] = hstate + 2 * S + 4 * dd[0];

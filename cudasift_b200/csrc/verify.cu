@@ -3,11 +3,11 @@
 // coordinates, refitted once.  The rules (validity, sampler, residuals, output order) are stated in cudasift_b200.h at
 // cs_verify_pairs; tests/verify_oracle.py restates them in float64.
 //
-// Eight launches, one host synchronisation (by the caller, after the result copy):
-//   1. flags     one thread per pair: valid (indices in range, four finite coordinates); a ballot word per 32 pairs and
-//                a count per CTA of 1024 pairs.
-//   2. compact   exclusive prefix (as mutual_write_kernel) -> the valid pairs' pixel coordinates (float4 x1 y1 x2 y2) and
-//                their input index, in input order; the last CTA writes the valid count.
+// Eight launches, one host synchronisation (by the caller, after the result copy).  The valid pairs and the inliers are
+// ordered lists of ordered_list.cuh: flags and compact build the first, refit's final mask and write the second.
+//   1. flags     one thread per pair: valid (indices in range, four finite coordinates).
+//   2. compact   the valid pairs' pixel coordinates (float4 x1 y1 x2 y2) and their input index, in input order, and the
+//                valid count.
 //   3. norm      one CTA: centroids c1, c2 and the common Hartley scale s in double, fixed-order reductions; writes the
 //                normalised FP32 coordinates and resets the arg-max key and the counters.
 //   4. hyp       one thread per sample: draws, the minimal solver in FP64, up to 3 models (slot sample*3 + root) stored
@@ -17,11 +17,11 @@
 //   7. refit     one CTA: the normal matrix of the best model's inliers (fixed-order double reduction), Jacobi, rank 2 for
 //                F, re-score, keep the refit unless it has fewer inliers; the final mask (ballot words, CTA counts), the
 //                pixel model and the statistics.
-//   8. write     exclusive prefix of the final mask -> the input pairs {i, j} of the inliers, in input order.
+//   8. write     the input pairs {i, j} of the inliers, in input order.
 //
 // Every launch verifies a wave of jobs (cs_verify_pairs_batch; a single call is a wave of one job).  A device table
 // (VerifyJob) gives each job its records, pairs, seed, inlier buffer and intrinsics, and the first CTA of its range in
-// the row kernels (1, 2, 8: one CTA per VP_ROWS pairs, each job on CTAs of its own) and among the point chunks of the
+// the row kernels (1, 2, 8: one CTA per LIST_ROWS pairs, each job on CTAs of its own) and among the point chunks of the
 // scoring kernel (grid y: the model blocks).  A CTA finds its job by binary search over those bases, built on the host.
 // Norm and refit run one CTA per job, hyp and argmax a fixed number of CTAs per job.  Per job, every kernel does what
 // it does for a single call, in the same CTA shapes and reduction orders, so a job's results do not depend on the
@@ -32,11 +32,11 @@
 #include <math_constants.h>
 
 #include "common.cuh"
+#include "ordered_list.cuh"
 #include "vp_math.cuh"
 
 namespace cs {
 
-#define VP_ROWS 1024          // pairs per CTA of the flags / compact / write kernels
 #define VP_HYP_T 128          // samples per CTA of the hypothesis kernel
 #define VP_SC_T 128           // models per CTA of the scoring kernel
 #define VP_TILE 1024          // points per shared-memory tile
@@ -232,52 +232,8 @@ __device__ __forceinline__ bool vp_inlier(const float *m, float4 p, float thr2, 
   return num * num < thr2 * den;
 }
 
-// This thread's exclusive position among the set bits of masks (one word per 32 rows, one count per CTA of VP_ROWS
-// rows), the bit itself in *bit, in CTA b of the job's nb; the job's last CTA's last warp writes the total to *total
-// when given.
-__device__ unsigned int vp_scan(const unsigned int *__restrict__ masks, const unsigned int *__restrict__ blockCounts, int n,
-                                int b, int nb, bool *bit, int *total)
-{
-  __shared__ unsigned int s_w[32];
-  __shared__ unsigned int s_base;
-  const unsigned int FULL = 0xffffffffu;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  unsigned int part = 0;
-  for (int k = threadIdx.x; k < b; k += VP_ROWS) part += blockCounts[k];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(FULL, part, o);
-  if (lane == 0) s_w[w] = part;
-  __syncthreads();
-  if (w == 0) {
-    unsigned int v = s_w[lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
-    if (lane == 0) s_base = v;
-  }
-  __syncthreads();
-  const unsigned int base = s_base;
-  const unsigned int bal = (b * VP_ROWS + w * 32 < n) ? masks[(b * VP_ROWS >> 5) + w] : 0u;
-  __syncthreads();
-  if (lane == 0) s_w[w] = __popc(bal);
-  __syncthreads();
-  if (w == 0) {
-    const unsigned int c = s_w[lane];
-    unsigned int inc = c;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int t = __shfl_up_sync(FULL, inc, o);
-      if (lane >= o) inc += t;
-    }
-    s_w[lane] = inc - c;
-    if (total && lane == 31 && b == nb - 1) *total = (int)(base + inc);
-  }
-  __syncthreads();
-  *bit = (bal >> lane) & 1u;
-  return base + s_w[w] + __popc(bal & ((1u << lane) - 1u));
-}
-
 // ---- kernels ----------------------------------------------------------------------------------------------------------
-// The scratch of a wave: per row CTA VP_ROWS / 32 mask words, one count and VP_ROWS coordinates and input indices;
+// The scratch of a wave: per row CTA LIST_ROWS / 32 mask words, one count and LIST_ROWS coordinates and input indices;
 // per job `slots` model slots, their counts and one state.
 struct VerifyWave {
   const VerifyJob *jobs;
@@ -303,11 +259,11 @@ struct VerifyJobScratch {
 __device__ __forceinline__ VerifyJobScratch vp_job_scratch(const VerifyWave &w, int j)
 {
   const size_t r = (size_t)w.jobs[j].rowBase;
-  return {w.masks + r * (VP_ROWS / 32), w.counts + r, w.xy + r * VP_ROWS, w.un + r * VP_ROWS, w.orig + r * VP_ROWS,
-          w.models + (size_t)j * w.slots * 9, w.slotCounts + (size_t)j * w.slots, w.st + j};
+  return {w.masks + r * (LIST_ROWS / 32), w.counts + r, w.xy + r * LIST_ROWS, w.un + r * LIST_ROWS,
+          w.orig + r * LIST_ROWS, w.models + (size_t)j * w.slots * 9, w.slotCounts + (size_t)j * w.slots, w.st + j};
 }
 
-__global__ void __launch_bounds__(VP_ROWS)
+__global__ void __launch_bounds__(LIST_ROWS)
 vp_flags_kernel(VerifyWave w)
 {
   const int j = table_find(w.jobs, w.numJobs, &VerifyJob::rowBase, (int)blockIdx.x);
@@ -316,20 +272,17 @@ vp_flags_kernel(VerifyWave w)
   const SiftPoint *__restrict__ s1 = job.s1, *__restrict__ s2 = job.s2;
   const int n1 = job.n1, n2 = job.n2, numPairs = job.numPairs;
   const int b = blockIdx.x - job.rowBase;
-  const int k = b * VP_ROWS + threadIdx.x;
+  const int k = b * LIST_ROWS + threadIdx.x;
   bool keep = false;
   if (k < numPairs) {
     const int2 p = job.pairs[k];
     if (p.x >= 0 && p.x < n1 && p.y >= 0 && p.y < n2)
       keep = isfinite(s1[p.x].xpos) && isfinite(s1[p.x].ypos) && isfinite(s2[p.y].xpos) && isfinite(s2[p.y].ypos);
   }
-  const unsigned int bal = __ballot_sync(0xffffffffu, keep);
-  if ((threadIdx.x & 31) == 0 && k < numPairs) js.masks[k >> 5] = bal;
-  const int cnt = __syncthreads_count(keep);
-  if (threadIdx.x == 0) js.counts[b] = (unsigned int)cnt;
+  list_flag(keep, k, numPairs, js.masks, js.counts, b);
 }
 
-__global__ void __launch_bounds__(VP_ROWS)
+__global__ void __launch_bounds__(LIST_ROWS)
 vp_compact_kernel(VerifyWave w)
 {
   const int j = table_find(w.jobs, w.numJobs, &VerifyJob::rowBase, (int)blockIdx.x);
@@ -337,10 +290,10 @@ vp_compact_kernel(VerifyWave w)
   const VerifyJobScratch js = vp_job_scratch(w, j);
   const int b = blockIdx.x - job.rowBase;
   bool bit;
-  const unsigned int pos = vp_scan(js.masks, js.counts, job.numPairs, b, (job.numPairs + VP_ROWS - 1) / VP_ROWS, &bit,
-                                   &js.st->numValid);
+  const unsigned int pos = list_position(js.masks, js.counts, job.numPairs, b, &bit,
+                                         reinterpret_cast<unsigned int *>(&js.st->numValid));
   if (bit) {
-    const int k = b * VP_ROWS + threadIdx.x;
+    const int k = b * LIST_ROWS + threadIdx.x;
     const int2 p = job.pairs[k];
     js.xy[pos] = make_float4(job.s1[p.x].xpos, job.s1[p.x].ypos, job.s2[p.y].xpos, job.s2[p.y].ypos);
     js.orig[pos] = k;
@@ -588,8 +541,8 @@ __device__ int vp_block_count(int v, int *s_cnt)
   return t;
 }
 
-// The final mask of a refit CTA: ballot words per 32 points of the FP32 test with m (all clear when m is null), then
-// counts per VP_ROWS points; returns the total in every thread.
+// The final mask of a refit CTA, in the layout of an ordered list (ordered_list.cuh): ballot words per 32 points of the
+// FP32 test with m (all clear when m is null), then counts per LIST_ROWS points; returns the total in every thread.
 __device__ int vp_final_mask(const float *m, const float4 *__restrict__ un, int n, float thr2, bool homography,
                              unsigned int *__restrict__ masks, unsigned int *__restrict__ blockCounts, int *s_cnt)
 {
@@ -602,14 +555,14 @@ __device__ int vp_final_mask(const float *m, const float4 *__restrict__ un, int 
       if (lane == 0 && k < n) masks[k >> 5] = bal;
     }
   } else {
-    for (int k = threadIdx.x; k < (n + 31) / 32; k += VP_REFIT_T) masks[k] = 0u;
+    for (int k = threadIdx.x; k < list_words(n); k += VP_REFIT_T) masks[k] = 0u;
   }
   __syncthreads();
-  const int words = (n + 31) / 32;
+  const int words = list_words(n);
   int tot = 0;
-  for (int b = threadIdx.x; b * (VP_ROWS / 32) < words; b += VP_REFIT_T) {
+  for (int b = threadIdx.x; b < list_ctas(n); b += VP_REFIT_T) {
     unsigned int t = 0;
-    for (int q = b * (VP_ROWS / 32); q < min(words, (b + 1) * (VP_ROWS / 32)); q++) t += __popc(masks[q]);
+    for (int q = b * (LIST_ROWS / 32); q < min(words, (b + 1) * (LIST_ROWS / 32)); q++) t += __popc(masks[q]);
     blockCounts[b] = t;
     tot += (int)t;
   }
@@ -647,7 +600,7 @@ __device__ void vp_smallest_eigvec(const double (*s_nm)[45], double (&f)[9])
   for (int i = 0; i < 9; i++) f[i] = V[i][lo];
 }
 
-__global__ void __launch_bounds__(VP_ROWS)
+__global__ void __launch_bounds__(LIST_ROWS)
 vp_write_kernel(VerifyWave w)
 {
   const int j = table_find(w.jobs, w.numJobs, &VerifyJob::rowBase, (int)blockIdx.x);
@@ -655,10 +608,10 @@ vp_write_kernel(VerifyWave w)
   const VerifyJobScratch js = vp_job_scratch(w, j);
   const int b = blockIdx.x - job.rowBase;
   const int n = js.st->numValid;
-  if (b * VP_ROWS >= n) return;                     // the whole CTA: no thread reaches the scan's barriers
+  if (b * LIST_ROWS >= n) return;                   // the whole CTA: no thread reaches the scan's barriers
   bool bit;
-  const unsigned int pos = vp_scan(js.masks, js.counts, n, b, 0, &bit, nullptr);
-  if (bit && pos < (unsigned int)job.maxInliers) job.inliers[pos] = job.pairs[js.orig[b * VP_ROWS + threadIdx.x]];
+  const unsigned int pos = list_position(js.masks, js.counts, n, b, &bit, nullptr);
+  if (bit && pos < (unsigned int)job.maxInliers) job.inliers[pos] = job.pairs[js.orig[b * LIST_ROWS + threadIdx.x]];
 }
 
 // ---- the calibrated path (cs_verify_essential) -------------------------------------------------------------------------
@@ -1299,7 +1252,7 @@ static int vp_slots_per_sample(int model) { return model == VERIFY_ESSENTIAL ? V
 static WavePlan verify_plan(const cs_verify_job *jobs, int numJobs, int numLoops, int model)
 {
   const size_t slotBytes = (size_t)vp_slots_per_sample(model) * numLoops * (9 * sizeof(double) + sizeof(unsigned int));
-  return wave_plan(jobs, numJobs, slotBytes, [](const cs_verify_job &a) { return (size_t)idivup(a.numPairs, VP_ROWS); });
+  return wave_plan(jobs, numJobs, slotBytes, [](const cs_verify_job &a) { return (size_t)list_ctas(a.numPairs); });
 }
 
 struct VerifyLayout {
@@ -1312,10 +1265,10 @@ static VerifyLayout verify_layout(const WavePlan &p, int numLoops, int model)
   VerifyLayout L;
   Layout o(256);
   const size_t live = std::max(p.live.size(), (size_t)1), J = std::min(live, (size_t)p.perWave);
-  const size_t P = std::max(p.extent, (size_t)1) * VP_ROWS, S = vp_slots_per_sample(model) * (size_t)numLoops * J;
+  const size_t P = std::max(p.extent, (size_t)1) * LIST_ROWS, S = vp_slots_per_sample(model) * (size_t)numLoops * J;
   L.jobs = o.take(live * sizeof(VerifyJob));
   L.masks = o.take(P / 32 * sizeof(unsigned int));
-  L.counts = o.take(P / VP_ROWS * sizeof(unsigned int));
+  L.counts = o.take(P / LIST_ROWS * sizeof(unsigned int));
   L.xy = o.take(P * sizeof(float4));
   L.un = o.take(P * sizeof(float4));
   L.orig = o.take(P * sizeof(int));
@@ -1359,7 +1312,7 @@ int verify_enqueue(DeviceCtx &c, const cs_verify_job *jobs, int numJobs, const V
     t.rowBase = rowBase;
     t.scoreBase = scoreBase;
     t.cal = cal ? cal[plan.live[q]] : VerifyCalib{};
-    rowBase += idivup(a.numPairs, VP_ROWS);
+    rowBase += list_ctas(a.numPairs);
     scoreBase += idivup(a.numPairs, VP_CHUNK);
   }
   VerifyJob *d_jobs = reinterpret_cast<VerifyJob *>(b + L.jobs);
@@ -1381,14 +1334,14 @@ int verify_enqueue(DeviceCtx &c, const cs_verify_job *jobs, int numJobs, const V
   for (int q0 = 0; q0 < live; q0 += plan.perWave) {
     const int nj = std::min(plan.perWave, live - q0);
     const VerifyJob &last = h_jobs[q0 + nj - 1];
-    const int rows = last.rowBase + idivup(last.numPairs, VP_ROWS);
+    const int rows = last.rowBase + list_ctas(last.numPairs);
     const int chunks = last.scoreBase + idivup(last.numPairs, VP_CHUNK);
     w.jobs = d_jobs + q0;
     w.numJobs = nj;
     if (tev) cudaEventRecord(tev[0], st);
-    vp_flags_kernel<<<rows, VP_ROWS, 0, st>>>(w);
+    vp_flags_kernel<<<rows, LIST_ROWS, 0, st>>>(w);
     if (tev) cudaEventRecord(tev[1], st);
-    vp_compact_kernel<<<rows, VP_ROWS, 0, st>>>(w);
+    vp_compact_kernel<<<rows, LIST_ROWS, 0, st>>>(w);
     if (tev) cudaEventRecord(tev[2], st);
     vp_norm_kernel<<<nj, 1024, 0, st>>>(w, thresh);
     if (tev) cudaEventRecord(tev[3], st);
@@ -1408,7 +1361,7 @@ int verify_enqueue(DeviceCtx &c, const cs_verify_job *jobs, int numJobs, const V
       else
         vp_refit_kernel<false><<<nj, VP_REFIT_T, 0, st>>>(w, model);
       if (tev) cudaEventRecord(tev[7], st);
-      vp_write_kernel<<<rows, VP_ROWS, 0, st>>>(w);
+      vp_write_kernel<<<rows, LIST_ROWS, 0, st>>>(w);
       if (tev) cudaEventRecord(tev[8], st);
       count_launch(3);
     }
