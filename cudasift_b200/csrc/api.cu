@@ -180,6 +180,7 @@ static int extract_sync(const float *d_img, int w, int h, int pitch, int numOcta
                         SiftPoint *h_pts, int maxPts, double *msKernel)
 {
   int err = 0;
+  if ((err = check_level0_size("ExtractSift", w, h, scaleUp)) < 0) return err;
   if (!d_img || !d_pts || maxPts < 1) { set_error("ExtractSift: missing image or SiftData"); return CS_E_ARG; }
   if ((reinterpret_cast<uintptr_t>(d_tmp) & 15) != 0) {   // the level textures and tensor maps start in it
     set_error("ExtractSift: tempMemory %p must be 16-byte aligned", (void *)d_tmp);
@@ -872,6 +873,7 @@ int cs_extract_host(const float *h_img, int w, int h, int numOctaves, double ini
                     float lowestScale, int scaleUp, void *h_pts, int maxPts)
 {
   int err = 0;
+  if ((err = check_level0_size("ExtractSift", w, h, scaleUp != 0)) < 0) return err;
   DeviceCtx *c = current_ctx(&err);
   if (!c) return err;
   int pitch = ialignup(w, 128);
@@ -1871,6 +1873,7 @@ static int extractor_capture(cs_extractor *ex, int n, const float *const *d_imgs
 static cs_extractor *extractor_create(int w, int h, int numOctaves, int maxPts, int scaleUp, int batch, int maxCand)
 {
   if (batch < 1 || batch > CS_MAX_BATCH) { set_error("cs_extractor_create_batch: batch %d out of range (1..%d)", batch, CS_MAX_BATCH); return nullptr; }
+  if (check_level0_size("cs_extractor_create", w, h, scaleUp != 0) < 0) return nullptr;
   cs_extractor *ex = new cs_extractor();
   ex->w = w; ex->h = h; ex->numOctaves = numOctaves; ex->maxPts = maxPts; ex->scaleUp = scaleUp; ex->B = batch;
   ex->pitch = ialignup(w, 128);

@@ -196,6 +196,9 @@ int launch_detect2(const Detect2Params &p, int sms, cudaStream_t st);
 int detect2_init_device();   // fills the device-side pow table (once per device; not inside a stream capture)
 int launch_cap32_fixup(const Detect2Params &p, int batch, cudaStream_t st);
 #define CS_D2_STRIP 244       // tested columns per detector strip (multiple of 4: TMA box alignment)
+// Widest and tallest level 0 (after scaleUp) the detector takes: an extremum's tag (detect2.cu, cap32.cu) packs gx and gy
+// into 13 bits each, and interior pixels reach w - 2 and h - 2.
+#define CS_MAX_LEVEL0 8193
 
 // ---- orientation + descriptor ---------------------------------------------------------
 struct DescribeParams {

@@ -95,8 +95,20 @@ static int debug_stage(cudaStream_t st, const char *name)
 }
 
 // ------------------------------------------------------------------------------ Pipeline
+int check_level0_size(const char *who, int w, int h, bool up)
+{
+  const long long W = (long long)w * (up ? 2 : 1), H = (long long)h * (up ? 2 : 1);
+  if (W > CS_MAX_LEVEL0 || H > CS_MAX_LEVEL0) {
+    set_error("%s: invalid argument (CS_E_ARG): level 0 of %lldx%lld exceeds the detector's size limit of %d pixels "
+              "(CS_MAX_LEVEL0: 13-bit extremum positions)", who, W, H, CS_MAX_LEVEL0);
+    return CS_E_ARG;
+  }
+  return 0;
+}
+
 int Pipeline::init(int w, int h, int octaves, bool up, int maxBatch, float *arenaPtr)
 {
+  { int r0 = check_level0_size("ExtractSift", w, h, up); if (r0 < 0) return r0; }
   if (w < 1 || h < 1 || octaves < 1 || octaves > 7) {   // quirk Q17: taps table holds octave <= 7
     set_error("ExtractSift: invalid size %dx%d or numOctaves %d (1..7)", w, h, octaves);
     return CS_E_ARG;

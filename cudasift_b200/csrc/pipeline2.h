@@ -54,6 +54,8 @@ struct Pipeline {
                      int maxPts, cudaStream_t st, cudaEvent_t *ev = nullptr);
 };
 
+// CS_E_ARG, naming `who`, when level 0 (w x h, doubled by scaleUp) is larger than CS_MAX_LEVEL0; no CUDA call.
+int check_level0_size(const char *who, int w, int h, bool up);
 void build_detector_items(const int *lw, const int *lh, int numLevels, int n, int hs, std::vector<uint4> &v);
 extern int g_d2_hs, g_pa_rows, g_cap32, g_cap_limit, g_sd_split;
 

@@ -60,7 +60,10 @@ size_t cs_temp_floats(int width, int height, int numOctaves, int scaleUp);
 /* ExtractSift (cudaSiftH.cu:72-144) on a device-resident float image (row stride
  * `pitch` floats).  d_pts: device array of maxPts records (required).  h_pts: optional
  * host array that receives the first numPts records.  d_tmp: optional arena from
- * cs_alloc_temp (NULL = internal, cached).  Returns numPts. */
+ * cs_alloc_temp (NULL = internal, cached).  Returns numPts.  CS_E_ARG, before any CUDA call,
+ * when level 0 (width x height, doubled by scaleUp) is wider or taller than 8193 px: an extremum's
+ * position is kept in 13-bit fields.  The same limit holds for cs_extract_host and every
+ * cs_extractor_create_*. */
 int cs_extract(const float *d_img, int width, int height, int pitch, int numOctaves,
                double initBlur, float thresh, float lowestScale, int scaleUp,
                float *d_tmp, void *d_pts, void *h_pts, int maxPts);
