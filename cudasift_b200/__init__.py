@@ -22,7 +22,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "VerifyPairsBatch", "VerifyEssentialBatch", "MatchSet", "MatchJob", "MatchSiftDataRatioBatch",
            "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
-           "RetrievePairs", "RotationAveraging", "GlobalPositioning"]
+           "RetrievePairs", "RotationAveraging", "GlobalPositioning", "UndistortImages", "PatchMatchStereo",
+           "FuseDepthMaps", "SelectStereoViews"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -109,6 +110,11 @@ def lib():
                                        c.c_double, vp, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_rotation_averaging": (ip, [ip, vp, ip, vp, vp, ip, ip, ip, c.c_double, c.c_double, c.c_double, vp, vp, vp,
                                        vp, vp, vp, vp]),
+        "cs_undistort_images": (ip, [vp, ip, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_patch_match_stereo": (ip, [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, ip, c.c_ulonglong, vp,
+                                       c.POINTER(c.c_double)]),
+        "cs_fuse_depth_maps": (ip, [vp, ip, vp, vp, vp, vp, ip, fp, ip, c.c_double, c.c_double, c.c_double, vp, vp, vp,
+                                    vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1114,6 +1120,204 @@ def GlobalPositioning(datas, Ks, Rs, offsets, members, use=None, refImage=0, see
         for buf in bufs:
             buf.free()
     return t, points, (cost[0], cost[1]), trace[:int(stats[6])].copy(), stats, ms.value
+
+
+class StereoImage(ctypes.Structure):
+    """cs_image: a device float32 grayscale image, pitch in floats."""
+    _fields_ = [("d_img", ctypes.c_void_p), ("width", ctypes.c_int), ("height", ctypes.c_int), ("pitch", ctypes.c_int)]
+
+
+class StereoJob(ctypes.Structure):
+    """cs_stereo_job: one depth map of image ref from its source images (a host array)."""
+    _fields_ = [("ref", ctypes.c_int), ("sources", ctypes.c_void_p), ("numSources", ctypes.c_int),
+                ("depthMin", ctypes.c_float), ("depthMax", ctypes.c_float), ("d_depth", ctypes.c_void_p),
+                ("d_normal", ctypes.c_void_p), ("d_cost", ctypes.c_void_p)]
+
+
+def _upload_images(images):
+    """Host float32 [H, W] images in dense device buffers, and their cs_image table."""
+    arrs = [np.ascontiguousarray(im, np.float32) for im in images]
+    for im in arrs:
+        if im.ndim != 2:
+            raise ValueError("images: 2-D float32 arrays, not shape %s" % (im.shape,))
+    bufs = []
+    try:
+        for im in arrs:
+            b = DeviceBuffer(max(im.nbytes, 4))
+            bufs.append(b)
+            b.upload(im)
+    except BaseException:
+        for b in bufs:
+            b.free()
+        raise
+    table = (StereoImage * max(len(arrs), 1))(*[StereoImage(b.ptr, im.shape[1], im.shape[0], im.shape[1])
+                                               for b, im in zip(bufs, arrs)])
+    return arrs, bufs, table
+
+
+def _stereo_jobs(jobs, shapes, maps):
+    """jobs as (ref, sources, depthMin, depthMax) tuples and their cs_stereo_job table, each with its three maps:
+    maps(shape) returns three device buffers (depth, normal, cost), or None to pass the jobs' existing maps."""
+    parsed = []
+    for ref, sources, dmin, dmax in jobs:
+        src = np.ascontiguousarray(np.asarray(sources, np.int64).reshape(-1).astype(np.int32))
+        parsed.append((int(ref), src, float(dmin), float(dmax)))
+    table = (StereoJob * max(len(parsed), 1))()
+    bufs = []
+    for p, (ref, src, dmin, dmax) in enumerate(parsed):
+        if not 0 <= ref < len(shapes):
+            raise ValueError("jobs[%d]: ref %d is not an image" % (p, ref))
+        m = maps(p, shapes[ref])
+        bufs.append(m)
+        table[p] = StereoJob(ref, src.ctypes.data if len(src) else None, len(src), dmin, dmax,
+                             *[b.ptr for b in m])
+    return parsed, table, bufs
+
+
+def UndistortImages(images, Ks, dists):
+    """Every image as the pinhole camera K would see it (cs_undistort_images): each output pixel sampled bilinearly
+    from the input at its position under the radial model (k1, k2) of BundleAdjustIntrinsics, 0 outside the input.
+    images are float32 [H, W] host arrays on any scale (the output keeps it; PatchMatchStereo expects grey levels
+    0..255); Ks [3, 3] and dists [2] per image or one for every image.  Returns (undistorted float32 [H, W] list,
+    outside counts int64 [S], ms)."""
+    S = len(images)
+    K, dist = _per_image(Ks, (3, 3), S, "Ks"), _per_image(dists, (2,), S, "dists")
+    arrs, bufs, table = _upload_images(images)
+    outs = []
+    try:
+        for im in arrs:
+            outs.append(DeviceBuffer(max(im.nbytes, 4)))
+        ptrs = (ctypes.c_void_p * max(S, 1))(*[o.ptr for o in outs])
+        outside, ms = np.zeros(S, np.int64), ctypes.c_double(0.0)
+        _check(lib().cs_undistort_images(table if S else None, S, _ptr(K) if S else None, _ptr(dist) if S else None,
+                                         ptrs if S else None, _ptr(outside) if S else None, ctypes.byref(ms)),
+               "UndistortImages")
+        res = [o.download(np.float32, im.size).reshape(im.shape) for o, im in zip(outs, arrs)]
+    finally:
+        for b in bufs + outs:
+            b.free()
+    return res, outside, ms.value
+
+
+def PatchMatchStereo(images, Ks, Rs, ts, jobs, windowRadius=5, windowStep=1, numIterations=5, topK=3, seed=0):
+    """A depth, normal and cost map for every job in one call (cs_patch_match_stereo): PatchMatch stereo with red-black
+    propagation, the cost the mean of the topK smallest 1 - NCC view costs.  images are float32 [H, W] host arrays
+    of grey levels on a 0..255 scale (pinhole: UndistortImages first): a window whose variance is below 1 grey
+    level^2 makes its view invalid, so images scaled to [0, 1] leave every cost at 2.  Ks, Rs, ts per image (X_c = R X + t), jobs (ref, sources, depthMin, depthMax)
+    tuples as SelectStereoViews returns them.  Returns (depth [J] of float32 [H, W], normal [J] of float32 [H, W, 3]
+    in the ref camera frame, cost [J] of float32 [H, W] (2: unsupported), stats int64 [J, 3] of {pixels, invalid view
+    evaluations, pixels of cost 2}, ms)."""
+    S = len(images)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    arrs, bufs, table = _upload_images(images)
+    shapes = [im.shape for im in arrs]
+    maps = []
+    try:
+        parsed, jt, maps = _stereo_jobs(jobs, shapes, lambda p, sh: [DeviceBuffer(4 * sh[0] * sh[1]),
+                                                                     DeviceBuffer(12 * sh[0] * sh[1]),
+                                                                     DeviceBuffer(4 * sh[0] * sh[1])])
+        J = len(parsed)
+        stats, ms = np.zeros((J, 3), np.int64), ctypes.c_double(0.0)
+        _check(lib().cs_patch_match_stereo(table if S else None, S, _ptr(K), _ptr(R), _ptr(t), jt if J else None, J,
+                                           int(windowRadius), int(windowStep), int(numIterations), int(topK),
+                                           int(seed), _ptr(stats) if J else None, ctypes.byref(ms)),
+               "PatchMatchStereo")
+        depth, normal, cost = [], [], []
+        for (ref, _, _, _), m in zip(parsed, maps):
+            h, w = shapes[ref]
+            depth.append(m[0].download(np.float32, h * w).reshape(h, w))
+            normal.append(m[1].download(np.float32, 3 * h * w).reshape(h, w, 3))
+            cost.append(m[2].download(np.float32, h * w).reshape(h, w))
+    finally:
+        for b in bufs + [b for m in maps for b in m]:
+            b.free()
+    return depth, normal, cost, stats, ms.value
+
+
+def FuseDepthMaps(images, Ks, Rs, ts, jobs, depth, normal, cost, maxCost=0.5, minConsistent=2, maxReprojError=2.0,
+                  maxDepthError=0.01, maxNormalErrorDeg=10.0, maxPoints=None):
+    """One point cloud from the maps of PatchMatchStereo (cs_fuse_depth_maps): a pixel with cost <= maxCost emits a
+    point when at least minConsistent of its sources that are themselves refs agree in depth (relative
+    maxDepthError), normal (maxNormalErrorDeg degrees) and reprojection (maxReprojError px), and none of them has a
+    lower image index.  Arguments as for PatchMatchStereo plus its maps; maxPoints None: room for every pixel.  Returns
+    (xyz float32 [P, 3], normal float32 [P, 3], intensity float32 [P], source int32 [P, 2] of {image, y W + x} in
+    ascending order, total (the full count, >= P), ms)."""
+    S = len(images)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    if not (len(depth) == len(normal) == len(cost) == len(jobs)):
+        raise ValueError("depth, normal and cost: one map per job")
+    arrs, bufs, table = _upload_images(images)
+    shapes = [im.shape for im in arrs]
+    maps = []
+    try:
+        def upload(p, sh):
+            m = [DeviceBuffer(4 * sh[0] * sh[1]), DeviceBuffer(12 * sh[0] * sh[1]), DeviceBuffer(4 * sh[0] * sh[1])]
+            for b, a in zip(m, (depth[p], normal[p], cost[p])):
+                b.upload(np.ascontiguousarray(a, np.float32))
+            return m
+        parsed, jt, maps = _stereo_jobs(jobs, shapes, upload)
+        J = len(parsed)
+        room = sum(shapes[ref][0] * shapes[ref][1] for ref, _, _, _ in parsed) if maxPoints is None else int(maxPoints)
+        outs = [DeviceBuffer(max(12 * room, 4)), DeviceBuffer(max(12 * room, 4)), DeviceBuffer(max(4 * room, 4)),
+                DeviceBuffer(max(8 * room, 8))]
+        bufs += outs
+        stats, ms = np.zeros(2, np.int64), ctypes.c_double(0.0)
+        n = _check(lib().cs_fuse_depth_maps(table if S else None, S, _ptr(K), _ptr(R), _ptr(t), jt if J else None, J,
+                                            float(maxCost), int(minConsistent), float(maxReprojError),
+                                            float(maxDepthError), float(maxNormalErrorDeg),
+                                            *[o.ptr if room else None for o in outs], room, _ptr(stats),
+                                            ctypes.byref(ms)), "FuseDepthMaps")
+        P = int(stats[1])
+        xyz = outs[0].download(np.float32, 3 * P).reshape(P, 3)
+        nrm = outs[1].download(np.float32, 3 * P).reshape(P, 3)
+        inten = outs[2].download(np.float32, P)
+        src = outs[3].download(np.int32, 2 * P).reshape(P, 2)
+    finally:
+        for b in bufs + [b for m in maps for b in m]:
+            b.free()
+    return xyz, nrm, inten, src, n, ms.value
+
+
+def SelectStereoViews(Ks, Rs, ts, offsets, members, points, numSources=8, minTriAngle=1.0):
+    """The stereo jobs of a sparse model (host, numpy): for every image a, the numSources images that share the most
+    tracks with a finite point whose triangulation angle between the two images' rays is >= minTriAngle degrees (ties
+    to the lower index, count > 0), and the depth range [0.75 p1, 1.25 p99] of the depths of a's observed points
+    (COLMAP's rule).  offsets and members are BuildTracks' outputs, points TriangulateTracks'.  An image without such a
+    point or without a source gets no job.  Returns a list of (ref, sources int32 array, depthMin, depthMax)."""
+    S = len(np.asarray(Rs, np.float64).reshape(-1, 3, 3))
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    off, mem, T, M = _tracks(offsets, members)
+    X = np.asarray(points, np.float64).reshape(-1, 3)
+    C = -np.einsum("aji,aj->ai", R, t)                      # camera centres
+    shared = np.zeros((S, S), np.int64)
+    depths = [[] for _ in range(S)]
+    cosMin = np.cos(np.radians(float(minTriAngle)))
+    for k in range(T):
+        if not np.all(np.isfinite(X[k])):
+            continue
+        imgs = np.unique(mem[off[k]:off[k + 1], 0])
+        imgs = imgs[(imgs >= 0) & (imgs < S)]
+        for a in imgs:
+            z = R[a, 2] @ X[k] + t[a, 2]
+            if z > 0:
+                depths[a].append(z)
+        rays = X[k] - C[imgs]
+        rays /= np.linalg.norm(rays, axis=1, keepdims=True)
+        cos = np.clip(rays @ rays.T, -1.0, 1.0)
+        ok = cos <= cosMin
+        np.fill_diagonal(ok, False)
+        shared[np.ix_(imgs, imgs)] += ok
+    jobs = []
+    for a in range(S):
+        if not depths[a]:
+            continue
+        order = sorted((b for b in range(S) if b != a and shared[a, b] > 0), key=lambda b: (-shared[a, b], b))
+        if not order:
+            continue
+        d = np.asarray(depths[a])
+        jobs.append((a, np.array(order[:int(numSources)], np.int32), 0.75 * np.percentile(d, 1),
+                     1.25 * np.percentile(d, 99)))
+    return jobs
 
 
 class PoseJob(ctypes.Structure):

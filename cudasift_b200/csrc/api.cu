@@ -1608,6 +1608,81 @@ int cs_global_positioning(const cs_match_set *sets, int numImages, const double 
   return globalpos_result(*c, numImages, Rs, maxIterations, t_out, cost_out, trace_out, stats_out);
 }
 
+int cs_undistort_images(const cs_image *images, int numImages, const double *Ks, const double *dists,
+                        float *const *d_out, long long *outside_out, double *ms)
+{
+  const char *fn = "cs_undistort_images";
+  if (ms) *ms = 0.0;
+  int r = undistort_images_args(fn, images, numImages, Ks, dists, d_out);
+  if (r < 0 || numImages == 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const unsigned long long *outside = nullptr;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return undistort_images_enqueue(*c, images, numImages, Ks, dists, d_out, &outside);
+       })) < 0)
+    return r;
+  for (int a = 0; outside_out && a < numImages; a++) outside_out[a] = (long long)outside[a];
+  return 0;
+}
+
+int cs_patch_match_stereo(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                          const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep, int numIterations,
+                          int topK, unsigned long long seed, long long *stats_out, double *ms)
+{
+  const char *fn = "cs_patch_match_stereo";
+  if (ms) *ms = 0.0;
+  int r = patch_match_args(fn, images, numImages, Ks, Rs, ts, jobs, numJobs, windowRadius, windowStep, numIterations,
+                           topK);
+  if (r < 0 || numJobs == 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const unsigned long long *counts = nullptr;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return patch_match_enqueue(*c, images, numImages, Ks, Rs, ts, jobs, numJobs, windowRadius, windowStep,
+                                    numIterations, topK, seed, &counts);
+       })) < 0)
+    return r;
+  for (int p = 0; stats_out && p < numJobs; p++) {
+    const cs_image &I = images[jobs[p].ref];
+    stats_out[3 * (size_t)p] = (long long)I.width * I.height;
+    stats_out[3 * (size_t)p + 1] = (long long)counts[3 * (size_t)p + 1];
+    stats_out[3 * (size_t)p + 2] = (long long)counts[3 * (size_t)p + 2];
+  }
+  return 0;
+}
+
+int cs_fuse_depth_maps(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                       const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent, double maxReprojError,
+                       double maxDepthError, double maxNormalErrorDeg, float *d_xyz, float *d_normal,
+                       float *d_intensity, int *d_source, int maxPoints, long long stats_out[2], double *ms)
+{
+  const char *fn = "cs_fuse_depth_maps";
+  if (ms) *ms = 0.0;
+  if (stats_out) stats_out[0] = stats_out[1] = 0;
+  int r = fuse_args(fn, images, numImages, Ks, Rs, ts, jobs, numJobs, maxCost, minConsistent, maxReprojError,
+                    maxDepthError, maxNormalErrorDeg, d_xyz, d_normal, d_intensity, d_source, maxPoints);
+  if (r < 0 || numJobs == 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  unsigned int *total = nullptr;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return fuse_enqueue(*c, images, numImages, Ks, Rs, ts, jobs, numJobs, maxCost, minConsistent,
+                             maxReprojError, maxDepthError, maxNormalErrorDeg, d_xyz, d_normal, d_intensity, d_source,
+                             maxPoints, &total);
+       })) < 0)
+    return r;
+  const int n = (int)*total;
+  if (stats_out) {
+    stats_out[0] = n;
+    stats_out[1] = std::min(n, maxPoints);
+  }
+  return n;
+}
+
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,
                            const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
                            int *counts_out, long long *stats_out, double *ms)

@@ -8,6 +8,7 @@
 #include <cmath>
 #include <cstdarg>
 #include <memory>
+#include <vector>
 
 namespace cs {
 
@@ -752,6 +753,172 @@ int pose_args(const char *fn, const double *points, int numPoints, const cs_pose
     rs.add(j.pointOf, (size_t)j.n * sizeof(int), 3, p, false);
   }
   rs.add(points, (size_t)numPoints * 3 * sizeof(double), 4, 0, false);
+  return rs.check(fn);
+}
+
+// ---- dense reconstruction -------------------------------------------------------------------------------------------
+
+// The bytes an image's rows span.
+static size_t image_bytes(const cs_image &I) { return ((size_t)(I.height - 1) * I.pitch + I.width) * sizeof(float); }
+
+// The images and cameras of the dense calls (Rs and ts only with poses): numImages in [lo, 65536].
+static int stereo_images(const char *fn, const cs_image *images, int numImages, int lo, const double *Ks,
+                         const double *Rs, const double *ts, bool poses)
+{
+  if (numImages < lo || numImages > 65536) return arg_error(fn, "numImages must be in [%d, 65536]", lo);
+  if (numImages > 0 && (!images || !Ks || (poses && (!Rs || !ts))))
+    return arg_error(fn, poses ? "images, Ks, Rs and ts must not be NULL" : "images and Ks must not be NULL");
+  for (int a = 0; a < numImages; a++) {
+    const cs_image &I = images[a];
+    if (!I.d_img || misaligned(I.d_img, 4)) return arg_error(fn, "images[%d].d_img must be a 4-byte aligned pointer", a);
+    if (I.width < 2 || I.width > 4096 || I.height < 2 || I.height > 4096)
+      return arg_error(fn, "images[%d]: width and height must be in [2, 4096]", a);
+    if (I.pitch < I.width) return arg_error(fn, "images[%d]: pitch must be >= width", a);
+    char name[32];
+    snprintf(name, sizeof name, "Ks[%d]", a);
+    int r;
+    if ((r = check_intrinsics(fn, Ks + 9 * (size_t)a, name)) < 0) return r;
+    if (!poses) continue;
+    const double *R = Rs + 9 * (size_t)a, *t = ts + 3 * (size_t)a;
+    bool ok = true;
+    for (int k = 0; k < 9; k++) ok = ok && std::isfinite(R[k]);
+    for (int i = 0; i < 3 && ok; i++)
+      for (int j = 0; j < 3; j++) {
+        const double d = R[3 * i] * R[3 * j] + R[3 * i + 1] * R[3 * j + 1] + R[3 * i + 2] * R[3 * j + 2];
+        ok = ok && std::fabs(d - (i == j ? 1.0 : 0.0)) <= 1e-6;
+      }
+    const double det = R[0] * (R[4] * R[8] - R[5] * R[7]) - R[1] * (R[3] * R[8] - R[5] * R[6]) +
+                       R[2] * (R[3] * R[7] - R[4] * R[6]);
+    if (!ok || !(det > 0.0)) return arg_error(fn, "Rs[%d] must be a rotation (R R^T = I within 1e-6, det R > 0)", a);
+    if (!std::isfinite(t[0]) || !std::isfinite(t[1]) || !std::isfinite(t[2]))
+      return arg_error(fn, "ts[%d] must be finite", a);
+  }
+  return 0;
+}
+
+int undistort_images_args(const char *fn, const cs_image *images, int numImages, const double *Ks,
+                          const double *dists, float *const *d_out)
+{
+  int r;
+  if ((r = stereo_images(fn, images, numImages, 0, Ks, nullptr, nullptr, false)) < 0) return r;
+  if (numImages > 0 && !d_out) return arg_error(fn, "numImages > 0 needs d_out");
+  for (int a = 0; a < numImages; a++) {
+    if (dists && (!std::isfinite(dists[2 * (size_t)a]) || !std::isfinite(dists[2 * (size_t)a + 1])))
+      return arg_error(fn, "dists[%d] must be finite", a);
+    if (!d_out[a] || misaligned(d_out[a], 4)) return arg_error(fn, "d_out[%d] must be a 4-byte aligned pointer", a);
+  }
+  // the outputs (written) and the images (read)
+  static const char *const names[2] = {"d_out[%d]", "images[%d].d_img"};
+  ArgRanges rs(names, 2 * (size_t)numImages);
+  for (int a = 0; a < numImages; a++) {
+    rs.add(d_out[a], (size_t)images[a].width * images[a].height * sizeof(float), 0, a, true);
+    rs.add(images[a].d_img, image_bytes(images[a]), 1, a, false);
+  }
+  return rs.check(fn);
+}
+
+// The jobs of the dense calls (topK checked when > 0); *pixels receives the pixels of all jobs.
+static int stereo_jobs(const char *fn, int numImages, const cs_image *images, const cs_stereo_job *jobs, int numJobs,
+                       int topK, long long *pixels)
+{
+  if (numJobs < 0 || numJobs > 65536) return arg_error(fn, "numJobs must be in [0, 65536]");
+  if (numJobs > 0 && !jobs) return arg_error(fn, "numJobs > 0 needs jobs");
+  std::vector<int> refOf(numImages, -1);
+  long long n = 0;
+  for (int p = 0; p < numJobs; p++) {
+    const cs_stereo_job &J = jobs[p];
+    if (J.ref < 0 || J.ref >= numImages) return arg_error(fn, "jobs[%d]: ref must be in [0, numImages)", p);
+    if (refOf[J.ref] >= 0) return arg_error(fn, "jobs[%d]: image %d is already the ref of jobs[%d]", p, J.ref, refOf[J.ref]);
+    refOf[J.ref] = p;
+    if (J.numSources < 1 || J.numSources > 32) return arg_error(fn, "jobs[%d]: numSources must be in [1, 32]", p);
+    if (!J.sources) return arg_error(fn, "jobs[%d]: sources must not be NULL", p);
+    for (int s = 0; s < J.numSources; s++) {
+      const int b = J.sources[s];
+      if (b < 0 || b >= numImages || b == J.ref)
+        return arg_error(fn, "jobs[%d]: sources[%d] must be in [0, numImages) and not ref", p, s);
+      for (int u = 0; u < s; u++)
+        if (J.sources[u] == b) return arg_error(fn, "jobs[%d]: sources[%d] repeats sources[%d]", p, s, u);
+    }
+    if (topK > 0 && topK > J.numSources) return arg_error(fn, "jobs[%d]: topK must be in [1, numSources]", p);
+    if (!std::isfinite(J.depthMin) || !std::isfinite(J.depthMax) || !(J.depthMin > 0.0f) ||
+        !(J.depthMin < J.depthMax))
+      return arg_error(fn, "jobs[%d]: depthMin and depthMax must be finite with 0 < depthMin < depthMax", p);
+    if (!J.d_depth || !J.d_normal || !J.d_cost || misaligned(J.d_depth, 4) || misaligned(J.d_normal, 4) ||
+        misaligned(J.d_cost, 4))
+      return arg_error(fn, "jobs[%d]: d_depth, d_normal and d_cost must be 4-byte aligned pointers", p);
+    n += (long long)images[J.ref].width * images[J.ref].height;
+  }
+  *pixels = n;
+  return 0;
+}
+
+// The maps (kinds 0..2, written when mapsWritten) and the images (kind 3) of a dense call.
+static void stereo_ranges(ArgRanges &rs, const cs_image *images, int numImages, const cs_stereo_job *jobs,
+                          int numJobs, bool mapsWritten, int kind0)
+{
+  for (int p = 0; p < numJobs; p++) {
+    const cs_image &I = images[jobs[p].ref];
+    const size_t px = (size_t)I.width * I.height * sizeof(float);
+    rs.add(jobs[p].d_depth, px, kind0, p, mapsWritten);
+    rs.add(jobs[p].d_normal, 3 * px, kind0 + 1, p, mapsWritten);
+    rs.add(jobs[p].d_cost, px, kind0 + 2, p, mapsWritten);
+  }
+  for (int a = 0; a < numImages; a++) rs.add(images[a].d_img, image_bytes(images[a]), kind0 + 3, a, false);
+}
+
+int patch_match_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                     const double *ts, const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
+                     int numIterations, int topK)
+{
+  int r;
+  if ((r = stereo_images(fn, images, numImages, 1, Ks, Rs, ts, true)) < 0) return r;
+  if (windowRadius < 1 || windowRadius > 7) return arg_error(fn, "windowRadius must be in [1, 7]");
+  if (windowStep < 1 || windowStep > windowRadius || windowRadius % windowStep != 0)
+    return arg_error(fn, "windowStep must be in [1, windowRadius] and divide windowRadius");
+  if (numIterations < 0 || numIterations > 32) return arg_error(fn, "numIterations must be in [0, 32]");
+  if (topK < 1) return arg_error(fn, "topK must be in [1, numSources]");
+  long long pixels = 0;
+  if ((r = stereo_jobs(fn, numImages, images, jobs, numJobs, topK, &pixels)) < 0) return r;
+  static const char *const names[4] = {"jobs[%d].d_depth", "jobs[%d].d_normal", "jobs[%d].d_cost",
+                                       "images[%d].d_img"};
+  ArgRanges rs(names, 3 * (size_t)numJobs + numImages);
+  stereo_ranges(rs, images, numImages, jobs, numJobs, true, 0);
+  return rs.check(fn);
+}
+
+int fuse_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+              const double *ts, const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent,
+              double maxReprojError, double maxDepthError, double maxNormalErrorDeg, const float *xyz,
+              const float *normal, const float *intensity, const int *source, int maxPoints)
+{
+  int r;
+  if ((r = stereo_images(fn, images, numImages, 1, Ks, Rs, ts, true)) < 0) return r;
+  long long pixels = 0;
+  if ((r = stereo_jobs(fn, numImages, images, jobs, numJobs, 0, &pixels)) < 0) return r;
+  if (pixels > INT_MAX) return arg_error(fn, "the pixels of all jobs must be at most 2^31 - 1");
+  if (!(maxCost >= 0.0f && maxCost <= 2.0f)) return arg_error(fn, "maxCost must be in [0, 2]");
+  if (minConsistent < 1 || minConsistent > 32) return arg_error(fn, "minConsistent must be in [1, 32]");
+  if (!std::isfinite(maxReprojError) || !(maxReprojError > 0.0))
+    return arg_error(fn, "maxReprojError must be finite and > 0");
+  if (!std::isfinite(maxDepthError) || !(maxDepthError > 0.0))
+    return arg_error(fn, "maxDepthError must be finite and > 0");
+  if (!(maxNormalErrorDeg > 0.0 && maxNormalErrorDeg <= 180.0))
+    return arg_error(fn, "maxNormalErrorDeg must be in (0, 180]");
+  if (maxPoints < 0) return arg_error(fn, "maxPoints must be >= 0");
+  if (maxPoints > 0 && (!xyz || !normal || !intensity || !source || misaligned(xyz, 4) || misaligned(normal, 4) ||
+                        misaligned(intensity, 4) || misaligned(source, 8)))
+    return arg_error(fn, "maxPoints > 0 needs d_xyz, d_normal, d_intensity (4-byte aligned) and d_source (8-byte)");
+  static const char *const names[8] = {"d_xyz", "d_normal", "d_intensity", "d_source", "jobs[%d].d_depth",
+                                       "jobs[%d].d_normal", "jobs[%d].d_cost", "images[%d].d_img"};
+  ArgRanges rs(names, 4 + 3 * (size_t)numJobs + numImages);
+  if (maxPoints > 0) {
+    const size_t m = (size_t)maxPoints;
+    rs.add(xyz, 12 * m, 0, 0, true);
+    rs.add(normal, 12 * m, 1, 0, true);
+    rs.add(intensity, 4 * m, 2, 0, true);
+    rs.add(source, 8 * m, 3, 0, true);
+  }
+  stereo_ranges(rs, images, numImages, jobs, numJobs, false, 4);
   return rs.check(fn);
 }
 

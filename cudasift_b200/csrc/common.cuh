@@ -417,6 +417,10 @@ struct DeviceCtx {
   GrowBuffer retrieve;
   PinnedBuffer h_retrieve;                 // the statistics (copied back), then the image table
   int retrieveWaves = 0;                   // the waves of the last cs_retrieve_pairs call
+  // cs_undistort_images, cs_patch_match_stereo, cs_fuse_depth_maps: the image, job and source tables, the per-job
+  // counters and the point list's scratch
+  GrowBuffer stereo;
+  PinnedBuffer h_stereo;                   // the same tables (uploaded), then the counters (copied back)
 
   // pinned host words, allocated by ensure()
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
@@ -684,6 +688,24 @@ int globalpos_enqueue(DeviceCtx &c, const cs_match_set *sets, int numImages, con
 // accepted steps
 int globalpos_result(const DeviceCtx &c, int numImages, const double *Rs, int maxIterations, double *t_out,
                      double cost[2], double *trace, long long stats[8]);
+
+// ---- dense reconstruction (stereo.cu) -----------------------------------------------------------------------------
+// The launch of cs_undistort_images (argument-checked, numImages > 0) on c.stream, without a synchronize; the outside
+// counts reach *outside (pinned, numImages of them) by the caller's synchronize.
+int undistort_images_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks,
+                             const double *dists, float *const *out, const unsigned long long **outside);
+// The launches of cs_patch_match_stereo (argument-checked, numJobs > 0) on c.stream, without a synchronize; per job
+// the counters {0, invalid view evaluations, pixels of final cost 2} reach *counts (pinned, 3 per job) by the caller's
+// synchronize.
+int patch_match_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                        const double *ts, const cs_stereo_job *jobs, int numJobs, int radius, int step,
+                        int numIterations, int topK, unsigned long long seed, const unsigned long long **counts);
+// The launches of cs_fuse_depth_maps (argument-checked, numJobs > 0) on c.stream, without a synchronize; the point
+// total reaches **total (pinned) by the caller's synchronize.
+int fuse_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                 const double *ts, const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent,
+                 double maxReprojError, double maxDepthError, double maxNormalErrorDeg, float *xyz, float *normal,
+                 float *intensity, int *source, int maxPoints, unsigned int **total);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

@@ -941,6 +941,139 @@ int cs_global_positioning(const cs_match_set *sets, int numImages, const double 
                           int maxIterations, int maxLinearIterations, double linearTol, double *t_out,
                           double *d_points, double cost_out[2], double *trace_out, long long stats_out[8], double *ms);
 
+/* ---- dense reconstruction: undistorted images, PatchMatch stereo, depth-map fusion ----
+ * Images are device float32 grayscale: pixel (col, row) is at d_img[row * pitch + col] (pitch in floats, >= width)
+ * and lies at (col, row) in the coordinates that K maps to, the coordinates of the extractor's record positions.
+ * Cameras are cs_bundle_adjust's: Ks[a] [9] (cs_verify_essential's rule), Rs[a] [9] a rotation, ts[a] [3], with
+ * X_c = R X + t.  Every call checks, with CS_E_ARG before any CUDA call and naming the argument: numImages outside
+ * [1, 65536] (cs_undistort_images: [0, 65536]), NULL images (or Ks, Rs, ts) with images, a NULL or not 4-byte aligned
+ * images[a].d_img, width or height outside [2, 4096], pitch < width, and an invalid Ks[a], Rs[a] (R^T R = I within
+ * 1e-6, det R > 0) or non-finite ts[a].
+ * The bilinear sample of an image at (u, v), in FP32: u and v are clamped to [0, W - 1] and [0, H - 1], x0 =
+ * min((int)u, W - 2), fx = u - x0 (likewise y0, fy), a = fmaf(fx, I(x0 + 1, y0) - I(x0, y0), I(x0, y0)),
+ * b = fmaf(fx, I(x0 + 1, y0 + 1) - I(x0, y0 + 1), I(x0, y0 + 1)), and the sample is fmaf(fy, b - a, a). */
+typedef struct {
+  const float *d_img;
+  int width, height, pitch;
+} cs_image;
+
+/* One depth map: image ref seen from the images sources[0 .. numSources) (a host array).  d_depth [H][W],
+ * d_normal [H][W][3] (the normal in ref's camera frame) and d_cost [H][W] are dense device float arrays of ref's size.
+ * An image is the ref of at most one job, so every random draw is keyed by the image and a job's maps do not depend
+ * on the batch it is in. */
+typedef struct {
+  int ref;
+  const int *sources;
+  int numSources;
+  float depthMin, depthMax;
+  float *d_depth;
+  float *d_normal;
+  float *d_cost;
+} cs_stereo_job;
+
+/* Undistortion of whole images under cs_bundle_adjust_intrinsics' radial model: d_out[a] (device, dense
+ * width x height floats) is images[a] as the pinhole camera Ks[a] would see it.  Size and K are kept.
+ * - Output pixel (x, y), in float64: b = (y - K5) / K4, a = (x - K2 - K1 b) / K0, s = 1 + k1 r^2 + k2 r^4 with
+ *   r^2 = a^2 + b^2 (the forward model of cs_undistort_records, in closed form), u = K0 a s + K1 b s + K2 and
+ *   v = K4 b s + K5, rounded to float; the output is the bilinear sample of images[a] at (u, v), or 0 when (u, v) is
+ *   outside [0, W - 1] x [0, H - 1] (counted in outside_out[a], may be NULL).  dists [numImages][2] (k1, k2) may be
+ *   NULL (all zero: the input itself inside a 1-pixel border, where the position may round just outside or
+ *   fx or fy = 1 may round the lerp).
+ * - One kernel launch (cs_launch_count) for all images, whatever their sizes; the call synchronises once; *ms (may be
+ *   NULL) gets its event time.  numImages == 0 makes no CUDA call.
+ * - CS_E_ARG, before any CUDA call: the image and camera checks above (Rs and ts are not taken), a non-finite
+ *   dists[a], NULL d_out, a NULL or not 4-byte aligned d_out[a], and an overlap of d_out[a] with another output or any
+ *   image (one sweep over sorted ranges). */
+int cs_undistort_images(const cs_image *images, int numImages, const double *Ks, const double *dists,
+                        float *const *d_out, long long *outside_out, double *ms);
+
+/* PatchMatch stereo (Bleyer et al., BMVC 2011) with red-black propagation (Gipuma, Galliani et al., ICCV 2015): a
+ * depth, a normal and a cost for every pixel of every job's ref image, all jobs in one call.
+ * - Hypothesis at pixel p = (x, y) of ref r: depth z along the camera axis and a unit normal n (ref camera frame) that
+ *   faces the ray, n . ray < 0 with ray = Kinv (x, y, 1), Kinv = K_r^-1 in float64.  Its plane passes through X = z ray.
+ * - Tables, on the host in float64 and rounded to float once: per source s of a job, A_s = K_s R_sr Kinv and
+ *   b_s = K_s t_sr with R_sr = R_s R_r^T, t_sr = t_s - R_sr t_r.  Homography of h into s, in float64 from those floats
+ *   and the float hypothesis, then rounded to float: m = (Kinv^T n) / (z (n . ray)), H_s = A_s + b_s m^T.
+ * - View cost of h in s: the window is the (2 windowRadius / windowStep + 1)^2 offsets (i, j) in steps of windowStep
+ *   from -windowRadius to windowRadius, rows j outer, columns i inner.  Reference sample R_ij = ref(clamp(x + i),
+ *   clamp(y + j)) at integer positions; q = H_s (x + i, y + j, 1) in FP32, source sample S_ij = the bilinear sample of
+ *   s at (q0 / q2, q1 / q2).  The view is invalid, and costs 2, when q2 <= 0 for some sample, when the centre's
+ *   (u, v) lies outside [0, W_s - 1] x [0, H_s - 1], or when either window's variance is below 1 (grey levels^2).
+ *   Otherwise, in FP32 in the window order, with the centre samples R_00 and S_00 taken first: d = R_ij - R_00,
+ *   e = S_ij - S_00, sums of d, e, d^2, e^2 and d e (each by fmaf for the products); mean = sum / N, var = sum of
+ *   squares / N - mean^2, cov = sum de / N - mean_d mean_e, and cost = 1 - cov / sqrtf(var_d var_e) clamped to [0, 2].
+ *   Against the same view cost in float64 (from the same float H_s), an FP32 cost differs by at most 2e-3 when no
+ *   decision above lies within 1e-3 of its threshold (a relative 1e-3 for the variance floor).
+ * - Aggregated cost of h: the mean of its topK smallest view costs, summed in ascending order.
+ * - Draws: u(slot) = (splitmix64(seed + 0x9E3779B97F4A7C15 c) >> 11) 2^-53 with the counter
+ *   c = ((ref 2^24 + y W + x) 64 + iteration) 16 + slot.  A random hypothesis takes u(s0) for the depth, uniform in
+ *   inverse depth: 1 / z = 1 / depthMax + u (1 / depthMin - 1 / depthMax), and u(s0 + 1 .. s0 + 3) for the normal,
+ *   normalise(2 u - 1), negated when n . ray > 0 (-ray / |ray| when n . ray = 0 or the draw is 0).  Every value
+ *   derived from draws is computed in float64 from the float state and rounded to float once.
+ * - Start (iteration 0): every pixel takes the random hypothesis of slot 0 and its aggregated cost.
+ * - Iteration k = 1 .. numIterations, rho = 2^-k: a half-step over the pixels with x + y even, then one over the odd
+ *   ones.  A pixel's candidates, in this order, from the state at the start of the half-step:
+ *   1. propagation from the neighbours at (-1, 0), (1, 0), (0, -1), (0, 1), (-5, 0), (5, 0), (0, -5), (0, 5) (all of the
+ *      other colour): the neighbour's plane, through z_q Kinv (x_q, y_q, 1), met by p's ray: z = (n_q . X_q) / (n_q . ray)
+ *      with n_q; skipped when q is off the image, when n_q . ray >= 0, or when z (as float) is outside
+ *      [depthMin, depthMax];
+ *   2. the depth moved in inverse depth, 1 / z + rho (2 u(0) - 1) (1 / depthMin - 1 / depthMax) clamped to
+ *      [1 / depthMax, 1 / depthMin], with the current normal;
+ *   3. the current depth with the normal normalise(n + rho (2 u(1 .. 3) - 1)), negated to face the ray as above;
+ *   4. both moves, with u(4) and u(5 .. 7);
+ *   5. the random hypothesis of slot 8.
+ *   The pixel keeps the candidate of strictly lowest aggregated cost: ties go to the current hypothesis, then to the
+ *   earlier candidate.  A half-step reads the other colour and the pixel's own state only, so the maps are the state,
+ *   and the result does not depend on the order in which pixels run: two calls give the same bytes, and a job's maps
+ *   are the same bytes alone or in any batch.
+ * - Outputs: every pixel ends with a finite hypothesis and its cost; cost 2 means no source supported it.
+ *   stats_out [numJobs][3] (may be NULL): pixels, invalid view evaluations in the whole call, pixels whose final cost
+ *   is 2.
+ * - Launches: 2 + 2 numIterations kernel launches (cs_launch_count) for all jobs together (start, the half-steps, a
+ *   final count); the call synchronises once; *ms (may be NULL) gets its event time.  Scratch in the per-device
+ *   context: the image, job and source tables (264 bytes per image, 144 per job, 52 per source) and 24 bytes per job
+ *   of counters; the same tables pinned.  numJobs == 0 makes no CUDA call.
+ * - CS_E_ARG, before any CUDA call: the image and camera checks above, numJobs outside [0, 65536], NULL jobs with
+ *   jobs, windowRadius outside [1, 7], windowStep outside [1, windowRadius] or not dividing windowRadius,
+ *   numIterations outside [0, 32], and per jobs[p]: ref outside [0, numImages) or the ref of an earlier job,
+ *   numSources outside [1, 32], NULL sources, a source outside [0, numImages), equal to ref or listed twice, topK
+ *   outside [1, numSources], depthMin and depthMax not finite or not 0 < depthMin < depthMax, and NULL or not 4-byte
+ *   aligned d_depth, d_normal or d_cost; then an overlap of a map with any other map or image (one sweep). */
+int cs_patch_match_stereo(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                          const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep, int numIterations,
+                          int topK, unsigned long long seed, long long *stats_out, double *ms);
+
+/* Fusion of the depth maps of cs_patch_match_stereo into one point cloud (COLMAP's stereo_fusion, as a parallel rule
+ * whose order follows from the values): jobs, their maps and the images as that call left them.
+ * - Pixel p = (x, y) of job a (image a = jobs[.].ref) with cost <= maxCost back-projects to X_p = R_a^T (z Kinv_a
+ *   (x, y, 1) - t_a) with world normal R_a^T n.  A source b of job a that is itself the ref of a job is consistent
+ *   when, in float64: Y = R_b X_p + t_b has Y_z > 0; q = (floor(u + 0.5), floor(v + 0.5)) for (u, v) = K_b Y / Y_z
+ *   lies in b; cost_b(q) <= maxCost; |z_b(q) - Y_z| <= maxDepthError Y_z; the world normals of p and q have a dot
+ *   product >= cos(maxNormalErrorDeg); and q back-projected with z_b(q) projects into a within maxReprojError pixels
+ *   of (x, y).
+ * - p emits a point when it has at least minConsistent consistent views and none of them has an image index below a,
+ *   so a surface point is emitted by the lowest-indexed image that sees it consistently.  A duplicate can still
+ *   appear when source lists are asymmetric: b emits its own point for q when a is not a source of b.
+ * - The point: position the mean of X_p and the consistent back-projections, normal the normalised sum of the world
+ *   normals, intensity the mean of image a at p and each consistent image at q, summed in float64 in source-list order
+ *   after p's own; d_source = {a, y W + x}.  Outputs d_xyz [][3], d_normal [][3], d_intensity [] (float) and d_source
+ *   [] (int2), in ascending (a, pixel) order, written by a flag kernel and a count-scan-write kernel (ordered_list.cuh),
+ *   at most maxPoints (the prefix of the full list).
+ * - Returns the number of points in the full list, or CS_E_*.  stats_out (may be NULL): [0] that number, [1] the
+ *   points written.  2 kernel launches; the call synchronises once; *ms (may be NULL) gets its event time.  Scratch:
+ *   cs_patch_match_stereo's tables and counters, plus, on the device only, the list's words (4 bytes per 32 pixels,
+ *   4 per 1024).
+ *   numJobs == 0 returns 0 and makes no CUDA call.
+ * - CS_E_ARG, before any CUDA call: cs_patch_match_stereo's image, camera and job checks (topK aside), the pixels of
+ *   all jobs above 2^31 - 1, maxCost not in [0, 2], minConsistent outside [1, 32], maxReprojError, maxDepthError not
+ *   finite or not > 0, maxNormalErrorDeg not in (0, 180], maxPoints < 0, NULL or not 4-byte aligned d_xyz, d_normal,
+ *   d_intensity or d_source (8-byte) with maxPoints > 0; and an overlap of an output with any other output, map or
+ *   image (one sweep). */
+int cs_fuse_depth_maps(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                       const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent, double maxReprojError,
+                       double maxDepthError, double maxNormalErrorDeg, float *d_xyz, float *d_normal,
+                       float *d_intensity, int *d_source, int maxPoints, long long stats_out[2], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
