@@ -23,7 +23,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
            "RetrievePairs", "RotationAveraging", "GlobalPositioning", "UndistortImages", "PatchMatchStereo",
-           "FuseDepthMaps", "SelectStereoViews"]
+           "PatchMatchStereoGeometric", "FuseDepthMaps", "SelectStereoViews"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -113,6 +113,8 @@ def lib():
         "cs_undistort_images": (ip, [vp, ip, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_patch_match_stereo": (ip, [vp, ip, vp, vp, vp, vp, ip, ip, ip, ip, ip, c.c_ulonglong, vp,
                                        c.POINTER(c.c_double)]),
+        "cs_patch_match_stereo_geometric": (ip, [vp, ip, vp, vp, vp, vp, vp, ip, ip, ip, ip, ip, c.c_double,
+                                                 c.c_double, c.c_ulonglong, vp, c.POINTER(c.c_double)]),
         "cs_fuse_depth_maps": (ip, [vp, ip, vp, vp, vp, vp, ip, fp, ip, c.c_double, c.c_double, c.c_double, vp, vp, vp,
                                     vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
@@ -1134,6 +1136,11 @@ class StereoJob(ctypes.Structure):
                 ("d_normal", ctypes.c_void_p), ("d_cost", ctypes.c_void_p)]
 
 
+class DepthPrior(ctypes.Structure):
+    """cs_depth_prior: an image's prior depth and normal maps (device floats), NULL for none."""
+    _fields_ = [("d_depth", ctypes.c_void_p), ("d_normal", ctypes.c_void_p)]
+
+
 def _upload_images(images):
     """Host float32 [H, W] images in dense device buffers, and their cs_image table."""
     arrs = [np.ascontiguousarray(im, np.float32) for im in images]
@@ -1232,6 +1239,55 @@ def PatchMatchStereo(images, Ks, Rs, ts, jobs, windowRadius=5, windowStep=1, num
         for b in bufs + [b for m in maps for b in m]:
             b.free()
     return depth, normal, cost, stats, ms.value
+
+
+def PatchMatchStereoGeometric(images, Ks, Rs, ts, jobs, depth, normal, windowRadius=5, windowStep=1, numIterations=5,
+                              topK=3, geomWeight=0.3, geomMaxError=3.0, seed=0):
+    """PatchMatch stereo with geometric consistency (cs_patch_match_stereo_geometric): every job's maps again, each
+    view's cost joined by geomWeight times its forward-backward reprojection error (pixels, capped at geomMaxError)
+    against that source's depth map.  depth and normal are PatchMatchStereo's maps for the same jobs, as FuseDepthMaps
+    takes them: each job's ref gets its maps as its prior, and an image that is no job's ref has none.  Other arguments
+    as for PatchMatchStereo; the defaults are COLMAP's.  Returns (depth [J], normal [J], cost [J], stats int64 [J, 5] of
+    {pixels, invalid view evaluations, pixels of cost >= 2, valid view evaluations capped at geomMaxError, pixels started
+    from a random hypothesis}, ms)."""
+    S = len(images)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    if not (len(depth) == len(normal) == len(jobs)):
+        raise ValueError("depth and normal: one map per job")
+    arrs, bufs, table = _upload_images(images)
+    shapes = [im.shape for im in arrs]
+    maps = []
+    try:
+        parsed, jt, maps = _stereo_jobs(jobs, shapes, lambda p, sh: [DeviceBuffer(4 * sh[0] * sh[1]),
+                                                                     DeviceBuffer(12 * sh[0] * sh[1]),
+                                                                     DeviceBuffer(4 * sh[0] * sh[1])])
+        J = len(parsed)
+        priors = (DepthPrior * max(S, 1))()
+        for p, (ref, _, _, _) in enumerate(parsed):
+            h, w = shapes[ref]
+            bufs.append(DeviceBuffer(4 * h * w))
+            bufs.append(DeviceBuffer(12 * h * w))
+            pd, pn = bufs[-2:]
+            pd.upload(np.ascontiguousarray(np.asarray(depth[p], np.float32).reshape(h, w)))
+            pn.upload(np.ascontiguousarray(np.asarray(normal[p], np.float32).reshape(h, w, 3)))
+            priors[ref] = DepthPrior(pd.ptr, pn.ptr)
+        stats, ms = np.zeros((J, 5), np.int64), ctypes.c_double(0.0)
+        _check(lib().cs_patch_match_stereo_geometric(table if S else None, S, _ptr(K), _ptr(R), _ptr(t),
+                                                     priors if S else None, jt if J else None, J, int(windowRadius),
+                                                     int(windowStep), int(numIterations), int(topK),
+                                                     float(geomWeight), float(geomMaxError), int(seed),
+                                                     _ptr(stats) if J else None, ctypes.byref(ms)),
+               "PatchMatchStereoGeometric")
+        dep, nrm, cost = [], [], []
+        for (ref, _, _, _), m in zip(parsed, maps):
+            h, w = shapes[ref]
+            dep.append(m[0].download(np.float32, h * w).reshape(h, w))
+            nrm.append(m[1].download(np.float32, 3 * h * w).reshape(h, w, 3))
+            cost.append(m[2].download(np.float32, h * w).reshape(h, w))
+    finally:
+        for b in bufs + [b for m in maps for b in m]:
+            b.free()
+    return dep, nrm, cost, stats, ms.value
 
 
 def FuseDepthMaps(images, Ks, Rs, ts, jobs, depth, normal, cost, maxCost=0.5, minConsistent=2, maxReprojError=2.0,

@@ -1654,6 +1654,40 @@ int cs_patch_match_stereo(const cs_image *images, int numImages, const double *K
   return 0;
 }
 
+int cs_patch_match_stereo_geometric(const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                                    const double *ts, const cs_depth_prior *priors, const cs_stereo_job *jobs,
+                                    int numJobs, int windowRadius, int windowStep, int numIterations, int topK,
+                                    double geomWeight, double geomMaxError, unsigned long long seed,
+                                    long long *stats_out, double *ms)
+{
+  const char *fn = "cs_patch_match_stereo_geometric";
+  if (ms) *ms = 0.0;
+  int r = patch_match_geometric_args(fn, images, numImages, Ks, Rs, ts, priors, jobs, numJobs, windowRadius,
+                                     windowStep, numIterations, topK, geomWeight, geomMaxError);
+  if (r < 0 || numJobs == 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  const unsigned long long *counts = nullptr;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return patch_match_geometric_enqueue(*c, images, numImages, Ks, Rs, ts, priors, jobs, numJobs, windowRadius,
+                                              windowStep, numIterations, topK, geomWeight, geomMaxError, seed,
+                                              &counts);
+       })) < 0)
+    return r;
+  const unsigned long long *extra = counts + 3 * (size_t)numJobs;
+  for (int p = 0; stats_out && p < numJobs; p++) {
+    const cs_image &I = images[jobs[p].ref];
+    long long *st = stats_out + 5 * (size_t)p;
+    st[0] = (long long)I.width * I.height;
+    st[1] = (long long)counts[3 * (size_t)p + 1];
+    st[2] = (long long)counts[3 * (size_t)p + 2];
+    st[3] = (long long)extra[3 * (size_t)p];
+    st[4] = (long long)extra[3 * (size_t)p + 1];
+  }
+  return 0;
+}
+
 int cs_fuse_depth_maps(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
                        const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent, double maxReprojError,
                        double maxDepthError, double maxNormalErrorDeg, float *d_xyz, float *d_normal,

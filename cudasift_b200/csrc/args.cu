@@ -866,23 +866,70 @@ static void stereo_ranges(ArgRanges &rs, const cs_image *images, int numImages, 
   for (int a = 0; a < numImages; a++) rs.add(images[a].d_img, image_bytes(images[a]), kind0 + 3, a, false);
 }
 
-int patch_match_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
-                     const double *ts, const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
-                     int numIterations, int topK)
+// The checks of the PatchMatch calls before their range sweeps; numIterations in [0, maxIterations].
+static int pm_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                   const double *ts, const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
+                   int numIterations, int maxIterations, int topK)
 {
   int r;
   if ((r = stereo_images(fn, images, numImages, 1, Ks, Rs, ts, true)) < 0) return r;
   if (windowRadius < 1 || windowRadius > 7) return arg_error(fn, "windowRadius must be in [1, 7]");
   if (windowStep < 1 || windowStep > windowRadius || windowRadius % windowStep != 0)
     return arg_error(fn, "windowStep must be in [1, windowRadius] and divide windowRadius");
-  if (numIterations < 0 || numIterations > 32) return arg_error(fn, "numIterations must be in [0, 32]");
+  if (numIterations < 0 || numIterations > maxIterations)
+    return arg_error(fn, "numIterations must be in [0, %d]", maxIterations);
   if (topK < 1) return arg_error(fn, "topK must be in [1, numSources]");
   long long pixels = 0;
-  if ((r = stereo_jobs(fn, numImages, images, jobs, numJobs, topK, &pixels)) < 0) return r;
+  return stereo_jobs(fn, numImages, images, jobs, numJobs, topK, &pixels);
+}
+
+int patch_match_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                     const double *ts, const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
+                     int numIterations, int topK)
+{
+  int r;
+  if ((r = pm_args(fn, images, numImages, Ks, Rs, ts, jobs, numJobs, windowRadius, windowStep, numIterations, 32,
+                   topK)) < 0)
+    return r;
   static const char *const names[4] = {"jobs[%d].d_depth", "jobs[%d].d_normal", "jobs[%d].d_cost",
                                        "images[%d].d_img"};
   ArgRanges rs(names, 3 * (size_t)numJobs + numImages);
   stereo_ranges(rs, images, numImages, jobs, numJobs, true, 0);
+  return rs.check(fn);
+}
+
+// The draws of the geometric pass use counter iterations 32 + k, within the counter's 6 bits: at most 31 iterations.
+int patch_match_geometric_args(const char *fn, const cs_image *images, int numImages, const double *Ks,
+                               const double *Rs, const double *ts, const cs_depth_prior *priors,
+                               const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
+                               int numIterations, int topK, double geomWeight, double geomMaxError)
+{
+  int r;
+  if ((r = pm_args(fn, images, numImages, Ks, Rs, ts, jobs, numJobs, windowRadius, windowStep, numIterations, 31,
+                   topK)) < 0)
+    return r;
+  if (numJobs > 0 && !priors) return arg_error(fn, "numJobs > 0 needs priors");
+  for (int p = 0; p < numJobs; p++) {
+    const cs_depth_prior &Pr = priors[jobs[p].ref];
+    if (!Pr.d_depth || !Pr.d_normal)
+      return arg_error(fn, "jobs[%d]: priors[%d] (its ref) needs d_depth and d_normal", p, jobs[p].ref);
+  }
+  for (int a = 0; priors && a < numImages; a++)
+    if (misaligned(priors[a].d_depth, 4) || misaligned(priors[a].d_normal, 4))
+      return arg_error(fn, "priors[%d]: d_depth and d_normal must be 4-byte aligned", a);
+  if (!std::isfinite(geomWeight) || !(geomWeight >= 0.0)) return arg_error(fn, "geomWeight must be finite and >= 0");
+  if (!std::isfinite(geomMaxError) || !(geomMaxError > 0.0))
+    return arg_error(fn, "geomMaxError must be finite and > 0");
+  // the maps (written), the images and the priors (read, so they may share bytes with each other)
+  static const char *const names[6] = {"jobs[%d].d_depth", "jobs[%d].d_normal", "jobs[%d].d_cost",
+                                       "images[%d].d_img", "priors[%d].d_depth", "priors[%d].d_normal"};
+  ArgRanges rs(names, 3 * (size_t)numJobs + 3 * (size_t)numImages);
+  stereo_ranges(rs, images, numImages, jobs, numJobs, true, 0);
+  for (int a = 0; priors && a < numImages; a++) {
+    const size_t px = (size_t)images[a].width * images[a].height * sizeof(float);
+    if (priors[a].d_depth) rs.add(priors[a].d_depth, px, 4, a, false);
+    if (priors[a].d_normal) rs.add(priors[a].d_normal, 3 * px, 5, a, false);
+  }
   return rs.check(fn);
 }
 

@@ -70,13 +70,17 @@ int globalpos_args(const char *fn, const cs_match_set *sets, int numImages, cons
                    int refImage, int loss, double lossScale, int maxIterations, int maxLinearIterations,
                    double linearTol, const double *t_out, const double *points, const double *cost_out,
                    const double *trace_out);
-// cs_undistort_images, cs_patch_match_stereo and cs_fuse_depth_maps: the images and cameras, the jobs, the
+// cs_undistort_images, cs_patch_match_stereo(_geometric) and cs_fuse_depth_maps: the images and cameras, the jobs, the
 // parameters and the range sweep.
 int undistort_images_args(const char *fn, const cs_image *images, int numImages, const double *Ks,
                           const double *dists, float *const *d_out);
 int patch_match_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
                      const double *ts, const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
                      int numIterations, int topK);
+int patch_match_geometric_args(const char *fn, const cs_image *images, int numImages, const double *Ks,
+                               const double *Rs, const double *ts, const cs_depth_prior *priors,
+                               const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep,
+                               int numIterations, int topK, double geomWeight, double geomMaxError);
 int fuse_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
               const double *ts, const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent,
               double maxReprojError, double maxDepthError, double maxNormalErrorDeg, const float *xyz,

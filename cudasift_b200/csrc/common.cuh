@@ -417,7 +417,7 @@ struct DeviceCtx {
   GrowBuffer retrieve;
   PinnedBuffer h_retrieve;                 // the statistics (copied back), then the image table
   int retrieveWaves = 0;                   // the waves of the last cs_retrieve_pairs call
-  // cs_undistort_images, cs_patch_match_stereo, cs_fuse_depth_maps: the image, job and source tables, the per-job
+  // cs_undistort_images, cs_patch_match_stereo(_geometric), cs_fuse_depth_maps: the image, job and source tables, the per-job
   // counters and the point list's scratch
   GrowBuffer stereo;
   PinnedBuffer h_stereo;                   // the same tables (uploaded), then the counters (copied back)
@@ -700,6 +700,14 @@ int undistort_images_enqueue(DeviceCtx &c, const cs_image *images, int numImages
 int patch_match_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
                         const double *ts, const cs_stereo_job *jobs, int numJobs, int radius, int step,
                         int numIterations, int topK, unsigned long long seed, const unsigned long long **counts);
+// The launches of cs_patch_match_stereo_geometric (argument-checked, numJobs > 0) on c.stream, without a synchronize;
+// per job the counters {0, invalid view evaluations, pixels of final cost >= 2}, then per job {valid view evaluations
+// capped at geomMaxError, pixels started from a draw, 0} reach *counts (pinned, 6 per job) by the caller's synchronize.
+int patch_match_geometric_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks,
+                                  const double *Rs, const double *ts, const cs_depth_prior *priors,
+                                  const cs_stereo_job *jobs, int numJobs, int radius, int step, int numIterations,
+                                  int topK, double geomWeight, double geomMaxError, unsigned long long seed,
+                                  const unsigned long long **counts);
 // The launches of cs_fuse_depth_maps (argument-checked, numJobs > 0) on c.stream, without a synchronize; the point
 // total reaches **total (pinned) by the caller's synchronize.
 int fuse_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,

@@ -1,9 +1,11 @@
 // stereo.cu -- dense reconstruction: undistorted images (cs_undistort_images), PatchMatch stereo with red-black
-// propagation (cs_patch_match_stereo) and the fusion of its depth maps (cs_fuse_depth_maps).  The header states every
-// rule; tests/stereo_oracle.py restates them in float64.
+// propagation (cs_patch_match_stereo), its geometric-consistency pass (cs_patch_match_stereo_geometric) and the fusion
+// of depth maps (cs_fuse_depth_maps).  The header states every rule; tests/stereo_oracle.py and
+// tests/stereo_geom_oracle.py restate them in float64.
 //
 // A half-step reads the other colour and the pixel's own state only, and writes the pixel's own state, so the maps are
-// the state and no pixel's result depends on the order in which threads run.  The only atomics are integer counts.
+// the state and no pixel's result depends on the order in which threads run.  The geometric pass also reads the
+// sources' prior maps, which are inputs of the call and never written.  The only atomics are integer counts.
 #include "common.cuh"
 #include "ordered_list.cuh"
 #include "vp_math.cuh"
@@ -41,9 +43,27 @@ struct StJob {
 struct StCounts {
   unsigned long long v[3];
 };
+// The geometric pass's table per source (parallel to the StSrc table): R_sr, t_sr in float64 and the source's prior
+// depth map (NULL: no prior) with its size.
+struct StGeo {
+  double R[9], t[3];
+  const float *depth;
+  int w, h;
+};
+
+// The geometric pass's prior of a job's ref.
+struct StPrior {
+  const float *depth, *normal;
+};
+
 // the scratch the header states
 static_assert(sizeof(StImage) == 264 && sizeof(StJob) == 144 && sizeof(StSrc) == 52 && sizeof(StCounts) == 24,
               "stereo table sizes");
+static_assert(sizeof(StGeo) == 112 && sizeof(StPrior) == 16, "geometric table sizes");
+
+// The draws of the geometric pass use counter iterations 32 (start) and 32 + k (iteration k <= 31), apart from the
+// photometric pass's 0 .. 32 under the same seed.
+constexpr int ST_GEOM_IT0 = 32;
 
 __device__ __forceinline__ float st_bilinear(const float *__restrict__ img, int w, int h, int pitch, float u, float v)
 {
@@ -98,6 +118,16 @@ struct PmParams {
   int radius, step, topK;
   unsigned long long seed;
   int iteration, colour;   // the half-step's iteration (1..) and colour (0 even, 1 odd)
+};
+
+// The geometric pass's own parameters: a kernel argument after PmParams and the total, so the photometric kernels'
+// arguments keep their offsets.
+struct PmGeom {
+  const StGeo *geo;        // per source, parallel to srcs
+  const StPrior *priors;   // per job
+  StCounts *counts;        // per job: {valid view evaluations capped at gmax, pixels started from a draw, 0}
+  float lambda;
+  double gmax;
 };
 
 struct Hyp {
@@ -230,6 +260,84 @@ __device__ __noinline__ float st_cost(const PmParams &P, const StJob &J, const S
   return sum / (float)P.topK;
 }
 
+// The geometric error of the point X (ref camera frame, on the ray of pixel (x, y) of R) in source S, the header's rule
+// in float64: forward into S, the prior depth at the nearest pixel, back from the continuous (u, v) into R.  gmax when
+// a depth is not positive, q is off S, S has no prior or the prior is not finite or <= 0; *capped when g is gmax.
+__device__ __forceinline__ float st_geom_error(const StGeo &G, const StImage &S, const StImage &R, const double (&X)[3],
+                                               int x, int y, double gmax, bool *capped)
+{
+  double e = gmax, Y[3];
+  for (int k = 0; k < 3; k++) Y[k] = G.R[3 * k] * X[0] + G.R[3 * k + 1] * X[1] + G.R[3 * k + 2] * X[2] + G.t[k];
+  if (G.depth && Y[2] > 0.0) {
+    const double u = (S.K[0] * Y[0] + S.K[1] * Y[1] + S.K[2] * Y[2]) / Y[2];
+    const double v = (S.K[4] * Y[1] + S.K[5] * Y[2]) / Y[2];
+    const double qx = floor(u + 0.5), qy = floor(v + 0.5);
+    if (qx >= 0.0 && qx < G.w && qy >= 0.0 && qy < G.h) {
+      const double zs = __ldg(G.depth + (size_t)qy * G.w + (size_t)qx);
+      if (isfinite(zs) && zs > 0.0) {
+        double c[3], Z[3];
+        for (int k = 0; k < 3; k++) c[k] = zs * (S.Kinv[3 * k] * u + S.Kinv[3 * k + 1] * v + S.Kinv[3 * k + 2]) - G.t[k];
+        for (int k = 0; k < 3; k++) Z[k] = G.R[k] * c[0] + G.R[3 + k] * c[1] + G.R[6 + k] * c[2];
+        if (Z[2] > 0.0) {
+          const double ex = (R.K[0] * Z[0] + R.K[1] * Z[1] + R.K[2] * Z[2]) / Z[2] - x;
+          const double ey = (R.K[4] * Z[1] + R.K[5] * Z[2]) / Z[2] - y;
+          e = fmin(hypot(ex, ey), gmax);
+        }
+      }
+    }
+  }
+  *capped = !(e < gmax);
+  return (float)e;
+}
+
+// The combined cost of h at (x, y): every view costs fmaf(lambda, g, c_photo), c_photo 2 for an invalid view;
+// *invalid counts the invalid views and *capped the valid ones whose g is gmax.  The steps are st_cost's, written out
+// again so that st_cost, and with it the photometric kernels, keep their instructions.  Not inlined, as st_cost.
+__device__ __noinline__ float st_cost_geom(const PmParams &P, const PmGeom &G, const StJob &J, const StImage &R, int x,
+                                           int y, const Hyp &h, const double (&ray)[3], int *invalid, int *capped)
+{
+  float best[ST_MAX_SOURCES];
+  const double nr = (double)h.n[0] * ray[0] + (double)h.n[1] * ray[1] + (double)h.n[2] * ray[2];
+  const double den = (double)h.z * nr;
+  double m[3], X[3];
+  for (int k = 0; k < 3; k++)
+    m[k] = (J.Kinv[k] * h.n[0] + J.Kinv[3 + k] * h.n[1] + J.Kinv[6 + k] * h.n[2]) / den;
+  for (int k = 0; k < 3; k++) X[k] = (double)h.z * ray[k];
+  int kept = 0;
+  for (int s = 0; s < J.numSources; s++) {
+    const StSrc &src = P.srcs[J.src0 + s];
+    const StImage &S = P.images[src.image];
+    float H[9];
+    for (int a = 0; a < 3; a++)
+      for (int k = 0; k < 3; k++) H[3 * a + k] = (float)((double)src.A[3 * a + k] + (double)src.b[a] * m[k]);
+    float c = st_view_cost(R, S, H, x, y, P.radius, P.step);
+    bool cap;
+    const float g = st_geom_error(G.geo[J.src0 + s], S, R, X, x, y, G.gmax, &cap);
+    if (c < 0.0f) { c = 2.0f; (*invalid)++; }
+    else if (cap) (*capped)++;
+    c = fmaf(G.lambda, g, c);
+    // insertion into the ascending list of the topK smallest
+    int k;
+    if (kept < P.topK) k = kept++;
+    else if (c < best[P.topK - 1]) k = P.topK - 1;
+    else continue;
+    while (k > 0 && best[k - 1] > c) { best[k] = best[k - 1]; k--; }
+    best[k] = c;
+  }
+  float sum = 0.0f;
+  for (int k = 0; k < P.topK; k++) sum += best[k];
+  return sum / (float)P.topK;
+}
+
+// The cost of the pass: photometric, or combined with the geometric term.
+template <bool GEOM>
+__device__ __forceinline__ float st_eval(const PmParams &P, const PmGeom &G, const StJob &J, const StImage &R, int x,
+                                         int y, const Hyp &h, const double (&ray)[3], int *invalid, int *capped)
+{
+  if constexpr (GEOM) return st_cost_geom(P, G, J, R, x, y, h, ray, invalid, capped);
+  else return st_cost(P, J, R, x, y, h, ray, invalid);
+}
+
 // The warp's lanes of one job add their count to that job's counter k.
 __device__ __forceinline__ void st_count(StCounts *counts, int job, int k, unsigned int n)
 {
@@ -238,29 +346,58 @@ __device__ __forceinline__ void st_count(StCounts *counts, int job, int k, unsig
   if (job >= 0 && total && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&counts[job].v[k], (unsigned long long)total);
 }
 
-__global__ void __launch_bounds__(ST_THREADS) pm_start_kernel(PmParams P, long long total)
+// The ref's prior (z, n) at pixel pix when the header's start rule takes it: z in [depthMin, depthMax], n finite,
+// facing the ray and of length 1 within 1e-3.
+__device__ __forceinline__ bool st_prior(const StPrior &Pr, const StJob &J, int pix, const double (&ray)[3], Hyp &h)
+{
+  h.z = Pr.depth[pix];
+  for (int k = 0; k < 3; k++) h.n[k] = Pr.normal[3 * (size_t)pix + k];
+  if (!(h.z >= J.dmin && h.z <= J.dmax) || !isfinite(h.n[0]) || !isfinite(h.n[1]) || !isfinite(h.n[2])) return false;
+  const double d = (double)h.n[0] * ray[0] + (double)h.n[1] * ray[1] + (double)h.n[2] * ray[2];
+  const double len = sqrt((double)h.n[0] * h.n[0] + (double)h.n[1] * h.n[1] + (double)h.n[2] * h.n[2]);
+  return d < 0.0 && fabs(len - 1.0) <= 1e-3;
+}
+
+// Iteration 0.  Photometric: every pixel takes the draws of slot 0.  Geometric: the ref's prior where the start rule
+// takes it, else the draws of iteration 32, slot 0.
+template <bool GEOM>
+__device__ __forceinline__ void pm_start(PmParams P, long long total, PmGeom G)
 {
   const long long t = (long long)blockIdx.x * ST_THREADS + threadIdx.x;
-  int job = -1, invalid = 0;
+  int job = -1, invalid = 0, capped = 0, drawn = 0;
   if (t < total) {
     job = st_find(P.jobs, P.numJobs, &StJob::all0, t);
     const StJob &J = P.jobs[job];
     const int pix = (int)(t - J.all0), x = pix % J.w, y = pix / J.w;
     double ray[3];
     st_ray(J.Kinv, x, y, ray);
-    const Hyp h = st_random(P, J, x, y, 0, 0, ray);
-    const float c = st_cost(P, J, P.images[J.ref], x, y, h, ray, &invalid);
+    Hyp h;
+    if constexpr (GEOM) {
+      if (!st_prior(G.priors[job], J, pix, ray, h)) {
+        h = st_random(P, J, x, y, ST_GEOM_IT0, 0, ray);
+        drawn = 1;
+      }
+    } else {
+      h = st_random(P, J, x, y, 0, 0, ray);
+    }
+    const float c = st_eval<GEOM>(P, G, J, P.images[J.ref], x, y, h, ray, &invalid, &capped);
     J.depth[pix] = h.z;
     for (int k = 0; k < 3; k++) J.normal[3 * (size_t)pix + k] = h.n[k];
     J.cost[pix] = c;
   }
   st_count(P.counts, job, 1, (unsigned int)invalid);
+  if constexpr (GEOM) {
+    st_count(G.counts, job, 0, (unsigned int)capped);
+    st_count(G.counts, job, 1, (unsigned int)drawn);
+  }
 }
 
-__global__ void __launch_bounds__(ST_THREADS) pm_half_kernel(PmParams P, long long total)
+// One half-step.  The geometric pass keeps rho = 2^-k and draws at counter iteration 32 + k.
+template <bool GEOM>
+__device__ __forceinline__ void pm_half(PmParams P, long long total, PmGeom G)
 {
   const long long t = (long long)blockIdx.x * ST_THREADS + threadIdx.x;
-  int job = -1, invalid = 0;
+  int job = -1, invalid = 0, capped = 0;
   if (t < total) {
     job = st_find(P.jobs, P.numJobs, &StJob::half0, t);
     const StJob &J = P.jobs[job];
@@ -269,6 +406,7 @@ __global__ void __launch_bounds__(ST_THREADS) pm_half_kernel(PmParams P, long lo
     if (x < J.w) {
       const StImage &R = P.images[J.ref];
       const int pix = y * J.w + x;
+      const int it = GEOM ? ST_GEOM_IT0 + P.iteration : P.iteration;   // the draws' counter iteration
       double ray[3];
       st_ray(J.Kinv, x, y, ray);
       Hyp cur;
@@ -277,7 +415,7 @@ __global__ void __launch_bounds__(ST_THREADS) pm_half_kernel(PmParams P, long lo
       Hyp best = cur;
       float bestCost = J.cost[pix];
       auto consider = [&](const Hyp &h) {
-        const float c = st_cost(P, J, R, x, y, h, ray, &invalid);
+        const float c = st_eval<GEOM>(P, G, J, R, x, y, h, ray, &invalid, &capped);
         if (c < bestCost) { bestCost = c; best = h; }
       };
       // 1. propagation
@@ -303,14 +441,14 @@ __global__ void __launch_bounds__(ST_THREADS) pm_half_kernel(PmParams P, long lo
       const double rho = ldexp(1.0, -P.iteration);
       const double lo = 1.0 / (double)J.dmax, hi = 1.0 / (double)J.dmin;
       auto moved_depth = [&](int slot) {
-        const double u = st_draw(P.seed, J, x, y, P.iteration, slot);
+        const double u = st_draw(P.seed, J, x, y, it, slot);
         const double inv = fmin(fmax(1.0 / (double)cur.z + rho * (2.0 * u - 1.0) * (hi - lo), lo), hi);
         return (float)(1.0 / inv);
       };
       auto moved_normal = [&](int slot, float *n) {
         double m[3];
         for (int c = 0; c < 3; c++)
-          m[c] = (double)cur.n[c] + rho * (2.0 * st_draw(P.seed, J, x, y, P.iteration, slot + c) - 1.0);
+          m[c] = (double)cur.n[c] + rho * (2.0 * st_draw(P.seed, J, x, y, it, slot + c) - 1.0);
         st_face(m, ray, n);
       };
       Hyp h = cur;
@@ -323,13 +461,31 @@ __global__ void __launch_bounds__(ST_THREADS) pm_half_kernel(PmParams P, long lo
       moved_normal(5, h.n);
       consider(h);
       // 5. a fresh random hypothesis
-      consider(st_random(P, J, x, y, P.iteration, 8, ray));
+      consider(st_random(P, J, x, y, it, 8, ray));
       J.depth[pix] = best.z;
       for (int c = 0; c < 3; c++) J.normal[3 * (size_t)pix + c] = best.n[c];
       J.cost[pix] = bestCost;
     }
   }
   st_count(P.counts, job, 1, (unsigned int)invalid);
+  if constexpr (GEOM) st_count(G.counts, job, 0, (unsigned int)capped);
+}
+
+__global__ void __launch_bounds__(ST_THREADS) pm_start_kernel(PmParams P, long long total)
+{
+  pm_start<false>(P, total, PmGeom{});
+}
+__global__ void __launch_bounds__(ST_THREADS) pm_half_kernel(PmParams P, long long total)
+{
+  pm_half<false>(P, total, PmGeom{});
+}
+__global__ void __launch_bounds__(ST_THREADS) pm_geom_start_kernel(PmParams P, long long total, PmGeom G)
+{
+  pm_start<true>(P, total, G);
+}
+__global__ void __launch_bounds__(ST_THREADS) pm_geom_half_kernel(PmParams P, long long total, PmGeom G)
+{
+  pm_half<true>(P, total, G);
 }
 
 __global__ void __launch_bounds__(ST_THREADS) pm_final_kernel(PmParams P, long long total)
@@ -514,19 +670,23 @@ void inv3(const double *K, double *Ki)
 }
 
 // The tables of a call, built in c.h_stereo and uploaded to c.stereo: images, jobs (in input order, or sorted by ref
-// for fusion), sources; then the job counters; then, for fusion and on the device only, the point list's scratch.
+// for fusion), sources, and with priors the geometric table per source and the prior per job; then the job counters
+// (a second set with priors); then, for fusion and on the device only, the point list's scratch.
 struct StTables {
   StImage *images;
   StJob *jobs;
   StSrc *srcs;
-  StCounts *counts;
-  const StCounts *h_counts;   // the counters' pinned copy
+  StGeo *geo;
+  StPrior *priors;
+  StCounts *counts, *gcounts;
+  const StCounts *h_counts;   // the counters' pinned copy (both sets)
   unsigned int *masks, *ctaCounts, *total;
   long long allPixels, halfPixels;
 };
 
 int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
-              const double *ts, const cs_stereo_job *jobs, int numJobs, bool fusion, StTables &T)
+              const double *ts, const cs_stereo_job *jobs, int numJobs, bool fusion, const cs_depth_prior *priors,
+              StTables &T)
 {
   std::vector<int> order(numJobs);
   for (int p = 0; p < numJobs; p++) order[p] = p;
@@ -542,8 +702,10 @@ int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double 
   const int rows = (int)std::min<long long>(all, INT32_MAX);
   Layout L(256);
   const size_t oIm = L.take(sizeof(StImage) * numImages), oJob = L.take(sizeof(StJob) * numJobs),
-               oSrc = L.take(sizeof(StSrc) * std::max(S, 1)), tables = L.bytes;
-  const size_t oCnt = L.take(sizeof(StCounts) * numJobs), hostBytes = L.bytes;
+               oSrc = L.take(sizeof(StSrc) * std::max(S, 1));
+  const size_t oGeo = priors ? L.take(sizeof(StGeo) * std::max(S, 1)) : 0;
+  const size_t oPri = priors ? L.take(sizeof(StPrior) * numJobs) : 0, tables = L.bytes;
+  const size_t oCnt = L.take(sizeof(StCounts) * numJobs * (priors ? 2 : 1)), hostBytes = L.bytes;
   const size_t oMask = fusion ? L.take(4 * (size_t)list_words(rows)) : 0;
   const size_t oCta = fusion ? L.take(4 * (size_t)list_ctas(rows)) : 0, oTot = fusion ? L.take(4) : 0;
   int r;
@@ -552,6 +714,8 @@ int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double 
   StImage *im = reinterpret_cast<StImage *>(h + oIm);
   StJob *jb = reinterpret_cast<StJob *>(h + oJob);
   StSrc *sr = reinterpret_cast<StSrc *>(h + oSrc);
+  StGeo *ge = reinterpret_cast<StGeo *>(h + oGeo);
+  StPrior *pr = reinterpret_cast<StPrior *>(h + oPri);
   for (int a = 0; a < numImages; a++) {
     StImage &m = im[a];
     m.img = images[a].d_img;
@@ -574,6 +738,7 @@ int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double 
     for (int k = 0; k < 9; k++) j.Kinv[k] = Rf.Kinv[k];
     j.depth = J.d_depth; j.normal = J.d_normal; j.cost = J.d_cost;
     j.all0 = all; j.half0 = half;
+    if (priors) pr[q] = {priors[J.ref].d_depth, priors[J.ref].d_normal};
     all += (long long)j.w * j.h;
     half += (long long)((j.w + 1) / 2) * j.h;
     for (int s = 0; s < J.numSources; s++) {
@@ -598,6 +763,13 @@ int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double 
           e.A[3 * a + b] = (float)(KR[3 * a] * Rf.Kinv[b] + KR[3 * a + 1] * Rf.Kinv[3 + b] + KR[3 * a + 2] * Rf.Kinv[6 + b]);
         e.b[a] = (float)(Sm.K[3 * a] * tsr[0] + Sm.K[3 * a + 1] * tsr[1] + Sm.K[3 * a + 2] * tsr[2]);
       }
+      if (priors) {
+        StGeo &g = ge[s0 + s];
+        for (int k = 0; k < 9; k++) g.R[k] = Rsr[k];
+        for (int k = 0; k < 3; k++) g.t[k] = tsr[k];
+        g.depth = priors[e.image].d_depth;
+        g.w = Sm.w; g.h = Sm.h;
+      }
     }
     s0 += J.numSources;
   }
@@ -605,7 +777,10 @@ int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double 
   T.images = reinterpret_cast<StImage *>(d + oIm);
   T.jobs = reinterpret_cast<StJob *>(d + oJob);
   T.srcs = reinterpret_cast<StSrc *>(d + oSrc);
+  T.geo = priors ? reinterpret_cast<StGeo *>(d + oGeo) : nullptr;
+  T.priors = priors ? reinterpret_cast<StPrior *>(d + oPri) : nullptr;
   T.counts = reinterpret_cast<StCounts *>(d + oCnt);
+  T.gcounts = priors ? T.counts + numJobs : nullptr;
   T.h_counts = reinterpret_cast<const StCounts *>(h + oCnt);
   T.masks = fusion ? reinterpret_cast<unsigned int *>(d + oMask) : nullptr;
   T.ctaCounts = fusion ? reinterpret_cast<unsigned int *>(d + oCta) : nullptr;
@@ -617,35 +792,64 @@ int st_tables(DeviceCtx &c, const cs_image *images, int numImages, const double 
 
 }  // namespace
 
-int patch_match_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
-                        const double *ts, const cs_stereo_job *jobs, int numJobs, int radius, int step,
-                        int numIterations, int topK, unsigned long long seed, const unsigned long long **counts)
+namespace {
+
+// The launches of a PatchMatch call (start, the half-steps, the final count) and the counters' copy back; with G the
+// geometric kernels.
+int pm_launch(DeviceCtx &c, const StTables &T, PmParams P, int numIterations, const PmGeom *G,
+              const unsigned long long **counts)
 {
-  StTables T;
-  int r;
-  if ((r = st_tables(c, images, numImages, Ks, Rs, ts, jobs, numJobs, false, T)) < 0) return r;
-  CS_CUDA(cudaMemsetAsync(T.counts, 0, sizeof(StCounts) * numJobs, c.stream));
-  PmParams P{T.images, T.jobs, T.srcs, T.counts, numJobs, radius, step, topK, seed, 0, 0};
+  const int sets = G ? 2 : 1;
+  CS_CUDA(cudaMemsetAsync(T.counts, 0, sizeof(StCounts) * P.numJobs * sets, c.stream));
   const unsigned int gAll = (unsigned int)((T.allPixels + ST_THREADS - 1) / ST_THREADS);
   const unsigned int gHalf = (unsigned int)((T.halfPixels + ST_THREADS - 1) / ST_THREADS);
-  pm_start_kernel<<<gAll, ST_THREADS, 0, c.stream>>>(P, T.allPixels);
+  if (G) pm_geom_start_kernel<<<gAll, ST_THREADS, 0, c.stream>>>(P, T.allPixels, *G);
+  else pm_start_kernel<<<gAll, ST_THREADS, 0, c.stream>>>(P, T.allPixels);
   count_launch();
   CS_CUDA(cudaGetLastError());
   for (int it = 1; it <= numIterations; it++)
     for (int colour = 0; colour < 2; colour++) {
       P.iteration = it;
       P.colour = colour;
-      pm_half_kernel<<<gHalf, ST_THREADS, 0, c.stream>>>(P, T.halfPixels);
+      if (G) pm_geom_half_kernel<<<gHalf, ST_THREADS, 0, c.stream>>>(P, T.halfPixels, *G);
+      else pm_half_kernel<<<gHalf, ST_THREADS, 0, c.stream>>>(P, T.halfPixels);
       count_launch();
       CS_CUDA(cudaGetLastError());
     }
   pm_final_kernel<<<gAll, ST_THREADS, 0, c.stream>>>(P, T.allPixels);
   count_launch();
   CS_CUDA(cudaGetLastError());
-  CS_CUDA(cudaMemcpyAsync(const_cast<StCounts *>(T.h_counts), T.counts, sizeof(StCounts) * numJobs,
+  CS_CUDA(cudaMemcpyAsync(const_cast<StCounts *>(T.h_counts), T.counts, sizeof(StCounts) * P.numJobs * sets,
                           cudaMemcpyDeviceToHost, c.stream));
   *counts = T.h_counts->v;
   return 0;
+}
+
+}  // namespace
+
+int patch_match_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                        const double *ts, const cs_stereo_job *jobs, int numJobs, int radius, int step,
+                        int numIterations, int topK, unsigned long long seed, const unsigned long long **counts)
+{
+  StTables T;
+  int r;
+  if ((r = st_tables(c, images, numImages, Ks, Rs, ts, jobs, numJobs, false, nullptr, T)) < 0) return r;
+  const PmParams P{T.images, T.jobs, T.srcs, T.counts, numJobs, radius, step, topK, seed, 0, 0};
+  return pm_launch(c, T, P, numIterations, nullptr, counts);
+}
+
+int patch_match_geometric_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks,
+                                  const double *Rs, const double *ts, const cs_depth_prior *priors,
+                                  const cs_stereo_job *jobs, int numJobs, int radius, int step, int numIterations,
+                                  int topK, double geomWeight, double geomMaxError, unsigned long long seed,
+                                  const unsigned long long **counts)
+{
+  StTables T;
+  int r;
+  if ((r = st_tables(c, images, numImages, Ks, Rs, ts, jobs, numJobs, false, priors, T)) < 0) return r;
+  const PmParams P{T.images, T.jobs, T.srcs, T.counts, numJobs, radius, step, topK, seed, 0, 0};
+  const PmGeom G{T.geo, T.priors, T.gcounts, (float)geomWeight, geomMaxError};
+  return pm_launch(c, T, P, numIterations, &G, counts);
 }
 
 int fuse_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const double *Ks, const double *Rs,
@@ -655,7 +859,7 @@ int fuse_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const doub
 {
   StTables T;
   int r;
-  if ((r = st_tables(c, images, numImages, Ks, Rs, ts, jobs, numJobs, true, T)) < 0) return r;
+  if ((r = st_tables(c, images, numImages, Ks, Rs, ts, jobs, numJobs, true, nullptr, T)) < 0) return r;
   FuParams P;
   P.images = T.images; P.jobs = T.jobs; P.srcs = T.srcs; P.numJobs = numJobs;
   P.maxCost = maxCost; P.minConsistent = minConsistent;

@@ -1043,6 +1043,47 @@ int cs_patch_match_stereo(const cs_image *images, int numImages, const double *K
                           const cs_stereo_job *jobs, int numJobs, int windowRadius, int windowStep, int numIterations,
                           int topK, unsigned long long seed, long long *stats_out, double *ms);
 
+/* A prior depth map of an image: d_depth [H][W] and d_normal [H][W][3], dense device floats of the image's size. */
+typedef struct {
+  const float *d_depth;    /* NULL: the image has no prior */
+  const float *d_normal;   /* needed only for an image that is the ref of a job */
+} cs_depth_prior;
+
+/* PatchMatch stereo with geometric consistency (Schoenberger et al., ECCV 2016: COLMAP's second pass): every job's
+ * maps again, each view's cost joined by a forward-backward reprojection error against that source's prior depth map.
+ * Images, cameras, jobs and window are cs_patch_match_stereo's; the jobs' d_depth, d_normal and d_cost are outputs
+ * only.  priors [numImages] are read only, and per image, so a call may refine some refs and read the priors of all.
+ * - Geometric error of hypothesis h = (z, n) at pixel (x, y) of ref r in source s, in float64: X = z Kinv_r (x, y, 1);
+ *   Y = R_sr X + t_sr (R_sr = R_s R_r^T, t_sr = t_s - R_sr t_r, from the double cameras); (u, v) = (K_s Y)_0,1 / Y_z;
+ *   q = (floor(u + 0.5), floor(v + 0.5)); z_s the prior depth of s at q; X_s = z_s Kinv_s (u, v, 1) (the continuous
+ *   (u, v), so a consistent pair gives an error near 0); Z = R_sr^T (X_s - t_sr); (u', v') = (K_r Z)_0,1 / Z_z;
+ *   e = hypot(u' - x, v' - y) and g = (float) min(e, geomMaxError).  g = geomMaxError when Y_z <= 0 or Z_z <= 0, q lies
+ *   outside s, s has no prior, or z_s is not finite or <= 0 (depth 0 masks a pixel out).
+ * - View cost: fmaf(lambda, g, c_photo) with lambda = (float) geomWeight, c_photo the photometric view cost (2 for an
+ *   invalid view, which still carries its g).  Aggregation (the mean of the topK smallest, in ascending order) and
+ *   selection are cs_patch_match_stereo's.
+ * - Start: each pixel takes its ref's prior (z_p, n_p) bit for bit when z_p is in [depthMin, depthMax], n_p is finite,
+ *   n_p . ray < 0 and | |n_p| - 1 | <= 1e-3 (in float64 from the floats); otherwise the random hypothesis of counter
+ *   iteration 32, slot 0.  Either way it gets its combined cost.
+ * - Iterations k = 1 .. numIterations: cs_patch_match_stereo's candidate list, order and rho = 2^-k, with the draws at
+ *   counter iteration 32 + k, so the two passes' draws differ under the same seed.  The priors are inputs, never state:
+ *   two calls give the same bytes, and a job's maps are the same alone or in any batch given the same priors.
+ * - stats_out [numJobs][5] (may be NULL): pixels, invalid view evaluations, pixels whose final cost is >= 2,
+ *   photometrically valid view evaluations whose g is geomMaxError, pixels started from a random hypothesis.
+ * - Launches: 2 + 2 numIterations (start, the half-steps, a final count); the call synchronises once; *ms (may be
+ *   NULL) gets its event time.  Scratch: cs_patch_match_stereo's tables, plus 112 bytes per source (R_sr, t_sr, the
+ *   source's prior and size) and 16 per job (the ref's prior), and 48 bytes per job of counters; the same pinned.
+ *   numJobs == 0 makes no CUDA call.
+ * - CS_E_ARG, before any CUDA call: cs_patch_match_stereo's checks, but numIterations outside [0, 31]; NULL priors with
+ *   jobs; a job whose ref has a NULL prior d_depth or d_normal; a prior pointer that is not 4-byte aligned;
+ *   geomWeight not finite or < 0; geomMaxError not finite or <= 0; then an overlap of a map with any other map, any
+ *   prior or any image (one sweep; priors may overlap each other and the images). */
+int cs_patch_match_stereo_geometric(const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                                    const double *ts, const cs_depth_prior *priors, const cs_stereo_job *jobs,
+                                    int numJobs, int windowRadius, int windowStep, int numIterations, int topK,
+                                    double geomWeight, double geomMaxError, unsigned long long seed,
+                                    long long *stats_out, double *ms);
+
 /* Fusion of the depth maps of cs_patch_match_stereo into one point cloud (COLMAP's stereo_fusion, as a parallel rule
  * whose order follows from the values): jobs, their maps and the images as that call left them.
  * - Pixel p = (x, y) of job a (image a = jobs[.].ref) with cost <= maxCost back-projects to X_p = R_a^T (z Kinv_a

@@ -2,7 +2,9 @@
 per-pixel rate on the CPU (the host arm).  Workload: --maps reference images of --width x --height, each with
 --sources sources (the others of a ring), window radius 5 at step 1 and radius 4 at step 2 (the radius must be a
 multiple of the step), --iterations iterations; medians of
---calls calls after one warm-up call.  Times are device events.  Prints one JSON line."""
+--calls calls after one warm-up call.  Then the geometric-consistency pass on the same workload (radius 5, step 1,
+--iterations iterations) from the step-1 photometric maps, and its time over the photometric one's.  Times are device
+events.  Prints one JSON line."""
 import argparse
 import json
 import os
@@ -55,16 +57,23 @@ def main():
     images = [synth.synth_image(W, H, seed=100 + k) for k in range(n)]
     jobs = [(r, [(r + 1 + k) % n for k in range(a.sources)], 4.0, 9.0) for r in range(a.maps)]
     out = dict(gpu=gpu_info(), maps=a.maps, sources=a.sources, width=W, height=H, iterations=a.iterations)
+    maps = None
     for r, step in ((5, 1), (4, 2)):
         cs.PatchMatchStereo(images, Ks, Rs, ts, jobs, windowRadius=r, windowStep=step, numIterations=1)
-        ms = [cs.PatchMatchStereo(images, Ks, Rs, ts, jobs, windowRadius=r, windowStep=step,
-                                  numIterations=a.iterations)[4] for _ in range(a.calls)]
-        t = float(np.median(ms))
+        runs = [cs.PatchMatchStereo(images, Ks, Rs, ts, jobs, windowRadius=r, windowStep=step,
+                                    numIterations=a.iterations) for _ in range(a.calls)]
+        maps = maps or runs[-1]
+        t = float(np.median([run[4] for run in runs]))
         side = 2 * r // step + 1
         # window samples: per pixel and iteration 12 candidates (fewer at the border), each over every source
         samples = a.maps * W * H * (1 + 12 * a.iterations) * a.sources * side * side
         out["ms_per_map_step%d" % step] = t / a.maps
         out["samples_per_s_step%d" % step] = samples / (t * 1e-3)
+    cs.PatchMatchStereoGeometric(images, Ks, Rs, ts, jobs, maps[0], maps[1], windowRadius=5, numIterations=1)
+    geo = [cs.PatchMatchStereoGeometric(images, Ks, Rs, ts, jobs, maps[0], maps[1], windowRadius=5,
+                                        numIterations=a.iterations)[4] for _ in range(a.calls)]
+    out["ms_per_map_geometric"] = float(np.median(geo)) / a.maps
+    out["geometric_over_photometric"] = out["ms_per_map_geometric"] / out["ms_per_map_step1"]
     d, nrm, c, _, _ = cs.PatchMatchStereo(images, Ks, Rs, ts, jobs, windowRadius=4, windowStep=2, numIterations=2)
     fus = [cs.FuseDepthMaps(images, Ks, Rs, ts, jobs, d, nrm, c, maxPoints=1 << 20)[5] for _ in range(a.calls)]
     out["fusion_ms"] = float(np.median(fus))
