@@ -969,4 +969,43 @@ int fuse_args(const char *fn, const cs_image *images, int numImages, const doubl
   return rs.check(fn);
 }
 
+int mesh_args(const char *fn, const float *xyz, const float *normal, const float *intensity, int numPoints, int depth,
+              double scale, int maxIterations, double tol, double trim, const float *vertices,
+              const float *vertexIntensity, int maxVertices, const int *triangles, int maxTriangles, const float *chi)
+{
+  if (numPoints < 0 || numPoints > (1 << 30)) return arg_error(fn, "numPoints must be in [0, 2^30]");
+  if (depth < 4 || depth > 9) return arg_error(fn, "depth must be in [4, 9]");
+  if (!std::isfinite(scale) || scale < 1.0 || scale > 4.0) return arg_error(fn, "scale must be finite and in [1, 4]");
+  if (maxIterations < 1 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [1, 1000]");
+  if (!(tol > 0.0 && tol < 1.0)) return arg_error(fn, "tol must be in (0, 1)");
+  if (!std::isfinite(trim) || trim < 0.0) return arg_error(fn, "trim must be finite and >= 0");
+  if (maxVertices < 0) return arg_error(fn, "maxVertices must be >= 0");
+  if (maxTriangles < 0) return arg_error(fn, "maxTriangles must be >= 0");
+  if (numPoints > 0 && (!xyz || misaligned(xyz, 4)))
+    return arg_error(fn, "numPoints > 0 needs d_xyz (4-byte aligned)");
+  if (numPoints > 0 && (!normal || misaligned(normal, 4)))
+    return arg_error(fn, "numPoints > 0 needs d_normal (4-byte aligned)");
+  if (maxVertices > 0 && (!vertices || misaligned(vertices, 4)))
+    return arg_error(fn, "maxVertices > 0 needs d_vertices (4-byte aligned)");
+  if (maxTriangles > 0 && (!triangles || misaligned(triangles, 4)))
+    return arg_error(fn, "maxTriangles > 0 needs d_triangles (4-byte aligned)");
+  if (misaligned(intensity, 4)) return arg_error(fn, "d_intensity must be 4-byte aligned");
+  if (misaligned(vertexIntensity, 4)) return arg_error(fn, "d_vertexIntensity must be 4-byte aligned");
+  if (misaligned(chi, 4)) return arg_error(fn, "d_chi must be 4-byte aligned");
+  if (!intensity != !vertexIntensity)
+    return arg_error(fn, "d_intensity and d_vertexIntensity must be given together or not at all");
+  static const char *const names[7] = {"d_vertices", "d_vertexIntensity", "d_triangles", "d_chi",
+                                       "d_xyz", "d_normal", "d_intensity"};
+  ArgRanges rs(names, 7);
+  const size_t n1 = ((size_t)1 << depth) + 1, P = (size_t)numPoints, V = (size_t)maxVertices;
+  rs.add(vertices, 12 * V, 0, 0, true);
+  if (vertexIntensity) rs.add(vertexIntensity, 4 * V, 1, 0, true);
+  rs.add(triangles, 12 * (size_t)maxTriangles, 2, 0, true);
+  if (chi) rs.add(chi, 4 * n1 * n1 * n1, 3, 0, true);
+  rs.add(xyz, 12 * P, 4, 0, false);
+  rs.add(normal, 12 * P, 5, 0, false);
+  if (intensity) rs.add(intensity, 4 * P, 6, 0, false);
+  return rs.check(fn);
+}
+
 }  // namespace cs

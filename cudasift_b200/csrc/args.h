@@ -85,6 +85,10 @@ int fuse_args(const char *fn, const cs_image *images, int numImages, const doubl
               const double *ts, const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent,
               double maxReprojError, double maxDepthError, double maxNormalErrorDeg, const float *xyz,
               const float *normal, const float *intensity, const int *source, int maxPoints);
+// cs_poisson_mesh: the points, the parameters, the buffers and the range sweep.
+int mesh_args(const char *fn, const float *xyz, const float *normal, const float *intensity, int numPoints, int depth,
+              double scale, int maxIterations, double tol, double trim, const float *vertices,
+              const float *vertexIntensity, int maxVertices, const int *triangles, int maxTriangles, const float *chi);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

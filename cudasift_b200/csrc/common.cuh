@@ -421,6 +421,8 @@ struct DeviceCtx {
   // counters and the point list's scratch
   GrowBuffer stereo;
   PinnedBuffer h_stereo;                   // the same tables (uploaded), then the counters (copied back)
+  // cs_poisson_mesh: the result words (copied back); its grid-sized scratch is allocated and freed per call
+  PinnedBuffer h_mesh;
 
   // pinned host words, allocated by ensure()
   unsigned int *h_counters = nullptr;      // 4: extraction, describe and rank counters
@@ -714,6 +716,17 @@ int fuse_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const doub
                  const double *ts, const cs_stereo_job *jobs, int numJobs, float maxCost, int minConsistent,
                  double maxReprojError, double maxDepthError, double maxNormalErrorDeg, float *xyz, float *normal,
                  float *intensity, int *source, int maxPoints, unsigned int **total);
+
+// ---- Poisson meshing (mesh.cu) -------------------------------------------------------------------------------------
+// The launches of cs_poisson_mesh (argument-checked) on st, with the scratch allocated and freed on st, without a
+// synchronize; the result words (mesh_result_bytes of them) reach h_result (pinned) by the caller's synchronize.
+int mesh_run(const float *xyz, const float *normal, const float *intensity, int numPoints, int depth, double scale,
+             int maxIterations, double tol, double trim, float *vertices, float *vertexIntensity, int maxVertices,
+             int *triangles, int maxTriangles, float *chiOut, cudaStream_t st, void *h_result);
+size_t mesh_result_bytes();
+// after the synchronize: info_out and stats_out (either may be NULL); returns the full triangle count
+int mesh_result(const void *h_result, int numPoints, int maxVertices, int maxTriangles, double info[7],
+                long long stats[10]);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

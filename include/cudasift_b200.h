@@ -1115,6 +1115,86 @@ int cs_fuse_depth_maps(const cs_image *images, int numImages, const double *Ks, 
                        double maxDepthError, double maxNormalErrorDeg, float *d_xyz, float *d_normal,
                        float *d_intensity, int *d_source, int maxPoints, long long stats_out[2], double *ms);
 
+/* Poisson surface reconstruction (Kazhdan, Bolitho & Hoppe, SGP 2006) of an oriented point cloud, such as the output
+ * of cs_fuse_depth_maps, on a dense regular grid: a closed, oriented triangle mesh.  The grid is dense, so the
+ * resolution is capped at 512 cells per axis (no octree); there is no screening term and no per-point weight.
+ * - Used points: d_xyz [numPoints][3], d_normal [numPoints][3] (device floats, outward normals of any length) and
+ *   d_intensity [numPoints] (may be NULL).  Point i is used when its six coordinates are finite and |n| > 0; its unit
+ *   normal n^ = n / |n| is computed in float64 from the floats.
+ * - Grid: N = 2^depth cells per axis, (N + 1)^3 nodes, node (i, j, k) at index (k (N + 1) + j) (N + 1) + i.  In float64:
+ *   lo, hi the component-wise min and max of the used xyz (exact in any order), c = (lo + hi) / 2, E = max(hi - lo),
+ *   L = max(scale, N / (N - 8)) E (at least 4 cells of margin on every side), h = L / N, o = c - L / 2, and a point's
+ *   grid coordinate g = (p - o) / h.  No used point, or E = 0: status 1, no triangles, info_out zero, chi zero.
+ * - Splat (a gather, no atomics): the used points sorted by cell floor(g) (index (c_z N + c_y) N + c_x) with a stable
+ *   radix sort, so ties keep the point order.  Node q sums over the points of its (up to 8) incident cells, cells in
+ *   ascending index and points in sorted order, with weight w = prod_a (1 - |g_a - q_a|): V(q) = sum w n^,
+ *   D(q) = sum w and, with intensities, S(q) = sum w I, each accumulated in float64 and rounded to float once.
+ * - System: chi = 0 on the boundary nodes; at each interior node 6 chi_q - sum of the 6 neighbours = b_q with
+ *   b_q = (h / 2) sum_a (V_a(q + e_a) - V_a(q - e_a)) (h^2 times the central-difference divergence), in float64 from
+ *   the float V, rounded to float, summed as (x + y) + z.  With outward normals chi is larger inside.
+ * - Solve: CG from chi = 0 preconditioned by one geometric-multigrid V-cycle (MGPCG; McAdams, Sifakis & Teran, SCA
+ *   2010).  Vectors are float32; every dot product and norm is float64.  Levels of n = N, N / 2, ..., 4 cells, each with
+ *   the 7-point operator above (6 x - neighbours, boundary 0).  On a level, from x = 0: 2 pairs of red-black
+ *   Gauss-Seidel half-sweeps (red: (i + j + k) even; x = (f + neighbours) / 6 in float), the residual t = f - A x, the
+ *   coarse right-hand side (1/2) P^T t (P trilinear prolongation: the 27 fine nodes 2Q + d weigh prod (1 - |d_a| / 2)),
+ *   the V-cycle on the coarser level, x += P x_c, then 2 pairs of black-red half-sweeps.  The coarsest level (4 cells)
+ *   runs 8 red-black pairs then 8 black-red pairs.  The sweep sequence is a palindrome and the restriction is a
+ *   multiple of P^T, so the preconditioner is symmetric positive definite.  CG: r = b, z = M r, p = z; per iteration
+ *   q = A p, alpha = r.z / p.q (stop when p.q is not > 0), chi += alpha p, r -= alpha q (each in float64 from the
+ *   floats, rounded to float), then it stops when r.r <= tol^2 b.b (the recurrence residual) or after maxIterations;
+ *   else z = M r, beta = r.z(new) / r.z(old), p = z + beta p.  alpha, beta and the stop test are computed on the
+ *   device.  After the loop the true relative residual |b - A chi| / |b| (0 when b = 0) in float64 from the floats.
+ * - Iso-value: tau the mean over the used points of chi trilinear at g (cell clamp(floor(g), 0, N - 1), corners z outer,
+ *   x inner), the mean density the same of D, summed in float64 in sorted order.  tau <= 0 (inconsistent normals, b = 0,
+ *   or an open surface seen from one side, whose points lie where chi < 0): status 2, no triangles.
+ * - Extraction (marching tetrahedra, Doi & Koide 1991, on the Freudenthal split: no case table, no ambiguous case): a
+ *   node is inside when (double) chi_q >= tau.  The lattice edges of node q go to q + delta for delta in the order
+ *   (1,0,0), (0,1,0), (0,0,1), (1,1,0), (1,0,1), (0,1,1), (1,1,1); edge id 7 index(q) + direction.  Every edge whose
+ *   ends differ in inside has a vertex at t = (tau - chi_a) / (chi_b - chi_a) (float64 from the floats), position
+ *   o + h (q + t delta) rounded to float; vertices are listed in ascending edge id.  Cell q0 splits into 6 tetrahedra,
+ *   one per axis permutation pi in lexicographic order, with corners q0, q0 + e_pi1, q0 + e_pi1 + e_pi2, q0 + (1,1,1).
+ *   One or three inside corners: one triangle on the three edges of the lone corner a, vertices in the order of the
+ *   other corners along the chain.  Two inside corners a, b and two outside c, d (chain order): the quad
+ *   (ac, ad, bd, bc), split along the diagonal ac-bd into (ac, ad, bd), (ac, bd, bc).  Orientation, decided on the
+ *   edge midpoints: (v1 - v0) x (v2 - v0) points to the outside corners (else the cycle is reversed after its first
+ *   vertex).  Triangles are listed in ascending (cell, tetrahedron, k).  Since tau > 0 and the boundary is 0, the mesh
+ *   is combinatorially a closed, oriented 2-manifold for any values; exact ties (t = 0) give zero-area triangles.
+ * - Trim (COLMAP's trim on a dense grid): a vertex's density is D_a + t (D_b - D_a) in float64; a triangle with a vertex
+ *   of density < trim x mean density is dropped; vertices no kept triangle uses are dropped, the rest keep their
+ *   order and the triangles are renumbered.  trim = 0 drops nothing.
+ * - Vertex intensity (with d_intensity and d_vertexIntensity): (S_a + t (S_b - S_a)) / (D_a + t (D_b - D_a)), 0 when
+ *   the denominator is 0.
+ * - Outputs: d_vertices [][3] float, d_triangles [][3] int32 (indices into the full trimmed vertex list, so a written
+ *   triangle may name a vertex at or beyond maxVertices) and d_vertexIntensity [], each the prefix of its full list
+ *   (at most maxVertices or maxTriangles entries).  d_chi [(N + 1)^3] (may be NULL): chi.  info_out [7] (may be NULL):
+ *   {o_x, o_y, o_z, h, tau, mean density, true relative residual}.  stats_out [10] (may be NULL): used points, refused
+ *   points, CG iterations, vertices and triangles before trimming, vertices and triangles after trimming (the full
+ *   counts), vertices written, triangles written, status (0 ok, 1 no used point or zero extent, 2 tau <= 0, 3 not
+ *   converged: the mesh is still extracted).  Returns the full trimmed triangle count, or CS_E_*.
+ * - Determinism: no floating-point atomics (integer atomics for the box, the cell histogram and the kept-vertex bits,
+ *   whose results do not depend on order); totals over nodes or points sum tiles of 2048 items (a thread adds items
+ *   thread + 256 m in order, then warp butterflies and the warps in order), then groups of 256 tile partials the same
+ *   way, then the group partials (lane-strided in ascending order and a butterfly): the order depends on N and the
+ *   used count only, so two calls give the same bytes.
+ * - Launches: 10 kernel launches (cs_launch_count) whatever the depth and the data (box, keys, points, splat,
+ *   right-hand side, one cooperative solve kernel, two counts, vertices, triangles), plus cub's sort and scans (not
+ *   counted).  The lists are written by per-block counts, cub::DeviceScan and a write pass.  The call synchronises
+ *   once; *ms (may be NULL) gets its event time.
+ * - Scratch, allocated on the call's stream and freed before it returns (no grid-sized memory is kept): 4 x 7 bytes
+ *   per node (8 with intensities: chi, r, b, the three V components reused as z, p, q, D, S), 12 per node of every
+ *   coarser level, 1 per node (kept-vertex bits), 64 per block of 256 nodes, 68 bytes per point (64 without
+ *   intensities), the sort and scan storage: about 4.3 GB at depth 9 (513^3 nodes) with intensities.
+ * - CS_E_ARG, before any CUDA call, naming the argument: numPoints outside [0, 2^30], depth outside [4, 9], scale not
+ *   finite or outside [1, 4], maxIterations outside [1, 1000], tol not in (0, 1), trim not finite or < 0, maxVertices
+ *   or maxTriangles < 0, NULL or not 4-byte aligned d_xyz or d_normal with numPoints > 0, d_vertices with
+ *   maxVertices > 0, d_triangles with maxTriangles > 0, a misaligned d_intensity, d_vertexIntensity or d_chi, one of
+ *   d_intensity and d_vertexIntensity given without the other, and an output (d_vertices, d_vertexIntensity,
+ *   d_triangles, d_chi) that overlaps another output or an input (one sweep over sorted ranges). */
+int cs_poisson_mesh(const float *d_xyz, const float *d_normal, const float *d_intensity, int numPoints, int depth,
+                    double scale, int maxIterations, double tol, double trim, float *d_vertices,
+                    float *d_vertexIntensity, int maxVertices, int *d_triangles, int maxTriangles, float *d_chi,
+                    double info_out[7], long long stats_out[10], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
