@@ -23,7 +23,8 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "MatchSiftDataGuidedBatch", "TrackList", "BuildTracks", "TriangulateTracks", "PoseJob", "AbsolutePoseBatch",
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
            "RetrievePairs", "RotationAveraging", "GlobalPositioning", "UndistortImages", "PatchMatchStereo",
-           "PatchMatchStereoGeometric", "FuseDepthMaps", "SelectStereoViews", "PoissonMesh"]
+           "PatchMatchStereoGeometric", "FuseDepthMaps", "SelectStereoViews", "PoissonMesh",
+           "PoissonMeshScreened"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -119,6 +120,8 @@ def lib():
                                     vp, ip, vp, c.POINTER(c.c_double)]),
         "cs_poisson_mesh": (ip, [vp, vp, vp, ip, ip, c.c_double, ip, c.c_double, c.c_double, vp, vp, ip, vp, ip, vp,
                                  vp, vp, c.POINTER(c.c_double)]),
+        "cs_poisson_mesh_screened": (ip, [vp, vp, vp, ip, ip, c.c_double, c.c_double, ip, c.c_double, c.c_double, vp,
+                                          vp, ip, vp, ip, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1336,17 +1339,10 @@ def FuseDepthMaps(images, Ks, Rs, ts, jobs, depth, normal, cost, maxCost=0.5, mi
     return xyz, nrm, inten, src, n, ms.value
 
 
-def PoissonMesh(xyz, normal, intensity=None, depth=8, scale=1.1, maxIterations=200, tol=1e-5, trim=0.0,
-                returnChi=False):
-    """A closed, oriented triangle mesh of an oriented point cloud (cs_poisson_mesh): Poisson reconstruction on a
-    regular grid of 2^depth cells per axis, solved by multigrid-preconditioned CG to tol, the surface at the mean of
-    chi over the points, extracted by marching tetrahedra; triangles with a vertex whose splatted density is below trim
-    times the mean density are dropped.  xyz and normal are float32 [P, 3] host arrays (outward normals, any length),
-    intensity [P] or None, as FuseDepthMaps returns them.  The output buffers first hold 12 N^2 vertices and 24 N^2
-    triangles (N = 2^depth); a mesh with more is computed again into buffers of its full size, so nothing is
-    truncated.  Returns (vertices float32 [V, 3], triangles int32 [T, 3], vertex intensity float32 [V] or None,
-    info float64 [7] {o_x, o_y, o_z, h, tau, mean density, true relative residual}, stats int64 [10] (the header's),
-    chi float32 [N + 1, N + 1, N + 1] indexed (z, y, x) or None, ms)."""
+def _poisson_call(call, name, nInfo, xyz, normal, intensity, depth, returnChi):
+    """The host side of cs_poisson_mesh and cs_poisson_mesh_screened: upload, call(ins, outs, maxV, maxT, info, stats,
+    ms) into output buffers of 12 N^2 vertices and 24 N^2 triangles, again into buffers of the full size while the mesh
+    is larger, and download."""
     X = np.ascontiguousarray(np.asarray(xyz, np.float32).reshape(-1, 3))
     Nr = np.ascontiguousarray(np.asarray(normal, np.float32).reshape(-1, 3))
     if len(Nr) != len(X):
@@ -1357,22 +1353,19 @@ def PoissonMesh(xyz, normal, intensity=None, depth=8, scale=1.1, maxIterations=2
     P, n = len(X), (1 << int(depth)) + 1 if 4 <= int(depth) <= 9 else 17
     maxV, maxT = 12 * (n - 1) ** 2, 24 * (n - 1) ** 2
     ins = [DeviceBuffer(max(X.nbytes, 4)), DeviceBuffer(max(Nr.nbytes, 4))] + ([DeviceBuffer(max(I.nbytes, 4))]
-                                                                               if I is not None else [])
+                                                                               if I is not None else [None])
     try:
         for b, a in zip(ins, (X, Nr, I)):
-            if P:
+            if P and b is not None:
                 b.upload(a)
         while True:
             outs = [DeviceBuffer(12 * maxV + 4), DeviceBuffer(12 * maxT + 4),
                     DeviceBuffer(4 * maxV + 4) if I is not None else None,
                     DeviceBuffer(4 * n ** 3) if returnChi else None]
             try:
-                info, stats, ms = np.zeros(7), np.zeros(10, np.int64), ctypes.c_double(0.0)
-                T = _check(lib().cs_poisson_mesh(ins[0].ptr, ins[1].ptr, ins[2].ptr if I is not None else None, P,
-                                                 int(depth), float(scale), int(maxIterations), float(tol), float(trim),
-                                                 outs[0].ptr, outs[2].ptr if outs[2] else None, maxV, outs[1].ptr,
-                                                 maxT, outs[3].ptr if outs[3] else None, _ptr(info), _ptr(stats),
-                                                 ctypes.byref(ms)), "PoissonMesh")
+                info, stats, ms = np.zeros(nInfo), np.zeros(10, np.int64), ctypes.c_double(0.0)
+                T = _check(call(*[b.ptr if b is not None else None for b in ins + outs], P, maxV, maxT, _ptr(info),
+                                _ptr(stats), ctypes.byref(ms)), name)
                 V = int(stats[5])
                 if V > maxV or T > maxT:
                     maxV, maxT = max(V, maxV), max(T, maxT)
@@ -1388,7 +1381,40 @@ def PoissonMesh(xyz, normal, intensity=None, depth=8, scale=1.1, maxIterations=2
                         b.free()
     finally:
         for b in ins:
-            b.free()
+            if b is not None:
+                b.free()
+
+
+def PoissonMesh(xyz, normal, intensity=None, depth=8, scale=1.1, maxIterations=200, tol=1e-5, trim=0.0,
+                returnChi=False):
+    """A closed, oriented triangle mesh of an oriented point cloud (cs_poisson_mesh): Poisson reconstruction on a
+    regular grid of 2^depth cells per axis, solved by multigrid-preconditioned CG to tol, the surface at the mean of
+    chi over the points, extracted by marching tetrahedra; triangles with a vertex whose splatted density is below trim
+    times the mean density are dropped.  xyz and normal are float32 [P, 3] host arrays (outward normals, any length),
+    intensity [P] or None, as FuseDepthMaps returns them.  The output buffers first hold 12 N^2 vertices and 24 N^2
+    triangles (N = 2^depth); a mesh with more is computed again into buffers of its full size, so nothing is
+    truncated.  Returns (vertices float32 [V, 3], triangles int32 [T, 3], vertex intensity float32 [V] or None,
+    info float64 [7] {o_x, o_y, o_z, h, tau, mean density, true relative residual}, stats int64 [10] (the header's),
+    chi float32 [N + 1, N + 1, N + 1] indexed (z, y, x) or None, ms)."""
+    def call(x, nr, inten, verts, tris, vint, chi, P, maxV, maxT, info, stats, ms):
+        return lib().cs_poisson_mesh(x, nr, inten, P, int(depth), float(scale), int(maxIterations), float(tol),
+                                     float(trim), verts, vint, maxV, tris, maxT, chi, info, stats, ms)
+    return _poisson_call(call, "PoissonMesh", 7, xyz, normal, intensity, depth, returnChi)
+
+
+def PoissonMeshScreened(xyz, normal, intensity=None, depth=8, scale=1.1, pointWeight=4.0, maxIterations=200, tol=1e-5,
+                        trim=0.0, returnChi=False):
+    """A triangle mesh of an oriented point cloud by screened Poisson reconstruction with a Neumann boundary
+    (cs_poisson_mesh_screened): PoissonMesh's grid, splat, solver and extraction, with chi pulled towards 0 at the
+    points by pointWeight (alpha; the effective weight is alpha over the mean density) and no boundary value, so open
+    surfaces seen from one side get a mesh; untrimmed, such a mesh ends on the grid's faces, and trim cuts it back to
+    where the points are.  Arguments and returns as PoissonMesh's, with info float64 [8]: PoissonMesh's 7 entries,
+    then the effective weight omega."""
+    def call(x, nr, inten, verts, tris, vint, chi, P, maxV, maxT, info, stats, ms):
+        return lib().cs_poisson_mesh_screened(x, nr, inten, P, int(depth), float(scale), float(pointWeight),
+                                              int(maxIterations), float(tol), float(trim), verts, vint, maxV, tris,
+                                              maxT, chi, info, stats, ms)
+    return _poisson_call(call, "PoissonMeshScreened", 8, xyz, normal, intensity, depth, returnChi)
 
 
 def SelectStereoViews(Ks, Rs, ts, offsets, members, points, numSources=8, minTriAngle=1.0):

@@ -1732,11 +1732,35 @@ int cs_poisson_mesh(const float *d_xyz, const float *d_normal, const float *d_in
   if (!c) return err;
   if ((r = c->h_mesh.grow(mesh_result_bytes())) < 0) return r;
   if ((r = timed_sync(fn, c, ms, [&] {
-         return mesh_run(d_xyz, d_normal, d_intensity, numPoints, depth, scale, maxIterations, tol, trim, d_vertices,
-                         d_vertexIntensity, maxVertices, d_triangles, maxTriangles, d_chi, c->stream, c->h_mesh.p);
+         return mesh_run(d_xyz, d_normal, d_intensity, numPoints, depth, scale, 0.0, maxIterations, tol, trim,
+                         d_vertices, d_vertexIntensity, maxVertices, d_triangles, maxTriangles, d_chi, c->stream,
+                         c->h_mesh.p);
        })) < 0)
     return r;
-  return mesh_result(c->h_mesh.p, numPoints, maxVertices, maxTriangles, info_out, stats_out);
+  return mesh_result(c->h_mesh.p, numPoints, maxVertices, maxTriangles, false, info_out, stats_out);
+}
+
+int cs_poisson_mesh_screened(const float *d_xyz, const float *d_normal, const float *d_intensity, int numPoints,
+                             int depth, double scale, double pointWeight, int maxIterations, double tol, double trim,
+                             float *d_vertices, float *d_vertexIntensity, int maxVertices, int *d_triangles,
+                             int maxTriangles, float *d_chi, double info_out[8], long long stats_out[10], double *ms)
+{
+  const char *fn = "cs_poisson_mesh_screened";
+  if (ms) *ms = 0.0;
+  int r = mesh_screened_args(fn, d_xyz, d_normal, d_intensity, numPoints, depth, scale, pointWeight, maxIterations,
+                             tol, trim, d_vertices, d_vertexIntensity, maxVertices, d_triangles, maxTriangles, d_chi);
+  if (r < 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(mesh_result_bytes())) < 0) return r;
+  if ((r = timed_sync(fn, c, ms, [&] {
+         return mesh_run(d_xyz, d_normal, d_intensity, numPoints, depth, scale, pointWeight, maxIterations, tol, trim,
+                         d_vertices, d_vertexIntensity, maxVertices, d_triangles, maxTriangles, d_chi, c->stream,
+                         c->h_mesh.p);
+       })) < 0)
+    return r;
+  return mesh_result(c->h_mesh.p, numPoints, maxVertices, maxTriangles, true, info_out, stats_out);
 }
 
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,

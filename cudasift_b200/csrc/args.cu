@@ -1008,4 +1008,15 @@ int mesh_args(const char *fn, const float *xyz, const float *normal, const float
   return rs.check(fn);
 }
 
+int mesh_screened_args(const char *fn, const float *xyz, const float *normal, const float *intensity, int numPoints,
+                       int depth, double scale, double pointWeight, int maxIterations, double tol, double trim,
+                       const float *vertices, const float *vertexIntensity, int maxVertices, const int *triangles,
+                       int maxTriangles, const float *chi)
+{
+  if (!std::isfinite(pointWeight) || pointWeight <= 0.0 || pointWeight > 1000.0)
+    return arg_error(fn, "pointWeight must be finite and in (0, 1000]");
+  return mesh_args(fn, xyz, normal, intensity, numPoints, depth, scale, maxIterations, tol, trim, vertices,
+                   vertexIntensity, maxVertices, triangles, maxTriangles, chi);
+}
+
 }  // namespace cs

@@ -89,6 +89,11 @@ int fuse_args(const char *fn, const cs_image *images, int numImages, const doubl
 int mesh_args(const char *fn, const float *xyz, const float *normal, const float *intensity, int numPoints, int depth,
               double scale, int maxIterations, double tol, double trim, const float *vertices,
               const float *vertexIntensity, int maxVertices, const int *triangles, int maxTriangles, const float *chi);
+// cs_poisson_mesh_screened: pointWeight, then mesh_args.
+int mesh_screened_args(const char *fn, const float *xyz, const float *normal, const float *intensity, int numPoints,
+                       int depth, double scale, double pointWeight, int maxIterations, double tol, double trim,
+                       const float *vertices, const float *vertexIntensity, int maxVertices, const int *triangles,
+                       int maxTriangles, const float *chi);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

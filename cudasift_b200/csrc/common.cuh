@@ -718,14 +718,16 @@ int fuse_enqueue(DeviceCtx &c, const cs_image *images, int numImages, const doub
                  float *intensity, int *source, int maxPoints, unsigned int **total);
 
 // ---- Poisson meshing (mesh.cu) -------------------------------------------------------------------------------------
-// The launches of cs_poisson_mesh (argument-checked) on st, with the scratch allocated and freed on st, without a
-// synchronize; the result words (mesh_result_bytes of them) reach h_result (pinned) by the caller's synchronize.
+// The launches of cs_poisson_mesh (pointWeight 0) or cs_poisson_mesh_screened (pointWeight > 0), argument-checked, on
+// st, with the scratch allocated and freed on st, without a synchronize; the result words (mesh_result_bytes of them)
+// reach h_result (pinned) by the caller's synchronize.
 int mesh_run(const float *xyz, const float *normal, const float *intensity, int numPoints, int depth, double scale,
-             int maxIterations, double tol, double trim, float *vertices, float *vertexIntensity, int maxVertices,
-             int *triangles, int maxTriangles, float *chiOut, cudaStream_t st, void *h_result);
+             double pointWeight, int maxIterations, double tol, double trim, float *vertices, float *vertexIntensity,
+             int maxVertices, int *triangles, int maxTriangles, float *chiOut, cudaStream_t st, void *h_result);
 size_t mesh_result_bytes();
-// after the synchronize: info_out and stats_out (either may be NULL); returns the full triangle count
-int mesh_result(const void *h_result, int numPoints, int maxVertices, int maxTriangles, double info[7],
+// after the synchronize: info_out ([7], or [8] when screened) and stats_out (either may be NULL); returns the full
+// triangle count
+int mesh_result(const void *h_result, int numPoints, int maxVertices, int maxTriangles, bool screened, double *info,
                 long long stats[10]);
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------

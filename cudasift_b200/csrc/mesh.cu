@@ -1,7 +1,9 @@
 // mesh.cu -- Poisson surface reconstruction of an oriented point cloud on a regular grid (cs_poisson_mesh): the splat
 // as a gather over cell-sorted points, the right-hand side, one cooperative kernel for the multigrid-preconditioned CG
 // solve and the iso-value, and marching tetrahedra with trimming as count-scan-write passes.  Every rule is stated in
-// cudasift_b200.h at cs_poisson_mesh; tests/mesh_oracle.py restates them in float64.
+// cudasift_b200.h at cs_poisson_mesh; tests/mesh_oracle.py restates them in float64.  cs_poisson_mesh_screened (screened
+// Poisson with a Neumann boundary) shares every kernel but the right-hand side and the solve; its rules are stated at
+// cs_poisson_mesh_screened and restated in tests/mesh_screened_oracle.py.
 //
 // Determinism: no floating-point atomics.  Integer atomics only where the result does not depend on their order (the
 // bounding box as ordered-integer max, the cell histogram, the kept-vertex bit masks).  Every floating-point sum has a
@@ -35,6 +37,7 @@ struct MeshResult {
   unsigned int status;            // 0 ok, 1 no used point or zero extent, 2 tau <= 0, 3 not converged
   int iters;
   long long counts[4];            // vertices and triangles before trimming, vertices and triangles after
+  double omega;                   // the screened call's effective point weight (its info_out[7])
 };
 
 struct MeshLevel {
@@ -68,6 +71,20 @@ struct MeshParams {
   float *vertices, *vertexIntensity;
   int *triangles;
   int maxVertices, maxTriangles;
+};
+
+// A level of the screened call's V-cycle: MeshLevel's arrays plus the diagonal of its screening operator.
+struct NLevel {
+  float *x, *f, *t, *s;
+  int n;
+};
+
+// The screened call's fields, a second kernel argument so that MeshParams (and the Dirichlet kernels' code) stay as
+// they are.
+struct ScreenParams {
+  double alpha;                   // pointWeight
+  double *u;                      // omega B_p^T x per sorted point [used]
+  NLevel lv[MAX_LEVELS];          // lv[l].x, f, t alias MeshParams::lv[l]
 };
 
 __device__ __forceinline__ unsigned int float_key(float f)
@@ -596,6 +613,388 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   }
 }
 
+// ---- screened Poisson with a Neumann boundary (cs_poisson_mesh_screened) ---------------------------------------------
+// The in-grid neighbours of node idx = (i, j, k) of a level with n cells in the order -x, +x, -y, +y, -z, +z (an absent
+// one adds 0, so an interior node gets nbr_sum's value), in float; deg receives their count.
+__device__ __forceinline__ float nbr_sum_nm(const float *x, int idx, int i, int j, int k, int n, float &deg)
+{
+  const int n1 = n + 1, s = n1 * n1;
+  const float a = i > 0 ? x[idx - 1] : 0.0f, b = i < n ? x[idx + 1] : 0.0f;
+  const float c = j > 0 ? x[idx - n1] : 0.0f, d = j < n ? x[idx + n1] : 0.0f;
+  const float e = k > 0 ? x[idx - s] : 0.0f, f = k < n ? x[idx + s] : 0.0f;
+  deg = (float)((i > 0) + (i < n) + (j > 0) + (j < n) + (k > 0) + (k < n));
+  return ((((a + b) + c) + d) + e) + f;
+}
+
+// The same in float64 from the floats.
+__device__ __forceinline__ double nbr_sum_nm_d(const float *x, int idx, int i, int j, int k, int n, double &deg)
+{
+  const int n1 = n + 1, s = n1 * n1;
+  const double a = i > 0 ? x[idx - 1] : 0.0, b = i < n ? x[idx + 1] : 0.0;
+  const double c = j > 0 ? x[idx - n1] : 0.0, d = j < n ? x[idx + n1] : 0.0;
+  const double e = k > 0 ? x[idx - s] : 0.0, f = k < n ? x[idx + s] : 0.0;
+  deg = (double)((i > 0) + (i < n) + (j > 0) + (j < n) + (k > 0) + (k < n));
+  return ((((a + b) + c) + d) + e) + f;
+}
+
+// Red-black Gauss-Seidel half-sweep over every node of one colour: x = (f + neighbours) / (deg + s).
+template <class T>
+__device__ void rb_sweep_nm(const NLevel &L, int colour, T &team)
+{
+  const int n1 = L.n + 1, m = n1 * n1 * n1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int i, j, k;
+    node_ijk(idx, n1, i, j, k);
+    if (((i + j + k) & 1) != colour) continue;
+    float deg;
+    const float nb = nbr_sum_nm(L.x, idx, i, j, k, L.n, deg);
+    L.x[idx] = (L.f[idx] + nb) / (deg + L.s[idx]);
+  }
+}
+
+template <class T>
+__device__ void smooth_pairs_nm(const NLevel &L, int pairs, bool redFirst, T &team)
+{
+  for (int s = 0; s < pairs; s++) {
+    rb_sweep_nm(L, redFirst ? 0 : 1, team);
+    team.sync();
+    rb_sweep_nm(L, redFirst ? 1 : 0, team);
+    team.sync();
+  }
+}
+
+// t = f - ((deg + s) x - neighbours) at every node.
+template <class T>
+__device__ void residual_nm(const NLevel &L, T &team)
+{
+  const int n1 = L.n + 1, m = n1 * n1 * n1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int i, j, k;
+    node_ijk(idx, n1, i, j, k);
+    float deg;
+    const float nb = nbr_sum_nm(L.x, idx, i, j, k, L.n, deg);
+    L.t[idx] = L.f[idx] - ((deg + L.s[idx]) * L.x[idx] - nb);
+  }
+}
+
+// fc = (1/2) P^T t at every coarse node over its in-grid fine nodes 2Q + d (dz outer, dx inner); xc = 0.
+template <class T>
+__device__ void restrict_to_nm(const NLevel &F, const NLevel &C, T &team)
+{
+  const int n1 = C.n + 1, m = n1 * n1 * n1, f1 = F.n + 1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int I, J, K;
+    node_ijk(idx, n1, I, J, K);
+    C.x[idx] = 0.0f;
+    float s = 0.0f;
+    for (int dz = -1; dz <= 1; dz++)
+      for (int dy = -1; dy <= 1; dy++)
+        for (int dx = -1; dx <= 1; dx++) {
+          const int fi = 2 * I + dx, fj = 2 * J + dy, fk = 2 * K + dz;
+          if (fi < 0 || fj < 0 || fk < 0 || fi > F.n || fj > F.n || fk > F.n) continue;
+          const float w = (dx ? 0.5f : 1.0f) * (dy ? 0.5f : 1.0f) * (dz ? 0.5f : 1.0f);
+          s = fmaf(w, F.t[(fk * f1 + fj) * f1 + fi], s);
+        }
+    C.f[idx] = 0.5f * s;
+  }
+}
+
+// x += P xc at every fine node.
+template <class T>
+__device__ void prolong_add_nm(const NLevel &C, const NLevel &F, T &team)
+{
+  const int n1 = F.n + 1, m = n1 * n1 * n1, c1 = C.n + 1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int i, j, k;
+    node_ijk(idx, n1, i, j, k);
+    float s = 0.0f;
+    for (int bz = 0; bz <= (k & 1); bz++)
+      for (int by = 0; by <= (j & 1); by++)
+        for (int bx = 0; bx <= (i & 1); bx++) {
+          const float w = ((i & 1) ? 0.5f : 1.0f) * ((j & 1) ? 0.5f : 1.0f) * ((k & 1) ? 0.5f : 1.0f);
+          s = fmaf(w, C.x[((k / 2 + bz) * c1 + j / 2 + by) * c1 + i / 2 + bx], s);
+        }
+    F.x[idx] += s;
+  }
+}
+
+template <class T>
+__device__ void v_down_nm(const NLevel *lv, int l, T &team)
+{
+  smooth_pairs_nm(lv[l], NU, true, team);
+  residual_nm(lv[l], team);
+  team.sync();
+  restrict_to_nm(lv[l], lv[l + 1], team);
+  team.sync();
+}
+
+template <class T>
+__device__ void v_up_nm(const NLevel *lv, int l, T &team)
+{
+  prolong_add_nm(lv[l + 1], lv[l], team);
+  team.sync();
+  smooth_pairs_nm(lv[l], NU, false, team);
+}
+
+// v_cycle's schedule on the levels L_l + diag(s_l).
+__device__ void v_cycle_nm(const MeshParams &p, const ScreenParams &sc, GridTeam &grid)
+{
+  const NLevel *lv = sc.lv;
+  const int last = p.levels - 1;
+  int lg = 0;
+  while (lg < last && lv[lg].n > LOCAL_N) lg++;
+  for (int l = 0; l < lg; l++) v_down_nm(lv, l, grid);
+  if (blockIdx.x == 0) {
+    CtaTeam cta{(int)threadIdx.x, (int)blockDim.x};
+    for (int l = lg; l < last; l++) v_down_nm(lv, l, cta);
+    smooth_pairs_nm(lv[last], NU_COARSE, true, cta);
+    smooth_pairs_nm(lv[last], NU_COARSE, false, cta);
+    for (int l = last - 1; l >= lg; l--) v_up_nm(lv, l, cta);
+  }
+  grid.sync();
+  for (int l = lg - 1; l >= 0; l--) v_up_nm(lv, l, grid);
+}
+
+// The trilinear weights B_p of a point at grid coordinates g, at the corners of its cell clamp(floor(g), 0, N - 1)
+// (z outer, x inner) in the splat's form prod (1 - |g_a - q_a|); returns the first corner's node.
+__device__ __forceinline__ int point_weights(const double *g, int N, double w[8])
+{
+  const int n1 = N + 1;
+  int c[3];
+  for (int a = 0; a < 3; a++) c[a] = min(max((int)floor(g[a]), 0), N - 1);
+  for (int b = 0; b < 8; b++)
+    w[b] = (1.0 - fabs(g[0] - (c[0] + (b & 1)))) * (1.0 - fabs(g[1] - (c[1] + ((b >> 1) & 1)))) *
+           (1.0 - fabs(g[2] - (c[2] + ((b >> 2) & 1))));
+  return (c[2] * n1 + c[1]) * n1 + c[0];
+}
+
+__device__ __forceinline__ int corner_offset(int b, int n1) { return (b & 1) + ((b >> 1) & 1) * n1 + (b >> 2) * n1 * n1; }
+
+// u_s = omega B_s^T x (float64 from the floats) over the used points, in sorted order.
+__device__ __forceinline__ void screen_points(const MeshParams &p, const ScreenParams &sc, const float *x, double omega,
+                                              int used, GridTeam &grid)
+{
+  const int n1 = p.N + 1;
+  for (int s = grid.tid; s < used; s += grid.nth) {
+    double w[8];
+    const int q0 = point_weights(p.gs + 3 * (size_t)s, p.N, w);
+    double acc = 0.0;
+    for (int b = 0; b < 8; b++) acc += w[b] * (double)x[q0 + corner_offset(b, n1)];
+    sc.u[s] = omega * acc;
+  }
+}
+
+// (S x)_q = sum B_s(q) u_s over the points of q's (up to 8) cells, cells in ascending index and points in sorted order
+// (each row of 2 cells is one contiguous run of sorted points), in float64.
+__device__ __forceinline__ double screen_gather(const MeshParams &p, const ScreenParams &sc, int i, int j, int k)
+{
+  const int N = p.N;
+  double acc = 0.0;
+  const int x0 = max(i - 1, 0), x1 = min(i, N - 1);
+  for (int cz = max(k - 1, 0); cz <= min(k, N - 1); cz++)
+    for (int cy = max(j - 1, 0); cy <= min(j, N - 1); cy++) {
+      const int row = (cz * N + cy) * N;
+      for (int e = p.cellStart[row + x0], end = p.cellStart[row + x1 + 1]; e < end; e++) {
+        const double *g = p.gs + 3 * (size_t)e;
+        acc += (1.0 - fabs(g[0] - i)) * (1.0 - fabs(g[1] - j)) * (1.0 - fabs(g[2] - k)) * sc.u[e];
+      }
+    }
+  return acc;
+}
+
+// b = div of the edge field g(q -> q + e_a) = (h / 2)(V_a(q) + V_a(q + e_a)) over the in-grid edges at every node, in
+// float64 from the floats, rounded once: per axis V_a(q + e_a) - V_a(q - e_a) with both neighbours (the Dirichlet
+// call's central difference), V_a(q) + V_a(q + e_a) at a low face, -(V_a(q - e_a) + V_a(q)) at a high face, then
+// (h / 2) ((x + y) + z).  chi = 0.
+__global__ void __launch_bounds__(MT) mesh_rhs_neumann_kernel(MeshParams p)
+{
+  const int N = p.N, n1 = N + 1, s = n1 * n1;
+  const double h = p.res->info[3];
+  const bool ok = p.res->status == 0;
+  const float *V[3] = {p.V0, p.V1, p.V2};
+  for (int idx = blockIdx.x * MT + threadIdx.x; idx < p.M; idx += gridDim.x * MT) {
+    int q[3];
+    node_ijk(idx, n1, q[0], q[1], q[2]);
+    double b = 0.0;
+    if (ok) {
+      double d[3];
+      for (int a = 0; a < 3; a++) {
+        const int st = a == 0 ? 1 : a == 1 ? n1 : s;
+        const float *Va = V[a];
+        d[a] = q[a] == 0   ? (double)Va[idx] + (double)Va[idx + st]
+               : q[a] == N ? -((double)Va[idx - st] + (double)Va[idx])
+                           : (double)Va[idx + st] - (double)Va[idx - st];
+      }
+      b = h / 2.0 * ((d[0] + d[1]) + d[2]);
+    }
+    p.b[idx] = (float)b;
+    p.chi[idx] = 0.0f;
+  }
+}
+
+// The screened solve: omega from the mean density, the levels' screening diagonals, CG on A = L + omega sum B B^T
+// preconditioned by one V-cycle on L_l + diag(s_l), then the true residual, tau and the mean density; one resident
+// wave.
+__global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, ScreenParams sc)
+{
+  MeshResult &R = *p.res;
+  if (R.status != 0) return;                           // every CTA reads the same word
+  GridTeam grid{cg::this_grid(), (int)(blockIdx.x * MT + threadIdx.x), (int)(gridDim.x * MT)};
+  const int N = p.N, n1 = N + 1, M = p.M, used = (int)R.used;
+  float *x = p.chi, *r = p.r, *b = p.b, *z = p.V0, *pp = p.V1, *q = p.V2;
+  auto total1 = [&](int n, double &out) {
+    grid.sync();
+    mesh_group_sums<1>(n, p.tilePart, p.groupPart);
+    grid.sync();
+    double t[1];
+    mesh_total<1>(n, p.groupPart, t);
+    out = t[0];
+  };
+  // chi (or D) trilinear at sorted point s, as the Dirichlet call's tau
+  auto interp = [&](const float *F, int s) {
+    const double *g = p.gs + 3 * (size_t)s;
+    int c[3];
+    double t[3];
+    for (int a = 0; a < 3; a++) {
+      c[a] = min(max((int)floor(g[a]), 0), N - 1);
+      t[a] = g[a] - c[a];
+    }
+    double v = 0.0;
+    for (int bz = 0; bz < 2; bz++)
+      for (int by = 0; by < 2; by++)
+        for (int bx = 0; bx < 2; bx++) {
+          const double w = (bx ? t[0] : 1.0 - t[0]) * (by ? t[1] : 1.0 - t[1]) * (bz ? t[2] : 1.0 - t[2]);
+          v += w * (double)F[((c[2] + bz) * n1 + c[1] + by) * n1 + c[0] + bx];
+        }
+    return v;
+  };
+
+  // omega = alpha / mean density
+  double dsum;
+  mesh_tile_sums<1>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(p.D, s); });
+  total1(used, dsum);
+  const double omega = sc.alpha / (dsum / used);
+  // the screening diagonal of every level: s_l(Q) = (omega / 2^l) sum (B^l_p(Q))^2 at g / 2^l, over the fine cells of
+  // Q's support in ascending index (rows of cells as contiguous runs of sorted points)
+  // (level 0: a thread per node over its rows in order; coarser levels: a warp per node, lane j summing the rows
+  // j, j + 32, ... in order, then warp_sum's butterfly, lane 0's value)
+  auto diag_rows = [&](int l, int idx, int lane, int step) {
+    const int c1 = sc.lv[l].n + 1, f = 1 << l;
+    const double inv = 1.0 / f;
+    int I, J, K;
+    node_ijk(idx, c1, I, J, K);
+    const int x0 = max(f * (I - 1), 0), x1 = min(f * (I + 1), N) - 1;
+    const int y0 = max(f * (J - 1), 0), ny = min(f * (J + 1), N) - y0;
+    const int z0 = max(f * (K - 1), 0), nz = min(f * (K + 1), N) - z0;
+    double acc = 0.0;
+    for (int rw = lane; rw < ny * nz; rw += step) {
+      const int row = ((z0 + rw / ny) * N + y0 + rw % ny) * N;
+      for (int e = p.cellStart[row + x0], end = p.cellStart[row + x1 + 1]; e < end; e++) {
+        const double *g = p.gs + 3 * (size_t)e;
+        const double w = (1.0 - fabs(g[0] * inv - I)) * (1.0 - fabs(g[1] * inv - J)) * (1.0 - fabs(g[2] * inv - K));
+        acc += w * w;
+      }
+    }
+    return acc;
+  };
+  for (int t = grid.tid; t < M; t += grid.nth) sc.lv[0].s[t] = (float)(omega * diag_rows(0, t, 0, 1));
+  {
+    const int lane = threadIdx.x & 31, warp = grid.tid >> 5, warps = grid.nth >> 5;
+    int coarse = 0;
+    for (int l = 1; l < p.levels; l++) coarse += (sc.lv[l].n + 1) * (sc.lv[l].n + 1) * (sc.lv[l].n + 1);
+    for (int t = warp; t < coarse; t += warps) {
+      int l = 1, idx = t;
+      while (idx >= (sc.lv[l].n + 1) * (sc.lv[l].n + 1) * (sc.lv[l].n + 1)) {
+        idx -= (sc.lv[l].n + 1) * (sc.lv[l].n + 1) * (sc.lv[l].n + 1);
+        l++;
+      }
+      double v[1] = {diag_rows(l, idx, lane, 32)};
+      warp_sum(v);
+      if (lane == 0) sc.lv[l].s[idx] = (float)(omega / (1 << l) * v[0]);
+    }
+  }
+
+  double bb, rr, rz = 0.0;
+  mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    r[i] = b[i];
+    z[i] = 0.0f;
+    v[0] += (double)b[i] * (double)b[i];
+  });
+  total1(M, bb);                                       // (its barrier also completes the diagonals)
+  rr = bb;
+  int k = 0;
+  bool done = rr <= p.tol2 * bb;
+  if (!done) {
+    v_cycle_nm(p, sc, grid);
+    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+      pp[i] = z[i];
+      v[0] += (double)r[i] * (double)z[i];
+    });
+    total1(M, rz);
+  }
+  while (!done) {
+    grid.sync();                                       // p complete before the point pass and A p read it
+    screen_points(p, sc, pp, omega, used, grid);
+    grid.sync();
+    double pq;
+    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+      int a, bq, c;
+      node_ijk(i, n1, a, bq, c);
+      float deg;
+      const float nb = nbr_sum_nm(pp, i, a, bq, c, N, deg);
+      const float aq = (deg * pp[i] - nb) + (float)screen_gather(p, sc, a, bq, c);
+      q[i] = aq;
+      v[0] += (double)pp[i] * (double)aq;
+    });
+    total1(M, pq);
+    if (!(pq > 0.0)) break;
+    const double alpha = rz / pq;
+    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+      x[i] = (float)((double)x[i] + alpha * (double)pp[i]);
+      const float ri = (float)((double)r[i] - alpha * (double)q[i]);
+      r[i] = ri;
+      z[i] = 0.0f;
+      v[0] += (double)ri * (double)ri;
+    });
+    total1(M, rr);
+    k++;
+    if (rr <= p.tol2 * bb || k >= p.maxIterations) break;
+    v_cycle_nm(p, sc, grid);
+    double rzNew;
+    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
+    total1(M, rzNew);
+    const double beta = rzNew / rz;
+    rz = rzNew;
+    for (int i = grid.tid; i < M; i += grid.nth) pp[i] = (float)((double)z[i] + beta * (double)pp[i]);
+  }
+  grid.sync();
+  // the true residual b - A chi, in float64 from the floats
+  screen_points(p, sc, x, omega, used, grid);
+  grid.sync();
+  double rt;
+  mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    int a, bq, c;
+    node_ijk(i, n1, a, bq, c);
+    double deg;
+    const double nb = nbr_sum_nm_d(x, i, a, bq, c, N, deg);
+    const double e = (double)b[i] - ((deg * (double)x[i] - nb) + screen_gather(p, sc, a, bq, c));
+    v[0] += e * e;
+  });
+  total1(M, rt);
+  // tau: chi trilinear at the used points, in sorted order
+  double tsum;
+  mesh_tile_sums<1>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(x, s); });
+  total1(used, tsum);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    R.info[4] = tsum / used;
+    R.info[5] = dsum / used;
+    R.info[6] = bb > 0.0 ? sqrt(rt / bb) : 0.0;
+    R.omega = omega;
+    R.iters = k;
+    R.status = rr <= p.tol2 * bb ? 0u : 3u;
+  }
+}
+
 // ---- extraction -----------------------------------------------------------------------------------------------------
 // Lattice direction of corner bits (x 1, y 2, z 4) -> direction index: (1,0,0) 0, (0,1,0) 1, (0,0,1) 2, (1,1,0) 3,
 // (1,0,1) 4, (0,1,1) 5, (1,1,1) 6.
@@ -875,9 +1274,10 @@ __global__ void __launch_bounds__(MT) mesh_triangles_kernel(MeshParams p)
 static size_t level_bytes(int n) { return (size_t)(n + 1) * (n + 1) * (n + 1) * sizeof(float); }
 
 int mesh_run(const float *xyz, const float *normal, const float *intensity, int numPoints, int depth, double scale,
-             int maxIterations, double tol, double trim, float *vertices, float *vertexIntensity, int maxVertices,
-             int *triangles, int maxTriangles, float *chiOut, cudaStream_t st, void *h_result)
+             double pointWeight, int maxIterations, double tol, double trim, float *vertices, float *vertexIntensity,
+             int maxVertices, int *triangles, int maxTriangles, float *chiOut, cudaStream_t st, void *h_result)
 {
+  const bool screened = pointWeight > 0.0;
   const int N = 1 << depth, n1 = N + 1;
   const int M = n1 * n1 * n1;
   const int P = numPoints;
@@ -911,6 +1311,13 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
   const size_t groupAt = L.take((size_t)groupsMax * 2 * sizeof(double));
   const size_t cntAt = L.take((size_t)4 * nb * sizeof(int)), offAt = L.take((size_t)4 * nb * sizeof(int));
   const size_t tempAt = L.take(std::max(sortBytes, std::max(scanBytes, scanBytes2)));
+  // the screened call: the levels' screening diagonals, u, and cell starts of their own (the solve reads them)
+  size_t diagAt[MAX_LEVELS] = {}, uAt = 0, startAt = 0;
+  if (screened) {
+    for (int l = 0, n = N; l < levels; l++, n /= 2) diagAt[l] = L.take(level_bytes(n));
+    uAt = L.take((size_t)P * sizeof(double));
+    startAt = L.take(((size_t)N * N * N + 1) * sizeof(int));
+  }
 
   char *base = nullptr;
   CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
@@ -941,7 +1348,7 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
   p.D = reinterpret_cast<float *>(at(dAt));
   p.S = hasI ? reinterpret_cast<float *>(at(sAt)) : nullptr;
   p.cellCount = reinterpret_cast<int *>(p.chi);        // dead before the right-hand side zeroes chi
-  p.cellStart = reinterpret_cast<int *>(p.r);          // dead before the solve writes r
+  p.cellStart = reinterpret_cast<int *>(screened ? at(startAt) : at(rAt));   // Dirichlet: dead before the solve writes r
   p.kstart = reinterpret_cast<int *>(p.r);             // r is dead after the solve
   p.lv[0] = MeshLevel{p.V0, p.r, p.V2, N};             // z = M r, with q as the residual scratch
   for (int l = 1, n = N / 2; l < levels; l++, n /= 2)
@@ -963,8 +1370,16 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
   p.maxVertices = maxVertices;
   p.maxTriangles = maxTriangles;
   void *temp = at(tempAt);
+  ScreenParams sc{};
+  sc.alpha = pointWeight;
+  if (screened) {
+    sc.u = reinterpret_cast<double *>(at(uAt));
+    for (int l = 0; l < levels; l++)
+      sc.lv[l] = NLevel{p.lv[l].x, p.lv[l].f, p.lv[l].t, reinterpret_cast<float *>(at(diagAt[l])), p.lv[l].n};
+  }
 
-  const int wave = coop_grid<mesh_solve_kernel, MT>("cs_poisson_mesh");
+  const int wave = screened ? coop_grid<mesh_screened_solve_kernel, MT>("cs_poisson_mesh_screened")
+                            : coop_grid<mesh_solve_kernel, MT>("cs_poisson_mesh");
   int r = wave < 0 ? wave : 0;
   cudaEvent_t *tev = match_timing_events();
   const int pointCtas = std::max(1, std::min(idivup(P, MT), 4096));
@@ -982,12 +1397,16 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
     CS_CUDA(cub::DeviceScan::ExclusiveSum(temp, scanBytes, p.cellCount, p.cellStart, N * N * N + 1, st));
     mesh_points_kernel<<<pointCtas, MT, 0, st>>>(p);
     mesh_splat_kernel<<<nodeCtas, MT, 0, st>>>(p);
-    mesh_rhs_kernel<<<nodeCtas, MT, 0, st>>>(p);
+    if (screened) mesh_rhs_neumann_kernel<<<nodeCtas, MT, 0, st>>>(p);
+    else mesh_rhs_kernel<<<nodeCtas, MT, 0, st>>>(p);
     count_launch(3);
     CS_CUDA(cudaGetLastError());
     if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
-    void *args[] = {&p};
-    CS_CUDA(cudaLaunchCooperativeKernel((const void *)mesh_solve_kernel, dim3(wave), dim3(MT), args, 0, st));
+    void *args[] = {&p, &sc};
+    if (screened)
+      CS_CUDA(cudaLaunchCooperativeKernel((const void *)mesh_screened_solve_kernel, dim3(wave), dim3(MT), args, 0, st));
+    else
+      CS_CUDA(cudaLaunchCooperativeKernel((const void *)mesh_solve_kernel, dim3(wave), dim3(MT), args, 0, st));
     count_launch();
     if (tev) CS_CUDA(cudaEventRecord(tev[2], st));
     mesh_count_kernel<<<nb, MT, 0, st>>>(p);
@@ -1006,7 +1425,7 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
     CS_CUDA(cudaMemcpyAsync(h_result, p.res, sizeof(MeshResult), cudaMemcpyDeviceToHost, st));
     if (tev) {
       static const char *const names[3] = {"splat", "solve", "extract"};
-      report_stage_times(tev, names, 3, "mesh timing depth=%d points=%d", depth, P);
+      report_stage_times(tev, names, 3, "mesh timing depth=%d points=%d%s", depth, P, screened ? " screened" : "");
     }
     return 0;
   };
@@ -1018,12 +1437,14 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
 size_t mesh_result_bytes() { return sizeof(MeshResult); }
 
 // stats_out and info_out from the result words (after the synchronize); returns the full triangle count.
-int mesh_result(const void *h_result, int numPoints, int maxVertices, int maxTriangles, double info[7],
+int mesh_result(const void *h_result, int numPoints, int maxVertices, int maxTriangles, bool screened, double *info,
                 long long stats[10])
 {
   const MeshResult &R = *static_cast<const MeshResult *>(h_result);
-  if (info)
+  if (info) {
     for (int k = 0; k < 7; k++) info[k] = R.info[k];
+    if (screened) info[7] = R.omega;
+  }
   const bool out = R.status == 0 || R.status == 3;
   const long long c[4] = {out ? R.counts[0] : 0, out ? R.counts[1] : 0, out ? R.counts[2] : 0, out ? R.counts[3] : 0};
   if (stats) {

@@ -1195,6 +1195,51 @@ int cs_poisson_mesh(const float *d_xyz, const float *d_normal, const float *d_in
                     float *d_vertexIntensity, int maxVertices, int *d_triangles, int maxTriangles, float *d_chi,
                     double info_out[7], long long stats_out[10], double *ms);
 
+/* Screened Poisson surface reconstruction (Kazhdan & Hoppe, ACM TOG 2013) with a Neumann boundary, on the same dense
+ * grid as cs_poisson_mesh: a mesh of open surfaces seen from one side (a terrain, a facade, a fused stereo scene) as
+ * well as closed ones.  The arguments are cs_poisson_mesh's plus pointWeight (alpha), after scale.
+ * - Used points, grid, sort, splat, V, D, S and intensities: exactly as in cs_poisson_mesh (the same kernels).
+ * - Operator (Neumann boundary): the graph Laplacian on all (N + 1)^3 nodes, (L x)_q = deg_q x_q - sum of the in-grid
+ *   neighbours (deg_q in [3, 6]).
+ * - Right-hand side: the divergence of the edge field g(q -> q + e_a) = (h / 2)(V_a(q) + V_a(q + e_a)): b_q = sum over
+ *   the in-grid edges leaving q of g - sum over those entering q of g.  In float64 from the float V, per axis
+ *   V_a(q + e_a) - V_a(q - e_a) with both neighbours (the central difference of cs_poisson_mesh), V_a(q) + V_a(q + e_a)
+ *   at a low face, -(V_a(q - e_a) + V_a(q)) at a high face, then (h / 2)((x + y) + z) rounded to float.  Sum b = 0 in
+ *   exact arithmetic.
+ * - Screening: A = L + omega sum_p B_p B_p^T, where B_p holds point p's trilinear weights prod_a (1 - |g_a - q_a|) at
+ *   the 8 corners of its cell clamp(floor(g), 0, N - 1) (z outer, x inner).  The target is 0, so b has no screening
+ *   term.  omega = pointWeight / mean density, the mean density computed before the solve exactly as info_out[5] of
+ *   cs_poisson_mesh.  Since 1^T L = 0, 1^T b = 0 and sum_c B_p(c) = 1, the mean of chi at the points is 0 in exact
+ *   arithmetic.
+ * - Solve: cs_poisson_mesh's CG with A p as L p in float plus (float) S p, where u_p = omega B_p^T p over the sorted
+ *   points (float64 from the floats), a grid barrier, then (S p)_q = sum B_p(q) u_p over the points of q's (up to 8)
+ *   cells, cells in ascending index and points in sorted order, in float64.  The preconditioner is one V-cycle with
+ *   cs_poisson_mesh's schedule (2 pairs, 8 coarsest pairs, levels down to 4 cells, restriction (1/2) P^T) on the level
+ *   operators L_l + diag(s_l) over every node, boundary included: the half-sweep x = (f + in-grid neighbours) /
+ *   (deg + s_q), the residual f - ((deg + s_q) x - neighbours), restriction and prolongation over the in-grid nodes.
+ *   s_l is the diagonal of the exact coarse screening (1/2) P^T S_(l-1) P = (omega / 2^l) sum B^l_p B^l_p^T at the
+ *   level-l coordinates g / 2^l: s_l(Q) = (omega / 2^l) sum (B^l_p(Q))^2 over the fine cells of Q's support in
+ *   ascending index, in float64, rounded once (level 0 a thread per node; coarser levels a warp per node, lane j
+ *   summing rows of cells j, j + 32, ... then a butterfly).  The V-cycle stays symmetric positive definite.  The true
+ *   relative residual uses the same A in float64 from the floats.
+ * - Iso-value: tau is the mean of chi at the used points, as in cs_poisson_mesh; it is near 0 and its sign means
+ *   nothing, so status 2 never occurs.  Extraction (inside: chi >= tau), trim, vertex intensity, outputs and their
+ *   order: as in cs_poisson_mesh (the same kernels).  Without trimming the mesh is an oriented 2-manifold whose
+ *   boundary edges all lie on the grid's faces.
+ * - info_out [8] (may be NULL): cs_poisson_mesh's 7 entries, then omega.  stats_out [10]: cs_poisson_mesh's layout;
+ *   status 0 ok, 1 no used point or zero extent, 3 not converged (the mesh is still extracted).
+ * - Determinism: no floating-point atomics; every sum has a fixed order (above, and cs_poisson_mesh's totals).
+ * - Launches: 10 kernel launches whatever the depth and the data (box, keys, points, splat, right-hand side, one
+ *   cooperative solve kernel, two counts, vertices, triangles), plus cub's sort and scans (not counted).
+ * - Scratch: cs_poisson_mesh's, plus 4 bytes per node of every level (s_l), 4 per node (cell starts the solve keeps)
+ *   and 8 per point (u): about 5.5 GB at depth 9 with intensities.
+ * - CS_E_ARG, before any CUDA call, naming the argument: pointWeight not finite or outside (0, 1000], then every check
+ *   of cs_poisson_mesh (the same ranges and the same overlap sweep). */
+int cs_poisson_mesh_screened(const float *d_xyz, const float *d_normal, const float *d_intensity, int numPoints,
+                             int depth, double scale, double pointWeight, int maxIterations, double tol, double trim,
+                             float *d_vertices, float *d_vertexIntensity, int maxVertices, int *d_triangles,
+                             int maxTriangles, float *d_chi, double info_out[8], long long stats_out[10], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
