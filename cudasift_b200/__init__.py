@@ -24,7 +24,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
            "RetrievePairs", "RotationAveraging", "GlobalPositioning", "UndistortImages", "PatchMatchStereo",
            "PatchMatchStereoGeometric", "FuseDepthMaps", "SelectStereoViews", "PoissonMesh",
-           "PoissonMeshScreened"]
+           "PoissonMeshScreened", "SimplifyMesh"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -122,6 +122,8 @@ def lib():
                                  vp, vp, c.POINTER(c.c_double)]),
         "cs_poisson_mesh_screened": (ip, [vp, vp, vp, ip, ip, c.c_double, c.c_double, ip, c.c_double, c.c_double, vp,
                                           vp, ip, vp, ip, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_simplify_mesh": (ip, [vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, vp, vp, ip, vp, ip, vp, vp,
+                                  c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1415,6 +1417,43 @@ def PoissonMeshScreened(xyz, normal, intensity=None, depth=8, scale=1.1, pointWe
                                               int(maxIterations), float(tol), float(trim), verts, vint, maxV, tris,
                                               maxT, chi, info, stats, ms)
     return _poisson_call(call, "PoissonMeshScreened", 8, xyz, normal, intensity, depth, returnChi)
+
+
+def SimplifyMesh(vertices, triangles, intensity=None, targetTriangles=0, maxError=float("inf"), boundaryWeight=1.0):
+    """Quadric-error edge collapse of a triangle mesh (cs_simplify_mesh) in parallel passes of independent collapses,
+    until at most targetTriangles remain (the result ends at the target or one below) or no collapse has
+    sqrt(cost / area) <= maxError.  vertices float32 [V, 3], triangles int32 [T, 3] and intensity [V] or None, as
+    PoissonMesh returns them; boundaryWeight weighs the planes that hold boundary edges in place.  The outputs are
+    never larger than the inputs, so buffers of the input's size hold them.  Returns (vertices float32 [V', 3],
+    triangles int32 [T', 3], intensity float32 [V'] or None, info float64 [1] {largest applied sqrt(cost / area)},
+    stats int64 [9] (the header's), ms)."""
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    I = None if intensity is None else np.ascontiguousarray(np.asarray(intensity, np.float32).reshape(-1))
+    if I is not None and len(I) != len(X):
+        raise ValueError("intensity: one value per vertex")
+    V, T = len(X), len(F)
+    ins = [DeviceBuffer(max(X.nbytes, 4)), DeviceBuffer(max(F.nbytes, 4)),
+           DeviceBuffer(max(I.nbytes, 4)) if I is not None else None]
+    outs = [DeviceBuffer(12 * V + 4), DeviceBuffer(12 * T + 4), DeviceBuffer(4 * V + 4) if I is not None else None]
+    try:
+        for b, a in zip(ins, (X, F, I)):
+            if b is not None and a.size:
+                b.upload(a)
+        ptr = lambda b: b.ptr if b is not None else None
+        info, stats, ms = np.zeros(1), np.zeros(9, np.int64), ctypes.c_double(0.0)
+        n = _check(lib().cs_simplify_mesh(ptr(ins[0]), ptr(ins[2]), V, ptr(ins[1]), T, int(targetTriangles),
+                                          float(maxError), float(boundaryWeight), ptr(outs[0]), ptr(outs[2]), V,
+                                          ptr(outs[1]), T, _ptr(info), _ptr(stats), ctypes.byref(ms)), "SimplifyMesh")
+        nv = int(stats[4])
+        verts = outs[0].download(np.float32, 3 * nv).reshape(nv, 3)
+        tris = outs[1].download(np.int32, 3 * n).reshape(n, 3)
+        vint = outs[2].download(np.float32, nv) if I is not None else None
+        return verts, tris, vint, info, stats, ms.value
+    finally:
+        for b in ins + outs:
+            if b is not None:
+                b.free()
 
 
 def SelectStereoViews(Ks, Rs, ts, offsets, members, points, numSources=8, minTriAngle=1.0):

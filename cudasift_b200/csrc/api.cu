@@ -1763,6 +1763,34 @@ int cs_poisson_mesh_screened(const float *d_xyz, const float *d_normal, const fl
   return mesh_result(c->h_mesh.p, numPoints, maxVertices, maxTriangles, true, info_out, stats_out);
 }
 
+int cs_simplify_mesh(const float *d_vertices, const float *d_vertexIntensity, int numVertices, const int *d_triangles,
+                     int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
+                     float *d_outVertices, float *d_outIntensity, int maxOutVertices, int *d_outTriangles,
+                     int maxOutTriangles, double info_out[1], long long stats_out[9], double *ms)
+{
+  const char *fn = "cs_simplify_mesh";
+  if (ms) *ms = 0.0;
+  int r = simplify_args(fn, d_vertices, d_vertexIntensity, numVertices, d_triangles, numTriangles, targetTriangles,
+                        maxError, boundaryWeight, d_outVertices, d_outIntensity, maxOutVertices, d_outTriangles,
+                        maxOutTriangles);
+  if (r < 0) return r;
+  if (numTriangles == 0) {
+    if (info_out) info_out[0] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 9; k++) stats_out[k] = 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(simplify_result_bytes())) < 0) return r;
+  return timed_sync(fn, c, ms, [&] {
+    return simplify_run(d_vertices, d_vertexIntensity, numVertices, d_triangles, numTriangles, targetTriangles,
+                        maxError, boundaryWeight, d_outVertices, d_outIntensity, maxOutVertices, d_outTriangles,
+                        maxOutTriangles, c->stream, c->h_mesh.p, info_out, stats_out);
+  });
+}
+
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,
                            const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
                            int *counts_out, long long *stats_out, double *ms)

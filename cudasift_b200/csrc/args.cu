@@ -1019,4 +1019,42 @@ int mesh_screened_args(const char *fn, const float *xyz, const float *normal, co
                    vertexIntensity, maxVertices, triangles, maxTriangles, chi);
 }
 
+int simplify_args(const char *fn, const float *vertices, const float *vertexIntensity, int numVertices,
+                  const int *triangles, int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
+                  const float *outVertices, const float *outIntensity, int maxOutVertices, const int *outTriangles,
+                  int maxOutTriangles)
+{
+  if (numVertices < 0 || numVertices > (1 << 30)) return arg_error(fn, "numVertices must be in [0, 2^30]");
+  if (numTriangles < 0 || numTriangles > (1 << 29)) return arg_error(fn, "numTriangles must be in [0, 2^29]");
+  if (targetTriangles < 0) return arg_error(fn, "targetTriangles must be >= 0");
+  if (!(maxError >= 0.0)) return arg_error(fn, "maxError must be >= 0 (inf allowed)");
+  if (!std::isfinite(boundaryWeight) || boundaryWeight < 0.0)
+    return arg_error(fn, "boundaryWeight must be finite and >= 0");
+  if (maxOutVertices < 0) return arg_error(fn, "maxOutVertices must be >= 0");
+  if (maxOutTriangles < 0) return arg_error(fn, "maxOutTriangles must be >= 0");
+  if (numVertices > 0 && (!vertices || misaligned(vertices, 4)))
+    return arg_error(fn, "numVertices > 0 needs d_vertices (4-byte aligned)");
+  if (numTriangles > 0 && (!triangles || misaligned(triangles, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_triangles (4-byte aligned)");
+  if (maxOutVertices > 0 && (!outVertices || misaligned(outVertices, 4)))
+    return arg_error(fn, "maxOutVertices > 0 needs d_outVertices (4-byte aligned)");
+  if (maxOutTriangles > 0 && (!outTriangles || misaligned(outTriangles, 4)))
+    return arg_error(fn, "maxOutTriangles > 0 needs d_outTriangles (4-byte aligned)");
+  if (misaligned(vertexIntensity, 4)) return arg_error(fn, "d_vertexIntensity must be 4-byte aligned");
+  if (misaligned(outIntensity, 4)) return arg_error(fn, "d_outIntensity must be 4-byte aligned");
+  if (!vertexIntensity != !outIntensity)
+    return arg_error(fn, "d_vertexIntensity and d_outIntensity must be given together or not at all");
+  static const char *const names[6] = {"d_outVertices", "d_outIntensity", "d_outTriangles",
+                                       "d_vertices", "d_vertexIntensity", "d_triangles"};
+  ArgRanges rs(names, 6);
+  const size_t V = (size_t)numVertices, W = (size_t)maxOutVertices;
+  rs.add(outVertices, 12 * W, 0, 0, true);
+  if (outIntensity) rs.add(outIntensity, 4 * W, 1, 0, true);
+  rs.add(outTriangles, 12 * (size_t)maxOutTriangles, 2, 0, true);
+  rs.add(vertices, 12 * V, 3, 0, false);
+  if (vertexIntensity) rs.add(vertexIntensity, 4 * V, 4, 0, false);
+  rs.add(triangles, 12 * (size_t)numTriangles, 5, 0, false);
+  return rs.check(fn);
+}
+
 }  // namespace cs

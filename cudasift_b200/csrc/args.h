@@ -94,6 +94,11 @@ int mesh_screened_args(const char *fn, const float *xyz, const float *normal, co
                        int depth, double scale, double pointWeight, int maxIterations, double tol, double trim,
                        const float *vertices, const float *vertexIntensity, int maxVertices, const int *triangles,
                        int maxTriangles, const float *chi);
+// cs_simplify_mesh: the mesh, the parameters, the buffers and the range sweep.
+int simplify_args(const char *fn, const float *vertices, const float *vertexIntensity, int numVertices,
+                  const int *triangles, int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
+                  const float *outVertices, const float *outIntensity, int maxOutVertices, const int *outTriangles,
+                  int maxOutTriangles);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

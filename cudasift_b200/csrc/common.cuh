@@ -421,7 +421,7 @@ struct DeviceCtx {
   // counters and the point list's scratch
   GrowBuffer stereo;
   PinnedBuffer h_stereo;                   // the same tables (uploaded), then the counters (copied back)
-  // cs_poisson_mesh: the result words (copied back); its grid-sized scratch is allocated and freed per call
+  // cs_poisson_mesh and cs_simplify_mesh: the result words (copied back); their scratch is allocated and freed per call
   PinnedBuffer h_mesh;
 
   // pinned host words, allocated by ensure()
@@ -729,6 +729,16 @@ size_t mesh_result_bytes();
 // triangle count
 int mesh_result(const void *h_result, int numPoints, int maxVertices, int maxTriangles, bool screened, double *info,
                 long long stats[10]);
+
+// ---- mesh simplification (simplify.cu) -----------------------------------------------------------------------------
+// cs_simplify_mesh after its argument checks, on st with per-pass readbacks through h_result (pinned,
+// simplify_result_bytes), the scratch allocated and freed on st; fills info (may be NULL) and stats (may be NULL) and
+// returns the full triangle count.
+int simplify_run(const float *vertices, const float *intensity, int numVertices, const int *triangles, int numTriangles,
+                 int targetTriangles, double maxError, double boundaryWeight, float *outVertices, float *outIntensity,
+                 int maxOutVertices, int *outTriangles, int maxOutTriangles, cudaStream_t st, void *h_result,
+                 double *info, long long *stats);
+size_t simplify_result_bytes();
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

@@ -1240,6 +1240,75 @@ int cs_poisson_mesh_screened(const float *d_xyz, const float *d_normal, const fl
                              float *d_vertices, float *d_vertexIntensity, int maxVertices, int *d_triangles,
                              int maxTriangles, float *d_chi, double info_out[8], long long stats_out[10], double *ms);
 
+/* Mesh simplification: Garland & Heckbert's quadric error metric edge collapse (SIGGRAPH 1997) in a sequence of
+ * parallel passes, each collapsing an independent set of edges chosen by values alone (after Papageorgiou & Platis
+ * 2015, with a stricter independence rule), so the result is deterministic.  The inputs are device buffers in the layout
+ * cs_poisson_mesh writes, so the two calls chain without a copy: d_vertices [numVertices][3] float,
+ * d_vertexIntensity [numVertices] (may be NULL), d_triangles [numTriangles][3] int32.  All arithmetic below is float64,
+ * each product, sum, quotient and square root rounded once, in the order written (no contraction).
+ * 1. Input: status 2 and nothing written when a triangle index lies outside [0, numVertices), a triangle repeats a
+ *    vertex, or a vertex some triangle uses has a non-finite coordinate.  A vertex is frozen (no edge at it ever
+ *    collapses) when its faces do not form a single fan (one cycle or one open chain), or an edge at it has more than
+ *    two faces or two faces that traverse it in the same direction.  Frozen status is computed once from the input;
+ *    the link condition (rule 4) keeps every other vertex manifold.
+ * 2. Quadrics (10 entries, the upper triangle of the 4x4 matrix row-major; plane p = (n, d) adds w (p_i p_j) to entry
+ *    (i, j)): a face with n = (p1 - p0) x (p2 - p0) (x, y, z components as a1 b2 - a2 b1, a2 b0 - a0 b2,
+ *    a0 b1 - a1 b0; dot products (x + y) + z), |n| = sqrt(n.n) > 0 adds its unit plane n / |n|, d = -(n^.p0) with
+ *    w = area = |n| / 2; a boundary edge a -> b of such a face adds the plane of unit normal m / |m|, m = (b - a) x n^,
+ *    through a, with w = boundaryWeight |b - a|^2.  A vertex that is not frozen sums its faces in ascending index, then
+ *    the boundary edges at it of those faces in (face, corner) order, and the area sum A of its faces.  A collapse of
+ *    (u, v) gives Q_u + Q_v and A_u + A_v.
+ * 3. Edges: an undirected edge is identified by one canonical corner 3t + k (t the input index of its face; the edge
+ *    runs from corner k to corner k + 1 mod 3): for an interior edge the corner with a < b, for a boundary edge its
+ *    only corner; the id breaks every tie.  For Q = Q_u + Q_v = (a11 a12 a13 b1 a22 a23 b2 a33 b3 c) the position is
+ *    the minimiser -A^-1 b by Cramer's rule when det(A) = (a11 (a22 a33 - a23^2) - a12 (a12 a33 - a23 a13)) +
+ *    a13 (a12 a23 - a22 a13) > 1e-6 a11 a22 a33 (scale-invariant), else the best of u, v and the midpoint (ties to u,
+ *    then v).  cost = ((a11 x0^2 + a22 x1^2) + a33 x2^2) + 2 ((a12 x0 x1 + a13 x0 x2) + a23 x1 x2) +
+ *    2 ((b1 x0 + b2 x1) + b3 x2) + c, clamped at 0; the error is cost / A (0 when A = 0 and cost = 0, else infinite
+ *    when A = 0), a mean squared distance.  An edge is admissible when its error is finite and sqrt(error) <= maxError.
+ * 4. Validity: neither end frozen; the link condition (Dey et al. 1999): every vertex adjacent to both u and v is an
+ *    apex of a face on uv, an interior edge whose apexes w1, w2 lie in a face with u and in a face with v is refused
+ *    (the tetrahedron), an interior edge may not join two boundary vertices, and a boundary edge whose apex meets u and
+ *    v by boundary edges is refused; every surviving face of u and v with n.n > 0 keeps n_old . n_new > 0 (no flip,
+ *    and no face goes from area > 0 to area 0).
+ * 5. Pass: a candidate's key is (float(error) bits << 32) | edge id.  Of the C admissible candidates only the ceil(C/2)
+ *    with the smallest keys compete (f = 1/2, chosen by a sweep, DESIGN.md section 9); each writes atomicMin of its key
+ *    onto every vertex of the faces of u and of v (the closed 1-rings), and is selected when all of them hold its key.
+ *    Selected edges have disjoint closed neighbourhoods, so their collapses do not interact.
+ * 6. Collapse: the lower index u survives at the position, v maps to u; faces holding both are dropped, the others
+ *    keep their cyclic order.  Intensity: I_u + t (I_v - I_u) with t = ((x - p_u).(p_v - p_u)) / |p_v - p_u|^2 clamped
+ *    to [0, 1] (0 when p_u = p_v), rounded to float.  Vertex ids stay those of the input.
+ * 7. Stop: before a pass, when T <= targetTriangles (status 0) or after 1000 passes (status 3); a pass with no
+ *    admissible candidate ends the call (status 1).  In a pass that would cross the target only the selected edges
+ *    with the smallest keys are applied, the fewest whose dropped faces reach T - targetTriangles, so the result ends
+ *    at the target or one below.  Status 2: invalid input, nothing written.
+ * 8. Outputs: d_outVertices [][3] float (the vertices the surviving triangles use, in ascending input index),
+ *    d_outIntensity [] (with d_vertexIntensity), d_outTriangles [][3] (the survivors in ascending input index,
+ *    renumbered into the full vertex list), each the prefix of its full list (at most maxOutVertices or
+ *    maxOutTriangles entries).  info_out [1] (may be NULL): the largest applied sqrt(cost / A).  stats_out [9] (may be
+ *    NULL): input triangles, frozen vertices, passes (that applied a collapse), collapses, full vertex and triangle
+ *    counts, vertices and triangles written, status.  Returns the full triangle count, or CS_E_*.  numTriangles == 0
+ *    returns 0 (status 0) and makes no CUDA call.
+ * - Launches (cs_launch_count): 4 setup kernels (validate, init, corner keys, frozen and quadrics; 1 when the input is
+ *   invalid), 8 per pass (candidates, threshold, scatter, select, collapse, face count, face write, corner keys), 4 in
+ *   a final pass that finds no admissible edge, 1 more in a pass that crosses the target, and 4 output kernels; plus
+ *   cub's sorts and scans (not counted).  The host reads a few words after the input check and after each pass's
+ *   selection (one synchronise each); *ms (may be NULL) gets the event time of the whole call.
+ * - Scratch, allocated on the call's stream and freed before it returns: 212 bytes per triangle (two triangle lists and
+ *   input indices, corner keys and values and their sorted copies, candidate and selected keys and their sorted
+ *   copies, dropped-face counts and their scan) and 141 per vertex (float64 position, quadric and area, intensity,
+ *   frozen flag, remap, output index, minimum key, face counts and starts), plus cub's storage.
+ * - CS_E_ARG, before any CUDA call, naming the argument: numVertices outside [0, 2^30], numTriangles outside [0, 2^29],
+ *   targetTriangles < 0, maxError NaN or < 0 (inf allowed), boundaryWeight not finite or < 0, maxOutVertices or
+ *   maxOutTriangles < 0, NULL or not 4-byte aligned d_vertices with numVertices > 0, d_triangles with
+ *   numTriangles > 0, d_outVertices with maxOutVertices > 0, d_outTriangles with maxOutTriangles > 0, a misaligned
+ *   d_vertexIntensity or d_outIntensity, one of them given without the other, and an output (d_outVertices,
+ *   d_outIntensity, d_outTriangles) that overlaps another output or an input (one sweep over sorted ranges). */
+int cs_simplify_mesh(const float *d_vertices, const float *d_vertexIntensity, int numVertices, const int *d_triangles,
+                     int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
+                     float *d_outVertices, float *d_outIntensity, int maxOutVertices, int *d_outTriangles,
+                     int maxOutTriangles, double info_out[1], long long stats_out[9], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
