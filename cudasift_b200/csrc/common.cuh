@@ -92,6 +92,18 @@ inline int radix_bits(long long maxKey)
   return bits;
 }
 
+// The ordered key of a float: keys compare as unsigned integers in the order of the floats they encode (finite values;
+// -0 before +0), so an integer atomicMax of keys is a max of the floats (mesh.cu's box, match_guided.cu's index box).
+__device__ __forceinline__ unsigned int float_key(float f)
+{
+  const unsigned int u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(unsigned int k)
+{
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
 // ---- filter taps (host) ----------------------------------------------------------
 void scaledown_taps(float variance, float k[5]);                  // cudaSiftH.cu:315-324
 void lowpass_taps(float sigma, float k[9]);                       // cudaSiftH.cu:408-419

@@ -1,13 +1,17 @@
-// coop.cuh -- the fixed-order machinery of a cooperative solver over a sorted incidence list: bundle adjustment
-// (bundle.cu), rotation averaging (rotavg.cu) and global positioning (globalpos.cu).  Each solver sorts its incidences
-// (observation or edge end) by item (camera or image) with a stable radix sort and runs one cooperative kernel whose
-// phases are separated by grid barriers.  Every floating-point sum has a fixed order that depends on the data only, not
-// on the grid or on scheduling:
+// coop.cuh -- the fixed-order machinery of a cooperative solver: bundle adjustment (bundle.cu), rotation averaging
+// (rotavg.cu) and global positioning (globalpos.cu) over a sorted incidence list, and the MGPCG solves of Poisson
+// meshing (mesh.cu, the three-level totals only).  The first three sort their incidences (observation or edge end) by
+// item (camera or image) with a stable radix sort; each solver runs one cooperative kernel whose phases are separated
+// by grid barriers.  Every floating-point sum has a fixed order that depends on the data only, not on the grid or on
+// scheduling:
 //   - per item: the sorted incidences are cut into tiles of CO_TILE; a warp sums an item's piece of a tile
 //     lane-strided, then by a fixed xor butterfly, and one lane per item adds its pieces in ascending tile order;
 //   - totals: a CTA sums a tile of its threads' values by butterflies and its warps in order, or a warp sums a tile of
 //     32 lanes' values by a butterfly; the tile partials are then added by warp 0 of every CTA, lane-strided in
-//     ascending order and by a butterfly.
+//     ascending order and by a butterfly;
+//   - three-level totals, for item counts whose tile partials are too many for every CTA to read: tiles of
+//     CO_TREE_TILE items, then groups of THREADS tile partials the same way, then the group partials by warp 0 of every
+//     CTA (co_tree_tiles, co_tree_groups, co_tree_total).
 // No floating-point atomics.  A total is read by every CTA after the grid barrier that follows the writes of its
 // partials, so every CTA computes it from the same words by the same instructions, and a branch around a grid barrier
 // taken on it is taken alike by every CTA.  That holds only while the partials stay put: a slot read after barrier b
@@ -19,6 +23,7 @@
 namespace cs {
 
 constexpr int CO_TILE = 256;         // sorted incidences per item tile
+constexpr int CO_TREE_TILE = 2048;   // items per tile of a three-level total
 
 // The K sums of n tile partials (part[tile * stride + j]): warp 0 adds them lane-strided in ascending order, then by a
 // fixed xor butterfly; every thread of the CTA receives them.  Every CTA reads the partials after the barrier that
@@ -88,6 +93,47 @@ __device__ __forceinline__ void co_per_item(int n, double *part, F &&f)
     if (i < n) f(i, v);
     if constexpr (K > 0) co_cta_partial<K, THREADS / 32>(v, part + (size_t)(base / THREADS) * K);
   }
+}
+
+// Level 1 of a three-level total over n items in CTAs of THREADS threads: every item i < n, tile by tile (tile t: items
+// t CO_TREE_TILE + m THREADS + thread), f(i, v) may do any per-item work and adds its K values to v (zero at the start
+// of the tile); each tile's partial goes to part[t][K].
+template <int K, int THREADS, class F>
+__device__ __forceinline__ void co_tree_tiles(int n, double *part, F &&f)
+{
+  const int tiles = (n + CO_TREE_TILE - 1) / CO_TREE_TILE;
+  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
+    double v[K];
+#pragma unroll
+    for (int j = 0; j < K; j++) v[j] = 0.0;
+    for (int m = 0; m < CO_TREE_TILE / THREADS; m++) {
+      const int i = t * CO_TREE_TILE + m * THREADS + (int)threadIdx.x;
+      if (i < n) f(i, v);
+    }
+    co_cta_partial<K, THREADS / 32>(v, part + (size_t)t * K);
+  }
+}
+
+// Level 2, after the grid barrier that follows level 1: group g of THREADS tile partials sums tiles g THREADS + thread
+// into group[g][K].
+template <int K, int THREADS>
+__device__ __forceinline__ void co_tree_groups(int n, const double *part, double *group)
+{
+  const int tiles = (n + CO_TREE_TILE - 1) / CO_TREE_TILE, groups = (tiles + THREADS - 1) / THREADS;
+  for (int g = blockIdx.x; g < groups; g += gridDim.x) {
+    double v[K];
+    const int t = g * THREADS + (int)threadIdx.x;
+#pragma unroll
+    for (int j = 0; j < K; j++) v[j] = t < tiles ? part[(size_t)t * K + j] : 0.0;
+    co_cta_partial<K, THREADS / 32>(v, group + (size_t)g * K);
+  }
+}
+
+// Level 3, after the grid barrier that follows level 2: the K totals of the group partials by co_totals.
+template <int K, int THREADS>
+__device__ __forceinline__ void co_tree_total(int n, const double *group, double (&out)[K])
+{
+  co_totals<K>(group, ((n + CO_TREE_TILE - 1) / CO_TREE_TILE + THREADS - 1) / THREADS, K, out);
 }
 
 // co_per_item over the tracks that have observations: f(k, s, e, v) with [s, e) = [start[k], start[k + 1]) not empty.

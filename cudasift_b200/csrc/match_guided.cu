@@ -113,17 +113,6 @@ __device__ __forceinline__ T gd_entry(const T *__restrict__ tab, int n, int T::*
   return e;
 }
 
-// float -> unsigned key with the order of the floats (finite values only)
-__device__ __forceinline__ unsigned int fkey(float f)
-{
-  const unsigned int u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float fdec(unsigned int k)
-{
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 // (a0 * x + a1 * y) + a2, three roundings
 __device__ __forceinline__ float dot3(float a0, float a1, float a2, float x, float y)
 {
@@ -150,8 +139,8 @@ __device__ GGrid grid_of(const GHdr &h, int dir, int capCells)
     g.x0 = g.y0 = g.x1 = g.y1 = 0.0f; g.inv = 1.0f; g.cs = 1.0; g.gx = g.gy = 1;
     return g;
   }
-  g.x0 = fdec(~h.bb[dir][0]); g.y0 = fdec(~h.bb[dir][1]);
-  g.x1 = fdec(h.bb[dir][2]); g.y1 = fdec(h.bb[dir][3]);
+  g.x0 = key_float(~h.bb[dir][0]); g.y0 = key_float(~h.bb[dir][1]);
+  g.x1 = key_float(h.bb[dir][2]); g.y1 = key_float(h.bb[dir][3]);
   const double n = (double)h.count[dir];
   const double wx = (double)g.x1 - g.x0, wy = (double)g.y1 - g.y0, w = fmax(wx, wy);
   double cs = fmax(sqrt(wx * wy * GD_PER_CELL / n), w * GD_PER_CELL / n);
@@ -237,10 +226,10 @@ guided_prep_kernel(const GJob *__restrict__ jobs, int numJobs)
     for (int d = 0; d < 2; d++) {
       const bool mine = indexed && dir == d;
       const unsigned int cnt = __reduce_add_sync(FULL, mine ? 1u : 0u);
-      const unsigned int k0 = __reduce_max_sync(FULL, mine ? ~fkey(g.key.x) : 0u);
-      const unsigned int k1 = __reduce_max_sync(FULL, mine ? ~fkey(g.key.y) : 0u);
-      const unsigned int k2 = __reduce_max_sync(FULL, mine ? fkey(g.key.x) : 0u);
-      const unsigned int k3 = __reduce_max_sync(FULL, mine ? fkey(g.key.y) : 0u);
+      const unsigned int k0 = __reduce_max_sync(FULL, mine ? ~float_key(g.key.x) : 0u);
+      const unsigned int k1 = __reduce_max_sync(FULL, mine ? ~float_key(g.key.y) : 0u);
+      const unsigned int k2 = __reduce_max_sync(FULL, mine ? float_key(g.key.x) : 0u);
+      const unsigned int k3 = __reduce_max_sync(FULL, mine ? float_key(g.key.y) : 0u);
       const unsigned int bad = __reduce_or_sync(FULL, (mine && !safe) ? 1u : 0u);
       if (lane == 0 && cnt) {
         atomicAdd(&h->count[d], cnt);

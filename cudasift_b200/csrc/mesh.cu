@@ -8,12 +8,16 @@
 // Determinism: no floating-point atomics.  Integer atomics only where the result does not depend on their order (the
 // bounding box as ordered-integer max, the cell histogram, the kept-vertex bit masks).  Every floating-point sum has a
 // fixed order that depends on the grid size or the point count only: a node's splat runs over its cells in ascending
-// index and each cell's points in sorted order; a total over nodes or points sums tiles of MTILE items, then groups of
-// MGROUP tile partials, then the group partials (mesh_tile_sums, mesh_group_sums, mesh_total).
+// index and each cell's points in sorted order; a total over nodes or points is coop.cuh's three-level total (tiles of
+// CO_TREE_TILE items, groups of MT tile partials, then the group partials: co_tree_tiles, co_tree_groups,
+// co_tree_total).  The vertex and triangle lists are counted lists (counted_list.cuh), and the box is a max of
+// common.cuh's ordered float keys (float_key).
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "coop.cuh"
+#include "counted_list.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -22,8 +26,6 @@ namespace cs {
 namespace {
 
 constexpr int MT = 256;           // threads per CTA of every mesh kernel
-constexpr int MTILE = 2048;       // items per tile of a fixed-order total (8 per thread)
-constexpr int MGROUP = MT;        // tile partials per group
 constexpr int NU = 2;             // red-black sweep pairs before (and black-red pairs after) the coarse correction
 constexpr int NU_COARSE = 8;      // the coarsest level (4 cells): 8 red-black pairs, then 8 black-red pairs
 constexpr int LOCAL_N = 16;       // levels of at most 16 cells per axis run inside CTA 0, without grid barriers
@@ -87,16 +89,6 @@ struct ScreenParams {
   NLevel lv[MAX_LEVELS];          // lv[l].x, f, t alias MeshParams::lv[l]
 };
 
-__device__ __forceinline__ unsigned int float_key(float f)
-{
-  const unsigned int u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_float(unsigned int k)
-{
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 __device__ __forceinline__ bool point_used(const MeshParams &p, int i, double nh[3])
 {
   const float *x = p.xyz + 3 * (size_t)i, *n = p.nrm + 3 * (size_t)i;
@@ -137,93 +129,6 @@ __device__ __forceinline__ void node_ijk(int idx, int n1, int &i, int &j, int &k
   const int r = idx / n1;
   j = r % n1;
   k = r / n1;
-}
-
-// ---- fixed-order totals ---------------------------------------------------------------------------------------------
-template <int K>
-__device__ __forceinline__ void warp_sum(double (&v)[K])
-{
-#pragma unroll
-  for (int o = 16; o; o >>= 1)
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] += __shfl_xor_sync(0xffffffffu, v[j], o);
-}
-
-// A CTA's sum of one value per thread: warp butterflies, then thread 0 adds the warps in order and writes out[K].
-template <int K>
-__device__ __forceinline__ void cta_sum(double (&v)[K], double *out)
-{
-  __shared__ double s_w[MT / 32][K];
-  warp_sum(v);
-  if ((threadIdx.x & 31) == 0)
-#pragma unroll
-    for (int j = 0; j < K; j++) s_w[threadIdx.x >> 5][j] = v[j];
-  __syncthreads();
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int j = 0; j < K; j++) {
-      double s = s_w[0][j];
-      for (int w = 1; w < MT / 32; w++) s += s_w[w][j];
-      out[j] = s;
-    }
-  __syncthreads();
-}
-
-// Every item i < n, tile by tile (tile t: items t MTILE + m MT + thread, m = 0..7): f(i, v) may do any per-item work
-// and adds its K values to v; each tile's partial goes to part[t][K].
-template <int K, class F>
-__device__ __forceinline__ void mesh_tile_sums(int n, double *part, F &&f)
-{
-  const int tiles = (n + MTILE - 1) / MTILE;
-  for (int t = blockIdx.x; t < tiles; t += gridDim.x) {
-    double v[K];
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] = 0.0;
-    for (int m = 0; m < MTILE / MT; m++) {
-      const int i = t * MTILE + m * MT + (int)threadIdx.x;
-      if (i < n) f(i, v);
-    }
-    cta_sum<K>(v, part + (size_t)t * K);
-  }
-}
-
-// The group partials of the tile partials of n items: group g sums tiles g MGROUP + thread.
-template <int K>
-__device__ __forceinline__ void mesh_group_sums(int n, const double *part, double *group)
-{
-  const int tiles = (n + MTILE - 1) / MTILE, groups = (tiles + MGROUP - 1) / MGROUP;
-  for (int g = blockIdx.x; g < groups; g += gridDim.x) {
-    double v[K];
-    const int t = g * MGROUP + (int)threadIdx.x;
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] = t < tiles ? part[(size_t)t * K + j] : 0.0;
-    cta_sum<K>(v, group + (size_t)g * K);
-  }
-}
-
-// The total of the group partials: warp 0 adds them lane-strided in ascending order, then by a butterfly; every thread
-// receives it.
-template <int K>
-__device__ __forceinline__ void mesh_total(int n, const double *group, double (&out)[K])
-{
-  __shared__ double s_tot[K];
-  const int groups = ((n + MTILE - 1) / MTILE + MGROUP - 1) / MGROUP;
-  if (threadIdx.x < 32) {
-    double v[K];
-#pragma unroll
-    for (int j = 0; j < K; j++) v[j] = 0.0;
-    for (int g = (int)threadIdx.x; g < groups; g += 32)
-#pragma unroll
-      for (int j = 0; j < K; j++) v[j] += group[(size_t)g * K + j];
-    warp_sum(v);
-    if (threadIdx.x == 0)
-#pragma unroll
-      for (int j = 0; j < K; j++) s_tot[j] = v[j];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int j = 0; j < K; j++) out[j] = s_tot[j];
-  __syncthreads();
 }
 
 // ---- multigrid level operations (tid / nth: the threads taking part; sync: their barrier) ---------------------------
@@ -511,15 +416,15 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   };
   auto total1 = [&](double &out) {
     grid.sync();
-    mesh_group_sums<1>(M, p.tilePart, p.groupPart);
+    co_tree_groups<1, MT>(M, p.tilePart, p.groupPart);
     grid.sync();
     double t[1];
-    mesh_total<1>(M, p.groupPart, t);
+    co_tree_total<1, MT>(M, p.groupPart, t);
     out = t[0];
   };
 
   double bb, rr, rz = 0.0;
-  mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
     r[i] = b[i];
     z[i] = 0.0f;
     v[0] += (double)b[i] * (double)b[i];
@@ -530,7 +435,7 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   bool done = rr <= p.tol2 * bb;
   if (!done) {
     v_cycle(p, grid);
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
       pp[i] = z[i];
       v[0] += (double)r[i] * (double)z[i];
     });
@@ -539,7 +444,7 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   while (!done) {
     grid.sync();                                       // p complete before A p reads its neighbours
     double pq;
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
       const float a = interior(i) ? 6.0f * pp[i] - nbr_sum(pp, i, n1) : 0.0f;
       q[i] = a;
       v[0] += (double)pp[i] * (double)a;
@@ -547,7 +452,7 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
     total1(pq);
     if (!(pq > 0.0)) break;
     const double alpha = rz / pq;
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
       x[i] = (float)((double)x[i] + alpha * (double)pp[i]);
       const float ri = (float)((double)r[i] - alpha * (double)q[i]);
       r[i] = ri;
@@ -559,7 +464,7 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
     if (rr <= p.tol2 * bb || k >= p.maxIterations) break;
     v_cycle(p, grid);
     double rzNew;
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
     total1(rzNew);
     const double beta = rzNew / rz;
     rz = rzNew;
@@ -568,7 +473,7 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   grid.sync();
   // the true residual b - A chi, in float64 from the floats
   double rt;
-  mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
     if (!interior(i)) return;
     const double ax = 6.0 * (double)x[i] - (((((double)x[i - 1] + (double)x[i + 1]) + (double)x[i - n1]) +
                                              (double)x[i + n1]) + (double)x[i - ss]) - (double)x[i + ss];
@@ -578,7 +483,7 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   total1(rt);
   // tau and the mean density: chi and D trilinear at each used point's g, in sorted order
   const int used = (int)R.used;
-  mesh_tile_sums<2>(used, p.tilePart, [&](int s, double *v) {
+  co_tree_tiles<2, MT>(used, p.tilePart, [&](int s, double *v) {
     const double *g = p.gs + 3 * (size_t)s;
     int c[3];
     double t[3];
@@ -599,10 +504,10 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
     v[1] += sd;
   });
   grid.sync();
-  mesh_group_sums<2>(used, p.tilePart, p.groupPart);
+  co_tree_groups<2, MT>(used, p.tilePart, p.groupPart);
   grid.sync();
   double td[2];
-  mesh_total<2>(used, p.groupPart, td);
+  co_tree_total<2, MT>(used, p.groupPart, td);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     const double tau = td[0] / used;
     R.info[4] = tau;
@@ -844,10 +749,10 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
   float *x = p.chi, *r = p.r, *b = p.b, *z = p.V0, *pp = p.V1, *q = p.V2;
   auto total1 = [&](int n, double &out) {
     grid.sync();
-    mesh_group_sums<1>(n, p.tilePart, p.groupPart);
+    co_tree_groups<1, MT>(n, p.tilePart, p.groupPart);
     grid.sync();
     double t[1];
-    mesh_total<1>(n, p.groupPart, t);
+    co_tree_total<1, MT>(n, p.groupPart, t);
     out = t[0];
   };
   // chi (or D) trilinear at sorted point s, as the Dirichlet call's tau
@@ -871,13 +776,13 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
 
   // omega = alpha / mean density
   double dsum;
-  mesh_tile_sums<1>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(p.D, s); });
+  co_tree_tiles<1, MT>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(p.D, s); });
   total1(used, dsum);
   const double omega = sc.alpha / (dsum / used);
   // the screening diagonal of every level: s_l(Q) = (omega / 2^l) sum (B^l_p(Q))^2 at g / 2^l, over the fine cells of
   // Q's support in ascending index (rows of cells as contiguous runs of sorted points)
   // (level 0: a thread per node over its rows in order; coarser levels: a warp per node, lane j summing the rows
-  // j, j + 32, ... in order, then warp_sum's butterfly, lane 0's value)
+  // j, j + 32, ... in order, then vp_warp_sum's butterfly, lane 0's value)
   auto diag_rows = [&](int l, int idx, int lane, int step) {
     const int c1 = sc.lv[l].n + 1, f = 1 << l;
     const double inv = 1.0 / f;
@@ -909,13 +814,13 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
         l++;
       }
       double v[1] = {diag_rows(l, idx, lane, 32)};
-      warp_sum(v);
+      vp_warp_sum(v);
       if (lane == 0) sc.lv[l].s[idx] = (float)(omega / (1 << l) * v[0]);
     }
   }
 
   double bb, rr, rz = 0.0;
-  mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
     r[i] = b[i];
     z[i] = 0.0f;
     v[0] += (double)b[i] * (double)b[i];
@@ -926,7 +831,7 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
   bool done = rr <= p.tol2 * bb;
   if (!done) {
     v_cycle_nm(p, sc, grid);
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
       pp[i] = z[i];
       v[0] += (double)r[i] * (double)z[i];
     });
@@ -937,7 +842,7 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
     screen_points(p, sc, pp, omega, used, grid);
     grid.sync();
     double pq;
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
       int a, bq, c;
       node_ijk(i, n1, a, bq, c);
       float deg;
@@ -949,7 +854,7 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
     total1(M, pq);
     if (!(pq > 0.0)) break;
     const double alpha = rz / pq;
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
       x[i] = (float)((double)x[i] + alpha * (double)pp[i]);
       const float ri = (float)((double)r[i] - alpha * (double)q[i]);
       r[i] = ri;
@@ -961,7 +866,7 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
     if (rr <= p.tol2 * bb || k >= p.maxIterations) break;
     v_cycle_nm(p, sc, grid);
     double rzNew;
-    mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
     total1(M, rzNew);
     const double beta = rzNew / rz;
     rz = rzNew;
@@ -972,7 +877,7 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
   screen_points(p, sc, x, omega, used, grid);
   grid.sync();
   double rt;
-  mesh_tile_sums<1>(M, p.tilePart, [&](int i, double *v) {
+  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
     int a, bq, c;
     node_ijk(i, n1, a, bq, c);
     double deg;
@@ -983,7 +888,7 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
   total1(M, rt);
   // tau: chi trilinear at the used points, in sorted order
   double tsum;
-  mesh_tile_sums<1>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(x, s); });
+  co_tree_tiles<1, MT>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(x, s); });
   total1(used, tsum);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     R.info[4] = tsum / used;
@@ -1150,6 +1055,10 @@ __device__ __forceinline__ bool vertex_kept(const Extract &X, const EdgeRef &e)
   return !(X.lerp_at(X.D, e.node, db, X.edge_t(e.node, db)) < X.thr);
 }
 
+// Step 1 of counted list `which` (counted_list.cuh) into blockCounts[which][blockIdx.x].  This is counted_cta_count
+// with the slot's address formed by thread 0 after the sum; handing counted_cta_count the slot's pointer forms it in
+// every thread before the sum, which changes the code of mesh_count_kernel and mesh_kept_kernel (whose SASS
+// tests/test_mesh_screened_cpu.py pins).
 __device__ __forceinline__ void block_counts(const MeshParams &p, int which, int v)
 {
   using BR = cub::BlockReduce<int, MT>;
@@ -1195,16 +1104,6 @@ __global__ void __launch_bounds__(MT) mesh_kept_kernel(MeshParams p)
   block_counts(p, 3, idx < p.M ? __popc(kept_bits(p, idx)) : 0);
 }
 
-__device__ __forceinline__ int block_exclusive(int v)
-{
-  using BS = cub::BlockScan<int, MT>;
-  __shared__ typename BS::TempStorage tmp;
-  int e;
-  BS(tmp).ExclusiveSum(v, e);
-  __syncthreads();
-  return e;
-}
-
 // The kept vertices in ascending edge id (node, then direction), and each node's first kept index; the last block
 // records the four totals.
 __global__ void __launch_bounds__(MT) mesh_vertices_kernel(MeshParams p)
@@ -1213,11 +1112,11 @@ __global__ void __launch_bounds__(MT) mesh_vertices_kernel(MeshParams p)
   const int nb = p.numBlocks;
   if (blockIdx.x == nb - 1 && threadIdx.x < 4) {
     const int w = threadIdx.x == 0 ? 0 : threadIdx.x == 1 ? 1 : threadIdx.x == 2 ? 3 : 2;   // counts[] order
-    R.counts[threadIdx.x] = (long long)p.blockOffsets[(size_t)w * nb + nb - 1] + p.blockCounts[(size_t)w * nb + nb - 1];
+    R.counts[threadIdx.x] = counted_total(p.blockOffsets, p.blockCounts, (size_t)w * nb + nb - 1);
   }
   const int idx = blockIdx.x * MT + threadIdx.x;
   const unsigned int m = idx < p.M ? kept_bits(p, idx) : 0u;
-  const int first = p.blockOffsets[3 * (size_t)nb + blockIdx.x] + block_exclusive(__popc(m));
+  const int first = p.blockOffsets[3 * (size_t)nb + blockIdx.x] + counted_position<MT>(__popc(m));
   if (idx >= p.M) return;
   p.kstart[idx] = first;
   if (!m) return;
@@ -1257,7 +1156,7 @@ __global__ void __launch_bounds__(MT) mesh_triangles_kernel(MeshParams p)
     });
   };
   if (cell) each([&](const EdgeRef *) { nk++; });
-  int t = p.blockOffsets[2 * (size_t)p.numBlocks + blockIdx.x] + block_exclusive(nk);
+  int t = p.blockOffsets[2 * (size_t)p.numBlocks + blockIdx.x] + counted_position<MT>(nk);
   if (!cell || !nk) return;
   each([&](const EdgeRef *e) {
     if (t < p.maxTriangles)
@@ -1283,8 +1182,8 @@ int mesh_run(const float *xyz, const float *normal, const float *intensity, int 
   const int P = numPoints;
   const bool hasI = intensity != nullptr;
   const int nb = idivup(M, MT);
-  const int tilesMax = std::max(idivup(M, MTILE), idivup(std::max(P, 1), MTILE));
-  const int groupsMax = idivup(tilesMax, MGROUP);
+  const int tilesMax = std::max(idivup(M, CO_TREE_TILE), idivup(std::max(P, 1), CO_TREE_TILE));
+  const int groupsMax = idivup(tilesMax, MT);          // a group is MT tile partials
   const int bits = radix_bits((long long)N * N * N);
 
   size_t sortBytes = 0, scanBytes = 0, scanBytes2 = 0;

@@ -1,12 +1,14 @@
-// ordered_list.cuh -- the ordered lists the matcher and verification write on the device: mutual pairs and ratio-test
-// pairs (single, batched and guided; match_mutual.cu), verification's valid pairs and its inliers (verify.cu).  Each is
-// built in three steps without atomics, so its order follows from the values alone:
+// ordered_list.cuh -- the keep-bit lists written on the device without atomics, so that their order follows from the
+// values alone: mutual pairs and ratio-test pairs (single, batched and guided; match_mutual.cu), verification's
+// valid pairs and its inliers (verify.cu) and fused points (stereo.cu).  Each is built in three steps:
 //   1. flag    one thread per row computes a keep bit; one ballot word per 32 rows and one count per CTA of LIST_ROWS
 //              rows (list_flag);
 //   2. scan    every CTA sums the counts of the CTAs before it, then scans its own ballot words (list_position);
 //   3. write   every kept row writes its entry at its exclusive position; the CTA that holds the last row writes the
 //              total.
-// The scratch of an n-row list is list_words(n) ballot words and list_ctas(n) CTA counts.
+// The scratch of an n-row list is list_words(n) ballot words and list_ctas(n) CTA counts (match_tc.cu and
+// match_guided.cu size their waves' pair scratch by them).  Lists where a thread emits any number of entries are the
+// counted lists of counted_list.cuh.
 #pragma once
 
 namespace cs {

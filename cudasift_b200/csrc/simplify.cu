@@ -1,8 +1,9 @@
 // simplify.cu -- quadric-error edge collapse (cs_simplify_mesh) in independent parallel passes: the vertex -> face
 // adjacency by a stable sort of corner keys, one thread per edge for the validity tests, position and cost, a radix
 // sort of the candidate keys for the gating threshold, an atomicMin scatter of keys onto the closed 1-rings of both
-// ends and the selection test, the collapse, and the face remap as count-scan-write passes.  Every rule is stated in
-// cudasift_b200.h at cs_simplify_mesh; tests/simplify_oracle.py restates them in float64.
+// ends and the selection test, the collapse, and the face remap as count-scan-write passes (the faces and the output
+// vertices are counted lists of counted_list.cuh).  Every rule is stated in cudasift_b200.h at cs_simplify_mesh;
+// tests/simplify_oracle.py restates them in float64.
 //
 // Determinism: no floating-point atomics; integer atomics only where the result does not depend on their order (counts,
 // the minimum key of a vertex, the largest applied error as ordered bits).  This unit is compiled with -fmad=false so
@@ -15,6 +16,7 @@
 #include <cub/cub.cuh>
 
 #include "common.cuh"
+#include "counted_list.cuh"
 
 namespace cs {
 
@@ -213,26 +215,6 @@ __device__ bool evaluate(const SimplifyParams &p, int t, int k, int &u, int &v, 
   if (any_face(p, uu, flips) || any_face(p, vv, flips)) return false;
   drops = interior ? 2 : 1;
   return true;
-}
-
-__device__ __forceinline__ int block_count(int v, int *out)
-{
-  using BR = cub::BlockReduce<int, ST>;
-  __shared__ typename BR::TempStorage tmp;
-  const int s = BR(tmp).Sum(v);
-  if (threadIdx.x == 0) *out = s;
-  __syncthreads();
-  return s;
-}
-
-__device__ __forceinline__ int block_exclusive(int v)
-{
-  using BS = cub::BlockScan<int, ST>;
-  __shared__ typename BS::TempStorage tmp;
-  int e;
-  BS(tmp).ExclusiveSum(v, e);
-  __syncthreads();
-  return e;
 }
 
 // ---- setup ------------------------------------------------------------------------------------------------------------
@@ -472,7 +454,7 @@ __global__ void __launch_bounds__(ST) simplify_face_count_kernel(SimplifyParams 
 {
   const int t = blockIdx.x * ST + threadIdx.x;
   int g[3];
-  block_count(t < p.T && kept_face(p, t, g) ? 1 : 0, p.blockCounts + blockIdx.x);
+  counted_cta_count<ST>(t < p.T && kept_face(p, t, g) ? 1 : 0, p.blockCounts + blockIdx.x);
 }
 
 __global__ void __launch_bounds__(ST) simplify_face_write_kernel(SimplifyParams p)
@@ -480,9 +462,9 @@ __global__ void __launch_bounds__(ST) simplify_face_write_kernel(SimplifyParams 
   const int t = blockIdx.x * ST + threadIdx.x;
   int g[3];
   const bool keep = t < p.T && kept_face(p, t, g);
-  const int at = p.blockOffsets[blockIdx.x] + block_exclusive(keep ? 1 : 0);
+  const int at = p.blockOffsets[blockIdx.x] + counted_position<ST>(keep ? 1 : 0);
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0)
-    p.res->tris = p.blockOffsets[gridDim.x - 1] + p.blockCounts[gridDim.x - 1];
+    p.res->tris = counted_total(p.blockOffsets, p.blockCounts, gridDim.x - 1);
   if (!keep) return;
   for (int j = 0; j < 3; j++) p.triN[3 * (size_t)at + j] = g[j];
   p.tidN[at] = p.tid[t];
@@ -497,7 +479,7 @@ __global__ void __launch_bounds__(ST) simplify_used_kernel(SimplifyParams p)
 __global__ void __launch_bounds__(ST) simplify_vcount_kernel(SimplifyParams p)
 {
   const int x = blockIdx.x * ST + threadIdx.x;
-  block_count(x < p.V ? p.used[x] : 0, p.blockCounts + blockIdx.x);
+  counted_cta_count<ST>(x < p.V ? p.used[x] : 0, p.blockCounts + blockIdx.x);
 }
 
 // the used vertices in ascending input index; used[] becomes the output index
@@ -505,9 +487,9 @@ __global__ void __launch_bounds__(ST) simplify_vwrite_kernel(SimplifyParams p)
 {
   const int x = blockIdx.x * ST + threadIdx.x;
   const int u = x < p.V ? p.used[x] : 0;
-  const int at = p.blockOffsets[blockIdx.x] + block_exclusive(u);
+  const int at = p.blockOffsets[blockIdx.x] + counted_position<ST>(u);
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0)
-    p.res->verts = p.blockOffsets[gridDim.x - 1] + p.blockCounts[gridDim.x - 1];
+    p.res->verts = counted_total(p.blockOffsets, p.blockCounts, gridDim.x - 1);
   if (!u) return;
   p.used[x] = at;
   if (at >= p.maxOutV) return;
