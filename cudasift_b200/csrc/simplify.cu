@@ -335,6 +335,14 @@ __global__ void __launch_bounds__(ST) simplify_vertex_kernel(SimplifyParams p)
 }
 
 // ---- a pass -----------------------------------------------------------------------------------------------------------
+// The tie order s(id) of rule 5: a bijection of the 32-bit ids (an odd multiplier mod 2^32, then an invertible
+// xorshift), so keys stay unique while equal errors are not ranked in raster order.
+__device__ __forceinline__ unsigned int tie_of(unsigned int id)
+{
+  const unsigned int m = id * 0x9E3779B1u;
+  return m ^ (m >> 16);
+}
+
 __global__ void __launch_bounds__(ST) simplify_candidate_kernel(SimplifyParams p)
 {
   unsigned int n = 0;
@@ -346,7 +354,7 @@ __global__ void __launch_bounds__(ST) simplify_candidate_kernel(SimplifyParams p
     unsigned long long key = NO_KEY;
     if (evaluate(p, t, k, u, v, x, err, drops)) {
       key = ((unsigned long long)__float_as_uint(__double2float_rn(err)) << 32) |
-            (unsigned int)(3 * p.tid[t] + k);
+            tie_of((unsigned int)(3 * p.tid[t] + k));
       n++;
     }
     p.key[c] = key;

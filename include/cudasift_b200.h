@@ -1260,7 +1260,7 @@ int cs_poisson_mesh_screened(const float *d_xyz, const float *d_normal, const fl
  *    (u, v) gives Q_u + Q_v and A_u + A_v.
  * 3. Edges: an undirected edge is identified by one canonical corner 3t + k (t the input index of its face; the edge
  *    runs from corner k to corner k + 1 mod 3): for an interior edge the corner with a < b, for a boundary edge its
- *    only corner; the id breaks every tie.  For Q = Q_u + Q_v = (a11 a12 a13 b1 a22 a23 b2 a33 b3 c) the position is
+ *    only corner; s(id) (rule 5) breaks every tie.  For Q = Q_u + Q_v = (a11 a12 a13 b1 a22 a23 b2 a33 b3 c) the position is
  *    the minimiser -A^-1 b by Cramer's rule when det(A) = (a11 (a22 a33 - a23^2) - a12 (a12 a33 - a23 a13)) +
  *    a13 (a12 a23 - a22 a13) > 1e-6 a11 a22 a33 (scale-invariant), else the best of u, v and the midpoint (ties to u,
  *    then v).  cost = ((a11 x0^2 + a22 x1^2) + a33 x2^2) + 2 ((a12 x0 x1 + a13 x0 x2) + a23 x1 x2) +
@@ -1271,8 +1271,11 @@ int cs_poisson_mesh_screened(const float *d_xyz, const float *d_normal, const fl
  *    (the tetrahedron), an interior edge may not join two boundary vertices, and a boundary edge whose apex meets u and
  *    v by boundary edges is refused; every surviving face of u and v with n.n > 0 keeps n_old . n_new > 0 (no flip,
  *    and no face goes from area > 0 to area 0).
- * 5. Pass: a candidate's key is (float(error) bits << 32) | edge id.  Of the C admissible candidates only the ceil(C/2)
- *    with the smallest keys compete (f = 1/2, chosen by a sweep, DESIGN.md section 9); each writes atomicMin of its key
+ * 5. Pass: a candidate's key is (float(error) bits << 32) | s(edge id), float() rounding to nearest, with the
+ *    bijection s(i) = m ^ (m >> 16), m = i * 0x9E3779B1 mod 2^32: keys are unique, and equal errors (a flat region)
+ *    are not ordered along the input's raster, where only one edge per pass would hold the minimum of its rings.  Of
+ *    the C admissible candidates only the ceil(C/2) with the smallest keys compete (f = 1/2, chosen by a sweep,
+ *    DESIGN.md section 9); each writes atomicMin of its key
  *    onto every vertex of the faces of u and of v (the closed 1-rings), and is selected when all of them hold its key.
  *    Selected edges have disjoint closed neighbourhoods, so their collapses do not interact.
  * 6. Collapse: the lower index u survives at the position, v maps to u; faces holding both are dropped, the others

@@ -118,8 +118,16 @@ def f32(x):
     return float(np.float32(x))
 
 
+def tie_of(eid):
+    """s(id): the bijection of the 32-bit ids that orders equal errors (m = id 0x9E3779B1 mod 2^32, m ^ (m >> 16))."""
+    m = (eid * 0x9E3779B1) & 0xFFFFFFFF
+    return m ^ (m >> 16)
+
+
 def key_of(err, eid):
-    return (int(np.float32(err).view(np.uint32)) << 32) | eid
+    with np.errstate(over="ignore"):        # an error above FLT_MAX rounds to an infinite key, as on the GPU
+        f = np.float32(err)
+    return (int(f.view(np.uint32)) << 32) | tie_of(eid)
 
 
 # ---- the mesh state ---------------------------------------------------------------------------------------------------

@@ -182,6 +182,34 @@ def test_boundary_weight_sweep(sheet):
     assert out[2][1] <= out[0][1]
 
 
+def test_tie_order_is_a_bijection():
+    """s(id) = m ^ (m >> 16), m = id 0x9E3779B1 mod 2^32: the xorshift is its own inverse and the odd multiplier has an
+    inverse mod 2^32, so s is a bijection of the 32-bit ids and keys stay unique; checked through the inverse on ids
+    across the whole range and exhaustively as distinct values over the first 3 * 2^20 ids."""
+    inv = pow(0x9E3779B1, -1, 1 << 32)
+    undo = lambda y: ((y ^ (y >> 16)) * inv) & 0xFFFFFFFF
+    rng = np.random.default_rng(3)
+    ids = [0, 1, 2, 3, (1 << 31) - 1, 1 << 31, (1 << 32) - 1] + [int(i) for i in rng.integers(0, 1 << 32, 20000)]
+    for i in ids:
+        s = so.tie_of(i)
+        assert 0 <= s < (1 << 32) and undo(s) == i
+    n = 3 << 20
+    m = (np.arange(n, dtype=np.uint64) * np.uint64(0x9E3779B1)) & np.uint64(0xFFFFFFFF)
+    s = m ^ (m >> np.uint64(16))
+    assert len(np.unique(s)) == n and [so.tie_of(int(i)) for i in (5, 77, n - 1)] == [int(s[5]), int(s[77]), int(s[-1])]
+    # equal errors: keys differ, and their order is not the ids' order
+    keys = [so.key_of(0.0, i) for i in range(3000)]
+    assert len(set(keys)) == 3000 and keys != sorted(keys)
+    assert so.key_of(1.0, 0) > so.key_of(0.5, 2999) and so.key_of(math.inf, 0) > so.key_of(1e38, 2999)
+
+
+def test_flat_grid_selects_many_edges_per_pass():
+    """Every error of a flat grid is 0, so the tie order alone decides the selection: more than one edge per pass."""
+    v, t = scs.grid(16)
+    r = so.simplify(v, t, target=len(t) // 10, max_passes=1)
+    assert r["stats"][2] == 1 and r["stats"][3] >= 10
+
+
 # ---- library --------------------------------------------------------------------------------------------------------
 
 def _call(verts=0x1000, vint=None, V=4, tris=0x2000, T=4, target=0, maxError=math.inf, bw=1.0, ov=0x10000, oi=None,
