@@ -124,6 +124,8 @@ def lib():
                                           vp, ip, vp, ip, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_simplify_mesh": (ip, [vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, vp, vp, ip, vp, ip, vp, vp,
                                   c.POINTER(c.c_double)]),
+        "cs_texture_mesh": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, c.c_double, c.c_double, c.c_double, ip, ip, ip,
+                                 vp, ip, vp, vp, vp, vp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1454,6 +1456,117 @@ def SimplifyMesh(vertices, triangles, intensity=None, targetTriangles=0, maxErro
         for b in ins + outs:
             if b is not None:
                 b.free()
+
+
+def TextureMesh(images, Ks, Rs, ts, vertices, triangles, smoothness=0.5, maxViewAngle=75.0, depthTol=0.01, padding=2,
+                atlasWidth=None, maxSweeps=100):
+    """A texture atlas for a triangle mesh from the images that see it (cs_texture_mesh): every face takes the image
+    that sees it largest, unoccluded (depth buffers, relative depthTol) and within maxViewAngle degrees of its normal,
+    traded against smoothness (the labelling's lambda) per pair of adjacent faces with different images; adjacent faces
+    with the same image form charts, whose image rectangles (padding pixels around) are copied into one atlas
+    atlasWidth texels wide (None: the widest image, rounded up to a multiple of 256, at least 1024).  images, Ks, Rs, ts
+    as for PatchMatchStereo (pinhole), vertices float32 [V, 3] and triangles int32 [T, 3] as SimplifyMesh or PoissonMesh
+    return them.  The atlas is computed again into a buffer of its full height when the first guess is too small, so
+    nothing is truncated.  Returns (atlas float32 [rows, atlasWidth], uv float32 [T, 3, 2] in atlas pixels (NaN for an
+    unseen face), labels int32 [T] (the image, -1 unseen), charts int32 [C, 8] {image, x0, y0, width, height, ox, oy,
+    faces}, info float64 [2] {energy before, after the sweeps}, stats int64 [11] (the header's), ms)."""
+    S = len(images)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    V, T = len(X), len(F)
+    arrs, bufs, table = _upload_images(images)
+    if atlasWidth is None:
+        atlasWidth = max(1024, -(-max([im.shape[1] for im in arrs] + [1]) // 256) * 256)
+    W = int(atlasWidth)
+    rows, maxCharts = max(64, int(np.sqrt(max(sum(im.size for im in arrs), 1)))), max(T, 1)
+    try:
+        ins = [DeviceBuffer(max(X.nbytes, 4)), DeviceBuffer(max(F.nbytes, 4))]
+        bufs += ins
+        for b, a in zip(ins, (X, F)):
+            if a.size:
+                b.upload(a)
+        outs = [DeviceBuffer(24 * T + 4), DeviceBuffer(4 * T + 4)]
+        bufs += outs
+        while True:
+            atlas = DeviceBuffer(4 * rows * W + 4)
+            try:
+                charts = np.zeros((maxCharts, 8), np.int32)
+                info, stats, ms = np.zeros(2), np.zeros(11, np.int64), ctypes.c_double(0.0)
+                C = _check(lib().cs_texture_mesh(table if S else None, S, _ptr(K), _ptr(R), _ptr(t), ins[0].ptr, V,
+                                                 ins[1].ptr, T, float(smoothness), float(maxViewAngle),
+                                                 float(depthTol), int(padding), W, int(maxSweeps), atlas.ptr, rows,
+                                                 outs[0].ptr, outs[1].ptr, None, _ptr(charts), maxCharts, _ptr(info),
+                                                 _ptr(stats), ctypes.byref(ms)), "TextureMesh")
+                full = int(stats[8])
+                if full > rows:
+                    rows = full
+                    continue
+                img = atlas.download(np.float32, full * W).reshape(full, W)
+                uv = outs[0].download(np.float32, 6 * T).reshape(T, 3, 2)
+                labels = outs[1].download(np.int32, T)
+                return img, uv, labels, charts[:C].copy(), info, stats, ms.value
+            finally:
+                atlas.free()
+    finally:
+        for b in bufs:
+            b.free()
+
+
+def _png_grey(path, img):
+    """An 8-bit greyscale PNG of img (uint8 [H, W]) by zlib and struct alone."""
+    import struct
+    import zlib
+    img = np.ascontiguousarray(img, np.uint8)
+    H, W = img.shape
+
+    def chunk(kind, data):
+        body = kind + data
+        return struct.pack(">I", len(data)) + body + struct.pack(">I", zlib.crc32(body) & 0xFFFFFFFF)
+
+    raw = np.concatenate([np.zeros((H, 1), np.uint8), img], axis=1).tobytes()   # filter type 0 per row
+    with open(path, "wb") as f:
+        f.write(b"\x89PNG\r\n\x1a\n")
+        f.write(chunk(b"IHDR", struct.pack(">IIBBBBB", W, H, 8, 0, 0, 0, 0)))
+        f.write(chunk(b"IDAT", zlib.compress(raw, 6)))
+        f.write(chunk(b"IEND", b""))
+
+
+def save_textured_obj(path, vertices, triangles, uv, atlas):
+    """A textured mesh as OBJ + MTL + PNG: path.obj (or path as given when it ends in .obj), its .mtl and .png beside
+    it.  uv are TextureMesh's atlas pixel coordinates (converted to OBJ's [0, 1] with v up); atlas the float atlas,
+    written as 8-bit grey (rounded, clipped to 0..255).  Faces with NaN coordinates (unseen) are written without
+    texture coordinates.  Returns the paths written (obj, mtl, png)."""
+    import os as _os
+    base = path[:-4] if path.endswith(".obj") else path
+    name = _os.path.basename(base)
+    objp, mtlp, pngp = base + ".obj", base + ".mtl", base + ".png"
+    atlas = np.asarray(atlas, np.float32)
+    H, W = atlas.shape
+    _png_grey(pngp, np.clip(np.rint(atlas), 0, 255).astype(np.uint8))
+    with open(mtlp, "w") as f:
+        f.write("newmtl atlas\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nmap_Kd %s.png\n" % name)
+    X = np.asarray(vertices, np.float32).reshape(-1, 3)
+    F = np.asarray(triangles, np.int64).reshape(-1, 3)
+    U = np.asarray(uv, np.float64).reshape(-1, 3, 2)
+    seen = np.isfinite(U).all(axis=(1, 2))
+    vt = np.stack([(U[..., 0] + 0.5) / W, 1.0 - (U[..., 1] + 0.5) / H], -1)   # texel (x, y) centred at x + 1/2, v up
+    lines = ["mtllib %s.mtl" % name, "usemtl atlas"]
+    lines += ["v %.9g %.9g %.9g" % tuple(p) for p in X]
+    k = 0
+    faces = []
+    for f in range(len(F)):
+        a, b, c = F[f] + 1
+        if seen[f]:
+            for j in range(3):
+                lines.append("vt %.9g %.9g" % tuple(vt[f, j]))
+            faces.append("f %d/%d %d/%d %d/%d" % (a, k + 1, b, k + 2, c, k + 3))
+            k += 3
+        else:
+            faces.append("f %d %d %d" % (a, b, c))
+    with open(objp, "w") as f:
+        f.write("\n".join(lines + faces) + "\n")
+    return objp, mtlp, pngp
 
 
 def SelectStereoViews(Ks, Rs, ts, offsets, members, points, numSources=8, minTriAngle=1.0):

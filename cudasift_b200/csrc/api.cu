@@ -785,6 +785,7 @@ int cs_set_tuning(const char *key, int value)
   if (key && strcmp(key, "sd_split") == 0) { cs::g_sd_split = value; return 0; }
   if (key && strcmp(key, "cap32") == 0) { cs::g_cap32 = value ? 1 : 0; return 0; }
   if (key && strcmp(key, "cap32_limit") == 0) { cs::g_cap_limit = (value > 0 && value < 200) ? value : 32; return 0; }
+  if (key && strcmp(key, "texture_group_bytes") == 0) { cs::g_texture_group_bytes = value; return 0; }
   cs::set_error("cs_set_tuning: unknown key");
   return CS_E_ARG;
 }
@@ -1788,6 +1789,35 @@ int cs_simplify_mesh(const float *d_vertices, const float *d_vertexIntensity, in
     return simplify_run(d_vertices, d_vertexIntensity, numVertices, d_triangles, numTriangles, targetTriangles,
                         maxError, boundaryWeight, d_outVertices, d_outIntensity, maxOutVertices, d_outTriangles,
                         maxOutTriangles, c->stream, c->h_mesh.p, info_out, stats_out);
+  });
+}
+
+int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                    const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles, double lambda,
+                    double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                    float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
+                    int *charts_out, int maxCharts, double info_out[2], long long stats_out[11], double *ms)
+{
+  const char *fn = "cs_texture_mesh";
+  if (ms) *ms = 0.0;
+  int r = texture_args(fn, images, numImages, Ks, Rs, ts, d_vertices, numVertices, d_triangles, numTriangles, lambda,
+                       maxViewAngleDeg, depthTol, padding, atlasWidth, maxSweeps, d_atlas, maxAtlasRows, d_uv,
+                       d_faceView, d_faceChart, charts_out, maxCharts);
+  if (r < 0) return r;
+  if (numTriangles == 0) {
+    if (info_out) info_out[0] = info_out[1] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 11; k++) stats_out[k] = 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(texture_result_bytes())) < 0) return r;
+  return timed_sync(fn, c, ms, [&] {
+    return texture_run(images, numImages, Ks, Rs, ts, d_vertices, numVertices, d_triangles, numTriangles, lambda,
+                       maxViewAngleDeg, depthTol, padding, atlasWidth, maxSweeps, d_atlas, maxAtlasRows, d_uv,
+                       d_faceView, d_faceChart, charts_out, maxCharts, c->stream, c->h_mesh.p, info_out, stats_out);
   });
 }
 

@@ -1057,4 +1057,52 @@ int simplify_args(const char *fn, const float *vertices, const float *vertexInte
   return rs.check(fn);
 }
 
+int texture_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                 const double *ts, const float *vertices, int numVertices, const int *triangles, int numTriangles,
+                 double lambda, double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                 const float *atlas, int maxAtlasRows, const float *uv, const int *faceView, const int *faceChart,
+                 const int *chartsOut, int maxCharts)
+{
+  int r;
+  if ((r = stereo_images(fn, images, numImages, 1, Ks, Rs, ts, true)) < 0) return r;
+  if (numVertices < 0 || numVertices > (1 << 30)) return arg_error(fn, "numVertices must be in [0, 2^30]");
+  if (numTriangles < 0 || numTriangles > (1 << 29)) return arg_error(fn, "numTriangles must be in [0, 2^29]");
+  if (!std::isfinite(lambda) || lambda < 0.0) return arg_error(fn, "lambda must be finite and >= 0");
+  if (!(maxViewAngleDeg > 0.0 && maxViewAngleDeg <= 90.0)) return arg_error(fn, "maxViewAngleDeg must be in (0, 90]");
+  if (!(depthTol >= 0.0 && depthTol <= 1.0)) return arg_error(fn, "depthTol must be finite and in [0, 1]");
+  if (padding < 0 || padding > 16) return arg_error(fn, "padding must be in [0, 16]");
+  int widest = 0;
+  for (int a = 0; a < numImages; a++) widest = std::max(widest, images[a].width);
+  if (atlasWidth < widest || atlasWidth > 32768)
+    return arg_error(fn, "atlasWidth must be in [the largest image width (%d), 32768]", widest);
+  if (maxSweeps < 0 || maxSweeps > 1000) return arg_error(fn, "maxSweeps must be in [0, 1000]");
+  if (maxAtlasRows < 0) return arg_error(fn, "maxAtlasRows must be >= 0");
+  if (maxCharts < 0) return arg_error(fn, "maxCharts must be >= 0");
+  if (numVertices > 0 && (!vertices || misaligned(vertices, 4)))
+    return arg_error(fn, "numVertices > 0 needs d_vertices (4-byte aligned)");
+  if (numTriangles > 0 && (!triangles || misaligned(triangles, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_triangles (4-byte aligned)");
+  if (numTriangles > 0 && (!uv || misaligned(uv, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_uv (4-byte aligned)");
+  if (numTriangles > 0 && (!faceView || misaligned(faceView, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_faceView (4-byte aligned)");
+  if (misaligned(faceChart, 4)) return arg_error(fn, "d_faceChart must be 4-byte aligned");
+  if (maxAtlasRows > 0 && (!atlas || misaligned(atlas, 4)))
+    return arg_error(fn, "maxAtlasRows > 0 needs d_atlas (4-byte aligned)");
+  if (maxCharts > 0 && !chartsOut) return arg_error(fn, "maxCharts > 0 needs charts_out");
+  // the outputs (written), the mesh and the images (read)
+  static const char *const names[7] = {"d_atlas", "d_uv", "d_faceView", "d_faceChart",
+                                       "d_vertices", "d_triangles", "images[%d].d_img"};
+  ArgRanges rs(names, 6 + (size_t)numImages);
+  const size_t T = (size_t)numTriangles;
+  rs.add(atlas, 4 * (size_t)maxAtlasRows * atlasWidth, 0, 0, true);
+  rs.add(uv, 24 * T, 1, 0, true);
+  rs.add(faceView, 4 * T, 2, 0, true);
+  if (faceChart) rs.add(faceChart, 4 * T, 3, 0, true);
+  rs.add(vertices, 12 * (size_t)numVertices, 4, 0, false);
+  rs.add(triangles, 12 * T, 5, 0, false);
+  for (int a = 0; a < numImages; a++) rs.add(images[a].d_img, image_bytes(images[a]), 6, a, false);
+  return rs.check(fn);
+}
+
 }  // namespace cs

@@ -99,6 +99,12 @@ int simplify_args(const char *fn, const float *vertices, const float *vertexInte
                   const int *triangles, int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
                   const float *outVertices, const float *outIntensity, int maxOutVertices, const int *outTriangles,
                   int maxOutTriangles);
+// cs_texture_mesh: the images and cameras, the mesh, the parameters, the buffers and the range sweep.
+int texture_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                 const double *ts, const float *vertices, int numVertices, const int *triangles, int numTriangles,
+                 double lambda, double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                 const float *atlas, int maxAtlasRows, const float *uv, const int *faceView, const int *faceChart,
+                 const int *chartsOut, int maxCharts);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

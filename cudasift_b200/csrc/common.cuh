@@ -752,6 +752,19 @@ int simplify_run(const float *vertices, const float *intensity, int numVertices,
                  double *info, long long *stats);
 size_t simplify_result_bytes();
 
+// ---- mesh texturing (texture.cu) -----------------------------------------------------------------------------------
+// The depth-buffer bytes of one image group (cs_set_tuning("texture_group_bytes"); 0 or less: 1 GiB).
+extern long long g_texture_group_bytes;
+// cs_texture_mesh after its argument checks (numTriangles > 0), on st with readbacks through h_result (pinned,
+// texture_result_bytes), the scratch allocated and freed on st; fills charts_out, info (may be NULL) and stats (may be
+// NULL) and returns the full chart count.
+int texture_run(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                const float *vertices, int numVertices, const int *triangles, int numTriangles, double lambda,
+                double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps, float *atlas,
+                int maxAtlasRows, float *uv, int *faceView, int *faceChart, int *chartsOut, int maxCharts,
+                cudaStream_t st, void *h_result, double *info, long long *stats);
+size_t texture_result_bytes();
+
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).
 #define VERIFY_ESSENTIAL 3

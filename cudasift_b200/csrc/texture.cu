@@ -1,0 +1,788 @@
+// texture.cu -- mesh texturing (cs_texture_mesh) after Waechter, Moehrle & Goesele 2014, without seam levelling: the
+// face adjacency by a radix sort of undirected edge keys, a depth buffer per image by 64-bit atomicMin of (depth, face)
+// keys, one thread per face for the visibility tests and its best candidates, a Jones-Plassmann colouring of the face
+// graph, ICM sweeps over the colours, charts by union-find, the shelf packing on the host, and the texel copy.  Every
+// rule is stated in cudasift_b200.h at cs_texture_mesh; tests/texture_oracle.py restates them in float64.
+//
+// Determinism: no floating-point atomics; integer atomics only where the result does not depend on their order (the
+// depth keys, counts, union-find links to the lower root, the chart rectangles).  The energy totals use coop.cuh's
+// three-level order.  This unit is compiled with -fmad=false so that every float64 product and sum is rounded once, in
+// the order written, as the oracle computes it.
+#include <climits>
+#include <cmath>
+#include <cstring>
+
+#include <cub/cub.cuh>
+
+#include "common.cuh"
+#include "coop.cuh"
+
+namespace cs {
+
+long long g_texture_group_bytes = 0;          // cs_set_tuning("texture_group_bytes"); 0: TEXTURE_GROUP_BYTES
+
+namespace {
+
+constexpr int TT = 256;                       // threads per CTA of every texture kernel
+constexpr int MCAND = 8;                      // candidates a face keeps
+constexpr long long TEXTURE_GROUP_BYTES = 1ll << 30;
+constexpr unsigned long long EMPTY = ~0ull;
+
+// One image of the call: its pixels, size, camera and, in the group being processed, its depth buffer.
+struct TexCam {
+  const float *img;
+  int W, H, pitch;
+  double K[9], R[9], t[3], C[3];
+  unsigned long long *buf;
+};
+
+// The device words of a call, copied back after each step that decides the next.
+struct TextureResult {
+  unsigned int bad;
+  unsigned int cand;                          // (face, image) pairs that passed every test
+  unsigned int unseen;
+  unsigned int left;                          // uncoloured faces after a round
+  int maxColour;
+  unsigned int changed;                       // labels changed in a sweep
+  int charts;                                 // exclusive scan of the root flags at T
+  double energy;
+};
+
+struct TextureParams {
+  TextureResult *res;
+  int V, T, numImages;
+  const float *vin;
+  const int *tin;
+  const TexCam *cams;
+  int g0, gn;                                 // the images of the current group
+  unsigned long long *ekey, *ekeyS;           // edge keys [3T] and sorted
+  int *eval, *evalS;                          // their corners
+  int *nbr;                                   // [3T]: the face across edge k of f, or -1
+  double *cq;                                 // [T][MCAND] candidate quality
+  int *ca, *cn;                               // [T][MCAND] candidate image, [T] count
+  int *label, *colA, *colB, *parent, *flag, *chartIdx;
+  double *part, *group;                       // energy tile and group partials
+  double lambda, cosLim, depthTol;
+  int padding;
+  int *craw;                                  // [C][6] {image, xmin, ymin, xmax, ymax, faces}
+  const int *ctab;                            // [C][8] the chart table of cs_texture_mesh
+  const long long *cstart;                    // [C + 1] first texel of each chart
+  int numCharts;
+  float *atlas, *uv;
+  int *faceView, *faceChart;
+  int atlasWidth, rowsWritten;
+};
+
+struct D3 {
+  double x, y, z;
+};
+__device__ __forceinline__ D3 sub3(D3 a, D3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
+__device__ __forceinline__ D3 cross3(D3 a, D3 b)
+{
+  return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
+}
+__device__ __forceinline__ double dot3(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ D3 vert(const TextureParams &p, int v)
+{
+  return {(double)p.vin[3 * (size_t)v], (double)p.vin[3 * (size_t)v + 1], (double)p.vin[3 * (size_t)v + 2]};
+}
+
+// Y = R X + t, (u, v) = (K Y)_{0,1} / Y_z (rule 2)
+__device__ __forceinline__ void project(const TexCam &c, D3 X, double &u, double &v, double &z)
+{
+  const double y0 = ((c.R[0] * X.x + c.R[1] * X.y) + c.R[2] * X.z) + c.t[0];
+  const double y1 = ((c.R[3] * X.x + c.R[4] * X.y) + c.R[5] * X.z) + c.t[1];
+  const double y2 = ((c.R[6] * X.x + c.R[7] * X.y) + c.R[8] * X.z) + c.t[2];
+  u = ((c.K[0] * y0 + c.K[1] * y1) + c.K[2] * y2) / y2;
+  v = ((c.K[3] * y0 + c.K[4] * y1) + c.K[5] * y2) / y2;
+  z = y2;
+}
+
+// The doubled signed area of a projected face, corners in face order.
+__device__ __forceinline__ double area2_of(const double *u, const double *v)
+{
+  return (u[1] - u[0]) * (v[2] - v[0]) - (v[1] - v[0]) * (u[2] - u[0]);
+}
+
+__device__ __forceinline__ unsigned int tie_of(unsigned int id)
+{
+  const unsigned int m = id * 0x9E3779B1u;
+  return m ^ (m >> 16);
+}
+
+// ---- input and adjacency (rule 1) ---------------------------------------------------------------------------------
+__global__ void __launch_bounds__(TT) texture_validate_kernel(TextureParams p)
+{
+  for (int t = blockIdx.x * TT + threadIdx.x; t < p.T; t += gridDim.x * TT) {
+    const int a = p.tin[3 * (size_t)t], b = p.tin[3 * (size_t)t + 1], c = p.tin[3 * (size_t)t + 2];
+    bool bad = a < 0 || a >= p.V || b < 0 || b >= p.V || c < 0 || c >= p.V || a == b || b == c || a == c;
+    for (int j = 0; j < 3 && !bad; j++) {
+      const int w = p.tin[3 * (size_t)t + j];
+      for (int d = 0; d < 3; d++) bad = bad || !isfinite(p.vin[3 * (size_t)w + d]);
+    }
+    if (bad) atomicOr(&p.res->bad, 1u);
+  }
+}
+
+__global__ void __launch_bounds__(TT) texture_edges_kernel(TextureParams p)
+{
+  for (int c = blockIdx.x * TT + threadIdx.x; c < 3 * p.T; c += gridDim.x * TT) {
+    const int t = c / 3, k = c - 3 * t;
+    const unsigned int a = p.tin[c], b = p.tin[3 * t + (k + 1) % 3];
+    p.ekey[c] = ((unsigned long long)min(a, b) << 32) | max(a, b);
+    p.eval[c] = c;
+    p.nbr[c] = -1;
+  }
+}
+
+// a run of exactly two equal keys in the sorted list joins its two faces
+__global__ void __launch_bounds__(TT) texture_adjacency_kernel(TextureParams p)
+{
+  const int n = 3 * p.T;
+  for (int i = blockIdx.x * TT + threadIdx.x; i + 1 < n; i += gridDim.x * TT) {
+    const unsigned long long k = p.ekeyS[i];
+    if ((i > 0 && p.ekeyS[i - 1] == k) || p.ekeyS[i + 1] != k || (i + 2 < n && p.ekeyS[i + 2] == k)) continue;
+    const int c1 = p.evalS[i], c2 = p.evalS[i + 1];
+    p.nbr[c1] = c2 / 3;
+    p.nbr[c2] = c1 / 3;
+  }
+}
+
+// ---- depth buffers (rule 2) ---------------------------------------------------------------------------------------
+// One thread per (image of the group, face): every pixel centre of the clipped bounding box that the three oriented
+// edge functions cover gets atomicMin of (float(depth) bits << 32) | face.
+__global__ void __launch_bounds__(TT) texture_raster_kernel(TextureParams p)
+{
+  const long long n = (long long)p.gn * p.T;
+  for (long long i = blockIdx.x * (long long)TT + threadIdx.x; i < n; i += (long long)gridDim.x * TT) {
+    const int g = p.g0 + (int)(i / p.T), f = (int)(i % p.T);
+    const TexCam &c = p.cams[g];
+    int id[3];
+    double u[3], v[3], z[3];
+    bool front = true;
+    for (int k = 0; k < 3; k++) {
+      id[k] = p.tin[3 * (size_t)f + k];
+      project(c, vert(p, id[k]), u[k], v[k], z[k]);
+      front = front && z[k] > 0.0;
+    }
+    if (!front) continue;
+    const double A = area2_of(u, v);
+    if (!(A != 0.0) || !isfinite(A)) continue;
+    const double s = A > 0.0 ? 1.0 : -1.0;
+    const double xlo = fmax(0.0, ceil(fmin(fmin(u[0], u[1]), u[2]))), xhi = fmin(c.W - 1.0, floor(fmax(fmax(u[0], u[1]), u[2])));
+    const double ylo = fmax(0.0, ceil(fmin(fmin(v[0], v[1]), v[2]))), yhi = fmin(c.H - 1.0, floor(fmax(fmax(v[0], v[1]), v[2])));
+    if (!(xlo <= xhi && ylo <= yhi)) continue;
+    // edge k runs corner k -> k + 1; it is evaluated from its lower vertex id P to the higher Q, then signed
+    int P[3];
+    double du[3], dv[3], sg[3];
+    for (int k = 0; k < 3; k++) {
+      const int a = k, b = (k + 1) % 3;
+      const bool lo = id[a] < id[b];
+      P[k] = lo ? a : b;
+      const int Q = lo ? b : a;
+      du[k] = u[Q] - u[P[k]];
+      dv[k] = v[Q] - v[P[k]];
+      sg[k] = lo ? s : -s;
+    }
+    for (int y = (int)ylo; y <= (int)yhi; y++)
+      for (int x = (int)xlo; x <= (int)xhi; x++) {
+        double w[3];
+        bool in = true;
+        for (int k = 0; k < 3 && in; k++) {
+          w[k] = sg[k] * (du[k] * ((double)y - v[P[k]]) - dv[k] * ((double)x - u[P[k]]));
+          in = w[k] >= 0.0;
+        }
+        if (!in) continue;
+        const double W = (w[0] + w[1]) + w[2];
+        if (!(W > 0.0)) continue;
+        const double iz = ((w[1] / z[0] + w[2] / z[1]) + w[0] / z[2]) / W;
+        const float d = __double2float_rn(1.0 / iz);
+        atomicMin(c.buf + (size_t)y * c.W + x, ((unsigned long long)__float_as_uint(d) << 32) | (unsigned int)f);
+      }
+  }
+}
+
+// ---- candidates (rule 3) ------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool sees(const TexCam &c, D3 X, int f, double depthTol, double &u, double &v)
+{
+  double z;
+  project(c, X, u, v, z);
+  if (!(z > 0.0 && u >= 0.0 && u <= c.W - 1.0 && v >= 0.0 && v <= c.H - 1.0)) return false;
+  const int px = (int)floor(u + 0.5), py = (int)floor(v + 0.5);
+  const unsigned long long key = c.buf[(size_t)py * c.W + px];
+  if (key == EMPTY || (unsigned int)key == (unsigned int)f) return true;
+  return z <= (double)__uint_as_float((unsigned int)(key >> 32)) * (1.0 + depthTol);
+}
+
+// One thread per face: the images of the group in ascending order, each that passes every test inserted into the
+// face's list by (q descending, image ascending), at most MCAND kept.
+__global__ void __launch_bounds__(TT) texture_candidate_kernel(TextureParams p)
+{
+  unsigned int found = 0;
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    const D3 p0 = vert(p, p.tin[3 * (size_t)f]), p1 = vert(p, p.tin[3 * (size_t)f + 1]),
+             p2 = vert(p, p.tin[3 * (size_t)f + 2]);
+    const D3 n = cross3(sub3(p1, p0), sub3(p2, p0));
+    const D3 cen = {((p0.x + p1.x) + p2.x) / 3.0, ((p0.y + p1.y) + p2.y) / 3.0, ((p0.z + p1.z) + p2.z) / 3.0};
+    const double ln = sqrt(dot3(n, n));
+    double *cq = p.cq + (size_t)f * MCAND;
+    int *ca = p.ca + (size_t)f * MCAND;
+    int cnt = p.cn[f];
+    for (int g = p.g0; g < p.g0 + p.gn; g++) {
+      const TexCam &c = p.cams[g];
+      const D3 d = sub3({c.C[0], c.C[1], c.C[2]}, cen);
+      const double dn = dot3(n, d);
+      if (!(dn > 0.0) || !(dn >= p.cosLim * (ln * sqrt(dot3(d, d))))) continue;
+      double u[3], v[3], uc, vc;
+      if (!sees(c, p0, f, p.depthTol, u[0], v[0]) || !sees(c, p1, f, p.depthTol, u[1], v[1]) ||
+          !sees(c, p2, f, p.depthTol, u[2], v[2]) || !sees(c, cen, f, p.depthTol, uc, vc))
+        continue;
+      const double q = 0.5 * fabs(area2_of(u, v));
+      if (!(q > 0.0)) continue;
+      found++;
+      int r = cnt < MCAND ? cnt : MCAND;
+      while (r > 0 && (q > cq[r - 1] || (q == cq[r - 1] && g < ca[r - 1]))) {
+        if (r < MCAND) { cq[r] = cq[r - 1]; ca[r] = ca[r - 1]; }
+        r--;
+      }
+      if (r < MCAND) { cq[r] = q; ca[r] = g; }
+      if (cnt < MCAND) cnt++;
+    }
+    p.cn[f] = cnt;
+  }
+  if (found) atomicAdd(&p.res->cand, found);
+}
+
+// ---- labelling (rule 4) -------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(TT) texture_label_init_kernel(TextureParams p)
+{
+  unsigned int unseen = 0;
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    const bool seen = p.cn[f] > 0;
+    p.label[f] = seen ? p.ca[(size_t)f * MCAND] : -1;
+    unseen += !seen;
+    p.colA[f] = -1;
+    p.parent[f] = f;
+  }
+  if (unseen) atomicAdd(&p.res->unseen, unseen);
+}
+
+// A Jones-Plassmann round: reads colA (the state at its start), writes colB.
+__global__ void __launch_bounds__(TT) texture_colour_kernel(TextureParams p)
+{
+  unsigned int left = 0;
+  int top = -1;
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    int col = p.colA[f];
+    if (col < 0) {
+      const unsigned int sf = tie_of((unsigned int)f);
+      bool wins = true;
+      unsigned int held = 0;
+      for (int k = 0; k < 3; k++) {
+        const int g = p.nbr[3 * (size_t)f + k];
+        if (g < 0) continue;
+        const int cg = p.colA[g];
+        if (cg < 0) wins = wins && sf > tie_of((unsigned int)g);
+        else held |= 1u << cg;
+      }
+      if (wins) {
+        col = 0;
+        while (held & (1u << col)) col++;
+        top = max(top, col);
+      } else {
+        left++;
+      }
+    }
+    p.colB[f] = col;
+  }
+  if (left) atomicAdd(&p.res->left, left);
+  if (top >= 0) atomicMax(&p.res->maxColour, top);
+}
+
+// the labelled neighbours of f whose label differs from l
+__device__ __forceinline__ int disagree(const TextureParams &p, int f, int l, bool above)
+{
+  int n = 0;
+  for (int k = 0; k < 3; k++) {
+    const int g = p.nbr[3 * (size_t)f + k];
+    if (g < 0 || (above && g < f)) continue;
+    const int lg = p.label[g];
+    n += lg >= 0 && lg != l;
+  }
+  return n;
+}
+
+// e_f = D(f, l_f) + lambda * (the labelled neighbours g > f across an edge with l_g != l_f): tile partials
+__global__ void __launch_bounds__(TT) texture_energy_kernel(TextureParams p)
+{
+  co_tree_tiles<1, TT>(p.T, p.part, [&](int f, double *v) {
+    const int l = p.label[f];
+    if (l < 0) return;
+    const double *cq = p.cq + (size_t)f * MCAND;
+    const int *ca = p.ca + (size_t)f * MCAND;
+    int r = 0;
+    while (ca[r] != l) r++;
+    v[0] += (1.0 - cq[r] / cq[0]) + p.lambda * (double)disagree(p, f, l, true);
+  });
+}
+
+// one CTA: the group partials and the total in co_tree_groups / co_tree_total's order
+__global__ void __launch_bounds__(TT) texture_total_kernel(TextureParams p)
+{
+  const int tiles = (p.T + CO_TREE_TILE - 1) / CO_TREE_TILE, groups = (tiles + TT - 1) / TT;
+  for (int g = 0; g < groups; g++) {
+    const int t = g * TT + (int)threadIdx.x;
+    double v[1] = {t < tiles ? p.part[t] : 0.0};
+    co_cta_partial<1, TT / 32>(v, p.group + g);
+  }
+  double tot[1];
+  co_totals<1>(p.group, groups, 1, tot);
+  if (threadIdx.x == 0) p.res->energy = tot[0];
+}
+
+// An ICM step of the faces of one colour: the candidate of lowest local energy, the current label on ties, then the
+// earlier rank.
+__global__ void __launch_bounds__(TT) texture_icm_kernel(TextureParams p, int colour)
+{
+  unsigned int changed = 0;
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    const int cur = p.label[f];
+    if (cur < 0 || p.colA[f] != colour) continue;
+    const double *cq = p.cq + (size_t)f * MCAND;
+    const int *ca = p.ca + (size_t)f * MCAND;
+    const int m = p.cn[f] < MCAND ? p.cn[f] : MCAND;
+    auto local = [&](int r) { return (1.0 - cq[r] / cq[0]) + p.lambda * (double)disagree(p, f, ca[r], false); };
+    int r0 = 0;
+    while (ca[r0] != cur) r0++;
+    int best = cur;
+    double bestE = local(r0);
+    for (int r = 0; r < m; r++) {
+      const double e = local(r);
+      if (e < bestE) { bestE = e; best = ca[r]; }
+    }
+    if (best != cur) {
+      p.label[f] = best;
+      changed++;
+    }
+  }
+  if (changed) atomicAdd(&p.res->changed, changed);
+}
+
+// ---- charts (rule 5) ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ int find_root(const int *parent, int x)
+{
+  for (;;) {
+    const int y = ((const volatile int *)parent)[x];
+    if (y == x) return x;
+    x = y;
+  }
+}
+
+// union of every adjacent pair with equal labels; the higher root is linked below the lower one, so every root is the
+// lowest face of its component whatever the order of the links
+__global__ void __launch_bounds__(TT) texture_hook_kernel(TextureParams p)
+{
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    const int l = p.label[f];
+    if (l < 0) continue;
+    for (int k = 0; k < 3; k++) {
+      const int g = p.nbr[3 * (size_t)f + k];
+      if (g <= f || p.label[g] != l) continue;
+      for (;;) {
+        const int a = find_root(p.parent, f), b = find_root(p.parent, g);
+        if (a == b) break;
+        const int hi = max(a, b), lo = min(a, b);
+        if (atomicCAS(&p.parent[hi], hi, lo) == hi) break;
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(TT) texture_roots_kernel(TextureParams p)
+{
+  for (int f = blockIdx.x * TT + threadIdx.x; f <= p.T; f += gridDim.x * TT) {
+    if (f == p.T) { p.flag[f] = 0; continue; }
+    const int r = find_root(p.parent, f);
+    p.parent[f] = r;
+    p.flag[f] = p.label[f] >= 0 && r == f;
+  }
+}
+
+__global__ void __launch_bounds__(TT) texture_chart_init_kernel(TextureParams p)
+{
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    if (!p.flag[f]) continue;
+    int *e = p.craw + 6 * (size_t)p.chartIdx[f];
+    e[0] = p.label[f];
+    e[1] = e[2] = INT_MAX;
+    e[3] = e[4] = INT_MIN;
+    e[5] = 0;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) p.res->charts = p.chartIdx[p.T];
+}
+
+__global__ void __launch_bounds__(TT) texture_rect_kernel(TextureParams p)
+{
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    const int l = p.label[f];
+    if (l < 0) continue;
+    int *e = p.craw + 6 * (size_t)p.chartIdx[p.parent[f]];
+    const TexCam &c = p.cams[l];
+    for (int k = 0; k < 3; k++) {
+      double u, v, z;
+      project(c, vert(p, p.tin[3 * (size_t)f + k]), u, v, z);
+      atomicMin(e + 1, (int)floor(u));
+      atomicMin(e + 2, (int)floor(v));
+      atomicMax(e + 3, (int)ceil(u));
+      atomicMax(e + 4, (int)ceil(v));
+    }
+    atomicAdd(e + 5, 1);
+  }
+}
+
+// ---- outputs (rule 6) ---------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(TT) texture_uv_kernel(TextureParams p)
+{
+  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+    const int l = p.label[f];
+    float *uv = p.uv + 6 * (size_t)f;
+    p.faceView[f] = l;
+    if (l < 0) {
+      for (int k = 0; k < 6; k++) uv[k] = __int_as_float(0x7fc00000);
+      if (p.faceChart) p.faceChart[f] = -1;
+      continue;
+    }
+    const int ch = p.chartIdx[p.parent[f]];
+    const int *e = p.ctab + 8 * (size_t)ch;
+    const TexCam &c = p.cams[l];
+    for (int k = 0; k < 3; k++) {
+      double u, v, z;
+      project(c, vert(p, p.tin[3 * (size_t)f + k]), u, v, z);
+      uv[2 * k] = __double2float_rn((u - (double)e[1]) + (double)e[5]);
+      uv[2 * k + 1] = __double2float_rn((v - (double)e[2]) + (double)e[6]);
+    }
+    if (p.faceChart) p.faceChart[f] = ch;
+  }
+}
+
+// one thread per chart texel (charts one after the other, rows of a chart in order)
+__global__ void __launch_bounds__(TT) texture_atlas_kernel(TextureParams p)
+{
+  const long long n = p.numCharts ? p.cstart[p.numCharts] : 0;
+  for (long long i = blockIdx.x * (long long)TT + threadIdx.x; i < n; i += (long long)gridDim.x * TT) {
+    int lo = 0, hi = p.numCharts - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (p.cstart[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    const int *e = p.ctab + 8 * (size_t)lo;
+    const int w = e[3];
+    const long long local = i - p.cstart[lo];
+    const int y = (int)(local / w), x = (int)(local - (long long)y * w);
+    const int Y = e[6] + y;
+    if (Y >= p.rowsWritten) continue;
+    const TexCam &c = p.cams[e[0]];
+    p.atlas[(size_t)Y * p.atlasWidth + e[5] + x] = c.img[(size_t)(e[2] + y) * c.pitch + e[1] + x];
+  }
+}
+
+int grid_of(long long n) { return (int)std::max(1ll, std::min((n + TT - 1) / TT, 8192ll)); }
+
+}  // namespace
+
+int texture_run(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                const float *vin, int V, const int *tin, int T, double lambda, double maxViewAngleDeg,
+                double depthTol, int padding, int atlasWidth, int maxSweeps, float *atlas, int maxAtlasRows, float *uv,
+                int *faceView, int *faceChart, int *chartsOut, int maxCharts, cudaStream_t st, void *h_res,
+                double *info, long long *stats)
+{
+  const size_t C3 = 3 * (size_t)T;
+  size_t tb[2] = {};
+  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (unsigned long long *)nullptr,
+                                          (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, (int)C3, 0,
+                                          64, st));
+  CS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb[1], (int *)nullptr, (int *)nullptr, T + 1, st));
+  size_t tempBytes = std::max(tb[0], tb[1]);
+  const long long cap = g_texture_group_bytes > 0 ? g_texture_group_bytes : TEXTURE_GROUP_BYTES;
+
+  // the image groups: consecutive images while their buffers fit the cap (at least one image each)
+  std::vector<int> groupStart{0};
+  long long bufMax = 0, acc = 0;
+  for (int a = 0; a < numImages; a++) {
+    const long long b = 8ll * images[a].width * images[a].height;
+    if (a > groupStart.back() && acc + b > cap) {
+      groupStart.push_back(a);
+      acc = 0;
+    }
+    acc += b;
+    bufMax = std::max(bufMax, acc);
+  }
+  groupStart.push_back(numImages);
+  const int tiles = (T + CO_TREE_TILE - 1) / CO_TREE_TILE, groups = (tiles + TT - 1) / TT;
+
+  Layout L(256);
+  const size_t resAt = L.take(sizeof(TextureResult));
+  const size_t camAt = L.take((size_t)numImages * sizeof(TexCam));
+  const size_t ekAt = L.take(C3 * 8), ekSAt = L.take(C3 * 8), evAt = L.take(C3 * 4), evSAt = L.take(C3 * 4);
+  const size_t nbrAt = L.take(C3 * 4);
+  const size_t cqAt = L.take((size_t)T * MCAND * 8), caAt = L.take((size_t)T * MCAND * 4), cnAt = L.take((size_t)T * 4);
+  const size_t labAt = L.take((size_t)T * 4), colAAt = L.take((size_t)T * 4), colBAt = L.take((size_t)T * 4);
+  const size_t parAt = L.take((size_t)T * 4), flagAt = L.take(((size_t)T + 1) * 4),
+               idxAt = L.take(((size_t)T + 1) * 4);
+  const size_t partAt = L.take((size_t)tiles * 8), groupAt = L.take((size_t)groups * 8);
+  const size_t crawAt = L.take((size_t)T * 24), ctabAt = L.take((size_t)T * 32),
+               cstartAt = L.take(((size_t)T + 1) * 8);
+  const size_t bufAt = L.take((size_t)bufMax);
+  const size_t tempAt = L.take(tempBytes);
+  char *base = nullptr;
+  CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
+  auto at = [&](size_t off) { return base + off; };
+
+  std::vector<TexCam> cams(numImages);
+  const double pi = 3.14159265358979323846;
+  for (int a = 0; a < numImages; a++) {
+    TexCam &c = cams[a];
+    c.img = images[a].d_img;
+    c.W = images[a].width;
+    c.H = images[a].height;
+    c.pitch = images[a].pitch;
+    for (int k = 0; k < 9; k++) c.K[k] = Ks[9 * (size_t)a + k], c.R[k] = Rs[9 * (size_t)a + k];
+    for (int k = 0; k < 3; k++) c.t[k] = ts[3 * (size_t)a + k];
+    for (int i = 0; i < 3; i++) c.C[i] = -((c.R[i] * c.t[0] + c.R[3 + i] * c.t[1]) + c.R[6 + i] * c.t[2]);
+    c.buf = nullptr;
+  }
+
+  TextureParams p{};
+  p.res = reinterpret_cast<TextureResult *>(at(resAt));
+  p.V = V;
+  p.T = T;
+  p.numImages = numImages;
+  p.vin = vin;
+  p.tin = tin;
+  p.cams = reinterpret_cast<const TexCam *>(at(camAt));
+  p.ekey = reinterpret_cast<unsigned long long *>(at(ekAt));
+  p.ekeyS = reinterpret_cast<unsigned long long *>(at(ekSAt));
+  p.eval = reinterpret_cast<int *>(at(evAt));
+  p.evalS = reinterpret_cast<int *>(at(evSAt));
+  p.nbr = reinterpret_cast<int *>(at(nbrAt));
+  p.cq = reinterpret_cast<double *>(at(cqAt));
+  p.ca = reinterpret_cast<int *>(at(caAt));
+  p.cn = reinterpret_cast<int *>(at(cnAt));
+  p.label = reinterpret_cast<int *>(at(labAt));
+  p.colA = reinterpret_cast<int *>(at(colAAt));
+  p.colB = reinterpret_cast<int *>(at(colBAt));
+  p.parent = reinterpret_cast<int *>(at(parAt));
+  p.flag = reinterpret_cast<int *>(at(flagAt));
+  p.chartIdx = reinterpret_cast<int *>(at(idxAt));
+  p.part = reinterpret_cast<double *>(at(partAt));
+  p.group = reinterpret_cast<double *>(at(groupAt));
+  p.lambda = lambda;
+  p.cosLim = std::cos(maxViewAngleDeg * pi / 180.0);
+  p.depthTol = depthTol;
+  p.padding = padding;
+  p.craw = reinterpret_cast<int *>(at(crawAt));
+  p.ctab = reinterpret_cast<const int *>(at(ctabAt));
+  p.cstart = reinterpret_cast<const long long *>(at(cstartAt));
+  p.atlas = atlas;
+  p.uv = uv;
+  p.faceView = faceView;
+  p.faceChart = faceChart;
+  p.atlasWidth = atlasWidth;
+  unsigned long long *buf = reinterpret_cast<unsigned long long *>(at(bufAt));
+  void *temp = at(tempAt);
+  TextureResult &R = *static_cast<TextureResult *>(h_res);
+  cudaEvent_t *tev = match_timing_events();
+
+  int status = 0, rounds = 0, sweeps = 0, colours = 0;
+  long long changed = 0, fullRows = 0, rowsWritten = 0;
+  double energy[2] = {0.0, 0.0};
+  std::vector<int> table;
+  auto readback = [&]() -> int {
+    CS_CUDA(cudaMemcpyAsync(h_res, p.res, sizeof(TextureResult), cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  auto total = [&](double &out) -> int {
+    texture_energy_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    texture_total_kernel<<<1, TT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    int r;
+    if ((r = readback()) < 0) return r;
+    out = R.energy;
+    return 0;
+  };
+  auto run = [&]() -> int {
+    int r;
+    if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
+    CS_CUDA(cudaMemsetAsync(p.res, 0, sizeof(TextureResult), st));
+    texture_validate_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    count_launch();
+    CS_CUDA(cudaGetLastError());
+    if ((r = readback()) < 0) return r;
+    if (R.bad) {
+      status = 2;
+      return 0;
+    }
+    texture_edges_kernel<<<grid_of(3ll * T), TT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempBytes, p.ekey, p.ekeyS, p.eval, p.evalS, (int)C3, 0, 64, st));
+    texture_adjacency_kernel<<<grid_of(3ll * T), TT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    CS_CUDA(cudaMemsetAsync(p.cn, 0, (size_t)T * 4, st));
+    if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
+    for (size_t gi = 0; gi + 1 < groupStart.size(); gi++) {
+      const int g0 = groupStart[gi], g1 = groupStart[gi + 1];
+      size_t off = 0;
+      for (int a = g0; a < g1; a++) {
+        cams[a].buf = buf + off;
+        off += (size_t)images[a].width * images[a].height;
+      }
+      CS_CUDA(cudaMemcpyAsync(at(camAt), cams.data(), (size_t)numImages * sizeof(TexCam), cudaMemcpyHostToDevice, st));
+      CS_CUDA(cudaMemsetAsync(buf, 0xff, off * 8, st));
+      p.g0 = g0;
+      p.gn = g1 - g0;
+      texture_raster_kernel<<<grid_of((long long)p.gn * T), TT, 0, st>>>(p);
+      if (tev && gi == 0) CS_CUDA(cudaEventRecord(tev[2], st));
+      texture_candidate_kernel<<<grid_of(T), TT, 0, st>>>(p);
+      count_launch(2);
+      CS_CUDA(cudaGetLastError());
+      // the host table is read by the copy above before the next group changes it
+      CS_CUDA(cudaStreamSynchronize(st));
+    }
+    if (tev) CS_CUDA(cudaEventRecord(tev[3], st));
+    texture_label_init_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    count_launch();
+    CS_CUDA(cudaGetLastError());
+    for (;;) {
+      CS_CUDA(cudaMemsetAsync(&p.res->left, 0, sizeof(unsigned int), st));
+      texture_colour_kernel<<<grid_of(T), TT, 0, st>>>(p);
+      count_launch();
+      CS_CUDA(cudaGetLastError());
+      std::swap(p.colA, p.colB);
+      rounds++;
+      if ((r = readback()) < 0) return r;
+      if (R.left == 0) break;
+    }
+    colours = R.maxColour + 1;
+    if ((r = total(energy[0])) < 0) return r;
+    for (;;) {
+      if (sweeps == maxSweeps) { status = 3; break; }
+      CS_CUDA(cudaMemsetAsync(&p.res->changed, 0, sizeof(unsigned int), st));
+      for (int c = 0; c < colours; c++) texture_icm_kernel<<<grid_of(T), TT, 0, st>>>(p, c);
+      count_launch(colours);
+      CS_CUDA(cudaGetLastError());
+      sweeps++;
+      if ((r = readback()) < 0) return r;
+      changed += R.changed;
+      if (R.changed == 0) { status = 0; break; }
+    }
+    if ((r = total(energy[1])) < 0) return r;
+    if (tev) CS_CUDA(cudaEventRecord(tev[4], st));
+    texture_hook_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    texture_roots_kernel<<<grid_of(T + 1ll), TT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    CS_CUDA(cub::DeviceScan::ExclusiveSum(temp, tempBytes, p.flag, p.chartIdx, T + 1, st));
+    texture_chart_init_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    texture_rect_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if ((r = readback()) < 0) return r;
+    const int C = R.charts;
+    std::vector<int> raw(6 * (size_t)C);
+    if (C) {
+      CS_CUDA(cudaMemcpyAsync(raw.data(), p.craw, raw.size() * 4, cudaMemcpyDeviceToHost, st));
+      CS_CUDA(cudaStreamSynchronize(st));
+    }
+    // the chart table, then the shelves (rule 6)
+    table.assign(8 * (size_t)C, 0);
+    for (int c = 0; c < C; c++) {
+      const int *e = &raw[6 * (size_t)c];
+      int *o = &table[8 * (size_t)c];
+      const cs_image &I = images[e[0]];
+      const int x0 = std::max(0, e[1] - padding), x1 = std::min(I.width - 1, e[3] + padding);
+      const int y0 = std::max(0, e[2] - padding), y1 = std::min(I.height - 1, e[4] + padding);
+      o[0] = e[0];
+      o[1] = x0;
+      o[2] = y0;
+      o[3] = x1 - x0 + 1;
+      o[4] = y1 - y0 + 1;
+      o[7] = e[5];
+    }
+    std::vector<int> order(C);
+    for (int c = 0; c < C; c++) order[c] = c;
+    std::sort(order.begin(), order.end(), [&](int a, int b) {
+      const int *x = &table[8 * (size_t)a], *y = &table[8 * (size_t)b];
+      if (x[4] != y[4]) return x[4] > y[4];
+      if (x[3] != y[3]) return x[3] > y[3];
+      return a < b;
+    });
+    long long shelfY = 0, shelfH = 0, cx = 0;
+    for (int c : order) {
+      int *o = &table[8 * (size_t)c];
+      if (cx + o[3] > atlasWidth) {
+        shelfY += shelfH;
+        shelfH = 0;
+        cx = 0;
+      }
+      o[5] = (int)cx;
+      o[6] = (int)shelfY;
+      cx += o[3];
+      shelfH = std::max(shelfH, (long long)o[4]);
+    }
+    fullRows = shelfY + shelfH;
+    rowsWritten = std::min(fullRows, (long long)maxAtlasRows);
+    std::vector<long long> starts((size_t)C + 1, 0);
+    for (int c = 0; c < C; c++) starts[c + 1] = starts[c] + (long long)table[8 * (size_t)c + 3] * table[8 * (size_t)c + 4];
+    if (C) {
+      CS_CUDA(cudaMemcpyAsync(at(ctabAt), table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
+      CS_CUDA(cudaMemcpyAsync(at(cstartAt), starts.data(), starts.size() * 8, cudaMemcpyHostToDevice, st));
+    }
+    p.numCharts = C;
+    p.rowsWritten = (int)rowsWritten;
+    if (tev) CS_CUDA(cudaEventRecord(tev[5], st));
+    if (rowsWritten) CS_CUDA(cudaMemsetAsync(atlas, 0, (size_t)rowsWritten * atlasWidth * 4, st));
+    texture_uv_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    texture_atlas_kernel<<<grid_of(starts[C]), TT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if (tev) CS_CUDA(cudaEventRecord(tev[6], st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    if (tev) {
+      static const char *const names[6] = {"adjacency", "depth", "candidates", "labelling", "charts", "atlas"};
+      report_stage_times(tev, names, 6, "texture timing faces=%d images=%d groups=%d", T, numImages,
+                         (int)groupStart.size() - 1);
+    }
+    return 0;
+  };
+  const int r = run();
+  cudaFreeAsync(base, st);
+  if (r < 0) return r;
+  const bool out = status != 2;
+  const int C = out ? R.charts : 0;
+  for (int c = 0; c < std::min(C, maxCharts); c++)
+    std::memcpy(chartsOut + 8 * (size_t)c, &table[8 * (size_t)c], 8 * sizeof(int));
+  if (info) {
+    info[0] = out ? energy[0] : 0.0;
+    info[1] = out ? energy[1] : 0.0;
+  }
+  if (stats) {
+    stats[0] = T;
+    stats[1] = out ? R.unseen : 0;
+    stats[2] = out ? R.cand : 0;
+    stats[3] = out ? colours : 0;
+    stats[4] = rounds;
+    stats[5] = sweeps;
+    stats[6] = changed;
+    stats[7] = C;
+    stats[8] = fullRows;
+    stats[9] = rowsWritten;
+    stats[10] = status;
+  }
+  return C;
+}
+
+size_t texture_result_bytes() { return sizeof(TextureResult); }
+
+}  // namespace cs

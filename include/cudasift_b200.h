@@ -37,7 +37,8 @@ unsigned long long cs_launch_count(void);
  * created afterwards, 0 = the batched TMA pipeline), "cap32" (0 = do not reproduce the reference's cap of 32
  * extrema per 30x8 block and scale, cudaSiftD.cu:1371), "d2_hs" / "pa_rows" (rows per detector stream / per CTA
  * of the first pyramid kernel, 0 = automatic), "sd_split" (0 = every ScaleDown of a batch in the chain kernel),
- * "cap32_limit" (the cap's limit, 1..199; default 32).  Returns 0, or CS_E_ARG for an unknown key. */
+ * "cap32_limit" (the cap's limit, 1..199; default 32), "texture_group_bytes" (the depth-buffer bytes of one image
+ * group of cs_texture_mesh, <= 0: 1 GiB).  Returns 0, or CS_E_ARG for an unknown key. */
 int cs_set_tuning(const char *key, int value);
 /* Number of launches one steady-state cs_extractor_submit_* / cs_match issues. */
 int cs_extract_launches_per_image(int numOctaves, int scaleUp);
@@ -1311,6 +1312,91 @@ int cs_simplify_mesh(const float *d_vertices, const float *d_vertexIntensity, in
                      int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
                      float *d_outVertices, float *d_outIntensity, int maxOutVertices, int *d_outTriangles,
                      int maxOutTriangles, double info_out[1], long long stats_out[9], double *ms);
+
+/* Mesh texturing (Waechter, Moehrle & Goesele, "Let There Be Color!", ECCV 2014, without global seam levelling): for
+ * every face one image to take its texture from, the charts of adjacent faces with the same image, and one atlas of
+ * the charts' image rectangles with per-corner texture coordinates.  Images and cameras are the dense calls' (pinhole:
+ * images with distortion go through cs_undistort_images first); the mesh is in the layout cs_poisson_mesh and
+ * cs_simplify_mesh write, device buffers passed in place: d_vertices [numVertices][3] float, d_triangles
+ * [numTriangles][3] int32.  All arithmetic below is float64, each operation rounded once in the order written (no
+ * contraction); the rules depend on values alone, so two calls give the same bytes.
+ * 1. Input and adjacency: status 2 and nothing written when a triangle index lies outside [0, numVertices), a triangle
+ *    repeats a vertex, or a vertex some triangle uses has a non-finite coordinate (cs_simplify_mesh's rule 1).  Corner
+ *    3t + k starts the edge from corner k to corner k + 1 mod 3.  Two faces are adjacent across an undirected edge when
+ *    exactly two faces hold it (found by a radix sort of the keys (min << 32) | max of the corners' edges); an edge with
+ *    one face or with three or more gives no adjacency, so a face has at most 3 neighbours.
+ * 2. Depth buffers: image a maps a vertex X (float, as float64) to Y = R_a X + t_a, component i
+ *    ((R_i0 X_0 + R_i1 X_1) + R_i2 X_2) + t_i, and (u, v) = (((K_0 Y_0 + K_1 Y_1) + K_2 Y_2) / Y_2,
+ *    ((K_3 Y_0 + K_4 Y_1) + K_5 Y_2) / Y_2); pixel (x, y) has its centre at integer (x, y).  Every face whose three
+ *    vertices have Y_z > 0 is rasterised, front-facing or not, so back faces of open meshes occlude.  With the doubled
+ *    area A = (u_1 - u_0)(v_2 - v_0) - (v_1 - v_0)(u_2 - u_0) (corners in face order; A = 0 or not finite: no pixel) and
+ *    s = sign(A): edge k from vertex P to vertex Q, P the corner of the lower vertex index, has
+ *    e_k = (u_Q - u_P)(y - v_P) - (v_Q - v_P)(x - u_P), and w_k = s e_k, negated when corner k holds the higher index,
+ *    so the two faces of an edge see exactly opposite values and no pixel centre on a shared edge is missed.  A pixel in
+ *    [0, W - 1] x [0, H - 1] is covered when w_0, w_1, w_2 >= 0 and S = (w_0 + w_1) + w_2 > 0; its depth is
+ *    float(1 / (((w_1 / z_0 + w_2 / z_1) + w_0 / z_2) / S)) (perspective-correct, rounded to float once).  The pixel's
+ *    key (float bits << 32) | face is combined by 64-bit atomicMin (empty: all ones), so the nearest surface wins, ties
+ *    go to the lower face, and the order of execution does not matter.  Images are processed in groups of consecutive
+ *    images whose buffers (8 bytes per pixel) fit 1 GiB (at least one image each); the result does not depend on the
+ *    grouping.
+ * 3. Candidates: with n_f = (p_1 - p_0) x (p_2 - p_0) (cs_simplify_mesh's products), the centroid
+ *    c = ((p_0 + p_1) + p_2) / 3, C_a = -R_a^T t_a (component i -((R_0i t_0 + R_1i t_1) + R_2i t_2)) and d = C_a - c,
+ *    image a is a candidate of face f when n_f . d > 0; n_f . d >= cos(maxViewAngleDeg pi / 180) (sqrt(n.n) sqrt(d.d))
+ *    (the cosine by the host's libm); p_0, p_1, p_2 and c project with Y_z > 0 into [0, W - 1] x [0, H - 1]; at each
+ *    of those 4 points the buffer at pixel (floor(u + 0.5), floor(v + 0.5)) is empty, holds f, or has a depth d with
+ *    Y_z <= d (1 + depthTol); and the quality q(f, a) = 0.5 |A| (the projected area in pixels) is > 0.  A face keeps
+ *    its best 8 candidates by (q descending, image ascending), a set that does not depend on the groups.  A face
+ *    without a candidate is unseen: label -1, NaN texture coordinates, in no chart.
+ * 4. Labelling: D(f, a) = 1 - q(f, a) / q(f, best), E = sum_f e_f with e_f = D(f, l_f) + lambda times the number of
+ *    f's edges whose neighbour g > f is labelled with l_g != l_f (each adjacent pair counted once per shared edge).
+ *    Every seen face starts at its best candidate.  The face graph is coloured by Jones-Plassmann with the priority
+ *    s(f) = m ^ (m >> 16), m = f 0x9E3779B1 mod 2^32 (cs_simplify_mesh's bijection): in a round, which reads the state
+ *    at its start, an uncoloured face whose priority is above every uncoloured neighbour's takes the smallest colour
+ *    no coloured neighbour holds (unseen faces take part; at most 4 colours).  A sweep updates the faces of colour 0,
+ *    then 1, and so on (ICM, iterated conditional modes: a seen face takes the candidate of lowest local energy
+ *    D(f, a) + lambda #{labelled neighbours across an edge with a label != a}, keeping its label on ties, then
+ *    preferring the earlier rank).  The call stops after a sweep that changes nothing (status 0) or after maxSweeps
+ *    sweeps (status 3).  E never increases; info_out [2] (may be NULL) gets E before and after the sweeps, each summed
+ *    in coop.cuh's three-level order (tiles of 2048 faces, groups of 256 tiles, the group partials).
+ * 5. Charts: the connected components of adjacent seen faces with equal labels (union-find, each link from the higher
+ *    root to the lower, so every root is the lowest face of its chart), ordered by that face.  A chart's rectangle in
+ *    its image is x0 = max(0, min floor(u) - padding), x1 = min(W - 1, max ceil(u) + padding) over its faces' corners,
+ *    likewise y0, y1 (integer atomics on floor and ceil).
+ * 6. Atlas, packed on the host over one copy of the chart table: the charts sorted by (height descending, width
+ *    descending, index ascending) go into shelves left to right, a new shelf starting under the current one when the
+ *    next chart does not fit in atlasWidth texels; the full atlas height is the sum of the shelf heights, and chart c
+ *    lies at (ox, oy).  Its texel (X, Y) is an exact copy of image_a(x0 + X - ox, y0 + Y - oy) (one texel per pixel:
+ *    no resampling, and the padding is real image data for bilinear filtering and mipmaps); texels outside every
+ *    chart are 0.  A corner's coordinate is (float((u - x0) + ox), float((v - y0) + oy)) in atlas pixels.
+ * - Outputs: d_atlas [maxAtlasRows][atlasWidth] float (the prefix of the full atlas's rows); d_uv [numTriangles][3][2]
+ *   float, d_faceView [numTriangles] int32 (the label) and d_faceChart [numTriangles] (may be NULL; -1 when unseen),
+ *   which always refer to the full atlas; charts_out [maxCharts][8] (host int32) {image, x0, y0, width, height, ox, oy,
+ *   faces}, the prefix of the chart list.  stats_out [11] (may be NULL): faces, unseen faces, candidate pairs (before
+ *   the cap of 8), colours, Jones-Plassmann rounds, sweeps, labels changed, charts, atlas rows (full), atlas rows
+ *   written, status.  Returns the full chart count, or CS_E_*.  numTriangles == 0 returns 0 (stats and info zero) and
+ *   makes no CUDA call.
+ * - Launches (cs_launch_count): 14 + 2 G + rounds + colours x sweeps for G image groups (validate; edge keys,
+ *   adjacency; per group raster and candidates; label start; one per colouring round; two per energy total; per sweep
+ *   one per colour; union, roots, chart start, rectangles; texture coordinates, texel copy), 1 when the input is
+ *   invalid; plus cub's sort and scan (not counted).  The host reads a few words after the input check, each group,
+ *   each colouring round, each total and each sweep, and the chart table (one synchronise each); *ms (may be NULL)
+ *   gets the event time of the whole call.
+ * - Scratch, allocated on the call's stream and freed before it returns: 272 bytes per face (edge keys and corners and
+ *   their sorted copies, neighbours, 8 candidates, labels, two colour arrays, parents, root flags, chart indices, chart
+ *   rectangles, the chart table and texel starts), 8 per group of 2048 faces, 8 bytes per pixel of the largest image
+ *   group (at most 1 GiB unless one image is larger), 224 per image, plus cub's storage.
+ * - CS_E_ARG, before any CUDA call, naming the argument: the dense calls' image and camera checks; numVertices outside
+ *   [0, 2^30], numTriangles outside [0, 2^29]; lambda not finite or < 0; maxViewAngleDeg not in (0, 90]; depthTol not
+ *   in [0, 1]; padding outside [0, 16]; atlasWidth outside [the largest image width, 32768]; maxSweeps outside
+ *   [0, 1000]; maxAtlasRows or maxCharts < 0; NULL or not 4-byte aligned d_vertices with numVertices > 0, d_triangles,
+ *   d_uv or d_faceView with numTriangles > 0, d_atlas with maxAtlasRows > 0; a misaligned d_faceChart; NULL charts_out
+ *   with maxCharts > 0; and an output (d_atlas, d_uv, d_faceView, d_faceChart) that overlaps another output, the mesh
+ *   or an image (one sweep over sorted ranges). */
+int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                    const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles, double lambda,
+                    double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                    float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
+                    int *charts_out, int maxCharts, double info_out[2], long long stats_out[11], double *ms);
 
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
