@@ -501,6 +501,40 @@ __device__ __forceinline__ int table_find(const T *__restrict__ a, int n, int T:
   return lo;
 }
 
+// ---- union-find (tracks.cu, texture.cu) -------------------------------------------------------------------------
+// Trees of parent links that keep parent[x] <= x for every x, so each root is the smallest id of its tree whatever the
+// order of the threads (DESIGN.md, "Feature tracks", gives the argument).
+//
+// The root of x with path halving.  Every store writes an ancestor, so parent[x] <= x keeps holding; a store racing
+// with another thread's can only leave a different ancestor.
+__device__ __forceinline__ int uf_find(int *parent, int x)
+{
+  volatile int *p = parent;
+  int cur = p[x];
+  if (cur != x) {
+    int prev = x, next;
+    while (cur > (next = p[cur])) {
+      p[prev] = next;
+      prev = cur;
+      cur = next;
+    }
+  }
+  return cur;
+}
+
+// Joins the trees of u and v (ECL-CC's hook): atomicCAS of the larger root onto the smaller; when the CAS fails, the
+// larger root has been hooked meanwhile and the walk continues from the root of the value it read.
+__device__ __forceinline__ void uf_link(int *parent, int u, int v)
+{
+  int ru = uf_find(parent, u), rv = uf_find(parent, v);
+  while (ru != rv) {
+    const int hi = ru > rv ? ru : rv, lo = ru > rv ? rv : ru;
+    const int old = atomicCAS(parent + hi, hi, lo);
+    if (old == hi) break;
+    if (hi == ru) ru = uf_find(parent, old); else rv = uf_find(parent, old);
+  }
+}
+
 // One pair list of the flags / write kernels (match_mutual.cu; an ordered list of ordered_list.cuh): the keep test of
 // rows [0, n1) of set 1, then pairs {i, jv[i * jstride]} at positions < maxPairs and the total.  A single call passes
 // one by value; a batch passes a table in device memory, job k owning the CTAs from cta0 on.

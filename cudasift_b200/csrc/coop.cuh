@@ -1,9 +1,9 @@
 // coop.cuh -- the fixed-order machinery of a cooperative solver: bundle adjustment (bundle.cu), rotation averaging
-// (rotavg.cu) and global positioning (globalpos.cu) over a sorted incidence list, and the MGPCG solves of Poisson
-// meshing (mesh.cu, the three-level totals only).  The first three sort their incidences (observation or edge end) by
-// item (camera or image) with a stable radix sort; each solver runs one cooperative kernel whose phases are separated
-// by grid barriers.  Every floating-point sum has a fixed order that depends on the data only, not on the grid or on
-// scheduling:
+// (rotavg.cu) and global positioning (globalpos.cu) over a sorted incidence list; the MGPCG solves of Poisson meshing
+// (mesh.cu) and the energy totals of mesh texturing (texture.cu) take the three-level totals only.  The first three
+// sort their incidences (observation or edge end) by item (camera or image) with a stable radix sort; each solver runs
+// one cooperative kernel whose phases are separated by grid barriers.  Every floating-point sum has a fixed order that
+// depends on the data only, not on the grid or on scheduling:
 //   - per item: the sorted incidences are cut into tiles of CO_TILE; a warp sums an item's piece of a tile
 //     lane-strided, then by a fixed xor butterfly, and one lane per item adds its pieces in ascending tile order;
 //   - totals: a CTA sums a tile of its threads' values by butterflies and its warps in order, or a warp sums a tile of

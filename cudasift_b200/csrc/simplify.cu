@@ -2,8 +2,9 @@
 // adjacency by a stable sort of corner keys, one thread per edge for the validity tests, position and cost, a radix
 // sort of the candidate keys for the gating threshold, an atomicMin scatter of keys onto the closed 1-rings of both
 // ends and the selection test, the collapse, and the face remap as count-scan-write passes (the faces and the output
-// vertices are counted lists of counted_list.cuh).  Every rule is stated in cudasift_b200.h at cs_simplify_mesh;
-// tests/simplify_oracle.py restates them in float64.
+// vertices are counted lists of counted_list.cuh).  The float64 vectors, the tie order s(id), the input check and the
+// launch shape are shared with texture.cu in trimesh.cuh.  Every rule is stated in cudasift_b200.h at
+// cs_simplify_mesh; tests/simplify_oracle.py restates them in float64.
 //
 // Determinism: no floating-point atomics; integer atomics only where the result does not depend on their order (counts,
 // the minimum key of a vertex, the largest applied error as ordered bits).  This unit is compiled with -fmad=false so
@@ -17,12 +18,12 @@
 
 #include "common.cuh"
 #include "counted_list.cuh"
+#include "trimesh.cuh"
 
 namespace cs {
 
 namespace {
 
-constexpr int ST = 256;                       // threads per CTA of every simplify kernel
 constexpr int F_SHIFT = 1;                    // f = 1/2: the cheapest ceil(C / 2) candidates compete in a pass
 constexpr double DET_EPS = 1e-6;              // the minimiser is used when det(A) > DET_EPS a11 a22 a33
 constexpr int MAX_PASSES = 1000;
@@ -60,21 +61,6 @@ struct SimplifyParams {
   int *outT;
   int maxOutV, maxOutT;
 };
-
-struct D3 {
-  double x, y, z;
-};
-__device__ __forceinline__ D3 sub3(D3 a, D3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
-__device__ __forceinline__ D3 cross3(D3 a, D3 b)
-{
-  return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
-}
-__device__ __forceinline__ double dot3(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ D3 normal3(D3 p0, D3 p1, D3 p2) { return cross3(sub3(p1, p0), sub3(p2, p0)); }
-__device__ __forceinline__ D3 pos_of(const SimplifyParams &p, int v)
-{
-  return {p.pos[3 * (size_t)v], p.pos[3 * (size_t)v + 1], p.pos[3 * (size_t)v + 2]};
-}
 
 // q += w p p^T for the plane (n, d): the upper triangle row-major, each entry w (p_i p_j)
 __device__ void plane_add(double *q, D3 n, double d, double w)
@@ -196,7 +182,7 @@ __device__ bool evaluate(const SimplifyParams &p, int t, int k, int &u, int &v, 
   double q[10];
   for (int i = 0; i < 10; i++) q[i] = p.Q[10 * (size_t)u + i] + p.Q[10 * (size_t)v + i];
   const double area = p.A[u] + p.A[v];
-  const D3 pu = pos_of(p, u), pv = pos_of(p, v);
+  const D3 pu = vertex_of(p.pos, u), pv = vertex_of(p.pos, v);
   const double cst = optimum(q, pu, pv, x);
   err = area > 0.0 ? cst / area : (cst == 0.0 ? 0.0 : CUDART_INF);
   if (!(err < CUDART_INF && sqrt(err) <= p.maxError)) return false;
@@ -206,7 +192,7 @@ __device__ bool evaluate(const SimplifyParams &p, int t, int k, int &u, int &v, 
     const int g0 = corner(p, s, 0), g1 = corner(p, s, 1), g2 = corner(p, s, 2);
     const bool hu = g0 == uu || g1 == uu || g2 == uu, hv = g0 == vv || g1 == vv || g2 == vv;
     if (hu && hv) return false;
-    const D3 p0 = pos_of(p, g0), p1 = pos_of(p, g1), p2 = pos_of(p, g2);
+    const D3 p0 = vertex_of(p.pos, g0), p1 = vertex_of(p.pos, g1), p2 = vertex_of(p.pos, g2);
     const D3 n0 = normal3(p0, p1, p2);
     if (!(dot3(n0, n0) > 0.0)) return false;
     auto moved = [&](int g, D3 q0) { return (g == uu || g == vv) ? xx : q0; };
@@ -218,23 +204,10 @@ __device__ bool evaluate(const SimplifyParams &p, int t, int k, int &u, int &v, 
 }
 
 // ---- setup ------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(ST) simplify_validate_kernel(SimplifyParams p)
-{
-  for (int t = blockIdx.x * ST + threadIdx.x; t < p.T; t += gridDim.x * ST) {
-    const int a = p.tin[3 * (size_t)t], b = p.tin[3 * (size_t)t + 1], c = p.tin[3 * (size_t)t + 2];
-    bool bad = a < 0 || a >= p.V || b < 0 || b >= p.V || c < 0 || c >= p.V || a == b || b == c || a == c;
-    for (int j = 0; j < 3 && !bad; j++) {
-      const int w = p.tin[3 * (size_t)t + j];
-      for (int d = 0; d < 3; d++) bad = bad || !isfinite(p.vin[3 * (size_t)w + d]);
-    }
-    if (bad) atomicOr(&p.res->bad, 1u);
-  }
-}
-
-__global__ void __launch_bounds__(ST) simplify_init_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_init_kernel(SimplifyParams p)
 {
   const int n = max(p.V, p.T);
-  for (int i = blockIdx.x * ST + threadIdx.x; i < n; i += gridDim.x * ST) {
+  for (int i = blockIdx.x * MT + threadIdx.x; i < n; i += gridDim.x * MT) {
     if (i < p.V) {
       for (int d = 0; d < 3; d++) p.pos[3 * (size_t)i + d] = (double)p.vin[3 * (size_t)i + d];
       if (p.inten) p.inten[i] = p.iin[i];
@@ -248,9 +221,9 @@ __global__ void __launch_bounds__(ST) simplify_init_kernel(SimplifyParams p)
 }
 
 // corner keys and the faces per vertex (cub's stable radix sort then orders each vertex's faces by index)
-__global__ void __launch_bounds__(ST) simplify_corners_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_corners_kernel(SimplifyParams p)
 {
-  for (int c = blockIdx.x * ST + threadIdx.x; c < 3 * p.T; c += gridDim.x * ST) {
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
     const int x = p.tri[c];
     p.ckey[c] = x;
     p.cval[c] = c;
@@ -259,9 +232,9 @@ __global__ void __launch_bounds__(ST) simplify_corners_kernel(SimplifyParams p)
 }
 
 // frozen status and the quadric of every vertex with faces (rules 1 and 2)
-__global__ void __launch_bounds__(ST) simplify_vertex_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_vertex_kernel(SimplifyParams p)
 {
-  const int x = blockIdx.x * ST + threadIdx.x;
+  const int x = blockIdx.x * MT + threadIdx.x;
   if (x >= p.V) return;
   const int s0 = p.vstart[x], k = p.vstart[x + 1] - s0;
   double *q = p.Q + 10 * (size_t)x;
@@ -309,7 +282,8 @@ __global__ void __launch_bounds__(ST) simplify_vertex_kernel(SimplifyParams p)
   for (int pass = 0; pass < 2; pass++)
     for (int i = 0; i < k; i++) {
       const int t = face(i);
-      const D3 p0 = pos_of(p, corner(p, t, 0)), p1 = pos_of(p, corner(p, t, 1)), p2 = pos_of(p, corner(p, t, 2));
+      const D3 p0 = vertex_of(p.pos, corner(p, t, 0)), p1 = vertex_of(p.pos, corner(p, t, 1)),
+               p2 = vertex_of(p.pos, corner(p, t, 2));
       const D3 n = normal3(p0, p1, p2);
       const double ln = sqrt(dot3(n, n));
       if (!(ln > 0.0)) continue;
@@ -323,7 +297,7 @@ __global__ void __launch_bounds__(ST) simplify_vertex_kernel(SimplifyParams p)
       for (int e = 0; e < 3; e++) {
         const int a = corner(p, t, e), b = corner(p, t, e + 1);
         if ((a != x && b != x) || has_directed(p, x, b, a)) continue;
-        const D3 pa = pos_of(p, a), ev = sub3(pos_of(p, b), pa);
+        const D3 pa = vertex_of(p.pos, a), ev = sub3(vertex_of(p.pos, b), pa);
         const D3 m = cross3(ev, un);
         const double lm = sqrt(dot3(m, m));
         if (!(lm > 0.0)) continue;
@@ -335,18 +309,10 @@ __global__ void __launch_bounds__(ST) simplify_vertex_kernel(SimplifyParams p)
 }
 
 // ---- a pass -----------------------------------------------------------------------------------------------------------
-// The tie order s(id) of rule 5: a bijection of the 32-bit ids (an odd multiplier mod 2^32, then an invertible
-// xorshift), so keys stay unique while equal errors are not ranked in raster order.
-__device__ __forceinline__ unsigned int tie_of(unsigned int id)
-{
-  const unsigned int m = id * 0x9E3779B1u;
-  return m ^ (m >> 16);
-}
-
-__global__ void __launch_bounds__(ST) simplify_candidate_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_candidate_kernel(SimplifyParams p)
 {
   unsigned int n = 0;
-  for (int c = blockIdx.x * ST + threadIdx.x; c < 3 * p.T; c += gridDim.x * ST) {
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
     const int t = c / 3, k = c - 3 * t;
     int u, v, drops = 0;
     D3 x;
@@ -382,21 +348,21 @@ __device__ __forceinline__ void closed_rings(const SimplifyParams &p, int c, F &
     });
 }
 
-__global__ void __launch_bounds__(ST) simplify_scatter_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_scatter_kernel(SimplifyParams p)
 {
   const unsigned long long thr = p.res->thr;
-  for (int c = blockIdx.x * ST + threadIdx.x; c < 3 * p.T; c += gridDim.x * ST) {
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
     const unsigned long long key = p.key[c];
     if (key == NO_KEY || key > thr) continue;
     closed_rings(p, c, [&](int w) { atomicMin(&p.mark[w], key); });
   }
 }
 
-__global__ void __launch_bounds__(ST) simplify_select_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_select_kernel(SimplifyParams p)
 {
   const unsigned long long thr = p.res->thr;
   unsigned int ns = 0, nd = 0;
-  for (int c = blockIdx.x * ST + threadIdx.x; c < 3 * p.T; c += gridDim.x * ST) {
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
     const unsigned long long key = p.key[c];
     bool sel = key != NO_KEY && key <= thr;
     if (sel) closed_rings(p, c, [&](int w) { sel = sel && p.mark[w] == key; });
@@ -412,20 +378,20 @@ __global__ void __launch_bounds__(ST) simplify_select_kernel(SimplifyParams p)
 }
 
 // the target pass: the selected edges by key, their faces summed; the last applied is where the sum reaches need
-__global__ void __launch_bounds__(ST) simplify_cut_kernel(SimplifyParams p, int need)
+__global__ void __launch_bounds__(MT) simplify_cut_kernel(SimplifyParams p, int need)
 {
   const int S = (int)p.res->sel;
-  for (int i = blockIdx.x * ST + threadIdx.x; i < S; i += gridDim.x * ST)
+  for (int i = blockIdx.x * MT + threadIdx.x; i < S; i += gridDim.x * MT)
     if (p.cum[i] >= need && (i == 0 || p.cum[i - 1] < need)) {
       p.res->cut = p.selKeyS[i];
       p.res->applied = i + 1;
     }
 }
 
-__global__ void __launch_bounds__(ST) simplify_collapse_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_collapse_kernel(SimplifyParams p)
 {
   const unsigned long long cut = p.res->cut;
-  for (int c = blockIdx.x * ST + threadIdx.x; c < 3 * p.T; c += gridDim.x * ST) {
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
     const unsigned long long key = p.selKey[c];
     if (key == NO_KEY || key > cut) continue;
     const int t = c / 3, k = c - 3 * t;
@@ -433,7 +399,7 @@ __global__ void __launch_bounds__(ST) simplify_collapse_kernel(SimplifyParams p)
     D3 x;
     double err;
     if (!evaluate(p, t, k, u, v, x, err, drops)) continue;   // cannot happen: the state it read is unchanged
-    const D3 pu = pos_of(p, u), pv = pos_of(p, v);
+    const D3 pu = vertex_of(p.pos, u), pv = vertex_of(p.pos, v);
     if (p.inten) {
       const D3 d = sub3(pv, pu);
       const double den = dot3(d, d);
@@ -458,19 +424,19 @@ __device__ __forceinline__ bool kept_face(const SimplifyParams &p, int t, int *g
   return g[0] != g[1] && g[1] != g[2] && g[0] != g[2];
 }
 
-__global__ void __launch_bounds__(ST) simplify_face_count_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_face_count_kernel(SimplifyParams p)
 {
-  const int t = blockIdx.x * ST + threadIdx.x;
+  const int t = blockIdx.x * MT + threadIdx.x;
   int g[3];
-  counted_cta_count<ST>(t < p.T && kept_face(p, t, g) ? 1 : 0, p.blockCounts + blockIdx.x);
+  counted_cta_count<MT>(t < p.T && kept_face(p, t, g) ? 1 : 0, p.blockCounts + blockIdx.x);
 }
 
-__global__ void __launch_bounds__(ST) simplify_face_write_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_face_write_kernel(SimplifyParams p)
 {
-  const int t = blockIdx.x * ST + threadIdx.x;
+  const int t = blockIdx.x * MT + threadIdx.x;
   int g[3];
   const bool keep = t < p.T && kept_face(p, t, g);
-  const int at = p.blockOffsets[blockIdx.x] + counted_position<ST>(keep ? 1 : 0);
+  const int at = p.blockOffsets[blockIdx.x] + counted_position<MT>(keep ? 1 : 0);
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0)
     p.res->tris = counted_total(p.blockOffsets, p.blockCounts, gridDim.x - 1);
   if (!keep) return;
@@ -479,23 +445,23 @@ __global__ void __launch_bounds__(ST) simplify_face_write_kernel(SimplifyParams 
 }
 
 // ---- output -----------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(ST) simplify_used_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_used_kernel(SimplifyParams p)
 {
-  for (int c = blockIdx.x * ST + threadIdx.x; c < 3 * p.T; c += gridDim.x * ST) p.used[p.tri[c]] = 1;
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) p.used[p.tri[c]] = 1;
 }
 
-__global__ void __launch_bounds__(ST) simplify_vcount_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_vcount_kernel(SimplifyParams p)
 {
-  const int x = blockIdx.x * ST + threadIdx.x;
-  counted_cta_count<ST>(x < p.V ? p.used[x] : 0, p.blockCounts + blockIdx.x);
+  const int x = blockIdx.x * MT + threadIdx.x;
+  counted_cta_count<MT>(x < p.V ? p.used[x] : 0, p.blockCounts + blockIdx.x);
 }
 
 // the used vertices in ascending input index; used[] becomes the output index
-__global__ void __launch_bounds__(ST) simplify_vwrite_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_vwrite_kernel(SimplifyParams p)
 {
-  const int x = blockIdx.x * ST + threadIdx.x;
+  const int x = blockIdx.x * MT + threadIdx.x;
   const int u = x < p.V ? p.used[x] : 0;
-  const int at = p.blockOffsets[blockIdx.x] + counted_position<ST>(u);
+  const int at = p.blockOffsets[blockIdx.x] + counted_position<MT>(u);
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0)
     p.res->verts = counted_total(p.blockOffsets, p.blockCounts, gridDim.x - 1);
   if (!u) return;
@@ -505,14 +471,12 @@ __global__ void __launch_bounds__(ST) simplify_vwrite_kernel(SimplifyParams p)
   if (p.outI) p.outI[at] = p.inten[x];
 }
 
-__global__ void __launch_bounds__(ST) simplify_twrite_kernel(SimplifyParams p)
+__global__ void __launch_bounds__(MT) simplify_twrite_kernel(SimplifyParams p)
 {
-  const int t = blockIdx.x * ST + threadIdx.x;
+  const int t = blockIdx.x * MT + threadIdx.x;
   if (t >= p.T || t >= p.maxOutT) return;
   for (int j = 0; j < 3; j++) p.outT[3 * (size_t)t + j] = p.used[p.tri[3 * (size_t)t + j]];
 }
-
-int grid_of(long long n) { return (int)std::max(1ll, std::min((n + ST - 1) / ST, 8192ll)); }
 
 }  // namespace
 
@@ -521,7 +485,7 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
                  void *h_res, double *info, long long *stats)
 {
   const size_t C3 = 3 * (size_t)T0;
-  const int nbT = idivup(std::max(T0, 1), ST), nbV = idivup(std::max(V, 1), ST);
+  const int nbT = idivup(std::max(T0, 1), MT), nbV = idivup(std::max(V, 1), MT);
   const int vbits = radix_bits(std::max(V, 1));
   size_t tb[7] = {};
   CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (int *)nullptr, (int *)nullptr, (int *)nullptr,
@@ -609,7 +573,7 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
   };
   auto adjacency = [&]() -> int {
     CS_CUDA(cudaMemsetAsync(p.vcount, 0, ((size_t)V + 1) * 4, st));
-    simplify_corners_kernel<<<grid_of(3ll * p.T), ST, 0, st>>>(p);
+    simplify_corners_kernel<<<grid_of(3ll * p.T), MT, 0, st>>>(p);
     count_launch();
     CS_CUDA(cudaGetLastError());
     CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempBytes, p.ckey, p.ckeyS, p.cval, p.cvalS, 3 * p.T, 0, vbits, st));
@@ -620,7 +584,7 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
     int r;
     if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
     CS_CUDA(cudaMemsetAsync(p.res, 0, sizeof(SimplifyResult), st));
-    simplify_validate_kernel<<<grid_of(T0), ST, 0, st>>>(p);
+    mesh_validate_kernel<<<grid_of(T0), MT, 0, st>>>(vin, V, tin, T0, &p.res->bad);
     count_launch();
     CS_CUDA(cudaGetLastError());
     if ((r = readback()) < 0) return r;
@@ -628,11 +592,11 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
       status = 2;
       return 0;
     }
-    simplify_init_kernel<<<grid_of(std::max(V, T0)), ST, 0, st>>>(p);
+    simplify_init_kernel<<<grid_of(std::max(V, T0)), MT, 0, st>>>(p);
     count_launch();
     CS_CUDA(cudaGetLastError());
     if ((r = adjacency()) < 0) return r;
-    simplify_vertex_kernel<<<nbV, ST, 0, st>>>(p);
+    simplify_vertex_kernel<<<nbV, MT, 0, st>>>(p);
     count_launch();
     CS_CUDA(cudaGetLastError());
     if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
@@ -643,11 +607,11 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
       CS_CUDA(cudaMemsetAsync(&p.res->cand, 0, 3 * sizeof(unsigned int), st));
       CS_CUDA(cudaMemsetAsync(&p.res->cut, 0xff, sizeof(unsigned long long), st));
       CS_CUDA(cudaMemsetAsync(p.mark, 0xff, (size_t)V * 8, st));
-      simplify_candidate_kernel<<<grid_of(C), ST, 0, st>>>(p);
+      simplify_candidate_kernel<<<grid_of(C), MT, 0, st>>>(p);
       CS_CUDA(cub::DeviceRadixSort::SortKeys(temp, tempBytes, p.key, p.keyS, (int)C, 0, 64, st));
       simplify_threshold_kernel<<<1, 1, 0, st>>>(p);
-      simplify_scatter_kernel<<<grid_of(C), ST, 0, st>>>(p);
-      simplify_select_kernel<<<grid_of(C), ST, 0, st>>>(p);
+      simplify_scatter_kernel<<<grid_of(C), MT, 0, st>>>(p);
+      simplify_select_kernel<<<grid_of(C), MT, 0, st>>>(p);
       count_launch(4);
       CS_CUDA(cudaGetLastError());
       if ((r = readback()) < 0) return r;
@@ -658,18 +622,18 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
         CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempBytes, p.selKey, p.selKeyS, p.drops, p.dropsS, (int)C, 0,
                                                 64, st));
         CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempBytes, p.dropsS, p.cum, (int)R.sel, st));
-        simplify_cut_kernel<<<grid_of(R.sel), ST, 0, st>>>(p, need);
+        simplify_cut_kernel<<<grid_of(R.sel), MT, 0, st>>>(p, need);
         count_launch();
         CS_CUDA(cudaGetLastError());
         last = true;
       }
-      simplify_collapse_kernel<<<grid_of(C), ST, 0, st>>>(p);
-      const int nb = idivup(p.T, ST);
-      simplify_face_count_kernel<<<nb, ST, 0, st>>>(p);
+      simplify_collapse_kernel<<<grid_of(C), MT, 0, st>>>(p);
+      const int nb = idivup(p.T, MT);
+      simplify_face_count_kernel<<<nb, MT, 0, st>>>(p);
       count_launch(2);
       CS_CUDA(cudaGetLastError());
       CS_CUDA(cub::DeviceScan::ExclusiveSum(temp, tempBytes, p.blockCounts, p.blockOffsets, nb, st));
-      simplify_face_write_kernel<<<nb, ST, 0, st>>>(p);
+      simplify_face_write_kernel<<<nb, MT, 0, st>>>(p);
       count_launch();
       CS_CUDA(cudaGetLastError());
       std::swap(p.tri, p.triN);
@@ -687,13 +651,13 @@ int simplify_run(const float *vin, const float *iin, int V, const int *tin, int 
     }
     if (tev) CS_CUDA(cudaEventRecord(tev[2], st));
     CS_CUDA(cudaMemsetAsync(p.used, 0, (size_t)V * 4, st));
-    simplify_used_kernel<<<grid_of(3ll * p.T), ST, 0, st>>>(p);
-    simplify_vcount_kernel<<<nbV, ST, 0, st>>>(p);
+    simplify_used_kernel<<<grid_of(3ll * p.T), MT, 0, st>>>(p);
+    simplify_vcount_kernel<<<nbV, MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     CS_CUDA(cub::DeviceScan::ExclusiveSum(temp, tempBytes, p.blockCounts, p.blockOffsets, nbV, st));
-    simplify_vwrite_kernel<<<nbV, ST, 0, st>>>(p);
-    simplify_twrite_kernel<<<idivup(std::max(p.T, 1), ST), ST, 0, st>>>(p);
+    simplify_vwrite_kernel<<<nbV, MT, 0, st>>>(p);
+    simplify_twrite_kernel<<<idivup(std::max(p.T, 1), MT), MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     if ((r = readback()) < 0) return r;

@@ -2,7 +2,9 @@
 // face adjacency by a radix sort of undirected edge keys, a depth buffer per image by 64-bit atomicMin of (depth, face)
 // keys, one thread per face for the visibility tests and its best candidates, a Jones-Plassmann colouring of the face
 // graph, ICM sweeps over the colours, charts by union-find, the shelf packing on the host, and the texel copy.  Every
-// rule is stated in cudasift_b200.h at cs_texture_mesh; tests/texture_oracle.py restates them in float64.
+// rule is stated in cudasift_b200.h at cs_texture_mesh; tests/texture_oracle.py restates them in float64.  The float64
+// vectors, the colouring priority s(f), the input check and the launch shape are shared with simplify.cu in
+// trimesh.cuh; the union-find is common.cuh's (uf_find, uf_link), shared with tracks.cu.
 //
 // Determinism: no floating-point atomics; integer atomics only where the result does not depend on their order (the
 // depth keys, counts, union-find links to the lower root, the chart rectangles).  The energy totals use coop.cuh's
@@ -16,6 +18,7 @@
 
 #include "common.cuh"
 #include "coop.cuh"
+#include "trimesh.cuh"
 
 namespace cs {
 
@@ -23,7 +26,6 @@ long long g_texture_group_bytes = 0;          // cs_set_tuning("texture_group_by
 
 namespace {
 
-constexpr int TT = 256;                       // threads per CTA of every texture kernel
 constexpr int MCAND = 8;                      // candidates a face keeps
 constexpr long long TEXTURE_GROUP_BYTES = 1ll << 30;
 constexpr unsigned long long EMPTY = ~0ull;
@@ -73,20 +75,6 @@ struct TextureParams {
   int atlasWidth, rowsWritten;
 };
 
-struct D3 {
-  double x, y, z;
-};
-__device__ __forceinline__ D3 sub3(D3 a, D3 b) { return {a.x - b.x, a.y - b.y, a.z - b.z}; }
-__device__ __forceinline__ D3 cross3(D3 a, D3 b)
-{
-  return {a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x};
-}
-__device__ __forceinline__ double dot3(D3 a, D3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ D3 vert(const TextureParams &p, int v)
-{
-  return {(double)p.vin[3 * (size_t)v], (double)p.vin[3 * (size_t)v + 1], (double)p.vin[3 * (size_t)v + 2]};
-}
-
 // Y = R X + t, (u, v) = (K Y)_{0,1} / Y_z (rule 2)
 __device__ __forceinline__ void project(const TexCam &c, D3 X, double &u, double &v, double &z)
 {
@@ -104,29 +92,10 @@ __device__ __forceinline__ double area2_of(const double *u, const double *v)
   return (u[1] - u[0]) * (v[2] - v[0]) - (v[1] - v[0]) * (u[2] - u[0]);
 }
 
-__device__ __forceinline__ unsigned int tie_of(unsigned int id)
-{
-  const unsigned int m = id * 0x9E3779B1u;
-  return m ^ (m >> 16);
-}
-
 // ---- input and adjacency (rule 1) ---------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TT) texture_validate_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_edges_kernel(TextureParams p)
 {
-  for (int t = blockIdx.x * TT + threadIdx.x; t < p.T; t += gridDim.x * TT) {
-    const int a = p.tin[3 * (size_t)t], b = p.tin[3 * (size_t)t + 1], c = p.tin[3 * (size_t)t + 2];
-    bool bad = a < 0 || a >= p.V || b < 0 || b >= p.V || c < 0 || c >= p.V || a == b || b == c || a == c;
-    for (int j = 0; j < 3 && !bad; j++) {
-      const int w = p.tin[3 * (size_t)t + j];
-      for (int d = 0; d < 3; d++) bad = bad || !isfinite(p.vin[3 * (size_t)w + d]);
-    }
-    if (bad) atomicOr(&p.res->bad, 1u);
-  }
-}
-
-__global__ void __launch_bounds__(TT) texture_edges_kernel(TextureParams p)
-{
-  for (int c = blockIdx.x * TT + threadIdx.x; c < 3 * p.T; c += gridDim.x * TT) {
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
     const int t = c / 3, k = c - 3 * t;
     const unsigned int a = p.tin[c], b = p.tin[3 * t + (k + 1) % 3];
     p.ekey[c] = ((unsigned long long)min(a, b) << 32) | max(a, b);
@@ -136,10 +105,10 @@ __global__ void __launch_bounds__(TT) texture_edges_kernel(TextureParams p)
 }
 
 // a run of exactly two equal keys in the sorted list joins its two faces
-__global__ void __launch_bounds__(TT) texture_adjacency_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_adjacency_kernel(TextureParams p)
 {
   const int n = 3 * p.T;
-  for (int i = blockIdx.x * TT + threadIdx.x; i + 1 < n; i += gridDim.x * TT) {
+  for (int i = blockIdx.x * MT + threadIdx.x; i + 1 < n; i += gridDim.x * MT) {
     const unsigned long long k = p.ekeyS[i];
     if ((i > 0 && p.ekeyS[i - 1] == k) || p.ekeyS[i + 1] != k || (i + 2 < n && p.ekeyS[i + 2] == k)) continue;
     const int c1 = p.evalS[i], c2 = p.evalS[i + 1];
@@ -151,10 +120,10 @@ __global__ void __launch_bounds__(TT) texture_adjacency_kernel(TextureParams p)
 // ---- depth buffers (rule 2) ---------------------------------------------------------------------------------------
 // One thread per (image of the group, face): every pixel centre of the clipped bounding box that the three oriented
 // edge functions cover gets atomicMin of (float(depth) bits << 32) | face.
-__global__ void __launch_bounds__(TT) texture_raster_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_raster_kernel(TextureParams p)
 {
   const long long n = (long long)p.gn * p.T;
-  for (long long i = blockIdx.x * (long long)TT + threadIdx.x; i < n; i += (long long)gridDim.x * TT) {
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < n; i += (long long)gridDim.x * MT) {
     const int g = p.g0 + (int)(i / p.T), f = (int)(i % p.T);
     const TexCam &c = p.cams[g];
     int id[3];
@@ -162,7 +131,7 @@ __global__ void __launch_bounds__(TT) texture_raster_kernel(TextureParams p)
     bool front = true;
     for (int k = 0; k < 3; k++) {
       id[k] = p.tin[3 * (size_t)f + k];
-      project(c, vert(p, id[k]), u[k], v[k], z[k]);
+      project(c, vertex_of(p.vin, id[k]), u[k], v[k], z[k]);
       front = front && z[k] > 0.0;
     }
     if (!front) continue;
@@ -216,13 +185,13 @@ __device__ __forceinline__ bool sees(const TexCam &c, D3 X, int f, double depthT
 
 // One thread per face: the images of the group in ascending order, each that passes every test inserted into the
 // face's list by (q descending, image ascending), at most MCAND kept.
-__global__ void __launch_bounds__(TT) texture_candidate_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_candidate_kernel(TextureParams p)
 {
   unsigned int found = 0;
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
-    const D3 p0 = vert(p, p.tin[3 * (size_t)f]), p1 = vert(p, p.tin[3 * (size_t)f + 1]),
-             p2 = vert(p, p.tin[3 * (size_t)f + 2]);
-    const D3 n = cross3(sub3(p1, p0), sub3(p2, p0));
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
+    const D3 p0 = vertex_of(p.vin, p.tin[3 * (size_t)f]), p1 = vertex_of(p.vin, p.tin[3 * (size_t)f + 1]),
+             p2 = vertex_of(p.vin, p.tin[3 * (size_t)f + 2]);
+    const D3 n = normal3(p0, p1, p2);
     const D3 cen = {((p0.x + p1.x) + p2.x) / 3.0, ((p0.y + p1.y) + p2.y) / 3.0, ((p0.z + p1.z) + p2.z) / 3.0};
     const double ln = sqrt(dot3(n, n));
     double *cq = p.cq + (size_t)f * MCAND;
@@ -254,10 +223,10 @@ __global__ void __launch_bounds__(TT) texture_candidate_kernel(TextureParams p)
 }
 
 // ---- labelling (rule 4) -------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TT) texture_label_init_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_label_init_kernel(TextureParams p)
 {
   unsigned int unseen = 0;
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     const bool seen = p.cn[f] > 0;
     p.label[f] = seen ? p.ca[(size_t)f * MCAND] : -1;
     unseen += !seen;
@@ -268,11 +237,11 @@ __global__ void __launch_bounds__(TT) texture_label_init_kernel(TextureParams p)
 }
 
 // A Jones-Plassmann round: reads colA (the state at its start), writes colB.
-__global__ void __launch_bounds__(TT) texture_colour_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_colour_kernel(TextureParams p)
 {
   unsigned int left = 0;
   int top = -1;
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     int col = p.colA[f];
     if (col < 0) {
       const unsigned int sf = tie_of((unsigned int)f);
@@ -313,9 +282,9 @@ __device__ __forceinline__ int disagree(const TextureParams &p, int f, int l, bo
 }
 
 // e_f = D(f, l_f) + lambda * (the labelled neighbours g > f across an edge with l_g != l_f): tile partials
-__global__ void __launch_bounds__(TT) texture_energy_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_energy_kernel(TextureParams p)
 {
-  co_tree_tiles<1, TT>(p.T, p.part, [&](int f, double *v) {
+  co_tree_tiles<1, MT>(p.T, p.part, [&](int f, double *v) {
     const int l = p.label[f];
     if (l < 0) return;
     const double *cq = p.cq + (size_t)f * MCAND;
@@ -326,26 +295,21 @@ __global__ void __launch_bounds__(TT) texture_energy_kernel(TextureParams p)
   });
 }
 
-// one CTA: the group partials and the total in co_tree_groups / co_tree_total's order
-__global__ void __launch_bounds__(TT) texture_total_kernel(TextureParams p)
+// one CTA: the group partials and the total of the tile partials
+__global__ void __launch_bounds__(MT) texture_total_kernel(TextureParams p)
 {
-  const int tiles = (p.T + CO_TREE_TILE - 1) / CO_TREE_TILE, groups = (tiles + TT - 1) / TT;
-  for (int g = 0; g < groups; g++) {
-    const int t = g * TT + (int)threadIdx.x;
-    double v[1] = {t < tiles ? p.part[t] : 0.0};
-    co_cta_partial<1, TT / 32>(v, p.group + g);
-  }
   double tot[1];
-  co_totals<1>(p.group, groups, 1, tot);
+  co_tree_groups<1, MT>(p.T, p.part, p.group);
+  co_tree_total<1, MT>(p.T, p.group, tot);
   if (threadIdx.x == 0) p.res->energy = tot[0];
 }
 
 // An ICM step of the faces of one colour: the candidate of lowest local energy, the current label on ties, then the
 // earlier rank.
-__global__ void __launch_bounds__(TT) texture_icm_kernel(TextureParams p, int colour)
+__global__ void __launch_bounds__(MT) texture_icm_kernel(TextureParams p, int colour)
 {
   unsigned int changed = 0;
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     const int cur = p.label[f];
     if (cur < 0 || p.colA[f] != colour) continue;
     const double *cq = p.cq + (size_t)f * MCAND;
@@ -369,48 +333,35 @@ __global__ void __launch_bounds__(TT) texture_icm_kernel(TextureParams p, int co
 }
 
 // ---- charts (rule 5) ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ int find_root(const int *parent, int x)
+// union of every adjacent pair with equal labels (uf_link: every root is the lowest face of its component)
+__global__ void __launch_bounds__(MT) texture_hook_kernel(TextureParams p)
 {
-  for (;;) {
-    const int y = ((const volatile int *)parent)[x];
-    if (y == x) return x;
-    x = y;
-  }
-}
-
-// union of every adjacent pair with equal labels; the higher root is linked below the lower one, so every root is the
-// lowest face of its component whatever the order of the links
-__global__ void __launch_bounds__(TT) texture_hook_kernel(TextureParams p)
-{
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     const int l = p.label[f];
     if (l < 0) continue;
     for (int k = 0; k < 3; k++) {
       const int g = p.nbr[3 * (size_t)f + k];
       if (g <= f || p.label[g] != l) continue;
-      for (;;) {
-        const int a = find_root(p.parent, f), b = find_root(p.parent, g);
-        if (a == b) break;
-        const int hi = max(a, b), lo = min(a, b);
-        if (atomicCAS(&p.parent[hi], hi, lo) == hi) break;
-      }
+      uf_link(p.parent, f, g);
     }
   }
 }
 
-__global__ void __launch_bounds__(TT) texture_roots_kernel(TextureParams p)
+// colB[f] = the root of f.  Not into parent: a halving store of another thread's search could overwrite a root stored
+// there with an ancestor that is not the root.  colB is free once the sweeps end; the host then passes it on as parent.
+__global__ void __launch_bounds__(MT) texture_roots_kernel(TextureParams p)
 {
-  for (int f = blockIdx.x * TT + threadIdx.x; f <= p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f <= p.T; f += gridDim.x * MT) {
     if (f == p.T) { p.flag[f] = 0; continue; }
-    const int r = find_root(p.parent, f);
-    p.parent[f] = r;
+    const int r = uf_find(p.parent, f);
+    p.colB[f] = r;
     p.flag[f] = p.label[f] >= 0 && r == f;
   }
 }
 
-__global__ void __launch_bounds__(TT) texture_chart_init_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_chart_init_kernel(TextureParams p)
 {
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     if (!p.flag[f]) continue;
     int *e = p.craw + 6 * (size_t)p.chartIdx[f];
     e[0] = p.label[f];
@@ -421,16 +372,16 @@ __global__ void __launch_bounds__(TT) texture_chart_init_kernel(TextureParams p)
   if (blockIdx.x == 0 && threadIdx.x == 0) p.res->charts = p.chartIdx[p.T];
 }
 
-__global__ void __launch_bounds__(TT) texture_rect_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_rect_kernel(TextureParams p)
 {
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     const int l = p.label[f];
     if (l < 0) continue;
     int *e = p.craw + 6 * (size_t)p.chartIdx[p.parent[f]];
     const TexCam &c = p.cams[l];
     for (int k = 0; k < 3; k++) {
       double u, v, z;
-      project(c, vert(p, p.tin[3 * (size_t)f + k]), u, v, z);
+      project(c, vertex_of(p.vin, p.tin[3 * (size_t)f + k]), u, v, z);
       atomicMin(e + 1, (int)floor(u));
       atomicMin(e + 2, (int)floor(v));
       atomicMax(e + 3, (int)ceil(u));
@@ -441,9 +392,9 @@ __global__ void __launch_bounds__(TT) texture_rect_kernel(TextureParams p)
 }
 
 // ---- outputs (rule 6) ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TT) texture_uv_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_uv_kernel(TextureParams p)
 {
-  for (int f = blockIdx.x * TT + threadIdx.x; f < p.T; f += gridDim.x * TT) {
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
     const int l = p.label[f];
     float *uv = p.uv + 6 * (size_t)f;
     p.faceView[f] = l;
@@ -457,7 +408,7 @@ __global__ void __launch_bounds__(TT) texture_uv_kernel(TextureParams p)
     const TexCam &c = p.cams[l];
     for (int k = 0; k < 3; k++) {
       double u, v, z;
-      project(c, vert(p, p.tin[3 * (size_t)f + k]), u, v, z);
+      project(c, vertex_of(p.vin, p.tin[3 * (size_t)f + k]), u, v, z);
       uv[2 * k] = __double2float_rn((u - (double)e[1]) + (double)e[5]);
       uv[2 * k + 1] = __double2float_rn((v - (double)e[2]) + (double)e[6]);
     }
@@ -466,10 +417,10 @@ __global__ void __launch_bounds__(TT) texture_uv_kernel(TextureParams p)
 }
 
 // one thread per chart texel (charts one after the other, rows of a chart in order)
-__global__ void __launch_bounds__(TT) texture_atlas_kernel(TextureParams p)
+__global__ void __launch_bounds__(MT) texture_atlas_kernel(TextureParams p)
 {
   const long long n = p.numCharts ? p.cstart[p.numCharts] : 0;
-  for (long long i = blockIdx.x * (long long)TT + threadIdx.x; i < n; i += (long long)gridDim.x * TT) {
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < n; i += (long long)gridDim.x * MT) {
     int lo = 0, hi = p.numCharts - 1;
     while (lo < hi) {
       const int mid = (lo + hi + 1) >> 1;
@@ -485,8 +436,6 @@ __global__ void __launch_bounds__(TT) texture_atlas_kernel(TextureParams p)
     p.atlas[(size_t)Y * p.atlasWidth + e[5] + x] = c.img[(size_t)(e[2] + y) * c.pitch + e[1] + x];
   }
 }
-
-int grid_of(long long n) { return (int)std::max(1ll, std::min((n + TT - 1) / TT, 8192ll)); }
 
 }  // namespace
 
@@ -518,7 +467,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     bufMax = std::max(bufMax, acc);
   }
   groupStart.push_back(numImages);
-  const int tiles = (T + CO_TREE_TILE - 1) / CO_TREE_TILE, groups = (tiles + TT - 1) / TT;
+  const int tiles = (T + CO_TREE_TILE - 1) / CO_TREE_TILE, groups = (tiles + MT - 1) / MT;
 
   Layout L(256);
   const size_t resAt = L.take(sizeof(TextureResult));
@@ -603,8 +552,8 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     return 0;
   };
   auto total = [&](double &out) -> int {
-    texture_energy_kernel<<<grid_of(T), TT, 0, st>>>(p);
-    texture_total_kernel<<<1, TT, 0, st>>>(p);
+    texture_energy_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    texture_total_kernel<<<1, MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     int r;
@@ -616,7 +565,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     int r;
     if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
     CS_CUDA(cudaMemsetAsync(p.res, 0, sizeof(TextureResult), st));
-    texture_validate_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    mesh_validate_kernel<<<grid_of(T), MT, 0, st>>>(vin, V, tin, T, &p.res->bad);
     count_launch();
     CS_CUDA(cudaGetLastError());
     if ((r = readback()) < 0) return r;
@@ -624,9 +573,9 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
       status = 2;
       return 0;
     }
-    texture_edges_kernel<<<grid_of(3ll * T), TT, 0, st>>>(p);
+    texture_edges_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
     CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempBytes, p.ekey, p.ekeyS, p.eval, p.evalS, (int)C3, 0, 64, st));
-    texture_adjacency_kernel<<<grid_of(3ll * T), TT, 0, st>>>(p);
+    texture_adjacency_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     CS_CUDA(cudaMemsetAsync(p.cn, 0, (size_t)T * 4, st));
@@ -642,21 +591,21 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
       CS_CUDA(cudaMemsetAsync(buf, 0xff, off * 8, st));
       p.g0 = g0;
       p.gn = g1 - g0;
-      texture_raster_kernel<<<grid_of((long long)p.gn * T), TT, 0, st>>>(p);
+      texture_raster_kernel<<<grid_of((long long)p.gn * T), MT, 0, st>>>(p);
       if (tev && gi == 0) CS_CUDA(cudaEventRecord(tev[2], st));
-      texture_candidate_kernel<<<grid_of(T), TT, 0, st>>>(p);
+      texture_candidate_kernel<<<grid_of(T), MT, 0, st>>>(p);
       count_launch(2);
       CS_CUDA(cudaGetLastError());
       // the host table is read by the copy above before the next group changes it
       CS_CUDA(cudaStreamSynchronize(st));
     }
     if (tev) CS_CUDA(cudaEventRecord(tev[3], st));
-    texture_label_init_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    texture_label_init_kernel<<<grid_of(T), MT, 0, st>>>(p);
     count_launch();
     CS_CUDA(cudaGetLastError());
     for (;;) {
       CS_CUDA(cudaMemsetAsync(&p.res->left, 0, sizeof(unsigned int), st));
-      texture_colour_kernel<<<grid_of(T), TT, 0, st>>>(p);
+      texture_colour_kernel<<<grid_of(T), MT, 0, st>>>(p);
       count_launch();
       CS_CUDA(cudaGetLastError());
       std::swap(p.colA, p.colB);
@@ -669,7 +618,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     for (;;) {
       if (sweeps == maxSweeps) { status = 3; break; }
       CS_CUDA(cudaMemsetAsync(&p.res->changed, 0, sizeof(unsigned int), st));
-      for (int c = 0; c < colours; c++) texture_icm_kernel<<<grid_of(T), TT, 0, st>>>(p, c);
+      for (int c = 0; c < colours; c++) texture_icm_kernel<<<grid_of(T), MT, 0, st>>>(p, c);
       count_launch(colours);
       CS_CUDA(cudaGetLastError());
       sweeps++;
@@ -679,13 +628,14 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     }
     if ((r = total(energy[1])) < 0) return r;
     if (tev) CS_CUDA(cudaEventRecord(tev[4], st));
-    texture_hook_kernel<<<grid_of(T), TT, 0, st>>>(p);
-    texture_roots_kernel<<<grid_of(T + 1ll), TT, 0, st>>>(p);
+    texture_hook_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    texture_roots_kernel<<<grid_of(T + 1ll), MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
+    std::swap(p.parent, p.colB);              // from here on every face's parent is its root
     CS_CUDA(cub::DeviceScan::ExclusiveSum(temp, tempBytes, p.flag, p.chartIdx, T + 1, st));
-    texture_chart_init_kernel<<<grid_of(T), TT, 0, st>>>(p);
-    texture_rect_kernel<<<grid_of(T), TT, 0, st>>>(p);
+    texture_chart_init_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    texture_rect_kernel<<<grid_of(T), MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     if ((r = readback()) < 0) return r;
@@ -743,8 +693,8 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     p.rowsWritten = (int)rowsWritten;
     if (tev) CS_CUDA(cudaEventRecord(tev[5], st));
     if (rowsWritten) CS_CUDA(cudaMemsetAsync(atlas, 0, (size_t)rowsWritten * atlasWidth * 4, st));
-    texture_uv_kernel<<<grid_of(T), TT, 0, st>>>(p);
-    texture_atlas_kernel<<<grid_of(starts[C]), TT, 0, st>>>(p);
+    texture_uv_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    texture_atlas_kernel<<<grid_of(starts[C]), MT, 0, st>>>(p);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     if (tev) CS_CUDA(cudaEventRecord(tev[6], st));

@@ -2,9 +2,9 @@
 //
 // Feature f of image a has the global id g = base[a] + f.  The kernels, in order (DESIGN section 4):
 //   init      parent[g] = g, value[g] = g, the matched and conflict bytes and the statistics cleared
-//   hook      one thread per pair of every list: validate, mark both endpoints matched, hook the two roots (ECL-CC:
-//             find with path halving, atomicCAS of the larger root onto the smaller, retried from the new root)
-//   compress  label[g] = the root of g; parent[x] <= x holds throughout, so the root is the component's smallest id
+//   hook      one thread per pair of every list: validate, mark both endpoints matched, join the two trees (uf_link,
+//             the union-find of common.cuh)
+//   compress  label[g] = uf_find(g), the root, which is the component's smallest id
 //   sort      (label, g) pairs of all N features, stably by label over ceil(log2 N) bits (cub::DeviceRadixSort): every
 //             component is one run, in ascending label, its members in ascending g
 //   mark      per run: its first and end positions, and whether two adjacent members share an image
@@ -74,23 +74,6 @@ __device__ __forceinline__ int image_of(const int *__restrict__ bases, int numIm
   return lo;
 }
 
-// The root of x with path halving.  Every store writes an ancestor, so parent[x] <= x keeps holding; a store racing
-// with another thread's can only leave a different ancestor.
-__device__ __forceinline__ int tk_find(int *parent, int x)
-{
-  volatile int *p = parent;
-  int cur = p[x];
-  if (cur != x) {
-    int prev = x, next;
-    while (cur > (next = p[cur])) {
-      p[prev] = next;
-      prev = cur;
-      cur = next;
-    }
-  }
-  return cur;
-}
-
 __global__ void __launch_bounds__(TK_THREADS) tracks_init_kernel(TkBufs b, int N)
 {
   const long long g = thread_index();
@@ -116,25 +99,17 @@ __global__ void __launch_bounds__(TK_THREADS) tracks_hook_kernel(TkBufs b, int n
     if (ib) atomicAdd(&b.stats[1], (unsigned long long)__popc(ib));
   }
   if (!ok) return;
-  int *parent = b.keys[1];
   const int u = L.base1 + p.x, v = L.base2 + p.y;
   b.matched[u] = 1;
   b.matched[v] = 1;
-  int ru = tk_find(parent, u), rv = tk_find(parent, v);
-  while (ru != rv) {
-    const int hi = ru > rv ? ru : rv, lo = ru > rv ? rv : ru;
-    const int old = atomicCAS(parent + hi, hi, lo);
-    if (old == hi) break;
-    // hi was hooked meanwhile: continue from its new root
-    if (hi == ru) ru = tk_find(parent, old); else rv = tk_find(parent, old);
-  }
+  uf_link(b.keys[1], u, v);   // keys[1] holds parent until the sort
 }
 
 // After every hook: the label of every feature.  The halving stores go to parent only, so each label is the root.
 __global__ void __launch_bounds__(TK_THREADS) tracks_compress_kernel(TkBufs b, int N)
 {
   const long long g = thread_index();
-  if (g < N) b.keys[0][g] = tk_find(b.keys[1], (int)g);
+  if (g < N) b.keys[0][g] = uf_find(b.keys[1], (int)g);
 }
 
 // Over the sorted positions (keys / vals the sort's output): the run of label L spans [start[L], end[L]).
