@@ -53,21 +53,43 @@ def adjacency(tris):
     order = np.argsort(key, kind="stable")
     ks = key[order]
     nbr = np.full(3 * T, -1, np.int64)
-    n = len(ks)
-    for i in range(n - 1):
-        if (i > 0 and ks[i - 1] == ks[i]) or ks[i + 1] != ks[i] or (i + 2 < n and ks[i + 2] == ks[i]):
-            continue
+    for i in pair_starts(ks):
         c1, c2 = order[i], order[i + 1]
         nbr[c1], nbr[c2] = c2 // 3, c1 // 3
     return nbr.reshape(T, 3)
 
 
+def pair_starts(ks):
+    """The positions i of the sorted edge keys where a run of exactly two equal keys starts."""
+    n = len(ks)
+    return [i for i in range(n - 1)
+            if not ((i > 0 and ks[i - 1] == ks[i]) or ks[i + 1] != ks[i] or (i + 2 < n and ks[i + 2] == ks[i]))]
+
+
 def depth_buffer(K, R, t, W, H, verts, tris):
     """The keys (float(depth) bits << 32) | face of one image [H, W] (EMPTY where no face covers the pixel)."""
+    buf = np.full(H * W, EMPTY, np.uint64)
+    for f, pix, d in face_depths(K, R, t, W, H, verts, tris):
+        combine(buf, pix, d, f)
+    return buf.reshape(H, W)
+
+
+def covers(w0, w1, w2, S):
+    return (w0 >= 0) & (w1 >= 0) & (w2 >= 0) & (S > 0)
+
+
+def combine(buf, pix, d, f):
+    """The pixels pix of face f with their float64 depths d into the buffer: the depth rounded to float once, then the
+    key's 64-bit minimum (the nearer float depth wins, ties go to the lower face)."""
+    key = (d.astype(np.float32).view(np.uint32).astype(np.uint64) << np.uint64(32)) | np.uint64(f)
+    np.minimum.at(buf, pix, key)
+
+
+def face_depths(K, R, t, W, H, verts, tris):
+    """Per rasterised face: (face, the flat indices y W + x of its covered pixels, their float64 depths)."""
     X = np.asarray(verts, np.float32).astype(np.float64)
     tr = np.asarray(tris, np.int64)
     u, v, z = project(K, R, t, X[tr])
-    buf = np.full(H * W, EMPTY, np.uint64)
     A = area2(u, v)
     with np.errstate(invalid="ignore"):
         ok = (z > 0).all(1) & (A != 0) & np.isfinite(A)
@@ -88,16 +110,12 @@ def depth_buffer(K, R, t, W, H, verts, tris):
             du, dv = u[f, Q] - u[f, P], v[f, Q] - v[f, P]
             w.append((s if lo else -s) * (du * (ys - v[f, P]) - dv * (xs - u[f, P])))
         S = (w[0] + w[1]) + w[2]
-        cov = (w[0] >= 0) & (w[1] >= 0) & (w[2] >= 0) & (S > 0)
+        cov = covers(w[0], w[1], w[2], S)
         if not cov.any():
             continue
         w0, w1, w2, S = w[0][cov], w[1][cov], w[2][cov], S[cov]
         iz = ((w1 / z[f, 0] + w2 / z[f, 1]) + w0 / z[f, 2]) / S
-        d = (1.0 / iz).astype(np.float32)
-        key = (d.view(np.uint32).astype(np.uint64) << np.uint64(32)) | np.uint64(f)
-        pix = ys[cov].astype(np.int64) * W + xs[cov].astype(np.int64)
-        np.minimum.at(buf, pix, key)
-    return buf.reshape(H, W)
+        yield f, ys[cov].astype(np.int64) * W + xs[cov].astype(np.int64), 1.0 / iz
 
 
 def candidates(cams, bufs, verts, tris, maxViewAngleDeg, depthTol):
@@ -141,7 +159,12 @@ def candidates(cams, bufs, verts, tris, maxViewAngleDeg, depthTol):
         for f in np.nonzero(ok)[0]:
             lists[f].append((float(q[f]), a))
         total += int(ok.sum())
-    return [sorted(c, key=lambda e: (-e[0], e[1]))[:MCAND] for c in lists], total
+    return [best_candidates(c) for c in lists], total
+
+
+def best_candidates(c):
+    """A face's (q, image) pairs in image order: its best MCAND by (q descending, image ascending)."""
+    return sorted(c, key=lambda e: (-e[0], e[1]))[:MCAND]
 
 
 def colouring(nbr):
@@ -281,20 +304,7 @@ def texture(images, Ks, Rs, ts, verts, tris, lam=0.5, maxViewAngleDeg=75.0, dept
             status = 0
             break
     e1 = energy(label, cands, nbr, lam)
-    # charts
-    parent = np.arange(T)
-
-    def find(x):
-        while parent[x] != x:
-            x = parent[x]
-        return x
-    for f in range(T):
-        for g in nbr[f]:
-            if g > f and label[f] >= 0 and label[g] == label[f]:
-                a, b = find(f), find(g)
-                if a != b:
-                    parent[max(a, b)] = min(a, b)
-    root = np.array([find(f) for f in range(T)])
+    root = chart_roots(label, nbr)
     roots = [f for f in range(T) if label[f] >= 0 and root[f] == f]
     idx = {r: c for c, r in enumerate(roots)}
     C = len(roots)
@@ -318,20 +328,9 @@ def texture(images, Ks, Rs, ts, verts, tris, lam=0.5, maxViewAngleDeg=75.0, dept
         e[5] += 1
     table = np.zeros((C, 8), np.int64)
     for c, e in enumerate(raw):
-        W, H = cams[e[0]][3], cams[e[0]][4]
-        x0, x1 = max(0, e[1] - padding), min(W - 1, e[3] + padding)
-        y0, y1 = max(0, e[2] - padding), min(H - 1, e[4] + padding)
+        x0, y0, x1, y1 = chart_rect(e, cams[e[0]][3], cams[e[0]][4], padding)
         table[c] = [e[0], x0, y0, x1 - x0 + 1, y1 - y0 + 1, 0, 0, e[5]]
-    order = sorted(range(C), key=lambda c: (-table[c, 4], -table[c, 3], c))
-    shelfY = shelfH = cx = 0
-    for c in order:
-        if cx + table[c, 3] > atlasWidth:
-            shelfY += shelfH
-            shelfH = cx = 0
-        table[c, 5], table[c, 6] = cx, shelfY
-        cx += table[c, 3]
-        shelfH = max(shelfH, table[c, 4])
-    full = shelfY + shelfH
+    full = pack(table, atlasWidth)
     rows = full if maxAtlasRows is None else min(full, maxAtlasRows)
     atlas = np.zeros((full, atlasWidth), np.float32)
     for c in range(C):
@@ -347,3 +346,42 @@ def texture(images, Ks, Rs, ts, verts, tris, lam=0.5, maxViewAngleDeg=75.0, dept
                 charts=table[:C if maxCharts is None else min(C, maxCharts)].astype(np.int32), info=[e0, e1],
                 stats=stats, colours=col, bufs=bufs, cands=cands, nbr=nbr, start=np.array(
                     [c[0][1] if c else -1 for c in cands], np.int64))
+
+
+def chart_roots(label, nbr):
+    """Rule 5's union-find: per face the root of its chart, the lowest face of the chart (every link from the higher
+    root to the lower); unseen faces are their own roots."""
+    T = len(label)
+    parent = np.arange(T)
+
+    def find(x):
+        while parent[x] != x:
+            x = parent[x]
+        return x
+    for f in range(T):
+        for g in nbr[f]:
+            if g > f and label[f] >= 0 and label[g] == label[f]:
+                a, b = find(f), find(g)
+                if a != b:
+                    parent[max(a, b)] = min(a, b)
+    return np.array([find(f) for f in range(T)])
+
+
+def chart_rect(e, W, H, padding):
+    """(x0, y0, x1, y1) of a chart's raw rectangle e {image, xmin, ymin, xmax, ymax, faces}, padded and clamped."""
+    return max(0, e[1] - padding), max(0, e[2] - padding), min(W - 1, e[3] + padding), min(H - 1, e[4] + padding)
+
+
+def pack(table, atlasWidth):
+    """Rule 6's shelves over the chart table [C, 8] (ox, oy written in place); returns the full atlas height."""
+    C = len(table)
+    order = sorted(range(C), key=lambda c: (-table[c, 4], -table[c, 3], c))
+    shelfY = shelfH = cx = 0
+    for c in order:
+        if cx + table[c, 3] > atlasWidth:
+            shelfY += shelfH
+            shelfH = cx = 0
+        table[c, 5], table[c, 6] = cx, shelfY
+        cx += table[c, 3]
+        shelfH = max(shelfH, table[c, 4])
+    return shelfY + shelfH
