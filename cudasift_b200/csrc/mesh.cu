@@ -3,7 +3,9 @@
 // solve and the iso-value, and marching tetrahedra with trimming as count-scan-write passes.  Every rule is stated in
 // cudasift_b200.h at cs_poisson_mesh; tests/mesh_oracle.py restates them in float64.  cs_poisson_mesh_screened (screened
 // Poisson with a Neumann boundary) shares every kernel but the right-hand side and the solve; its rules are stated at
-// cs_poisson_mesh_screened and restated in tests/mesh_screened_oracle.py.
+// cs_poisson_mesh_screened and restated in tests/mesh_screened_oracle.py.  The two solve kernels share the V-cycle
+// schedule (over two overloads of each level operation), the preconditioned CG loop (mgpcg, given each call's operator
+// pass) and the trilinear field at a point; each keeps its own set-up, true residual, tau and status rule.
 //
 // Determinism: no floating-point atomics.  Integer atomics only where the result does not depend on their order (the
 // bounding box as ordered-integer max, the cell histogram, the kept-vertex bit masks).  Every floating-point sum has a
@@ -75,14 +77,15 @@ struct MeshParams {
   int maxVertices, maxTriangles;
 };
 
-// A level of the screened call's V-cycle: MeshLevel's arrays plus the diagonal of its screening operator.
+// A level of the screened call's V-cycle: MeshLevel's arrays plus the diagonal of its screening operator.  The level
+// operations have an overload for each of MeshLevel and NLevel; the V-cycle schedule over them is one template.
 struct NLevel {
   float *x, *f, *t, *s;
   int n;
 };
 
-// The screened call's fields, a second kernel argument so that MeshParams (and the Dirichlet kernels' code) stay as
-// they are.
+// The screened call's fields, a second kernel argument so that MeshParams keeps its layout (the Dirichlet kernels read
+// it through the constant bank, and their code stays as it was).
 struct ScreenParams {
   double alpha;                   // pointWeight
   double *u;                      // omega B_p^T x per sorted point [used]
@@ -132,6 +135,8 @@ __device__ __forceinline__ void node_ijk(int idx, int n1, int &i, int &j, int &k
 }
 
 // ---- multigrid level operations (tid / nth: the threads taking part; sync: their barrier) ---------------------------
+// Each operation has two overloads: on a MeshLevel the Dirichlet call's (interior nodes only, diagonal 6), on an NLevel
+// the screened call's (every node, its in-grid neighbours, diagonal deg + s).  The V-cycle schedule over them is one.
 struct GridTeam {
   cg::grid_group g;
   int tid, nth;
@@ -150,6 +155,29 @@ __device__ __forceinline__ float nbr_sum(const float *x, int idx, int n1)
   return ((((x[idx - 1] + x[idx + 1]) + x[idx - n1]) + x[idx + n1]) + x[idx - s]) + x[idx + s];
 }
 
+// The in-grid neighbours of node idx = (i, j, k) of a level with n cells in the order -x, +x, -y, +y, -z, +z (an absent
+// one adds 0, so an interior node gets nbr_sum's value), in float; deg receives their count.
+__device__ __forceinline__ float nbr_sum_nm(const float *x, int idx, int i, int j, int k, int n, float &deg)
+{
+  const int n1 = n + 1, s = n1 * n1;
+  const float a = i > 0 ? x[idx - 1] : 0.0f, b = i < n ? x[idx + 1] : 0.0f;
+  const float c = j > 0 ? x[idx - n1] : 0.0f, d = j < n ? x[idx + n1] : 0.0f;
+  const float e = k > 0 ? x[idx - s] : 0.0f, f = k < n ? x[idx + s] : 0.0f;
+  deg = (float)((i > 0) + (i < n) + (j > 0) + (j < n) + (k > 0) + (k < n));
+  return ((((a + b) + c) + d) + e) + f;
+}
+
+// The same in float64 from the floats.
+__device__ __forceinline__ double nbr_sum_nm_d(const float *x, int idx, int i, int j, int k, int n, double &deg)
+{
+  const int n1 = n + 1, s = n1 * n1;
+  const double a = i > 0 ? x[idx - 1] : 0.0, b = i < n ? x[idx + 1] : 0.0;
+  const double c = j > 0 ? x[idx - n1] : 0.0, d = j < n ? x[idx + n1] : 0.0;
+  const double e = k > 0 ? x[idx - s] : 0.0, f = k < n ? x[idx + s] : 0.0;
+  deg = (double)((i > 0) + (i < n) + (j > 0) + (j < n) + (k > 0) + (k < n));
+  return ((((a + b) + c) + d) + e) + f;
+}
+
 // One Gauss-Seidel half-sweep over the interior nodes of one colour ((i + j + k) & 1): x = (f + neighbours) / 6.
 template <class T>
 __device__ void rb_sweep(const MeshLevel &L, int colour, T &team)
@@ -163,14 +191,18 @@ __device__ void rb_sweep(const MeshLevel &L, int colour, T &team)
   }
 }
 
+// The same over every node of one colour: x = (f + in-grid neighbours) / (deg + s).
 template <class T>
-__device__ void smooth_pairs(const MeshLevel &L, int pairs, bool redFirst, T &team)
+__device__ void rb_sweep(const NLevel &L, int colour, T &team)
 {
-  for (int s = 0; s < pairs; s++) {
-    rb_sweep(L, redFirst ? 0 : 1, team);
-    team.sync();
-    rb_sweep(L, redFirst ? 1 : 0, team);
-    team.sync();
+  const int n1 = L.n + 1, m = n1 * n1 * n1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int i, j, k;
+    node_ijk(idx, n1, i, j, k);
+    if (((i + j + k) & 1) != colour) continue;
+    float deg;
+    const float nb = nbr_sum_nm(L.x, idx, i, j, k, L.n, deg);
+    L.x[idx] = (L.f[idx] + nb) / (deg + L.s[idx]);
   }
 }
 
@@ -184,6 +216,20 @@ __device__ void residual(const MeshLevel &L, T &team)
     node_ijk(idx, n1, i, j, k);
     const bool bnd = i == 0 || j == 0 || k == 0 || i == L.n || j == L.n || k == L.n;
     L.t[idx] = bnd ? 0.0f : L.f[idx] - (6.0f * L.x[idx] - nbr_sum(L.x, idx, n1));
+  }
+}
+
+// t = f - ((deg + s) x - in-grid neighbours) at every node.
+template <class T>
+__device__ void residual(const NLevel &L, T &team)
+{
+  const int n1 = L.n + 1, m = n1 * n1 * n1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int i, j, k;
+    node_ijk(idx, n1, i, j, k);
+    float deg;
+    const float nb = nbr_sum_nm(L.x, idx, i, j, k, L.n, deg);
+    L.t[idx] = L.f[idx] - ((deg + L.s[idx]) * L.x[idx] - nb);
   }
 }
 
@@ -212,6 +258,28 @@ __device__ void restrict_to(const MeshLevel &F, const MeshLevel &C, T &team)
   }
 }
 
+// The same at every coarse node over its in-grid fine nodes.
+template <class T>
+__device__ void restrict_to(const NLevel &F, const NLevel &C, T &team)
+{
+  const int n1 = C.n + 1, m = n1 * n1 * n1, f1 = F.n + 1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int I, J, K;
+    node_ijk(idx, n1, I, J, K);
+    C.x[idx] = 0.0f;
+    float s = 0.0f;
+    for (int dz = -1; dz <= 1; dz++)
+      for (int dy = -1; dy <= 1; dy++)
+        for (int dx = -1; dx <= 1; dx++) {
+          const int fi = 2 * I + dx, fj = 2 * J + dy, fk = 2 * K + dz;
+          if (fi < 0 || fj < 0 || fk < 0 || fi > F.n || fj > F.n || fk > F.n) continue;
+          const float w = (dx ? 0.5f : 1.0f) * (dy ? 0.5f : 1.0f) * (dz ? 0.5f : 1.0f);
+          s = fmaf(w, F.t[(fk * f1 + fj) * f1 + fi], s);
+        }
+    C.f[idx] = 0.5f * s;
+  }
+}
+
 // x += P xc at the fine interior nodes: trilinear interpolation of the coarse nodes (odd coordinates take the two
 // neighbours with 1/2 each; z outer, x inner).
 template <class T>
@@ -233,8 +301,39 @@ __device__ void prolong_add(const MeshLevel &C, const MeshLevel &F, T &team)
   }
 }
 
+// The same at every fine node.
 template <class T>
-__device__ void v_down(const MeshLevel *lv, int l, T &team)
+__device__ void prolong_add(const NLevel &C, const NLevel &F, T &team)
+{
+  const int n1 = F.n + 1, m = n1 * n1 * n1, c1 = C.n + 1;
+  for (int idx = team.tid; idx < m; idx += team.nth) {
+    int i, j, k;
+    node_ijk(idx, n1, i, j, k);
+    float s = 0.0f;
+    for (int bz = 0; bz <= (k & 1); bz++)
+      for (int by = 0; by <= (j & 1); by++)
+        for (int bx = 0; bx <= (i & 1); bx++) {
+          const float w = ((i & 1) ? 0.5f : 1.0f) * ((j & 1) ? 0.5f : 1.0f) * ((k & 1) ? 0.5f : 1.0f);
+          s = fmaf(w, C.x[((k / 2 + bz) * c1 + j / 2 + by) * c1 + i / 2 + bx], s);
+        }
+    F.x[idx] += s;
+  }
+}
+
+// ---- the V-cycle schedule, on MeshLevel or NLevel levels ------------------------------------------------------------
+template <class Lv, class T>
+__device__ void smooth_pairs(const Lv &L, int pairs, bool redFirst, T &team)
+{
+  for (int s = 0; s < pairs; s++) {
+    rb_sweep(L, redFirst ? 0 : 1, team);
+    team.sync();
+    rb_sweep(L, redFirst ? 1 : 0, team);
+    team.sync();
+  }
+}
+
+template <class Lv, class T>
+__device__ void v_down(const Lv *lv, int l, T &team)
 {
   smooth_pairs(lv[l], NU, true, team);
   residual(lv[l], team);
@@ -243,8 +342,8 @@ __device__ void v_down(const MeshLevel *lv, int l, T &team)
   team.sync();
 }
 
-template <class T>
-__device__ void v_up(const MeshLevel *lv, int l, T &team)
+template <class Lv, class T>
+__device__ void v_up(const Lv *lv, int l, T &team)
 {
   prolong_add(lv[l + 1], lv[l], team);
   team.sync();
@@ -253,10 +352,10 @@ __device__ void v_up(const MeshLevel *lv, int l, T &team)
 
 // One V-cycle from x = 0 on level 0 (lv[0].x zeroed, lv[0].f set): the levels of more than LOCAL_N cells with grid
 // barriers, the rest inside CTA 0.
-__device__ void v_cycle(const MeshParams &p, GridTeam &grid)
+template <class Lv>
+__device__ void v_cycle(const Lv *lv, int levels, GridTeam &grid)
 {
-  const MeshLevel *lv = p.lv;
-  const int last = p.levels - 1;
+  const int last = levels - 1;
   int lg = 0;
   while (lg < last && lv[lg].n > LOCAL_N) lg++;
   for (int l = 0; l < lg; l++) v_down(lv, l, grid);
@@ -269,6 +368,106 @@ __device__ void v_cycle(const MeshParams &p, GridTeam &grid)
   }
   grid.sync();
   for (int l = lg - 1; l >= 0; l--) v_up(lv, l, grid);
+}
+
+// ---- the solve ------------------------------------------------------------------------------------------------------
+// The three-level total of the tile partials over n items (co_tree_groups, then co_tree_total, each after a grid
+// barrier); every thread receives the K totals.
+template <int K>
+__device__ __forceinline__ void grid_total(const MeshParams &p, int n, GridTeam &grid, double (&out)[K])
+{
+  grid.sync();
+  co_tree_groups<K, MT>(n, p.tilePart, p.groupPart);
+  grid.sync();
+  co_tree_total<K, MT>(n, p.groupPart, out);
+}
+
+__device__ __forceinline__ double grid_total(const MeshParams &p, int n, GridTeam &grid)
+{
+  double t[1];
+  grid_total<1>(p, n, grid, t);
+  return t[0];
+}
+
+// A field trilinear at grid coordinates g (tau, the mean density): add(w, node) for the corners of g's cell
+// c = clamp(floor(g), 0, N - 1), z outer and x inner, w = prod (t_a or 1 - t_a) with t = g - c.  The caller keeps the
+// sums, so one weight serves chi and D together.
+template <class F>
+__device__ __forceinline__ void trilinear(const double *g, int N, int n1, F &&add)
+{
+  int c[3];
+  double t[3];
+  for (int a = 0; a < 3; a++) {
+    c[a] = min(max((int)floor(g[a]), 0), N - 1);
+    t[a] = g[a] - c[a];
+  }
+  for (int bz = 0; bz < 2; bz++)
+    for (int by = 0; by < 2; by++)
+      for (int bx = 0; bx < 2; bx++) {
+        const double w = (bx ? t[0] : 1.0 - t[0]) * (by ? t[1] : 1.0 - t[1]) * (bz ? t[2] : 1.0 - t[2]);
+        add(w, ((c[2] + bz) * n1 + c[1] + by) * n1 + c[0] + bx);
+      }
+}
+
+// CG for A chi = b from chi = 0, preconditioned by one V-cycle on the levels lv (z = B r), until r.r <= tol^2 b.b,
+// after maxIterations iterations, or when p.A p is not positive; z, p and q are V0, V1 and V2.  The operator pass of an
+// iteration is pre_ap(p) once p is complete, then q_i = ap(p, i), the float (A p)_i, in one tile pass with p.q.  Every
+// total is a fixed-order one in float64; the vectors are floats, updated in float64.  Returns the iterations; bb and
+// rr receive b.b and the last r.r; chi is complete on return.
+template <class Lv, class Pre, class Ap>
+__device__ __forceinline__ int mgpcg(const MeshParams &p, const Lv *lv, GridTeam &grid, Pre &&pre_ap, Ap &&ap,
+                                     double &bb, double &rr)
+{
+  const int M = p.M;
+  float *x = p.chi, *r = p.r, *b = p.b, *z = p.V0, *pp = p.V1, *q = p.V2;
+  double rz = 0.0;
+  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
+    r[i] = b[i];
+    z[i] = 0.0f;
+    v[0] += (double)b[i] * (double)b[i];
+  });
+  bb = grid_total(p, M, grid);
+  rr = bb;
+  int k = 0;
+  bool done = rr <= p.tol2 * bb;
+  if (!done) {
+    v_cycle(lv, p.levels, grid);
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
+      pp[i] = z[i];
+      v[0] += (double)r[i] * (double)z[i];
+    });
+    rz = grid_total(p, M, grid);
+  }
+  while (!done) {
+    grid.sync();                                       // p complete before pre_ap and A p read it
+    pre_ap(pp);
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
+      const float a = ap(pp, i);
+      q[i] = a;
+      v[0] += (double)pp[i] * (double)a;
+    });
+    const double pq = grid_total(p, M, grid);
+    if (!(pq > 0.0)) break;
+    const double alpha = rz / pq;
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
+      x[i] = (float)((double)x[i] + alpha * (double)pp[i]);
+      const float ri = (float)((double)r[i] - alpha * (double)q[i]);
+      r[i] = ri;
+      z[i] = 0.0f;
+      v[0] += (double)ri * (double)ri;
+    });
+    rr = grid_total(p, M, grid);
+    k++;
+    if (rr <= p.tol2 * bb || k >= p.maxIterations) break;
+    v_cycle(lv, p.levels, grid);
+    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
+    const double rzNew = grid_total(p, M, grid);
+    const double beta = rzNew / rz;
+    rz = rzNew;
+    for (int i = grid.tid; i < M; i += grid.nth) pp[i] = (float)((double)z[i] + beta * (double)pp[i]);
+  }
+  grid.sync();
+  return k;
 }
 
 // ---- kernels --------------------------------------------------------------------------------------------------------
@@ -408,71 +607,17 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
   if (R.status != 0) return;                           // every CTA reads the same word
   GridTeam grid{cg::this_grid(), (int)(blockIdx.x * MT + threadIdx.x), (int)(gridDim.x * MT)};
   const int N = p.N, n1 = N + 1, ss = n1 * n1, M = p.M;
-  float *x = p.chi, *r = p.r, *b = p.b, *z = p.V0, *pp = p.V1, *q = p.V2;
+  const float *x = p.chi, *b = p.b;
   auto interior = [&](int idx) {
     int i, j, k;
     node_ijk(idx, n1, i, j, k);
     return i > 0 && j > 0 && k > 0 && i < N && j < N && k < N;
   };
-  auto total1 = [&](double &out) {
-    grid.sync();
-    co_tree_groups<1, MT>(M, p.tilePart, p.groupPart);
-    grid.sync();
-    double t[1];
-    co_tree_total<1, MT>(M, p.groupPart, t);
-    out = t[0];
-  };
-
-  double bb, rr, rz = 0.0;
-  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-    r[i] = b[i];
-    z[i] = 0.0f;
-    v[0] += (double)b[i] * (double)b[i];
-  });
-  total1(bb);
-  rr = bb;
-  int k = 0;
-  bool done = rr <= p.tol2 * bb;
-  if (!done) {
-    v_cycle(p, grid);
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-      pp[i] = z[i];
-      v[0] += (double)r[i] * (double)z[i];
-    });
-    total1(rz);
-  }
-  while (!done) {
-    grid.sync();                                       // p complete before A p reads its neighbours
-    double pq;
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-      const float a = interior(i) ? 6.0f * pp[i] - nbr_sum(pp, i, n1) : 0.0f;
-      q[i] = a;
-      v[0] += (double)pp[i] * (double)a;
-    });
-    total1(pq);
-    if (!(pq > 0.0)) break;
-    const double alpha = rz / pq;
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-      x[i] = (float)((double)x[i] + alpha * (double)pp[i]);
-      const float ri = (float)((double)r[i] - alpha * (double)q[i]);
-      r[i] = ri;
-      z[i] = 0.0f;
-      v[0] += (double)ri * (double)ri;
-    });
-    total1(rr);
-    k++;
-    if (rr <= p.tol2 * bb || k >= p.maxIterations) break;
-    v_cycle(p, grid);
-    double rzNew;
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
-    total1(rzNew);
-    const double beta = rzNew / rz;
-    rz = rzNew;
-    for (int i = grid.tid; i < M; i += grid.nth) pp[i] = (float)((double)z[i] + beta * (double)pp[i]);
-  }
-  grid.sync();
+  double bb, rr;
+  const int k = mgpcg(
+      p, p.lv, grid, [](const float *) {},
+      [&](const float *pp, int i) { return interior(i) ? 6.0f * pp[i] - nbr_sum(pp, i, n1) : 0.0f; }, bb, rr);
   // the true residual b - A chi, in float64 from the floats
-  double rt;
   co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
     if (!interior(i)) return;
     const double ax = 6.0 * (double)x[i] - (((((double)x[i - 1] + (double)x[i + 1]) + (double)x[i - n1]) +
@@ -480,34 +625,20 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
     const double e = (double)b[i] - ax;
     v[0] += e * e;
   });
-  total1(rt);
+  const double rt = grid_total(p, M, grid);
   // tau and the mean density: chi and D trilinear at each used point's g, in sorted order
   const int used = (int)R.used;
   co_tree_tiles<2, MT>(used, p.tilePart, [&](int s, double *v) {
-    const double *g = p.gs + 3 * (size_t)s;
-    int c[3];
-    double t[3];
-    for (int a = 0; a < 3; a++) {
-      c[a] = min(max((int)floor(g[a]), 0), N - 1);
-      t[a] = g[a] - c[a];
-    }
     double sc = 0.0, sd = 0.0;
-    for (int bz = 0; bz < 2; bz++)
-      for (int by = 0; by < 2; by++)
-        for (int bx = 0; bx < 2; bx++) {
-          const double w = (bx ? t[0] : 1.0 - t[0]) * (by ? t[1] : 1.0 - t[1]) * (bz ? t[2] : 1.0 - t[2]);
-          const int node = ((c[2] + bz) * n1 + c[1] + by) * n1 + c[0] + bx;
-          sc += w * (double)x[node];
-          sd += w * (double)p.D[node];
-        }
+    trilinear(p.gs + 3 * (size_t)s, N, n1, [&](double w, int node) {
+      sc += w * (double)x[node];
+      sd += w * (double)p.D[node];
+    });
     v[0] += sc;
     v[1] += sd;
   });
-  grid.sync();
-  co_tree_groups<2, MT>(used, p.tilePart, p.groupPart);
-  grid.sync();
   double td[2];
-  co_tree_total<2, MT>(used, p.groupPart, td);
+  grid_total<2>(p, used, grid, td);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     const double tau = td[0] / used;
     R.info[4] = tau;
@@ -519,147 +650,6 @@ __global__ void __launch_bounds__(MT) mesh_solve_kernel(MeshParams p)
 }
 
 // ---- screened Poisson with a Neumann boundary (cs_poisson_mesh_screened) ---------------------------------------------
-// The in-grid neighbours of node idx = (i, j, k) of a level with n cells in the order -x, +x, -y, +y, -z, +z (an absent
-// one adds 0, so an interior node gets nbr_sum's value), in float; deg receives their count.
-__device__ __forceinline__ float nbr_sum_nm(const float *x, int idx, int i, int j, int k, int n, float &deg)
-{
-  const int n1 = n + 1, s = n1 * n1;
-  const float a = i > 0 ? x[idx - 1] : 0.0f, b = i < n ? x[idx + 1] : 0.0f;
-  const float c = j > 0 ? x[idx - n1] : 0.0f, d = j < n ? x[idx + n1] : 0.0f;
-  const float e = k > 0 ? x[idx - s] : 0.0f, f = k < n ? x[idx + s] : 0.0f;
-  deg = (float)((i > 0) + (i < n) + (j > 0) + (j < n) + (k > 0) + (k < n));
-  return ((((a + b) + c) + d) + e) + f;
-}
-
-// The same in float64 from the floats.
-__device__ __forceinline__ double nbr_sum_nm_d(const float *x, int idx, int i, int j, int k, int n, double &deg)
-{
-  const int n1 = n + 1, s = n1 * n1;
-  const double a = i > 0 ? x[idx - 1] : 0.0, b = i < n ? x[idx + 1] : 0.0;
-  const double c = j > 0 ? x[idx - n1] : 0.0, d = j < n ? x[idx + n1] : 0.0;
-  const double e = k > 0 ? x[idx - s] : 0.0, f = k < n ? x[idx + s] : 0.0;
-  deg = (double)((i > 0) + (i < n) + (j > 0) + (j < n) + (k > 0) + (k < n));
-  return ((((a + b) + c) + d) + e) + f;
-}
-
-// Red-black Gauss-Seidel half-sweep over every node of one colour: x = (f + neighbours) / (deg + s).
-template <class T>
-__device__ void rb_sweep_nm(const NLevel &L, int colour, T &team)
-{
-  const int n1 = L.n + 1, m = n1 * n1 * n1;
-  for (int idx = team.tid; idx < m; idx += team.nth) {
-    int i, j, k;
-    node_ijk(idx, n1, i, j, k);
-    if (((i + j + k) & 1) != colour) continue;
-    float deg;
-    const float nb = nbr_sum_nm(L.x, idx, i, j, k, L.n, deg);
-    L.x[idx] = (L.f[idx] + nb) / (deg + L.s[idx]);
-  }
-}
-
-template <class T>
-__device__ void smooth_pairs_nm(const NLevel &L, int pairs, bool redFirst, T &team)
-{
-  for (int s = 0; s < pairs; s++) {
-    rb_sweep_nm(L, redFirst ? 0 : 1, team);
-    team.sync();
-    rb_sweep_nm(L, redFirst ? 1 : 0, team);
-    team.sync();
-  }
-}
-
-// t = f - ((deg + s) x - neighbours) at every node.
-template <class T>
-__device__ void residual_nm(const NLevel &L, T &team)
-{
-  const int n1 = L.n + 1, m = n1 * n1 * n1;
-  for (int idx = team.tid; idx < m; idx += team.nth) {
-    int i, j, k;
-    node_ijk(idx, n1, i, j, k);
-    float deg;
-    const float nb = nbr_sum_nm(L.x, idx, i, j, k, L.n, deg);
-    L.t[idx] = L.f[idx] - ((deg + L.s[idx]) * L.x[idx] - nb);
-  }
-}
-
-// fc = (1/2) P^T t at every coarse node over its in-grid fine nodes 2Q + d (dz outer, dx inner); xc = 0.
-template <class T>
-__device__ void restrict_to_nm(const NLevel &F, const NLevel &C, T &team)
-{
-  const int n1 = C.n + 1, m = n1 * n1 * n1, f1 = F.n + 1;
-  for (int idx = team.tid; idx < m; idx += team.nth) {
-    int I, J, K;
-    node_ijk(idx, n1, I, J, K);
-    C.x[idx] = 0.0f;
-    float s = 0.0f;
-    for (int dz = -1; dz <= 1; dz++)
-      for (int dy = -1; dy <= 1; dy++)
-        for (int dx = -1; dx <= 1; dx++) {
-          const int fi = 2 * I + dx, fj = 2 * J + dy, fk = 2 * K + dz;
-          if (fi < 0 || fj < 0 || fk < 0 || fi > F.n || fj > F.n || fk > F.n) continue;
-          const float w = (dx ? 0.5f : 1.0f) * (dy ? 0.5f : 1.0f) * (dz ? 0.5f : 1.0f);
-          s = fmaf(w, F.t[(fk * f1 + fj) * f1 + fi], s);
-        }
-    C.f[idx] = 0.5f * s;
-  }
-}
-
-// x += P xc at every fine node.
-template <class T>
-__device__ void prolong_add_nm(const NLevel &C, const NLevel &F, T &team)
-{
-  const int n1 = F.n + 1, m = n1 * n1 * n1, c1 = C.n + 1;
-  for (int idx = team.tid; idx < m; idx += team.nth) {
-    int i, j, k;
-    node_ijk(idx, n1, i, j, k);
-    float s = 0.0f;
-    for (int bz = 0; bz <= (k & 1); bz++)
-      for (int by = 0; by <= (j & 1); by++)
-        for (int bx = 0; bx <= (i & 1); bx++) {
-          const float w = ((i & 1) ? 0.5f : 1.0f) * ((j & 1) ? 0.5f : 1.0f) * ((k & 1) ? 0.5f : 1.0f);
-          s = fmaf(w, C.x[((k / 2 + bz) * c1 + j / 2 + by) * c1 + i / 2 + bx], s);
-        }
-    F.x[idx] += s;
-  }
-}
-
-template <class T>
-__device__ void v_down_nm(const NLevel *lv, int l, T &team)
-{
-  smooth_pairs_nm(lv[l], NU, true, team);
-  residual_nm(lv[l], team);
-  team.sync();
-  restrict_to_nm(lv[l], lv[l + 1], team);
-  team.sync();
-}
-
-template <class T>
-__device__ void v_up_nm(const NLevel *lv, int l, T &team)
-{
-  prolong_add_nm(lv[l + 1], lv[l], team);
-  team.sync();
-  smooth_pairs_nm(lv[l], NU, false, team);
-}
-
-// v_cycle's schedule on the levels L_l + diag(s_l).
-__device__ void v_cycle_nm(const MeshParams &p, const ScreenParams &sc, GridTeam &grid)
-{
-  const NLevel *lv = sc.lv;
-  const int last = p.levels - 1;
-  int lg = 0;
-  while (lg < last && lv[lg].n > LOCAL_N) lg++;
-  for (int l = 0; l < lg; l++) v_down_nm(lv, l, grid);
-  if (blockIdx.x == 0) {
-    CtaTeam cta{(int)threadIdx.x, (int)blockDim.x};
-    for (int l = lg; l < last; l++) v_down_nm(lv, l, cta);
-    smooth_pairs_nm(lv[last], NU_COARSE, true, cta);
-    smooth_pairs_nm(lv[last], NU_COARSE, false, cta);
-    for (int l = last - 1; l >= lg; l--) v_up_nm(lv, l, cta);
-  }
-  grid.sync();
-  for (int l = lg - 1; l >= 0; l--) v_up_nm(lv, l, grid);
-}
-
 // The trilinear weights B_p of a point at grid coordinates g, at the corners of its cell clamp(floor(g), 0, N - 1)
 // (z outer, x inner) in the splat's form prod (1 - |g_a - q_a|); returns the first corner's node.
 __device__ __forceinline__ int point_weights(const double *g, int N, double w[8])
@@ -746,38 +736,17 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
   if (R.status != 0) return;                           // every CTA reads the same word
   GridTeam grid{cg::this_grid(), (int)(blockIdx.x * MT + threadIdx.x), (int)(gridDim.x * MT)};
   const int N = p.N, n1 = N + 1, M = p.M, used = (int)R.used;
-  float *x = p.chi, *r = p.r, *b = p.b, *z = p.V0, *pp = p.V1, *q = p.V2;
-  auto total1 = [&](int n, double &out) {
-    grid.sync();
-    co_tree_groups<1, MT>(n, p.tilePart, p.groupPart);
-    grid.sync();
-    double t[1];
-    co_tree_total<1, MT>(n, p.groupPart, t);
-    out = t[0];
-  };
-  // chi (or D) trilinear at sorted point s, as the Dirichlet call's tau
-  auto interp = [&](const float *F, int s) {
-    const double *g = p.gs + 3 * (size_t)s;
-    int c[3];
-    double t[3];
-    for (int a = 0; a < 3; a++) {
-      c[a] = min(max((int)floor(g[a]), 0), N - 1);
-      t[a] = g[a] - c[a];
-    }
-    double v = 0.0;
-    for (int bz = 0; bz < 2; bz++)
-      for (int by = 0; by < 2; by++)
-        for (int bx = 0; bx < 2; bx++) {
-          const double w = (bx ? t[0] : 1.0 - t[0]) * (by ? t[1] : 1.0 - t[1]) * (bz ? t[2] : 1.0 - t[2]);
-          v += w * (double)F[((c[2] + bz) * n1 + c[1] + by) * n1 + c[0] + bx];
-        }
-    return v;
+  const float *x = p.chi, *b = p.b;
+  // F trilinear at sorted point s
+  auto at_point = [&](const float *F, int s) {
+    double acc = 0.0;
+    trilinear(p.gs + 3 * (size_t)s, N, n1, [&](double w, int node) { acc += w * (double)F[node]; });
+    return acc;
   };
 
   // omega = alpha / mean density
-  double dsum;
-  co_tree_tiles<1, MT>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(p.D, s); });
-  total1(used, dsum);
+  co_tree_tiles<1, MT>(used, p.tilePart, [&](int s, double *v) { v[0] += at_point(p.D, s); });
+  const double dsum = grid_total(p, used, grid);
   const double omega = sc.alpha / (dsum / used);
   // the screening diagonal of every level: s_l(Q) = (omega / 2^l) sum (B^l_p(Q))^2 at g / 2^l, over the fine cells of
   // Q's support in ascending index (rows of cells as contiguous runs of sorted points)
@@ -819,64 +788,24 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
     }
   }
 
-  double bb, rr, rz = 0.0;
-  co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-    r[i] = b[i];
-    z[i] = 0.0f;
-    v[0] += (double)b[i] * (double)b[i];
-  });
-  total1(M, bb);                                       // (its barrier also completes the diagonals)
-  rr = bb;
-  int k = 0;
-  bool done = rr <= p.tol2 * bb;
-  if (!done) {
-    v_cycle_nm(p, sc, grid);
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-      pp[i] = z[i];
-      v[0] += (double)r[i] * (double)z[i];
-    });
-    total1(M, rz);
-  }
-  while (!done) {
-    grid.sync();                                       // p complete before the point pass and A p read it
-    screen_points(p, sc, pp, omega, used, grid);
-    grid.sync();
-    double pq;
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-      int a, bq, c;
-      node_ijk(i, n1, a, bq, c);
-      float deg;
-      const float nb = nbr_sum_nm(pp, i, a, bq, c, N, deg);
-      const float aq = (deg * pp[i] - nb) + (float)screen_gather(p, sc, a, bq, c);
-      q[i] = aq;
-      v[0] += (double)pp[i] * (double)aq;
-    });
-    total1(M, pq);
-    if (!(pq > 0.0)) break;
-    const double alpha = rz / pq;
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
-      x[i] = (float)((double)x[i] + alpha * (double)pp[i]);
-      const float ri = (float)((double)r[i] - alpha * (double)q[i]);
-      r[i] = ri;
-      z[i] = 0.0f;
-      v[0] += (double)ri * (double)ri;
-    });
-    total1(M, rr);
-    k++;
-    if (rr <= p.tol2 * bb || k >= p.maxIterations) break;
-    v_cycle_nm(p, sc, grid);
-    double rzNew;
-    co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) { v[0] += (double)r[i] * (double)z[i]; });
-    total1(M, rzNew);
-    const double beta = rzNew / rz;
-    rz = rzNew;
-    for (int i = grid.tid; i < M; i += grid.nth) pp[i] = (float)((double)z[i] + beta * (double)pp[i]);
-  }
-  grid.sync();
+  // (mgpcg's first total, b.b, is behind a grid barrier, which also completes the diagonals)
+  double bb, rr;
+  const int k = mgpcg(p, sc.lv, grid,
+                      [&](const float *pp) {
+                        screen_points(p, sc, pp, omega, used, grid);
+                        grid.sync();
+                      },
+                      [&](const float *pp, int i) {
+                        int a, bq, c;
+                        node_ijk(i, n1, a, bq, c);
+                        float deg;
+                        const float nb = nbr_sum_nm(pp, i, a, bq, c, N, deg);
+                        return (deg * pp[i] - nb) + (float)screen_gather(p, sc, a, bq, c);
+                      },
+                      bb, rr);
   // the true residual b - A chi, in float64 from the floats
   screen_points(p, sc, x, omega, used, grid);
   grid.sync();
-  double rt;
   co_tree_tiles<1, MT>(M, p.tilePart, [&](int i, double *v) {
     int a, bq, c;
     node_ijk(i, n1, a, bq, c);
@@ -885,11 +814,10 @@ __global__ void __launch_bounds__(MT) mesh_screened_solve_kernel(MeshParams p, S
     const double e = (double)b[i] - ((deg * (double)x[i] - nb) + screen_gather(p, sc, a, bq, c));
     v[0] += e * e;
   });
-  total1(M, rt);
+  const double rt = grid_total(p, M, grid);
   // tau: chi trilinear at the used points, in sorted order
-  double tsum;
-  co_tree_tiles<1, MT>(used, p.tilePart, [&](int s, double *v) { v[0] += interp(x, s); });
-  total1(used, tsum);
+  co_tree_tiles<1, MT>(used, p.tilePart, [&](int s, double *v) { v[0] += at_point(x, s); });
+  const double tsum = grid_total(p, used, grid);
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     R.info[4] = tsum / used;
     R.info[5] = dsum / used;
