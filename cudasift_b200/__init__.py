@@ -126,6 +126,8 @@ def lib():
                                   c.POINTER(c.c_double)]),
         "cs_texture_mesh": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, c.c_double, c.c_double, c.c_double, ip, ip, ip,
                                  vp, ip, vp, vp, vp, vp, ip, vp, vp, c.POINTER(c.c_double)]),
+        "cs_level_texture_seams": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, c.c_double, c.c_double, ip,
+                                        c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1508,6 +1510,43 @@ def TextureMesh(images, Ks, Rs, ts, vertices, triangles, smoothness=0.5, maxView
                 return img, uv, labels, charts[:C].copy(), info, stats, ms.value
             finally:
                 atlas.free()
+    finally:
+        for b in bufs:
+            b.free()
+
+
+def LevelTextureSeams(vertices, triangles, atlas, uv, labels, charts, padding=2, smoothness=0.1, regularization=1e-3,
+                      maxIterations=1000, tol=1e-4):
+    """Global seam levelling of a textured mesh (cs_level_texture_seams): one additive offset per (vertex, image) pair,
+    solved so that the two sides of every seam agree while the offsets vary smoothly along each chart (smoothness, the
+    weight of those rows; regularization, the pull of every offset towards 0), and added to the atlas texel by texel.
+    The inputs are TextureMesh's outputs as it returns them (padding the value given to it); no image is needed.
+    Returns (levelled atlas float32 [rows, width], corner offsets float32 [T, 3] (NaN for an unseen face), info
+    float64 [3] {seam energy before, after, relative residual}, stats int64 [8] (the header's), ms)."""
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    A = np.ascontiguousarray(np.asarray(atlas, np.float32))
+    U = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 3, 2))
+    Lb = np.ascontiguousarray(np.asarray(labels, np.int32).reshape(-1))
+    Ct = np.ascontiguousarray(np.asarray(charts, np.int32).reshape(-1, 8))
+    V, T, (H, W) = len(X), len(F), A.shape
+    bufs = []
+    try:
+        ins = [DeviceBuffer(max(a.nbytes, 4)) for a in (X, F, Lb, U, A)]
+        bufs += ins
+        for b, a in zip(ins, (X, F, Lb, U, A)):
+            if a.size:
+                b.upload(a)
+        outs = [DeviceBuffer(max(A.nbytes, 4)), DeviceBuffer(12 * T + 4)]
+        bufs += outs
+        info, stats, ms = np.zeros(3), np.zeros(8, np.int64), ctypes.c_double(0.0)
+        _check(lib().cs_level_texture_seams(ins[0].ptr, V, ins[1].ptr, T, ins[2].ptr, ins[3].ptr, _ptr(Ct), len(Ct),
+                                            ins[4].ptr, H, W, int(padding), float(smoothness), float(regularization),
+                                            int(maxIterations), float(tol), outs[0].ptr, outs[1].ptr, _ptr(info),
+                                            _ptr(stats), ctypes.byref(ms)), "LevelTextureSeams")
+        out = outs[0].download(np.float32, H * W).reshape(H, W)
+        off = outs[1].download(np.float32, 3 * T).reshape(T, 3)
+        return out, off, info, stats, ms.value
     finally:
         for b in bufs:
             b.free()

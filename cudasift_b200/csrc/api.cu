@@ -1821,6 +1821,29 @@ int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, con
   });
 }
 
+int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                           const int *d_faceView, const float *d_uv, const int *charts, int numCharts,
+                           const float *d_atlas, int atlasRows, int atlasWidth, int padding, double smoothness,
+                           double regularization, int maxIterations, double tol, float *d_outAtlas,
+                           float *d_cornerOffset, double info_out[3], long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_level_texture_seams";
+  if (ms) *ms = 0.0;
+  int r = seams_args(fn, d_vertices, numVertices, d_triangles, numTriangles, d_faceView, d_uv, charts, numCharts,
+                     d_atlas, atlasRows, atlasWidth, padding, smoothness, regularization, maxIterations, tol,
+                     d_outAtlas, d_cornerOffset);
+  if (r < 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(seams_result_bytes())) < 0) return r;
+  return timed_sync(fn, c, ms, [&] {
+    return seams_run(d_vertices, numVertices, d_triangles, numTriangles, d_faceView, d_uv, charts, numCharts, d_atlas,
+                     atlasRows, atlasWidth, padding, smoothness, regularization, maxIterations, tol, d_outAtlas,
+                     d_cornerOffset, c->stream, c->h_mesh.p, info_out, stats_out);
+  });
+}
+
 int cs_absolute_pose_batch(const double *d_points, int numPoints, const cs_pose_job *jobs, int numJobs,
                            const double *Ks, int numLoops, double maxError, double *R_out, double *t_out,
                            int *counts_out, long long *stats_out, double *ms)

@@ -1105,4 +1105,57 @@ int texture_args(const char *fn, const cs_image *images, int numImages, const do
   return rs.check(fn);
 }
 
+int seams_args(const char *fn, const float *vertices, int numVertices, const int *triangles, int numTriangles,
+               const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
+               int atlasRows, int atlasWidth, int padding, double smoothness, double regularization,
+               int maxIterations, double tol, const float *outAtlas, const float *cornerOffset)
+{
+  if (numVertices < 0 || numVertices > (1 << 30)) return arg_error(fn, "numVertices must be in [0, 2^30]");
+  if (numTriangles < 0 || numTriangles > (1 << 29)) return arg_error(fn, "numTriangles must be in [0, 2^29]");
+  if (atlasRows < 0 || atlasRows > 32768) return arg_error(fn, "atlasRows must be in [0, 32768]");
+  if (atlasWidth < 1 || atlasWidth > 32768) return arg_error(fn, "atlasWidth must be in [1, 32768]");
+  if (padding < 0 || padding > 16) return arg_error(fn, "padding must be in [0, 16]");
+  if (!std::isfinite(smoothness) || smoothness < 0.0) return arg_error(fn, "smoothness must be finite and >= 0");
+  if (!std::isfinite(regularization) || regularization <= 0.0)
+    return arg_error(fn, "regularization must be finite and > 0");
+  if (maxIterations < 0 || maxIterations > 100000) return arg_error(fn, "maxIterations must be in [0, 100000]");
+  if (!(tol >= 0.0 && tol < 1.0)) return arg_error(fn, "tol must be in [0, 1)");
+  if (numCharts < 0) return arg_error(fn, "numCharts must be >= 0");
+  if (numCharts > 0 && !charts) return arg_error(fn, "numCharts > 0 needs charts");
+  for (int c = 0; c < numCharts; c++) {
+    const int *e = charts + 8 * (size_t)c;
+    if (e[0] < 0 || e[3] < 1 || e[4] < 1 || e[5] < 0 || e[6] < 0 || e[3] > atlasWidth - e[5] ||
+        e[4] > atlasRows - e[6])
+      return arg_error(fn, "charts[%d] must have an image >= 0 and a rectangle of at least one texel inside the atlas",
+                       c);
+  }
+  if (numVertices > 0 && (!vertices || misaligned(vertices, 4)))
+    return arg_error(fn, "numVertices > 0 needs d_vertices (4-byte aligned)");
+  if (numTriangles > 0 && (!triangles || misaligned(triangles, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_triangles (4-byte aligned)");
+  if (numTriangles > 0 && (!faceView || misaligned(faceView, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_faceView (4-byte aligned)");
+  if (numTriangles > 0 && (!uv || misaligned(uv, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_uv (4-byte aligned)");
+  if (numTriangles > 0 && (!cornerOffset || misaligned(cornerOffset, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_cornerOffset (4-byte aligned)");
+  const size_t texels = (size_t)atlasRows * atlasWidth;
+  if (texels > 0 && (!atlas || misaligned(atlas, 4))) return arg_error(fn, "atlasRows > 0 needs d_atlas (4-byte aligned)");
+  if (texels > 0 && (!outAtlas || misaligned(outAtlas, 4)))
+    return arg_error(fn, "atlasRows > 0 needs d_outAtlas (4-byte aligned)");
+  // the outputs (written), the mesh, the labels, the coordinates and the atlas (read)
+  static const char *const names[7] = {"d_outAtlas", "d_cornerOffset", "d_vertices", "d_triangles",
+                                       "d_faceView", "d_uv", "d_atlas"};
+  ArgRanges rs(names, 7);
+  const size_t T = (size_t)numTriangles;
+  rs.add(outAtlas, 4 * texels, 0, 0, true);
+  rs.add(cornerOffset, 12 * T, 1, 0, true);
+  rs.add(vertices, 12 * (size_t)numVertices, 2, 0, false);
+  rs.add(triangles, 12 * T, 3, 0, false);
+  rs.add(faceView, 4 * T, 4, 0, false);
+  rs.add(uv, 24 * T, 5, 0, false);
+  rs.add(atlas, 4 * texels, 6, 0, false);
+  return rs.check(fn);
+}
+
 }  // namespace cs

@@ -799,6 +799,16 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
                 cudaStream_t st, void *h_result, double *info, long long *stats);
 size_t texture_result_bytes();
 
+// ---- seam levelling (seams.cu) -------------------------------------------------------------------------------------
+// cs_level_texture_seams after its argument checks, on st with readbacks through h_result (pinned,
+// seams_result_bytes), the scratch allocated and freed on st; fills info (may be NULL) and stats (may be NULL) and
+// returns the unknown count (0 for invalid input).
+int seams_run(const float *vertices, int numVertices, const int *triangles, int numTriangles, const int *faceView,
+              const float *uv, const int *charts, int numCharts, const float *atlas, int atlasRows, int atlasWidth,
+              int padding, double smoothness, double regularization, int maxIterations, double tol, float *outAtlas,
+              float *cornerOffset, cudaStream_t st, void *h_result, double *info, long long *stats);
+size_t seams_result_bytes();
+
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).
 #define VERIFY_ESSENTIAL 3

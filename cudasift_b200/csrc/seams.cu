@@ -1,0 +1,779 @@
+// seams.cu -- global seam levelling of a textured mesh (cs_level_texture_seams) after Lempitsky & Ivanov 2007 as
+// Waechter, Moehrle & Goesele 2014 apply it: one offset per (vertex, label) pair, seam rows that pull the two sides of
+// every seam vertex together and smoothness rows along the edges of each label, their weighted graph Laplacian solved
+// by Jacobi-preconditioned CG in one cooperative kernel, and the offsets added to the atlas texel by texel.  Every
+// rule is stated in cudasift_b200.h at cs_level_texture_seams; tests/seam_oracle.py restates them in float64.  The edge
+// keys, the adjacency and the lower-vertex edge rule are texturing's (trimesh.cuh); the sorted
+// incidences, the per-unknown pieces and the three-level totals are coop.cuh's.
+//
+// Determinism: no floating-point atomics.  Integer atomics only where the result does not depend on their order (the
+// input flag, the 64-bit (distance, face) texel keys, the count of visited texels).  Every floating-point sum has a
+// fixed order: a seam row's samples in k order per edge, then its edges in sorted key order; an unknown's incidences
+// in sorted (row, side) order by coop.cuh's pieces; the totals in coop.cuh's three-level order.  This unit is compiled
+// with -fmad=false so that every float64 product and sum is rounded once, in the order written, as the oracle
+// computes it.
+#include <climits>
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#include <cooperative_groups.h>
+#include <cub/cub.cuh>
+
+#include "common.cuh"
+#include "coop.cuh"
+#include "trimesh.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace cs {
+
+namespace {
+
+constexpr unsigned long long NONE = ~0ull;
+constexpr int SL_PV = 2;                       // an unknown's piece: the sum of w, then b or the neighbours' w p
+
+// The device words of a call; the host reads them after the input check, the counts and the solve.
+struct SeamsResult {
+  unsigned int bad, seen;
+  int unknowns, seamEdges, smoothRows, seamRows;  // copied from the last entries of their scans
+  int iters, converged;
+  unsigned long long texels;
+  double info[3];
+};
+
+// An unknown's sorted incidences [start, end) (coop.cuh's item).
+struct SeamUnk {
+  int start, end;
+};
+
+struct SeamsParams {
+  SeamsResult *res;
+  int V, T;
+  const float *vin;
+  const int *tin, *view;
+  const float *uv, *atlas;
+  float *out, *corner;
+  int rows, width, padding, copyAll;
+  const int *ctab;                            // [C][8] the chart table
+  const int *rowStart, *rowList;              // per atlas row, the charts that cover it by ox
+  int *faceChart;                             // [T]
+  unsigned long long *ekey, *ekeyS, *ukey, *ukeyS, *skeyS;
+  int *eval, *evalS, *uval, *uvalS, *nbr;
+  int *uHead, *uScan, *seFlag, *seScan, *sHead, *sScan, *cornerUnk;
+  unsigned long long *xkey, *xkeyS;           // [2E] seam ends: (g(v, a) << 32) | g(v, b)
+  int *xval, *xvalS, *xHead, *xScan;
+  double *xsum;                               // [2E][3]: sum w I_a, sum w I_b, sum w
+  int *ri, *rj;                               // [R] rows: g_i - g_j = d with weight w
+  double *rw, *rd, *rfa, *rfb;                // rfa, rfb: F_a, F_b of the seam rows
+  int *ikey, *ikeyS, *ival, *ivalS;           // [2R] incidences (unknown; 2 row + side)
+  SeamUnk *unk;
+  double *x, *r, *z, *p, *q, *diag, *b;
+  double *pieces, *partA, *groupA, *partB, *groupB, *partE, *groupE;
+  unsigned long long *tkey;                   // [rows][width] texel keys
+  double smooth, reg, tol2;
+  int maxIt, N, E, Rs, Rm;
+};
+
+// ---- input (rule 1) -----------------------------------------------------------------------------------------------
+// A seen face's chart: the chart of the row index whose rectangle holds floor of corner 0's uv, with the face's label.
+__global__ void __launch_bounds__(MT) seams_check_kernel(SeamsParams p)
+{
+  bool bad = false;
+  unsigned int seen = 0;
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
+    const int l = p.view[f];
+    int ch = -1;
+    if (l >= 0) {
+      const float *u = p.uv + 6 * (size_t)f;
+      bool fin = true;
+      for (int k = 0; k < 6; k++) fin = fin && isfinite(u[k]);
+      const double fx = fin ? floor((double)u[0]) : -1.0, fy = fin ? floor((double)u[1]) : -1.0;
+      if (fx >= 0.0 && fx < (double)p.width && fy >= 0.0 && fy < (double)p.rows) {
+        const int x = (int)fx, y = (int)fy;
+        int lo = p.rowStart[y], hi = p.rowStart[y + 1] - 1;   // the last entry with ox <= x
+        int at = -1;
+        while (lo <= hi) {
+          const int mid = (lo + hi) >> 1;
+          if (p.ctab[8 * (size_t)p.rowList[mid] + 5] <= x) { at = mid; lo = mid + 1; } else hi = mid - 1;
+        }
+        if (at >= 0) {
+          const int c = p.rowList[at];
+          const int *e = p.ctab + 8 * (size_t)c;
+          if (x < e[5] + e[3] && e[0] == l) ch = c;
+        }
+      }
+      bad = bad || ch < 0;
+      seen++;
+    }
+    p.faceChart[f] = ch;
+  }
+  if (bad) atomicOr(&p.res->bad, 1u);
+  if (seen) atomicAdd(&p.res->seen, seen);
+}
+
+// ---- unknowns, adjacency, smoothness rows and seam edges (rules 2-4) ----------------------------------------------
+__global__ void __launch_bounds__(MT) seams_keys_kernel(SeamsParams p)
+{
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
+    p.ekey[c] = edge_key_of(p.tin, c);
+    p.eval[c] = c;
+    p.nbr[c] = -1;
+    const int l = p.view[c / 3];
+    p.ukey[c] = l >= 0 ? ((unsigned long long)(unsigned int)p.tin[c] << 32) | (unsigned int)l : NONE;
+    p.uval[c] = c;
+  }
+}
+
+// texturing's adjacency; the first corner of every distinct (vertex, label) key
+__global__ void __launch_bounds__(MT) seams_adjacency_kernel(SeamsParams p)
+{
+  const int n = 3 * p.T;
+  for (int i = blockIdx.x * MT + threadIdx.x; i < n; i += gridDim.x * MT) {
+    if (i + 1 < n) edge_pair_join(p.ekeyS, p.evalS, p.nbr, i, n);
+    const unsigned long long k = p.ukeyS[i];
+    p.uHead[i] = k != NONE && (i == 0 || p.ukeyS[i - 1] != k);
+  }
+}
+
+// every corner's unknown (-1 for an unseen face); the seam edges at the first of their two sorted positions
+__global__ void __launch_bounds__(MT) seams_unknown_kernel(SeamsParams p)
+{
+  const int n = 3 * p.T;
+  for (int i = blockIdx.x * MT + threadIdx.x; i < n; i += gridDim.x * MT) {
+    p.cornerUnk[p.uvalS[i]] = p.ukeyS[i] != NONE ? p.uScan[i] - 1 : -1;
+    const int c = p.evalS[i], g = p.nbr[c];
+    bool seam = false;
+    if (g >= 0 && (i == 0 || p.ekeyS[i - 1] != p.ekeyS[i])) {
+      const int a = p.view[c / 3], b = p.view[g];
+      seam = a >= 0 && b >= 0 && a != b;
+    }
+    p.seFlag[i] = seam;
+  }
+}
+
+// the smoothness key (min << 32) | max of the two unknowns of every edge of a seen face (rule 4)
+__global__ void __launch_bounds__(MT) seams_smooth_keys_kernel(SeamsParams p)
+{
+  for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
+    const int t = c / 3, k = c - 3 * t;
+    const int a = p.cornerUnk[c], b = p.cornerUnk[3 * t + (k + 1) % 3];
+    p.ukey[c] = a >= 0 ? ((unsigned long long)(unsigned int)min(a, b) << 32) | (unsigned int)max(a, b) : NONE;
+  }
+}
+
+__global__ void __launch_bounds__(MT) seams_smooth_heads_kernel(SeamsParams p)
+{
+  const int n = 3 * p.T;
+  for (int i = blockIdx.x * MT + threadIdx.x; i < n; i += gridDim.x * MT) {
+    const unsigned long long k = p.skeyS[i];
+    p.sHead[i] = k != NONE && (i == 0 || p.skeyS[i - 1] != k);
+  }
+}
+
+// Bilinear read of the atlas at (x, y), texel centres at integers, taps clamped to the chart rectangle e.
+__device__ __forceinline__ double seams_bilinear(const SeamsParams &p, const int *e, double x, double y)
+{
+  const double x0 = floor(x), y0 = floor(y), fx = x - x0, fy = y - y0;
+  const double xl = (double)e[5], xh = (double)(e[5] + e[3] - 1), yl = (double)e[6], yh = (double)(e[6] + e[4] - 1);
+  const int xa = (int)fmin(fmax(x0, xl), xh), xb = (int)fmin(fmax(x0 + 1.0, xl), xh);
+  const int ya = (int)fmin(fmax(y0, yl), yh), yb = (int)fmin(fmax(y0 + 1.0, yl), yh);
+  const float *ra = p.atlas + (size_t)ya * p.width, *rb = p.atlas + (size_t)yb * p.width;
+  const double r0 = (1.0 - fx) * (double)ra[xa] + fx * (double)ra[xb];
+  const double r1 = (1.0 - fx) * (double)rb[xa] + fx * (double)rb[xb];
+  return (1.0 - fy) * r0 + fy * r1;
+}
+
+// the uv of vertex w in face f (one of its corners holds it)
+__device__ __forceinline__ void seams_uv_of(const SeamsParams &p, int f, int w, double &u, double &v, int &corner)
+{
+  int k = 0;
+  while (p.tin[3 * (size_t)f + k] != w) k++;
+  corner = 3 * f + k;
+  u = (double)p.uv[2 * (size_t)corner];
+  v = (double)p.uv[2 * (size_t)corner + 1];
+}
+
+// One thread per seam edge (rule 3): its samples, the partial sums of its two ends and their keys.
+__global__ void __launch_bounds__(MT) seams_sample_kernel(SeamsParams p)
+{
+  const int n = 3 * p.T;
+  for (int i = blockIdx.x * MT + threadIdx.x; i < n; i += gridDim.x * MT) {
+    if (!p.seFlag[i]) continue;
+    const int e = p.seScan[i] - 1;
+    const unsigned long long key = p.ekeyS[i];
+    const int P = (int)(key >> 32), Q = (int)(unsigned int)key;
+    int fs[2] = {p.evalS[i] / 3, p.nbr[p.evalS[i]]};
+    if (p.view[fs[0]] > p.view[fs[1]]) { const int t = fs[0]; fs[0] = fs[1]; fs[1] = t; }   // side 0: label a < b
+    double uP[2], vP[2], uQ[2], vQ[2], len[2];
+    int cP[2], cQ[2];
+    for (int s = 0; s < 2; s++) {
+      seams_uv_of(p, fs[s], P, uP[s], vP[s], cP[s]);
+      seams_uv_of(p, fs[s], Q, uQ[s], vQ[s], cQ[s]);
+      const double du = uQ[s] - uP[s], dv = vQ[s] - vP[s];
+      len[s] = sqrt(du * du + dv * dv);
+    }
+    const int S = (int)fmax(1.0, ceil(fmax(len[0], len[1])));
+    const int *ea = p.ctab + 8 * (size_t)p.faceChart[fs[0]], *eb = p.ctab + 8 * (size_t)p.faceChart[fs[1]];
+    double sum[2][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
+    for (int k = 0; k < S; k++) {
+      const double t = ((double)k + 0.5) / (double)S;
+      const double Ia = seams_bilinear(p, ea, uP[0] + t * (uQ[0] - uP[0]), vP[0] + t * (vQ[0] - vP[0]));
+      const double Ib = seams_bilinear(p, eb, uP[1] + t * (uQ[1] - uP[1]), vP[1] + t * (vQ[1] - vP[1]));
+      const double w[2] = {1.0 - t, t};
+      for (int end = 0; end < 2; end++) {
+        sum[end][0] = sum[end][0] + w[end] * Ia;
+        sum[end][1] = sum[end][1] + w[end] * Ib;
+        sum[end][2] = sum[end][2] + w[end];
+      }
+    }
+    for (int end = 0; end < 2; end++) {
+      const int j = 2 * e + end;
+      const unsigned int ga = (unsigned int)p.cornerUnk[end ? cQ[0] : cP[0]],
+                         gb = (unsigned int)p.cornerUnk[end ? cQ[1] : cP[1]];
+      p.xkey[j] = ((unsigned long long)ga << 32) | gb;
+      p.xval[j] = j;
+      for (int m = 0; m < 3; m++) p.xsum[3 * (size_t)j + m] = sum[end][m];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(MT) seams_row_heads_kernel(SeamsParams p)
+{
+  const int n = 2 * p.E;
+  for (int j = blockIdx.x * MT + threadIdx.x; j < n; j += gridDim.x * MT)
+    p.xHead[j] = j == 0 || p.xkeyS[j - 1] != p.xkeyS[j];
+}
+
+// The rows (rule 5): seam rows at [0, Rs) in (g_a, g_b) order, each the sum of its ends' partials in sorted edge order;
+// smoothness rows at [Rs, Rs + Rm) in key order.  Every row's two incidences.
+__global__ void __launch_bounds__(MT) seams_rows_kernel(SeamsParams p)
+{
+  const int n2 = 2 * p.E, n3 = 3 * p.T;
+  for (int j = blockIdx.x * MT + threadIdx.x; j < n2 + n3; j += gridDim.x * MT) {
+    int r, gi, gj;
+    double w, d;
+    if (j < n2) {
+      if (!p.xHead[j]) continue;
+      r = p.xScan[j] - 1;
+      const unsigned long long key = p.xkeyS[j];
+      double s[3] = {0.0, 0.0, 0.0};
+      for (int m = j; m < n2 && p.xkeyS[m] == key; m++)
+        for (int c = 0; c < 3; c++) s[c] = s[c] + p.xsum[3 * (size_t)p.xvalS[m] + c];
+      const double Fa = s[0] / s[2], Fb = s[1] / s[2];
+      gi = (int)(key >> 32);
+      gj = (int)(unsigned int)key;
+      w = 1.0;
+      d = Fb - Fa;
+      p.rfa[r] = Fa;
+      p.rfb[r] = Fb;
+    } else {
+      const int i = j - n2;
+      if (!p.sHead[i]) continue;
+      r = p.Rs + p.sScan[i] - 1;
+      const unsigned long long key = p.skeyS[i];
+      gi = (int)(key >> 32);
+      gj = (int)(unsigned int)key;
+      w = p.smooth;
+      d = 0.0;
+    }
+    p.ri[r] = gi;
+    p.rj[r] = gj;
+    p.rw[r] = w;
+    p.rd[r] = d;
+    p.ikey[2 * r] = gi;
+    p.ival[2 * r] = 2 * r;
+    p.ikey[2 * r + 1] = gj;
+    p.ival[2 * r + 1] = 2 * r + 1;
+  }
+}
+
+// ---- the solve (rule 6) -------------------------------------------------------------------------------------------
+// The seam energy term of seam row r at offsets g (0 when g is null).
+__device__ __forceinline__ double seams_energy(const SeamsParams &p, int r, const double *g)
+{
+  const double e = (p.rfa[r] + (g ? g[p.ri[r]] : 0.0)) - (p.rfb[r] + (g ? g[p.rj[r]] : 0.0));
+  return e * e;
+}
+
+__global__ void __launch_bounds__(MT) seams_solve_kernel(SeamsParams p)
+{
+  cg::grid_group grid = cg::this_grid();
+  const int tid = (int)(blockIdx.x * MT + threadIdx.x), nthreads = (int)gridDim.x * MT;
+  const int N = p.N, R = p.Rs + p.Rm, n = 2 * R;
+
+  // 0. every unknown's sorted incidences; its pieces of the diagonal and of b
+  co_ranges(p.ikeyS, n, p.unk, tid, nthreads);
+  grid.sync();
+  co_pieces<2, 0, SL_PV, MT>(p.ikeyS, p.ivalS, p.pieces, n, p.unk, [&](int code, int, double *v) {
+    const int r = code >> 1;
+    const double wd = p.rw[r] * p.rd[r];
+    v[0] = p.rw[r];
+    v[1] = (code & 1) ? -wd : wd;
+  });
+  grid.sync();
+  // 1. per unknown: diag = sum w + reg, b, x = 0, r = b, z = r / diag, p = 0; the totals of b.b and r.z; the seam
+  // energy before
+  co_tree_tiles<2, MT>(N, p.partA, [&](int i, double *v) {
+    double G[2];
+    co_gather<2, 0, SL_PV>(p.pieces, i, p.unk[i], G);
+    const double dg = G[0] + p.reg, rv = G[1], zv = rv / dg;
+    p.diag[i] = dg;
+    p.b[i] = rv;
+    p.x[i] = 0.0;
+    p.r[i] = rv;
+    p.z[i] = zv;
+    p.p[i] = 0.0;
+    v[0] += rv * rv;
+    v[1] += rv * zv;
+  });
+  co_tree_tiles<1, MT>(p.Rs, p.partE, [&](int r, double *v) { v[0] += seams_energy(p, r, nullptr); });
+  grid.sync();
+  co_tree_groups<2, MT>(N, p.partA, p.groupA);
+  co_tree_groups<1, MT>(p.Rs, p.partE, p.groupE);
+  grid.sync();
+  double t2[2], t1[1], e0[1];
+  co_tree_total<2, MT>(N, p.groupA, t2);
+  co_tree_total<1, MT>(p.Rs, p.groupE, e0);
+  const double bb = t2[0], thr = p.tol2 * bb;
+  double rr = t2[0], rz = t2[1], beta = 0.0;
+  int it = 0;
+  while (it < p.maxIt && !(rr <= thr)) {
+    // 2. the pieces of sum w p_other, p = z + beta p_old of the other unknown
+    co_pieces<1, 1, SL_PV, MT>(p.ikeyS, p.ivalS, p.pieces, n, p.unk, [&](int code, int, double *v) {
+      const int r = code >> 1, o = (code & 1) ? p.ri[r] : p.rj[r];
+      v[0] = p.rw[r] * (p.z[o] + beta * p.p[o]);
+    });
+    grid.sync();
+    // 3. p = z + beta p_old, q = A p = diag p - sum w p_other; the total of p.q
+    co_tree_tiles<1, MT>(N, p.partB, [&](int i, double *v) {
+      double Wp[1];
+      co_gather<1, 1, SL_PV>(p.pieces, i, p.unk[i], Wp);
+      const double pn = p.z[i] + beta * p.p[i], qv = p.diag[i] * pn - Wp[0];
+      p.p[i] = pn;
+      p.q[i] = qv;
+      v[0] += pn * qv;
+    });
+    grid.sync();
+    co_tree_groups<1, MT>(N, p.partB, p.groupB);
+    grid.sync();
+    co_tree_total<1, MT>(N, p.groupB, t1);
+    if (!(t1[0] > 0.0)) break;
+    const double alpha = rz / t1[0];
+    // 4. x += alpha p, r -= alpha q, z = r / diag; the totals of r.r and r.z
+    co_tree_tiles<2, MT>(N, p.partA, [&](int i, double *v) {
+      p.x[i] = p.x[i] + alpha * p.p[i];
+      const double rv = p.r[i] - alpha * p.q[i], zv = rv / p.diag[i];
+      p.r[i] = rv;
+      p.z[i] = zv;
+      v[0] += rv * rv;
+      v[1] += rv * zv;
+    });
+    it++;
+    grid.sync();
+    co_tree_groups<2, MT>(N, p.partA, p.groupA);
+    grid.sync();
+    co_tree_total<2, MT>(N, p.groupA, t2);
+    rr = t2[0];
+    beta = t2[1] / rz;
+    rz = t2[1];
+  }
+  // 5. the true residual b - A x and the seam energy after; the corner offsets
+  co_pieces<1, 1, SL_PV, MT>(p.ikeyS, p.ivalS, p.pieces, n, p.unk, [&](int code, int, double *v) {
+    const int r = code >> 1, o = (code & 1) ? p.ri[r] : p.rj[r];
+    v[0] = p.rw[r] * p.x[o];
+  });
+  for (int c = tid; c < 3 * p.T; c += nthreads) {
+    const int g = p.cornerUnk[c];
+    p.corner[c] = g >= 0 ? __double2float_rn(p.x[g]) : __int_as_float(0x7fc00000);
+  }
+  grid.sync();
+  co_tree_tiles<1, MT>(N, p.partB, [&](int i, double *v) {
+    double Wx[1];
+    co_gather<1, 1, SL_PV>(p.pieces, i, p.unk[i], Wx);
+    const double res = p.b[i] - (p.diag[i] * p.x[i] - Wx[0]);
+    v[0] += res * res;
+  });
+  co_tree_tiles<1, MT>(p.Rs, p.partE, [&](int r, double *v) { v[0] += seams_energy(p, r, p.x); });
+  grid.sync();
+  co_tree_groups<1, MT>(N, p.partB, p.groupB);
+  co_tree_groups<1, MT>(p.Rs, p.partE, p.groupE);
+  grid.sync();
+  double e1[1];
+  co_tree_total<1, MT>(N, p.groupB, t1);
+  co_tree_total<1, MT>(p.Rs, p.groupE, e1);
+  if (tid == 0) {
+    p.res->iters = it;
+    p.res->converged = rr <= thr;
+    p.res->info[0] = e0[0];
+    p.res->info[1] = e1[0];
+    p.res->info[2] = bb > 0.0 ? sqrt(t1[0] / bb) : 0.0;
+  }
+}
+
+// ---- texels (rule 7) ----------------------------------------------------------------------------------------------
+// The squared distance from (X, Y) to face f's uv triangle and the barycentric weights of the closest point: inside by
+// the lower-vertex edge rule (distance 0), else the nearest of the three segments (ties to the lower edge).
+__device__ __forceinline__ double seams_closest(const SeamsParams &p, int f, double X, double Y, double (&bw)[3])
+{
+  int id[3];
+  double u[3], v[3];
+  for (int k = 0; k < 3; k++) {
+    id[k] = p.tin[3 * (size_t)f + k];
+    u[k] = (double)p.uv[6 * (size_t)f + 2 * k];
+    v[k] = (double)p.uv[6 * (size_t)f + 2 * k + 1];
+  }
+  const double A = (u[1] - u[0]) * (v[2] - v[0]) - (v[1] - v[0]) * (u[2] - u[0]);
+  if (A != 0.0) {
+    EdgeFns ef;
+    edge_fns_of(id, u, v, A > 0.0 ? 1.0 : -1.0, ef);
+    double w[3];
+    bool in = true;
+    for (int k = 0; k < 3 && in; k++) {
+      w[k] = edge_fn(ef, u, v, k, X, Y);
+      in = w[k] >= 0.0;
+    }
+    if (in) {
+      const double S = (w[0] + w[1]) + w[2];
+      if (S > 0.0) {
+        bw[0] = w[1] / S;
+        bw[1] = w[2] / S;
+        bw[2] = w[0] / S;
+        return 0.0;
+      }
+    }
+  }
+  double best = INFINITY;
+  for (int k = 0; k < 3; k++) {
+    const int k1 = (k + 1) % 3;
+    const double dx = u[k1] - u[k], dy = v[k1] - v[k], l2 = dx * dx + dy * dy;
+    const double t = l2 > 0.0 ? fmin(fmax(((X - u[k]) * dx + (Y - v[k]) * dy) / l2, 0.0), 1.0) : 0.0;
+    const double ex = X - (u[k] + t * dx), ey = Y - (v[k] + t * dy), d2 = ex * ex + ey * ey;
+    if (d2 < best) {
+      best = d2;
+      bw[k] = 1.0 - t;
+      bw[k1] = t;
+      bw[(k + 2) % 3] = 0.0;
+    }
+  }
+  return best;
+}
+
+// One thread per seen face: every texel of its chart rectangle inside its uv box grown by padding + 1 gets atomicMin
+// of (float(distance) bits << 32) | face.
+__global__ void __launch_bounds__(MT) seams_raster_kernel(SeamsParams p)
+{
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
+    if (p.view[f] < 0) continue;
+    const int *e = p.ctab + 8 * (size_t)p.faceChart[f];
+    const float *u = p.uv + 6 * (size_t)f;
+    const double g = (double)(p.padding + 1);
+    const double xlo = fmax((double)e[5], floor(fmin(fmin((double)u[0], (double)u[2]), (double)u[4])) - g);
+    const double xhi = fmin((double)(e[5] + e[3] - 1), ceil(fmax(fmax((double)u[0], (double)u[2]), (double)u[4])) + g);
+    const double ylo = fmax((double)e[6], floor(fmin(fmin((double)u[1], (double)u[3]), (double)u[5])) - g);
+    const double yhi = fmin((double)(e[6] + e[4] - 1), ceil(fmax(fmax((double)u[1], (double)u[3]), (double)u[5])) + g);
+    for (int y = (int)ylo; y <= (int)yhi; y++)
+      for (int x = (int)xlo; x <= (int)xhi; x++) {
+        double bw[3];
+        const float d = __double2float_rn(sqrt(seams_closest(p, f, (double)x, (double)y, bw)));
+        atomicMin(p.tkey + (size_t)y * p.width + x, ((unsigned long long)__float_as_uint(d) << 32) | (unsigned int)f);
+      }
+  }
+}
+
+// One thread per atlas texel: atlas + the winning face's interpolated corner offset (rounded to float), or a copy.
+__global__ void __launch_bounds__(MT) seams_texel_kernel(SeamsParams p)
+{
+  const long long n = (long long)p.rows * p.width;
+  unsigned long long visited = 0;
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < n; i += (long long)gridDim.x * MT) {
+    const unsigned long long key = p.tkey[i];
+    const float a = p.atlas[i];
+    if (key == NONE) { p.out[i] = a; continue; }
+    visited++;
+    if (p.copyAll) { p.out[i] = a; continue; }
+    const int f = (int)(unsigned int)key, y = (int)(i / p.width), x = (int)(i - (long long)y * p.width);
+    double bw[3];
+    seams_closest(p, f, (double)x, (double)y, bw);
+    const float *o = p.corner + 3 * (size_t)f;
+    const double off = (bw[0] * (double)o[0] + bw[1] * (double)o[1]) + bw[2] * (double)o[2];
+    p.out[i] = __fadd_rn(a, __double2float_rn(off));
+  }
+  if (visited) atomicAdd(&p.res->texels, visited);
+}
+
+}  // namespace
+
+int seams_run(const float *vin, int V, const int *tin, int T, const int *faceView, const float *uv, const int *charts,
+              int numCharts, const float *atlas, int atlasRows, int atlasWidth, int padding, double smoothness,
+              double regularization, int maxIterations, double tol, float *outAtlas, float *cornerOffset,
+              cudaStream_t st, void *h_res, double *info, long long *stats)
+{
+  const size_t atlasBytes = (size_t)atlasRows * atlasWidth * 4;
+  long long st_[8] = {};
+  double info_[3] = {};
+  auto finish = [&](int status) {
+    st_[7] = status;
+    if (info)
+      for (int k = 0; k < 3; k++) info[k] = status == 2 ? 0.0 : info_[k];
+    if (stats)
+      for (int k = 0; k < 8; k++) stats[k] = st_[k];
+  };
+  if (T == 0) {                                // no face: no seam row, the atlas copied
+    if (atlasBytes) CS_CUDA(cudaMemcpyAsync(outAtlas, atlas, atlasBytes, cudaMemcpyDeviceToDevice, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    finish(1);
+    return 0;
+  }
+
+  // the row index of the chart table: per atlas row, the charts that cover it by (ox, index)
+  std::vector<int> rowStart((size_t)atlasRows + 1, 0), rowList;
+  for (int c = 0; c < numCharts; c++)
+    for (int y = charts[8 * (size_t)c + 6]; y < charts[8 * (size_t)c + 6] + charts[8 * (size_t)c + 4]; y++)
+      rowStart[y + 1]++;
+  for (int y = 0; y < atlasRows; y++) rowStart[y + 1] += rowStart[y];
+  rowList.resize(std::max(1, rowStart[atlasRows]));
+  {
+    std::vector<int> order(numCharts), fill(rowStart.begin(), rowStart.end() - 1);
+    for (int c = 0; c < numCharts; c++) order[c] = c;
+    std::stable_sort(order.begin(), order.end(),
+                     [&](int a, int b) { return charts[8 * (size_t)a + 5] < charts[8 * (size_t)b + 5]; });
+    for (int c : order)
+      for (int y = charts[8 * (size_t)c + 6]; y < charts[8 * (size_t)c + 6] + charts[8 * (size_t)c + 4]; y++)
+        rowList[fill[y]++] = c;
+  }
+
+  const size_t C3 = 3 * (size_t)T, E2 = C3, R2 = 2 * (2 * C3);   // seam ends <= 3T, rows <= 2 (3T)
+  size_t tb[4] = {};
+  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (unsigned long long *)nullptr,
+                                          (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, (int)C3, 0,
+                                          64, st));
+  CS_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb[1], (unsigned long long *)nullptr,
+                                         (unsigned long long *)nullptr, (int)C3, 0, 64, st));
+  CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb[2], (int *)nullptr, (int *)nullptr, (int)C3, st));
+  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[3], (int *)nullptr, (int *)nullptr, (int *)nullptr,
+                                          (int *)nullptr, (int)R2, 0, 32, st));
+  const size_t tempBytes = std::max(std::max(tb[0], tb[1]), std::max(tb[2], tb[3]));
+  const int tiles3 = (int)((C3 + CO_TREE_TILE - 1) / CO_TREE_TILE), groups3 = (tiles3 + MT - 1) / MT;
+
+  Layout L(256);
+  const size_t resAt = L.take(sizeof(SeamsResult));
+  const size_t ctabAt = L.take(std::max(1, numCharts) * 32ull), rsAt = L.take(rowStart.size() * 4),
+               rlAt = L.take(rowList.size() * 4);
+  const size_t fcAt = L.take((size_t)T * 4);
+  const size_t ekAt = L.take(C3 * 8), ekSAt = L.take(C3 * 8), ukAt = L.take(C3 * 8), ukSAt = L.take(C3 * 8),
+               skSAt = L.take(C3 * 8);
+  const size_t evAt = L.take(C3 * 4), evSAt = L.take(C3 * 4), uvAt = L.take(C3 * 4), uvSAt = L.take(C3 * 4),
+               nbrAt = L.take(C3 * 4);
+  const size_t uhAt = L.take(C3 * 4), usAt = L.take(C3 * 4), sfAt = L.take(C3 * 4), ssAt = L.take(C3 * 4),
+               shAt = L.take(C3 * 4), shsAt = L.take(C3 * 4), cuAt = L.take(C3 * 4);
+  const size_t xkAt = L.take(E2 * 8), xkSAt = L.take(E2 * 8), xvAt = L.take(E2 * 4), xvSAt = L.take(E2 * 4),
+               xhAt = L.take(E2 * 4), xsAt = L.take(E2 * 4), xsumAt = L.take(E2 * 24);
+  const size_t Rmax = 2 * C3;                 // seam rows <= seam ends, smoothness rows <= corners
+  const size_t riAt = L.take(Rmax * 4), rjAt = L.take(Rmax * 4), rwAt = L.take(Rmax * 8), rdAt = L.take(Rmax * 8),
+               rfaAt = L.take(C3 * 8), rfbAt = L.take(C3 * 8);
+  const size_t ikAt = L.take(R2 * 4), ikSAt = L.take(R2 * 4), ivAt = L.take(R2 * 4), ivSAt = L.take(R2 * 4);
+  const size_t unkAt = L.take(C3 * sizeof(SeamUnk));
+  const size_t vecAt = L.take(7 * C3 * 8);
+  const size_t piecesAt = L.take(((R2 + CO_TILE - 1) / CO_TILE + C3) * SL_PV * 8);
+  const size_t partAAt = L.take((size_t)tiles3 * 16), groupAAt = L.take((size_t)groups3 * 16),
+               partBAt = L.take((size_t)tiles3 * 8), groupBAt = L.take((size_t)groups3 * 8),
+               partEAt = L.take((size_t)tiles3 * 8), groupEAt = L.take((size_t)groups3 * 8);
+  const size_t tkeyAt = L.take(atlasBytes * 2);
+  const size_t tempAt = L.take(tempBytes);
+  char *base = nullptr;
+  CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
+  auto at = [&](size_t off) { return base + off; };
+
+  SeamsParams p{};
+  p.res = reinterpret_cast<SeamsResult *>(at(resAt));
+  p.V = V;
+  p.T = T;
+  p.vin = vin;
+  p.tin = tin;
+  p.view = faceView;
+  p.uv = uv;
+  p.atlas = atlas;
+  p.out = outAtlas;
+  p.corner = cornerOffset;
+  p.rows = atlasRows;
+  p.width = atlasWidth;
+  p.padding = padding;
+  p.ctab = reinterpret_cast<const int *>(at(ctabAt));
+  p.rowStart = reinterpret_cast<const int *>(at(rsAt));
+  p.rowList = reinterpret_cast<const int *>(at(rlAt));
+  p.faceChart = reinterpret_cast<int *>(at(fcAt));
+  p.ekey = reinterpret_cast<unsigned long long *>(at(ekAt));
+  p.ekeyS = reinterpret_cast<unsigned long long *>(at(ekSAt));
+  p.ukey = reinterpret_cast<unsigned long long *>(at(ukAt));
+  p.ukeyS = reinterpret_cast<unsigned long long *>(at(ukSAt));
+  p.skeyS = reinterpret_cast<unsigned long long *>(at(skSAt));
+  p.eval = reinterpret_cast<int *>(at(evAt));
+  p.evalS = reinterpret_cast<int *>(at(evSAt));
+  p.uval = reinterpret_cast<int *>(at(uvAt));
+  p.uvalS = reinterpret_cast<int *>(at(uvSAt));
+  p.nbr = reinterpret_cast<int *>(at(nbrAt));
+  p.uHead = reinterpret_cast<int *>(at(uhAt));
+  p.uScan = reinterpret_cast<int *>(at(usAt));
+  p.seFlag = reinterpret_cast<int *>(at(sfAt));
+  p.seScan = reinterpret_cast<int *>(at(ssAt));
+  p.sHead = reinterpret_cast<int *>(at(shAt));
+  p.sScan = reinterpret_cast<int *>(at(shsAt));
+  p.cornerUnk = reinterpret_cast<int *>(at(cuAt));
+  p.xkey = reinterpret_cast<unsigned long long *>(at(xkAt));
+  p.xkeyS = reinterpret_cast<unsigned long long *>(at(xkSAt));
+  p.xval = reinterpret_cast<int *>(at(xvAt));
+  p.xvalS = reinterpret_cast<int *>(at(xvSAt));
+  p.xHead = reinterpret_cast<int *>(at(xhAt));
+  p.xScan = reinterpret_cast<int *>(at(xsAt));
+  p.xsum = reinterpret_cast<double *>(at(xsumAt));
+  p.ri = reinterpret_cast<int *>(at(riAt));
+  p.rj = reinterpret_cast<int *>(at(rjAt));
+  p.rw = reinterpret_cast<double *>(at(rwAt));
+  p.rd = reinterpret_cast<double *>(at(rdAt));
+  p.rfa = reinterpret_cast<double *>(at(rfaAt));
+  p.rfb = reinterpret_cast<double *>(at(rfbAt));
+  p.ikey = reinterpret_cast<int *>(at(ikAt));
+  p.ikeyS = reinterpret_cast<int *>(at(ikSAt));
+  p.ival = reinterpret_cast<int *>(at(ivAt));
+  p.ivalS = reinterpret_cast<int *>(at(ivSAt));
+  p.unk = reinterpret_cast<SeamUnk *>(at(unkAt));
+  double *vec = reinterpret_cast<double *>(at(vecAt));
+  p.x = vec;
+  p.r = vec + C3;
+  p.z = vec + 2 * C3;
+  p.p = vec + 3 * C3;
+  p.q = vec + 4 * C3;
+  p.diag = vec + 5 * C3;
+  p.b = vec + 6 * C3;
+  p.pieces = reinterpret_cast<double *>(at(piecesAt));
+  p.partA = reinterpret_cast<double *>(at(partAAt));
+  p.groupA = reinterpret_cast<double *>(at(groupAAt));
+  p.partB = reinterpret_cast<double *>(at(partBAt));
+  p.groupB = reinterpret_cast<double *>(at(groupBAt));
+  p.partE = reinterpret_cast<double *>(at(partEAt));
+  p.groupE = reinterpret_cast<double *>(at(groupEAt));
+  p.tkey = reinterpret_cast<unsigned long long *>(at(tkeyAt));
+  p.smooth = smoothness;
+  p.reg = regularization;
+  p.tol2 = tol * tol;
+  p.maxIt = maxIterations;
+  void *temp = at(tempAt);
+  size_t tempB = tempBytes;
+  SeamsResult &R = *static_cast<SeamsResult *>(h_res);
+  cudaEvent_t *tev = match_timing_events();
+  const int n3 = (int)C3;
+
+  int status = 0;
+  auto readback = [&]() -> int {
+    CS_CUDA(cudaMemcpyAsync(h_res, p.res, sizeof(SeamsResult), cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  // the count of a flag list: the last entry of its inclusive scan, into a result word
+  auto last = [&](int *word, const int *scan, int n) -> int {
+    if (n > 0) CS_CUDA(cudaMemcpyAsync(word, scan + n - 1, 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  };
+  auto run = [&]() -> int {
+    int r;
+    if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
+    CS_CUDA(cudaMemsetAsync(p.res, 0, sizeof(SeamsResult), st));
+    if (numCharts)
+      CS_CUDA(cudaMemcpyAsync(at(ctabAt), charts, (size_t)numCharts * 32, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(at(rsAt), rowStart.data(), rowStart.size() * 4, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(at(rlAt), rowList.data(), rowList.size() * 4, cudaMemcpyHostToDevice, st));
+    mesh_validate_kernel<<<grid_of(T), MT, 0, st>>>(vin, V, tin, T, &p.res->bad);
+    seams_check_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if ((r = readback()) < 0) return r;
+    if (R.bad) {
+      status = 2;
+      return 0;
+    }
+    // unknowns, adjacency, smoothness rows, seam edges
+    if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
+    seams_keys_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ekey, p.ekeyS, p.eval, p.evalS, n3, 0, 64, st));
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ukey, p.ukeyS, p.uval, p.uvalS, n3, 0, 64, st));
+    seams_adjacency_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.uHead, p.uScan, n3, st));
+    seams_unknown_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.seFlag, p.seScan, n3, st));
+    seams_smooth_keys_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortKeys(temp, tempB, p.ukey, p.skeyS, n3, 0, 64, st));
+    seams_smooth_heads_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.sHead, p.sScan, n3, st));
+    count_launch(5);
+    CS_CUDA(cudaGetLastError());
+    if ((r = last(&p.res->unknowns, p.uScan, n3)) < 0) return r;
+    if ((r = last(&p.res->seamEdges, p.seScan, n3)) < 0) return r;
+    if ((r = last(&p.res->smoothRows, p.sScan, n3)) < 0) return r;
+    if ((r = readback()) < 0) return r;
+    p.N = R.unknowns;
+    p.E = R.seamEdges;
+    p.Rm = R.smoothRows;
+    // the seam rows
+    if (tev) CS_CUDA(cudaEventRecord(tev[2], st));
+    seams_sample_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.xkey, p.xkeyS, p.xval, p.xvalS, 2 * p.E, 0, 64, st));
+    seams_row_heads_kernel<<<grid_of(2ll * p.E), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.xHead, p.xScan, 2 * p.E, st));
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if ((r = last(&p.res->seamRows, p.xScan, 2 * p.E)) < 0) return r;
+    if ((r = readback()) < 0) return r;
+    p.Rs = R.seamRows;
+    p.copyAll = p.Rs == 0;
+    const int nInc = 2 * (p.Rs + p.Rm);
+    seams_rows_kernel<<<grid_of(2ll * p.E + 3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ikey, p.ikeyS, p.ival, p.ivalS, nInc, 0,
+                                            radix_bits(std::max(0, p.N - 1)), st));
+    CS_CUDA(cudaMemsetAsync(p.unk, 0, (size_t)p.N * sizeof(SeamUnk), st));
+    count_launch();
+    CS_CUDA(cudaGetLastError());
+    // the solve
+    if (tev) CS_CUDA(cudaEventRecord(tev[3], st));
+    const int wave = coop_grid<seams_solve_kernel, MT>("cs_level_texture_seams");
+    if (wave < 0) return wave;
+    void *args[] = {&p};
+    CS_CUDA(cudaLaunchCooperativeKernel((const void *)seams_solve_kernel, dim3(wave), dim3(MT), args, 0, st));
+    count_launch();
+    // the texels
+    if (tev) CS_CUDA(cudaEventRecord(tev[4], st));
+    CS_CUDA(cudaMemsetAsync(p.tkey, 0xff, atlasBytes * 2, st));
+    seams_raster_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    seams_texel_kernel<<<grid_of((long long)atlasRows * atlasWidth), MT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if (tev) CS_CUDA(cudaEventRecord(tev[5], st));
+    if ((r = readback()) < 0) return r;
+    status = p.Rs == 0 ? 1 : R.converged ? 0 : 3;
+    if (tev) {
+      static const char *const names[5] = {"check", "unknowns", "seam rows", "solve", "texels"};
+      report_stage_times(tev, names, 5, "seams timing faces=%d unknowns=%d rows=%d iterations=%d", T, p.N,
+                         p.Rs + p.Rm, R.iters);
+    }
+    return 0;
+  };
+  const int r = run();
+  cudaFreeAsync(base, st);
+  if (r < 0) return r;
+  if (status != 2) {
+    st_[0] = R.seen;
+    st_[1] = R.unknowns;
+    st_[2] = R.seamEdges;
+    st_[3] = R.seamRows;
+    st_[4] = R.smoothRows;
+    st_[5] = R.iters;
+    st_[6] = (long long)R.texels;
+    for (int k = 0; k < 3; k++) info_[k] = R.info[k];
+  }
+  finish(status);
+  return status == 2 ? 0 : R.unknowns;
+}
+
+size_t seams_result_bytes() { return sizeof(SeamsResult); }
+
+}  // namespace cs

@@ -96,9 +96,7 @@ __device__ __forceinline__ double area2_of(const double *u, const double *v)
 __global__ void __launch_bounds__(MT) texture_edges_kernel(TextureParams p)
 {
   for (int c = blockIdx.x * MT + threadIdx.x; c < 3 * p.T; c += gridDim.x * MT) {
-    const int t = c / 3, k = c - 3 * t;
-    const unsigned int a = p.tin[c], b = p.tin[3 * t + (k + 1) % 3];
-    p.ekey[c] = ((unsigned long long)min(a, b) << 32) | max(a, b);
+    p.ekey[c] = edge_key_of(p.tin, c);
     p.eval[c] = c;
     p.nbr[c] = -1;
   }
@@ -109,11 +107,7 @@ __global__ void __launch_bounds__(MT) texture_adjacency_kernel(TextureParams p)
 {
   const int n = 3 * p.T;
   for (int i = blockIdx.x * MT + threadIdx.x; i + 1 < n; i += gridDim.x * MT) {
-    const unsigned long long k = p.ekeyS[i];
-    if ((i > 0 && p.ekeyS[i - 1] == k) || p.ekeyS[i + 1] != k || (i + 2 < n && p.ekeyS[i + 2] == k)) continue;
-    const int c1 = p.evalS[i], c2 = p.evalS[i + 1];
-    p.nbr[c1] = c2 / 3;
-    p.nbr[c2] = c1 / 3;
+    edge_pair_join(p.ekeyS, p.evalS, p.nbr, i, n);
   }
 }
 
@@ -141,24 +135,14 @@ __global__ void __launch_bounds__(MT) texture_raster_kernel(TextureParams p)
     const double xlo = fmax(0.0, ceil(fmin(fmin(u[0], u[1]), u[2]))), xhi = fmin(c.W - 1.0, floor(fmax(fmax(u[0], u[1]), u[2])));
     const double ylo = fmax(0.0, ceil(fmin(fmin(v[0], v[1]), v[2]))), yhi = fmin(c.H - 1.0, floor(fmax(fmax(v[0], v[1]), v[2])));
     if (!(xlo <= xhi && ylo <= yhi)) continue;
-    // edge k runs corner k -> k + 1; it is evaluated from its lower vertex id P to the higher Q, then signed
-    int P[3];
-    double du[3], dv[3], sg[3];
-    for (int k = 0; k < 3; k++) {
-      const int a = k, b = (k + 1) % 3;
-      const bool lo = id[a] < id[b];
-      P[k] = lo ? a : b;
-      const int Q = lo ? b : a;
-      du[k] = u[Q] - u[P[k]];
-      dv[k] = v[Q] - v[P[k]];
-      sg[k] = lo ? s : -s;
-    }
+    EdgeFns ef;
+    edge_fns_of(id, u, v, s, ef);
     for (int y = (int)ylo; y <= (int)yhi; y++)
       for (int x = (int)xlo; x <= (int)xhi; x++) {
         double w[3];
         bool in = true;
         for (int k = 0; k < 3 && in; k++) {
-          w[k] = sg[k] * (du[k] * ((double)y - v[P[k]]) - dv[k] * ((double)x - u[P[k]]));
+          w[k] = edge_fn(ef, u, v, k, (double)x, (double)y);
           in = w[k] >= 0.0;
         }
         if (!in) continue;

@@ -1,5 +1,6 @@
-// trimesh.cuh -- the triangle-mesh helpers of mesh simplification (simplify.cu) and mesh texturing (texture.cu): the
-// float64 vectors, the vertex load, the tie order s(id), the input check of rule 1 and the launch shape.
+// trimesh.cuh -- the triangle-mesh helpers of mesh simplification (simplify.cu), mesh texturing (texture.cu) and seam
+// levelling (seams.cu): the float64 vectors, the vertex load, the tie order s(id), the input check of rule 1, the edge
+// keys and adjacency, the lower-vertex edge rule and the launch shape.
 //
 // Include it only from units compiled with -fmad=false (build.py's UNIT_FLAGS).  Its float64 expressions must round
 // once per product and sum, in the order written, as tests/simplify_oracle.py and tests/texture_oracle.py compute
@@ -55,6 +56,54 @@ __global__ void __launch_bounds__(MT) mesh_validate_kernel(const float *vin, int
     }
     if (fail) atomicOr(bad, 1u);
   }
+}
+
+// Rule 1 of cs_texture_mesh, the edge keys of texturing (texture.cu) and seam levelling (seams.cu): corner c = 3t + k
+// starts the undirected edge from corner k to corner k + 1 mod 3, keyed (min << 32) | max of its two vertices.
+__device__ __forceinline__ unsigned long long edge_key_of(const int *tin, int c)
+{
+  const int t = c / 3, k = c - 3 * t;
+  const unsigned int a = tin[c], b = tin[3 * t + (k + 1) % 3];
+  return ((unsigned long long)min(a, b) << 32) | max(a, b);
+}
+
+// Two faces are adjacent across an edge when exactly two corners hold its key: at position i of the n sorted keys
+// (keysS, their corners valsS), a run of exactly two equal keys joins its two faces in nbr [3T].
+__device__ __forceinline__ void edge_pair_join(const unsigned long long *keysS, const int *valsS, int *nbr, int i, int n)
+{
+  const unsigned long long k = keysS[i];
+  if ((i > 0 && keysS[i - 1] == k) || keysS[i + 1] != k || (i + 2 < n && keysS[i + 2] == k)) return;
+  const int c1 = valsS[i], c2 = valsS[i + 1];
+  nbr[c1] = c2 / 3;
+  nbr[c2] = c1 / 3;
+}
+
+// The lower-vertex edge rule of texturing's key rasters (rule 2 of cs_texture_mesh, rule 7 of
+// cs_level_texture_seams): edge k runs corner k -> k + 1; it is evaluated from its lower vertex id P to the higher Q,
+// then signed by s = sign(doubled area) and negated when corner k holds the higher id, so the two faces of an edge see
+// exactly opposite values and no sample centre on a shared edge is missed.
+struct EdgeFns {
+  int P[3];
+  double du[3], dv[3], sg[3];
+};
+__device__ __forceinline__ void edge_fns_of(const int (&id)[3], const double (&u)[3], const double (&v)[3], double s,
+                                            EdgeFns &e)
+{
+  for (int k = 0; k < 3; k++) {
+    const int a = k, b = (k + 1) % 3;
+    const bool lo = id[a] < id[b];
+    e.P[k] = lo ? a : b;
+    const int Q = lo ? b : a;
+    e.du[k] = u[Q] - u[e.P[k]];
+    e.dv[k] = v[Q] - v[e.P[k]];
+    e.sg[k] = lo ? s : -s;
+  }
+}
+// w_k at the sample centre (x, y)
+__device__ __forceinline__ double edge_fn(const EdgeFns &e, const double (&u)[3], const double (&v)[3], int k, double x,
+                                          double y)
+{
+  return e.sg[k] * (e.du[k] * (y - v[e.P[k]]) - e.dv[k] * (x - u[e.P[k]]));
 }
 
 // CTAs of a grid-stride launch over n items: one per MT items, at least 1, at most 8192.

@@ -1398,6 +1398,77 @@ int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, con
                     float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
                     int *charts_out, int maxCharts, double info_out[2], long long stats_out[11], double *ms);
 
+/* Global seam levelling of a textured mesh (Lempitsky & Ivanov 2007 as Waechter, Moehrle & Goesele 2014 apply it,
+ * section 4.2): one additive offset per (vertex, label) pair that evens out the colour steps where charts from
+ * different images meet, added to the atlas texel by texel.  The inputs are cs_texture_mesh's outputs as it returns
+ * them: the mesh (d_vertices [numVertices][3] float, d_triangles [numTriangles][3] int32), d_faceView [numTriangles]
+ * (the label, < 0 unseen), d_uv [numTriangles][3][2] float in atlas pixels, the host chart table charts [numCharts][8]
+ * {image, x0, y0, width, height, ox, oy, faces} and d_atlas [atlasRows][atlasWidth] float; padding is the value given to
+ * cs_texture_mesh.  No images or cameras are needed: every chart's texels are copies of its image.  All arithmetic
+ * below is float64, each operation rounded once in the order written (no contraction).
+ * 1. Input: status 2, and only stats_out and a zero info_out written, when cs_texture_mesh's rule 1 fails, a seen
+ *    face has a non-finite uv, or a seen face lies in no chart of its own label.  A seen face's chart is the one whose rectangle
+ *    [ox, ox + width) x [oy, oy + height) holds (floor(u_0), floor(v_0)) of its corner 0 and whose image is the
+ *    face's label; the host builds a row index of the table (per atlas row, the charts covering it by ox) and the
+ *    device searches it.
+ * 2. Unknowns: one offset g(v, l) per distinct (vertex, label) over the corners of seen faces, in ascending (v, l).
+ * 3. Seam edges: an undirected edge held by exactly two faces (cs_texture_mesh's adjacency), both seen, with labels
+ *    a < b, endpoints P < Q (vertex ids).  On each side the uv runs from its corner at P to its corner at Q:
+ *    x(t) = u_P + t (u_Q - u_P) (likewise y), L_s = sqrt(du^2 + dv^2); S = max(1, ceil(max(L_a, L_b))) samples at
+ *    t_k = (k + 0.5) / S.  A side's value I is the bilinear read of the atlas at x(t), y(t): x0 = floor(x), fx = x - x0,
+ *    taps x0 and x0 + 1 clamped to that face's chart rectangle (likewise y), r0 = (1 - fx) A(ya, xa) + fx A(ya, xb),
+ *    r1 = (1 - fx) A(yb, xa) + fx A(yb, xb), I = (1 - fy) r0 + fy r1.  Sample k counts towards P with w = 1 - t_k and
+ *    towards Q with w = t_k: each end of an edge keeps (sum w I_a, sum w I_b, sum w) over its samples in k order.  For
+ *    every (v, a, b) the ends at v of the seam edges between a and b are added in sorted edge-key order, and
+ *    F(v, a) = (sum w I_a) / (sum w), F(v, b) likewise; the triple gives one seam row
+ *    g(v, a) - g(v, b) = F(v, b) - F(v, a) with weight 1.  Seam rows are ordered by (g(v, a), g(v, b)).
+ * 4. Smoothness: every distinct (label, min(v, w), max(v, w)) over the edges of seen faces gives g(v, l) - g(w, l) = 0
+ *    with weight smoothness; these rows follow the seam rows, ordered by their two unknowns.
+ * 5. System: (L_w + regularization I) g = b, L_w the weighted graph Laplacian of the rows (row r: g_i - g_j = d_r with
+ *    weight w_r adds w_r to the diagonal of i and j, -w_r off the diagonal, w_r d_r to b_i and -w_r d_r to b_j).
+ *    regularization > 0 makes the system symmetric positive definite.
+ * 6. Solve: Jacobi-preconditioned CG from g = 0 in float64 in one cooperative kernel; an unknown's incidences are
+ *    sorted by a stable radix sort and summed in coop.cuh's piece order, every dot product in its three-level order.
+ *    It stops when r.r <= tol^2 b.b (status 0) or after maxIterations (status 3).  Status 1: no seam row; the offsets
+ *    are 0 and the atlas is copied bit for bit.
+ * 7. Texels: every seen face visits the texels (X, Y) of its chart rectangle inside
+ *    [floor(min u) - (padding + 1), ceil(max u) + padding + 1] x (likewise v), each texel centre at integer (X, Y).
+ *    Its distance to the face's uv triangle is 0 inside (doubled area A != 0 and w_0, w_1, w_2 >= 0 with
+ *    S = (w_0 + w_1) + w_2 > 0 by cs_texture_mesh's lower-vertex edge rule, so shared edges leave no gap; weights
+ *    (w_1, w_2, w_0) / S), else the nearest of the three segments k -> k + 1 (t = clamp(((p - a).(b - a)) / |b - a|^2,
+ *    0, 1), 0 when |b - a| = 0; ties to the lower k; weights 1 - t, t).  The texel takes the 64-bit atomicMin of
+ *    (float(distance) bits << 32) | face.  A texel with a key becomes atlas + float((b_0 o_0 + b_1 o_1) + b_2 o_2), the
+ *    winning face's weights at the closest point and its float corner offsets o (d_cornerOffset), the sum in float;
+ *    every other texel, and every texel outside every chart, is copied.
+ * - Outputs: d_outAtlas [atlasRows][atlasWidth] (a separate buffer); d_cornerOffset [numTriangles][3] float, the
+ *   offset g at each corner of a seen face, NaN for an unseen face.  info_out [3] (may be NULL): the seam energy
+ *   sum over seam rows of ((F_a + g_a) - (F_b + g_b))^2 before (g = 0) and after, and the true relative residual
+ *   sqrt(|b - A g|^2 / |b|^2) (0 when b = 0), each total in coop.cuh's three-level order.  stats_out [8] (may be NULL):
+ *   seen faces, unknowns, seam edges, seam rows, smoothness rows, CG iterations, texels visited, status.  Returns the
+ *   unknown count, or CS_E_*.  numTriangles == 0: the atlas is copied, status 1.
+ * - Determinism: no floating-point atomics; two calls give the same bytes.
+ * - Launches (cs_launch_count): 13 whatever the data (validate, chart check; keys, adjacency, unknowns, smoothness
+ *   keys, smoothness heads; samples, row heads, rows; one cooperative solve kernel; texel keys, texels), 2 when the
+ *   input is invalid; plus cub's sorts and scans (not counted).  The host reads a few words after the input check,
+ *   the counts and the seam rows, and after the texels (one synchronise each); *ms (may be NULL) gets the event time
+ *   of the whole call.
+ * - Scratch, allocated on the call's stream and freed before it returns: 1061 bytes per face (edge, unknown and
+ *   smoothness keys and their corners, flags and scans, seam ends, rows, incidences, the CG vectors, an unknown's
+ *   range and pieces for up to 3 unknowns per face), 8 bytes per atlas texel (the texel keys), 4 per atlas row and
+ *   32 per chart plus 4 per chart row (the table and its row index), plus cub's storage.
+ * - CS_E_ARG, before any CUDA call, naming the argument: numVertices outside [0, 2^30], numTriangles outside
+ *   [0, 2^29], atlasRows outside [0, 32768], atlasWidth outside [1, 32768], padding outside [0, 16], smoothness not
+ *   finite or < 0, regularization not finite or <= 0, maxIterations outside [0, 100000], tol not in [0, 1),
+ *   numCharts < 0, NULL charts with numCharts > 0, a chart with an image < 0 or a rectangle outside the atlas; NULL or
+ *   not 4-byte aligned d_vertices with numVertices > 0, d_triangles, d_faceView, d_uv or d_cornerOffset with
+ *   numTriangles > 0, d_atlas or d_outAtlas with atlasRows > 0; and an output (d_outAtlas, d_cornerOffset) that
+ *   overlaps another output or an input (one sweep over sorted ranges). */
+int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                           const int *d_faceView, const float *d_uv, const int *charts, int numCharts,
+                           const float *d_atlas, int atlasRows, int atlasWidth, int padding, double smoothness,
+                           double regularization, int maxIterations, double tol, float *d_outAtlas,
+                           float *d_cornerOffset, double info_out[3], long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
