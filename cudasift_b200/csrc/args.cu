@@ -4,10 +4,13 @@
 #include "common.cuh"
 
 #include <algorithm>
+#include <array>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
+#include <iterator>
 #include <memory>
+#include <set>
 #include <vector>
 
 namespace cs {
@@ -1128,6 +1131,38 @@ int seams_args(const char *fn, const float *vertices, int numVertices, const int
         e[4] > atlasRows - e[6])
       return arg_error(fn, "charts[%d] must have an image >= 0 and a rectangle of at least one texel inside the atlas",
                        c);
+  }
+  // No two chart rectangles may share a texel: a texel belongs to one image, and rule 1 finds a face's chart by one
+  // search of the row index.  A sweep over x (a chart leaves at ox + width before any chart enters there) keeps the
+  // charts that cover the current column by oy; they are disjoint in y, so a chart entering overlaps one of them
+  // exactly when it overlaps its neighbour below or above in oy.
+  {
+    std::vector<std::array<int, 3>> events;   // (x, enters, chart)
+    events.reserve((size_t)2 * numCharts);
+    for (int c = 0; c < numCharts; c++) {
+      const int *e = charts + 8 * (size_t)c;
+      events.push_back({e[5] + e[3], 0, c});
+      events.push_back({e[5], 1, c});
+    }
+    std::sort(events.begin(), events.end());
+    std::set<std::pair<int, int>> active;     // (oy, chart)
+    for (const auto &ev : events) {
+      const int c = ev[2], oy = charts[8 * (size_t)c + 6], h = charts[8 * (size_t)c + 4];
+      if (!ev[1]) {
+        active.erase({oy, c});
+        continue;
+      }
+      auto above = active.lower_bound({oy, -1});
+      int other = -1;
+      if (above != active.end() && above->first < oy + h) other = above->second;
+      if (other < 0 && above != active.begin()) {
+        const auto below = std::prev(above);
+        if (below->first + charts[8 * (size_t)below->second + 4] > oy) other = below->second;
+      }
+      if (other >= 0)
+        return arg_error(fn, "charts[%d] and charts[%d] must not overlap", std::min(c, other), std::max(c, other));
+      active.insert({oy, c});
+    }
   }
   if (numVertices > 0 && (!vertices || misaligned(vertices, 4)))
     return arg_error(fn, "numVertices > 0 needs d_vertices (4-byte aligned)");

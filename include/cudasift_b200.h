@@ -1409,8 +1409,8 @@ int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, con
  * 1. Input: status 2, and only stats_out and a zero info_out written, when cs_texture_mesh's rule 1 fails, a seen
  *    face has a non-finite uv, or a seen face lies in no chart of its own label.  A seen face's chart is the one whose rectangle
  *    [ox, ox + width) x [oy, oy + height) holds (floor(u_0), floor(v_0)) of its corner 0 and whose image is the
- *    face's label; the host builds a row index of the table (per atlas row, the charts covering it by ox) and the
- *    device searches it.
+ *    face's label (the rectangles do not overlap, so at most one holds it); the host builds a row index of the table
+ *    (per atlas row, the charts covering it by ox) and the device searches it.
  * 2. Unknowns: one offset g(v, l) per distinct (vertex, label) over the corners of seen faces, in ascending (v, l).
  * 3. Seam edges: an undirected edge held by exactly two faces (cs_texture_mesh's adjacency), both seen, with labels
  *    a < b, endpoints P < Q (vertex ids).  On each side the uv runs from its corner at P to its corner at Q:
@@ -1459,7 +1459,8 @@ int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, con
  * - CS_E_ARG, before any CUDA call, naming the argument: numVertices outside [0, 2^30], numTriangles outside
  *   [0, 2^29], atlasRows outside [0, 32768], atlasWidth outside [1, 32768], padding outside [0, 16], smoothness not
  *   finite or < 0, regularization not finite or <= 0, maxIterations outside [0, 100000], tol not in [0, 1),
- *   numCharts < 0, NULL charts with numCharts > 0, a chart with an image < 0 or a rectangle outside the atlas; NULL or
+ *   numCharts < 0, NULL charts with numCharts > 0, a chart with an image < 0 or a rectangle outside the atlas, two
+ *   charts whose rectangles share a texel (one sweep over x, naming both charts); NULL or
  *   not 4-byte aligned d_vertices with numVertices > 0, d_triangles, d_faceView, d_uv or d_cornerOffset with
  *   numTriangles > 0, d_atlas or d_outAtlas with atlasRows > 0; and an output (d_outAtlas, d_cornerOffset) that
  *   overlaps another output or an input (one sweep over sorted ranges). */

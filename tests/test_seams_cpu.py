@@ -1,7 +1,8 @@
 """CPU checks of seam levelling (tests/seam_oracle.py) and of cs_level_texture_seams's argument checks: the system is
 symmetric positive definite, the exact solution never raises the seam energy, per-view constant offsets are recovered
 up to a common shift, a sweep of smoothness and regularization that fixed the defaults, every CS_E_ARG case with the
-overlap sweep, and texture.o's kernels unchanged by the helpers it now shares with seams.cu."""
+overlap sweeps (buffers and chart rectangles), every chart table the texturing oracle writes passing the chart
+checks, and texture.o's kernels unchanged by the helpers it now shares with seams.cu."""
 import ctypes
 import hashlib
 import math
@@ -146,8 +147,38 @@ def test_argument_checks():
     _rejects(_call(atlas=0x10001), "d_atlas")
     _rejects(_call(out=None), "d_outAtlas")
     _rejects(_call(out=0x20002), "d_outAtlas")
+    # charts whose rectangles share a texel, named by both indices: nested, partial, the same ox, the same oy, and
+    # three charts of which only the last overlaps the first
+    for rects, pair in (([(0, 0, 20, 4), (5, 1, 3, 2)], (0, 1)),
+                        ([(0, 0, 10, 4), (9, 3, 5, 1)], (0, 1)),
+                        ([(4, 0, 6, 2), (4, 1, 2, 3)], (0, 1)),
+                        ([(0, 2, 4, 1), (3, 2, 8, 2)], (0, 1)),
+                        ([(2, 0, 6, 2), (0, 2, 3, 2), (0, 1, 3, 1)], (0, 2)),
+                        ([(0, 0, 32, 4), (31, 3, 1, 1)], (0, 1))):
+        c = np.array([[l, 0, 0, w, h, ox, oy, 1] for l, (ox, oy, w, h) in enumerate(rects)], np.int32)
+        _rejects(_call(charts=c, nc=len(c)), "charts[%d] and charts[%d] must not overlap" % pair)
+    # rectangles that only touch (a shared edge or corner) pass the sweep; the call then stops at the overlapping
+    # buffers
+    c = np.array([[0, 0, 0, 4, 2, 0, 0, 1], [0, 0, 0, 4, 2, 4, 0, 1], [1, 0, 0, 4, 2, 0, 2, 1],
+                  [2, 0, 0, 4, 2, 4, 2, 1], [3, 0, 0, 24, 4, 8, 0, 1]], np.int32)
+    _rejects(_call(charts=c, nc=len(c), out=0x10000), "d_outAtlas and d_atlas overlap")
     # accepted edges of the ranges reach the overlap sweep only
     _rejects(_call(out=0x10000), "overlap")
+
+
+@pytest.mark.parametrize("make", ["topology", "occluder", "coplanar", "single_charts", "atlas", "atlas16",
+                                  "deep_strip", "raster_edges", "depth_ratio", "labelling"])
+def test_texturing_chart_tables_pass_the_overlap_check(make):
+    """Every chart table the texturing oracle writes for texture_cases' inputs passes the chart checks: the call stops
+    at its overlapping output buffers instead."""
+    c = tc.atlas(16) if make == "atlas16" else getattr(tc, make)()
+    r = to.texture(c["imgs"], c["Ks"], c["Rs"], c["ts"], c["v"], c["t"], **c["kw"])
+    ch = np.ascontiguousarray(r["charts"], np.int32)
+    rows, width = r["atlas"].shape
+    assert len(ch) > 0
+    res = _call(charts=ch, nc=len(ch), rows=rows, width=width, out=0x10000)
+    msg = cs.lib().cs_last_error().decode()
+    assert res == CS_E_ARG and "charts[" not in msg and msg.endswith("overlap"), msg
 
 
 def _seams_layout(rng):
