@@ -128,6 +128,8 @@ def lib():
                                  vp, ip, vp, vp, vp, vp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_level_texture_seams": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, c.c_double, c.c_double, ip,
                                         c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
+        "cs_level_texture_seams_local": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, ip, ip, c.c_double, vp,
+                                              vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_batch": (ip, [vp, ip, vp, ip, vp, ip, c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_absolute_pose_models": (ip, [vp, ip, vp, vp, ip, c.c_double, vp, vp, vp]),
         "cs_find_homography": (ip, [vp, ip, vp, c.POINTER(c.c_int), ip, fp, fp, fp, c.POINTER(c.c_double)]),
@@ -1547,6 +1549,42 @@ def LevelTextureSeams(vertices, triangles, atlas, uv, labels, charts, padding=2,
         out = outs[0].download(np.float32, H * W).reshape(H, W)
         off = outs[1].download(np.float32, 3 * T).reshape(T, 3)
         return out, off, info, stats, ms.value
+    finally:
+        for b in bufs:
+            b.free()
+
+
+def LevelTextureSeamsLocal(vertices, triangles, atlas, uv, labels, charts, padding=2, stripWidth=20, maxIterations=1000,
+                           tol=1e-4):
+    """Local seam levelling of a textured mesh (cs_level_texture_seams_local): Poisson editing of the texel strips
+    along every seam.  Each seam texel takes the mean of the two sides' values sampled along the seam; the texels within
+    stripWidth neighbour steps of a seam, in the same chart, get the smooth correction that keeps the atlas's own
+    gradients and meets those values (a membrane solved by CG to tol).  Run it after LevelTextureSeams, on its output:
+    the inputs are TextureMesh's (padding the value given to it) with the atlas replaced.  Returns (levelled atlas
+    float32 [rows, width], info float64 [3] {sum (f* - g)^2 over seam texels, relative residual, max |delta|}, stats
+    int64 [8] (the header's), ms)."""
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    A = np.ascontiguousarray(np.asarray(atlas, np.float32))
+    U = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 3, 2))
+    Lb = np.ascontiguousarray(np.asarray(labels, np.int32).reshape(-1))
+    Ct = np.ascontiguousarray(np.asarray(charts, np.int32).reshape(-1, 8))
+    V, T, (H, W) = len(X), len(F), A.shape
+    bufs = []
+    try:
+        ins = [DeviceBuffer(max(a.nbytes, 4)) for a in (X, F, Lb, U, A)]
+        bufs += ins
+        for b, a in zip(ins, (X, F, Lb, U, A)):
+            if a.size:
+                b.upload(a)
+        out = DeviceBuffer(max(A.nbytes, 4))
+        bufs.append(out)
+        info, stats, ms = np.zeros(3), np.zeros(8, np.int64), ctypes.c_double(0.0)
+        _check(lib().cs_level_texture_seams_local(ins[0].ptr, V, ins[1].ptr, T, ins[2].ptr, ins[3].ptr, _ptr(Ct),
+                                                  len(Ct), ins[4].ptr, H, W, int(padding), int(stripWidth),
+                                                  int(maxIterations), float(tol), out.ptr, _ptr(info), _ptr(stats),
+                                                  ctypes.byref(ms)), "LevelTextureSeamsLocal")
+        return out.download(np.float32, H * W).reshape(H, W), info, stats, ms.value
     finally:
         for b in bufs:
             b.free()

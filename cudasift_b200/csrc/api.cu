@@ -1830,8 +1830,8 @@ int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *
   const char *fn = "cs_level_texture_seams";
   if (ms) *ms = 0.0;
   int r = seams_args(fn, d_vertices, numVertices, d_triangles, numTriangles, d_faceView, d_uv, charts, numCharts,
-                     d_atlas, atlasRows, atlasWidth, padding, smoothness, regularization, maxIterations, tol,
-                     d_outAtlas, d_cornerOffset);
+                     d_atlas, atlasRows, atlasWidth, padding, smoothness, regularization, false, 0, maxIterations,
+                     tol, d_outAtlas, d_cornerOffset);
   if (r < 0) return r;
   int err = 0;
   DeviceCtx *c = current_ctx(&err);
@@ -1841,6 +1841,29 @@ int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *
     return seams_run(d_vertices, numVertices, d_triangles, numTriangles, d_faceView, d_uv, charts, numCharts, d_atlas,
                      atlasRows, atlasWidth, padding, smoothness, regularization, maxIterations, tol, d_outAtlas,
                      d_cornerOffset, c->stream, c->h_mesh.p, info_out, stats_out);
+  });
+}
+
+int cs_level_texture_seams_local(const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                                 const int *d_faceView, const float *d_uv, const int *charts, int numCharts,
+                                 const float *d_atlas, int atlasRows, int atlasWidth, int padding, int stripWidth,
+                                 int maxIterations, double tol, float *d_outAtlas, double info_out[3],
+                                 long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_level_texture_seams_local";
+  if (ms) *ms = 0.0;
+  int r = seams_args(fn, d_vertices, numVertices, d_triangles, numTriangles, d_faceView, d_uv, charts, numCharts,
+                     d_atlas, atlasRows, atlasWidth, padding, 0.0, 0.0, true, stripWidth, maxIterations, tol,
+                     d_outAtlas, nullptr);
+  if (r < 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(seams_local_result_bytes())) < 0) return r;
+  return timed_sync(fn, c, ms, [&] {
+    return seams_local_run(d_vertices, numVertices, d_triangles, numTriangles, d_faceView, d_uv, charts, numCharts,
+                           d_atlas, atlasRows, atlasWidth, padding, stripWidth, maxIterations, tol, d_outAtlas,
+                           c->stream, c->h_mesh.p, info_out, stats_out);
   });
 }
 

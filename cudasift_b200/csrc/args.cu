@@ -1110,17 +1110,19 @@ int texture_args(const char *fn, const cs_image *images, int numImages, const do
 
 int seams_args(const char *fn, const float *vertices, int numVertices, const int *triangles, int numTriangles,
                const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
-               int atlasRows, int atlasWidth, int padding, double smoothness, double regularization,
-               int maxIterations, double tol, const float *outAtlas, const float *cornerOffset)
+               int atlasRows, int atlasWidth, int padding, double smoothness, double regularization, bool local,
+               int stripWidth, int maxIterations, double tol, const float *outAtlas, const float *cornerOffset)
 {
   if (numVertices < 0 || numVertices > (1 << 30)) return arg_error(fn, "numVertices must be in [0, 2^30]");
   if (numTriangles < 0 || numTriangles > (1 << 29)) return arg_error(fn, "numTriangles must be in [0, 2^29]");
   if (atlasRows < 0 || atlasRows > 32768) return arg_error(fn, "atlasRows must be in [0, 32768]");
   if (atlasWidth < 1 || atlasWidth > 32768) return arg_error(fn, "atlasWidth must be in [1, 32768]");
   if (padding < 0 || padding > 16) return arg_error(fn, "padding must be in [0, 16]");
-  if (!std::isfinite(smoothness) || smoothness < 0.0) return arg_error(fn, "smoothness must be finite and >= 0");
-  if (!std::isfinite(regularization) || regularization <= 0.0)
+  if (!local && (!std::isfinite(smoothness) || smoothness < 0.0))
+    return arg_error(fn, "smoothness must be finite and >= 0");
+  if (!local && (!std::isfinite(regularization) || regularization <= 0.0))
     return arg_error(fn, "regularization must be finite and > 0");
+  if (local && (stripWidth < 1 || stripWidth > 128)) return arg_error(fn, "stripWidth must be in [1, 128]");
   if (maxIterations < 0 || maxIterations > 100000) return arg_error(fn, "maxIterations must be in [0, 100000]");
   if (!(tol >= 0.0 && tol < 1.0)) return arg_error(fn, "tol must be in [0, 1)");
   if (numCharts < 0) return arg_error(fn, "numCharts must be >= 0");
@@ -1172,7 +1174,7 @@ int seams_args(const char *fn, const float *vertices, int numVertices, const int
     return arg_error(fn, "numTriangles > 0 needs d_faceView (4-byte aligned)");
   if (numTriangles > 0 && (!uv || misaligned(uv, 4)))
     return arg_error(fn, "numTriangles > 0 needs d_uv (4-byte aligned)");
-  if (numTriangles > 0 && (!cornerOffset || misaligned(cornerOffset, 4)))
+  if (!local && numTriangles > 0 && (!cornerOffset || misaligned(cornerOffset, 4)))
     return arg_error(fn, "numTriangles > 0 needs d_cornerOffset (4-byte aligned)");
   const size_t texels = (size_t)atlasRows * atlasWidth;
   if (texels > 0 && (!atlas || misaligned(atlas, 4))) return arg_error(fn, "atlasRows > 0 needs d_atlas (4-byte aligned)");
@@ -1184,7 +1186,7 @@ int seams_args(const char *fn, const float *vertices, int numVertices, const int
   ArgRanges rs(names, 7);
   const size_t T = (size_t)numTriangles;
   rs.add(outAtlas, 4 * texels, 0, 0, true);
-  rs.add(cornerOffset, 12 * T, 1, 0, true);
+  if (!local) rs.add(cornerOffset, 12 * T, 1, 0, true);
   rs.add(vertices, 12 * (size_t)numVertices, 2, 0, false);
   rs.add(triangles, 12 * T, 3, 0, false);
   rs.add(faceView, 4 * T, 4, 0, false);

@@ -105,11 +105,13 @@ int texture_args(const char *fn, const cs_image *images, int numImages, const do
                  double lambda, double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
                  const float *atlas, int maxAtlasRows, const float *uv, const int *faceView, const int *faceChart,
                  const int *chartsOut, int maxCharts);
-// cs_level_texture_seams: the mesh, the chart table, the parameters, the buffers and the range sweep.
+// cs_level_texture_seams (local false: smoothness, regularization and d_cornerOffset checked) and
+// cs_level_texture_seams_local (local true: stripWidth checked, no corner offsets): the mesh, the chart table, the
+// parameters, the buffers and the range sweep.
 int seams_args(const char *fn, const float *vertices, int numVertices, const int *triangles, int numTriangles,
                const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
-               int atlasRows, int atlasWidth, int padding, double smoothness, double regularization,
-               int maxIterations, double tol, const float *outAtlas, const float *cornerOffset);
+               int atlasRows, int atlasWidth, int padding, double smoothness, double regularization, bool local,
+               int stripWidth, int maxIterations, double tol, const float *outAtlas, const float *cornerOffset);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

@@ -808,6 +808,13 @@ int seams_run(const float *vertices, int numVertices, const int *triangles, int 
               int padding, double smoothness, double regularization, int maxIterations, double tol, float *outAtlas,
               float *cornerOffset, cudaStream_t st, void *h_result, double *info, long long *stats);
 size_t seams_result_bytes();
+// cs_level_texture_seams_local after its argument checks, likewise (h_result pinned, seams_local_result_bytes); returns
+// the free-texel count (0 for invalid input).
+int seams_local_run(const float *vertices, int numVertices, const int *triangles, int numTriangles,
+                    const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
+                    int atlasRows, int atlasWidth, int padding, int stripWidth, int maxIterations, double tol,
+                    float *outAtlas, cudaStream_t st, void *h_result, double *info, long long *stats);
+size_t seams_local_result_bytes();
 
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).

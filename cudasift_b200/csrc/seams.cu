@@ -12,6 +12,7 @@
 // in sorted (row, side) order by coop.cuh's pieces; the totals in coop.cuh's three-level order.  This unit is compiled
 // with -fmad=false so that every float64 product and sum is rounded once, in the order written, as the oracle
 // computes it.
+#include <cassert>
 #include <climits>
 #include <cmath>
 #include <cstring>
@@ -194,6 +195,30 @@ __device__ __forceinline__ void seams_uv_of(const SeamsParams &p, int f, int w, 
   v = (double)p.uv[2 * (size_t)corner + 1];
 }
 
+// The two sides of the seam edge at sorted position i (rule 3): faces fs (side 0 the lower label), the uv of the ends
+// P and Q on each side and their corners, and the sample count S.
+struct SeamSides {
+  int fs[2], cP[2], cQ[2], S;
+  double uP[2], vP[2], uQ[2], vQ[2];
+};
+
+__device__ __forceinline__ void seams_edge_sides(const SeamsParams &p, int i, SeamSides &s)
+{
+  const unsigned long long key = p.ekeyS[i];
+  const int P = (int)(key >> 32), Q = (int)(unsigned int)key;
+  s.fs[0] = p.evalS[i] / 3;
+  s.fs[1] = p.nbr[p.evalS[i]];
+  if (p.view[s.fs[0]] > p.view[s.fs[1]]) { const int t = s.fs[0]; s.fs[0] = s.fs[1]; s.fs[1] = t; }
+  double len[2];
+  for (int k = 0; k < 2; k++) {
+    seams_uv_of(p, s.fs[k], P, s.uP[k], s.vP[k], s.cP[k]);
+    seams_uv_of(p, s.fs[k], Q, s.uQ[k], s.vQ[k], s.cQ[k]);
+    const double du = s.uQ[k] - s.uP[k], dv = s.vQ[k] - s.vP[k];
+    len[k] = sqrt(du * du + dv * dv);
+  }
+  s.S = (int)fmax(1.0, ceil(fmax(len[0], len[1])));
+}
+
 // One thread per seam edge (rule 3): its samples, the partial sums of its two ends and their keys.
 __global__ void __launch_bounds__(MT) seams_sample_kernel(SeamsParams p)
 {
@@ -201,19 +226,10 @@ __global__ void __launch_bounds__(MT) seams_sample_kernel(SeamsParams p)
   for (int i = blockIdx.x * MT + threadIdx.x; i < n; i += gridDim.x * MT) {
     if (!p.seFlag[i]) continue;
     const int e = p.seScan[i] - 1;
-    const unsigned long long key = p.ekeyS[i];
-    const int P = (int)(key >> 32), Q = (int)(unsigned int)key;
-    int fs[2] = {p.evalS[i] / 3, p.nbr[p.evalS[i]]};
-    if (p.view[fs[0]] > p.view[fs[1]]) { const int t = fs[0]; fs[0] = fs[1]; fs[1] = t; }   // side 0: label a < b
-    double uP[2], vP[2], uQ[2], vQ[2], len[2];
-    int cP[2], cQ[2];
-    for (int s = 0; s < 2; s++) {
-      seams_uv_of(p, fs[s], P, uP[s], vP[s], cP[s]);
-      seams_uv_of(p, fs[s], Q, uQ[s], vQ[s], cQ[s]);
-      const double du = uQ[s] - uP[s], dv = vQ[s] - vP[s];
-      len[s] = sqrt(du * du + dv * dv);
-    }
-    const int S = (int)fmax(1.0, ceil(fmax(len[0], len[1])));
+    SeamSides sd;
+    seams_edge_sides(p, i, sd);
+    const int *fs = sd.fs, *cP = sd.cP, *cQ = sd.cQ, S = sd.S;
+    const double *uP = sd.uP, *vP = sd.vP, *uQ = sd.uQ, *vQ = sd.vQ;
     const int *ea = p.ctab + 8 * (size_t)p.faceChart[fs[0]], *eb = p.ctab + 8 * (size_t)p.faceChart[fs[1]];
     double sum[2][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
     for (int k = 0; k < S; k++) {
@@ -504,6 +520,26 @@ __global__ void __launch_bounds__(MT) seams_texel_kernel(SeamsParams p)
 
 }  // namespace
 
+// The row index of the chart table (rule 1): per atlas row y, rowList[rowStart[y], rowStart[y + 1]) the charts that
+// cover it by (ox, index); rowList holds at least one entry.
+static void seams_row_index(const int *charts, int numCharts, int atlasRows, std::vector<int> &rowStart,
+                            std::vector<int> &rowList)
+{
+  rowStart.assign((size_t)atlasRows + 1, 0);
+  for (int c = 0; c < numCharts; c++)
+    for (int y = charts[8 * (size_t)c + 6]; y < charts[8 * (size_t)c + 6] + charts[8 * (size_t)c + 4]; y++)
+      rowStart[y + 1]++;
+  for (int y = 0; y < atlasRows; y++) rowStart[y + 1] += rowStart[y];
+  rowList.assign(std::max(1, rowStart[atlasRows]), 0);
+  std::vector<int> order(numCharts), fill(rowStart.begin(), rowStart.end() - 1);
+  for (int c = 0; c < numCharts; c++) order[c] = c;
+  std::stable_sort(order.begin(), order.end(),
+                   [&](int a, int b) { return charts[8 * (size_t)a + 5] < charts[8 * (size_t)b + 5]; });
+  for (int c : order)
+    for (int y = charts[8 * (size_t)c + 6]; y < charts[8 * (size_t)c + 6] + charts[8 * (size_t)c + 4]; y++)
+      rowList[fill[y]++] = c;
+}
+
 int seams_run(const float *vin, int V, const int *tin, int T, const int *faceView, const float *uv, const int *charts,
               int numCharts, const float *atlas, int atlasRows, int atlasWidth, int padding, double smoothness,
               double regularization, int maxIterations, double tol, float *outAtlas, float *cornerOffset,
@@ -526,22 +562,8 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
     return 0;
   }
 
-  // the row index of the chart table: per atlas row, the charts that cover it by (ox, index)
-  std::vector<int> rowStart((size_t)atlasRows + 1, 0), rowList;
-  for (int c = 0; c < numCharts; c++)
-    for (int y = charts[8 * (size_t)c + 6]; y < charts[8 * (size_t)c + 6] + charts[8 * (size_t)c + 4]; y++)
-      rowStart[y + 1]++;
-  for (int y = 0; y < atlasRows; y++) rowStart[y + 1] += rowStart[y];
-  rowList.resize(std::max(1, rowStart[atlasRows]));
-  {
-    std::vector<int> order(numCharts), fill(rowStart.begin(), rowStart.end() - 1);
-    for (int c = 0; c < numCharts; c++) order[c] = c;
-    std::stable_sort(order.begin(), order.end(),
-                     [&](int a, int b) { return charts[8 * (size_t)a + 5] < charts[8 * (size_t)b + 5]; });
-    for (int c : order)
-      for (int y = charts[8 * (size_t)c + 6]; y < charts[8 * (size_t)c + 6] + charts[8 * (size_t)c + 4]; y++)
-        rowList[fill[y]++] = c;
-  }
+  std::vector<int> rowStart, rowList;
+  seams_row_index(charts, numCharts, atlasRows, rowStart, rowList);
 
   const size_t C3 = 3 * (size_t)T, E2 = C3, R2 = 2 * (2 * C3);   // seam ends <= 3T, rows <= 2 (3T)
   size_t tb[4] = {};
@@ -775,5 +797,569 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
 }
 
 size_t seams_result_bytes() { return sizeof(SeamsResult); }
+
+// ---- local seam levelling (cs_level_texture_seams_local) -----------------------------------------------------------
+// Poisson editing of the texel strips along the seams (Waechter, Moehrle & Goesele 2014, section 4.2): rule 1's check,
+// the adjacency and the seam edges, rule 3's sample positions and bilinear reads and rule 7's texel keys are the
+// global call's kernels and helpers above; the kernels below add the seam texels, the strip, the 5-point system, its
+// solve and the output.  Every rule is stated in cudasift_b200.h at cs_level_texture_seams_local;
+// tests/seam_local_oracle.py restates them in float64.
+//
+// Determinism: integer atomics only for counts and for the bits of max |delta| (a max of non-negative doubles is exact
+// in any order).  A seam texel's targets are added in slot order (seam edge, side, k) after a stable radix sort by
+// texel; a free texel's stencil in neighbour order; the totals in coop.cuh's three-level order.
+namespace {
+
+constexpr int LOC_NONE = -1;                   // a neighbour code: no neighbour (a Neumann edge)
+constexpr int LOC_FIXED = -2;                  // a neighbour code: a seam or fixed texel (in the diagonal only)
+constexpr int LOC_FAR = INT_MAX;               // a domain texel's hop distance before it is reached
+
+struct LocalResult {
+  SeamsResult g;                               // the words of the reused kernels (bad, seen, seamEdges)
+  int samples, seamTexels, freeTexels;         // copied from the last entries of their scans
+  int iters, converged;
+  unsigned long long domain, maxDelta;         // maxDelta: the bits of max |delta|
+  double info[2];                              // sum (f* - g)^2, the true relative residual
+};
+
+struct LocalParams {
+  SeamsParams s;
+  LocalResult *res;
+  int n, strip, M, Ns, N, maxIt;               // n: atlas texels; M: samples; Ns: seam texels; N: free texels
+  double tol2;
+  int *scnt, *sscan;                           // [E] per seam edge: S, its inclusive scan
+  int *skey, *skeyS, *head, *hscan;            // [2M] sample slots: texel, sorted; run heads and their scan
+  double *sval, *svalS;                        // [2M] m_k
+  int *stexel;                                 // [Ns] seam texels in texel order
+  double *sf;                                  // [Ns] f*
+  int *chart, *dA, *dB, *sidx, *uidx;          // [n] chart (-1 outside the domain), distances, seam index, free scan
+  int *dist;                                   // the final distances (dA or dB)
+  int4 *nb;                                    // [N] neighbour codes
+  double *x, *r, *z, *pA, *pB, *q, *diag, *b;
+  double *partA, *groupA, *partB, *groupB, *partE, *groupE;
+};
+
+// One thread per seam edge (rule 3): its sample count S.
+__global__ void __launch_bounds__(MT) local_count_kernel(LocalParams q)
+{
+  const SeamsParams &p = q.s;
+  for (int i = blockIdx.x * MT + threadIdx.x; i < 3 * p.T; i += gridDim.x * MT) {
+    if (!p.seFlag[i]) continue;
+    SeamSides sd;
+    seams_edge_sides(p, i, sd);
+    q.scnt[p.seScan[i] - 1] = sd.S;
+  }
+}
+
+// One thread per seam edge: target m_k = 0.5 (I_a + I_b) of every sample, landed on each side's nearest texel
+// (clamped to that face's chart rectangle) at slot 2 base + side S + k.
+__global__ void __launch_bounds__(MT) local_sample_kernel(LocalParams q)
+{
+  const SeamsParams &p = q.s;
+  for (int i = blockIdx.x * MT + threadIdx.x; i < 3 * p.T; i += gridDim.x * MT) {
+    if (!p.seFlag[i]) continue;
+    SeamSides sd;
+    seams_edge_sides(p, i, sd);
+    const int S = sd.S, base = 2 * (q.sscan[p.seScan[i] - 1] - S);
+    const int *e[2] = {p.ctab + 8 * (size_t)p.faceChart[sd.fs[0]], p.ctab + 8 * (size_t)p.faceChart[sd.fs[1]]};
+    for (int k = 0; k < S; k++) {
+      const double t = ((double)k + 0.5) / (double)S;
+      double X[2], Y[2];
+      for (int s = 0; s < 2; s++) {
+        X[s] = sd.uP[s] + t * (sd.uQ[s] - sd.uP[s]);
+        Y[s] = sd.vP[s] + t * (sd.vQ[s] - sd.vP[s]);
+      }
+      const double m = 0.5 * (seams_bilinear(p, e[0], X[0], Y[0]) + seams_bilinear(p, e[1], X[1], Y[1]));
+      for (int s = 0; s < 2; s++) {
+        const int *c = e[s];
+        const int tx = (int)fmin(fmax(floor(X[s] + 0.5), (double)c[5]), (double)(c[5] + c[3] - 1));
+        const int ty = (int)fmin(fmax(floor(Y[s] + 0.5), (double)c[6]), (double)(c[6] + c[4] - 1));
+        const int slot = base + s * S + k;
+        q.skey[slot] = ty * p.width + tx;
+        q.sval[slot] = m;
+      }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(MT) local_heads_kernel(LocalParams q)
+{
+  for (int j = blockIdx.x * MT + threadIdx.x; j < 2 * q.M; j += gridDim.x * MT)
+    q.head[j] = j == 0 || q.skeyS[j - 1] != q.skeyS[j];
+}
+
+// One thread per atlas texel (rule 2): its chart (its key face's, -1 outside the domain) and distance (LOC_FAR in the
+// domain, -1 outside); the domain count.
+__global__ void __launch_bounds__(MT) local_domain_kernel(LocalParams q)
+{
+  unsigned long long inside = 0;
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < q.n; i += (long long)gridDim.x * MT) {
+    const unsigned long long key = q.s.tkey[i];
+    const bool in = key != NONE;
+    q.chart[i] = in ? q.s.faceChart[(unsigned int)key] : -1;
+    q.dA[i] = in ? LOC_FAR : -1;
+    inside += in;
+  }
+  if (inside) atomicAdd(&q.res->domain, inside);
+}
+
+// One thread per run of sorted slots (rule 3): the seam texel's f*, the mean of its targets in slot order; distance 0.
+__global__ void __launch_bounds__(MT) local_seam_kernel(LocalParams q)
+{
+  const int n = 2 * q.M;
+  for (int j = blockIdx.x * MT + threadIdx.x; j < n; j += gridDim.x * MT) {
+    if (!q.head[j]) continue;
+    const int texel = q.skeyS[j], s = q.hscan[j] - 1;
+    double sum = 0.0;
+    int cnt = 0;
+    for (int m = j; m < n && q.skeyS[m] == texel; m++, cnt++) sum = sum + q.svalS[m];
+    assert(q.chart[texel] >= 0);               // within sqrt(2)/2 of its face, so inside its face's key box
+    q.stexel[s] = texel;
+    q.sf[s] = sum / (double)cnt;
+    q.dA[texel] = 0;
+    q.sidx[texel] = s;
+  }
+}
+
+// One synchronous relaxation round (rule 4): d = min(d, d of a neighbour + 1) over the 4-neighbours of the same chart.
+__global__ void __launch_bounds__(MT) local_relax_kernel(LocalParams q, const int *din, int *dout)
+{
+  const int W = q.s.width, H = q.s.rows;
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < q.n; i += (long long)gridDim.x * MT) {
+    int d = din[i];
+    const int c = q.chart[i];
+    if (c >= 0 && d > 0) {
+      const int y = (int)(i / W), x = (int)(i - (long long)y * W);
+      const long long nbr[4] = {x > 0 ? i - 1 : -1, x + 1 < W ? i + 1 : -1, y > 0 ? i - W : -1, y + 1 < H ? i + W : -1};
+      for (int k = 0; k < 4; k++)
+        if (nbr[k] >= 0 && q.chart[nbr[k]] == c && din[nbr[k]] != LOC_FAR) d = min(d, din[nbr[k]] + 1);
+    }
+    dout[i] = d;
+  }
+}
+
+// Rule 4: the free-texel flags (1 <= d <= stripWidth), over the spare distance buffer.
+__global__ void __launch_bounds__(MT) local_flag_kernel(LocalParams q, int *flag)
+{
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < q.n; i += (long long)gridDim.x * MT) {
+    const int d = q.dist[i];
+    flag[i] = d >= 1 && d <= q.strip;
+  }
+}
+
+// One thread per free texel (rule 5): its neighbour codes, diagonal and right-hand side.
+__global__ void __launch_bounds__(MT) local_unknowns_kernel(LocalParams q)
+{
+  const int W = q.s.width, H = q.s.rows;
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < q.n; i += (long long)gridDim.x * MT) {
+    const int d = q.dist[i];
+    if (!(d >= 1 && d <= q.strip)) continue;
+    const int u = q.uidx[i] - 1, c = q.chart[i];
+    const int y = (int)(i / W), x = (int)(i - (long long)y * W);
+    const long long nbr[4] = {x > 0 ? i - 1 : -1, x + 1 < W ? i + 1 : -1, y > 0 ? i - W : -1, y + 1 < H ? i + W : -1};
+    int code[4];
+    int count = 0;
+    double bv = 0.0;
+    for (int k = 0; k < 4; k++) {
+      code[k] = LOC_NONE;
+      const long long j = nbr[k];
+      if (j < 0 || q.chart[j] != c) continue;
+      const int dj = q.dist[j];
+      count++;
+      if (dj >= 1 && dj <= q.strip) {
+        code[k] = q.uidx[j] - 1;
+      } else {
+        code[k] = LOC_FIXED;
+        if (dj == 0) bv = bv + (q.sf[q.sidx[j]] - (double)q.s.atlas[j]);
+      }
+    }
+    q.nb[u] = make_int4(code[0], code[1], code[2], code[3]);
+    q.diag[u] = (double)count;
+    q.b[u] = bv;
+  }
+}
+
+// (A v)_i = diag_i v_i - sum over free neighbours of v_j (in neighbour order), v_j = a_j + beta c_j (c may be null).
+__device__ __forceinline__ double local_stencil(const LocalParams &q, int i, double vi, const double *a, const double *c,
+                                               double beta)
+{
+  const int4 m = q.nb[i];
+  const int code[4] = {m.x, m.y, m.z, m.w};
+  double s = 0.0;
+  for (int k = 0; k < 4; k++)
+    if (code[k] >= 0) s = s + (c ? a[code[k]] + beta * c[code[k]] : a[code[k]]);
+  return q.diag[i] * vi - s;
+}
+
+// Rule 6: Jacobi-PCG from delta = 0 over the free texels; four grid barriers per iteration, p double-buffered so that
+// q = A p reads the neighbours' z and old p without a barrier between the update of p and the product.
+__global__ void __launch_bounds__(MT) local_solve_kernel(LocalParams q)
+{
+  cg::grid_group grid = cg::this_grid();
+  const int N = q.N, Ns = q.Ns;
+  co_tree_tiles<2, MT>(N, q.partA, [&](int i, double *v) {
+    const double rv = q.b[i], zv = rv / q.diag[i];
+    q.x[i] = 0.0;
+    q.r[i] = rv;
+    q.z[i] = zv;
+    q.pA[i] = 0.0;
+    v[0] += rv * rv;
+    v[1] += rv * zv;
+  });
+  co_tree_tiles<1, MT>(Ns, q.partE, [&](int s, double *v) {
+    const double e = q.sf[s] - (double)q.s.atlas[q.stexel[s]];
+    v[0] += e * e;
+  });
+  grid.sync();
+  co_tree_groups<2, MT>(N, q.partA, q.groupA);
+  co_tree_groups<1, MT>(Ns, q.partE, q.groupE);
+  grid.sync();
+  double t2[2], t1[1], e0[1];
+  co_tree_total<2, MT>(N, q.groupA, t2);
+  co_tree_total<1, MT>(Ns, q.groupE, e0);
+  const double bb = t2[0], thr = q.tol2 * bb;
+  double rr = t2[0], rz = t2[1], beta = 0.0;
+  int it = 0;
+  while (it < q.maxIt && !(rr <= thr)) {
+    const double *pold = (it & 1) ? q.pB : q.pA;
+    double *pnew = (it & 1) ? q.pA : q.pB;
+    // p = z + beta p_old, q = A p; the total of p.q
+    co_tree_tiles<1, MT>(N, q.partB, [&](int i, double *v) {
+      const double pn = q.z[i] + beta * pold[i], qv = local_stencil(q, i, pn, q.z, pold, beta);
+      pnew[i] = pn;
+      q.q[i] = qv;
+      v[0] += pn * qv;
+    });
+    grid.sync();
+    co_tree_groups<1, MT>(N, q.partB, q.groupB);
+    grid.sync();
+    co_tree_total<1, MT>(N, q.groupB, t1);
+    if (!(t1[0] > 0.0)) break;
+    const double alpha = rz / t1[0];
+    // x += alpha p, r -= alpha q, z = r / diag; the totals of r.r and r.z
+    co_tree_tiles<2, MT>(N, q.partA, [&](int i, double *v) {
+      q.x[i] = q.x[i] + alpha * pnew[i];
+      const double rv = q.r[i] - alpha * q.q[i], zv = rv / q.diag[i];
+      q.r[i] = rv;
+      q.z[i] = zv;
+      v[0] += rv * rv;
+      v[1] += rv * zv;
+    });
+    it++;
+    grid.sync();
+    co_tree_groups<2, MT>(N, q.partA, q.groupA);
+    grid.sync();
+    co_tree_total<2, MT>(N, q.groupA, t2);
+    rr = t2[0];
+    beta = t2[1] / rz;
+    rz = t2[1];
+  }
+  // the true residual b - A x; max |x|
+  unsigned long long mx = 0;
+  co_tree_tiles<1, MT>(N, q.partB, [&](int i, double *v) {
+    const double res = q.b[i] - local_stencil(q, i, q.x[i], q.x, nullptr, 0.0);
+    v[0] += res * res;
+    mx = max(mx, (unsigned long long)__double_as_longlong(fabs(q.x[i])));
+  });
+  if (mx) atomicMax(&q.res->maxDelta, mx);
+  grid.sync();
+  co_tree_groups<1, MT>(N, q.partB, q.groupB);
+  grid.sync();
+  co_tree_total<1, MT>(N, q.groupB, t1);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    q.res->iters = it;
+    q.res->converged = rr <= thr;
+    q.res->info[0] = e0[0];
+    q.res->info[1] = bb > 0.0 ? sqrt(t1[0] / bb) : 0.0;
+  }
+}
+
+// One thread per atlas texel (rule 7): a seam texel becomes float(f*), a free texel float(g + delta), the rest a copy.
+__global__ void __launch_bounds__(MT) local_output_kernel(LocalParams q)
+{
+  for (long long i = blockIdx.x * (long long)MT + threadIdx.x; i < q.n; i += (long long)gridDim.x * MT) {
+    const int d = q.dist[i];
+    const float a = q.s.atlas[i];
+    float o = a;
+    if (d == 0) o = __double2float_rn(q.sf[q.sidx[i]]);
+    else if (d >= 1 && d <= q.strip) o = __double2float_rn((double)a + q.x[q.uidx[i] - 1]);
+    q.s.out[i] = o;
+  }
+}
+
+}  // namespace
+
+int seams_local_run(const float *vin, int V, const int *tin, int T, const int *faceView, const float *uv,
+                    const int *charts, int numCharts, const float *atlas, int atlasRows, int atlasWidth, int padding,
+                    int stripWidth, int maxIterations, double tol, float *outAtlas, cudaStream_t st, void *h_res,
+                    double *info, long long *stats)
+{
+  const size_t n = (size_t)atlasRows * atlasWidth, atlasBytes = n * 4;
+  long long st_[8] = {};
+  double info_[3] = {};
+  auto finish = [&](int status) {
+    st_[7] = status;
+    if (info)
+      for (int k = 0; k < 3; k++) info[k] = status == 2 ? 0.0 : info_[k];
+    if (stats)
+      for (int k = 0; k < 8; k++) stats[k] = st_[k];
+  };
+  if (T == 0) {                                // no face: no seam texel, the atlas copied
+    if (atlasBytes) CS_CUDA(cudaMemcpyAsync(outAtlas, atlas, atlasBytes, cudaMemcpyDeviceToDevice, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    finish(1);
+    return 0;
+  }
+  std::vector<int> rowStart, rowList;
+  seams_row_index(charts, numCharts, atlasRows, rowStart, rowList);
+
+  const size_t C3 = 3 * (size_t)T;
+  size_t tb[4] = {};
+  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (unsigned long long *)nullptr,
+                                          (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, (int)C3, 0,
+                                          64, st));
+  CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb[1], (int *)nullptr, (int *)nullptr, (int)std::max(C3, n), st));
+  const size_t tempBytes = std::max(tb[0], tb[1]);
+
+  // the first allocation: the mesh stage and the texel arrays
+  Layout L(256);
+  const size_t resAt = L.take(sizeof(LocalResult));
+  const size_t ctabAt = L.take(std::max(1, numCharts) * 32ull), rsAt = L.take(rowStart.size() * 4),
+               rlAt = L.take(rowList.size() * 4);
+  const size_t fcAt = L.take((size_t)T * 4);
+  const size_t ekAt = L.take(C3 * 8), ekSAt = L.take(C3 * 8), ukAt = L.take(C3 * 8), ukSAt = L.take(C3 * 8);
+  const size_t evAt = L.take(C3 * 4), evSAt = L.take(C3 * 4), uvAt = L.take(C3 * 4), uvSAt = L.take(C3 * 4),
+               nbrAt = L.take(C3 * 4);
+  const size_t uhAt = L.take(C3 * 4), usAt = L.take(C3 * 4), sfAt = L.take(C3 * 4), ssAt = L.take(C3 * 4),
+               cuAt = L.take(C3 * 4), scAt = L.take(C3 * 4), scsAt = L.take(C3 * 4);
+  const size_t tkeyAt = L.take(n * 8), chAt = L.take(n * 4), daAt = L.take(n * 4), dbAt = L.take(n * 4),
+               siAt = L.take(n * 4), uiAt = L.take(n * 4);
+  const size_t tempAt = L.take(tempBytes);
+  char *base = nullptr, *base2 = nullptr, *base3 = nullptr;
+  CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
+  auto at = [&](size_t off) { return base + off; };
+
+  LocalParams q{};
+  SeamsParams &p = q.s;
+  q.res = reinterpret_cast<LocalResult *>(at(resAt));
+  p.res = &q.res->g;
+  p.V = V;
+  p.T = T;
+  p.vin = vin;
+  p.tin = tin;
+  p.view = faceView;
+  p.uv = uv;
+  p.atlas = atlas;
+  p.out = outAtlas;
+  p.rows = atlasRows;
+  p.width = atlasWidth;
+  p.padding = padding;
+  p.ctab = reinterpret_cast<const int *>(at(ctabAt));
+  p.rowStart = reinterpret_cast<const int *>(at(rsAt));
+  p.rowList = reinterpret_cast<const int *>(at(rlAt));
+  p.faceChart = reinterpret_cast<int *>(at(fcAt));
+  p.ekey = reinterpret_cast<unsigned long long *>(at(ekAt));
+  p.ekeyS = reinterpret_cast<unsigned long long *>(at(ekSAt));
+  p.ukey = reinterpret_cast<unsigned long long *>(at(ukAt));
+  p.ukeyS = reinterpret_cast<unsigned long long *>(at(ukSAt));
+  p.eval = reinterpret_cast<int *>(at(evAt));
+  p.evalS = reinterpret_cast<int *>(at(evSAt));
+  p.uval = reinterpret_cast<int *>(at(uvAt));
+  p.uvalS = reinterpret_cast<int *>(at(uvSAt));
+  p.nbr = reinterpret_cast<int *>(at(nbrAt));
+  p.uHead = reinterpret_cast<int *>(at(uhAt));
+  p.uScan = reinterpret_cast<int *>(at(usAt));
+  p.seFlag = reinterpret_cast<int *>(at(sfAt));
+  p.seScan = reinterpret_cast<int *>(at(ssAt));
+  p.cornerUnk = reinterpret_cast<int *>(at(cuAt));
+  p.tkey = reinterpret_cast<unsigned long long *>(at(tkeyAt));
+  q.scnt = reinterpret_cast<int *>(at(scAt));
+  q.sscan = reinterpret_cast<int *>(at(scsAt));
+  q.chart = reinterpret_cast<int *>(at(chAt));
+  q.dA = reinterpret_cast<int *>(at(daAt));
+  q.dB = reinterpret_cast<int *>(at(dbAt));
+  q.sidx = reinterpret_cast<int *>(at(siAt));
+  q.uidx = reinterpret_cast<int *>(at(uiAt));
+  q.n = (int)n;
+  q.strip = stripWidth;
+  q.maxIt = maxIterations;
+  q.tol2 = tol * tol;
+  void *temp = at(tempAt);
+  size_t tempB = tempBytes;
+  LocalResult &R = *static_cast<LocalResult *>(h_res);
+  cudaEvent_t *tev = match_timing_events();
+  const int n3 = (int)C3;
+
+  int status = 0;
+  auto readback = [&]() -> int {
+    CS_CUDA(cudaMemcpyAsync(h_res, q.res, sizeof(LocalResult), cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  };
+  auto last = [&](int *word, const int *scan, int len) -> int {
+    if (len > 0) CS_CUDA(cudaMemcpyAsync(word, scan + len - 1, 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  };
+  auto run = [&]() -> int {
+    int r;
+    if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
+    CS_CUDA(cudaMemsetAsync(q.res, 0, sizeof(LocalResult), st));
+    if (numCharts)
+      CS_CUDA(cudaMemcpyAsync(at(ctabAt), charts, (size_t)numCharts * 32, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(at(rsAt), rowStart.data(), rowStart.size() * 4, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(at(rlAt), rowList.data(), rowList.size() * 4, cudaMemcpyHostToDevice, st));
+    mesh_validate_kernel<<<grid_of(T), MT, 0, st>>>(vin, V, tin, T, &p.res->bad);
+    seams_check_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if ((r = readback()) < 0) return r;
+    if (R.g.bad) {
+      status = 2;
+      return 0;
+    }
+    // the seam edges and their sample counts
+    if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
+    seams_keys_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ekey, p.ekeyS, p.eval, p.evalS, n3, 0, 64, st));
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ukey, p.ukeyS, p.uval, p.uvalS, n3, 0, 64, st));
+    seams_adjacency_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.uHead, p.uScan, n3, st));
+    seams_unknown_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.seFlag, p.seScan, n3, st));
+    local_count_kernel<<<grid_of(3ll * T), MT, 0, st>>>(q);
+    count_launch(4);
+    CS_CUDA(cudaGetLastError());
+    if ((r = last(&p.res->seamEdges, p.seScan, n3)) < 0) return r;
+    if ((r = readback()) < 0) return r;
+    p.E = R.g.seamEdges;
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, q.scnt, q.sscan, p.E, st));
+    if ((r = last(&q.res->samples, q.sscan, p.E)) < 0) return r;
+    // the domain: texel keys, charts and distances
+    if (tev) CS_CUDA(cudaEventRecord(tev[2], st));
+    CS_CUDA(cudaMemsetAsync(p.tkey, 0xff, n * 8, st));
+    seams_raster_kernel<<<grid_of(T), MT, 0, st>>>(p);
+    local_domain_kernel<<<grid_of((long long)n), MT, 0, st>>>(q);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if ((r = readback()) < 0) return r;
+    // the seam texels: the samples' slots sorted by texel, one run per seam texel
+    if (tev) CS_CUDA(cudaEventRecord(tev[3], st));
+    q.M = R.samples;
+    const size_t S2 = 2 * (size_t)q.M;
+    size_t sortB = 0, scanB = 0;
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, sortB, (int *)nullptr, (int *)nullptr, (double *)nullptr,
+                                            (double *)nullptr, (int)S2, 0, 32, st));
+    CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, scanB, (int *)nullptr, (int *)nullptr, (int)S2, st));
+    Layout L2(256);
+    const size_t skAt = L2.take(S2 * 4), skSAt = L2.take(S2 * 4), hdAt = L2.take(S2 * 4), hsAt = L2.take(S2 * 4),
+                 svAt = L2.take(S2 * 8), svSAt = L2.take(S2 * 8), stAt = L2.take(S2 * 4), sfvAt = L2.take(S2 * 8),
+                 t2At = L2.take(std::max(sortB, scanB));
+    CS_CUDA(cudaMallocAsync((void **)&base2, std::max<size_t>(L2.bytes, 256), st));
+    q.skey = reinterpret_cast<int *>(base2 + skAt);
+    q.skeyS = reinterpret_cast<int *>(base2 + skSAt);
+    q.head = reinterpret_cast<int *>(base2 + hdAt);
+    q.hscan = reinterpret_cast<int *>(base2 + hsAt);
+    q.sval = reinterpret_cast<double *>(base2 + svAt);
+    q.svalS = reinterpret_cast<double *>(base2 + svSAt);
+    q.stexel = reinterpret_cast<int *>(base2 + stAt);
+    q.sf = reinterpret_cast<double *>(base2 + sfvAt);
+    void *temp2 = base2 + t2At;
+    size_t temp2B = std::max(sortB, scanB);
+    local_sample_kernel<<<grid_of(3ll * T), MT, 0, st>>>(q);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp2, temp2B, q.skey, q.skeyS, q.sval, q.svalS, (int)S2, 0,
+                                            radix_bits((long long)n - 1), st));
+    local_heads_kernel<<<grid_of((long long)S2), MT, 0, st>>>(q);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp2, temp2B, q.head, q.hscan, (int)S2, st));
+    local_seam_kernel<<<grid_of((long long)S2), MT, 0, st>>>(q);
+    count_launch(3);
+    CS_CUDA(cudaGetLastError());
+    if ((r = last(&q.res->seamTexels, q.hscan, (int)S2)) < 0) return r;
+    // the strip: stripWidth relaxation rounds, the free texels numbered in atlas order
+    if (tev) CS_CUDA(cudaEventRecord(tev[4], st));
+    for (int k = 0; k < stripWidth; k++)
+      local_relax_kernel<<<grid_of((long long)n), MT, 0, st>>>(q, (k & 1) ? q.dB : q.dA, (k & 1) ? q.dA : q.dB);
+    q.dist = (stripWidth & 1) ? q.dB : q.dA;
+    int *flag = (stripWidth & 1) ? q.dA : q.dB;
+    local_flag_kernel<<<grid_of((long long)n), MT, 0, st>>>(q, flag);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, flag, q.uidx, (int)n, st));
+    count_launch(stripWidth + 1);
+    CS_CUDA(cudaGetLastError());
+    if ((r = last(&q.res->freeTexels, q.uidx, (int)n)) < 0) return r;
+    if ((r = readback()) < 0) return r;
+    q.Ns = R.seamTexels;
+    q.N = R.freeTexels;
+    // the system and its solve
+    if (tev) CS_CUDA(cudaEventRecord(tev[5], st));
+    const size_t N = (size_t)q.N, Ns = (size_t)q.Ns;
+    const size_t tilesN = (N + CO_TREE_TILE - 1) / CO_TREE_TILE, groupsN = (tilesN + MT - 1) / MT;
+    const size_t tilesS = (Ns + CO_TREE_TILE - 1) / CO_TREE_TILE, groupsS = (tilesS + MT - 1) / MT;
+    Layout L3(256);
+    const size_t nbAt = L3.take(N * 16), vecAt = L3.take(8 * N * 8),
+                 paAt = L3.take(tilesN * 16), gaAt = L3.take(groupsN * 16), pbAt = L3.take(tilesN * 8),
+                 gbAt = L3.take(groupsN * 8), peAt = L3.take(tilesS * 8), geAt = L3.take(groupsS * 8);
+    CS_CUDA(cudaMallocAsync((void **)&base3, std::max<size_t>(L3.bytes, 256), st));
+    q.nb = reinterpret_cast<int4 *>(base3 + nbAt);
+    double *vec = reinterpret_cast<double *>(base3 + vecAt);
+    q.x = vec;
+    q.r = vec + N;
+    q.z = vec + 2 * N;
+    q.pA = vec + 3 * N;
+    q.pB = vec + 4 * N;
+    q.q = vec + 5 * N;
+    q.diag = vec + 6 * N;
+    q.b = vec + 7 * N;
+    q.partA = reinterpret_cast<double *>(base3 + paAt);
+    q.groupA = reinterpret_cast<double *>(base3 + gaAt);
+    q.partB = reinterpret_cast<double *>(base3 + pbAt);
+    q.groupB = reinterpret_cast<double *>(base3 + gbAt);
+    q.partE = reinterpret_cast<double *>(base3 + peAt);
+    q.groupE = reinterpret_cast<double *>(base3 + geAt);
+    local_unknowns_kernel<<<grid_of((long long)n), MT, 0, st>>>(q);
+    count_launch();
+    CS_CUDA(cudaGetLastError());
+    const int wave = coop_grid<local_solve_kernel, MT>("cs_level_texture_seams_local");
+    if (wave < 0) return wave;
+    void *args[] = {&q};
+    CS_CUDA(cudaLaunchCooperativeKernel((const void *)local_solve_kernel, dim3(wave), dim3(MT), args, 0, st));
+    count_launch();
+    // the output
+    if (tev) CS_CUDA(cudaEventRecord(tev[6], st));
+    local_output_kernel<<<grid_of((long long)n), MT, 0, st>>>(q);
+    count_launch();
+    CS_CUDA(cudaGetLastError());
+    if (tev) CS_CUDA(cudaEventRecord(tev[7], st));
+    if ((r = readback()) < 0) return r;
+    status = q.Ns == 0 ? 1 : R.converged ? 0 : 3;
+    if (tev) {
+      static const char *const names[7] = {"check", "seam edges", "domain", "seam texels", "strip", "solve",
+                                           "output"};
+      report_stage_times(tev, names, 7, "seams local timing faces=%d seam texels=%d free texels=%d iterations=%d", T,
+                         q.Ns, q.N, R.iters);
+    }
+    return 0;
+  };
+  const int r = run();
+  if (base3) cudaFreeAsync(base3, st);
+  if (base2) cudaFreeAsync(base2, st);
+  cudaFreeAsync(base, st);
+  if (r < 0) return r;
+  if (status != 2) {
+    st_[0] = R.g.seen;
+    st_[1] = R.g.seamEdges;
+    st_[2] = R.samples;
+    st_[3] = R.seamTexels;
+    st_[4] = R.freeTexels;
+    st_[5] = (long long)R.domain;
+    st_[6] = R.iters;
+    info_[0] = R.info[0];
+    info_[1] = R.info[1];
+    const unsigned long long bits = R.maxDelta;
+    std::memcpy(&info_[2], &bits, 8);
+  }
+  finish(status);
+  return status == 2 ? 0 : R.freeTexels;
+}
+
+size_t seams_local_result_bytes() { return sizeof(LocalResult); }
 
 }  // namespace cs

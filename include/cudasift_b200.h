@@ -1470,6 +1470,60 @@ int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *
                            double regularization, int maxIterations, double tol, float *d_outAtlas,
                            float *d_cornerOffset, double info_out[3], long long stats_out[8], double *ms);
 
+/* Local seam levelling of a textured mesh (Waechter, Moehrle & Goesele 2014, section 4.2, after Perez et al. 2003):
+ * Poisson editing of the texel strips along every seam, which removes the steps the global call's per-vertex offsets
+ * cannot (a mismatch that varies faster than the mesh or along one seam edge).  The inputs are
+ * cs_level_texture_seams's, and d_atlas is normally its output.  All arithmetic below is float64, each operation
+ * rounded once in the order written (no contraction).
+ * 1. Input: cs_level_texture_seams's rule 1 unchanged (the same checks, status 2, the chart of each seen face).
+ * 2. Domain: the texels that cs_level_texture_seams's rule 7 gives a key (every texel of a seen face's chart rectangle
+ *    inside its uv box grown by padding + 1); a texel belongs to its key face's chart.  Two texels are neighbours when
+ *    they are 4-adjacent, both in the domain and in the same chart, taken in the order (x - 1, y), (x + 1, y),
+ *    (x, y - 1), (x, y + 1).
+ * 3. Seam texels: cs_level_texture_seams's rule 3 seam edges (sorted by key), sides, sample count S, positions t_k and
+ *    bilinear reads I_a, I_b of d_atlas.  Sample k has the target m_k = 0.5 (I_a + I_b) and lands on each side s at
+ *    the nearest texel (floor(x + 0.5), floor(y + 0.5)) of x(t_k), y(t_k), clamped to that face's chart rectangle
+ *    (always in the domain: within sqrt(2)/2 of the face).  A seam texel's value f* is the sum of the targets landing
+ *    on it in (seam edge, side, k) order divided by their count.
+ * 4. Strip: the hop distance d is 0 at seam texels and grows by one per neighbour step, computed by stripWidth
+ *    synchronous rounds d <- min(d, d of a neighbour + 1).  Free texels have 1 <= d <= stripWidth and are the
+ *    unknowns, numbered in row-major atlas order; every other domain texel is fixed.
+ * 5. System: for the correction delta = f - g (g the input atlas), with the atlas's own gradients as guidance:
+ *    diag_p = the number of neighbours of p, (A delta)_p = diag_p delta_p - sum over free neighbours q of delta_q
+ *    (in neighbour order), b_p = sum over seam neighbours q of (f*_q - g_q) (in neighbour order).  Fixed neighbours
+ *    hold delta = 0 and a missing neighbour is a Neumann edge.  Every free texel reaches a seam texel through free
+ *    texels of decreasing d, so A is irreducibly diagonally dominant, hence symmetric positive definite.
+ * 6. Solve: Jacobi-preconditioned CG from delta = 0 in one cooperative kernel, every dot product in coop.cuh's
+ *    three-level order; it stops when r.r <= tol^2 b.b (status 0; 0 iterations when b = 0) or after maxIterations
+ *    (status 3).  Status 1: no seam texel; the atlas is copied bit for bit.
+ * 7. Output, texel by texel: a seam texel becomes float(f*), a free texel float(g + delta), every other texel (fixed,
+ *    outside the domain or outside every chart) is copied bit for bit.  Padding texels beyond a seam line are free
+ *    texels, so bilinear filtering across the seam reads levelled data.
+ * - Outputs: d_outAtlas [atlasRows][atlasWidth] (a separate buffer).  info_out [3] (may be NULL): the sum over seam
+ *   texels of (f* - g)^2 in texel order by coop.cuh's three-level order, the true relative residual
+ *   sqrt(|b - A delta|^2 / |b|^2) (0 when b = 0), and max |delta| over the free texels.  stats_out [8] (may be NULL):
+ *   seen faces, seam edges, samples (sum of S), seam texels, free texels, domain texels, CG iterations, status.
+ *   Returns the free-texel count, or CS_E_*.  numTriangles == 0: the atlas is copied, status 1.
+ * - Determinism: no floating-point atomics (max |delta| by an integer max of its bits); two calls give the same bytes.
+ * - Launches (cs_launch_count): 15 + stripWidth whatever the data (validate, chart check; keys, adjacency, unknowns,
+ *   sample counts; texel keys, domain; samples, run heads, seam texels; stripWidth relaxation rounds, free flags;
+ *   system; one cooperative solve kernel; output), 2 when the input is invalid; plus cub's sorts and scans (not
+ *   counted).  The host reads a few words after the input check, the seam edges, the domain and the strip (one
+ *   synchronise each) and after the output; *ms (may be NULL) gets the event time of the whole call.
+ * - Scratch, allocated on the call's stream and freed before it returns: 244 bytes per face (edge and unknown keys
+ *   and their corners, flags and scans, sample counts), 28 bytes per atlas texel (texel key, chart, two distances,
+ *   seam index, free-texel scan), 88 bytes per sample (two slots: texel and target and their sorted copies, run head
+ *   and scan, seam texel and f*), 80 bytes per free texel (neighbour codes and the CG vectors) plus 24 per 2048, 4 per
+ *   atlas row and 32 per chart plus 4 per chart row, plus cub's storage.
+ * - CS_E_ARG, before any CUDA call, naming the argument: cs_level_texture_seams's checks of the mesh, the atlas, the
+ *   padding, maxIterations, tol and the chart table (including overlapping rectangles); stripWidth outside [1, 128];
+ *   NULL or misaligned buffers as there; and d_outAtlas overlapping an input (one sweep over sorted ranges). */
+int cs_level_texture_seams_local(const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                                 const int *d_faceView, const float *d_uv, const int *charts, int numCharts,
+                                 const float *d_atlas, int atlasRows, int atlasWidth, int padding, int stripWidth,
+                                 int maxIterations, double tol, float *d_outAtlas, double info_out[3],
+                                 long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
