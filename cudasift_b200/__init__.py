@@ -1517,6 +1517,24 @@ def TextureMesh(images, Ks, Rs, ts, vertices, triangles, smoothness=0.5, maxView
             b.free()
 
 
+def _seams_inputs(bufs, vertices, triangles, atlas, uv, labels, charts):
+    """The inputs of LevelTextureSeams and LevelTextureSeamsLocal as the C calls take them: the vertices, triangles,
+    labels, uv and atlas in device buffers (appended to bufs, which the caller frees) and the chart table on the host.
+    Returns (device buffers in that order, chart table, V, T, atlas rows, atlas width)."""
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    A = np.ascontiguousarray(np.asarray(atlas, np.float32))
+    U = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 3, 2))
+    Lb = np.ascontiguousarray(np.asarray(labels, np.int32).reshape(-1))
+    Ct = np.ascontiguousarray(np.asarray(charts, np.int32).reshape(-1, 8))
+    ins = [DeviceBuffer(max(a.nbytes, 4)) for a in (X, F, Lb, U, A)]
+    bufs += ins
+    for b, a in zip(ins, (X, F, Lb, U, A)):
+        if a.size:
+            b.upload(a)
+    return ins, Ct, len(X), len(F), A.shape[0], A.shape[1]
+
+
 def LevelTextureSeams(vertices, triangles, atlas, uv, labels, charts, padding=2, smoothness=0.1, regularization=1e-3,
                       maxIterations=1000, tol=1e-4):
     """Global seam levelling of a textured mesh (cs_level_texture_seams): one additive offset per (vertex, image) pair,
@@ -1525,21 +1543,10 @@ def LevelTextureSeams(vertices, triangles, atlas, uv, labels, charts, padding=2,
     The inputs are TextureMesh's outputs as it returns them (padding the value given to it); no image is needed.
     Returns (levelled atlas float32 [rows, width], corner offsets float32 [T, 3] (NaN for an unseen face), info
     float64 [3] {seam energy before, after, relative residual}, stats int64 [8] (the header's), ms)."""
-    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
-    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
-    A = np.ascontiguousarray(np.asarray(atlas, np.float32))
-    U = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 3, 2))
-    Lb = np.ascontiguousarray(np.asarray(labels, np.int32).reshape(-1))
-    Ct = np.ascontiguousarray(np.asarray(charts, np.int32).reshape(-1, 8))
-    V, T, (H, W) = len(X), len(F), A.shape
     bufs = []
     try:
-        ins = [DeviceBuffer(max(a.nbytes, 4)) for a in (X, F, Lb, U, A)]
-        bufs += ins
-        for b, a in zip(ins, (X, F, Lb, U, A)):
-            if a.size:
-                b.upload(a)
-        outs = [DeviceBuffer(max(A.nbytes, 4)), DeviceBuffer(12 * T + 4)]
+        ins, Ct, V, T, H, W = _seams_inputs(bufs, vertices, triangles, atlas, uv, labels, charts)
+        outs = [DeviceBuffer(max(4 * H * W, 4)), DeviceBuffer(12 * T + 4)]
         bufs += outs
         info, stats, ms = np.zeros(3), np.zeros(8, np.int64), ctypes.c_double(0.0)
         _check(lib().cs_level_texture_seams(ins[0].ptr, V, ins[1].ptr, T, ins[2].ptr, ins[3].ptr, _ptr(Ct), len(Ct),
@@ -1563,21 +1570,10 @@ def LevelTextureSeamsLocal(vertices, triangles, atlas, uv, labels, charts, paddi
     the inputs are TextureMesh's (padding the value given to it) with the atlas replaced.  Returns (levelled atlas
     float32 [rows, width], info float64 [3] {sum (f* - g)^2 over seam texels, relative residual, max |delta|}, stats
     int64 [8] (the header's), ms)."""
-    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
-    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
-    A = np.ascontiguousarray(np.asarray(atlas, np.float32))
-    U = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 3, 2))
-    Lb = np.ascontiguousarray(np.asarray(labels, np.int32).reshape(-1))
-    Ct = np.ascontiguousarray(np.asarray(charts, np.int32).reshape(-1, 8))
-    V, T, (H, W) = len(X), len(F), A.shape
     bufs = []
     try:
-        ins = [DeviceBuffer(max(a.nbytes, 4)) for a in (X, F, Lb, U, A)]
-        bufs += ins
-        for b, a in zip(ins, (X, F, Lb, U, A)):
-            if a.size:
-                b.upload(a)
-        out = DeviceBuffer(max(A.nbytes, 4))
+        ins, Ct, V, T, H, W = _seams_inputs(bufs, vertices, triangles, atlas, uv, labels, charts)
+        out = DeviceBuffer(max(4 * H * W, 4))
         bufs.append(out)
         info, stats, ms = np.zeros(3), np.zeros(8, np.int64), ctypes.c_double(0.0)
         _check(lib().cs_level_texture_seams_local(ins[0].ptr, V, ins[1].ptr, T, ins[2].ptr, ins[3].ptr, _ptr(Ct),

@@ -312,6 +312,46 @@ __device__ __forceinline__ double seams_energy(const SeamsParams &p, int r, cons
   return e * e;
 }
 
+// Jacobi-PCG over N unknowns and P's x, r, z, q, diag, maxIt and totals (partA, groupA for r.r and r.z; partB, groupB
+// for p.q), from rr = r.r and rz = r.z totalled to the stop: r.r <= thr, maxIt iterations, or p.q not positive.
+// Returns the iteration count.  product(it, beta) writes p = z + beta p_old, q = A p and the tile partials of p.q into
+// partB, and returns the p it wrote.  N, t2 and t1 come from the caller: with the loop's own copies, the solve kernels
+// compile to other instructions.
+template <class P, class Product>
+__device__ __forceinline__ int seams_pcg(cg::grid_group &grid, const P &p, int N, double thr, double &rr, double rz,
+                                         double (&t2)[2], double (&t1)[1], Product product)
+{
+  double beta = 0.0;
+  int it = 0;
+  while (it < p.maxIt && !(rr <= thr)) {
+    const double *pv = product(it, beta);
+    grid.sync();
+    co_tree_groups<1, MT>(N, p.partB, p.groupB);
+    grid.sync();
+    co_tree_total<1, MT>(N, p.groupB, t1);
+    if (!(t1[0] > 0.0)) break;
+    const double alpha = rz / t1[0];
+    // x += alpha p, r -= alpha q, z = r / diag; the totals of r.r and r.z
+    co_tree_tiles<2, MT>(N, p.partA, [&](int i, double *v) {
+      p.x[i] = p.x[i] + alpha * pv[i];
+      const double rv = p.r[i] - alpha * p.q[i], zv = rv / p.diag[i];
+      p.r[i] = rv;
+      p.z[i] = zv;
+      v[0] += rv * rv;
+      v[1] += rv * zv;
+    });
+    it++;
+    grid.sync();
+    co_tree_groups<2, MT>(N, p.partA, p.groupA);
+    grid.sync();
+    co_tree_total<2, MT>(N, p.groupA, t2);
+    rr = t2[0];
+    beta = t2[1] / rz;
+    rz = t2[1];
+  }
+  return it;
+}
+
 __global__ void __launch_bounds__(MT) seams_solve_kernel(SeamsParams p)
 {
   cg::grid_group grid = cg::this_grid();
@@ -352,16 +392,15 @@ __global__ void __launch_bounds__(MT) seams_solve_kernel(SeamsParams p)
   co_tree_total<2, MT>(N, p.groupA, t2);
   co_tree_total<1, MT>(p.Rs, p.groupE, e0);
   const double bb = t2[0], thr = p.tol2 * bb;
-  double rr = t2[0], rz = t2[1], beta = 0.0;
-  int it = 0;
-  while (it < p.maxIt && !(rr <= thr)) {
+  double rr = t2[0];
+  const int it = seams_pcg(grid, p, N, thr, rr, t2[1], t2, t1, [&](int, double beta) {
     // 2. the pieces of sum w p_other, p = z + beta p_old of the other unknown
     co_pieces<1, 1, SL_PV, MT>(p.ikeyS, p.ivalS, p.pieces, n, p.unk, [&](int code, int, double *v) {
       const int r = code >> 1, o = (code & 1) ? p.ri[r] : p.rj[r];
       v[0] = p.rw[r] * (p.z[o] + beta * p.p[o]);
     });
     grid.sync();
-    // 3. p = z + beta p_old, q = A p = diag p - sum w p_other; the total of p.q
+    // 3. p = z + beta p_old, q = A p = diag p - sum w p_other; the partials of p.q
     co_tree_tiles<1, MT>(N, p.partB, [&](int i, double *v) {
       double Wp[1];
       co_gather<1, 1, SL_PV>(p.pieces, i, p.unk[i], Wp);
@@ -370,30 +409,8 @@ __global__ void __launch_bounds__(MT) seams_solve_kernel(SeamsParams p)
       p.q[i] = qv;
       v[0] += pn * qv;
     });
-    grid.sync();
-    co_tree_groups<1, MT>(N, p.partB, p.groupB);
-    grid.sync();
-    co_tree_total<1, MT>(N, p.groupB, t1);
-    if (!(t1[0] > 0.0)) break;
-    const double alpha = rz / t1[0];
-    // 4. x += alpha p, r -= alpha q, z = r / diag; the totals of r.r and r.z
-    co_tree_tiles<2, MT>(N, p.partA, [&](int i, double *v) {
-      p.x[i] = p.x[i] + alpha * p.p[i];
-      const double rv = p.r[i] - alpha * p.q[i], zv = rv / p.diag[i];
-      p.r[i] = rv;
-      p.z[i] = zv;
-      v[0] += rv * rv;
-      v[1] += rv * zv;
-    });
-    it++;
-    grid.sync();
-    co_tree_groups<2, MT>(N, p.partA, p.groupA);
-    grid.sync();
-    co_tree_total<2, MT>(N, p.groupA, t2);
-    rr = t2[0];
-    beta = t2[1] / rz;
-    rz = t2[1];
-  }
+    return (const double *)p.p;
+  });
   // 5. the true residual b - A x and the seam energy after; the corner offsets
   co_pieces<1, 1, SL_PV, MT>(p.ikeyS, p.ivalS, p.pieces, n, p.unk, [&](int code, int, double *v) {
     const int r = code >> 1, o = (code & 1) ? p.ri[r] : p.rj[r];
@@ -540,55 +557,191 @@ static void seams_row_index(const int *charts, int numCharts, int atlasRows, std
       rowList[fill[y]++] = c;
 }
 
+// info_out and stats_out (either may be NULL) from the call's seven counts and three info words; status 2 writes 0
+// but for the status.
+static void seams_report(int status, const long long (&words)[7], const double (&inf)[3], double *info,
+                         long long *stats)
+{
+  if (info)
+    for (int k = 0; k < 3; k++) info[k] = status == 2 ? 0.0 : inf[k];
+  if (stats) {
+    for (int k = 0; k < 7; k++) stats[k] = status == 2 ? 0 : words[k];
+    stats[7] = status;
+  }
+}
+
+// No face: the atlas copied, status 1.
+static int seams_no_faces(const float *atlas, float *outAtlas, size_t atlasBytes, cudaStream_t st, double *info,
+                          long long *stats)
+{
+  if (atlasBytes) CS_CUDA(cudaMemcpyAsync(outAtlas, atlas, atlasBytes, cudaMemcpyDeviceToDevice, st));
+  CS_CUDA(cudaStreamSynchronize(st));
+  const long long words[7] = {};
+  const double inf[3] = {};
+  seams_report(1, words, inf, info, stats);
+  return 0;
+}
+
+// The host side of both calls up to their own stages: the row index, the scratch of the input check and the edge stage
+// (and SeamsParams's pointers into it), the result words, the input check and the edge stage.  A call takes its own
+// buffers from L between the constructor and alloc(); the scratch is freed on the stream when the object goes.
+struct SeamsHost {
+  SeamsParams &p;
+  const int *charts;
+  int numCharts;
+  size_t resBytes;                            // the caller's result words, SeamsResult first
+  void *h_res;
+  cudaStream_t st;
+  cudaEvent_t *tev = match_timing_events();
+  std::vector<int> rowStart, rowList;
+  Layout L{256};
+  size_t resAt, ctabAt, rsAt, rlAt, fcAt, ekAt, ekSAt, ukAt, ukSAt, evAt, evSAt, uvAt, uvSAt, nbrAt, uhAt, usAt, sfAt,
+      ssAt, cuAt;
+  char *base = nullptr;
+  void *temp = nullptr;
+  size_t tempB = 0;
+
+  SeamsHost(SeamsParams &p_, const float *vin, int V, const int *tin, int T, const int *faceView, const float *uv,
+            const int *charts_, int numCharts_, const float *atlas, int atlasRows, int atlasWidth, int padding,
+            float *outAtlas, size_t resBytes_, void *h_res_, cudaStream_t st_)
+      : p(p_), charts(charts_), numCharts(numCharts_), resBytes(resBytes_), h_res(h_res_), st(st_)
+  {
+    p.V = V;
+    p.T = T;
+    p.vin = vin;
+    p.tin = tin;
+    p.view = faceView;
+    p.uv = uv;
+    p.atlas = atlas;
+    p.out = outAtlas;
+    p.rows = atlasRows;
+    p.width = atlasWidth;
+    p.padding = padding;
+    seams_row_index(charts, numCharts, atlasRows, rowStart, rowList);
+    const size_t C3 = 3 * (size_t)T;
+    resAt = L.take(resBytes);
+    ctabAt = L.take(std::max(1, numCharts) * 32ull), rsAt = L.take(rowStart.size() * 4);
+    rlAt = L.take(rowList.size() * 4);
+    fcAt = L.take((size_t)T * 4);
+    ekAt = L.take(C3 * 8), ekSAt = L.take(C3 * 8), ukAt = L.take(C3 * 8), ukSAt = L.take(C3 * 8);
+    evAt = L.take(C3 * 4), evSAt = L.take(C3 * 4), uvAt = L.take(C3 * 4), uvSAt = L.take(C3 * 4);
+    nbrAt = L.take(C3 * 4);
+    uhAt = L.take(C3 * 4), usAt = L.take(C3 * 4), sfAt = L.take(C3 * 4), ssAt = L.take(C3 * 4), cuAt = L.take(C3 * 4);
+  }
+  ~SeamsHost()
+  {
+    if (base) cudaFreeAsync(base, st);
+  }
+  char *at(size_t off) const { return base + off; }
+
+  // The scratch, with cub's storage for the edge stage's sorts and scans and for the caller's cubBytes.
+  int alloc(size_t cubBytes)
+  {
+    const int n3 = 3 * p.T;
+    size_t tb[2] = {};
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (unsigned long long *)nullptr,
+                                            (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, n3, 0, 64,
+                                            st));
+    CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb[1], (int *)nullptr, (int *)nullptr, n3, st));
+    tempB = std::max(std::max(tb[0], tb[1]), cubBytes);
+    const size_t tempAt = L.take(tempB);
+    CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
+    temp = at(tempAt);
+    p.res = reinterpret_cast<SeamsResult *>(at(resAt));
+    p.ctab = reinterpret_cast<const int *>(at(ctabAt));
+    p.rowStart = reinterpret_cast<const int *>(at(rsAt));
+    p.rowList = reinterpret_cast<const int *>(at(rlAt));
+    p.faceChart = reinterpret_cast<int *>(at(fcAt));
+    p.ekey = reinterpret_cast<unsigned long long *>(at(ekAt));
+    p.ekeyS = reinterpret_cast<unsigned long long *>(at(ekSAt));
+    p.ukey = reinterpret_cast<unsigned long long *>(at(ukAt));
+    p.ukeyS = reinterpret_cast<unsigned long long *>(at(ukSAt));
+    p.eval = reinterpret_cast<int *>(at(evAt));
+    p.evalS = reinterpret_cast<int *>(at(evSAt));
+    p.uval = reinterpret_cast<int *>(at(uvAt));
+    p.uvalS = reinterpret_cast<int *>(at(uvSAt));
+    p.nbr = reinterpret_cast<int *>(at(nbrAt));
+    p.uHead = reinterpret_cast<int *>(at(uhAt));
+    p.uScan = reinterpret_cast<int *>(at(usAt));
+    p.seFlag = reinterpret_cast<int *>(at(sfAt));
+    p.seScan = reinterpret_cast<int *>(at(ssAt));
+    p.cornerUnk = reinterpret_cast<int *>(at(cuAt));
+    return 0;
+  }
+
+  // the result words to the host (one synchronise)
+  int readback()
+  {
+    CS_CUDA(cudaMemcpyAsync(h_res, p.res, resBytes, cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
+
+  // the count of a flag list: the last entry of its inclusive scan, into a result word
+  int last(int *word, const int *scan, int n)
+  {
+    if (n > 0) CS_CUDA(cudaMemcpyAsync(word, scan + n - 1, 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+
+  // Rule 1: the result words cleared, the chart table and its row index uploaded, the mesh and every seen face's chart
+  // checked, and the words read back; bad when the input is invalid (status 2).
+  int check(bool &bad)
+  {
+    int r;
+    if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
+    CS_CUDA(cudaMemsetAsync(p.res, 0, resBytes, st));
+    if (numCharts) CS_CUDA(cudaMemcpyAsync(at(ctabAt), charts, (size_t)numCharts * 32, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(at(rsAt), rowStart.data(), rowStart.size() * 4, cudaMemcpyHostToDevice, st));
+    CS_CUDA(cudaMemcpyAsync(at(rlAt), rowList.data(), rowList.size() * 4, cudaMemcpyHostToDevice, st));
+    mesh_validate_kernel<<<grid_of(p.T), MT, 0, st>>>(p.vin, p.V, p.tin, p.T, &p.res->bad);
+    seams_check_kernel<<<grid_of(p.T), MT, 0, st>>>(p);
+    count_launch(2);
+    CS_CUDA(cudaGetLastError());
+    if ((r = readback()) < 0) return r;
+    bad = static_cast<SeamsResult *>(h_res)->bad;
+    return 0;
+  }
+
+  // The edges (rules 2 and 3): the adjacency, every corner's unknown and the seam edge flags and their scans.
+  int edges()
+  {
+    const int n3 = 3 * p.T;
+    if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
+    seams_keys_kernel<<<grid_of(3ll * p.T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ekey, p.ekeyS, p.eval, p.evalS, n3, 0, 64, st));
+    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ukey, p.ukeyS, p.uval, p.uvalS, n3, 0, 64, st));
+    seams_adjacency_kernel<<<grid_of(3ll * p.T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.uHead, p.uScan, n3, st));
+    seams_unknown_kernel<<<grid_of(3ll * p.T), MT, 0, st>>>(p);
+    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.seFlag, p.seScan, n3, st));
+    count_launch(3);
+    CS_CUDA(cudaGetLastError());
+    return 0;
+  }
+};
+
 int seams_run(const float *vin, int V, const int *tin, int T, const int *faceView, const float *uv, const int *charts,
               int numCharts, const float *atlas, int atlasRows, int atlasWidth, int padding, double smoothness,
               double regularization, int maxIterations, double tol, float *outAtlas, float *cornerOffset,
               cudaStream_t st, void *h_res, double *info, long long *stats)
 {
   const size_t atlasBytes = (size_t)atlasRows * atlasWidth * 4;
-  long long st_[8] = {};
-  double info_[3] = {};
-  auto finish = [&](int status) {
-    st_[7] = status;
-    if (info)
-      for (int k = 0; k < 3; k++) info[k] = status == 2 ? 0.0 : info_[k];
-    if (stats)
-      for (int k = 0; k < 8; k++) stats[k] = st_[k];
-  };
-  if (T == 0) {                                // no face: no seam row, the atlas copied
-    if (atlasBytes) CS_CUDA(cudaMemcpyAsync(outAtlas, atlas, atlasBytes, cudaMemcpyDeviceToDevice, st));
-    CS_CUDA(cudaStreamSynchronize(st));
-    finish(1);
-    return 0;
-  }
+  if (T == 0) return seams_no_faces(atlas, outAtlas, atlasBytes, st, info, stats);   // no seam row
 
-  std::vector<int> rowStart, rowList;
-  seams_row_index(charts, numCharts, atlasRows, rowStart, rowList);
-
+  SeamsParams p{};
+  SeamsHost H(p, vin, V, tin, T, faceView, uv, charts, numCharts, atlas, atlasRows, atlasWidth, padding, outAtlas,
+              sizeof(SeamsResult), h_res, st);
   const size_t C3 = 3 * (size_t)T, E2 = C3, R2 = 2 * (2 * C3);   // seam ends <= 3T, rows <= 2 (3T)
-  size_t tb[4] = {};
-  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (unsigned long long *)nullptr,
-                                          (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, (int)C3, 0,
-                                          64, st));
-  CS_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb[1], (unsigned long long *)nullptr,
+  size_t tb[2] = {};
+  CS_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tb[0], (unsigned long long *)nullptr,
                                          (unsigned long long *)nullptr, (int)C3, 0, 64, st));
-  CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb[2], (int *)nullptr, (int *)nullptr, (int)C3, st));
-  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[3], (int *)nullptr, (int *)nullptr, (int *)nullptr,
+  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[1], (int *)nullptr, (int *)nullptr, (int *)nullptr,
                                           (int *)nullptr, (int)R2, 0, 32, st));
-  const size_t tempBytes = std::max(std::max(tb[0], tb[1]), std::max(tb[2], tb[3]));
   const int tiles3 = (int)((C3 + CO_TREE_TILE - 1) / CO_TREE_TILE), groups3 = (tiles3 + MT - 1) / MT;
 
-  Layout L(256);
-  const size_t resAt = L.take(sizeof(SeamsResult));
-  const size_t ctabAt = L.take(std::max(1, numCharts) * 32ull), rsAt = L.take(rowStart.size() * 4),
-               rlAt = L.take(rowList.size() * 4);
-  const size_t fcAt = L.take((size_t)T * 4);
-  const size_t ekAt = L.take(C3 * 8), ekSAt = L.take(C3 * 8), ukAt = L.take(C3 * 8), ukSAt = L.take(C3 * 8),
-               skSAt = L.take(C3 * 8);
-  const size_t evAt = L.take(C3 * 4), evSAt = L.take(C3 * 4), uvAt = L.take(C3 * 4), uvSAt = L.take(C3 * 4),
-               nbrAt = L.take(C3 * 4);
-  const size_t uhAt = L.take(C3 * 4), usAt = L.take(C3 * 4), sfAt = L.take(C3 * 4), ssAt = L.take(C3 * 4),
-               shAt = L.take(C3 * 4), shsAt = L.take(C3 * 4), cuAt = L.take(C3 * 4);
+  Layout &L = H.L;
+  const size_t skSAt = L.take(C3 * 8), shAt = L.take(C3 * 4), shsAt = L.take(C3 * 4);
   const size_t xkAt = L.take(E2 * 8), xkSAt = L.take(E2 * 8), xvAt = L.take(E2 * 4), xvSAt = L.take(E2 * 4),
                xhAt = L.take(E2 * 4), xsAt = L.take(E2 * 4), xsumAt = L.take(E2 * 24);
   const size_t Rmax = 2 * C3;                 // seam rows <= seam ends, smoothness rows <= corners
@@ -602,46 +755,13 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
                partBAt = L.take((size_t)tiles3 * 8), groupBAt = L.take((size_t)groups3 * 8),
                partEAt = L.take((size_t)tiles3 * 8), groupEAt = L.take((size_t)groups3 * 8);
   const size_t tkeyAt = L.take(atlasBytes * 2);
-  const size_t tempAt = L.take(tempBytes);
-  char *base = nullptr;
-  CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
-  auto at = [&](size_t off) { return base + off; };
+  if (const int e = H.alloc(std::max(tb[0], tb[1])); e < 0) return e;
+  auto at = [&](size_t off) { return H.at(off); };
 
-  SeamsParams p{};
-  p.res = reinterpret_cast<SeamsResult *>(at(resAt));
-  p.V = V;
-  p.T = T;
-  p.vin = vin;
-  p.tin = tin;
-  p.view = faceView;
-  p.uv = uv;
-  p.atlas = atlas;
-  p.out = outAtlas;
   p.corner = cornerOffset;
-  p.rows = atlasRows;
-  p.width = atlasWidth;
-  p.padding = padding;
-  p.ctab = reinterpret_cast<const int *>(at(ctabAt));
-  p.rowStart = reinterpret_cast<const int *>(at(rsAt));
-  p.rowList = reinterpret_cast<const int *>(at(rlAt));
-  p.faceChart = reinterpret_cast<int *>(at(fcAt));
-  p.ekey = reinterpret_cast<unsigned long long *>(at(ekAt));
-  p.ekeyS = reinterpret_cast<unsigned long long *>(at(ekSAt));
-  p.ukey = reinterpret_cast<unsigned long long *>(at(ukAt));
-  p.ukeyS = reinterpret_cast<unsigned long long *>(at(ukSAt));
   p.skeyS = reinterpret_cast<unsigned long long *>(at(skSAt));
-  p.eval = reinterpret_cast<int *>(at(evAt));
-  p.evalS = reinterpret_cast<int *>(at(evSAt));
-  p.uval = reinterpret_cast<int *>(at(uvAt));
-  p.uvalS = reinterpret_cast<int *>(at(uvSAt));
-  p.nbr = reinterpret_cast<int *>(at(nbrAt));
-  p.uHead = reinterpret_cast<int *>(at(uhAt));
-  p.uScan = reinterpret_cast<int *>(at(usAt));
-  p.seFlag = reinterpret_cast<int *>(at(sfAt));
-  p.seScan = reinterpret_cast<int *>(at(ssAt));
   p.sHead = reinterpret_cast<int *>(at(shAt));
   p.sScan = reinterpret_cast<int *>(at(shsAt));
-  p.cornerUnk = reinterpret_cast<int *>(at(cuAt));
   p.xkey = reinterpret_cast<unsigned long long *>(at(xkAt));
   p.xkeyS = reinterpret_cast<unsigned long long *>(at(xkSAt));
   p.xval = reinterpret_cast<int *>(at(xvAt));
@@ -680,59 +800,33 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
   p.reg = regularization;
   p.tol2 = tol * tol;
   p.maxIt = maxIterations;
-  void *temp = at(tempAt);
-  size_t tempB = tempBytes;
+  void *temp = H.temp;
+  size_t tempB = H.tempB;
   SeamsResult &R = *static_cast<SeamsResult *>(h_res);
-  cudaEvent_t *tev = match_timing_events();
+  cudaEvent_t *tev = H.tev;
   const int n3 = (int)C3;
 
   int status = 0;
-  auto readback = [&]() -> int {
-    CS_CUDA(cudaMemcpyAsync(h_res, p.res, sizeof(SeamsResult), cudaMemcpyDeviceToHost, st));
-    CS_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  };
-  // the count of a flag list: the last entry of its inclusive scan, into a result word
-  auto last = [&](int *word, const int *scan, int n) -> int {
-    if (n > 0) CS_CUDA(cudaMemcpyAsync(word, scan + n - 1, 4, cudaMemcpyDeviceToDevice, st));
-    return 0;
-  };
   auto run = [&]() -> int {
     int r;
-    if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
-    CS_CUDA(cudaMemsetAsync(p.res, 0, sizeof(SeamsResult), st));
-    if (numCharts)
-      CS_CUDA(cudaMemcpyAsync(at(ctabAt), charts, (size_t)numCharts * 32, cudaMemcpyHostToDevice, st));
-    CS_CUDA(cudaMemcpyAsync(at(rsAt), rowStart.data(), rowStart.size() * 4, cudaMemcpyHostToDevice, st));
-    CS_CUDA(cudaMemcpyAsync(at(rlAt), rowList.data(), rowList.size() * 4, cudaMemcpyHostToDevice, st));
-    mesh_validate_kernel<<<grid_of(T), MT, 0, st>>>(vin, V, tin, T, &p.res->bad);
-    seams_check_kernel<<<grid_of(T), MT, 0, st>>>(p);
-    count_launch(2);
-    CS_CUDA(cudaGetLastError());
-    if ((r = readback()) < 0) return r;
-    if (R.bad) {
+    bool bad;
+    if ((r = H.check(bad)) < 0) return r;
+    if (bad) {
       status = 2;
       return 0;
     }
     // unknowns, adjacency, smoothness rows, seam edges
-    if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
-    seams_keys_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
-    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ekey, p.ekeyS, p.eval, p.evalS, n3, 0, 64, st));
-    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ukey, p.ukeyS, p.uval, p.uvalS, n3, 0, 64, st));
-    seams_adjacency_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
-    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.uHead, p.uScan, n3, st));
-    seams_unknown_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
-    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.seFlag, p.seScan, n3, st));
+    if ((r = H.edges()) < 0) return r;
     seams_smooth_keys_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
     CS_CUDA(cub::DeviceRadixSort::SortKeys(temp, tempB, p.ukey, p.skeyS, n3, 0, 64, st));
     seams_smooth_heads_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
     CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.sHead, p.sScan, n3, st));
-    count_launch(5);
+    count_launch(2);
     CS_CUDA(cudaGetLastError());
-    if ((r = last(&p.res->unknowns, p.uScan, n3)) < 0) return r;
-    if ((r = last(&p.res->seamEdges, p.seScan, n3)) < 0) return r;
-    if ((r = last(&p.res->smoothRows, p.sScan, n3)) < 0) return r;
-    if ((r = readback()) < 0) return r;
+    if ((r = H.last(&p.res->unknowns, p.uScan, n3)) < 0) return r;
+    if ((r = H.last(&p.res->seamEdges, p.seScan, n3)) < 0) return r;
+    if ((r = H.last(&p.res->smoothRows, p.sScan, n3)) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     p.N = R.unknowns;
     p.E = R.seamEdges;
     p.Rm = R.smoothRows;
@@ -744,8 +838,8 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
     CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.xHead, p.xScan, 2 * p.E, st));
     count_launch(2);
     CS_CUDA(cudaGetLastError());
-    if ((r = last(&p.res->seamRows, p.xScan, 2 * p.E)) < 0) return r;
-    if ((r = readback()) < 0) return r;
+    if ((r = H.last(&p.res->seamRows, p.xScan, 2 * p.E)) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     p.Rs = R.seamRows;
     p.copyAll = p.Rs == 0;
     const int nInc = 2 * (p.Rs + p.Rm);
@@ -770,7 +864,7 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     if (tev) CS_CUDA(cudaEventRecord(tev[5], st));
-    if ((r = readback()) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     status = p.Rs == 0 ? 1 : R.converged ? 0 : 3;
     if (tev) {
       static const char *const names[5] = {"check", "unknowns", "seam rows", "solve", "texels"};
@@ -780,19 +874,9 @@ int seams_run(const float *vin, int V, const int *tin, int T, const int *faceVie
     return 0;
   };
   const int r = run();
-  cudaFreeAsync(base, st);
   if (r < 0) return r;
-  if (status != 2) {
-    st_[0] = R.seen;
-    st_[1] = R.unknowns;
-    st_[2] = R.seamEdges;
-    st_[3] = R.seamRows;
-    st_[4] = R.smoothRows;
-    st_[5] = R.iters;
-    st_[6] = (long long)R.texels;
-    for (int k = 0; k < 3; k++) info_[k] = R.info[k];
-  }
-  finish(status);
+  const long long words[7] = {R.seen, R.unknowns, R.seamEdges, R.seamRows, R.smoothRows, R.iters, (long long)R.texels};
+  seams_report(status, words, R.info, info, stats);
   return status == 2 ? 0 : R.unknowns;
 }
 
@@ -1018,42 +1102,19 @@ __global__ void __launch_bounds__(MT) local_solve_kernel(LocalParams q)
   co_tree_total<2, MT>(N, q.groupA, t2);
   co_tree_total<1, MT>(Ns, q.groupE, e0);
   const double bb = t2[0], thr = q.tol2 * bb;
-  double rr = t2[0], rz = t2[1], beta = 0.0;
-  int it = 0;
-  while (it < q.maxIt && !(rr <= thr)) {
+  double rr = t2[0];
+  const int it = seams_pcg(grid, q, N, thr, rr, t2[1], t2, t1, [&](int it, double beta) {
     const double *pold = (it & 1) ? q.pB : q.pA;
     double *pnew = (it & 1) ? q.pA : q.pB;
-    // p = z + beta p_old, q = A p; the total of p.q
+    // p = z + beta p_old, q = A p; the partials of p.q
     co_tree_tiles<1, MT>(N, q.partB, [&](int i, double *v) {
       const double pn = q.z[i] + beta * pold[i], qv = local_stencil(q, i, pn, q.z, pold, beta);
       pnew[i] = pn;
       q.q[i] = qv;
       v[0] += pn * qv;
     });
-    grid.sync();
-    co_tree_groups<1, MT>(N, q.partB, q.groupB);
-    grid.sync();
-    co_tree_total<1, MT>(N, q.groupB, t1);
-    if (!(t1[0] > 0.0)) break;
-    const double alpha = rz / t1[0];
-    // x += alpha p, r -= alpha q, z = r / diag; the totals of r.r and r.z
-    co_tree_tiles<2, MT>(N, q.partA, [&](int i, double *v) {
-      q.x[i] = q.x[i] + alpha * pnew[i];
-      const double rv = q.r[i] - alpha * q.q[i], zv = rv / q.diag[i];
-      q.r[i] = rv;
-      q.z[i] = zv;
-      v[0] += rv * rv;
-      v[1] += rv * zv;
-    });
-    it++;
-    grid.sync();
-    co_tree_groups<2, MT>(N, q.partA, q.groupA);
-    grid.sync();
-    co_tree_total<2, MT>(N, q.groupA, t2);
-    rr = t2[0];
-    beta = t2[1] / rz;
-    rz = t2[1];
-  }
+    return (const double *)pnew;
+  });
   // the true residual b - A x; max |x|
   unsigned long long mx = 0;
   co_tree_tiles<1, MT>(N, q.partB, [&](int i, double *v) {
@@ -1095,83 +1156,25 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
                     double *info, long long *stats)
 {
   const size_t n = (size_t)atlasRows * atlasWidth, atlasBytes = n * 4;
-  long long st_[8] = {};
-  double info_[3] = {};
-  auto finish = [&](int status) {
-    st_[7] = status;
-    if (info)
-      for (int k = 0; k < 3; k++) info[k] = status == 2 ? 0.0 : info_[k];
-    if (stats)
-      for (int k = 0; k < 8; k++) stats[k] = st_[k];
-  };
-  if (T == 0) {                                // no face: no seam texel, the atlas copied
-    if (atlasBytes) CS_CUDA(cudaMemcpyAsync(outAtlas, atlas, atlasBytes, cudaMemcpyDeviceToDevice, st));
-    CS_CUDA(cudaStreamSynchronize(st));
-    finish(1);
-    return 0;
-  }
-  std::vector<int> rowStart, rowList;
-  seams_row_index(charts, numCharts, atlasRows, rowStart, rowList);
-
-  const size_t C3 = 3 * (size_t)T;
-  size_t tb[4] = {};
-  CS_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb[0], (unsigned long long *)nullptr,
-                                          (unsigned long long *)nullptr, (int *)nullptr, (int *)nullptr, (int)C3, 0,
-                                          64, st));
-  CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb[1], (int *)nullptr, (int *)nullptr, (int)std::max(C3, n), st));
-  const size_t tempBytes = std::max(tb[0], tb[1]);
+  if (T == 0) return seams_no_faces(atlas, outAtlas, atlasBytes, st, info, stats);   // no seam texel
 
   // the first allocation: the mesh stage and the texel arrays
-  Layout L(256);
-  const size_t resAt = L.take(sizeof(LocalResult));
-  const size_t ctabAt = L.take(std::max(1, numCharts) * 32ull), rsAt = L.take(rowStart.size() * 4),
-               rlAt = L.take(rowList.size() * 4);
-  const size_t fcAt = L.take((size_t)T * 4);
-  const size_t ekAt = L.take(C3 * 8), ekSAt = L.take(C3 * 8), ukAt = L.take(C3 * 8), ukSAt = L.take(C3 * 8);
-  const size_t evAt = L.take(C3 * 4), evSAt = L.take(C3 * 4), uvAt = L.take(C3 * 4), uvSAt = L.take(C3 * 4),
-               nbrAt = L.take(C3 * 4);
-  const size_t uhAt = L.take(C3 * 4), usAt = L.take(C3 * 4), sfAt = L.take(C3 * 4), ssAt = L.take(C3 * 4),
-               cuAt = L.take(C3 * 4), scAt = L.take(C3 * 4), scsAt = L.take(C3 * 4);
-  const size_t tkeyAt = L.take(n * 8), chAt = L.take(n * 4), daAt = L.take(n * 4), dbAt = L.take(n * 4),
-               siAt = L.take(n * 4), uiAt = L.take(n * 4);
-  const size_t tempAt = L.take(tempBytes);
-  char *base = nullptr, *base2 = nullptr, *base3 = nullptr;
-  CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
-  auto at = [&](size_t off) { return base + off; };
-
   LocalParams q{};
   SeamsParams &p = q.s;
-  q.res = reinterpret_cast<LocalResult *>(at(resAt));
-  p.res = &q.res->g;
-  p.V = V;
-  p.T = T;
-  p.vin = vin;
-  p.tin = tin;
-  p.view = faceView;
-  p.uv = uv;
-  p.atlas = atlas;
-  p.out = outAtlas;
-  p.rows = atlasRows;
-  p.width = atlasWidth;
-  p.padding = padding;
-  p.ctab = reinterpret_cast<const int *>(at(ctabAt));
-  p.rowStart = reinterpret_cast<const int *>(at(rsAt));
-  p.rowList = reinterpret_cast<const int *>(at(rlAt));
-  p.faceChart = reinterpret_cast<int *>(at(fcAt));
-  p.ekey = reinterpret_cast<unsigned long long *>(at(ekAt));
-  p.ekeyS = reinterpret_cast<unsigned long long *>(at(ekSAt));
-  p.ukey = reinterpret_cast<unsigned long long *>(at(ukAt));
-  p.ukeyS = reinterpret_cast<unsigned long long *>(at(ukSAt));
-  p.eval = reinterpret_cast<int *>(at(evAt));
-  p.evalS = reinterpret_cast<int *>(at(evSAt));
-  p.uval = reinterpret_cast<int *>(at(uvAt));
-  p.uvalS = reinterpret_cast<int *>(at(uvSAt));
-  p.nbr = reinterpret_cast<int *>(at(nbrAt));
-  p.uHead = reinterpret_cast<int *>(at(uhAt));
-  p.uScan = reinterpret_cast<int *>(at(usAt));
-  p.seFlag = reinterpret_cast<int *>(at(sfAt));
-  p.seScan = reinterpret_cast<int *>(at(ssAt));
-  p.cornerUnk = reinterpret_cast<int *>(at(cuAt));
+  SeamsHost H(p, vin, V, tin, T, faceView, uv, charts, numCharts, atlas, atlasRows, atlasWidth, padding, outAtlas,
+              sizeof(LocalResult), h_res, st);
+  const size_t C3 = 3 * (size_t)T;
+  size_t cubB = 0;
+  CS_CUDA(cub::DeviceScan::InclusiveSum(nullptr, cubB, (int *)nullptr, (int *)nullptr, (int)std::max(C3, n), st));
+  Layout &L = H.L;
+  const size_t scAt = L.take(C3 * 4), scsAt = L.take(C3 * 4);
+  const size_t tkeyAt = L.take(n * 8), chAt = L.take(n * 4), daAt = L.take(n * 4), dbAt = L.take(n * 4),
+               siAt = L.take(n * 4), uiAt = L.take(n * 4);
+  if (const int e = H.alloc(cubB); e < 0) return e;
+  auto at = [&](size_t off) { return H.at(off); };
+  char *base2 = nullptr, *base3 = nullptr;
+
+  q.res = reinterpret_cast<LocalResult *>(p.res);
   p.tkey = reinterpret_cast<unsigned long long *>(at(tkeyAt));
   q.scnt = reinterpret_cast<int *>(at(scAt));
   q.sscan = reinterpret_cast<int *>(at(scsAt));
@@ -1184,56 +1187,31 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
   q.strip = stripWidth;
   q.maxIt = maxIterations;
   q.tol2 = tol * tol;
-  void *temp = at(tempAt);
-  size_t tempB = tempBytes;
+  void *temp = H.temp;
+  size_t tempB = H.tempB;
   LocalResult &R = *static_cast<LocalResult *>(h_res);
-  cudaEvent_t *tev = match_timing_events();
+  cudaEvent_t *tev = H.tev;
   const int n3 = (int)C3;
 
   int status = 0;
-  auto readback = [&]() -> int {
-    CS_CUDA(cudaMemcpyAsync(h_res, q.res, sizeof(LocalResult), cudaMemcpyDeviceToHost, st));
-    CS_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  };
-  auto last = [&](int *word, const int *scan, int len) -> int {
-    if (len > 0) CS_CUDA(cudaMemcpyAsync(word, scan + len - 1, 4, cudaMemcpyDeviceToDevice, st));
-    return 0;
-  };
   auto run = [&]() -> int {
     int r;
-    if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
-    CS_CUDA(cudaMemsetAsync(q.res, 0, sizeof(LocalResult), st));
-    if (numCharts)
-      CS_CUDA(cudaMemcpyAsync(at(ctabAt), charts, (size_t)numCharts * 32, cudaMemcpyHostToDevice, st));
-    CS_CUDA(cudaMemcpyAsync(at(rsAt), rowStart.data(), rowStart.size() * 4, cudaMemcpyHostToDevice, st));
-    CS_CUDA(cudaMemcpyAsync(at(rlAt), rowList.data(), rowList.size() * 4, cudaMemcpyHostToDevice, st));
-    mesh_validate_kernel<<<grid_of(T), MT, 0, st>>>(vin, V, tin, T, &p.res->bad);
-    seams_check_kernel<<<grid_of(T), MT, 0, st>>>(p);
-    count_launch(2);
-    CS_CUDA(cudaGetLastError());
-    if ((r = readback()) < 0) return r;
-    if (R.g.bad) {
+    bool bad;
+    if ((r = H.check(bad)) < 0) return r;
+    if (bad) {
       status = 2;
       return 0;
     }
     // the seam edges and their sample counts
-    if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
-    seams_keys_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
-    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ekey, p.ekeyS, p.eval, p.evalS, n3, 0, 64, st));
-    CS_CUDA(cub::DeviceRadixSort::SortPairs(temp, tempB, p.ukey, p.ukeyS, p.uval, p.uvalS, n3, 0, 64, st));
-    seams_adjacency_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
-    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.uHead, p.uScan, n3, st));
-    seams_unknown_kernel<<<grid_of(3ll * T), MT, 0, st>>>(p);
-    CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, p.seFlag, p.seScan, n3, st));
+    if ((r = H.edges()) < 0) return r;
     local_count_kernel<<<grid_of(3ll * T), MT, 0, st>>>(q);
-    count_launch(4);
+    count_launch();
     CS_CUDA(cudaGetLastError());
-    if ((r = last(&p.res->seamEdges, p.seScan, n3)) < 0) return r;
-    if ((r = readback()) < 0) return r;
+    if ((r = H.last(&p.res->seamEdges, p.seScan, n3)) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     p.E = R.g.seamEdges;
     CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, q.scnt, q.sscan, p.E, st));
-    if ((r = last(&q.res->samples, q.sscan, p.E)) < 0) return r;
+    if ((r = H.last(&q.res->samples, q.sscan, p.E)) < 0) return r;
     // the domain: texel keys, charts and distances
     if (tev) CS_CUDA(cudaEventRecord(tev[2], st));
     CS_CUDA(cudaMemsetAsync(p.tkey, 0xff, n * 8, st));
@@ -1241,7 +1219,7 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
     local_domain_kernel<<<grid_of((long long)n), MT, 0, st>>>(q);
     count_launch(2);
     CS_CUDA(cudaGetLastError());
-    if ((r = readback()) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     // the seam texels: the samples' slots sorted by texel, one run per seam texel
     if (tev) CS_CUDA(cudaEventRecord(tev[3], st));
     q.M = R.samples;
@@ -1273,7 +1251,7 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
     local_seam_kernel<<<grid_of((long long)S2), MT, 0, st>>>(q);
     count_launch(3);
     CS_CUDA(cudaGetLastError());
-    if ((r = last(&q.res->seamTexels, q.hscan, (int)S2)) < 0) return r;
+    if ((r = H.last(&q.res->seamTexels, q.hscan, (int)S2)) < 0) return r;
     // the strip: stripWidth relaxation rounds, the free texels numbered in atlas order
     if (tev) CS_CUDA(cudaEventRecord(tev[4], st));
     for (int k = 0; k < stripWidth; k++)
@@ -1284,8 +1262,8 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
     CS_CUDA(cub::DeviceScan::InclusiveSum(temp, tempB, flag, q.uidx, (int)n, st));
     count_launch(stripWidth + 1);
     CS_CUDA(cudaGetLastError());
-    if ((r = last(&q.res->freeTexels, q.uidx, (int)n)) < 0) return r;
-    if ((r = readback()) < 0) return r;
+    if ((r = H.last(&q.res->freeTexels, q.uidx, (int)n)) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     q.Ns = R.seamTexels;
     q.N = R.freeTexels;
     // the system and its solve
@@ -1328,7 +1306,7 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
     count_launch();
     CS_CUDA(cudaGetLastError());
     if (tev) CS_CUDA(cudaEventRecord(tev[7], st));
-    if ((r = readback()) < 0) return r;
+    if ((r = H.readback()) < 0) return r;
     status = q.Ns == 0 ? 1 : R.converged ? 0 : 3;
     if (tev) {
       static const char *const names[7] = {"check", "seam edges", "domain", "seam texels", "strip", "solve",
@@ -1341,22 +1319,13 @@ int seams_local_run(const float *vin, int V, const int *tin, int T, const int *f
   const int r = run();
   if (base3) cudaFreeAsync(base3, st);
   if (base2) cudaFreeAsync(base2, st);
-  cudaFreeAsync(base, st);
   if (r < 0) return r;
-  if (status != 2) {
-    st_[0] = R.g.seen;
-    st_[1] = R.g.seamEdges;
-    st_[2] = R.samples;
-    st_[3] = R.seamTexels;
-    st_[4] = R.freeTexels;
-    st_[5] = (long long)R.domain;
-    st_[6] = R.iters;
-    info_[0] = R.info[0];
-    info_[1] = R.info[1];
-    const unsigned long long bits = R.maxDelta;
-    std::memcpy(&info_[2], &bits, 8);
-  }
-  finish(status);
+  double inf[3] = {R.info[0], R.info[1], 0.0};
+  const unsigned long long bits = R.maxDelta;
+  std::memcpy(&inf[2], &bits, 8);
+  const long long words[7] = {R.g.seen, R.g.seamEdges, R.samples, R.seamTexels, R.freeTexels, (long long)R.domain,
+                              R.iters};
+  seams_report(status, words, inf, info, stats);
   return status == 2 ? 0 : R.freeTexels;
 }
 
