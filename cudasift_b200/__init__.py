@@ -126,6 +126,9 @@ def lib():
                                   c.POINTER(c.c_double)]),
         "cs_texture_mesh": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, c.c_double, c.c_double, c.c_double, ip, ip, ip,
                                  vp, ip, vp, vp, vp, vp, ip, vp, vp, c.POINTER(c.c_double)]),
+        "cs_texture_mesh_photo": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, c.c_double,
+                                       c.c_double, c.c_double, ip, ip, ip, vp, ip, vp, vp, vp, vp, ip, vp, vp,
+                                       c.POINTER(c.c_double)]),
         "cs_level_texture_seams": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, c.c_double, c.c_double, ip,
                                         c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_level_texture_seams_local": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, ip, ip, c.c_double, vp,
@@ -1474,6 +1477,33 @@ def TextureMesh(images, Ks, Rs, ts, vertices, triangles, smoothness=0.5, maxView
     nothing is truncated.  Returns (atlas float32 [rows, atlasWidth], uv float32 [T, 3, 2] in atlas pixels (NaN for an
     unseen face), labels int32 [T] (the image, -1 unseen), charts int32 [C, 8] {image, x0, y0, width, height, ox, oy,
     faces}, info float64 [2] {energy before, after the sweeps}, stats int64 [11] (the header's), ms)."""
+    return _texture_mesh("TextureMesh", lib().cs_texture_mesh, 11, images, Ks, Rs, ts, vertices,
+                         triangles, smoothness, maxViewAngle, depthTol, padding, atlasWidth, maxSweeps)
+
+
+def TextureMeshPhoto(images, Ks, Rs, ts, vertices, triangles, dataTerm="gmi", outlierK=3.0, outlierMinSigma=4.0,
+                     smoothness=0.5, maxViewAngle=75.0, depthTol=0.01, padding=2, atlasWidth=None, maxSweeps=100):
+    """TextureMesh with Waechter et al.'s view selection (cs_texture_mesh_photo): dataTerm "gmi" ranks a face's views
+    by the projected area times (1 + the mean Sobel magnitude over its visible pixels, in grey levels per pixel), so a
+    sharp view beats a blurred one of the same size ("area": TextureMesh's ranking); outlierK > 0 removes the views
+    whose mean intensity over the face lies more than outlierK max(1.4826 MAD, outlierMinSigma) from the median of its
+    views (MAD: the median absolute deviation), so an object seen in one view only (a passer-by) does not texture the
+    face; 0 turns the test off.  Images on a 0..255 scale.  The other arguments and the returned tuple are TextureMesh's,
+    with stats int64 [16]: TextureMesh's 11, then samples, centroid fallbacks, faces tested, candidates removed, faces
+    whose best candidate was removed."""
+    terms = {"area": 0, "gmi": 1}
+    if dataTerm not in terms:
+        raise ValueError("dataTerm: 'area' or 'gmi', not %r" % (dataTerm,))
+    extra = (terms[dataTerm], float(outlierK), float(outlierMinSigma))
+    return _texture_mesh("TextureMeshPhoto", lambda *a: lib().cs_texture_mesh_photo(*a[:9], *extra, *a[9:]), 16,
+                         images, Ks, Rs, ts, vertices, triangles, smoothness, maxViewAngle, depthTol, padding,
+                         atlasWidth, maxSweeps)
+
+
+def _texture_mesh(name, call, nstats, images, Ks, Rs, ts, vertices, triangles, smoothness, maxViewAngle,
+                  depthTol, padding, atlasWidth, maxSweeps):
+    """The body of TextureMesh and TextureMeshPhoto: call takes cs_texture_mesh's arguments (the photo call's three
+    settings inserted by the caller) and stats has nstats entries."""
     S = len(images)
     K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
     X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
@@ -1496,12 +1526,11 @@ def TextureMesh(images, Ks, Rs, ts, vertices, triangles, smoothness=0.5, maxView
             atlas = DeviceBuffer(4 * rows * W + 4)
             try:
                 charts = np.zeros((maxCharts, 8), np.int32)
-                info, stats, ms = np.zeros(2), np.zeros(11, np.int64), ctypes.c_double(0.0)
-                C = _check(lib().cs_texture_mesh(table if S else None, S, _ptr(K), _ptr(R), _ptr(t), ins[0].ptr, V,
-                                                 ins[1].ptr, T, float(smoothness), float(maxViewAngle),
-                                                 float(depthTol), int(padding), W, int(maxSweeps), atlas.ptr, rows,
-                                                 outs[0].ptr, outs[1].ptr, None, _ptr(charts), maxCharts, _ptr(info),
-                                                 _ptr(stats), ctypes.byref(ms)), "TextureMesh")
+                info, stats, ms = np.zeros(2), np.zeros(nstats, np.int64), ctypes.c_double(0.0)
+                C = _check(call(table if S else None, S, _ptr(K), _ptr(R), _ptr(t), ins[0].ptr, V, ins[1].ptr, T,
+                                float(smoothness), float(maxViewAngle), float(depthTol), int(padding), W,
+                                int(maxSweeps), atlas.ptr, rows, outs[0].ptr, outs[1].ptr, None, _ptr(charts),
+                                maxCharts, _ptr(info), _ptr(stats), ctypes.byref(ms)), name)
                 full = int(stats[8])
                 if full > rows:
                     rows = full

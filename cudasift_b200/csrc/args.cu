@@ -1108,6 +1108,16 @@ int texture_args(const char *fn, const cs_image *images, int numImages, const do
   return rs.check(fn);
 }
 
+int texture_photo_args(const char *fn, int dataTerm, double outlierK, double outlierMinSigma)
+{
+  if (dataTerm != 0 && dataTerm != 1) return arg_error(fn, "dataTerm must be 0 (area) or 1 (GMI)");
+  if (!(outlierK == 0.0 || (outlierK >= 1.0 && outlierK <= 100.0)))
+    return arg_error(fn, "outlierK must be 0 or in [1, 100]");
+  if (!(outlierMinSigma > 0.0 && outlierMinSigma <= 1000.0))
+    return arg_error(fn, "outlierMinSigma must be finite and in (0, 1000]");
+  return 0;
+}
+
 int seams_args(const char *fn, const float *vertices, int numVertices, const int *triangles, int numTriangles,
                const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
                int atlasRows, int atlasWidth, int padding, double smoothness, double regularization, bool local,

@@ -105,6 +105,8 @@ int texture_args(const char *fn, const cs_image *images, int numImages, const do
                  double lambda, double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
                  const float *atlas, int maxAtlasRows, const float *uv, const int *faceView, const int *faceChart,
                  const int *chartsOut, int maxCharts);
+// cs_texture_mesh_photo's three view-selection settings (after texture_args).
+int texture_photo_args(const char *fn, int dataTerm, double outlierK, double outlierMinSigma);
 // cs_level_texture_seams (local false: smoothness, regularization and d_cornerOffset checked) and
 // cs_level_texture_seams_local (local true: stripWidth checked, no corner offsets): the mesh, the chart table, the
 // parameters, the buffers and the range sweep.

@@ -789,14 +789,19 @@ size_t simplify_result_bytes();
 // ---- mesh texturing (texture.cu) -----------------------------------------------------------------------------------
 // The depth-buffer bytes of one image group (cs_set_tuning("texture_group_bytes"); 0 or less: 1 GiB).
 extern long long g_texture_group_bytes;
-// cs_texture_mesh after its argument checks (numTriangles > 0), on st with readbacks through h_result (pinned,
-// texture_result_bytes), the scratch allocated and freed on st; fills charts_out, info (may be NULL) and stats (may be
-// NULL) and returns the full chart count.
+// cs_texture_mesh_photo's view selection: the data term (0 area, 1 GMI) and the outlier test (outlierK 0: off).
+struct TexturePhoto {
+  int dataTerm;
+  double outlierK, outlierMinSigma;
+};
+// cs_texture_mesh (photo NULL) and cs_texture_mesh_photo after their argument checks (numTriangles > 0), on st with
+// readbacks through h_result (pinned, texture_result_bytes), the scratch allocated and freed on st; fills charts_out,
+// info (may be NULL) and stats (may be NULL; 11 entries, 16 with photo) and returns the full chart count.
 int texture_run(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
                 const float *vertices, int numVertices, const int *triangles, int numTriangles, double lambda,
                 double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps, float *atlas,
                 int maxAtlasRows, float *uv, int *faceView, int *faceChart, int *chartsOut, int maxCharts,
-                cudaStream_t st, void *h_result, double *info, long long *stats);
+                cudaStream_t st, void *h_result, double *info, long long *stats, const TexturePhoto *photo = nullptr);
 size_t texture_result_bytes();
 
 // ---- seam levelling (seams.cu) -------------------------------------------------------------------------------------

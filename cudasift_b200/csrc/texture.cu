@@ -4,7 +4,10 @@
 // graph, ICM sweeps over the colours, charts by union-find, the shelf packing on the host, and the texel copy.  Every
 // rule is stated in cudasift_b200.h at cs_texture_mesh; tests/texture_oracle.py restates them in float64.  The float64
 // vectors, the colouring priority s(f), the input check and the launch shape are shared with simplify.cu in
-// trimesh.cuh; the union-find is common.cuh's (uf_find, uf_link), shared with tracks.cu.
+// trimesh.cuh; the union-find is common.cuh's (uf_find, uf_link), shared with tracks.cu.  cs_texture_mesh_photo runs
+// the same body with a warp per face in place of the candidate thread (each passing view sampled over the face's
+// visible pixels for its Sobel magnitude and mean intensity) and one outlier kernel before the labelling; its rules
+// are stated at cs_texture_mesh_photo and restated in tests/texture_photo_oracle.py.
 //
 // Determinism: no floating-point atomics; integer atomics only where the result does not depend on their order (the
 // depth keys, counts, union-find links to the lower root, the chart rectangles).  The energy totals use coop.cuh's
@@ -204,6 +207,176 @@ __global__ void __launch_bounds__(MT) texture_candidate_kernel(TextureParams p)
     p.cn[f] = cnt;
   }
   if (found) atomicAdd(&p.res->cand, found);
+}
+
+// ---- candidates of cs_texture_mesh_photo (rules 3a to 3c) ---------------------------------------------------------
+// The photo call's device words and settings travel as a second kernel argument, so TextureParams and TextureResult
+// keep their layout and the kernels above their instructions.
+struct PhotoResult {
+  unsigned long long samples;                 // visible pixels summed over the passing pairs
+  unsigned long long fallbacks;               // passing pairs with no visible pixel centre
+  unsigned int tested, removed, bestRemoved;
+};
+
+struct PhotoParams {
+  PhotoResult *res;
+  double *mu;                                 // [T][MCAND] mean intensity of each kept candidate
+  int dataTerm;                               // 0 area, 1 GMI
+  double outlierK, minSigma;
+};
+
+// pixel (x, y) of c, indices clamped to the image
+__device__ __forceinline__ double pixel_at(const TexCam &c, int x, int y)
+{
+  x = min(max(x, 0), c.W - 1);
+  y = min(max(y, 0), c.H - 1);
+  return (double)c.img[(size_t)y * c.pitch + x];
+}
+
+// the Sobel magnitude at (x, y) over 8, so that a ramp of slope s gives s (rule 3a)
+__device__ __forceinline__ double sobel_at(const TexCam &c, int x, int y)
+{
+  const double gx = ((pixel_at(c, x + 1, y - 1) - pixel_at(c, x - 1, y - 1)) +
+                     2.0 * (pixel_at(c, x + 1, y) - pixel_at(c, x - 1, y))) +
+                    (pixel_at(c, x + 1, y + 1) - pixel_at(c, x - 1, y + 1));
+  const double gy = ((pixel_at(c, x - 1, y + 1) - pixel_at(c, x - 1, y - 1)) +
+                     2.0 * (pixel_at(c, x, y + 1) - pixel_at(c, x, y - 1))) +
+                    (pixel_at(c, x + 1, y + 1) - pixel_at(c, x + 1, y - 1));
+  return sqrt(gx * gx + gy * gy) / 8.0;
+}
+
+// A warp per face: lane l runs rule 3's tests for image b + l of the group, a ballot collects the images that pass,
+// then the warp samples each of them in ascending order (lane j the box indices j mod 32, the sums combined by the
+// xor butterfly) and lane 0 inserts it with its mean intensity, as texture_candidate_kernel does.
+__global__ void __launch_bounds__(MT) texture_photo_candidate_kernel(TextureParams p, PhotoParams h)
+{
+  const int lane = threadIdx.x & 31;
+  unsigned int found = 0;
+  unsigned long long samples = 0, fallbacks = 0;
+  for (int f = blockIdx.x * (MT / 32) + (threadIdx.x >> 5); f < p.T; f += gridDim.x * (MT / 32)) {
+    const D3 p0 = vertex_of(p.vin, p.tin[3 * (size_t)f]), p1 = vertex_of(p.vin, p.tin[3 * (size_t)f + 1]),
+             p2 = vertex_of(p.vin, p.tin[3 * (size_t)f + 2]);
+    const D3 n = normal3(p0, p1, p2);
+    const D3 cen = {((p0.x + p1.x) + p2.x) / 3.0, ((p0.y + p1.y) + p2.y) / 3.0, ((p0.z + p1.z) + p2.z) / 3.0};
+    const double ln = sqrt(dot3(n, n));
+    double *cq = p.cq + (size_t)f * MCAND, *mu = h.mu + (size_t)f * MCAND;
+    int *ca = p.ca + (size_t)f * MCAND;
+    int cnt = p.cn[f];
+    for (int b = p.g0; b < p.g0 + p.gn; b += 32) {
+      bool pass = false;
+      const int g = b + lane;
+      if (g < p.g0 + p.gn) {
+        const TexCam &c = p.cams[g];
+        const D3 d = sub3({c.C[0], c.C[1], c.C[2]}, cen);
+        const double dn = dot3(n, d);
+        double u[3], v[3], uc, vc;
+        pass = dn > 0.0 && dn >= p.cosLim * (ln * sqrt(dot3(d, d))) && sees(c, p0, f, p.depthTol, u[0], v[0]) &&
+               sees(c, p1, f, p.depthTol, u[1], v[1]) && sees(c, p2, f, p.depthTol, u[2], v[2]) &&
+               sees(c, cen, f, p.depthTol, uc, vc) && 0.5 * fabs(area2_of(u, v)) > 0.0;
+      }
+      for (unsigned int m = __ballot_sync(~0u, pass); m; m &= m - 1) {
+        const int a = b + __ffs(m) - 1;
+        const TexCam &c = p.cams[a];
+        double u[3], v[3], z, uc, vc;
+        project(c, p0, u[0], v[0], z);
+        project(c, p1, u[1], v[1], z);
+        project(c, p2, u[2], v[2], z);
+        project(c, cen, uc, vc, z);
+        const double area = 0.5 * fabs(area2_of(u, v));
+        // rule 2's clipped box of f in image a; its samples are the pixels whose key names f
+        const double xlo = fmax(0.0, ceil(fmin(fmin(u[0], u[1]), u[2]))), xhi = fmin(c.W - 1.0, floor(fmax(fmax(u[0], u[1]), u[2])));
+        const double ylo = fmax(0.0, ceil(fmin(fmin(v[0], v[1]), v[2]))), yhi = fmin(c.H - 1.0, floor(fmax(fmax(v[0], v[1]), v[2])));
+        int cntS = 0;
+        double sg = 0.0, si = 0.0;
+        if (xlo <= xhi && ylo <= yhi) {
+          const int x0 = (int)xlo, y0 = (int)ylo, bw = (int)xhi - x0 + 1, N = bw * ((int)yhi - y0 + 1);
+          for (int i = lane; i < N; i += 32) {
+            const int dy = i / bw, x = x0 + (i - dy * bw), y = y0 + dy;
+            if ((unsigned int)c.buf[(size_t)y * c.W + x] != (unsigned int)f) continue;
+            cntS++;
+            sg = sg + sobel_at(c, x, y);
+            si = si + pixel_at(c, x, y);
+          }
+        }
+        for (int o = 16; o > 0; o >>= 1) {
+          cntS += __shfl_xor_sync(~0u, cntS, o);
+          sg = sg + __shfl_xor_sync(~0u, sg, o);
+          si = si + __shfl_xor_sync(~0u, si, o);
+        }
+        double gm, mean;
+        if (cntS > 0) {
+          gm = sg / (double)cntS;
+          mean = si / (double)cntS;
+        } else {
+          const int px = (int)floor(uc + 0.5), py = (int)floor(vc + 0.5);
+          gm = sobel_at(c, px, py);
+          mean = pixel_at(c, px, py);
+        }
+        const double q = h.dataTerm ? area * (gm + 1.0) : area;
+        if (lane == 0) {
+          found++;
+          samples += (unsigned int)cntS;
+          fallbacks += cntS == 0;
+          int r = cnt < MCAND ? cnt : MCAND;
+          while (r > 0 && (q > cq[r - 1] || (q == cq[r - 1] && a < ca[r - 1]))) {
+            if (r < MCAND) { cq[r] = cq[r - 1]; ca[r] = ca[r - 1]; mu[r] = mu[r - 1]; }
+            r--;
+          }
+          if (r < MCAND) { cq[r] = q; ca[r] = a; mu[r] = mean; }
+        }
+        if (cnt < MCAND) cnt++;
+      }
+    }
+    if (lane == 0) p.cn[f] = cnt;
+  }
+  if (found) atomicAdd(&p.res->cand, found);
+  if (samples) atomicAdd(&h.res->samples, samples);
+  if (fallbacks) atomicAdd(&h.res->fallbacks, fallbacks);
+}
+
+// the median of s [m], sorted in place: the middle value, or (a + b) * 0.5 of the two middle values for even m
+__device__ __forceinline__ double median_of(double *s, int m)
+{
+  for (int i = 1; i < m; i++)
+    for (int j = i; j > 0 && s[j] < s[j - 1]; j--) {
+      const double t = s[j];
+      s[j] = s[j - 1];
+      s[j - 1] = t;
+    }
+  return m & 1 ? s[m / 2] : (s[m / 2 - 1] + s[m / 2]) * 0.5;
+}
+
+// One thread per face (rule 3c): with outlierK > 0 and m >= 3 kept candidates, every candidate whose mean is further
+// than outlierK max(1.4826 MAD, minSigma) from the median of the means leaves the list; the survivors keep their order.
+__global__ void __launch_bounds__(MT) texture_outlier_kernel(TextureParams p, PhotoParams h)
+{
+  unsigned int tested = 0, removed = 0, best = 0;
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
+    const int m = p.cn[f];
+    if (!(h.outlierK > 0.0) || m < 3) continue;
+    double *cq = p.cq + (size_t)f * MCAND, *mu = h.mu + (size_t)f * MCAND;
+    int *ca = p.ca + (size_t)f * MCAND;
+    double s[MCAND];
+    for (int i = 0; i < m; i++) s[i] = mu[i];
+    const double med = median_of(s, m);
+    for (int i = 0; i < m; i++) s[i] = fabs(mu[i] - med);
+    const double lim = h.outlierK * fmax(1.4826 * median_of(s, m), h.minSigma);
+    best += fabs(mu[0] - med) > lim;
+    int k = 0;
+    for (int i = 0; i < m; i++) {
+      if (fabs(mu[i] - med) > lim) continue;
+      cq[k] = cq[i];
+      ca[k] = ca[i];
+      mu[k] = mu[i];
+      k++;
+    }
+    tested++;
+    removed += m - k;
+    p.cn[f] = k;
+  }
+  if (tested) atomicAdd(&h.res->tested, tested);
+  if (removed) atomicAdd(&h.res->removed, removed);
+  if (best) atomicAdd(&h.res->bestRemoved, best);
 }
 
 // ---- labelling (rule 4) -------------------------------------------------------------------------------------------
@@ -421,13 +594,16 @@ __global__ void __launch_bounds__(MT) texture_atlas_kernel(TextureParams p)
   }
 }
 
+// where PhotoResult starts in the pinned readback buffer
+size_t photo_result_at() { return (sizeof(TextureResult) + 15) & ~(size_t)15; }
+
 }  // namespace
 
 int texture_run(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
                 const float *vin, int V, const int *tin, int T, double lambda, double maxViewAngleDeg,
                 double depthTol, int padding, int atlasWidth, int maxSweeps, float *atlas, int maxAtlasRows, float *uv,
                 int *faceView, int *faceChart, int *chartsOut, int maxCharts, cudaStream_t st, void *h_res,
-                double *info, long long *stats)
+                double *info, long long *stats, const TexturePhoto *photo)
 {
   const size_t C3 = 3 * (size_t)T;
   size_t tb[2] = {};
@@ -467,6 +643,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
                cstartAt = L.take(((size_t)T + 1) * 8);
   const size_t bufAt = L.take((size_t)bufMax);
   const size_t tempAt = L.take(tempBytes);
+  const size_t phResAt = photo ? L.take(sizeof(PhotoResult)) : 0, muAt = photo ? L.take((size_t)T * MCAND * 8) : 0;
   char *base = nullptr;
   CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
   auto at = [&](size_t off) { return base + off; };
@@ -524,6 +701,16 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
   unsigned long long *buf = reinterpret_cast<unsigned long long *>(at(bufAt));
   void *temp = at(tempAt);
   TextureResult &R = *static_cast<TextureResult *>(h_res);
+  PhotoParams ph{};
+  PhotoResult *hPhoto = reinterpret_cast<PhotoResult *>(static_cast<char *>(h_res) + photo_result_at());
+  if (photo) {
+    ph.res = reinterpret_cast<PhotoResult *>(at(phResAt));
+    ph.mu = reinterpret_cast<double *>(at(muAt));
+    ph.dataTerm = photo->dataTerm;
+    ph.outlierK = photo->outlierK;
+    ph.minSigma = photo->outlierMinSigma;
+    std::memset(hPhoto, 0, sizeof(PhotoResult));
+  }
   cudaEvent_t *tev = match_timing_events();
 
   int status = 0, rounds = 0, sweeps = 0, colours = 0;
@@ -563,6 +750,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     CS_CUDA(cudaMemsetAsync(p.cn, 0, (size_t)T * 4, st));
+    if (photo) CS_CUDA(cudaMemsetAsync(ph.res, 0, sizeof(PhotoResult), st));
     if (tev) CS_CUDA(cudaEventRecord(tev[1], st));
     for (size_t gi = 0; gi + 1 < groupStart.size(); gi++) {
       const int g0 = groupStart[gi], g1 = groupStart[gi + 1];
@@ -577,11 +765,17 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
       p.gn = g1 - g0;
       texture_raster_kernel<<<grid_of((long long)p.gn * T), MT, 0, st>>>(p);
       if (tev && gi == 0) CS_CUDA(cudaEventRecord(tev[2], st));
-      texture_candidate_kernel<<<grid_of(T), MT, 0, st>>>(p);
+      if (photo) texture_photo_candidate_kernel<<<grid_of(32ll * T), MT, 0, st>>>(p, ph);
+      else texture_candidate_kernel<<<grid_of(T), MT, 0, st>>>(p);
       count_launch(2);
       CS_CUDA(cudaGetLastError());
       // the host table is read by the copy above before the next group changes it
       CS_CUDA(cudaStreamSynchronize(st));
+    }
+    if (photo) {
+      texture_outlier_kernel<<<grid_of(T), MT, 0, st>>>(p, ph);
+      count_launch();
+      CS_CUDA(cudaGetLastError());
     }
     if (tev) CS_CUDA(cudaEventRecord(tev[3], st));
     texture_label_init_kernel<<<grid_of(T), MT, 0, st>>>(p);
@@ -682,6 +876,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     count_launch(2);
     CS_CUDA(cudaGetLastError());
     if (tev) CS_CUDA(cudaEventRecord(tev[6], st));
+    if (photo) CS_CUDA(cudaMemcpyAsync(hPhoto, ph.res, sizeof(PhotoResult), cudaMemcpyDeviceToHost, st));
     CS_CUDA(cudaStreamSynchronize(st));
     if (tev) {
       static const char *const names[6] = {"adjacency", "depth", "candidates", "labelling", "charts", "atlas"};
@@ -713,10 +908,18 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     stats[8] = fullRows;
     stats[9] = rowsWritten;
     stats[10] = status;
+    if (photo) {
+      stats[11] = out ? (long long)hPhoto->samples : 0;
+      stats[12] = out ? (long long)hPhoto->fallbacks : 0;
+      stats[13] = out ? hPhoto->tested : 0;
+      stats[14] = out ? hPhoto->removed : 0;
+      stats[15] = out ? hPhoto->bestRemoved : 0;
+    }
   }
   return C;
 }
 
-size_t texture_result_bytes() { return sizeof(TextureResult); }
+// the photo call's counters follow TextureResult in the pinned readback buffer
+size_t texture_result_bytes() { return photo_result_at() + sizeof(PhotoResult); }
 
 }  // namespace cs

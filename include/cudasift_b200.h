@@ -1398,6 +1398,51 @@ int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, con
                     float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
                     int *charts_out, int maxCharts, double info_out[2], long long stats_out[11], double *ms);
 
+/* Mesh texturing with Waechter, Moehrle & Goesele's view selection (ECCV 2014, section 4.1): cs_texture_mesh with a
+ * data term that prefers sharp views, the gradient magnitude integrated over the face's projection (GMI), and the
+ * rejection of views whose colour over the face disagrees with the others' (a pedestrian, a car, a reflection seen
+ * in one view only).  The arguments are cs_texture_mesh's, with dataTerm, outlierK and outlierMinSigma after
+ * numTriangles.  Rules 1, 2 and 4 to 6 are cs_texture_mesh's; rule 3 is replaced by 3a to 3c.  All arithmetic is
+ * float64, each operation rounded once in the order written (no contraction); the result depends on values alone,
+ * not on scheduling or on the image groups, so two calls give the same bytes.
+ * 3a. Samples: a pair (f, a) that passes every test of cs_texture_mesh's rule 3 is sampled over its box, rule 2's
+ *    clipped bounding box xlo..xhi, ylo..yhi of f's projection in image a.  Its samples are the box pixels whose
+ *    depth-buffer key names f, exactly the pixels where f is visible.  With the box index i = (y - ylo) boxWidth +
+ *    (x - xlo), lane j of a warp sums the samples with i = j mod 32 in ascending i (a count n, sum G and sum I), and the
+ *    three sums are combined by the xor butterfly 16, 8, 4, 2, 1 (lane 0's value is used).  I is the pixel value (pitch
+ *    respected); G is the Sobel magnitude with indices clamped to the image:
+ *    gx = ((I(x+1,y-1) - I(x-1,y-1)) + 2 (I(x+1,y) - I(x-1,y))) + (I(x+1,y+1) - I(x-1,y+1)),
+ *    gy = ((I(x-1,y+1) - I(x-1,y-1)) + 2 (I(x,y+1) - I(x,y-1))) + (I(x+1,y+1) - I(x+1,y-1)),
+ *    G = sqrt(gx gx + gy gy) / 8 (a ramp of slope s gives s).  The means are g = sum G / n and mu = sum I / n; with
+ *    n = 0 (a face smaller than a pixel, or hidden at every pixel centre) g and mu are read at the centroid pixel
+ *    (floor(uc + 0.5), floor(vc + 0.5)) that rule 3 tested.
+ * 3b. Data term: dataTerm 0 is the area, q = 0.5 |A| as in cs_texture_mesh; dataTerm 1 is GMI, q = (0.5 |A|) (g + 1).
+ *    The 1 is a floor in grey levels per pixel, so textureless faces still rank by area and never get q = 0; like the
+ *    stereo variance floor it assumes images on a 0..255 scale.  A face keeps its best 8 candidates by (q descending,
+ *    image ascending), and mu travels with each kept candidate.
+ * 3c. Outliers, after every image group and before the labelling: with outlierK > 0, a face with m >= 3 kept
+ *    candidates is tested.  med is the median of its m values of mu ((a + b) * 0.5 of the two middle values for even
+ *    m), MAD the median of |mu_i - med| likewise, and s = max(1.4826 MAD, outlierMinSigma).  A candidate leaves the
+ *    list when |mu_i - med| > outlierK s; the survivors keep their order.  With outlierK >= 1 at least ceil(m / 2)
+ *    candidates survive (half the values lie within MAD of med), so a tested face is never left unseen.  When the best
+ *    candidate leaves, the face starts at the new first candidate and D (rule 4) is normalised by its q.
+ * - Outputs: cs_texture_mesh's.  stats_out [16] (may be NULL): cs_texture_mesh's 11 entries in place (status at
+ *   [10]), then samples summed over every passing pair, pairs that fell back to the centroid pixel, faces tested,
+ *   candidates removed, and faces whose best candidate was removed.  numTriangles == 0 returns 0 (stats and info
+ *   zero) and makes no CUDA call.
+ * - Launches (cs_launch_count): 15 + 2 G + rounds + colours x sweeps (the candidate kernel replaced by the sampling
+ *   kernel, a warp per face, and one outlier kernel, a thread per face, that always runs), 1 when the input is
+ *   invalid.  With dataTerm 0 and outlierK 0 every output and stats_out [0..10] equal cs_texture_mesh's.
+ * - Scratch: cs_texture_mesh's plus 64 bytes per face (mu of the 8 candidates) and 32 bytes.
+ * - CS_E_ARG, before any CUDA call, naming the argument: cs_texture_mesh's checks; dataTerm not 0 or 1; outlierK not 0
+ *   and not in [1, 100] (NaN rejected); outlierMinSigma not finite or not in (0, 1000]. */
+int cs_texture_mesh_photo(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                          const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                          int dataTerm, double outlierK, double outlierMinSigma, double lambda,
+                          double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                          float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
+                          int *charts_out, int maxCharts, double info_out[2], long long stats_out[16], double *ms);
+
 /* Global seam levelling of a textured mesh (Lempitsky & Ivanov 2007 as Waechter, Moehrle & Goesele 2014 apply it,
  * section 4.2): one additive offset per (vertex, label) pair that evens out the colour steps where charts from
  * different images meet, added to the atlas texel by texel.  The inputs are cs_texture_mesh's outputs as it returns
