@@ -1853,6 +1853,40 @@ int cs_texture_mesh_photo(const cs_image *images, int numImages, const double *K
   });
 }
 
+int cs_texture_mesh_bp(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                       const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                       int dataTerm, double outlierK, double outlierMinSigma, int maxBpSweeps, double lambda,
+                       double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                       float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
+                       int *charts_out, int maxCharts, double info_out[3], long long stats_out[20], double *ms)
+{
+  const char *fn = "cs_texture_mesh_bp";
+  if (ms) *ms = 0.0;
+  int r = texture_args(fn, images, numImages, Ks, Rs, ts, d_vertices, numVertices, d_triangles, numTriangles, lambda,
+                       maxViewAngleDeg, depthTol, padding, atlasWidth, maxSweeps, d_atlas, maxAtlasRows, d_uv,
+                       d_faceView, d_faceChart, charts_out, maxCharts);
+  if (r < 0 || (r = texture_photo_args(fn, dataTerm, outlierK, outlierMinSigma)) < 0 ||
+      (r = texture_bp_args(fn, maxBpSweeps)) < 0)
+    return r;
+  if (numTriangles == 0) {
+    if (info_out) info_out[0] = info_out[1] = info_out[2] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 20; k++) stats_out[k] = 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(texture_result_bytes())) < 0) return r;
+  const TexturePhoto photo{dataTerm, outlierK, outlierMinSigma};
+  return timed_sync(fn, c, ms, [&] {
+    return texture_run(images, numImages, Ks, Rs, ts, d_vertices, numVertices, d_triangles, numTriangles, lambda,
+                       maxViewAngleDeg, depthTol, padding, atlasWidth, maxSweeps, d_atlas, maxAtlasRows, d_uv,
+                       d_faceView, d_faceChart, charts_out, maxCharts, c->stream, c->h_mesh.p, info_out, stats_out,
+                       &photo, maxBpSweeps);
+  });
+}
+
 int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
                            const int *d_faceView, const float *d_uv, const int *charts, int numCharts,
                            const float *d_atlas, int atlasRows, int atlasWidth, int padding, double smoothness,

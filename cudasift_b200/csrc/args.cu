@@ -1118,6 +1118,12 @@ int texture_photo_args(const char *fn, int dataTerm, double outlierK, double out
   return 0;
 }
 
+int texture_bp_args(const char *fn, int maxBpSweeps)
+{
+  if (maxBpSweeps < 0 || maxBpSweeps > 1000) return arg_error(fn, "maxBpSweeps must be in [0, 1000]");
+  return 0;
+}
+
 int seams_args(const char *fn, const float *vertices, int numVertices, const int *triangles, int numTriangles,
                const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
                int atlasRows, int atlasWidth, int padding, double smoothness, double regularization, bool local,

@@ -107,6 +107,8 @@ int texture_args(const char *fn, const cs_image *images, int numImages, const do
                  const int *chartsOut, int maxCharts);
 // cs_texture_mesh_photo's three view-selection settings (after texture_args).
 int texture_photo_args(const char *fn, int dataTerm, double outlierK, double outlierMinSigma);
+// cs_texture_mesh_bp's sweep cap (after texture_photo_args).
+int texture_bp_args(const char *fn, int maxBpSweeps);
 // cs_level_texture_seams (local false: smoothness, regularization and d_cornerOffset checked) and
 // cs_level_texture_seams_local (local true: stripWidth checked, no corner offsets): the mesh, the chart table, the
 // parameters, the buffers and the range sweep.

@@ -794,14 +794,16 @@ struct TexturePhoto {
   int dataTerm;
   double outlierK, outlierMinSigma;
 };
-// cs_texture_mesh (photo NULL) and cs_texture_mesh_photo after their argument checks (numTriangles > 0), on st with
-// readbacks through h_result (pinned, texture_result_bytes), the scratch allocated and freed on st; fills charts_out,
-// info (may be NULL) and stats (may be NULL; 11 entries, 16 with photo) and returns the full chart count.
+// cs_texture_mesh (photo NULL), cs_texture_mesh_photo and cs_texture_mesh_bp (maxBpSweeps >= 0, with photo) after
+// their argument checks (numTriangles > 0), on st with readbacks through h_result (pinned, texture_result_bytes), the
+// scratch allocated and freed on st; fills charts_out, info (may be NULL; 2 entries, 3 with BP) and stats (may be NULL;
+// 11 entries, 16 with photo, 20 with BP) and returns the full chart count.
 int texture_run(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
                 const float *vertices, int numVertices, const int *triangles, int numTriangles, double lambda,
                 double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps, float *atlas,
                 int maxAtlasRows, float *uv, int *faceView, int *faceChart, int *chartsOut, int maxCharts,
-                cudaStream_t st, void *h_result, double *info, long long *stats, const TexturePhoto *photo = nullptr);
+                cudaStream_t st, void *h_result, double *info, long long *stats, const TexturePhoto *photo = nullptr,
+                int maxBpSweeps = -1);
 size_t texture_result_bytes();
 
 // ---- seam levelling (seams.cu) -------------------------------------------------------------------------------------

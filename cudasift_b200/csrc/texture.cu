@@ -7,7 +7,9 @@
 // trimesh.cuh; the union-find is common.cuh's (uf_find, uf_link), shared with tracks.cu.  cs_texture_mesh_photo runs
 // the same body with a warp per face in place of the candidate thread (each passing view sampled over the face's
 // visible pixels for its Sobel magnitude and mean intensity) and one outlier kernel before the labelling; its rules
-// are stated at cs_texture_mesh_photo and restated in tests/texture_photo_oracle.py.
+// are stated at cs_texture_mesh_photo and restated in tests/texture_photo_oracle.py.  cs_texture_mesh_bp is the photo
+// call with min-sum belief propagation between the colouring and the ICM sweeps: a message step per colour, a decode
+// and the energy total per sweep, the labelling of lowest energy kept (rule 4b, tests/texture_bp_oracle.py).
 //
 // Determinism: no floating-point atomics; integer atomics only where the result does not depend on their order (the
 // depth keys, counts, union-find links to the lower root, the chart rectangles).  The energy totals use coop.cuh's
@@ -489,6 +491,93 @@ __global__ void __launch_bounds__(MT) texture_icm_kernel(TextureParams p, int co
   if (changed) atomicAdd(&p.res->changed, changed);
 }
 
+// ---- belief propagation of cs_texture_mesh_bp (rule 4b) -----------------------------------------------------------
+// Min-sum messages over the Potts factors of the seen faces, a colour per step, then a decode.  Like the photo call's,
+// the new words and fields travel as a second kernel argument.
+struct BpResult {
+  unsigned int changed;                       // messages with an entry that changed in a sweep
+  unsigned int moved;                         // decoded labels that differ from the start label
+};
+
+struct BpParams {
+  BpResult *res;
+  double *msg;                                // [T][3][MCAND]: the message into f across its edge k, over f's ranks
+};
+
+// A step of the faces of one colour: every message out of every seen face of the colour, into the slot of the seen
+// neighbour across the same edge.  It reads only the messages into faces of the colour, which no face of it writes.
+__global__ void __launch_bounds__(MT) texture_bp_kernel(TextureParams p, BpParams b, int colour)
+{
+  unsigned int changed = 0;
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
+    const int m = p.cn[f];
+    if (m <= 0 || p.colA[f] != colour) continue;
+    const double *cq = p.cq + (size_t)f * MCAND;
+    const int *ca = p.ca + (size_t)f * MCAND;
+    const double *in = b.msg + (size_t)f * 3 * MCAND;
+    for (int k = 0; k < 3; k++) {
+      const int g = p.nbr[3 * (size_t)f + k];
+      if (g < 0 || p.cn[g] <= 0) continue;
+      // g's slot with f's edge k: the two vertex ids compared (rule 1 makes it unique)
+      const int v0 = p.tin[3 * (size_t)f + k], v1 = p.tin[3 * (size_t)f + (k + 1) % 3];
+      const int *tg = p.tin + 3 * (size_t)g;
+      int kg = 0;
+      while (!((tg[kg] == v0 && tg[(kg + 1) % 3] == v1) || (tg[kg] == v1 && tg[(kg + 1) % 3] == v0))) kg++;
+      // h(r) = D(f, r) + the messages into f at the slots j != k, in ascending j
+      double h[MCAND], hmin = 0.0;
+      for (int r = 0; r < m; r++) {
+        double s = 1.0 - cq[r] / cq[0];
+        for (int j = 0; j < 3; j++)
+          if (j != k) s = s + in[j * MCAND + r];
+        h[r] = s;
+        if (r == 0 || s < hmin) hmin = s;
+      }
+      const double jump = hmin + p.lambda;
+      const int mg = p.cn[g];
+      const int *cag = p.ca + (size_t)g * MCAND;
+      double M[MCAND], Mmin = 0.0;
+      for (int q = 0; q < mg; q++) {
+        double x = jump;
+        for (int r = 0; r < m; r++)
+          if (ca[r] == cag[q] && h[r] < x) x = h[r];
+        M[q] = x;
+        if (q == 0 || x < Mmin) Mmin = x;
+      }
+      double *out = b.msg + ((size_t)g * 3 + kg) * MCAND;
+      bool diff = false;
+      for (int q = 0; q < mg; q++) {
+        const double x = M[q] - Mmin;
+        diff = diff || __double_as_longlong(out[q]) != __double_as_longlong(x);
+        out[q] = x;
+      }
+      changed += diff;
+    }
+  }
+  if (changed) atomicAdd(&b.res->changed, changed);
+}
+
+// The labels after a sweep: b_f(r) = D(f, r) + every message into f in ascending slot order, the lowest rank of
+// minimum b; counts the labels that differ from the start label (rank 0).
+__global__ void __launch_bounds__(MT) texture_bp_decode_kernel(TextureParams p, BpParams b)
+{
+  unsigned int moved = 0;
+  for (int f = blockIdx.x * MT + threadIdx.x; f < p.T; f += gridDim.x * MT) {
+    const int m = p.cn[f];
+    if (m <= 0) continue;
+    const double *cq = p.cq + (size_t)f * MCAND;
+    const double *in = b.msg + (size_t)f * 3 * MCAND;
+    int best = 0;
+    double bestB = 0.0;
+    for (int r = 0; r < m; r++) {
+      const double s = (((1.0 - cq[r] / cq[0]) + in[r]) + in[MCAND + r]) + in[2 * MCAND + r];
+      if (r == 0 || s < bestB) { bestB = s; best = r; }
+    }
+    p.label[f] = p.ca[(size_t)f * MCAND + best];
+    moved += best != 0;
+  }
+  if (moved) atomicAdd(&b.res->moved, moved);
+}
+
 // ---- charts (rule 5) ----------------------------------------------------------------------------------------------
 // union of every adjacent pair with equal labels (uf_link: every root is the lowest face of its component)
 __global__ void __launch_bounds__(MT) texture_hook_kernel(TextureParams p)
@@ -594,8 +683,9 @@ __global__ void __launch_bounds__(MT) texture_atlas_kernel(TextureParams p)
   }
 }
 
-// where PhotoResult starts in the pinned readback buffer
+// where PhotoResult and BpResult start in the pinned readback buffer
 size_t photo_result_at() { return (sizeof(TextureResult) + 15) & ~(size_t)15; }
+size_t bp_result_at() { return (photo_result_at() + sizeof(PhotoResult) + 15) & ~(size_t)15; }
 
 }  // namespace
 
@@ -603,7 +693,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
                 const float *vin, int V, const int *tin, int T, double lambda, double maxViewAngleDeg,
                 double depthTol, int padding, int atlasWidth, int maxSweeps, float *atlas, int maxAtlasRows, float *uv,
                 int *faceView, int *faceChart, int *chartsOut, int maxCharts, cudaStream_t st, void *h_res,
-                double *info, long long *stats, const TexturePhoto *photo)
+                double *info, long long *stats, const TexturePhoto *photo, int maxBpSweeps)
 {
   const size_t C3 = 3 * (size_t)T;
   size_t tb[2] = {};
@@ -644,6 +734,9 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
   const size_t bufAt = L.take((size_t)bufMax);
   const size_t tempAt = L.take(tempBytes);
   const size_t phResAt = photo ? L.take(sizeof(PhotoResult)) : 0, muAt = photo ? L.take((size_t)T * MCAND * 8) : 0;
+  const bool withBp = maxBpSweeps >= 0;
+  const size_t bpResAt = withBp ? L.take(sizeof(BpResult)) : 0, msgAt = withBp ? L.take((size_t)T * 3 * MCAND * 8) : 0,
+               keptAt = withBp ? L.take((size_t)T * 4) : 0;
   char *base = nullptr;
   CS_CUDA(cudaMallocAsync((void **)&base, L.bytes, st));
   auto at = [&](size_t off) { return base + off; };
@@ -711,14 +804,23 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     ph.minSigma = photo->outlierMinSigma;
     std::memset(hPhoto, 0, sizeof(PhotoResult));
   }
+  BpParams bp{};
+  BpResult *hBp = reinterpret_cast<BpResult *>(static_cast<char *>(h_res) + bp_result_at());
+  int *kept = nullptr;
+  if (withBp) {
+    bp.res = reinterpret_cast<BpResult *>(at(bpResAt));
+    bp.msg = reinterpret_cast<double *>(at(msgAt));
+    kept = reinterpret_cast<int *>(at(keptAt));
+  }
   cudaEvent_t *tev = match_timing_events();
 
-  int status = 0, rounds = 0, sweeps = 0, colours = 0;
-  long long changed = 0, fullRows = 0, rowsWritten = 0;
-  double energy[2] = {0.0, 0.0};
+  int status = 0, rounds = 0, sweeps = 0, colours = 0, bpSweeps = 0, bpKept = 0;
+  long long changed = 0, fullRows = 0, rowsWritten = 0, bpChanged = 0, bpMoved = 0;
+  double energy[3] = {0.0, 0.0, 0.0};
   std::vector<int> table;
   auto readback = [&]() -> int {
     CS_CUDA(cudaMemcpyAsync(h_res, p.res, sizeof(TextureResult), cudaMemcpyDeviceToHost, st));
+    if (withBp) CS_CUDA(cudaMemcpyAsync(hBp, bp.res, sizeof(BpResult), cudaMemcpyDeviceToHost, st));
     CS_CUDA(cudaStreamSynchronize(st));
     return 0;
   };
@@ -736,6 +838,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     int r;
     if (tev) CS_CUDA(cudaEventRecord(tev[0], st));
     CS_CUDA(cudaMemsetAsync(p.res, 0, sizeof(TextureResult), st));
+    if (withBp) CS_CUDA(cudaMemsetAsync(bp.res, 0, sizeof(BpResult), st));
     mesh_validate_kernel<<<grid_of(T), MT, 0, st>>>(vin, V, tin, T, &p.res->bad);
     count_launch();
     CS_CUDA(cudaGetLastError());
@@ -793,6 +896,31 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
     }
     colours = R.maxColour + 1;
     if ((r = total(energy[0])) < 0) return r;
+    // rule 4b: BP sweeps from zero messages, the labelling of lowest E kept (the start labelling first)
+    energy[2] = energy[0];
+    if (maxBpSweeps > 0) {
+      CS_CUDA(cudaMemsetAsync(bp.msg, 0, (size_t)T * 3 * MCAND * 8, st));
+      CS_CUDA(cudaMemcpyAsync(kept, p.label, (size_t)T * 4, cudaMemcpyDeviceToDevice, st));
+      while (bpSweeps < maxBpSweeps) {
+        CS_CUDA(cudaMemsetAsync(bp.res, 0, sizeof(BpResult), st));
+        for (int c = 0; c < colours; c++) texture_bp_kernel<<<grid_of(T), MT, 0, st>>>(p, bp, c);
+        texture_bp_decode_kernel<<<grid_of(T), MT, 0, st>>>(p, bp);
+        count_launch(colours + 1);
+        CS_CUDA(cudaGetLastError());
+        double e;
+        if ((r = total(e)) < 0) return r;
+        bpSweeps++;
+        bpChanged = hBp->changed;
+        if (e < energy[2]) {
+          energy[2] = e;
+          bpKept = bpSweeps;
+          bpMoved = hBp->moved;
+          CS_CUDA(cudaMemcpyAsync(kept, p.label, (size_t)T * 4, cudaMemcpyDeviceToDevice, st));
+        }
+        if (bpChanged == 0) break;
+      }
+      if (bpKept != bpSweeps) CS_CUDA(cudaMemcpyAsync(p.label, kept, (size_t)T * 4, cudaMemcpyDeviceToDevice, st));
+    }
     for (;;) {
       if (sweeps == maxSweeps) { status = 3; break; }
       CS_CUDA(cudaMemsetAsync(&p.res->changed, 0, sizeof(unsigned int), st));
@@ -895,6 +1023,7 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
   if (info) {
     info[0] = out ? energy[0] : 0.0;
     info[1] = out ? energy[1] : 0.0;
+    if (withBp) info[2] = out ? energy[2] : 0.0;
   }
   if (stats) {
     stats[0] = T;
@@ -915,11 +1044,17 @@ int texture_run(const cs_image *images, int numImages, const double *Ks, const d
       stats[14] = out ? hPhoto->removed : 0;
       stats[15] = out ? hPhoto->bestRemoved : 0;
     }
+    if (withBp) {
+      stats[16] = bpSweeps;
+      stats[17] = bpKept;
+      stats[18] = bpChanged;
+      stats[19] = bpMoved;
+    }
   }
   return C;
 }
 
-// the photo call's counters follow TextureResult in the pinned readback buffer
-size_t texture_result_bytes() { return photo_result_at() + sizeof(PhotoResult); }
+// the photo call's counters follow TextureResult in the pinned readback buffer, and the BP call's follow those
+size_t texture_result_bytes() { return bp_result_at() + sizeof(BpResult); }
 
 }  // namespace cs

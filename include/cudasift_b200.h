@@ -1443,6 +1443,52 @@ int cs_texture_mesh_photo(const cs_image *images, int numImages, const double *K
                           float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
                           int *charts_out, int maxCharts, double info_out[2], long long stats_out[16], double *ms);
 
+/* Mesh texturing with Waechter, Moehrle & Goesele's view selection and their MRF solved by loopy belief propagation
+ * (min-sum) before the ICM sweeps: cs_texture_mesh_photo with rule 4 split into 4a and 4b.  ICM alone stops at the
+ * first labelling no single face can improve, so it keeps islands of faces that all prefer another view by a small
+ * margin (m faces with D = delta inside a region of another label cost m delta to flip and save 2 lambda); BP passes
+ * evidence along the mesh and removes them, which means fewer seams and fewer charts.  The arguments are
+ * cs_texture_mesh_photo's, with maxBpSweeps after outlierMinSigma.  Rules 1 to 3c, 5 and 6 are the photo call's.
+ * D(f, r) = 1 - q(f, r) / q(f, 0) over f's candidates a_f[0..m_f - 1] (rank r), lambda and E are rule 4's; all arithmetic
+ * is float64, each operation rounded once in the order written, and every minimum is exact, so the result depends on
+ * values alone, not on scheduling or on the image groups.
+ * 4a. Start and colouring: as rule 4; E_0 is E of the start labelling.
+ * 4b. Factors: each edge shared by two seen faces is a Potts factor lambda [l_f != l_g] (rule 1's adjacency slots; a
+ *    pair that shares two edges has two factors).  Messages: for seen f and slot k (f's edge from corner k to k + 1)
+ *    with seen g across it, the message is a vector over g's ranks r', stored at g's slot k', the slot of g whose two
+ *    vertex ids are those of f's slot k.  Every message starts at 0.  h(r) = D(f, r) + the messages into f at the slots
+ *    j != k, added in ascending j (a fresh sum, never a subtraction from the full sum); M(r') = min(h(r_a) if a_g[r']
+ *    is f's candidate at rank r_a else +inf, min_r h(r) + lambda); the message is M(r') - min_r' M(r') (its smallest
+ *    entry exactly 0, every entry at most lambda).  Schedule: a sweep takes colours 0, 1, ... in order; a step writes
+ *    every message out of every seen face of its colour and reads only messages into faces of that colour, which no
+ *    face of the colour writes, so a step is race-free and equals a sequential pass.  Decode, after every sweep:
+ *    b_f(r) = D(f, r) + every message into f, added in ascending slot order; the label is a_f[r*], r* the lowest rank of
+ *    minimum b.  Keep: E of the decoded labels (rule 4's total) is compared with the kept labelling's; a labelling is
+ *    kept when its E is strictly lower.  The start labelling (E_0, sweep 0) is kept first; it is the decode with every
+ *    message 0.  Stop: after a sweep in which no message entry changed a bit, or after maxBpSweeps sweeps.  The labels
+ *    then become the kept labelling, and rule 4's ICM sweeps run from it unchanged (maxSweeps, status 0 or 3), so
+ *    E_final <= E_kept <= E_0.  On a face graph without cycles (a strip) the messages are exact min-marginals after
+ *    enough sweeps, and the kept labelling is a minimum of E.
+ * - Outputs: cs_texture_mesh_photo's.  info_out [3] (may be NULL): E_0, E after the ICM sweeps (the final E), E of the
+ *   labelling BP kept.  stats_out [20] (may be NULL): the photo call's 16 in place (status at [10]), then BP sweeps
+ *   run, the sweep whose labelling was kept (0: the start labelling), messages changed in the last BP sweep (0:
+ *   converged), faces whose kept label differs from the start label.  With maxBpSweeps 0 every output and
+ *   stats_out [0..15] equal cs_texture_mesh_photo's, info_out [2] = info_out [0] and stats_out [16..19] are 0.
+ *   numTriangles == 0 returns 0 (stats and info zero) and makes no CUDA call.
+ * - Launches (cs_launch_count): 15 + 2 G + rounds + colours x sweeps + (colours + 3) x BP sweeps (per BP sweep one
+ *   message step per colour, one decode and two for the energy total), 1 when the input is invalid.  The host reads a
+ *   few words after each BP sweep (one synchronise each); the kept labels are a device-to-device copy.
+ * - Scratch: cs_texture_mesh_photo's plus 196 bytes per face (the messages [T][3][8] float64, 192, and the kept labels,
+ *   4) and 8 bytes.
+ * - CS_E_ARG, before any CUDA call, naming the argument: cs_texture_mesh_photo's checks; maxBpSweeps outside
+ *   [0, 1000]. */
+int cs_texture_mesh_bp(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                       const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                       int dataTerm, double outlierK, double outlierMinSigma, int maxBpSweeps, double lambda,
+                       double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,
+                       float *d_atlas, int maxAtlasRows, float *d_uv, int *d_faceView, int *d_faceChart,
+                       int *charts_out, int maxCharts, double info_out[3], long long stats_out[20], double *ms);
+
 /* Global seam levelling of a textured mesh (Lempitsky & Ivanov 2007 as Waechter, Moehrle & Goesele 2014 apply it,
  * section 4.2): one additive offset per (vertex, label) pair that evens out the colour steps where charts from
  * different images meet, added to the atlas texel by texel.  The inputs are cs_texture_mesh's outputs as it returns
