@@ -24,7 +24,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
            "RetrievePairs", "RotationAveraging", "GlobalPositioning", "UndistortImages", "PatchMatchStereo",
            "PatchMatchStereoGeometric", "FuseDepthMaps", "SelectStereoViews", "PoissonMesh",
-           "PoissonMeshScreened", "SimplifyMesh"]
+           "PoissonMeshScreened", "SimplifyMesh", "RefineMesh"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -132,6 +132,8 @@ def lib():
         "cs_texture_mesh_bp": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, ip, c.c_double,
                                     c.c_double, c.c_double, ip, ip, ip, vp, ip, vp, vp, vp, vp, ip, vp, vp,
                                     c.POINTER(c.c_double)]),
+        "cs_mesh_refine": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, vp, ip, ip, c.c_double, c.c_double, ip,
+                                c.c_double, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_level_texture_seams": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, c.c_double, c.c_double, ip,
                                         c.c_double, vp, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_level_texture_seams_local": (ip, [vp, ip, vp, ip, vp, vp, vp, ip, vp, ip, ip, ip, ip, ip, c.c_double, vp,
@@ -1521,6 +1523,44 @@ def TextureMeshBP(images, Ks, Rs, ts, vertices, triangles, dataTerm="gmi", outli
     return _texture_mesh("TextureMeshBP", lambda *a: lib().cs_texture_mesh_bp(*a[:9], *extra, *a[9:]), 20,
                          images, Ks, Rs, ts, vertices, triangles, smoothness, maxViewAngle, depthTol, padding,
                          atlasWidth, maxSweeps, ninfo=3)
+
+
+def RefineMesh(images, Ks, Rs, ts, vertices, triangles, pairs, windowRadius=4, smoothness=0.2, step=0.1,
+               maxIterations=100, depthTol=0.01):
+    """Photometric refinement of a triangle mesh (cs_mesh_refine, after Vu et al. and OpenMVS's RefineMesh): every
+    free vertex moves by gradient descent on the windowed NCC (window 2 windowRadius + 1) between each ordered image
+    pair, reprojected through the mesh, plus smoothness times a thin-plate term; each step moves a vertex by at most
+    2 step mean edge lengths, and a halving line search accepts only steps that lower the energy, at most maxIterations
+    of them.  Vertices on a boundary or non-manifold edge, and unused ones, stay put; the topology does not change.
+    images, Ks, Rs, ts as for TextureMesh (pinhole, 0..255), vertices float32 [V, 3] and triangles int32 [T, 3];
+    pairs an int [n, 2] array of (ref, src) or SelectStereoViews' jobs (each source of each job paired with its ref).
+    Returns (vertices float32 [V, 3], info float64 [4] {E_photo, E_s at the start, at the end}, stats int64 [8]
+    {pairs, free vertices, fixed vertices, P0, evaluations, accepted steps, halvings of the final step, status}, ms)."""
+    if len(pairs) and not np.isscalar(pairs[0]) and len(pairs[0]) == 4:
+        pairs = [(int(ref), int(s)) for ref, srcs, _, _ in pairs for s in np.asarray(srcs).reshape(-1)]
+    P = np.ascontiguousarray(np.asarray(pairs, np.int64).reshape(-1, 2).astype(np.int32))
+    S = len(images)
+    K, R, t = _per_image(Ks, (3, 3), S, "Ks"), _per_image(Rs, (3, 3), S, "Rs"), _per_image(ts, (3,), S, "ts")
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    V, T = len(X), len(F)
+    arrs, bufs, table = _upload_images(images)
+    try:
+        ins = [DeviceBuffer(max(X.nbytes, 4)), DeviceBuffer(max(F.nbytes, 4)), DeviceBuffer(max(X.nbytes, 4))]
+        bufs += ins
+        for b, a in zip(ins, (X, F)):
+            if a.size:
+                b.upload(a)
+        info, stats, ms = np.zeros(4), np.zeros(8, np.int64), ctypes.c_double(0.0)
+        _check(lib().cs_mesh_refine(table if S else None, S, _ptr(K), _ptr(R), _ptr(t), ins[0].ptr, V, ins[1].ptr, T,
+                                    _ptr(P) if len(P) else None, len(P), int(windowRadius), float(smoothness),
+                                    float(step), int(maxIterations), float(depthTol), ins[2].ptr, _ptr(info),
+                                    _ptr(stats), ctypes.byref(ms)), "RefineMesh")
+        out = ins[2].download(np.float32, 3 * V).reshape(V, 3) if V and stats[7] != 2 else X.copy()
+        return out, info, stats, ms.value
+    finally:
+        for b in bufs:
+            b.free()
 
 
 def _texture_mesh(name, call, nstats, images, Ks, Rs, ts, vertices, triangles, smoothness, maxViewAngle,

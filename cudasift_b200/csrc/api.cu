@@ -1887,6 +1887,43 @@ int cs_texture_mesh_bp(const cs_image *images, int numImages, const double *Ks, 
   });
 }
 
+int cs_mesh_refine(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                   const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                   const int *pairs, int numPairs, int windowRadius, double smoothness, double step,
+                   int maxIterations, double depthTol, float *d_outVertices, double info_out[4],
+                   long long stats_out[8], double *ms)
+{
+  const char *fn = "cs_mesh_refine";
+  if (ms) *ms = 0.0;
+  int r = refine_args(fn, images, numImages, Ks, Rs, ts, d_vertices, numVertices, d_triangles, numTriangles, pairs,
+                      numPairs, windowRadius, smoothness, step, maxIterations, depthTol, d_outVertices);
+  if (r < 0) return r;
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if (numTriangles == 0) {
+    // no face: every vertex is fixed and copied, status 1
+    if (info_out)
+      for (int k = 0; k < 4; k++) info_out[k] = 0.0;
+    if (stats_out) {
+      const long long s[8] = {numPairs, 0, numVertices, 0, 0, 0, 0, 1};
+      for (int k = 0; k < 8; k++) stats_out[k] = s[k];
+    }
+    return timed_sync(fn, c, ms, [&]() -> int {
+      if (numVertices)
+        CS_CUDA(cudaMemcpyAsync(d_outVertices, d_vertices, (size_t)numVertices * 12, cudaMemcpyDeviceToDevice,
+                                c->stream));
+      return 1;
+    });
+  }
+  if ((r = c->h_mesh.grow(refine_result_bytes())) < 0) return r;
+  return timed_sync(fn, c, ms, [&] {
+    return refine_run(images, numImages, Ks, Rs, ts, d_vertices, numVertices, d_triangles, numTriangles, pairs,
+                      numPairs, windowRadius, smoothness, step, maxIterations, depthTol, d_outVertices, c->stream,
+                      c->h_mesh.p, info_out, stats_out);
+  });
+}
+
 int cs_level_texture_seams(const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
                            const int *d_faceView, const float *d_uv, const int *charts, int numCharts,
                            const float *d_atlas, int atlasRows, int atlasWidth, int padding, double smoothness,

@@ -1124,6 +1124,44 @@ int texture_bp_args(const char *fn, int maxBpSweeps)
   return 0;
 }
 
+int refine_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                const double *ts, const float *vertices, int numVertices, const int *triangles, int numTriangles,
+                const int *pairs, int numPairs, int windowRadius, double smoothness, double step, int maxIterations,
+                double depthTol, const float *outVertices)
+{
+  int r;
+  if ((r = stereo_images(fn, images, numImages, 1, Ks, Rs, ts, true)) < 0) return r;
+  if (numVertices < 0 || numVertices > (1 << 30)) return arg_error(fn, "numVertices must be in [0, 2^30]");
+  if (numTriangles < 0 || numTriangles > (1 << 28)) return arg_error(fn, "numTriangles must be in [0, 2^28]");
+  if (numPairs < 0) return arg_error(fn, "numPairs must be >= 0");
+  if (numPairs > 0 && !pairs) return arg_error(fn, "numPairs > 0 needs pairs");
+  for (int q = 0; q < numPairs; q++) {
+    const int a = pairs[2 * q], b = pairs[2 * q + 1];
+    if (a < 0 || a >= numImages || b < 0 || b >= numImages)
+      return arg_error(fn, "pairs[%d] = {%d, %d} names an image outside [0, %d)", q, a, b, numImages);
+    if (a == b) return arg_error(fn, "pairs[%d] has ref == src (%d)", q, a);
+  }
+  if (windowRadius < 1 || windowRadius > 5) return arg_error(fn, "windowRadius must be in [1, 5]");
+  if (!std::isfinite(smoothness) || smoothness < 0.0) return arg_error(fn, "smoothness must be finite and >= 0");
+  if (!(step > 0.0 && step <= 1.0)) return arg_error(fn, "step must be in (0, 1]");
+  if (maxIterations < 0 || maxIterations > 1000) return arg_error(fn, "maxIterations must be in [0, 1000]");
+  if (!(depthTol >= 0.0 && depthTol <= 1.0)) return arg_error(fn, "depthTol must be finite and in [0, 1]");
+  if (numVertices > 0 && (!vertices || misaligned(vertices, 4)))
+    return arg_error(fn, "numVertices > 0 needs d_vertices (4-byte aligned)");
+  if (numVertices > 0 && (!outVertices || misaligned(outVertices, 4)))
+    return arg_error(fn, "numVertices > 0 needs d_outVertices (4-byte aligned)");
+  if (numTriangles > 0 && (!triangles || misaligned(triangles, 4)))
+    return arg_error(fn, "numTriangles > 0 needs d_triangles (4-byte aligned)");
+  // the output (written), the mesh and the images (read)
+  static const char *const names[4] = {"d_outVertices", "d_vertices", "d_triangles", "images[%d].d_img"};
+  ArgRanges rs(names, 3 + (size_t)numImages);
+  rs.add(outVertices, 12 * (size_t)numVertices, 0, 0, true);
+  rs.add(vertices, 12 * (size_t)numVertices, 1, 0, false);
+  rs.add(triangles, 12 * (size_t)numTriangles, 2, 0, false);
+  for (int a = 0; a < numImages; a++) rs.add(images[a].d_img, image_bytes(images[a]), 3, a, false);
+  return rs.check(fn);
+}
+
 int seams_args(const char *fn, const float *vertices, int numVertices, const int *triangles, int numTriangles,
                const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
                int atlasRows, int atlasWidth, int padding, double smoothness, double regularization, bool local,

@@ -116,6 +116,11 @@ int seams_args(const char *fn, const float *vertices, int numVertices, const int
                const int *faceView, const float *uv, const int *charts, int numCharts, const float *atlas,
                int atlasRows, int atlasWidth, int padding, double smoothness, double regularization, bool local,
                int stripWidth, int maxIterations, double tol, const float *outAtlas, const float *cornerOffset);
+// cs_mesh_refine: the images and cameras, the mesh, the pairs, the parameters, the buffers and the range sweep.
+int refine_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
+                const double *ts, const float *vertices, int numVertices, const int *triangles, int numTriangles,
+                const int *pairs, int numPairs, int windowRadius, double smoothness, double step, int maxIterations,
+                double depthTol, const float *outVertices);
 int pose_args(const char *fn, const double *points, int numPoints, const cs_pose_job *jobs, int numJobs,
               const double *Ks, int numLoops, double maxError);
 // cs_vocab_assign, cs_vocab_train and cs_retrieve_pairs; *M and *N receive the feature totals.

@@ -823,6 +823,16 @@ int seams_local_run(const float *vertices, int numVertices, const int *triangles
                     float *outAtlas, cudaStream_t st, void *h_result, double *info, long long *stats);
 size_t seams_local_result_bytes();
 
+// ---- photometric mesh refinement (refine.cu) -----------------------------------------------------------------------
+// cs_mesh_refine after its argument checks (numTriangles > 0), on st with readbacks through h_result (pinned,
+// refine_result_bytes), the scratch allocated and freed on st; writes outVertices, fills info (may be NULL; 4 entries)
+// and stats (may be NULL; 8 entries) and returns the status.
+int refine_run(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+               const float *vertices, int numVertices, const int *triangles, int numTriangles, const int *pairs,
+               int numPairs, int windowRadius, double smoothness, double step, int maxIterations, double depthTol,
+               float *outVertices, cudaStream_t st, void *h_result, double *info, long long *stats);
+size_t refine_result_bytes();
+
 // ---- geometric verification (verify.cu) -------------------------------------------------------------------------
 // The model id verify_enqueue uses for cs_verify_essential (not a model value of the public cs_verify_pairs).
 #define VERIFY_ESSENTIAL 3

@@ -1615,6 +1615,89 @@ int cs_level_texture_seams_local(const float *d_vertices, int numVertices, const
                                  int maxIterations, double tol, float *d_outAtlas, double info_out[3],
                                  long long stats_out[8], double *ms);
 
+/* Photometric mesh refinement (Vu, Labatut, Pons & Keriven, PAMI 2012, as OpenMVS's RefineMesh): every free vertex
+ * moves so that each ordered image pair (ref, src), reprojected through the mesh, agrees photometrically (windowed
+ * NCC), with a thin-plate term that keeps the surface regular.  It recovers the corners, thin parts and fine relief
+ * that the Poisson grid and simplification round away.  Images and cameras are the dense calls' (pinhole, images on a
+ * 0..255 scale); the mesh is cs_texture_mesh's, d_vertices [numVertices][3] float and d_triangles [numTriangles][3]
+ * int32, and the refined vertices go to the separate d_outVertices [numVertices][3]; the topology does not change.
+ * pairs [numPairs][2] (host int32) {ref, src}.  All arithmetic is float64, each operation rounded once in the order
+ * written (no contraction); no floating-point atomics, so two calls give the same bytes.
+ * 1. Input: status 2, with only stats_out and a zero info_out written, when cs_texture_mesh's rule 1 fails.  Every
+ *    corner emits the directed edge keys (a << 32) | b and (b << 32) | a of its edge a -> b, sorted; a run of equal
+ *    keys is a distinct directed edge and its length is the number of faces holding the edge.  A vertex is fixed when
+ *    it starts a run of length != 2 (a boundary or non-manifold edge) or starts no run (no face uses it); every other
+ *    vertex is free (F of them) and has its distinct neighbours N(v) in ascending id.  l0 is the mean length of the
+ *    distinct undirected edges (the runs with a < b, lengths summed over the sorted positions in coop.cuh's
+ *    three-level order).  Fixed vertices never move.
+ * 2. Depth buffers: cs_texture_mesh's rule 2, restated in this unit, for every image a pair names, rebuilt at every
+ *    evaluation from the vertices being evaluated.
+ * 3. Mapping, for pair p = (i, j): pixel x of image i is mapped when its key names a face f and: with rule 2's edge
+ *    values w at x, S = (w_0 + w_1) + w_2, screen weights (b_0, b_1, b_2) = (w_1 / S, w_2 / S, w_0 / S), t_k = b_k / z_k
+ *    and phi_k = t_k / ((t_0 + t_1) + t_2), the point X = (phi_0 P_0 + phi_1 P_1) + phi_2 P_2 (per component) projects
+ *    into j with Y_z > 0 inside [0, W_j - 1] x [0, H_j - 1]; it passes cs_texture_mesh's visibility test in j's buffer
+ *    (pixel (floor(u + 0.5), floor(v + 0.5)) empty, naming f, or Y_z <= depth (1 + depthTol)); and n_f . r != 0, with
+ *    n_f = (P_1 - P_0) x (P_2 - P_0) and r = X - C_i.  Then J(x) is the bilinear read of j at (u, v): x0 = min(floor(u),
+ *    W_j - 2), fx = u - x0 (likewise y0, fy), a = I00 + fx (I10 - I00), b = I01 + fx (I11 - I01), J = a + fy (b - a).
+ *    The chain factor is c(x) = (g_u a_u + g_v a_v) / (n_f . r) with the derivatives of that read, g_u = (I10 - I00) +
+ *    fy ((I11 - I01) - (I10 - I00)) and g_v = b - a (a change of the proposed design, which read central differences:
+ *    this way the gradient is the exact derivative of E inside a cell), and the derivative of j's projection along r,
+ *    dY = R_j r (rule 2's row order), a_u = (((K_0 dY_0 + K_1 dY_1) + K_2 dY_2) - u dY_2) / Y_z, a_v likewise with K_3..5
+ *    and v.  The scales of n_f and r cancel.
+ * 4. Score: x is scored when every pixel of its (2 windowRadius + 1)^2 window lies in image i and is mapped.  Over the
+ *    window in row-major order, from 0: sums of I, J, I I, J J and I J; n the window size, mu = sum / n, the raw
+ *    variance s = sum sq / n - mu mu, floored as max(s, 1) (the stereo call's floor of 1 grey level^2; J floored when
+ *    s < 1); q = sqrt(var_I var_J), NCC = (sum IJ / n - mu_I mu_J) / q, e(x) = 1 - NCC.
+ * 5. Image gradient: per scored x, A = 1 / q, B = mu_I A, Cc = NCC / var_J (0 when J is floored), D = Cc mu_J.  For
+ *    mapped y, the sums SA, SB, SC, SD over the scored x whose window holds y (x in row-major order, from 0);
+ *    dE/dJ(y) = -((((I(y) SA - SB) - J(y) SC) + SD)) / n and s(y) = dE/dJ(y) c(y).
+ * 6. Face and vertex gradient: per pair, a warp per face f takes rule 2's clipped box of f in image i and the mapped
+ *    box pixels whose key names f; lane l sums s(y) phi_k(y) over the box indices i = l mod 32 in ascending i, the xor
+ *    butterfly 16, 8, 4, 2, 1 combines the lanes, and acc_{f,k} = acc_{f,k} + S_{f,k} for every face, pairs in input
+ *    order, acc starting at 0 in every evaluation.  The photometric gradient of free v is the sum over its corners
+ *    (ascending corner 3f + k) of acc_{f,k} n_f, from 0, each component divided by P0.  P0 is the number of scored
+ *    pixels over all pairs at the input mesh: a fixed normaliser, so E does not change scale as coverage changes.
+ * 7. Thin plate: for free v, U_v = (the sum of N(v)'s positions in ascending id, from 0) / |N(v)| - V_v;
+ *    D_s = F (l0 l0); E_s = (the three-level total over vertices of (U_x U_x + U_y U_y) + U_z U_z, free only) / D_s;
+ *    the gradient is (2 / D_s) (-U_v + the sum over free w in N(v), ascending, of U_w / |N(w)|).  E_photo = (the sum over
+ *    pairs in input order, from 0, of each pair's three-level total of e over its pixels) / P0, and E = E_photo +
+ *    smoothness E_s; G_v = G_photo + smoothness G_s per component.  F = 0 or l0 = 0: E_s and its gradient are 0.
+ * 8. Descent: g_rms = sqrt(G2 / F) with G2 the three-level total over free vertices of (G_x G_x + G_y G_y) + G_z G_z
+ *    (0 when F = 0).  A step from the accepted vertices with alpha: al = alpha l0, Delta_v = -((al / g_rms) G_v); when
+ *    |Delta_v| > 2 al it is scaled by (2 al) / |Delta_v|; the candidate is float(V_v + Delta_v), fixed vertices copied.
+ *    The first evaluation is the input (E_0, and P0 from its count).  Status 1: P0 = 0 (the vertices are copied).
+ *    Then, before each step: g_rms = 0 or alpha < step / 1024 ends the call with status 0, and maxIterations candidate
+ *    evaluations end it with status 3.  alpha starts at step; a candidate whose E is strictly lower than the accepted
+ *    E is accepted (with its gradient) and alpha returns to step, otherwise alpha halves.  The output is the accepted
+ *    vertices, so E_out <= E_0.  The host decides every branch on totals it reads.
+ * - Outputs: d_outVertices.  info_out [4] (may be NULL): E_photo and E_s of the input, then of the output.
+ *   stats_out [8] (may be NULL): pairs, free vertices, fixed vertices, P0, evaluations (the first included), accepted
+ *   steps, halvings of the final alpha (alpha = step / 2^h), status.  Returns the status, or CS_E_*.  numTriangles == 0:
+ *   the vertices are copied, every vertex is fixed and the status is 1, with no kernel launch.
+ * - Launches (cs_launch_count): 5 setup kernels (validate; keys; runs; compaction; edge total), then 5 numPairs + 5 per
+ *   evaluation (raster of every paired image; per pair map, score, pair total, image gradient, face gather; thin
+ *   plate, its total, vertex gradient, its total) and one step kernel before every evaluation but the first: 5 +
+ *   evaluations (5 numPairs + 5) + evaluations - 1; 1 when the input is invalid; plus cub's sorts and scan (not
+ *   counted).  The host reads a few words after the input check, the setup and each evaluation (one synchronise
+ *   each); *ms (may be NULL) gets the event time of the whole call.
+ * - Scratch, allocated on the call's stream and freed before it returns: 8 bytes per pixel of every image a pair
+ *   names (the depth keys); 50 bytes per pixel of the largest ref image (J, c then s, A, B, Cc, D, the mapped and
+ *   scored flags), reused by every pair, and 8 per 2048 of its pixels; 240 bytes per face (directed keys and their
+ *   sorted copies, corner keys and corners and their sorted copies, run heads and their scan, the neighbour list, the
+ *   corner sums) and 104 per vertex (flags, neighbour and corner ranges, U, two gradients, the candidate), 224 per
+ *   paired image and 8 per pair, plus cub's storage.
+ * - CS_E_ARG, before any CUDA call, naming the argument: the dense calls' image and camera checks; numVertices outside
+ *   [0, 2^30], numTriangles outside [0, 2^28] (the 6 numTriangles directed keys fit an int); numPairs < 0, NULL pairs with numPairs > 0, a pair naming an image
+ *   outside [0, numImages) or with ref == src; windowRadius outside [1, 5]; smoothness not finite or < 0; step not in
+ *   (0, 1]; maxIterations outside [0, 1000]; depthTol not in [0, 1]; NULL or not 4-byte aligned d_vertices or
+ *   d_outVertices with numVertices > 0, d_triangles with numTriangles > 0; and d_outVertices overlapping the mesh or
+ *   an image (one sweep over sorted ranges). */
+int cs_mesh_refine(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
+                   const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles,
+                   const int *pairs, int numPairs, int windowRadius, double smoothness, double step,
+                   int maxIterations, double depthTol, float *d_outVertices, double info_out[4],
+                   long long stats_out[8], double *ms);
+
 /* FindHomography (matching.cu:1000-1087): RANSAC over the matches of set 1.  homography: 9 floats
  * (row-major 3x3, [8] = 1).  Samples are drawn with rand(): srand() beforehand for repeatability. */
 int cs_find_homography(void *d_pts, int numPts, float *homography, int *numMatches, int numLoops,
