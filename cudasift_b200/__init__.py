@@ -24,7 +24,7 @@ __all__ = ["SIFT_DTYPE", "lib", "set_tuning", "InitCuda", "CudaImage", "SiftData
            "BundleAdjust", "BundleAdjustIntrinsics", "UndistortRecords", "TrainVocabulary", "AssignWords",
            "RetrievePairs", "RotationAveraging", "GlobalPositioning", "UndistortImages", "PatchMatchStereo",
            "PatchMatchStereoGeometric", "FuseDepthMaps", "SelectStereoViews", "PoissonMesh",
-           "PoissonMeshScreened", "SimplifyMesh", "RefineMesh"]
+           "PoissonMeshScreened", "SimplifyMesh", "RefineMesh", "CleanMesh"]
 
 from .records import SIFT_DTYPE   # cudaSift.h:6-22 -- 576-byte record, descriptor at byte 64
 assert SIFT_DTYPE.itemsize == 576
@@ -124,6 +124,8 @@ def lib():
                                           vp, ip, vp, ip, vp, vp, vp, c.POINTER(c.c_double)]),
         "cs_simplify_mesh": (ip, [vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, vp, vp, ip, vp, ip, vp, vp,
                                   c.POINTER(c.c_double)]),
+        "cs_clean_mesh": (ip, [vp, vp, ip, vp, ip, ip, c.c_double, ip, ip, c.c_double, ip, ip, c.c_double, c.c_double,
+                               vp, vp, ip, vp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_texture_mesh": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, c.c_double, c.c_double, c.c_double, ip, ip, ip,
                                  vp, ip, vp, vp, vp, vp, ip, vp, vp, c.POINTER(c.c_double)]),
         "cs_texture_mesh_photo": (ip, [vp, ip, vp, vp, vp, vp, ip, vp, ip, ip, c.c_double, c.c_double, c.c_double,
@@ -1466,6 +1468,60 @@ def SimplifyMesh(vertices, triangles, intensity=None, targetTriangles=0, maxErro
         return verts, tris, vint, info, stats, ms.value
     finally:
         for b in ins + outs:
+            if b is not None:
+                b.free()
+
+
+def CleanMesh(vertices, triangles, intensity=None, removeDegenerate=True, longEdgeFactor=20.0, removeNonManifold=True,
+              minComponentFaces=50, minComponentFraction=0.0, maxHoleEdges=30, smoothIterations=0, smoothLambda=0.5,
+              smoothMu=-0.53):
+    """Mesh cleaning (cs_clean_mesh), in the header's order: degenerate and duplicate faces (removeDegenerate), faces
+    with an edge longer than mean + longEdgeFactor * stddev of the edge lengths (0: off), faces past the first two on
+    an edge held by three or more (removeNonManifold), components of fewer than minComponentFaces faces or
+    minComponentFraction of the largest, then boundary loops of at most maxHoleEdges edges (0: off, at most 256) closed
+    by ear cutting, and smoothIterations Taubin steps (smoothLambda, smoothMu).  vertices float32 [V, 3], triangles
+    int32 [T, 3] and intensity [V] or None, as PoissonMesh returns them.  Returns (vertices float32 [V', 3], triangles
+    int32 [T', 3], intensity float32 [V'] or None, info float64 [3] {edge length mean, stddev, threshold}, stats int64
+    [19] (the header's), ms)."""
+    X = np.ascontiguousarray(np.asarray(vertices, np.float32).reshape(-1, 3))
+    F = np.ascontiguousarray(np.asarray(triangles, np.int32).reshape(-1, 3))
+    I = None if intensity is None else np.ascontiguousarray(np.asarray(intensity, np.float32).reshape(-1))
+    if I is not None and len(I) != len(X):
+        raise ValueError("intensity: one value per vertex")
+    V, T = len(X), len(F)
+    ins = [DeviceBuffer(max(X.nbytes, 4)), DeviceBuffer(max(F.nbytes, 4)),
+           DeviceBuffer(max(I.nbytes, 4)) if I is not None else None]
+    maxT = T + T // 4 + 256 if maxHoleEdges else T
+    try:
+        for b, a in zip(ins, (X, F, I)):
+            if b is not None and a.size:
+                b.upload(a)
+        ptr = lambda b: b.ptr if b is not None else None
+        while True:
+            outs = [DeviceBuffer(12 * V + 4), DeviceBuffer(12 * maxT + 4),
+                    DeviceBuffer(4 * V + 4) if I is not None else None]
+            try:
+                info, stats, ms = np.zeros(3), np.zeros(19, np.int64), ctypes.c_double(0.0)
+                n = _check(lib().cs_clean_mesh(ptr(ins[0]), ptr(ins[2]), V, ptr(ins[1]), T, int(bool(removeDegenerate)),
+                                               float(longEdgeFactor), int(bool(removeNonManifold)),
+                                               int(minComponentFaces), float(minComponentFraction), int(maxHoleEdges),
+                                               int(smoothIterations), float(smoothLambda), float(smoothMu),
+                                               ptr(outs[0]), ptr(outs[2]), V, ptr(outs[1]), maxT, _ptr(info),
+                                               _ptr(stats), ctypes.byref(ms)), "CleanMesh")
+                if n > maxT:
+                    maxT = n
+                    continue
+                nv = int(stats[14])
+                verts = outs[0].download(np.float32, 3 * nv).reshape(nv, 3)
+                tris = outs[1].download(np.int32, 3 * n).reshape(n, 3)
+                vint = outs[2].download(np.float32, nv) if I is not None else None
+                return verts, tris, vint, info, stats, ms.value
+            finally:
+                for b in outs:
+                    if b is not None:
+                        b.free()
+    finally:
+        for b in ins:
             if b is not None:
                 b.free()
 

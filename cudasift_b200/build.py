@@ -28,12 +28,12 @@ SOURCES = ["api.cu", "args.cu", "pipeline2.cu", "pyramid.cu", "pyramid2.cu", "de
            "describe.cu", "match.cu", "match_tc.cu", "match_mutual.cu", "match_knn.cu", "match_guided.cu", "homography.cu",
            "geom.cu", "rank.cu", "verify.cu", "tracks.cu", "triangulate.cu", "pose.cu", "bundle.cu", "rotavg.cu", "globalpos.cu",
            "vocab.cu", "stereo.cu", "mesh.cu", "simplify.cu", "texture.cu", "seams.cu",
-           "refine.cu"]
+           "refine.cu", "clean.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC,-O2,-Wall", "-shared"]
 # Units whose float64 arithmetic a test oracle replays bit for bit: every product and sum rounded once.
 UNIT_FLAGS = {"simplify.cu": ["-fmad=false"], "texture.cu": ["-fmad=false"], "seams.cu": ["-fmad=false"],
-              "refine.cu": ["-fmad=false"]}
+              "refine.cu": ["-fmad=false"], "clean.cu": ["-fmad=false"]}
 
 
 def headers():

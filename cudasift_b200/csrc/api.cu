@@ -1792,6 +1792,38 @@ int cs_simplify_mesh(const float *d_vertices, const float *d_vertexIntensity, in
   });
 }
 
+int cs_clean_mesh(const float *d_vertices, const float *d_vertexIntensity, int numVertices, const int *d_triangles,
+                  int numTriangles, int removeDegenerate, double longEdgeFactor, int removeNonManifold,
+                  int minComponentFaces, double minComponentFraction, int maxHoleEdges, int smoothIterations,
+                  double lambda, double mu, float *d_outVertices, float *d_outIntensity, int maxOutVertices,
+                  int *d_outTriangles, int maxOutTriangles, double info_out[3], long long stats_out[19], double *ms)
+{
+  const char *fn = "cs_clean_mesh";
+  if (ms) *ms = 0.0;
+  int r = clean_args(fn, d_vertices, d_vertexIntensity, numVertices, d_triangles, numTriangles, removeDegenerate,
+                     longEdgeFactor, removeNonManifold, minComponentFaces, minComponentFraction, maxHoleEdges,
+                     smoothIterations, lambda, mu, d_outVertices, d_outIntensity, maxOutVertices, d_outTriangles,
+                     maxOutTriangles);
+  if (r < 0) return r;
+  if (numTriangles == 0) {
+    if (info_out)
+      for (int k = 0; k < 3; k++) info_out[k] = 0.0;
+    if (stats_out)
+      for (int k = 0; k < 19; k++) stats_out[k] = 0;
+    return 0;
+  }
+  int err = 0;
+  DeviceCtx *c = current_ctx(&err);
+  if (!c) return err;
+  if ((r = c->h_mesh.grow(clean_result_bytes())) < 0) return r;
+  return timed_sync(fn, c, ms, [&] {
+    return clean_run(d_vertices, d_vertexIntensity, numVertices, d_triangles, numTriangles, removeDegenerate,
+                     longEdgeFactor, removeNonManifold, minComponentFaces, minComponentFraction, maxHoleEdges,
+                     smoothIterations, lambda, mu, d_outVertices, d_outIntensity, maxOutVertices, d_outTriangles,
+                     maxOutTriangles, c->stream, c->h_mesh.p, info_out, stats_out);
+  });
+}
+
 int cs_texture_mesh(const cs_image *images, int numImages, const double *Ks, const double *Rs, const double *ts,
                     const float *d_vertices, int numVertices, const int *d_triangles, int numTriangles, double lambda,
                     double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,

@@ -1060,6 +1060,29 @@ int simplify_args(const char *fn, const float *vertices, const float *vertexInte
   return rs.check(fn);
 }
 
+int clean_args(const char *fn, const float *vertices, const float *vertexIntensity, int numVertices,
+               const int *triangles, int numTriangles, int removeDegenerate, double longEdgeFactor,
+               int removeNonManifold, int minComponentFaces, double minComponentFraction, int maxHoleEdges,
+               int smoothIterations, double lambda, double mu, const float *outVertices, const float *outIntensity,
+               int maxOutVertices, const int *outTriangles, int maxOutTriangles)
+{
+  if (numTriangles < 0 || numTriangles > (1 << 26)) return arg_error(fn, "numTriangles must be in [0, 2^26]");
+  if (removeDegenerate != 0 && removeDegenerate != 1) return arg_error(fn, "removeDegenerate must be 0 or 1");
+  if (!std::isfinite(longEdgeFactor) || longEdgeFactor < 0.0)
+    return arg_error(fn, "longEdgeFactor must be finite and >= 0");
+  if (removeNonManifold != 0 && removeNonManifold != 1) return arg_error(fn, "removeNonManifold must be 0 or 1");
+  if (minComponentFaces < 0) return arg_error(fn, "minComponentFaces must be >= 0");
+  if (!(minComponentFraction >= 0.0 && minComponentFraction <= 1.0))
+    return arg_error(fn, "minComponentFraction must be in [0, 1]");
+  if (maxHoleEdges != 0 && (maxHoleEdges < 3 || maxHoleEdges > 256))
+    return arg_error(fn, "maxHoleEdges must be 0 or in [3, 256]");
+  if (smoothIterations < 0 || smoothIterations > 1000) return arg_error(fn, "smoothIterations must be in [0, 1000]");
+  if (!(lambda > 0.0 && lambda <= 1.0)) return arg_error(fn, "lambda must be in (0, 1]");
+  if (!(mu >= -1.0 && mu < 0.0)) return arg_error(fn, "mu must be in [-1, 0)");
+  return simplify_args(fn, vertices, vertexIntensity, numVertices, triangles, numTriangles, 0, 0.0, 0.0, outVertices,
+                       outIntensity, maxOutVertices, outTriangles, maxOutTriangles);
+}
+
 int texture_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
                  const double *ts, const float *vertices, int numVertices, const int *triangles, int numTriangles,
                  double lambda, double maxViewAngleDeg, double depthTol, int padding, int atlasWidth, int maxSweeps,

@@ -99,6 +99,12 @@ int simplify_args(const char *fn, const float *vertices, const float *vertexInte
                   const int *triangles, int numTriangles, int targetTriangles, double maxError, double boundaryWeight,
                   const float *outVertices, const float *outIntensity, int maxOutVertices, const int *outTriangles,
                   int maxOutTriangles);
+// cs_clean_mesh: the mesh size, the stage parameters, then simplify_args's buffer checks and range sweep.
+int clean_args(const char *fn, const float *vertices, const float *vertexIntensity, int numVertices,
+               const int *triangles, int numTriangles, int removeDegenerate, double longEdgeFactor,
+               int removeNonManifold, int minComponentFaces, double minComponentFraction, int maxHoleEdges,
+               int smoothIterations, double lambda, double mu, const float *outVertices, const float *outIntensity,
+               int maxOutVertices, const int *outTriangles, int maxOutTriangles);
 // cs_texture_mesh: the images and cameras, the mesh, the parameters, the buffers and the range sweep.
 int texture_args(const char *fn, const cs_image *images, int numImages, const double *Ks, const double *Rs,
                  const double *ts, const float *vertices, int numVertices, const int *triangles, int numTriangles,

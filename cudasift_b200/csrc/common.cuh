@@ -786,6 +786,17 @@ int simplify_run(const float *vertices, const float *intensity, int numVertices,
                  double *info, long long *stats);
 size_t simplify_result_bytes();
 
+// ---- mesh cleaning (clean.cu) ----------------------------------------------------------------------------------------
+// cs_clean_mesh after its argument checks (numTriangles > 0), on st with readbacks through h_result (pinned,
+// clean_result_bytes), the scratch allocated and freed on st; fills info (may be NULL; 3 entries) and stats (may be
+// NULL; 19 entries) and returns the full triangle count.
+int clean_run(const float *vertices, const float *intensity, int numVertices, const int *triangles, int numTriangles,
+              int removeDegenerate, double longEdgeFactor, int removeNonManifold, int minComponentFaces,
+              double minComponentFraction, int maxHoleEdges, int smoothIterations, double lambda, double mu,
+              float *outVertices, float *outIntensity, int maxOutVertices, int *outTriangles, int maxOutTriangles,
+              cudaStream_t st, void *h_result, double *info, long long *stats);
+size_t clean_result_bytes();
+
 // ---- mesh texturing (texture.cu) -----------------------------------------------------------------------------------
 // The depth-buffer bytes of one image group (cs_set_tuning("texture_group_bytes"); 0 or less: 1 GiB).
 extern long long g_texture_group_bytes;

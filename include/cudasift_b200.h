@@ -1313,6 +1313,77 @@ int cs_simplify_mesh(const float *d_vertices, const float *d_vertexIntensity, in
                      float *d_outVertices, float *d_outIntensity, int maxOutVertices, int *d_outTriangles,
                      int maxOutTriangles, double info_out[1], long long stats_out[9], double *ms);
 
+/* Mesh cleaning: the clean-up between meshing and the later mesh stages (OpenMVS's Mesh::Clean), in one deterministic
+ * call.  It drops degenerate, duplicate, long-edge and non-manifold-edge faces and small components, closes small holes
+ * by ear cutting without new vertices, and optionally smooths.  The inputs and outputs are in cs_simplify_mesh's
+ * layout, so the calls chain without a copy: d_vertices [numVertices][3] float, d_vertexIntensity [numVertices] (may
+ * be NULL), d_triangles [numTriangles][3] int32.  All arithmetic below is float64 from the float positions, each
+ * product, sum, quotient and square root rounded once, in the order written (no contraction); n(a, b, c) =
+ * (p_b - p_a) x (p_c - p_a) and dot products as in cs_simplify_mesh's rule 2.  Corner 3t + k starts the edge from corner
+ * k to corner k + 1 mod 3.  The rules run in this order, each on the faces the rules before it keep:
+ * 1. Input: cs_simplify_mesh's rule 1; status 2 and nothing written when it fails.
+ * 2. (removeDegenerate) A face with n.n == 0 is dropped (degenerate), unless each of its three edges is held by another
+ *    input face: such a face lies inside the surface (marching tetrahedra leaves them in closed meshes), and dropping
+ *    it would open a flat slit that no allowed ear of rule 6 closes, so it stays.  Of the remaining faces with the same
+ *    vertex set, in either orientation, the lowest index stays and the others are dropped (duplicate).
+ * 3. (longEdgeFactor > 0) Over the distinct undirected edges of the kept faces, in ascending key (min << 32) | max,
+ *    with length l = sqrt(d.d), d = p_max - p_min: N = sum 1, S1 = sum l and S2 = sum l l in coop.cuh's three-level
+ *    order (tiles of 2048 positions of the sorted corner edge keys of all 3 numTriangles input corners, a value at the
+ *    first position of each kept edge; groups of 256 tiles); m = S1 / N, s = sqrt(S2 / N - m m) (0 when
+ *    not positive), threshold m + longEdgeFactor s.  A face with an edge longer than the threshold is dropped.
+ * 4. (removeNonManifold) On an edge held by three or more kept faces, the two lowest-index faces stay and the others
+ *    are dropped, all against the faces kept before the rule.  Dropping faces creates no new non-manifold edge, so one
+ *    pass suffices.  Non-manifold vertices are not split: a vertex is counted as non-manifold when the corners at it
+ *    of the faces kept after this rule form more than one fan, corners of two faces joining across an edge at the
+ *    vertex held by exactly two of those faces.
+ * 5. Faces join across edges held by exactly two kept faces; the components are built by union-find whose root is the
+ *    lowest face.  With minComponentFaces > 1 or minComponentFraction > 0, a component is dropped when its face count
+ *    n < minComponentFaces or n < minComponentFraction n_max (as float64), n_max the largest component's count.
+ * 6. (maxHoleEdges > 0, at most 256) A kept face's corner edge a -> b held by no other kept face gives the boundary
+ *    half-edge b -> a (the loop direction, so fill faces take their neighbours' orientation).  A half-edge's successor
+ *    is the half-edge out of its end vertex when that vertex has exactly one boundary half-edge in and one out; the
+ *    half-edges on a successor cycle form a loop that starts at its lowest vertex id (found by pointer jumping); the
+ *    others lie on no loop.  A loop of L <= maxHoleEdges edges (L >= 3 always) is filled by ear cutting over its
+ *    vertices r_0 .. r_{L-1} in loop order: with the reference normal N = sum_{i=1}^{L-2} n(r_0, r_i, r_{i+1}) summed
+ *    in i order, the ear at position i of the current ring (prev, cur, next) is allowed when n(prev, cur, next).N > 0
+ *    (no reflex and no zero-area ear), no kept face holds the edge {prev, next}, and no other ring vertex q has
+ *    n(prev, cur, q).N > 0, n(cur, next, q).N > 0 and n(next, prev, q).N > 0 (inside the ear); of the allowed ears the one with the largest
+ *    c = (u.w) / sqrt((u.u)(w.w)), u = p_prev - p_cur, w = p_next - p_cur (the smallest apex angle) is cut, ties to the
+ *    lowest position; the face (prev, cur, next) is added and cur leaves the ring.  With three vertices left, the face
+ *    (r'_0, r'_1, r'_2) of the ring in its current order closes the loop when n.N > 0.  A loop with no allowed ear left
+ *    stays open and adds no face.  Fill faces follow the kept input faces, by loop (ascending start vertex), then in
+ *    cutting order.
+ * 7. (smoothIterations > 0) Taubin steps over the output faces: per iteration a step with f = lambda (0 < lambda <= 1)
+ *    from the positions, then one with f = mu (-1 <= mu < 0) from the result: x' = x + f (s / k - x) per component, s
+ *    the sum, in ascending id, of the k distinct neighbours' positions (starting from 0).  Vertices on an edge held by
+ *    other than two output faces stay fixed.  The neighbours come from the sorted directed edge keys.
+ * 8. Outputs: d_outVertices [][3] float (the vertices the output faces use, in ascending input index, rounded to
+ *    float), d_outIntensity [] (with d_vertexIntensity, copied), d_outTriangles [][3] (renumbered), each the prefix of
+ *    its full list (at most maxOutVertices or maxOutTriangles entries).  info_out [3] (may be NULL): m, s and the
+ *    threshold of rule 3 (0 when it is off).  stats_out [19] (may be NULL): input triangles; faces dropped as
+ *    degenerate, duplicate, long-edge, non-manifold-edge and small-component; components (after rule 4), components
+ *    dropped, non-manifold vertices; loops, loops filled, loops left open, boundary half-edges on no loop, fill faces;
+ *    full vertex and triangle counts, vertices and triangles written, status.  Returns the full triangle count, or
+ *    CS_E_*.  numTriangles == 0 returns 0 (status 0) and makes no CUDA call.
+ * - Determinism: two calls give the same bytes; integer atomics only, each with an order-independent result.
+ * - Launches (cs_launch_count): validate (only that one when the input is invalid), init, 3 for rule 2, edge keys, 4 for
+ *   rule 3, 2 for rule 4, 3 for the links, roots and counts, 1 for rule 5's drop, 6 + R for rule 6 (boundary, count,
+ *   write, successors, R = ceil(log2(3 numTriangles + 1)) jumps, loops, ears) plus its copy of the fill faces, 2 for
+ *   the kept faces, 2 + 2 smoothIterations for rule 7 and 4 for the output; each stage's only when it is on.  Plus
+ *   cub's sorts and scans (not counted).  The host synchronises after the input check, before smoothing when it is on,
+ *   and at the end; *ms (may be NULL) gets the event time of the whole call.
+ * - Scratch, allocated on the call's stream and freed before it returns: 292 bytes per triangle and 97 per vertex, and
+ *   with smoothing 96 more per output triangle, plus cub's storage.
+ * - CS_E_ARG, before any CUDA call, naming the argument: numTriangles outside [0, 2^26], removeDegenerate or
+ *   removeNonManifold not 0 or 1, longEdgeFactor not finite or < 0, minComponentFaces < 0, minComponentFraction outside
+ *   [0, 1], maxHoleEdges not 0 and outside [3, 256], smoothIterations outside [0, 1000], lambda outside (0, 1], mu
+ *   outside [-1, 0); then cs_simplify_mesh's checks of numVertices, the buffers and their overlap. */
+int cs_clean_mesh(const float *d_vertices, const float *d_vertexIntensity, int numVertices, const int *d_triangles,
+                  int numTriangles, int removeDegenerate, double longEdgeFactor, int removeNonManifold,
+                  int minComponentFaces, double minComponentFraction, int maxHoleEdges, int smoothIterations,
+                  double lambda, double mu, float *d_outVertices, float *d_outIntensity, int maxOutVertices,
+                  int *d_outTriangles, int maxOutTriangles, double info_out[3], long long stats_out[19], double *ms);
+
 /* Mesh texturing (Waechter, Moehrle & Goesele, "Let There Be Color!", ECCV 2014, without global seam levelling): for
  * every face one image to take its texture from, the charts of adjacent faces with the same image, and one atlas of
  * the charts' image rectangles with per-corner texture coordinates.  Images and cameras are the dense calls' (pinhole:
